@@ -85,6 +85,8 @@ struct bf_ctx {
   bf::Slot* slots_dev = nullptr;
   size_t slots_dev_cap = 0;
   bool slots_dirty = true;
+  std::vector<uint32_t> ff_host;       // fail-fast masks, bf::FF_STRIDE words per slot (device_record.h), mirrored with the slots
+  uint32_t* ff_dev = nullptr;          // capacity: slots_dev_cap rows
   uint32_t max_rec_bytes = 0;          // largest live record
   uint32_t max_rec_by_w[33] = {};      // ... among the topologies of W = ceil(S/32) words (a batch of layout.words = w stages only W <= w)
   bool rec_max_dirty = false;          // a drop may have lowered the maxima: recomputed at the next plan
@@ -195,6 +197,7 @@ static int forced_format() {
 
 struct RecPlan {
   uint32_t off_col, off_planes, off_par, off_allow, rec_bytes, W, child_nibbles, ell, max_deg;
+  uint32_t ff[bf::FF_STRIDE];   // the topology's row of the fail-fast mask table
   std::vector<uint32_t> child_first, allow_off;
 };
 
@@ -250,6 +253,15 @@ int plan_record(const bf_topology& t, RecPlan& p, std::string& why, bool host_ka
   if (nib > 0xFFFF) { why = "too many parallel branches"; return BF_ETOPO; }
   p.child_nibbles = round_up(nib, 8);
   p.W = (S + 31) / 32;
+  memset(p.ff, 0, sizeof p.ff);
+  if (p.W <= bf::FF_STRIDE) {
+    bool main_only = true;
+    for (uint32_t i = 0; i < S && main_only; ++i) {
+      main_only = ((t.step_flags[i] & BF_SF_GROUP_MASK) >> BF_SF_GROUP_SHIFT) == BF_GROUP_MAIN;
+      if (!(t.step_flags[i] & BF_SF_ALLOW_FAILURE)) p.ff[i >> 5] |= 1u << (i & 31u);
+    }
+    if (!main_only) memset(p.ff, 0, sizeof p.ff);
+  }
   uint32_t off = sizeof(bf::TopoHeader);
   // Row format (device_record.h): fixed-width rows of K = 2 / 4 entries (no row_ptr; unused entries = PAD) when no step
   // has more than K needs and the block is not larger than the CSR block it replaces, else CSR.
@@ -403,12 +415,17 @@ int sync_slots(bf_ctx* c, cudaStream_t stream) {
     size_t ncap = c->slots_dev_cap ? c->slots_dev_cap : 1024;
     while (ncap < n) ncap *= 2;
     bf::Slot* np = nullptr;
+    uint32_t* nf = nullptr;
     BF_CUDA(c, cudaMalloc(&np, ncap * sizeof(bf::Slot)));
+    if (cudaError_t e = cudaMalloc(&nf, ncap * bf::FF_STRIDE * sizeof(uint32_t))) { cudaFree(np); return cuda_fail(c, e, "cudaMalloc fail-fast masks"); }
     if (c->slots_dev) cudaFree(c->slots_dev);
+    if (c->ff_dev) cudaFree(c->ff_dev);
     c->slots_dev = np;
+    c->ff_dev = nf;
     c->slots_dev_cap = ncap;
   }
   if (n) BF_CUDA(c, cudaMemcpyAsync(c->slots_dev, c->slots_host.data(), n * sizeof(bf::Slot), cudaMemcpyHostToDevice, stream));
+  if (n) BF_CUDA(c, cudaMemcpyAsync(c->ff_dev, c->ff_host.data(), n * bf::FF_STRIDE * sizeof(uint32_t), cudaMemcpyHostToDevice, stream));
   BF_CUDA(c, cudaStreamSynchronize(stream));
   c->slots_dirty = false;
   return BF_OK;
@@ -460,7 +477,7 @@ int run_pass(bf_ctx* c, const bf_batch& b, const uint8_t* d_state, uint8_t* d_re
   if (batch_rec_bytes == 0) batch_rec_bytes = 64;   // no topology fits the layout: every run will be marked dead
 
   bf::KParams P{};
-  P.state = d_state; P.result = d_result; P.slots = c->slots_dev;
+  P.state = d_state; P.result = d_result; P.slots = c->slots_dev; P.ff_mask = c->ff_dev;
   P.counts = (b.flags & BF_EVAL_NO_COUNTS) ? nullptr : d_counts;
   P.n_slots = (uint32_t)c->slots_host.size();
   P.n_runs = b.n_runs; P.flags = b.flags; P.max_iter = b.max_iterations;
@@ -835,13 +852,19 @@ int put_many_locked(bf_ctx* c, const bf_topology* topos, uint32_t count, uint32_
   for (uint32_t i = 0; i < count; ++i) {
     uint32_t slot;
     if (!c->free_slots.empty()) { slot = c->free_slots.back(); c->free_slots.pop_back(); }
-    else { slot = (uint32_t)c->meta.size(); c->meta.emplace_back(); c->slots_host.push_back(bf::Slot{0, 0, 0}); }
+    else {
+      slot = (uint32_t)c->meta.size();
+      c->meta.emplace_back();
+      c->slots_host.push_back(bf::Slot{0, 0, 0});
+      c->ff_host.resize(c->ff_host.size() + bf::FF_STRIDE, 0u);
+    }
     TopoMeta& m = c->meta[slot];
     m.alive = true; m.S = topos[i].n_steps; m.E = topos[i].n_edges; m.P = topos[i].n_parallel;
     m.bytes = plans[i].rec_bytes; m.offset = base + off; m.child_first = plans[i].child_first;
     m.child_nibbles = plans[i].child_nibbles;
     c->slots_host[slot] = bf::Slot{(uint64_t)(uintptr_t)(c->arena + m.offset), m.bytes,
                                    m.S | (m.P << 16) | (bf::slot_row_bytes(plans[i].ell) << 24)};
+    memcpy(&c->ff_host[(size_t)slot * bf::FF_STRIDE], plans[i].ff, sizeof plans[i].ff);
     if (m.bytes > c->max_rec_bytes) c->max_rec_bytes = m.bytes;
     if (m.bytes > c->max_rec_by_w[plans[i].W]) c->max_rec_by_w[plans[i].W] = m.bytes;
     off += plans[i].rec_bytes;
@@ -904,7 +927,7 @@ int bf_create(bf_ctx** out, const bf_config* cfg) {
     std::lock_guard<std::mutex> g(c->mu);
     if (grow_arena(c, (size_t)cfg->arena_bytes) != BF_OK) { bf_destroy(c); return BF_ENOMEM; }
   }
-  if (cfg && cfg->max_topologies) { c->meta.reserve(cfg->max_topologies); c->slots_host.reserve(cfg->max_topologies); }
+  if (cfg && cfg->max_topologies) { c->meta.reserve(cfg->max_topologies); c->slots_host.reserve(cfg->max_topologies); c->ff_host.reserve((size_t)cfg->max_topologies * bf::FF_STRIDE); }
   *out = c;
   return BF_OK;
 }
@@ -920,7 +943,7 @@ void bf_destroy(bf_ctx* c) {
     if (c->ev_k[k]) cudaEventDestroy(c->ev_k[k]);
   }
   cudaFreeHost(c->h_counts);
-  cudaFree(c->arena); cudaFree(c->slots_dev); cudaFree(c->d_state); cudaFree(c->d_result); cudaFree(c->d_counts); cudaFree(c->d_acc);
+  cudaFree(c->arena); cudaFree(c->slots_dev); cudaFree(c->ff_dev); cudaFree(c->d_state); cudaFree(c->d_result); cudaFree(c->d_counts); cudaFree(c->d_acc);
   cudaFree(c->d_defer); cudaFree(c->d_exp); cudaFree(c->d_exp_counts); cudaFree(c->d_offsets); cudaFree(c->d_block_sums); cudaFree(c->d_sched); cudaFree(c->d_deltas); cudaFree(c->d_rejected);
   cudaFree(c->d_head); cudaFree(c->d_events); cudaFree(c->d_cblock);
   for (Resident& r : c->resident) { cudaFree(r.d_state); cudaFree(r.d_result); cudaFree(r.d_result_prev); }
@@ -1013,6 +1036,7 @@ static int drop_locked(bf_ctx* c, uint32_t slot) {
   c->meta[slot].alive = false;
   if (c->meta[slot].P) c->n_with_parallel--;
   c->slots_host[slot] = bf::Slot{0, 0, 0};
+  memset(&c->ff_host[(size_t)slot * bf::FF_STRIDE], 0, bf::FF_STRIDE * sizeof(uint32_t));
   c->free_slots.push_back(slot);
   c->n_alive--;
   c->slots_dirty = true;

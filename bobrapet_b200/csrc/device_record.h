@@ -98,11 +98,17 @@ struct Slot {          // device slot table entry
 // bits 24-31 of Slot::meta (abi.cu writes them, the packed-lanes kernel reads them to stage only the rows it can walk)
 __host__ __device__ inline uint32_t slot_row_bytes(uint32_t ell) { return (ell != 0 && !(ell & ELL_PACK10)) ? ell_row_bytes(ell) : 0u; }
 static_assert(sizeof(Slot) == 16, "Slot must be 16 bytes");
+// Fail-fast mask table beside the slot table: FF_STRIDE words per slot id.  Word w holds the bits of word w of the main
+// steps without allowFailure, for a topology of at most 512 steps that has no compensation or finally step; every other
+// topology (and a dead slot) has an all-zero row.  A fail-fast run with a Failed step under its mask has no candidate step
+// in its pass, so the packed-lanes kernel stages none of its needs rows (the cut, frontier_pack.cu).
+constexpr uint32_t FF_STRIDE = 16;
 
 struct KParams {
   const uint8_t* state;
   uint8_t* result;
   const Slot* slots;
+  const uint32_t* ff_mask;      // [n_slots][FF_STRIDE] fail-fast masks (read by the packed-lanes kernel only)
   unsigned long long* counts;   // bf_counts (4 x u64) or nullptr
   // compact ticks whose pass is the packed-lanes kernel alone: the pass itself leaves every run's head word (summary | listed |
   // event count) and adds the counts to the per-512-run totals the emit kernel scans — no separate heads kernel

@@ -240,27 +240,33 @@ __global__ void __launch_bounds__(32 * PACK_MAX_WARPS, PACK_MIN_BLOCKS) frontier
   // issue 0 (lq == 0) hold the group my warp will issue when it is done with the current one.
   const uint32_t GB = 32u >> (5 - lg);        // = Wq: issues per prologue batch
   const uint32_t lq = lane >> (5 - lg), lr = lane & (R - 1u);   // my pair inside a batch: issue lq, run lr
-  uint32_t pf_sid = 0xFFFFFFFFu, pf_run = 0xFFFFFFFFu, pf_lo = 0, pf_hi = 0, pf_bytes = 0, pf_meta = 0;
-  auto load_sid = [&](uint32_t t, bool mine) {   // first link: my run's topology slot id (the head word of its state record)
-    pf_sid = 0xFFFFFFFFu; pf_run = 0xFFFFFFFFu;
+  constexpr bool FF = !CD;   // the fail-fast skip of the cut below
+  // A lane without a run keeps pf_sid all ones, so load_ent leaves its entry zero and issue() writes a dead marker.
+  uint32_t pf_sid = 0xFFFFFFFFu, pf_rf = 0, pf_lo = 0, pf_hi = 0, pf_bytes = 0, pf_meta = 0;
+  auto load_sid = [&](uint32_t t, bool mine) {   // first link: my run's topology slot id and run flags (bf_run_header)
+    pf_sid = 0xFFFFFFFFu; pf_rf = 0;
     if (mine && t < T) {
       const uint32_t r = ((blockIdx.x + t * gridDim.x) << (5 - lg)) + lr;
       if (r < N) {
-        pf_run = r;
         const uint8_t* sr = P.state + (size_t)r * P.state_stride;
-        pf_sid = __ldg(reinterpret_cast<const uint32_t*>(sr));
+        const uint2 hv = __ldg(reinterpret_cast<const uint2*>(sr));
+        pf_sid = hv.x; pf_rf = hv.y;
         // the phase words load_cut() reads for this run: into L2 now, so that they are there when it asks
         asm volatile("prefetch.global.L2 [%0];" ::"l"(sr + P.off_phase));
         asm volatile("prefetch.global.L2 [%0];" ::"l"(sr + P.off_phase + 16u * Wmax - 4u));
       }
     }
   };
-  auto load_ent = [&]() {                        // second link: the slot entry (address, bytes, meta)
+  // second link: the slot entry (address, bytes, meta).  From here on pf_sid is the slot whose fail-fast mask load_cut()
+  // reads, all ones for a run that is not fail-fast or whose group the host sets (stage I does not mark it).
+  auto load_ent = [&]() {
     pf_lo = 0; pf_hi = 0; pf_bytes = 0; pf_meta = 0;
     if (pf_sid < P.n_slots) {
       const uint4 v = __ldg(reinterpret_cast<const uint4*>(P.slots + pf_sid));
       pf_lo = v.x; pf_hi = v.y; pf_bytes = v.z; pf_meta = v.w;
     }
+    if (!FF || (pf_rf & (BF_RF_FAIL_FAST | BF_RF_HOST_GROUP)) != BF_RF_FAIL_FAST) pf_sid = 0xFFFFFFFFu;
+    if (FF && pf_sid < P.n_slots) asm volatile("prefetch.global.L2 [%0];" ::"l"(P.ff_mask + (size_t)pf_sid * FF_STRIDE));
   };
   // The cut: a run's topology buffer receives its header and the rows from the run's first word that can hold a candidate
   // step on; the rows below stay whatever an earlier group left there.  Stage D and the cond-FAIL fix-up read the rows of
@@ -269,29 +275,49 @@ __global__ void __launch_bounds__(32 * PACK_MAX_WARPS, PACK_MIN_BLOCKS) frontier
   // NODEP only narrow.  Should a stage ever turn a step into a candidate from a code in TERMINAL | RUNNING_Q, this cut
   // must go.  The phase words of the group's runs are read from global memory (lane g * Wq + w: word w of run g; load_sid
   // prefetches them into L2): the same lines the group's state copy reads, and like it before griddepcontrol.wait.
+  // A run that cannot have a candidate at all receives no rows: a fail-fast run (stage I chooses its group) with a code of
+  // TERMINAL \ COMPLETED0 (4, 5, 6, 7, 11, 12) on a step of its topology's fail-fast mask (FF_STRIDE, device_record.h: main
+  // steps without allowFailure, and only in topologies with G1 = G2 = 0).  Stage G rewrites only RUNNING sync steps, so that
+  // code survives it and the step is FAILED & GM: amf holds, and stage I marks mark_ff = GM & ~COMPL & ~RUNQ & ~TERM
+  // Skipped.  With G1 = G2 = 0 GSEL is GM (CAND0 = GM minus what mark_ff just covered: empty) or the group is DONE (CAND0 =
+  // 0); the topology-terminated branch only adds Failed steps.  So CAND = 0 in every word and stage D and the fix-up read no
+  // row.  Should a later stage ever make a candidate of such a run, this skip must go.  Only passes without cond and
+  // decision codes (!CD) test for such runs: with them the test cost more than the rows it saved (H100 SXM at 700 W, cfg4,
+  // µs per pipelined pass in three rounds: 52.3 - 52.5 without the test, 52.8 - 53.1 with it).
+  // Passes without decision codes read neither T0, T1, T2 nor TS: a run that receives no rows then receives its planes from
+  // AF on (rounded down to 16 B).
   constexpr uint32_t LUT_CAND_POSSIBLE = ~(BF_LUT_TERMINAL | BF_LUT_RUNNING_Q) & 0xFFFFu;   // codes 0, 9, 10, 14, 15
-  uint32_t cp0 = 0, cp1 = 0, cp2 = 0, cp3 = 0;
-  auto load_cut = [&](uint32_t t) {
-    cp0 = 0; cp1 = 0; cp2 = 0; cp3 = 0;
+  constexpr uint32_t LUT_FAILED = BF_LUT_TERMINAL & ~BF_LUT_COMPLETED0;                       // codes 4, 5, 6, 7, 11, 12
+  const bool trim_planes = P.off_decision == BF_OFF_NONE;
+  uint32_t cp0 = 0, cp1 = 0, cp2 = 0, cp3 = 0, ffm = 0;
+  // the phase words and fail-fast mask word of lane g * Wq + w for group t, whose slot entries the lanes of issue k hold
+  // (load_ent has run)
+  auto load_cut = [&](uint32_t t, uint32_t k) {
+    cp0 = 0; cp1 = 0; cp2 = 0; cp3 = 0; ffm = 0;
     const uint32_t r = ((blockIdx.x + t * gridDim.x) << (5 - lg)) + g;
-    if (t < T && r < N && w < Wmax) {
+    const bool mine = t < T && r < N && w < Wmax;
+    if (mine) {
       const uint32_t* pw = reinterpret_cast<const uint32_t*>(P.state + (size_t)r * P.state_stride + P.off_phase) + w;
       cp0 = __ldg(pw); cp1 = __ldg(pw + Wmax); cp2 = __ldg(pw + 2u * Wmax); cp3 = __ldg(pw + 3u * Wmax);
     }
+    if (!FF) return;
+    const uint32_t sid = __shfl_sync(FULL, pf_sid, (k << (5 - lg)) + g);
+    if (mine && sid < P.n_slots) ffm = __ldg(P.ff_mask + (size_t)sid * FF_STRIDE + w);
   };
   // issue the copies of group t into slot group `sg`, which thereby starts its use number `use`; the lanes of issue `k`
-  // (lq == k) own its runs and hold their slot entries, load_cut(t) has been called
+  // (lq == k) own its runs and hold their slot entries, load_cut(t, k) has been called
   auto issue = [&](uint32_t t, uint32_t sg, uint32_t use, uint32_t k) {
     const uint32_t Sg = __shfl_sync(FULL, pf_meta, (k << (5 - lg)) + g) & 0xFFFFu;   // steps of run g
     const uint32_t cpw = w * 32u < Sg ? bmsk_clamp(0u, Sg - w * 32u) & plut<LUT_CAND_POSSIBLE>(cp0, cp1, cp2, cp3) : 0u;
-    const uint32_t cand_words = (__ballot_sync(FULL, cpw != 0) >> (lr << lg)) & wq_mask;   // of my run (issuing lanes)
+    const uint32_t cand_b = __ballot_sync(FULL, cpw != 0);
+    const uint32_t ff_b = FF ? __ballot_sync(FULL, (plut<LUT_FAILED>(cp0, cp1, cp2, cp3) & ffm) != 0) : 0u;
+    const uint32_t cand_words = ((ff_b >> (lr << lg)) & wq_mask) ? 0u : (cand_b >> (lr << lg)) & wq_mask;   // of my run (issuing lanes)
     if (t < T && lq == k) {
       const uint32_t buf = groups_a + sg * group_bytes;
       const uint32_t bar = bars + 8u * sg;
       const uint32_t tb = buf + R * P.state_stride + lr * P.topo_buf_bytes;   // my run's topology buffer
-      const bool valid = pf_run != 0xFFFFFFFFu;
-      const bool dfr = valid && P.defer_list != nullptr && ((pf_meta >> 16) & 0xFFu) != 0;  // topology with parallel steps
-      const bool ok = valid && !dfr && (pf_lo | pf_hi) != 0 && pf_bytes <= P.topo_buf_bytes;
+      const bool dfr = P.defer_list != nullptr && ((pf_meta >> 16) & 0xFFu) != 0;  // topology with parallel steps
+      const bool ok = !dfr && (pf_lo | pf_hi) != 0 && pf_bytes <= P.topo_buf_bytes;
       if (!ok) sts_v4(tb, dfr ? 0xFFFFFFFFu : 0u, 0u, 0u, 0u);   // marker header (W = 0: dead, all-ones: deferred)
       uint32_t sbytes = 0;
       const uint32_t first = (blockIdx.x + t * gridDim.x) << (5 - lg);
@@ -299,27 +325,33 @@ __global__ void __launch_bounds__(32 * PACK_MAX_WARPS, PACK_MIN_BLOCKS) frontier
         sbytes = min(R, N - first) * P.state_stride;   // the group's state records are adjacent: one copy
         sts_u32(armed_a + 4u * sg, use + 1u);          // published before my arrive: the previous use is over, this one is armed
       }
-      // row bytes below the first word that can hold a candidate (none: all rows; 0 for CSR and formats not cut)
-      const uint32_t lo_word = cand_words ? __ffs(cand_words) - 1u : ((pf_meta & 0xFFFFu) + 31u) >> 5;
-      const uint32_t skip = ok ? lo_word * (pf_meta >> 24) * 32u : 0u;
-      mbar_expect_tx(bar, (ok ? pf_bytes - skip : 0u) + sbytes);
+      // fixed-width rows (rb = row bytes per step; 0 for CSR and formats not cut: one copy of the whole record): the header,
+      // then the rows from the first word that can hold a candidate on.  A run without such a word receives the header and
+      // the planes, from AF when the pass reads no decision codes.  A run with rows keeps its two copies: splitting its
+      // rows from its planes would make three, and on H100 the extra copy per run cost more than the 96 B it saves.
+      const uint32_t Wr = ((pf_meta & 0xFFFFu) + 31u) >> 5, rb = ok ? pf_meta >> 24 : 0u;
+      const uint32_t lo_word = cand_words ? __ffs(cand_words) - 1u : Wr;
+      const uint32_t hdr = (uint32_t)sizeof(TopoHeader), rows_end = hdr + 32u * rb * Wr;   // rows_end = off_planes
+      uint32_t from = hdr + 32u * rb * lo_word;
+      if (rb && trim_planes && from == rows_end) from = (rows_end + PL_AF * 4u * Wr) & ~15u;
+      mbar_expect_tx(bar, (ok ? pf_bytes - (from - hdr) : 0u) + sbytes);
       if (lr == 0) bulk_g2s(buf, P.state + (size_t)first * P.state_stride, sbytes, bar);
       if (ok) {
         const uint8_t* src = reinterpret_cast<const uint8_t*>((uint64_t)pf_lo | ((uint64_t)pf_hi << 32));
-        const uint32_t from = skip ? (uint32_t)sizeof(TopoHeader) + skip : 0u;
-        if (skip) bulk_g2s(tb, src, (uint32_t)sizeof(TopoHeader), bar);
-        bulk_g2s(tb + from, src + from, pf_bytes - from, bar);
+        const uint32_t at = from != hdr ? from : 0u;
+        if (at) bulk_g2s(tb, src, hdr, bar);
+        bulk_g2s(tb + at, src + at, pf_bytes - at, bar);
       }
     }
   };
   for (uint32_t q0 = 0; q0 < n_pro; q0 += GB) {      // prologue: GB of my issues at a time (both links of all of them in flight together)
     const bool in_pro = q0 + lq < n_pro;
-    load_cut(warp + q0 * NW);                        // the batch's first issue: beside both links
     load_sid(warp + (q0 + lq) * NW, in_pro);
     load_ent();
+    load_cut(warp + q0 * NW, 0u);                    // the batch's first issue: its phase words beside the second link
     for (uint32_t k = 0; k < GB && q0 + k < n_pro; ++k) {
       const uint32_t t = warp + (q0 + k) * NW;       // < NG: its slot group is t itself, use 0
-      if (k) load_cut(t);
+      if (k) load_cut(t, k);
       issue(t, t, 0u, k);
     }
   }
@@ -547,7 +579,7 @@ __global__ void __launch_bounds__(32 * PACK_MAX_WARPS, PACK_MIN_BLOCKS) frontier
       else walk_items<FMT_CSRL, false>(lane, CAND, lg, wctx, met_w, fd_w);
     }
     met_w |= FREE;
-    load_cut(t + NG);   // the phase words for the cut of the group I shall issue (issue() reduces them)
+    load_cut(t + NG, 0u);   // the phase words and masks for the cut of the group I shall issue (issue() reduces them)
     uint32_t ready_w = met_w, skipc_w = 0, fail_w = 0;
     if (CD) {
       ready_w = met_w & ~c0 & ~c1;   // BF_COND_PASS
