@@ -18,8 +18,8 @@
 // PTX).  The kernel is compiled in variants <CD, CH, FX, XO, LIST, RB> (cond/decision codes present, parallel
 // steps present, device fixpoint, extra outputs, run-list tier, register budget of the build) so the common
 // pass carries no dead work.  Integer only; no tensor cores.  ~3 KB in, 80 B out per run at the BASELINE
-// configuration (measured rates: DESIGN.md section 5).
-#include "kernel_common.cuh"
+// configuration (measured rates: DESIGN.md section 5).  The bit-plane stages are shared with frontier_pack.cu (stages.cuh).
+#include "stages.cuh"
 
 namespace bf {
 
@@ -190,10 +190,7 @@ __global__ void __launch_bounds__(RB == 2 ? 768 : 512, RB == 1 ? 2 : 1) frontier
     const uint32_t T_PAR = ~t0 & t1 & ~t2 & VALID;   // 2
     const uint32_t T_STOP = ~t0 & ~t1 & t2 & VALID;  // 4
 
-    const bool fail_fast = rflags & BF_RF_FAIL_FAST;
     const bool realtime = rflags & BF_RF_REALTIME;
-    const bool topo_term = rflags & BF_RF_TOPOLOGY_TERMINATED;
-    const bool host_group = rflags & BF_RF_HOST_GROUP;
 
     uint32_t acc_ready = 0, acc_skip = 0, acc_fail = 0, acc_needs = 0, acc_skipdep = 0;
     uint32_t summary = 0, iters = 0;
@@ -308,123 +305,17 @@ __global__ void __launch_bounds__(RB == 2 ? 768 : 512, RB == 1 ? 2 : 1) frontier
         }
       }
 
-      // ---------------- stage G: gate / sleep / wait sync (dag.go:1469-1533, 1235-1277, 1327-1437) ----------------
-      if (CD) {
-        if (has_dec) {
-          const uint32_t syn = SYNC_T & plut<BF_LUT_RUNNING>(p0, p1, p2, p3);
-          const uint32_t n0 = d0;
-          const uint32_t n1 = d0 & ~(d1 & TS);
-          const uint32_t n2 = d1 & (~d0 | TS);
-          const uint32_t n3 = ~(d0 ^ d1);
-          gdirty |= syn & ((p0 ^ n0) | (p1 ^ n1) | (p2 ^ n2) | (p3 ^ n3));
-          p0 = (p0 & ~syn) | (n0 & syn);
-          p1 = (p1 & ~syn) | (n1 & syn);
-          p2 = (p2 & ~syn) | (n2 & syn);
-          p3 = (p3 & ~syn) | (n3 & syn);
-        }
-      }
-
-      // ---------------- stage B: classification (dag.go:3377-3388, 2020-2033) ----------------
-      uint32_t TERM = plut<BF_LUT_TERMINAL>(p0, p1, p2, p3);
-      uint32_t COMPL = plut<BF_LUT_COMPLETED0>(p0, p1, p2, p3) | (TERM & AF);
-      uint32_t RUNQ = plut<BF_LUT_RUNNING_Q>(p0, p1, p2, p3);
-      uint32_t FAILED = TERM & ~COMPL;
-      uint32_t group;
-      uint32_t sum = 0;
-      if (host_group) {
-        group = (rflags >> BF_RF_HOST_GROUP_SHIFT) & 3u;
-      } else if ((n_comp | n_final) == 0) {
-        // ---------------- stage I, stories with main steps only (dag.go:422-431, 482-495) ----------------
-        const uint32_t DONE = COMPL | FAILED;
-        const uint32_t mark_ff = GM & ~COMPL & ~RUNQ & ~TERM;  // markFailFastSkipped candidates (:3289-3312)
-        bool amf = __any_sync(FULL, FAILED != 0);
-        const bool do_ff = fail_fast && amf;
-        bool main_done;
-        if (do_ff) {
-          marked = marked || __any_sync(FULL, mark_ff != 0);
-          pset<BF_PHASE_SKIPPED>(mark_ff, p0, p1, p2, p3);
-          TERM |= mark_ff; COMPL |= mark_ff;
-          main_done = !__any_sync(FULL, (GM & ~DONE & ~mark_ff) != 0);
-        } else {
-          main_done = !__any_sync(FULL, (GM & ~DONE) != 0);
-        }
-        if (!main_done && realtime && topo_term) {  // dag.go:436-464
-          const uint32_t m = GM & (p0 | p1 | p2 | p3) & ~TERM;
-          marked = marked || __any_sync(FULL, m != 0);
-          pset<BF_PHASE_FAILED>(m, p0, p1, p2, p3);
-          TERM |= m; COMPL |= m & AF; FAILED |= m & ~AF; RUNQ &= ~m;
-          main_done = true;
-          amf = __any_sync(FULL, FAILED != 0);
-        }
-        group = main_done ? BF_GROUP_DONE : BF_GROUP_MAIN;
-        sum = (main_done ? BF_SUM_MAIN_DONE : 0u) | (amf ? BF_SUM_MAIN_FAILED : 0u) | BF_SUM_COMP_DONE | BF_SUM_FINAL_DONE;
-      } else {
-        // ---------------- stage I, general: dag.go:422-495, all reductions in one redux.or ----------------
-        uint32_t RUN = plut<BF_LUT_RUNNING>(p0, p1, p2, p3);
-        const uint32_t DONE = COMPL | FAILED;
-        const uint32_t mark_ff = GM & ~COMPL & ~RUNQ & ~TERM;           // markFailFastSkipped candidates (:3289-3312)
-        const uint32_t mark_cs = G1 & ~COMPL & ~RUN & ~FAILED & ~TERM;   // markCompensationsSkipped candidates (:3314-3342)
-        uint32_t bits = ((FAILED & GM) != 0 ? 1u : 0u)                   // any main failed
-                        | ((GM & ~DONE) != 0 ? 2u : 0u)                  // main not done (no marking)
-                        | ((GM & ~DONE & ~mark_ff) != 0 ? 4u : 0u)       // main not done even after fail-fast marking
-                        | ((G1 & ~DONE) != 0 ? 8u : 0u)                  // comp not done (no marking)
-                        | ((G1 & ~DONE & ~mark_cs) != 0 ? 16u : 0u)      // comp not done after comp-skip marking
-                        | ((G2 & ~DONE) != 0 ? 32u : 0u)                 // finally not done
-                        | ((FAILED & G1) != 0 ? 64u : 0u)
-                        | ((FAILED & G2) != 0 ? 128u : 0u)
-                        | (mark_ff != 0 ? 256u : 0u)
-                        | (mark_cs != 0 ? 512u : 0u);
-        bits = redux_or(bits);
-        bool amf = bits & 1u;
-        const bool do_ff = fail_fast && amf;
-        if (do_ff) {
-          marked = marked || (bits & 256u);
-          pset<BF_PHASE_SKIPPED>(mark_ff, p0, p1, p2, p3);
-          TERM |= mark_ff; COMPL |= mark_ff; RUN &= ~mark_ff;
-        }
-        bool main_done = n_main == 0 || !(bits & (do_ff ? 4u : 2u));
-        const bool acf = bits & 64u;
-        if (!main_done && realtime && topo_term) {  // dag.go:436-464 (rare: its own reduction)
-          const uint32_t m = GM & (p0 | p1 | p2 | p3) & ~TERM;
-          marked = marked || __any_sync(FULL, m != 0);
-          pset<BF_PHASE_FAILED>(m, p0, p1, p2, p3);
-          TERM |= m; COMPL |= m & AF; FAILED |= m & ~AF; RUN &= ~m; RUNQ &= ~m;
-          main_done = true;
-          amf = __any_sync(FULL, (FAILED & GM) != 0);
-        }
-        bool comp_done;
-        if (main_done && !amf && n_comp != 0) {
-          marked = marked || (bits & 512u);
-          pset<BF_PHASE_SKIPPED>(mark_cs, p0, p1, p2, p3);
-          TERM |= mark_cs; COMPL |= mark_cs;
-          comp_done = !(bits & 16u);
-        } else {
-          comp_done = n_comp == 0 || !(bits & 8u);
-        }
-        const bool final_done = n_final == 0 || !(bits & 32u);
-        const bool aff = bits & 128u;
-        if (!main_done) group = BF_GROUP_MAIN;
-        else if (amf && n_comp != 0 && !comp_done) group = BF_GROUP_COMPENSATION;
-        else if (n_final != 0 && !final_done) group = BF_GROUP_FINALLY;
-        else group = BF_GROUP_DONE;
-        sum = (main_done ? BF_SUM_MAIN_DONE : 0u) | (amf ? BF_SUM_MAIN_FAILED : 0u) |
-              (comp_done ? BF_SUM_COMP_DONE : 0u) | (final_done ? BF_SUM_FINAL_DONE : 0u) |
-              (acf ? BF_SUM_COMP_FAILED : 0u) | (aff ? BF_SUM_FINAL_FAILED : 0u);
-      }
-      summary = sum | group;
+      // ---------------- stages G, B, I and D-prep (stages.cuh) ----------------
+      if (has_dec) gdirty |= stage_g(SYNC_T, TS, d0, d1, p0, p1, p2, p3);
+      const RunClass rc = stage_bi<CD>(FULL, rflags, n_main, n_comp, n_final, AF, GM, G1, G2, p0, p1, p2, p3);
+      marked = marked || rc.marked;
+      summary = rc.sum | rc.group;
 
       uint32_t it_ready = 0, it_skip = 0, it_fail = 0;
-      if (group != BF_GROUP_DONE) {
-        // ------------- D-prep: dependency classes under this pass's policy (dag.go:499-502) -------------
-        const bool allow_failed = group != BF_GROUP_MAIN;
-        const bool skip_on_failed = group == BF_GROUP_MAIN && !fail_fast;
-        const uint32_t GSEL = group == BF_GROUP_MAIN ? GM : (group == BF_GROUP_COMPENSATION ? G1 : G2);
-        const uint32_t SAT = COMPL | (realtime ? plut<BF_LUT_RT_SAT>(p0, p1, p2, p3) : 0u) | (allow_failed ? TERM : 0u);
-        const uint32_t U = ~SAT;
-        const uint32_t FD = skip_on_failed ? (TERM & ~SAT) : 0u;
-        const uint32_t CAND0 = GSEL & ~COMPL & ~RUNQ & ~TERM;
-        const uint32_t FREE = CAND0 & NODEP;   // candidates without needs: met by definition (byte-entry rows only)
-        const uint32_t CAND = CAND0 & ~NODEP;  // the candidates whose rows are walked
+      if (rc.group != BF_GROUP_DONE) {
+        const DepClass dc = stage_dprep(rc, rflags, VALID, GM, G1, G2, NODEP, p0, p1, p2, p3);
+        const bool skip_on_failed = dc.skip_on_failed;
+        const uint32_t U = dc.U, FD = dc.FD, CAND = dc.CAND;
         // ------------- stage C: masks -> one status byte per step (bit0 unmet, bit1 failed-dep) -------------
         __syncwarp();
         uint32_t m0 = 0;
@@ -452,37 +343,14 @@ __global__ void __launch_bounds__(RB == 2 ? 768 : 512, RB == 1 ? 2 : 1) frontier
         constexpr int WK = RB == 1 ? 2 : 4;
         if (skip_on_failed) walk_words_fmt<WK, true>(fmt, lane, CAND, rp_a, col_a, st_a, met_w, fd_w);  // warp-uniform dispatch
         else walk_words_fmt<WK, false>(fmt, lane, CAND, rp_a, col_a, st_a, met_w, fd_w);
-        met_w |= FREE;
+        met_w |= dc.FREE;
         uint32_t ready_w = met_w, skipc_w = 0, fail_w = 0;
         if (CD) {
-          ready_w = met_w & ~c0 & ~c1;   // BF_COND_PASS
-          skipc_w = met_w & c0 & ~c1;    // BF_COND_SKIP
-          fail_w = met_w & c0 & c1;      // BF_COND_FAIL (HOLD = c1 & ~c0: nothing)
-          if (__any_sync(FULL, fail_w != 0)) {
-            // A step set Failed inside the loop is visible to LATER steps of the list only; iterate
-            // to the unique fixed point (one extra round per chained failure).
-            marked = true;
-            const uint32_t fclass = allow_failed ? 0u : (skip_on_failed ? 3u : 1u);
-            for (uint32_t round = 0; round <= S; ++round) {
-              __syncwarp();
-              if (act) sts_u32(mfail_a + lane * 4u, fail_w);
-              __syncwarp();
-              met_w = 0; fd_w = 0;
-              for (uint32_t todo = __ballot_sync(FULL, CAND != 0); todo; todo &= todo - 1) {
-                const uint32_t j = __ffs(todo) - 1;
-                uint32_t mb, fb;
-                fixup_item(lane, __shfl_sync(FULL, CAND, j), j, ell, rp_a, col_a, st_a, mfail_a, fclass, mb, fb);
-                if (lane == j) { met_w = mb; fd_w = fb; }
-              }
-              met_w |= FREE;
-              const uint32_t nf = met_w & c0 & c1;
-              const bool same = !__any_sync(FULL, nf != fail_w);
-              fail_w = nf;
-              if (same) break;
-            }
-            ready_w = met_w & ~c0 & ~c1;
-            skipc_w = met_w & c0 & ~c1;
-          }
+          // item j: word j of the run; the scratch holds fail words for the run's words only (the lanes of `act`)
+          auto fixup = [&](uint32_t j, uint32_t candw, uint32_t fclass, uint32_t& mb, uint32_t& fb) {
+            fixup_item(lane, candw, j, ell, rp_a, col_a, st_a, mfail_a, fclass, mb, fb);
+          };
+          if (stage_cond(lane, c0, c1, dc, mfail_a, act, S, fixup, met_w, fd_w, ready_w, skipc_w, fail_w, p0, p1, p2, p3)) marked = true;
         }
         it_ready = ready_w;
         it_skip = fd_w | skipc_w;
@@ -491,12 +359,11 @@ __global__ void __launch_bounds__(RB == 2 ? 768 : 512, RB == 1 ? 2 : 1) frontier
           acc_needs |= realtime ? 0u : (met_w & HASIF);
           acc_skipdep |= fd_w;
         }
-        if (CD) pset<BF_PHASE_FAILED>(fail_w, p0, p1, p2, p3);  // dag.go:2745-2747, 2810-2812
       }
       acc_ready |= it_ready; acc_skip |= it_skip; acc_fail |= it_fail;
 
       if (!FX) break;
-      if (group == BF_GROUP_DONE) break;
+      if (rc.group == BF_GROUP_DONE) break;
       // ------------- launch effects (dag.go:1735-1775, step_executor.go:132-185) -------------
       const uint32_t o0 = p0, o1 = p1, o2 = p2, o3 = p3;
       pset<BF_PHASE_SKIPPED>(it_skip, p0, p1, p2, p3);
@@ -534,21 +401,7 @@ __global__ void __launch_bounds__(RB == 2 ? 768 : 512, RB == 1 ? 2 : 1) frontier
       *reinterpret_cast<uint4*>(rr) = make_uint4(summary, n_ready, n_skip, n_exp);
       if (CH && P.exp_counts) P.exp_counts[r] = n_exp;
     }
-    if (lane < Wmax) {
-      reinterpret_cast<uint32_t*>(rr + P.off_ready)[lane] = acc_ready;
-      reinterpret_cast<uint32_t*>(rr + P.off_skip)[lane] = acc_skip;
-      if (XO) {
-        if (P.off_fail != BF_OFF_NONE) reinterpret_cast<uint32_t*>(rr + P.off_fail)[lane] = acc_fail;
-        if (P.off_needs_cond != BF_OFF_NONE) reinterpret_cast<uint32_t*>(rr + P.off_needs_cond)[lane] = acc_needs;
-        if (P.off_skip_dep != BF_OFF_NONE) reinterpret_cast<uint32_t*>(rr + P.off_skip_dep)[lane] = acc_skipdep;
-        if (P.off_phase_out != BF_OFF_NONE) {
-          uint32_t* po = reinterpret_cast<uint32_t*>(rr + P.off_phase_out) + lane;
-          po[0] = p0; po[Wmax] = p1; po[2 * Wmax] = p2; po[3 * Wmax] = p3;
-        }
-      }
-    }
-    if (P.result_tail != P.result_stride)
-      for (uint32_t x = P.result_tail / 4 + lane; x < P.result_stride / 4; x += 32) reinterpret_cast<uint32_t*>(rr)[x] = 0u;
+    store_words<XO>(P, rr, lane, 32u, acc_ready, acc_skip, acc_fail, acc_needs, acc_skipdep, p0, p1, p2, p3);
     tot_ready += n_ready; tot_skip += n_skip; tot_exp += n_exp; tot_evals += S;
 
     __syncwarp();  // every lane is done with this stage's buffers
@@ -569,50 +422,43 @@ __global__ void __launch_bounds__(RB == 2 ? 768 : 512, RB == 1 ? 2 : 1) frontier
 }
 
 // ------------------------------------------------------------------ host-side dispatch
-typedef void (*KernelFn)(const KParams);
-template <bool LIST, int RB>
-static KernelFn pick_kernel(bool cd, bool ch, bool fx, bool xo) {
+// index: variant_bits (CD, XO) | CH << 2 | FX << 3; the fixpoint variants exist as RB = 0 only
+template <int RB>
+static KernelFn pick_kernel(uint32_t v) {
   static const KernelFn table[16] = {
-      frontier_kernel<false, false, false, false, LIST, RB>, frontier_kernel<false, false, false, true, LIST, RB>,
-      frontier_kernel<false, false, true, false, LIST, 0>,   frontier_kernel<false, false, true, true, LIST, 0>,
-      frontier_kernel<false, true, false, false, LIST, RB>,  frontier_kernel<false, true, false, true, LIST, RB>,
-      frontier_kernel<false, true, true, false, LIST, 0>,    frontier_kernel<false, true, true, true, LIST, 0>,
-      frontier_kernel<true, false, false, false, LIST, RB>,  frontier_kernel<true, false, false, true, LIST, RB>,
-      frontier_kernel<true, false, true, false, LIST, 0>,    frontier_kernel<true, false, true, true, LIST, 0>,
-      frontier_kernel<true, true, false, false, LIST, RB>,   frontier_kernel<true, true, false, true, LIST, RB>,
-      frontier_kernel<true, true, true, false, LIST, 0>,     frontier_kernel<true, true, true, true, LIST, 0>,
+      frontier_kernel<false, false, false, false, false, RB>, frontier_kernel<false, false, false, true, false, RB>,
+      frontier_kernel<true, false, false, false, false, RB>,  frontier_kernel<true, false, false, true, false, RB>,
+      frontier_kernel<false, true, false, false, false, RB>,  frontier_kernel<false, true, false, true, false, RB>,
+      frontier_kernel<true, true, false, false, false, RB>,   frontier_kernel<true, true, false, true, false, RB>,
+      frontier_kernel<false, false, true, false, false, 0>,   frontier_kernel<false, false, true, true, false, 0>,
+      frontier_kernel<true, false, true, false, false, 0>,    frontier_kernel<true, false, true, true, false, 0>,
+      frontier_kernel<false, true, true, false, false, 0>,    frontier_kernel<false, true, true, true, false, 0>,
+      frontier_kernel<true, true, true, false, false, 0>,     frontier_kernel<true, true, true, true, false, 0>,
   };
-  return table[(cd ? 8 : 0) | (ch ? 4 : 0) | (fx ? 2 : 0) | (xo ? 1 : 0)];
+  return table[v];
 }
 
-// rb: the build (template parameter RB); the fixpoint and run-list variants exist as RB = 0 only
+// rb: the build (template parameter RB)
 static KernelFn kernel_for(const KParams& P, uint32_t rb) {
-  const bool cd = P.off_cond != BF_OFF_NONE || P.off_decision != BF_OFF_NONE;
-  const bool ch = P.any_parallel != 0;  // join needs the child area; the expansion count needs only the descs
-  const bool fx = (P.flags & BF_EVAL_FIXPOINT) != 0;
-  const bool xo = P.off_fail != BF_OFF_NONE || P.off_needs_cond != BF_OFF_NONE || P.off_skip_dep != BF_OFF_NONE ||
-                  P.off_phase_out != BF_OFF_NONE;
-  if (P.run_list) return pick_kernel<true, 0>(cd, ch, fx, xo);   // second tier: a handful of runs
-  if (rb == 2 && !fx) return pick_kernel<false, 2>(cd, ch, fx, xo);
-  return rb == 1 ? pick_kernel<false, 1>(cd, ch, fx, xo) : pick_kernel<false, 0>(cd, ch, fx, xo);
+  uint32_t v = variant_bits(P);
+  if (P.run_list) {
+    // The run-list tier is the second launch of a two-tier pass (abi.cu), which the packed-lanes kernel takes first: a
+    // single pass (FX = 0) of a batch with some topology that has parallel steps (CH = 1), planned as the 16-warp build
+    // (RB = 0).  Only these four variants can run.
+    static const KernelFn list_table[4] = {
+        frontier_kernel<false, true, false, false, true, 0>, frontier_kernel<false, true, false, true, true, 0>,
+        frontier_kernel<true, true, false, false, true, 0>,  frontier_kernel<true, true, false, true, true, 0>};
+    return list_table[v];
+  }
+  v |= (P.any_parallel != 0 ? 4u : 0u)            // CH: the join needs the child area; the expansion count needs only the descs
+       | ((P.flags & BF_EVAL_FIXPOINT) ? 8u : 0u);  // FX
+  return rb == 2 ? pick_kernel<2>(v) : rb == 1 ? pick_kernel<1>(v) : pick_kernel<0>(v);
 }
 
 cudaError_t launch_frontier(const KParams& P, uint32_t grid, uint32_t smem_bytes, cudaStream_t stream) {
-  KernelFn fn = kernel_for(P, P.occ2);
-  static KernelFn configured[8][64] = {};
-  int dev = 0;
-  cudaError_t e = cudaGetDevice(&dev);
+  const KernelFn fn = kernel_for(P, P.occ2);
+  const cudaError_t e = allow_max_smem(fn);
   if (e != cudaSuccess) return e;
-  bool known = false;
-  if (dev >= 0 && dev < 8)
-    for (int i = 0; i < 64; ++i) known = known || configured[dev][i] == fn;
-  if (!known) {
-    e = cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
-    if (e != cudaSuccess) return e;
-    if (dev >= 0 && dev < 8)
-      for (int i = 0; i < 64; ++i)
-        if (configured[dev][i] == nullptr) { configured[dev][i] = fn; break; }
-  }
   fn<<<grid, P.warps_per_block * 32, smem_bytes, stream>>>(P);
   return cudaGetLastError();
 }
@@ -625,19 +471,19 @@ int frontier_max_blocks_per_sm(const KParams& P, uint32_t threads, uint32_t smem
   if (threads > 512) {   // more than 16 warps per CTA: the 80-register build, one CTA per SM (no fixpoint variants)
     if (P.flags & BF_EVAL_FIXPOINT) return 0;
     KernelFn fn3 = kernel_for(P, 2);
-    cudaFuncSetAttribute(fn3, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
+    allow_max_smem(fn3);
     if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, fn3, (int)threads, smem_bytes) != cudaSuccess || n < 1) return 0;
     *occ2 = 2;
     return 1;
   }
   KernelFn fn2 = kernel_for(P, 1);
-  cudaFuncSetAttribute(fn2, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
+  allow_max_smem(fn2);
   if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, fn2, (int)threads, smem_bytes) == cudaSuccess && n >= 2) {
     *occ2 = 1;
     return n;
   }
   KernelFn fn = kernel_for(P, 0);
-  cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
+  allow_max_smem(fn);
   if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, fn, (int)threads, smem_bytes) != cudaSuccess) return 1;
   return n;
 }

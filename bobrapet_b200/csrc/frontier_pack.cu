@@ -31,7 +31,7 @@
 // launch gap and tail overlap; griddepcontrol.wait sits in front of the counters.
 //
 // All shared-memory traffic goes through 32-bit shared-window addresses.  Integer only; no tensor cores.
-#include "kernel_common.cuh"
+#include "stages.cuh"
 
 namespace bf {
 
@@ -270,18 +270,14 @@ __global__ void __launch_bounds__(32 * PACK_MAX_WARPS, PACK_MIN_BLOCKS) frontier
   };
   // The cut: a run's topology buffer receives its header and the rows from the run's first word that can hold a candidate
   // step on; the rows below stay whatever an earlier group left there.  Stage D and the cond-FAIL fix-up read the rows of
-  // the words with CAND != 0 only, and a candidate's INPUT code (15 read as 0) lies outside TERMINAL and RUNNING_Q: stage G
-  // rewrites only RUNNING sync steps, into 8 or a terminal code; stage I and the fix-up only set Skipped / Failed; GSEL and
-  // NODEP only narrow.  Should a stage ever turn a step into a candidate from a code in TERMINAL | RUNNING_Q, this cut
-  // must go.  The phase words of the group's runs are read from global memory (lane g * Wq + w: word w of run g; load_sid
-  // prefetches them into L2): the same lines the group's state copy reads, and like it before griddepcontrol.wait.
+  // the words with CAND != 0 only, and by condition (1) at the top of stages.cuh a candidate's input code lies outside
+  // TERMINAL and RUNNING_Q.  Should the stages ever break that condition, this cut must go.  The phase words of the group's
+  // runs are read from global memory (lane g * Wq + w: word w of run g; load_sid prefetches them into L2): the same lines
+  // the group's state copy reads, and like it before griddepcontrol.wait.
   // A run that cannot have a candidate at all receives no rows: a fail-fast run (stage I chooses its group) with a code of
-  // TERMINAL \ COMPLETED0 (4, 5, 6, 7, 11, 12) on a step of its topology's fail-fast mask (FF_STRIDE, device_record.h: main
-  // steps without allowFailure, and only in topologies with G1 = G2 = 0).  Stage G rewrites only RUNNING sync steps, so that
-  // code survives it and the step is FAILED & GM: amf holds, and stage I marks mark_ff = GM & ~COMPL & ~RUNQ & ~TERM
-  // Skipped.  With G1 = G2 = 0 GSEL is GM (CAND0 = GM minus what mark_ff just covered: empty) or the group is DONE (CAND0 =
-  // 0); the topology-terminated branch only adds Failed steps.  So CAND = 0 in every word and stage D and the fix-up read no
-  // row.  Should a later stage ever make a candidate of such a run, this skip must go.  Only passes without cond and
+  // TERMINAL \ COMPLETED0 on a step of its topology's fail-fast mask (FF_STRIDE, device_record.h: main steps without
+  // allowFailure, and only in topologies with G1 = G2 = 0).  Condition (2) in stages.cuh says why such a run has CAND = 0
+  // in every word; should the stages ever break it, this skip must go.  Only passes without cond and
   // decision codes (!CD) test for such runs: with them the test cost more than the rows it saved (H100 SXM at 700 W, cfg4,
   // µs per pipelined pass in three rounds: 52.3 - 52.5 without the test, 52.8 - 53.1 with it).
   // Passes without decision codes read neither T0, T1, T2 nor TS: a run that receives no rows then receives its planes from
@@ -425,106 +421,16 @@ __global__ void __launch_bounds__(32 * PACK_MAX_WARPS, PACK_MIN_BLOCKS) frontier
     }
     const uint32_t q0 = p0, q1 = p1, q2 = p2, q3 = p3;
     const uint32_t GM = VALID & ~G1 & ~G2;
-    const bool fail_fast = rflags & BF_RF_FAIL_FAST;
     const bool realtime = rflags & BF_RF_REALTIME;
-    const bool topo_term = rflags & BF_RF_TOPOLOGY_TERMINATED;
-    const bool host_group = rflags & BF_RF_HOST_GROUP;
-    bool marked = false;  // group-uniform
 
-    // ---------------- stage G: gate / sleep / wait sync (dag.go:1469-1533, 1235-1277, 1327-1437) ----------------
-    if (CD) {
-      if (has_dec) {
-        const uint32_t syn = SYNC_T & plut<BF_LUT_RUNNING>(p0, p1, p2, p3);
-        const uint32_t n0 = d0;
-        const uint32_t n1 = d0 & ~(d1 & TS);
-        const uint32_t n2 = d1 & (~d0 | TS);
-        const uint32_t n3 = ~(d0 ^ d1);
-        p0 = (p0 & ~syn) | (n0 & syn);
-        p1 = (p1 & ~syn) | (n1 & syn);
-        p2 = (p2 & ~syn) | (n2 & syn);
-        p3 = (p3 & ~syn) | (n3 & syn);
-      }
-    }
-
-    // ---------------- stage B: classification (dag.go:3377-3388, 2020-2033) ----------------
-    uint32_t TERM = plut<BF_LUT_TERMINAL>(p0, p1, p2, p3);
-    uint32_t COMPL = plut<BF_LUT_COMPLETED0>(p0, p1, p2, p3) | (TERM & AF);
-    uint32_t RUNQ = plut<BF_LUT_RUNNING_Q>(p0, p1, p2, p3);
-    uint32_t FAILED = TERM & ~COMPL;
-    uint32_t group, sum = 0;
-    // ---------------- stage I (dag.go:422-495): per-run reductions = one sub-warp redux.or ----------------
-    {
-      uint32_t RUN = plut<BF_LUT_RUNNING>(p0, p1, p2, p3);
-      const uint32_t DONE = COMPL | FAILED;
-      const uint32_t mark_ff = GM & ~COMPL & ~RUNQ & ~TERM;           // markFailFastSkipped candidates (:3289-3312)
-      const uint32_t mark_cs = G1 & ~COMPL & ~RUN & ~FAILED & ~TERM;   // markCompensationsSkipped candidates (:3314-3342)
-      uint32_t bits = ((FAILED & GM) != 0 ? 1u : 0u) | ((GM & ~DONE) != 0 ? 2u : 0u) | ((GM & ~DONE & ~mark_ff) != 0 ? 4u : 0u) |
-                      ((G1 & ~DONE) != 0 ? 8u : 0u) | ((G1 & ~DONE & ~mark_cs) != 0 ? 16u : 0u) | ((G2 & ~DONE) != 0 ? 32u : 0u) |
-                      ((FAILED & G1) != 0 ? 64u : 0u) | ((FAILED & G2) != 0 ? 128u : 0u) | (mark_ff != 0 ? 256u : 0u) |
-                      (mark_cs != 0 ? 512u : 0u);
-      bits = __reduce_or_sync(gmask, bits);
-      // no collective may sit under a per-run branch: host-group runs (tier K1) take part in every
-      // vote below and simply never qualify for a marking
-      const bool auto_group = !host_group;
-      bool amf = bits & 1u;
-      const bool do_ff = auto_group && fail_fast && amf;
-      if (do_ff) {
-        marked = marked || (bits & 256u);
-        pset<BF_PHASE_SKIPPED>(mark_ff, p0, p1, p2, p3);
-        TERM |= mark_ff; COMPL |= mark_ff; RUN &= ~mark_ff;
-      }
-      bool main_done = n_main == 0 || !(bits & (do_ff ? 4u : 2u));
-      const bool acf = bits & 64u;
-      // dag.go:436-464 (rare)
-      const bool tt = auto_group && !main_done && realtime && topo_term;
-      if (__any_sync(FULL, tt)) {
-        const uint32_t mtt = tt ? (GM & (p0 | p1 | p2 | p3) & ~TERM) : 0u;
-        pset<BF_PHASE_FAILED>(mtt, p0, p1, p2, p3);
-        TERM |= mtt; COMPL |= mtt & AF; FAILED |= mtt & ~AF; RUN &= ~mtt; RUNQ &= ~mtt;
-        const uint32_t b2 = __reduce_or_sync(gmask, (mtt != 0 ? 1u : 0u) | ((FAILED & GM) != 0 ? 2u : 0u));
-        if (tt) {
-          marked = marked || (b2 & 1u);
-          main_done = true;
-          amf = b2 & 2u;
-        }
-      }
-      bool comp_done;
-      if (auto_group && main_done && !amf && n_comp != 0) {
-        marked = marked || (bits & 512u);
-        pset<BF_PHASE_SKIPPED>(mark_cs, p0, p1, p2, p3);
-        TERM |= mark_cs; COMPL |= mark_cs;
-        comp_done = !(bits & 16u);
-      } else {
-        comp_done = n_comp == 0 || !(bits & 8u);
-      }
-      const bool final_done = n_final == 0 || !(bits & 32u);
-      const bool aff = bits & 128u;
-      if (!main_done) group = BF_GROUP_MAIN;
-      else if (amf && n_comp != 0 && !comp_done) group = BF_GROUP_COMPENSATION;
-      else if (n_final != 0 && !final_done) group = BF_GROUP_FINALLY;
-      else group = BF_GROUP_DONE;
-      sum = (main_done ? BF_SUM_MAIN_DONE : 0u) | (amf ? BF_SUM_MAIN_FAILED : 0u) | (comp_done ? BF_SUM_COMP_DONE : 0u) |
-            (final_done ? BF_SUM_FINAL_DONE : 0u) | (acf ? BF_SUM_COMP_FAILED : 0u) | (aff ? BF_SUM_FINAL_FAILED : 0u);
-      if (host_group) {
-        group = (rflags >> BF_RF_HOST_GROUP_SHIFT) & 3u;
-        sum = 0;
-      }
-    }
-    uint32_t summary = sum | group;
-
-    // ------------- D-prep: dependency classes under this pass's policy (dag.go:499-502) -------------
-    const bool evaluate = group != BF_GROUP_DONE;
-    const bool allow_failed = group != BF_GROUP_MAIN;
-    const bool skip_on_failed = group == BF_GROUP_MAIN && !fail_fast;
-    const uint32_t GSEL = group == BF_GROUP_MAIN ? GM : (group == BF_GROUP_COMPENSATION ? G1 : G2);
-    const uint32_t SAT = COMPL | (realtime ? plut<BF_LUT_RT_SAT>(p0, p1, p2, p3) : 0u) | (allow_failed ? TERM : 0u);
-    const uint32_t U = VALID & ~SAT;   // & VALID: bytes past the last step (the PAD byte of a narrower run) read "satisfied"
-    const uint32_t FD = skip_on_failed ? (TERM & ~SAT) : 0u;
-    const uint32_t CAND0 = evaluate ? (GSEL & ~COMPL & ~RUNQ & ~TERM) : 0u;
-    const uint32_t FREE = CAND0 & NODEP;   // candidates without needs: met by definition (byte-entry rows only)
-    const uint32_t CAND = CAND0 & ~NODEP;  // the candidates whose rows are walked
+    // ---------------- stages G, B, I and D-prep (stages.cuh); U & VALID: the PAD byte of a narrower run reads "satisfied"
+    if (has_dec) stage_g(SYNC_T, TS, d0, d1, p0, p1, p2, p3);
+    const RunClass rc = stage_bi<CD>(gmask, rflags, n_main, n_comp, n_final, AF, GM, G1, G2, p0, p1, p2, p3);
+    uint32_t summary = rc.sum | rc.group;
+    const DepClass dc = stage_dprep(rc, rflags, VALID, GM, G1, G2, NODEP, p0, p1, p2, p3);
+    const uint32_t U = dc.U, FD = dc.FD, CAND = dc.CAND;
     // ------------- stage C: one status byte per step (bit0 unmet, bit1 failed-dep), all R runs -------------
-    const bool any_fd = __any_sync(FULL, skip_on_failed);              // some run of the group has a failed-dependency class
+    const bool any_fd = __any_sync(FULL, dc.skip_on_failed);           // some run of the group has a failed-dependency class
     const int my_fmt = fmt_of(ell, max_deg);
     const int fmt0 = __shfl_sync(FULL, live ? my_fmt : -1, __ffs(__ballot_sync(FULL, live) | 0x80000000u) - 1);  // format of the first live run
     const bool mixed = __any_sync(FULL, live && my_fmt != fmt0);
@@ -578,46 +484,22 @@ __global__ void __launch_bounds__(32 * PACK_MAX_WARPS, PACK_MIN_BLOCKS) frontier
       if (any_fd) walk_items<FMT_CSRL, true>(lane, CAND, lg, wctx, met_w, fd_w);
       else walk_items<FMT_CSRL, false>(lane, CAND, lg, wctx, met_w, fd_w);
     }
-    met_w |= FREE;
+    met_w |= dc.FREE;
     load_cut(t + NG, 0u);   // the phase words and masks for the cut of the group I shall issue (issue() reduces them)
     uint32_t ready_w = met_w, skipc_w = 0, fail_w = 0;
     if (CD) {
-      ready_w = met_w & ~c0 & ~c1;   // BF_COND_PASS
-      skipc_w = met_w & c0 & ~c1;    // BF_COND_SKIP
-      fail_w = met_w & c0 & c1;      // BF_COND_FAIL
-      if (__any_sync(FULL, fail_w != 0)) {
-        // a step set Failed inside the loop is visible to LATER steps of the list only (dag.go:2745, :497)
-        const uint32_t fclass = allow_failed ? 0u : (skip_on_failed ? 3u : 1u);
-        const uint32_t wmask = (1u << lg) - 1u;
-        for (uint32_t round = 0; round <= 32u * Wmax; ++round) {
-          __syncwarp();
-          sts_u32(mfail_a + lane * 4u, fail_w);
-          __syncwarp();
-          met_w = 0; fd_w = 0;
-          for (uint32_t todo = __ballot_sync(FULL, CAND != 0); todo; todo &= todo - 1) {
-            const uint32_t L = __ffs(todo) - 1;
-            const uint4 te = lds_v4(tab_a + (L >> lg) * 16u);
-            uint32_t mb, fb;
-            fixup_item(lane, __shfl_sync(FULL, CAND, L), L & wmask, te.w >> 16, te.y, te.x, te.z, mfail_a + ((L >> lg) << lg) * 4u,
-                       __shfl_sync(FULL, fclass, L), mb, fb);
-            if (lane == L) { met_w = mb; fd_w = fb; }
-          }
-          met_w |= FREE;
-          const uint32_t nf = met_w & c0 & c1;
-          const bool same = !__any_sync(FULL, nf != fail_w);
-          fail_w = nf;
-          if (same) break;
-        }
-        ready_w = met_w & ~c0 & ~c1;
-        skipc_w = met_w & c0 & ~c1;
-      }
-      pset<BF_PHASE_FAILED>(fail_w, p0, p1, p2, p3);  // dag.go:2745-2747, 2810-2812
+      // item L: word L & (Wq - 1) of run L >> lg, its rows and status bytes from the run's walk-table entry
+      auto fixup = [&](uint32_t L, uint32_t candw, uint32_t fclass, uint32_t& mb, uint32_t& fb) {
+        const uint4 te = lds_v4(tab_a + (L >> lg) * 16u);
+        fixup_item(lane, candw, L & ((1u << lg) - 1u), te.w >> 16, te.y, te.x, te.z, mfail_a + ((L >> lg) << lg) * 4u, fclass, mb, fb);
+      };
+      stage_cond(lane, c0, c1, dc, mfail_a, true, 32u * Wmax, fixup, met_w, fd_w, ready_w, skipc_w, fail_w, p0, p1, p2, p3);
     }
     const uint32_t acc_ready = ready_w, acc_skip = fd_w | skipc_w;
 
     // ---------------- stage E: result records ----------------
     const uint32_t cnt = __reduce_add_sync(gmask, (uint32_t)__popc(acc_ready) | ((uint32_t)__popc(acc_skip) << 16));
-    bool changed = marked;
+    bool changed = rc.marked;   // with cond / decision codes: stage G may write the code a step already has
     if (CD) changed = (__ballot_sync(FULL, ((p0 ^ q0) | (p1 ^ q1) | (p2 ^ q2) | (p3 ^ q3)) != 0) & gmask) != 0;
     // fused compaction head (compact.cu): events of the run = steps with a bit in any result mask the layout carries
     uint32_t n_events = 0;
@@ -642,21 +524,7 @@ __global__ void __launch_bounds__(32 * PACK_MAX_WARPS, PACK_MIN_BLOCKS) frontier
           if (live && n_events) atomicAdd(&P.head_sums[r >> 9], (unsigned long long)n_events);
         }
       }
-      if (w < Wmax) {
-        reinterpret_cast<uint32_t*>(rr + P.off_ready)[w] = acc_ready;
-        reinterpret_cast<uint32_t*>(rr + P.off_skip)[w] = acc_skip;
-        if (XO) {
-          if (P.off_fail != BF_OFF_NONE) reinterpret_cast<uint32_t*>(rr + P.off_fail)[w] = fail_w;
-          if (P.off_needs_cond != BF_OFF_NONE) reinterpret_cast<uint32_t*>(rr + P.off_needs_cond)[w] = realtime ? 0u : (met_w & HASIF);
-          if (P.off_skip_dep != BF_OFF_NONE) reinterpret_cast<uint32_t*>(rr + P.off_skip_dep)[w] = fd_w;
-          if (P.off_phase_out != BF_OFF_NONE) {
-            uint32_t* po = reinterpret_cast<uint32_t*>(rr + P.off_phase_out) + w;
-            po[0] = p0; po[Wmax] = p1; po[2 * Wmax] = p2; po[3 * Wmax] = p3;
-          }
-        }
-      }
-      if (P.result_tail != P.result_stride)
-        for (uint32_t x = P.result_tail / 4 + w; x < P.result_stride / 4; x += Wq) reinterpret_cast<uint32_t*>(rr)[x] = 0u;
+      store_words<XO>(P, rr, w, Wq, acc_ready, acc_skip, fail_w, realtime ? 0u : (met_w & HASIF), fd_w, p0, p1, p2, p3);
     }
     lane_ready += (uint32_t)__popc(acc_ready);
     lane_skip += (uint32_t)__popc(acc_skip);
@@ -718,14 +586,6 @@ __global__ void __launch_bounds__(32 * PACK_MAX_WARPS, PACK_MIN_BLOCKS) frontier
 #endif
 }
 
-typedef void (*PackFn)(const KParams);
-static PackFn pick_pack(const KParams& P) {
-  const bool cd = P.off_cond != BF_OFF_NONE || P.off_decision != BF_OFF_NONE;
-  const bool xo = P.off_fail != BF_OFF_NONE || P.off_needs_cond != BF_OFF_NONE || P.off_skip_dep != BF_OFF_NONE ||
-                  P.off_phase_out != BF_OFF_NONE;
-  if (cd) return xo ? frontier_pack_kernel<true, true> : frontier_pack_kernel<true, false>;
-  return xo ? frontier_pack_kernel<false, true> : frontier_pack_kernel<false, false>;
-}
 
 uint32_t frontier_pack_max_warps() { return PACK_MAX_WARPS; }
 #ifdef PACK_TRACE
@@ -737,21 +597,11 @@ extern "C" int bf_debug_pack_trace(unsigned long long* out, unsigned int* launch
 #endif
 
 cudaError_t launch_frontier_pack(const KParams& P, uint32_t grid, uint32_t smem_bytes, cudaStream_t stream) {
-  PackFn fn = pick_pack(P);
-  static PackFn configured[8][4] = {};
-  int dev = 0;
-  cudaError_t e = cudaGetDevice(&dev);
+  static const KernelFn table[4] = {frontier_pack_kernel<false, false>, frontier_pack_kernel<false, true>,
+                                    frontier_pack_kernel<true, false>, frontier_pack_kernel<true, true>};
+  const KernelFn fn = table[variant_bits(P)];
+  const cudaError_t e = allow_max_smem(fn);
   if (e != cudaSuccess) return e;
-  bool known = false;
-  if (dev >= 0 && dev < 8)
-    for (int i = 0; i < 4; ++i) known = known || configured[dev][i] == fn;
-  if (!known) {
-    e = cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
-    if (e != cudaSuccess) return e;
-    if (dev >= 0 && dev < 8)
-      for (int i = 0; i < 4; ++i)
-        if (configured[dev][i] == nullptr) { configured[dev][i] = fn; break; }
-  }
   if (P.flags & BF_EVAL_PIPELINED) {   // programmatic dependent launch: may start while the preceding kernel drains
     cudaLaunchConfig_t cfg{};
     cfg.gridDim = dim3(grid); cfg.blockDim = dim3(P.warps_per_block * 32); cfg.dynamicSmemBytes = smem_bytes; cfg.stream = stream;
