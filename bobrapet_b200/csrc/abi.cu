@@ -136,8 +136,9 @@ struct bf_ctx {
   // counter and the listed-runs total), so the steady-state tick carries no memset launches; a failed call marks it dirty
   bool rejected_clean = false, cblock_clean = false;
 
-  // cached shared-memory plan (recomputed when the layout or the largest record changes)
+  // cached shared-memory plan (recomputed when the layout, the largest record or a launch-shape knob changes)
   uint32_t plan_key_stride = 0, plan_key_words = 0, plan_key_rec = 0, plan_key_variant = 0xFFFFFFFFu;
+  int plan_key_knobs[3] = {0, 0, 0};   // BF_STAGES, BF_WARPS, BF_BLOCKS_PER_SM as last planned (0: unset)
   uint32_t plan_stages = 0, plan_wpb = 0, plan_per_sm = 0, plan_occ2 = 0;
 
   bf_stats stats{};
@@ -546,6 +547,7 @@ int run_pass(bf_ctx* c, const bf_batch& b, const uint8_t* d_state, uint8_t* d_re
     };
     while (nw > 1 && groups_for(nw) < nw) --nw;               // never more warps than slot groups
     ng = groups_for(nw);
+    if (ng > 32u * nw) ng = 32u * nw;   // never more slot groups than threads: thread i sets up slot group i (frontier_pack.cu)
     if (const char* e = getenv("BF_GROUPS")) { const uint32_t v = (uint32_t)atoi(e); if (v >= nw && v <= ng) ng = v; }
     if (ng < kMinGroups || ng < nw) pack = false;   // records too large for a useful ring: one run per warp instead
     else {
@@ -570,16 +572,19 @@ int run_pass(bf_ctx* c, const bf_batch& b, const uint8_t* d_state, uint8_t* d_re
     bf::KParams PG = P;
     PG.work_bytes = work_general;
     const uint32_t variant = (b.flags & BF_EVAL_FIXPOINT) | (P.any_parallel << 8) | ((two_tier ? 1u : 0u) << 9) | (L.fields << 16);
+    // the shape knobs are read on every pass and are part of the plan key: a changed knob re-plans on the same ctx
+    const char* env_st = getenv("BF_STAGES");
+    const char* env_w = getenv("BF_WARPS");
+    const char* env_b = getenv("BF_BLOCKS_PER_SM");
+    const int knobs[3] = {env_st ? atoi(env_st) : 0, env_w ? atoi(env_w) : 0, env_b ? atoi(env_b) : 0};
     if (c->plan_wpb == 0 || c->plan_key_stride != L.state_stride || c->plan_key_words != L.words ||
-        c->plan_key_rec != batch_rec_bytes || c->plan_key_variant != variant) {
+        c->plan_key_rec != batch_rec_bytes || c->plan_key_variant != variant ||
+        memcmp(c->plan_key_knobs, knobs, sizeof knobs) != 0) {
       // Plan: as many resident warps per SM as registers / shared memory allow — the pass is latency/issue bound
       // before it is HBM bound — then ring depth: >= 2 stages keep the next trip's TMA copies in flight under the
       // current evaluation.
       uint32_t best_st = 0, best_wpb = 0, best_score = 0, best_occ2 = 0;
       int best_ctas = 1;
-      const char* env_st = getenv("BF_STAGES");
-      const char* env_w = getenv("BF_WARPS");
-      const char* env_b = getenv("BF_BLOCKS_PER_SM");
       for (uint32_t st = 1; st <= 4; ++st) {
         if (env_st && (uint32_t)atoi(env_st) != st) continue;
         for (uint32_t wpb = 24; wpb >= 1; wpb = (wpb > 4 ? wpb - 4 : wpb - 1)) {   // 24 / 20: the 80-register build (frontier_kernel.cu)
@@ -602,6 +607,7 @@ int run_pass(bf_ctx* c, const bf_batch& b, const uint8_t* d_state, uint8_t* d_re
       c->plan_stages = best_st; c->plan_wpb = best_wpb; c->plan_per_sm = (uint32_t)best_ctas; c->plan_occ2 = best_occ2;
       c->plan_key_stride = L.state_stride; c->plan_key_words = L.words; c->plan_key_rec = batch_rec_bytes;
       c->plan_key_variant = variant;
+      memcpy(c->plan_key_knobs, knobs, sizeof knobs);
     }
     g_st = c->plan_stages; g_wpb = c->plan_wpb; g_occ2 = c->plan_occ2; g_per_sm = (int)c->plan_per_sm;
   }

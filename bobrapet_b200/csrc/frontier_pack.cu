@@ -218,7 +218,7 @@ __global__ void __launch_bounds__(32 * PACK_MAX_WARPS, PACK_MIN_BLOCKS) frontier
   const uint32_t tab_a = mfail_a + 128u;
 
   if (threadIdx.x < 5) blk_counts[threadIdx.x] = 0ull;   // four counters + the group ticket
-  if (threadIdx.x < NG) {
+  if (threadIdx.x < NG) {   // NG <= blockDim.x: the planner (abi.cu) gives a CTA no more slot groups than threads
     mbar_init(bars + 8u * threadIdx.x, R);
     sts_u32(armed_a + 4u * threadIdx.x, 0u);
     fence_barrier_init();

@@ -79,8 +79,14 @@ def child_layout(ts: TopologySet):
 
 
 def random_state(rng: np.random.Generator, ts: TopologySet, slots: np.ndarray, n_runs: int, fields: int,
-                 phase_mix: str = "any", fail_codes: bool = True, run_flag_mix: bool = True):
-    """-> (layout, state records, topo index per run).  `slots[t]` is the slot of topology t."""
+                 phase_mix: str = "any", fail_codes: bool = True, run_flag_mix: bool = True,
+                 reserved: float = 0.0, padding: bool = False, fail_fast=None):
+    """-> (layout, state records, topo index per run).  `slots[t]` is the slot of topology t.
+
+    Records no well-behaved producer writes, which the kernels must read exactly as their `cleaned` twin:
+    reserved: the rate at which phase codes below S and child nibbles are replaced by the reserved code 15;
+    padding: random phase, cond and decision codes in the steps from a run's S up to the layout width (32 * words).
+    fail_fast: True / False sets RF_FAIL_FAST on every run instead of the random mix."""
     cfs, child_max = child_layout(ts)
     if child_max:
         fields |= A.F_CHILD
@@ -110,9 +116,46 @@ def random_state(rng: np.random.Generator, ts: TopologySet, slots: np.ndarray, n
         hg = rng.random(n_runs) < 0.2
         rflags |= hg.astype(np.uint8) * A.RF_HOST_GROUP
         rflags |= (hg * rng.integers(0, 4, size=n_runs)).astype(np.uint8) << A.RF_HOST_GROUP_SHIFT
+    if fail_fast is not None:
+        rflags = (rflags & ~np.uint8(A.RF_FAIL_FAST)) | (np.uint8(A.RF_FAIL_FAST) if fail_fast else np.uint8(0))
     # zero the codes beyond each run's own S (padding must not matter, but keep records canonical)
     Srun = ts.S[topo].astype(np.int64)[:, None]
     pad = np.arange(s_max)[None, :] >= Srun
     phase[pad] = 0; cond[pad] = 0; dec[pad] = 0
+    if reserved:   # drawn after every canonical field: the same seed gives the same run otherwise
+        phase[(rng.random(phase.shape) < reserved) & ~pad] = 15
+        child[rng.random(child.shape) < reserved] = 15
+    if padding:
+        width = 32 * L.words
+        wpad = np.arange(width)[None, :] >= Srun
+        wide = lambda a: np.concatenate([a, np.zeros((n_runs, width - s_max), np.uint8)], axis=1)  # noqa: E731
+        phase, cond, dec = wide(phase), wide(cond), wide(dec)
+        phase[wpad] = rng.integers(0, 16, size=int(wpad.sum()), dtype=np.uint8)
+        cond[wpad] = rng.integers(0, 4, size=int(wpad.sum()), dtype=np.uint8)
+        dec[wpad] = rng.integers(0, 4, size=int(wpad.sum()), dtype=np.uint8)
     state = pack_state(L, np.asarray(slots)[topo], rflags, phase, cond, dec, child if child_max else None, reg)
     return L, state, topo
+
+
+def cleaned(L, state: np.ndarray, ts: TopologySet, topo: np.ndarray) -> np.ndarray:
+    """The canonical twin of a state batch: phase code 15 -> 0, child nibble 15 -> 0, and every phase / cond / decision
+    code at or past a run's own S zeroed.  Every evaluator must give a record and its twin the same result."""
+    from bobrapet_b200.records import _pack_nibbles, _pack_planes, _unpack_planes
+    out = state.copy()
+    W = L.words
+    pad = np.arange(32 * W)[None, :] >= ts.S[topo].astype(np.int64)[:, None]
+    for off, nbits in ((L.off_phase, 4), (L.off_cond, 2), (L.off_decision, 2)):
+        if off == A.OFF_NONE:
+            continue
+        codes = _unpack_planes(out[:, off:off + nbits * W * 4], W, nbits, 32 * W)
+        codes[pad] = 0
+        if nbits == 4:
+            codes[codes == 15] = 0
+        out[:, off:off + nbits * W * 4] = _pack_planes(codes, W, nbits)
+    if L.off_child != A.OFF_NONE and L.child_nibbles:
+        nb = (L.child_nibbles + 1) // 2
+        raw = out[:, L.off_child:L.off_child + nb]
+        nib = np.stack([raw & 0xF, raw >> 4], axis=2).reshape(raw.shape[0], 2 * nb)
+        nib[nib == 15] = 0
+        out[:, L.off_child:L.off_child + nb] = _pack_nibbles(nib, nb)
+    return out

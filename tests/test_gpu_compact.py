@@ -6,7 +6,7 @@ import pytest
 
 from bobrapet_b200 import _abi as A
 from bobrapet_b200 import Frontier, synth
-from bobrapet_b200.records import make_layout
+from bobrapet_b200.records import make_layout, pack_state
 from oracle import packed as PK
 from tests import randgen
 
@@ -197,3 +197,64 @@ def test_fused_heads_ticks_of_different_sizes():
             batches[b] = (n, S, L, pt, h, want, live5)
     finally:
         f.close()
+
+
+def _no_deps_topology(S):
+    from bobrapet_b200.frontier import TopologySet
+    return TopologySet([S], [0], np.zeros(S + 1, np.uint32), np.zeros(0, np.uint16), np.zeros(S, np.uint8))
+
+
+@pytest.mark.parametrize("pattern", ["all-direct", "alternating"])
+def test_compact_direct_and_staged_blocks(fr, pattern):
+    """a 512-run block whose slice holds more than 8192 events writes it directly instead of staging it in shared memory:
+    S = 1024 steps without needs, all ready, in every block ("all-direct"), or in every other block with 1-2 events per run
+    between ("alternating": staged slices at odd and even bases).  Caps inside a direct slice and inside a staged slice that
+    starts at an odd base: only the first `cap` events are written, n_events still counts them all."""
+    S, n, CB = 1024, 4096, 512
+    slots = fr.put_topologies(_no_deps_topology(S))
+    ts = _no_deps_topology(S)
+    L = make_layout(S, 0, 0)
+    phase = np.zeros((n, S), np.uint8)
+    heavy = np.ones(n, bool) if pattern == "all-direct" else (np.arange(n) // CB) % 2 == 0
+    rng = np.random.default_rng(31)
+    for r in np.nonzero(~heavy)[0]:
+        phase[r, :] = 3                                      # Succeeded: no event
+        phase[r, rng.choice(S, size=(2 if r == CB else 1), replace=False)] = 0   # one ready step (two in run 512: an odd slice)
+    state = pack_state(L, np.full(n, slots[0], np.uint32), np.zeros(n, np.uint8), phase)
+    want, wcounts = PK.evaluate(PK.PackedTopologies(ts, slots), L, state, 0, 0, threads=8)
+    whead, wev, _ = PK.compact_events(L, want)
+    per_block = (whead >> A.HEAD_COUNT_SHIFT).reshape(-1, CB).sum(axis=1).astype(np.int64)
+    base = np.concatenate(([0], np.cumsum(per_block)))
+    direct = per_block > 8192
+    assert direct.all() if pattern == "all-direct" else (direct == heavy[::CB]).all()
+    assert _check(fr, ts, slots, L, state, want=want, wcounts=wcounts) == len(wev)
+    caps = [int(base[np.nonzero(direct)[0][-1]]) + 777]                        # inside a direct slice
+    if pattern == "alternating":
+        odd = [b for b in np.nonzero(~direct)[0] if base[b] % 2 == 1]
+        assert odd, base
+        caps += [int(base[odd[0]]) + 1, int(base[odd[0]]) + 2]                 # inside a staged slice at an odd base
+        caps += [int(base[1]) + 1]                                               # and at an even one
+    for cap in caps:
+        _check(fr, ts, slots, L, state, cap=cap, want=want, wcounts=wcounts)
+
+
+@pytest.mark.parametrize("max_iter", [1, 2, 3, "S+5"])
+def test_resident_tick_compact_iteration_cap(fr, max_iter):
+    """max_iterations reaches the fixpoint of a compact resident tick"""
+    rng = np.random.default_rng(950)
+    ts = randgen.random_topologies(rng, 40, 1, 200, max_deg=3, fill=0.5)
+    slots = fr.put_topologies(ts)
+    n = 3001
+    L, state, _ = randgen.random_state(rng, ts, slots, n, ALL, phase_mix="progress")
+    k = int(ts.S.max()) + 5 if max_iter == "S+5" else max_iter
+    h = fr.resident_create(L, n)
+    try:
+        fr.resident_upload(h, 0, state)
+        head, events, n_events, counts, _ = fr.resident_tick_compact(h, n, np.zeros(0, dtype=fr.DELTA_DTYPE), 2_000_000,
+                                                                      flags=A.EVAL_FIXPOINT, max_iterations=k)
+        want, wcounts = PK.evaluate(PK.PackedTopologies(ts, slots), L, state, A.EVAL_FIXPOINT, k, threads=8)
+        whead, wev, _ = PK.compact_events(L, want)
+        assert counts == wcounts and n_events == len(wev)
+        assert np.array_equal(head, whead) and np.array_equal(events, wev)
+    finally:
+        fr.resident_destroy(h)

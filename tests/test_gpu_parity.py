@@ -43,18 +43,23 @@ def kernel(request, monkeypatch):
     return k
 
 
-def _compare(fr, ts, slots, L, state, flags=0, max_iter=0, expansion=False):
+def _compare(fr, ts, slots, L, state, flags=0, max_iter=0, expansion=False, validate=True, cap=None):
+    """cap: the expansion capacity (default: room for every tuple); the kernel must keep the oracle's first `cap` tuples
+    and still report the full total.  validate=False for records with reserved codes, which the validation rejects."""
     pt = PK.PackedTopologies(ts, slots)
     want, wcounts = PK.evaluate(pt, L, state, flags, max_iter, threads=8)
+    vflag = A.EVAL_VALIDATE if validate else 0
     if expansion:
-        cap = int(wcounts["expansion"]) + 8
-        got, gcounts, gexp = fr.eval(L, state, flags=flags | A.EVAL_EXPANSION | A.EVAL_VALIDATE, max_iterations=max_iter,
+        if cap is None:
+            cap = int(wcounts["expansion"]) + 8
+        got, gcounts, gexp = fr.eval(L, state, flags=flags | A.EVAL_EXPANSION | vflag, max_iterations=max_iter,
                                      expansion_cap=cap)
         wexp, n = PK.expand(pt, L, state, want, cap)
         assert n == wcounts["expansion"] == gcounts["expansion"]
+        assert len(gexp) == len(wexp) == min(cap, n)
         assert np.array_equal(gexp, wexp), "expansion tuples differ"
     else:
-        got, gcounts = fr.eval(L, state, flags=flags | A.EVAL_VALIDATE, max_iterations=max_iter)
+        got, gcounts = fr.eval(L, state, flags=flags | vflag, max_iterations=max_iter)
     if not np.array_equal(got, want):
         bad = np.nonzero((got != want).any(axis=1))[0]
         r = int(bad[0])
@@ -92,21 +97,81 @@ def test_synthetic_configs(fr, kernel, cfg, n, S):
     assert out["ready"].any() or S < 3
 
 
+# "dirty": records no producer should write but the kernels must read exactly as the oracle does — the reserved phase /
+# child code 15 (read as 0) and random codes past each run's S (not read); EVAL_VALIDATE would reject them
+EDGES = {"clean": {}, "dirty": {"reserved": 0.05, "padding": True}}
+
+
 @pytest.mark.parametrize("seed", range(6))
 @pytest.mark.parametrize("mode", ["single", "fixpoint"])
 def test_random_adversarial(fr, seed, mode):
+    _random_adversarial(fr, seed, mode, "clean")
+
+
+@pytest.mark.parametrize("seed", range(6))
+@pytest.mark.parametrize("mode", ["single", "fixpoint"])
+def test_random_adversarial_dirty(fr, seed, mode):
+    _random_adversarial(fr, seed, mode, "dirty")
+
+
+def _random_adversarial(fr, seed, mode, edges):
     rng = np.random.default_rng(1000 + seed)
     smax = [40, 257, 1024, 96, 600, 33][seed]
     deg, fill = [(5, 0.0), (4, 0.9), (5, 0.0), (2, 0.9), (4, 0.85), (5, 0.0)][seed]
     ts = randgen.random_topologies(rng, 60, 1, smax, max_deg=deg, fill=fill)
     slots = fr.put_topologies(ts)
-    L, state, _ = randgen.random_state(rng, ts, slots, 4000, ALL, phase_mix=("any" if seed % 2 else "progress"))
-    _compare(fr, ts, slots, L, state, flags=(A.EVAL_FIXPOINT if mode == "fixpoint" else 0), expansion=True)
+    L, state, _ = randgen.random_state(rng, ts, slots, 4000, ALL, phase_mix=("any" if seed % 2 else "progress"), **EDGES[edges])
+    _compare(fr, ts, slots, L, state, flags=(A.EVAL_FIXPOINT if mode == "fixpoint" else 0), expansion=True,
+             validate=(edges == "clean"))
+
+
+@pytest.mark.parametrize("max_iter", [1, 2, 3, "S+5"])
+def test_fixpoint_iteration_cap(fr, max_iter):
+    """max_iterations caps the device fixpoint (the loop stops after k iterations, its launch effects kept)"""
+    rng = np.random.default_rng(1500)
+    ts = randgen.random_topologies(rng, 60, 1, 200, max_deg=3, fill=0.5)
+    slots = fr.put_topologies(ts)
+    L, state, _ = randgen.random_state(rng, ts, slots, 3000, ALL, phase_mix="progress")
+    k = int(ts.S.max()) + 5 if max_iter == "S+5" else max_iter
+    got = _compare(fr, ts, slots, L, state, flags=A.EVAL_FIXPOINT, max_iter=k, expansion=True)
+    iters = np.ascontiguousarray(got[:, 0:4]).view("<u4")[:, 0] >> A.SUM_ITER_SHIFT
+    assert (iters <= k).all()
+    if k <= 3:
+        assert (iters == k).any()   # some run was still progressing when the cap stopped it
+
+
+@pytest.mark.parametrize("which", ["zero", "one", "inside", "total-1", "total"])
+def test_expansion_cap(fr, which):
+    """a cap below the tuple count keeps the oracle's first `cap` tuples (run-major, step / branch order) and still
+    reports the full total in counts.expansion"""
+    rng = np.random.default_rng(1600)
+    ts = randgen.random_topologies(rng, 40, 5, 120, max_deg=3, fill=0.5, branch_choices=(3, 9, 33, 40))
+    slots = fr.put_topologies(ts)
+    L, state, _ = randgen.random_state(rng, ts, slots, 2000, ALL, phase_mix="progress")
+    pt = PK.PackedTopologies(ts, slots)
+    want, wc = PK.evaluate(pt, L, state, threads=8)
+    total = int(wc["expansion"])
+    assert total > 100
+    hdr = np.ascontiguousarray(want[:, 0:16]).view("<u4").reshape(-1, 4)
+    first = int(np.nonzero(hdr[:, 3] > 2)[0][0])                    # a run with a branch list of several tuples
+    inside = int(hdr[:first, 3].sum()) + 1                          # the cap ends inside that run's list
+    cap = {"zero": 0, "one": 1, "inside": inside, "total-1": total - 1, "total": total}[which]
+    _compare(fr, ts, slots, L, state, expansion=True, cap=cap)
 
 
 @pytest.mark.parametrize("seed", range(8))
 def test_random_adversarial_no_parallel(fr, kernel, seed):
     """all phase codes / groups / flags / FAIL codes, no parallel steps: the packed-lanes kernel's domain"""
+    _random_adversarial_no_parallel(fr, kernel, seed, "clean")
+
+
+@pytest.mark.parametrize("seed", range(8))
+def test_random_adversarial_no_parallel_dirty(fr, kernel, seed):
+    """the same batches with reserved codes and padding (EDGES)"""
+    _random_adversarial_no_parallel(fr, kernel, seed, "dirty")
+
+
+def _random_adversarial_no_parallel(fr, kernel, seed, edges):
     rng = np.random.default_rng(5000 + seed)
     smax = [40, 257, 1024, 96, 600, 33, 8, 130][seed]
     # seeds 0-2: sparse rows up to 5 needs (CSR, long rows); 3-5: dense rows of <= 4 (fixed-width 4); 6-7: dense <= 2
@@ -115,8 +180,8 @@ def test_random_adversarial_no_parallel(fr, kernel, seed):
     slots = fr.put_topologies(ts)
     n = [4000, 4001, 999, 4003, 1500, 4005, 4006, 4007][seed]
     L, state, _ = randgen.random_state(rng, ts, slots, n, ALL if seed % 3 else (A.F_COND | A.F_ALL_OUT),
-                                       phase_mix=("any" if seed % 2 else "progress"))
-    _compare(fr, ts, slots, L, state)
+                                       phase_mix=("any" if seed % 2 else "progress"), **EDGES[edges])
+    _compare(fr, ts, slots, L, state, validate=(edges == "clean"))
     st = fr.stats()
     # the ctx also holds topologies with parallel steps (earlier tests): packed lanes + deferred general; layouts wider
     # than 16 words (S > 512) always take the general kernel

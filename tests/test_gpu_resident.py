@@ -33,13 +33,28 @@ def _decode(L, state):
     return slots, rflags, phase, cond, dec, child, reg
 
 
+def _want_with_dead(pt, L, state, dead, flags, max_iter):
+    """oracle records of a batch whose runs in `dead` point at a dropped slot: the kernels mark such a run (summary all-ones,
+    empty record) and count nothing for it; every other run is independent of them"""
+    want = np.zeros((state.shape[0], L.result_stride), dtype=np.uint8)
+    live = np.nonzero(~dead)[0]
+    want[live], wcounts = PK.evaluate(pt, L, np.ascontiguousarray(state[live]), flags, max_iter, threads=8)
+    want[dead, 0:4] = 0xFF
+    return want, wcounts
+
+
 @pytest.mark.parametrize("seed", range(3))
 def test_deltas_equal_full_upload(seed):
+    """random deltas of every field, including indices in [S, 32 * words) (accepted: the bound is the layout width) and
+    DELTA_TOPO_SLOT re-pointing runs at a smaller topology (stale codes stay behind past its S), at one with parallel steps,
+    or at a dropped slot (the run is marked dead); fixpoint ticks with and without an iteration cap"""
     rng = np.random.default_rng(8800 + seed)
     fr = Frontier(0)
     try:
         ts = randgen.random_topologies(rng, 30, 1, [70, 300, 1000][seed])
         tslots = fr.put_topologies(ts)
+        dropped = int(fr.put_topologies(randgen.random_topologies(rng, 1, 1, 10))[0])
+        fr.drop_topology(dropped)
         n = 1500
         L, state, topo = randgen.random_state(rng, ts, tslots, n, ALL, phase_mix="progress")
         pt = PK.PackedTopologies(ts, tslots)
@@ -49,14 +64,21 @@ def test_deltas_equal_full_upload(seed):
         h = fr.resident_create(L, n + 7)
         fr.resident_upload(h, 0, state)
         S_run = ts.S[topo].astype(np.int64)
-        for tick in range(4):
+        S_of = {int(tslots[t]): int(ts.S[t]) for t in range(ts.count)}
+        with_par = [int(tslots[t]) for t in range(ts.count) if ts.P[t]]
+        dead = np.zeros(n, dtype=bool)
+        W32 = 32 * L.words
+        for tick in range(6):
             k = int(rng.integers(1, 4000))
             recs = {}
             for _ in range(k):
                 r = int(rng.integers(0, n))
-                f = int(rng.choice([A.DELTA_PHASE] * 6 + [A.DELTA_COND, A.DELTA_DECISION, A.DELTA_CHILD, A.DELTA_RUN_FLAGS, A.DELTA_REGISTERED]))
+                f = int(rng.choice([A.DELTA_PHASE] * 6 + [A.DELTA_COND, A.DELTA_DECISION, A.DELTA_CHILD, A.DELTA_RUN_FLAGS, A.DELTA_REGISTERED,
+                                                          A.DELTA_TOPO_SLOT]))
+                key = None
                 if f in (A.DELTA_PHASE, A.DELTA_COND, A.DELTA_DECISION):
-                    idx = int(rng.integers(0, S_run[r]))
+                    hi = W32 if (rng.random() < 0.2 and S_run[r] < W32) else S_run[r]   # past S: padding the kernels must not read
+                    idx = int(rng.integers(0, hi))
                     code = int(rng.integers(0, 15 if f == A.DELTA_PHASE else 4))
                 elif f == A.DELTA_CHILD:
                     if child is None:
@@ -64,30 +86,49 @@ def test_deltas_equal_full_upload(seed):
                     idx, code = int(rng.integers(0, L.child_nibbles)), int(rng.choice([0, 2, 3, 4, 13]))
                 elif f == A.DELTA_RUN_FLAGS:
                     idx, code = 0, int(rng.choice([0, A.RF_FAIL_FAST, A.RF_FAIL_FAST | A.RF_REALTIME, A.RF_TOPOLOGY_TERMINATED]))
+                elif f == A.DELTA_TOPO_SLOT:
+                    kind = rng.integers(0, 8)
+                    smaller = [s for s, S in S_of.items() if S < S_run[r]]
+                    if kind == 0:
+                        new = dropped
+                    elif kind <= 3 and smaller:
+                        new = int(rng.choice(smaller))
+                    elif kind <= 5 and with_par:
+                        new = int(rng.choice(with_par))
+                    else:
+                        new = int(rng.choice(tslots))
+                    idx, code, key = new & 0xFFFF, new >> 16, 0     # one slot delta per run and tick
                 else:
                     idx, code = int(rng.integers(0, 64)), int(rng.integers(0, 2))
-                recs[(r, f, idx)] = code          # the host coalesces: last value of the tick wins
+                recs[(r, f, idx if key is None else key)] = (idx, code)   # the host coalesces: last value of the tick wins
             d = np.zeros(len(recs), dtype=Frontier.DELTA_DTYPE)
-            for i, ((r, f, idx), code) in enumerate(recs.items()):
+            for i, ((r, f, _), (idx, code)) in enumerate(recs.items()):
                 d[i] = (r, idx, f, code)
                 if f == A.DELTA_PHASE: phase[r, idx] = code
                 elif f == A.DELTA_COND: cond[r, idx] = code
                 elif f == A.DELTA_DECISION: dec[r, idx] = code
                 elif f == A.DELTA_CHILD: child[r, idx] = code
                 elif f == A.DELTA_RUN_FLAGS: rflags[r] = code
+                elif f == A.DELTA_TOPO_SLOT:
+                    slots[r] = idx | (code << 16)
+                    dead[r] = slots[r] == dropped
+                    if not dead[r]:
+                        S_run[r] = S_of[int(slots[r])]
                 else: reg[r] = (int(reg[r]) & ~(1 << idx)) | (code << idx)
             flags = A.EVAL_FIXPOINT if tick % 2 else 0
+            max_iter = {1: 0, 3: 1, 5: 3}.get(tick, 0)
             dp = np.ascontiguousarray(d[rng.permutation(len(d))])
             want_state = pack_state(L, slots, rflags, phase, cond, dec, child, reg)
             if tick % 2:   # the fused call: deltas + pass + results, one synchronisation
-                got, gcounts = fr.resident_tick(h, L, n, dp, flags=flags)
+                got, gcounts = fr.resident_tick(h, L, n, dp, flags=flags, max_iterations=max_iter)
             else:
                 fr.resident_apply(h, dp)
                 got, gcounts = fr.resident_eval(h, L, n, flags=flags)
             assert np.array_equal(fr.resident_download(h, 0, n, L.state_stride), want_state), "tick %d: device copy differs" % tick
-            want, wcounts = PK.evaluate(pt, L, want_state, flags, 0, threads=8)
+            want, wcounts = _want_with_dead(pt, L, want_state, dead, flags, max_iter)
             assert np.array_equal(got, want), "tick %d" % tick
             assert gcounts == wcounts
+        assert dead.any() and (S_run < W32).any()
         # a delta outside the batch is rejected, the rest of the call still lands
         bad = np.zeros(2, dtype=Frontier.DELTA_DTYPE)
         bad[0] = (n + 1000, 0, A.DELTA_PHASE, 3)

@@ -145,6 +145,18 @@ def test_single_pass_object_vs_packed(seed):
 
 @pytest.mark.parametrize("seed", range(1000, 1250))
 def test_fixpoint_object_vs_packed(seed):
+    _fixpoint_object_vs_packed(seed, 0)
+
+
+@pytest.mark.parametrize("cap", [1, 2, 3, "S+5"])
+@pytest.mark.parametrize("seed", range(1000, 1250))
+def test_fixpoint_iteration_cap_object_vs_packed(seed, cap):
+    """max_iterations = cap: the object oracle's loop and the packed oracle's stop after the same iteration"""
+    _fixpoint_object_vs_packed(seed, cap)
+
+
+def _fixpoint_object_vs_packed(seed, cap):
+    """cap: the iteration limit (max_iterations), 0 = the default S + 1"""
     rng = random.Random(seed)
     story, codes = _rand_story(rng)
     if O.validate_runtime_dependency_graph(O.all_story_steps(story)) is not None:
@@ -157,13 +169,16 @@ def test_fixpoint_object_vs_packed(seed):
     ev, now = _evaluator(codes), 100.0
     L, state = P.pack_runs([story], [ps], [_clone_run(srun)], [0], [0], [step_runs], ev, {"inputs": {}, "steps": {}}, now)
     pt = PK.PackedTopologies(P.topology_set([ps]))
-    res, counts = PK.evaluate(pt, L, state, A.EVAL_FIXPOINT)
+    max_iter = ps.S + 5 if cap == "S+5" else cap
+    res, counts = PK.evaluate(pt, L, state, A.EVAL_FIXPOINT, max_iter)
     got = unpack_result(L, res, ps.S)
     names = ps.names
     pick = lambda key: [names[i] for i in np.nonzero(got[key][0])[0]]
 
     iters, launched, skipped, expansion, last = O.run_dag_iterations(srun, story, step_runs, ev, {"inputs": {}, "steps": {}},
-                                                                     now, device_contract=True)
+                                                                     now, max_iterations=(max_iter or None), device_contract=True)
+    if max_iter:
+        assert iters <= max_iter
     order = {n: i for i, n in enumerate(names)}
     srt = lambda xs: sorted(set(xs), key=order.get)
     assert pick("ready") == srt(launched)
@@ -175,3 +190,29 @@ def test_fixpoint_object_vs_packed(seed):
     assert n == len(set(expansion)) == int(got["n_expansion"][0])
     assert [(names[e["step"]], ps.par_branches[ps.par_steps.index(int(e["step"]))][int(e["branch"])]) for e in exp] == \
         sorted(set(expansion), key=lambda t: (order[t[0]], ps.par_branches[ps.par_steps.index(order[t[0]])].index(t[1])))
+
+
+@pytest.mark.parametrize("mode", ["single", "fixpoint"])
+@pytest.mark.parametrize("seed", range(4))
+def test_packed_reads_reserved_and_padding_as_clean(seed, mode):
+    """The reserved phase / child code 15 reads as 0, and codes at or past a run's own S are not read: the packed oracle
+    gives a batch full of both the same bytes as its cleaned twin.  The GPU cases with `reserved=` / `padding=` rely on it."""
+    from tests import randgen
+    rng = np.random.default_rng(7000 + seed)
+    smax = [40, 257, 96, 33][seed]
+    ts = randgen.random_topologies(rng, 30, 1, smax, max_deg=4, fill=0.5, branch_choices=(0, 3, 8, 9, 33, 300))
+    slots = np.arange(ts.count, dtype=np.uint32)
+    fields = A.F_COND | A.F_DECISION | A.F_ALL_OUT
+    L, dirty, topo = randgen.random_state(rng, ts, slots, 600, fields, phase_mix=("any" if seed % 2 else "progress"),
+                                          reserved=0.1, padding=True)
+    clean = randgen.cleaned(L, dirty, ts, topo)
+    assert not np.array_equal(dirty, clean)
+    flags = A.EVAL_FIXPOINT if mode == "fixpoint" else 0
+    pt = PK.PackedTopologies(ts, slots)
+    got, gc = PK.evaluate(pt, L, dirty, flags)
+    want, wc = PK.evaluate(pt, L, clean, flags)
+    assert np.array_equal(got, want) and gc == wc
+    assert np.array_equal(randgen.cleaned(L, clean, ts, topo), clean)
+    gexp, gn = PK.expand(pt, L, dirty, got, int(gc["expansion"]))
+    wexp, wn = PK.expand(pt, L, clean, want, int(wc["expansion"]))
+    assert gn == wn and np.array_equal(gexp, wexp)
