@@ -110,6 +110,12 @@ class CompactOut(C.Structure):
                 ("events_cap", C.c_uint64), ("n_events", C.c_uint64)]
 
 
+class TouchedOut(C.Structure):
+    _fields_ = [("struct_size", C.c_uint32), ("full", C.c_uint32), ("runs", C.c_void_p), ("head", C.c_void_p),
+                ("runs_cap", C.c_uint32), ("n_listed", C.c_uint32), ("n_evaluated", C.c_uint32), ("reserved", C.c_uint32),
+                ("events", C.c_void_p), ("events_cap", C.c_uint64), ("n_events", C.c_uint64)]
+
+
 class SchedTables(C.Structure):
     _fields_ = [("struct_size", C.c_uint32), ("n_stories", C.c_uint32), ("n_queues", C.c_uint32), ("global_limit", C.c_int32),
                 ("global_running_base", C.c_uint32), ("story_limit", C.c_void_p), ("story_running_base", C.c_void_p),
@@ -154,6 +160,7 @@ SYMBOLS = [
     ("bf_resident_download", C.c_int, [C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32, C.c_void_p]),
     ("bf_eval_compact", C.c_int, [C.c_void_p, C.POINTER(Batch), C.POINTER(CompactOut)]),
     ("bf_resident_tick_compact", C.c_int, [C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.POINTER(CompactOut), C.POINTER(Counts)]),
+    ("bf_resident_tick_touched", C.c_int, [C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.POINTER(TouchedOut), C.POINTER(Counts)]),
     ("bf_group_create", C.c_int, [C.POINTER(C.c_void_p), C.POINTER(C.c_int32), C.c_uint32, C.POINTER(Config)]),
     ("bf_group_destroy", None, [C.c_void_p]),
     ("bf_group_size", C.c_uint32, [C.c_void_p]),

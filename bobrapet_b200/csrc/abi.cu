@@ -11,6 +11,7 @@
 #include <string.h>
 
 #include <algorithm>
+#include <map>
 #include <mutex>
 #include <new>
 #include <thread>
@@ -29,6 +30,9 @@ cudaError_t launch_frontier_pack(const KParams& P, uint32_t grid, uint32_t smem_
 uint32_t frontier_pack_max_warps();
 cudaError_t launch_apply_deltas(const DeltaParams& P, cudaStream_t stream);
 cudaError_t launch_compact(const CompactParams& P, cudaStream_t stream);
+cudaError_t launch_touched_list(const TouchedParams& P, cudaStream_t stream);
+cudaError_t launch_touched_compact(const TouchedParams& P, cudaStream_t stream);
+cudaError_t launch_mark_runs(uint32_t* mark, uint32_t first, uint32_t n, uint32_t value, cudaStream_t stream);
 cudaError_t launch_move_records(const uint8_t* src, uint8_t* dst, const void* moves, uint32_t n, cudaStream_t stream);
 cudaError_t launch_schedule(const SchedParams& P, uint32_t sm_count, cudaStream_t stream, uint32_t phases = 3);
 cudaError_t launch_closure(const Slot* slots, const uint32_t* slot_ids, const uint32_t* starts, uint32_t n, uint32_t n_slots,
@@ -51,6 +55,20 @@ struct Resident {  // a device-resident batch (row f2)
   uint8_t* d_result_prev = nullptr;  // records of the pass before (changed-only compaction); allocated on first use
   bool prev_valid = false;           // d_result holds a pass over the current device state lineage
   uint32_t prev_runs = 0;            // ... over this many runs
+  // Touched ticks (bf_resident_tick_touched).  Every delta and upload raises its run's mark to epoch << 1 (| 1 = must list, by
+  // an upload); a full tick records the epoch it ended in full_epoch and opens the next one, so a mark at or below full_epoch
+  // is stale by comparison alone: a full tick clears nothing and adds no launch.  A touched tick evaluates the runs whose
+  // mark is newer than full_epoch and zeroes their marks itself (list-mode compaction, compact.cu).
+  uint32_t* d_mark = nullptr;        // [cap rounded up to 4]
+  uint32_t epoch = 1, full_epoch = 0;
+  uint32_t full_runs = 0;            // runs the last full tick evaluated
+  bool need_full = true;             // no tick yet, or a tick failed: the current records are not known to be complete
+  uint32_t last_fixpoint = 0, last_max_iter = 0;   // BF_EVAL_FIXPOINT and max_iterations of the last tick
+  uint64_t drops_seen = 0;           // bf_ctx::topo_drops at the last full tick
+  uint64_t pending = 0;              // bound on the touched runs: those the last touched tick left at or above its n_runs (its
+                                     // list build counts them), plus the deltas and uploaded runs since
+  std::map<uint32_t, uint32_t> uploaded;   // runs at or above full_runs uploaded since the last full tick: disjoint, merged
+                                           // [first, end) ranges keyed by first
 };
 
 struct TopoMeta {
@@ -92,6 +110,7 @@ struct bf_ctx {
   bool rec_max_dirty = false;          // a drop may have lowered the maxima: recomputed at the next plan
   uint32_t n_alive = 0;
   uint32_t n_with_parallel = 0;  // live topologies that have parallel steps
+  uint64_t topo_drops = 0;       // bf_topology_drop calls so far (a touched tick after one evaluates every run)
 
   // host-API staging
   uint8_t* d_state = nullptr; size_t d_state_cap = 0;
@@ -120,6 +139,14 @@ struct bf_ctx {
   unsigned long long* d_offsets = nullptr; size_t d_offsets_cap = 0;
   unsigned long long* d_block_sums = nullptr; size_t d_block_sums_cap = 0;
   uint32_t* d_defer = nullptr; size_t d_defer_cap = 0;  // [0] = count, [1..] = run ids
+  // touched ticks: [0] = list length, [1..] = the list | head word per list position | listed runs and their heads (when the
+  // caller's buffers are not pinned) | per-block sums
+  uint32_t* d_tlist = nullptr; size_t d_tlist_cap = 0;
+  uint32_t* d_tpos_head = nullptr; size_t d_tpos_head_cap = 0;
+  uint32_t* d_truns = nullptr; size_t d_truns_cap = 0;
+  uint32_t* d_thead = nullptr; size_t d_thead_cap = 0;
+  unsigned long long* d_tsums = nullptr; size_t d_tsums_cap = 0;
+  uint64_t last_touched_events = 0;   // events of the previous touched tick (sizes the first D2H)
 
   // limiters (bf_schedule): what the last bf_eval left on the device + scratch
   bool last_eval_valid = false;
@@ -136,10 +163,14 @@ struct bf_ctx {
   // counter and the listed-runs total), so the steady-state tick carries no memset launches; a failed call marks it dirty
   bool rejected_clean = false, cblock_clean = false;
 
-  // cached shared-memory plan (recomputed when the layout, the largest record or a launch-shape knob changes)
-  uint32_t plan_key_stride = 0, plan_key_words = 0, plan_key_rec = 0, plan_key_variant = 0xFFFFFFFFu;
-  int plan_key_knobs[3] = {0, 0, 0};   // BF_STAGES, BF_WARPS, BF_BLOCKS_PER_SM as last planned (0: unset)
-  uint32_t plan_stages = 0, plan_wpb = 0, plan_per_sm = 0, plan_occ2 = 0;
+  // cached shared-memory plans of the general kernel (recomputed when the layout, the largest record or a launch-shape knob
+  // changes): [0] for passes over whole batches, [1] for passes over a run list (touched ticks), so that a batch that mixes
+  // full and touched ticks keeps both
+  struct Plan {
+    uint32_t key_stride = 0, key_words = 0, key_rec = 0, key_variant = 0xFFFFFFFFu;
+    int key_knobs[3] = {0, 0, 0};   // BF_STAGES, BF_WARPS, BF_BLOCKS_PER_SM as last planned (0: unset)
+    uint32_t stages = 0, wpb = 0, per_sm = 0, occ2 = 0;
+  } plan[2];
 
   bf_stats stats{};
 };
@@ -455,8 +486,11 @@ int check_layout(bf_ctx* c, const bf_layout& L) {
 }
 
 // shared-memory plan + launch of one pass on device buffers
+// run_list (touched ticks): the pass takes the runs run_list[0 .. *run_list_count) (b.n_runs bounds the count) and writes
+// each run's record at its own index
 int run_pass(bf_ctx* c, const bf_batch& b, const uint8_t* d_state, uint8_t* d_result, bf_expansion* d_exp,
-             unsigned long long* d_counts, cudaStream_t stream) {
+             unsigned long long* d_counts, cudaStream_t stream, const uint32_t* run_list = nullptr,
+             const uint32_t* run_list_count = nullptr) {
   const bf_layout& L = b.layout;
   if (int rc = sync_slots(c, stream)) return rc;
   if (c->rec_max_dirty) {  // drops since the last plan: the largest live record per word count
@@ -572,14 +606,15 @@ int run_pass(bf_ctx* c, const bf_batch& b, const uint8_t* d_state, uint8_t* d_re
     bf::KParams PG = P;
     PG.work_bytes = work_general;
     const uint32_t variant = (b.flags & BF_EVAL_FIXPOINT) | (P.any_parallel << 8) | ((two_tier ? 1u : 0u) << 9) | (L.fields << 16);
+    bf_ctx::Plan& pl = c->plan[run_list ? 1 : 0];
     // the shape knobs are read on every pass and are part of the plan key: a changed knob re-plans on the same ctx
     const char* env_st = getenv("BF_STAGES");
     const char* env_w = getenv("BF_WARPS");
     const char* env_b = getenv("BF_BLOCKS_PER_SM");
     const int knobs[3] = {env_st ? atoi(env_st) : 0, env_w ? atoi(env_w) : 0, env_b ? atoi(env_b) : 0};
-    if (c->plan_wpb == 0 || c->plan_key_stride != L.state_stride || c->plan_key_words != L.words ||
-        c->plan_key_rec != batch_rec_bytes || c->plan_key_variant != variant ||
-        memcmp(c->plan_key_knobs, knobs, sizeof knobs) != 0) {
+    if (pl.wpb == 0 || pl.key_stride != L.state_stride || pl.key_words != L.words ||
+        pl.key_rec != batch_rec_bytes || pl.key_variant != variant ||
+        memcmp(pl.key_knobs, knobs, sizeof knobs) != 0) {
       // Plan: as many resident warps per SM as registers / shared memory allow — the pass is latency/issue bound
       // before it is HBM bound — then ring depth: >= 2 stages keep the next trip's TMA copies in flight under the
       // current evaluation.
@@ -589,7 +624,7 @@ int run_pass(bf_ctx* c, const bf_batch& b, const uint8_t* d_state, uint8_t* d_re
         if (env_st && (uint32_t)atoi(env_st) != st) continue;
         for (uint32_t wpb = 24; wpb >= 1; wpb = (wpb > 4 ? wpb - 4 : wpb - 1)) {   // 24 / 20: the 80-register build (frontier_kernel.cu)
           if (env_w && !pack && (uint32_t)atoi(env_w) != wpb) continue;
-          if (wpb > 16 && two_tier) continue;   // the run-list tier exists as the 16-warp build only
+          if (wpb > 16 && (two_tier || run_list)) continue;   // the run-list builds are the 16-warp build only
           const uint32_t smem_try = 128 + wpb * (st * P.stage_bytes + work_general + 64);
           if (smem_try > budget) continue;
           uint32_t occ2 = 0;
@@ -604,12 +639,12 @@ int run_pass(bf_ctx* c, const bf_batch& b, const uint8_t* d_state, uint8_t* d_re
         }
       }
       if (best_wpb == 0) return fail(c, BF_ETOPO, "topology record + run state do not fit shared memory");
-      c->plan_stages = best_st; c->plan_wpb = best_wpb; c->plan_per_sm = (uint32_t)best_ctas; c->plan_occ2 = best_occ2;
-      c->plan_key_stride = L.state_stride; c->plan_key_words = L.words; c->plan_key_rec = batch_rec_bytes;
-      c->plan_key_variant = variant;
-      memcpy(c->plan_key_knobs, knobs, sizeof knobs);
+      pl.stages = best_st; pl.wpb = best_wpb; pl.per_sm = (uint32_t)best_ctas; pl.occ2 = best_occ2;
+      pl.key_stride = L.state_stride; pl.key_words = L.words; pl.key_rec = batch_rec_bytes;
+      pl.key_variant = variant;
+      memcpy(pl.key_knobs, knobs, sizeof knobs);
     }
-    g_st = c->plan_stages; g_wpb = c->plan_wpb; g_occ2 = c->plan_occ2; g_per_sm = (int)c->plan_per_sm;
+    g_st = pl.stages; g_wpb = pl.wpb; g_occ2 = pl.occ2; g_per_sm = (int)pl.per_sm;
   }
   const uint32_t g_smem = 128 + g_wpb * (g_st * P.stage_bytes + work_general + 64);
 
@@ -620,7 +655,7 @@ int run_pass(bf_ctx* c, const bf_batch& b, const uint8_t* d_state, uint8_t* d_re
   if (counts_set && !counts_in_kernel) BF_CUDA(c, cudaMemsetAsync(P.counts, 0, sizeof(bf_counts), stream));
   P.acc = counts_in_kernel ? c->d_acc + 8 * (size_t)(c->acc_seq++ % bf_ctx::kAccSlots) : nullptr;
   c->fused_done = false;
-  if (c->fuse_head && pack && !two_tier && b.n_runs != 0) {   // a compact tick: the packed-lanes pass leaves heads + block totals itself
+  if (c->fuse_head && pack && !two_tier && !run_list && b.n_runs != 0) {   // a compact tick: the packed-lanes pass leaves heads + block totals itself
     P.head = c->fuse_head; P.head_sums = c->fuse_sums;
     c->fused_done = true;
   }
@@ -630,6 +665,7 @@ int run_pass(bf_ctx* c, const bf_batch& b, const uint8_t* d_state, uint8_t* d_re
   uint32_t grid = 0, smem = 0;
   if (pack) {
     P.wq = wq; P.wq_log2 = lg; P.warps_per_block = nw; P.slot_groups = ng; P.stages = 1;
+    P.run_list = run_list; P.run_list_count = run_list_count;
     if (two_tier) {
       if (int rc = ensure_dev(c, c->d_defer, c->d_defer_cap, (size_t)b.n_runs + 1)) return rc;
       P.defer_count = c->d_defer;
@@ -658,6 +694,10 @@ int run_pass(bf_ctx* c, const bf_batch& b, const uint8_t* d_state, uint8_t* d_re
     P.wq = 32u; P.wq_log2 = 5u; P.work_bytes = work_general;
     P.stages = g_st; P.warps_per_block = g_wpb; P.occ2 = g_occ2;
     grid = (uint32_t)c->sm_count * (uint32_t)g_per_sm;
+    if (run_list) {   // the 16-warp run-list build, one CTA per SM
+      P.run_list = run_list; P.run_list_count = run_list_count; P.occ2 = 0;
+      grid = (uint32_t)c->sm_count;
+    }
     const uint32_t need_blocks = (b.n_runs + g_wpb - 1) / g_wpb;
     if (grid > need_blocks) grid = need_blocks ? need_blocks : 1;
     smem = g_smem;
@@ -671,7 +711,7 @@ int run_pass(bf_ctx* c, const bf_batch& b, const uint8_t* d_state, uint8_t* d_re
     BF_CUDA(c, bf::launch_expansion(P, c->d_block_sums, c->d_offsets, d_exp, b.expansion_cap, stream, &nl));
     c->stats.kernel_launches += nl;
   }
-  c->stats.last_kernel = pack ? (two_tier ? 2u : 1u) : 0u; c->stats.last_runs_per_trip = pack ? R : 1u;
+  c->stats.last_kernel = (pack ? (two_tier ? 2u : 1u) : 0u) + (run_list ? 3u : 0u); c->stats.last_runs_per_trip = pack ? R : 1u;
   c->stats.last_grid = grid; c->stats.last_block = (pack ? nw : g_wpb) * 32; c->stats.last_smem_bytes = smem;
   c->stats.last_stages = pack ? ng : g_st;
   return BF_OK;
@@ -718,6 +758,14 @@ int compact_arena(bf_ctx* c, size_t incoming) {
   c->arena_compactions++;
   c->stats.kernel_launches += live.empty() ? 0 : 1;
   return BF_OK;
+}
+
+// the device address of a buffer in pinned host memory (bf_alloc_pinned, cudaHostAlloc / cudaHostRegister), else nullptr
+void* pinned_dev(const void* p) {
+  cudaPointerAttributes at{};
+  if (p && cudaPointerGetAttributes(&at, p) == cudaSuccess && at.type == cudaMemoryTypeHost && at.devicePointer) return at.devicePointer;
+  cudaGetLastError();   // an unregistered host pointer is not an error here
+  return nullptr;
 }
 
 // ---- compact results: masks -> heads + 16-bit events on the device, then two small D2H copies ----
@@ -768,21 +816,13 @@ int compact_enqueue(bf_ctx* c, const bf_layout& L, const uint8_t* d_result, cons
   // a head buffer in pinned host memory (bf_alloc_pinned, cudaHostAlloc / cudaHostRegister) gets the head words posted by the
   // kernel itself; any other buffer gets them by a download
   P.host_head = nullptr;
-  if (out->head && n_runs && !getenv("BF_NO_ZC_HEADS")) {
-    cudaPointerAttributes at{};
-    if (cudaPointerGetAttributes(&at, out->head) == cudaSuccess && at.type == cudaMemoryTypeHost && at.devicePointer)
-      P.host_head = static_cast<uint32_t*>(at.devicePointer);
-    else
-      cudaGetLastError();   // an unregistered host pointer is not an error here
-  }
+  if (out->head && n_runs && !getenv("BF_NO_ZC_HEADS")) P.host_head = static_cast<uint32_t*>(pinned_dev(out->head));
   bool events_posted = false;
   if (out->events && cap && !getenv("BF_NO_ZC_EVENTS")) {   // the event list likewise: posted by the emit kernel, no download
-    cudaPointerAttributes at{};
-    if (cudaPointerGetAttributes(&at, out->events) == cudaSuccess && at.type == cudaMemoryTypeHost && at.devicePointer) {
-      P.events = static_cast<uint16_t*>(at.devicePointer);
+    if (void* d = pinned_dev(out->events)) {
+      P.events = static_cast<uint16_t*>(d);
       events_posted = true;
-    } else
-      cudaGetLastError();
+    }
   }
   if (n_runs == 0) BF_CUDA(c, cudaStreamSynchronize(s));   // the empty case stores to the pinned block from the host
   c->cblock_clean = false;   // until the call has gone through (resident_tick_locked / eval_host set it again after the sync)
@@ -924,7 +964,7 @@ int bf_create(bf_ctx** out, const bf_config* cfg) {
   if (cudaSetDevice(dev) != cudaSuccess || cudaStreamCreateWithFlags(&c->stream, cudaStreamNonBlocking) != cudaSuccess ||
       cudaMalloc(&c->d_counts, sizeof(bf_counts)) != cudaSuccess ||
       cudaMalloc(&c->d_acc, bf_ctx::kAccSlots * 64) != cudaSuccess || cudaMemset(c->d_acc, 0, bf_ctx::kAccSlots * 64) != cudaSuccess ||
-      cudaHostAlloc(reinterpret_cast<void**>(&c->h_counts), 4 * sizeof(bf_counts), cudaHostAllocDefault) != cudaSuccess) {
+      cudaHostAlloc(reinterpret_cast<void**>(&c->h_counts), 5 * sizeof(bf_counts), cudaHostAllocDefault) != cudaSuccess) {
     cudaGetLastError();
     bf_destroy(c);  // releases whatever was created
     return BF_ECUDA;
@@ -1040,6 +1080,7 @@ int bf_topology_put_many_checked_on_device(bf_ctx* c, const bf_topology* topos, 
 static int drop_locked(bf_ctx* c, uint32_t slot) {
   if (slot >= c->meta.size() || !c->meta[slot].alive) return fail(c, BF_ETOPO, "drop of an unknown slot");
   c->meta[slot].alive = false;
+  c->topo_drops++;
   if (c->meta[slot].P) c->n_with_parallel--;
   c->slots_host[slot] = bf::Slot{0, 0, 0};
   memset(&c->ff_host[(size_t)slot * bf::FF_STRIDE], 0, bf::FF_STRIDE * sizeof(uint32_t));
@@ -1371,11 +1412,14 @@ int bf_resident_create(bf_ctx* c, const bf_layout* L, uint32_t capacity, uint32_
   BF_CUDA(c, cudaSetDevice(c->device));
   Resident r;
   r.L = *L; r.cap = capacity;
+  const size_t mark_bytes = ((size_t)capacity + 3) / 4 * 16;   // padded: the list build reads four marks at a time
   cudaError_t e = cudaMalloc(&r.d_state, (size_t)capacity * L->state_stride);
   if (e == cudaSuccess) e = cudaMalloc(&r.d_result, (size_t)capacity * L->result_stride);
+  if (e == cudaSuccess) e = cudaMalloc(&r.d_mark, mark_bytes);
   if (e == cudaSuccess) e = cudaMemsetAsync(r.d_state, 0, (size_t)capacity * L->state_stride, c->stream);
+  if (e == cudaSuccess) e = cudaMemsetAsync(r.d_mark, 0, mark_bytes, c->stream);
   if (e == cudaSuccess) e = cudaStreamSynchronize(c->stream);
-  if (e != cudaSuccess) { cudaFree(r.d_state); cudaFree(r.d_result); return fail(c, BF_ENOMEM, std::string("resident batch: ") + cudaGetErrorString(e)); }
+  if (e != cudaSuccess) { cudaFree(r.d_state); cudaFree(r.d_result); cudaFree(r.d_mark); return fail(c, BF_ENOMEM, std::string("resident batch: ") + cudaGetErrorString(e)); }
   r.alive = true;
   uint32_t h = 0;
   while (h < c->resident.size() && c->resident[h].alive) ++h;
@@ -1392,7 +1436,7 @@ int bf_resident_destroy(bf_ctx* c, uint32_t h) {
   BF_CUDA(c, cudaSetDevice(c->device));
   cudaStreamSynchronize(c->stream);
   if (c->last_state == r->d_state) c->last_eval_valid = false;
-  cudaFree(r->d_state); cudaFree(r->d_result); cudaFree(r->d_result_prev);
+  cudaFree(r->d_state); cudaFree(r->d_result); cudaFree(r->d_result_prev); cudaFree(r->d_mark);
   *r = Resident();
   return BF_OK;
 }
@@ -1408,6 +1452,22 @@ int bf_resident_upload(bf_ctx* c, uint32_t h, uint32_t first, uint32_t n, const 
   if (c->last_state == r->d_state) c->last_eval_valid = false;   // the evaluated snapshot is gone: bf_schedule must follow a new pass
   r->prev_valid = false;                                          // full records arrived: the next changed-only tick lists every run
   BF_CUDA(c, cudaMemcpyAsync(r->d_state + (size_t)first * r->L.state_stride, records, (size_t)n * r->L.state_stride, cudaMemcpyHostToDevice, c->stream));
+  BF_CUDA(c, bf::launch_mark_runs(r->d_mark, first, n, r->epoch << 1 | 1u, c->stream));   // touched and must be listed
+  c->stats.kernel_launches += 1;
+  r->pending += n;
+  {   // record the part at or above full_runs, merged with the ranges it touches
+    uint32_t lo = std::max(first, r->full_runs), hi = first + n;
+    if (lo < hi) {
+      auto it = r->uploaded.upper_bound(lo);
+      if (it != r->uploaded.begin() && std::prev(it)->second >= lo) {
+        --it;
+        lo = it->first; hi = std::max(hi, it->second);
+        it = r->uploaded.erase(it);
+      }
+      while (it != r->uploaded.end() && it->first <= hi) { hi = std::max(hi, it->second); it = r->uploaded.erase(it); }
+      r->uploaded.emplace(lo, hi);
+    }
+  }
   BF_CUDA(c, cudaStreamSynchronize(c->stream));
   return BF_OK;
 }
@@ -1438,12 +1498,10 @@ static int resident_apply_async(bf_ctx* c, Resident* r, const bf_delta* deltas, 
   const bf_delta* d_src = c->d_deltas;
   bool direct = false;
   if (!getenv("BF_NO_ZC_DELTAS")) {
-    cudaPointerAttributes at{};
-    if (cudaPointerGetAttributes(&at, deltas) == cudaSuccess && at.type == cudaMemoryTypeHost && at.devicePointer) {
-      d_src = static_cast<const bf_delta*>(at.devicePointer);
+    if (void* d = pinned_dev(deltas)) {
+      d_src = static_cast<const bf_delta*>(d);
       direct = true;
-    } else
-      cudaGetLastError();
+    }
   }
   if (!direct) BF_CUDA(c, cudaMemcpyAsync(c->d_deltas, deltas, (size_t)n * sizeof(bf_delta), cudaMemcpyHostToDevice, s));
   bf::DeltaParams P{};
@@ -1451,6 +1509,7 @@ static int resident_apply_async(bf_ctx* c, Resident* r, const bf_delta* deltas, 
   P.words = r->L.words; P.state_stride = r->L.state_stride; P.off_phase = r->L.off_phase; P.off_cond = r->L.off_cond;
   P.off_decision = r->L.off_decision; P.off_child = r->L.off_child; P.child_nibbles = r->L.child_nibbles;
   P.rejected = c->d_rejected;
+  P.mark = r->d_mark; P.mark_value = r->epoch << 1;
   BF_CUDA(c, bf::launch_apply_deltas(P, s));
   c->stats.kernel_launches += 1;
   return BF_OK;
@@ -1465,6 +1524,7 @@ int bf_resident_apply(bf_ctx* c, uint32_t h, const bf_delta* deltas, uint32_t n)
   if (n == 0) return BF_OK;
   BF_CUDA(c, cudaSetDevice(c->device));
   if (c->last_state == r->d_state) c->last_eval_valid = false;
+  r->pending += n;
   const int rc = resident_apply_async(c, r, deltas, n);
   cudaError_t e = rc == BF_OK ? cudaMemcpyAsync(c->h_counts, c->d_rejected, 4, cudaMemcpyDeviceToHost, c->stream) : cudaSuccess;
   const cudaError_t es = cudaStreamSynchronize(c->stream);  // the caller's delta buffer may be reused after return
@@ -1555,6 +1615,7 @@ static int resident_tick_locked(bf_ctx* c, Resident* r, const bf_delta* deltas, 
     if (es == cudaSuccess) es = e2;
   }
   r->prev_valid = false;
+  r->need_full = true;
   if (rc != BF_OK || es != cudaSuccess) {   // whatever the kernels left in the self-cleaning scratch is unknown: zero it before the next use
     c->cblock_clean = false; c->rejected_clean = false;
     c->fuse_head = nullptr; c->fuse_sums = nullptr;
@@ -1562,6 +1623,15 @@ static int resident_tick_locked(bf_ctx* c, Resident* r, const bf_delta* deltas, 
   if (rc != BF_OK) return rc;
   if (es != cudaSuccess) return cuda_fail(c, es, "cudaStreamSynchronize");
   r->prev_valid = true; r->prev_runs = n_runs;
+  // a full evaluation: it ends the current touch epoch (touched ticks, above Resident)
+  r->need_full = false;
+  r->full_epoch = r->epoch++; r->full_runs = n_runs;
+  r->last_fixpoint = flags & BF_EVAL_FIXPOINT; r->last_max_iter = max_iterations; r->drops_seen = c->topo_drops;
+  r->pending = 0; r->uploaded.clear();
+  if (r->epoch >= 0x7FFFFFFFu) {   // the epoch must fit mark >> 1: once per 2^31 full ticks the marks start over
+    BF_CUDA(c, cudaMemsetAsync(r->d_mark, 0, ((size_t)r->cap + 3) / 4 * 16, s));
+    r->epoch = 1; r->full_epoch = 0;
+  }
   if (co) {
     c->cblock_clean = true; c->rejected_clean = true;   // the compaction's tail block delivered and cleared both
     const unsigned long long* tail = reinterpret_cast<const unsigned long long*>(c->h_counts + 2);
@@ -1603,6 +1673,143 @@ int bf_resident_tick_compact(bf_ctx* c, uint32_t h, const bf_delta* deltas, uint
   Resident* r = resident_of(c, h);
   if (!r) return fail(c, BF_EINVAL, "unknown resident batch");
   return resident_tick_locked(c, r, deltas, n_deltas, n_runs, flags, max_iterations, nullptr, counts, out);
+}
+
+// Were all runs of [lo, hi) uploaded since the last full tick?  (The ranges are merged: one of them must hold all of it.)
+static bool uploads_cover(const std::map<uint32_t, uint32_t>& ranges, uint32_t lo, uint32_t hi) {
+  auto it = ranges.upper_bound(lo);
+  if (it == ranges.begin()) return false;
+  --it;
+  return it->first <= lo && it->second >= hi;
+}
+
+// A touched tick: scatter -> list build -> pass over the list (into the second result buffer) -> list-mode compaction, which
+// brings the current result records up to date.  Falls back to a full compact tick where the baseline rules require one.
+static int touched_tick_locked(bf_ctx* c, Resident* r, const bf_delta* deltas, uint32_t n_deltas, uint32_t n_runs, uint32_t flags,
+                               uint32_t max_iterations, bf_touched_out* out, bf_counts* counts) {
+  if (out->struct_size != sizeof(bf_touched_out)) return fail(c, BF_EINVAL, "bad bf_touched_out.struct_size");
+  if (flags & ~(uint32_t)(BF_EVAL_FIXPOINT | BF_EVAL_NO_COUNTS)) return fail(c, BF_EINVAL, "touched ticks take BF_EVAL_FIXPOINT and BF_EVAL_NO_COUNTS only");
+  if (out->runs_cap && (!out->runs || !out->head)) return fail(c, BF_EINVAL, "null runs / head with a non-zero runs_cap");
+  if (out->events_cap && !out->events) return fail(c, BF_EINVAL, "null events with a non-zero events_cap");
+  if (n_runs > r->cap) return fail(c, BF_EINVAL, "n_runs exceeds the resident batch");
+  if (n_deltas && !deltas) return fail(c, BF_EINVAL, "null deltas");
+  BF_CUDA(c, cudaSetDevice(c->device));
+  const bool full = r->need_full || c->topo_drops != r->drops_seen || (flags & BF_EVAL_FIXPOINT) != r->last_fixpoint ||
+                    max_iterations != r->last_max_iter || r->epoch >= 0x7FFFFFFEu ||
+                    (n_runs > r->full_runs && !uploads_cover(r->uploaded, r->full_runs, n_runs));
+  if (full) {   // a plain compact tick: every run evaluated and listed, heads in run order
+    bf_compact_out co{};
+    co.struct_size = sizeof co; co.events = out->events; co.events_cap = out->events_cap;
+    const int rc = resident_tick_locked(c, r, deltas, n_deltas, n_runs, flags, max_iterations, nullptr, counts, &co);
+    if (!c->last_eval_valid || c->last_state != r->d_state) return rc;   // no results (rejected deltas alone still deliver them)
+    const uint32_t n = std::min(n_runs, out->runs_cap);
+    if (n) BF_CUDA(c, cudaMemcpy(out->head, c->d_head, (size_t)n * 4, cudaMemcpyDeviceToHost));
+    for (uint32_t i = 0; i < n; ++i) out->runs[i] = i;
+    out->full = 1; out->n_listed = n_runs; out->n_evaluated = n_runs; out->n_events = co.n_events;
+    return rc;
+  }
+
+  c->last_eval_valid = false;
+  cudaStream_t s = c->stream;
+  const bf_layout& L = r->L;
+  const uint32_t bound = (uint32_t)std::min<uint64_t>(n_runs, r->pending + n_deltas);   // >= the touched runs below n_runs
+  r->pending += n_deltas;
+  const uint64_t cap = out->events ? out->events_cap : 0;
+  const uint32_t runs_n = std::min(bound, out->runs_cap);
+  if (!r->d_result_prev) {
+    cudaError_t e = cudaMalloc(&r->d_result_prev, (size_t)r->cap * L.result_stride);
+    if (e != cudaSuccess) return fail(c, BF_ENOMEM, std::string("resident batch (second result buffer): ") + cudaGetErrorString(e));
+  }
+  const uint32_t nb = (bound + 511) / 512, nbl = (r->cap + 2047) / 2048;
+  if (int rc = ensure_dev(c, c->d_tlist, c->d_tlist_cap, (size_t)bound + 1)) return rc;
+  if (int rc = ensure_dev(c, c->d_tpos_head, c->d_tpos_head_cap, bound ? bound : 1)) return rc;
+  if (int rc = ensure_dev(c, c->d_tsums, c->d_tsums_cap, 2 * (size_t)nb + 2 * (size_t)nbl + 1)) return rc;
+  if (int rc = ensure_dev(c, c->d_events, c->d_events_cap, cap ? (size_t)cap : 1)) return rc;
+  // the caller's pinned buffers get the lists posted by the emit kernel, any other buffer gets them by a download
+  uint32_t* p_runs = static_cast<uint32_t*>(pinned_dev(out->runs));
+  uint32_t* p_head = static_cast<uint32_t*>(pinned_dev(out->head));
+  uint16_t* p_events = cap ? static_cast<uint16_t*>(pinned_dev(out->events)) : nullptr;
+  if (!p_runs || !p_head) {
+    if (int rc = ensure_dev(c, c->d_truns, c->d_truns_cap, runs_n ? runs_n : 1)) return rc;
+    if (int rc = ensure_dev(c, c->d_thead, c->d_thead_cap, runs_n ? runs_n : 1)) return rc;
+  }
+  unsigned long long* tail = reinterpret_cast<unsigned long long*>(c->h_counts + 2);   // 9 x u64 in the pinned block
+  uint64_t first_slice = 0;
+  auto body = [&]() -> int {
+    if (int rc = resident_apply_async(c, r, deltas, n_deltas)) return rc;
+    if (bound == 0) {   // nothing below n_runs can be touched: no launch beyond the scatter
+      if (n_deltas) BF_CUDA(c, cudaMemcpyAsync(tail + 5, c->d_rejected, 4, cudaMemcpyDeviceToHost, s));
+      return BF_OK;
+    }
+    bf::TouchedParams T{};
+    bf::CompactParams& P = T.C;
+    P.result = r->d_result_prev; P.prev_result = r->d_result;
+    P.events = p_events ? p_events : c->d_events; P.cap = cap;
+    P.host_tail = tail; P.counts = (flags & BF_EVAL_NO_COUNTS) ? nullptr : c->d_counts; P.rejected = c->d_rejected;
+    P.n_runs = bound; P.words = L.words; P.result_stride = L.result_stride; P.result_tail = result_tail_of(L);
+    P.off_ready = L.off_ready; P.off_skip = L.off_skip;
+    P.off_fail = L.off_fail; P.off_needs_cond = L.off_needs_cond; P.off_skip_dep = L.off_skip_dep;
+    T.mark = r->d_mark; T.full_epoch = r->full_epoch; T.n_scan = n_runs; T.n_marks = r->cap; T.bound = bound;
+    T.list = c->d_tlist + 1; T.list_count = c->d_tlist; T.pos_head = c->d_tpos_head;
+    T.sums = c->d_tsums; T.sums_listed = c->d_tsums + nb; T.scan_sums = c->d_tsums + 2 * (size_t)nb;
+    T.carry_sums = T.scan_sums + nbl;
+    T.out_runs = p_runs && p_head ? p_runs : c->d_truns; T.out_head = p_runs && p_head ? p_head : c->d_thead; T.runs_cap = runs_n;
+    c->rejected_clean = false;   // the emit kernel delivers and clears the counter; a failed call leaves it to be zeroed
+    BF_CUDA(c, bf::launch_touched_list(T, s));
+    bf_batch db{};
+    db.struct_size = sizeof(bf_batch);
+    db.flags = flags | BF_EVAL_COUNTS_SET; db.max_iterations = max_iterations; db.layout = L; db.n_runs = bound;
+    if (int rc = run_pass(c, db, r->d_state, r->d_result_prev, nullptr, c->d_counts, s, c->d_tlist + 1, c->d_tlist)) return rc;
+    BF_CUDA(c, bf::launch_touched_compact(T, s));
+    c->stats.kernel_launches += 4;
+    if (runs_n && !(p_runs && p_head)) {
+      BF_CUDA(c, cudaMemcpyAsync(out->runs, c->d_truns, (size_t)runs_n * 4, cudaMemcpyDeviceToHost, s));
+      BF_CUDA(c, cudaMemcpyAsync(out->head, c->d_thead, (size_t)runs_n * 4, cudaMemcpyDeviceToHost, s));
+    }
+    uint64_t guess = c->last_touched_events + c->last_touched_events / 32 + 1024;   // the previous touched tick's list + 3 %
+    if (guess > cap) guess = cap;
+    if (p_events) guess = 0;
+    if (guess) BF_CUDA(c, cudaMemcpyAsync(out->events, c->d_events, (size_t)guess * sizeof(uint16_t), cudaMemcpyDeviceToHost, s));
+    first_slice = p_events ? cap : guess;
+    return BF_OK;
+  };
+  const int rc = body();
+  const cudaError_t es = cudaStreamSynchronize(s);
+  if (rc != BF_OK || es != cudaSuccess) {   // marks and current records may be half updated: the next touched tick is a full one
+    r->need_full = true; c->rejected_clean = false;
+    if (rc != BF_OK) return rc;
+    return cuda_fail(c, es, "cudaStreamSynchronize");
+  }
+  bf_counts hc{};
+  uint64_t n_events = 0, listed = 0, evaluated = 0, rejected = 0;
+  if (bound == 0) {
+    rejected = n_deltas ? *reinterpret_cast<const uint32_t*>(tail + 5) : 0u;   // (the counter is zeroed before its next use)
+  } else {
+    n_events = tail[0]; memcpy(&hc, tail + 1, sizeof hc); rejected = tail[5]; listed = tail[6]; evaluated = tail[7];
+    r->pending = tail[8];       // every touched run below n_runs was evaluated: the ones above it are all that is left
+    c->rejected_clean = true;   // delivered and cleared by the emit kernel
+  }
+  const uint64_t have = std::min<uint64_t>(n_events, cap);
+  if (have > first_slice)
+    BF_CUDA(c, cudaMemcpy(out->events + first_slice, c->d_events + first_slice, (size_t)(have - first_slice) * sizeof(uint16_t),
+                          cudaMemcpyDeviceToHost));
+  c->last_touched_events = n_events;
+  out->full = 0; out->n_listed = (uint32_t)listed; out->n_evaluated = (uint32_t)evaluated; out->n_events = n_events;
+  if (counts) *counts = hc;
+  c->last_eval_valid = true; c->last_eval_runs = n_runs; c->last_eval_layout = L;
+  c->last_state = r->d_state; c->last_result = r->d_result;
+  if (rejected) return fail(c, BF_EINVAL, std::to_string(rejected) + " delta(s) outside the record (run, index, code or absent field); the others were applied and the pass ran");
+  return BF_OK;
+}
+
+int bf_resident_tick_touched(bf_ctx* c, uint32_t h, const bf_delta* deltas, uint32_t n_deltas, uint32_t n_runs, uint32_t flags,
+                             uint32_t max_iterations, bf_touched_out* out, bf_counts* counts) {
+  if (!c) return BF_EINVAL;
+  std::lock_guard<std::mutex> g(c->mu);
+  if (!out) return fail(c, BF_EINVAL, "null bf_touched_out");
+  Resident* r = resident_of(c, h);
+  if (!r) return fail(c, BF_EINVAL, "unknown resident batch");
+  return touched_tick_locked(c, r, deltas, n_deltas, n_runs, flags, max_iterations, out, counts);
 }
 
 int bf_alloc_pinned(bf_ctx* c, size_t bytes, void** out) {

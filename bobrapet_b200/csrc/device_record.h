@@ -168,6 +168,29 @@ struct CompactParams {
   uint32_t n_runs, words, result_stride, result_tail, off_ready, off_skip, off_fail, off_needs_cond, off_skip_dep;
 };
 
+// compact.cu, touched ticks (bf_resident_tick_touched, abi.cu): the list build in front of the pass and the list-mode compaction
+// behind it.  Every scratch array is written before it is read in the same tick (no self-cleaning needed).
+struct TouchedParams {
+  CompactParams C;               // result = the pass's new records (the batch's second buffer), prev_result = the batch's current
+                                 // records (brought up to date here); events, cap, host_tail, counts, rejected as for compact_emit;
+                                 // host_tail[7] = runs evaluated, [8] = touched runs in [n_scan, n_marks) (the list build)
+  uint32_t* mark;                // [n_marks rounded up to 4] touch marks: touched when mark >> 1 > full_epoch, bit 0 = must list
+  uint32_t full_epoch;
+  uint32_t n_scan;               // the list takes the touched runs of [0, n_scan)
+  uint32_t n_marks;              // the list build counts the touched runs of [n_scan, n_marks) too (they stay touched)
+  uint32_t bound;                // the host's bound on the list length: list capacity, grid of the compaction
+  uint32_t* list;                // [bound] touched runs, ascending
+  uint32_t* list_count;          // [1] their number
+  uint32_t* pos_head;            // [bound] head word per list position
+  unsigned long long* sums;      // [ceil(bound / 512)] events per compaction block
+  unsigned long long* sums_listed;  // [ceil(bound / 512)] listed runs per compaction block
+  unsigned long long* scan_sums; // [ceil(n_marks / 2048)] touched runs below n_scan per list-build block
+  unsigned long long* carry_sums;   // [ceil(n_marks / 2048)] touched runs at or above n_scan per list-build block
+  uint32_t* out_runs;            // [runs_cap] listed runs (device scratch or the caller's pinned buffer)
+  uint32_t* out_head;            // [runs_cap]
+  uint32_t runs_cap;
+};
+
 // resident.cu (row f2)
 struct DeltaParams {
   uint8_t* state;
@@ -175,6 +198,8 @@ struct DeltaParams {
   uint32_t n, n_runs;
   uint32_t words, state_stride, off_phase, off_cond, off_decision, off_child, child_nibbles;
   uint32_t* rejected;  // count of deltas outside the record (bad run / index / absent field)
+  uint32_t* mark;      // [n_runs] touch marks (abi.cu, touched ticks): every delta of a run in range raises its mark to mark_value
+  uint32_t mark_value;
 };
 
 // limiters.cu (rows a9 / f4)

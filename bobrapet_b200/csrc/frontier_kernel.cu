@@ -441,17 +441,25 @@ static KernelFn pick_kernel(uint32_t v) {
 // rb: the build (template parameter RB)
 static KernelFn kernel_for(const KParams& P, uint32_t rb) {
   uint32_t v = variant_bits(P);
-  if (P.run_list) {
-    // The run-list tier is the second launch of a two-tier pass (abi.cu), which the packed-lanes kernel takes first: a
-    // single pass (FX = 0) of a batch with some topology that has parallel steps (CH = 1), planned as the 16-warp build
-    // (RB = 0).  Only these four variants can run.
-    static const KernelFn list_table[4] = {
-        frontier_kernel<false, true, false, false, true, 0>, frontier_kernel<false, true, false, true, true, 0>,
-        frontier_kernel<true, true, false, false, true, 0>,  frontier_kernel<true, true, false, true, true, 0>};
-    return list_table[v];
-  }
   v |= (P.any_parallel != 0 ? 4u : 0u)            // CH: the join needs the child area; the expansion count needs only the descs
        | ((P.flags & BF_EVAL_FIXPOINT) ? 8u : 0u);  // FX
+  if (P.run_list) {
+    // Run lists reach this kernel in two ways, both planned as the 16-warp build (RB = 0, abi.cu):
+    //  - the second tier of a two-tier pass, after the packed-lanes kernel: a single pass (FX = 0) of a batch with some
+    //    topology that has parallel steps (CH = 1) — indices 4-7;
+    //  - a touched tick (bf_resident_tick_touched) that the packed-lanes kernel cannot take: S > 512, the device fixpoint or
+    //    BF_KERNEL=general, with or without parallel topologies — every index.
+    static const KernelFn list_table[16] = {
+        frontier_kernel<false, false, false, false, true, 0>, frontier_kernel<false, false, false, true, true, 0>,
+        frontier_kernel<true, false, false, false, true, 0>,  frontier_kernel<true, false, false, true, true, 0>,
+        frontier_kernel<false, true, false, false, true, 0>,  frontier_kernel<false, true, false, true, true, 0>,
+        frontier_kernel<true, true, false, false, true, 0>,   frontier_kernel<true, true, false, true, true, 0>,
+        frontier_kernel<false, false, true, false, true, 0>,  frontier_kernel<false, false, true, true, true, 0>,
+        frontier_kernel<true, false, true, false, true, 0>,   frontier_kernel<true, false, true, true, true, 0>,
+        frontier_kernel<false, true, true, false, true, 0>,   frontier_kernel<false, true, true, true, true, 0>,
+        frontier_kernel<true, true, true, false, true, 0>,    frontier_kernel<true, true, true, true, true, 0>};
+    return list_table[v];
+  }
   return rb == 2 ? pick_kernel<2>(v) : rb == 1 ? pick_kernel<1>(v) : pick_kernel<0>(v);
 }
 

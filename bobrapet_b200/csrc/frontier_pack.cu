@@ -175,7 +175,11 @@ DI void walk_items_any(uint32_t lane, uint32_t CAND, uint32_t lg, const WalkCtx&
 }
 
 // CD: cond and/or decision codes present   XO: any of fail/needs_cond/skip_dep/phase_out requested
-template <bool CD, bool XO>
+// LIST: run-list mode (touched ticks, abi.cu): group t takes the runs at list positions [t * R, t * R + R) of P.run_list, whose
+//       length the list build left at *P.run_list_count (P.n_runs is the host's bound on it).  The runs' state records are not
+//       adjacent, so the lane that owns a run copies its record itself; results go to each run's own index, and no fused head
+//       words are written.
+template <bool CD, bool XO, bool LIST>
 #ifndef PACK_MIN_BLOCKS
 #define PACK_MIN_BLOCKS 1   // resident CTAs per SM the build is compiled for (BF_PACK_CTAS experiments)
 #endif
@@ -227,7 +231,7 @@ __global__ void __launch_bounds__(32 * PACK_MAX_WARPS, PACK_MIN_BLOCKS) frontier
   __syncthreads();
 
   // ---- the CTA's groups: global group id = blockIdx.x + t * gridDim.x, runs R * gid .. R * gid + R - 1
-  const uint32_t N = P.n_runs;
+  const uint32_t N = LIST ? min(*reinterpret_cast<const volatile uint32_t*>(P.run_list_count), P.n_runs) : P.n_runs;
   const uint32_t n_groups = (N + R - 1) >> (5 - lg);
   const uint32_t T = blockIdx.x < n_groups ? (n_groups - blockIdx.x + gridDim.x - 1) / gridDim.x : 0;
   // Schedule: groups are CONSUMED in ticket order — a warp that is free takes the next group of the CTA from a shared
@@ -243,11 +247,14 @@ __global__ void __launch_bounds__(32 * PACK_MAX_WARPS, PACK_MIN_BLOCKS) frontier
   constexpr bool FF = !CD;   // the fail-fast skip of the cut below
   // A lane without a run keeps pf_sid all ones, so load_ent leaves its entry zero and issue() writes a dead marker.
   uint32_t pf_sid = 0xFFFFFFFFu, pf_rf = 0, pf_lo = 0, pf_hi = 0, pf_bytes = 0, pf_meta = 0;
+  uint32_t pf_run = 0xFFFFFFFFu;   // LIST: my run of the group I shall issue (all ones: none)
   auto load_sid = [&](uint32_t t, bool mine) {   // first link: my run's topology slot id and run flags (bf_run_header)
     pf_sid = 0xFFFFFFFFu; pf_rf = 0;
+    if (LIST) pf_run = 0xFFFFFFFFu;
     if (mine && t < T) {
-      const uint32_t r = ((blockIdx.x + t * gridDim.x) << (5 - lg)) + lr;
+      uint32_t r = ((blockIdx.x + t * gridDim.x) << (5 - lg)) + lr;
       if (r < N) {
+        if (LIST) { r = __ldg(P.run_list + r); pf_run = r; }
         const uint8_t* sr = P.state + (size_t)r * P.state_stride;
         const uint2 hv = __ldg(reinterpret_cast<const uint2*>(sr));
         pf_sid = hv.x; pf_rf = hv.y;
@@ -290,9 +297,10 @@ __global__ void __launch_bounds__(32 * PACK_MAX_WARPS, PACK_MIN_BLOCKS) frontier
   // (load_ent has run)
   auto load_cut = [&](uint32_t t, uint32_t k) {
     cp0 = 0; cp1 = 0; cp2 = 0; cp3 = 0; ffm = 0;
-    const uint32_t r = ((blockIdx.x + t * gridDim.x) << (5 - lg)) + g;
+    uint32_t r = ((blockIdx.x + t * gridDim.x) << (5 - lg)) + g;
     const bool mine = t < T && r < N && w < Wmax;
     if (mine) {
+      if (LIST) r = __ldg(P.run_list + r);
       const uint32_t* pw = reinterpret_cast<const uint32_t*>(P.state + (size_t)r * P.state_stride + P.off_phase) + w;
       cp0 = __ldg(pw); cp1 = __ldg(pw + Wmax); cp2 = __ldg(pw + 2u * Wmax); cp3 = __ldg(pw + 3u * Wmax);
     }
@@ -317,8 +325,9 @@ __global__ void __launch_bounds__(32 * PACK_MAX_WARPS, PACK_MIN_BLOCKS) frontier
       if (!ok) sts_v4(tb, dfr ? 0xFFFFFFFFu : 0u, 0u, 0u, 0u);   // marker header (W = 0: dead, all-ones: deferred)
       uint32_t sbytes = 0;
       const uint32_t first = (blockIdx.x + t * gridDim.x) << (5 - lg);
+      if (LIST) sbytes = pf_run != 0xFFFFFFFFu ? P.state_stride : 0u;   // my run's record: a copy of its own
       if (lr == 0) {
-        sbytes = min(R, N - first) * P.state_stride;   // the group's state records are adjacent: one copy
+        if (!LIST) sbytes = min(R, N - first) * P.state_stride;   // the group's state records are adjacent: one copy
         sts_u32(armed_a + 4u * sg, use + 1u);          // published before my arrive: the previous use is over, this one is armed
       }
       // fixed-width rows (rb = row bytes per step; 0 for CSR and formats not cut: one copy of the whole record): the header,
@@ -331,7 +340,11 @@ __global__ void __launch_bounds__(32 * PACK_MAX_WARPS, PACK_MIN_BLOCKS) frontier
       uint32_t from = hdr + 32u * rb * lo_word;
       if (rb && trim_planes && from == rows_end) from = (rows_end + PL_AF * 4u * Wr) & ~15u;
       mbar_expect_tx(bar, (ok ? pf_bytes - (from - hdr) : 0u) + sbytes);
-      if (lr == 0) bulk_g2s(buf, P.state + (size_t)first * P.state_stride, sbytes, bar);
+      if (LIST) {
+        if (sbytes) bulk_g2s(buf + lr * P.state_stride, P.state + (size_t)pf_run * P.state_stride, sbytes, bar);
+      } else if (lr == 0) {
+        bulk_g2s(buf, P.state + (size_t)first * P.state_stride, sbytes, bar);
+      }
       if (ok) {
         const uint8_t* src = reinterpret_cast<const uint8_t*>((uint64_t)pf_lo | ((uint64_t)pf_hi << 32));
         const uint32_t at = from != hdr ? from : 0u;
@@ -364,6 +377,11 @@ __global__ void __launch_bounds__(32 * PACK_MAX_WARPS, PACK_MIN_BLOCKS) frontier
     t = __shfl_sync(FULL, t, 0);
     if (t >= T) break;
     const uint32_t cur_use = __umulhi(t, ng_magic), cur_sg = t - cur_use * NG;   // t / NG, t % NG
+    uint32_t r_list = 0;   // LIST: my run, fetched before the waits
+    if (LIST) {
+      const uint32_t pos = ((blockIdx.x + t * gridDim.x) << (5 - lg)) + g;
+      if (pos < N) r_list = __ldg(P.run_list + pos);
+    }
     load_sid(t + NG, lq == 0);   // first link of the group I shall issue into this slot group when I am done with it
     // The slot group is shared between warps: its use `cur_use` is armed by the warp that consumed the previous use.
     // A parity wait alone cannot tell "use u - 1 still pending" from "use u complete" (the parity then names the phase
@@ -375,13 +393,14 @@ __global__ void __launch_bounds__(32 * PACK_MAX_WARPS, PACK_MIN_BLOCKS) frontier
 #endif
 
     const uint32_t gid = blockIdx.x + t * gridDim.x;
-    const uint32_t r = (gid << (5 - lg)) + g;                 // my run
+    const uint32_t pos = (gid << (5 - lg)) + g;               // my run (LIST: my list position)
+    const uint32_t r = LIST ? r_list : pos;
     uint8_t* const rr = P.result + (size_t)r * P.result_stride;
     const uint32_t grp_a = groups_a + cur_sg * group_bytes;
     const uint32_t sr_a = grp_a + g * P.state_stride;                                   // my run's state record
     const uint32_t tr_a = grp_a + R * P.state_stride + g * P.topo_buf_bytes;            // my run's topology record
 
-    const bool in_batch = r < N;
+    const bool in_batch = pos < N;
     const uint4 h0 = lds_v4(tr_a);
     const uint4 h1 = lds_v4(tr_a + 16);
     const bool deferred = in_batch && h0.x == 0xFFFFFFFFu;
@@ -597,9 +616,11 @@ extern "C" int bf_debug_pack_trace(unsigned long long* out, unsigned int* launch
 #endif
 
 cudaError_t launch_frontier_pack(const KParams& P, uint32_t grid, uint32_t smem_bytes, cudaStream_t stream) {
-  static const KernelFn table[4] = {frontier_pack_kernel<false, false>, frontier_pack_kernel<false, true>,
-                                    frontier_pack_kernel<true, false>, frontier_pack_kernel<true, true>};
-  const KernelFn fn = table[variant_bits(P)];
+  static const KernelFn table[8] = {frontier_pack_kernel<false, false, false>, frontier_pack_kernel<false, true, false>,
+                                    frontier_pack_kernel<true, false, false>,  frontier_pack_kernel<true, true, false>,
+                                    frontier_pack_kernel<false, false, true>,  frontier_pack_kernel<false, true, true>,
+                                    frontier_pack_kernel<true, false, true>,   frontier_pack_kernel<true, true, true>};
+  const KernelFn fn = table[variant_bits(P) | (P.run_list ? 4u : 0u)];
   const cudaError_t e = allow_max_smem(fn);
   if (e != cudaSuccess) return e;
   if (P.flags & BF_EVAL_PIPELINED) {   // programmatic dependent launch: may start while the preceding kernel drains

@@ -194,6 +194,31 @@ class Frontier:
         cdict = {"ready": counts.ready, "skip": counts.skip, "expansion": counts.expansion, "evals": counts.evals}
         return head[:n_runs], events[:min(int(co.n_events), events_cap)], int(co.n_events), cdict, int(co.n_listed)
 
+    def resident_tick_touched(self, handle: int, n_runs: int, deltas: np.ndarray, runs_cap: int, events_cap: int, flags: int = 0,
+                              max_iterations: int = 0, runs: Optional[np.ndarray] = None, head: Optional[np.ndarray] = None,
+                              events: Optional[np.ndarray] = None):
+        """bf_resident_tick_touched: evaluate and list only the runs touched since they were last evaluated.
+        -> dict(full, runs, head, events, n_listed, n_evaluated, n_events, counts); runs / head hold the first
+        min(n_listed, runs_cap) entries, events the first min(n_events, events_cap)."""
+        assert deltas.dtype == self.DELTA_DTYPE and deltas.flags["C_CONTIGUOUS"]
+        if runs is None:
+            runs = np.zeros(max(runs_cap, 1), dtype=np.uint32)
+        if head is None:
+            head = np.zeros(max(runs_cap, 1), dtype=np.uint32)
+        if events is None:
+            events = np.zeros(max(events_cap, 1), dtype=np.uint16)
+        for a, dt, n in ((runs, np.uint32, runs_cap), (head, np.uint32, runs_cap), (events, np.uint16, events_cap)):
+            assert a.dtype == dt and a.flags["C_CONTIGUOUS"] and a.shape[0] >= n
+        to = A.TouchedOut(struct_size=C.sizeof(A.TouchedOut), runs=runs.ctypes.data, head=head.ctypes.data, runs_cap=runs_cap,
+                          events=events.ctypes.data, events_cap=events_cap)
+        counts = A.Counts()
+        self._check(self._lib.bf_resident_tick_touched(self._ctx, handle, deltas.ctypes.data, deltas.shape[0], n_runs, flags,
+                                                       max_iterations, C.byref(to), C.byref(counts)), "bf_resident_tick_touched")
+        nl = min(int(to.n_listed), runs_cap)
+        return {"full": int(to.full), "runs": runs[:nl], "head": head[:nl], "events": events[:min(int(to.n_events), events_cap)],
+                "n_listed": int(to.n_listed), "n_evaluated": int(to.n_evaluated), "n_events": int(to.n_events),
+                "counts": {"ready": counts.ready, "skip": counts.skip, "expansion": counts.expansion, "evals": counts.evals}}
+
     # -- resident batches: device-side state, delta uploads (row f2)
     DELTA_DTYPE = np.dtype([("run", "<u4"), ("index", "<u2"), ("field", "u1"), ("code", "u1")])
 

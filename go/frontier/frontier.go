@@ -293,6 +293,40 @@ func (r *Resident) Tick(deltas []Delta, n, flags uint32, head []uint32, events [
 	return uint64(ne), uint32(nl), k, r.c.err(rc)
 }
 
+// Touched describes a TickTouched call: Full when every run in [0, n) was evaluated and listed (first tick, topology drop,
+// changed fixpoint flag or iteration cap, n beyond the last full tick), else only the runs touched since they were last
+// evaluated were; runs / head / events then hold what a changed-only Tick would list for them.
+type Touched struct {
+	Full       bool
+	NListed    uint32 // listed runs; runs / head hold the first min(NListed, len) of them
+	NEvaluated uint32
+	NEvents    uint64
+}
+
+// TickTouched is the steady-state tick of a batcher that ticks often: the deltas go up, and only the runs that received a
+// delta or an upload since they were last evaluated are evaluated; of those, the ones whose result changed (or that were
+// uploaded) come back in runs (ascending) with their head words and events.  Counts cover the evaluated runs.  Use Tick with
+// EvalChangedOnly as the resync check.
+func (r *Resident) TickTouched(deltas []Delta, n, flags uint32, runs, head []uint32, events []uint16) (t Touched, k Counts, err error) {
+	var dp *C.bf_delta
+	if len(deltas) > 0 {
+		dp = (*C.bf_delta)(unsafe.Pointer(&deltas[0]))
+	}
+	var ev *C.uint16_t
+	if len(events) > 0 {
+		ev = (*C.uint16_t)(unsafe.Pointer(&events[0]))
+	}
+	capRuns := len(runs)
+	if len(head) < capRuns {
+		capRuns = len(head)
+	}
+	var full, nl, ne C.uint32_t
+	var nev C.uint64_t
+	rc := C.bfgo_resident_tick_touched(r.c.p, r.handle, dp, C.uint32_t(len(deltas)), C.uint32_t(n), C.uint32_t(flags), 0, u32p(runs),
+		u32p(head), C.uint32_t(capRuns), ev, C.uint64_t(len(events)), &full, &nl, &ne, &nev, (*C.bf_counts)(unsafe.Pointer(&k)))
+	return Touched{Full: full != 0, NListed: uint32(nl), NEvaluated: uint32(ne), NEvents: uint64(nev)}, k, r.c.err(rc)
+}
+
 // Group is one operator process driving several GPUs (bf_group_*): contiguous blocks of runs per device, one NCCL
 // all-gather of the per-shard counts per pass, limiter totals all-reduced across the shards.
 type Group struct{ p *C.bf_group }

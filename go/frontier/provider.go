@@ -55,6 +55,24 @@ func Rows(head []uint32, events []uint16, set func(run uint32, row Row)) {
 	}
 }
 
+// RowsTouched walks the lists of a touched tick (Resident.TickTouched): runs[i] is listed with head word head[i], and its
+// events are the next head[i]>>16 entries.  Every other run keeps its previous Row.  The caller passes runs[:k] and head[:k],
+// k = min(t.NListed, len(runs), len(head)), never the whole buffers (entries past NListed are stale).  Only rows whose events
+// arrived whole are handed to `set`; RowsTouched returns false when the event list was cut short, and the caller then resyncs
+// (a Tick with EvalChangedOnly, or larger buffers) — as it must when t.NListed exceeded its buffers.
+func RowsTouched(runs, head []uint32, events []uint16, set func(run uint32, row Row)) bool {
+	pos := 0
+	for i, h := range head {
+		n := int(h >> HeadCountShift)
+		if i >= len(runs) || pos+n > len(events) {
+			return false
+		}
+		set(runs[i], Row{Summary: h & HeadSummaryMask, Events: events[pos : pos+n]})
+		pos += n
+	}
+	return true
+}
+
 // Steps turns the row back into the three results of findReadySteps (dag.go:2631-2641) over `steps` =
 // allStorySteps(story) — index i of the packed topology is &steps[i].
 func (r Row) Steps(steps []bubuv1alpha1.Step) (ready, skipped []*bubuv1alpha1.Step, reasons map[string]string) {

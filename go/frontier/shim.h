@@ -81,6 +81,22 @@ static inline int bfgo_resident_tick_compact(bf_ctx* c, uint32_t handle, const b
   return rc;
 }
 
+static inline int bfgo_resident_tick_touched(bf_ctx* c, uint32_t handle, const bf_delta* deltas, uint32_t n_deltas, uint32_t n_runs,
+                                             uint32_t flags, uint32_t max_iterations, uint32_t* runs, uint32_t* head, uint32_t runs_cap,
+                                             uint16_t* events, uint64_t events_cap, uint32_t* full, uint32_t* n_listed,
+                                             uint32_t* n_evaluated, uint64_t* n_events, bf_counts* counts) {
+  bf_touched_out to;
+  memset(&to, 0, sizeof to);
+  to.struct_size = (uint32_t)sizeof to;
+  to.runs = runs; to.head = head; to.runs_cap = runs_cap; to.events = events; to.events_cap = events_cap;
+  const int rc = bf_resident_tick_touched(c, handle, deltas, n_deltas, n_runs, flags, max_iterations, &to, counts);
+  *full = to.full;
+  *n_listed = to.n_listed;
+  *n_evaluated = to.n_evaluated;
+  *n_events = to.n_events;
+  return rc;
+}
+
 static inline void bfgo_tables(bf_sched_tables* t, uint32_t n_stories, uint32_t n_queues, int32_t global_limit, uint32_t global_base,
                                const int32_t* story_limit, const uint32_t* story_base, const int32_t* queue_limit,
                                const int32_t* queue_aging_s, const uint32_t* queue_base, const int32_t* queue_max_priority_base) {

@@ -498,6 +498,43 @@ int bf_eval_compact(bf_ctx* ctx, const bf_batch* batch, bf_compact_out* out);
 int bf_resident_tick_compact(bf_ctx* ctx, uint32_t handle, const bf_delta* deltas, uint32_t n_deltas, uint32_t n_runs,
                              uint32_t flags, uint32_t max_iterations, bf_compact_out* out, bf_counts* counts);
 
+/* ------------------------------------------------------------------ touched ticks
+ * The steady-state tick of a batcher that ticks often: only the runs that changed are evaluated and listed, so both the work
+ * and the traffic of a tick follow the number of changes, not n_runs.  A run's result is a function of its state record, its
+ * topology and the pass parameters alone, and the state changes only through deltas and uploads, so a run that received
+ * neither since it was last evaluated would not be listed by a BF_EVAL_CHANGED_ONLY tick either.
+ *   touched run   a run in [0, n_runs) that received a delta (this call's, bf_resident_apply's or an earlier tick's; applied
+ *                 or rejected) or an upload since the last tick that evaluated it.  Touched runs at or above n_runs stay
+ *                 touched for a later tick that covers them.
+ *   listed run    a touched run whose new result record differs from the one it had (the bytes BF_EVAL_CHANGED_ONLY compares),
+ *                 or that was uploaded since it was last listed (the batcher has no row for it).
+ * With full == 0, runs / head / events are exactly what a BF_EVAL_CHANGED_ONLY compact tick on the same device state gives for
+ * its listed runs: the same head words and the same events in the same order (ascending run index).  counts covers the
+ * evaluated runs only (evals = sum of S over them).
+ * The tick evaluates every run in [0, n_runs), lists them all (runs[i] = i) and sets full = 1 when: no tick has run on the batch
+ * yet (or the last one failed); bf_topology_drop was called on the ctx since the last tick (a dropped slot kills its runs, a
+ * reused one re-points them); BF_EVAL_FIXPOINT or max_iterations differs from the last tick's; or n_runs exceeds the run count
+ * of the last full evaluation and not every run beyond it was uploaded since.  Any tick of the other kinds (bf_resident_tick,
+ * _eval, _tick_compact) may come between touched ticks, and bf_schedule may follow a touched tick.
+ * flags: BF_EVAL_FIXPOINT and BF_EVAL_NO_COUNTS only (else BF_EINVAL).  Pinned buffers are used in place as by
+ * bf_resident_tick_compact; the call returns when they are filled.                                                  */
+typedef struct bf_touched_out {
+  uint32_t struct_size;
+  uint32_t full;               /* out: 1 when the tick evaluated and listed every run in [0, n_runs) (see above)         */
+  uint32_t* runs;              /* [runs_cap] out: ascending indices of the listed runs                                  */
+  uint32_t* head;              /* [runs_cap] out: head word of runs[i], same bits as bf_compact_out.head                */
+  uint32_t runs_cap;
+  uint32_t n_listed;           /* out: listed runs; only the first runs_cap are written when larger                      */
+  uint32_t n_evaluated;        /* out: runs the pass evaluated                                                           */
+  uint32_t reserved;
+  uint16_t* events;            /* [events_cap] out: events of the listed runs, same format and order as the compact lists */
+  uint64_t events_cap;
+  uint64_t n_events;           /* out: as bf_compact_out.n_events                                                        */
+} bf_touched_out;
+
+int bf_resident_tick_touched(bf_ctx* ctx, uint32_t handle, const bf_delta* deltas, uint32_t n_deltas, uint32_t n_runs,
+                             uint32_t flags, uint32_t max_iterations, bf_touched_out* out, bf_counts* counts);
+
 /* ------------------------------------------------------------------ device groups (SURVEY.md row e)
  * The reference is ONE operator process (cmd/main.go:220, StoryRunReconciler storyrun_controller.go:216), so the
  * multi-GPU path must be reachable from one process through this ABI: a group owns one ctx per device and an NCCL
@@ -545,7 +582,8 @@ typedef struct bf_stats {
   uint32_t n_topologies;
   uint32_t sm_count;
   uint32_t last_grid, last_block, last_smem_bytes, last_stages;
-  uint32_t last_kernel;        /* 0 = one run per warp (general), 1 = packed lanes, 2 = packed lanes + deferred general */
+  uint32_t last_kernel;        /* 0 = one run per warp (general), 1 = packed lanes, 2 = packed lanes + deferred general;
+                                  3, 4, 5: the same over the run list of a touched tick                                   */
   uint32_t last_runs_per_trip; /* StoryRuns evaluated per warp trip by the last pass                                   */
   uint32_t last_eval_chunks;   /* run chunks the last bf_eval pipelined over its copy/compute streams (1 = serial)      */
   uint32_t arena_compactions;  /* times the topology arena was re-packed (dropped records reclaimed)                             */
