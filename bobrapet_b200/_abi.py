@@ -116,6 +116,14 @@ class TouchedOut(C.Structure):
                 ("events", C.c_void_p), ("events_cap", C.c_uint64), ("n_events", C.c_uint64)]
 
 
+MIGRATE_GONE = 0xFFFF   # BF_MIGRATE_GONE: the old step has no step of the new generation
+
+
+class Migration(C.Structure):
+    _fields_ = [("struct_size", C.c_uint32), ("old_slot", C.c_uint32), ("new_slot", C.c_uint32), ("n_runs", C.c_uint32),
+                ("step_map", C.c_void_p), ("n_old_steps", C.c_uint32), ("migrated", C.c_uint32)]
+
+
 class SchedTables(C.Structure):
     _fields_ = [("struct_size", C.c_uint32), ("n_stories", C.c_uint32), ("n_queues", C.c_uint32), ("global_limit", C.c_int32),
                 ("global_running_base", C.c_uint32), ("story_limit", C.c_void_p), ("story_running_base", C.c_void_p),
@@ -161,6 +169,7 @@ SYMBOLS = [
     ("bf_eval_compact", C.c_int, [C.c_void_p, C.POINTER(Batch), C.POINTER(CompactOut)]),
     ("bf_resident_tick_compact", C.c_int, [C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.POINTER(CompactOut), C.POINTER(Counts)]),
     ("bf_resident_tick_touched", C.c_int, [C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.POINTER(TouchedOut), C.POINTER(Counts)]),
+    ("bf_resident_migrate", C.c_int, [C.c_void_p, C.c_uint32, C.POINTER(Migration)]),
     ("bf_group_create", C.c_int, [C.POINTER(C.c_void_p), C.POINTER(C.c_int32), C.c_uint32, C.POINTER(Config)]),
     ("bf_group_destroy", None, [C.c_void_p]),
     ("bf_group_size", C.c_uint32, [C.c_void_p]),

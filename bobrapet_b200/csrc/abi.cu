@@ -34,6 +34,7 @@ cudaError_t launch_touched_list(const TouchedParams& P, cudaStream_t stream);
 cudaError_t launch_touched_compact(const TouchedParams& P, cudaStream_t stream);
 cudaError_t launch_mark_runs(uint32_t* mark, uint32_t first, uint32_t n, uint32_t value, cudaStream_t stream);
 cudaError_t launch_move_records(const uint8_t* src, uint8_t* dst, const void* moves, uint32_t n, cudaStream_t stream);
+cudaError_t launch_migrate(const MigrateParams& P, cudaStream_t stream);
 cudaError_t launch_schedule(const SchedParams& P, uint32_t sm_count, cudaStream_t stream, uint32_t phases = 3);
 cudaError_t launch_closure(const Slot* slots, const uint32_t* slot_ids, const uint32_t* starts, uint32_t n, uint32_t n_slots,
                            uint32_t words_out, uint32_t* masks, cudaStream_t stream);
@@ -76,6 +77,7 @@ struct TopoMeta {
   uint32_t S = 0, E = 0, P = 0, bytes = 0;
   size_t offset = 0;  // in arena
   std::vector<uint32_t> child_first;
+  std::vector<uint16_t> par_step, par_branches;   // step and branch count of each parallel desc (bf_resident_migrate)
   uint32_t child_nibbles = 0;
 };
 
@@ -147,6 +149,8 @@ struct bf_ctx {
   uint32_t* d_thead = nullptr; size_t d_thead_cap = 0;
   unsigned long long* d_tsums = nullptr; size_t d_tsums_cap = 0;
   uint64_t last_touched_events = 0;   // events of the previous touched tick (sizes the first D2H)
+  // migrations (bf_resident_migrate): [0, 16) the migrated-run counter | inverse step map | desc table
+  uint8_t* d_mig = nullptr; size_t d_mig_cap = 0;
 
   // limiters (bf_schedule): what the last bf_eval left on the device + scratch
   bool last_eval_valid = false;
@@ -908,6 +912,8 @@ int put_many_locked(bf_ctx* c, const bf_topology* topos, uint32_t count, uint32_
     m.alive = true; m.S = topos[i].n_steps; m.E = topos[i].n_edges; m.P = topos[i].n_parallel;
     m.bytes = plans[i].rec_bytes; m.offset = base + off; m.child_first = plans[i].child_first;
     m.child_nibbles = plans[i].child_nibbles;
+    m.par_step.resize(m.P); m.par_branches.resize(m.P);
+    for (uint32_t q = 0; q < m.P; ++q) { m.par_step[q] = topos[i].parallel[q].step; m.par_branches[q] = topos[i].parallel[q].branches; }
     c->slots_host[slot] = bf::Slot{(uint64_t)(uintptr_t)(c->arena + m.offset), m.bytes,
                                    m.S | (m.P << 16) | (bf::slot_row_bytes(plans[i].ell) << 24)};
     memcpy(&c->ff_host[(size_t)slot * bf::FF_STRIDE], plans[i].ff, sizeof plans[i].ff);
@@ -991,7 +997,7 @@ void bf_destroy(bf_ctx* c) {
   cudaFreeHost(c->h_counts);
   cudaFree(c->arena); cudaFree(c->slots_dev); cudaFree(c->ff_dev); cudaFree(c->d_state); cudaFree(c->d_result); cudaFree(c->d_counts); cudaFree(c->d_acc);
   cudaFree(c->d_defer); cudaFree(c->d_exp); cudaFree(c->d_exp_counts); cudaFree(c->d_offsets); cudaFree(c->d_block_sums); cudaFree(c->d_sched); cudaFree(c->d_deltas); cudaFree(c->d_rejected);
-  cudaFree(c->d_head); cudaFree(c->d_events); cudaFree(c->d_cblock);
+  cudaFree(c->d_head); cudaFree(c->d_events); cudaFree(c->d_cblock); cudaFree(c->d_mig);
   for (Resident& r : c->resident) { cudaFree(r.d_state); cudaFree(r.d_result); cudaFree(r.d_result_prev); }
   delete c;
 }
@@ -1810,6 +1816,79 @@ int bf_resident_tick_touched(bf_ctx* c, uint32_t h, const bf_delta* deltas, uint
   Resident* r = resident_of(c, h);
   if (!r) return fail(c, BF_EINVAL, "unknown resident batch");
   return touched_tick_locked(c, r, deltas, n_deltas, n_runs, flags, max_iterations, out, counts);
+}
+
+// A Story edited while its runs are live: re-index the runs of old_slot to new_slot's step indices in place (resident.cu).  All
+// checks come first, so a rejected call changes nothing; then one upload of the tables, one launch, one synchronisation.
+int bf_resident_migrate(bf_ctx* c, uint32_t h, bf_migration* m) {
+  if (!c) return BF_EINVAL;
+  std::lock_guard<std::mutex> g(c->mu);
+  if (!m || m->struct_size != sizeof(bf_migration)) return fail(c, BF_EINVAL, "null bf_migration or bad struct_size");
+  Resident* r = resident_of(c, h);
+  if (!r) return fail(c, BF_EINVAL, "unknown resident batch");
+  const bf_layout& L = r->L;
+  if (m->n_runs > r->cap) return fail(c, BF_EINVAL, "n_runs exceeds the resident batch");
+  auto alive = [&](uint32_t s) { return s < c->meta.size() && c->meta[s].alive; };
+  if (!alive(m->old_slot) || !alive(m->new_slot)) return fail(c, BF_ETOPO, "migration between unknown topology slots");
+  if (m->old_slot == m->new_slot) return fail(c, BF_EINVAL, "migration from a slot to itself");
+  const TopoMeta& mo = c->meta[m->old_slot];
+  const TopoMeta& mn = c->meta[m->new_slot];
+  if (m->n_old_steps != mo.S || !m->step_map) return fail(c, BF_EINVAL, "step_map must have one entry per step of old_slot");
+  const bool child = L.off_child != BF_OFF_NONE;
+  if (mo.S > L.steps_max || mn.S > L.steps_max || (child && (mo.child_nibbles > L.child_nibbles || mn.child_nibbles > L.child_nibbles)))
+    return fail(c, BF_ETOPO, "topology does not fit the batch layout (steps_max / child_nibbles)");
+  std::vector<uint16_t> inv((size_t)L.words * 32, (uint16_t)BF_MIGRATE_GONE);
+  for (uint32_t i = 0; i < mo.S; ++i) {
+    const uint32_t t = m->step_map[i];
+    if (t == BF_MIGRATE_GONE) continue;
+    if (t >= mn.S) return fail(c, BF_EINVAL, "step_map[" + std::to_string(i) + "] is not a step of new_slot");
+    if (inv[t] != BF_MIGRATE_GONE) return fail(c, BF_EINVAL, "step_map is not injective (new step " + std::to_string(t) + ")");
+    inv[t] = (uint16_t)i;
+  }
+  std::vector<bf::MigrateDesc> descs;
+  for (uint32_t q = 0; q < mn.P; ++q) {
+    const uint32_t o = inv[mn.par_step[q]];
+    if (o == BF_MIGRATE_GONE) continue;
+    const auto it = std::lower_bound(mo.par_step.begin(), mo.par_step.end(), (uint16_t)o);   // descs ascend by step
+    if (it == mo.par_step.end() || *it != o) continue;   // the old step was not parallel: the desc starts unregistered
+    const uint32_t p = (uint32_t)(it - mo.par_step.begin());
+    if (mo.par_branches[p] != mn.par_branches[q])
+      return fail(c, BF_EINVAL, "parallel step " + std::to_string(o) + " changes its branch count: re-pack its runs on the host");
+    bf::MigrateDesc d{};
+    d.old_first = mo.child_first[p]; d.new_first = mn.child_first[q];
+    d.branches = mn.par_branches[q]; d.old_p = (uint16_t)p; d.new_p = (uint16_t)q;
+    descs.push_back(d);
+  }
+  m->migrated = 0;
+  BF_CUDA(c, cudaSetDevice(c->device));
+  cudaStream_t s = c->stream;
+  const size_t o_inv = 16, o_desc = round_up_sz(o_inv + inv.size() * 2, 16), bytes = o_desc + descs.size() * sizeof(bf::MigrateDesc);
+  if (int rc = ensure_dev(c, c->d_mig, c->d_mig_cap, bytes)) return rc;
+  std::vector<uint8_t> blob(bytes, 0);   // the counter starts at zero
+  memcpy(blob.data() + o_inv, inv.data(), inv.size() * 2);
+  if (!descs.empty()) memcpy(blob.data() + o_desc, descs.data(), descs.size() * sizeof(bf::MigrateDesc));
+  if (c->last_state == r->d_state) c->last_eval_valid = false;   // as after an upload: bf_schedule must follow a new pass
+  bf::MigrateParams P{};
+  P.state = r->d_state; P.mark = r->d_mark; P.mark_value = r->epoch << 1 | 1u;   // touched and must be listed
+  P.migrated = reinterpret_cast<uint32_t*>(c->d_mig);
+  P.inv = reinterpret_cast<const uint16_t*>(c->d_mig + o_inv);
+  P.desc = reinterpret_cast<const bf::MigrateDesc*>(c->d_mig + o_desc); P.n_desc = (uint32_t)descs.size();
+  P.n_runs = m->n_runs; P.old_slot = m->old_slot; P.new_slot = m->new_slot;
+  P.words = L.words; P.state_stride = L.state_stride; P.off_phase = L.off_phase; P.off_cond = L.off_cond;
+  P.off_decision = L.off_decision; P.off_child = L.off_child; P.child_nibbles = L.child_nibbles;
+  cudaError_t e = cudaMemcpyAsync(c->d_mig, blob.data(), bytes, cudaMemcpyHostToDevice, s);
+  if (e == cudaSuccess) e = bf::launch_migrate(P, s);
+  if (e == cudaSuccess) e = cudaMemcpyAsync(c->h_counts, c->d_mig, 4, cudaMemcpyDeviceToHost, s);
+  const cudaError_t es = cudaStreamSynchronize(s);
+  if (e == cudaSuccess) e = es;
+  if (e != cudaSuccess) {   // some records may have moved: the next touched tick evaluates and lists every run
+    r->need_full = true; r->prev_valid = false;
+    return cuda_fail(c, e, "bf_resident_migrate");
+  }
+  c->stats.kernel_launches += m->n_runs ? 1 : 0;
+  m->migrated = *reinterpret_cast<const uint32_t*>(c->h_counts);
+  r->pending += m->migrated;   // the touched-list bound counts the migrated runs as it counts uploaded ones
+  return BF_OK;
 }
 
 int bf_alloc_pinned(bf_ctx* c, size_t bytes, void** out) {

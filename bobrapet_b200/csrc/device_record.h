@@ -202,6 +202,25 @@ struct DeltaParams {
   uint32_t mark_value;
 };
 
+// bf_resident_migrate (resident.cu): the records of the runs on old_slot are re-indexed in place to new_slot's step indices
+struct MigrateDesc {   // a parallel desc of the new topology whose step is the image of a parallel step of the old one
+  uint32_t old_first, new_first;   // child_first of the old / new desc: multiples of 8 nibbles, so whole u32 words of the child area
+  uint16_t branches, old_p, new_p, reserved;
+};
+static_assert(sizeof(MigrateDesc) == 16, "MigrateDesc must be 16 bytes");
+struct MigrateParams {
+  uint8_t* state;
+  uint32_t* mark;                // touch marks: a migrated run's is set to mark_value (touched and must be listed)
+  uint32_t mark_value;
+  uint32_t* migrated;            // [1] runs migrated (zeroed by the caller)
+  const uint16_t* inv;           // [words * 32] old index of new step j, or BF_MIGRATE_GONE
+  const MigrateDesc* desc;       // [n_desc]
+  uint32_t n_desc;
+  uint32_t n_runs, old_slot, new_slot;
+  uint32_t words, state_stride, off_phase, off_cond, off_decision, off_child;
+  uint32_t child_nibbles;        // of the layout; the child area is ceil(child_nibbles / 8) u32 words
+};
+
 // limiters.cu (rows a9 / f4)
 struct SchedParams {
   const uint8_t* state;

@@ -525,6 +525,136 @@ int bfh_batch_eval(bfh_batch* b, uint32_t eval_flags, bf_counts* counts) {
   return rc;
 }
 
+int bfh_story_migration_map(const bfh_story* os, const bfh_story* ns, uint16_t* map, uint32_t cap) {
+  if (!os || !ns || !os->finalized || !ns->finalized || (cap && !map)) return BF_EINVAL;
+  const uint32_t S = (uint32_t)os->order.size();
+  for (uint32_t i = 0; i < S && i < cap; ++i) {
+    auto it = ns->index.find(os->defs[os->order[i]].name);
+    map[i] = it == ns->index.end() ? (uint16_t)BF_MIGRATE_GONE : (uint16_t)it->second;
+  }
+  return (int)S;
+}
+
+int bfh_batch_migrate(bfh_batch* b, const bfh_story* os, const bfh_story* ns, uint32_t old_slot, uint32_t new_slot) {
+  if (!b || !os || !ns || !os->finalized || !ns->finalized) return BF_EINVAL;
+  const bf_layout& L = b->L;
+  const uint32_t So = (uint32_t)os->flags.size(), W = L.words;
+  if (old_slot == new_slot) { b->err = "migration from a slot to itself"; return BF_EINVAL; }
+  if (ns->flags.size() > L.steps_max || (L.off_child != BF_OFF_NONE && ns->child_nibbles > L.child_nibbles)) {
+    b->err = "the new story does not fit the batch layout";
+    return BF_EINVAL;
+  }
+  std::vector<uint16_t> map(So);
+  bfh_story_migration_map(os, ns, map.data(), So);
+  std::vector<uint16_t> inv((size_t)W * 32, (uint16_t)BF_MIGRATE_GONE);
+  for (uint32_t i = 0; i < So; ++i)
+    if (map[i] != BF_MIGRATE_GONE) inv[map[i]] = (uint16_t)i;
+  std::vector<int> desc_to(os->par.size(), -1);   // old parallel desc -> new desc, or -1
+  for (size_t p = 0; p < os->par.size(); ++p) {
+    const uint16_t j = map[os->par[p].step];
+    if (j == BF_MIGRATE_GONE) continue;
+    for (size_t q = 0; q < ns->par.size(); ++q)
+      if (ns->par[q].step == j) {
+        if (ns->par[q].branches != os->par[p].branches) {
+          b->err = "parallel step " + os->defs[os->order[os->par[p].step]].name + " changes its branch count: re-pack its runs";
+          return BF_EINVAL;
+        }
+        desc_to[p] = (int)q;
+      }
+  }
+  std::vector<uint8_t> moved(b->n, 0);
+  uint32_t n_moved = 0, n_on_device = 0;
+  for (uint32_t r = 0; r < b->n; ++r) {
+    if (reinterpret_cast<const bf_run_header*>(b->state + (size_t)r * L.state_stride)->topo_slot != old_slot) continue;
+    if (b->story_of_run[r] != os) { b->err = "run " + std::to_string(r) + " holds old_slot but is not a run of old_story"; return BF_EINVAL; }
+    moved[r] = 1;
+    ++n_moved;
+    if (r < b->uploaded) ++n_on_device;
+  }
+  if (b->resident && b->uploaded) {   // the device first: it validates what the mirror cannot (live slots), and fails without changes
+    bf_migration m{};
+    m.struct_size = sizeof m; m.old_slot = old_slot; m.new_slot = new_slot; m.n_runs = b->uploaded;
+    m.step_map = map.data(); m.n_old_steps = So;
+    const int rc = bf_resident_migrate(b->ctx, b->handle, &m);
+    if (rc != BF_OK) { b->err = bf_last_error(b->ctx); return rc; }
+    if (m.migrated != n_on_device) {
+      // the device copy had diverged from the mirror (its records were changed behind the mirror's back) and has now moved
+      // runs the mirror did not: the mirror stays as it was, and the next bfh_batch_eval re-sends every record in full
+      b->uploaded = 0;
+      b->deltas.clear();
+      b->delta_at.clear();
+      b->err = "the device moved " + std::to_string(m.migrated) + " runs, the mirror holds " + std::to_string(n_on_device) +
+               " on the old slot: the mirror is unchanged and its records will be uploaded in full";
+      return BF_EINVAL;
+    }
+  }
+  // re-pack the mirror's records: codes by step name, child phases and registered bits by parallel desc
+  std::vector<uint8_t> old(L.state_stride);
+  for (uint32_t r = 0; r < b->n; ++r) {
+    if (!moved[r]) continue;
+    uint8_t* rec = b->state + (size_t)r * L.state_stride;
+    memcpy(old.data(), rec, L.state_stride);
+    for (uint32_t j = 0; j < W * 32; ++j) {
+      const uint32_t o = inv[j];
+      set_code(rec + L.off_phase, W, 4, j, o == BF_MIGRATE_GONE ? 0 : get_code(old.data() + L.off_phase, W, 4, o));
+      if (L.off_cond != BF_OFF_NONE) set_code(rec + L.off_cond, W, 2, j, o == BF_MIGRATE_GONE ? 0 : get_code(old.data() + L.off_cond, W, 2, o));
+      if (L.off_decision != BF_OFF_NONE)
+        set_code(rec + L.off_decision, W, 2, j, o == BF_MIGRATE_GONE ? 0 : get_code(old.data() + L.off_decision, W, 2, o));
+    }
+    bf_run_header* h = reinterpret_cast<bf_run_header*>(rec);
+    const uint64_t reg_old = h->children_registered;
+    uint64_t reg = 0;
+    if (L.off_child != BF_OFF_NONE)
+      for (uint32_t i = 0; i < L.child_nibbles; ++i) rec[L.off_child + (i >> 1)] &= (uint8_t)~(0xFu << ((i & 1u) * 4u));
+    for (size_t p = 0; p < os->par.size(); ++p) {
+      if (desc_to[p] < 0) continue;
+      const uint32_t q = (uint32_t)desc_to[p];
+      if ((reg_old >> p) & 1u) reg |= 1ull << q;
+      if (L.off_child == BF_OFF_NONE) continue;
+      for (uint32_t br = 0; br < os->par[p].branches; ++br) {
+        const uint32_t si = os->child_first[p] + br, di = ns->child_first[q] + br;
+        const uint32_t v = (old[L.off_child + (si >> 1)] >> ((si & 1u) * 4u)) & 0xFu;
+        rec[L.off_child + (di >> 1)] |= (uint8_t)(v << ((di & 1u) * 4u));
+      }
+    }
+    h->children_registered = reg;
+    h->topo_slot = new_slot;
+    b->story_of_run[r] = ns;
+  }
+  // pending deltas of the moved runs follow their step / desc, or are dropped with a removed step
+  if (!b->deltas.empty()) {
+    size_t keep = 0;
+    for (size_t k = 0; k < b->deltas.size(); ++k) {
+      bf_delta d = b->deltas[k];
+      bool ok = true;
+      if (d.run < b->n && moved[d.run]) {
+        if (d.field == BF_DELTA_PHASE || d.field == BF_DELTA_COND || d.field == BF_DELTA_DECISION) {
+          ok = d.index < So && map[d.index] != BF_MIGRATE_GONE;
+          if (ok) d.index = map[d.index];
+        } else if (d.field == BF_DELTA_REGISTERED) {
+          ok = d.index < desc_to.size() && desc_to[d.index] >= 0;
+          if (ok) d.index = (uint16_t)desc_to[d.index];
+        } else if (d.field == BF_DELTA_CHILD) {
+          ok = false;
+          for (size_t p = 0; p < os->par.size() && !ok; ++p)
+            if (desc_to[p] >= 0 && d.index >= os->child_first[p] && d.index < os->child_first[p] + os->par[p].branches) {
+              d.index = (uint16_t)(ns->child_first[desc_to[p]] + (d.index - os->child_first[p]));
+              ok = true;
+            }
+        }
+      }
+      if (ok) b->deltas[keep++] = d;
+    }
+    b->deltas.resize(keep);
+    b->delta_at.clear();
+    for (size_t i = 0; i < keep; ++i) {
+      const bf_delta& d = b->deltas[i];
+      b->delta_at[((uint64_t)d.run << 32) | ((uint64_t)d.field << 16) | d.index] = (uint32_t)i;
+    }
+  }
+  return (int)n_moved;
+}
+
 int bfh_batch_set_resident(bfh_batch* b, int on) {
   if (!b) return BF_EINVAL;
   if (!b->ctx) { b->err = "batch was created without a device context"; return BF_ENODEV; }

@@ -106,4 +106,102 @@ cudaError_t launch_apply_deltas(const DeltaParams& P, cudaStream_t stream) {
   return cudaGetLastError();
 }
 
+// Migration of the runs of one topology slot to another (bf_resident_migrate).  One warp per run: a run of another slot leaves
+// after reading its header word.  A run of old_slot stages the code planes its layout has (phase, then cond, then decision) and
+// its child area in shared memory, then rebuilds every plane word in place: lane t gathers the codes of new step 32w + t from the
+// old step the inverse map names, and one ballot per plane assembles the word.  The child area is zeroed and each kept parallel
+// desc's words are copied to their new place (child_first is a multiple of 8 nibbles); the children_registered bits follow their
+// descs.  All shared memory is dynamic: word 0 is the CTA's count, the warps' stages start at word 4 (migrate_stage_words each).
+__host__ __device__ inline uint32_t migrate_planes(const MigrateParams& P) {
+  return 4u + (P.off_cond != BF_OFF_NONE ? 2u : 0u) + (P.off_decision != BF_OFF_NONE ? 2u : 0u);
+}
+__host__ __device__ inline uint32_t migrate_child_words(const MigrateParams& P) {
+  return P.off_child != BF_OFF_NONE ? (P.child_nibbles + 7) / 8 : 0u;
+}
+__host__ __device__ inline uint32_t migrate_stage_words(const MigrateParams& P) {
+  return migrate_planes(P) * P.words + migrate_child_words(P);
+}
+
+__global__ void __launch_bounds__(256) migrate_runs(const MigrateParams P) {
+  extern __shared__ uint32_t smem[];
+  uint32_t& block_count = smem[0];
+  const uint32_t warp = threadIdx.x >> 5, lane = threadIdx.x & 31u, W = P.words;
+  const uint32_t np = migrate_planes(P), child_words = migrate_child_words(P);
+  if (threadIdx.x == 0) block_count = 0;
+  __syncthreads();
+  const uint32_t run = blockIdx.x * (blockDim.x >> 5) + warp;
+  uint8_t* rec = P.state + (size_t)run * P.state_stride;
+  if (run < P.n_runs && *reinterpret_cast<const uint32_t*>(rec) == P.old_slot) {
+    uint32_t* st = smem + 4u + warp * migrate_stage_words(P);   // np planes of W words | child words
+    const bool has_cond = P.off_cond != BF_OFF_NONE, has_dec = P.off_decision != BF_OFF_NONE;
+    // plane k lives at plane_of(k) in the record: 0-3 phase, then cond's two planes, then decision's
+    auto plane_of = [&](uint32_t k) -> uint32_t* {
+      if (k < 4u) return reinterpret_cast<uint32_t*>(rec + P.off_phase) + k * W;
+      if (has_cond && k < 6u) return reinterpret_cast<uint32_t*>(rec + P.off_cond) + (k - 4u) * W;
+      return reinterpret_cast<uint32_t*>(rec + P.off_decision) + (k - (has_cond ? 6u : 4u)) * W;
+    };
+    for (uint32_t i = lane; i < np * W; i += 32u) st[i] = plane_of(i / W)[i % W];   // all lanes load, plane after plane
+    uint32_t* child = child_words ? reinterpret_cast<uint32_t*>(rec + P.off_child) : nullptr;
+    uint32_t* st_child = st + np * W;
+    for (uint32_t i = lane; i < child_words; i += 32u) st_child[i] = child[i];
+    const uint64_t reg_old = *reinterpret_cast<const uint64_t*>(rec + 8);
+    __syncwarp();
+    uint32_t* dst = lane < np ? plane_of(lane) : nullptr;   // lane k stores plane k's words
+    for (uint32_t w = 0; w < W; ++w) {
+      const uint32_t o = P.inv[w * 32u + lane];
+      uint32_t code = 0;
+      if (o != BF_MIGRATE_GONE)
+        for (uint32_t k = 0; k < np; ++k) code |= ((st[k * W + (o >> 5)] >> (o & 31u)) & 1u) << k;
+      uint32_t word = 0;
+      for (uint32_t k = 0; k < np; ++k) {
+        const uint32_t b = __ballot_sync(0xFFFFFFFFu, (code >> k) & 1u);
+        if (lane == k) word = b;
+      }
+      if (dst) dst[w] = word;
+    }
+    // child area: nibbles past the layout's child_nibbles (the last word's padding) are kept
+    for (uint32_t i = lane; i < child_words; i += 32u) {
+      const uint32_t used = P.child_nibbles - i * 8u;
+      child[i] = used >= 8u ? 0u : st_child[i] & ~((1u << (4u * used)) - 1u);
+    }
+    __syncwarp();
+    uint64_t reg_new = 0;
+    for (uint32_t d = 0; d < P.n_desc; ++d) {
+      const MigrateDesc md = P.desc[d];
+      reg_new |= ((reg_old >> md.old_p) & 1ull) << md.new_p;
+      if (!child_words) continue;
+      const uint32_t nw = (md.branches + 7u) / 8u, tail = md.branches & 7u;
+      for (uint32_t i = lane; i < nw; i += 32u) {
+        uint32_t v = st_child[md.old_first / 8u + i];
+        if (i == nw - 1u && tail) v &= (1u << (4u * tail)) - 1u;
+        child[md.new_first / 8u + i] = v;
+      }
+    }
+    if (lane == 0) {
+      *reinterpret_cast<uint32_t*>(rec) = P.new_slot;
+      *reinterpret_cast<uint64_t*>(rec + 8) = reg_new;
+      P.mark[run] = P.mark_value;
+      atomicAdd(&block_count, 1u);
+    }
+  }
+  __syncthreads();
+  if (threadIdx.x == 0 && block_count) atomicAdd(P.migrated, block_count);
+}
+
+// Warps per CTA: 8, fewer when their stages and the 16-byte count header pass the 48 KiB a launch gets without an opt-in.  One
+// warp always fits: its stage is at most 8 * 32 + 8192 words (33 KiB).
+uint32_t migrate_warps_per_block(const MigrateParams& P) {
+  const uint32_t warp_bytes = migrate_stage_words(P) * 4u;
+  uint32_t wpb = 8;
+  while (wpb > 1 && 16u + wpb * warp_bytes > (48u << 10)) --wpb;
+  return wpb;
+}
+
+cudaError_t launch_migrate(const MigrateParams& P, cudaStream_t stream) {
+  if (P.n_runs == 0) return cudaSuccess;
+  const uint32_t wpb = migrate_warps_per_block(P);
+  migrate_runs<<<(P.n_runs + wpb - 1) / wpb, wpb * 32, 16u + wpb * migrate_stage_words(P) * 4u, stream>>>(P);
+  return cudaGetLastError();
+}
+
 }  // namespace bf

@@ -219,6 +219,15 @@ class Frontier:
                 "n_listed": int(to.n_listed), "n_evaluated": int(to.n_evaluated), "n_events": int(to.n_events),
                 "counts": {"ready": counts.ready, "skip": counts.skip, "expansion": counts.expansion, "evals": counts.evals}}
 
+    def resident_migrate(self, handle: int, old_slot: int, new_slot: int, step_map, n_runs: int) -> int:
+        """bf_resident_migrate: move the runs in [0, n_runs) on old_slot to new_slot (an edited Story), re-indexing their step
+        state in place.  step_map[i] = new index of old step i, or A.MIGRATE_GONE.  -> number of runs migrated."""
+        sm = np.ascontiguousarray(step_map, dtype=np.uint16)
+        m = A.Migration(struct_size=C.sizeof(A.Migration), old_slot=int(old_slot), new_slot=int(new_slot), n_runs=int(n_runs),
+                        step_map=sm.ctypes.data, n_old_steps=sm.shape[0])
+        self._check(self._lib.bf_resident_migrate(self._ctx, handle, C.byref(m)), "bf_resident_migrate")
+        return int(m.migrated)
+
     # -- resident batches: device-side state, delta uploads (row f2)
     DELTA_DTYPE = np.dtype([("run", "<u4"), ("index", "<u2"), ("field", "u1"), ("code", "u1")])
 

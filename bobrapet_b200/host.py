@@ -41,6 +41,8 @@ _SYMS = [
     ("bfh_run_set_run_flags", C.c_int, [C.c_void_p, C.c_uint32, C.c_int, C.c_int]),
     ("bfh_run_register_children", C.c_int, [C.c_void_p, C.c_uint32, C.c_uint32, C.c_int]),
     ("bfh_run_set_child_phase", C.c_int, [C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32, C.c_char_p]),
+    ("bfh_story_migration_map", C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32]),
+    ("bfh_batch_migrate", C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32, C.c_uint32]),
     ("bfh_batch_eval", C.c_int, [C.c_void_p, C.c_uint32, C.POINTER(A.Counts)]),
     ("bfh_batch_set_resident", C.c_int, [C.c_void_p, C.c_int]),
     ("bfh_batch_traffic", C.c_int, [C.c_void_p, C.POINTER(C.c_uint64), C.POINTER(C.c_uint64), C.POINTER(C.c_uint32)]),
@@ -153,6 +155,15 @@ class HostStory:
     def run_flags(self) -> int:
         return self._l.bfh_story_run_flags(self._p)
 
+    def migration_map(self, new: "HostStory") -> np.ndarray:
+        """bfh_story_migration_map: [S] uint16, the index in `new` of each step of this story by name, or A.MIGRATE_GONE"""
+        n = self._l.bfh_story_migration_map(self._p, new._p, None, 0)
+        if n < 0:
+            raise A.FrontierError(n, "bfh_story_migration_map")
+        out = np.zeros(max(n, 1), np.uint16)
+        self._l.bfh_story_migration_map(self._p, new._p, out.ctypes.data, n)
+        return out[:n]
+
 
 def scan_step_refs(expr: str) -> List[str]:
     buf = C.create_string_buffer(65536)
@@ -225,6 +236,10 @@ class HostBatch:
 
     def set_child_phase(self, run, q, branch, phase):
         self._chk(self._l.bfh_run_set_child_phase(self._p, run, q, branch, _b(phase)), "bfh_run_set_child_phase")
+
+    def migrate(self, old: HostStory, new: HostStory, old_slot: int, new_slot: int) -> int:
+        """bfh_batch_migrate: move the runs on old_slot to `new` / new_slot (in resident mode on the device too) -> runs moved"""
+        return self._chk(self._l.bfh_batch_migrate(self._p, old._p, new._p, old_slot, new_slot), "bfh_batch_migrate")
 
     def size(self) -> int:
         return self._l.bfh_batch_size(self._p)

@@ -327,6 +327,22 @@ func (r *Resident) TickTouched(deltas []Delta, n, flags uint32, runs, head []uin
 	return Touched{Full: full != 0, NListed: uint32(nl), NEvaluated: uint32(ne), NEvents: uint64(nev)}, k, r.c.err(rc)
 }
 
+// MigrateGone marks an old step that has no step of the new Story generation (BF_MIGRATE_GONE).
+const MigrateGone = 0xFFFF
+
+// Migrate moves the live runs in [0, n) of an edited Story from its old topology slot to the new one, re-indexing their step
+// state on the device by name (stepMap from MigrationMap).  Afterwards the old slot may be dropped; the next TickTouched lists
+// every migrated run.  A kept parallel step whose branch count changed is rejected: re-pack and Upload those runs instead.
+func (r *Resident) Migrate(oldSlot, newSlot uint32, stepMap []uint16, n uint32) (migrated uint32, err error) {
+	var mp *C.uint16_t
+	if len(stepMap) > 0 {
+		mp = (*C.uint16_t)(unsafe.Pointer(&stepMap[0]))
+	}
+	var m C.uint32_t
+	rc := C.bfgo_resident_migrate(r.c.p, r.handle, C.uint32_t(oldSlot), C.uint32_t(newSlot), mp, C.uint32_t(len(stepMap)), C.uint32_t(n), &m)
+	return uint32(m), r.c.err(rc)
+}
+
 // Group is one operator process driving several GPUs (bf_group_*): contiguous blocks of runs per device, one NCCL
 // all-gather of the per-shard counts per pass, limiter totals all-reduced across the shards.
 type Group struct{ p *C.bf_group }

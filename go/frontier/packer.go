@@ -208,6 +208,27 @@ const (
 	rfTopologyTerminated = 0x04
 )
 
+// MigrationMap is the step map of Resident.Migrate for an edited Story: stepMap[i] is the index in newer of the step named
+// older.Names[i], or MigrateGone.  The reference keys StepStates, Gates and PrimitiveChildren by name and walks the current
+// Story's allStorySteps on every reconcile (getStoryForRun, storyrun_controller.go:1297-1313), so state follows the name.
+// added lists the names of newer that older lacks: a name that existed in an earlier generation may still have a StepState
+// in the StoryRun, which the migrated record does not carry; send deltas for it.
+func MigrationMap(older, newer *PackedStory) (stepMap []uint16, added []string) {
+	stepMap = make([]uint16, len(older.Names))
+	for i, n := range older.Names {
+		stepMap[i] = MigrateGone
+		if j, ok := newer.Index[n]; ok {
+			stepMap[i] = j
+		}
+	}
+	for _, n := range newer.Names {
+		if _, ok := older.Index[n]; !ok {
+			added = append(added, n)
+		}
+	}
+	return stepMap, added
+}
+
 // RunFlags: shouldFailFast (dag.go:3504-3511), Pattern.IsRealtime (enums.go:335), and the Degraded /
 // TopologyTerminated condition the caller read from the StoryRun (dag.go:436-464).
 func RunFlags(story *bubuv1alpha1.Story, topologyTerminated bool) uint8 {

@@ -97,6 +97,17 @@ static inline int bfgo_resident_tick_touched(bf_ctx* c, uint32_t handle, const b
   return rc;
 }
 
+static inline int bfgo_resident_migrate(bf_ctx* c, uint32_t handle, uint32_t old_slot, uint32_t new_slot, const uint16_t* step_map,
+                                        uint32_t n_old_steps, uint32_t n_runs, uint32_t* migrated) {
+  bf_migration m;
+  memset(&m, 0, sizeof m);
+  m.struct_size = (uint32_t)sizeof m;
+  m.old_slot = old_slot; m.new_slot = new_slot; m.n_runs = n_runs; m.step_map = step_map; m.n_old_steps = n_old_steps;
+  const int rc = bf_resident_migrate(c, handle, &m);
+  *migrated = m.migrated;
+  return rc;
+}
+
 static inline void bfgo_tables(bf_sched_tables* t, uint32_t n_stories, uint32_t n_queues, int32_t global_limit, uint32_t global_base,
                                const int32_t* story_limit, const uint32_t* story_base, const int32_t* queue_limit,
                                const int32_t* queue_aging_s, const uint32_t* queue_base, const int32_t* queue_max_priority_base) {

@@ -535,6 +535,35 @@ typedef struct bf_touched_out {
 int bf_resident_tick_touched(bf_ctx* ctx, uint32_t handle, const bf_delta* deltas, uint32_t n_deltas, uint32_t n_runs,
                              uint32_t flags, uint32_t max_iterations, bf_touched_out* out, bf_counts* counts);
 
+/* ------------------------------------------------------------------ migrations (a Story edited while its runs are live)
+ * The reference does not pin a StoryRun to the Story generation it started with: every reconcile loads the current Story
+ * (getStoryForRun, storyrun_controller.go:1297-1313) and walks allStorySteps of that spec, with StepStates, Gates and
+ * PrimitiveChildren keyed by step name (buildStateMaps ignores names the list no longer has, dag.go:3373-3376).  Here state is
+ * kept by step INDEX, and an edit moves indices.  bf_resident_migrate re-indexes, in place on the device, every run in
+ * [0, n_runs) whose header holds old_slot, so that its record equals what packing its by-name state against new_slot gives:
+ *   - new step j carries the phase / cond / decision codes of the old step mapped to j; steps without one carry 0;
+ *   - a parallel desc of new_slot whose step is the image of an old parallel step takes that step's children_registered bit
+ *     and child nibbles (branches matched by index); other descs start unregistered with zero nibbles;
+ *   - topo_slot = new_slot; run_flags and every other run are untouched (a changed policy travels as BF_DELTA_RUN_FLAGS).
+ * Checked before anything runs, else BF_EINVAL / BF_ETOPO and nothing changed: both slots alive and different; n_old_steps ==
+ * S of old_slot; the map injective with targets below S of new_slot; both topologies fit the batch layout (steps_max,
+ * child_nibbles); every surviving parallel step keeps its branch count (else BF_EINVAL: re-pack those runs on the host).
+ * Migrated runs are touched and must be listed by the next bf_resident_tick_touched, as uploaded runs are; a changed-only
+ * compact tick lists them when their result record changed.  Like an upload, the call ends the evaluated snapshot (bf_schedule
+ * must follow a new pass).  A step name removed in an earlier generation and re-added now starts at 0: the caller sends deltas
+ * for it.  One launch and one synchronisation.                                                                        */
+#define BF_MIGRATE_GONE 0xFFFFu
+typedef struct bf_migration {
+  uint32_t struct_size;        /* sizeof(bf_migration)                                                         */
+  uint32_t old_slot, new_slot;
+  uint32_t n_runs;             /* runs [0, n_runs) of the resident batch are considered                        */
+  const uint16_t* step_map;    /* [n_old_steps]: new index of old step i, or BF_MIGRATE_GONE; injective         */
+  uint32_t n_old_steps;        /* must equal S of old_slot                                                     */
+  uint32_t migrated;           /* out: runs whose header held old_slot and were moved                          */
+} bf_migration;
+
+int bf_resident_migrate(bf_ctx* ctx, uint32_t handle, bf_migration* m);
+
 /* ------------------------------------------------------------------ device groups (SURVEY.md row e)
  * The reference is ONE operator process (cmd/main.go:220, StoryRunReconciler storyrun_controller.go:216), so the
  * multi-GPU path must be reachable from one process through this ABI: a group owns one ctx per device and an NCCL

@@ -94,6 +94,20 @@ int bfh_batch_set_resident(bfh_batch* b, int on);
 /* bytes sent so far as full records / as deltas, and the deltas logged since the last eval */
 int bfh_batch_traffic(const bfh_batch* b, uint64_t* full_record_bytes, uint64_t* delta_bytes, uint32_t* pending_deltas);
 
+/* A Story edited while its runs are live (see bf_resident_migrate).  bfh_story_migration_map writes, for each step i of `old_story`
+ * (finalized, allStorySteps order), the index of the step of the same name in `new_story`, or BF_MIGRATE_GONE, into map[i] for
+ * i < cap, and returns the step count of old_story.  bfh_batch_migrate moves every run whose record holds old_slot (each must be
+ * a run of old_story) to new_story / new_slot: the mirror re-packs its own records by step name (parallel steps keep their
+ * registered bit and child phases, branches by index; a kept parallel step whose branch count changed is BF_EINVAL), rewrites
+ * the step, child and desc indices of the pending deltas of those runs and drops the ones of removed steps; in resident mode it
+ * first calls bf_resident_migrate over the uploaded runs, so that the device and the mirror stay identical.  Nothing changes
+ * on an error, with one exception: when the device copy had diverged from the mirror and bf_resident_migrate moved a different
+ * number of runs than the mirror holds, the mirror stays unchanged, its pending deltas are discarded and the next
+ * bfh_batch_eval uploads every record in full (BF_EINVAL reports it).  Returns the number of runs moved.  Steps new to this generation start with no state; re-send what they had
+ * if their name existed in an earlier generation.                                                                         */
+int bfh_story_migration_map(const bfh_story* old_story, const bfh_story* new_story, uint16_t* map, uint32_t cap);
+int bfh_batch_migrate(bfh_batch* b, const bfh_story* old_story, const bfh_story* new_story, uint32_t old_slot, uint32_t new_slot);
+
 /* One frontier pass over the batch through bf_eval (or, in resident mode, bf_resident_*) (eval_flags: BF_EVAL_*). */
 int bfh_batch_eval(bfh_batch* b, uint32_t eval_flags, bf_counts* counts);
 
