@@ -124,6 +124,13 @@ class Migration(C.Structure):
                 ("step_map", C.c_void_p), ("n_old_steps", C.c_uint32), ("migrated", C.c_uint32)]
 
 
+REDRIVE_ALL = 0xFFFFFFFF   # BF_REDRIVE_ALL: bf_redrive.step for a redrive of the whole run
+
+
+class Redrive(C.Structure):
+    _fields_ = [("run", C.c_uint32), ("slot", C.c_uint32), ("step", C.c_uint32), ("reserved", C.c_uint32)]
+
+
 class SchedTables(C.Structure):
     _fields_ = [("struct_size", C.c_uint32), ("n_stories", C.c_uint32), ("n_queues", C.c_uint32), ("global_limit", C.c_int32),
                 ("global_running_base", C.c_uint32), ("story_limit", C.c_void_p), ("story_running_base", C.c_void_p),
@@ -170,6 +177,7 @@ SYMBOLS = [
     ("bf_resident_tick_compact", C.c_int, [C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.POINTER(CompactOut), C.POINTER(Counts)]),
     ("bf_resident_tick_touched", C.c_int, [C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.POINTER(TouchedOut), C.POINTER(Counts)]),
     ("bf_resident_migrate", C.c_int, [C.c_void_p, C.c_uint32, C.POINTER(Migration)]),
+    ("bf_resident_redrive", C.c_int, [C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_void_p, C.POINTER(C.c_uint32)]),
     ("bf_group_create", C.c_int, [C.POINTER(C.c_void_p), C.POINTER(C.c_int32), C.c_uint32, C.POINTER(Config)]),
     ("bf_group_destroy", None, [C.c_void_p]),
     ("bf_group_size", C.c_uint32, [C.c_void_p]),

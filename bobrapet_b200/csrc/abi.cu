@@ -16,6 +16,7 @@
 #include <new>
 #include <thread>
 #include <string>
+#include <unordered_map>
 #include <vector>
 
 #include "../../include/bobrafrontier.h"
@@ -35,6 +36,7 @@ cudaError_t launch_touched_compact(const TouchedParams& P, cudaStream_t stream);
 cudaError_t launch_mark_runs(uint32_t* mark, uint32_t first, uint32_t n, uint32_t value, cudaStream_t stream);
 cudaError_t launch_move_records(const uint8_t* src, uint8_t* dst, const void* moves, uint32_t n, cudaStream_t stream);
 cudaError_t launch_migrate(const MigrateParams& P, cudaStream_t stream);
+cudaError_t launch_redrive(const RedriveParams& P, cudaStream_t stream);
 cudaError_t launch_schedule(const SchedParams& P, uint32_t sm_count, cudaStream_t stream, uint32_t phases = 3);
 cudaError_t launch_closure(const Slot* slots, const uint32_t* slot_ids, const uint32_t* starts, uint32_t n, uint32_t n_slots,
                            uint32_t words_out, uint32_t* masks, cudaStream_t stream);
@@ -151,6 +153,8 @@ struct bf_ctx {
   uint64_t last_touched_events = 0;   // events of the previous touched tick (sizes the first D2H)
   // migrations (bf_resident_migrate): [0, 16) the migrated-run counter | inverse step map | desc table
   uint8_t* d_mig = nullptr; size_t d_mig_cap = 0;
+  // redrives (bf_resident_redrive): statuses | requests | key per request | key slots | key steps | closure masks
+  uint8_t* d_redrive = nullptr; size_t d_redrive_cap = 0;
 
   // limiters (bf_schedule): what the last bf_eval left on the device + scratch
   bool last_eval_valid = false;
@@ -997,7 +1001,7 @@ void bf_destroy(bf_ctx* c) {
   cudaFreeHost(c->h_counts);
   cudaFree(c->arena); cudaFree(c->slots_dev); cudaFree(c->ff_dev); cudaFree(c->d_state); cudaFree(c->d_result); cudaFree(c->d_counts); cudaFree(c->d_acc);
   cudaFree(c->d_defer); cudaFree(c->d_exp); cudaFree(c->d_exp_counts); cudaFree(c->d_offsets); cudaFree(c->d_block_sums); cudaFree(c->d_sched); cudaFree(c->d_deltas); cudaFree(c->d_rejected);
-  cudaFree(c->d_head); cudaFree(c->d_events); cudaFree(c->d_cblock); cudaFree(c->d_mig);
+  cudaFree(c->d_head); cudaFree(c->d_events); cudaFree(c->d_cblock); cudaFree(c->d_mig); cudaFree(c->d_redrive);
   for (Resident& r : c->resident) { cudaFree(r.d_state); cudaFree(r.d_result); cudaFree(r.d_result_prev); }
   delete c;
 }
@@ -1888,6 +1892,82 @@ int bf_resident_migrate(bf_ctx* c, uint32_t h, bf_migration* m) {
   c->stats.kernel_launches += m->n_runs ? 1 : 0;
   m->migrated = *reinterpret_cast<const uint32_t*>(c->h_counts);
   r->pending += m->migrated;   // the touched-list bound counts the migrated runs as it counts uploaded ones
+  return BF_OK;
+}
+
+// An operator redrive of live runs (resident.cu).  All checks come first, so a rejected call changes nothing.  The distinct
+// (slot, step) keys get one closure mask each from the closure kernel (a mass redrive of one Story from one step costs one
+// closure), then one launch resets every request's set.  One H2D copy, at most two launches, one D2H copy, one synchronisation.
+int bf_resident_redrive(bf_ctx* c, uint32_t h, const bf_redrive* req, uint32_t n, uint8_t* status_out, uint32_t* applied_out) {
+  if (!c) return BF_EINVAL;
+  std::lock_guard<std::mutex> g(c->mu);
+  Resident* r = resident_of(c, h);
+  if (!r) return fail(c, BF_EINVAL, "unknown resident batch");
+  if (n && !req) return fail(c, BF_EINVAL, "null requests");
+  const bf_layout& L = r->L;
+  const bool child = L.off_child != BF_OFF_NONE;
+  std::unordered_map<uint64_t, uint32_t> key_of;   // (slot, step) -> key index
+  std::vector<uint32_t> key(n), key_slot, key_step;
+  for (uint32_t i = 0; i < n; ++i) {
+    const bf_redrive& q = req[i];
+    auto at = [i] { return "request " + std::to_string(i) + ": "; };   // built on failure only
+    if (q.run >= r->cap) return fail(c, BF_EINVAL, at() + "run outside the resident batch");
+    if (q.reserved != 0) return fail(c, BF_EINVAL, at() + "reserved must be 0");
+    if (q.slot >= c->meta.size() || !c->meta[q.slot].alive) return fail(c, BF_ETOPO, at() + "unknown topology slot");
+    const TopoMeta& m = c->meta[q.slot];
+    if (q.step != BF_REDRIVE_ALL && q.step >= m.S) return fail(c, BF_EINVAL, at() + "step index out of range");  // "step %q not found", :541
+    if (m.S > L.steps_max || (child && m.child_nibbles > L.child_nibbles))
+      return fail(c, BF_ETOPO, at() + "topology does not fit the batch layout (steps_max / child_nibbles)");
+    key[i] = BF_REDRIVE_ALL;
+    if (q.step == BF_REDRIVE_ALL) continue;
+    const auto it = key_of.emplace((uint64_t)q.slot << 32 | q.step, (uint32_t)key_slot.size());
+    if (it.second) { key_slot.push_back(q.slot); key_step.push_back(q.step); }
+    key[i] = it.first->second;
+  }
+  if (applied_out) *applied_out = 0;
+  if (n == 0) return BF_OK;
+  BF_CUDA(c, cudaSetDevice(c->device));
+  if (int rc = sync_slots(c, c->stream)) return rc;
+  const size_t K = key_slot.size();
+  const size_t o_req = round_up_sz(n, 16), o_key = o_req + (size_t)n * sizeof(bf_redrive), o_ks = o_key + (size_t)n * 4,
+               o_mask = round_up_sz(o_ks + K * 8, 16), bytes = o_mask + K * L.words * 4;
+  if (int rc = ensure_dev(c, c->d_redrive, c->d_redrive_cap, bytes)) return rc;
+  std::vector<uint8_t> blob(o_mask - o_req);   // requests | keys | key slots | key steps (the statuses are written by the kernel)
+  memcpy(blob.data(), req, (size_t)n * sizeof(bf_redrive));
+  memcpy(blob.data() + (o_key - o_req), key.data(), (size_t)n * 4);
+  if (K) {
+    memcpy(blob.data() + (o_ks - o_req), key_slot.data(), K * 4);
+    memcpy(blob.data() + (o_ks - o_req) + K * 4, key_step.data(), K * 4);
+  }
+  if (c->last_state == r->d_state) c->last_eval_valid = false;   // as after an upload: bf_schedule must follow a new pass
+  uint8_t* d = c->d_redrive;
+  uint32_t* d_ks = reinterpret_cast<uint32_t*>(d + o_ks);
+  uint32_t* d_mask = reinterpret_cast<uint32_t*>(d + o_mask);
+  bf::RedriveParams P{};
+  P.state = r->d_state; P.mark = r->d_mark; P.mark_value = r->epoch << 1;   // touched, as by a delta
+  P.req = reinterpret_cast<const bf_redrive*>(d + o_req); P.key = reinterpret_cast<const uint32_t*>(d + o_key);
+  P.masks = d_mask; P.status = d; P.slots = c->slots_dev; P.n = n;
+  P.words = L.words; P.state_stride = L.state_stride; P.off_phase = L.off_phase; P.off_cond = L.off_cond;
+  P.off_decision = L.off_decision; P.off_child = L.off_child;
+  std::vector<uint8_t> status(n);
+  cudaStream_t s = c->stream;
+  cudaError_t e = cudaMemcpyAsync(d + o_req, blob.data(), blob.size(), cudaMemcpyHostToDevice, s);
+  if (e == cudaSuccess)
+    e = bf::launch_closure(c->slots_dev, d_ks, d_ks + K, (uint32_t)K, (uint32_t)c->slots_host.size(), L.words, d_mask, s);
+  if (e == cudaSuccess) e = bf::launch_redrive(P, s);
+  if (e == cudaSuccess) e = cudaMemcpyAsync(status.data(), d, n, cudaMemcpyDeviceToHost, s);
+  const cudaError_t es = cudaStreamSynchronize(s);
+  if (e == cudaSuccess) e = es;
+  if (e != cudaSuccess) {   // some records may have been reset: the next touched tick evaluates and lists every run
+    r->need_full = true; r->prev_valid = false;
+    return cuda_fail(c, e, "bf_resident_redrive");
+  }
+  c->stats.kernel_launches += K ? 2 : 1;
+  uint32_t applied = 0;
+  for (uint32_t i = 0; i < n; ++i) applied += status[i];
+  if (status_out) memcpy(status_out, status.data(), n);
+  if (applied_out) *applied_out = applied;
+  r->pending += applied;   // the touched-list bound counts the reset runs as it counts deltas
   return BF_OK;
 }
 

@@ -221,6 +221,20 @@ struct MigrateParams {
   uint32_t child_nibbles;        // of the layout; the child area is ceil(child_nibbles / 8) u32 words
 };
 
+// bf_resident_redrive (resident.cu): the reset sets of the requests are cleared in the records of their runs
+struct RedriveParams {
+  uint8_t* state;
+  uint32_t* mark;                // touch marks: an applied request raises its run's to mark_value (touched, as by a delta)
+  uint32_t mark_value;
+  const bf_redrive* req;         // [n]
+  const uint32_t* key;           // [n] row of `masks` holding request i's reset set, or BF_REDRIVE_ALL
+  const uint32_t* masks;         // [keys][words] closure masks (launch_closure)
+  uint8_t* status;               // [n] out: 1 = the run held the request's slot and was reset
+  const Slot* slots;
+  uint32_t n;
+  uint32_t words, state_stride, off_phase, off_cond, off_decision, off_child;
+};
+
 // limiters.cu (rows a9 / f4)
 struct SchedParams {
   const uint8_t* state;

@@ -6,6 +6,7 @@
 #include <string.h>
 
 #include <algorithm>
+#include <map>
 #include <string>
 #include <unordered_map>
 #include <vector>
@@ -653,6 +654,119 @@ int bfh_batch_migrate(bfh_batch* b, const bfh_story* os, const bfh_story* ns, ui
     }
   }
   return (int)n_moved;
+}
+
+// Reset set of a redrive from `start` (resolveRedriveFromStepSet, storyrun_controller.go:535-558): start plus every step of its
+// group reachable through the dependents edges, by a queue over the story's rows reversed.  mask: ceil(S/32) words.
+static void redrive_closure(const bfh_story* s, uint32_t start, std::vector<uint32_t>& mask) {
+  const uint32_t S = (uint32_t)s->flags.size();
+  std::vector<std::vector<uint32_t>> dependents(S);
+  for (uint32_t i = 0; i < S; ++i)
+    for (uint32_t e = s->row_ptr[i]; e < s->row_ptr[i + 1]; ++e) dependents[s->col_idx[e]].push_back(i);
+  auto group = [&](uint32_t i) { return (s->flags[i] & BF_SF_GROUP_MASK) >> BF_SF_GROUP_SHIFT; };
+  mask.assign((S + 31) / 32, 0u);
+  mask[start >> 5] |= 1u << (start & 31u);
+  std::vector<uint32_t> queue{start};
+  for (size_t k = 0; k < queue.size(); ++k)
+    for (uint32_t i : dependents[queue[k]])
+      if (group(i) == group(start) && !((mask[i >> 5] >> (i & 31u)) & 1u)) {
+        mask[i >> 5] |= 1u << (i & 31u);
+        queue.push_back(i);
+      }
+}
+
+int bfh_batch_redrive(bfh_batch* b, const uint32_t* runs, const int32_t* steps, uint32_t n) {
+  if (!b || (n && (!runs || !steps))) return BF_EINVAL;
+  const bf_layout& L = b->L;
+  const uint32_t W = L.words;
+  for (uint32_t i = 0; i < n; ++i) {
+    if (runs[i] >= b->n) { b->err = "request " + std::to_string(i) + ": run out of range"; return BF_EINVAL; }
+    if (steps[i] < -1 || (steps[i] >= 0 && (uint32_t)steps[i] >= b->story_of_run[runs[i]]->flags.size())) {
+      b->err = "request " + std::to_string(i) + ": step not found in the run's story";
+      return BF_EINVAL;
+    }
+  }
+  bool resync = false;
+  if (b->resident) {   // the device first: it fails without changes, and then the mirror stays as it was too
+    std::vector<bf_redrive> req;
+    for (uint32_t i = 0; i < n; ++i) {
+      if (runs[i] >= b->uploaded) continue;   // not on the device yet: it travels as a full record
+      bf_redrive q{};
+      q.run = runs[i];
+      q.slot = reinterpret_cast<const bf_run_header*>(b->state + (size_t)runs[i] * L.state_stride)->topo_slot;
+      q.step = steps[i] < 0 ? BF_REDRIVE_ALL : (uint32_t)steps[i];
+      req.push_back(q);
+    }
+    if (!req.empty()) {
+      std::vector<uint8_t> status(req.size());
+      uint32_t applied = 0;
+      const int rc = bf_resident_redrive(b->ctx, b->handle, req.data(), (uint32_t)req.size(), status.data(), &applied);
+      if (rc != BF_OK) { b->err = bf_last_error(b->ctx); return rc; }
+      resync = applied != req.size();   // a device record held another slot: it diverged from the mirror
+    }
+  }
+  // reset the mirror's records; reset[(run, field, index)] marks the pending deltas the reset supersedes
+  std::map<std::pair<const bfh_story*, int32_t>, std::vector<uint32_t>> closures;
+  std::unordered_map<uint64_t, bool> superseded;
+  auto key = [](uint32_t run, uint32_t field, uint32_t index) { return ((uint64_t)run << 32) | ((uint64_t)field << 16) | index; };
+  std::vector<uint8_t> reset_runs(b->n, 0);
+  for (uint32_t i = 0; i < n; ++i) {
+    const uint32_t run = runs[i];
+    const bfh_story* st = b->story_of_run[run];
+    const uint32_t S = (uint32_t)st->flags.size();
+    std::vector<uint32_t>& m = closures[{st, steps[i]}];
+    if (m.empty()) {
+      if (steps[i] < 0) {
+        m.assign((S + 31) / 32, 0u);
+        for (uint32_t j = 0; j < S; ++j) m[j >> 5] |= 1u << (j & 31u);
+      } else {
+        redrive_closure(st, (uint32_t)steps[i], m);
+      }
+    }
+    uint8_t* rec = b->state + (size_t)run * L.state_stride;
+    auto in = [&](uint32_t j) { return ((m[j >> 5] >> (j & 31u)) & 1u) != 0; };
+    for (uint32_t j = 0; j < S; ++j) {
+      if (!in(j)) continue;
+      set_code(rec + L.off_phase, W, 4, j, 0);
+      superseded[key(run, BF_DELTA_PHASE, j)] = true;
+      if (L.off_decision != BF_OFF_NONE) { set_code(rec + L.off_decision, W, 2, j, BF_DEC_PENDING); superseded[key(run, BF_DELTA_DECISION, j)] = true; }
+      if (L.off_cond != BF_OFF_NONE) {
+        set_code(rec + L.off_cond, W, 2, j, (st->flags[j] & BF_SF_HAS_IF) ? BF_COND_HOLD : BF_COND_PASS);
+        superseded[key(run, BF_DELTA_COND, j)] = true;
+      }
+    }
+    bf_run_header* h = reinterpret_cast<bf_run_header*>(rec);
+    for (size_t p = 0; p < st->par.size(); ++p) {
+      if (!in(st->par[p].step)) continue;
+      h->children_registered &= ~(1ull << p);
+      superseded[key(run, BF_DELTA_REGISTERED, (uint32_t)p)] = true;
+      if (L.off_child == BF_OFF_NONE) continue;
+      for (uint32_t br = 0; br < st->par[p].branches; ++br) {
+        const uint32_t c = st->child_first[p] + br;
+        rec[L.off_child + (c >> 1)] &= (uint8_t)~(0xFu << ((c & 1u) * 4u));
+        superseded[key(run, BF_DELTA_CHILD, c)] = true;
+      }
+    }
+    h->run_flags &= (uint8_t)~BF_RF_TOPOLOGY_TERMINATED;
+    reset_runs[run] = 1;
+  }
+  if (resync) {   // the mirror's records are the truth: the next bfh_batch_eval sends them all in full
+    b->uploaded = 0;
+    b->deltas.clear();
+    b->delta_at.clear();
+  } else if (!b->deltas.empty()) {
+    size_t keep = 0;
+    for (size_t k = 0; k < b->deltas.size(); ++k) {
+      bf_delta d = b->deltas[k];
+      if (superseded.count(key(d.run, d.field, d.index))) continue;
+      if (d.field == BF_DELTA_RUN_FLAGS && d.run < b->n && reset_runs[d.run]) d.code &= (uint8_t)~BF_RF_TOPOLOGY_TERMINATED;
+      b->deltas[keep++] = d;
+    }
+    b->deltas.resize(keep);
+    b->delta_at.clear();
+    for (size_t i = 0; i < keep; ++i) b->delta_at[key(b->deltas[i].run, b->deltas[i].field, b->deltas[i].index)] = (uint32_t)i;
+  }
+  return BF_OK;
 }
 
 int bfh_batch_set_resident(bfh_batch* b, int on) {

@@ -204,4 +204,75 @@ cudaError_t launch_migrate(const MigrateParams& P, cudaStream_t stream) {
   return cudaGetLastError();
 }
 
+// Redrive (bf_resident_redrive).  One warp per request: a run holding another slot leaves after reading its header word.  Lane w
+// takes plane word w: it reads word w of the request's reset set R (a closure mask, or the low S bits for BF_REDRIVE_ALL) and
+// clears those bits in every phase and decision plane and in cond plane 0; on cond plane 1 it clears them and then sets the ones
+// of steps with an `if` (HOLD), read from the topology's HAS_IF plane.  Lane p (and p + 32) takes parallel desc p: when its step
+// is in R it zeroes the desc's child nibbles (whole words up to the last, whose padding nibbles a masked AND keeps), and one
+// ballot per half gives the children_registered bits lane 0 clears, with BF_RF_TOPOLOGY_TERMINATED, by one atomicAnd each.
+// Requests are not sorted by run, and two requests of one run may run at once: every operation drives a bit to a value fixed per
+// (run, step) (0, or HAS_IF on cond plane 1), and each request's OR follows its own AND, so any interleaving of two requests
+// leaves the same word as applying them one after the other.  Child words outside a desc's tail are only ever stored as 0.
+__global__ void __launch_bounds__(256) redrive_runs(const RedriveParams P) {
+  const uint32_t i = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31u;
+  if (i >= P.n) return;
+  const bf_redrive q = P.req[i];
+  uint8_t* rec = P.state + (size_t)q.run * P.state_stride;
+  const bool hit = *reinterpret_cast<const uint32_t*>(rec) == q.slot;   // no request of this launch writes the slot word
+  if (lane == 0) P.status[i] = hit ? 1u : 0u;
+  if (!hit) return;
+  const uint8_t* topo = reinterpret_cast<const uint8_t*>(P.slots[q.slot].addr);
+  const TopoHeader* th = reinterpret_cast<const TopoHeader*>(topo);
+  const uint32_t S = th->S, TW = th->W, W = P.words, key = P.key[i];
+  uint32_t m = 0;   // word `lane` of R (TW <= W: the topology fits the layout)
+  if (lane < TW)
+    m = key == BF_REDRIVE_ALL ? (S - lane * 32u >= 32u ? ~0u : (1u << (S - lane * 32u)) - 1u) : P.masks[(size_t)key * W + lane];
+  if (m) {
+    uint32_t* ph = reinterpret_cast<uint32_t*>(rec + P.off_phase) + lane;
+    for (uint32_t b = 0; b < 4; ++b) atomicAnd(ph + b * W, ~m);
+    if (P.off_decision != BF_OFF_NONE) {
+      uint32_t* dc = reinterpret_cast<uint32_t*>(rec + P.off_decision) + lane;
+      atomicAnd(dc, ~m);
+      atomicAnd(dc + W, ~m);
+    }
+    if (P.off_cond != BF_OFF_NONE) {
+      uint32_t* cd = reinterpret_cast<uint32_t*>(rec + P.off_cond) + lane;
+      const uint32_t hold = m & reinterpret_cast<const uint32_t*>(topo + th->off_planes)[PL_HASIF * TW + lane];
+      atomicAnd(cd, ~m);
+      atomicAnd(cd + W, ~m);
+      if (hold) atomicOr(cd + W, hold);
+    }
+  }
+  const ParDesc* pd = reinterpret_cast<const ParDesc*>(topo + th->off_par);
+  const uint32_t n_par = th->P;
+  uint32_t reg[2];
+  for (uint32_t h = 0; h < 2; ++h) {   // BF_MAX_PARALLEL = 64 descs: lane p and lane p + 32
+    const uint32_t p = lane + 32u * h;
+    const ParDesc d = p < n_par ? pd[p] : ParDesc{};
+    const uint32_t mw = __shfl_sync(0xFFFFFFFFu, m, (d.step >> 5) & 31u);
+    const bool in = p < n_par && ((mw >> (d.step & 31u)) & 1u);
+    reg[h] = __ballot_sync(0xFFFFFFFFu, in);
+    if (in && P.off_child != BF_OFF_NONE) {
+      uint32_t* cw = reinterpret_cast<uint32_t*>(rec + P.off_child) + d.child_first / 8u;   // child_first: a multiple of 8 nibbles
+      const uint32_t nw = (d.branches + 7u) / 8u, tail = d.branches & 7u;
+      for (uint32_t k = 0; k < nw; ++k) {
+        if (k == nw - 1u && tail) atomicAnd(cw + k, ~((1u << (4u * tail)) - 1u));
+        else cw[k] = 0u;
+      }
+    }
+  }
+  if (lane == 0) {
+    const unsigned long long gone = (unsigned long long)reg[1] << 32 | reg[0];
+    if (gone) atomicAnd(reinterpret_cast<unsigned long long*>(rec + 8), ~gone);
+    atomicAnd(reinterpret_cast<uint32_t*>(rec + 4), ~(uint32_t)BF_RF_TOPOLOGY_TERMINATED);   // run_flags is the low byte
+    atomicMax(P.mark + q.run, P.mark_value);   // max: an upload's "must list" bit stays
+  }
+}
+
+cudaError_t launch_redrive(const RedriveParams& P, cudaStream_t stream) {
+  if (P.n == 0) return cudaSuccess;
+  redrive_runs<<<(P.n + 7) / 8, 256, 0, stream>>>(P);
+  return cudaGetLastError();
+}
+
 }  // namespace bf

@@ -228,6 +228,18 @@ class Frontier:
         self._check(self._lib.bf_resident_migrate(self._ctx, handle, C.byref(m)), "bf_resident_migrate")
         return int(m.migrated)
 
+    REDRIVE_DTYPE = np.dtype([("run", "<u4"), ("slot", "<u4"), ("step", "<u4"), ("reserved", "<u4")])
+
+    def resident_redrive(self, handle: int, requests: np.ndarray):
+        """bf_resident_redrive: reset, in place, the step set of each request (run, slot, step or A.REDRIVE_ALL) in the records of
+        the runs that hold the request's slot.  -> (status [n] uint8: 1 = applied, 0 = the run holds another slot; applied)"""
+        rq = np.ascontiguousarray(requests, dtype=self.REDRIVE_DTYPE)
+        status = np.zeros(max(rq.shape[0], 1), dtype=np.uint8)
+        applied = C.c_uint32()
+        self._check(self._lib.bf_resident_redrive(self._ctx, handle, rq.ctypes.data, rq.shape[0], status.ctypes.data,
+                                                  C.byref(applied)), "bf_resident_redrive")
+        return status[:rq.shape[0]], int(applied.value)
+
     # -- resident batches: device-side state, delta uploads (row f2)
     DELTA_DTYPE = np.dtype([("run", "<u4"), ("index", "<u2"), ("field", "u1"), ("code", "u1")])
 

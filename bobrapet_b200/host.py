@@ -43,6 +43,7 @@ _SYMS = [
     ("bfh_run_set_child_phase", C.c_int, [C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32, C.c_char_p]),
     ("bfh_story_migration_map", C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32]),
     ("bfh_batch_migrate", C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32, C.c_uint32]),
+    ("bfh_batch_redrive", C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32]),
     ("bfh_batch_eval", C.c_int, [C.c_void_p, C.c_uint32, C.POINTER(A.Counts)]),
     ("bfh_batch_set_resident", C.c_int, [C.c_void_p, C.c_int]),
     ("bfh_batch_traffic", C.c_int, [C.c_void_p, C.POINTER(C.c_uint64), C.POINTER(C.c_uint64), C.POINTER(C.c_uint32)]),
@@ -240,6 +241,14 @@ class HostBatch:
     def migrate(self, old: HostStory, new: HostStory, old_slot: int, new_slot: int) -> int:
         """bfh_batch_migrate: move the runs on old_slot to `new` / new_slot (in resident mode on the device too) -> runs moved"""
         return self._chk(self._l.bfh_batch_migrate(self._p, old._p, new._p, old_slot, new_slot), "bfh_batch_migrate")
+
+    def redrive(self, runs, steps) -> None:
+        """bfh_batch_redrive: reset runs[i] from step steps[i] (an index of its story) or, for -1, the whole run (in resident
+        mode on the device too)"""
+        r = np.ascontiguousarray(runs, dtype=np.uint32)
+        s = np.ascontiguousarray(steps, dtype=np.int32)
+        assert r.shape == s.shape
+        self._chk(self._l.bfh_batch_redrive(self._p, r.ctypes.data, s.ctypes.data, r.shape[0]), "bfh_batch_redrive")
 
     def size(self) -> int:
         return self._l.bfh_batch_size(self._p)

@@ -343,6 +343,40 @@ func (r *Resident) Migrate(oldSlot, newSlot uint32, stepMap []uint16, n uint32) 
 	return uint32(m), r.c.err(rc)
 }
 
+// RedriveAll is the Redrive.Step of a redrive of the whole run (BF_REDRIVE_ALL, resetStoryRunForRedrive).
+const RedriveAll = 0xFFFFFFFF
+
+// Redrive is one request of Resident.Redrive (bf_redrive, 16 bytes): reset run Run, held on topology slot Slot, from step
+// Step (an allStorySteps index: the step and everything downstream of it in its group) or, with RedriveAll, entirely.
+type Redrive struct {
+	Run      uint32
+	Slot     uint32
+	Step     uint32
+	Reserved uint32 // 0
+}
+
+// Redrive applies operator redrives to live runs on the device: the reset steps lose their phase, gate decision and
+// primitive children, their cond codes become HOLD (steps with an `if`) or PASS, and the TopologyTerminated flag is cleared.
+// Call it once the reference's cleanup of the StepRuns and child StoryRuns has finished, then patch the observed annotation.
+// status (nil, or at least len(reqs) long) receives 1 per applied request and 0 for a run that no longer holds the slot.
+// The next TickTouched evaluates the reset runs and lists the ones whose result changed.
+func (r *Resident) Redrive(reqs []Redrive, status []uint8) (applied uint32, err error) {
+	if status != nil && len(status) < len(reqs) {
+		return 0, fmt.Errorf("frontier: status holds %d entries for %d requests", len(status), len(reqs))
+	}
+	var rp *C.bf_redrive
+	if len(reqs) > 0 {
+		rp = (*C.bf_redrive)(unsafe.Pointer(&reqs[0]))
+	}
+	var sp *C.uint8_t
+	if len(status) > 0 {
+		sp = (*C.uint8_t)(unsafe.Pointer(&status[0]))
+	}
+	var a C.uint32_t
+	rc := C.bfgo_resident_redrive(r.c.p, r.handle, rp, C.uint32_t(len(reqs)), sp, &a)
+	return uint32(a), r.c.err(rc)
+}
+
 // Group is one operator process driving several GPUs (bf_group_*): contiguous blocks of runs per device, one NCCL
 // all-gather of the per-shard counts per pass, limiter totals all-reduced across the shards.
 type Group struct{ p *C.bf_group }

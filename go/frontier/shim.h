@@ -108,6 +108,12 @@ static inline int bfgo_resident_migrate(bf_ctx* c, uint32_t handle, uint32_t old
   return rc;
 }
 
+static inline int bfgo_resident_redrive(bf_ctx* c, uint32_t handle, const bf_redrive* requests, uint32_t n, uint8_t* status,
+                                        uint32_t* applied) {
+  *applied = 0;
+  return bf_resident_redrive(c, handle, requests, n, status, applied);
+}
+
 static inline void bfgo_tables(bf_sched_tables* t, uint32_t n_stories, uint32_t n_queues, int32_t global_limit, uint32_t global_base,
                                const int32_t* story_limit, const uint32_t* story_base, const int32_t* queue_limit,
                                const int32_t* queue_aging_s, const uint32_t* queue_base, const int32_t* queue_max_priority_base) {

@@ -564,6 +564,43 @@ typedef struct bf_migration {
 
 int bf_resident_migrate(bf_ctx* ctx, uint32_t handle, bf_migration* m);
 
+/* ------------------------------------------------------------------ redrives (an operator re-drives a live run)
+ * Redrive from a step (annotation <step>:<token>, handleRedriveFromStepIfRequested, storyrun_controller.go:293-348): the reset
+ * set R is the step plus everything downstream of it inside its own group (resolveRedriveFromStepSet :535-558, the set
+ * bf_topology_closure returns), and resetStoryRunForStepRedrive (:740-789) deletes StepStates, Gates and PrimitiveChildren of
+ * every step of R and clears Conditions.  Redrive of the whole run (token annotation, resetStoryRunForRedrive :415-439) clears
+ * all four for every step: step = BF_REDRIVE_ALL, R = every step of the topology.
+ * For each request whose run's header holds `slot` (status_out[i] = 1) bf_resident_redrive sets, in place on the device:
+ *   - the phase code of every step of R to 0 (delete(StepStates, ...));
+ *   - the decision code to BF_DEC_PENDING (delete(Gates, ...)), when the layout has decision planes;
+ *   - the cond code, when the layout has cond planes, to BF_COND_HOLD for steps with BF_SF_HAS_IF and BF_COND_PASS for the
+ *     others.  Cond codes are host inputs, not reference state: those of R were computed from outputs the redrive discards
+ *     (their StepRuns are deleted).  HOLD is what the lazy needs_cond protocol gives an `if` the host has not evaluated yet,
+ *     so no redriven `if` step launches on a stale verdict; the host sends the fresh cond code as a delta when it has one;
+ *   - the children_registered bit of every parallel desc whose step is in R to 0, and that desc's child nibbles to 0
+ *     (delete(PrimitiveChildren, ...)); nibbles past the desc's branches (padding) are kept;
+ *   - BF_RF_TOPOLOGY_TERMINATED in run_flags to 0 (Conditions = nil: the Degraded/TopologyTerminated condition, dag.go:436-464).
+ * Every other run_flags bit, the slot and every step outside R are unchanged.  A request whose run holds another slot (stale
+ * request, dead slot, never uploaded) changes nothing and gets status_out[i] = 0.  Several requests may name the same run: the
+ * result is the union of their resets (each reset is idempotent, as the reference's annotations applied one at a time are).
+ * Checked before anything runs, else BF_EINVAL / BF_ETOPO and nothing changed: the handle; run < capacity; slot alive;
+ * step < S of slot or BF_REDRIVE_ALL ("step %q not found", :539-541); reserved == 0; the slot's topology fits the batch layout
+ * (steps_max, child_nibbles).  *applied_out = the requests with status 1.
+ * Ordering: a redrive applies at the call; deltas given afterwards (bf_resident_apply, the next tick) apply after it.  Applied
+ * runs are touched as by a delta: the next bf_resident_tick_touched evaluates them and lists those whose result changed.  Like
+ * an upload, the call ends the evaluated snapshot (bf_schedule must follow a new pass).  One H2D copy, the closure launch
+ * (when a request names a step), one redrive launch, one D2H copy and one synchronisation.                              */
+#define BF_REDRIVE_ALL 0xFFFFFFFFu
+typedef struct bf_redrive {    /* 16 B, no pointers                                                                   */
+  uint32_t run;                /* index in the resident batch                                                         */
+  uint32_t slot;               /* topology slot the caller holds the run on                                           */
+  uint32_t step;               /* allStorySteps index of the redrive-from step, or BF_REDRIVE_ALL (the whole run)     */
+  uint32_t reserved;           /* 0                                                                                   */
+} bf_redrive;
+
+int bf_resident_redrive(bf_ctx* ctx, uint32_t handle, const bf_redrive* requests, uint32_t n, uint8_t* status_out,
+                        uint32_t* applied_out);
+
 /* ------------------------------------------------------------------ device groups (SURVEY.md row e)
  * The reference is ONE operator process (cmd/main.go:220, StoryRunReconciler storyrun_controller.go:216), so the
  * multi-GPU path must be reachable from one process through this ABI: a group owns one ctx per device and an NCCL

@@ -108,6 +108,16 @@ int bfh_batch_traffic(const bfh_batch* b, uint64_t* full_record_bytes, uint64_t*
 int bfh_story_migration_map(const bfh_story* old_story, const bfh_story* new_story, uint16_t* map, uint32_t cap);
 int bfh_batch_migrate(bfh_batch* b, const bfh_story* old_story, const bfh_story* new_story, uint32_t old_slot, uint32_t new_slot);
 
+/* An operator redrive of live runs (see bf_resident_redrive).  Request i resets run runs[i] from step steps[i] (an index of the
+ * run's story) or, for steps[i] = -1, the whole run.  The mirror re-packs its own records by the rules of bf_resident_redrive,
+ * with the reset set computed here from the story's dependency rows; it drops the pending deltas that would undo the reset when
+ * sent (phase / cond / decision of reset steps, child phases and registered bits of reset parallel steps) and clears
+ * BF_RF_TOPOLOGY_TERMINATED in a pending run-flags delta; other pending deltas still apply after the reset.  In resident mode it
+ * also calls bf_resident_redrive once for the uploaded runs, so that the device and the mirror stay identical; should a device
+ * record not hold the slot the mirror holds (a copy changed behind the mirror's back), the next bfh_batch_eval uploads every
+ * record in full.  A run or step out of range is BF_EINVAL and changes nothing.  Returns BF_OK.                            */
+int bfh_batch_redrive(bfh_batch* b, const uint32_t* runs, const int32_t* steps, uint32_t n);
+
 /* One frontier pass over the batch through bf_eval (or, in resident mode, bf_resident_*) (eval_flags: BF_EVAL_*). */
 int bfh_batch_eval(bfh_batch* b, uint32_t eval_flags, bf_counts* counts);
 
