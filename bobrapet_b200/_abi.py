@@ -178,6 +178,7 @@ SYMBOLS = [
     ("bf_resident_tick_touched", C.c_int, [C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.POINTER(TouchedOut), C.POINTER(Counts)]),
     ("bf_resident_migrate", C.c_int, [C.c_void_p, C.c_uint32, C.POINTER(Migration)]),
     ("bf_resident_redrive", C.c_int, [C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_void_p, C.POINTER(C.c_uint32)]),
+    ("bf_resident_reshape", C.c_int, [C.c_void_p, C.c_uint32, C.POINTER(Layout), C.c_uint32]),
     ("bf_group_create", C.c_int, [C.POINTER(C.c_void_p), C.POINTER(C.c_int32), C.c_uint32, C.POINTER(Config)]),
     ("bf_group_destroy", None, [C.c_void_p]),
     ("bf_group_size", C.c_uint32, [C.c_void_p]),

@@ -37,6 +37,7 @@ cudaError_t launch_mark_runs(uint32_t* mark, uint32_t first, uint32_t n, uint32_
 cudaError_t launch_move_records(const uint8_t* src, uint8_t* dst, const void* moves, uint32_t n, cudaStream_t stream);
 cudaError_t launch_migrate(const MigrateParams& P, cudaStream_t stream);
 cudaError_t launch_redrive(const RedriveParams& P, cudaStream_t stream);
+cudaError_t launch_reshape(const ReshapeParams& P, cudaStream_t stream);
 cudaError_t launch_schedule(const SchedParams& P, uint32_t sm_count, cudaStream_t stream, uint32_t phases = 3);
 cudaError_t launch_closure(const Slot* slots, const uint32_t* slot_ids, const uint32_t* starts, uint32_t n, uint32_t n_slots,
                            uint32_t words_out, uint32_t* masks, cudaStream_t stream);
@@ -65,7 +66,8 @@ struct Resident {  // a device-resident batch (row f2)
   uint32_t* d_mark = nullptr;        // [cap rounded up to 4]
   uint32_t epoch = 1, full_epoch = 0;
   uint32_t full_runs = 0;            // runs the last full tick evaluated
-  bool need_full = true;             // no tick yet, or a tick failed: the current records are not known to be complete
+  bool need_full = true;             // no tick yet, a tick failed, or a reshape added decision planes or output fields: the
+                                     // current records are not known to be complete
   uint32_t last_fixpoint = 0, last_max_iter = 0;   // BF_EVAL_FIXPOINT and max_iterations of the last tick
   uint64_t drops_seen = 0;           // bf_ctx::topo_drops at the last full tick
   uint64_t pending = 0;              // bound on the touched runs: those the last touched tick left at or above its n_runs (its
@@ -1968,6 +1970,65 @@ int bf_resident_redrive(bf_ctx* c, uint32_t h, const bf_redrive* req, uint32_t n
   if (status_out) memcpy(status_out, status.data(), n);
   if (applied_out) *applied_out = applied;
   r->pending += applied;   // the touched-list bound counts the reset runs as it counts deltas
+  return BF_OK;
+}
+
+// A live batch grows its capacity and / or layout (resident.cu).  All checks come first, and the new buffers are allocated and
+// filled before the old ones are freed, so a rejected or failed call changes nothing.  One launch (both record arrays), one
+// device copy of the touch marks, one synchronisation.
+int bf_resident_reshape(bf_ctx* c, uint32_t h, const bf_layout* layout, uint32_t capacity) {
+  if (!c) return BF_EINVAL;
+  std::lock_guard<std::mutex> g(c->mu);
+  Resident* r = resident_of(c, h);
+  if (!r) return fail(c, BF_EINVAL, "unknown resident batch");
+  if (!layout) return fail(c, BF_EINVAL, "null layout");
+  if (int rc = check_layout(c, *layout)) return rc;
+  const bf_layout F = r->L, T = *layout;
+  if (capacity < r->cap) return fail(c, BF_EINVAL, "reshape cannot lower the capacity");
+  if (T.steps_max < F.steps_max) return fail(c, BF_EINVAL, "reshape cannot lower steps_max");
+  if (F.fields & ~T.fields) return fail(c, BF_EINVAL, "reshape cannot drop a field");
+  if (F.off_child != BF_OFF_NONE && T.child_nibbles < F.child_nibbles) return fail(c, BF_EINVAL, "reshape cannot shrink the child area");
+  // the kernel follows the offsets: every field the batch places must have a place in the new layout
+  const uint32_t from[] = {F.off_cond, F.off_decision, F.off_child, F.off_fail, F.off_needs_cond, F.off_skip_dep, F.off_phase_out};
+  const uint32_t to[] = {T.off_cond, T.off_decision, T.off_child, T.off_fail, T.off_needs_cond, T.off_skip_dep, T.off_phase_out};
+  // zero decision planes are PENDING, which a pass applies to RUNNING gate / sleep / wait steps (an absent plane leaves them
+  // alone), and added output masks may gain bits: either may change a result the touch marks know nothing of
+  bool results_may_change = false;
+  for (int i = 0; i < 7; ++i) {
+    if (from[i] != BF_OFF_NONE && to[i] == BF_OFF_NONE) return fail(c, BF_EINVAL, "the new layout drops a field the batch has");
+    if (i != 0 && i != 2 && from[i] == BF_OFF_NONE && to[i] != BF_OFF_NONE) results_may_change = true;
+  }
+  BF_CUDA(c, cudaSetDevice(c->device));
+  const size_t old_mark = ((size_t)r->cap + 3) / 4 * 16, new_mark = ((size_t)capacity + 3) / 4 * 16;   // as bf_resident_create
+  uint8_t *st = nullptr, *res = nullptr;
+  uint32_t* mk = nullptr;
+  cudaError_t e = cudaMalloc(&st, (size_t)capacity * T.state_stride);
+  if (e == cudaSuccess) e = cudaMalloc(&res, (size_t)capacity * T.result_stride);
+  if (e == cudaSuccess) e = cudaMalloc(&mk, new_mark);
+  if (e != cudaSuccess) {
+    cudaFree(st); cudaFree(res); cudaFree(mk);
+    cudaGetLastError();   // an allocation failure is not a launch failure of the next call
+    return fail(c, BF_ENOMEM, std::string("resident reshape: ") + cudaGetErrorString(e));
+  }
+  bf::ReshapeParams P{};
+  P.old_state = r->d_state; P.old_result = r->d_result; P.state = st; P.result = res;
+  P.n_old = r->cap; P.n_new = capacity; P.from = F; P.to = T;
+  cudaStream_t s = c->stream;
+  e = bf::launch_reshape(P, s);
+  if (e == cudaSuccess) e = cudaMemcpyAsync(mk, r->d_mark, old_mark, cudaMemcpyDeviceToDevice, s);   // with the list-build padding
+  if (e == cudaSuccess && new_mark > old_mark) e = cudaMemsetAsync(reinterpret_cast<uint8_t*>(mk) + old_mark, 0, new_mark - old_mark, s);
+  const cudaError_t es = cudaStreamSynchronize(s);
+  if (e == cudaSuccess) e = es;
+  if (e != cudaSuccess) {   // the old buffers were only read: the batch is as it was
+    cudaFree(st); cudaFree(res); cudaFree(mk);
+    return cuda_fail(c, e, "bf_resident_reshape");
+  }
+  if (c->last_state == r->d_state) c->last_eval_valid = false;   // as after an upload: bf_schedule must follow a new pass
+  cudaFree(r->d_state); cudaFree(r->d_result); cudaFree(r->d_result_prev); cudaFree(r->d_mark);
+  r->d_state = st; r->d_result = res; r->d_mark = mk;
+  r->d_result_prev = nullptr;   // never read before a pass overwrites it: allocated at the new size when next used
+  r->L = T; r->cap = capacity;
+  if (results_may_change) r->need_full = true;
   return BF_OK;
 }
 

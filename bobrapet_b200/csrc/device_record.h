@@ -235,6 +235,16 @@ struct RedriveParams {
   uint32_t words, state_stride, off_phase, off_cond, off_decision, off_child;
 };
 
+// bf_resident_reshape (resident.cu): both record arrays re-laid from layout `from` into new buffers at layout `to`
+struct ReshapeParams {
+  const uint8_t* old_state;
+  const uint8_t* old_result;
+  uint8_t* state;                // [n_new][to.state_stride]
+  uint8_t* result;               // [n_new][to.result_stride]
+  uint32_t n_old, n_new;         // runs r >= n_old get zero records
+  bf_layout from, to;
+};
+
 // limiters.cu (rows a9 / f4)
 struct SchedParams {
   const uint8_t* state;

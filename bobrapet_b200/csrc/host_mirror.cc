@@ -359,30 +359,40 @@ int bfh_scan_step_refs(const char* expression, char* out, size_t cap) {
 }
 
 // ------------------------------------------------------------------------------------------ Batch
+// Zeroed state and result arrays of a batch: pinned when a ctx is given and can pin them, else plain host memory.
+static bool alloc_records(bf_ctx* ctx, size_t sb, size_t rb, uint8_t** state, uint8_t** result, bool* pinned) {
+  void *ps = nullptr, *pr = nullptr;
+  *pinned = ctx && bf_alloc_pinned(ctx, sb, &ps) == BF_OK && bf_alloc_pinned(ctx, rb, &pr) == BF_OK;
+  if (!*pinned) {
+    if (ctx && ps) bf_free_pinned(ctx, ps);
+    ps = malloc(sb); pr = malloc(rb);
+    if (!ps || !pr) { free(ps); free(pr); return false; }
+  }
+  *state = static_cast<uint8_t*>(ps); *result = static_cast<uint8_t*>(pr);
+  memset(ps, 0, sb); memset(pr, 0, rb);
+  return true;
+}
+static void free_records(bfh_batch* b) {
+  if (b->pinned) { bf_free_pinned(b->ctx, b->state); bf_free_pinned(b->ctx, b->result); }
+  else { free(b->state); free(b->result); }
+}
+
 bfh_batch* bfh_batch_new(bf_ctx* ctx, uint32_t steps_max, uint32_t child_nibbles, uint32_t fields, uint32_t capacity) {
   bfh_batch* b = new (std::nothrow) bfh_batch();
   if (!b) return nullptr;
   b->ctx = ctx;
   if (bf_layout_init(&b->L, steps_max, child_nibbles, fields) != BF_OK || capacity == 0) { delete b; return nullptr; }
   b->cap = capacity;
-  const size_t sb = (size_t)capacity * b->L.state_stride, rb = (size_t)capacity * b->L.result_stride;
-  void *ps = nullptr, *pr = nullptr;
-  if (ctx && bf_alloc_pinned(ctx, sb, &ps) == BF_OK && bf_alloc_pinned(ctx, rb, &pr) == BF_OK) {
-    b->pinned = true;
-  } else {
-    if (ctx && ps) bf_free_pinned(ctx, ps);
-    ps = malloc(sb); pr = malloc(rb);
-    if (!ps || !pr) { free(ps); free(pr); delete b; return nullptr; }
+  if (!alloc_records(ctx, (size_t)capacity * b->L.state_stride, (size_t)capacity * b->L.result_stride, &b->state, &b->result, &b->pinned)) {
+    delete b;
+    return nullptr;
   }
-  b->state = static_cast<uint8_t*>(ps); b->result = static_cast<uint8_t*>(pr);
-  memset(b->state, 0, sb); memset(b->result, 0, rb);
   return b;
 }
 void bfh_batch_free(bfh_batch* b) {
   if (!b) return;
   if (b->resident) bf_resident_destroy(b->ctx, b->handle);
-  if (b->pinned) { bf_free_pinned(b->ctx, b->state); bf_free_pinned(b->ctx, b->result); }
-  else { free(b->state); free(b->result); }
+  free_records(b);
   delete b;
 }
 const char* bfh_batch_error(const bfh_batch* b) { return b ? b->err.c_str() : "null batch"; }
@@ -766,6 +776,62 @@ int bfh_batch_redrive(bfh_batch* b, const uint32_t* runs, const int32_t* steps, 
     b->delta_at.clear();
     for (size_t i = 0; i < keep; ++i) b->delta_at[key(b->deltas[i].run, b->deltas[i].field, b->deltas[i].index)] = (uint32_t)i;
   }
+  return BF_OK;
+}
+
+// Plane field of a record re-laid from `from_off` (Wo words per plane) to `to_off` (Wn words per plane, zeroed): each plane
+// keeps its old words, the words above them stay 0; a field the old layout lacks stays 0.
+static void relay_planes(uint8_t* dst, const uint8_t* src, uint32_t to_off, uint32_t from_off, uint32_t planes, uint32_t Wn, uint32_t Wo) {
+  if (to_off == BF_OFF_NONE || from_off == BF_OFF_NONE) return;
+  for (uint32_t p = 0; p < planes; ++p) memcpy(dst + to_off + (size_t)p * Wn * 4, src + from_off + (size_t)p * Wo * 4, (size_t)Wo * 4);
+}
+
+int bfh_batch_reshape(bfh_batch* b, uint32_t steps_max, uint32_t child_nibbles, uint32_t fields, uint32_t capacity) {
+  if (!b) return BF_EINVAL;
+  bf_layout T;
+  if (bf_layout_init(&T, steps_max, child_nibbles, fields) != BF_OK) { b->err = "steps_max out of range"; return BF_EINVAL; }
+  const bf_layout F = b->L;
+  if (capacity < b->cap || T.steps_max < F.steps_max || (F.fields & ~T.fields) ||
+      (F.off_child != BF_OFF_NONE && T.child_nibbles < F.child_nibbles)) {
+    b->err = "a reshape only grows the batch (capacity, steps_max, fields, child_nibbles)";
+    return BF_EINVAL;
+  }
+  uint8_t *st = nullptr, *res = nullptr;
+  bool pinned = false;
+  if (!alloc_records(b->ctx, (size_t)capacity * T.state_stride, (size_t)capacity * T.result_stride, &st, &res, &pinned)) {
+    b->err = "out of host memory";
+    return BF_ENOMEM;
+  }
+  if (b->resident) {   // the device first: it fails without changes, and then the mirror stays as it was too
+    const int rc = bf_resident_reshape(b->ctx, b->handle, &T, capacity);
+    if (rc != BF_OK) {
+      b->err = bf_last_error(b->ctx);
+      if (pinned) { bf_free_pinned(b->ctx, st); bf_free_pinned(b->ctx, res); } else { free(st); free(res); }
+      return rc;
+    }
+  }
+  const uint32_t Wn = T.words, Wo = F.words;
+  for (uint32_t r = 0; r < b->cap; ++r) {
+    const uint8_t* s = b->state + (size_t)r * F.state_stride;
+    uint8_t* d = st + (size_t)r * T.state_stride;
+    memcpy(d, s, sizeof(bf_run_header));
+    relay_planes(d, s, T.off_phase, F.off_phase, 4, Wn, Wo);
+    relay_planes(d, s, T.off_cond, F.off_cond, 2, Wn, Wo);
+    relay_planes(d, s, T.off_decision, F.off_decision, 2, Wn, Wo);
+    if (F.off_child != BF_OFF_NONE) memcpy(d + T.off_child, s + F.off_child, ((F.child_nibbles + 1) / 2 + 3) / 4 * 4);
+    s = b->result + (size_t)r * F.result_stride;
+    d = res + (size_t)r * T.result_stride;
+    memcpy(d, s, sizeof(bf_result_header));
+    relay_planes(d, s, T.off_ready, F.off_ready, 1, Wn, Wo);
+    relay_planes(d, s, T.off_skip, F.off_skip, 1, Wn, Wo);
+    relay_planes(d, s, T.off_fail, F.off_fail, 1, Wn, Wo);
+    relay_planes(d, s, T.off_needs_cond, F.off_needs_cond, 1, Wn, Wo);
+    relay_planes(d, s, T.off_skip_dep, F.off_skip_dep, 1, Wn, Wo);
+    relay_planes(d, s, T.off_phase_out, F.off_phase_out, 4, Wn, Wo);
+  }
+  free_records(b);
+  b->state = st; b->result = res; b->pinned = pinned;
+  b->L = T; b->cap = capacity;
   return BF_OK;
 }
 

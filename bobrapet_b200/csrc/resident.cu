@@ -275,4 +275,64 @@ cudaError_t launch_redrive(const RedriveParams& P, cudaStream_t stream) {
   return cudaGetLastError();
 }
 
+// Reshape (bf_resident_reshape).  Each new record word is computed from its byte offset o alone, so any pair of layouts that
+// pass check_layout works and every word is stored once.  A plane field [to_off, to_off + planes * Wn * 4): word w of plane p
+// is word w of plane p at from_off when w < Wo and the old layout has the field, else 0.
+DI bool reshape_planes(const uint32_t* src, uint32_t o, uint32_t to_off, uint32_t from_off, uint32_t planes, uint32_t Wn,
+                       uint32_t Wo, uint32_t& v) {
+  if (to_off == BF_OFF_NONE || o < to_off || o >= to_off + planes * Wn * 4u) return false;
+  const uint32_t k = (o - to_off) >> 2, p = k / Wn, w = k - p * Wn;
+  v = from_off != BF_OFF_NONE && w < Wo ? src[(from_off >> 2) + p * Wo + w] : 0u;
+  return true;
+}
+DI uint32_t child_area_words(const bf_layout& L) { return ((L.child_nibbles + 1u) / 2u + 3u) / 4u; }
+
+DI uint32_t reshape_state_word(const uint32_t* s, uint32_t o, const bf_layout& F, const bf_layout& T) {
+  if (o < 16u) return s[o >> 2];   // bf_run_header
+  uint32_t v = 0;
+  if (reshape_planes(s, o, T.off_phase, F.off_phase, 4, T.words, F.words, v) ||
+      reshape_planes(s, o, T.off_cond, F.off_cond, 2, T.words, F.words, v) ||
+      reshape_planes(s, o, T.off_decision, F.off_decision, 2, T.words, F.words, v))
+    return v;
+  if (T.off_child != BF_OFF_NONE && o >= T.off_child && o < T.off_child + child_area_words(T) * 4u) {
+    const uint32_t k = (o - T.off_child) >> 2;   // child_first does not depend on the layout: the old bytes stay in place
+    return F.off_child != BF_OFF_NONE && k < child_area_words(F) ? s[(F.off_child >> 2) + k] : 0u;
+  }
+  return 0u;   // padding
+}
+
+DI uint32_t reshape_result_word(const uint32_t* s, uint32_t o, const bf_layout& F, const bf_layout& T) {
+  if (o < 16u) return s[o >> 2];   // bf_result_header
+  uint32_t v = 0;
+  if (reshape_planes(s, o, T.off_ready, F.off_ready, 1, T.words, F.words, v) ||
+      reshape_planes(s, o, T.off_skip, F.off_skip, 1, T.words, F.words, v) ||
+      reshape_planes(s, o, T.off_fail, F.off_fail, 1, T.words, F.words, v) ||
+      reshape_planes(s, o, T.off_needs_cond, F.off_needs_cond, 1, T.words, F.words, v) ||
+      reshape_planes(s, o, T.off_skip_dep, F.off_skip_dep, 1, T.words, F.words, v) ||
+      reshape_planes(s, o, T.off_phase_out, F.off_phase_out, 4, T.words, F.words, v))
+    return v;
+  return 0u;   // stride padding, as store_words leaves it
+}
+
+// One warp per run of the new capacity; lane t stores words t, t + 32, ... of the new state record, then of the new result
+// record (coalesced 4-byte stores; planes start on 8-byte boundaries with an odd word count, so no 16-byte vectors).
+// Runs at or above n_old get zero records.
+__global__ void __launch_bounds__(256) reshape_runs(const ReshapeParams P) {
+  const uint32_t r = blockIdx.x * 8u + (threadIdx.x >> 5), lane = threadIdx.x & 31u;
+  if (r >= P.n_new) return;
+  const bool keep = r < P.n_old;
+  const uint32_t* s = reinterpret_cast<const uint32_t*>(P.old_state + (size_t)r * P.from.state_stride);
+  uint32_t* d = reinterpret_cast<uint32_t*>(P.state + (size_t)r * P.to.state_stride);
+  for (uint32_t o = lane * 4u; o < P.to.state_stride; o += 128u) d[o >> 2] = keep ? reshape_state_word(s, o, P.from, P.to) : 0u;
+  s = reinterpret_cast<const uint32_t*>(P.old_result + (size_t)r * P.from.result_stride);
+  d = reinterpret_cast<uint32_t*>(P.result + (size_t)r * P.to.result_stride);
+  for (uint32_t o = lane * 4u; o < P.to.result_stride; o += 128u) d[o >> 2] = keep ? reshape_result_word(s, o, P.from, P.to) : 0u;
+}
+
+cudaError_t launch_reshape(const ReshapeParams& P, cudaStream_t stream) {
+  if (P.n_new == 0) return cudaSuccess;
+  reshape_runs<<<(P.n_new - 1u) / 8u + 1u, 256, 0, stream>>>(P);
+  return cudaGetLastError();
+}
+
 }  // namespace bf

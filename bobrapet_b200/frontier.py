@@ -240,6 +240,11 @@ class Frontier:
                                                   C.byref(applied)), "bf_resident_redrive")
         return status[:rq.shape[0]], int(applied.value)
 
+    def resident_reshape(self, handle: int, L: A.Layout, capacity: int):
+        """bf_resident_reshape: grow the batch to layout L (from make_layout) and `capacity` runs in place, keeping every run's
+        state, the current result records and the touch marks"""
+        self._check(self._lib.bf_resident_reshape(self._ctx, handle, C.byref(L), capacity), "bf_resident_reshape")
+
     # -- resident batches: device-side state, delta uploads (row f2)
     DELTA_DTYPE = np.dtype([("run", "<u4"), ("index", "<u2"), ("field", "u1"), ("code", "u1")])
 

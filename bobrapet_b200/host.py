@@ -44,6 +44,7 @@ _SYMS = [
     ("bfh_story_migration_map", C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32]),
     ("bfh_batch_migrate", C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32, C.c_uint32]),
     ("bfh_batch_redrive", C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32]),
+    ("bfh_batch_reshape", C.c_int, [C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32]),
     ("bfh_batch_eval", C.c_int, [C.c_void_p, C.c_uint32, C.POINTER(A.Counts)]),
     ("bfh_batch_set_resident", C.c_int, [C.c_void_p, C.c_int]),
     ("bfh_batch_traffic", C.c_int, [C.c_void_p, C.POINTER(C.c_uint64), C.POINTER(C.c_uint64), C.POINTER(C.c_uint32)]),
@@ -249,6 +250,11 @@ class HostBatch:
         s = np.ascontiguousarray(steps, dtype=np.int32)
         assert r.shape == s.shape
         self._chk(self._l.bfh_batch_redrive(self._p, r.ctypes.data, s.ctypes.data, r.shape[0]), "bfh_batch_redrive")
+
+    def reshape(self, steps_max, child_nibbles, fields, capacity) -> None:
+        """bfh_batch_reshape: grow the layout to bf_layout_init(steps_max, child_nibbles, fields) and the capacity, keeping every
+        run's records and the pending deltas (in resident mode on the device too)"""
+        self._chk(self._l.bfh_batch_reshape(self._p, steps_max, child_nibbles, fields, capacity), "bfh_batch_reshape")
 
     def size(self) -> int:
         return self._l.bfh_batch_size(self._p)

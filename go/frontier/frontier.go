@@ -377,6 +377,20 @@ func (r *Resident) Redrive(reqs []Redrive, status []uint8) (applied uint32, err 
 	return uint32(a), r.c.err(rc)
 }
 
+// Reshape grows the batch in place to the layout bf_layout_init(stepsMax, childNibbles, fields) and capacity runs, keeping
+// every run's state, the current results and the touched-tick bookkeeping (bf_resident_reshape).  Growth only: a smaller
+// capacity, steps_max or child area, or a dropped field, is an error and changes nothing.  Call it when a Story or the run
+// count does not fit, then upload or migrate.  With an output field added, the next TickTouched is a full one.
+func (r *Resident) Reshape(stepsMax, childNibbles, fields, capacity uint32) error {
+	var L C.bf_layout
+	rc := C.bfgo_resident_reshape(r.c.p, r.handle, C.uint32_t(stepsMax), C.uint32_t(childNibbles), C.uint32_t(fields),
+		C.uint32_t(capacity), &L)
+	if rc == C.BF_OK {
+		r.layout = L
+	}
+	return r.c.err(rc)
+}
+
 // Group is one operator process driving several GPUs (bf_group_*): contiguous blocks of runs per device, one NCCL
 // all-gather of the per-shard counts per pass, limiter totals all-reduced across the shards.
 type Group struct{ p *C.bf_group }

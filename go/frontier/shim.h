@@ -114,6 +114,17 @@ static inline int bfgo_resident_redrive(bf_ctx* c, uint32_t handle, const bf_red
   return bf_resident_redrive(c, handle, requests, n, status, applied);
 }
 
+/* bf_resident_reshape with the new layout built here by bf_layout_init; *layout_out receives it when the reshape succeeded. */
+static inline int bfgo_resident_reshape(bf_ctx* c, uint32_t handle, uint32_t steps_max, uint32_t child_nibbles, uint32_t fields,
+                                        uint32_t capacity, bf_layout* layout_out) {
+  bf_layout L;
+  const int rc = bf_layout_init(&L, steps_max, child_nibbles, fields);
+  if (rc != BF_OK) return rc;
+  const int rc2 = bf_resident_reshape(c, handle, &L, capacity);
+  if (rc2 == BF_OK) *layout_out = L;
+  return rc2;
+}
+
 static inline void bfgo_tables(bf_sched_tables* t, uint32_t n_stories, uint32_t n_queues, int32_t global_limit, uint32_t global_base,
                                const int32_t* story_limit, const uint32_t* story_base, const int32_t* queue_limit,
                                const int32_t* queue_aging_s, const uint32_t* queue_base, const int32_t* queue_max_priority_base) {

@@ -513,8 +513,9 @@ int bf_resident_tick_compact(bf_ctx* ctx, uint32_t handle, const bf_delta* delta
  * evaluated runs only (evals = sum of S over them).
  * The tick evaluates every run in [0, n_runs), lists them all (runs[i] = i) and sets full = 1 when: no tick has run on the batch
  * yet (or the last one failed); bf_topology_drop was called on the ctx since the last tick (a dropped slot kills its runs, a
- * reused one re-points them); BF_EVAL_FIXPOINT or max_iterations differs from the last tick's; or n_runs exceeds the run count
- * of the last full evaluation and not every run beyond it was uploaded since.  Any tick of the other kinds (bf_resident_tick,
+ * reused one re-points them); BF_EVAL_FIXPOINT or max_iterations differs from the last tick's; bf_resident_reshape added
+ * decision planes or an output field since (either may change any run's result); or n_runs exceeds the run count of the last full evaluation and not
+ * every run beyond it was uploaded since.  Any tick of the other kinds (bf_resident_tick,
  * _eval, _tick_compact) may come between touched ticks, and bf_schedule may follow a touched tick.
  * flags: BF_EVAL_FIXPOINT and BF_EVAL_NO_COUNTS only (else BF_EINVAL).  Pinned buffers are used in place as by
  * bf_resident_tick_compact; the call returns when they are filled.                                                  */
@@ -600,6 +601,34 @@ typedef struct bf_redrive {    /* 16 B, no pointers                             
 
 int bf_resident_redrive(bf_ctx* ctx, uint32_t handle, const bf_redrive* requests, uint32_t n, uint8_t* status_out,
                         uint32_t* applied_out);
+
+/* ------------------------------------------------------------------ reshapes (a live batch outgrows its shape)
+ * bf_resident_create fixes a batch's capacity and layout.  bf_resident_reshape grows both in place, keeping every run's state,
+ * the current result records and the touch marks, so that a batcher can keep the tightest layout its live Stories allow and
+ * widen it when a larger Story, a parallel step with more branches, the first `if` or gate, or more runs arrive.
+ * Growth only.  `layout` passes the checks of bf_resident_create, and else BF_EINVAL and nothing changed: a known handle;
+ * capacity >= the current capacity; layout->steps_max >= the current steps_max; layout->fields a superset of the current
+ * fields (input and output fields alike), and every field the current layout places is placed by the new one too;
+ * layout->child_nibbles >= the current child_nibbles when the batch has BF_F_CHILD.  Should an allocation fail, BF_ENOMEM and
+ * nothing changed: the new buffers are allocated before the old ones are freed, and those are freed after the copy completed.
+ * Afterwards, by the bytes:
+ *   - state record r < old capacity equals pack_state of the same codes at the new layout: the header (slot, run flags,
+ *     children_registered) as it was; each phase / cond / decision plane its old words, zero words above them; the planes of
+ *     an added field zero (the host sends the real codes as deltas); the child area its old bytes, the rest zero (child_first
+ *     does not depend on the layout: child delta indices stay valid); every other byte zero.  Records r >= old capacity are
+ *     zero, as after create.  Zero cond planes are BF_COND_PASS, which is how a pass reads absent ones; zero decision planes
+ *     are BF_DEC_PENDING, which a pass applies to RUNNING gate / sleep / wait steps where absent planes leave them alone;
+ *   - the current result records (those BF_EVAL_CHANGED_ONLY and touched ticks compare with) are re-laid out the same way:
+ *     header kept; each mask and phase_out plane its old words, zeros above them (exactly what a pass at the new layout
+ *     writes for an unchanged run); the masks of an added output field zero;
+ *   - touch marks and the touched-tick bookkeeping are kept; the runs of the new capacity start untouched.
+ * So with neither decision planes nor an output field added, the next touched tick is not full and evaluates only the runs
+ * touched before or after the call, and the next changed-only tick lists what it would have listed without it.  With
+ * decision planes or an output field added (e.g. BF_F_OUT_NEEDS_COND with BF_F_COND) the next touched tick is full; a
+ * changed-only tick lists the runs whose result changed, the zeroed new masks and planes included.  Like an upload, the call ends the evaluated snapshot (bf_schedule must follow a new pass).  bf_stats and the
+ * ctx's staging buffers are unaffected.  One launch, one device copy of the marks and one synchronisation.
+ * Shrinking a batch or dropping a field is not offered (it loses codes): create a new batch and upload.             */
+int bf_resident_reshape(bf_ctx* ctx, uint32_t handle, const bf_layout* layout, uint32_t capacity);
 
 /* ------------------------------------------------------------------ device groups (SURVEY.md row e)
  * The reference is ONE operator process (cmd/main.go:220, StoryRunReconciler storyrun_controller.go:216), so the

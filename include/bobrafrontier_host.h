@@ -118,6 +118,14 @@ int bfh_batch_migrate(bfh_batch* b, const bfh_story* old_story, const bfh_story*
  * record in full.  A run or step out of range is BF_EINVAL and changes nothing.  Returns BF_OK.                            */
 int bfh_batch_redrive(bfh_batch* b, const uint32_t* runs, const int32_t* steps, uint32_t n);
 
+/* Grow the batch (see bf_resident_reshape): the layout becomes bf_layout_init(steps_max, child_nibbles, fields) and the capacity
+ * `capacity`, by the same growth rules.  The mirror re-lays its own state and result records as bf_resident_reshape re-lays the
+ * device's, and keeps its pending deltas (their run, step and child indices do not change).  In resident mode it calls
+ * bf_resident_reshape first; when that fails, the mirror changes nothing either.  A shrinking or invalid shape is BF_EINVAL, a
+ * failed allocation BF_ENOMEM, and both change nothing.  Afterwards bfh_batch_add_run takes the larger Stories and the
+ * additional runs.                                                                                                         */
+int bfh_batch_reshape(bfh_batch* b, uint32_t steps_max, uint32_t child_nibbles, uint32_t fields, uint32_t capacity);
+
 /* One frontier pass over the batch through bf_eval (or, in resident mode, bf_resident_*) (eval_flags: BF_EVAL_*). */
 int bfh_batch_eval(bfh_batch* b, uint32_t eval_flags, bf_counts* counts);
 
