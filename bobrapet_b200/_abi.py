@@ -131,6 +131,11 @@ class Redrive(C.Structure):
     _fields_ = [("run", C.c_uint32), ("slot", C.c_uint32), ("step", C.c_uint32), ("reserved", C.c_uint32)]
 
 
+class Retire(C.Structure):
+    _fields_ = [("struct_size", C.c_uint32), ("n_runs", C.c_uint32), ("runs", C.c_void_p), ("n", C.c_uint32),
+                ("capacity", C.c_uint32), ("moves_from", C.c_void_p), ("moves_to", C.c_void_p), ("n_moves", C.c_uint32)]
+
+
 class SchedTables(C.Structure):
     _fields_ = [("struct_size", C.c_uint32), ("n_stories", C.c_uint32), ("n_queues", C.c_uint32), ("global_limit", C.c_int32),
                 ("global_running_base", C.c_uint32), ("story_limit", C.c_void_p), ("story_running_base", C.c_void_p),
@@ -179,6 +184,7 @@ SYMBOLS = [
     ("bf_resident_migrate", C.c_int, [C.c_void_p, C.c_uint32, C.POINTER(Migration)]),
     ("bf_resident_redrive", C.c_int, [C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_void_p, C.POINTER(C.c_uint32)]),
     ("bf_resident_reshape", C.c_int, [C.c_void_p, C.c_uint32, C.POINTER(Layout), C.c_uint32]),
+    ("bf_resident_retire", C.c_int, [C.c_void_p, C.c_uint32, C.POINTER(Retire)]),
     ("bf_group_create", C.c_int, [C.POINTER(C.c_void_p), C.POINTER(C.c_int32), C.c_uint32, C.POINTER(Config)]),
     ("bf_group_destroy", None, [C.c_void_p]),
     ("bf_group_size", C.c_uint32, [C.c_void_p]),

@@ -38,6 +38,7 @@ cudaError_t launch_move_records(const uint8_t* src, uint8_t* dst, const void* mo
 cudaError_t launch_migrate(const MigrateParams& P, cudaStream_t stream);
 cudaError_t launch_redrive(const RedriveParams& P, cudaStream_t stream);
 cudaError_t launch_reshape(const ReshapeParams& P, cudaStream_t stream);
+cudaError_t launch_retire(const RetireParams& P, cudaStream_t stream);
 cudaError_t launch_schedule(const SchedParams& P, uint32_t sm_count, cudaStream_t stream, uint32_t phases = 3);
 cudaError_t launch_closure(const Slot* slots, const uint32_t* slot_ids, const uint32_t* starts, uint32_t n, uint32_t n_slots,
                            uint32_t words_out, uint32_t* masks, cudaStream_t stream);
@@ -157,6 +158,8 @@ struct bf_ctx {
   uint8_t* d_mig = nullptr; size_t d_mig_cap = 0;
   // redrives (bf_resident_redrive): statuses | requests | key per request | key slots | key steps | closure masks
   uint8_t* d_redrive = nullptr; size_t d_redrive_cap = 0;
+  // retirements (bf_resident_retire): the new index of each vacated run
+  uint32_t* d_retire = nullptr; size_t d_retire_cap = 0;
 
   // limiters (bf_schedule): what the last bf_eval left on the device + scratch
   bool last_eval_valid = false;
@@ -1003,7 +1006,7 @@ void bf_destroy(bf_ctx* c) {
   cudaFreeHost(c->h_counts);
   cudaFree(c->arena); cudaFree(c->slots_dev); cudaFree(c->ff_dev); cudaFree(c->d_state); cudaFree(c->d_result); cudaFree(c->d_counts); cudaFree(c->d_acc);
   cudaFree(c->d_defer); cudaFree(c->d_exp); cudaFree(c->d_exp_counts); cudaFree(c->d_offsets); cudaFree(c->d_block_sums); cudaFree(c->d_sched); cudaFree(c->d_deltas); cudaFree(c->d_rejected);
-  cudaFree(c->d_head); cudaFree(c->d_events); cudaFree(c->d_cblock); cudaFree(c->d_mig); cudaFree(c->d_redrive);
+  cudaFree(c->d_head); cudaFree(c->d_events); cudaFree(c->d_cblock); cudaFree(c->d_mig); cudaFree(c->d_redrive); cudaFree(c->d_retire);
   for (Resident& r : c->resident) { cudaFree(r.d_state); cudaFree(r.d_result); cudaFree(r.d_result_prev); }
   delete c;
 }
@@ -1453,6 +1456,21 @@ int bf_resident_destroy(bf_ctx* c, uint32_t h) {
   return BF_OK;
 }
 
+// Record the runs [first, end) as uploaded since the last full tick: the part at or above full_runs, merged with the ranges it
+// touches.
+static void note_uploaded(Resident* r, uint32_t first, uint32_t end) {
+  uint32_t lo = std::max(first, r->full_runs), hi = end;
+  if (lo >= hi) return;
+  auto it = r->uploaded.upper_bound(lo);
+  if (it != r->uploaded.begin() && std::prev(it)->second >= lo) {
+    --it;
+    lo = it->first; hi = std::max(hi, it->second);
+    it = r->uploaded.erase(it);
+  }
+  while (it != r->uploaded.end() && it->first <= hi) { hi = std::max(hi, it->second); it = r->uploaded.erase(it); }
+  r->uploaded.emplace(lo, hi);
+}
+
 int bf_resident_upload(bf_ctx* c, uint32_t h, uint32_t first, uint32_t n, const void* records) {
   if (!c) return BF_EINVAL;
   std::lock_guard<std::mutex> g(c->mu);
@@ -1467,19 +1485,7 @@ int bf_resident_upload(bf_ctx* c, uint32_t h, uint32_t first, uint32_t n, const 
   BF_CUDA(c, bf::launch_mark_runs(r->d_mark, first, n, r->epoch << 1 | 1u, c->stream));   // touched and must be listed
   c->stats.kernel_launches += 1;
   r->pending += n;
-  {   // record the part at or above full_runs, merged with the ranges it touches
-    uint32_t lo = std::max(first, r->full_runs), hi = first + n;
-    if (lo < hi) {
-      auto it = r->uploaded.upper_bound(lo);
-      if (it != r->uploaded.begin() && std::prev(it)->second >= lo) {
-        --it;
-        lo = it->first; hi = std::max(hi, it->second);
-        it = r->uploaded.erase(it);
-      }
-      while (it != r->uploaded.end() && it->first <= hi) { hi = std::max(hi, it->second); it = r->uploaded.erase(it); }
-      r->uploaded.emplace(lo, hi);
-    }
-  }
+  note_uploaded(r, first, first + n);
   BF_CUDA(c, cudaStreamSynchronize(c->stream));
   return BF_OK;
 }
@@ -2029,6 +2035,105 @@ int bf_resident_reshape(bf_ctx* c, uint32_t h, const bf_layout* layout, uint32_t
   r->d_result_prev = nullptr;   // never read before a pass overwrites it: allocated at the new size when next used
   r->L = T; r->cap = capacity;
   if (results_may_change) r->need_full = true;
+  return BF_OK;
+}
+
+// Runs leave a live batch (resident.cu): the last live runs move into the indices the retired ones free, so the batch's runs
+// stay [0, n_runs - n).  All checks and allocations come first, so a rejected call or a failed allocation changes nothing.
+// One H2D copy of the move table, one launch, one synchronisation; a new capacity adds the prefix copies into its buffers.
+int bf_resident_retire(bf_ctx* c, uint32_t h, bf_retire* rt) {
+  if (!c) return BF_EINVAL;
+  std::lock_guard<std::mutex> g(c->mu);
+  if (!rt || rt->struct_size != sizeof(bf_retire)) return fail(c, BF_EINVAL, "null bf_retire or bad struct_size");
+  Resident* r = resident_of(c, h);
+  if (!r) return fail(c, BF_EINVAL, "unknown resident batch");
+  const uint32_t N = rt->n_runs, n = rt->n;
+  if (N > r->cap) return fail(c, BF_EINVAL, "n_runs exceeds the resident batch");
+  if (n && !rt->runs) return fail(c, BF_EINVAL, "null runs");
+  std::vector<uint8_t> gone(N, 0);
+  for (uint32_t i = 0; i < n; ++i) {
+    const uint32_t q = rt->runs[i];
+    if (q >= N) return fail(c, BF_EINVAL, "runs[" + std::to_string(i) + "] is not below n_runs");
+    if (gone[q]) return fail(c, BF_EINVAL, "runs[" + std::to_string(i) + "] is retired twice");
+    gone[q] = 1;
+  }
+  const uint32_t m = N - n, cap = rt->capacity ? rt->capacity : r->cap;
+  if (cap < m || cap > r->cap) return fail(c, BF_EINVAL, "capacity must be 0 or within [n_runs - n, the current capacity]");
+  const bool resize = cap != r->cap;
+  if (n == 0 && !resize) { rt->n_moves = 0; return BF_OK; }
+  // the move rule: the k-th retired index below m (ascending) receives the k-th live index of [m, N); there are as many of each
+  std::vector<uint32_t> to(n, bf::kRetireNoMove);   // new index of run m + i
+  uint32_t n_moves = 0;
+  for (uint32_t i = 0, hole = 0; i < n; ++i) {
+    if (gone[m + i]) continue;
+    while (!gone[hole]) ++hole;
+    to[i] = hole++;
+    ++n_moves;
+  }
+  BF_CUDA(c, cudaSetDevice(c->device));
+  if (int rc = ensure_dev(c, c->d_retire, c->d_retire_cap, n ? n : 1)) return rc;
+  const bf_layout& L = r->L;
+  const size_t mark_bytes = ((size_t)cap + 3) / 4 * 16;   // as bf_resident_create
+  uint8_t *st = nullptr, *res = nullptr;
+  uint32_t* mk = nullptr;
+  if (resize) {
+    cudaError_t e = cudaMalloc(&st, (size_t)cap * L.state_stride);
+    if (e == cudaSuccess) e = cudaMalloc(&res, (size_t)cap * L.result_stride);
+    if (e == cudaSuccess) e = cudaMalloc(&mk, mark_bytes);
+    if (e != cudaSuccess) {
+      cudaFree(st); cudaFree(res); cudaFree(mk);
+      cudaGetLastError();   // an allocation failure is not a launch failure of the next call
+      return fail(c, BF_ENOMEM, std::string("resident retire: ") + cudaGetErrorString(e));
+    }
+  }
+  if (c->last_state == r->d_state) c->last_eval_valid = false;   // as after an upload: bf_schedule must follow a new pass
+  bf::RetireParams P{};
+  P.state = r->d_state; P.result = r->d_result; P.mark = r->d_mark; P.mark_value = r->epoch << 1 | 1u;   // touched, must list
+  P.to = c->d_retire; P.m = m; P.n = n; P.state_stride = L.state_stride; P.result_stride = L.result_stride;
+  cudaStream_t s = c->stream;
+  cudaError_t e = n ? cudaMemcpyAsync(c->d_retire, to.data(), (size_t)n * 4, cudaMemcpyHostToDevice, s) : cudaSuccess;
+  if (e == cudaSuccess) e = bf::launch_retire(P, s);
+  if (resize) {   // in place first, then the prefix into the new buffers (the mark padding past cap is never read)
+    if (e == cudaSuccess) e = cudaMemcpyAsync(st, r->d_state, (size_t)cap * L.state_stride, cudaMemcpyDeviceToDevice, s);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(res, r->d_result, (size_t)cap * L.result_stride, cudaMemcpyDeviceToDevice, s);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(mk, r->d_mark, mark_bytes, cudaMemcpyDeviceToDevice, s);
+  }
+  const cudaError_t es = cudaStreamSynchronize(s);
+  if (e == cudaSuccess) e = es;
+  if (e != cudaSuccess) {   // some records may have moved: the next touched tick evaluates and lists every run
+    cudaFree(st); cudaFree(res); cudaFree(mk);
+    r->need_full = true; r->prev_valid = false;
+    return cuda_fail(c, e, "bf_resident_retire");
+  }
+  c->stats.kernel_launches += n ? 1 : 0;
+  if (resize) {
+    cudaFree(r->d_state); cudaFree(r->d_result); cudaFree(r->d_result_prev); cudaFree(r->d_mark);
+    r->d_state = st; r->d_result = res; r->d_mark = mk;
+    r->d_result_prev = nullptr;   // never read before a pass overwrites it: allocated at the new size when next used
+    r->cap = cap;
+  }
+  // touched-tick bookkeeping: the batch's runs are [0, m) now, and the moved runs are as good as uploaded at their new index
+  r->full_runs = std::min(r->full_runs, m);
+  for (auto it = r->uploaded.begin(); it != r->uploaded.end();) {
+    if (it->first >= m) { it = r->uploaded.erase(it); continue; }
+    it->second = std::min(it->second, m);
+    ++it;
+  }
+  for (uint32_t i = 0; i < n; ++i)
+    if (to[i] != bf::kRetireNoMove) note_uploaded(r, to[i], to[i] + 1);
+  r->pending += n_moves;
+  // the current result records moved with their runs: a changed-only tick over [0, m) compares each run with its own record
+  if (r->prev_valid && r->prev_runs == N) r->prev_runs = m;
+  else r->prev_valid = false;
+  if (n_moves && (rt->moves_from || rt->moves_to)) {
+    for (uint32_t i = 0, k = 0; i < n; ++i) {
+      if (to[i] == bf::kRetireNoMove) continue;
+      if (rt->moves_from) rt->moves_from[k] = m + i;
+      if (rt->moves_to) rt->moves_to[k] = to[i];
+      ++k;
+    }
+  }
+  rt->n_runs = m; rt->n_moves = n_moves;
   return BF_OK;
 }
 

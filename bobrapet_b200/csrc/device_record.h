@@ -245,6 +245,18 @@ struct ReshapeParams {
   bf_layout from, to;
 };
 
+// bf_resident_retire (resident.cu): the runs [m, m + n) vacate their indices; the live ones among them move below m
+constexpr uint32_t kRetireNoMove = 0xFFFFFFFFu;
+struct RetireParams {
+  uint8_t* state;
+  uint8_t* result;               // the current result records
+  uint32_t* mark;                // touch marks: a target's becomes mark_value (touched and must be listed), a vacated one 0
+  uint32_t mark_value;
+  const uint32_t* to;            // [n] the new index of run m + i, or kRetireNoMove for a retired run
+  uint32_t m, n;
+  uint32_t state_stride, result_stride;   // multiples of 16
+};
+
 // limiters.cu (rows a9 / f4)
 struct SchedParams {
   const uint8_t* state;

@@ -835,6 +835,87 @@ int bfh_batch_reshape(bfh_batch* b, uint32_t steps_max, uint32_t child_nibbles, 
   return BF_OK;
 }
 
+int bfh_batch_retire(bfh_batch* b, const uint32_t* runs, uint32_t n, uint32_t capacity, uint32_t* moves_from, uint32_t* moves_to) {
+  if (!b) return BF_EINVAL;
+  const uint32_t N = b->n;
+  if (n && !runs) { b->err = "null runs"; return BF_EINVAL; }
+  std::vector<uint8_t> gone(N, 0);
+  for (uint32_t i = 0; i < n; ++i) {
+    if (runs[i] >= N || gone[runs[i]]) { b->err = "runs[" + std::to_string(i) + "] is out of range or retired twice"; return BF_EINVAL; }
+    gone[runs[i]] = 1;
+  }
+  const uint32_t m = N - n, cap = capacity ? capacity : b->cap;
+  if (cap < m || cap > b->cap) { b->err = "capacity must be 0 or within [size - n, the current capacity]"; return BF_EINVAL; }
+  if (n == 0 && cap == b->cap) return 0;
+  // the move rule of bf_resident_retire: the k-th retired index below m receives the k-th live index of [m, N)
+  std::vector<uint32_t> from, to, new_index(n, UINT32_MAX);   // new_index[i]: where run m + i goes
+  for (uint32_t i = 0, hole = 0; i < n; ++i) {
+    if (gone[m + i]) continue;
+    while (!gone[hole]) ++hole;
+    from.push_back(m + i); to.push_back(hole); new_index[i] = hole++;
+  }
+  const bf_layout& L = b->L;
+  uint8_t *st = nullptr, *res = nullptr;
+  bool pinned = false;
+  if (cap != b->cap && !alloc_records(b->ctx, (size_t)cap * L.state_stride, (size_t)cap * L.result_stride, &st, &res, &pinned)) {
+    b->err = "out of host memory";
+    return BF_ENOMEM;
+  }
+  if (b->resident) {   // every run on the device first, then the device: it fails without changes, and so does the mirror
+    int rc = BF_OK;
+    if (b->uploaded < N) {
+      rc = bf_resident_upload(b->ctx, b->handle, b->uploaded, N - b->uploaded, b->state + (size_t)b->uploaded * L.state_stride);
+      if (rc == BF_OK) { b->full_bytes_sent += (uint64_t)(N - b->uploaded) * L.state_stride; b->uploaded = N; }
+    }
+    if (rc == BF_OK) {
+      bf_retire rt{};
+      rt.struct_size = sizeof rt; rt.n_runs = N; rt.runs = runs; rt.n = n; rt.capacity = capacity;
+      rc = bf_resident_retire(b->ctx, b->handle, &rt);
+    }
+    if (rc != BF_OK) {
+      b->err = bf_last_error(b->ctx);
+      if (st) { if (pinned) { bf_free_pinned(b->ctx, st); bf_free_pinned(b->ctx, res); } else { free(st); free(res); } }
+      return rc;
+    }
+  }
+  const size_t ss = L.state_stride, rs = L.result_stride;
+  for (size_t k = 0; k < from.size(); ++k) {
+    memcpy(b->state + to[k] * ss, b->state + from[k] * ss, ss);
+    memcpy(b->result + to[k] * rs, b->result + from[k] * rs, rs);
+    b->story_of_run[to[k]] = b->story_of_run[from[k]];
+  }
+  memset(b->state + (size_t)m * ss, 0, (size_t)n * ss);
+  memset(b->result + (size_t)m * rs, 0, (size_t)n * rs);
+  b->story_of_run.resize(m);
+  if (st) {
+    memcpy(st, b->state, (size_t)m * ss);
+    memcpy(res, b->result, (size_t)m * rs);
+    free_records(b);
+    b->state = st; b->result = res; b->pinned = pinned; b->cap = cap;
+  }
+  // pending deltas: those of retired runs go, those of moved runs apply at the new index (no two keys meet: a target was retired)
+  if (!b->deltas.empty()) {
+    size_t keep = 0;
+    for (size_t k = 0; k < b->deltas.size(); ++k) {
+      bf_delta d = b->deltas[k];
+      if (gone[d.run]) continue;
+      if (d.run >= m) d.run = new_index[d.run - m];
+      b->deltas[keep++] = d;
+    }
+    b->deltas.resize(keep);
+    b->delta_at.clear();
+    for (size_t i = 0; i < keep; ++i) {
+      const bf_delta& d = b->deltas[i];
+      b->delta_at[((uint64_t)d.run << 32) | ((uint64_t)d.field << 16) | d.index] = (uint32_t)i;
+    }
+  }
+  b->n = m;
+  if (b->uploaded > m) b->uploaded = m;
+  if (moves_from && !from.empty()) memcpy(moves_from, from.data(), from.size() * 4);
+  if (moves_to && !to.empty()) memcpy(moves_to, to.data(), to.size() * 4);
+  return (int)from.size();
+}
+
 int bfh_batch_set_resident(bfh_batch* b, int on) {
   if (!b) return BF_EINVAL;
   if (!b->ctx) { b->err = "batch was created without a device context"; return BF_ENODEV; }

@@ -335,4 +335,31 @@ cudaError_t launch_reshape(const ReshapeParams& P, cudaStream_t stream) {
   return cudaGetLastError();
 }
 
+// Retire (bf_resident_retire).  One warp per vacated index m + i: when the run there lives on, the warp copies its state record
+// and current result record to its target (16-byte accesses, lane t takes vectors t, t + 32, ...) and lane 0 marks the target;
+// then the warp zeroes the vacated state record and its mark.  Targets lie below m and vacated indices at or above it, and
+// each lane zeroes only the vectors it read itself, so no warp reads what another writes.
+__global__ void __launch_bounds__(256) retire_runs(const RetireParams P) {
+  const uint32_t i = blockIdx.x * 8u + (threadIdx.x >> 5), lane = threadIdx.x & 31u;
+  if (i >= P.n) return;
+  const uint32_t from = P.m + i, to = P.to[i], sv = P.state_stride >> 4;
+  uint4* s = reinterpret_cast<uint4*>(P.state + (size_t)from * P.state_stride);
+  if (to != kRetireNoMove) {
+    uint4* d = reinterpret_cast<uint4*>(P.state + (size_t)to * P.state_stride);
+    for (uint32_t k = lane; k < sv; k += 32u) d[k] = s[k];
+    const uint4* rs = reinterpret_cast<const uint4*>(P.result + (size_t)from * P.result_stride);
+    uint4* rd = reinterpret_cast<uint4*>(P.result + (size_t)to * P.result_stride);
+    for (uint32_t k = lane; k < (P.result_stride >> 4); k += 32u) rd[k] = rs[k];
+    if (lane == 0) P.mark[to] = P.mark_value;
+  }
+  for (uint32_t k = lane; k < sv; k += 32u) s[k] = make_uint4(0u, 0u, 0u, 0u);
+  if (lane == 0) P.mark[from] = 0u;
+}
+
+cudaError_t launch_retire(const RetireParams& P, cudaStream_t stream) {
+  if (P.n == 0) return cudaSuccess;
+  retire_runs<<<(P.n - 1u) / 8u + 1u, 256, 0, stream>>>(P);
+  return cudaGetLastError();
+}
+
 }  // namespace bf

@@ -245,6 +245,19 @@ class Frontier:
         state, the current result records and the touch marks"""
         self._check(self._lib.bf_resident_reshape(self._ctx, handle, C.byref(L), capacity), "bf_resident_reshape")
 
+    def resident_retire(self, handle: int, n_runs: int, runs, capacity: int = 0):
+        """bf_resident_retire: take `runs` (distinct indices below n_runs) out of the batch; the last live runs move into the
+        freed indices.  capacity 0 keeps the capacity, else it becomes `capacity` (n_runs - len(runs) <= capacity <= current).
+        -> (new n_runs, moves_from, moves_to): run moves_from[i] now lives at moves_to[i], ascending by target"""
+        rs = np.ascontiguousarray(runs, dtype=np.uint32)
+        n = rs.shape[0]
+        mf = np.zeros(max(n, 1), dtype=np.uint32)
+        mt = np.zeros(max(n, 1), dtype=np.uint32)
+        rt = A.Retire(struct_size=C.sizeof(A.Retire), n_runs=int(n_runs), runs=rs.ctypes.data if n else None, n=n,
+                      capacity=int(capacity), moves_from=mf.ctypes.data, moves_to=mt.ctypes.data)
+        self._check(self._lib.bf_resident_retire(self._ctx, handle, C.byref(rt)), "bf_resident_retire")
+        return int(rt.n_runs), mf[:rt.n_moves].copy(), mt[:rt.n_moves].copy()
+
     # -- resident batches: device-side state, delta uploads (row f2)
     DELTA_DTYPE = np.dtype([("run", "<u4"), ("index", "<u2"), ("field", "u1"), ("code", "u1")])
 

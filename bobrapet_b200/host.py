@@ -45,6 +45,7 @@ _SYMS = [
     ("bfh_batch_migrate", C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32, C.c_uint32]),
     ("bfh_batch_redrive", C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32]),
     ("bfh_batch_reshape", C.c_int, [C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32]),
+    ("bfh_batch_retire", C.c_int, [C.c_void_p, C.c_void_p, C.c_uint32, C.c_uint32, C.c_void_p, C.c_void_p]),
     ("bfh_batch_eval", C.c_int, [C.c_void_p, C.c_uint32, C.POINTER(A.Counts)]),
     ("bfh_batch_set_resident", C.c_int, [C.c_void_p, C.c_int]),
     ("bfh_batch_traffic", C.c_int, [C.c_void_p, C.POINTER(C.c_uint64), C.POINTER(C.c_uint64), C.POINTER(C.c_uint32)]),
@@ -255,6 +256,16 @@ class HostBatch:
         """bfh_batch_reshape: grow the layout to bf_layout_init(steps_max, child_nibbles, fields) and the capacity, keeping every
         run's records and the pending deltas (in resident mode on the device too)"""
         self._chk(self._l.bfh_batch_reshape(self._p, steps_max, child_nibbles, fields, capacity), "bfh_batch_reshape")
+
+    def retire(self, runs, capacity=0):
+        """bfh_batch_retire: take `runs` out of the batch; the last live runs move into the freed indices (in resident mode on the
+        device too), and pending deltas follow them.  -> (moves_from, moves_to), ascending by target"""
+        rs = np.ascontiguousarray(runs, dtype=np.uint32)
+        mf = np.zeros(max(rs.shape[0], 1), np.uint32)
+        mt = np.zeros(max(rs.shape[0], 1), np.uint32)
+        k = self._chk(self._l.bfh_batch_retire(self._p, rs.ctypes.data if rs.shape[0] else None, rs.shape[0], capacity,
+                                               mf.ctypes.data, mt.ctypes.data), "bfh_batch_retire")
+        return mf[:k].copy(), mt[:k].copy()
 
     def size(self) -> int:
         return self._l.bfh_batch_size(self._p)

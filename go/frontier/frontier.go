@@ -391,6 +391,24 @@ func (r *Resident) Reshape(stepsMax, childNibbles, fields, capacity uint32) erro
 	return r.c.err(rc)
 }
 
+// Retire takes runs (distinct indices below nRuns) out of the batch, typically terminal StoryRuns the batcher no longer
+// needs rows for, at the latest on the informer's delete (bf_resident_retire).  The last live runs move into the freed
+// indices: run from[i] now lives at to[i], ascending by target, and the batch's runs become [0, newN).  Re-key the rows by the
+// moves; the next TickTouched lists every moved run under its new index.  capacity 0 keeps the capacity, else it becomes
+// capacity (newN <= capacity <= current) and the memory above it is released.  A bad argument changes nothing.
+func (r *Resident) Retire(nRuns uint32, runs []uint32, capacity uint32) (newN uint32, from, to []uint32, err error) {
+	from = make([]uint32, len(runs)+1)
+	to = make([]uint32, len(runs)+1)
+	var rp *C.uint32_t
+	if len(runs) > 0 {
+		rp = (*C.uint32_t)(unsafe.Pointer(&runs[0]))
+	}
+	var nOut, nMoves C.uint32_t
+	rc := C.bfgo_resident_retire(r.c.p, r.handle, C.uint32_t(nRuns), rp, C.uint32_t(len(runs)), C.uint32_t(capacity),
+		(*C.uint32_t)(unsafe.Pointer(&from[0])), (*C.uint32_t)(unsafe.Pointer(&to[0])), &nOut, &nMoves)
+	return uint32(nOut), from[:nMoves], to[:nMoves], r.c.err(rc)
+}
+
 // Group is one operator process driving several GPUs (bf_group_*): contiguous blocks of runs per device, one NCCL
 // all-gather of the per-shard counts per pass, limiter totals all-reduced across the shards.
 type Group struct{ p *C.bf_group }

@@ -125,6 +125,19 @@ static inline int bfgo_resident_reshape(bf_ctx* c, uint32_t handle, uint32_t ste
   return rc2;
 }
 
+/* bf_resident_retire with the bf_retire built here on the C stack (a Go struct holding Go pointers may not be passed to C). */
+static inline int bfgo_resident_retire(bf_ctx* c, uint32_t handle, uint32_t n_runs, const uint32_t* runs, uint32_t n, uint32_t capacity,
+                                       uint32_t* moves_from, uint32_t* moves_to, uint32_t* n_runs_out, uint32_t* n_moves_out) {
+  bf_retire r;
+  memset(&r, 0, sizeof r);
+  r.struct_size = (uint32_t)sizeof r;
+  r.n_runs = n_runs; r.runs = runs; r.n = n; r.capacity = capacity; r.moves_from = moves_from; r.moves_to = moves_to;
+  const int rc = bf_resident_retire(c, handle, &r);
+  *n_runs_out = rc == BF_OK ? r.n_runs : n_runs;
+  *n_moves_out = rc == BF_OK ? r.n_moves : 0;
+  return rc;
+}
+
 static inline void bfgo_tables(bf_sched_tables* t, uint32_t n_stories, uint32_t n_queues, int32_t global_limit, uint32_t global_base,
                                const int32_t* story_limit, const uint32_t* story_base, const int32_t* queue_limit,
                                const int32_t* queue_aging_s, const uint32_t* queue_base, const int32_t* queue_max_priority_base) {

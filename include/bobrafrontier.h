@@ -630,6 +630,44 @@ int bf_resident_redrive(bf_ctx* ctx, uint32_t handle, const bf_redrive* requests
  * Shrinking a batch or dropping a field is not offered (it loses codes): create a new batch and upload.             */
 int bf_resident_reshape(bf_ctx* ctx, uint32_t handle, const bf_layout* layout, uint32_t capacity);
 
+/* ------------------------------------------------------------------ retirements (runs leave a live batch)
+ * The reference stops evaluating a StoryRun once it is terminal (handleTerminalStoryRun, storyrun_controller.go:282-288) and
+ * retention deletes it later.  bf_resident_retire takes such runs out of a live batch, so that passes, ticks and memory follow
+ * the live runs instead of every run the batch ever held.  The batch's runs are [0, n_runs); `runs` lists n of them.  The last
+ * live runs move into the indices the retired ones free, by a rule the host can compute itself: with m = n_runs - n, the
+ * retired indices below m ("holes", ascending) receive the live indices of [m, n_runs) ("sources", ascending), hole k source k.
+ * Runs below m that are not retired keep their index.  moves_from / moves_to (each may be NULL) receive the n_moves moves,
+ * ascending by target (and by source); a batcher re-keys its rows by them.  Afterwards, by the bytes:
+ *   - the state record and the current result record (those BF_EVAL_CHANGED_ONLY and touched ticks compare with) at each target
+ *     equal the source's; state records and touch marks in [m, old n_runs) are zero, as after bf_resident_create;
+ *   - records at or above the old n_runs are not runs for this call: they keep their bytes and marks below the capacity;
+ *   - with capacity != 0 the buffers are reallocated at that size (new ones are allocated and filled before the old ones are
+ *     freed); records from the capacity on are released.  The layout does not change.
+ * Touched ticks: every moved run is touched and must be listed by the next bf_resident_tick_touched, as an uploaded run is, so
+ * the batcher gets a row under its new index.  The call never makes the next touched tick full by itself: the run count of the
+ * last full evaluation drops to m at most, the runs uploaded since are kept below m only, and the moved runs count as uploaded.
+ * A later tick over more than m runs is full unless uploads cover the difference, as before.  A BF_EVAL_CHANGED_ONLY tick over
+ * [0, m) right after the call lists what it would list had every moved run always had its new index (when the last tick
+ * covered the old n_runs; otherwise it lists every run).  Like an upload, the call ends the evaluated snapshot (bf_schedule must
+ * follow a new pass).
+ * Checked before anything changes, else BF_EINVAL and nothing changed: struct_size and the handle; n_runs <= capacity of the
+ * batch; runs not NULL when n > 0; every index below n_runs, none twice; capacity 0 or within [m, current capacity].  A failed
+ * allocation is BF_ENOMEM and changes nothing.  n == 0 with capacity set only trims the capacity; n == 0 without is a no-op.
+ * One H2D copy of the move table, one launch and one synchronisation, plus the copies into the new buffers of a new capacity.
+ * What is terminal is the host's decision: the device does not retire runs by itself.                                    */
+typedef struct bf_retire {
+  uint32_t struct_size;        /* sizeof(bf_retire)                                                                   */
+  uint32_t n_runs;             /* in: the batch's runs are [0, n_runs); out: n_runs - n                               */
+  const uint32_t* runs;        /* [n] indices to retire: distinct, each < n_runs, any order                           */
+  uint32_t n;
+  uint32_t capacity;           /* 0 = keep; else the new capacity, new n_runs <= capacity <= current                  */
+  uint32_t* moves_from;        /* [n] out, may be NULL: run moves_from[i] now lives at moves_to[i]                    */
+  uint32_t* moves_to;          /* [n] out, may be NULL                                                                */
+  uint32_t n_moves;            /* out                                                                                 */
+} bf_retire;
+
+int bf_resident_retire(bf_ctx* ctx, uint32_t handle, bf_retire* r);
+
 /* ------------------------------------------------------------------ device groups (SURVEY.md row e)
  * The reference is ONE operator process (cmd/main.go:220, StoryRunReconciler storyrun_controller.go:216), so the
  * multi-GPU path must be reachable from one process through this ABI: a group owns one ctx per device and an NCCL

@@ -126,6 +126,15 @@ int bfh_batch_redrive(bfh_batch* b, const uint32_t* runs, const int32_t* steps, 
  * additional runs.                                                                                                         */
 int bfh_batch_reshape(bfh_batch* b, uint32_t steps_max, uint32_t child_nibbles, uint32_t fields, uint32_t capacity);
 
+/* Retire runs (see bf_resident_retire): `runs` lists n distinct runs below bfh_batch_size; the last live runs move into the
+ * indices they free, by the same rule, and the size becomes size - n.  capacity 0 keeps the capacity, else it becomes
+ * `capacity` (size - n <= capacity <= current).  The mirror moves its own records, drops the pending deltas of retired runs and
+ * re-keys those of moved runs, which then apply at the new index.  In resident mode it first uploads its runs not yet on the
+ * device, then calls bf_resident_retire; when that fails, the mirror's records and deltas do not change.  moves_from / moves_to
+ * ([n] each, may be NULL) receive the moves, ascending by target.  Returns the number of moves, or BF_EINVAL (bad arguments,
+ * nothing changed), BF_ENOMEM or the device's error.                                                                        */
+int bfh_batch_retire(bfh_batch* b, const uint32_t* runs, uint32_t n, uint32_t capacity, uint32_t* moves_from, uint32_t* moves_to);
+
 /* One frontier pass over the batch through bf_eval (or, in resident mode, bf_resident_*) (eval_flags: BF_EVAL_*). */
 int bfh_batch_eval(bfh_batch* b, uint32_t eval_flags, bf_counts* counts);
 
