@@ -70,7 +70,7 @@ struct Resident {  // a device-resident batch (row f2)
   bool need_full = true;             // no tick yet, a tick failed, or a reshape added decision planes or output fields: the
                                      // current records are not known to be complete
   uint32_t last_fixpoint = 0, last_max_iter = 0;   // BF_EVAL_FIXPOINT and max_iterations of the last tick
-  uint64_t drops_seen = 0;           // bf_ctx::topo_drops at the last full tick
+  uint64_t slot_changes_seen = 0;    // bf_ctx::slot_changes at the last full tick
   uint64_t pending = 0;              // bound on the touched runs: those the last touched tick left at or above its n_runs (its
                                      // list build counts them), plus the deltas and uploaded runs since
   std::map<uint32_t, uint32_t> uploaded;   // runs at or above full_runs uploaded since the last full tick: disjoint, merged
@@ -117,7 +117,8 @@ struct bf_ctx {
   bool rec_max_dirty = false;          // a drop may have lowered the maxima: recomputed at the next plan
   uint32_t n_alive = 0;
   uint32_t n_with_parallel = 0;  // live topologies that have parallel steps
-  uint64_t topo_drops = 0;       // bf_topology_drop calls so far (a touched tick after one evaluates every run)
+  uint64_t slot_changes = 0;     // slot drops and reuses so far: either changes what the runs holding the slot evaluate
+                                 // to, so a touched tick after one evaluates every run
 
   // host-API staging
   uint8_t* d_state = nullptr; size_t d_state_cap = 0;
@@ -910,7 +911,7 @@ int put_many_locked(bf_ctx* c, const bf_topology* topos, uint32_t count, uint32_
   off = 0;
   for (uint32_t i = 0; i < count; ++i) {
     uint32_t slot;
-    if (!c->free_slots.empty()) { slot = c->free_slots.back(); c->free_slots.pop_back(); }
+    if (!c->free_slots.empty()) { slot = c->free_slots.back(); c->free_slots.pop_back(); c->slot_changes++; }
     else {
       slot = (uint32_t)c->meta.size();
       c->meta.emplace_back();
@@ -1095,7 +1096,7 @@ int bf_topology_put_many_checked_on_device(bf_ctx* c, const bf_topology* topos, 
 static int drop_locked(bf_ctx* c, uint32_t slot) {
   if (slot >= c->meta.size() || !c->meta[slot].alive) return fail(c, BF_ETOPO, "drop of an unknown slot");
   c->meta[slot].alive = false;
-  c->topo_drops++;
+  c->slot_changes++;
   if (c->meta[slot].P) c->n_with_parallel--;
   c->slots_host[slot] = bf::Slot{0, 0, 0};
   memset(&c->ff_host[(size_t)slot * bf::FF_STRIDE], 0, bf::FF_STRIDE * sizeof(uint32_t));
@@ -1644,7 +1645,7 @@ static int resident_tick_locked(bf_ctx* c, Resident* r, const bf_delta* deltas, 
   // a full evaluation: it ends the current touch epoch (touched ticks, above Resident)
   r->need_full = false;
   r->full_epoch = r->epoch++; r->full_runs = n_runs;
-  r->last_fixpoint = flags & BF_EVAL_FIXPOINT; r->last_max_iter = max_iterations; r->drops_seen = c->topo_drops;
+  r->last_fixpoint = flags & BF_EVAL_FIXPOINT; r->last_max_iter = max_iterations; r->slot_changes_seen = c->slot_changes;
   r->pending = 0; r->uploaded.clear();
   if (r->epoch >= 0x7FFFFFFFu) {   // the epoch must fit mark >> 1: once per 2^31 full ticks the marks start over
     BF_CUDA(c, cudaMemsetAsync(r->d_mark, 0, ((size_t)r->cap + 3) / 4 * 16, s));
@@ -1712,7 +1713,7 @@ static int touched_tick_locked(bf_ctx* c, Resident* r, const bf_delta* deltas, u
   if (n_runs > r->cap) return fail(c, BF_EINVAL, "n_runs exceeds the resident batch");
   if (n_deltas && !deltas) return fail(c, BF_EINVAL, "null deltas");
   BF_CUDA(c, cudaSetDevice(c->device));
-  const bool full = r->need_full || c->topo_drops != r->drops_seen || (flags & BF_EVAL_FIXPOINT) != r->last_fixpoint ||
+  const bool full = r->need_full || c->slot_changes != r->slot_changes_seen || (flags & BF_EVAL_FIXPOINT) != r->last_fixpoint ||
                     max_iterations != r->last_max_iter || r->epoch >= 0x7FFFFFFEu ||
                     (n_runs > r->full_runs && !uploads_cover(r->uploaded, r->full_runs, n_runs));
   if (full) {   // a plain compact tick: every run evaluated and listed, heads in run order

@@ -512,10 +512,12 @@ int bf_resident_tick_compact(bf_ctx* ctx, uint32_t handle, const bf_delta* delta
  * its listed runs: the same head words and the same events in the same order (ascending run index).  counts covers the
  * evaluated runs only (evals = sum of S over them).
  * The tick evaluates every run in [0, n_runs), lists them all (runs[i] = i) and sets full = 1 when: no tick has run on the batch
- * yet (or the last one failed); bf_topology_drop was called on the ctx since the last tick (a dropped slot kills its runs, a
- * reused one re-points them); BF_EVAL_FIXPOINT or max_iterations differs from the last tick's; bf_resident_reshape added
+ * yet (or the last one failed); a slot of the ctx was dropped, or a put reused a dropped slot, since the last tick (a dropped
+ * slot kills its runs, a reused one re-points them); BF_EVAL_FIXPOINT or max_iterations differs from the last tick's; bf_resident_reshape added
  * decision planes or an output field since (either may change any run's result); or n_runs exceeds the run count of the last full evaluation and not
- * every run beyond it was uploaded since.  Any tick of the other kinds (bf_resident_tick,
+ * every run beyond it was uploaded since.  A run may hold only a slot a put has returned (alive or dropped since): a put that
+ * creates a new slot index is not a change, so runs that already held that index (by a delta or an upload) keep the dead
+ * result of their last evaluation until they are touched again.  Any tick of the other kinds (bf_resident_tick,
  * _eval, _tick_compact) may come between touched ticks, and bf_schedule may follow a touched tick.
  * flags: BF_EVAL_FIXPOINT and BF_EVAL_NO_COUNTS only (else BF_EINVAL).  Pinned buffers are used in place as by
  * bf_resident_tick_compact; the call returns when they are filled.                                                  */
