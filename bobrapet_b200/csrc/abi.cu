@@ -4,232 +4,18 @@
 // (device_record.h), validates what validateRuntimeDependencyGraph validates
 // (internal/controller/runs/dag.go:3076-3146), plans shared memory for the frontier
 // kernel and drives H2D -> kernels -> D2H for the host-buffer entry point.
-#include <cuda_runtime.h>
-#include <stdint.h>
 #include <stdio.h>
 #include <stdlib.h>
 #include <string.h>
 
-#include <algorithm>
-#include <map>
-#include <mutex>
 #include <new>
 #include <thread>
-#include <string>
-#include <unordered_map>
-#include <vector>
 
-#include "../../include/bobrafrontier.h"
-#include "device_record.h"
+#include "ctx.h"
 
-namespace bf {
-cudaError_t launch_frontier(const KParams& P, uint32_t grid, uint32_t smem_bytes, cudaStream_t stream);
-cudaError_t launch_expansion(const KParams& P, unsigned long long* block_sums, unsigned long long* offsets,
-                             bf_expansion* out, unsigned long long cap, cudaStream_t stream, uint32_t* launches);
-int frontier_max_blocks_per_sm(const KParams& P, uint32_t threads, uint32_t smem_bytes, uint32_t* occ2);
-cudaError_t launch_frontier_pack(const KParams& P, uint32_t grid, uint32_t smem_bytes, cudaStream_t stream);
-uint32_t frontier_pack_max_warps();
-cudaError_t launch_apply_deltas(const DeltaParams& P, cudaStream_t stream);
-cudaError_t launch_compact(const CompactParams& P, cudaStream_t stream);
-cudaError_t launch_touched_list(const TouchedParams& P, cudaStream_t stream);
-cudaError_t launch_touched_compact(const TouchedParams& P, cudaStream_t stream);
-cudaError_t launch_mark_runs(uint32_t* mark, uint32_t first, uint32_t n, uint32_t value, cudaStream_t stream);
-cudaError_t launch_move_records(const uint8_t* src, uint8_t* dst, const void* moves, uint32_t n, cudaStream_t stream);
-cudaError_t launch_migrate(const MigrateParams& P, cudaStream_t stream);
-cudaError_t launch_redrive(const RedriveParams& P, cudaStream_t stream);
-cudaError_t launch_reshape(const ReshapeParams& P, cudaStream_t stream);
-cudaError_t launch_retire(const RetireParams& P, cudaStream_t stream);
-cudaError_t launch_schedule(const SchedParams& P, uint32_t sm_count, cudaStream_t stream, uint32_t phases = 3);
-cudaError_t launch_closure(const Slot* slots, const uint32_t* slot_ids, const uint32_t* starts, uint32_t n, uint32_t n_slots,
-                           uint32_t words_out, uint32_t* masks, cudaStream_t stream);
-cudaError_t launch_validate(const Slot* slots, const uint32_t* slot_ids, uint32_t n, uint32_t n_slots, uint32_t* status,
-                            cudaStream_t stream);
-}  // namespace bf
+using bf::cuda_fail; using bf::fail; using bf::round_up; using bf::round_up_sz;
 
 namespace {
-
-inline uint32_t round_up(uint32_t v, uint32_t a) { return (v + a - 1) / a * a; }
-inline size_t round_up_sz(size_t v, size_t a) { return (v + a - 1) / a * a; }
-
-struct Resident {  // a device-resident batch (row f2)
-  bool alive = false;
-  bf_layout L{};
-  uint32_t cap = 0;
-  uint8_t* d_state = nullptr;
-  uint8_t* d_result = nullptr;       // records of the last pass
-  uint8_t* d_result_prev = nullptr;  // records of the pass before (changed-only compaction); allocated on first use
-  bool prev_valid = false;           // d_result holds a pass over the current device state lineage
-  uint32_t prev_runs = 0;            // ... over this many runs
-  // Touched ticks (bf_resident_tick_touched).  Every delta and upload raises its run's mark to epoch << 1 (| 1 = must list, by
-  // an upload); a full tick records the epoch it ended in full_epoch and opens the next one, so a mark at or below full_epoch
-  // is stale by comparison alone: a full tick clears nothing and adds no launch.  A touched tick evaluates the runs whose
-  // mark is newer than full_epoch and zeroes their marks itself (list-mode compaction, compact.cu).
-  uint32_t* d_mark = nullptr;        // [cap rounded up to 4]
-  uint32_t epoch = 1, full_epoch = 0;
-  uint32_t full_runs = 0;            // runs the last full tick evaluated
-  bool need_full = true;             // no tick yet, a tick failed, or a reshape added decision planes or output fields: the
-                                     // current records are not known to be complete
-  uint32_t last_fixpoint = 0, last_max_iter = 0;   // BF_EVAL_FIXPOINT and max_iterations of the last tick
-  uint64_t slot_changes_seen = 0;    // bf_ctx::slot_changes at the last full tick
-  uint64_t pending = 0;              // bound on the touched runs: those the last touched tick left at or above its n_runs (its
-                                     // list build counts them), plus the deltas and uploaded runs since
-  std::map<uint32_t, uint32_t> uploaded;   // runs at or above full_runs uploaded since the last full tick: disjoint, merged
-                                           // [first, end) ranges keyed by first
-};
-
-struct TopoMeta {
-  bool alive = false;
-  uint32_t S = 0, E = 0, P = 0, bytes = 0;
-  size_t offset = 0;  // in arena
-  std::vector<uint32_t> child_first;
-  std::vector<uint16_t> par_step, par_branches;   // step and branch count of each parallel desc (bf_resident_migrate)
-  uint32_t child_nibbles = 0;
-};
-
-}  // namespace
-
-struct bf_ctx {
-  int device = 0;
-  int sm_count = 0;                    // SMs the frontier kernels spread over (device SMs minus the reserved ones)
-  cudaStream_t stream = nullptr;
-  // bf_eval pipeline: H2D copies, kernels and D2H copies of consecutive run chunks overlap on three streams
-  static constexpr uint32_t kMaxChunks = 32;
-  cudaStream_t s_in = nullptr, s_out = nullptr;
-  cudaEvent_t ev_in[kMaxChunks] = {}, ev_k[kMaxChunks] = {};
-  bool pipe_ready = false;
-  std::mutex mu;
-  std::string err;
-
-  uint8_t* arena = nullptr;
-  size_t arena_cap = 0, arena_used = 0;
-  size_t arena_dead = 0;               // bytes of dropped records below arena_used (reclaimed by compact_arena)
-  uint64_t arena_compactions = 0;
-  std::vector<TopoMeta> meta;
-  std::vector<uint32_t> free_slots;
-  std::vector<bf::Slot> slots_host;
-  bf::Slot* slots_dev = nullptr;
-  size_t slots_dev_cap = 0;
-  bool slots_dirty = true;
-  std::vector<uint32_t> ff_host;       // fail-fast masks, bf::FF_STRIDE words per slot (device_record.h), mirrored with the slots
-  uint32_t* ff_dev = nullptr;          // capacity: slots_dev_cap rows
-  uint32_t max_rec_bytes = 0;          // largest live record
-  uint32_t max_rec_by_w[33] = {};      // ... among the topologies of W = ceil(S/32) words (a batch of layout.words = w stages only W <= w)
-  bool rec_max_dirty = false;          // a drop may have lowered the maxima: recomputed at the next plan
-  uint32_t n_alive = 0;
-  uint32_t n_with_parallel = 0;  // live topologies that have parallel steps
-  uint64_t slot_changes = 0;     // slot drops and reuses so far: either changes what the runs holding the slot evaluate
-                                 // to, so a touched tick after one evaluates every run
-
-  // host-API staging
-  uint8_t* d_state = nullptr; size_t d_state_cap = 0;
-  uint8_t* d_result = nullptr; size_t d_result_cap = 0;
-  unsigned long long* d_counts = nullptr;
-  // BF_EVAL_COUNTS_SET scratch of the packed-lanes kernel (device_record.h): a ring of kAccSlots blocks of 8 u64, one per launch
-  // in turn (launches of different streams may overlap; a block is left zeroed by the launch that used it)
-  static constexpr uint32_t kAccSlots = 256;
-  unsigned long long* d_acc = nullptr;
-  uint32_t acc_seq = 0;
-  bf_counts* h_counts = nullptr;  // pinned landing zone for the counts block (a pageable target would make the copy synchronous)
-  bf_expansion* d_exp = nullptr; size_t d_exp_cap = 0;
-  // compact results (bf_eval_compact / bf_resident_tick_compact)
-  uint32_t* d_head = nullptr; size_t d_head_cap = 0;
-  uint16_t* d_events = nullptr; size_t d_events_cap = 0;
-  // [0] = events, [1] = listed runs, then TWO buffers of per-512-run event totals used in turn: a tick's emit kernel leaves the
-  // other one zeroed, so a pass that adds its runs' counts itself (fused heads, device_record.h) finds a clean buffer
-  unsigned long long* d_cblock = nullptr; size_t d_cblock_cap = 0;
-  uint32_t cblock_flip = 0;
-  // set by a compact tick around its run_pass: where a packed-lanes pass may leave head words and block totals; run_pass reports
-  // through fused_done whether it did
-  uint32_t* fuse_head = nullptr; unsigned long long* fuse_sums = nullptr; bool fused_done = false;
-  uint64_t last_events = 0;                                          // events of the previous compact pass (sizes the first D2H)
-  // scratch shared by both entry points
-  uint32_t* d_exp_counts = nullptr; size_t d_exp_counts_cap = 0;
-  unsigned long long* d_offsets = nullptr; size_t d_offsets_cap = 0;
-  unsigned long long* d_block_sums = nullptr; size_t d_block_sums_cap = 0;
-  uint32_t* d_defer = nullptr; size_t d_defer_cap = 0;  // [0] = count, [1..] = run ids
-  // touched ticks: [0] = list length, [1..] = the list | head word per list position | listed runs and their heads (when the
-  // caller's buffers are not pinned) | per-block sums
-  uint32_t* d_tlist = nullptr; size_t d_tlist_cap = 0;
-  uint32_t* d_tpos_head = nullptr; size_t d_tpos_head_cap = 0;
-  uint32_t* d_truns = nullptr; size_t d_truns_cap = 0;
-  uint32_t* d_thead = nullptr; size_t d_thead_cap = 0;
-  unsigned long long* d_tsums = nullptr; size_t d_tsums_cap = 0;
-  uint64_t last_touched_events = 0;   // events of the previous touched tick (sizes the first D2H)
-  // migrations (bf_resident_migrate): [0, 16) the migrated-run counter | inverse step map | desc table
-  uint8_t* d_mig = nullptr; size_t d_mig_cap = 0;
-  // redrives (bf_resident_redrive): statuses | requests | key per request | key slots | key steps | closure masks
-  uint8_t* d_redrive = nullptr; size_t d_redrive_cap = 0;
-  // retirements (bf_resident_retire): the new index of each vacated run
-  uint32_t* d_retire = nullptr; size_t d_retire_cap = 0;
-
-  // limiters (bf_schedule): what the last bf_eval left on the device + scratch
-  bool last_eval_valid = false;
-  uint32_t last_eval_runs = 0;
-  bf_layout last_eval_layout{};
-  uint8_t* d_sched = nullptr; size_t d_sched_cap = 0;   // runs | records | tables, one allocation
-  const uint8_t* last_state = nullptr;                  // device records of the last evaluated batch (bf_eval or resident)
-  const uint8_t* last_result = nullptr;
-  // resident batches (row f2)
-  std::vector<Resident> resident;
-  bf_delta* d_deltas = nullptr; size_t d_deltas_cap = 0;
-  uint32_t* d_rejected = nullptr;
-  // small device scratch that its consumers leave zeroed (the compaction's tail block reads and clears the rejected-delta
-  // counter and the listed-runs total), so the steady-state tick carries no memset launches; a failed call marks it dirty
-  bool rejected_clean = false, cblock_clean = false;
-
-  // cached shared-memory plans of the general kernel (recomputed when the layout, the largest record or a launch-shape knob
-  // changes): [0] for passes over whole batches, [1] for passes over a run list (touched ticks), so that a batch that mixes
-  // full and touched ticks keeps both
-  struct Plan {
-    uint32_t key_stride = 0, key_words = 0, key_rec = 0, key_variant = 0xFFFFFFFFu;
-    int key_knobs[3] = {0, 0, 0};   // BF_STAGES, BF_WARPS, BF_BLOCKS_PER_SM as last planned (0: unset)
-    uint32_t stages = 0, wpb = 0, per_sm = 0, occ2 = 0;
-  } plan[2];
-
-  bf_stats stats{};
-};
-
-namespace {
-
-int fail(bf_ctx* c, int code, const std::string& msg) {
-  if (c) c->err = msg;
-  return code;
-}
-int cuda_fail(bf_ctx* c, cudaError_t e, const char* what) {
-  return fail(c, BF_ECUDA, std::string(what) + ": " + cudaGetErrorString(e));
-}
-#define BF_CUDA(c, call)                                   \
-  do {                                                     \
-    cudaError_t e__ = (call);                              \
-    if (e__ != cudaSuccess) return cuda_fail(c, e__, #call); \
-  } while (0)
-
-// copy / compute streams and events of the chunked pipelines (bf_eval, bf_resident_tick); created on first use
-int ensure_pipe(bf_ctx* c) {
-  if (c->pipe_ready) return BF_OK;
-  if (!c->s_in) BF_CUDA(c, cudaStreamCreateWithFlags(&c->s_in, cudaStreamNonBlocking));
-  if (!c->s_out) BF_CUDA(c, cudaStreamCreateWithFlags(&c->s_out, cudaStreamNonBlocking));
-  for (uint32_t k = 0; k < bf_ctx::kMaxChunks; ++k) {
-    if (!c->ev_in[k]) BF_CUDA(c, cudaEventCreateWithFlags(&c->ev_in[k], cudaEventDisableTiming));
-    if (!c->ev_k[k]) BF_CUDA(c, cudaEventCreateWithFlags(&c->ev_k[k], cudaEventDisableTiming));
-  }
-  c->pipe_ready = true;
-  return BF_OK;
-}
-
-template <typename T>
-int ensure_dev(bf_ctx* c, T*& p, size_t& cap, size_t need_elems) {
-  if (need_elems <= cap) return BF_OK;
-  size_t ncap = cap ? cap : 1;
-  while (ncap < need_elems) ncap *= 2;
-  T* np = nullptr;
-  cudaError_t e = cudaMalloc(&np, ncap * sizeof(T));
-  if (e != cudaSuccess) return fail(c, BF_ENOMEM, std::string("cudaMalloc: ") + cudaGetErrorString(e));
-  if (p) cudaFree(p);
-  p = np;
-  cap = ncap;
-  return BF_OK;
-}
 
 // ---- record building -----------------------------------------------------------------------
 // BF_TOPO_FORMAT=csr keeps every topology in CSR form, =ell16 keeps the fixed-width rows at u16 entries (A/B timing and
@@ -429,46 +215,172 @@ void build_record(const bf_topology& t, const RecPlan& p, uint8_t* rec) {
 }
 
 int grow_arena(bf_ctx* c, size_t need_total) {
-  if (need_total <= c->arena_cap) return BF_OK;
-  size_t ncap = c->arena_cap ? c->arena_cap : (size_t)64 << 20;
+  if (need_total <= c->arena.cap) return BF_OK;
+  size_t ncap = c->arena.cap ? c->arena.cap : (size_t)64 << 20;
   while (ncap < need_total) ncap *= 2;
-  uint8_t* na = nullptr;
-  cudaError_t e = cudaMalloc(&na, ncap);
+  DevBuf<uint8_t> na;
+  cudaError_t e = na.alloc(ncap);
   if (e != cudaSuccess) {  // retry exact
-    ncap = round_up_sz(need_total, (size_t)1 << 20);
-    e = cudaMalloc(&na, ncap);
+    e = na.alloc(round_up_sz(need_total, (size_t)1 << 20));
     if (e != cudaSuccess) return fail(c, BF_ENOMEM, std::string("arena cudaMalloc: ") + cudaGetErrorString(e));
   }
   if (c->arena && c->arena_used) {
     e = cudaMemcpy(na, c->arena, c->arena_used, cudaMemcpyDeviceToDevice);
-    if (e != cudaSuccess) { cudaFree(na); return cuda_fail(c, e, "arena copy"); }
+    if (e != cudaSuccess) return cuda_fail(c, e, "arena copy");
   }
-  if (c->arena) cudaFree(c->arena);
-  c->arena = na;
-  c->arena_cap = ncap;
+  c->arena = std::move(na);
   for (size_t s = 0; s < c->meta.size(); ++s)
-    if (c->meta[s].alive) {
-      c->slots_host[s].addr = (uint64_t)(uintptr_t)(c->arena + c->meta[s].offset);
-    }
+    if (c->meta[s].alive) c->slots_host[s].addr = (uint64_t)(uintptr_t)(c->arena + c->meta[s].offset);
   c->slots_dirty = true;
+  return BF_OK;
+}
+
+// The arena is a bump allocator; a long-lived operator puts one topology per Story generation and drops the old one, so
+// dead records pile up below arena_used.  When they outweigh the live ones the live records are re-packed into a fresh
+// arena (one warp per record on the device), the slot table follows, and the freed space is reusable again.
+int compact_arena(bf_ctx* c, size_t incoming) {
+  std::vector<uint32_t> live;
+  size_t live_bytes = 0;
+  for (uint32_t s = 0; s < c->meta.size(); ++s)
+    if (c->meta[s].alive) { live.push_back(s); live_bytes += round_up_sz(c->meta[s].bytes, 16); }
+  size_t ncap = (size_t)64 << 20;
+  while (ncap < live_bytes + incoming) ncap *= 2;
+  DevBuf<uint8_t> na;
+  cudaError_t e = na.alloc(ncap);
+  if (e != cudaSuccess) return BF_OK;   // no room for a second arena right now: keep appending
+  std::vector<unsigned long long> moves(4 * live.size());
+  size_t off = 0;
+  for (size_t i = 0; i < live.size(); ++i) {
+    const TopoMeta& m = c->meta[live[i]];
+    moves[4 * i] = m.offset; moves[4 * i + 1] = off; moves[4 * i + 2] = m.bytes; moves[4 * i + 3] = 0;
+    off += round_up_sz(m.bytes, 16);
+  }
+  void* d_moves = nullptr;
+  if (!live.empty()) {
+    e = cudaMalloc(&d_moves, moves.size() * sizeof(unsigned long long));
+    if (e == cudaSuccess) e = cudaMemcpyAsync(d_moves, moves.data(), moves.size() * sizeof(unsigned long long), cudaMemcpyHostToDevice, c->stream);
+    if (e == cudaSuccess) e = bf::launch_move_records(c->arena, na, d_moves, (uint32_t)live.size(), c->stream);
+  }
+  if (e == cudaSuccess) e = cudaDeviceSynchronize();   // nothing may still read the old arena when it is freed
+  cudaFree(d_moves);
+  if (e != cudaSuccess) return cuda_fail(c, e, "arena compaction");
+  c->arena = std::move(na); c->arena_used = off; c->arena_dead = 0;
+  for (size_t i = 0; i < live.size(); ++i) {
+    TopoMeta& m = c->meta[live[i]];
+    m.offset = (size_t)moves[4 * i + 1];
+    c->slots_host[live[i]].addr = (uint64_t)(uintptr_t)(c->arena + m.offset);
+  }
+  c->slots_dirty = true;
+  c->rec_max_dirty = true;
+  c->arena_compactions++;
+  c->stats.kernel_launches += live.empty() ? 0 : 1;
+  return BF_OK;
+}
+
+int put_many_locked(bf_ctx* c, const bf_topology* topos, uint32_t count, uint32_t* slots_out, bool host_kahn = true) {
+  std::vector<RecPlan> plans(count);
+  size_t total = 0;
+  std::string why;
+  const int forced = forced_format();
+  // validation (Kahn) and record building are per topology: spread a bulk upload over the host cores
+  const uint32_t n_thr = count >= 512 ? std::min<uint32_t>(16, std::max(1u, std::thread::hardware_concurrency())) : 1;
+  auto parallel_for = [&](auto&& fn) {
+    if (n_thr == 1) { fn(0u, count); return; }
+    std::vector<std::thread> th;
+    for (uint32_t t = 0; t < n_thr; ++t)
+      th.emplace_back([&, t] { fn((uint32_t)((uint64_t)count * t / n_thr), (uint32_t)((uint64_t)count * (t + 1) / n_thr)); });
+    for (auto& x : th) x.join();
+  };
+  std::vector<int> rcs(count, BF_OK);
+  std::mutex why_mu;
+  uint32_t first_bad = count;
+  parallel_for([&](uint32_t lo, uint32_t hi) {
+    std::string w;
+    for (uint32_t i = lo; i < hi; ++i) {
+      rcs[i] = plan_record(topos[i], plans[i], w, host_kahn, forced);
+      if (rcs[i] != BF_OK) {
+        std::lock_guard<std::mutex> g(why_mu);
+        if (i < first_bad) { first_bad = i; why = w; }
+        return;
+      }
+    }
+  });
+  if (first_bad < count) return fail(c, rcs[first_bad], "topology " + std::to_string(first_bad) + ": " + why);
+  for (uint32_t i = 0; i < count; ++i) total += plans[i].rec_bytes;
+  if (c->arena_dead > ((size_t)1 << 20) && c->arena_dead * 2 > c->arena_used)
+    if (int rc = compact_arena(c, total)) return rc;
+  const size_t base = round_up_sz(c->arena_used, 16);
+  if (int rc = grow_arena(c, base + total)) return rc;
+  std::vector<uint8_t> staging;
+  try { staging.resize(total); } catch (const std::bad_alloc&) { return fail(c, BF_ENOMEM, "host staging allocation failed"); }
+  std::vector<size_t> rec_off(count);
+  size_t off = 0;
+  for (uint32_t i = 0; i < count; ++i) { rec_off[i] = off; off += plans[i].rec_bytes; }
+  parallel_for([&](uint32_t lo, uint32_t hi) {
+    for (uint32_t i = lo; i < hi; ++i) build_record(topos[i], plans[i], staging.data() + rec_off[i]);
+  });
+  if (total) BF_CUDA(c, cudaMemcpy(c->arena + base, staging.data(), total, cudaMemcpyHostToDevice));
+  off = 0;
+  for (uint32_t i = 0; i < count; ++i) {
+    uint32_t slot;
+    if (!c->free_slots.empty()) { slot = c->free_slots.back(); c->free_slots.pop_back(); c->slot_changes++; }
+    else {
+      slot = (uint32_t)c->meta.size();
+      c->meta.emplace_back();
+      c->slots_host.push_back(bf::Slot{0, 0, 0});
+      c->ff_host.resize(c->ff_host.size() + bf::FF_STRIDE, 0u);
+    }
+    TopoMeta& m = c->meta[slot];
+    m.alive = true; m.S = topos[i].n_steps; m.E = topos[i].n_edges; m.P = topos[i].n_parallel;
+    m.bytes = plans[i].rec_bytes; m.offset = base + off; m.child_first = plans[i].child_first;
+    m.child_nibbles = plans[i].child_nibbles;
+    m.par_step.resize(m.P); m.par_branches.resize(m.P);
+    for (uint32_t q = 0; q < m.P; ++q) { m.par_step[q] = topos[i].parallel[q].step; m.par_branches[q] = topos[i].parallel[q].branches; }
+    c->slots_host[slot] = bf::Slot{(uint64_t)(uintptr_t)(c->arena + m.offset), m.bytes,
+                                   m.S | (m.P << 16) | (bf::slot_row_bytes(plans[i].ell) << 24)};
+    memcpy(&c->ff_host[(size_t)slot * bf::FF_STRIDE], plans[i].ff, sizeof plans[i].ff);
+    if (m.bytes > c->max_rec_bytes) c->max_rec_bytes = m.bytes;
+    if (m.bytes > c->max_rec_by_w[plans[i].W]) c->max_rec_by_w[plans[i].W] = m.bytes;
+    off += plans[i].rec_bytes;
+    slots_out[i] = slot;
+    c->n_alive++;
+    if (m.P) c->n_with_parallel++;
+  }
+  c->arena_used = base + total;
+  c->slots_dirty = true;
+  return BF_OK;
+}
+
+}  // namespace
+
+// ---- host helpers of a pass, shared with resident_abi.cu (ctx.h) ----------------------------
+namespace bf {
+
+// copy / compute streams and events of the chunked pipelines (bf_eval, bf_resident_tick); created on first use
+int ensure_pipe(bf_ctx* c) {
+  if (c->pipe_ready) return BF_OK;
+  if (!c->s_in) BF_CUDA(c, cudaStreamCreateWithFlags(&c->s_in, cudaStreamNonBlocking));
+  if (!c->s_out) BF_CUDA(c, cudaStreamCreateWithFlags(&c->s_out, cudaStreamNonBlocking));
+  for (uint32_t k = 0; k < bf_ctx::kMaxChunks; ++k) {
+    if (!c->ev_in[k]) BF_CUDA(c, cudaEventCreateWithFlags(&c->ev_in[k], cudaEventDisableTiming));
+    if (!c->ev_k[k]) BF_CUDA(c, cudaEventCreateWithFlags(&c->ev_k[k], cudaEventDisableTiming));
+  }
+  c->pipe_ready = true;
   return BF_OK;
 }
 
 int sync_slots(bf_ctx* c, cudaStream_t stream) {
   if (!c->slots_dirty) return BF_OK;
   const size_t n = c->slots_host.size();
-  if (n > c->slots_dev_cap) {
-    size_t ncap = c->slots_dev_cap ? c->slots_dev_cap : 1024;
+  if (n > c->slots_dev.cap) {
+    size_t ncap = c->slots_dev.cap ? c->slots_dev.cap : 1024;
     while (ncap < n) ncap *= 2;
-    bf::Slot* np = nullptr;
-    uint32_t* nf = nullptr;
-    BF_CUDA(c, cudaMalloc(&np, ncap * sizeof(bf::Slot)));
-    if (cudaError_t e = cudaMalloc(&nf, ncap * bf::FF_STRIDE * sizeof(uint32_t))) { cudaFree(np); return cuda_fail(c, e, "cudaMalloc fail-fast masks"); }
-    if (c->slots_dev) cudaFree(c->slots_dev);
-    if (c->ff_dev) cudaFree(c->ff_dev);
-    c->slots_dev = np;
-    c->ff_dev = nf;
-    c->slots_dev_cap = ncap;
+    DevBuf<bf::Slot> np;
+    DevBuf<uint32_t> nf;
+    if (cudaError_t e = np.alloc(ncap)) return cuda_fail(c, e, "cudaMalloc slot table");
+    if (cudaError_t e = nf.alloc(ncap * bf::FF_STRIDE)) return cuda_fail(c, e, "cudaMalloc fail-fast masks");
+    c->slots_dev = std::move(np);
+    c->ff_dev = std::move(nf);
   }
   if (n) BF_CUDA(c, cudaMemcpyAsync(c->slots_dev, c->slots_host.data(), n * sizeof(bf::Slot), cudaMemcpyHostToDevice, stream));
   if (n) BF_CUDA(c, cudaMemcpyAsync(c->ff_dev, c->ff_host.data(), n * bf::FF_STRIDE * sizeof(uint32_t), cudaMemcpyHostToDevice, stream));
@@ -503,8 +415,7 @@ int check_layout(bf_ctx* c, const bf_layout& L) {
 // run_list (touched ticks): the pass takes the runs run_list[0 .. *run_list_count) (b.n_runs bounds the count) and writes
 // each run's record at its own index
 int run_pass(bf_ctx* c, const bf_batch& b, const uint8_t* d_state, uint8_t* d_result, bf_expansion* d_exp,
-             unsigned long long* d_counts, cudaStream_t stream, const uint32_t* run_list = nullptr,
-             const uint32_t* run_list_count = nullptr) {
+             unsigned long long* d_counts, cudaStream_t stream, const uint32_t* run_list, const uint32_t* run_list_count) {
   const bf_layout& L = b.layout;
   if (int rc = sync_slots(c, stream)) return rc;
   if (c->rec_max_dirty) {  // drops since the last plan: the largest live record per word count
@@ -536,21 +447,15 @@ int run_pass(bf_ctx* c, const bf_batch& b, const uint8_t* d_state, uint8_t* d_re
   P.off_decision = L.off_decision; P.off_child = L.off_child;
   P.result_stride = L.result_stride; P.off_ready = L.off_ready; P.off_skip = L.off_skip; P.off_fail = L.off_fail;
   P.off_needs_cond = L.off_needs_cond; P.off_skip_dep = L.off_skip_dep; P.off_phase_out = L.off_phase_out;
-  {
-    uint32_t tail = (uint32_t)sizeof(bf_result_header);
-    auto upd = [&](uint32_t off, uint32_t len) { if (off != BF_OFF_NONE && off + len > tail) tail = off + len; };
-    upd(L.off_ready, L.words * 4); upd(L.off_skip, L.words * 4); upd(L.off_fail, L.words * 4);
-    upd(L.off_needs_cond, L.words * 4); upd(L.off_skip_dep, L.words * 4); upd(L.off_phase_out, L.words * 16);
-    P.result_tail = tail;
-  }
+  P.result_tail = result_tail_of(L);
 
   P.run_blocked = 0;
   if (const char* e = getenv("BF_ASSIGN")) P.run_blocked = !strcmp(e, "blocked");
   const bool want_exp = (b.flags & BF_EVAL_EXPANSION) && d_exp != nullptr;
   if (want_exp) {
-    if (int rc = ensure_dev(c, c->d_exp_counts, c->d_exp_counts_cap, b.n_runs)) return rc;
-    if (int rc = ensure_dev(c, c->d_offsets, c->d_offsets_cap, b.n_runs)) return rc;
-    if (int rc = ensure_dev(c, c->d_block_sums, c->d_block_sums_cap, (size_t)(b.n_runs + 1023) / 1024 + 1)) return rc;
+    if (int rc = c->d_exp_counts.ensure(c, b.n_runs)) return rc;
+    if (int rc = c->d_offsets.ensure(c, b.n_runs)) return rc;
+    if (int rc = c->d_block_sums.ensure(c, (size_t)(b.n_runs + 1023) / 1024 + 1)) return rc;
     P.exp_counts = c->d_exp_counts;
   }
 
@@ -681,7 +586,7 @@ int run_pass(bf_ctx* c, const bf_batch& b, const uint8_t* d_state, uint8_t* d_re
     P.wq = wq; P.wq_log2 = lg; P.warps_per_block = nw; P.slot_groups = ng; P.stages = 1;
     P.run_list = run_list; P.run_list_count = run_list_count;
     if (two_tier) {
-      if (int rc = ensure_dev(c, c->d_defer, c->d_defer_cap, (size_t)b.n_runs + 1)) return rc;
+      if (int rc = c->d_defer.ensure(c, (size_t)b.n_runs + 1)) return rc;
       P.defer_count = c->d_defer;
       P.defer_list = c->d_defer + 1;
     }
@@ -731,49 +636,6 @@ int run_pass(bf_ctx* c, const bf_batch& b, const uint8_t* d_state, uint8_t* d_re
   return BF_OK;
 }
 
-// The arena is a bump allocator; a long-lived operator puts one topology per Story generation and drops the old one, so
-// dead records pile up below arena_used.  When they outweigh the live ones the live records are re-packed into a fresh
-// arena (one warp per record on the device), the slot table follows, and the freed space is reusable again.
-int compact_arena(bf_ctx* c, size_t incoming) {
-  std::vector<uint32_t> live;
-  size_t live_bytes = 0;
-  for (uint32_t s = 0; s < c->meta.size(); ++s)
-    if (c->meta[s].alive) { live.push_back(s); live_bytes += round_up_sz(c->meta[s].bytes, 16); }
-  size_t ncap = (size_t)64 << 20;
-  while (ncap < live_bytes + incoming) ncap *= 2;
-  uint8_t* na = nullptr;
-  cudaError_t e = cudaMalloc(&na, ncap);
-  if (e != cudaSuccess) { cudaGetLastError(); return BF_OK; }   // no room for a second arena right now: keep appending
-  std::vector<unsigned long long> moves(4 * live.size());
-  size_t off = 0;
-  for (size_t i = 0; i < live.size(); ++i) {
-    const TopoMeta& m = c->meta[live[i]];
-    moves[4 * i] = m.offset; moves[4 * i + 1] = off; moves[4 * i + 2] = m.bytes; moves[4 * i + 3] = 0;
-    off += round_up_sz(m.bytes, 16);
-  }
-  void* d_moves = nullptr;
-  if (!live.empty()) {
-    e = cudaMalloc(&d_moves, moves.size() * sizeof(unsigned long long));
-    if (e == cudaSuccess) e = cudaMemcpyAsync(d_moves, moves.data(), moves.size() * sizeof(unsigned long long), cudaMemcpyHostToDevice, c->stream);
-    if (e == cudaSuccess) e = bf::launch_move_records(c->arena, na, d_moves, (uint32_t)live.size(), c->stream);
-  }
-  if (e == cudaSuccess) e = cudaDeviceSynchronize();   // nothing may still read the old arena when it is freed
-  cudaFree(d_moves);
-  if (e != cudaSuccess) { cudaFree(na); return cuda_fail(c, e, "arena compaction"); }
-  cudaFree(c->arena);
-  c->arena = na; c->arena_cap = ncap; c->arena_used = off; c->arena_dead = 0;
-  for (size_t i = 0; i < live.size(); ++i) {
-    TopoMeta& m = c->meta[live[i]];
-    m.offset = (size_t)moves[4 * i + 1];
-    c->slots_host[live[i]].addr = (uint64_t)(uintptr_t)(c->arena + m.offset);
-  }
-  c->slots_dirty = true;
-  c->rec_max_dirty = true;
-  c->arena_compactions++;
-  c->stats.kernel_launches += live.empty() ? 0 : 1;
-  return BF_OK;
-}
-
 // the device address of a buffer in pinned host memory (bf_alloc_pinned, cudaHostAlloc / cudaHostRegister), else nullptr
 void* pinned_dev(const void* p) {
   cudaPointerAttributes at{};
@@ -797,27 +659,27 @@ uint32_t result_tail_of(const bf_layout& L) {
 // head words + the scratch block of a compaction (zeroed once; the kernels leave it clean): before the pass, so that a fused
 // pass can write into them
 int compact_prepare(bf_ctx* c, uint32_t n_runs, cudaStream_t s) {
-  if (int rc = ensure_dev(c, c->d_head, c->d_head_cap, n_runs ? n_runs : 1)) return rc;
-  const size_t cap_before = c->d_cblock_cap;
-  if (int rc = ensure_dev(c, c->d_cblock, c->d_cblock_cap, 2 * ((size_t)(n_runs + 511) / 512 + 1) + 2)) return rc;
-  if (c->d_cblock_cap != cap_before) c->cblock_clean = false;
+  if (int rc = c->d_head.ensure(c, n_runs ? n_runs : 1)) return rc;
+  const size_t cap_before = c->d_cblock.cap;
+  if (int rc = c->d_cblock.ensure(c, 2 * ((size_t)(n_runs + 511) / 512 + 1) + 2)) return rc;
+  if (c->d_cblock.cap != cap_before) c->cblock_clean = false;
   if (!c->cblock_clean) {
-    BF_CUDA(c, cudaMemsetAsync(c->d_cblock, 0, c->d_cblock_cap * sizeof(unsigned long long), s));
+    BF_CUDA(c, cudaMemsetAsync(c->d_cblock, 0, c->d_cblock.cap * sizeof(unsigned long long), s));
     c->cblock_clean = true;
   }
   return BF_OK;
 }
-static unsigned long long* cblock_sums(bf_ctx* c, uint32_t which) { return c->d_cblock + 2 + (size_t)which * ((c->d_cblock_cap - 2) / 2); }
+unsigned long long* cblock_sums(bf_ctx* c, uint32_t which) { return c->d_cblock + 2 + (size_t)which * ((c->d_cblock.cap - 2) / 2); }
 
 int compact_enqueue(bf_ctx* c, const bf_layout& L, const uint8_t* d_result, const uint8_t* d_prev, uint32_t n_runs, bf_compact_out* out,
-                    cudaStream_t s, uint64_t* first_slice, bool with_rejected, bool heads_done = false) {
+                    cudaStream_t s, uint64_t* first_slice, bool with_rejected, bool heads_done) {
   const uint64_t cap = out->events ? out->events_cap : 0;
   if (int rc = compact_prepare(c, n_runs, s)) return rc;
-  if (int rc = ensure_dev(c, c->d_events, c->d_events_cap, cap ? (size_t)cap : 1)) return rc;
+  if (int rc = c->d_events.ensure(c, cap ? (size_t)cap : 1)) return rc;
   bf::CompactParams P{};
   P.result = d_result; P.prev_result = d_prev; P.head = c->d_head; P.events = c->d_events; P.cap = cap;
   P.block_sums = cblock_sums(c, c->cblock_flip); P.zero_sums = cblock_sums(c, c->cblock_flip ^ 1u); P.total = c->d_cblock;
-  P.zero_len = (uint32_t)((c->d_cblock_cap - 2) / 2);
+  P.zero_len = (uint32_t)((c->d_cblock.cap - 2) / 2);
   P.heads_done = heads_done ? 1u : 0u;
   c->cblock_flip ^= 1u;   // the next compaction (and a pass fused with it) uses the buffer this one leaves zeroed
   P.n_runs = n_runs; P.words = L.words; P.result_stride = L.result_stride; P.result_tail = result_tail_of(L);
@@ -826,7 +688,7 @@ int compact_enqueue(bf_ctx* c, const bf_layout& L, const uint8_t* d_result, cons
   // the small results (event total, counts, rejected deltas, listed runs) are written to the pinned block by the last kernel
   // itself: no latency-bound small D2H copies
   unsigned long long* tail = reinterpret_cast<unsigned long long*>(c->h_counts + 2);   // 7 x u64 in the pinned block
-  P.host_tail = tail; P.counts = c->d_counts; P.rejected = with_rejected ? c->d_rejected : nullptr;
+  P.host_tail = tail; P.counts = c->d_counts; P.rejected = with_rejected ? c->d_rejected.p : nullptr;
   // a head buffer in pinned host memory (bf_alloc_pinned, cudaHostAlloc / cudaHostRegister) gets the head words posted by the
   // kernel itself; any other buffer gets them by a download
   P.host_head = nullptr;
@@ -865,81 +727,7 @@ int compact_finish(bf_ctx* c, bf_compact_out* out, uint64_t first_slice) {
   return BF_OK;
 }
 
-int put_many_locked(bf_ctx* c, const bf_topology* topos, uint32_t count, uint32_t* slots_out, bool host_kahn = true) {
-  std::vector<RecPlan> plans(count);
-  size_t total = 0;
-  std::string why;
-  const int forced = forced_format();
-  // validation (Kahn) and record building are per topology: spread a bulk upload over the host cores
-  const uint32_t n_thr = count >= 512 ? std::min<uint32_t>(16, std::max(1u, std::thread::hardware_concurrency())) : 1;
-  auto parallel_for = [&](auto&& fn) {
-    if (n_thr == 1) { fn(0u, count); return; }
-    std::vector<std::thread> th;
-    for (uint32_t t = 0; t < n_thr; ++t)
-      th.emplace_back([&, t] { fn((uint32_t)((uint64_t)count * t / n_thr), (uint32_t)((uint64_t)count * (t + 1) / n_thr)); });
-    for (auto& x : th) x.join();
-  };
-  std::vector<int> rcs(count, BF_OK);
-  std::mutex why_mu;
-  uint32_t first_bad = count;
-  parallel_for([&](uint32_t lo, uint32_t hi) {
-    std::string w;
-    for (uint32_t i = lo; i < hi; ++i) {
-      rcs[i] = plan_record(topos[i], plans[i], w, host_kahn, forced);
-      if (rcs[i] != BF_OK) {
-        std::lock_guard<std::mutex> g(why_mu);
-        if (i < first_bad) { first_bad = i; why = w; }
-        return;
-      }
-    }
-  });
-  if (first_bad < count) return fail(c, rcs[first_bad], "topology " + std::to_string(first_bad) + ": " + why);
-  for (uint32_t i = 0; i < count; ++i) total += plans[i].rec_bytes;
-  if (c->arena_dead > ((size_t)1 << 20) && c->arena_dead * 2 > c->arena_used)
-    if (int rc = compact_arena(c, total)) return rc;
-  const size_t base = round_up_sz(c->arena_used, 16);
-  if (int rc = grow_arena(c, base + total)) return rc;
-  std::vector<uint8_t> staging;
-  try { staging.resize(total); } catch (const std::bad_alloc&) { return fail(c, BF_ENOMEM, "host staging allocation failed"); }
-  std::vector<size_t> rec_off(count);
-  size_t off = 0;
-  for (uint32_t i = 0; i < count; ++i) { rec_off[i] = off; off += plans[i].rec_bytes; }
-  parallel_for([&](uint32_t lo, uint32_t hi) {
-    for (uint32_t i = lo; i < hi; ++i) build_record(topos[i], plans[i], staging.data() + rec_off[i]);
-  });
-  if (total) BF_CUDA(c, cudaMemcpy(c->arena + base, staging.data(), total, cudaMemcpyHostToDevice));
-  off = 0;
-  for (uint32_t i = 0; i < count; ++i) {
-    uint32_t slot;
-    if (!c->free_slots.empty()) { slot = c->free_slots.back(); c->free_slots.pop_back(); c->slot_changes++; }
-    else {
-      slot = (uint32_t)c->meta.size();
-      c->meta.emplace_back();
-      c->slots_host.push_back(bf::Slot{0, 0, 0});
-      c->ff_host.resize(c->ff_host.size() + bf::FF_STRIDE, 0u);
-    }
-    TopoMeta& m = c->meta[slot];
-    m.alive = true; m.S = topos[i].n_steps; m.E = topos[i].n_edges; m.P = topos[i].n_parallel;
-    m.bytes = plans[i].rec_bytes; m.offset = base + off; m.child_first = plans[i].child_first;
-    m.child_nibbles = plans[i].child_nibbles;
-    m.par_step.resize(m.P); m.par_branches.resize(m.P);
-    for (uint32_t q = 0; q < m.P; ++q) { m.par_step[q] = topos[i].parallel[q].step; m.par_branches[q] = topos[i].parallel[q].branches; }
-    c->slots_host[slot] = bf::Slot{(uint64_t)(uintptr_t)(c->arena + m.offset), m.bytes,
-                                   m.S | (m.P << 16) | (bf::slot_row_bytes(plans[i].ell) << 24)};
-    memcpy(&c->ff_host[(size_t)slot * bf::FF_STRIDE], plans[i].ff, sizeof plans[i].ff);
-    if (m.bytes > c->max_rec_bytes) c->max_rec_bytes = m.bytes;
-    if (m.bytes > c->max_rec_by_w[plans[i].W]) c->max_rec_by_w[plans[i].W] = m.bytes;
-    off += plans[i].rec_bytes;
-    slots_out[i] = slot;
-    c->n_alive++;
-    if (m.P) c->n_with_parallel++;
-  }
-  c->arena_used = base + total;
-  c->slots_dirty = true;
-  return BF_OK;
-}
-
-}  // namespace
+}  // namespace bf
 
 // =============================================================================== C ABI
 extern "C" {
@@ -978,8 +766,8 @@ int bf_create(bf_ctx** out, const bf_config* cfg) {
   if (cfg && (cfg->flags & 0xFFu) && (int)(cfg->flags & 0xFFu) < c->sm_count) c->sm_count -= (int)(cfg->flags & 0xFFu);   // BF_CFG_RESERVE_SMS
   c->stats.sm_count = (uint32_t)prop.multiProcessorCount;
   if (cudaSetDevice(dev) != cudaSuccess || cudaStreamCreateWithFlags(&c->stream, cudaStreamNonBlocking) != cudaSuccess ||
-      cudaMalloc(&c->d_counts, sizeof(bf_counts)) != cudaSuccess ||
-      cudaMalloc(&c->d_acc, bf_ctx::kAccSlots * 64) != cudaSuccess || cudaMemset(c->d_acc, 0, bf_ctx::kAccSlots * 64) != cudaSuccess ||
+      c->d_counts.alloc(sizeof(bf_counts) / 8) != cudaSuccess ||
+      c->d_acc.alloc(bf_ctx::kAccSlots * 8) != cudaSuccess || cudaMemset(c->d_acc, 0, bf_ctx::kAccSlots * 64) != cudaSuccess ||
       cudaHostAlloc(reinterpret_cast<void**>(&c->h_counts), 5 * sizeof(bf_counts), cudaHostAllocDefault) != cudaSuccess) {
     cudaGetLastError();
     bf_destroy(c);  // releases whatever was created
@@ -1005,11 +793,7 @@ void bf_destroy(bf_ctx* c) {
     if (c->ev_k[k]) cudaEventDestroy(c->ev_k[k]);
   }
   cudaFreeHost(c->h_counts);
-  cudaFree(c->arena); cudaFree(c->slots_dev); cudaFree(c->ff_dev); cudaFree(c->d_state); cudaFree(c->d_result); cudaFree(c->d_counts); cudaFree(c->d_acc);
-  cudaFree(c->d_defer); cudaFree(c->d_exp); cudaFree(c->d_exp_counts); cudaFree(c->d_offsets); cudaFree(c->d_block_sums); cudaFree(c->d_sched); cudaFree(c->d_deltas); cudaFree(c->d_rejected);
-  cudaFree(c->d_head); cudaFree(c->d_events); cudaFree(c->d_cblock); cudaFree(c->d_mig); cudaFree(c->d_redrive); cudaFree(c->d_retire);
-  for (Resident& r : c->resident) { cudaFree(r.d_state); cudaFree(r.d_result); cudaFree(r.d_result_prev); }
-  delete c;
+  delete c;   // the device buffers of the ctx and of its resident batches free themselves
 }
 
 int bf_topology_put_many(bf_ctx* c, const bf_topology* topos, uint32_t count, uint32_t* slots_out) {
@@ -1024,7 +808,7 @@ int bf_topology_put(bf_ctx* c, const bf_topology* topo, uint32_t* slot_out) { re
 
 static int check_locked(bf_ctx* c, const uint32_t* slots, uint32_t count, uint32_t* status_out) {
   if (count == 0) return BF_OK;
-  if (int rc = sync_slots(c, c->stream)) return rc;
+  if (int rc = bf::sync_slots(c, c->stream)) return rc;
   uint32_t* d_ids = nullptr;
   uint32_t* d_status = nullptr;
   BF_CUDA(c, cudaMalloc(&d_ids, (size_t)count * 4));
@@ -1060,7 +844,7 @@ int bf_topology_closure(bf_ctx* c, const uint32_t* slots, const uint32_t* steps,
   }
   if (count == 0) return BF_OK;
   BF_CUDA(c, cudaSetDevice(c->device));
-  if (int rc = sync_slots(c, c->stream)) return rc;
+  if (int rc = bf::sync_slots(c, c->stream)) return rc;
   uint32_t* d = nullptr;
   const size_t q_bytes = (size_t)count * 4, m_bytes = (size_t)count * words * 4;
   BF_CUDA(c, cudaMalloc(&d, 2 * q_bytes + m_bytes));
@@ -1174,10 +958,10 @@ int bf_eval_device(bf_ctx* c, const bf_batch* b, void* stream) {
   if (!c) return BF_EINVAL;
   std::lock_guard<std::mutex> g(c->mu);
   if (!b || b->struct_size != sizeof(bf_batch)) return fail(c, BF_EINVAL, "bad bf_batch.struct_size");
-  if (int rc = check_layout(c, b->layout)) return rc;
+  if (int rc = bf::check_layout(c, b->layout)) return rc;
   if (b->n_runs && (!b->state || !b->result)) return fail(c, BF_EINVAL, "null state/result");
   BF_CUDA(c, cudaSetDevice(c->device));
-  return run_pass(c, *b, static_cast<const uint8_t*>(b->state), static_cast<uint8_t*>(b->result), b->expansion,
+  return bf::run_pass(c, *b, static_cast<const uint8_t*>(b->state), static_cast<uint8_t*>(b->result), b->expansion,
                   reinterpret_cast<unsigned long long*>(b->counts), static_cast<cudaStream_t>(stream));
 }
 
@@ -1187,7 +971,7 @@ static int eval_host(bf_ctx* c, const bf_batch* b, bf_compact_out* co) {
   if (!b || b->struct_size != sizeof(bf_batch)) return fail(c, BF_EINVAL, "bad bf_batch.struct_size");
   if (co && co->struct_size != sizeof(bf_compact_out)) return fail(c, BF_EINVAL, "bad bf_compact_out.struct_size");
   if (co && co->events_cap && !co->events) return fail(c, BF_EINVAL, "null events with a non-zero events_cap");
-  if (int rc = check_layout(c, b->layout)) return rc;
+  if (int rc = bf::check_layout(c, b->layout)) return rc;
   if (b->n_runs && (!b->state || (!b->result && !co))) return fail(c, BF_EINVAL, "null state/result");
   c->last_eval_valid = false;
   const bf_layout& L = b->layout;
@@ -1209,11 +993,11 @@ static int eval_host(bf_ctx* c, const bf_batch* b, bf_compact_out* co) {
     }
   }
   BF_CUDA(c, cudaSetDevice(c->device));
-  if (int rc = ensure_dev(c, c->d_state, c->d_state_cap, sbytes)) return rc;
-  if (int rc = ensure_dev(c, c->d_result, c->d_result_cap, rbytes)) return rc;
+  if (int rc = c->d_state.ensure(c, sbytes)) return rc;
+  if (int rc = c->d_result.ensure(c, rbytes)) return rc;
   const bool want_exp = (b->flags & BF_EVAL_EXPANSION) && b->expansion && b->expansion_cap;
   if (want_exp)
-    if (int rc = ensure_dev(c, c->d_exp, c->d_exp_cap, (size_t)b->expansion_cap)) return rc;
+    if (int rc = c->d_exp.ensure(c, (size_t)b->expansion_cap)) return rc;
   cudaStream_t s = c->stream;
   // Large batches are cut into chunks of runs (runs are independent) so that the upload of chunk k+1, the
   // kernel of chunk k and the download of chunk k-1 overlap: PCIe is full duplex and the pass itself is ~5x
@@ -1229,7 +1013,7 @@ static int eval_host(bf_ctx* c, const bf_batch* b, bf_compact_out* co) {
     if (chunks < 1) chunks = 1;
   }
   if (chunks > 1)
-    if (int rc = ensure_pipe(c)) return rc;
+    if (int rc = bf::ensure_pipe(c)) return rc;
   const char* shape_env = getenv("BF_E2E_SHAPE");
   const bool taper = shape_env && !strcmp(shape_env, "taper");
   bf_counts hc{};
@@ -1260,7 +1044,7 @@ static int eval_host(bf_ctx* c, const bf_batch* b, bf_compact_out* co) {
         BF_CUDA(c, cudaStreamWaitEvent(s, c->ev_in[k], 0));
       }
       db.n_runs = (uint32_t)(hi - lo);
-      if (int rc = run_pass(c, db, c->d_state + so, c->d_result + ro, want_exp ? c->d_exp : nullptr, c->d_counts, s)) return rc;
+      if (int rc = bf::run_pass(c, db, c->d_state + so, c->d_result + ro, want_exp ? c->d_exp.p : nullptr, c->d_counts, s)) return rc;
       if (piped) {
         BF_CUDA(c, cudaEventRecord(c->ev_k[k], s));
         BF_CUDA(c, cudaStreamWaitEvent(c->s_out, c->ev_k[k], 0));
@@ -1268,7 +1052,7 @@ static int eval_host(bf_ctx* c, const bf_batch* b, bf_compact_out* co) {
       if (rb && !co) BF_CUDA(c, cudaMemcpyAsync(hr + ro, c->d_result + ro, rb, cudaMemcpyDeviceToHost, piped ? c->s_out : s));
     }
     if (co) {   // counts travel with the compaction's tail block
-      if (int rc = compact_enqueue(c, L, c->d_result, nullptr, b->n_runs, co, s, &first_slice, false)) return rc;
+      if (int rc = bf::compact_enqueue(c, L, c->d_result, nullptr, b->n_runs, co, s, &first_slice, false)) return rc;
     } else {
       BF_CUDA(c, cudaMemcpyAsync(c->h_counts, c->d_counts, sizeof hc, cudaMemcpyDeviceToHost, s));
     }
@@ -1294,7 +1078,7 @@ static int eval_host(bf_ctx* c, const bf_batch* b, bf_compact_out* co) {
     if (n) BF_CUDA(c, cudaMemcpy(b->expansion, c->d_exp, (size_t)n * sizeof(bf_expansion), cudaMemcpyDeviceToHost));
   }
   if (b->counts) *b->counts = hc;
-  if (co) return compact_finish(c, co, first_slice);
+  if (co) return bf::compact_finish(c, co, first_slice);
   return BF_OK;
 }
 
@@ -1308,7 +1092,7 @@ int bf_eval_compact(bf_ctx* c, const bf_batch* b, bf_compact_out* out) {
 static int fill_sched_params(bf_ctx* c, const bf_batch* b, const bf_sched_tables* t, bf::SchedParams& P) {
   if (!b || b->struct_size != sizeof(bf_batch)) return fail(c, BF_EINVAL, "bad bf_batch.struct_size");
   if (!t || t->struct_size != sizeof(bf_sched_tables)) return fail(c, BF_EINVAL, "bad bf_sched_tables.struct_size");
-  if (int rc = check_layout(c, b->layout)) return rc;
+  if (int rc = bf::check_layout(c, b->layout)) return rc;
   if ((t->n_stories && !t->story_limit) || (t->n_queues && (!t->queue_limit || !t->queue_aging_s)))
     return fail(c, BF_EINVAL, "null limit table");
   const bf_layout& L = b->layout;
@@ -1332,7 +1116,7 @@ int bf_schedule_device(bf_ctx* c, const bf_batch* b, const bf_sched_run* runs, c
   if (!out->story_running || !out->queue_running || !out->queue_max_priority || !out->global_running)
     return fail(c, BF_EINVAL, "device path: the totals arrays are the reduction scratch and must be given");
   BF_CUDA(c, cudaSetDevice(c->device));
-  if (int rc = sync_slots(c, static_cast<cudaStream_t>(stream))) return rc;
+  if (int rc = bf::sync_slots(c, static_cast<cudaStream_t>(stream))) return rc;
   P.slots = c->slots_dev;
   P.state = static_cast<const uint8_t*>(b->state); P.result = static_cast<const uint8_t*>(b->result);
   P.runs = runs; P.records = static_cast<uint8_t*>(out->records);
@@ -1368,7 +1152,7 @@ static int schedule_host(bf_ctx* c, const bf_batch* b, const bf_sched_run* runs,
   const size_t o_runs = take(n * sizeof(bf_sched_run)), o_rec = take(n * (size_t)P.stride), o_sr = take(ns * 4), o_qr = take(nq * 4),
                o_mp = take(nq * 4), o_gl = take(4), o_sl = take(ns * 4), o_ql = take(nq * 4), o_qa = take(nq * 4), o_sb = take(ns * 4),
                o_qb = take(nq * 4), o_pb = take(nq * 4);
-  if (int rc = ensure_dev(c, c->d_sched, c->d_sched_cap, off ? off : 16)) return rc;
+  if (int rc = c->d_sched.ensure(c, off ? off : 16)) return rc;
   uint8_t* d = c->d_sched;
   auto up = [&](size_t o, const void* src, size_t bytes) -> cudaError_t {
     return (src && bytes) ? cudaMemcpyAsync(d + o, src, bytes, cudaMemcpyHostToDevice, s) : cudaSuccess;
@@ -1417,727 +1201,6 @@ int bf_schedule(bf_ctx* c, const bf_batch* b, const bf_sched_run* runs, const bf
   return schedule_host(c, b, runs, t, out, nullptr, nullptr, true);
 }
 
-// ---- resident batches (row f2: incremental state upload) --------------------------------------------------
-static Resident* resident_of(bf_ctx* c, uint32_t h) { return h < c->resident.size() && c->resident[h].alive ? &c->resident[h] : nullptr; }
-
-int bf_resident_create(bf_ctx* c, const bf_layout* L, uint32_t capacity, uint32_t* handle_out) {
-  if (!c) return BF_EINVAL;
-  std::lock_guard<std::mutex> g(c->mu);
-  if (!L || !handle_out || capacity == 0) return fail(c, BF_EINVAL, "null layout / handle or zero capacity");
-  if (int rc = check_layout(c, *L)) return rc;
-  BF_CUDA(c, cudaSetDevice(c->device));
-  Resident r;
-  r.L = *L; r.cap = capacity;
-  const size_t mark_bytes = ((size_t)capacity + 3) / 4 * 16;   // padded: the list build reads four marks at a time
-  cudaError_t e = cudaMalloc(&r.d_state, (size_t)capacity * L->state_stride);
-  if (e == cudaSuccess) e = cudaMalloc(&r.d_result, (size_t)capacity * L->result_stride);
-  if (e == cudaSuccess) e = cudaMalloc(&r.d_mark, mark_bytes);
-  if (e == cudaSuccess) e = cudaMemsetAsync(r.d_state, 0, (size_t)capacity * L->state_stride, c->stream);
-  if (e == cudaSuccess) e = cudaMemsetAsync(r.d_mark, 0, mark_bytes, c->stream);
-  if (e == cudaSuccess) e = cudaStreamSynchronize(c->stream);
-  if (e != cudaSuccess) { cudaFree(r.d_state); cudaFree(r.d_result); cudaFree(r.d_mark); return fail(c, BF_ENOMEM, std::string("resident batch: ") + cudaGetErrorString(e)); }
-  r.alive = true;
-  uint32_t h = 0;
-  while (h < c->resident.size() && c->resident[h].alive) ++h;
-  if (h == c->resident.size()) c->resident.push_back(r); else c->resident[h] = r;
-  *handle_out = h;
-  return BF_OK;
-}
-
-int bf_resident_destroy(bf_ctx* c, uint32_t h) {
-  if (!c) return BF_EINVAL;
-  std::lock_guard<std::mutex> g(c->mu);
-  Resident* r = resident_of(c, h);
-  if (!r) return fail(c, BF_EINVAL, "unknown resident batch");
-  BF_CUDA(c, cudaSetDevice(c->device));
-  cudaStreamSynchronize(c->stream);
-  if (c->last_state == r->d_state) c->last_eval_valid = false;
-  cudaFree(r->d_state); cudaFree(r->d_result); cudaFree(r->d_result_prev); cudaFree(r->d_mark);
-  *r = Resident();
-  return BF_OK;
-}
-
-// Record the runs [first, end) as uploaded since the last full tick: the part at or above full_runs, merged with the ranges it
-// touches.
-static void note_uploaded(Resident* r, uint32_t first, uint32_t end) {
-  uint32_t lo = std::max(first, r->full_runs), hi = end;
-  if (lo >= hi) return;
-  auto it = r->uploaded.upper_bound(lo);
-  if (it != r->uploaded.begin() && std::prev(it)->second >= lo) {
-    --it;
-    lo = it->first; hi = std::max(hi, it->second);
-    it = r->uploaded.erase(it);
-  }
-  while (it != r->uploaded.end() && it->first <= hi) { hi = std::max(hi, it->second); it = r->uploaded.erase(it); }
-  r->uploaded.emplace(lo, hi);
-}
-
-int bf_resident_upload(bf_ctx* c, uint32_t h, uint32_t first, uint32_t n, const void* records) {
-  if (!c) return BF_EINVAL;
-  std::lock_guard<std::mutex> g(c->mu);
-  Resident* r = resident_of(c, h);
-  if (!r) return fail(c, BF_EINVAL, "unknown resident batch");
-  if ((uint64_t)first + n > r->cap || (n && !records)) return fail(c, BF_EINVAL, "run range outside the resident batch");
-  if (n == 0) return BF_OK;
-  BF_CUDA(c, cudaSetDevice(c->device));
-  if (c->last_state == r->d_state) c->last_eval_valid = false;   // the evaluated snapshot is gone: bf_schedule must follow a new pass
-  r->prev_valid = false;                                          // full records arrived: the next changed-only tick lists every run
-  BF_CUDA(c, cudaMemcpyAsync(r->d_state + (size_t)first * r->L.state_stride, records, (size_t)n * r->L.state_stride, cudaMemcpyHostToDevice, c->stream));
-  BF_CUDA(c, bf::launch_mark_runs(r->d_mark, first, n, r->epoch << 1 | 1u, c->stream));   // touched and must be listed
-  c->stats.kernel_launches += 1;
-  r->pending += n;
-  note_uploaded(r, first, first + n);
-  BF_CUDA(c, cudaStreamSynchronize(c->stream));
-  return BF_OK;
-}
-
-int bf_resident_download(bf_ctx* c, uint32_t h, uint32_t first, uint32_t n, void* records) {
-  if (!c) return BF_EINVAL;
-  std::lock_guard<std::mutex> g(c->mu);
-  Resident* r = resident_of(c, h);
-  if (!r) return fail(c, BF_EINVAL, "unknown resident batch");
-  if ((uint64_t)first + n > r->cap || (n && !records)) return fail(c, BF_EINVAL, "run range outside the resident batch");
-  if (n == 0) return BF_OK;
-  BF_CUDA(c, cudaSetDevice(c->device));
-  BF_CUDA(c, cudaMemcpyAsync(records, r->d_state + (size_t)first * r->L.state_stride, (size_t)n * r->L.state_stride, cudaMemcpyDeviceToHost, c->stream));
-  BF_CUDA(c, cudaStreamSynchronize(c->stream));
-  return BF_OK;
-}
-
-// H2D of the deltas + the scatter kernel on the ctx stream, no synchronisation; the rejected counter is read by the caller
-static int resident_apply_async(bf_ctx* c, Resident* r, const bf_delta* deltas, uint32_t n) {
-  if (int rc = ensure_dev(c, c->d_deltas, c->d_deltas_cap, n ? n : 1)) return rc;
-  if (!c->d_rejected) { BF_CUDA(c, cudaMalloc(&c->d_rejected, 16)); c->rejected_clean = false; }
-  cudaStream_t s = c->stream;
-  if (!c->rejected_clean) { BF_CUDA(c, cudaMemsetAsync(c->d_rejected, 0, 4, s)); c->rejected_clean = true; }
-  if (n == 0) return BF_OK;
-  c->rejected_clean = false;   // the scatter kernel may count; whoever reads the counter decides whether it is clean again
-  // deltas in pinned host memory are read by the scatter kernel itself over PCIe (one launch instead of a copy and a launch:
-  // BF_NO_ZC_DELTAS restores the upload), any other buffer is uploaded first
-  const bf_delta* d_src = c->d_deltas;
-  bool direct = false;
-  if (!getenv("BF_NO_ZC_DELTAS")) {
-    if (void* d = pinned_dev(deltas)) {
-      d_src = static_cast<const bf_delta*>(d);
-      direct = true;
-    }
-  }
-  if (!direct) BF_CUDA(c, cudaMemcpyAsync(c->d_deltas, deltas, (size_t)n * sizeof(bf_delta), cudaMemcpyHostToDevice, s));
-  bf::DeltaParams P{};
-  P.state = r->d_state; P.deltas = d_src; P.n = n; P.n_runs = r->cap;
-  P.words = r->L.words; P.state_stride = r->L.state_stride; P.off_phase = r->L.off_phase; P.off_cond = r->L.off_cond;
-  P.off_decision = r->L.off_decision; P.off_child = r->L.off_child; P.child_nibbles = r->L.child_nibbles;
-  P.rejected = c->d_rejected;
-  P.mark = r->d_mark; P.mark_value = r->epoch << 1;
-  BF_CUDA(c, bf::launch_apply_deltas(P, s));
-  c->stats.kernel_launches += 1;
-  return BF_OK;
-}
-
-int bf_resident_apply(bf_ctx* c, uint32_t h, const bf_delta* deltas, uint32_t n) {
-  if (!c) return BF_EINVAL;
-  std::lock_guard<std::mutex> g(c->mu);
-  Resident* r = resident_of(c, h);
-  if (!r) return fail(c, BF_EINVAL, "unknown resident batch");
-  if (n && !deltas) return fail(c, BF_EINVAL, "null deltas");
-  if (n == 0) return BF_OK;
-  BF_CUDA(c, cudaSetDevice(c->device));
-  if (c->last_state == r->d_state) c->last_eval_valid = false;
-  r->pending += n;
-  const int rc = resident_apply_async(c, r, deltas, n);
-  cudaError_t e = rc == BF_OK ? cudaMemcpyAsync(c->h_counts, c->d_rejected, 4, cudaMemcpyDeviceToHost, c->stream) : cudaSuccess;
-  const cudaError_t es = cudaStreamSynchronize(c->stream);  // the caller's delta buffer may be reused after return
-  if (rc != BF_OK) return rc;
-  if (e != cudaSuccess) return cuda_fail(c, e, "bf_resident_apply");
-  if (es != cudaSuccess) return cuda_fail(c, es, "cudaStreamSynchronize");
-  const uint32_t rejected = *reinterpret_cast<const uint32_t*>(c->h_counts);
-  if (rejected) return fail(c, BF_EINVAL, std::to_string(rejected) + " delta(s) outside the record (run, index, code or absent field); the others were applied");
-  return BF_OK;
-}
-
-// deltas (optional) + one pass + results, one synchronisation: the pass is cut into run chunks whose kernels overlap
-// the download of the previous chunk's result records (as bf_eval does for both directions)
-static int resident_tick_locked(bf_ctx* c, Resident* r, const bf_delta* deltas, uint32_t n_deltas, uint32_t n_runs, uint32_t flags,
-                                uint32_t max_iterations, void* result, bf_counts* counts, bf_compact_out* co = nullptr) {
-  c->last_eval_valid = false;
-  if (co && co->struct_size != sizeof(bf_compact_out)) return fail(c, BF_EINVAL, "bad bf_compact_out.struct_size");
-  if (co && co->events_cap && !co->events) return fail(c, BF_EINVAL, "null events with a non-zero events_cap");
-  if (n_runs > r->cap || (n_runs && !result && !co)) return fail(c, BF_EINVAL, "n_runs exceeds the resident batch / null result");
-  if (flags & BF_EVAL_EXPANSION) return fail(c, BF_EINVAL, "expansion is not offered on the resident path");
-  if (n_deltas && !deltas) return fail(c, BF_EINVAL, "null deltas");
-  BF_CUDA(c, cudaSetDevice(c->device));
-  cudaStream_t s = c->stream;
-  const bf_layout& L = r->L;
-  const size_t rbytes = (size_t)n_runs * L.result_stride;
-  const bool changed_only = co && (flags & BF_EVAL_CHANGED_ONLY);
-  flags &= ~(uint32_t)BF_EVAL_CHANGED_ONLY;
-  const uint8_t* d_prev = nullptr;
-  if (changed_only) {   // this pass writes the other buffer; the one it leaves behind is what "changed" is measured against
-    if (!r->d_result_prev) {
-      cudaError_t e = cudaMalloc(&r->d_result_prev, (size_t)r->cap * L.result_stride);
-      if (e != cudaSuccess) return fail(c, BF_ENOMEM, std::string("resident batch (second result buffer): ") + cudaGetErrorString(e));
-    }
-    std::swap(r->d_result, r->d_result_prev);
-    if (r->prev_valid && r->prev_runs == n_runs) d_prev = r->d_result_prev;
-  }
-  uint32_t chunks = 1;
-  uint64_t first_slice = 0;
-  if (!co && rbytes >= (2u << 20)) {
-    chunks = (uint32_t)((rbytes + (1u << 20)) / (2u << 20));   // ~2 MB of result records per chunk
-    if (const char* e = getenv("BF_E2E_CHUNKS")) chunks = (uint32_t)atoi(e);
-    if (chunks > bf_ctx::kMaxChunks) chunks = bf_ctx::kMaxChunks;
-    if (chunks < 1) chunks = 1;
-  }
-  if (chunks > 1)
-    if (int rc = ensure_pipe(c)) return rc;
-  uint32_t* h_rej = reinterpret_cast<uint32_t*>(c->h_counts + 1);  // second pinned slot: h_counts is 2 x bf_counts
-  auto body = [&]() -> int {
-    if (int rc = resident_apply_async(c, r, deltas, n_deltas)) return rc;
-    const bool may_fuse = co && chunks == 1 && !d_prev && !changed_only && !getenv("BF_NO_FUSED_HEADS");
-    if (may_fuse) {
-      if (int rc = compact_prepare(c, n_runs, s)) return rc;
-      c->fuse_head = c->d_head; c->fuse_sums = cblock_sums(c, c->cblock_flip);
-    }
-    bf_batch db{};
-    db.struct_size = sizeof(bf_batch);
-    db.flags = flags & ~(uint32_t)(BF_EVAL_VALIDATE | BF_EVAL_COUNTS_SET | BF_EVAL_PIPELINED); db.max_iterations = max_iterations; db.layout = L;
-    // one chunk: the pass overwrites the counts block itself (no memset in front of it); several chunks add into a zeroed block
-    if (chunks == 1) db.flags |= BF_EVAL_COUNTS_SET;
-    else BF_CUDA(c, cudaMemsetAsync(c->d_counts, 0, sizeof(bf_counts), s));
-    for (uint32_t k = 0; k < chunks; ++k) {
-      const size_t lo = (size_t)n_runs * k / chunks, hi = (size_t)n_runs * (k + 1) / chunks;
-      db.n_runs = (uint32_t)(hi - lo);
-      const int rc_pass = run_pass(c, db, r->d_state + lo * L.state_stride, r->d_result + lo * L.result_stride, nullptr, c->d_counts, s);
-      c->fuse_head = nullptr; c->fuse_sums = nullptr;
-      if (rc_pass) return rc_pass;
-      const bool piped = chunks > 1;
-      if (piped) {
-        BF_CUDA(c, cudaEventRecord(c->ev_k[k], s));
-        BF_CUDA(c, cudaStreamWaitEvent(c->s_out, c->ev_k[k], 0));
-      }
-      if (hi > lo && !co)
-        BF_CUDA(c, cudaMemcpyAsync(static_cast<uint8_t*>(result) + lo * L.result_stride, r->d_result + lo * L.result_stride,
-                                   (hi - lo) * L.result_stride, cudaMemcpyDeviceToHost, piped ? c->s_out : s));
-    }
-    if (co) {   // counts and the rejected-delta counter travel with the compaction's tail block
-      if (int rc2 = compact_enqueue(c, L, r->d_result, d_prev, n_runs, co, s, &first_slice, true, may_fuse && c->fused_done)) return rc2;
-    } else {
-      BF_CUDA(c, cudaMemcpyAsync(c->h_counts, c->d_counts, sizeof(bf_counts), cudaMemcpyDeviceToHost, s));
-      BF_CUDA(c, cudaMemcpyAsync(h_rej, c->d_rejected, 4, cudaMemcpyDeviceToHost, s));
-    }
-    return BF_OK;
-  };
-  const int rc = body();
-  cudaError_t es = cudaStreamSynchronize(s);
-  if (chunks > 1) {
-    const cudaError_t e2 = cudaStreamSynchronize(c->s_out);
-    if (es == cudaSuccess) es = e2;
-  }
-  r->prev_valid = false;
-  r->need_full = true;
-  if (rc != BF_OK || es != cudaSuccess) {   // whatever the kernels left in the self-cleaning scratch is unknown: zero it before the next use
-    c->cblock_clean = false; c->rejected_clean = false;
-    c->fuse_head = nullptr; c->fuse_sums = nullptr;
-  }
-  if (rc != BF_OK) return rc;
-  if (es != cudaSuccess) return cuda_fail(c, es, "cudaStreamSynchronize");
-  r->prev_valid = true; r->prev_runs = n_runs;
-  // a full evaluation: it ends the current touch epoch (touched ticks, above Resident)
-  r->need_full = false;
-  r->full_epoch = r->epoch++; r->full_runs = n_runs;
-  r->last_fixpoint = flags & BF_EVAL_FIXPOINT; r->last_max_iter = max_iterations; r->slot_changes_seen = c->slot_changes;
-  r->pending = 0; r->uploaded.clear();
-  if (r->epoch >= 0x7FFFFFFFu) {   // the epoch must fit mark >> 1: once per 2^31 full ticks the marks start over
-    BF_CUDA(c, cudaMemsetAsync(r->d_mark, 0, ((size_t)r->cap + 3) / 4 * 16, s));
-    r->epoch = 1; r->full_epoch = 0;
-  }
-  if (co) {
-    c->cblock_clean = true; c->rejected_clean = true;   // the compaction's tail block delivered and cleared both
-    const unsigned long long* tail = reinterpret_cast<const unsigned long long*>(c->h_counts + 2);
-    memcpy(c->h_counts, tail + 1, sizeof(bf_counts));
-    *h_rej = (uint32_t)tail[5];
-  }
-  if (counts) *counts = *c->h_counts;
-  c->stats.last_eval_chunks = chunks;
-  c->last_eval_valid = true; c->last_eval_runs = n_runs; c->last_eval_layout = L;
-  c->last_state = r->d_state; c->last_result = r->d_result;
-  if (co)
-    if (int rc2 = compact_finish(c, co, first_slice)) return rc2;
-  if (n_deltas && *h_rej) return fail(c, BF_EINVAL, std::to_string(*h_rej) + " delta(s) outside the record (run, index, code or absent field); the others were applied and the pass ran");
-  return BF_OK;
-}
-
-int bf_resident_eval(bf_ctx* c, uint32_t h, uint32_t n_runs, uint32_t flags, uint32_t max_iterations, void* result, bf_counts* counts) {
-  if (!c) return BF_EINVAL;
-  std::lock_guard<std::mutex> g(c->mu);
-  Resident* r = resident_of(c, h);
-  if (!r) return fail(c, BF_EINVAL, "unknown resident batch");
-  return resident_tick_locked(c, r, nullptr, 0, n_runs, flags, max_iterations, result, counts);
-}
-
-int bf_resident_tick(bf_ctx* c, uint32_t h, const bf_delta* deltas, uint32_t n_deltas, uint32_t n_runs, uint32_t flags,
-                     uint32_t max_iterations, void* result, bf_counts* counts) {
-  if (!c) return BF_EINVAL;
-  std::lock_guard<std::mutex> g(c->mu);
-  Resident* r = resident_of(c, h);
-  if (!r) return fail(c, BF_EINVAL, "unknown resident batch");
-  return resident_tick_locked(c, r, deltas, n_deltas, n_runs, flags, max_iterations, result, counts);
-}
-
-int bf_resident_tick_compact(bf_ctx* c, uint32_t h, const bf_delta* deltas, uint32_t n_deltas, uint32_t n_runs, uint32_t flags,
-                             uint32_t max_iterations, bf_compact_out* out, bf_counts* counts) {
-  if (!c) return BF_EINVAL;
-  std::lock_guard<std::mutex> g(c->mu);
-  if (!out) return fail(c, BF_EINVAL, "null bf_compact_out");
-  Resident* r = resident_of(c, h);
-  if (!r) return fail(c, BF_EINVAL, "unknown resident batch");
-  return resident_tick_locked(c, r, deltas, n_deltas, n_runs, flags, max_iterations, nullptr, counts, out);
-}
-
-// Were all runs of [lo, hi) uploaded since the last full tick?  (The ranges are merged: one of them must hold all of it.)
-static bool uploads_cover(const std::map<uint32_t, uint32_t>& ranges, uint32_t lo, uint32_t hi) {
-  auto it = ranges.upper_bound(lo);
-  if (it == ranges.begin()) return false;
-  --it;
-  return it->first <= lo && it->second >= hi;
-}
-
-// A touched tick: scatter -> list build -> pass over the list (into the second result buffer) -> list-mode compaction, which
-// brings the current result records up to date.  Falls back to a full compact tick where the baseline rules require one.
-static int touched_tick_locked(bf_ctx* c, Resident* r, const bf_delta* deltas, uint32_t n_deltas, uint32_t n_runs, uint32_t flags,
-                               uint32_t max_iterations, bf_touched_out* out, bf_counts* counts) {
-  if (out->struct_size != sizeof(bf_touched_out)) return fail(c, BF_EINVAL, "bad bf_touched_out.struct_size");
-  if (flags & ~(uint32_t)(BF_EVAL_FIXPOINT | BF_EVAL_NO_COUNTS)) return fail(c, BF_EINVAL, "touched ticks take BF_EVAL_FIXPOINT and BF_EVAL_NO_COUNTS only");
-  if (out->runs_cap && (!out->runs || !out->head)) return fail(c, BF_EINVAL, "null runs / head with a non-zero runs_cap");
-  if (out->events_cap && !out->events) return fail(c, BF_EINVAL, "null events with a non-zero events_cap");
-  if (n_runs > r->cap) return fail(c, BF_EINVAL, "n_runs exceeds the resident batch");
-  if (n_deltas && !deltas) return fail(c, BF_EINVAL, "null deltas");
-  BF_CUDA(c, cudaSetDevice(c->device));
-  const bool full = r->need_full || c->slot_changes != r->slot_changes_seen || (flags & BF_EVAL_FIXPOINT) != r->last_fixpoint ||
-                    max_iterations != r->last_max_iter || r->epoch >= 0x7FFFFFFEu ||
-                    (n_runs > r->full_runs && !uploads_cover(r->uploaded, r->full_runs, n_runs));
-  if (full) {   // a plain compact tick: every run evaluated and listed, heads in run order
-    bf_compact_out co{};
-    co.struct_size = sizeof co; co.events = out->events; co.events_cap = out->events_cap;
-    const int rc = resident_tick_locked(c, r, deltas, n_deltas, n_runs, flags, max_iterations, nullptr, counts, &co);
-    if (!c->last_eval_valid || c->last_state != r->d_state) return rc;   // no results (rejected deltas alone still deliver them)
-    const uint32_t n = std::min(n_runs, out->runs_cap);
-    if (n) BF_CUDA(c, cudaMemcpy(out->head, c->d_head, (size_t)n * 4, cudaMemcpyDeviceToHost));
-    for (uint32_t i = 0; i < n; ++i) out->runs[i] = i;
-    out->full = 1; out->n_listed = n_runs; out->n_evaluated = n_runs; out->n_events = co.n_events;
-    return rc;
-  }
-
-  c->last_eval_valid = false;
-  cudaStream_t s = c->stream;
-  const bf_layout& L = r->L;
-  const uint32_t bound = (uint32_t)std::min<uint64_t>(n_runs, r->pending + n_deltas);   // >= the touched runs below n_runs
-  r->pending += n_deltas;
-  const uint64_t cap = out->events ? out->events_cap : 0;
-  const uint32_t runs_n = std::min(bound, out->runs_cap);
-  if (!r->d_result_prev) {
-    cudaError_t e = cudaMalloc(&r->d_result_prev, (size_t)r->cap * L.result_stride);
-    if (e != cudaSuccess) return fail(c, BF_ENOMEM, std::string("resident batch (second result buffer): ") + cudaGetErrorString(e));
-  }
-  const uint32_t nb = (bound + 511) / 512, nbl = (r->cap + 2047) / 2048;
-  if (int rc = ensure_dev(c, c->d_tlist, c->d_tlist_cap, (size_t)bound + 1)) return rc;
-  if (int rc = ensure_dev(c, c->d_tpos_head, c->d_tpos_head_cap, bound ? bound : 1)) return rc;
-  if (int rc = ensure_dev(c, c->d_tsums, c->d_tsums_cap, 2 * (size_t)nb + 2 * (size_t)nbl + 1)) return rc;
-  if (int rc = ensure_dev(c, c->d_events, c->d_events_cap, cap ? (size_t)cap : 1)) return rc;
-  // the caller's pinned buffers get the lists posted by the emit kernel, any other buffer gets them by a download
-  uint32_t* p_runs = static_cast<uint32_t*>(pinned_dev(out->runs));
-  uint32_t* p_head = static_cast<uint32_t*>(pinned_dev(out->head));
-  uint16_t* p_events = cap ? static_cast<uint16_t*>(pinned_dev(out->events)) : nullptr;
-  if (!p_runs || !p_head) {
-    if (int rc = ensure_dev(c, c->d_truns, c->d_truns_cap, runs_n ? runs_n : 1)) return rc;
-    if (int rc = ensure_dev(c, c->d_thead, c->d_thead_cap, runs_n ? runs_n : 1)) return rc;
-  }
-  unsigned long long* tail = reinterpret_cast<unsigned long long*>(c->h_counts + 2);   // 9 x u64 in the pinned block
-  uint64_t first_slice = 0;
-  auto body = [&]() -> int {
-    if (int rc = resident_apply_async(c, r, deltas, n_deltas)) return rc;
-    if (bound == 0) {   // nothing below n_runs can be touched: no launch beyond the scatter
-      if (n_deltas) BF_CUDA(c, cudaMemcpyAsync(tail + 5, c->d_rejected, 4, cudaMemcpyDeviceToHost, s));
-      return BF_OK;
-    }
-    bf::TouchedParams T{};
-    bf::CompactParams& P = T.C;
-    P.result = r->d_result_prev; P.prev_result = r->d_result;
-    P.events = p_events ? p_events : c->d_events; P.cap = cap;
-    P.host_tail = tail; P.counts = (flags & BF_EVAL_NO_COUNTS) ? nullptr : c->d_counts; P.rejected = c->d_rejected;
-    P.n_runs = bound; P.words = L.words; P.result_stride = L.result_stride; P.result_tail = result_tail_of(L);
-    P.off_ready = L.off_ready; P.off_skip = L.off_skip;
-    P.off_fail = L.off_fail; P.off_needs_cond = L.off_needs_cond; P.off_skip_dep = L.off_skip_dep;
-    T.mark = r->d_mark; T.full_epoch = r->full_epoch; T.n_scan = n_runs; T.n_marks = r->cap; T.bound = bound;
-    T.list = c->d_tlist + 1; T.list_count = c->d_tlist; T.pos_head = c->d_tpos_head;
-    T.sums = c->d_tsums; T.sums_listed = c->d_tsums + nb; T.scan_sums = c->d_tsums + 2 * (size_t)nb;
-    T.carry_sums = T.scan_sums + nbl;
-    T.out_runs = p_runs && p_head ? p_runs : c->d_truns; T.out_head = p_runs && p_head ? p_head : c->d_thead; T.runs_cap = runs_n;
-    c->rejected_clean = false;   // the emit kernel delivers and clears the counter; a failed call leaves it to be zeroed
-    BF_CUDA(c, bf::launch_touched_list(T, s));
-    bf_batch db{};
-    db.struct_size = sizeof(bf_batch);
-    db.flags = flags | BF_EVAL_COUNTS_SET; db.max_iterations = max_iterations; db.layout = L; db.n_runs = bound;
-    if (int rc = run_pass(c, db, r->d_state, r->d_result_prev, nullptr, c->d_counts, s, c->d_tlist + 1, c->d_tlist)) return rc;
-    BF_CUDA(c, bf::launch_touched_compact(T, s));
-    c->stats.kernel_launches += 4;
-    if (runs_n && !(p_runs && p_head)) {
-      BF_CUDA(c, cudaMemcpyAsync(out->runs, c->d_truns, (size_t)runs_n * 4, cudaMemcpyDeviceToHost, s));
-      BF_CUDA(c, cudaMemcpyAsync(out->head, c->d_thead, (size_t)runs_n * 4, cudaMemcpyDeviceToHost, s));
-    }
-    uint64_t guess = c->last_touched_events + c->last_touched_events / 32 + 1024;   // the previous touched tick's list + 3 %
-    if (guess > cap) guess = cap;
-    if (p_events) guess = 0;
-    if (guess) BF_CUDA(c, cudaMemcpyAsync(out->events, c->d_events, (size_t)guess * sizeof(uint16_t), cudaMemcpyDeviceToHost, s));
-    first_slice = p_events ? cap : guess;
-    return BF_OK;
-  };
-  const int rc = body();
-  const cudaError_t es = cudaStreamSynchronize(s);
-  if (rc != BF_OK || es != cudaSuccess) {   // marks and current records may be half updated: the next touched tick is a full one
-    r->need_full = true; c->rejected_clean = false;
-    if (rc != BF_OK) return rc;
-    return cuda_fail(c, es, "cudaStreamSynchronize");
-  }
-  bf_counts hc{};
-  uint64_t n_events = 0, listed = 0, evaluated = 0, rejected = 0;
-  if (bound == 0) {
-    rejected = n_deltas ? *reinterpret_cast<const uint32_t*>(tail + 5) : 0u;   // (the counter is zeroed before its next use)
-  } else {
-    n_events = tail[0]; memcpy(&hc, tail + 1, sizeof hc); rejected = tail[5]; listed = tail[6]; evaluated = tail[7];
-    r->pending = tail[8];       // every touched run below n_runs was evaluated: the ones above it are all that is left
-    c->rejected_clean = true;   // delivered and cleared by the emit kernel
-  }
-  const uint64_t have = std::min<uint64_t>(n_events, cap);
-  if (have > first_slice)
-    BF_CUDA(c, cudaMemcpy(out->events + first_slice, c->d_events + first_slice, (size_t)(have - first_slice) * sizeof(uint16_t),
-                          cudaMemcpyDeviceToHost));
-  c->last_touched_events = n_events;
-  out->full = 0; out->n_listed = (uint32_t)listed; out->n_evaluated = (uint32_t)evaluated; out->n_events = n_events;
-  if (counts) *counts = hc;
-  c->last_eval_valid = true; c->last_eval_runs = n_runs; c->last_eval_layout = L;
-  c->last_state = r->d_state; c->last_result = r->d_result;
-  if (rejected) return fail(c, BF_EINVAL, std::to_string(rejected) + " delta(s) outside the record (run, index, code or absent field); the others were applied and the pass ran");
-  return BF_OK;
-}
-
-int bf_resident_tick_touched(bf_ctx* c, uint32_t h, const bf_delta* deltas, uint32_t n_deltas, uint32_t n_runs, uint32_t flags,
-                             uint32_t max_iterations, bf_touched_out* out, bf_counts* counts) {
-  if (!c) return BF_EINVAL;
-  std::lock_guard<std::mutex> g(c->mu);
-  if (!out) return fail(c, BF_EINVAL, "null bf_touched_out");
-  Resident* r = resident_of(c, h);
-  if (!r) return fail(c, BF_EINVAL, "unknown resident batch");
-  return touched_tick_locked(c, r, deltas, n_deltas, n_runs, flags, max_iterations, out, counts);
-}
-
-// A Story edited while its runs are live: re-index the runs of old_slot to new_slot's step indices in place (resident.cu).  All
-// checks come first, so a rejected call changes nothing; then one upload of the tables, one launch, one synchronisation.
-int bf_resident_migrate(bf_ctx* c, uint32_t h, bf_migration* m) {
-  if (!c) return BF_EINVAL;
-  std::lock_guard<std::mutex> g(c->mu);
-  if (!m || m->struct_size != sizeof(bf_migration)) return fail(c, BF_EINVAL, "null bf_migration or bad struct_size");
-  Resident* r = resident_of(c, h);
-  if (!r) return fail(c, BF_EINVAL, "unknown resident batch");
-  const bf_layout& L = r->L;
-  if (m->n_runs > r->cap) return fail(c, BF_EINVAL, "n_runs exceeds the resident batch");
-  auto alive = [&](uint32_t s) { return s < c->meta.size() && c->meta[s].alive; };
-  if (!alive(m->old_slot) || !alive(m->new_slot)) return fail(c, BF_ETOPO, "migration between unknown topology slots");
-  if (m->old_slot == m->new_slot) return fail(c, BF_EINVAL, "migration from a slot to itself");
-  const TopoMeta& mo = c->meta[m->old_slot];
-  const TopoMeta& mn = c->meta[m->new_slot];
-  if (m->n_old_steps != mo.S || !m->step_map) return fail(c, BF_EINVAL, "step_map must have one entry per step of old_slot");
-  const bool child = L.off_child != BF_OFF_NONE;
-  if (mo.S > L.steps_max || mn.S > L.steps_max || (child && (mo.child_nibbles > L.child_nibbles || mn.child_nibbles > L.child_nibbles)))
-    return fail(c, BF_ETOPO, "topology does not fit the batch layout (steps_max / child_nibbles)");
-  std::vector<uint16_t> inv((size_t)L.words * 32, (uint16_t)BF_MIGRATE_GONE);
-  for (uint32_t i = 0; i < mo.S; ++i) {
-    const uint32_t t = m->step_map[i];
-    if (t == BF_MIGRATE_GONE) continue;
-    if (t >= mn.S) return fail(c, BF_EINVAL, "step_map[" + std::to_string(i) + "] is not a step of new_slot");
-    if (inv[t] != BF_MIGRATE_GONE) return fail(c, BF_EINVAL, "step_map is not injective (new step " + std::to_string(t) + ")");
-    inv[t] = (uint16_t)i;
-  }
-  std::vector<bf::MigrateDesc> descs;
-  for (uint32_t q = 0; q < mn.P; ++q) {
-    const uint32_t o = inv[mn.par_step[q]];
-    if (o == BF_MIGRATE_GONE) continue;
-    const auto it = std::lower_bound(mo.par_step.begin(), mo.par_step.end(), (uint16_t)o);   // descs ascend by step
-    if (it == mo.par_step.end() || *it != o) continue;   // the old step was not parallel: the desc starts unregistered
-    const uint32_t p = (uint32_t)(it - mo.par_step.begin());
-    if (mo.par_branches[p] != mn.par_branches[q])
-      return fail(c, BF_EINVAL, "parallel step " + std::to_string(o) + " changes its branch count: re-pack its runs on the host");
-    bf::MigrateDesc d{};
-    d.old_first = mo.child_first[p]; d.new_first = mn.child_first[q];
-    d.branches = mn.par_branches[q]; d.old_p = (uint16_t)p; d.new_p = (uint16_t)q;
-    descs.push_back(d);
-  }
-  m->migrated = 0;
-  BF_CUDA(c, cudaSetDevice(c->device));
-  cudaStream_t s = c->stream;
-  const size_t o_inv = 16, o_desc = round_up_sz(o_inv + inv.size() * 2, 16), bytes = o_desc + descs.size() * sizeof(bf::MigrateDesc);
-  if (int rc = ensure_dev(c, c->d_mig, c->d_mig_cap, bytes)) return rc;
-  std::vector<uint8_t> blob(bytes, 0);   // the counter starts at zero
-  memcpy(blob.data() + o_inv, inv.data(), inv.size() * 2);
-  if (!descs.empty()) memcpy(blob.data() + o_desc, descs.data(), descs.size() * sizeof(bf::MigrateDesc));
-  if (c->last_state == r->d_state) c->last_eval_valid = false;   // as after an upload: bf_schedule must follow a new pass
-  bf::MigrateParams P{};
-  P.state = r->d_state; P.mark = r->d_mark; P.mark_value = r->epoch << 1 | 1u;   // touched and must be listed
-  P.migrated = reinterpret_cast<uint32_t*>(c->d_mig);
-  P.inv = reinterpret_cast<const uint16_t*>(c->d_mig + o_inv);
-  P.desc = reinterpret_cast<const bf::MigrateDesc*>(c->d_mig + o_desc); P.n_desc = (uint32_t)descs.size();
-  P.n_runs = m->n_runs; P.old_slot = m->old_slot; P.new_slot = m->new_slot;
-  P.words = L.words; P.state_stride = L.state_stride; P.off_phase = L.off_phase; P.off_cond = L.off_cond;
-  P.off_decision = L.off_decision; P.off_child = L.off_child; P.child_nibbles = L.child_nibbles;
-  cudaError_t e = cudaMemcpyAsync(c->d_mig, blob.data(), bytes, cudaMemcpyHostToDevice, s);
-  if (e == cudaSuccess) e = bf::launch_migrate(P, s);
-  if (e == cudaSuccess) e = cudaMemcpyAsync(c->h_counts, c->d_mig, 4, cudaMemcpyDeviceToHost, s);
-  const cudaError_t es = cudaStreamSynchronize(s);
-  if (e == cudaSuccess) e = es;
-  if (e != cudaSuccess) {   // some records may have moved: the next touched tick evaluates and lists every run
-    r->need_full = true; r->prev_valid = false;
-    return cuda_fail(c, e, "bf_resident_migrate");
-  }
-  c->stats.kernel_launches += m->n_runs ? 1 : 0;
-  m->migrated = *reinterpret_cast<const uint32_t*>(c->h_counts);
-  r->pending += m->migrated;   // the touched-list bound counts the migrated runs as it counts uploaded ones
-  return BF_OK;
-}
-
-// An operator redrive of live runs (resident.cu).  All checks come first, so a rejected call changes nothing.  The distinct
-// (slot, step) keys get one closure mask each from the closure kernel (a mass redrive of one Story from one step costs one
-// closure), then one launch resets every request's set.  One H2D copy, at most two launches, one D2H copy, one synchronisation.
-int bf_resident_redrive(bf_ctx* c, uint32_t h, const bf_redrive* req, uint32_t n, uint8_t* status_out, uint32_t* applied_out) {
-  if (!c) return BF_EINVAL;
-  std::lock_guard<std::mutex> g(c->mu);
-  Resident* r = resident_of(c, h);
-  if (!r) return fail(c, BF_EINVAL, "unknown resident batch");
-  if (n && !req) return fail(c, BF_EINVAL, "null requests");
-  const bf_layout& L = r->L;
-  const bool child = L.off_child != BF_OFF_NONE;
-  std::unordered_map<uint64_t, uint32_t> key_of;   // (slot, step) -> key index
-  std::vector<uint32_t> key(n), key_slot, key_step;
-  for (uint32_t i = 0; i < n; ++i) {
-    const bf_redrive& q = req[i];
-    auto at = [i] { return "request " + std::to_string(i) + ": "; };   // built on failure only
-    if (q.run >= r->cap) return fail(c, BF_EINVAL, at() + "run outside the resident batch");
-    if (q.reserved != 0) return fail(c, BF_EINVAL, at() + "reserved must be 0");
-    if (q.slot >= c->meta.size() || !c->meta[q.slot].alive) return fail(c, BF_ETOPO, at() + "unknown topology slot");
-    const TopoMeta& m = c->meta[q.slot];
-    if (q.step != BF_REDRIVE_ALL && q.step >= m.S) return fail(c, BF_EINVAL, at() + "step index out of range");  // "step %q not found", :541
-    if (m.S > L.steps_max || (child && m.child_nibbles > L.child_nibbles))
-      return fail(c, BF_ETOPO, at() + "topology does not fit the batch layout (steps_max / child_nibbles)");
-    key[i] = BF_REDRIVE_ALL;
-    if (q.step == BF_REDRIVE_ALL) continue;
-    const auto it = key_of.emplace((uint64_t)q.slot << 32 | q.step, (uint32_t)key_slot.size());
-    if (it.second) { key_slot.push_back(q.slot); key_step.push_back(q.step); }
-    key[i] = it.first->second;
-  }
-  if (applied_out) *applied_out = 0;
-  if (n == 0) return BF_OK;
-  BF_CUDA(c, cudaSetDevice(c->device));
-  if (int rc = sync_slots(c, c->stream)) return rc;
-  const size_t K = key_slot.size();
-  const size_t o_req = round_up_sz(n, 16), o_key = o_req + (size_t)n * sizeof(bf_redrive), o_ks = o_key + (size_t)n * 4,
-               o_mask = round_up_sz(o_ks + K * 8, 16), bytes = o_mask + K * L.words * 4;
-  if (int rc = ensure_dev(c, c->d_redrive, c->d_redrive_cap, bytes)) return rc;
-  std::vector<uint8_t> blob(o_mask - o_req);   // requests | keys | key slots | key steps (the statuses are written by the kernel)
-  memcpy(blob.data(), req, (size_t)n * sizeof(bf_redrive));
-  memcpy(blob.data() + (o_key - o_req), key.data(), (size_t)n * 4);
-  if (K) {
-    memcpy(blob.data() + (o_ks - o_req), key_slot.data(), K * 4);
-    memcpy(blob.data() + (o_ks - o_req) + K * 4, key_step.data(), K * 4);
-  }
-  if (c->last_state == r->d_state) c->last_eval_valid = false;   // as after an upload: bf_schedule must follow a new pass
-  uint8_t* d = c->d_redrive;
-  uint32_t* d_ks = reinterpret_cast<uint32_t*>(d + o_ks);
-  uint32_t* d_mask = reinterpret_cast<uint32_t*>(d + o_mask);
-  bf::RedriveParams P{};
-  P.state = r->d_state; P.mark = r->d_mark; P.mark_value = r->epoch << 1;   // touched, as by a delta
-  P.req = reinterpret_cast<const bf_redrive*>(d + o_req); P.key = reinterpret_cast<const uint32_t*>(d + o_key);
-  P.masks = d_mask; P.status = d; P.slots = c->slots_dev; P.n = n;
-  P.words = L.words; P.state_stride = L.state_stride; P.off_phase = L.off_phase; P.off_cond = L.off_cond;
-  P.off_decision = L.off_decision; P.off_child = L.off_child;
-  std::vector<uint8_t> status(n);
-  cudaStream_t s = c->stream;
-  cudaError_t e = cudaMemcpyAsync(d + o_req, blob.data(), blob.size(), cudaMemcpyHostToDevice, s);
-  if (e == cudaSuccess)
-    e = bf::launch_closure(c->slots_dev, d_ks, d_ks + K, (uint32_t)K, (uint32_t)c->slots_host.size(), L.words, d_mask, s);
-  if (e == cudaSuccess) e = bf::launch_redrive(P, s);
-  if (e == cudaSuccess) e = cudaMemcpyAsync(status.data(), d, n, cudaMemcpyDeviceToHost, s);
-  const cudaError_t es = cudaStreamSynchronize(s);
-  if (e == cudaSuccess) e = es;
-  if (e != cudaSuccess) {   // some records may have been reset: the next touched tick evaluates and lists every run
-    r->need_full = true; r->prev_valid = false;
-    return cuda_fail(c, e, "bf_resident_redrive");
-  }
-  c->stats.kernel_launches += K ? 2 : 1;
-  uint32_t applied = 0;
-  for (uint32_t i = 0; i < n; ++i) applied += status[i];
-  if (status_out) memcpy(status_out, status.data(), n);
-  if (applied_out) *applied_out = applied;
-  r->pending += applied;   // the touched-list bound counts the reset runs as it counts deltas
-  return BF_OK;
-}
-
-// A live batch grows its capacity and / or layout (resident.cu).  All checks come first, and the new buffers are allocated and
-// filled before the old ones are freed, so a rejected or failed call changes nothing.  One launch (both record arrays), one
-// device copy of the touch marks, one synchronisation.
-int bf_resident_reshape(bf_ctx* c, uint32_t h, const bf_layout* layout, uint32_t capacity) {
-  if (!c) return BF_EINVAL;
-  std::lock_guard<std::mutex> g(c->mu);
-  Resident* r = resident_of(c, h);
-  if (!r) return fail(c, BF_EINVAL, "unknown resident batch");
-  if (!layout) return fail(c, BF_EINVAL, "null layout");
-  if (int rc = check_layout(c, *layout)) return rc;
-  const bf_layout F = r->L, T = *layout;
-  if (capacity < r->cap) return fail(c, BF_EINVAL, "reshape cannot lower the capacity");
-  if (T.steps_max < F.steps_max) return fail(c, BF_EINVAL, "reshape cannot lower steps_max");
-  if (F.fields & ~T.fields) return fail(c, BF_EINVAL, "reshape cannot drop a field");
-  if (F.off_child != BF_OFF_NONE && T.child_nibbles < F.child_nibbles) return fail(c, BF_EINVAL, "reshape cannot shrink the child area");
-  // the kernel follows the offsets: every field the batch places must have a place in the new layout
-  const uint32_t from[] = {F.off_cond, F.off_decision, F.off_child, F.off_fail, F.off_needs_cond, F.off_skip_dep, F.off_phase_out};
-  const uint32_t to[] = {T.off_cond, T.off_decision, T.off_child, T.off_fail, T.off_needs_cond, T.off_skip_dep, T.off_phase_out};
-  // zero decision planes are PENDING, which a pass applies to RUNNING gate / sleep / wait steps (an absent plane leaves them
-  // alone), and added output masks may gain bits: either may change a result the touch marks know nothing of
-  bool results_may_change = false;
-  for (int i = 0; i < 7; ++i) {
-    if (from[i] != BF_OFF_NONE && to[i] == BF_OFF_NONE) return fail(c, BF_EINVAL, "the new layout drops a field the batch has");
-    if (i != 0 && i != 2 && from[i] == BF_OFF_NONE && to[i] != BF_OFF_NONE) results_may_change = true;
-  }
-  BF_CUDA(c, cudaSetDevice(c->device));
-  const size_t old_mark = ((size_t)r->cap + 3) / 4 * 16, new_mark = ((size_t)capacity + 3) / 4 * 16;   // as bf_resident_create
-  uint8_t *st = nullptr, *res = nullptr;
-  uint32_t* mk = nullptr;
-  cudaError_t e = cudaMalloc(&st, (size_t)capacity * T.state_stride);
-  if (e == cudaSuccess) e = cudaMalloc(&res, (size_t)capacity * T.result_stride);
-  if (e == cudaSuccess) e = cudaMalloc(&mk, new_mark);
-  if (e != cudaSuccess) {
-    cudaFree(st); cudaFree(res); cudaFree(mk);
-    cudaGetLastError();   // an allocation failure is not a launch failure of the next call
-    return fail(c, BF_ENOMEM, std::string("resident reshape: ") + cudaGetErrorString(e));
-  }
-  bf::ReshapeParams P{};
-  P.old_state = r->d_state; P.old_result = r->d_result; P.state = st; P.result = res;
-  P.n_old = r->cap; P.n_new = capacity; P.from = F; P.to = T;
-  cudaStream_t s = c->stream;
-  e = bf::launch_reshape(P, s);
-  if (e == cudaSuccess) e = cudaMemcpyAsync(mk, r->d_mark, old_mark, cudaMemcpyDeviceToDevice, s);   // with the list-build padding
-  if (e == cudaSuccess && new_mark > old_mark) e = cudaMemsetAsync(reinterpret_cast<uint8_t*>(mk) + old_mark, 0, new_mark - old_mark, s);
-  const cudaError_t es = cudaStreamSynchronize(s);
-  if (e == cudaSuccess) e = es;
-  if (e != cudaSuccess) {   // the old buffers were only read: the batch is as it was
-    cudaFree(st); cudaFree(res); cudaFree(mk);
-    return cuda_fail(c, e, "bf_resident_reshape");
-  }
-  if (c->last_state == r->d_state) c->last_eval_valid = false;   // as after an upload: bf_schedule must follow a new pass
-  cudaFree(r->d_state); cudaFree(r->d_result); cudaFree(r->d_result_prev); cudaFree(r->d_mark);
-  r->d_state = st; r->d_result = res; r->d_mark = mk;
-  r->d_result_prev = nullptr;   // never read before a pass overwrites it: allocated at the new size when next used
-  r->L = T; r->cap = capacity;
-  if (results_may_change) r->need_full = true;
-  return BF_OK;
-}
-
-// Runs leave a live batch (resident.cu): the last live runs move into the indices the retired ones free, so the batch's runs
-// stay [0, n_runs - n).  All checks and allocations come first, so a rejected call or a failed allocation changes nothing.
-// One H2D copy of the move table, one launch, one synchronisation; a new capacity adds the prefix copies into its buffers.
-int bf_resident_retire(bf_ctx* c, uint32_t h, bf_retire* rt) {
-  if (!c) return BF_EINVAL;
-  std::lock_guard<std::mutex> g(c->mu);
-  if (!rt || rt->struct_size != sizeof(bf_retire)) return fail(c, BF_EINVAL, "null bf_retire or bad struct_size");
-  Resident* r = resident_of(c, h);
-  if (!r) return fail(c, BF_EINVAL, "unknown resident batch");
-  const uint32_t N = rt->n_runs, n = rt->n;
-  if (N > r->cap) return fail(c, BF_EINVAL, "n_runs exceeds the resident batch");
-  if (n && !rt->runs) return fail(c, BF_EINVAL, "null runs");
-  std::vector<uint8_t> gone(N, 0);
-  for (uint32_t i = 0; i < n; ++i) {
-    const uint32_t q = rt->runs[i];
-    if (q >= N) return fail(c, BF_EINVAL, "runs[" + std::to_string(i) + "] is not below n_runs");
-    if (gone[q]) return fail(c, BF_EINVAL, "runs[" + std::to_string(i) + "] is retired twice");
-    gone[q] = 1;
-  }
-  const uint32_t m = N - n, cap = rt->capacity ? rt->capacity : r->cap;
-  if (cap < m || cap > r->cap) return fail(c, BF_EINVAL, "capacity must be 0 or within [n_runs - n, the current capacity]");
-  const bool resize = cap != r->cap;
-  if (n == 0 && !resize) { rt->n_moves = 0; return BF_OK; }
-  // the move rule: the k-th retired index below m (ascending) receives the k-th live index of [m, N); there are as many of each
-  std::vector<uint32_t> to(n, bf::kRetireNoMove);   // new index of run m + i
-  uint32_t n_moves = 0;
-  for (uint32_t i = 0, hole = 0; i < n; ++i) {
-    if (gone[m + i]) continue;
-    while (!gone[hole]) ++hole;
-    to[i] = hole++;
-    ++n_moves;
-  }
-  BF_CUDA(c, cudaSetDevice(c->device));
-  if (int rc = ensure_dev(c, c->d_retire, c->d_retire_cap, n ? n : 1)) return rc;
-  const bf_layout& L = r->L;
-  const size_t mark_bytes = ((size_t)cap + 3) / 4 * 16;   // as bf_resident_create
-  uint8_t *st = nullptr, *res = nullptr;
-  uint32_t* mk = nullptr;
-  if (resize) {
-    cudaError_t e = cudaMalloc(&st, (size_t)cap * L.state_stride);
-    if (e == cudaSuccess) e = cudaMalloc(&res, (size_t)cap * L.result_stride);
-    if (e == cudaSuccess) e = cudaMalloc(&mk, mark_bytes);
-    if (e != cudaSuccess) {
-      cudaFree(st); cudaFree(res); cudaFree(mk);
-      cudaGetLastError();   // an allocation failure is not a launch failure of the next call
-      return fail(c, BF_ENOMEM, std::string("resident retire: ") + cudaGetErrorString(e));
-    }
-  }
-  if (c->last_state == r->d_state) c->last_eval_valid = false;   // as after an upload: bf_schedule must follow a new pass
-  bf::RetireParams P{};
-  P.state = r->d_state; P.result = r->d_result; P.mark = r->d_mark; P.mark_value = r->epoch << 1 | 1u;   // touched, must list
-  P.to = c->d_retire; P.m = m; P.n = n; P.state_stride = L.state_stride; P.result_stride = L.result_stride;
-  cudaStream_t s = c->stream;
-  cudaError_t e = n ? cudaMemcpyAsync(c->d_retire, to.data(), (size_t)n * 4, cudaMemcpyHostToDevice, s) : cudaSuccess;
-  if (e == cudaSuccess) e = bf::launch_retire(P, s);
-  if (resize) {   // in place first, then the prefix into the new buffers (the mark padding past cap is never read)
-    if (e == cudaSuccess) e = cudaMemcpyAsync(st, r->d_state, (size_t)cap * L.state_stride, cudaMemcpyDeviceToDevice, s);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(res, r->d_result, (size_t)cap * L.result_stride, cudaMemcpyDeviceToDevice, s);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(mk, r->d_mark, mark_bytes, cudaMemcpyDeviceToDevice, s);
-  }
-  const cudaError_t es = cudaStreamSynchronize(s);
-  if (e == cudaSuccess) e = es;
-  if (e != cudaSuccess) {   // some records may have moved: the next touched tick evaluates and lists every run
-    cudaFree(st); cudaFree(res); cudaFree(mk);
-    r->need_full = true; r->prev_valid = false;
-    return cuda_fail(c, e, "bf_resident_retire");
-  }
-  c->stats.kernel_launches += n ? 1 : 0;
-  if (resize) {
-    cudaFree(r->d_state); cudaFree(r->d_result); cudaFree(r->d_result_prev); cudaFree(r->d_mark);
-    r->d_state = st; r->d_result = res; r->d_mark = mk;
-    r->d_result_prev = nullptr;   // never read before a pass overwrites it: allocated at the new size when next used
-    r->cap = cap;
-  }
-  // touched-tick bookkeeping: the batch's runs are [0, m) now, and the moved runs are as good as uploaded at their new index
-  r->full_runs = std::min(r->full_runs, m);
-  for (auto it = r->uploaded.begin(); it != r->uploaded.end();) {
-    if (it->first >= m) { it = r->uploaded.erase(it); continue; }
-    it->second = std::min(it->second, m);
-    ++it;
-  }
-  for (uint32_t i = 0; i < n; ++i)
-    if (to[i] != bf::kRetireNoMove) note_uploaded(r, to[i], to[i] + 1);
-  r->pending += n_moves;
-  // the current result records moved with their runs: a changed-only tick over [0, m) compares each run with its own record
-  if (r->prev_valid && r->prev_runs == N) r->prev_runs = m;
-  else r->prev_valid = false;
-  if (n_moves && (rt->moves_from || rt->moves_to)) {
-    for (uint32_t i = 0, k = 0; i < n; ++i) {
-      if (to[i] == bf::kRetireNoMove) continue;
-      if (rt->moves_from) rt->moves_from[k] = m + i;
-      if (rt->moves_to) rt->moves_to[k] = to[i];
-      ++k;
-    }
-  }
-  rt->n_runs = m; rt->n_moves = n_moves;
-  return BF_OK;
-}
-
 int bf_alloc_pinned(bf_ctx* c, size_t bytes, void** out) {
   if (!c || !out) return BF_EINVAL;
   std::lock_guard<std::mutex> g(c->mu);
@@ -2160,7 +1223,7 @@ int bf_get_stats(const bf_ctx* c, bf_stats* out) {
   *out = c->stats;
   out->arena_used_bytes = c->arena_used;
   out->arena_compactions = (uint32_t)c->arena_compactions;
-  out->arena_cap_bytes = c->arena_cap;
+  out->arena_cap_bytes = c->arena.cap;
   out->n_topologies = c->n_alive;
   out->sm_count = (uint32_t)c->sm_count;
   return BF_OK;

@@ -1,0 +1,331 @@
+// ctx.h — what the C ABI's translation units share (abi.cu: context, topology arena, batch evaluation; resident_abi.cu:
+// resident batches): bf_ctx and the records it keeps, the device-buffer owner, the error helpers, the kernel launchers and
+// the host helpers of a pass.  Private to the library: include/bobrafrontier.h is the public surface.
+#pragma once
+
+#include <cuda_runtime.h>
+#include <stdint.h>
+
+#include <algorithm>
+#include <map>
+#include <mutex>
+#include <string>
+#include <utility>
+#include <vector>
+
+#include "../../include/bobrafrontier.h"
+#include "device_record.h"
+
+namespace bf {
+cudaError_t launch_frontier(const KParams& P, uint32_t grid, uint32_t smem_bytes, cudaStream_t stream);
+cudaError_t launch_expansion(const KParams& P, unsigned long long* block_sums, unsigned long long* offsets,
+                             bf_expansion* out, unsigned long long cap, cudaStream_t stream, uint32_t* launches);
+int frontier_max_blocks_per_sm(const KParams& P, uint32_t threads, uint32_t smem_bytes, uint32_t* occ2);
+cudaError_t launch_frontier_pack(const KParams& P, uint32_t grid, uint32_t smem_bytes, cudaStream_t stream);
+uint32_t frontier_pack_max_warps();
+cudaError_t launch_apply_deltas(const DeltaParams& P, cudaStream_t stream);
+cudaError_t launch_compact(const CompactParams& P, cudaStream_t stream);
+cudaError_t launch_touched_list(const TouchedParams& P, cudaStream_t stream);
+cudaError_t launch_touched_compact(const TouchedParams& P, cudaStream_t stream);
+cudaError_t launch_mark_runs(uint32_t* mark, uint32_t first, uint32_t n, uint32_t value, cudaStream_t stream);
+cudaError_t launch_move_records(const uint8_t* src, uint8_t* dst, const void* moves, uint32_t n, cudaStream_t stream);
+cudaError_t launch_migrate(const MigrateParams& P, cudaStream_t stream);
+cudaError_t launch_redrive(const RedriveParams& P, cudaStream_t stream);
+cudaError_t launch_reshape(const ReshapeParams& P, cudaStream_t stream);
+cudaError_t launch_retire(const RetireParams& P, cudaStream_t stream);
+cudaError_t launch_schedule(const SchedParams& P, uint32_t sm_count, cudaStream_t stream, uint32_t phases = 3);
+cudaError_t launch_closure(const Slot* slots, const uint32_t* slot_ids, const uint32_t* starts, uint32_t n, uint32_t n_slots,
+                           uint32_t words_out, uint32_t* masks, cudaStream_t stream);
+cudaError_t launch_validate(const Slot* slots, const uint32_t* slot_ids, uint32_t n, uint32_t n_slots, uint32_t* status,
+                            cudaStream_t stream);
+
+inline uint32_t round_up(uint32_t v, uint32_t a) { return (v + a - 1) / a * a; }
+inline size_t round_up_sz(size_t v, size_t a) { return (v + a - 1) / a * a; }
+inline int fail(bf_ctx* c, int code, const std::string& msg);
+}  // namespace bf
+
+// The owner of one device allocation: a pointer and a capacity in elements, freed by the destructor.  It converts to its
+// pointer, so kernel parameters and address arithmetic read it as a plain T*.
+template <typename T>
+struct DevBuf {
+  T* p = nullptr;
+  size_t cap = 0;
+
+  DevBuf() = default;
+  DevBuf(DevBuf&& o) noexcept : p(std::exchange(o.p, nullptr)), cap(std::exchange(o.cap, 0)) {}
+  DevBuf& operator=(DevBuf&& o) noexcept {
+    if (this != &o) { reset(); p = std::exchange(o.p, nullptr); cap = std::exchange(o.cap, 0); }
+    return *this;
+  }
+  ~DevBuf() { reset(); }
+
+  operator T*() const { return p; }
+  void reset() { if (p) cudaFree(p); p = nullptr; cap = 0; }
+  // Exactly n elements, which replace the old ones once they exist (no old contents kept).  A failed allocation changes
+  // nothing and clears the error it left behind: an allocation failure is not a launch failure of the next call.
+  cudaError_t alloc(size_t n) {
+    T* np = nullptr;
+    const cudaError_t e = cudaMalloc(&np, n * sizeof(T));
+    if (e != cudaSuccess) { cudaGetLastError(); return e; }
+    reset();
+    p = np; cap = n;
+    return e;
+  }
+  // At least n elements: doubles from the current capacity (or 1).  BF_ENOMEM on failure.
+  int ensure(bf_ctx* c, size_t n) {
+    if (n <= cap) return BF_OK;
+    size_t ncap = cap ? cap : 1;
+    while (ncap < n) ncap *= 2;
+    const cudaError_t e = alloc(ncap);
+    return e == cudaSuccess ? BF_OK : bf::fail(c, BF_ENOMEM, std::string("cudaMalloc: ") + cudaGetErrorString(e));
+  }
+};
+
+struct Resident;
+
+struct TopoMeta {
+  bool alive = false;
+  uint32_t S = 0, E = 0, P = 0, bytes = 0;
+  size_t offset = 0;  // in arena
+  std::vector<uint32_t> child_first;
+  std::vector<uint16_t> par_step, par_branches;   // step and branch count of each parallel desc (bf_resident_migrate)
+  uint32_t child_nibbles = 0;
+  bool fits(const bf_layout& L) const { return S <= L.steps_max && (L.off_child == BF_OFF_NONE || child_nibbles <= L.child_nibbles); }
+};
+
+struct bf_ctx {
+  int device = 0;
+  int sm_count = 0;                    // SMs the frontier kernels spread over (device SMs minus the reserved ones)
+  cudaStream_t stream = nullptr;
+  // bf_eval pipeline: H2D copies, kernels and D2H copies of consecutive run chunks overlap on three streams
+  static constexpr uint32_t kMaxChunks = 32;
+  cudaStream_t s_in = nullptr, s_out = nullptr;
+  cudaEvent_t ev_in[kMaxChunks] = {}, ev_k[kMaxChunks] = {};
+  bool pipe_ready = false;
+  std::mutex mu;
+  std::string err;
+
+  DevBuf<uint8_t> arena;               // capacity: arena.cap bytes
+  size_t arena_used = 0;
+  size_t arena_dead = 0;               // bytes of dropped records below arena_used (reclaimed by compact_arena)
+  uint64_t arena_compactions = 0;
+  std::vector<TopoMeta> meta;
+  std::vector<uint32_t> free_slots;
+  std::vector<bf::Slot> slots_host;
+  DevBuf<bf::Slot> slots_dev;
+  bool slots_dirty = true;
+  std::vector<uint32_t> ff_host;       // fail-fast masks, bf::FF_STRIDE words per slot (device_record.h), mirrored with the slots
+  DevBuf<uint32_t> ff_dev;             // capacity: slots_dev.cap rows
+  uint32_t max_rec_bytes = 0;          // largest live record
+  uint32_t max_rec_by_w[33] = {};      // ... among the topologies of W = ceil(S/32) words (a batch of layout.words = w stages only W <= w)
+  bool rec_max_dirty = false;          // a drop may have lowered the maxima: recomputed at the next plan
+  uint32_t n_alive = 0;
+  uint32_t n_with_parallel = 0;  // live topologies that have parallel steps
+  uint64_t slot_changes = 0;     // slot drops and reuses so far: either changes what the runs holding the slot evaluate
+                                 // to, so a touched tick after one evaluates every run
+
+  // host-API staging
+  DevBuf<uint8_t> d_state, d_result;
+  DevBuf<unsigned long long> d_counts;
+  // BF_EVAL_COUNTS_SET scratch of the packed-lanes kernel (device_record.h): a ring of kAccSlots blocks of 8 u64, one per launch
+  // in turn (launches of different streams may overlap; a block is left zeroed by the launch that used it)
+  static constexpr uint32_t kAccSlots = 256;
+  DevBuf<unsigned long long> d_acc;
+  uint32_t acc_seq = 0;
+  bf_counts* h_counts = nullptr;  // pinned landing zone for the counts block (a pageable target would make the copy synchronous)
+  DevBuf<bf_expansion> d_exp;
+  // compact results (bf_eval_compact / bf_resident_tick_compact)
+  DevBuf<uint32_t> d_head;
+  DevBuf<uint16_t> d_events;
+  // [0] = events, [1] = listed runs, then TWO buffers of per-512-run event totals used in turn: a tick's emit kernel leaves the
+  // other one zeroed, so a pass that adds its runs' counts itself (fused heads, device_record.h) finds a clean buffer
+  DevBuf<unsigned long long> d_cblock;
+  uint32_t cblock_flip = 0;
+  // set by a compact tick around its run_pass: where a packed-lanes pass may leave head words and block totals; run_pass reports
+  // through fused_done whether it did
+  uint32_t* fuse_head = nullptr; unsigned long long* fuse_sums = nullptr; bool fused_done = false;
+  uint64_t last_events = 0;                                          // events of the previous compact pass (sizes the first D2H)
+  // scratch shared by both entry points
+  DevBuf<uint32_t> d_exp_counts;
+  DevBuf<unsigned long long> d_offsets, d_block_sums;
+  DevBuf<uint32_t> d_defer;  // [0] = count, [1..] = run ids
+  // touched ticks: [0] = list length, [1..] = the list | head word per list position | listed runs and their heads (when the
+  // caller's buffers are not pinned) | per-block sums
+  DevBuf<uint32_t> d_tlist, d_tpos_head, d_truns, d_thead;
+  DevBuf<unsigned long long> d_tsums;
+  uint64_t last_touched_events = 0;   // events of the previous touched tick (sizes the first D2H)
+  // migrations (bf_resident_migrate): [0, 16) the migrated-run counter | inverse step map | desc table
+  DevBuf<uint8_t> d_mig;
+  // redrives (bf_resident_redrive): statuses | requests | key per request | key slots | key steps | closure masks
+  DevBuf<uint8_t> d_redrive;
+  // retirements (bf_resident_retire): the new index of each vacated run
+  DevBuf<uint32_t> d_retire;
+
+  // limiters (bf_schedule): what the last bf_eval left on the device + scratch
+  bool last_eval_valid = false;
+  uint32_t last_eval_runs = 0;
+  bf_layout last_eval_layout{};
+  DevBuf<uint8_t> d_sched;                              // runs | records | tables, one allocation
+  const uint8_t* last_state = nullptr;                  // device records of the last evaluated batch (bf_eval or resident)
+  const uint8_t* last_result = nullptr;
+  // resident batches (row f2)
+  std::vector<Resident> resident;
+  DevBuf<bf_delta> d_deltas;
+  DevBuf<uint32_t> d_rejected;
+  // small device scratch that its consumers leave zeroed (the compaction's tail block reads and clears the rejected-delta
+  // counter and the listed-runs total), so the steady-state tick carries no memset launches; a failed call marks it dirty
+  bool rejected_clean = false, cblock_clean = false;
+
+  // cached shared-memory plans of the general kernel (recomputed when the layout, the largest record or a launch-shape knob
+  // changes): [0] for passes over whole batches, [1] for passes over a run list (touched ticks), so that a batch that mixes
+  // full and touched ticks keeps both
+  struct Plan {
+    uint32_t key_stride = 0, key_words = 0, key_rec = 0, key_variant = 0xFFFFFFFFu;
+    int key_knobs[3] = {0, 0, 0};   // BF_STAGES, BF_WARPS, BF_BLOCKS_PER_SM as last planned (0: unset)
+    uint32_t stages = 0, wpb = 0, per_sm = 0, occ2 = 0;
+  } plan[2];
+
+  bf_stats stats{};
+};
+
+namespace bf {
+inline int fail(bf_ctx* c, int code, const std::string& msg) {
+  if (c) c->err = msg;
+  return code;
+}
+inline int cuda_fail(bf_ctx* c, cudaError_t e, const char* what) {
+  return fail(c, BF_ECUDA, std::string(what) + ": " + cudaGetErrorString(e));
+}
+}  // namespace bf
+#define BF_CUDA(c, call)                                       \
+  do {                                                         \
+    cudaError_t e__ = (call);                                  \
+    if (e__ != cudaSuccess) return bf::cuda_fail(c, e__, #call); \
+  } while (0)
+
+// A device-resident batch (row f2), with the bookkeeping of touched ticks that tests/resident_model.py restates under the
+// same names.  Each field and the calls that change it:
+//   L, cap, d_state,   create, and reshape / retire (adopt).  d_state also: upload, deltas, migrate, redrive, retire.
+//   d_result           full ticks write it; a touched tick's list-mode compaction updates the runs it evaluated; reshape re-lays
+//                      it out; retire moves records with their runs.
+//   d_result_prev      result_prev allocates it on first use, adopt drops it; a changed-only tick swaps it with d_result and a
+//                      touched tick passes into it, so it is never read before a pass writes it.
+//   prev_valid, _runs  d_result holds a pass over the current state lineage of prev_runs runs: full_tick_done sets it; an upload
+//                      and records_unknown clear it; compact_to follows the run count.
+//   d_mark, epoch,     deltas and redrives raise a run's mark to mark_touched() (epoch << 1); uploads, migrations and retires to
+//   full_epoch         mark_must_list() (| 1: listed even if unchanged).  full_tick_done records the ending epoch in full_epoch
+//                      and opens the next, so older marks are stale by comparison alone (no clear, no launch), and zeroes the
+//                      marks on epoch wrap.  A touched tick evaluates the runs marked after full_epoch and zeroes their marks.
+//   full_runs          runs of the last full tick (full_tick_done); compact_to clamps it.
+//   need_full          the current records are not known to be complete: no tick yet, a failed call (records_unknown, a failed
+//                      touched tick), or a reshape that added decision planes or output fields.  full_tick_done clears it.
+//   last_fixpoint, last_max_iter, slot_changes_seen: BF_EVAL_FIXPOINT, max_iterations and bf_ctx::slot_changes at the last
+//                      full tick.  A touched tick with other parameters, or after a slot drop or reuse, is full (full_due).
+//   pending            bound on the touched runs: those the last touched tick left at or above its n_runs, plus the deltas,
+//                      uploaded, migrated, redriven and moved runs since.  full_tick_done zeroes it.
+//   uploaded           merged [first, end) ranges, keyed by first, of the runs at or above full_runs uploaded since the last full
+//                      tick (note_uploaded); compact_to clips them; full_tick_done clears them.
+// A call that changes d_state ends the evaluated snapshot (end_snapshot): bf_schedule must follow a new pass.
+struct Resident {
+  bool alive = false, prev_valid = false, need_full = true;
+  bf_layout L{};
+  uint32_t cap = 0, prev_runs = 0, epoch = 1, full_epoch = 0, full_runs = 0, last_fixpoint = 0, last_max_iter = 0;
+  DevBuf<uint8_t> d_state, d_result, d_result_prev;
+  DevBuf<uint32_t> d_mark;
+  uint64_t slot_changes_seen = 0, pending = 0;
+  std::map<uint32_t, uint32_t> uploaded;
+
+  uint32_t mark_touched() const { return epoch << 1; }
+  uint32_t mark_must_list() const { return epoch << 1 | 1u; }
+  void end_snapshot(bf_ctx* c) const { if (c->last_state == d_state) c->last_eval_valid = false; }
+  // the runs [first, end) were uploaded: the part at or above full_runs, merged with the ranges it touches
+  void note_uploaded(uint32_t first, uint32_t end) {
+    uint32_t lo = std::max(first, full_runs), hi = end;
+    if (lo >= hi) return;
+    auto it = uploaded.upper_bound(lo);
+    if (it != uploaded.begin() && std::prev(it)->second >= lo) {
+      --it;
+      lo = it->first; hi = std::max(hi, it->second);
+      it = uploaded.erase(it);
+    }
+    while (it != uploaded.end() && it->first <= hi) { hi = std::max(hi, it->second); it = uploaded.erase(it); }
+    uploaded.emplace(lo, hi);
+  }
+  // Were all runs of [lo, hi) uploaded since the last full tick?  (The ranges are merged: one of them must hold all of it.)
+  bool uploads_cover(uint32_t lo, uint32_t hi) const {
+    auto it = uploaded.upper_bound(lo);
+    if (it == uploaded.begin()) return false;
+    --it;
+    return it->first <= lo && it->second >= hi;
+  }
+  // must a touched tick over n_runs with these parameters be full?  Also just before the epoch wraps (full_tick_done)
+  bool full_due(const bf_ctx* c, uint32_t n_runs, uint32_t flags, uint32_t max_iter) const {
+    return need_full || c->slot_changes != slot_changes_seen || (flags & BF_EVAL_FIXPOINT) != last_fixpoint ||
+           max_iter != last_max_iter || epoch >= 0x7FFFFFFEu || (n_runs > full_runs && !uploads_cover(full_runs, n_runs));
+  }
+  int full_tick_done(bf_ctx* c, uint32_t n_runs, uint32_t flags, uint32_t max_iter, cudaStream_t s) {
+    prev_valid = true; prev_runs = n_runs; need_full = false;
+    full_epoch = epoch++; full_runs = n_runs;
+    last_fixpoint = flags & BF_EVAL_FIXPOINT; last_max_iter = max_iter; slot_changes_seen = c->slot_changes;
+    pending = 0; uploaded.clear();
+    if (epoch >= 0x7FFFFFFFu) {   // the epoch must fit mark >> 1: once per 2^31 full ticks the marks start over
+      BF_CUDA(c, cudaMemsetAsync(d_mark, 0, d_mark.cap * sizeof(uint32_t), s));
+      epoch = 1; full_epoch = 0;
+    }
+    return BF_OK;
+  }
+  void records_unknown() { need_full = true; prev_valid = false; }
+  // the synchronise that ends a call rewriting records in place (migrate, redrive, retire): after a failure some records may
+  // have changed, so the next touched tick evaluates and lists every run
+  int sync_in_place(bf_ctx* c, cudaError_t e, const char* what) {
+    const cudaError_t es = cudaStreamSynchronize(c->stream);
+    if (e == cudaSuccess) e = es;
+    if (e == cudaSuccess) return BF_OK;
+    records_unknown();
+    return bf::cuda_fail(c, e, what);
+  }
+  int result_prev(bf_ctx* c) {
+    const cudaError_t e = d_result_prev ? cudaSuccess : d_result_prev.alloc((size_t)cap * L.result_stride);
+    return e == cudaSuccess ? BF_OK : bf::fail(c, BF_ENOMEM, std::string("resident batch (second result buffer): ") + cudaGetErrorString(e));
+  }
+  // the state, result and touch-mark buffers of a new batch (create), or of new ones a batch adopts (reshape, retire): a call
+  // that fails first frees them with its locals
+  cudaError_t alloc(const bf_layout& layout, uint32_t capacity) {
+    cudaError_t e = d_state.alloc((size_t)capacity * layout.state_stride);
+    if (e == cudaSuccess) e = d_result.alloc((size_t)capacity * layout.result_stride);
+    return e == cudaSuccess ? d_mark.alloc(((size_t)capacity + 3) / 4 * 4) : e;   // padded: the list build reads four marks at a time
+  }
+  // new buffers at a new layout and capacity; the second result buffer is allocated at the new size when next used
+  void adopt(Resident&& b, const bf_layout& layout, uint32_t capacity) {
+    d_state = std::move(b.d_state); d_result = std::move(b.d_result); d_result_prev.reset(); d_mark = std::move(b.d_mark);
+    L = layout; cap = capacity;
+  }
+  // retire left the runs [0, m) of [0, N); moves[i] is the new index of run m + i, or kRetireNoMove.  A moved run counts as
+  // uploaded at its new index, and its result record moved with it (a changed-only tick compares it with its own record).
+  void compact_to(uint32_t m, uint32_t N, const std::vector<uint32_t>& moves) {
+    full_runs = std::min(full_runs, m);
+    uploaded.erase(uploaded.lower_bound(m), uploaded.end());
+    for (auto& u : uploaded) u.second = std::min(u.second, m);
+    for (uint32_t to : moves)
+      if (to != bf::kRetireNoMove) { note_uploaded(to, to + 1); ++pending; }
+    if (prev_valid && prev_runs == N) prev_runs = m;
+    else prev_valid = false;
+  }
+};
+
+// host helpers of a pass, defined in abi.cu and used by resident_abi.cu too
+namespace bf {
+int ensure_pipe(bf_ctx* c);
+int sync_slots(bf_ctx* c, cudaStream_t stream);
+int check_layout(bf_ctx* c, const bf_layout& L);
+int run_pass(bf_ctx* c, const bf_batch& b, const uint8_t* d_state, uint8_t* d_result, bf_expansion* d_exp,
+             unsigned long long* d_counts, cudaStream_t stream, const uint32_t* run_list = nullptr,
+             const uint32_t* run_list_count = nullptr);
+void* pinned_dev(const void* p);
+uint32_t result_tail_of(const bf_layout& L);
+int compact_prepare(bf_ctx* c, uint32_t n_runs, cudaStream_t s);
+unsigned long long* cblock_sums(bf_ctx* c, uint32_t which);
+int compact_enqueue(bf_ctx* c, const bf_layout& L, const uint8_t* d_result, const uint8_t* d_prev, uint32_t n_runs, bf_compact_out* out,
+                    cudaStream_t s, uint64_t* first_slice, bool with_rejected, bool heads_done = false);
+int compact_finish(bf_ctx* c, bf_compact_out* out, uint64_t first_slice);
+}  // namespace bf

@@ -168,7 +168,7 @@ struct CompactParams {
   uint32_t n_runs, words, result_stride, result_tail, off_ready, off_skip, off_fail, off_needs_cond, off_skip_dep;
 };
 
-// compact.cu, touched ticks (bf_resident_tick_touched, abi.cu): the list build in front of the pass and the list-mode compaction
+// compact.cu, touched ticks (bf_resident_tick_touched, resident_abi.cu): the list build in front of the pass and the list-mode compaction
 // behind it.  Every scratch array is written before it is read in the same tick (no self-cleaning needed).
 struct TouchedParams {
   CompactParams C;               // result = the pass's new records (the batch's second buffer), prev_result = the batch's current
@@ -198,7 +198,7 @@ struct DeltaParams {
   uint32_t n, n_runs;
   uint32_t words, state_stride, off_phase, off_cond, off_decision, off_child, child_nibbles;
   uint32_t* rejected;  // count of deltas outside the record (bad run / index / absent field)
-  uint32_t* mark;      // [n_runs] touch marks (abi.cu, touched ticks): every delta of a run in range raises its mark to mark_value
+  uint32_t* mark;      // [n_runs] touch marks (Resident in ctx.h, touched ticks): every delta of a run in range raises its mark to mark_value
   uint32_t mark_value;
 };
 

@@ -175,7 +175,7 @@ DI void walk_items_any(uint32_t lane, uint32_t CAND, uint32_t lg, const WalkCtx&
 }
 
 // CD: cond and/or decision codes present   XO: any of fail/needs_cond/skip_dep/phase_out requested
-// LIST: run-list mode (touched ticks, abi.cu): group t takes the runs at list positions [t * R, t * R + R) of P.run_list, whose
+// LIST: run-list mode (touched ticks, resident_abi.cu): group t takes the runs at list positions [t * R, t * R + R) of P.run_list, whose
 //       length the list build left at *P.run_list_count (P.n_runs is the host's bound on it).  The runs' state records are not
 //       adjacent, so the lane that owns a run copies its record itself; results go to each run's own index, and no fused head
 //       words are written.

@@ -129,6 +129,42 @@ inline int get_code(const uint8_t* base, uint32_t W, int nbits, uint32_t i) {
   return v;
 }
 
+// (run, field, index) of a pending delta: the key of bfh_batch::delta_at
+inline uint64_t delta_key(uint32_t run, uint32_t field, uint32_t index) { return ((uint64_t)run << 32) | ((uint64_t)field << 16) | index; }
+
+// A batch's state and result arrays, zeroed: pinned when a ctx is given and can pin them, else plain host memory.  The
+// destructor frees them; reshape and retire allocate the new arrays first and swap them in once nothing can fail.
+struct HostRecords {
+  bf_ctx* ctx = nullptr;
+  uint8_t* state = nullptr;
+  uint8_t* result = nullptr;
+  bool pinned = false;
+
+  HostRecords() = default;
+  HostRecords(const HostRecords&) = delete;
+  HostRecords& operator=(const HostRecords&) = delete;
+  ~HostRecords() {
+    if (pinned) { bf_free_pinned(ctx, state); bf_free_pinned(ctx, result); }
+    else { free(state); free(result); }
+  }
+  bool alloc(bf_ctx* c, size_t sb, size_t rb) {
+    void *ps = nullptr, *pr = nullptr;
+    const bool pin = c && bf_alloc_pinned(c, sb, &ps) == BF_OK && bf_alloc_pinned(c, rb, &pr) == BF_OK;
+    if (!pin) {
+      if (c && ps) bf_free_pinned(c, ps);
+      ps = malloc(sb); pr = malloc(rb);
+      if (!ps || !pr) { free(ps); free(pr); return false; }
+    }
+    ctx = c; pinned = pin;
+    state = static_cast<uint8_t*>(ps); result = static_cast<uint8_t*>(pr);
+    memset(ps, 0, sb); memset(pr, 0, rb);
+    return true;
+  }
+  void swap(HostRecords& o) {
+    std::swap(ctx, o.ctx); std::swap(state, o.state); std::swap(result, o.result); std::swap(pinned, o.pinned);
+  }
+};
+
 }  // namespace
 
 struct bfh_story {
@@ -154,9 +190,7 @@ struct bfh_batch {
   bf_ctx* ctx = nullptr;
   bf_layout L{};
   uint32_t cap = 0, n = 0;
-  uint8_t* state = nullptr;
-  uint8_t* result = nullptr;
-  bool pinned = false;
+  HostRecords rec;
   std::vector<const bfh_story*> story_of_run;
   std::string err;
   // resident mode (row f2): the device holds the records, setters log coalesced deltas, eval sends only those
@@ -169,7 +203,7 @@ struct bfh_batch {
 
   void log_delta(uint32_t run, uint32_t field, uint32_t index, uint32_t code) {
     if (!resident || run >= uploaded) return;        // a run not yet on the device travels as a full record
-    const uint64_t key = ((uint64_t)run << 32) | ((uint64_t)field << 16) | index;
+    const uint64_t key = delta_key(run, field, index);
     auto it = delta_at.find(key);
     if (it != delta_at.end()) { deltas[it->second].code = (uint8_t)code; return; }   // the last value of a tick wins
     delta_at[key] = (uint32_t)deltas.size();
@@ -178,6 +212,28 @@ struct bfh_batch {
     deltas.push_back(d);
   }
 };
+
+// Rewrite the pending deltas in order: fn edits a delta in place and returns whether it stays.  delta_at follows.
+template <typename Fn>
+static void rewrite_deltas(bfh_batch* b, Fn fn) {
+  if (b->deltas.empty()) return;
+  size_t keep = 0;
+  for (size_t k = 0; k < b->deltas.size(); ++k) {
+    bf_delta d = b->deltas[k];
+    if (fn(d)) b->deltas[keep++] = d;
+  }
+  b->deltas.resize(keep);
+  b->delta_at.clear();
+  for (size_t i = 0; i < keep; ++i) b->delta_at[delta_key(b->deltas[i].run, b->deltas[i].field, b->deltas[i].index)] = (uint32_t)i;
+}
+
+// Resident mode: the runs not yet on the device go up as full records
+static int flush_uploads(bfh_batch* b) {
+  if (b->uploaded >= b->n) return BF_OK;
+  const int rc = bf_resident_upload(b->ctx, b->handle, b->uploaded, b->n - b->uploaded, b->rec.state + (size_t)b->uploaded * b->L.state_stride);
+  if (rc == BF_OK) { b->full_bytes_sent += (uint64_t)(b->n - b->uploaded) * b->L.state_stride; b->uploaded = b->n; }
+  return rc;
+}
 
 extern "C" {
 
@@ -359,31 +415,13 @@ int bfh_scan_step_refs(const char* expression, char* out, size_t cap) {
 }
 
 // ------------------------------------------------------------------------------------------ Batch
-// Zeroed state and result arrays of a batch: pinned when a ctx is given and can pin them, else plain host memory.
-static bool alloc_records(bf_ctx* ctx, size_t sb, size_t rb, uint8_t** state, uint8_t** result, bool* pinned) {
-  void *ps = nullptr, *pr = nullptr;
-  *pinned = ctx && bf_alloc_pinned(ctx, sb, &ps) == BF_OK && bf_alloc_pinned(ctx, rb, &pr) == BF_OK;
-  if (!*pinned) {
-    if (ctx && ps) bf_free_pinned(ctx, ps);
-    ps = malloc(sb); pr = malloc(rb);
-    if (!ps || !pr) { free(ps); free(pr); return false; }
-  }
-  *state = static_cast<uint8_t*>(ps); *result = static_cast<uint8_t*>(pr);
-  memset(ps, 0, sb); memset(pr, 0, rb);
-  return true;
-}
-static void free_records(bfh_batch* b) {
-  if (b->pinned) { bf_free_pinned(b->ctx, b->state); bf_free_pinned(b->ctx, b->result); }
-  else { free(b->state); free(b->result); }
-}
-
 bfh_batch* bfh_batch_new(bf_ctx* ctx, uint32_t steps_max, uint32_t child_nibbles, uint32_t fields, uint32_t capacity) {
   bfh_batch* b = new (std::nothrow) bfh_batch();
   if (!b) return nullptr;
   b->ctx = ctx;
   if (bf_layout_init(&b->L, steps_max, child_nibbles, fields) != BF_OK || capacity == 0) { delete b; return nullptr; }
   b->cap = capacity;
-  if (!alloc_records(ctx, (size_t)capacity * b->L.state_stride, (size_t)capacity * b->L.result_stride, &b->state, &b->result, &b->pinned)) {
+  if (!b->rec.alloc(ctx, (size_t)capacity * b->L.state_stride, (size_t)capacity * b->L.result_stride)) {
     delete b;
     return nullptr;
   }
@@ -392,21 +430,20 @@ bfh_batch* bfh_batch_new(bf_ctx* ctx, uint32_t steps_max, uint32_t child_nibbles
 void bfh_batch_free(bfh_batch* b) {
   if (!b) return;
   if (b->resident) bf_resident_destroy(b->ctx, b->handle);
-  free_records(b);
   delete b;
 }
 const char* bfh_batch_error(const bfh_batch* b) { return b ? b->err.c_str() : "null batch"; }
 const bf_layout* bfh_batch_layout(const bfh_batch* b) { return b ? &b->L : nullptr; }
 uint32_t bfh_batch_size(const bfh_batch* b) { return b ? b->n : 0; }
-const void* bfh_batch_state(const bfh_batch* b) { return b ? b->state : nullptr; }
-const void* bfh_batch_result(const bfh_batch* b) { return b ? b->result : nullptr; }
+const void* bfh_batch_state(const bfh_batch* b) { return b ? b->rec.state : nullptr; }
+const void* bfh_batch_result(const bfh_batch* b) { return b ? b->rec.result : nullptr; }
 
 int bfh_batch_add_run(bfh_batch* b, const bfh_story* story, uint32_t slot) {
   if (!b || !story || !story->finalized) return BF_EINVAL;
   if (b->n >= b->cap) { b->err = "batch full"; return BF_ENOMEM; }
   if (story->flags.size() > b->L.steps_max) { b->err = "story larger than the batch layout"; return BF_EINVAL; }
   if (b->L.off_child != BF_OFF_NONE && story->child_nibbles > b->L.child_nibbles) { b->err = "child area too small"; return BF_EINVAL; }
-  uint8_t* rec = b->state + (size_t)b->n * b->L.state_stride;
+  uint8_t* rec = b->rec.state + (size_t)b->n * b->L.state_stride;
   memset(rec, 0, b->L.state_stride);
   bf_run_header* h = reinterpret_cast<bf_run_header*>(rec);
   h->topo_slot = slot;
@@ -420,20 +457,7 @@ int bfh_batch_remove_last_run(bfh_batch* b) {
   --b->n;
   if (b->uploaded > b->n) b->uploaded = b->n;  // the slot's next occupant is uploaded as a full record
   // pending deltas of the removed run must not land on the slot's next occupant (whose full record is uploaded first)
-  if (b->resident && !b->deltas.empty()) {
-    const uint32_t gone = b->n;
-    size_t keep = 0;
-    for (size_t i = 0; i < b->deltas.size(); ++i)
-      if (b->deltas[i].run != gone) b->deltas[keep++] = b->deltas[i];
-    if (keep != b->deltas.size()) {
-      b->deltas.resize(keep);
-      b->delta_at.clear();
-      for (size_t i = 0; i < keep; ++i) {
-        const bf_delta& d = b->deltas[i];
-        b->delta_at[((uint64_t)d.run << 32) | ((uint64_t)d.field << 16) | d.index] = (uint32_t)i;
-      }
-    }
-  }
+  if (b->resident) rewrite_deltas(b, [gone = b->n](bf_delta& d) { return d.run != gone; });
   return BF_OK;
 }
 
@@ -441,7 +465,7 @@ int bfh_batch_remove_last_run(bfh_batch* b) {
   if (!(b) || (run) >= (b)->n) return BF_EINVAL;                                                                 \
   const bfh_story* st = (b)->story_of_run[run];                                                                  \
   if ((step) >= st->flags.size()) return BF_EINVAL;                                                              \
-  uint8_t* rec = (b)->state + (size_t)(run) * (b)->L.state_stride;
+  uint8_t* rec = (b)->rec.state + (size_t)(run) * (b)->L.state_stride;
 
 int bfh_run_set_phase_code(bfh_batch* b, uint32_t run, uint32_t step, int code) {
   RUN_CHECK(b, run, step)
@@ -478,7 +502,7 @@ int bfh_run_set_gate(bfh_batch* b, uint32_t run, uint32_t step, const char* gate
 }
 int bfh_run_set_run_flags(bfh_batch* b, uint32_t run, int topology_terminated, int host_group) {
   if (!b || run >= b->n) return BF_EINVAL;
-  bf_run_header* h = reinterpret_cast<bf_run_header*>(b->state + (size_t)run * b->L.state_stride);
+  bf_run_header* h = reinterpret_cast<bf_run_header*>(b->rec.state + (size_t)run * b->L.state_stride);
   uint8_t f = (uint8_t)bfh_story_run_flags(b->story_of_run[run]);
   if (topology_terminated) f |= BF_RF_TOPOLOGY_TERMINATED;
   if (host_group >= 0) f |= (uint8_t)(BF_RF_HOST_GROUP | ((host_group & 3) << BF_RF_HOST_GROUP_SHIFT));
@@ -488,7 +512,7 @@ int bfh_run_set_run_flags(bfh_batch* b, uint32_t run, int topology_terminated, i
 }
 int bfh_run_register_children(bfh_batch* b, uint32_t run, uint32_t q, int on) {
   if (!b || run >= b->n || q >= b->story_of_run[run]->par.size()) return BF_EINVAL;
-  bf_run_header* h = reinterpret_cast<bf_run_header*>(b->state + (size_t)run * b->L.state_stride);
+  bf_run_header* h = reinterpret_cast<bf_run_header*>(b->rec.state + (size_t)run * b->L.state_stride);
   if (on) h->children_registered |= 1ull << q; else h->children_registered &= ~(1ull << q);
   b->log_delta(run, BF_DELTA_REGISTERED, q, on ? 1u : 0u);
   return BF_OK;
@@ -499,7 +523,7 @@ int bfh_run_set_child_phase(bfh_batch* b, uint32_t run, uint32_t q, uint32_t bra
   if (q >= st->par.size() || branch >= st->par[q].branches) return BF_EINVAL;
   const int c = phase_code_of(phase, nullptr);
   if (c < 0) return BF_EINVAL;
-  uint8_t* ch = b->state + (size_t)run * b->L.state_stride + b->L.off_child;
+  uint8_t* ch = b->rec.state + (size_t)run * b->L.state_stride + b->L.off_child;
   const uint32_t i = st->child_first[q] + branch;
   const uint8_t sh = (uint8_t)((i & 1u) * 4u);
   ch[i >> 1] = (uint8_t)((ch[i >> 1] & ~(0xFu << sh)) | ((unsigned)c << sh));
@@ -512,25 +536,21 @@ int bfh_batch_eval(bfh_batch* b, uint32_t eval_flags, bf_counts* counts) {
   if (!b->ctx) { b->err = "batch was created without a device context"; return BF_ENODEV; }
   if (b->resident) {
     // new runs as full records, everything else as the tick's coalesced deltas, then one pass over the device copy
-    int rc = BF_OK;
-    if (b->uploaded < b->n) {
-      rc = bf_resident_upload(b->ctx, b->handle, b->uploaded, b->n - b->uploaded, b->state + (size_t)b->uploaded * b->L.state_stride);
-      if (rc == BF_OK) { b->full_bytes_sent += (uint64_t)(b->n - b->uploaded) * b->L.state_stride; b->uploaded = b->n; }
-    }
+    int rc = flush_uploads(b);
     if (rc == BF_OK && !b->deltas.empty()) {
       rc = bf_resident_apply(b->ctx, b->handle, b->deltas.data(), (uint32_t)b->deltas.size());
       b->delta_bytes_sent += b->deltas.size() * sizeof(bf_delta);
     }
     b->deltas.clear();
     b->delta_at.clear();
-    if (rc == BF_OK) rc = bf_resident_eval(b->ctx, b->handle, b->n, eval_flags & ~(uint32_t)BF_EVAL_EXPANSION, 0, b->result, counts);
+    if (rc == BF_OK) rc = bf_resident_eval(b->ctx, b->handle, b->n, eval_flags & ~(uint32_t)BF_EVAL_EXPANSION, 0, b->rec.result, counts);
     if (rc != BF_OK) b->err = bf_last_error(b->ctx);
     return rc;
   }
   bf_batch bb{};
   bb.struct_size = sizeof(bf_batch);
   bb.n_runs = b->n; bb.flags = eval_flags; bb.layout = b->L;
-  bb.state = b->state; bb.result = b->result; bb.counts = counts;
+  bb.state = b->rec.state; bb.result = b->rec.result; bb.counts = counts;
   const int rc = bf_eval(b->ctx, &bb);
   if (rc != BF_OK) b->err = bf_last_error(b->ctx);
   return rc;
@@ -576,7 +596,7 @@ int bfh_batch_migrate(bfh_batch* b, const bfh_story* os, const bfh_story* ns, ui
   std::vector<uint8_t> moved(b->n, 0);
   uint32_t n_moved = 0, n_on_device = 0;
   for (uint32_t r = 0; r < b->n; ++r) {
-    if (reinterpret_cast<const bf_run_header*>(b->state + (size_t)r * L.state_stride)->topo_slot != old_slot) continue;
+    if (reinterpret_cast<const bf_run_header*>(b->rec.state + (size_t)r * L.state_stride)->topo_slot != old_slot) continue;
     if (b->story_of_run[r] != os) { b->err = "run " + std::to_string(r) + " holds old_slot but is not a run of old_story"; return BF_EINVAL; }
     moved[r] = 1;
     ++n_moved;
@@ -603,7 +623,7 @@ int bfh_batch_migrate(bfh_batch* b, const bfh_story* os, const bfh_story* ns, ui
   std::vector<uint8_t> old(L.state_stride);
   for (uint32_t r = 0; r < b->n; ++r) {
     if (!moved[r]) continue;
-    uint8_t* rec = b->state + (size_t)r * L.state_stride;
+    uint8_t* rec = b->rec.state + (size_t)r * L.state_stride;
     memcpy(old.data(), rec, L.state_stride);
     for (uint32_t j = 0; j < W * 32; ++j) {
       const uint32_t o = inv[j];
@@ -633,36 +653,24 @@ int bfh_batch_migrate(bfh_batch* b, const bfh_story* os, const bfh_story* ns, ui
     b->story_of_run[r] = ns;
   }
   // pending deltas of the moved runs follow their step / desc, or are dropped with a removed step
-  if (!b->deltas.empty()) {
-    size_t keep = 0;
-    for (size_t k = 0; k < b->deltas.size(); ++k) {
-      bf_delta d = b->deltas[k];
-      bool ok = true;
-      if (d.run < b->n && moved[d.run]) {
-        if (d.field == BF_DELTA_PHASE || d.field == BF_DELTA_COND || d.field == BF_DELTA_DECISION) {
-          ok = d.index < So && map[d.index] != BF_MIGRATE_GONE;
-          if (ok) d.index = map[d.index];
-        } else if (d.field == BF_DELTA_REGISTERED) {
-          ok = d.index < desc_to.size() && desc_to[d.index] >= 0;
-          if (ok) d.index = (uint16_t)desc_to[d.index];
-        } else if (d.field == BF_DELTA_CHILD) {
-          ok = false;
-          for (size_t p = 0; p < os->par.size() && !ok; ++p)
-            if (desc_to[p] >= 0 && d.index >= os->child_first[p] && d.index < os->child_first[p] + os->par[p].branches) {
-              d.index = (uint16_t)(ns->child_first[desc_to[p]] + (d.index - os->child_first[p]));
-              ok = true;
-            }
+  rewrite_deltas(b, [&](bf_delta& d) {
+    if (d.run >= b->n || !moved[d.run]) return true;
+    if (d.field == BF_DELTA_PHASE || d.field == BF_DELTA_COND || d.field == BF_DELTA_DECISION) {
+      if (d.index >= So || map[d.index] == BF_MIGRATE_GONE) return false;
+      d.index = map[d.index];
+    } else if (d.field == BF_DELTA_REGISTERED) {
+      if (d.index >= desc_to.size() || desc_to[d.index] < 0) return false;
+      d.index = (uint16_t)desc_to[d.index];
+    } else if (d.field == BF_DELTA_CHILD) {
+      for (size_t p = 0; p < os->par.size(); ++p)
+        if (desc_to[p] >= 0 && d.index >= os->child_first[p] && d.index < os->child_first[p] + os->par[p].branches) {
+          d.index = (uint16_t)(ns->child_first[desc_to[p]] + (d.index - os->child_first[p]));
+          return true;
         }
-      }
-      if (ok) b->deltas[keep++] = d;
+      return false;
     }
-    b->deltas.resize(keep);
-    b->delta_at.clear();
-    for (size_t i = 0; i < keep; ++i) {
-      const bf_delta& d = b->deltas[i];
-      b->delta_at[((uint64_t)d.run << 32) | ((uint64_t)d.field << 16) | d.index] = (uint32_t)i;
-    }
-  }
+    return true;
+  });
   return (int)n_moved;
 }
 
@@ -703,7 +711,7 @@ int bfh_batch_redrive(bfh_batch* b, const uint32_t* runs, const int32_t* steps, 
       if (runs[i] >= b->uploaded) continue;   // not on the device yet: it travels as a full record
       bf_redrive q{};
       q.run = runs[i];
-      q.slot = reinterpret_cast<const bf_run_header*>(b->state + (size_t)runs[i] * L.state_stride)->topo_slot;
+      q.slot = reinterpret_cast<const bf_run_header*>(b->rec.state + (size_t)runs[i] * L.state_stride)->topo_slot;
       q.step = steps[i] < 0 ? BF_REDRIVE_ALL : (uint32_t)steps[i];
       req.push_back(q);
     }
@@ -718,7 +726,6 @@ int bfh_batch_redrive(bfh_batch* b, const uint32_t* runs, const int32_t* steps, 
   // reset the mirror's records; reset[(run, field, index)] marks the pending deltas the reset supersedes
   std::map<std::pair<const bfh_story*, int32_t>, std::vector<uint32_t>> closures;
   std::unordered_map<uint64_t, bool> superseded;
-  auto key = [](uint32_t run, uint32_t field, uint32_t index) { return ((uint64_t)run << 32) | ((uint64_t)field << 16) | index; };
   std::vector<uint8_t> reset_runs(b->n, 0);
   for (uint32_t i = 0; i < n; ++i) {
     const uint32_t run = runs[i];
@@ -733,28 +740,28 @@ int bfh_batch_redrive(bfh_batch* b, const uint32_t* runs, const int32_t* steps, 
         redrive_closure(st, (uint32_t)steps[i], m);
       }
     }
-    uint8_t* rec = b->state + (size_t)run * L.state_stride;
+    uint8_t* rec = b->rec.state + (size_t)run * L.state_stride;
     auto in = [&](uint32_t j) { return ((m[j >> 5] >> (j & 31u)) & 1u) != 0; };
     for (uint32_t j = 0; j < S; ++j) {
       if (!in(j)) continue;
       set_code(rec + L.off_phase, W, 4, j, 0);
-      superseded[key(run, BF_DELTA_PHASE, j)] = true;
-      if (L.off_decision != BF_OFF_NONE) { set_code(rec + L.off_decision, W, 2, j, BF_DEC_PENDING); superseded[key(run, BF_DELTA_DECISION, j)] = true; }
+      superseded[delta_key(run, BF_DELTA_PHASE, j)] = true;
+      if (L.off_decision != BF_OFF_NONE) { set_code(rec + L.off_decision, W, 2, j, BF_DEC_PENDING); superseded[delta_key(run, BF_DELTA_DECISION, j)] = true; }
       if (L.off_cond != BF_OFF_NONE) {
         set_code(rec + L.off_cond, W, 2, j, (st->flags[j] & BF_SF_HAS_IF) ? BF_COND_HOLD : BF_COND_PASS);
-        superseded[key(run, BF_DELTA_COND, j)] = true;
+        superseded[delta_key(run, BF_DELTA_COND, j)] = true;
       }
     }
     bf_run_header* h = reinterpret_cast<bf_run_header*>(rec);
     for (size_t p = 0; p < st->par.size(); ++p) {
       if (!in(st->par[p].step)) continue;
       h->children_registered &= ~(1ull << p);
-      superseded[key(run, BF_DELTA_REGISTERED, (uint32_t)p)] = true;
+      superseded[delta_key(run, BF_DELTA_REGISTERED, (uint32_t)p)] = true;
       if (L.off_child == BF_OFF_NONE) continue;
       for (uint32_t br = 0; br < st->par[p].branches; ++br) {
         const uint32_t c = st->child_first[p] + br;
         rec[L.off_child + (c >> 1)] &= (uint8_t)~(0xFu << ((c & 1u) * 4u));
-        superseded[key(run, BF_DELTA_CHILD, c)] = true;
+        superseded[delta_key(run, BF_DELTA_CHILD, c)] = true;
       }
     }
     h->run_flags &= (uint8_t)~BF_RF_TOPOLOGY_TERMINATED;
@@ -764,17 +771,12 @@ int bfh_batch_redrive(bfh_batch* b, const uint32_t* runs, const int32_t* steps, 
     b->uploaded = 0;
     b->deltas.clear();
     b->delta_at.clear();
-  } else if (!b->deltas.empty()) {
-    size_t keep = 0;
-    for (size_t k = 0; k < b->deltas.size(); ++k) {
-      bf_delta d = b->deltas[k];
-      if (superseded.count(key(d.run, d.field, d.index))) continue;
+  } else {
+    rewrite_deltas(b, [&](bf_delta& d) {
+      if (superseded.count(delta_key(d.run, d.field, d.index))) return false;
       if (d.field == BF_DELTA_RUN_FLAGS && d.run < b->n && reset_runs[d.run]) d.code &= (uint8_t)~BF_RF_TOPOLOGY_TERMINATED;
-      b->deltas[keep++] = d;
-    }
-    b->deltas.resize(keep);
-    b->delta_at.clear();
-    for (size_t i = 0; i < keep; ++i) b->delta_at[key(b->deltas[i].run, b->deltas[i].field, b->deltas[i].index)] = (uint32_t)i;
+      return true;
+    });
   }
   return BF_OK;
 }
@@ -796,31 +798,26 @@ int bfh_batch_reshape(bfh_batch* b, uint32_t steps_max, uint32_t child_nibbles, 
     b->err = "a reshape only grows the batch (capacity, steps_max, fields, child_nibbles)";
     return BF_EINVAL;
   }
-  uint8_t *st = nullptr, *res = nullptr;
-  bool pinned = false;
-  if (!alloc_records(b->ctx, (size_t)capacity * T.state_stride, (size_t)capacity * T.result_stride, &st, &res, &pinned)) {
+  HostRecords nr;
+  if (!nr.alloc(b->ctx, (size_t)capacity * T.state_stride, (size_t)capacity * T.result_stride)) {
     b->err = "out of host memory";
     return BF_ENOMEM;
   }
   if (b->resident) {   // the device first: it fails without changes, and then the mirror stays as it was too
     const int rc = bf_resident_reshape(b->ctx, b->handle, &T, capacity);
-    if (rc != BF_OK) {
-      b->err = bf_last_error(b->ctx);
-      if (pinned) { bf_free_pinned(b->ctx, st); bf_free_pinned(b->ctx, res); } else { free(st); free(res); }
-      return rc;
-    }
+    if (rc != BF_OK) { b->err = bf_last_error(b->ctx); return rc; }
   }
   const uint32_t Wn = T.words, Wo = F.words;
   for (uint32_t r = 0; r < b->cap; ++r) {
-    const uint8_t* s = b->state + (size_t)r * F.state_stride;
-    uint8_t* d = st + (size_t)r * T.state_stride;
+    const uint8_t* s = b->rec.state + (size_t)r * F.state_stride;
+    uint8_t* d = nr.state + (size_t)r * T.state_stride;
     memcpy(d, s, sizeof(bf_run_header));
     relay_planes(d, s, T.off_phase, F.off_phase, 4, Wn, Wo);
     relay_planes(d, s, T.off_cond, F.off_cond, 2, Wn, Wo);
     relay_planes(d, s, T.off_decision, F.off_decision, 2, Wn, Wo);
     if (F.off_child != BF_OFF_NONE) memcpy(d + T.off_child, s + F.off_child, ((F.child_nibbles + 1) / 2 + 3) / 4 * 4);
-    s = b->result + (size_t)r * F.result_stride;
-    d = res + (size_t)r * T.result_stride;
+    s = b->rec.result + (size_t)r * F.result_stride;
+    d = nr.result + (size_t)r * T.result_stride;
     memcpy(d, s, sizeof(bf_result_header));
     relay_planes(d, s, T.off_ready, F.off_ready, 1, Wn, Wo);
     relay_planes(d, s, T.off_skip, F.off_skip, 1, Wn, Wo);
@@ -829,8 +826,7 @@ int bfh_batch_reshape(bfh_batch* b, uint32_t steps_max, uint32_t child_nibbles, 
     relay_planes(d, s, T.off_skip_dep, F.off_skip_dep, 1, Wn, Wo);
     relay_planes(d, s, T.off_phase_out, F.off_phase_out, 4, Wn, Wo);
   }
-  free_records(b);
-  b->state = st; b->result = res; b->pinned = pinned;
+  b->rec.swap(nr);
   b->L = T; b->cap = capacity;
   return BF_OK;
 }
@@ -855,60 +851,41 @@ int bfh_batch_retire(bfh_batch* b, const uint32_t* runs, uint32_t n, uint32_t ca
     from.push_back(m + i); to.push_back(hole); new_index[i] = hole++;
   }
   const bf_layout& L = b->L;
-  uint8_t *st = nullptr, *res = nullptr;
-  bool pinned = false;
-  if (cap != b->cap && !alloc_records(b->ctx, (size_t)cap * L.state_stride, (size_t)cap * L.result_stride, &st, &res, &pinned)) {
+  HostRecords nr;
+  if (cap != b->cap && !nr.alloc(b->ctx, (size_t)cap * L.state_stride, (size_t)cap * L.result_stride)) {
     b->err = "out of host memory";
     return BF_ENOMEM;
   }
   if (b->resident) {   // every run on the device first, then the device: it fails without changes, and so does the mirror
-    int rc = BF_OK;
-    if (b->uploaded < N) {
-      rc = bf_resident_upload(b->ctx, b->handle, b->uploaded, N - b->uploaded, b->state + (size_t)b->uploaded * L.state_stride);
-      if (rc == BF_OK) { b->full_bytes_sent += (uint64_t)(N - b->uploaded) * L.state_stride; b->uploaded = N; }
-    }
+    int rc = flush_uploads(b);
     if (rc == BF_OK) {
       bf_retire rt{};
       rt.struct_size = sizeof rt; rt.n_runs = N; rt.runs = runs; rt.n = n; rt.capacity = capacity;
       rc = bf_resident_retire(b->ctx, b->handle, &rt);
     }
-    if (rc != BF_OK) {
-      b->err = bf_last_error(b->ctx);
-      if (st) { if (pinned) { bf_free_pinned(b->ctx, st); bf_free_pinned(b->ctx, res); } else { free(st); free(res); } }
-      return rc;
-    }
+    if (rc != BF_OK) { b->err = bf_last_error(b->ctx); return rc; }
   }
   const size_t ss = L.state_stride, rs = L.result_stride;
   for (size_t k = 0; k < from.size(); ++k) {
-    memcpy(b->state + to[k] * ss, b->state + from[k] * ss, ss);
-    memcpy(b->result + to[k] * rs, b->result + from[k] * rs, rs);
+    memcpy(b->rec.state + to[k] * ss, b->rec.state + from[k] * ss, ss);
+    memcpy(b->rec.result + to[k] * rs, b->rec.result + from[k] * rs, rs);
     b->story_of_run[to[k]] = b->story_of_run[from[k]];
   }
-  memset(b->state + (size_t)m * ss, 0, (size_t)n * ss);
-  memset(b->result + (size_t)m * rs, 0, (size_t)n * rs);
+  memset(b->rec.state + (size_t)m * ss, 0, (size_t)n * ss);
+  memset(b->rec.result + (size_t)m * rs, 0, (size_t)n * rs);
   b->story_of_run.resize(m);
-  if (st) {
-    memcpy(st, b->state, (size_t)m * ss);
-    memcpy(res, b->result, (size_t)m * rs);
-    free_records(b);
-    b->state = st; b->result = res; b->pinned = pinned; b->cap = cap;
+  if (nr.state) {
+    memcpy(nr.state, b->rec.state, (size_t)m * ss);
+    memcpy(nr.result, b->rec.result, (size_t)m * rs);
+    b->rec.swap(nr);
+    b->cap = cap;
   }
   // pending deltas: those of retired runs go, those of moved runs apply at the new index (no two keys meet: a target was retired)
-  if (!b->deltas.empty()) {
-    size_t keep = 0;
-    for (size_t k = 0; k < b->deltas.size(); ++k) {
-      bf_delta d = b->deltas[k];
-      if (gone[d.run]) continue;
-      if (d.run >= m) d.run = new_index[d.run - m];
-      b->deltas[keep++] = d;
-    }
-    b->deltas.resize(keep);
-    b->delta_at.clear();
-    for (size_t i = 0; i < keep; ++i) {
-      const bf_delta& d = b->deltas[i];
-      b->delta_at[((uint64_t)d.run << 32) | ((uint64_t)d.field << 16) | d.index] = (uint32_t)i;
-    }
-  }
+  rewrite_deltas(b, [&](bf_delta& d) {
+    if (gone[d.run]) return false;
+    if (d.run >= m) d.run = new_index[d.run - m];
+    return true;
+  });
   b->n = m;
   if (b->uploaded > m) b->uploaded = m;
   if (moves_from && !from.empty()) memcpy(moves_from, from.data(), from.size() * 4);
@@ -941,11 +918,11 @@ int bfh_batch_traffic(const bfh_batch* b, uint64_t* full_record_bytes, uint64_t*
 
 uint32_t bfh_run_summary(const bfh_batch* b, uint32_t run) {
   if (!b || run >= b->n) return 0xFFFFFFFFu;
-  return reinterpret_cast<const bf_result_header*>(b->result + (size_t)run * b->L.result_stride)->summary;
+  return reinterpret_cast<const bf_result_header*>(b->rec.result + (size_t)run * b->L.result_stride)->summary;
 }
 static int mask_list(const bfh_batch* b, uint32_t run, uint32_t off, uint32_t* out, uint32_t cap) {
   if (!b || run >= b->n || off == BF_OFF_NONE) return BF_EINVAL;
-  const uint32_t* m = reinterpret_cast<const uint32_t*>(b->result + (size_t)run * b->L.result_stride + off);
+  const uint32_t* m = reinterpret_cast<const uint32_t*>(b->rec.result + (size_t)run * b->L.result_stride + off);
   const uint32_t S = (uint32_t)b->story_of_run[run]->flags.size();
   int n = 0;
   for (uint32_t i = 0; i < S; ++i)
@@ -961,13 +938,13 @@ int bfh_run_failed(const bfh_batch* b, uint32_t run, uint32_t* out, uint32_t cap
 int bfh_run_needs_cond(const bfh_batch* b, uint32_t run, uint32_t* out, uint32_t cap) { return mask_list(b, run, b ? b->L.off_needs_cond : BF_OFF_NONE, out, cap); }
 int bfh_run_phase_out(const bfh_batch* b, uint32_t run, uint32_t step) {
   if (!b || run >= b->n || b->L.off_phase_out == BF_OFF_NONE || step >= b->story_of_run[run]->flags.size()) return -1;
-  return get_code(b->result + (size_t)run * b->L.result_stride + b->L.off_phase_out, b->L.words, 4, step);
+  return get_code(b->rec.result + (size_t)run * b->L.result_stride + b->L.off_phase_out, b->L.words, 4, step);
 }
 int bfh_run_skip_reason(const bfh_batch* b, uint32_t run, uint32_t step, char* out, size_t cap) {
   if (!b || run >= b->n || !out || !cap) return BF_EINVAL;
   const bfh_story* st = b->story_of_run[run];
   if (step >= st->flags.size()) return BF_EINVAL;
-  const uint8_t* rrec = b->result + (size_t)run * b->L.result_stride;
+  const uint8_t* rrec = b->rec.result + (size_t)run * b->L.result_stride;
   std::string msg = "Skipped due to 'if' condition";  // dag.go:2831
   bool by_dep = false;
   if (b->L.off_skip_dep != BF_OFF_NONE)
@@ -975,7 +952,7 @@ int bfh_run_skip_reason(const bfh_batch* b, uint32_t run, uint32_t step, char* o
   if (by_dep) {
     msg = "Skipped due to failed dependency: ";  // dag.go:2737; the named dep = first failed one in CSR order
     const uint8_t* ph = b->L.off_phase_out != BF_OFF_NONE ? rrec + b->L.off_phase_out
-                                                         : b->state + (size_t)run * b->L.state_stride + b->L.off_phase;
+                                                         : b->rec.state + (size_t)run * b->L.state_stride + b->L.off_phase;
     for (uint32_t e = st->row_ptr[step]; e < st->row_ptr[step + 1]; ++e) {
       const uint32_t d = st->col_idx[e];
       const int p = get_code(ph, b->L.words, 4, d);

@@ -29,7 +29,7 @@ __global__ void __launch_bounds__(256) apply_deltas(const DeltaParams P) {
   if (i >= P.n) return;
   const bf_delta d = P.deltas[i];
   bool ok = d.run < P.n_runs;
-  if (ok) atomicMax(P.mark + d.run, P.mark_value);   // touch mark (abi.cu, touched ticks); max: an upload's "must list" bit stays
+  if (ok) atomicMax(P.mark + d.run, P.mark_value);   // touch mark (Resident in ctx.h, touched ticks); max: an upload's "must list" bit stays
   uint8_t* rec = P.state + (size_t)d.run * P.state_stride;
   const uint32_t S_max = P.words * 32u;
   if (ok) switch (d.field) {
@@ -70,7 +70,7 @@ __global__ void __launch_bounds__(256) apply_deltas(const DeltaParams P) {
   if (!ok) atomicAdd(P.rejected, 1u);
 }
 
-// Touch marks of runs [first, first + n) after an upload: epoch << 1 | 1 ("must list", abi.cu)
+// Touch marks of runs [first, first + n) after an upload: epoch << 1 | 1 ("must list", Resident in ctx.h)
 __global__ void __launch_bounds__(256) mark_runs(uint32_t* mark, uint32_t first, uint32_t n, uint32_t value) {
   const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i < n) mark[first + i] = value;
