@@ -411,6 +411,14 @@ int check_layout(bf_ctx* c, const bf_layout& L) {
   return BF_OK;
 }
 
+uint32_t result_tail_of(const bf_layout& L) {
+  uint32_t tail = (uint32_t)sizeof(bf_result_header);
+  auto upd = [&](uint32_t off, uint32_t len) { if (off != BF_OFF_NONE && off + len > tail) tail = off + len; };
+  upd(L.off_ready, L.words * 4); upd(L.off_skip, L.words * 4); upd(L.off_fail, L.words * 4);
+  upd(L.off_needs_cond, L.words * 4); upd(L.off_skip_dep, L.words * 4); upd(L.off_phase_out, L.words * 16);
+  return tail;
+}
+
 // shared-memory plan + launch of one pass on device buffers
 // run_list (touched ticks): the pass takes the runs run_list[0 .. *run_list_count) (b.n_runs bounds the count) and writes
 // each run's record at its own index
@@ -645,15 +653,26 @@ void* pinned_dev(const void* p) {
 }
 
 // ---- compact results: masks -> heads + 16-bit events on the device, then two small D2H copies ----
-// Enqueue on `s` (after the passes that wrote d_result): compaction kernels, D2H of the head words and of a first slice of
-// the event list sized from the previous pass (the exact length is only known after the sync; it arrives, with the counts,
-// in the pinned tail block the last kernel writes itself).
-uint32_t result_tail_of(const bf_layout& L) {
-  uint32_t tail = (uint32_t)sizeof(bf_result_header);
-  auto upd = [&](uint32_t off, uint32_t len) { if (off != BF_OFF_NONE && off + len > tail) tail = off + len; };
-  upd(L.off_ready, L.words * 4); upd(L.off_skip, L.words * 4); upd(L.off_fail, L.words * 4);
-  upd(L.off_needs_cond, L.words * 4); upd(L.off_skip_dep, L.words * 4); upd(L.off_phase_out, L.words * 16);
-  return tail;
+// Enqueue on `s` (after the passes that wrote d_result): compaction kernels, D2H of the head words and of a first slice of the
+// event list sized from the previous list (+ 3 % + slack; none when the kernel posts the list).  The exact length arrives after
+// the sync, with the counts, in the pinned tail the last kernel writes; compact_finish then fetches the rest.
+
+// what every compaction takes from the layout and the ctx: the result fields it reads, and the pinned tail its last kernel
+// writes with the counts and the rejected-delta counter (the kernel reads and clears it) when asked for them
+CompactParams compact_params(bf_ctx* c, const bf_layout& L, uint32_t n_runs, bool want_counts, bool want_rejected) {
+  CompactParams P{};
+  P.n_runs = n_runs; P.words = L.words; P.result_stride = L.result_stride; P.result_tail = result_tail_of(L);
+  P.off_ready = L.off_ready; P.off_skip = L.off_skip;
+  P.off_fail = L.off_fail; P.off_needs_cond = L.off_needs_cond; P.off_skip_dep = L.off_skip_dep;
+  P.host_tail = &c->pinned->tail; P.counts = want_counts ? c->d_counts.p : nullptr; P.rejected = want_rejected ? c->d_rejected.p : nullptr;
+  return P;
+}
+
+int events_first(bf_ctx* c, uint16_t* events, uint64_t prev, uint64_t slack, uint64_t cap, bool posted, cudaStream_t s, uint64_t& first) {
+  const uint64_t n = posted ? 0 : std::min(prev + prev / 32 + slack, cap);
+  first = posted ? cap : n;   // posted: the whole list is in the caller's buffer after the synchronise
+  if (n) BF_CUDA(c, cudaMemcpyAsync(events, c->d_events, (size_t)n * sizeof(uint16_t), cudaMemcpyDeviceToHost, s));
+  return BF_OK;
 }
 
 // head words + the scratch block of a compaction (zeroed once; the kernels leave it clean): before the pass, so that a fused
@@ -672,58 +691,41 @@ int compact_prepare(bf_ctx* c, uint32_t n_runs, cudaStream_t s) {
 unsigned long long* cblock_sums(bf_ctx* c, uint32_t which) { return c->d_cblock + 2 + (size_t)which * ((c->d_cblock.cap - 2) / 2); }
 
 int compact_enqueue(bf_ctx* c, const bf_layout& L, const uint8_t* d_result, const uint8_t* d_prev, uint32_t n_runs, bf_compact_out* out,
-                    cudaStream_t s, uint64_t* first_slice, bool with_rejected, bool heads_done) {
+                    cudaStream_t s, uint64_t& first_slice, bool with_rejected, bool heads_done) {
   const uint64_t cap = out->events ? out->events_cap : 0;
   if (int rc = compact_prepare(c, n_runs, s)) return rc;
   if (int rc = c->d_events.ensure(c, cap ? (size_t)cap : 1)) return rc;
-  bf::CompactParams P{};
-  P.result = d_result; P.prev_result = d_prev; P.head = c->d_head; P.events = c->d_events; P.cap = cap;
+  CompactParams P = compact_params(c, L, n_runs, true, with_rejected);
+  P.result = d_result; P.prev_result = d_prev; P.head = c->d_head; P.cap = cap;
   P.block_sums = cblock_sums(c, c->cblock_flip); P.zero_sums = cblock_sums(c, c->cblock_flip ^ 1u); P.total = c->d_cblock;
   P.zero_len = (uint32_t)((c->d_cblock.cap - 2) / 2);
   P.heads_done = heads_done ? 1u : 0u;
   c->cblock_flip ^= 1u;   // the next compaction (and a pass fused with it) uses the buffer this one leaves zeroed
-  P.n_runs = n_runs; P.words = L.words; P.result_stride = L.result_stride; P.result_tail = result_tail_of(L);
-  P.off_ready = L.off_ready; P.off_skip = L.off_skip;
-  P.off_fail = L.off_fail; P.off_needs_cond = L.off_needs_cond; P.off_skip_dep = L.off_skip_dep;
-  // the small results (event total, counts, rejected deltas, listed runs) are written to the pinned block by the last kernel
-  // itself: no latency-bound small D2H copies
-  unsigned long long* tail = reinterpret_cast<unsigned long long*>(c->h_counts + 2);   // 7 x u64 in the pinned block
-  P.host_tail = tail; P.counts = c->d_counts; P.rejected = with_rejected ? c->d_rejected.p : nullptr;
   // a head buffer in pinned host memory (bf_alloc_pinned, cudaHostAlloc / cudaHostRegister) gets the head words posted by the
   // kernel itself; any other buffer gets them by a download
-  P.host_head = nullptr;
   if (out->head && n_runs && !getenv("BF_NO_ZC_HEADS")) P.host_head = static_cast<uint32_t*>(pinned_dev(out->head));
-  bool events_posted = false;
-  if (out->events && cap && !getenv("BF_NO_ZC_EVENTS")) {   // the event list likewise: posted by the emit kernel, no download
-    if (void* d = pinned_dev(out->events)) {
-      P.events = static_cast<uint16_t*>(d);
-      events_posted = true;
-    }
-  }
+  // the event list likewise: posted by the emit kernel, no download
+  uint16_t* p_events = cap && !getenv("BF_NO_ZC_EVENTS") ? static_cast<uint16_t*>(pinned_dev(out->events)) : nullptr;
+  P.events = p_events ? p_events : c->d_events;
   if (n_runs == 0) BF_CUDA(c, cudaStreamSynchronize(s));   // the empty case stores to the pinned block from the host
   c->cblock_clean = false;   // until the call has gone through (resident_tick_locked / eval_host set it again after the sync)
   BF_CUDA(c, bf::launch_compact(P, s));
   c->stats.kernel_launches += n_runs ? (heads_done ? 1 : 2) : 0;
-  uint64_t guess = c->last_events + c->last_events / 32 + 4096;   // the previous tick's list + 3 %: one copy in the steady state
-  if (guess > cap) guess = cap;
-  if (events_posted) guess = 0;
-  if (guess) BF_CUDA(c, cudaMemcpyAsync(out->events, c->d_events, (size_t)guess * sizeof(uint16_t), cudaMemcpyDeviceToHost, s));
+  if (int rc = events_first(c, out->events, c->last_events, 4096, cap, p_events != nullptr, s, first_slice)) return rc;
   if (out->head && n_runs && !P.host_head) BF_CUDA(c, cudaMemcpyAsync(out->head, c->d_head, (size_t)n_runs * 4, cudaMemcpyDeviceToHost, s));
-  *first_slice = events_posted ? cap : guess;   // posted: the whole list is in the caller's buffer after the synchronise
   return BF_OK;
 }
-// after the stream has been synchronised: fetch what the first slice missed
-int compact_finish(bf_ctx* c, bf_compact_out* out, uint64_t first_slice) {
-  const unsigned long long* tail = reinterpret_cast<const unsigned long long*>(c->h_counts + 2);
-  const uint64_t total = tail[0];
+// after the stream has been synchronised: fetch what the first slice missed; the length sizes the next first slice (prev)
+int compact_finish(bf_ctx* c, bf_compact_out* out, uint64_t first_slice, uint64_t& prev) {
+  const ResultTail& tail = c->pinned->tail;
   const uint64_t cap = out->events ? out->events_cap : 0;
-  const uint64_t have = total < cap ? total : cap;
+  const uint64_t have = tail.events < cap ? tail.events : cap;
   if (have > first_slice)
     BF_CUDA(c, cudaMemcpy(out->events + first_slice, c->d_events + first_slice, (size_t)(have - first_slice) * sizeof(uint16_t),
                           cudaMemcpyDeviceToHost));
-  out->n_events = total;
-  out->n_listed = (uint32_t)tail[6];
-  c->last_events = total;
+  out->n_events = tail.events;
+  out->n_listed = (uint32_t)tail.listed;
+  prev = tail.events;
   return BF_OK;
 }
 
@@ -768,7 +770,7 @@ int bf_create(bf_ctx** out, const bf_config* cfg) {
   if (cudaSetDevice(dev) != cudaSuccess || cudaStreamCreateWithFlags(&c->stream, cudaStreamNonBlocking) != cudaSuccess ||
       c->d_counts.alloc(sizeof(bf_counts) / 8) != cudaSuccess ||
       c->d_acc.alloc(bf_ctx::kAccSlots * 8) != cudaSuccess || cudaMemset(c->d_acc, 0, bf_ctx::kAccSlots * 64) != cudaSuccess ||
-      cudaHostAlloc(reinterpret_cast<void**>(&c->h_counts), 5 * sizeof(bf_counts), cudaHostAllocDefault) != cudaSuccess) {
+      cudaHostAlloc(&c->pinned, sizeof *c->pinned, cudaHostAllocDefault) != cudaSuccess) {
     cudaGetLastError();
     bf_destroy(c);  // releases whatever was created
     return BF_ECUDA;
@@ -792,7 +794,7 @@ void bf_destroy(bf_ctx* c) {
     if (c->ev_in[k]) cudaEventDestroy(c->ev_in[k]);
     if (c->ev_k[k]) cudaEventDestroy(c->ev_k[k]);
   }
-  cudaFreeHost(c->h_counts);
+  cudaFreeHost(c->pinned);
   delete c;   // the device buffers of the ctx and of its resident batches free themselves
 }
 
@@ -973,7 +975,7 @@ static int eval_host(bf_ctx* c, const bf_batch* b, bf_compact_out* co) {
   if (co && co->events_cap && !co->events) return fail(c, BF_EINVAL, "null events with a non-zero events_cap");
   if (int rc = bf::check_layout(c, b->layout)) return rc;
   if (b->n_runs && (!b->state || (!b->result && !co))) return fail(c, BF_EINVAL, "null state/result");
-  c->last_eval_valid = false;
+  c->snap.valid = false;
   const bf_layout& L = b->layout;
   const size_t sbytes = (size_t)b->n_runs * L.state_stride, rbytes = (size_t)b->n_runs * L.result_stride;
   if (b->flags & BF_EVAL_VALIDATE) {
@@ -1016,7 +1018,6 @@ static int eval_host(bf_ctx* c, const bf_batch* b, bf_compact_out* co) {
     if (int rc = bf::ensure_pipe(c)) return rc;
   const char* shape_env = getenv("BF_E2E_SHAPE");
   const bool taper = shape_env && !strcmp(shape_env, "taper");
-  bf_counts hc{};
   uint64_t first_slice = 0;
   auto body = [&]() -> int {
     BF_CUDA(c, cudaMemsetAsync(c->d_counts, 0, sizeof(bf_counts), s));
@@ -1052,9 +1053,9 @@ static int eval_host(bf_ctx* c, const bf_batch* b, bf_compact_out* co) {
       if (rb && !co) BF_CUDA(c, cudaMemcpyAsync(hr + ro, c->d_result + ro, rb, cudaMemcpyDeviceToHost, piped ? c->s_out : s));
     }
     if (co) {   // counts travel with the compaction's tail block
-      if (int rc = bf::compact_enqueue(c, L, c->d_result, nullptr, b->n_runs, co, s, &first_slice, false)) return rc;
+      if (int rc = bf::compact_enqueue(c, L, c->d_result, nullptr, b->n_runs, co, s, first_slice, false)) return rc;
     } else {
-      BF_CUDA(c, cudaMemcpyAsync(c->h_counts, c->d_counts, sizeof hc, cudaMemcpyDeviceToHost, s));
+      BF_CUDA(c, cudaMemcpyAsync(c->pinned->tail.counts, c->d_counts, sizeof(bf_counts), cudaMemcpyDeviceToHost, s));
     }
     return BF_OK;
   };
@@ -1068,17 +1069,16 @@ static int eval_host(bf_ctx* c, const bf_batch* b, bf_compact_out* co) {
   if (body_rc != BF_OK || e_sync != cudaSuccess) c->cblock_clean = false;   // (the compaction scratch may hold a partial pass)
   if (body_rc != BF_OK) return body_rc;
   if (e_sync != cudaSuccess) return cuda_fail(c, e_sync, "cudaStreamSynchronize");
-  hc = *c->h_counts;
-  if (co) { memcpy(&hc, reinterpret_cast<const unsigned long long*>(c->h_counts + 2) + 1, sizeof hc); c->cblock_clean = true; }
+  const bf_counts hc = c->pinned->counts();
+  if (co) c->cblock_clean = true;
   c->stats.last_eval_chunks = chunks;
-  c->last_eval_valid = true; c->last_eval_runs = b->n_runs; c->last_eval_layout = L;
-  c->last_state = c->d_state; c->last_result = c->d_result;
+  c->snap = {true, b->n_runs, L, c->d_state, c->d_result};
   if (want_exp) {
     const uint64_t n = hc.expansion < b->expansion_cap ? hc.expansion : b->expansion_cap;
     if (n) BF_CUDA(c, cudaMemcpy(b->expansion, c->d_exp, (size_t)n * sizeof(bf_expansion), cudaMemcpyDeviceToHost));
   }
   if (b->counts) *b->counts = hc;
-  if (co) return bf::compact_finish(c, co, first_slice);
+  if (co) return bf::compact_finish(c, co, first_slice, c->last_events);
   return BF_OK;
 }
 
@@ -1141,7 +1141,7 @@ static int schedule_host(bf_ctx* c, const bf_batch* b, const bf_sched_run* runs,
   if (int rc = fill_sched_params(c, b, t, P)) return rc;
   if (!out || out->struct_size != sizeof(bf_sched_out)) return fail(c, BF_EINVAL, "bad bf_sched_out.struct_size");
   if (b->n_runs && (!runs || !out->records)) return fail(c, BF_EINVAL, "null runs/records");
-  if (!c->last_eval_valid || c->last_eval_runs != b->n_runs || memcmp(&c->last_eval_layout, &b->layout, sizeof(bf_layout)) != 0)
+  if (!c->snap.matches(b->n_runs, b->layout))
     return fail(c, BF_EINVAL, "bf_schedule must follow bf_eval / bf_resident_eval of the same batch (n_runs and layout) on this ctx");
   BF_CUDA(c, cudaSetDevice(c->device));
   cudaStream_t s = c->stream;
@@ -1166,7 +1166,7 @@ static int schedule_host(bf_ctx* c, const bf_batch* b, const bf_sched_run* runs,
     BF_CUDA(c, up(o_qb, t->queue_running_base, nq * 4));
   }
   BF_CUDA(c, up(o_pb, t->queue_max_priority_base, nq * 4));
-  P.state = c->last_state; P.result = c->last_result;
+  P.state = c->snap.state; P.result = c->snap.result;
   P.runs = reinterpret_cast<const bf_sched_run*>(d + o_runs); P.records = d + o_rec;
   P.story_running = reinterpret_cast<uint32_t*>(d + o_sr); P.queue_running = reinterpret_cast<uint32_t*>(d + o_qr);
   P.queue_maxprio = reinterpret_cast<int32_t*>(d + o_mp); P.global_running = reinterpret_cast<uint32_t*>(d + o_gl);
@@ -1491,10 +1491,7 @@ int bf_group_schedule(bf_group* g, const bf_batch* b, const bf_sched_run* runs, 
     so.records = static_cast<uint8_t*>(out->records) + (size_t)first * stride;
     if (k) { so.story_running = nullptr; so.queue_running = nullptr; so.queue_max_priority = nullptr; so.global_running = nullptr; }
     Hook h{g, k};
-    if (count == 0) {   // an empty shard still takes part in the reductions, with zero contributions
-      bf_ctx* c = g->ctx[k];
-      c->last_eval_valid = true; c->last_eval_runs = 0; c->last_eval_layout = b->layout;
-    }
+    if (count == 0) g->ctx[k]->snap = {true, 0, b->layout, nullptr, nullptr};   // an empty shard still takes part in the reductions
     rcs[k] = schedule_host(g->ctx[k], &sb, runs ? runs + first : nullptr, t, &so, between, &h, k == 0);
     if (rcs[k] != BF_OK) errs[k] = bf_last_error(g->ctx[k]);
   };

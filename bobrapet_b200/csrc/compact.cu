@@ -10,7 +10,6 @@
 // own runs and emits through shared memory (deterministic order: bit-exact against the oracle's masks).
 #include <cuda_runtime.h>
 #include <stdint.h>
-#include <string.h>
 
 #include "../../include/bobrafrontier.h"
 #include "device_record.h"
@@ -162,10 +161,10 @@ __global__ void __launch_bounds__(CB) compact_emit(const CompactParams P) {
   if (blockIdx.x == gridDim.x - 1 && threadIdx.x == 0) {
     P.total[0] = base + btot;  // the batch's event count
     if (P.host_tail) {         // posted writes to pinned host memory; visible to the host once the stream has been synchronised
-      P.host_tail[0] = base + btot;
-      for (int k = 0; k < 4; ++k) P.host_tail[1 + k] = P.counts ? P.counts[k] : 0ull;
-      P.host_tail[5] = P.rejected ? (unsigned long long)*P.rejected : 0ull;
-      P.host_tail[6] = P.heads_done ? (unsigned long long)P.n_runs : P.total[1];   // (total[1]: every compact_heads block has finished)
+      P.host_tail->events = base + btot;
+      for (int k = 0; k < 4; ++k) P.host_tail->counts[k] = P.counts ? P.counts[k] : 0ull;
+      P.host_tail->rejected = P.rejected ? (unsigned long long)*P.rejected : 0ull;
+      P.host_tail->listed = P.heads_done ? (unsigned long long)P.n_runs : P.total[1];   // (total[1]: every compact_heads block has finished)
     }
     // leave the scratch the way the next tick expects it (no memset launches in the steady state): the listed-runs total
     // and the rejected-delta counter have been delivered
@@ -219,7 +218,7 @@ __global__ void __launch_bounds__(CB) touched_list(const TouchedParams P) {
     const unsigned long long carried = blocks_before(P.carry_sums) + P.carry_sums[blockIdx.x];
     if (threadIdx.x == 0) {
       *P.list_count = (uint32_t)min(base + btot, (unsigned long long)P.bound);
-      P.C.host_tail[8] = carried;
+      P.C.host_tail->carried = carried;
     }
   }
 }
@@ -280,12 +279,12 @@ __global__ void __launch_bounds__(CB) touched_emit(const TouchedParams P) {
     if (k < P.runs_cap) { P.out_runs[k] = r; P.out_head[k] = hw; }
   }
   if (blockIdx.x == gridDim.x - 1 && threadIdx.x == 0) {
-    unsigned long long* t = C.host_tail;   // pinned host memory: visible to the host once the stream has been synchronised
-    t[0] = base + btot;
-    for (int k = 0; k < 4; ++k) t[1 + k] = C.counts ? C.counts[k] : 0ull;
-    t[5] = C.rejected ? (unsigned long long)*C.rejected : 0ull;
-    t[6] = base_l + (tot >> 20);
-    t[7] = n;
+    ResultTail& t = *C.host_tail;   // pinned host memory: visible to the host once the stream has been synchronised
+    t.events = base + btot;
+    for (int k = 0; k < 4; ++k) t.counts[k] = C.counts ? C.counts[k] : 0ull;
+    t.rejected = C.rejected ? (unsigned long long)*C.rejected : 0ull;
+    t.listed = base_l + (tot >> 20);
+    t.evaluated = n;
     if (C.rejected) *const_cast<uint32_t*>(C.rejected) = 0u;   // delivered: clean for the next tick
   }
   const bool staged = btot <= STAGE_EVENTS;
@@ -312,7 +311,7 @@ cudaError_t launch_touched_compact(const TouchedParams& P, cudaStream_t stream) 
 // scratch: block_sums needs ceil(n / 512) u64; total[2] is zero on entry (the caller zeroes it once, compact_emit leaves it zeroed)
 cudaError_t launch_compact(const CompactParams& P, cudaStream_t stream) {
   if (P.n_runs == 0) {
-    if (P.host_tail) memset(P.host_tail, 0, 7 * sizeof(unsigned long long));   // pinned host memory: plain store (caller synchronised)
+    if (P.host_tail) *P.host_tail = ResultTail{};   // pinned host memory: plain store (caller synchronised)
     return cudaSuccess;
   }
   const uint32_t nb = (P.n_runs + CB - 1) / CB;

@@ -5,6 +5,7 @@
 
 #include <cuda_runtime.h>
 #include <stdint.h>
+#include <string.h>
 
 #include <algorithm>
 #include <map>
@@ -132,7 +133,12 @@ struct bf_ctx {
   static constexpr uint32_t kAccSlots = 256;
   DevBuf<unsigned long long> d_acc;
   uint32_t acc_seq = 0;
-  bf_counts* h_counts = nullptr;  // pinned landing zone for the counts block (a pageable target would make the copy synchronous)
+  // where a pass's small results land on the host, pinned (a pageable target would make a copy synchronous)
+  struct Pinned {
+    uint32_t word;         // a 4-byte device counter: rejected deltas where no compaction delivers them, migrated runs
+    bf::ResultTail tail;   // written by a compaction's last kernel; a pass without one copies its counts into tail.counts
+    bf_counts counts() const { return {tail.counts[0], tail.counts[1], tail.counts[2], tail.counts[3]}; }
+  }* pinned = nullptr;
   DevBuf<bf_expansion> d_exp;
   // compact results (bf_eval_compact / bf_resident_tick_compact)
   DevBuf<uint32_t> d_head;
@@ -161,13 +167,17 @@ struct bf_ctx {
   // retirements (bf_resident_retire): the new index of each vacated run
   DevBuf<uint32_t> d_retire;
 
-  // limiters (bf_schedule): what the last bf_eval left on the device + scratch
-  bool last_eval_valid = false;
-  uint32_t last_eval_runs = 0;
-  bf_layout last_eval_layout{};
+  // limiters (bf_schedule): the records the last pass evaluated (bf_eval's staging or a resident batch), read in place.  Cleared
+  // (valid = false) when a pass starts or a call changes those records (end_snapshot); assigned whole once a pass went through.
+  struct Snapshot {
+    bool valid = false;
+    uint32_t n_runs = 0;
+    bf_layout layout{};
+    const uint8_t *state = nullptr, *result = nullptr;
+    bool holds(const uint8_t* st) const { return valid && state == st; }
+    bool matches(uint32_t n, const bf_layout& L) const { return valid && n_runs == n && memcmp(&layout, &L, sizeof L) == 0; }
+  } snap;
   DevBuf<uint8_t> d_sched;                              // runs | records | tables, one allocation
-  const uint8_t* last_state = nullptr;                  // device records of the last evaluated batch (bf_eval or resident)
-  const uint8_t* last_result = nullptr;
   // resident batches (row f2)
   std::vector<Resident> resident;
   DevBuf<bf_delta> d_deltas;
@@ -237,7 +247,7 @@ struct Resident {
 
   uint32_t mark_touched() const { return epoch << 1; }
   uint32_t mark_must_list() const { return epoch << 1 | 1u; }
-  void end_snapshot(bf_ctx* c) const { if (c->last_state == d_state) c->last_eval_valid = false; }
+  void end_snapshot(bf_ctx* c) const { if (c->snap.holds(d_state)) c->snap.valid = false; }
   // the runs [first, end) were uploaded: the part at or above full_runs, merged with the ranges it touches
   void note_uploaded(uint32_t first, uint32_t end) {
     uint32_t lo = std::max(first, full_runs), hi = end;
@@ -322,10 +332,11 @@ int run_pass(bf_ctx* c, const bf_batch& b, const uint8_t* d_state, uint8_t* d_re
              unsigned long long* d_counts, cudaStream_t stream, const uint32_t* run_list = nullptr,
              const uint32_t* run_list_count = nullptr);
 void* pinned_dev(const void* p);
-uint32_t result_tail_of(const bf_layout& L);
+CompactParams compact_params(bf_ctx* c, const bf_layout& L, uint32_t n_runs, bool want_counts, bool want_rejected);
+int events_first(bf_ctx* c, uint16_t* events, uint64_t prev, uint64_t slack, uint64_t cap, bool posted, cudaStream_t s, uint64_t& first);
 int compact_prepare(bf_ctx* c, uint32_t n_runs, cudaStream_t s);
 unsigned long long* cblock_sums(bf_ctx* c, uint32_t which);
 int compact_enqueue(bf_ctx* c, const bf_layout& L, const uint8_t* d_result, const uint8_t* d_prev, uint32_t n_runs, bf_compact_out* out,
-                    cudaStream_t s, uint64_t* first_slice, bool with_rejected, bool heads_done = false);
-int compact_finish(bf_ctx* c, bf_compact_out* out, uint64_t first_slice);
+                    cudaStream_t s, uint64_t& first_slice, bool with_rejected, bool heads_done = false);
+int compact_finish(bf_ctx* c, bf_compact_out* out, uint64_t first_slice, uint64_t& prev);
 }  // namespace bf

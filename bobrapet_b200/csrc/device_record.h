@@ -146,6 +146,18 @@ struct KParams {
   uint32_t slot_groups;
 };
 
+// a pass's small results, posted to pinned host memory by the last block of a compaction (no separate small D2H copies)
+struct ResultTail {
+  unsigned long long events;      // events of the batch (touched ticks: of the listed runs)
+  unsigned long long counts[4];   // bf_counts of the pass, or zero
+  unsigned long long rejected;    // rejected deltas, or zero without a counter
+  unsigned long long listed;      // listed runs
+  unsigned long long evaluated;   // touched ticks: runs evaluated (touched_emit)
+  unsigned long long carried;     // touched ticks: touched runs in [n_scan, n_marks), left for a later tick (touched_list)
+};
+static_assert(offsetof(ResultTail, counts) == 8 && offsetof(ResultTail, rejected) == 40 && offsetof(ResultTail, listed) == 48 &&
+              offsetof(ResultTail, evaluated) == 56 && offsetof(ResultTail, carried) == 64, "ResultTail: word k at byte 8 * k");
+
 // compact.cu: result records -> one head word per run + 16-bit (step | kind << 10) events
 struct CompactParams {
   const uint8_t* result;
@@ -160,9 +172,7 @@ struct CompactParams {
   uint32_t zero_len;                 // entries of zero_sums
   uint32_t heads_done;               // the pass wrote head words and block totals itself (every run listed): no compact_heads
   unsigned long long* total;         // out: [0] events of the batch, [1] listed runs
-  // the pass's small results, written straight to pinned host memory by the last block (no separate small D2H copies):
-  // host_tail[0] = events, [1..4] = bf_counts, [5] = rejected deltas, [6] = listed runs
-  unsigned long long* host_tail;     // device-visible address of the pinned block, or nullptr
+  ResultTail* host_tail;             // device-visible address of the pinned tail (all but evaluated and carried), or nullptr
   const unsigned long long* counts;  // device bf_counts of the pass
   const uint32_t* rejected;          // device counter of rejected deltas, or nullptr
   uint32_t n_runs, words, result_stride, result_tail, off_ready, off_skip, off_fail, off_needs_cond, off_skip_dep;
@@ -172,8 +182,7 @@ struct CompactParams {
 // behind it.  Every scratch array is written before it is read in the same tick (no self-cleaning needed).
 struct TouchedParams {
   CompactParams C;               // result = the pass's new records (the batch's second buffer), prev_result = the batch's current
-                                 // records (brought up to date here); events, cap, host_tail, counts, rejected as for compact_emit;
-                                 // host_tail[7] = runs evaluated, [8] = touched runs in [n_scan, n_marks) (the list build)
+                                 // records (brought up to date here); events, cap, host_tail, counts, rejected as for compact_emit
   uint32_t* mark;                // [n_marks rounded up to 4] touch marks: touched when mark >> 1 > full_epoch, bit 0 = must list
   uint32_t full_epoch;
   uint32_t n_scan;               // the list takes the touched runs of [0, n_scan)

@@ -119,12 +119,12 @@ int bf_resident_apply(bf_ctx* c, uint32_t h, const bf_delta* deltas, uint32_t n)
   r->end_snapshot(c);
   r->pending += n;
   const int rc = resident_apply_async(c, r, deltas, n);
-  cudaError_t e = rc == BF_OK ? cudaMemcpyAsync(c->h_counts, c->d_rejected, 4, cudaMemcpyDeviceToHost, c->stream) : cudaSuccess;
+  cudaError_t e = rc == BF_OK ? cudaMemcpyAsync(&c->pinned->word, c->d_rejected, 4, cudaMemcpyDeviceToHost, c->stream) : cudaSuccess;
   const cudaError_t es = cudaStreamSynchronize(c->stream);  // the caller's delta buffer may be reused after return
   if (rc != BF_OK) return rc;
   if (e != cudaSuccess) return cuda_fail(c, e, "bf_resident_apply");
   if (es != cudaSuccess) return cuda_fail(c, es, "cudaStreamSynchronize");
-  const uint32_t rejected = *reinterpret_cast<const uint32_t*>(c->h_counts);
+  const uint32_t rejected = c->pinned->word;
   if (rejected) return fail(c, BF_EINVAL, std::to_string(rejected) + " delta(s) outside the record (run, index, code or absent field); the others were applied");
   return BF_OK;
 }
@@ -133,7 +133,7 @@ int bf_resident_apply(bf_ctx* c, uint32_t h, const bf_delta* deltas, uint32_t n)
 // the download of the previous chunk's result records (as bf_eval does for both directions)
 static int resident_tick_locked(bf_ctx* c, Resident* r, const bf_delta* deltas, uint32_t n_deltas, uint32_t n_runs, uint32_t flags,
                                 uint32_t max_iterations, void* result, bf_counts* counts, bf_compact_out* co = nullptr) {
-  c->last_eval_valid = false;
+  c->snap.valid = false;
   if (co && co->struct_size != sizeof(bf_compact_out)) return fail(c, BF_EINVAL, "bad bf_compact_out.struct_size");
   if (co && co->events_cap && !co->events) return fail(c, BF_EINVAL, "null events with a non-zero events_cap");
   if (n_runs > r->cap || (n_runs && !result && !co)) return fail(c, BF_EINVAL, "n_runs exceeds the resident batch / null result");
@@ -161,7 +161,9 @@ static int resident_tick_locked(bf_ctx* c, Resident* r, const bf_delta* deltas, 
   }
   if (chunks > 1)
     if (int rc = bf::ensure_pipe(c)) return rc;
-  uint32_t* h_rej = reinterpret_cast<uint32_t*>(c->h_counts + 1);  // second pinned slot: h_counts is 2 x bf_counts
+  // a compaction over runs delivers the rejected-delta counter in the pinned tail and clears it; otherwise a counter that may have
+  // counted lands in the pinned word and is zeroed before its next use
+  const bool tail_delivers = co && n_runs;
   auto body = [&]() -> int {
     if (int rc = resident_apply_async(c, r, deltas, n_deltas)) return rc;
     const bool may_fuse = co && chunks == 1 && !d_prev && !changed_only && !getenv("BF_NO_FUSED_HEADS");
@@ -190,12 +192,12 @@ static int resident_tick_locked(bf_ctx* c, Resident* r, const bf_delta* deltas, 
         BF_CUDA(c, cudaMemcpyAsync(static_cast<uint8_t*>(result) + lo * L.result_stride, r->d_result + lo * L.result_stride,
                                    (hi - lo) * L.result_stride, cudaMemcpyDeviceToHost, piped ? c->s_out : s));
     }
-    if (co) {   // counts and the rejected-delta counter travel with the compaction's tail block
-      if (int rc2 = bf::compact_enqueue(c, L, r->d_result, d_prev, n_runs, co, s, &first_slice, true, may_fuse && c->fused_done)) return rc2;
+    if (co) {
+      if (int rc2 = bf::compact_enqueue(c, L, r->d_result, d_prev, n_runs, co, s, first_slice, true, may_fuse && c->fused_done)) return rc2;
     } else {
-      BF_CUDA(c, cudaMemcpyAsync(c->h_counts, c->d_counts, sizeof(bf_counts), cudaMemcpyDeviceToHost, s));
-      BF_CUDA(c, cudaMemcpyAsync(h_rej, c->d_rejected, 4, cudaMemcpyDeviceToHost, s));
+      BF_CUDA(c, cudaMemcpyAsync(c->pinned->tail.counts, c->d_counts, sizeof(bf_counts), cudaMemcpyDeviceToHost, s));
     }
+    if (!tail_delivers && (!co || n_deltas)) BF_CUDA(c, cudaMemcpyAsync(&c->pinned->word, c->d_rejected, 4, cudaMemcpyDeviceToHost, s));
     return BF_OK;
   };
   const int rc = body();
@@ -212,19 +214,15 @@ static int resident_tick_locked(bf_ctx* c, Resident* r, const bf_delta* deltas, 
   if (rc != BF_OK) return rc;
   if (es != cudaSuccess) return cuda_fail(c, es, "cudaStreamSynchronize");
   if (int rc2 = r->full_tick_done(c, n_runs, flags, max_iterations, s)) return rc2;
-  if (co) {
-    c->cblock_clean = true; c->rejected_clean = true;   // the compaction's tail block delivered and cleared both
-    const unsigned long long* tail = reinterpret_cast<const unsigned long long*>(c->h_counts + 2);
-    memcpy(c->h_counts, tail + 1, sizeof(bf_counts));
-    *h_rej = (uint32_t)tail[5];
-  }
-  if (counts) *counts = *c->h_counts;
+  if (co) c->cblock_clean = true;   // the compaction's kernels leave their scratch zeroed
+  if (tail_delivers) c->rejected_clean = true;
+  if (counts) *counts = c->pinned->counts();
+  const uint64_t rejected = tail_delivers ? c->pinned->tail.rejected : c->pinned->word;
   c->stats.last_eval_chunks = chunks;
-  c->last_eval_valid = true; c->last_eval_runs = n_runs; c->last_eval_layout = L;
-  c->last_state = r->d_state; c->last_result = r->d_result;
+  c->snap = {true, n_runs, L, r->d_state, r->d_result};
   if (co)
-    if (int rc2 = bf::compact_finish(c, co, first_slice)) return rc2;
-  if (n_deltas && *h_rej) return fail(c, BF_EINVAL, std::to_string(*h_rej) + " delta(s) outside the record (run, index, code or absent field); the others were applied and the pass ran");
+    if (int rc2 = bf::compact_finish(c, co, first_slice, c->last_events)) return rc2;
+  if (n_deltas && rejected) return fail(c, BF_EINVAL, std::to_string(rejected) + " delta(s) outside the record (run, index, code or absent field); the others were applied and the pass ran");
   return BF_OK;
 }
 
@@ -258,11 +256,11 @@ static int touched_tick_locked(bf_ctx* c, Resident* r, const bf_delta* deltas, u
   if (n_runs > r->cap) return fail(c, BF_EINVAL, "n_runs exceeds the resident batch");
   if (n_deltas && !deltas) return fail(c, BF_EINVAL, "null deltas");
   BF_CUDA(c, cudaSetDevice(c->device));
+  bf_compact_out co{};   // the event list, as a compact tick returns it
+  co.struct_size = sizeof co; co.events = out->events; co.events_cap = out->events_cap;
   if (r->full_due(c, n_runs, flags, max_iterations)) {   // a plain compact tick: every run evaluated and listed, heads in run order
-    bf_compact_out co{};
-    co.struct_size = sizeof co; co.events = out->events; co.events_cap = out->events_cap;
     const int rc = resident_tick_locked(c, r, deltas, n_deltas, n_runs, flags, max_iterations, nullptr, counts, &co);
-    if (!c->last_eval_valid || c->last_state != r->d_state) return rc;   // no results (rejected deltas alone still deliver them)
+    if (!c->snap.holds(r->d_state)) return rc;   // no results (rejected deltas alone still deliver them)
     const uint32_t n = std::min(n_runs, out->runs_cap);
     if (n) BF_CUDA(c, cudaMemcpy(out->head, c->d_head, (size_t)n * 4, cudaMemcpyDeviceToHost));
     for (uint32_t i = 0; i < n; ++i) out->runs[i] = i;
@@ -270,7 +268,7 @@ static int touched_tick_locked(bf_ctx* c, Resident* r, const bf_delta* deltas, u
     return rc;
   }
 
-  c->last_eval_valid = false;
+  c->snap.valid = false;
   cudaStream_t s = c->stream;
   const bf_layout& L = r->L;
   const uint32_t bound = (uint32_t)std::min<uint64_t>(n_runs, r->pending + n_deltas);   // >= the touched runs below n_runs
@@ -291,22 +289,17 @@ static int touched_tick_locked(bf_ctx* c, Resident* r, const bf_delta* deltas, u
     if (int rc = c->d_truns.ensure(c, runs_n ? runs_n : 1)) return rc;
     if (int rc = c->d_thead.ensure(c, runs_n ? runs_n : 1)) return rc;
   }
-  unsigned long long* tail = reinterpret_cast<unsigned long long*>(c->h_counts + 2);   // 9 x u64 in the pinned block
   uint64_t first_slice = 0;
   auto body = [&]() -> int {
     if (int rc = resident_apply_async(c, r, deltas, n_deltas)) return rc;
     if (bound == 0) {   // nothing below n_runs can be touched: no launch beyond the scatter
-      if (n_deltas) BF_CUDA(c, cudaMemcpyAsync(tail + 5, c->d_rejected, 4, cudaMemcpyDeviceToHost, s));
+      if (n_deltas) BF_CUDA(c, cudaMemcpyAsync(&c->pinned->word, c->d_rejected, 4, cudaMemcpyDeviceToHost, s));
       return BF_OK;
     }
     bf::TouchedParams T{};
-    bf::CompactParams& P = T.C;
-    P.result = r->d_result_prev; P.prev_result = r->d_result;
-    P.events = p_events ? p_events : c->d_events; P.cap = cap;
-    P.host_tail = tail; P.counts = (flags & BF_EVAL_NO_COUNTS) ? nullptr : c->d_counts.p; P.rejected = c->d_rejected;
-    P.n_runs = bound; P.words = L.words; P.result_stride = L.result_stride; P.result_tail = bf::result_tail_of(L);
-    P.off_ready = L.off_ready; P.off_skip = L.off_skip;
-    P.off_fail = L.off_fail; P.off_needs_cond = L.off_needs_cond; P.off_skip_dep = L.off_skip_dep;
+    T.C = bf::compact_params(c, L, bound, !(flags & BF_EVAL_NO_COUNTS), true);
+    T.C.result = r->d_result_prev; T.C.prev_result = r->d_result;
+    T.C.events = p_events ? p_events : c->d_events; T.C.cap = cap;
     T.mark = r->d_mark; T.full_epoch = r->full_epoch; T.n_scan = n_runs; T.n_marks = r->cap; T.bound = bound;
     T.list = c->d_tlist + 1; T.list_count = c->d_tlist; T.pos_head = c->d_tpos_head;
     T.sums = c->d_tsums; T.sums_listed = c->d_tsums + nb; T.scan_sums = c->d_tsums + 2 * (size_t)nb;
@@ -324,12 +317,7 @@ static int touched_tick_locked(bf_ctx* c, Resident* r, const bf_delta* deltas, u
       BF_CUDA(c, cudaMemcpyAsync(out->runs, c->d_truns, (size_t)runs_n * 4, cudaMemcpyDeviceToHost, s));
       BF_CUDA(c, cudaMemcpyAsync(out->head, c->d_thead, (size_t)runs_n * 4, cudaMemcpyDeviceToHost, s));
     }
-    uint64_t guess = c->last_touched_events + c->last_touched_events / 32 + 1024;   // the previous touched tick's list + 3 %
-    if (guess > cap) guess = cap;
-    if (p_events) guess = 0;
-    if (guess) BF_CUDA(c, cudaMemcpyAsync(out->events, c->d_events, (size_t)guess * sizeof(uint16_t), cudaMemcpyDeviceToHost, s));
-    first_slice = p_events ? cap : guess;
-    return BF_OK;
+    return bf::events_first(c, out->events, c->last_touched_events, 1024, cap, p_events != nullptr, s, first_slice);
   };
   const int rc = body();
   const cudaError_t es = cudaStreamSynchronize(s);
@@ -338,24 +326,19 @@ static int touched_tick_locked(bf_ctx* c, Resident* r, const bf_delta* deltas, u
     if (rc != BF_OK) return rc;
     return cuda_fail(c, es, "cudaStreamSynchronize");
   }
-  bf_counts hc{};
-  uint64_t n_events = 0, listed = 0, evaluated = 0, rejected = 0;
-  if (bound == 0) {
-    rejected = n_deltas ? *reinterpret_cast<const uint32_t*>(tail + 5) : 0u;   // (the counter is zeroed before its next use)
+  bf::ResultTail& tail = c->pinned->tail;
+  uint64_t rejected = tail.rejected;
+  if (bound == 0) {   // no kernel ran: the counter is zeroed before its next use
+    rejected = n_deltas ? c->pinned->word : 0u;
+    tail = bf::ResultTail{};   // no kernel wrote the tail: compact_finish and the counts read nothing evaluated or listed
   } else {
-    n_events = tail[0]; memcpy(&hc, tail + 1, sizeof hc); rejected = tail[5]; listed = tail[6]; evaluated = tail[7];
-    r->pending = tail[8];       // every touched run below n_runs was evaluated: the ones above it are all that is left
-    c->rejected_clean = true;   // delivered and cleared by the emit kernel
+    r->pending = tail.carried;   // every touched run below n_runs was evaluated: the ones above it are all that is left
+    c->rejected_clean = true;    // delivered and cleared by the emit kernel
   }
-  const uint64_t have = std::min<uint64_t>(n_events, cap);
-  if (have > first_slice)
-    BF_CUDA(c, cudaMemcpy(out->events + first_slice, c->d_events + first_slice, (size_t)(have - first_slice) * sizeof(uint16_t),
-                          cudaMemcpyDeviceToHost));
-  c->last_touched_events = n_events;
-  out->full = 0; out->n_listed = (uint32_t)listed; out->n_evaluated = (uint32_t)evaluated; out->n_events = n_events;
-  if (counts) *counts = hc;
-  c->last_eval_valid = true; c->last_eval_runs = n_runs; c->last_eval_layout = L;
-  c->last_state = r->d_state; c->last_result = r->d_result;
+  if (int rc2 = bf::compact_finish(c, &co, first_slice, c->last_touched_events)) return rc2;
+  out->full = 0; out->n_listed = co.n_listed; out->n_evaluated = (uint32_t)tail.evaluated; out->n_events = co.n_events;
+  if (counts) *counts = c->pinned->counts();
+  c->snap = {true, n_runs, L, r->d_state, r->d_result};
   if (rejected) return fail(c, BF_EINVAL, std::to_string(rejected) + " delta(s) outside the record (run, index, code or absent field); the others were applied and the pass ran");
   return BF_OK;
 }
@@ -424,10 +407,10 @@ int bf_resident_migrate(bf_ctx* c, uint32_t h, bf_migration* m) {
   P.off_decision = L.off_decision; P.off_child = L.off_child; P.child_nibbles = L.child_nibbles;
   cudaError_t e = cudaMemcpyAsync(c->d_mig, blob.data(), bytes, cudaMemcpyHostToDevice, s);
   if (e == cudaSuccess) e = bf::launch_migrate(P, s);
-  if (e == cudaSuccess) e = cudaMemcpyAsync(c->h_counts, c->d_mig, 4, cudaMemcpyDeviceToHost, s);
+  if (e == cudaSuccess) e = cudaMemcpyAsync(&c->pinned->word, c->d_mig, 4, cudaMemcpyDeviceToHost, s);
   if (int rc = r->sync_in_place(c, e, "bf_resident_migrate")) return rc;
   c->stats.kernel_launches += m->n_runs ? 1 : 0;
-  m->migrated = *reinterpret_cast<const uint32_t*>(c->h_counts);
+  m->migrated = c->pinned->word;
   r->pending += m->migrated;   // the touched-list bound counts the migrated runs as it counts uploaded ones
   return BF_OK;
 }
