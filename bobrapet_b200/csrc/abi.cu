@@ -29,7 +29,7 @@ static int forced_format() {
 
 struct RecPlan {
   uint32_t off_col, off_planes, off_par, off_allow, rec_bytes, W, child_nibbles, ell, max_deg;
-  uint32_t ff[bf::FF_STRIDE];   // the topology's row of the fail-fast mask table
+  uint32_t ff[bf::FF_STRIDE];   // the topology's row of the cut table: fail-fast mask, then dependency floors
   std::vector<uint32_t> child_first, allow_off;
 };
 
@@ -86,14 +86,12 @@ int plan_record(const bf_topology& t, RecPlan& p, std::string& why, bool host_ka
   p.child_nibbles = round_up(nib, 8);
   p.W = (S + 31) / 32;
   memset(p.ff, 0, sizeof p.ff);
-  if (p.W <= bf::FF_STRIDE) {
-    bool main_only = true;
-    for (uint32_t i = 0; i < S && main_only; ++i) {
-      main_only = ((t.step_flags[i] & BF_SF_GROUP_MASK) >> BF_SF_GROUP_SHIFT) == BF_GROUP_MAIN;
-      if (!(t.step_flags[i] & BF_SF_ALLOW_FAILURE)) p.ff[i >> 5] |= 1u << (i & 31u);
-    }
-    if (!main_only) memset(p.ff, 0, sizeof p.ff);
+  bool main_only = p.W <= bf::FF_WORDS;
+  for (uint32_t i = 0; i < S && main_only; ++i) {
+    main_only = ((t.step_flags[i] & BF_SF_GROUP_MASK) >> BF_SF_GROUP_SHIFT) == BF_GROUP_MAIN;
+    if (!(t.step_flags[i] & BF_SF_ALLOW_FAILURE)) p.ff[i >> 5] |= 1u << (i & 31u);
   }
+  if (!main_only) memset(p.ff, 0, sizeof p.ff);
   uint32_t off = sizeof(bf::TopoHeader);
   // Row format (device_record.h): fixed-width rows of K = 2 / 4 entries (no row_ptr; unused entries = PAD) when no step
   // has more than K needs and the block is not larger than the CSR block it replaces, else CSR.
@@ -124,6 +122,15 @@ int plan_record(const bf_topology& t, RecPlan& p, std::string& why, bool host_ka
     off += round_up(2 * (S + 1), 16);
     p.off_col = off;
     off += round_up(2 * E + 8, 16);
+  }
+  // dependency floors (device_record.h): a step without needs is NODEP in byte-entry rows (never walked), walked otherwise
+  for (uint32_t w = 0; main_only && w < p.W; ++w) {
+    uint32_t fl = bf::FF_FLOOR_NONE;
+    for (uint32_t i = 32 * w; i < S && i < 32 * w + 32 && fl != 0; ++i) {
+      if (t.row_ptr[i + 1] == t.row_ptr[i]) { if (!bf::ell_has_nodep(p.ell)) fl = 0; continue; }
+      for (uint32_t e = t.row_ptr[i]; e < t.row_ptr[i + 1]; ++e) fl = std::min(fl, (uint32_t)t.col_idx[e] + 1u);
+    }
+    p.ff[bf::FF_WORDS + w] = fl;
   }
   p.off_planes = off;
   off += round_up(bf::plane_count(p.ell) * p.W * 4, 16);

@@ -115,7 +115,7 @@ struct bf_ctx {
   std::vector<bf::Slot> slots_host;
   DevBuf<bf::Slot> slots_dev;
   bool slots_dirty = true;
-  std::vector<uint32_t> ff_host;       // fail-fast masks, bf::FF_STRIDE words per slot (device_record.h), mirrored with the slots
+  std::vector<uint32_t> ff_host;       // cut table (fail-fast masks, dependency floors), bf::FF_STRIDE words per slot (device_record.h), mirrored with the slots
   DevBuf<uint32_t> ff_dev;             // capacity: slots_dev.cap rows
   uint32_t max_rec_bytes = 0;          // largest live record
   uint32_t max_rec_by_w[33] = {};      // ... among the topologies of W = ceil(S/32) words (a batch of layout.words = w stages only W <= w)

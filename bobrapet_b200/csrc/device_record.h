@@ -98,17 +98,26 @@ struct Slot {          // device slot table entry
 // bits 24-31 of Slot::meta (abi.cu writes them, the packed-lanes kernel reads them to stage only the rows it can walk)
 __host__ __device__ inline uint32_t slot_row_bytes(uint32_t ell) { return (ell != 0 && !(ell & ELL_PACK10)) ? ell_row_bytes(ell) : 0u; }
 static_assert(sizeof(Slot) == 16, "Slot must be 16 bytes");
-// Fail-fast mask table beside the slot table: FF_STRIDE words per slot id.  Word w holds the bits of word w of the main
-// steps without allowFailure, for a topology of at most 512 steps that has no compensation or finally step; every other
-// topology (and a dead slot) has an all-zero row.  A fail-fast run with a Failed step under its mask has no candidate step
-// in its pass, so the packed-lanes kernel stages none of its needs rows (the cut, frontier_pack.cu).
-constexpr uint32_t FF_STRIDE = 16;
+// Cut table beside the slot table: FF_STRIDE words per slot id, filled for a topology of at most FF_WORDS words (512
+// steps) that has no compensation or finally step; every other topology (and a dead slot) has an all-zero row.  The
+// packed-lanes kernel reads it to stage fewer needs rows (the cut, frontier_pack.cu).
+//   words 0 .. FF_WORDS - 1          fail-fast mask: word w holds the bits of word w of the main steps without allowFailure.
+//                                    A fail-fast run with a Failed step under its mask has no candidate step in its pass,
+//                                    so none of its rows are staged.
+//   words FF_WORDS .. FF_STRIDE - 1  dependency floor of word w: 1 + the smallest real dependency index of the steps of word
+//                                    w that are walked (PAD entries and NODEP steps do not count), or 0 ("never") when such
+//                                    a step has no real dependency, or FF_FLOOR_NONE when no step of the word is walked.  A
+//                                    run none of whose steps at or above floor_w is satisfied or failed cannot meet or fail
+//                                    a dependency of a candidate of word w, so that word is neither staged nor walked.
+constexpr uint32_t FF_WORDS = 16;
+constexpr uint32_t FF_STRIDE = 2 * FF_WORDS;
+constexpr uint32_t FF_FLOOR_NONE = 0xFFFFu;
 
 struct KParams {
   const uint8_t* state;
   uint8_t* result;
   const Slot* slots;
-  const uint32_t* ff_mask;      // [n_slots][FF_STRIDE] fail-fast masks (read by the packed-lanes kernel only)
+  const uint32_t* ff_mask;      // [n_slots][FF_STRIDE] cut table: fail-fast masks and dependency floors (packed-lanes kernel only)
   unsigned long long* counts;   // bf_counts (4 x u64) or nullptr
   // compact ticks whose pass is the packed-lanes kernel alone: the pass itself leaves every run's head word (summary | listed |
   // event count) and adds the counts to the per-512-run totals the emit kernel scans — no separate heads kernel

@@ -195,6 +195,7 @@ __global__ void __launch_bounds__(32 * PACK_MAX_WARPS, PACK_MIN_BLOCKS) frontier
   const uint32_t wq_mask = Wq == 32u ? FULL : ((1u << Wq) - 1u);
   const uint32_t gmask = wq_mask << (g << lg);
   const uint32_t Wmax = P.words;
+  constexpr bool FF = !CD;   // the fail-fast skip and the floor cut below
 
 #ifdef PACK_TRACE
   const unsigned long long tr_start = gtime();
@@ -220,6 +221,11 @@ __global__ void __launch_bounds__(32 * PACK_MAX_WARPS, PACK_MIN_BLOCKS) frontier
   const uint32_t st0_a = scratch_a;
   const uint32_t mfail_a = st0_a + R * st_stride;
   const uint32_t tab_a = mfail_a + 128u;
+  // !CD passes (no fix-up): the fix-up words of the NW warps hold the needed word of slot group sg (issue(); NG <= 32 NW)
+  // at word sg % 32 of warp sg / 32, an address recomputed from the parameters at each use (a register more spills)
+  auto need_a = [&](uint32_t sg) {
+    return ((groups_a + NG * (R * (P.state_stride + P.topo_buf_bytes)) + 255u) & ~255u) + (sg >> 5) * P.work_bytes + R * st_stride + (sg & 31u) * 4u;
+  };
 
   if (threadIdx.x < 5) blk_counts[threadIdx.x] = 0ull;   // four counters + the group ticket
   if (threadIdx.x < NG) {   // NG <= blockDim.x: the planner (abi.cu) gives a CTA no more slot groups than threads
@@ -244,7 +250,6 @@ __global__ void __launch_bounds__(32 * PACK_MAX_WARPS, PACK_MIN_BLOCKS) frontier
   // issue 0 (lq == 0) hold the group my warp will issue when it is done with the current one.
   const uint32_t GB = 32u >> (5 - lg);        // = Wq: issues per prologue batch
   const uint32_t lq = lane >> (5 - lg), lr = lane & (R - 1u);   // my pair inside a batch: issue lq, run lr
-  constexpr bool FF = !CD;   // the fail-fast skip of the cut below
   // A lane without a run keeps pf_sid all ones, so load_ent leaves its entry zero and issue() writes a dead marker.
   uint32_t pf_sid = 0xFFFFFFFFu, pf_rf = 0, pf_lo = 0, pf_hi = 0, pf_bytes = 0, pf_meta = 0;
   uint32_t pf_run = 0xFFFFFFFFu;   // LIST: my run of the group I shall issue (all ones: none)
@@ -264,16 +269,24 @@ __global__ void __launch_bounds__(32 * PACK_MAX_WARPS, PACK_MIN_BLOCKS) frontier
       }
     }
   };
-  // second link: the slot entry (address, bytes, meta).  From here on pf_sid is the slot whose fail-fast mask load_cut()
-  // reads, all ones for a run that is not fail-fast or whose group the host sets (stage I does not mark it).
+  // second link: the slot entry (address, bytes, meta).  From here on pf_sid is the slot whose cut-table row load_cut() reads,
+  // with SID_NO_FF for a run that is not fail-fast or whose group the host sets (stage I does not mark it), SID_NO_FLOOR for
+  // a topology-terminated run (condition (3) in stages.cuh) and SID_RT for a realtime one; all ones: no row (a run without a
+  // live slot, slot ids above SID_SLOT, passes with cond or decision codes).
+  constexpr uint32_t SID_NO_FF = 1u << 31, SID_NO_FLOOR = 1u << 30, SID_RT = 1u << 29, SID_SLOT = SID_RT - 1u;
   auto load_ent = [&]() {
     pf_lo = 0; pf_hi = 0; pf_bytes = 0; pf_meta = 0;
     if (pf_sid < P.n_slots) {
       const uint4 v = __ldg(reinterpret_cast<const uint4*>(P.slots + pf_sid));
       pf_lo = v.x; pf_hi = v.y; pf_bytes = v.z; pf_meta = v.w;
     }
-    if (!FF || (pf_rf & (BF_RF_FAIL_FAST | BF_RF_HOST_GROUP)) != BF_RF_FAIL_FAST) pf_sid = 0xFFFFFFFFu;
-    if (FF && pf_sid < P.n_slots) asm volatile("prefetch.global.L2 [%0];" ::"l"(P.ff_mask + (size_t)pf_sid * FF_STRIDE));
+    if (FF && pf_sid < P.n_slots && pf_sid <= SID_SLOT) {
+      asm volatile("prefetch.global.L2 [%0];" ::"l"(P.ff_mask + (size_t)pf_sid * FF_STRIDE));
+      pf_sid |= ((pf_rf & (BF_RF_FAIL_FAST | BF_RF_HOST_GROUP)) != BF_RF_FAIL_FAST ? SID_NO_FF : 0u) |
+                ((pf_rf & BF_RF_TOPOLOGY_TERMINATED) ? SID_NO_FLOOR : 0u) | ((pf_rf & BF_RF_REALTIME) ? SID_RT : 0u);
+    } else {
+      pf_sid = 0xFFFFFFFFu;
+    }
   };
   // The cut: a run's topology buffer receives its header and the rows from the run's first word that can hold a candidate
   // step on; the rows below stay whatever an earlier group left there.  Stage D and the cond-FAIL fix-up read the rows of
@@ -289,14 +302,21 @@ __global__ void __launch_bounds__(32 * PACK_MAX_WARPS, PACK_MIN_BLOCKS) frontier
   // µs per pipelined pass in three rounds: 52.3 - 52.5 without the test, 52.8 - 53.1 with it).
   // Passes without decision codes read neither T0, T1, T2 nor TS: a run that receives no rows then receives its planes from
   // AF on (rounded down to 16 B).
+  // The floor cut, also in !CD passes only: word w of a run is NEEDED when it can hold a candidate and its dependency floor
+  // (FF_STRIDE, device_record.h) is at most hs_p = 1 + the highest step with a TERMINAL code (or an RT_SAT code, realtime
+  // runs).  In any other word every dependency of a candidate lies at or above hs_p, on a step that is unsatisfied and not a
+  // failed dependency by condition (3) in stages.cuh, so the walk would find met = fd = 0 for every candidate: the producer stages the
+  // rows of the needed words lo .. hi only (with the planes a third copy when hi is not the last word) and leaves the group's
+  // needed words at need_a for the consumer, whose walk takes CAND of those words alone.  Should the stages ever break condition
+  // (3), this cut must go.
   constexpr uint32_t LUT_CAND_POSSIBLE = ~(BF_LUT_TERMINAL | BF_LUT_RUNNING_Q) & 0xFFFFu;   // codes 0, 9, 10, 14, 15
   constexpr uint32_t LUT_FAILED = BF_LUT_TERMINAL & ~BF_LUT_COMPLETED0;                       // codes 4, 5, 6, 7, 11, 12
   const bool trim_planes = P.off_decision == BF_OFF_NONE;
-  uint32_t cp0 = 0, cp1 = 0, cp2 = 0, cp3 = 0, ffm = 0;
-  // the phase words and fail-fast mask word of lane g * Wq + w for group t, whose slot entries the lanes of issue k hold
-  // (load_ent has run)
+  uint32_t cp0 = 0, cp1 = 0, cp2 = 0, cp3 = 0, ffm = 0, flr = 0;
+  // the phase words, fail-fast mask word and dependency floor (| SID_RT for a realtime run; 0 = never cut) of lane g * Wq + w
+  // for group t, whose slot entries the lanes of issue k hold (load_ent has run)
   auto load_cut = [&](uint32_t t, uint32_t k) {
-    cp0 = 0; cp1 = 0; cp2 = 0; cp3 = 0; ffm = 0;
+    cp0 = 0; cp1 = 0; cp2 = 0; cp3 = 0; ffm = 0; flr = 0;
     uint32_t r = ((blockIdx.x + t * gridDim.x) << (5 - lg)) + g;
     const bool mine = t < T && r < N && w < Wmax;
     if (mine) {
@@ -306,7 +326,9 @@ __global__ void __launch_bounds__(32 * PACK_MAX_WARPS, PACK_MIN_BLOCKS) frontier
     }
     if (!FF) return;
     const uint32_t sid = __shfl_sync(FULL, pf_sid, (k << (5 - lg)) + g);
-    if (mine && sid < P.n_slots) ffm = __ldg(P.ff_mask + (size_t)sid * FF_STRIDE + w);
+    const uint32_t* row = P.ff_mask + (size_t)(sid & SID_SLOT) * FF_STRIDE;   // a clear SID_NO_* bit: a live slot
+    if (mine && !(sid & SID_NO_FF)) ffm = __ldg(row + w);
+    if (mine && !(sid & SID_NO_FLOOR)) flr = __ldg(row + FF_WORDS + w) | (sid & SID_RT);
   };
   // issue the copies of group t into slot group `sg`, which thereby starts its use number `use`; the lanes of issue `k`
   // (lq == k) own its runs and hold their slot entries, load_cut(t, k) has been called
@@ -314,8 +336,14 @@ __global__ void __launch_bounds__(32 * PACK_MAX_WARPS, PACK_MIN_BLOCKS) frontier
     const uint32_t Sg = __shfl_sync(FULL, pf_meta, (k << (5 - lg)) + g) & 0xFFFFu;   // steps of run g
     const uint32_t cpw = w * 32u < Sg ? bmsk_clamp(0u, Sg - w * 32u) & plut<LUT_CAND_POSSIBLE>(cp0, cp1, cp2, cp3) : 0u;
     const uint32_t cand_b = __ballot_sync(FULL, cpw != 0);
-    const uint32_t ff_b = FF ? __ballot_sync(FULL, (plut<LUT_FAILED>(cp0, cp1, cp2, cp3) & ffm) != 0) : 0u;
-    const uint32_t cand_words = ((ff_b >> (lr << lg)) & wq_mask) ? 0u : (cand_b >> (lr << lg)) & wq_mask;   // of my run (issuing lanes)
+    uint32_t need_b = cand_b;   // bit g * Wq + w: word w of run g is staged (and walked)
+    if (FF) {
+      const uint32_t ff_b = __ballot_sync(FULL, (plut<LUT_FAILED>(cp0, cp1, cp2, cp3) & ffm) != 0);
+      const uint32_t bp = plut<BF_LUT_TERMINAL>(cp0, cp1, cp2, cp3) | (plut<BF_LUT_RT_SAT>(cp0, cp1, cp2, cp3) & (0u - ((flr >> 29) & 1u)));   // bit 29: SID_RT
+      const uint32_t hs_p = __reduce_max_sync(gmask, bp ? w * 32u + 32u - __clz(bp) : 0u);
+      need_b = __ballot_sync(FULL, cpw != 0 && (flr & 0xFFFFu) <= hs_p && (ff_b & gmask) == 0);
+    }
+    const uint32_t cand_words = (need_b >> (lr << lg)) & wq_mask;   // of my run (issuing lanes)
     if (t < T && lq == k) {
       const uint32_t buf = groups_a + sg * group_bytes;
       const uint32_t bar = bars + 8u * sg;
@@ -329,17 +357,22 @@ __global__ void __launch_bounds__(32 * PACK_MAX_WARPS, PACK_MIN_BLOCKS) frontier
       if (lr == 0) {
         if (!LIST) sbytes = min(R, N - first) * P.state_stride;   // the group's state records are adjacent: one copy
         sts_u32(armed_a + 4u * sg, use + 1u);          // published before my arrive: the previous use is over, this one is armed
+        if (FF) sts_u32(need_a(sg), need_b);           // likewise, as a marker header
       }
       // fixed-width rows (rb = row bytes per step; 0 for CSR and formats not cut: one copy of the whole record): the header,
-      // then the rows from the first word that can hold a candidate on.  A run without such a word receives the header and
-      // the planes, from AF when the pass reads no decision codes.  A run with rows keeps its two copies: splitting its
-      // rows from its planes would make three, and on H100 the extra copy per run cost more than the 96 B it saves.
+      // then the rows of the needed words lo .. hi (!CD; else from the first word that can hold a candidate on) and the
+      // planes, from AF when the pass reads no decision codes.  Up to the last word that is one copy, as is a run without
+      // rows (header and planes); a run whose hi is below its last word takes a third copy for the planes (on H100 the
+      // extra copy cost more than the 96 B of T0 - T2 it would save alone).
       const uint32_t Wr = ((pf_meta & 0xFFFFu) + 31u) >> 5, rb = ok ? pf_meta >> 24 : 0u;
       const uint32_t lo_word = cand_words ? __ffs(cand_words) - 1u : Wr;
+      const uint32_t hi_end = FF && cand_words ? 32u - __clz(cand_words) : Wr;   // one past the last word staged
       const uint32_t hdr = (uint32_t)sizeof(TopoHeader), rows_end = hdr + 32u * rb * Wr;   // rows_end = off_planes
-      uint32_t from = hdr + 32u * rb * lo_word;
-      if (rb && trim_planes && from == rows_end) from = (rows_end + PL_AF * 4u * Wr) & ~15u;
-      mbar_expect_tx(bar, (ok ? pf_bytes - (from - hdr) : 0u) + sbytes);
+      const uint32_t planes_from = trim_planes ? (rows_end + PL_AF * 4u * Wr) & ~15u : rows_end;
+      uint32_t from = hdr + 32u * rb * lo_word, mid = pf_bytes, rest = pf_bytes;   // copies [0, hdr), [from, mid), [rest, pf_bytes)
+      if (rb && from == rows_end) from = planes_from;
+      else if (rb && hi_end < Wr) { mid = hdr + 32u * rb * hi_end; rest = planes_from; }
+      mbar_expect_tx(bar, (ok ? pf_bytes - (from - hdr) - (rest - mid) : 0u) + sbytes);
       if (LIST) {
         if (sbytes) bulk_g2s(buf + lr * P.state_stride, P.state + (size_t)pf_run * P.state_stride, sbytes, bar);
       } else if (lr == 0) {
@@ -349,7 +382,8 @@ __global__ void __launch_bounds__(32 * PACK_MAX_WARPS, PACK_MIN_BLOCKS) frontier
         const uint8_t* src = reinterpret_cast<const uint8_t*>((uint64_t)pf_lo | ((uint64_t)pf_hi << 32));
         const uint32_t at = from != hdr ? from : 0u;
         if (at) bulk_g2s(tb, src, hdr, bar);
-        bulk_g2s(tb + at, src + at, pf_bytes - at, bar);
+        bulk_g2s(tb + at, src + at, mid - at, bar);
+        if (rest != mid) bulk_g2s(tb + rest, src + rest, pf_bytes - rest, bar);
       }
     }
   };
@@ -447,7 +481,10 @@ __global__ void __launch_bounds__(32 * PACK_MAX_WARPS, PACK_MIN_BLOCKS) frontier
     const RunClass rc = stage_bi<CD>(gmask, rflags, n_main, n_comp, n_final, AF, GM, G1, G2, p0, p1, p2, p3);
     uint32_t summary = rc.sum | rc.group;
     const DepClass dc = stage_dprep(rc, rflags, VALID, GM, G1, G2, NODEP, p0, p1, p2, p3);
-    const uint32_t U = dc.U, FD = dc.FD, CAND = dc.CAND;
+    const uint32_t U = dc.U, FD = dc.FD;
+    // the floor cut: the walk takes the words the producer staged (bit `lane` of the slot group's needed word); a word it
+    // left out has met = FREE, fd = 0
+    const uint32_t CAND = FF ? ((lds_u32(need_a(cur_sg)) >> lane) & 1u ? dc.CAND : 0u) : dc.CAND;
     // ------------- stage C: one status byte per step (bit0 unmet, bit1 failed-dep), all R runs -------------
     const bool any_fd = __any_sync(FULL, dc.skip_on_failed);           // some run of the group has a failed-dependency class
     const int my_fmt = fmt_of(ell, max_deg);

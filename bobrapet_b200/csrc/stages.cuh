@@ -10,7 +10,7 @@
 namespace bf {
 
 // ------------------------------------------------------------------ conditions the packed-lanes producer relies on
-// Any edit to stages G, I or the cond-FAIL fix-up below must keep both.
+// Any edit to stages G, I, D-prep or the cond-FAIL fix-up below must keep all three.
 //
 // (1) No stage of a single pass makes a candidate of a step whose INPUT code (15 read as 0) lies in TERMINAL ∪ RUNNING_Q:
 //     stage G rewrites only RUNNING sync steps, into 8 or a terminal code; stage I and the fix-up only set Skipped /
@@ -22,6 +22,12 @@ namespace bf {
 //     GM & ~COMPL & ~RUNQ & ~TERM Skipped.  With G1 = G2 = 0, GSEL is GM (CAND0 = GM minus what mark_ff just covered:
 //     empty) or the group is DONE (CAND0 = 0); the topology-terminated branch only adds Failed steps.  The producer stages
 //     none of such a run's rows (the fail-fast skip of the cut).
+// (3) In a pass without cond and decision codes, a run without BF_RF_TOPOLOGY_TERMINATED in a topology with G1 = G2 = 0
+//     that condition (2) does not exempt has every step that is satisfied or a failed dependency ((VALID & ~U) | FD) among
+//     the steps whose INPUT code is TERMINAL, or TERMINAL ∪ RT_SAT for a realtime run: without stage G and the fix-up,
+//     SAT ⊆ COMPLETED0 ∪ TERM ∪ RT_SAT and FD ⊆ TERM; mark_cs needs a compensation step, mark_ff fires only under
+//     condition (2), and only the topology-terminated branch sets other Failed codes.  The producer stages and the walk
+//     reads no rows of a word whose dependency floor lies above the highest such step (the floor cut, frontier_pack.cu).
 
 // ------------------------------------------------------------------ stage G: gate / sleep / wait sync
 // dag.go:1469-1533, 1235-1277, 1327-1437.  A RUNNING sync step (SYNC_T: sleep, wait, gate) takes the code its decision
