@@ -1,6 +1,7 @@
-// ctx.h — what the C ABI's translation units share (abi.cu: context, topology arena, batch evaluation; resident_abi.cu:
-// resident batches): bf_ctx and the records it keeps, the device-buffer owner, the error helpers, the kernel launchers and
-// the host helpers of a pass.  Private to the library: include/bobrafrontier.h is the public surface.
+// ctx.h — what the C ABI's translation units share (abi.cu: context, batch evaluation, limiters; topology.cu: topology
+// arena; resident_abi.cu: resident batches; group.cu: device groups): bf_ctx and the records it keeps, the device-buffer
+// owner, the error helpers, the kernel launchers and the host helpers of a pass.  Private to the library:
+// include/bobrafrontier.h is the public surface.
 #pragma once
 
 #include <cuda_runtime.h>
@@ -11,6 +12,7 @@
 #include <map>
 #include <mutex>
 #include <string>
+#include <tuple>
 #include <utility>
 #include <vector>
 
@@ -43,6 +45,29 @@ cudaError_t launch_validate(const Slot* slots, const uint32_t* slot_ids, uint32_
 inline uint32_t round_up(uint32_t v, uint32_t a) { return (v + a - 1) / a * a; }
 inline size_t round_up_sz(size_t v, size_t a) { return (v + a - 1) / a * a; }
 inline int fail(bf_ctx* c, int code, const std::string& msg);
+
+// The launch-shape knobs of a pass (A/B timing and the launch-shape tests, DESIGN.md), read at the start of every pass so
+// that a changed knob takes effect on the same ctx.  A number that is unset, 0 or not a number is 0: the planner's choice.
+struct Knobs {
+  bool general = false;    // BF_KERNEL=general: the one-run-per-warp kernel for every pass
+  bool blocked = false;    // BF_ASSIGN=blocked: each CTA takes a block of consecutive runs (KParams::run_blocked)
+  int warps = 0;           // BF_WARPS: warps per CTA of the packed-lanes kernel, else of the general kernel alone
+  int groups = 0;          // BF_GROUPS: slot groups of the packed-lanes ring (taken when it fits)
+  int stages = 0;          // BF_STAGES: ring stages of the general kernel
+  int blocks_per_sm = 0;   // BF_BLOCKS_PER_SM: at most this many general-kernel CTAs per SM
+  int wq = 0;              // BF_WQ: at least this many lanes per run in the packed-lanes kernel
+  int pack_ctas = 0;       // BF_PACK_CTAS: packed-lanes CTAs per SM, 1..4 (a build with -DPACK_MIN_BLOCKS; else 1)
+  auto tie() const { return std::tie(general, blocked, warps, groups, stages, blocks_per_sm, wq, pack_ctas); }
+  bool operator==(const Knobs& o) const { return tie() == o.tie(); }
+};
+
+// A compact tick's head words and per-block event totals, offered to its pass: a packed-lanes pass may write them itself
+// (device_record.h) and then sets done, so that the compaction skips its head kernel
+struct FusedHeads {
+  uint32_t* head;
+  unsigned long long* sums;
+  bool done;
+};
 }  // namespace bf
 
 // The owner of one device allocation: a pointer and a capacity in elements, freed by the destructor.  It converts to its
@@ -117,8 +142,7 @@ struct bf_ctx {
   bool slots_dirty = true;
   std::vector<uint32_t> ff_host;       // cut table (fail-fast masks, dependency floors), bf::FF_STRIDE words per slot (device_record.h), mirrored with the slots
   DevBuf<uint32_t> ff_dev;             // capacity: slots_dev.cap rows
-  uint32_t max_rec_bytes = 0;          // largest live record
-  uint32_t max_rec_by_w[33] = {};      // ... among the topologies of W = ceil(S/32) words (a batch of layout.words = w stages only W <= w)
+  uint32_t max_rec_by_w[33] = {};      // largest live record among the topologies of W = ceil(S/32) words (bf::largest_record)
   bool rec_max_dirty = false;          // a drop may have lowered the maxima: recomputed at the next plan
   uint32_t n_alive = 0;
   uint32_t n_with_parallel = 0;  // live topologies that have parallel steps
@@ -147,9 +171,6 @@ struct bf_ctx {
   // other one zeroed, so a pass that adds its runs' counts itself (fused heads, device_record.h) finds a clean buffer
   DevBuf<unsigned long long> d_cblock;
   uint32_t cblock_flip = 0;
-  // set by a compact tick around its run_pass: where a packed-lanes pass may leave head words and block totals; run_pass reports
-  // through fused_done whether it did
-  uint32_t* fuse_head = nullptr; unsigned long long* fuse_sums = nullptr; bool fused_done = false;
   uint64_t last_events = 0;                                          // events of the previous compact pass (sizes the first D2H)
   // scratch shared by both entry points
   DevBuf<uint32_t> d_exp_counts;
@@ -191,8 +212,8 @@ struct bf_ctx {
   // full and touched ticks keeps both
   struct Plan {
     uint32_t key_stride = 0, key_words = 0, key_rec = 0, key_variant = 0xFFFFFFFFu;
-    int key_knobs[3] = {0, 0, 0};   // BF_STAGES, BF_WARPS, BF_BLOCKS_PER_SM as last planned (0: unset)
-    uint32_t stages = 0, wpb = 0, per_sm = 0, occ2 = 0;
+    bf::Knobs key_knobs;   // as last planned
+    uint32_t stages = 0, wpb = 0, per_sm = 0, occ2 = 0, smem = 0;
   } plan[2];
 
   bf_stats stats{};
@@ -323,14 +344,18 @@ struct Resident {
   }
 };
 
-// host helpers of a pass, defined in abi.cu and used by resident_abi.cu too
 namespace bf {
-int ensure_pipe(bf_ctx* c);
+// the topology arena (topology.cu)
+int grow_arena(bf_ctx* c, size_t need_total);
 int sync_slots(bf_ctx* c, cudaStream_t stream);
+uint32_t largest_record(bf_ctx* c, uint32_t w);
+
+// host helpers of a pass, defined in abi.cu and used by resident_abi.cu too
+int ensure_pipe(bf_ctx* c);
 int check_layout(bf_ctx* c, const bf_layout& L);
 int run_pass(bf_ctx* c, const bf_batch& b, const uint8_t* d_state, uint8_t* d_result, bf_expansion* d_exp,
              unsigned long long* d_counts, cudaStream_t stream, const uint32_t* run_list = nullptr,
-             const uint32_t* run_list_count = nullptr);
+             const uint32_t* run_list_count = nullptr, FusedHeads* heads = nullptr);
 void* pinned_dev(const void* p);
 CompactParams compact_params(bf_ctx* c, const bf_layout& L, uint32_t n_runs, bool want_counts, bool want_rejected);
 int events_first(bf_ctx* c, uint16_t* events, uint64_t prev, uint64_t slack, uint64_t cap, bool posted, cudaStream_t s, uint64_t& first);
@@ -339,4 +364,12 @@ unsigned long long* cblock_sums(bf_ctx* c, uint32_t which);
 int compact_enqueue(bf_ctx* c, const bf_layout& L, const uint8_t* d_result, const uint8_t* d_prev, uint32_t n_runs, bf_compact_out* out,
                     cudaStream_t s, uint64_t& first_slice, bool with_rejected, bool heads_done = false);
 int compact_finish(bf_ctx* c, bf_compact_out* out, uint64_t first_slice, uint64_t& prev);
+
+// host-buffer evaluation and scheduling (abi.cu), which a device group (group.cu) runs once per shard
+int eval_host(bf_ctx* c, const bf_batch* b, bf_compact_out* co);
+// totals hook of a sharded schedule: called between the counting and the truncation kernels with the device totals
+struct SchedTotals { uint32_t* story_running; uint32_t* queue_running; int32_t* queue_maxprio; uint32_t* global_running; uint32_t ns, nq; };
+typedef int (*sched_between_fn)(void* user, const SchedTotals& t, cudaStream_t s);
+int schedule_host(bf_ctx* c, const bf_batch* b, const bf_sched_run* runs, const bf_sched_tables* t, bf_sched_out* out,
+                  sched_between_fn between, void* user, bool with_bases);
 }  // namespace bf

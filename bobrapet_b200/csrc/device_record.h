@@ -1,9 +1,9 @@
-// device_record.h — HBM layouts shared by the host packer (abi.cu) and the kernels.
+// device_record.h — HBM layouts shared by the host packer (topology.cu) and the kernels.
 //
 // A topology (one Story generation: needs-adjacency + static step flags) is one
 // contiguous, 16-byte aligned, 16-byte padded record in the arena so that a warp
 // stages it into shared memory with ONE cp.async.bulk (TMA) copy.  Two adjacency formats,
-// chosen per topology when it is uploaded (plan_record, abi.cu):
+// chosen per topology when it is uploaded (plan_record, topology.cu):
 //
 //   CSR (ell = 0)
 //   +0            TopoHeader (32 B)
@@ -95,7 +95,7 @@ struct Slot {          // device slot table entry
   uint32_t meta;       // S | P << 16 | row_bytes << 24 (P = number of parallel descs; row_bytes = bytes of one needs row of a
                        // byte-entry or u16 fixed-width record, whose rows of a 32-step word are row_bytes * 32 bytes, else 0)
 };
-// bits 24-31 of Slot::meta (abi.cu writes them, the packed-lanes kernel reads them to stage only the rows it can walk)
+// bits 24-31 of Slot::meta (topology.cu writes them, the packed-lanes kernel reads them to stage only the rows it can walk)
 __host__ __device__ inline uint32_t slot_row_bytes(uint32_t ell) { return (ell != 0 && !(ell & ELL_PACK10)) ? ell_row_bytes(ell) : 0u; }
 static_assert(sizeof(Slot) == 16, "Slot must be 16 bytes");
 // Cut table beside the slot table: FF_STRIDE words per slot id, filled for a topology of at most FF_WORDS words (512

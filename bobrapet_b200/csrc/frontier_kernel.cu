@@ -444,7 +444,7 @@ static KernelFn kernel_for(const KParams& P, uint32_t rb) {
   v |= (P.any_parallel != 0 ? 4u : 0u)            // CH: the join needs the child area; the expansion count needs only the descs
        | ((P.flags & BF_EVAL_FIXPOINT) ? 8u : 0u);  // FX
   if (P.run_list) {
-    // Run lists reach this kernel in two ways, both planned as the 16-warp build (RB = 0, abi.cu):
+    // Run lists reach this kernel in two ways, both planned as the 16-warp build (RB = 0, plan_general in abi.cu):
     //  - the second tier of a two-tier pass, after the packed-lanes kernel: a single pass (FX = 0) of a batch with some
     //    topology that has parallel steps (CH = 1) — indices 4-7;
     //  - a touched tick (bf_resident_tick_touched) that the packed-lanes kernel cannot take: S > 512, the device fixpoint or

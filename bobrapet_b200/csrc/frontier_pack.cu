@@ -215,7 +215,7 @@ __global__ void __launch_bounds__(32 * PACK_MAX_WARPS, PACK_MIN_BLOCKS) frontier
   // scratch (per warp, 256-byte aligned, work_bytes a multiple of 256): [status bytes: R x st_stride][fix-up fail words 128 B]
   // [walk table: R x 16 B].  st_stride = 32*Wq + 16 (the PAD byte of a full-width run with u16 rows lives in the + 16) except at
   // Wq = 8, where it is 256 so that every run's status bytes start on a 256-byte boundary (walk_items_k, AL; no topology of
-  // 8 words has u16 fixed-width rows: plan_record, abi.cu)
+  // 8 words has u16 fixed-width rows: plan_record, topology.cu)
   const uint32_t st_stride = Wq == 8u ? 256u : 32u * Wq + 16u;
   const uint32_t scratch_a = ((groups_a + NG * group_bytes + 255u) & ~255u) + warp * P.work_bytes;
   const uint32_t st0_a = scratch_a;
@@ -228,7 +228,7 @@ __global__ void __launch_bounds__(32 * PACK_MAX_WARPS, PACK_MIN_BLOCKS) frontier
   };
 
   if (threadIdx.x < 5) blk_counts[threadIdx.x] = 0ull;   // four counters + the group ticket
-  if (threadIdx.x < NG) {   // NG <= blockDim.x: the planner (abi.cu) gives a CTA no more slot groups than threads
+  if (threadIdx.x < NG) {   // NG <= blockDim.x: the planner (plan_pack, abi.cu) gives a CTA no more slot groups than threads
     mbar_init(bars + 8u * threadIdx.x, R);
     sts_u32(armed_a + 4u * threadIdx.x, 0u);
     fence_barrier_init();

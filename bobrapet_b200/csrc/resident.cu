@@ -82,7 +82,7 @@ cudaError_t launch_mark_runs(uint32_t* mark, uint32_t first, uint32_t n, uint32_
   return cudaGetLastError();
 }
 
-// Arena compaction (abi.cu): record i moves from src + moves[i].x to dst + moves[i].y (moves[i].z bytes, multiples of 16).
+// Arena compaction (topology.cu): record i moves from src + moves[i].x to dst + moves[i].y (moves[i].z bytes, multiples of 16).
 // One warp per record, 16 bytes per lane per trip.
 __global__ void __launch_bounds__(256) move_records(const uint8_t* __restrict__ src, uint8_t* __restrict__ dst, const ulonglong4* __restrict__ moves,
                                                     uint32_t n) {

@@ -167,9 +167,10 @@ static int resident_tick_locked(bf_ctx* c, Resident* r, const bf_delta* deltas, 
   auto body = [&]() -> int {
     if (int rc = resident_apply_async(c, r, deltas, n_deltas)) return rc;
     const bool may_fuse = co && chunks == 1 && !d_prev && !changed_only && !getenv("BF_NO_FUSED_HEADS");
+    bf::FusedHeads heads{};
     if (may_fuse) {
       if (int rc = bf::compact_prepare(c, n_runs, s)) return rc;
-      c->fuse_head = c->d_head; c->fuse_sums = bf::cblock_sums(c, c->cblock_flip);
+      heads = {c->d_head, bf::cblock_sums(c, c->cblock_flip), false};
     }
     bf_batch db{};
     db.struct_size = sizeof(bf_batch);
@@ -180,9 +181,9 @@ static int resident_tick_locked(bf_ctx* c, Resident* r, const bf_delta* deltas, 
     for (uint32_t k = 0; k < chunks; ++k) {
       const size_t lo = (size_t)n_runs * k / chunks, hi = (size_t)n_runs * (k + 1) / chunks;
       db.n_runs = (uint32_t)(hi - lo);
-      const int rc_pass = bf::run_pass(c, db, r->d_state + lo * L.state_stride, r->d_result + lo * L.result_stride, nullptr, c->d_counts, s);
-      c->fuse_head = nullptr; c->fuse_sums = nullptr;
-      if (rc_pass) return rc_pass;
+      if (int rc = bf::run_pass(c, db, r->d_state + lo * L.state_stride, r->d_result + lo * L.result_stride, nullptr, c->d_counts, s,
+                                nullptr, nullptr, may_fuse ? &heads : nullptr))
+        return rc;
       const bool piped = chunks > 1;
       if (piped) {
         BF_CUDA(c, cudaEventRecord(c->ev_k[k], s));
@@ -193,7 +194,7 @@ static int resident_tick_locked(bf_ctx* c, Resident* r, const bf_delta* deltas, 
                                    (hi - lo) * L.result_stride, cudaMemcpyDeviceToHost, piped ? c->s_out : s));
     }
     if (co) {
-      if (int rc2 = bf::compact_enqueue(c, L, r->d_result, d_prev, n_runs, co, s, first_slice, true, may_fuse && c->fused_done)) return rc2;
+      if (int rc2 = bf::compact_enqueue(c, L, r->d_result, d_prev, n_runs, co, s, first_slice, true, heads.done)) return rc2;
     } else {
       BF_CUDA(c, cudaMemcpyAsync(c->pinned->tail.counts, c->d_counts, sizeof(bf_counts), cudaMemcpyDeviceToHost, s));
     }
@@ -209,7 +210,6 @@ static int resident_tick_locked(bf_ctx* c, Resident* r, const bf_delta* deltas, 
   r->records_unknown();
   if (rc != BF_OK || es != cudaSuccess) {   // whatever the kernels left in the self-cleaning scratch is unknown: zero it before the next use
     c->cblock_clean = false; c->rejected_clean = false;
-    c->fuse_head = nullptr; c->fuse_sums = nullptr;
   }
   if (rc != BF_OK) return rc;
   if (es != cudaSuccess) return cuda_fail(c, es, "cudaStreamSynchronize");

@@ -47,7 +47,7 @@ def _lib():
 
 def child_first_of(branches) -> np.ndarray:
     """Nibble offsets of parallel descs in the child area: each desc starts 8-nibble aligned
-    (the rule bf_topology_put applies, bobrapet_b200/csrc/abi.cu plan_record)."""
+    (the rule bf_topology_put applies, bobrapet_b200/csrc/topology.cu plan_record)."""
     out, nib = [], 0
     for b in branches:
         nib = (nib + 7) // 8 * 8

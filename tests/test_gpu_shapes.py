@@ -16,7 +16,7 @@ pytestmark = pytest.mark.gpu
 ALL = A.F_COND | A.F_DECISION | A.F_ALL_OUT
 KNOBS = ("BF_KERNEL", "BF_TOPO_FORMAT", "BF_WARPS", "BF_GROUPS", "BF_STAGES", "BF_BLOCKS_PER_SM", "BF_WQ", "BF_ASSIGN",
          "BF_PACK_CTAS", "BF_E2E_CHUNKS")
-BUDGET = 227 * 1024          # shared memory a CTA may use (abi.cu)
+BUDGET = 227 * 1024          # shared memory a CTA may use (kSmemBudget, abi.cu)
 PACK_MAX_WARPS = 24
 
 
@@ -74,7 +74,7 @@ def _row_kinds(f, ts, slots, fmt=None):
 
 
 def _pack_plan(f, L, slots, warps=PACK_MAX_WARPS, groups=None, wq_min=0):
-    """the packed-lanes plan of abi.cu for a batch large enough that no CTA is short of groups: (R, warps, slot groups,
+    """the packed-lanes plan of abi.cu (plan_pack) for a batch large enough that no CTA is short of groups: (R, warps, slot groups,
     shared memory, bytes per group)"""
     wq = 1
     while wq < L.words:
