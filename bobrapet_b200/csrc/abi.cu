@@ -14,19 +14,6 @@ using bf::cuda_fail; using bf::fail; using bf::round_up; using bf::round_up_sz;
 // ---- host helpers of a pass, shared with resident_abi.cu (ctx.h) ----------------------------
 namespace bf {
 
-// copy / compute streams and events of the chunked pipelines (bf_eval, bf_resident_tick); created on first use
-int ensure_pipe(bf_ctx* c) {
-  if (c->pipe_ready) return BF_OK;
-  if (!c->s_in) BF_CUDA(c, cudaStreamCreateWithFlags(&c->s_in, cudaStreamNonBlocking));
-  if (!c->s_out) BF_CUDA(c, cudaStreamCreateWithFlags(&c->s_out, cudaStreamNonBlocking));
-  for (uint32_t k = 0; k < bf_ctx::kMaxChunks; ++k) {
-    if (!c->ev_in[k]) BF_CUDA(c, cudaEventCreateWithFlags(&c->ev_in[k], cudaEventDisableTiming));
-    if (!c->ev_k[k]) BF_CUDA(c, cudaEventCreateWithFlags(&c->ev_k[k], cudaEventDisableTiming));
-  }
-  c->pipe_ready = true;
-  return BF_OK;
-}
-
 int check_layout(bf_ctx* c, const bf_layout& L) {
   if (L.steps_max == 0 || L.steps_max > BF_MAX_STEPS) return fail(c, BF_EINVAL, "layout.steps_max out of range");
   if (L.words != (L.steps_max + 31) / 32) return fail(c, BF_EINVAL, "layout.words != ceil(steps_max/32)");
@@ -348,7 +335,7 @@ int compact_enqueue(bf_ctx* c, const bf_layout& L, const uint8_t* d_result, cons
   uint16_t* p_events = cap && !getenv("BF_NO_ZC_EVENTS") ? static_cast<uint16_t*>(pinned_dev(out->events)) : nullptr;
   P.events = p_events ? p_events : c->d_events;
   if (n_runs == 0) BF_CUDA(c, cudaStreamSynchronize(s));   // the empty case stores to the pinned block from the host
-  c->cblock_clean = false;   // until the call has gone through (resident_tick_locked / eval_host set it again after the sync)
+  c->cblock_clean = false;   // until the call has gone through (pass_end sets it again after the sync)
   BF_CUDA(c, bf::launch_compact(P, s));
   c->stats.kernel_launches += n_runs ? (heads_done ? 1 : 2) : 0;
   if (int rc = events_first(c, out->events, c->last_events, 4096, cap, p_events != nullptr, s, first_slice)) return rc;
@@ -367,6 +354,107 @@ int compact_finish(bf_ctx* c, bf_compact_out* out, uint64_t first_slice, uint64_
   out->n_listed = (uint32_t)tail.listed;
   prev = tail.events;
   return BF_OK;
+}
+
+// ---- the chunked pipeline of a pass between host buffers and the device: bf_eval, bf_eval_compact, each shard of bf_group_eval,
+// and the full resident ticks (resident_abi.cu), which keep their state on the device and so upload nothing ----
+// Large batches are cut into chunks of runs (runs are independent) so that the upload of chunk k+1, the pass of chunk k and the
+// download of chunk k-1 overlap on three streams: PCIe is full duplex and the pass itself is ~5x faster than either copy, so the
+// call costs about max(H2D, D2H) instead of their sum.
+
+// The chunk count of a call that moves `bytes` through the pipeline: one below 2 MiB, else bytes / per_chunk rounded, at least
+// at_least; BF_E2E_CHUNKS overrides it there (tools/e2e_sweep.py sweeps it).  Several chunks need the copy streams and events,
+// created on first use.
+int plan_chunks(bf_ctx* c, size_t bytes, size_t per_chunk, uint32_t at_least, uint32_t& chunks) {
+  chunks = 1;
+  if (bytes >= (2u << 20)) {
+    chunks = std::max((uint32_t)((bytes + per_chunk / 2) / per_chunk), at_least);
+    if (const char* e = getenv("BF_E2E_CHUNKS")) chunks = (uint32_t)atoi(e);
+    chunks = std::clamp(chunks, 1u, bf_ctx::kMaxChunks);
+  }
+  if (chunks == 1 || c->pipe_ready) return BF_OK;
+  if (!c->s_in) BF_CUDA(c, cudaStreamCreateWithFlags(&c->s_in, cudaStreamNonBlocking));
+  if (!c->s_out) BF_CUDA(c, cudaStreamCreateWithFlags(&c->s_out, cudaStreamNonBlocking));
+  for (uint32_t k = 0; k < bf_ctx::kMaxChunks; ++k) {
+    if (!c->ev_in[k]) BF_CUDA(c, cudaEventCreateWithFlags(&c->ev_in[k], cudaEventDisableTiming));
+    if (!c->ev_k[k]) BF_CUDA(c, cudaEventCreateWithFlags(&c->ev_k[k], cudaEventDisableTiming));
+  }
+  c->pipe_ready = true;
+  return BF_OK;
+}
+
+// The pass over db.n_runs runs as `chunks` passes on c->stream that add into c->d_counts.  h_state (optional): the host records,
+// each chunk's uploaded in front of its pass; h_result (optional): where each chunk's result records are downloaded behind its
+// pass.  The copies run on s_in / s_out when there are several chunks.  taper: chunk sizes shrink linearly (weights c, c-1, .., 1):
+// big early copies overlap best, a small last chunk leaves a short un-overlapped tail (kernel + download of that chunk).
+int chunked_pass(bf_ctx* c, bf_batch db, uint32_t chunks, bool taper, uint8_t* d_state, uint8_t* d_result, const uint8_t* h_state,
+                 uint8_t* h_result, bf_expansion* d_exp, FusedHeads* heads) {
+  const bf_layout& L = db.layout;
+  const size_t n = db.n_runs;
+  const bool piped = chunks > 1;
+  cudaStream_t s = c->stream, s_in = piped ? c->s_in : s, s_out = piped ? c->s_out : s;
+  for (uint32_t k = 0; k < chunks; ++k) {
+    size_t lo = n * k / chunks, hi = n * (k + 1) / chunks;
+    if (taper && piped) {
+      const uint64_t tot = (uint64_t)chunks * (chunks + 1) / 2;
+      auto cum = [&](uint32_t kk) { return (uint64_t)kk * chunks - (uint64_t)kk * (kk - 1) / 2; };  // sum of the first kk weights
+      lo = (size_t)(n * cum(k) / tot);
+      hi = (size_t)(n * cum(k + 1) / tot);
+    }
+    const size_t so = lo * L.state_stride, ro = lo * L.result_stride;
+    if (h_state) {
+      if (hi > lo) BF_CUDA(c, cudaMemcpyAsync(d_state + so, h_state + so, (hi - lo) * L.state_stride, cudaMemcpyHostToDevice, s_in));
+      if (piped) {
+        BF_CUDA(c, cudaEventRecord(c->ev_in[k], s_in));
+        BF_CUDA(c, cudaStreamWaitEvent(s, c->ev_in[k], 0));
+      }
+    }
+    db.n_runs = (uint32_t)(hi - lo);
+    if (int rc = run_pass(c, db, d_state + so, d_result + ro, d_exp, c->d_counts, s, nullptr, nullptr, heads)) return rc;
+    if (piped) {
+      BF_CUDA(c, cudaEventRecord(c->ev_k[k], s));
+      BF_CUDA(c, cudaStreamWaitEvent(s_out, c->ev_k[k], 0));
+    }
+    if (hi > lo && h_result)
+      BF_CUDA(c, cudaMemcpyAsync(h_result + ro, d_result + ro, (hi - lo) * L.result_stride, cudaMemcpyDeviceToHost, s_out));
+  }
+  return BF_OK;
+}
+
+// behind the chunks: the compaction of the records, whose last kernel posts the counts in the pinned tail, or the counts alone
+int pass_results(bf_ctx* c, const bf_layout& L, const uint8_t* d_result, const uint8_t* d_prev, uint32_t n_runs, bf_compact_out* co,
+                 uint64_t& first_slice, bool with_rejected, bool heads_done) {
+  if (co) return compact_enqueue(c, L, d_result, d_prev, n_runs, co, c->stream, first_slice, with_rejected, heads_done);
+  BF_CUDA(c, cudaMemcpyAsync(c->pinned->tail.counts, c->d_counts, sizeof(bf_counts), cudaMemcpyDeviceToHost, c->stream));
+  return BF_OK;
+}
+
+// The end of a pipelined call whose enqueueing returned rc: never return while a copy that touches the caller's buffers is still in
+// flight (the first error wins).  A failed call leaves the self-cleaning scratch in an unknown state, to be zeroed before its next
+// use; a compaction that went through has left its scratch zeroed.
+int pass_end(bf_ctx* c, int rc, uint32_t chunks, bool uploaded, bool compacted) {
+  cudaError_t es = cudaStreamSynchronize(c->stream);
+  if (chunks > 1) {
+    const cudaError_t ei = uploaded ? cudaStreamSynchronize(c->s_in) : cudaSuccess, eo = cudaStreamSynchronize(c->s_out);
+    if (es == cudaSuccess) es = ei != cudaSuccess ? ei : eo;
+  }
+  if (rc == BF_OK && es != cudaSuccess) rc = cuda_fail(c, es, "cudaStreamSynchronize");
+  if (rc != BF_OK) {
+    c->cblock_clean = false; c->rejected_clean = false;
+    return rc;
+  }
+  if (compacted) c->cblock_clean = true;
+  c->stats.last_eval_chunks = chunks;
+  return BF_OK;
+}
+
+// A pass went through: its records are what bf_schedule reads, and its counts and event list go to the caller.  prev: the
+// event count that sizes the first slice of the next list of this kind (compact_finish).
+int publish_pass(bf_ctx* c, uint32_t n_runs, const bf_layout& L, const uint8_t* d_state, const uint8_t* d_result, bf_counts* counts,
+                 bf_compact_out* co, uint64_t first_slice, uint64_t& prev) {
+  c->snap = {true, n_runs, L, d_state, d_result};
+  if (counts) *counts = c->pinned->counts();
+  return co ? compact_finish(c, co, first_slice, prev) : BF_OK;
 }
 
 }  // namespace bf
@@ -513,86 +601,28 @@ int eval_host(bf_ctx* c, const bf_batch* b, bf_compact_out* co) {
   const bool want_exp = (b->flags & BF_EVAL_EXPANSION) && b->expansion && b->expansion_cap;
   if (want_exp)
     if (int rc = c->d_exp.ensure(c, (size_t)b->expansion_cap)) return rc;
-  cudaStream_t s = c->stream;
-  // Large batches are cut into chunks of runs (runs are independent) so that the upload of chunk k+1, the
-  // kernel of chunk k and the download of chunk k-1 overlap: PCIe is full duplex and the pass itself is ~5x
-  // faster than either copy, so the call costs about max(H2D, D2H) instead of their sum.  Expansion needs a
-  // batch-wide scan and stays on the single-stream path.
+  // ~5.5 MB of state and results per chunk, at least two; expansion needs a batch-wide scan and stays on one stream
   uint32_t chunks = 1;
-  if (!want_exp && sbytes + rbytes >= (2u << 20)) {
-    // ~5.5 MB per chunk, at least two (tools/e2e_sweep.py sweeps the chunk count through BF_E2E_CHUNKS)
-    chunks = (uint32_t)((sbytes + rbytes + (11u << 18)) / (11u << 19));
-    if (chunks < 2) chunks = 2;
-    if (const char* e = getenv("BF_E2E_CHUNKS")) chunks = (uint32_t)atoi(e);
-    if (chunks > bf_ctx::kMaxChunks) chunks = bf_ctx::kMaxChunks;
-    if (chunks < 1) chunks = 1;
-  }
-  if (chunks > 1)
-    if (int rc = bf::ensure_pipe(c)) return rc;
+  if (int rc = bf::plan_chunks(c, want_exp ? 0 : sbytes + rbytes, 11u << 19, 2, chunks)) return rc;
   const char* shape_env = getenv("BF_E2E_SHAPE");
   const bool taper = shape_env && !strcmp(shape_env, "taper");
   uint64_t first_slice = 0;
   auto body = [&]() -> int {
-    BF_CUDA(c, cudaMemsetAsync(c->d_counts, 0, sizeof(bf_counts), s));
+    BF_CUDA(c, cudaMemsetAsync(c->d_counts, 0, sizeof(bf_counts), c->stream));
     bf_batch db = *b;
     db.flags &= ~(uint32_t)(BF_EVAL_COUNTS_SET | BF_EVAL_PIPELINED);   // bf_eval_device only: the chunks here add into one block
     if (!want_exp) db.flags &= ~BF_EVAL_EXPANSION;
-    const uint8_t* hs = static_cast<const uint8_t*>(b->state);
-    uint8_t* hr = static_cast<uint8_t*>(b->result);
-    for (uint32_t k = 0; k < chunks; ++k) {
-      // chunk sizes shrink linearly (weights c, c-1, .., 1) when BF_E2E_SHAPE=taper: big early copies overlap best,
-      // a small last chunk leaves a short un-overlapped tail (kernel + download of that chunk)
-      size_t lo = (size_t)b->n_runs * k / chunks, hi = (size_t)b->n_runs * (k + 1) / chunks;
-      if (taper && chunks > 1) {
-        const uint64_t tot = (uint64_t)chunks * (chunks + 1) / 2;
-        auto cum = [&](uint32_t kk) { return (uint64_t)kk * chunks - (uint64_t)kk * (kk - 1) / 2; };  // sum of the first kk weights
-        lo = (size_t)((uint64_t)b->n_runs * cum(k) / tot);
-        hi = (size_t)((uint64_t)b->n_runs * cum(k + 1) / tot);
-      }
-      const size_t so = lo * L.state_stride, ro = lo * L.result_stride;
-      const size_t sb = (hi - lo) * L.state_stride, rb = (hi - lo) * L.result_stride;
-      const bool piped = chunks > 1;
-      if (sb) BF_CUDA(c, cudaMemcpyAsync(c->d_state + so, hs + so, sb, cudaMemcpyHostToDevice, piped ? c->s_in : s));
-      if (piped) {
-        BF_CUDA(c, cudaEventRecord(c->ev_in[k], c->s_in));
-        BF_CUDA(c, cudaStreamWaitEvent(s, c->ev_in[k], 0));
-      }
-      db.n_runs = (uint32_t)(hi - lo);
-      if (int rc = bf::run_pass(c, db, c->d_state + so, c->d_result + ro, want_exp ? c->d_exp.p : nullptr, c->d_counts, s)) return rc;
-      if (piped) {
-        BF_CUDA(c, cudaEventRecord(c->ev_k[k], s));
-        BF_CUDA(c, cudaStreamWaitEvent(c->s_out, c->ev_k[k], 0));
-      }
-      if (rb && !co) BF_CUDA(c, cudaMemcpyAsync(hr + ro, c->d_result + ro, rb, cudaMemcpyDeviceToHost, piped ? c->s_out : s));
-    }
-    if (co) {   // counts travel with the compaction's tail block
-      if (int rc = bf::compact_enqueue(c, L, c->d_result, nullptr, b->n_runs, co, s, first_slice, false)) return rc;
-    } else {
-      BF_CUDA(c, cudaMemcpyAsync(c->pinned->tail.counts, c->d_counts, sizeof(bf_counts), cudaMemcpyDeviceToHost, s));
-    }
-    return BF_OK;
+    if (int rc = bf::chunked_pass(c, db, chunks, taper, c->d_state, c->d_result, static_cast<const uint8_t*>(b->state),
+                                  co ? nullptr : static_cast<uint8_t*>(b->result), want_exp ? c->d_exp.p : nullptr, nullptr))
+      return rc;
+    return bf::pass_results(c, L, c->d_result, nullptr, b->n_runs, co, first_slice, false, false);
   };
-  const int body_rc = body();
-  // never return while a copy that touches the caller's buffers is still in flight
-  cudaError_t e_sync = cudaStreamSynchronize(s);
-  if (chunks > 1) {
-    const cudaError_t e1 = cudaStreamSynchronize(c->s_in), e2 = cudaStreamSynchronize(c->s_out);
-    if (e_sync == cudaSuccess) e_sync = e1 != cudaSuccess ? e1 : e2;
-  }
-  if (body_rc != BF_OK || e_sync != cudaSuccess) c->cblock_clean = false;   // (the compaction scratch may hold a partial pass)
-  if (body_rc != BF_OK) return body_rc;
-  if (e_sync != cudaSuccess) return cuda_fail(c, e_sync, "cudaStreamSynchronize");
-  const bf_counts hc = c->pinned->counts();
-  if (co) c->cblock_clean = true;
-  c->stats.last_eval_chunks = chunks;
-  c->snap = {true, b->n_runs, L, c->d_state, c->d_result};
+  if (int rc = bf::pass_end(c, body(), chunks, true, co != nullptr)) return rc;
   if (want_exp) {
-    const uint64_t n = hc.expansion < b->expansion_cap ? hc.expansion : b->expansion_cap;
+    const uint64_t n = std::min<uint64_t>(c->pinned->counts().expansion, b->expansion_cap);
     if (n) BF_CUDA(c, cudaMemcpy(b->expansion, c->d_exp, (size_t)n * sizeof(bf_expansion), cudaMemcpyDeviceToHost));
   }
-  if (b->counts) *b->counts = hc;
-  if (co) return bf::compact_finish(c, co, first_slice, c->last_events);
-  return BF_OK;
+  return bf::publish_pass(c, b->n_runs, L, c->d_state, c->d_result, b->counts, co, first_slice, c->last_events);
 }
 
 }  // namespace bf

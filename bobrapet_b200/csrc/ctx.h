@@ -123,7 +123,8 @@ struct bf_ctx {
   int device = 0;
   int sm_count = 0;                    // SMs the frontier kernels spread over (device SMs minus the reserved ones)
   cudaStream_t stream = nullptr;
-  // bf_eval pipeline: H2D copies, kernels and D2H copies of consecutive run chunks overlap on three streams
+  // the chunked pipeline that bf_eval and the full resident ticks share (abi.cu): H2D copies (bf_eval only), kernels and D2H
+  // copies of consecutive run chunks overlap on three streams
   static constexpr uint32_t kMaxChunks = 32;
   cudaStream_t s_in = nullptr, s_out = nullptr;
   cudaEvent_t ev_in[kMaxChunks] = {}, ev_k[kMaxChunks] = {};
@@ -351,7 +352,6 @@ int sync_slots(bf_ctx* c, cudaStream_t stream);
 uint32_t largest_record(bf_ctx* c, uint32_t w);
 
 // host helpers of a pass, defined in abi.cu and used by resident_abi.cu too
-int ensure_pipe(bf_ctx* c);
 int check_layout(bf_ctx* c, const bf_layout& L);
 int run_pass(bf_ctx* c, const bf_batch& b, const uint8_t* d_state, uint8_t* d_result, bf_expansion* d_exp,
              unsigned long long* d_counts, cudaStream_t stream, const uint32_t* run_list = nullptr,
@@ -364,6 +364,16 @@ unsigned long long* cblock_sums(bf_ctx* c, uint32_t which);
 int compact_enqueue(bf_ctx* c, const bf_layout& L, const uint8_t* d_result, const uint8_t* d_prev, uint32_t n_runs, bf_compact_out* out,
                     cudaStream_t s, uint64_t& first_slice, bool with_rejected, bool heads_done = false);
 int compact_finish(bf_ctx* c, bf_compact_out* out, uint64_t first_slice, uint64_t& prev);
+// the chunked pipeline of bf_eval and the full resident ticks: chunk count, the chunks' passes and copies, the results behind
+// them, the synchronise that ends the call, and what a pass that went through publishes
+int plan_chunks(bf_ctx* c, size_t bytes, size_t per_chunk, uint32_t at_least, uint32_t& chunks);
+int chunked_pass(bf_ctx* c, bf_batch db, uint32_t chunks, bool taper, uint8_t* d_state, uint8_t* d_result, const uint8_t* h_state,
+                 uint8_t* h_result, bf_expansion* d_exp, FusedHeads* heads);
+int pass_results(bf_ctx* c, const bf_layout& L, const uint8_t* d_result, const uint8_t* d_prev, uint32_t n_runs, bf_compact_out* co,
+                 uint64_t& first_slice, bool with_rejected, bool heads_done);
+int pass_end(bf_ctx* c, int rc, uint32_t chunks, bool uploaded, bool compacted);
+int publish_pass(bf_ctx* c, uint32_t n_runs, const bf_layout& L, const uint8_t* d_state, const uint8_t* d_result, bf_counts* counts,
+                 bf_compact_out* co, uint64_t first_slice, uint64_t& prev);
 
 // host-buffer evaluation and scheduling (abi.cu), which a device group (group.cu) runs once per shard
 int eval_host(bf_ctx* c, const bf_batch* b, bf_compact_out* co);

@@ -110,6 +110,13 @@ static int resident_apply_async(bf_ctx* c, Resident* r, const bf_delta* deltas, 
   return BF_OK;
 }
 
+// the end of a call whose scatter rejected n deltas: the others were applied (and the call's pass ran over them)
+static int rejected_deltas(bf_ctx* c, uint64_t n, bool pass_ran) {
+  if (n == 0) return BF_OK;
+  return fail(c, BF_EINVAL, std::to_string(n) + " delta(s) outside the record (run, index, code or absent field); the others were applied" +
+                                (pass_ran ? " and the pass ran" : ""));
+}
+
 int bf_resident_apply(bf_ctx* c, uint32_t h, const bf_delta* deltas, uint32_t n) {
   auto [g, r] = lock_resident(c, h);
   if (!r) return BF_EINVAL;
@@ -124,13 +131,11 @@ int bf_resident_apply(bf_ctx* c, uint32_t h, const bf_delta* deltas, uint32_t n)
   if (rc != BF_OK) return rc;
   if (e != cudaSuccess) return cuda_fail(c, e, "bf_resident_apply");
   if (es != cudaSuccess) return cuda_fail(c, es, "cudaStreamSynchronize");
-  const uint32_t rejected = c->pinned->word;
-  if (rejected) return fail(c, BF_EINVAL, std::to_string(rejected) + " delta(s) outside the record (run, index, code or absent field); the others were applied");
-  return BF_OK;
+  return rejected_deltas(c, c->pinned->word, false);
 }
 
-// deltas (optional) + one pass + results, one synchronisation: the pass is cut into run chunks whose kernels overlap
-// the download of the previous chunk's result records (as bf_eval does for both directions)
+// deltas (optional) + one pass + results, one synchronisation: the pass goes through the chunked pipeline of bf_eval (abi.cu)
+// without its upload, the state being on the device already, so each chunk's pass overlaps the download of the chunk before
 static int resident_tick_locked(bf_ctx* c, Resident* r, const bf_delta* deltas, uint32_t n_deltas, uint32_t n_runs, uint32_t flags,
                                 uint32_t max_iterations, void* result, bf_counts* counts, bf_compact_out* co = nullptr) {
   c->snap.valid = false;
@@ -142,7 +147,6 @@ static int resident_tick_locked(bf_ctx* c, Resident* r, const bf_delta* deltas, 
   BF_CUDA(c, cudaSetDevice(c->device));
   cudaStream_t s = c->stream;
   const bf_layout& L = r->L;
-  const size_t rbytes = (size_t)n_runs * L.result_stride;
   const bool changed_only = co && (flags & BF_EVAL_CHANGED_ONLY);
   flags &= ~(uint32_t)BF_EVAL_CHANGED_ONLY;
   const uint8_t* d_prev = nullptr;
@@ -151,16 +155,10 @@ static int resident_tick_locked(bf_ctx* c, Resident* r, const bf_delta* deltas, 
     std::swap(r->d_result, r->d_result_prev);
     if (r->prev_valid && r->prev_runs == n_runs) d_prev = r->d_result_prev;
   }
+  // ~2 MB of result records per chunk; compact results stay on the device, so one chunk
   uint32_t chunks = 1;
+  if (int rc = bf::plan_chunks(c, co ? 0 : (size_t)n_runs * L.result_stride, 2u << 20, 1, chunks)) return rc;
   uint64_t first_slice = 0;
-  if (!co && rbytes >= (2u << 20)) {
-    chunks = (uint32_t)((rbytes + (1u << 20)) / (2u << 20));   // ~2 MB of result records per chunk
-    if (const char* e = getenv("BF_E2E_CHUNKS")) chunks = (uint32_t)atoi(e);
-    if (chunks > bf_ctx::kMaxChunks) chunks = bf_ctx::kMaxChunks;
-    if (chunks < 1) chunks = 1;
-  }
-  if (chunks > 1)
-    if (int rc = bf::ensure_pipe(c)) return rc;
   // a compaction over runs delivers the rejected-delta counter in the pinned tail and clears it; otherwise a counter that may have
   // counted lands in the pinned word and is zeroed before its next use
   const bool tail_delivers = co && n_runs;
@@ -175,55 +173,25 @@ static int resident_tick_locked(bf_ctx* c, Resident* r, const bf_delta* deltas, 
     bf_batch db{};
     db.struct_size = sizeof(bf_batch);
     db.flags = flags & ~(uint32_t)(BF_EVAL_VALIDATE | BF_EVAL_COUNTS_SET | BF_EVAL_PIPELINED); db.max_iterations = max_iterations; db.layout = L;
+    db.n_runs = n_runs;
     // one chunk: the pass overwrites the counts block itself (no memset in front of it); several chunks add into a zeroed block
     if (chunks == 1) db.flags |= BF_EVAL_COUNTS_SET;
     else BF_CUDA(c, cudaMemsetAsync(c->d_counts, 0, sizeof(bf_counts), s));
-    for (uint32_t k = 0; k < chunks; ++k) {
-      const size_t lo = (size_t)n_runs * k / chunks, hi = (size_t)n_runs * (k + 1) / chunks;
-      db.n_runs = (uint32_t)(hi - lo);
-      if (int rc = bf::run_pass(c, db, r->d_state + lo * L.state_stride, r->d_result + lo * L.result_stride, nullptr, c->d_counts, s,
-                                nullptr, nullptr, may_fuse ? &heads : nullptr))
-        return rc;
-      const bool piped = chunks > 1;
-      if (piped) {
-        BF_CUDA(c, cudaEventRecord(c->ev_k[k], s));
-        BF_CUDA(c, cudaStreamWaitEvent(c->s_out, c->ev_k[k], 0));
-      }
-      if (hi > lo && !co)
-        BF_CUDA(c, cudaMemcpyAsync(static_cast<uint8_t*>(result) + lo * L.result_stride, r->d_result + lo * L.result_stride,
-                                   (hi - lo) * L.result_stride, cudaMemcpyDeviceToHost, piped ? c->s_out : s));
-    }
-    if (co) {
-      if (int rc2 = bf::compact_enqueue(c, L, r->d_result, d_prev, n_runs, co, s, first_slice, true, heads.done)) return rc2;
-    } else {
-      BF_CUDA(c, cudaMemcpyAsync(c->pinned->tail.counts, c->d_counts, sizeof(bf_counts), cudaMemcpyDeviceToHost, s));
-    }
+    if (int rc = bf::chunked_pass(c, db, chunks, false, r->d_state, r->d_result, nullptr, static_cast<uint8_t*>(result), nullptr,
+                                  may_fuse ? &heads : nullptr))
+      return rc;
+    if (int rc = bf::pass_results(c, L, r->d_result, d_prev, n_runs, co, first_slice, true, heads.done)) return rc;
     if (!tail_delivers && (!co || n_deltas)) BF_CUDA(c, cudaMemcpyAsync(&c->pinned->word, c->d_rejected, 4, cudaMemcpyDeviceToHost, s));
     return BF_OK;
   };
-  const int rc = body();
-  cudaError_t es = cudaStreamSynchronize(s);
-  if (chunks > 1) {
-    const cudaError_t e2 = cudaStreamSynchronize(c->s_out);
-    if (es == cudaSuccess) es = e2;
-  }
+  const int rc = bf::pass_end(c, body(), chunks, false, co != nullptr);
   r->records_unknown();
-  if (rc != BF_OK || es != cudaSuccess) {   // whatever the kernels left in the self-cleaning scratch is unknown: zero it before the next use
-    c->cblock_clean = false; c->rejected_clean = false;
-  }
   if (rc != BF_OK) return rc;
-  if (es != cudaSuccess) return cuda_fail(c, es, "cudaStreamSynchronize");
   if (int rc2 = r->full_tick_done(c, n_runs, flags, max_iterations, s)) return rc2;
-  if (co) c->cblock_clean = true;   // the compaction's kernels leave their scratch zeroed
   if (tail_delivers) c->rejected_clean = true;
-  if (counts) *counts = c->pinned->counts();
   const uint64_t rejected = tail_delivers ? c->pinned->tail.rejected : c->pinned->word;
-  c->stats.last_eval_chunks = chunks;
-  c->snap = {true, n_runs, L, r->d_state, r->d_result};
-  if (co)
-    if (int rc2 = bf::compact_finish(c, co, first_slice, c->last_events)) return rc2;
-  if (n_deltas && rejected) return fail(c, BF_EINVAL, std::to_string(rejected) + " delta(s) outside the record (run, index, code or absent field); the others were applied and the pass ran");
-  return BF_OK;
+  if (int rc2 = bf::publish_pass(c, n_runs, L, r->d_state, r->d_result, counts, co, first_slice, c->last_events)) return rc2;
+  return rejected_deltas(c, n_deltas ? rejected : 0, true);
 }
 
 int bf_resident_eval(bf_ctx* c, uint32_t h, uint32_t n_runs, uint32_t flags, uint32_t max_iterations, void* result, bf_counts* counts) {
@@ -335,12 +303,9 @@ static int touched_tick_locked(bf_ctx* c, Resident* r, const bf_delta* deltas, u
     r->pending = tail.carried;   // every touched run below n_runs was evaluated: the ones above it are all that is left
     c->rejected_clean = true;    // delivered and cleared by the emit kernel
   }
-  if (int rc2 = bf::compact_finish(c, &co, first_slice, c->last_touched_events)) return rc2;
+  if (int rc2 = bf::publish_pass(c, n_runs, L, r->d_state, r->d_result, counts, &co, first_slice, c->last_touched_events)) return rc2;
   out->full = 0; out->n_listed = co.n_listed; out->n_evaluated = (uint32_t)tail.evaluated; out->n_events = co.n_events;
-  if (counts) *counts = c->pinned->counts();
-  c->snap = {true, n_runs, L, r->d_state, r->d_result};
-  if (rejected) return fail(c, BF_EINVAL, std::to_string(rejected) + " delta(s) outside the record (run, index, code or absent field); the others were applied and the pass ran");
-  return BF_OK;
+  return rejected_deltas(c, rejected, true);
 }
 
 int bf_resident_tick_touched(bf_ctx* c, uint32_t h, const bf_delta* deltas, uint32_t n_deltas, uint32_t n_runs, uint32_t flags,

@@ -5,7 +5,7 @@ import pytest
 
 from bobrapet_b200 import _abi as A
 from bobrapet_b200 import Frontier
-from bobrapet_b200.records import _unpack_planes, pack_state
+from bobrapet_b200.records import _unpack_planes, make_layout, pack_state
 from oracle import packed as PK
 from tests import randgen
 
@@ -144,6 +144,33 @@ def test_deltas_equal_full_upload(seed):
         out = fr.schedule(L, n, sched, [0], [0], [0])
         assert out["records"].shape[0] == n
         fr.resident_destroy(h)
+    finally:
+        fr.close()
+
+
+def test_tick_default_chunk_count(monkeypatch):
+    """without BF_E2E_CHUNKS, a dense tick whose result records pass 2 MiB is cut into one chunk per ~2 MiB of them (rounded) and
+    returns the oracle's records; a compact tick over the same batch keeps its results on the device and runs as one chunk"""
+    monkeypatch.delenv("BF_E2E_CHUNKS", raising=False)
+    rng = np.random.default_rng(6120)
+    fr = Frontier(0)
+    try:
+        ts = randgen.random_topologies(rng, 30, 30, 256, parallel=False)
+        slots = fr.put_topologies(ts)
+        n = int(3.6 * (2 << 20)) // make_layout(int(ts.S.max()), 0, ALL).result_stride
+        L, state, _ = randgen.random_state(rng, ts, slots, n, ALL, phase_mix="progress")
+        rbytes = n * L.result_stride
+        want_chunks = (rbytes + (1 << 20)) // (2 << 20)
+        assert L.off_child == A.OFF_NONE and want_chunks == 4
+        want, wcounts = PK.evaluate(PK.PackedTopologies(ts, slots), L, state, threads=8)
+        h = fr.resident_create(L, n)
+        fr.resident_upload(h, 0, state)
+        none = np.zeros(0, dtype=Frontier.DELTA_DTYPE)
+        got, counts = fr.resident_tick(h, L, n, none)
+        assert fr.stats()["last_eval_chunks"] == want_chunks
+        assert np.array_equal(got, want) and counts == wcounts
+        fr.resident_tick_compact(h, n, none, 1 << 22)
+        assert fr.stats()["last_eval_chunks"] == 1
     finally:
         fr.close()
 
