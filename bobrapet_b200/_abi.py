@@ -136,6 +136,17 @@ class Retire(C.Structure):
                 ("capacity", C.c_uint32), ("moves_from", C.c_void_p), ("moves_to", C.c_void_p), ("n_moves", C.c_uint32)]
 
 
+EXTENT_NO_RUN = 0xFFFFFFFF   # BF_EXTENT_NO_RUN: bf_extent.widest_run when no run needs any step
+
+
+class Extent(C.Structure):
+    _fields_ = [("struct_size", C.c_uint32), ("n_runs", C.c_uint32), ("steps_max", C.c_uint32), ("child_nibbles", C.c_uint32),
+                ("fields", C.c_uint32), ("widest_run", C.c_uint32), ("reserved", C.c_uint32 * 2)]
+
+    def as_dict(self):
+        return {n: getattr(self, n) for n in ("steps_max", "child_nibbles", "fields", "widest_run")}
+
+
 class SchedTables(C.Structure):
     _fields_ = [("struct_size", C.c_uint32), ("n_stories", C.c_uint32), ("n_queues", C.c_uint32), ("global_limit", C.c_int32),
                 ("global_running_base", C.c_uint32), ("story_limit", C.c_void_p), ("story_running_base", C.c_void_p),
@@ -185,6 +196,8 @@ SYMBOLS = [
     ("bf_resident_redrive", C.c_int, [C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_void_p, C.POINTER(C.c_uint32)]),
     ("bf_resident_reshape", C.c_int, [C.c_void_p, C.c_uint32, C.POINTER(Layout), C.c_uint32]),
     ("bf_resident_retire", C.c_int, [C.c_void_p, C.c_uint32, C.POINTER(Retire)]),
+    ("bf_resident_extent", C.c_int, [C.c_void_p, C.c_uint32, C.POINTER(Extent)]),
+    ("bf_resident_narrow", C.c_int, [C.c_void_p, C.c_uint32, C.POINTER(Layout), C.POINTER(Extent)]),
     ("bf_group_create", C.c_int, [C.POINTER(C.c_void_p), C.POINTER(C.c_int32), C.c_uint32, C.POINTER(Config)]),
     ("bf_group_destroy", None, [C.c_void_p]),
     ("bf_group_size", C.c_uint32, [C.c_void_p]),

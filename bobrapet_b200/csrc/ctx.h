@@ -36,6 +36,7 @@ cudaError_t launch_migrate(const MigrateParams& P, cudaStream_t stream);
 cudaError_t launch_redrive(const RedriveParams& P, cudaStream_t stream);
 cudaError_t launch_reshape(const ReshapeParams& P, cudaStream_t stream);
 cudaError_t launch_retire(const RetireParams& P, cudaStream_t stream);
+cudaError_t launch_extent(const ExtentParams& P, uint32_t sm_count, cudaStream_t stream);
 cudaError_t launch_schedule(const SchedParams& P, uint32_t sm_count, cudaStream_t stream, uint32_t phases = 3);
 cudaError_t launch_closure(const Slot* slots, const uint32_t* slot_ids, const uint32_t* starts, uint32_t n, uint32_t n_slots,
                            uint32_t words_out, uint32_t* masks, cudaStream_t stream);
@@ -188,6 +189,8 @@ struct bf_ctx {
   DevBuf<uint8_t> d_redrive;
   // retirements (bf_resident_retire): the new index of each vacated run
   DevBuf<uint32_t> d_retire;
+  // extents (bf_resident_extent / _narrow): the three words extent_runs reduces into
+  DevBuf<unsigned long long> d_extent;
 
   // limiters (bf_schedule): the records the last pass evaluated (bf_eval's staging or a resident batch), read in place.  Cleared
   // (valid = false) when a pass starts or a call changes those records (end_snapshot); assigned whole once a pass went through.
@@ -237,20 +240,21 @@ inline int cuda_fail(bf_ctx* c, cudaError_t e, const char* what) {
 
 // A device-resident batch (row f2), with the bookkeeping of touched ticks that tests/resident_model.py restates under the
 // same names.  Each field and the calls that change it:
-//   L, cap, d_state,   create, and reshape / retire (adopt).  d_state also: upload, deltas, migrate, redrive, retire.
-//   d_result           full ticks write it; a touched tick's list-mode compaction updates the runs it evaluated; reshape re-lays
-//                      it out; retire moves records with their runs.
+//   L, cap, d_state,   create, and reshape / retire / narrow (adopt).  d_state also: upload, deltas, migrate, redrive, retire.
+//   d_result           full ticks write it; a touched tick's list-mode compaction updates the runs it evaluated; reshape and
+//                      narrow re-lay it out; retire moves records with their runs.
 //   d_result_prev      result_prev allocates it on first use, adopt drops it; a changed-only tick swaps it with d_result and a
 //                      touched tick passes into it, so it is never read before a pass writes it.
 //   prev_valid, _runs  d_result holds a pass over the current state lineage of prev_runs runs: full_tick_done sets it; an upload
-//                      and records_unknown clear it; compact_to follows the run count.
+//                      and records_unknown clear it; compact_to follows the run count; narrowed clears it past its n_runs.
 //   d_mark, epoch,     deltas and redrives raise a run's mark to mark_touched() (epoch << 1); uploads, migrations and retires to
 //   full_epoch         mark_must_list() (| 1: listed even if unchanged).  full_tick_done records the ending epoch in full_epoch
 //                      and opens the next, so older marks are stale by comparison alone (no clear, no launch), and zeroes the
 //                      marks on epoch wrap.  A touched tick evaluates the runs marked after full_epoch and zeroes their marks.
-//   full_runs          runs of the last full tick (full_tick_done); compact_to clamps it.
+//   full_runs          runs of the last full tick (full_tick_done); compact_to and narrowed clamp it.
 //   need_full          the current records are not known to be complete: no tick yet, a failed call (records_unknown, a failed
-//                      touched tick), or a reshape that added decision planes or output fields.  full_tick_done clears it.
+//                      touched tick), a reshape that added decision planes or output fields, or a narrow that dropped decision
+//                      planes, the child area or output fields.  full_tick_done clears it.
 //   last_fixpoint, last_max_iter, slot_changes_seen: BF_EVAL_FIXPOINT, max_iterations and bf_ctx::slot_changes at the last
 //                      full tick.  A touched tick with other parameters, or after a slot drop or reuse, is full (full_due).
 //   pending            bound on the touched runs: those the last touched tick left at or above its n_runs, plus the deltas,
@@ -342,6 +346,24 @@ struct Resident {
       if (to != bf::kRetireNoMove) { note_uploaded(to, to + 1); ++pending; }
     if (prev_valid && prev_runs == N) prev_runs = m;
     else prev_valid = false;
+  }
+  // The runs below this bound whose current result record a touched tick may compare with: none while the next touched tick is
+  // full; else those of the last full tick, and the runs uploaded since in one range from there on that a touched tick has
+  // evaluated (a touched tick over more runs than full_runs is full unless such a range covers them).  Runs still marked
+  // "must list" are listed whatever their record holds, and records past the bound were never written by a pass or are not
+  // compared any more: neither limits a narrow.
+  uint32_t touched_baseline_runs() const {
+    if (need_full) return 0;
+    auto it = uploaded.find(full_runs);
+    return it == uploaded.end() ? full_runs : it->second;
+  }
+  // narrow re-laid every record at a smaller layout (adopt) after checking the result records of [0, n_runs) only: those above
+  // may have lost bits, so neither a full tick nor a changed-only baseline reaches past n_runs.  results_may_change: decision
+  // planes, the child area or an output field were dropped, which may change any run's result.
+  void narrowed(uint32_t n_runs, bool results_may_change) {
+    full_runs = std::min(full_runs, n_runs);
+    if (prev_runs > n_runs) prev_valid = false;
+    if (results_may_change) need_full = true;
   }
 };
 

@@ -275,6 +275,25 @@ struct RetireParams {
   uint32_t state_stride, result_stride;   // multiples of 16
 };
 
+// bf_resident_extent / _narrow (resident.cu): the smallest layout a batch's records and the topologies of its runs allow.  Each
+// extent is reduced into out[] as extent << 32 | ~index, so that one 64-bit atomicMax keeps the largest extent and the lowest
+// index that needs it.
+struct ExtentParams {
+  const uint8_t* state;          // [n_records][L.state_stride]
+  const uint8_t* result;         // [n_runs][L.result_stride]: the current result records
+  const uint32_t* mark;          // touch marks (Resident in ctx.h)
+  const Slot* slots;
+  uint32_t n_slots;
+  uint32_t n_records;            // state records scanned (the capacity)
+  uint32_t n_runs;               // runs whose slot counts, and whose result record counts when a later tick may compare with it:
+  uint32_t prev_runs;            //   run r < prev_runs (the changed-only baseline), or
+  uint32_t eval_runs;            //   run r < eval_runs (the touched baseline) not marked "must list" after full_epoch
+  uint32_t full_epoch;
+  bf_layout L;                   // the batch's layout
+  bf_layout R;                   // L with the result fields that do not count set to BF_OFF_NONE
+  unsigned long long* out;       // [3], zeroed by the caller: steps, child nibbles (both extent << 32 | ~index), BF_F_* input fields
+};
+
 // limiters.cu (rows a9 / f4)
 struct SchedParams {
   const uint8_t* state;

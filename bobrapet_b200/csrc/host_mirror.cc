@@ -197,6 +197,7 @@ struct bfh_batch {
   bool resident = false;
   uint32_t handle = 0;
   uint32_t uploaded = 0;                             // runs [0, uploaded) exist on the device
+  uint32_t evaluated = 0;                            // the result records of runs [0, evaluated) hold the last eval's results
   std::unordered_map<uint64_t, uint32_t> delta_at;   // (run, field, index) -> position in `deltas`
   std::vector<bf_delta> deltas;
   uint64_t delta_bytes_sent = 0, full_bytes_sent = 0;
@@ -456,6 +457,7 @@ int bfh_batch_remove_last_run(bfh_batch* b) {
   b->story_of_run.pop_back();
   --b->n;
   if (b->uploaded > b->n) b->uploaded = b->n;  // the slot's next occupant is uploaded as a full record
+  if (b->evaluated > b->n) b->evaluated = b->n;   // and has not been evaluated
   // pending deltas of the removed run must not land on the slot's next occupant (whose full record is uploaded first)
   if (b->resident) rewrite_deltas(b, [gone = b->n](bf_delta& d) { return d.run != gone; });
   return BF_OK;
@@ -545,6 +547,7 @@ int bfh_batch_eval(bfh_batch* b, uint32_t eval_flags, bf_counts* counts) {
     b->delta_at.clear();
     if (rc == BF_OK) rc = bf_resident_eval(b->ctx, b->handle, b->n, eval_flags & ~(uint32_t)BF_EVAL_EXPANSION, 0, b->rec.result, counts);
     if (rc != BF_OK) b->err = bf_last_error(b->ctx);
+    b->evaluated = rc == BF_OK ? b->n : 0;
     return rc;
   }
   bf_batch bb{};
@@ -553,6 +556,7 @@ int bfh_batch_eval(bfh_batch* b, uint32_t eval_flags, bf_counts* counts) {
   bb.state = b->rec.state; bb.result = b->rec.result; bb.counts = counts;
   const int rc = bf_eval(b->ctx, &bb);
   if (rc != BF_OK) b->err = bf_last_error(b->ctx);
+  b->evaluated = rc == BF_OK ? b->n : 0;
   return rc;
 }
 
@@ -782,10 +786,38 @@ int bfh_batch_redrive(bfh_batch* b, const uint32_t* runs, const int32_t* steps, 
 }
 
 // Plane field of a record re-laid from `from_off` (Wo words per plane) to `to_off` (Wn words per plane, zeroed): each plane
-// keeps its old words, the words above them stay 0; a field the old layout lacks stays 0.
+// keeps its low min(Wn, Wo) words, the words above them stay 0; a field either layout lacks stays 0 / is dropped.
 static void relay_planes(uint8_t* dst, const uint8_t* src, uint32_t to_off, uint32_t from_off, uint32_t planes, uint32_t Wn, uint32_t Wo) {
   if (to_off == BF_OFF_NONE || from_off == BF_OFF_NONE) return;
-  for (uint32_t p = 0; p < planes; ++p) memcpy(dst + to_off + (size_t)p * Wn * 4, src + from_off + (size_t)p * Wo * 4, (size_t)Wo * 4);
+  const size_t w = std::min(Wn, Wo);
+  for (uint32_t p = 0; p < planes; ++p) memcpy(dst + to_off + (size_t)p * Wn * 4, src + from_off + (size_t)p * Wo * 4, w * 4);
+}
+
+static uint32_t child_area_bytes(const bf_layout& L) { return L.off_child == BF_OFF_NONE ? 0u : ((L.child_nibbles + 1) / 2 + 3) / 4 * 4; }
+
+// The mirror's state and result records re-laid from F to T into nr (zeroed), as bf_resident_reshape / _narrow re-lay the
+// device's: the headers kept, each plane and mask its low words, the child area its low bytes.
+static void relay_records(const bfh_batch* b, HostRecords& nr, const bf_layout& F, const bf_layout& T) {
+  const uint32_t Wn = T.words, Wo = F.words;
+  for (uint32_t r = 0; r < b->cap; ++r) {
+    const uint8_t* s = b->rec.state + (size_t)r * F.state_stride;
+    uint8_t* d = nr.state + (size_t)r * T.state_stride;
+    memcpy(d, s, sizeof(bf_run_header));
+    relay_planes(d, s, T.off_phase, F.off_phase, 4, Wn, Wo);
+    relay_planes(d, s, T.off_cond, F.off_cond, 2, Wn, Wo);
+    relay_planes(d, s, T.off_decision, F.off_decision, 2, Wn, Wo);
+    if (F.off_child != BF_OFF_NONE && T.off_child != BF_OFF_NONE)
+      memcpy(d + T.off_child, s + F.off_child, std::min(child_area_bytes(F), child_area_bytes(T)));
+    s = b->rec.result + (size_t)r * F.result_stride;
+    d = nr.result + (size_t)r * T.result_stride;
+    memcpy(d, s, sizeof(bf_result_header));
+    relay_planes(d, s, T.off_ready, F.off_ready, 1, Wn, Wo);
+    relay_planes(d, s, T.off_skip, F.off_skip, 1, Wn, Wo);
+    relay_planes(d, s, T.off_fail, F.off_fail, 1, Wn, Wo);
+    relay_planes(d, s, T.off_needs_cond, F.off_needs_cond, 1, Wn, Wo);
+    relay_planes(d, s, T.off_skip_dep, F.off_skip_dep, 1, Wn, Wo);
+    relay_planes(d, s, T.off_phase_out, F.off_phase_out, 4, Wn, Wo);
+  }
 }
 
 int bfh_batch_reshape(bfh_batch* b, uint32_t steps_max, uint32_t child_nibbles, uint32_t fields, uint32_t capacity) {
@@ -807,27 +839,88 @@ int bfh_batch_reshape(bfh_batch* b, uint32_t steps_max, uint32_t child_nibbles, 
     const int rc = bf_resident_reshape(b->ctx, b->handle, &T, capacity);
     if (rc != BF_OK) { b->err = bf_last_error(b->ctx); return rc; }
   }
-  const uint32_t Wn = T.words, Wo = F.words;
-  for (uint32_t r = 0; r < b->cap; ++r) {
-    const uint8_t* s = b->rec.state + (size_t)r * F.state_stride;
-    uint8_t* d = nr.state + (size_t)r * T.state_stride;
-    memcpy(d, s, sizeof(bf_run_header));
-    relay_planes(d, s, T.off_phase, F.off_phase, 4, Wn, Wo);
-    relay_planes(d, s, T.off_cond, F.off_cond, 2, Wn, Wo);
-    relay_planes(d, s, T.off_decision, F.off_decision, 2, Wn, Wo);
-    if (F.off_child != BF_OFF_NONE) memcpy(d + T.off_child, s + F.off_child, ((F.child_nibbles + 1) / 2 + 3) / 4 * 4);
-    s = b->rec.result + (size_t)r * F.result_stride;
-    d = nr.result + (size_t)r * T.result_stride;
-    memcpy(d, s, sizeof(bf_result_header));
-    relay_planes(d, s, T.off_ready, F.off_ready, 1, Wn, Wo);
-    relay_planes(d, s, T.off_skip, F.off_skip, 1, Wn, Wo);
-    relay_planes(d, s, T.off_fail, F.off_fail, 1, Wn, Wo);
-    relay_planes(d, s, T.off_needs_cond, F.off_needs_cond, 1, Wn, Wo);
-    relay_planes(d, s, T.off_skip_dep, F.off_skip_dep, 1, Wn, Wo);
-    relay_planes(d, s, T.off_phase_out, F.off_phase_out, 4, Wn, Wo);
-  }
+  relay_records(b, nr, F, T);
   b->rec.swap(nr);
   b->L = T; b->cap = capacity;
+  return BF_OK;
+}
+
+// steps needed by plane word w holding v: one past its highest set bit
+static uint32_t word_extent(uint32_t w, uint32_t v) { return v ? 32u * w + 32u - (uint32_t)__builtin_clz(v) : 0u; }
+
+int bfh_batch_narrow(bfh_batch* b, uint32_t steps_max, uint32_t child_nibbles, uint32_t fields) {
+  if (!b) return BF_EINVAL;
+  bf_layout T;
+  if (bf_layout_init(&T, steps_max, child_nibbles, fields) != BF_OK) { b->err = "steps_max out of range"; return BF_EINVAL; }
+  const bf_layout F = b->L;
+  if (T.steps_max > F.steps_max || (T.fields & ~F.fields) ||
+      (F.off_child != BF_OFF_NONE && T.off_child != BF_OFF_NONE && T.child_nibbles > F.child_nibbles)) {
+    b->err = "a narrow only shrinks the layout (steps_max, fields, child_nibbles)";
+    return BF_EINVAL;
+  }
+  if (memcmp(&F, &T, sizeof T) == 0) return BF_OK;
+  // the extent of bf_resident_narrow over the mirror's own records, the stories of its runs and the result records of the runs
+  // the last eval evaluated
+  uint32_t steps = 0, child = 0, in_fields = 0;
+  const uint32_t W = F.words;
+  for (uint32_t r = 0; r < b->cap; ++r) {
+    const uint8_t* rec = b->rec.state + (size_t)r * F.state_stride;
+    auto planes = [&](uint32_t off, uint32_t n, uint32_t field) {
+      if (off == BF_OFF_NONE) return;
+      const uint32_t* p = reinterpret_cast<const uint32_t*>(rec + off);
+      for (uint32_t k = 0; k < n * W; ++k)
+        if (p[k]) { steps = std::max(steps, word_extent(k % W, p[k])); in_fields |= field; }
+    };
+    planes(F.off_phase, 4, 0);
+    planes(F.off_cond, 2, BF_F_COND);
+    planes(F.off_decision, 2, BF_F_DECISION);
+    for (uint32_t i = 0; F.off_child != BF_OFF_NONE && i < F.child_nibbles; ++i)
+      if ((rec[F.off_child + i / 2] >> ((i & 1u) * 4u)) & 0xFu) { child = std::max(child, i + 1); in_fields |= BF_F_CHILD; }
+    if (r >= b->n) continue;
+    steps = std::max(steps, (uint32_t)b->story_of_run[r]->flags.size());
+    child = std::max(child, b->story_of_run[r]->child_nibbles);
+    if (r >= b->evaluated) continue;   // a run added since the last eval has no results yet
+    const uint8_t* res = b->rec.result + (size_t)r * F.result_stride;
+    const std::pair<uint32_t, uint32_t> masks[] = {{F.off_ready, 1}, {F.off_skip, 1}, {T.off_fail != BF_OFF_NONE ? F.off_fail : BF_OFF_NONE, 1},
+                                                   {T.off_needs_cond != BF_OFF_NONE ? F.off_needs_cond : BF_OFF_NONE, 1},
+                                                   {T.off_skip_dep != BF_OFF_NONE ? F.off_skip_dep : BF_OFF_NONE, 1},
+                                                   {T.off_phase_out != BF_OFF_NONE ? F.off_phase_out : BF_OFF_NONE, 4}};
+    for (const auto& m : masks) {
+      if (m.first == BF_OFF_NONE) continue;
+      const uint32_t* p = reinterpret_cast<const uint32_t*>(res + m.first);
+      for (uint32_t k = 0; k < m.second * W; ++k) steps = std::max(steps, word_extent(k % W, p[k]));
+    }
+  }
+  const uint32_t placed = (T.off_cond != BF_OFF_NONE ? BF_F_COND : 0u) | (T.off_decision != BF_OFF_NONE ? BF_F_DECISION : 0u) |
+                          (T.off_child != BF_OFF_NONE ? BF_F_CHILD : 0u);
+  if (steps > T.steps_max) { b->err = "the batch needs steps_max " + std::to_string(steps); return BF_EINVAL; }
+  if (T.off_child != BF_OFF_NONE && child > T.child_nibbles) { b->err = "the batch needs child_nibbles " + std::to_string(child); return BF_EINVAL; }
+  if (in_fields & ~placed) { b->err = "the new layout drops an input field holding a non-default code"; return BF_EINVAL; }
+  for (const bf_delta& d : b->deltas) {   // a pending delta must still have its place: none is dropped
+    const bool fits = d.field == BF_DELTA_PHASE ? d.index < T.steps_max
+                      : d.field == BF_DELTA_COND ? T.off_cond != BF_OFF_NONE && d.index < T.steps_max
+                      : d.field == BF_DELTA_DECISION ? T.off_decision != BF_OFF_NONE && d.index < T.steps_max
+                      : d.field == BF_DELTA_CHILD ? T.off_child != BF_OFF_NONE && d.index < T.child_nibbles
+                      : true;
+    if (!fits) { b->err = "a pending delta of run " + std::to_string(d.run) + " lies outside the new layout"; return BF_EINVAL; }
+  }
+  HostRecords nr;
+  if (!nr.alloc(b->ctx, (size_t)b->cap * T.state_stride, (size_t)b->cap * T.result_stride)) {
+    b->err = "out of host memory";
+    return BF_ENOMEM;
+  }
+  if (b->resident) {   // every run on the device first, then the device: it fails without changes, and so does the mirror
+    int rc = flush_uploads(b);
+    if (rc == BF_OK) {
+      bf_extent e{};
+      e.struct_size = sizeof e; e.n_runs = b->n;
+      rc = bf_resident_narrow(b->ctx, b->handle, &T, &e);
+    }
+    if (rc != BF_OK) { b->err = bf_last_error(b->ctx); return rc; }
+  }
+  relay_records(b, nr, F, T);
+  b->rec.swap(nr);
+  b->L = T;
   return BF_OK;
 }
 
@@ -888,6 +981,10 @@ int bfh_batch_retire(bfh_batch* b, const uint32_t* runs, uint32_t n, uint32_t ca
   });
   b->n = m;
   if (b->uploaded > m) b->uploaded = m;
+  // a run moved from at or above `evaluated` takes its unevaluated record below it
+  for (size_t k = 0; k < from.size(); ++k)
+    if (from[k] >= b->evaluated) b->evaluated = std::min(b->evaluated, to[k]);
+  if (b->evaluated > m) b->evaluated = m;
   if (moves_from && !from.empty()) memcpy(moves_from, from.data(), from.size() * 4);
   if (moves_to && !to.empty()) memcpy(moves_to, to.data(), to.size() * 4);
   return (int)from.size();

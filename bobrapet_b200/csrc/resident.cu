@@ -362,4 +362,111 @@ cudaError_t launch_retire(const RetireParams& P, cudaStream_t stream) {
   return cudaGetLastError();
 }
 
+// Extent (bf_resident_extent, bf_resident_narrow).  Word o of a record lies in the plane field at `off` (planes * W words): w is
+// its word within its plane.
+DI bool in_planes(uint32_t o, uint32_t off, uint32_t planes, uint32_t W, uint32_t& w) {
+  if (off == BF_OFF_NONE || o < off || o >= off + planes * W * 4u) return false;
+  w = ((o - off) >> 2) % W;
+  return true;
+}
+// steps needed by plane word w holding v: one past its highest set bit
+DI uint32_t word_extent(uint32_t w, uint32_t v) { return v ? 32u * w + 32u - __clz(v) : 0u; }
+
+// State word o holding v: the steps its codes need, the nibbles of the child area it needs, the input fields it needs.
+DI void state_word_extent(const bf_layout& L, uint32_t o, uint32_t v, uint32_t& steps, uint32_t& child, uint32_t& fields) {
+  if (o < 16u || v == 0u) return;   // bf_run_header
+  uint32_t w;
+  if (in_planes(o, L.off_phase, 4, L.words, w)) {
+    steps = max(steps, word_extent(w, v));
+  } else if (in_planes(o, L.off_cond, 2, L.words, w)) {
+    steps = max(steps, word_extent(w, v));
+    fields |= BF_F_COND;
+  } else if (in_planes(o, L.off_decision, 2, L.words, w)) {
+    steps = max(steps, word_extent(w, v));
+    fields |= BF_F_DECISION;
+  } else if (L.off_child != BF_OFF_NONE && o >= L.off_child && o < L.off_child + child_area_words(L) * 4u) {
+    const uint32_t first = ((o - L.off_child) >> 2) * 8u;   // nibbles first .. first + 7, those below child_nibbles count
+    if (first >= L.child_nibbles) return;
+    const uint32_t n = min(8u, L.child_nibbles - first), m = n == 8u ? v : v & ((1u << (4u * n)) - 1u);
+    if (m) { child = max(child, first + (31u - __clz(m)) / 4u + 1u); fields |= BF_F_CHILD; }
+  }
+}
+
+// Result word o holding v: the steps its masks need (only the fields R places count).
+DI uint32_t result_word_extent(const bf_layout& R, uint32_t o, uint32_t v) {
+  uint32_t w;
+  if (o >= 16u && v && (in_planes(o, R.off_ready, 1, R.words, w) || in_planes(o, R.off_skip, 1, R.words, w) ||
+                        in_planes(o, R.off_fail, 1, R.words, w) || in_planes(o, R.off_needs_cond, 1, R.words, w) ||
+                        in_planes(o, R.off_skip_dep, 1, R.words, w) || in_planes(o, R.off_phase_out, 4, R.words, w)))
+    return word_extent(w, v);
+  return 0u;
+}
+
+// One warp per record, grid-stride: lane t reads the 16-byte vectors t, t + 32, ... of the state record (and of the result record
+// of a run below n_runs that a later tick may compare with), so a warp streams each record once with coalesced loads; lane 0 adds the S and the child area of the
+// run's topology when its slot is alive.  Warp reductions, then each warp folds its record's extents into its running maxima (its
+// records ascend, so the running maximum keeps the lowest index), the CTA's warps meet in shared memory and one thread per CTA
+// adds the CTA's three words to P.out.
+__global__ void __launch_bounds__(256) extent_runs(const ExtentParams P) {
+  __shared__ unsigned long long cta[3];
+  if (threadIdx.x < 3) cta[threadIdx.x] = 0ull;
+  __syncthreads();
+  const uint32_t lane = threadIdx.x & 31u, warps = gridDim.x * 8u;
+  unsigned long long best_steps = 0ull, best_child = 0ull;
+  uint32_t all_fields = 0u;
+  for (uint32_t r = blockIdx.x * 8u + (threadIdx.x >> 5); r < P.n_records; r += warps) {
+    uint32_t steps = 0u, child = 0u, fields = 0u;
+    const uint8_t* s = P.state + (size_t)r * P.L.state_stride;
+    for (uint32_t o = lane * 16u; o < P.L.state_stride; o += 512u) {
+      const uint4 q = *reinterpret_cast<const uint4*>(s + o);
+      state_word_extent(P.L, o, q.x, steps, child, fields);
+      state_word_extent(P.L, o + 4u, q.y, steps, child, fields);
+      state_word_extent(P.L, o + 8u, q.z, steps, child, fields);
+      state_word_extent(P.L, o + 12u, q.w, steps, child, fields);
+    }
+    if (r < P.n_runs) {
+      const uint32_t m = P.mark[r];
+      const bool baseline = r < P.prev_runs || (r < P.eval_runs && !((m & 1u) && (m >> 1) > P.full_epoch));
+      const uint8_t* res = P.result + (size_t)r * P.L.result_stride;
+      for (uint32_t o = lane * 16u; baseline && o < P.L.result_stride; o += 512u) {
+        const uint4 q = *reinterpret_cast<const uint4*>(res + o);
+        steps = max(steps, max(max(result_word_extent(P.R, o, q.x), result_word_extent(P.R, o + 4u, q.y)),
+                               max(result_word_extent(P.R, o + 8u, q.z), result_word_extent(P.R, o + 12u, q.w))));
+      }
+      if (lane == 0) {
+        const uint32_t slot = *reinterpret_cast<const uint32_t*>(s);
+        const Slot sl = slot < P.n_slots ? P.slots[slot] : Slot{};
+        if (sl.addr) {
+          steps = max(steps, sl.meta & 0xFFFFu);
+          child = max(child, (uint32_t)reinterpret_cast<const TopoHeader*>(sl.addr)->child_nibbles);
+        }
+      }
+    }
+    steps = __reduce_max_sync(FULL, steps);
+    child = __reduce_max_sync(FULL, child);
+    all_fields |= __reduce_or_sync(FULL, fields);
+    const unsigned long long idx = ~r & 0xFFFFFFFFull;
+    if (steps) best_steps = max(best_steps, (unsigned long long)steps << 32 | idx);
+    if (child) best_child = max(best_child, (unsigned long long)child << 32 | idx);
+  }
+  if (lane == 0) {
+    if (best_steps) atomicMax(&cta[0], best_steps);
+    if (best_child) atomicMax(&cta[1], best_child);
+    if (all_fields) atomicOr(&cta[2], (unsigned long long)all_fields);
+  }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    if (cta[0]) atomicMax(P.out, cta[0]);
+    if (cta[1]) atomicMax(P.out + 1, cta[1]);
+    if (cta[2]) atomicOr(P.out + 2, cta[2]);
+  }
+}
+
+cudaError_t launch_extent(const ExtentParams& P, uint32_t sm_count, cudaStream_t stream) {
+  if (P.n_records == 0) return cudaSuccess;
+  const uint32_t grid = min((P.n_records - 1u) / 8u + 1u, max(sm_count, 1u) * 8u);   // 8 CTAs of 8 warps per SM at most
+  extent_runs<<<grid, 256, 0, stream>>>(P);
+  return cudaGetLastError();
+}
+
 }  // namespace bf

@@ -1,5 +1,5 @@
 // resident_abi.cu — the C ABI of include/bobrafrontier.h for resident batches (row f2): a batch's records stay on the device
-// between ticks; uploads, deltas, migrations, redrives, reshapes and retirements change them in place, and full, compact,
+// between ticks; uploads, deltas, migrations, redrives, reshapes, retirements and narrowings change them in place, and full, compact,
 // changed-only and touched ticks evaluate them.  The bookkeeping of touched ticks lives in Resident (ctx.h).
 #include <stdlib.h>
 #include <string.h>
@@ -487,6 +487,122 @@ int bf_resident_reshape(bf_ctx* c, uint32_t h, const bf_layout* layout, uint32_t
   r->end_snapshot(c);   // as after an upload
   r->adopt(std::move(nb), T, capacity);
   if (results_may_change) r->need_full = true;
+  return BF_OK;
+}
+
+// The extent kernel over the batch, counting the result fields R places, on the ctx stream; the caller downloads the three words
+// of c->d_extent (download_extent) behind whatever else it launches.  Nothing of the batch changes.
+static int extent_async(bf_ctx* c, Resident* r, uint32_t n_runs, const bf_layout& R) {
+  cudaStream_t s = c->stream;
+  if (int rc = c->d_extent.ensure(c, 3)) return rc;
+  if (int rc = bf::sync_slots(c, s)) return rc;
+  bf::ExtentParams P{};
+  P.state = r->d_state; P.result = r->d_result; P.mark = r->d_mark; P.slots = c->slots_dev; P.n_slots = (uint32_t)c->slots_host.size();
+  P.n_records = r->cap; P.n_runs = n_runs; P.L = r->L; P.R = R; P.out = c->d_extent;
+  // only result records a later tick compares with count: the changed-only baseline and the touched one (ctx.h)
+  P.prev_runs = r->prev_valid ? r->prev_runs : 0u; P.eval_runs = r->touched_baseline_runs(); P.full_epoch = r->full_epoch;
+  BF_CUDA(c, cudaMemsetAsync(c->d_extent, 0, 3 * sizeof(unsigned long long), s));
+  BF_CUDA(c, bf::launch_extent(P, c->sm_count, s));
+  c->stats.kernel_launches += 1;
+  return BF_OK;
+}
+
+static cudaError_t download_extent(bf_ctx* c, unsigned long long* out) {
+  return cudaMemcpyAsync(out, c->d_extent, 3 * sizeof(unsigned long long), cudaMemcpyDeviceToHost, c->stream);
+}
+
+static void fill_extent(const unsigned long long* out, bf_extent* e) {
+  e->steps_max = std::max(1u, (uint32_t)(out[0] >> 32));
+  e->widest_run = out[0] ? ~(uint32_t)out[0] : BF_EXTENT_NO_RUN;
+  e->child_nibbles = (uint32_t)(out[1] >> 32);
+  e->fields = (uint32_t)out[2];
+}
+
+int bf_resident_extent(bf_ctx* c, uint32_t h, bf_extent* e) {
+  auto [g, r] = lock_resident(c, h);
+  if (!e || e->struct_size != sizeof(bf_extent)) return fail(c, BF_EINVAL, "null bf_extent or bad struct_size");
+  if (!r) return BF_EINVAL;
+  if (e->n_runs > r->cap) return fail(c, BF_EINVAL, "n_runs exceeds the resident batch");
+  BF_CUDA(c, cudaSetDevice(c->device));
+  unsigned long long out[3] = {};
+  if (int rc = extent_async(c, r, e->n_runs, r->L)) return rc;
+  BF_CUDA(c, download_extent(c, out));
+  BF_CUDA(c, cudaStreamSynchronize(c->stream));
+  fill_extent(out, e);
+  return BF_OK;
+}
+
+// A live batch narrows its layout (resident.cu).  The layout checks come first; then the new buffers are allocated, the extent
+// kernel, the re-layout into the new buffers and the copy of the marks run back to back, and after the one synchronisation the
+// new buffers replace the old ones only when the extent passes.  A rejected or failed call changes nothing: the old buffers were
+// only read.
+int bf_resident_narrow(bf_ctx* c, uint32_t h, const bf_layout* layout, bf_extent* e) {
+  auto [g, r] = lock_resident(c, h);
+  if (!e || e->struct_size != sizeof(bf_extent)) return fail(c, BF_EINVAL, "null bf_extent or bad struct_size");
+  if (!r) return BF_EINVAL;
+  const uint32_t N = e->n_runs;
+  if (N > r->cap) return fail(c, BF_EINVAL, "n_runs exceeds the resident batch");
+  BF_CUDA(c, cudaSetDevice(c->device));
+  unsigned long long out[3] = {};
+  // a layout rejected before the extent is known still reports the extent (over every result plane), so the caller sees what fits
+  auto reject = [&](const std::string& why) {
+    if (extent_async(c, r, N, r->L) == BF_OK && download_extent(c, out) == cudaSuccess && cudaStreamSynchronize(c->stream) == cudaSuccess)
+      fill_extent(out, e);
+    return fail(c, BF_EINVAL, why);
+  };
+  if (!layout) return reject("null layout");
+  if (bf::check_layout(c, *layout)) return reject(std::string(c->err));
+  const bf_layout F = r->L, T = *layout;
+  if (T.steps_max > F.steps_max) return reject("narrow cannot raise steps_max (reshape grows a batch)");
+  if (T.fields & ~F.fields) return reject("narrow cannot add a field (reshape grows a batch)");
+  if (F.off_child != BF_OFF_NONE && T.off_child != BF_OFF_NONE && T.child_nibbles > F.child_nibbles)
+    return reject("narrow cannot enlarge the child area (reshape grows a batch)");
+  // the kernel follows the offsets: every field the new layout places must be placed by the batch's.  Dropping decision planes
+  // (zero ones are PENDING, which a pass applies; absent ones skip it), the child area (a registered parallel step without
+  // branches joins with an area and not without one) or an output mask (the event kinds change) may change any run's result
+  const uint32_t from[] = {F.off_cond, F.off_decision, F.off_child, F.off_fail, F.off_needs_cond, F.off_skip_dep, F.off_phase_out};
+  const uint32_t to[] = {T.off_cond, T.off_decision, T.off_child, T.off_fail, T.off_needs_cond, T.off_skip_dep, T.off_phase_out};
+  bool results_may_change = false;
+  for (int i = 0; i < 7; ++i) {
+    if (from[i] == BF_OFF_NONE && to[i] != BF_OFF_NONE) return reject("the new layout places a field the batch lacks");
+    if (i != 0 && from[i] != BF_OFF_NONE && to[i] == BF_OFF_NONE) results_may_change = true;
+  }
+  bf_layout R = F;   // the result planes that count: those the new layout keeps
+  if (T.off_fail == BF_OFF_NONE) R.off_fail = BF_OFF_NONE;
+  if (T.off_needs_cond == BF_OFF_NONE) R.off_needs_cond = BF_OFF_NONE;
+  if (T.off_skip_dep == BF_OFF_NONE) R.off_skip_dep = BF_OFF_NONE;
+  if (T.off_phase_out == BF_OFF_NONE) R.off_phase_out = BF_OFF_NONE;
+  const bool same = memcmp(&F, &T, sizeof T) == 0;
+  Resident nb;
+  if (!same)
+    if (cudaError_t e2 = nb.alloc(T, r->cap)) return fail(c, BF_ENOMEM, std::string("resident narrow: ") + cudaGetErrorString(e2));
+  if (int rc = extent_async(c, r, N, R)) { cudaStreamSynchronize(c->stream); return rc; }
+  cudaStream_t s = c->stream;
+  cudaError_t err = cudaSuccess;
+  if (!same) {
+    bf::ReshapeParams P{};
+    P.old_state = r->d_state; P.old_result = r->d_result; P.state = nb.d_state; P.result = nb.d_result;
+    P.n_old = r->cap; P.n_new = r->cap; P.from = F; P.to = T;
+    err = bf::launch_reshape(P, s);
+    if (err == cudaSuccess) err = cudaMemcpyAsync(nb.d_mark, r->d_mark, r->d_mark.cap * sizeof(uint32_t), cudaMemcpyDeviceToDevice, s);
+    c->stats.kernel_launches += 1;
+  }
+  if (err == cudaSuccess) err = download_extent(c, out);
+  const cudaError_t es = cudaStreamSynchronize(s);
+  if (err == cudaSuccess) err = es;
+  if (err != cudaSuccess) return cuda_fail(c, err, "bf_resident_narrow");   // the old buffers were only read: the batch is as it was
+  fill_extent(out, e);
+  if (same) return BF_OK;
+  const uint32_t placed = (T.off_cond != BF_OFF_NONE ? BF_F_COND : 0u) | (T.off_decision != BF_OFF_NONE ? BF_F_DECISION : 0u) |
+                          (T.off_child != BF_OFF_NONE ? BF_F_CHILD : 0u);
+  if (T.steps_max < e->steps_max)
+    return fail(c, BF_EINVAL, "run " + std::to_string(e->widest_run) + " needs steps_max " + std::to_string(e->steps_max));
+  if (T.off_child != BF_OFF_NONE && T.child_nibbles < e->child_nibbles)
+    return fail(c, BF_EINVAL, "the batch needs child_nibbles " + std::to_string(e->child_nibbles));
+  if (e->fields & ~placed) return fail(c, BF_EINVAL, "the new layout drops an input field holding a non-default code");
+  r->end_snapshot(c);   // as after an upload
+  r->adopt(std::move(nb), T, r->cap);
+  r->narrowed(N, results_may_change);
   return BF_OK;
 }
 

@@ -258,6 +258,24 @@ class Frontier:
         self._check(self._lib.bf_resident_retire(self._ctx, handle, C.byref(rt)), "bf_resident_retire")
         return int(rt.n_runs), mf[:rt.n_moves].copy(), mt[:rt.n_moves].copy()
 
+    def resident_extent(self, handle: int, n_runs: int) -> dict:
+        """bf_resident_extent: the smallest layout the batch's runs [0, n_runs) and records allow -> dict(steps_max, child_nibbles,
+        fields, widest_run)"""
+        e = A.Extent(struct_size=C.sizeof(A.Extent), n_runs=int(n_runs))
+        self._check(self._lib.bf_resident_extent(self._ctx, handle, C.byref(e)), "bf_resident_extent")
+        return e.as_dict()
+
+    def resident_narrow(self, handle: int, L: A.Layout, n_runs: int) -> dict:
+        """bf_resident_narrow: re-lay the batch at the smaller layout L (from make_layout) in place when its runs [0, n_runs) and
+        records allow it -> the extent (dict as resident_extent).  A rejection raises FrontierError with the extent as .extent"""
+        e = A.Extent(struct_size=C.sizeof(A.Extent), n_runs=int(n_runs))
+        rc = self._lib.bf_resident_narrow(self._ctx, handle, C.byref(L), C.byref(e))
+        if rc != A.BF_OK:
+            err = A.FrontierError(rc, "bf_resident_narrow: %s" % self._lib.bf_last_error(self._ctx).decode())
+            err.extent = e.as_dict()
+            raise err
+        return e.as_dict()
+
     # -- resident batches: device-side state, delta uploads (row f2)
     DELTA_DTYPE = np.dtype([("run", "<u4"), ("index", "<u2"), ("field", "u1"), ("code", "u1")])
 

@@ -46,6 +46,7 @@ _SYMS = [
     ("bfh_batch_redrive", C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32]),
     ("bfh_batch_reshape", C.c_int, [C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32]),
     ("bfh_batch_retire", C.c_int, [C.c_void_p, C.c_void_p, C.c_uint32, C.c_uint32, C.c_void_p, C.c_void_p]),
+    ("bfh_batch_narrow", C.c_int, [C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32]),
     ("bfh_batch_eval", C.c_int, [C.c_void_p, C.c_uint32, C.POINTER(A.Counts)]),
     ("bfh_batch_set_resident", C.c_int, [C.c_void_p, C.c_int]),
     ("bfh_batch_traffic", C.c_int, [C.c_void_p, C.POINTER(C.c_uint64), C.POINTER(C.c_uint64), C.POINTER(C.c_uint32)]),
@@ -256,6 +257,12 @@ class HostBatch:
         """bfh_batch_reshape: grow the layout to bf_layout_init(steps_max, child_nibbles, fields) and the capacity, keeping every
         run's records and the pending deltas (in resident mode on the device too)"""
         self._chk(self._l.bfh_batch_reshape(self._p, steps_max, child_nibbles, fields, capacity), "bfh_batch_reshape")
+
+    def narrow(self, steps_max, child_nibbles, fields) -> None:
+        """bfh_batch_narrow: shrink the layout to bf_layout_init(steps_max, child_nibbles, fields) when the records, the runs'
+        stories and the pending deltas allow it, keeping every run's records and the pending deltas (in resident mode on the
+        device too)"""
+        self._chk(self._l.bfh_batch_narrow(self._p, steps_max, child_nibbles, fields), "bfh_batch_narrow")
 
     def retire(self, runs, capacity=0):
         """bfh_batch_retire: take `runs` out of the batch; the last live runs move into the freed indices (in resident mode on the

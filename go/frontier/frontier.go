@@ -409,6 +409,35 @@ func (r *Resident) Retire(nRuns uint32, runs []uint32, capacity uint32) (newN ui
 	return uint32(nOut), from[:nMoves], to[:nMoves], r.c.err(rc)
 }
 
+// Extent is the smallest layout a batch's contents allow (bf_extent): a Narrow to StepsMax, ChildNibbles and a superset of
+// Fields succeeds.  WidestRun is the lowest run that needs StepsMax, or 0xFFFFFFFF when none does.
+type Extent struct {
+	StepsMax, ChildNibbles, Fields, WidestRun uint32
+}
+
+// Extent reports the smallest layout the runs [0, nRuns) and every record of the batch allow (bf_resident_extent).  Query it
+// after a Retire: when it is well below the layout, Narrow; when one straggler holds the width, WidestRun names it.
+func (r *Resident) Extent(nRuns uint32) (Extent, error) {
+	var out [4]C.uint32_t
+	rc := C.bfgo_resident_extent(r.c.p, r.handle, C.uint32_t(nRuns), &out[0])
+	return Extent{uint32(out[0]), uint32(out[1]), uint32(out[2]), uint32(out[3])}, r.c.err(rc)
+}
+
+// Narrow re-lays the batch in place at the smaller layout bf_layout_init(stepsMax, childNibbles, fields), keeping every run's
+// state, the current results and, unless decision planes, the child area or an output field are dropped, the touched-tick
+// bookkeeping (bf_resident_narrow).  A layout below the extent of the runs [0, nRuns) and the batch's records is an error that
+// changes nothing; the returned Extent says why.
+func (r *Resident) Narrow(stepsMax, childNibbles, fields, nRuns uint32) (Extent, error) {
+	var out [4]C.uint32_t
+	var L C.bf_layout
+	rc := C.bfgo_resident_narrow(r.c.p, r.handle, C.uint32_t(stepsMax), C.uint32_t(childNibbles), C.uint32_t(fields),
+		C.uint32_t(nRuns), &out[0], &L)
+	if rc == C.BF_OK {
+		r.layout = L
+	}
+	return Extent{uint32(out[0]), uint32(out[1]), uint32(out[2]), uint32(out[3])}, r.c.err(rc)
+}
+
 // Group is one operator process driving several GPUs (bf_group_*): contiguous blocks of runs per device, one NCCL
 // all-gather of the per-shard counts per pass, limiter totals all-reduced across the shards.
 type Group struct{ p *C.bf_group }

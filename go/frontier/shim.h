@@ -138,6 +138,34 @@ static inline int bfgo_resident_retire(bf_ctx* c, uint32_t handle, uint32_t n_ru
   return rc;
 }
 
+/* bf_resident_extent / bf_resident_narrow with the bf_extent built here on the C stack; narrow builds the new layout with
+ * bf_layout_init and *layout_out receives it when the narrow succeeded.  out[4] = steps_max, child_nibbles, fields, widest_run
+ * (filled by a rejected narrow too, so that the caller sees why). */
+static inline int bfgo_resident_extent(bf_ctx* c, uint32_t handle, uint32_t n_runs, uint32_t* out) {
+  bf_extent e;
+  memset(&e, 0, sizeof e);
+  e.struct_size = (uint32_t)sizeof e;
+  e.n_runs = n_runs;
+  const int rc = bf_resident_extent(c, handle, &e);
+  out[0] = e.steps_max; out[1] = e.child_nibbles; out[2] = e.fields; out[3] = e.widest_run;
+  return rc;
+}
+
+static inline int bfgo_resident_narrow(bf_ctx* c, uint32_t handle, uint32_t steps_max, uint32_t child_nibbles, uint32_t fields,
+                                       uint32_t n_runs, uint32_t* out, bf_layout* layout_out) {
+  bf_layout L;
+  int rc = bf_layout_init(&L, steps_max, child_nibbles, fields);
+  if (rc != BF_OK) return rc;
+  bf_extent e;
+  memset(&e, 0, sizeof e);
+  e.struct_size = (uint32_t)sizeof e;
+  e.n_runs = n_runs;
+  rc = bf_resident_narrow(c, handle, &L, &e);
+  out[0] = e.steps_max; out[1] = e.child_nibbles; out[2] = e.fields; out[3] = e.widest_run;
+  if (rc == BF_OK) *layout_out = L;
+  return rc;
+}
+
 static inline void bfgo_tables(bf_sched_tables* t, uint32_t n_stories, uint32_t n_queues, int32_t global_limit, uint32_t global_base,
                                const int32_t* story_limit, const uint32_t* story_base, const int32_t* queue_limit,
                                const int32_t* queue_aging_s, const uint32_t* queue_base, const int32_t* queue_max_priority_base) {

@@ -514,7 +514,8 @@ int bf_resident_tick_compact(bf_ctx* ctx, uint32_t handle, const bf_delta* delta
  * The tick evaluates every run in [0, n_runs), lists them all (runs[i] = i) and sets full = 1 when: no tick has run on the batch
  * yet (or the last one failed); a slot of the ctx was dropped, or a put reused a dropped slot, since the last tick (a dropped
  * slot kills its runs, a reused one re-points them); BF_EVAL_FIXPOINT or max_iterations differs from the last tick's; bf_resident_reshape added
- * decision planes or an output field since (either may change any run's result); or n_runs exceeds the run count of the last full evaluation and not
+ * decision planes or an output field since, or bf_resident_narrow dropped decision planes, the child area or an output field
+ * (each may change any run's result); or n_runs exceeds the run count of the last full evaluation and not
  * every run beyond it was uploaded since.  A run may hold only a slot a put has returned (alive or dropped since): a put that
  * creates a new slot index is not a change, so runs that already held that index (by a delta or an upload) keep the dead
  * result of their last evaluation until they are touched again.  Any tick of the other kinds (bf_resident_tick,
@@ -629,7 +630,7 @@ int bf_resident_redrive(bf_ctx* ctx, uint32_t handle, const bf_redrive* requests
  * decision planes or an output field added (e.g. BF_F_OUT_NEEDS_COND with BF_F_COND) the next touched tick is full; a
  * changed-only tick lists the runs whose result changed, the zeroed new masks and planes included.  Like an upload, the call ends the evaluated snapshot (bf_schedule must follow a new pass).  bf_stats and the
  * ctx's staging buffers are unaffected.  One launch, one device copy of the marks and one synchronisation.
- * Shrinking a batch or dropping a field is not offered (it loses codes): create a new batch and upload.             */
+ * Shrinking a batch or dropping a field is bf_resident_retire's (capacity) and bf_resident_narrow's (layout) job.         */
 int bf_resident_reshape(bf_ctx* ctx, uint32_t handle, const bf_layout* layout, uint32_t capacity);
 
 /* ------------------------------------------------------------------ retirements (runs leave a live batch)
@@ -669,6 +670,59 @@ typedef struct bf_retire {
 } bf_retire;
 
 int bf_resident_retire(bf_ctx* ctx, uint32_t handle, bf_retire* r);
+
+/* ------------------------------------------------------------------ narrowings (a live batch sheds the shape its wide Stories needed)
+ * bf_resident_reshape only grows a layout, so one 200-step Story, one `if` or one `parallel` step would cost every later pass its
+ * width, planes and child area for the life of the batch.  bf_resident_extent reports the smallest layout the batch's contents
+ * allow, and bf_resident_narrow re-lays the batch to a smaller one in place once the Stories that needed the width have left.
+ * The extent of runs [0, n_runs) is taken over three sets:
+ *   - the topology slot of each run below n_runs whose slot is alive: its S counts towards steps_max, its child area towards
+ *     child_nibbles (what bf_resident_migrate and _redrive require of a slot: it fits the layout);
+ *   - every state record below the capacity, records at or above n_runs included (a batcher may upload ahead): the highest step
+ *     with a non-zero phase, cond or decision code sets steps_max, the highest non-zero child nibble below the layout's
+ *     child_nibbles sets child_nibbles; a non-PASS cond code, a non-PENDING decision code and a non-zero child nibble set
+ *     BF_F_COND, BF_F_DECISION and BF_F_CHILD in `fields`;
+ *   - the current result record of each run below n_runs that a later tick compares with: the runs a BF_EVAL_CHANGED_ONLY tick
+ *     would compare over (when one would), and, unless the next touched tick is full, the runs of the last full evaluation and
+ *     the runs uploaded since that a touched tick has evaluated, except runs uploaded, migrated or moved since their last
+ *     evaluation (a touched tick lists those whatever their record holds).  Records never written by a pass (a batch before its
+ *     first tick) therefore never count.  The highest set bit of a mask or phase_out plane counts towards steps_max;
+ *     bf_resident_narrow counts only the planes the new layout keeps, bf_resident_extent all of them.
+ * widest_run is the lowest index of a run (or a record, when it lies at or above n_runs) that needs all of steps_max.
+ * bf_resident_narrow(layout T) accepts exactly this region.  Checked before anything changes, else BF_EINVAL, nothing changed and
+ * `e` still filled (so that the caller sees why): n_runs <= capacity; T passes the checks of bf_resident_create; T grows no
+ * dimension (T.steps_max <= the current steps_max, T.fields a subset of the current fields, every field T places placed by the
+ * current layout too, T.child_nibbles <= the current child_nibbles when both have BF_F_CHILD); T.steps_max >= e.steps_max;
+ * T.child_nibbles >= e.child_nibbles when T has BF_F_CHILD; T.fields a superset of e.fields (an input plane holding a
+ * non-default code is never dropped).  Output fields may always be dropped: they hold results, not codes.  T equal to the
+ * current layout is BF_OK and changes nothing.  Should an allocation fail, BF_ENOMEM and nothing changed.
+ * Afterwards, by the bytes (the capacity does not change: bf_resident_retire owns it):
+ *   - every state record equals pack_state of the same codes at T: the header as it was, each plane its low T.words words, the
+ *     child area its low bytes;
+ *   - every current result record equals what a pass at T writes for an unchanged run: the header as it was, each kept mask and
+ *     phase_out plane its low T.words words, dropped masks gone.
+ * Touched ticks: narrowing steps_max or child_nibbles, and dropping cond planes (all PASS, as absent planes read), keep the touch
+ * marks and the touched-tick bookkeeping, so the next touched tick stays incremental.  Dropping decision planes (zero planes are
+ * PENDING, which a pass applies; absent ones skip it), the child area (a registered parallel step without branches joins with an
+ * area and not without one) or an output field (the event kinds change) makes the next touched tick full.  Result records at or
+ * above n_runs were not checked, so the run count of the last full evaluation drops to n_runs at most and a BF_EVAL_CHANGED_ONLY
+ * tick over more than n_runs runs lists every run, as after bf_resident_retire.  Like an upload, the call ends the evaluated
+ * snapshot (bf_schedule must follow a new pass).  bf_resident_narrow: the extent launch, the re-layout launch and a device copy
+ * of the marks into new buffers, one synchronisation; the new buffers replace the old ones only when the extent passes.
+ * bf_resident_extent: one launch, one synchronisation, nothing changed.                                                   */
+#define BF_EXTENT_NO_RUN 0xFFFFFFFFu
+typedef struct bf_extent {
+  uint32_t struct_size;        /* sizeof(bf_extent)                                                                   */
+  uint32_t n_runs;             /* in: the batch's runs are [0, n_runs), n_runs <= capacity                            */
+  uint32_t steps_max;          /* out: the smallest steps_max a narrow accepts (>= 1)                                 */
+  uint32_t child_nibbles;      /* out: the smallest child_nibbles a narrow that keeps BF_F_CHILD accepts              */
+  uint32_t fields;             /* out: input fields (BF_F_COND / _DECISION / _CHILD) holding a non-default code       */
+  uint32_t widest_run;         /* out: the lowest run index that needs steps_max, BF_EXTENT_NO_RUN when none does     */
+  uint32_t reserved[2];        /* 0                                                                                   */
+} bf_extent;
+
+int bf_resident_extent(bf_ctx* ctx, uint32_t handle, bf_extent* e);
+int bf_resident_narrow(bf_ctx* ctx, uint32_t handle, const bf_layout* layout, bf_extent* e);
 
 /* ------------------------------------------------------------------ device groups (SURVEY.md row e)
  * The reference is ONE operator process (cmd/main.go:220, StoryRunReconciler storyrun_controller.go:216), so the

@@ -126,6 +126,15 @@ int bfh_batch_redrive(bfh_batch* b, const uint32_t* runs, const int32_t* steps, 
  * additional runs.                                                                                                         */
 int bfh_batch_reshape(bfh_batch* b, uint32_t steps_max, uint32_t child_nibbles, uint32_t fields, uint32_t capacity);
 
+/* Narrow the batch (see bf_resident_narrow): the layout becomes bf_layout_init(steps_max, child_nibbles, fields), the capacity
+ * stays.  The same acceptance test is applied to the mirror's own records (every record below the capacity, the Story of every
+ * run, the result record of every run) and to its pending deltas: a pending delta whose step, child index or field the new
+ * layout lacks blocks the call, so nothing is dropped silently.  The mirror re-lays its records as bf_resident_narrow re-lays
+ * the device's and keeps its pending deltas.  In resident mode it first uploads its runs not yet on the device, then calls
+ * bf_resident_narrow over its runs; when that fails, the mirror changes nothing.  A growing, invalid or blocked shape is
+ * BF_EINVAL, a failed allocation BF_ENOMEM, and both change nothing.                                                       */
+int bfh_batch_narrow(bfh_batch* b, uint32_t steps_max, uint32_t child_nibbles, uint32_t fields);
+
 /* Retire runs (see bf_resident_retire): `runs` lists n distinct runs below bfh_batch_size; the last live runs move into the
  * indices they free, by the same rule, and the size becomes size - n.  capacity 0 keeps the capacity, else it becomes
  * `capacity` (size - n <= capacity <= current).  The mirror moves its own records, drops the pending deltas of retired runs and

@@ -1,6 +1,7 @@
 #!/bin/bash
 # tools/sanitize.sh: compute-sanitizer (memcheck, racecheck, synccheck) over small passes of every kernel shape — smoke() plus a
-# wide (S = 1024, parallel joins, 10-bit rows) and a pipelined batch.  Prints the tools' summaries.
+# wide (S = 1024, parallel joins, 10-bit rows) and a pipelined batch, and a resident batch that takes an extent, a narrow (the
+# extent and re-layout kernels) and touched ticks on either side of it.  Prints the tools' summaries.
 cd "$(dirname "$0")/.."
 cat > /tmp/san_probe.py <<'PY'
 import os, sys
@@ -40,6 +41,29 @@ with torch.cuda.stream(s):
 torch.cuda.synchronize()
 for k in range(3):
     assert np.array_equal(res[k].cpu().numpy(), w3) and cnt[k].cpu().numpy().tolist() == [wc3["ready"], wc3["skip"], wc3["expansion"], wc3["evals"]]
+from tests import randgen
+from tests import reshape as RS
+rng = np.random.default_rng(5)
+f3 = Frontier(0)
+ts4 = randgen.random_topologies(rng, 16, 8, 32, max_deg=4, parallel=False, fill=0.5)
+s4 = f3.put_topologies(ts4)
+L0, st0, _ = randgen.random_state(rng, ts4, s4, 600, 0, phase_mix="progress")
+Lw, Ln = make_layout(256, 0, A.F_COND | A.F_ALL_OUT), make_layout(32, 0, A.F_ALL_OUT)
+h = f3.resident_create(Lw, 640)
+f3.resident_upload(h, 0, RS.reshape_state(L0, Lw, st0, 600))
+e = f3.resident_extent(h, 600)
+assert e["steps_max"] <= 32 and e["fields"] == 0, e
+f3.resident_tick_touched(h, 600, np.zeros(0, dtype=Frontier.DELTA_DTYPE), 600, 1 << 20)
+f3.resident_narrow(h, Ln, 600)
+d = np.zeros(50, dtype=Frontier.DELTA_DTYPE)
+d["run"], d["index"], d["field"], d["code"] = np.arange(0, 600, 12), 0, A.DELTA_PHASE, 3
+o = f3.resident_tick_touched(h, 600, d, 600, 1 << 20)
+assert o["full"] == 0 and o["n_evaluated"] == 50
+st4 = f3.resident_download(h, 0, 600, Ln.state_stride)
+got, _ = f3.resident_tick(h, Ln, 600, np.zeros(0, dtype=Frontier.DELTA_DTYPE))
+want, _ = PK.evaluate(PK.PackedTopologies(ts4, s4), Ln, st4, threads=4)
+assert np.array_equal(got, want)
+f3.resident_destroy(h)
 print("probe ok")
 PY
 for tool in memcheck racecheck synccheck; do
