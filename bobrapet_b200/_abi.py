@@ -147,6 +147,12 @@ class Extent(C.Structure):
         return {n: getattr(self, n) for n in ("steps_max", "child_nibbles", "fields", "widest_run")}
 
 
+class Transfer(C.Structure):
+    _fields_ = [("struct_size", C.c_uint32), ("src_n_runs", C.c_uint32), ("dst_n_runs", C.c_uint32), ("runs", C.c_void_p),
+                ("n", C.c_uint32), ("moves_from", C.c_void_p), ("moves_to", C.c_void_p), ("n_moves", C.c_uint32),
+                ("unfit", C.c_uint32), ("why", Extent)]
+
+
 class SchedTables(C.Structure):
     _fields_ = [("struct_size", C.c_uint32), ("n_stories", C.c_uint32), ("n_queues", C.c_uint32), ("global_limit", C.c_int32),
                 ("global_running_base", C.c_uint32), ("story_limit", C.c_void_p), ("story_running_base", C.c_void_p),
@@ -198,6 +204,7 @@ SYMBOLS = [
     ("bf_resident_retire", C.c_int, [C.c_void_p, C.c_uint32, C.POINTER(Retire)]),
     ("bf_resident_extent", C.c_int, [C.c_void_p, C.c_uint32, C.POINTER(Extent)]),
     ("bf_resident_narrow", C.c_int, [C.c_void_p, C.c_uint32, C.POINTER(Layout), C.POINTER(Extent)]),
+    ("bf_resident_transfer", C.c_int, [C.c_void_p, C.c_uint32, C.c_uint32, C.POINTER(Transfer)]),
     ("bf_group_create", C.c_int, [C.POINTER(C.c_void_p), C.POINTER(C.c_int32), C.c_uint32, C.POINTER(Config)]),
     ("bf_group_destroy", None, [C.c_void_p]),
     ("bf_group_size", C.c_uint32, [C.c_void_p]),

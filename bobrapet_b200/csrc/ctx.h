@@ -37,6 +37,8 @@ cudaError_t launch_redrive(const RedriveParams& P, cudaStream_t stream);
 cudaError_t launch_reshape(const ReshapeParams& P, cudaStream_t stream);
 cudaError_t launch_retire(const RetireParams& P, cudaStream_t stream);
 cudaError_t launch_extent(const ExtentParams& P, uint32_t sm_count, cudaStream_t stream);
+cudaError_t launch_transfer_fit(const TransferParams& P, cudaStream_t stream);
+cudaError_t launch_transfer(const TransferParams& P, cudaStream_t stream);
 cudaError_t launch_schedule(const SchedParams& P, uint32_t sm_count, cudaStream_t stream, uint32_t phases = 3);
 cudaError_t launch_closure(const Slot* slots, const uint32_t* slot_ids, const uint32_t* starts, uint32_t n, uint32_t n_slots,
                            uint32_t words_out, uint32_t* masks, cudaStream_t stream);
@@ -191,6 +193,8 @@ struct bf_ctx {
   DevBuf<uint32_t> d_retire;
   // extents (bf_resident_extent / _narrow): the three words extent_runs reduces into
   DevBuf<unsigned long long> d_extent;
+  // transfers (bf_resident_transfer): [0, 16) the unfit word | source runs | retire moves | per-run extents (uint4)
+  DevBuf<uint8_t> d_transfer;
 
   // limiters (bf_schedule): the records the last pass evaluated (bf_eval's staging or a resident batch), read in place.  Cleared
   // (valid = false) when a pass starts or a call changes those records (end_snapshot); assigned whole once a pass went through.
@@ -258,7 +262,8 @@ inline int cuda_fail(bf_ctx* c, cudaError_t e, const char* what) {
 //   last_fixpoint, last_max_iter, slot_changes_seen: BF_EVAL_FIXPOINT, max_iterations and bf_ctx::slot_changes at the last
 //                      full tick.  A touched tick with other parameters, or after a slot drop or reuse, is full (full_due).
 //   pending            bound on the touched runs: those the last touched tick left at or above its n_runs, plus the deltas,
-//                      uploaded, migrated, redriven and moved runs since.  full_tick_done zeroes it.
+//                      uploaded, migrated, redriven, moved and received runs since.  full_tick_done zeroes it.
+//   (transfer)         the source compacts as by retire (compact_to); the destination takes the arrivals as uploads (received).
 //   uploaded           merged [first, end) ranges, keyed by first, of the runs at or above full_runs uploaded since the last full
 //                      tick (note_uploaded); compact_to clips them; full_tick_done clears them.
 // A call that changes d_state ends the evaluated snapshot (end_snapshot): bf_schedule must follow a new pass.
@@ -364,6 +369,15 @@ struct Resident {
     full_runs = std::min(full_runs, n_runs);
     if (prev_runs > n_runs) prev_valid = false;
     if (results_may_change) need_full = true;
+  }
+  // transfer wrote n arrivals at [first, first + n), marked "must list": they count as uploaded.  The changed-only baseline
+  // reaches over them when it covered exactly `first` runs and their result records were a baseline of their source
+  // (src_baseline), else the next changed-only tick lists every run.
+  void received(uint32_t first, uint32_t n, bool src_baseline) {
+    note_uploaded(first, first + n);
+    pending += n;
+    if (prev_valid && prev_runs == first && src_baseline) prev_runs = first + n;
+    else prev_valid = false;
   }
 };
 

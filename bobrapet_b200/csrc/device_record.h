@@ -294,6 +294,27 @@ struct ExtentParams {
   unsigned long long* out;       // [3], zeroed by the caller: steps, child nibbles (both extent << 32 | ~index), BF_F_* input fields
 };
 
+// bf_resident_transfer (resident.cu): runs[i] of the source batch (layout F) is checked against the destination layout T
+// (transfer_fit), then re-laid into destination record dst_first + i (transfer_runs).  The source's compaction is retire_runs.
+struct TransferParams {
+  const uint8_t* src_state;
+  const uint8_t* src_result;     // the source's current result records
+  const uint32_t* src_mark;
+  uint8_t* dst_state;
+  uint8_t* dst_result;
+  uint32_t* dst_mark;            // an arrival's becomes mark_value (touched and must be listed)
+  uint32_t mark_value;
+  const uint32_t* runs;          // [n] source indices
+  uint32_t n, dst_first;
+  const Slot* slots;
+  uint32_t n_slots;
+  uint32_t prev_runs, eval_runs, full_epoch;   // the source's baselines: which result records count (ExtentParams)
+  bf_layout F, T;
+  bf_layout R;                   // F with the result fields T lacks set to BF_OFF_NONE
+  uint4* extent;                 // [n] out: steps, child nibbles, BF_F_* input fields of each run
+  uint32_t* unfit;               // [1] the lowest i that T cannot hold (atomicMin; 0xFFFFFFFF from the caller)
+};
+
 // limiters.cu (rows a9 / f4)
 struct SchedParams {
   const uint8_t* state;

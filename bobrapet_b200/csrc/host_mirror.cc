@@ -990,6 +990,145 @@ int bfh_batch_retire(bfh_batch* b, const uint32_t* runs, uint32_t n, uint32_t ca
   return (int)from.size();
 }
 
+int bfh_batch_transfer(bfh_batch* src, bfh_batch* dst, const uint32_t* runs, uint32_t n, uint32_t* moves_from, uint32_t* moves_to) {
+  if (!src || !dst) return BF_EINVAL;
+  auto refuse = [&](const std::string& why) { src->err = why; dst->err = why; return BF_EINVAL; };
+  if (src == dst) return refuse("a transfer from a batch to itself");
+  if (src->ctx != dst->ctx || src->resident != dst->resident) return refuse("both batches must be of one ctx and in the same mode");
+  const uint32_t N = src->n, D = dst->n;
+  if (n && !runs) return refuse("null runs");
+  if ((uint64_t)D + n > dst->cap) return refuse("the destination batch is full (reshape it first)");
+  std::vector<uint8_t> gone(N, 0);
+  for (uint32_t i = 0; i < n; ++i) {
+    if (runs[i] >= N || gone[runs[i]]) return refuse("runs[" + std::to_string(i) + "] is out of range or moved twice");
+    gone[runs[i]] = 1;
+  }
+  if (n == 0) return 0;
+  // each run must fit the destination layout by bf_resident_narrow's test applied to it alone: its record, its Story and the
+  // result record of a run the last eval covered (the planes T keeps)
+  const bf_layout F = src->L, T = dst->L;
+  const uint32_t W = F.words;
+  const uint32_t placed = (T.off_cond != BF_OFF_NONE ? BF_F_COND : 0u) | (T.off_decision != BF_OFF_NONE ? BF_F_DECISION : 0u) |
+                          (T.off_child != BF_OFF_NONE ? BF_F_CHILD : 0u);
+  for (uint32_t i = 0; i < n; ++i) {
+    const uint32_t r = runs[i];
+    uint32_t steps = (uint32_t)src->story_of_run[r]->flags.size(), child = src->story_of_run[r]->child_nibbles, in_fields = 0;
+    const uint8_t* rec = src->rec.state + (size_t)r * F.state_stride;
+    auto planes = [&](uint32_t off, uint32_t np, uint32_t field) {
+      if (off == BF_OFF_NONE) return;
+      const uint32_t* p = reinterpret_cast<const uint32_t*>(rec + off);
+      for (uint32_t k = 0; k < np * W; ++k)
+        if (p[k]) { steps = std::max(steps, word_extent(k % W, p[k])); in_fields |= field; }
+    };
+    planes(F.off_phase, 4, 0);
+    planes(F.off_cond, 2, BF_F_COND);
+    planes(F.off_decision, 2, BF_F_DECISION);
+    for (uint32_t k = 0; F.off_child != BF_OFF_NONE && k < F.child_nibbles; ++k)
+      if ((rec[F.off_child + k / 2] >> ((k & 1u) * 4u)) & 0xFu) { child = std::max(child, k + 1); in_fields |= BF_F_CHILD; }
+    if (r < src->evaluated) {
+      const uint8_t* res = src->rec.result + (size_t)r * F.result_stride;
+      const std::pair<uint32_t, uint32_t> masks[] = {{F.off_ready, 1}, {F.off_skip, 1}, {T.off_fail != BF_OFF_NONE ? F.off_fail : BF_OFF_NONE, 1},
+                                                     {T.off_needs_cond != BF_OFF_NONE ? F.off_needs_cond : BF_OFF_NONE, 1},
+                                                     {T.off_skip_dep != BF_OFF_NONE ? F.off_skip_dep : BF_OFF_NONE, 1},
+                                                     {T.off_phase_out != BF_OFF_NONE ? F.off_phase_out : BF_OFF_NONE, 4}};
+      for (const auto& mk : masks) {
+        if (mk.first == BF_OFF_NONE) continue;
+        const uint32_t* p = reinterpret_cast<const uint32_t*>(res + mk.first);
+        for (uint32_t k = 0; k < mk.second * W; ++k) steps = std::max(steps, word_extent(k % W, p[k]));
+      }
+    }
+    if (steps > T.steps_max || (T.off_child != BF_OFF_NONE && child > T.child_nibbles) || (in_fields & ~placed))
+      return refuse("runs[" + std::to_string(i) + "] (run " + std::to_string(r) + ") does not fit the destination layout");
+  }
+  for (const bf_delta& d : src->deltas) {   // a pending delta of a moved run must still have its place: none is dropped
+    if (d.run >= N || !gone[d.run]) continue;
+    const bool fits = d.field == BF_DELTA_PHASE ? d.index < T.steps_max
+                      : d.field == BF_DELTA_COND ? T.off_cond != BF_OFF_NONE && d.index < T.steps_max
+                      : d.field == BF_DELTA_DECISION ? T.off_decision != BF_OFF_NONE && d.index < T.steps_max
+                      : d.field == BF_DELTA_CHILD ? T.off_child != BF_OFF_NONE && d.index < T.child_nibbles
+                      : true;
+    if (!fits) return refuse("a pending delta of run " + std::to_string(d.run) + " lies outside the destination layout");
+  }
+  const uint32_t m = N - n;
+  std::vector<uint32_t> from, to, new_index(n, UINT32_MAX);   // the move rule of bfh_batch_retire
+  for (uint32_t i = 0, hole = 0; i < n; ++i) {
+    if (gone[m + i]) continue;
+    while (!gone[hole]) ++hole;
+    from.push_back(m + i); to.push_back(hole); new_index[i] = hole++;
+  }
+  if (src->resident) {   // every run of both batches on the device first, then the device: it fails without changes, and so do the mirrors
+    int rc = flush_uploads(src);
+    if (rc == BF_OK) rc = flush_uploads(dst);
+    if (rc == BF_OK) {
+      bf_transfer t{};
+      t.struct_size = sizeof t; t.src_n_runs = N; t.dst_n_runs = D; t.runs = runs; t.n = n;
+      rc = bf_resident_transfer(src->ctx, src->handle, dst->handle, &t);
+    }
+    if (rc != BF_OK) { src->err = dst->err = bf_last_error(src->ctx); return rc; }
+  }
+  // arrivals: re-laid at the destination layout, in the order of runs[]
+  const size_t ss = F.state_stride, rs = F.result_stride;
+  for (uint32_t i = 0; i < n; ++i) {
+    const uint8_t* s = src->rec.state + (size_t)runs[i] * ss;
+    uint8_t* d = dst->rec.state + (size_t)(D + i) * T.state_stride;
+    memset(d, 0, T.state_stride);
+    memcpy(d, s, sizeof(bf_run_header));
+    relay_planes(d, s, T.off_phase, F.off_phase, 4, T.words, W);
+    relay_planes(d, s, T.off_cond, F.off_cond, 2, T.words, W);
+    relay_planes(d, s, T.off_decision, F.off_decision, 2, T.words, W);
+    if (F.off_child != BF_OFF_NONE && T.off_child != BF_OFF_NONE)
+      memcpy(d + T.off_child, s + F.off_child, std::min(child_area_bytes(F), child_area_bytes(T)));
+    s = src->rec.result + (size_t)runs[i] * rs;
+    d = dst->rec.result + (size_t)(D + i) * T.result_stride;
+    memset(d, 0, T.result_stride);
+    memcpy(d, s, sizeof(bf_result_header));
+    relay_planes(d, s, T.off_ready, F.off_ready, 1, T.words, W);
+    relay_planes(d, s, T.off_skip, F.off_skip, 1, T.words, W);
+    relay_planes(d, s, T.off_fail, F.off_fail, 1, T.words, W);
+    relay_planes(d, s, T.off_needs_cond, F.off_needs_cond, 1, T.words, W);
+    relay_planes(d, s, T.off_skip_dep, F.off_skip_dep, 1, T.words, W);
+    relay_planes(d, s, T.off_phase_out, F.off_phase_out, 4, T.words, W);
+    dst->story_of_run.push_back(src->story_of_run[runs[i]]);
+  }
+  // pending deltas of moved runs go to the destination's log under their new index (no key meets one there: every index from
+  // D on was free); an arrival is on the device in resident mode, and its evaluated results travelled with it
+  std::vector<uint32_t> arrival(N, UINT32_MAX);
+  for (uint32_t i = 0; i < n; ++i) arrival[runs[i]] = D + i;
+  for (const bf_delta& d0 : src->deltas) {
+    if (d0.run >= N || !gone[d0.run]) continue;
+    bf_delta d = d0;
+    d.run = arrival[d0.run];
+    dst->delta_at[delta_key(d.run, d.field, d.index)] = (uint32_t)dst->deltas.size();
+    dst->deltas.push_back(d);
+  }
+  const bool all_evaluated = dst->evaluated == D && std::all_of(runs, runs + n, [&](uint32_t r) { return r < src->evaluated; });
+  dst->n = D + n;
+  if (dst->resident) dst->uploaded = dst->n;
+  if (all_evaluated) dst->evaluated = dst->n;
+  // the source compacts as bfh_batch_retire does
+  for (size_t k = 0; k < from.size(); ++k) {
+    memcpy(src->rec.state + to[k] * ss, src->rec.state + from[k] * ss, ss);
+    memcpy(src->rec.result + to[k] * rs, src->rec.result + from[k] * rs, rs);
+    src->story_of_run[to[k]] = src->story_of_run[from[k]];
+  }
+  memset(src->rec.state + (size_t)m * ss, 0, (size_t)n * ss);
+  memset(src->rec.result + (size_t)m * rs, 0, (size_t)n * rs);
+  src->story_of_run.resize(m);
+  rewrite_deltas(src, [&](bf_delta& d) {
+    if (d.run < N && gone[d.run]) return false;
+    if (d.run >= m) d.run = new_index[d.run - m];
+    return true;
+  });
+  src->n = m;
+  if (src->uploaded > m) src->uploaded = m;
+  for (size_t k = 0; k < from.size(); ++k)
+    if (from[k] >= src->evaluated) src->evaluated = std::min(src->evaluated, to[k]);
+  if (src->evaluated > m) src->evaluated = m;
+  if (moves_from && !from.empty()) memcpy(moves_from, from.data(), from.size() * 4);
+  if (moves_to && !to.empty()) memcpy(moves_to, to.data(), to.size() * 4);
+  return (int)from.size();
+}
+
 int bfh_batch_set_resident(bfh_batch* b, int on) {
   if (!b) return BF_EINVAL;
   if (!b->ctx) { b->err = "batch was created without a device context"; return BF_ENODEV; }

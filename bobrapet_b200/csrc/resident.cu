@@ -469,4 +469,76 @@ cudaError_t launch_extent(const ExtentParams& P, uint32_t sm_count, cudaStream_t
   return cudaGetLastError();
 }
 
+// Transfer (bf_resident_transfer), fit check.  One warp per listed run: the extent of its state record, of its result record when
+// a later tick of the source compares with it (counting the planes T keeps), and of its slot when alive, as extent_runs takes
+// them.  Lane 0 stores the run's extent and, when T cannot hold it, lowers P.unfit to its position.
+__global__ void __launch_bounds__(256) transfer_fit(const TransferParams P) {
+  const uint32_t i = blockIdx.x * 8u + (threadIdx.x >> 5), lane = threadIdx.x & 31u;
+  if (i >= P.n) return;
+  const uint32_t r = P.runs[i];
+  uint32_t steps = 0u, child = 0u, fields = 0u;
+  const uint8_t* s = P.src_state + (size_t)r * P.F.state_stride;
+  for (uint32_t o = lane * 16u; o < P.F.state_stride; o += 512u) {
+    const uint4 q = *reinterpret_cast<const uint4*>(s + o);
+    state_word_extent(P.F, o, q.x, steps, child, fields);
+    state_word_extent(P.F, o + 4u, q.y, steps, child, fields);
+    state_word_extent(P.F, o + 8u, q.z, steps, child, fields);
+    state_word_extent(P.F, o + 12u, q.w, steps, child, fields);
+  }
+  const uint32_t m = P.src_mark[r];
+  const bool baseline = r < P.prev_runs || (r < P.eval_runs && !((m & 1u) && (m >> 1) > P.full_epoch));
+  const uint8_t* res = P.src_result + (size_t)r * P.F.result_stride;
+  for (uint32_t o = lane * 16u; baseline && o < P.F.result_stride; o += 512u) {
+    const uint4 q = *reinterpret_cast<const uint4*>(res + o);
+    steps = max(steps, max(max(result_word_extent(P.R, o, q.x), result_word_extent(P.R, o + 4u, q.y)),
+                           max(result_word_extent(P.R, o + 8u, q.z), result_word_extent(P.R, o + 12u, q.w))));
+  }
+  if (lane == 0) {
+    const uint32_t slot = *reinterpret_cast<const uint32_t*>(s);
+    const Slot sl = slot < P.n_slots ? P.slots[slot] : Slot{};
+    if (sl.addr) {
+      steps = max(steps, sl.meta & 0xFFFFu);
+      child = max(child, (uint32_t)reinterpret_cast<const TopoHeader*>(sl.addr)->child_nibbles);
+    }
+  }
+  steps = __reduce_max_sync(FULL, steps);
+  child = __reduce_max_sync(FULL, child);
+  fields = __reduce_or_sync(FULL, fields);
+  if (lane == 0) {
+    const bf_layout& T = P.T;
+    const uint32_t placed = (T.off_cond != BF_OFF_NONE ? BF_F_COND : 0u) | (T.off_decision != BF_OFF_NONE ? BF_F_DECISION : 0u) |
+                            (T.off_child != BF_OFF_NONE ? BF_F_CHILD : 0u);
+    P.extent[i] = make_uint4(steps, child, fields, 0u);
+    if (steps > T.steps_max || (T.off_child != BF_OFF_NONE && child > T.child_nibbles) || (fields & ~placed)) atomicMin(P.unfit, i);
+  }
+}
+
+// Transfer, the move.  One warp per listed run: lane t stores words t, t + 32, ... of destination record dst_first + i, each
+// re-laid from F to T by its byte offset as reshape_runs does (state, then current result), and lane 0 marks the arrival.  The
+// source records are only read; retire_runs compacts the source behind this launch on the same stream.
+__global__ void __launch_bounds__(256) transfer_runs(const TransferParams P) {
+  const uint32_t i = blockIdx.x * 8u + (threadIdx.x >> 5), lane = threadIdx.x & 31u;
+  if (i >= P.n) return;
+  const uint32_t r = P.runs[i], to = P.dst_first + i;
+  const uint32_t* s = reinterpret_cast<const uint32_t*>(P.src_state + (size_t)r * P.F.state_stride);
+  uint32_t* d = reinterpret_cast<uint32_t*>(P.dst_state + (size_t)to * P.T.state_stride);
+  for (uint32_t o = lane * 4u; o < P.T.state_stride; o += 128u) d[o >> 2] = reshape_state_word(s, o, P.F, P.T);
+  s = reinterpret_cast<const uint32_t*>(P.src_result + (size_t)r * P.F.result_stride);
+  d = reinterpret_cast<uint32_t*>(P.dst_result + (size_t)to * P.T.result_stride);
+  for (uint32_t o = lane * 4u; o < P.T.result_stride; o += 128u) d[o >> 2] = reshape_result_word(s, o, P.F, P.T);
+  if (lane == 0) P.dst_mark[to] = P.mark_value;
+}
+
+cudaError_t launch_transfer_fit(const TransferParams& P, cudaStream_t stream) {
+  if (P.n == 0) return cudaSuccess;
+  transfer_fit<<<(P.n - 1u) / 8u + 1u, 256, 0, stream>>>(P);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_transfer(const TransferParams& P, cudaStream_t stream) {
+  if (P.n == 0) return cudaSuccess;
+  transfer_runs<<<(P.n - 1u) / 8u + 1u, 256, 0, stream>>>(P);
+  return cudaGetLastError();
+}
+
 }  // namespace bf

@@ -1,6 +1,6 @@
 // resident_abi.cu — the C ABI of include/bobrafrontier.h for resident batches (row f2): a batch's records stay on the device
-// between ticks; uploads, deltas, migrations, redrives, reshapes, retirements and narrowings change them in place, and full, compact,
-// changed-only and touched ticks evaluate them.  The bookkeeping of touched ticks lives in Resident (ctx.h).
+// between ticks; uploads, deltas, migrations, redrives, reshapes, retirements and narrowings change them in place, transfers move
+// runs between batches, and full, compact, changed-only and touched ticks evaluate them.  The bookkeeping of touched ticks lives in Resident (ctx.h).
 #include <stdlib.h>
 #include <string.h>
 
@@ -606,6 +606,30 @@ int bf_resident_narrow(bf_ctx* c, uint32_t h, const bf_layout* layout, bf_extent
   return BF_OK;
 }
 
+// The move rule of a retirement, shared with transfers: the k-th retired index below m (ascending) receives the k-th live index
+// of [m, m + n); there are as many of each.  to[i] is the new index of run m + i, or kRetireNoMove.  -> the number of moves
+static uint32_t retire_moves(const std::vector<uint8_t>& gone, uint32_t m, uint32_t n, std::vector<uint32_t>& to) {
+  to.assign(n, bf::kRetireNoMove);
+  uint32_t n_moves = 0;
+  for (uint32_t i = 0, hole = 0; i < n; ++i) {
+    if (gone[m + i]) continue;
+    while (!gone[hole]) ++hole;
+    to[i] = hole++;
+    ++n_moves;
+  }
+  return n_moves;
+}
+
+// the moves of `to` into the caller's arrays (either may be NULL), ascending by target
+static void write_moves(const std::vector<uint32_t>& to, uint32_t m, uint32_t* moves_from, uint32_t* moves_to) {
+  for (uint32_t i = 0, k = 0; i < to.size() && (moves_from || moves_to); ++i) {
+    if (to[i] == bf::kRetireNoMove) continue;
+    if (moves_from) moves_from[k] = m + i;
+    if (moves_to) moves_to[k] = to[i];
+    ++k;
+  }
+}
+
 // Runs leave a live batch (resident.cu): the last live runs move into the indices the retired ones free, so the batch's runs
 // stay [0, n_runs - n).  All checks and allocations come first, so a rejected call or a failed allocation changes nothing.
 // One H2D copy of the move table, one launch, one synchronisation; a new capacity adds the prefix copies into its buffers.
@@ -627,15 +651,8 @@ int bf_resident_retire(bf_ctx* c, uint32_t h, bf_retire* rt) {
   if (cap < m || cap > r->cap) return fail(c, BF_EINVAL, "capacity must be 0 or within [n_runs - n, the current capacity]");
   const bool resize = cap != r->cap;
   if (n == 0 && !resize) { rt->n_moves = 0; return BF_OK; }
-  // the move rule: the k-th retired index below m (ascending) receives the k-th live index of [m, N); there are as many of each
-  std::vector<uint32_t> to(n, bf::kRetireNoMove);   // new index of run m + i
-  uint32_t n_moves = 0;
-  for (uint32_t i = 0, hole = 0; i < n; ++i) {
-    if (gone[m + i]) continue;
-    while (!gone[hole]) ++hole;
-    to[i] = hole++;
-    ++n_moves;
-  }
+  std::vector<uint32_t> to;
+  const uint32_t n_moves = retire_moves(gone, m, n, to);
   BF_CUDA(c, cudaSetDevice(c->device));
   if (int rc = c->d_retire.ensure(c, n ? n : 1)) return rc;
   const bf_layout& L = r->L;
@@ -658,12 +675,96 @@ int bf_resident_retire(bf_ctx* c, uint32_t h, bf_retire* rt) {
   c->stats.kernel_launches += n ? 1 : 0;
   if (resize) r->adopt(std::move(nb), L, cap);
   r->compact_to(m, N, to);
-  for (uint32_t i = 0, k = 0; i < n && (rt->moves_from || rt->moves_to); ++i) {
-    if (to[i] == bf::kRetireNoMove) continue;
-    if (rt->moves_from) rt->moves_from[k] = m + i;
-    if (rt->moves_to) rt->moves_to[k] = to[i];
-    ++k;
-  }
+  write_moves(to, m, rt->moves_from, rt->moves_to);
   rt->n_runs = m; rt->n_moves = n_moves;
+  return BF_OK;
+}
+
+// Live runs move from one batch of the ctx to another (resident.cu), re-laid to the destination's layout.  Both batches are
+// looked up under one hold of the ctx lock.  All argument checks, the allocation and the fit check (one H2D copy, one launch,
+// one D2H copy, one synchronisation) come before anything is written, so a refused or failed call changes nothing; then the
+// transfer launch, the source's retire launch and one synchronisation.
+int bf_resident_transfer(bf_ctx* c, uint32_t hs, uint32_t hd, bf_transfer* t) {
+  auto [g, src] = lock_resident(c, hs);
+  if (!t || t->struct_size != sizeof(bf_transfer)) return fail(c, BF_EINVAL, "null bf_transfer or bad struct_size");
+  t->unfit = BF_EXTENT_NO_RUN;
+  t->why = bf_extent{};
+  if (!src) return BF_EINVAL;
+  Resident* dst = hd < c->resident.size() && c->resident[hd].alive ? &c->resident[hd] : nullptr;
+  if (!dst) return fail(c, BF_EINVAL, "unknown resident batch");
+  if (hs == hd) return fail(c, BF_EINVAL, "a transfer from a batch to itself");
+  const uint32_t N = t->src_n_runs, D = t->dst_n_runs, n = t->n;
+  if (N > src->cap) return fail(c, BF_EINVAL, "src_n_runs exceeds the source batch");
+  if ((uint64_t)D + n > dst->cap) return fail(c, BF_EINVAL, "dst_n_runs + n exceeds the destination batch (reshape it first)");
+  if (n && !t->runs) return fail(c, BF_EINVAL, "null runs");
+  std::vector<uint8_t> gone(N, 0);
+  for (uint32_t i = 0; i < n; ++i) {
+    const uint32_t q = t->runs[i];
+    if (q >= N) return fail(c, BF_EINVAL, "runs[" + std::to_string(i) + "] is not below src_n_runs");
+    if (gone[q]) return fail(c, BF_EINVAL, "runs[" + std::to_string(i) + "] is moved twice");
+    gone[q] = 1;
+  }
+  if (n == 0) { t->n_moves = 0; return BF_OK; }
+  const uint32_t m = N - n;
+  std::vector<uint32_t> to;
+  const uint32_t n_moves = retire_moves(gone, m, n, to);
+  BF_CUDA(c, cudaSetDevice(c->device));
+  const size_t o_runs = 16, o_to = o_runs + (size_t)n * 4, o_ext = round_up_sz(o_to + (size_t)n * 4, 16), bytes = o_ext + (size_t)n * 16;
+  if (int rc = c->d_transfer.ensure(c, bytes)) return rc;
+  if (int rc = bf::sync_slots(c, c->stream)) return rc;
+  std::vector<uint8_t> blob(o_ext, 0);   // unfit word | runs | moves
+  const uint32_t none = BF_EXTENT_NO_RUN;
+  memcpy(blob.data(), &none, 4);
+  memcpy(blob.data() + o_runs, t->runs, (size_t)n * 4);
+  memcpy(blob.data() + o_to, to.data(), (size_t)n * 4);
+  const bf_layout F = src->L, T = dst->L;
+  bf::TransferParams P{};
+  P.src_state = src->d_state; P.src_result = src->d_result; P.src_mark = src->d_mark;
+  P.dst_state = dst->d_state; P.dst_result = dst->d_result; P.dst_mark = dst->d_mark; P.mark_value = dst->mark_must_list();
+  P.runs = reinterpret_cast<const uint32_t*>(c->d_transfer + o_runs); P.n = n; P.dst_first = D;
+  P.slots = c->slots_dev; P.n_slots = (uint32_t)c->slots_host.size();
+  // only result records a later tick of the source compares with count (bf_resident_extent's rule)
+  P.prev_runs = src->prev_valid ? src->prev_runs : 0u; P.eval_runs = src->touched_baseline_runs(); P.full_epoch = src->full_epoch;
+  P.F = F; P.T = T; P.R = F;
+  if (T.off_fail == BF_OFF_NONE) P.R.off_fail = BF_OFF_NONE;
+  if (T.off_needs_cond == BF_OFF_NONE) P.R.off_needs_cond = BF_OFF_NONE;
+  if (T.off_skip_dep == BF_OFF_NONE) P.R.off_skip_dep = BF_OFF_NONE;
+  if (T.off_phase_out == BF_OFF_NONE) P.R.off_phase_out = BF_OFF_NONE;
+  P.extent = reinterpret_cast<uint4*>(c->d_transfer + o_ext); P.unfit = reinterpret_cast<uint32_t*>(c->d_transfer.p);
+  cudaStream_t s = c->stream;
+  BF_CUDA(c, cudaMemcpyAsync(c->d_transfer, blob.data(), blob.size(), cudaMemcpyHostToDevice, s));
+  BF_CUDA(c, bf::launch_transfer_fit(P, s));
+  BF_CUDA(c, cudaMemcpyAsync(&c->pinned->word, c->d_transfer, 4, cudaMemcpyDeviceToHost, s));
+  BF_CUDA(c, cudaStreamSynchronize(s));
+  c->stats.kernel_launches += 1;
+  const uint32_t unfit = c->pinned->word;
+  if (unfit != BF_EXTENT_NO_RUN) {   // the refused run's extent, read on this path only
+    uint32_t x[4] = {};
+    BF_CUDA(c, cudaMemcpy(x, c->d_transfer + o_ext + (size_t)unfit * 16, 16, cudaMemcpyDeviceToHost));
+    t->unfit = unfit;
+    t->why.struct_size = sizeof(bf_extent); t->why.n_runs = N;
+    t->why.steps_max = std::max(1u, x[0]); t->why.child_nibbles = x[1]; t->why.fields = x[2];
+    t->why.widest_run = x[0] ? t->runs[unfit] : BF_EXTENT_NO_RUN;
+    return fail(c, BF_EINVAL, "runs[" + std::to_string(unfit) + "] (run " + std::to_string(t->runs[unfit]) +
+                                  ") does not fit the destination layout: it needs steps_max " + std::to_string(x[0]) +
+                                  ", child_nibbles " + std::to_string(x[1]) + ", fields " + std::to_string(x[2]));
+  }
+  // every arrival's record is a changed-only baseline of the source: the destination's may reach over them
+  bool src_baseline = src->prev_valid;
+  for (uint32_t i = 0; i < n && src_baseline; ++i) src_baseline = t->runs[i] < src->prev_runs;
+  src->end_snapshot(c);   // as after an upload, both batches
+  dst->end_snapshot(c);
+  bf::RetireParams Q{};
+  Q.state = src->d_state; Q.result = src->d_result; Q.mark = src->d_mark; Q.mark_value = src->mark_must_list();
+  Q.to = reinterpret_cast<const uint32_t*>(c->d_transfer + o_to); Q.m = m; Q.n = n;
+  Q.state_stride = F.state_stride; Q.result_stride = F.result_stride;
+  cudaError_t e = bf::launch_transfer(P, s);
+  if (e == cudaSuccess) e = bf::launch_retire(Q, s);   // behind the transfer on the stream: the sources are read first
+  if (int rc = src->sync_in_place(c, e, "bf_resident_transfer")) { dst->records_unknown(); return rc; }
+  c->stats.kernel_launches += 2;
+  src->compact_to(m, N, to);
+  dst->received(D, n, src_baseline);
+  write_moves(to, m, t->moves_from, t->moves_to);
+  t->src_n_runs = m; t->dst_n_runs = D + n; t->n_moves = n_moves;
   return BF_OK;
 }

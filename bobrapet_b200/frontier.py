@@ -276,6 +276,26 @@ class Frontier:
             raise err
         return e.as_dict()
 
+    def resident_transfer(self, src: int, dst: int, src_n: int, dst_n: int, runs) -> dict:
+        """bf_resident_transfer: move `runs` (distinct indices below src_n) of batch src to the end of batch dst's runs [0, dst_n),
+        re-laid at dst's layout; src compacts as after resident_retire.  -> dict(src_n_runs, dst_n_runs, moves_from, moves_to).
+        A refusal raises FrontierError with .unfit (position in runs of the first run dst cannot hold, or A.EXTENT_NO_RUN) and
+        .why (that run's extent, as resident_extent's dict)"""
+        rs = np.ascontiguousarray(runs, dtype=np.uint32)
+        n = rs.shape[0]
+        mf = np.zeros(max(n, 1), dtype=np.uint32)
+        mt = np.zeros(max(n, 1), dtype=np.uint32)
+        t = A.Transfer(struct_size=C.sizeof(A.Transfer), src_n_runs=int(src_n), dst_n_runs=int(dst_n), runs=rs.ctypes.data if n else None,
+                       n=n, moves_from=mf.ctypes.data, moves_to=mt.ctypes.data)
+        rc = self._lib.bf_resident_transfer(self._ctx, src, dst, C.byref(t))
+        if rc != A.BF_OK:
+            err = A.FrontierError(rc, "bf_resident_transfer: %s" % self._lib.bf_last_error(self._ctx).decode())
+            err.unfit = int(t.unfit)
+            err.why = t.why.as_dict()
+            raise err
+        return {"src_n_runs": int(t.src_n_runs), "dst_n_runs": int(t.dst_n_runs), "moves_from": mf[:t.n_moves].copy(),
+                "moves_to": mt[:t.n_moves].copy()}
+
     # -- resident batches: device-side state, delta uploads (row f2)
     DELTA_DTYPE = np.dtype([("run", "<u4"), ("index", "<u2"), ("field", "u1"), ("code", "u1")])
 

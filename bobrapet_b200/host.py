@@ -47,6 +47,7 @@ _SYMS = [
     ("bfh_batch_reshape", C.c_int, [C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32]),
     ("bfh_batch_retire", C.c_int, [C.c_void_p, C.c_void_p, C.c_uint32, C.c_uint32, C.c_void_p, C.c_void_p]),
     ("bfh_batch_narrow", C.c_int, [C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32]),
+    ("bfh_batch_transfer", C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p]),
     ("bfh_batch_eval", C.c_int, [C.c_void_p, C.c_uint32, C.POINTER(A.Counts)]),
     ("bfh_batch_set_resident", C.c_int, [C.c_void_p, C.c_int]),
     ("bfh_batch_traffic", C.c_int, [C.c_void_p, C.POINTER(C.c_uint64), C.POINTER(C.c_uint64), C.POINTER(C.c_uint32)]),
@@ -272,6 +273,16 @@ class HostBatch:
         mt = np.zeros(max(rs.shape[0], 1), np.uint32)
         k = self._chk(self._l.bfh_batch_retire(self._p, rs.ctypes.data if rs.shape[0] else None, rs.shape[0], capacity,
                                                mf.ctypes.data, mt.ctypes.data), "bfh_batch_retire")
+        return mf[:k].copy(), mt[:k].copy()
+
+    def transfer(self, dst: "HostBatch", runs):
+        """bfh_batch_transfer: move `runs` to the end of `dst`, re-laid at its layout, with their Stories and pending deltas (in
+        resident mode on the device too); this batch compacts as after retire.  -> (moves_from, moves_to), ascending by target"""
+        rs = np.ascontiguousarray(runs, dtype=np.uint32)
+        mf = np.zeros(max(rs.shape[0], 1), np.uint32)
+        mt = np.zeros(max(rs.shape[0], 1), np.uint32)
+        k = self._chk(self._l.bfh_batch_transfer(self._p, dst._p, rs.ctypes.data if rs.shape[0] else None, rs.shape[0],
+                                                 mf.ctypes.data, mt.ctypes.data), "bfh_batch_transfer")
         return mf[:k].copy(), mt[:k].copy()
 
     def size(self) -> int:

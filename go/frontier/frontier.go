@@ -438,6 +438,36 @@ func (r *Resident) Narrow(stepsMax, childNibbles, fields, nRuns uint32) (Extent,
 	return Extent{uint32(out[0]), uint32(out[1]), uint32(out[2]), uint32(out[3])}, r.c.err(rc)
 }
 
+// Transfer is what TransferTo reports.  SrcN and DstN are the batches' run counts afterwards; the source's run From[i] moved to
+// To[i] (bf_resident_retire's moves).  On a refusal because a run does not fit the destination layout, Unfit is its position
+// in runs and Why its own extent; otherwise Unfit is 0xFFFFFFFF.
+type Transfer struct {
+	SrcN, DstN uint32
+	From, To   []uint32
+	Unfit      uint32
+	Why        Extent
+}
+
+// TransferTo moves runs (distinct indices below srcN) of this batch to dst, a batch of the same Frontier, where runs[i] becomes
+// run dstN + i, re-laid to dst's layout with its state, its current result and a must-list mark (bf_resident_transfer).  This
+// batch compacts as by Retire: re-key its rows by From / To and the moved ones to dstN + i.  Use it for width classes: after
+// (or instead of) Migrate when a Story edit changes a run's class, and for a live straggler that holds a batch's width.  Grow
+// dst with Reshape first when it is full.  A refusal changes neither batch.
+func (r *Resident) TransferTo(dst *Resident, srcN, dstN uint32, runs []uint32) (Transfer, error) {
+	from := make([]uint32, len(runs)+1)
+	to := make([]uint32, len(runs)+1)
+	var rp *C.uint32_t
+	if len(runs) > 0 {
+		rp = (*C.uint32_t)(unsafe.Pointer(&runs[0]))
+	}
+	var counts, why [4]C.uint32_t
+	rc := C.bfgo_resident_transfer(r.c.p, r.handle, dst.handle, C.uint32_t(srcN), C.uint32_t(dstN), rp, C.uint32_t(len(runs)),
+		(*C.uint32_t)(unsafe.Pointer(&from[0])), (*C.uint32_t)(unsafe.Pointer(&to[0])), &counts[0], &why[0])
+	t := Transfer{SrcN: uint32(counts[0]), DstN: uint32(counts[1]), From: from[:counts[2]], To: to[:counts[2]], Unfit: uint32(counts[3]),
+		Why: Extent{uint32(why[0]), uint32(why[1]), uint32(why[2]), uint32(why[3])}}
+	return t, r.c.err(rc)
+}
+
 // Group is one operator process driving several GPUs (bf_group_*): contiguous blocks of runs per device, one NCCL
 // all-gather of the per-shard counts per pass, limiter totals all-reduced across the shards.
 type Group struct{ p *C.bf_group }

@@ -166,6 +166,25 @@ static inline int bfgo_resident_narrow(bf_ctx* c, uint32_t handle, uint32_t step
   return rc;
 }
 
+/* bf_resident_transfer with the bf_transfer built here on the C stack.  counts[4] = src_n_runs, dst_n_runs, n_moves, unfit
+ * (the n_runs given back and BF_EXTENT_NO_RUN moves on a refusal); why[4] = steps_max, child_nibbles, fields, widest_run of
+ * the run a fit refusal names. */
+static inline int bfgo_resident_transfer(bf_ctx* c, uint32_t src, uint32_t dst, uint32_t src_n_runs, uint32_t dst_n_runs,
+                                         const uint32_t* runs, uint32_t n, uint32_t* moves_from, uint32_t* moves_to,
+                                         uint32_t* counts, uint32_t* why) {
+  bf_transfer t;
+  memset(&t, 0, sizeof t);
+  t.struct_size = (uint32_t)sizeof t;
+  t.src_n_runs = src_n_runs; t.dst_n_runs = dst_n_runs; t.runs = runs; t.n = n; t.moves_from = moves_from; t.moves_to = moves_to;
+  const int rc = bf_resident_transfer(c, src, dst, &t);
+  counts[0] = rc == BF_OK ? t.src_n_runs : src_n_runs;
+  counts[1] = rc == BF_OK ? t.dst_n_runs : dst_n_runs;
+  counts[2] = rc == BF_OK ? t.n_moves : 0;
+  counts[3] = t.unfit;
+  why[0] = t.why.steps_max; why[1] = t.why.child_nibbles; why[2] = t.why.fields; why[3] = t.why.widest_run;
+  return rc;
+}
+
 static inline void bfgo_tables(bf_sched_tables* t, uint32_t n_stories, uint32_t n_queues, int32_t global_limit, uint32_t global_base,
                                const int32_t* story_limit, const uint32_t* story_base, const int32_t* queue_limit,
                                const int32_t* queue_aging_s, const uint32_t* queue_base, const int32_t* queue_max_priority_base) {

@@ -724,6 +724,53 @@ typedef struct bf_extent {
 int bf_resident_extent(bf_ctx* ctx, uint32_t handle, bf_extent* e);
 int bf_resident_narrow(bf_ctx* ctx, uint32_t handle, const bf_layout* layout, bf_extent* e);
 
+/* ------------------------------------------------------------------ transfers (live runs move between batches of one ctx)
+ * A batch has one layout, and every run in it pays for that layout on every pass: one Story of more than 512 steps moves the
+ * whole batch from the packed-lanes kernel to the one-run-per-warp one.  A batcher keeps width classes instead (several batches
+ * in one ctx, e.g. <= 64, <= 512 and <= 1024 steps, with and without decision planes or a child area; topology slots belong to
+ * the ctx, so a slot is valid in every batch of it).  bf_resident_transfer moves live runs from the batch src_handle to the
+ * batch dst_handle of the same ctx: when a Story edit changes a run's class, or a straggler holds a batch's width.
+ * The source's runs are [0, src_n_runs), the destination's [0, dst_n_runs); `runs` lists n distinct source runs, any order.
+ * Afterwards, by the bytes, with F the source layout and T the destination's:
+ *   - runs[i] lives at destination index dst_n_runs + i.  Its state record equals pack_state of the same codes at T: the header
+ *     as it was, each plane its low words with zero words above them, planes F lacks zero (cond PASS; decision PENDING, which a
+ *     pass applies where absent planes do not, exactly as after bf_resident_reshape), the child area its low bytes.  Its
+ *     current result record is what a pass at T writes for an unchanged run: the header as it was, each mask and phase_out plane
+ *     its low words, masks T lacks dropped, masks only T has zero.  Records at or above dst_n_runs before the call are not runs
+ *     and the arrivals overwrite them; records from dst_n_runs + n on keep their bytes.
+ *   - the source is byte-identical to bf_resident_retire of the same runs with capacity 0, and moves_from / moves_to receive
+ *     the same moves.
+ * Fit: each moved run must fit T under bf_resident_narrow's acceptance test applied to that run alone: the S and the child
+ * area of its slot when alive; its state record (highest non-zero code, non-PASS cond and non-PENDING decision codes, non-zero
+ * child nibbles); its current result record when a later tick of the source compares with it (the rule of bf_resident_extent),
+ * counting the planes T keeps.  unfit is the position in runs[] of the first run T cannot hold, and `why` that run's own extent
+ * (widest_run = its source index, or BF_EXTENT_NO_RUN when it needs no step).
+ * Checked before anything changes, else BF_EINVAL and both batches byte-identical: struct_size and both handles, src_handle !=
+ * dst_handle; src_n_runs <= the source capacity; dst_n_runs + n <= the destination capacity (bf_resident_reshape grows it
+ * first); runs not NULL when n > 0, every index below src_n_runs, none twice; every run fits.  A failed allocation is BF_ENOMEM
+ * and changes nothing.  n == 0 is a no-op.
+ * Touched ticks: the source follows bf_resident_retire (moved runs are listed, the call never forces a full tick by itself).
+ * In the destination the arrivals count as uploaded: the next bf_resident_tick_touched lists them and is not full because of
+ * them.  A BF_EVAL_CHANGED_ONLY tick of the destination over [0, dst_n_runs + n) right after the call lists what it would list
+ * had the arrivals always been there, when its last tick covered dst_n_runs and the source's last tick covered every moved
+ * run (else it lists every run).  Both batches end their evaluated snapshot (bf_schedule must follow a new pass).
+ * Cost: one H2D copy (runs and moves), the fit launch, one D2H copy and one synchronisation before anything is written; then
+ * the transfer and retire launches and one synchronisation.  Moving runs to another ctx (another GPU) is not offered.       */
+typedef struct bf_transfer {
+  uint32_t struct_size;        /* sizeof(bf_transfer)                                                                 */
+  uint32_t src_n_runs;         /* in: source runs are [0, src_n_runs); out: src_n_runs - n                            */
+  uint32_t dst_n_runs;         /* in: destination runs are [0, dst_n_runs); out: dst_n_runs + n                      */
+  const uint32_t* runs;        /* [n] source indices: distinct, each < src_n_runs, any order                          */
+  uint32_t n;
+  uint32_t* moves_from;        /* [n] out, may be NULL: the source's compaction moves, exactly bf_retire's            */
+  uint32_t* moves_to;          /* [n] out, may be NULL                                                                */
+  uint32_t n_moves;            /* out                                                                                 */
+  uint32_t unfit;              /* out: position in runs[] of the first run T cannot hold, BF_EXTENT_NO_RUN when all fit */
+  bf_extent why;               /* out on a fit refusal: that run's own extent                                         */
+} bf_transfer;
+
+int bf_resident_transfer(bf_ctx* ctx, uint32_t src_handle, uint32_t dst_handle, bf_transfer* t);
+
 /* ------------------------------------------------------------------ device groups (SURVEY.md row e)
  * The reference is ONE operator process (cmd/main.go:220, StoryRunReconciler storyrun_controller.go:216), so the
  * multi-GPU path must be reachable from one process through this ABI: a group owns one ctx per device and an NCCL

@@ -144,6 +144,17 @@ int bfh_batch_narrow(bfh_batch* b, uint32_t steps_max, uint32_t child_nibbles, u
  * nothing changed), BF_ENOMEM or the device's error.                                                                        */
 int bfh_batch_retire(bfh_batch* b, const uint32_t* runs, uint32_t n, uint32_t capacity, uint32_t* moves_from, uint32_t* moves_to);
 
+/* Move runs to another batch (see bf_resident_transfer): `runs` lists n distinct runs below bfh_batch_size(src); runs[i] becomes
+ * run bfh_batch_size(dst) + i of dst, with its Story, its records re-laid at dst's layout as bf_resident_transfer re-lays the
+ * device's, and its pending deltas, re-keyed to the new index.  src then equals bfh_batch_retire of the same runs with capacity
+ * 0 (the same moves into moves_from / moves_to, [n] each, may be NULL; the other pending deltas re-keyed likewise).  Each run
+ * must fit dst's layout by bf_resident_narrow's test applied to it alone (its record, its Story, its result record when the last
+ * eval covered it), and a pending delta of a moved run whose step, child index or field dst's layout lacks blocks the call.
+ * Both batches must be of one ctx (or both without one) and in the same mode.  In resident mode it first uploads the runs of
+ * both batches not yet on the device, then calls bf_resident_transfer; when that fails, neither mirror changes.  Returns the
+ * number of moves, or BF_EINVAL (bad arguments or a refusal, nothing changed) or the device's error.                       */
+int bfh_batch_transfer(bfh_batch* src, bfh_batch* dst, const uint32_t* runs, uint32_t n, uint32_t* moves_from, uint32_t* moves_to);
+
 /* One frontier pass over the batch through bf_eval (or, in resident mode, bf_resident_*) (eval_flags: BF_EVAL_*). */
 int bfh_batch_eval(bfh_batch* b, uint32_t eval_flags, bf_counts* counts);
 

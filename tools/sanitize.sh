@@ -1,7 +1,8 @@
 #!/bin/bash
 # tools/sanitize.sh: compute-sanitizer (memcheck, racecheck, synccheck) over small passes of every kernel shape — smoke() plus a
 # wide (S = 1024, parallel joins, 10-bit rows) and a pipelined batch, and a resident batch that takes an extent, a narrow (the
-# extent and re-layout kernels) and touched ticks on either side of it.  Prints the tools' summaries.
+# extent and re-layout kernels) and touched ticks on either side of it, then a transfer of some of its runs into a wider batch and
+# a transfer the fit check refuses (the fit, transfer and retire kernels).  Prints the tools' summaries.
 cd "$(dirname "$0")/.."
 cat > /tmp/san_probe.py <<'PY'
 import os, sys
@@ -63,7 +64,21 @@ st4 = f3.resident_download(h, 0, 600, Ln.state_stride)
 got, _ = f3.resident_tick(h, Ln, 600, np.zeros(0, dtype=Frontier.DELTA_DTYPE))
 want, _ = PK.evaluate(PK.PackedTopologies(ts4, s4), Ln, st4, threads=4)
 assert np.array_equal(got, want)
-f3.resident_destroy(h)
+# a transfer into a wider batch with every field (the fit and transfer kernels, the source's retire), one refused by the fit
+Lx = make_layout(1024, 16, A.F_COND | A.F_DECISION | A.F_CHILD | A.F_ALL_OUT)
+hx = f3.resident_create(Lx, 64)
+t = f3.resident_transfer(h, hx, 600, 0, np.arange(0, 600, 13, dtype=np.uint32))
+assert t["dst_n_runs"] == 47 and t["src_n_runs"] == 553
+o = f3.resident_tick_touched(hx, 47, np.zeros(0, dtype=Frontier.DELTA_DTYPE), 64, 1 << 20)
+assert o["full"] == 1 and o["n_listed"] == 47   # the destination's first tick
+hy = f3.resident_create(make_layout(8, 0, 0), 8)
+try:
+    f3.resident_transfer(hx, hy, 47, 0, np.arange(4, dtype=np.uint32))
+    raise AssertionError("a transfer the destination cannot hold was accepted")
+except A.FrontierError as err:
+    assert err.unfit != A.EXTENT_NO_RUN
+for x in (h, hx, hy):
+    f3.resident_destroy(x)
 print("probe ok")
 PY
 for tool in memcheck racecheck synccheck; do
