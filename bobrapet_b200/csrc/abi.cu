@@ -692,6 +692,10 @@ int schedule_host(bf_ctx* c, const bf_batch* b, const bf_sched_run* runs, const 
     return fail(c, BF_EINVAL, "bf_schedule must follow bf_eval / bf_resident_eval of the same batch (n_runs and layout) on this ctx");
   BF_CUDA(c, cudaSetDevice(c->device));
   cudaStream_t s = c->stream;
+  // topology puts and drops since the pass: the reduction reads the slot table as it is now (a dropped slot counts nothing; a
+  // stale device table could point at moved arena records, or hold fewer slots than n_slots)
+  if (int rc = bf::sync_slots(c, s)) return rc;
+  P.slots = c->slots_dev;
   // one device allocation: runs | records | story_running | queue_running | queue_maxprio | global | limits | bases
   const size_t n = b->n_runs, ns = t->n_stories, nq = t->n_queues;
   size_t off = 0;

@@ -23,7 +23,7 @@ DI int32_t effective_priority(int32_t base, uint32_t elapsed_s, int32_t aging) {
   if (elapsed_s == BF_SCHED_NONE || aging <= 0 || elapsed_s == 0u) return base;
   const uint32_t e = elapsed_s > 0x7FFFFFFFu ? 0x7FFFFFFFu : elapsed_s;  // int32(elapsed.Seconds())
   const int32_t steps = (int32_t)e / aging;
-  return steps > 0 ? base + steps : base;
+  return steps > 0 ? (int32_t)((uint32_t)base + (uint32_t)steps) : base;   // Go's int32 sum wraps; signed overflow is UB here
 }
 
 // totals start from the host's base counts (StepRuns of stories / queues the batch does not hold)

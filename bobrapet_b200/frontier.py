@@ -387,6 +387,25 @@ class Frontier:
         return {"records": rec, "story_running": sr[:sl.size], "queue_running": qr[:ql.size], "queue_max_priority": mp[:ql.size],
                 "global_running": int(gr[0])}
 
+    def schedule_device(self, L: A.Layout, n_runs: int, state_ptr: int, result_ptr: int, runs_ptr: int, records_ptr: int,
+                        story_running_ptr: int, queue_running_ptr: int, queue_max_priority_ptr: int, global_running_ptr: int,
+                        n_stories: int, n_queues: int, story_limit_ptr: int, queue_limit_ptr: int, queue_aging_ptr: int,
+                        global_limit: int = 0, global_running_base: int = 0, story_running_base_ptr: int = 0,
+                        queue_running_base_ptr: int = 0, queue_max_priority_base_ptr: int = 0, stream: int = 0):
+        """bf_schedule_device: every pointer is a device address (0 = NULL); the batch is the (state, result) pair of a
+        preceding eval_device.  The totals arrays are the reduction scratch and must be given.  Asynchronous on `stream`."""
+        t = A.SchedTables(struct_size=C.sizeof(A.SchedTables), n_stories=n_stories, n_queues=n_queues, global_limit=global_limit,
+                          global_running_base=global_running_base, story_limit=(story_limit_ptr or None),
+                          story_running_base=(story_running_base_ptr or None), queue_limit=(queue_limit_ptr or None),
+                          queue_aging_s=(queue_aging_ptr or None), queue_running_base=(queue_running_base_ptr or None),
+                          queue_max_priority_base=(queue_max_priority_base_ptr or None))
+        out = A.SchedOut(struct_size=C.sizeof(A.SchedOut), records=(records_ptr or None), story_running=(story_running_ptr or None),
+                         queue_running=(queue_running_ptr or None), queue_max_priority=(queue_max_priority_ptr or None),
+                         global_running=(global_running_ptr or None))
+        b = A.Batch(struct_size=C.sizeof(A.Batch), n_runs=n_runs, layout=L, state=(state_ptr or None), result=(result_ptr or None))
+        self._check(self._lib.bf_schedule_device(self._ctx, C.byref(b), C.c_void_p(runs_ptr or None), C.byref(t), C.byref(out),
+                                                 C.c_void_p(stream)), "bf_schedule_device")
+
     # -- evaluation over DEVICE buffers (async on `stream`)
     def eval_device(self, L: A.Layout, n_runs: int, state_ptr: int, result_ptr: int, counts_ptr: int = 0,
                     stream: int = 0, flags: int = 0, max_iterations: int = 0, expansion_ptr: int = 0,

@@ -340,6 +340,21 @@ int bf_eval_device(bf_ctx* ctx, const bf_batch* batch, void* stream);
  * time (queued_elapsed_s = int32((now - storyRunQueuedSince).Seconds()), BF_SCHED_NONE when nothing is queued
  * with a StartedAt), formatting "(%d running, limit %d)" from the totals returned here.
  * A run's own label priority is the priority its Story resolves to (ensureSchedulingLabels, scheduling.go:48-70).
+ *
+ * Edges (pinned by tests/test_gpu_schedule.py against oracle/limiters.py):
+ *   - a story_key >= n_stories / queue_key >= n_queues is counted in no story / queue total and gets no story limit,
+ *     no queue limit, no aging and no priority ordering; its Running steps still count globally, and the global
+ *     limit still applies to it;
+ *   - only the low 4 bits of run_phase are read;
+ *   - a run whose slot was dropped or never put contributes no Running steps and no step demand; its run_phase
+ *     still makes demand.  The slot table is read as it stands at the bf_schedule call: a slot dropped after the
+ *     pass counts nothing, a slot reused since counts its new topology;
+ *   - nothing is counted for phase codes at or past the topology's S, for registered bits >= its parallel step
+ *     count, or for a parallel step whose children lie past the layout's child area; a topology wider than the
+ *     layout (more words) counts nothing;
+ *   - the reduction reads the state records as stored, also after BF_EVAL_FIXPOINT: the counts stand for the
+ *     StepRuns of the cluster LISTs, which the in-memory iterations of runDagIterations do not change;
+ *   - effective priority = priority + aging steps in int32 arithmetic that wraps, as in Go (dag.go:1960).
  */
 #define BF_SCHED_NONE 0xFFFFFFFFu
 enum {                       /* why the steps in queued_sched were queued                               */

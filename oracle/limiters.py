@@ -129,17 +129,27 @@ def is_concurrency_queued(state: StepState) -> bool:
     return state.phase == "Pending" and state.message.startswith(QUEUED_PREFIXES)
 
 
+def wrap_int32(v: int) -> int:
+    """Go int32 arithmetic: the result modulo 2^32, read as signed."""
+    return ((int(v) + (1 << 31)) & 0xFFFFFFFF) - (1 << 31)
+
+
 def effective_priority(base: int, queued_since: Optional[float], aging_seconds: int, now: float) -> int:
-    """dag.go:1948-1961.  int32(elapsed.Seconds()) / agingSeconds, Go integer division."""
+    """dag.go:1948-1961.  int32(elapsed.Seconds()) / agingSeconds, Go integer division; `base + steps` is an int32 sum and
+    wraps as in Go (a priority near INT32_MAX that ages becomes a very low one).
+
+    One departure from Go: an elapsed time past INT32_MAX seconds (68 years) is read as INT32_MAX, the clamp of the
+    bf_sched_run contract (include/bobrafrontier.h: the host fills queued_elapsed_s so, and the kernel clamps).  Go's
+    int32(elapsed.Seconds()) is implementation-defined there (INT32_MIN on amd64, which makes effectivePriority return base)."""
     if queued_since is None or aging_seconds <= 0:
         return base
     elapsed = now - queued_since
     if elapsed <= 0:
         return base
-    steps = int(elapsed) // aging_seconds
+    steps = min(int(elapsed), 0x7FFFFFFF) // aging_seconds
     if steps <= 0:
         return base
-    return base + steps
+    return wrap_int32(base + steps)
 
 
 def story_run_queued_since(srun: ClusterStoryRun) -> Optional[float]:
@@ -271,10 +281,12 @@ assert SCHED_RUN_DTYPE.itemsize == 32
 
 
 def effective_priority_packed(priority: int, elapsed_s: int, aging: int) -> int:
+    """effective_priority over the bf_sched_run fields: elapsed_s above INT32_MAX reads as INT32_MAX (the host's
+    int32(elapsed.Seconds())), and the sum wraps to int32 as in Go."""
     if elapsed_s == NONE_U32 or aging <= 0 or elapsed_s == 0:
         return priority
     steps = min(elapsed_s, 0x7FFFFFFF) // aging
-    return priority + steps if steps > 0 else priority
+    return wrap_int32(priority + steps) if steps > 0 else priority
 
 
 def truncate_mask(words: np.ndarray, keep: int) -> np.ndarray:
@@ -293,28 +305,44 @@ def truncate_mask(words: np.ndarray, keep: int) -> np.ndarray:
     return out
 
 
+TERMINAL_PHASES = (3, 4, 5, 6, 7, 11, 12, 13)   # BF_LUT_TERMINAL
+
+
 def schedule_packed(run_running: np.ndarray, run_demand: np.ndarray, sched: np.ndarray, ready_masks: np.ndarray,
                     story_limit: np.ndarray, story_base: np.ndarray, queue_limit: np.ndarray, queue_aging: np.ndarray,
-                    queue_base: np.ndarray, global_limit: int, global_base: int):
+                    queue_base: np.ndarray, global_limit: int, global_base: int, queue_maxprio_base=None):
     """run_running[r]: Running StepRuns the batch attributes to run r (engram steps in phase Running + Running
     children of registered parallel steps); run_demand[r]: some step Running or queued (the run-phase part of
     storyRunHasDemand is added here from sched.run_phase).  Returns (launch, queued_story, queued_sched, info,
     story_running, queue_running, global_running, queue_maxprio); info[r] = (n_launch, n_queued_story,
-    n_queued_sched, reason)."""
+    n_queued_sched, reason).
+
+    The edges include/bobrafrontier.h pins in its limiter block: a story_key >= n_stories / queue_key >= n_queues is
+    counted in no story / queue total and gets no story limit, no queue limit, no aging and no priority ordering (its
+    steps still count globally and the global limit still applies); only the low 4 bits of run_phase are read; effective
+    priorities and the queue maxima are int32, the aging sum wrapping as in Go."""
     n, W = ready_masks.shape
+    ns, nq = len(story_limit), len(queue_limit)
     story_running = story_base.astype(np.int64).copy()
     queue_running = queue_base.astype(np.int64).copy()
-    np.add.at(story_running, sched["story_key"], run_running)
-    np.add.at(queue_running, sched["queue_key"], run_running)
-    global_running = int(global_base) + int(run_running.sum())
-    eff = np.array([effective_priority_packed(int(sched["priority"][r]), int(sched["queued_elapsed_s"][r]),
-                                              int(queue_aging[sched["queue_key"][r]])) for r in range(n)], dtype=np.int64)
-    term = np.isin(sched["run_phase"], [3, 4, 5, 6, 7, 11, 12, 13])
-    demand = np.isin(sched["run_phase"], [1, 2]) | (run_demand != 0)
-    maxprio = np.full(len(queue_limit), INT32_MIN, dtype=np.int64)
     for r in range(n):
-        if not term[r] and demand[r]:
-            q = sched["queue_key"][r]
+        k, q = int(sched["story_key"][r]), int(sched["queue_key"][r])
+        if k < ns:
+            story_running[k] += int(run_running[r])
+        if q < nq:
+            queue_running[q] += int(run_running[r])
+    global_running = int(global_base) + int(run_running.astype(np.int64).sum())
+    eff = np.array([effective_priority_packed(int(sched["priority"][r]), int(sched["queued_elapsed_s"][r]),
+                                              int(queue_aging[sched["queue_key"][r]]) if sched["queue_key"][r] < nq else 0)
+                    for r in range(n)], dtype=np.int32)
+    phase = sched["run_phase"] & 0xF
+    term = np.isin(phase, TERMINAL_PHASES)
+    demand = np.isin(phase, [1, 2]) | (run_demand != 0)
+    maxprio = (np.full(nq, INT32_MIN, dtype=np.int32) if queue_maxprio_base is None
+               else np.asarray(queue_maxprio_base, dtype=np.int32).copy())
+    for r in range(n):
+        q = int(sched["queue_key"][r])
+        if not term[r] and demand[r] and q < nq:
             maxprio[q] = max(maxprio[q], eff[r])
     launch = np.zeros_like(ready_masks)
     q_story = np.zeros_like(ready_masks)
@@ -324,7 +352,7 @@ def schedule_packed(run_running: np.ndarray, run_demand: np.ndarray, sched: np.n
         cur = ready_masks[r].copy()
         cnt = int(sum(bin(int(x)).count("1") for x in cur))
         k, q = int(sched["story_key"][r]), int(sched["queue_key"][r])
-        lim = int(story_limit[k])
+        lim = int(story_limit[k]) if k < ns else 0
         if cnt and lim > 0:
             slots = max(lim - int(story_running[k]), 0)
             if slots < cnt:
@@ -334,12 +362,12 @@ def schedule_packed(run_running: np.ndarray, run_demand: np.ndarray, sched: np.n
                 cnt = slots
         reason = REASON_NONE
         if cnt:
-            if maxprio[q] > eff[r]:
+            if q < nq and maxprio[q] > eff[r]:
                 q_sched[r] = cur
                 cur = np.zeros_like(cur)
                 reason = REASON_PRIORITY
             else:
-                gl, ql = int(global_limit), int(queue_limit[q])
+                gl, ql = int(global_limit), int(queue_limit[q]) if q < nq else 0
                 gslots = cnt if gl <= 0 else max(gl - global_running, 0)
                 qslots = cnt if ql <= 0 else max(ql - int(queue_running[q]), 0)
                 slots = min(cnt, gslots, qslots)

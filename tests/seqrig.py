@@ -2,6 +2,9 @@
 the device state are compared after it.  Used by the random sequences and the directed cases of test_gpu_resident_sequences.py."""
 from __future__ import annotations
 
+import zlib
+from collections import Counter
+
 import numpy as np
 
 from bobrapet_b200 import _abi as A
@@ -10,9 +13,11 @@ from bobrapet_b200.records import make_layout, pack_state
 from tests import migration as M
 from tests import redrive as RD
 from tests import resident_model as RM
+from tests import schedref as SR
 from tests.packing import topology_set
 
 NONE = np.zeros(0, dtype=Frontier.DELTA_DTYPE)
+TICK_KINDS = ("dense", "eval", "compact", "changed", "touched")
 
 
 def story_pool(rng, s_lo, s_hi, n_par, n_base, n_spare=2):
@@ -53,14 +58,6 @@ def random_records(rng, L, stories, slots):
                       dec if L.off_decision != A.OFF_NONE else None, child if L.off_child != A.OFF_NONE else None, reg)
 
 
-def sched_args(n):
-    from oracle import limiters as LM
-    sched = np.zeros(n, dtype=LM.SCHED_RUN_DTYPE)
-    sched["story_key"], sched["queue_key"] = np.arange(n) % 7, np.arange(n) % 3
-    sched["priority"], sched["queued_elapsed_s"], sched["run_phase"] = np.arange(n) % 5, LM.NONE_U32, 2
-    return sched, np.array([0, 1, 50, 400, 0, 3, 2000], np.int32), np.array([0, 300, 5000], np.int32), np.array([60, 0, 30], np.int32)
-
-
 class Rig:
     """one ctx and its model; batches are addressed by their model (RM.Batch) objects"""
 
@@ -69,6 +66,12 @@ class Rig:
         self.ts1 = [topology_set([p]) for p in stories]   # one TopologySet per pool Story, for bf_topology_put
         self.handles = {}
         self.log, self.label = [], label
+        # schedules: their own generator (the drivers' draws stay as they were), the last accepted tick as (batch, n_runs, kind,
+        # the call before it), and the compared schedules counted by that tick's kind and by the call before the tick
+        self.srng = np.random.default_rng(zlib.crc32(label.encode()))
+        self.prior, self.after = None, None
+        self.compared = Counter()
+        self.rotation = 0
 
     # -------------------------------------------------------------- failure reports name the sequence
     def where(self):
@@ -140,9 +143,11 @@ class Rig:
     def tick(self, b, kind, n_runs, d=NONE, flags=0, max_iter=0, runs_cap=None, events_cap=None, pinned=False):
         """kind: dense / eval / compact / changed / touched -> the touched tick's output dict (touched), else None"""
         h, fr = self.handles[b], self.fr
+        before = self.after or (self.log[-1].split()[0] if self.log else "start")
+        self.after = None
         self.log.append("%s b%d n %d deltas %d flags %d iter %d caps %s/%s%s" % (kind, h, n_runs, len(d), flags, max_iter, runs_cap,
                                                                           events_cap, " pinned" if pinned else ""))
-        out = None
+        out, r = None, None
         if kind in ("dense", "eval"):
             if kind == "dense":
                 r, _ = self._call(lambda: fr.resident_tick(h, b.L, n_runs, d, flags=flags, max_iterations=max_iter),
@@ -195,18 +200,50 @@ class Rig:
                            "touched events differ")
                 if not flags & A.EVAL_NO_COUNTS:
                     self.check(out["counts"] == want["counts"], "counts %s, want %s" % (out["counts"], want["counts"]))
+        if r:
+            self.prior = (b, n_runs, kind, before)
         self.sync()
         return out
 
     def schedule(self, b, n_runs):
-        self.log.append("schedule b%d n %d" % (self.handles[b], n_runs))
+        """bf_schedule with random sched runs and tables (tests/schedref.py generators); accepted or refused as the model says, and
+        when accepted, equal to the reference over the model's current result and state records"""
+        g = self.srng
+        ns, nq = int(g.choice([0, 1, 7, 40, 600])), int(g.choice([0, 1, 3, 9, 300]))
+        sched = SR.random_sched(g, n_runs, ns, nq, out_of_range=float(g.choice([0.0, 0.05])))
+        tables = SR.random_tables(g, ns, nq, n_runs, maxprio_base=bool(g.random() < 0.5))
+        self.log.append("schedule b%d n %d tables %d/%d" % (self.handles[b], n_runs, ns, nq))
         ok = b.schedule_ok(n_runs)
         try:
-            self.fr.schedule(b.L, n_runs, *sched_args(n_runs), global_limit=20000)
-            got = True
+            got = self.fr.schedule(b.L, n_runs, sched, **tables)
         except A.FrontierError:
-            got = False
-        self.check(got == ok, "bf_schedule %s, the model says %s" % ("accepted" if got else "refused", "accept" if ok else "refuse"))
+            got = None
+        self.check((got is not None) == ok, "bf_schedule %s, the model says %s" % ("accepted" if got is not None else "refused",
+                                                                                    "accept" if ok else "refuse"))
+        if got is None:
+            return
+        want = SR.expected(b.L, b.state[:n_runs], b.cur[:n_runs], SR.from_registry(self.reg), sched, tables)
+        try:
+            SR.assert_schedule(got, want)
+        except AssertionError as e:
+            self.check(False, str(e))
+        _, _, kind, before = self.prior
+        self.compared["tick " + kind] += 1
+        self.compared["after " + before] += 1
+
+    def tick_and_schedule(self, b, n_runs, after, flags=0, max_iter=0):
+        """a tick of the next kind in turn (no deltas) over the batch, then a schedule compared after it and counted as following
+        the call `after`"""
+        kind = TICK_KINDS[self.rotation % len(TICK_KINDS)]
+        self.rotation += 1
+        self.after = after
+        self.tick(b, kind, n_runs, NONE, flags, max_iter)
+        self.schedule_last()
+
+    def schedule_last(self):
+        """bf_schedule over the batch and n_runs of the last accepted tick (accepted unless a call since ended the snapshot)"""
+        if self.prior is not None:
+            self.schedule(*self.prior[:2])
 
     def migrate(self, b, old, new, n_runs):
         ps_old, ps_new = self.reg.stories[self.reg.live[old]], self.reg.stories[self.reg.live[new]] if new in self.reg.live else None

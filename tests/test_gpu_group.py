@@ -11,7 +11,7 @@ from bobrapet_b200.records import make_layout
 from oracle import limiters as LM
 from oracle import packed as PK
 from tests import randgen
-from tests.test_gpu_limiters import _running_and_demand
+from tests import schedref as SR
 
 pytestmark = pytest.mark.gpu
 
@@ -68,8 +68,6 @@ def test_group_schedule_holds_limits_across_shards(group, seed):
     want, wcounts = PK.evaluate(PK.PackedTopologies(ts, slots), L, state, threads=8)
     result, counts, _ = group.eval(L, state)
     assert np.array_equal(result, want) and counts == wcounts
-    W = L.words
-    ready = np.ascontiguousarray(result[:, L.off_ready:L.off_ready + 4 * W]).view("<u4").reshape(n, W)
     n_stories, n_queues = int(rng.integers(1, 20)), int(rng.integers(1, 5))
     sched = np.zeros(n, dtype=LM.SCHED_RUN_DTYPE)
     sched["story_key"] = rng.integers(0, n_stories, size=n)
@@ -86,16 +84,28 @@ def test_group_schedule_holds_limits_across_shards(group, seed):
     story_base = rng.integers(0, 5, size=n_stories).astype(np.uint32)
     queue_base = rng.integers(0, 50, size=n_queues).astype(np.uint32)
     global_base = int(queue_base.sum())
-    got = group.schedule(L, n, sched, story_limit, queue_limit, queue_aging, global_limit, story_base, queue_base, global_base)
-    run_running, run_demand = _running_and_demand(ts, topo, L, state)
-    launch, q_story, q_sched, info, sr, qr, gr, mp = LM.schedule_packed(
-        run_running, run_demand, sched, ready, story_limit, story_base, queue_limit, queue_aging, queue_base, global_limit, global_base)
-    assert np.array_equal(got["story_running"], sr.astype(np.uint32)) and np.array_equal(got["queue_running"], qr.astype(np.uint32))
-    assert got["global_running"] == gr and np.array_equal(got["queue_max_priority"].astype(np.int64), mp)
-    rec = got["records"]
-    masks = np.ascontiguousarray(rec[:, 16:16 + 12 * W]).view("<u4").reshape(n, 3, W)
-    assert np.array_equal(masks[:, 0], launch) and np.array_equal(masks[:, 1], q_story) and np.array_equal(masks[:, 2], q_sched)
-    assert np.array_equal(np.ascontiguousarray(rec[:, 0:16]).view("<u4").reshape(n, 4), info)
+    tables = dict(story_limit=story_limit, queue_limit=queue_limit, queue_aging_s=queue_aging, global_limit=global_limit,
+                  story_running_base=story_base, queue_running_base=queue_base, global_running_base=global_base)
+    got = group.schedule(L, n, sched, **tables)
+    SR.assert_schedule(got, SR.expected(L, state, result, SR.from_topology_set(ts, slots), sched, tables, loop=True))
+
+
+@pytest.mark.parametrize("seed", range(2))
+def test_group_schedule_edges(group, seed):
+    """the edge generator of test_gpu_schedule.py across shards: keys out of range, every run_phase, int32 priority extremes and
+    the wrap, limits at their extremes, padding and reserved codes, thousands of story keys, and queue_max_priority_base set"""
+    rng = np.random.default_rng(8200 + seed)
+    ts = randgen.random_topologies(rng, 30, 1, [300, 1024][seed], parallel=True)
+    slots = group.put_topologies_replicated(ts)
+    n = [6001, 3001][seed]
+    L, state, topo = randgen.random_state(rng, ts, slots, n, A.F_COND | A.F_DECISION, phase_mix="any", reserved=0.1, padding=True)
+    result, _, _ = group.eval(L, state)
+    descs = SR.from_topology_set(ts, slots)
+    for ns, nq in ((3000, 300), (0, 0), (7, 3)):
+        sched = SR.random_sched(rng, n, ns, nq, out_of_range=0.1)
+        tables = SR.random_tables(rng, ns, nq, n, maxprio_base=True)
+        SR.assert_schedule(group.schedule(L, n, sched, **tables), SR.expected(L, state, result, descs, sched, tables),
+                           "tables %d/%d" % (ns, nq))
 
 
 def test_group_rejects_bad_arguments(group):

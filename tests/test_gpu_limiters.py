@@ -1,4 +1,4 @@
-"""GPU parity of the limiters (rows a9 / f4): bf_eval -> bf_schedule through the C ABI vs oracle.limiters.schedule_packed,
+"""GPU parity of the limiters (rows a9 / f4): bf_eval -> bf_schedule through the C ABI vs tests/schedref.py (oracle.limiters.schedule_packed),
 bit for bit, on adversarial random batches (all step types, parallel children, every phase code) and random
 stories / queues / limits / priorities."""
 import numpy as np
@@ -6,9 +6,9 @@ import pytest
 
 from bobrapet_b200 import _abi as A
 from bobrapet_b200 import Frontier
-from bobrapet_b200.records import _unpack_planes
 from oracle import limiters as LM
 from tests import randgen
+from tests import schedref as SR
 
 pytestmark = pytest.mark.gpu
 
@@ -18,41 +18,6 @@ def fr():
     f = Frontier(0)
     yield f
     f.close()
-
-
-def _running_and_demand(ts, topo, L, state):
-    """the checker's own derivation of the per-run reductions from the packed state records"""
-    n = state.shape[0]
-    W = L.words
-    S_off = np.concatenate(([0], np.cumsum(ts.S.astype(np.int64))))
-    P_off = np.concatenate(([0], np.cumsum(ts.P.astype(np.int64))))
-    cfs, _ = randgen.child_layout(ts)
-    run_running = np.zeros(n, dtype=np.uint32)
-    run_demand = np.zeros(n, dtype=np.uint32)
-    codes = _unpack_planes(state[:, L.off_phase:L.off_phase + W * 16], W, 4, W * 32)
-    codes[codes == 15] = 0
-    for r in range(n):
-        t = int(topo[r])
-        S = int(ts.S[t])
-        ph = codes[r, :S]
-        types = ts.step_flags[S_off[t]:S_off[t] + S] & A.SF_TYPE_MASK
-        cnt = int(((ph == 2) & (types == 0)).sum())
-        if L.off_child != A.OFF_NONE and int(ts.P[t]):
-            reg = int(np.ascontiguousarray(state[r, 8:16]).view("<u8")[0])
-            nb = (L.child_nibbles + 1) // 2
-            raw = state[r, L.off_child:L.off_child + nb]
-            nib = np.empty(nb * 2, dtype=np.uint8)
-            nib[0::2] = raw & 0xF
-            nib[1::2] = raw >> 4
-            nib[nib == 15] = 0
-            for q in range(int(ts.P[t])):
-                if (reg >> q) & 1:
-                    B = int(ts.parallel["branches"][P_off[t] + q])
-                    c0 = int(cfs[t][q])
-                    cnt += int((nib[c0:c0 + B] == 2).sum())
-        run_running[r] = cnt
-        run_demand[r] = int(((ph == 2) | (ph == 14)).any())
-    return run_running, run_demand
 
 
 @pytest.mark.parametrize("seed", range(8))
@@ -83,22 +48,12 @@ def test_schedule_matches_oracle(fr, seed):
     story_base = rng.integers(0, 5, size=n_stories).astype(np.uint32)
     queue_base = rng.integers(0, 50, size=n_queues).astype(np.uint32)
     global_base = int(queue_base.sum())
-    got = fr.schedule(L, n, sched, story_limit, queue_limit, queue_aging, global_limit, story_base, queue_base, global_base)
-    run_running, run_demand = _running_and_demand(ts, topo, L, state)
-    launch, q_story, q_sched, info, sr, qr, gr, mp = LM.schedule_packed(
-        run_running, run_demand, sched, ready, story_limit, story_base, queue_limit, queue_aging, queue_base, global_limit, global_base)
-    assert np.array_equal(got["story_running"], sr.astype(np.uint32))
-    assert np.array_equal(got["queue_running"], qr.astype(np.uint32))
-    assert got["global_running"] == gr
-    assert np.array_equal(got["queue_max_priority"].astype(np.int64), mp)
+    tables = dict(story_limit=story_limit, queue_limit=queue_limit, queue_aging_s=queue_aging, global_limit=global_limit,
+                  story_running_base=story_base, queue_running_base=queue_base, global_running_base=global_base)
+    got = fr.schedule(L, n, sched, **tables)
+    SR.assert_schedule(got, SR.expected(L, state, result, SR.from_topology_set(ts, slots), sched, tables, loop=True))
     rec = got["records"]
-    hdr = np.ascontiguousarray(rec[:, 0:16]).view("<u4").reshape(n, 4)
     masks = np.ascontiguousarray(rec[:, 16:16 + 12 * W]).view("<u4").reshape(n, 3, W)
-    assert np.array_equal(masks[:, 0], launch), "launch masks differ"
-    assert np.array_equal(masks[:, 1], q_story), "story-queued masks differ"
-    assert np.array_equal(masks[:, 2], q_sched), "sched-queued masks differ"
-    assert np.array_equal(hdr, info)
-    assert not rec[:, 16 + 12 * W:].any()
     # the three masks partition the ready set (every ready step is launched or queued, dag.go:1709-1728)
     assert np.array_equal(masks[:, 0] | masks[:, 1] | masks[:, 2], ready)
 

@@ -10,7 +10,7 @@ from bobrapet_b200 import Frontier
 from bobrapet_b200.records import make_layout
 from tests.narrowing import NarrowRig
 from tests.seqrig import NONE, layout_for, story_pool
-from tests.test_gpu_resident_sequences import N_BASE, Driver
+from tests.test_gpu_resident_sequences import N_BASE, Driver, assert_schedules_compared, close_with_schedules
 
 pytestmark = pytest.mark.gpu
 
@@ -49,6 +49,7 @@ class NarrowDriver(Driver):
             rig.upload(b, 0, self._fresh(L, n))
             self.bs.append([b, n])
         self.flags, self.max_iter, self.accepted = 0, 0, 0
+        self.followed = set()
 
     def _fresh(self, L, n):
         recs = super()._fresh(L, n)
@@ -60,7 +61,8 @@ class NarrowDriver(Driver):
 
     def narrow(self):
         rng, rig = self.rng, self.rig
-        b, n = self.bs[0 if rng.random() < 0.75 else 1]
+        bi = 0 if rng.random() < 0.75 else 1
+        b, n = self.bs[bi]
         L = b.L
         nr = n if rng.random() < 0.8 else int(rng.integers(0, b.cap + 1))
         e = rig.extent(b, nr)
@@ -76,6 +78,7 @@ class NarrowDriver(Driver):
             f = L.fields & ~int(rng.choice([0, 0, COND, DEC, CHILD, OUT]))
             child = int(rng.integers(0, L.child_nibbles + 1)) if f & CHILD else 0
         self.accepted += rig.narrow(b, make_layout(S, child, f), nr)
+        self.follow(bi, "narrow")
 
     def step(self):
         u = self.rng.random()
@@ -102,6 +105,8 @@ def test_random_sequences_with_narrows(fr, shape, seed):
         for b, n in dr.bs:   # a closing tick of each kind over the batch as it ends
             dr.rig.tick(b, "touched", n, NONE, dr.flags, dr.max_iter)
             dr.rig.tick(b, "changed", n, NONE, dr.flags, dr.max_iter)
+        close_with_schedules(dr)
     finally:
         dr.rig.destroy()
     assert dr.accepted > 0, "no narrow was accepted"
+    assert_schedules_compared(dr)

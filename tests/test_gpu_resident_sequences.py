@@ -1,7 +1,8 @@
 """Random sequences of resident-batch calls in the order a batcher makes them (INTEGRATION.md: put, create, upload, tick; put an
 edited Story, migrate, drop the old one; redrive; reshape an outgrown batch; retire finished runs), two batches on one ctx,
 checked after every call against the host model of tests/resident_model.py: the device state, every tick output, the `full`
-flag of every touched tick, the moves, statuses and counts, and which calls are refused.  Then directed cases for the
+flag of every touched tick, the moves, statuses and counts, which calls are refused, and every accepted bf_schedule against
+tests/schedref.py over the model's records.  Then directed cases for the
 combinations the random draws reach rarely."""
 import numpy as np
 import pytest
@@ -10,7 +11,7 @@ from bobrapet_b200 import _abi as A
 from bobrapet_b200 import Frontier
 from bobrapet_b200.records import make_layout
 from tests import retire as RT
-from tests.seqrig import NONE, Rig, layout_for, random_records, story_pool
+from tests.seqrig import NONE, TICK_KINDS, Rig, layout_for, random_records, story_pool
 
 pytestmark = pytest.mark.gpu
 
@@ -82,6 +83,16 @@ class Driver:
             rig.upload(b, 0, self._fresh(L, n))
             self.bs.append([b, n])
         self.flags, self.max_iter = 0, 0
+        self.followed = set()
+
+    def follow(self, bi, op):
+        """after a resident operation: the first time for each kind of operation and then now and then, a tick over the batch and
+        a schedule compared after it"""
+        if op in self.followed and self.rig.srng.random() >= 0.5:
+            return
+        self.followed.add(op)
+        b, n = self.bs[bi]
+        self.rig.tick_and_schedule(b, n, op, self.flags, self.max_iter)
 
     def _fresh(self, L, n):
         live = [s for s in self.rig.reg.live if s in self.base or s in self.edited]
@@ -107,6 +118,8 @@ class Driver:
         elif op == "tick":
             kind = str(rng.choice(["dense", "eval", "compact", "changed", "changed"]))
             rig.tick(b, kind, n, _deltas(rng, rig, b, max(n, 1), int(rng.integers(0, 200))) if n else NONE, self.flags, self.max_iter)
+            if rig.srng.random() < 0.5:
+                rig.schedule_last()
         elif op == "touched":
             u = rng.random()   # mostly the live runs; sometimes fewer, or more (records the batch holds past its live runs)
             nr = n if u < 0.8 else int(rng.integers(0, n + 1)) if u < 0.93 else int(rng.integers(n, b.cap + 1))
@@ -115,6 +128,8 @@ class Driver:
             rig.tick(b, "touched", nr, d, self.flags | (A.EVAL_NO_COUNTS if rng.random() < 0.1 else 0), self.max_iter,
                      runs_cap=int(rng.integers(0, 50)) if caps else None, events_cap=int(rng.integers(0, 500)) if caps else None,
                      pinned=rng.random() < 0.2)
+            if rig.srng.random() < 0.5:
+                rig.schedule_last()
         elif op == "migrate":
             todo = [k for k in range(N_BASE) if k not in self.migrated and self.base[k] in rig.reg.live]
             if todo:
@@ -129,6 +144,7 @@ class Driver:
                         rig.drop(self.base[k])
                 else:
                     rig.drop(new)
+                self.follow(bi, "migrate")
         elif op == "redrive" and n:
             k = int(rng.integers(1, 40))
             runs = rng.integers(0, n, size=k)
@@ -140,6 +156,7 @@ class Driver:
             req["slot"] = [s if (s in rig.reg.live and rng.random() < 0.9) else int(rng.choice(live)) for s in slots.tolist()]
             req["step"] = [A.REDRIVE_ALL if rng.random() < 0.3 else int(rng.integers(0, rig.reg.story(int(s)).S)) for s in req["slot"]]
             rig.redrive(b, req)
+            self.follow(bi, "redrive")
         elif op == "reshape":
             L = b.L
             S = L.steps_max + (32 if rng.random() < 0.3 else 0)
@@ -148,6 +165,7 @@ class Driver:
             f = L.fields | int(rng.choice([0, COND, DEC, A.F_OUT_FAIL, A.F_OUT_NEEDS_COND, A.F_OUT_SKIP_DEP]))
             child = L.child_nibbles + (8 if (L.off_child != A.OFF_NONE and rng.random() < 0.3) else 0)
             rig.reshape(b, make_layout(S, child, f), b.cap + int(rng.choice([0, 0, 16, b.cap])))
+            self.follow(bi, "reshape")
         elif op == "retire" and n:
             k = int(rng.integers(0, n // 3 + 1))
             runs = rng.choice(n, size=k, replace=False)
@@ -155,6 +173,7 @@ class Driver:
             cap = int(rng.choice([0, m, (m + b.cap + 1) // 2])) if m else 0
             if rig.retire(b, n, runs, cap) is not None:
                 self.bs[bi][1] = m
+            self.follow(bi, "retire")
         elif op == "slots":
             if rng.random() < 0.5:   # drop a slot runs still hold (not one of the base Stories the generators draw from)
                 held = [s for s in rig.reg.live if s not in self.base and s not in self.edited]
@@ -173,8 +192,11 @@ class Driver:
         elif op == "params":
             self.flags = int(rng.choice([0, A.EVAL_FIXPOINT]))
             self.max_iter = int(rng.choice([0, 0, 1, 3])) if self.flags else 0
-        elif op == "schedule" and n:
-            rig.schedule(b, n)
+        elif op == "schedule" and n:   # mostly over the last tick's batch and n_runs; sometimes a batch or count it did not evaluate
+            if rig.srng.random() < 0.85:
+                rig.schedule_last()
+            else:
+                rig.schedule(b, n)
         elif op == "invalid":
             kind = int(rng.integers(0, 6))
             if kind == 0 and n:
@@ -205,8 +227,25 @@ def test_random_sequences(fr, shape, seed):
         for b, n in dr.bs:   # a closing tick of each kind over the batch as it ends
             dr.rig.tick(b, "touched", n, NONE, dr.flags, dr.max_iter)
             dr.rig.tick(b, "changed", n, NONE, dr.flags, dr.max_iter)
+        close_with_schedules(dr)
     finally:
         dr.rig.destroy()
+    assert_schedules_compared(dr)
+
+
+def close_with_schedules(dr):
+    """a tick of every kind over batch A as it ends, each followed by a compared schedule"""
+    b, n = dr.bs[0]
+    for kind in TICK_KINDS:
+        dr.rig.tick(b, kind, n, NONE, dr.flags, dr.max_iter)
+        dr.rig.schedule_last()
+
+
+def assert_schedules_compared(dr):
+    """the sequence compared schedules after every tick kind, and after every kind of resident operation it made"""
+    c = dr.rig.compared
+    missing = ["tick " + k for k in TICK_KINDS if not c["tick " + k]] + ["after " + op for op in sorted(dr.followed) if not c["after " + op]]
+    assert not missing, "no schedule compared for %s; compared: %s" % (missing, dict(c))
 
 
 # ------------------------------------------------------------------------------------------------ directed cases

@@ -11,7 +11,7 @@ from bobrapet_b200 import Frontier
 from bobrapet_b200.records import make_layout
 from tests.seqrig import NONE, layout_for, random_records, story_pool
 from tests.test_gpu_narrow_sequences import NarrowDriver
-from tests.test_gpu_resident_sequences import N_BASE
+from tests.test_gpu_resident_sequences import N_BASE, assert_schedules_compared, close_with_schedules
 from tests.transfer import TransferRig, fits, run_extent
 
 pytestmark = pytest.mark.gpu
@@ -53,6 +53,7 @@ class TransferDriver(NarrowDriver):
             rig.upload(b, 0, self._fresh(L, n))
             self.bs.append([b, n])
         self.flags, self.max_iter, self.accepted, self.moved = 0, 0, 0, 0
+        self.followed = set()
 
     def _fresh(self, L, n):
         """new runs on the live Stories the layout holds (a narrow may have taken a batch below some of them); runs on a slot no
@@ -92,6 +93,7 @@ class TransferDriver(NarrowDriver):
         if out is not None:
             self.bs[i][1], self.bs[1 - i][1] = out["src_n_runs"], out["dst_n_runs"]
             self.moved += len(runs)
+        self.follow(1 - i, "transfer")
 
     def step(self):
         if self.rng.random() < 0.15:
@@ -113,6 +115,8 @@ def test_random_sequences_with_transfers(fr, shape, seed):
         for b, n in dr.bs:   # a closing tick of each kind over the batch as it ends
             dr.rig.tick(b, "touched", n, NONE, dr.flags, dr.max_iter)
             dr.rig.tick(b, "changed", n, NONE, dr.flags, dr.max_iter)
+        close_with_schedules(dr)
     finally:
         dr.rig.destroy()
     assert dr.moved > 0, "no transfer was accepted"
+    assert_schedules_compared(dr)

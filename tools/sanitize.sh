@@ -1,8 +1,9 @@
 #!/bin/bash
 # tools/sanitize.sh: compute-sanitizer (memcheck, racecheck, synccheck) over small passes of every kernel shape — smoke() plus a
-# wide (S = 1024, parallel joins, 10-bit rows) and a pipelined batch, and a resident batch that takes an extent, a narrow (the
-# extent and re-layout kernels) and touched ticks on either side of it, then a transfer of some of its runs into a wider batch and
-# a transfer the fit check refuses (the fit, transfer and retire kernels).  Prints the tools' summaries.
+# wide (S = 1024, parallel joins, 10-bit rows) and a pipelined batch, the limiters over the latter (bf_schedule_device), and a
+# resident batch that takes an extent, a narrow (the extent and re-layout kernels) and touched ticks on either side of it, then a
+# transfer of some of its runs into a wider batch and a transfer the fit check refuses (the fit, transfer and retire kernels).
+# Prints the tools' summaries.
 cd "$(dirname "$0")/.."
 cat > /tmp/san_probe.py <<'PY'
 import os, sys
@@ -42,6 +43,13 @@ with torch.cuda.stream(s):
 torch.cuda.synchronize()
 for k in range(3):
     assert np.array_equal(res[k].cpu().numpy(), w3) and cnt[k].cpu().numpy().tolist() == [wc3["ready"], wc3["skip"], wc3["expansion"], wc3["evals"]]
+# the limiters on the device path over the pipelined batch: tables that span several sched_init blocks, keys out of range
+from tests import schedref as SR
+rs = np.random.default_rng(6)
+sched = SR.random_sched(rs, 1500, 700, 40, out_of_range=0.05)
+tables = SR.random_tables(rs, 700, 40, 1500, maxprio_base=True)
+got = SR.schedule_device(f2, L3, 1500, d_state, res[2], sched, tables, s)
+SR.assert_schedule(got, SR.expected(L3, st3, w3, SR.from_topology_set(ts3, s3), sched, tables))
 from tests import randgen
 from tests import reshape as RS
 rng = np.random.default_rng(5)
