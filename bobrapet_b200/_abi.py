@@ -153,6 +153,16 @@ class Transfer(C.Structure):
                 ("unfit", C.c_uint32), ("why", Extent)]
 
 
+TIMER_NONE = 0xFFFFFFFF   # BF_TIMER_NONE: an empty slot's deadline; as a request's deadline it cancels
+TIMER_MAX_SLOTS = 64      # BF_TIMER_MAX_SLOTS
+
+
+class FireOut(C.Structure):
+    _fields_ = [("struct_size", C.c_uint32), ("n_runs", C.c_uint32), ("n_fired", C.c_uint32), ("n_written", C.c_uint32),
+                ("n_pruned", C.c_uint32), ("next_deadline", C.c_uint32), ("fired", C.c_void_p), ("fired_cap", C.c_uint32),
+                ("reserved", C.c_uint32)]
+
+
 class SchedTables(C.Structure):
     _fields_ = [("struct_size", C.c_uint32), ("n_stories", C.c_uint32), ("n_queues", C.c_uint32), ("global_limit", C.c_int32),
                 ("global_running_base", C.c_uint32), ("story_limit", C.c_void_p), ("story_running_base", C.c_void_p),
@@ -205,6 +215,10 @@ SYMBOLS = [
     ("bf_resident_extent", C.c_int, [C.c_void_p, C.c_uint32, C.POINTER(Extent)]),
     ("bf_resident_narrow", C.c_int, [C.c_void_p, C.c_uint32, C.POINTER(Layout), C.POINTER(Extent)]),
     ("bf_resident_transfer", C.c_int, [C.c_void_p, C.c_uint32, C.c_uint32, C.POINTER(Transfer)]),
+    ("bf_resident_timers", C.c_int, [C.c_void_p, C.c_uint32, C.c_uint32]),
+    ("bf_resident_timers_arm", C.c_int, [C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32]),
+    ("bf_resident_fire", C.c_int, [C.c_void_p, C.c_uint32, C.c_uint32, C.POINTER(FireOut)]),
+    ("bf_resident_timers_download", C.c_int, [C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32, C.c_void_p]),
     ("bf_group_create", C.c_int, [C.POINTER(C.c_void_p), C.POINTER(C.c_int32), C.c_uint32, C.POINTER(Config)]),
     ("bf_group_destroy", None, [C.c_void_p]),
     ("bf_group_size", C.c_uint32, [C.c_void_p]),

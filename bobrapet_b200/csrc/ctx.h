@@ -39,6 +39,9 @@ cudaError_t launch_retire(const RetireParams& P, cudaStream_t stream);
 cudaError_t launch_extent(const ExtentParams& P, uint32_t sm_count, cudaStream_t stream);
 cudaError_t launch_transfer_fit(const TransferParams& P, cudaStream_t stream);
 cudaError_t launch_transfer(const TransferParams& P, cudaStream_t stream);
+cudaError_t launch_relay_timers(const TimerRelayParams& P, cudaStream_t stream);
+cudaError_t launch_arm_timers(const TimerArmParams& P, bool merge, cudaStream_t stream);
+cudaError_t launch_fire(const FireParams& P, cudaStream_t stream);
 cudaError_t launch_schedule(const SchedParams& P, uint32_t sm_count, cudaStream_t stream, uint32_t phases = 3);
 cudaError_t launch_closure(const Slot* slots, const uint32_t* slot_ids, const uint32_t* starts, uint32_t n, uint32_t n_slots,
                            uint32_t words_out, uint32_t* masks, cudaStream_t stream);
@@ -165,6 +168,7 @@ struct bf_ctx {
   struct Pinned {
     uint32_t word;         // a 4-byte device counter: rejected deltas where no compaction delivers them, migrated runs
     bf::ResultTail tail;   // written by a compaction's last kernel; a pass without one copies its counts into tail.counts
+    uint32_t fire[4];      // bf_resident_fire: n_fired, n_written, n_pruned, next_deadline
     bf_counts counts() const { return {tail.counts[0], tail.counts[1], tail.counts[2], tail.counts[3]}; }
   }* pinned = nullptr;
   DevBuf<bf_expansion> d_exp;
@@ -195,6 +199,9 @@ struct bf_ctx {
   DevBuf<unsigned long long> d_extent;
   // transfers (bf_resident_transfer): [0, 16) the unfit word | source runs | retire moves | per-run extents (uint4)
   DevBuf<uint8_t> d_transfer;
+  // step timers: arms ([0, 16) the overflow word | group starts | arming prefix | sorted requests) and fires ([0, 16) the four
+  // output words | per-CTA fired counts | the fired list)
+  DevBuf<uint8_t> d_timer;
 
   // limiters (bf_schedule): the records the last pass evaluated (bf_eval's staging or a resident batch), read in place.  Cleared
   // (valid = false) when a pass starts or a call changes those records (end_snapshot); assigned whole once a pass went through.
@@ -266,6 +273,9 @@ inline int cuda_fail(bf_ctx* c, cudaError_t e, const char* what) {
 //   (transfer)         the source compacts as by retire (compact_to); the destination takes the arrivals as uploads (received).
 //   uploaded           merged [first, end) ranges, keyed by first, of the runs at or above full_runs uploaded since the last full
 //                      tick (note_uploaded); compact_to clips them; full_tick_done clears them.
+//   d_timers, timer_k  the step-timer area (bf_resident_timers): cap * timer_k slots, or none (timer_k = 0).  Arm and fire
+//                      change it; retire, transfer, migrate and redrive re-key it in the launches that move the records;
+//                      reshape and a retire to a new capacity re-allocate it; narrow keeps it (the capacity stays).
 // A call that changes d_state ends the evaluated snapshot (end_snapshot): bf_schedule must follow a new pass.
 struct Resident {
   bool alive = false, prev_valid = false, need_full = true;
@@ -273,6 +283,8 @@ struct Resident {
   uint32_t cap = 0, prev_runs = 0, epoch = 1, full_epoch = 0, full_runs = 0, last_fixpoint = 0, last_max_iter = 0;
   DevBuf<uint8_t> d_state, d_result, d_result_prev;
   DevBuf<uint32_t> d_mark;
+  DevBuf<unsigned long long> d_timers;
+  uint32_t timer_k = 0;
   uint64_t slot_changes_seen = 0, pending = 0;
   std::map<uint32_t, uint32_t> uploaded;
 

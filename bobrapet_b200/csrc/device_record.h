@@ -237,6 +237,9 @@ struct MigrateParams {
   uint32_t n_runs, old_slot, new_slot;
   uint32_t words, state_stride, off_phase, off_cond, off_decision, off_child;
   uint32_t child_nibbles;        // of the layout; the child area is ceil(child_nibbles / 8) u32 words
+  unsigned long long* timers;    // [capacity][timer_k] the batch's timer slots (bf_timer_slot), or nullptr: no area
+  const uint16_t* fwd;           // [n_old_steps] the step map (new index of old step i, or BF_MIGRATE_GONE), for the timers
+  uint32_t timer_k, n_old_steps;
 };
 
 // bf_resident_redrive (resident.cu): the reset sets of the requests are cleared in the records of their runs
@@ -251,6 +254,8 @@ struct RedriveParams {
   const Slot* slots;
   uint32_t n;
   uint32_t words, state_stride, off_phase, off_cond, off_decision, off_child;
+  unsigned long long* timers;    // [capacity][timer_k] timer slots, or nullptr: an applied request empties its run's
+  uint32_t timer_k;
 };
 
 // bf_resident_reshape (resident.cu): both record arrays re-laid from layout `from` into new buffers at layout `to`
@@ -273,6 +278,8 @@ struct RetireParams {
   const uint32_t* to;            // [n] the new index of run m + i, or kRetireNoMove for a retired run
   uint32_t m, n;
   uint32_t state_stride, result_stride;   // multiples of 16
+  unsigned long long* timers;    // [capacity][timer_k] timer slots, or nullptr: a mover's slots move with it, vacated ones empty
+  uint32_t timer_k;
 };
 
 // bf_resident_extent / _narrow (resident.cu): the smallest layout a batch's records and the topologies of its runs allow.  Each
@@ -292,6 +299,8 @@ struct ExtentParams {
   bf_layout L;                   // the batch's layout
   bf_layout R;                   // L with the result fields that do not count set to BF_OFF_NONE
   unsigned long long* out;       // [3], zeroed by the caller: steps, child nibbles (both extent << 32 | ~index), BF_F_* input fields
+  const unsigned long long* timers;   // [n_records][timer_k] timer slots, or nullptr: an armed step s counts s + 1, a non-PENDING
+  uint32_t timer_k;                   //   code BF_F_DECISION
 };
 
 // bf_resident_transfer (resident.cu): runs[i] of the source batch (layout F) is checked against the destination layout T
@@ -313,6 +322,51 @@ struct TransferParams {
   bf_layout R;                   // F with the result fields T lacks set to BF_OFF_NONE
   uint4* extent;                 // [n] out: steps, child nibbles, BF_F_* input fields of each run
   uint32_t* unfit;               // [1] the lowest i that T cannot hold (atomicMin; 0xFFFFFFFF from the caller)
+  const unsigned long long* src_timers;   // [src capacity][src_k] or nullptr
+  unsigned long long* dst_timers;         // [dst capacity][dst_k] or nullptr: an arrival's armed slots, the rest empty
+  uint32_t src_k, dst_k;                  // a run with more armed slots than dst_k is unfit
+};
+
+// step timers (resident.cu): slot = deadline | step << 32 | code << 48 (bf_timer_slot read as one little-endian u64); an empty
+// slot is kTimerEmpty.  A run's armed slots come first, ascending by step.
+constexpr unsigned long long kTimerEmpty = 0xFFFFFFFFull;
+__host__ __device__ inline uint32_t timer_deadline(unsigned long long v) { return (uint32_t)v; }
+__host__ __device__ inline uint32_t timer_step(unsigned long long v) { return (uint32_t)(v >> 32) & 0xFFFFu; }
+__host__ __device__ inline uint32_t timer_code(unsigned long long v) { return (uint32_t)(v >> 48) & 0xFFu; }
+__host__ __device__ inline bool timer_armed(unsigned long long v) { return (uint32_t)v != 0xFFFFFFFFu; }
+
+// bf_resident_timers / _reshape: run r < n of the new area gets the first min(src_k, dst_k) slots of run r of the old one (when
+// r < n_src), the rest empty
+struct TimerRelayParams {
+  const unsigned long long* src;   // or nullptr: every slot empty
+  unsigned long long* dst;
+  uint32_t n, n_src, src_k, dst_k;
+};
+
+// bf_resident_timers_arm: requests sorted by (run, step), grouped by run.  Group g is requests [first[g], first[g + 1]) of
+// run run[g]; arm_before[j] is the number of arming (not cancelling) requests of j's group before j.
+struct TimerArmParams {
+  unsigned long long* timers;
+  uint32_t timer_k;
+  const bf_timer* req;
+  const uint32_t* first;           // [n_groups + 1]
+  const uint32_t* arm_before;      // [n]
+  uint32_t n_groups;
+  uint32_t* overflow;              // [1] lowest group whose run would hold more than timer_k armed slots (atomicMin)
+};
+
+// bf_resident_fire: one thread per run, a warp per chunk of 32 runs
+struct FireParams {
+  uint8_t* state;
+  unsigned long long* timers;
+  uint32_t* mark;                  // a run whose code was written is raised to mark_value, as by a delta
+  uint32_t mark_value;
+  uint32_t n_runs, timer_k, now;
+  uint32_t words, state_stride, off_phase, off_decision;
+  uint32_t* block_sums;            // [blocks] fired timers per block (fire_count), read by fire_apply for its offsets
+  uint32_t* out;                   // [4] n_fired, n_written, n_pruned, next_deadline (fire_count initialises them)
+  bf_fired* fired;                 // [fired_cap]
+  uint32_t fired_cap;
 };
 
 // limiters.cu (rows a9 / f4)

@@ -122,6 +122,37 @@ __host__ __device__ inline uint32_t migrate_stage_words(const MigrateParams& P) 
   return migrate_planes(P) * P.words + migrate_child_words(P);
 }
 
+// The timer slots of a migrated run (whole warp): lane t holds slots t and t + 32, maps each armed step through the step map (a
+// gone step, or one past the map, cancels the slot), ranks the survivors by their new step (the map is injective: no ties) and,
+// after every lane has read, stores them in that order with empty slots behind.
+DI void migrate_timers(const MigrateParams& P, uint32_t run, uint32_t lane) {
+  unsigned long long* t = P.timers + (size_t)run * P.timer_k;
+  unsigned long long v[2];
+  uint32_t to[2];
+  for (uint32_t h = 0; h < 2; ++h) {
+    const uint32_t k = lane + 32u * h;
+    v[h] = k < P.timer_k ? t[k] : kTimerEmpty;
+    to[h] = BF_MIGRATE_GONE;
+    if (timer_armed(v[h])) {
+      const uint32_t s = timer_step(v[h]);
+      to[h] = s < P.n_old_steps ? P.fwd[s] : BF_MIGRATE_GONE;
+    }
+  }
+  uint32_t rank[2] = {0u, 0u}, kept = 0u;
+  for (uint32_t j = 0; j < 64u; ++j) {
+    const uint32_t tj = __shfl_sync(FULL, to[j >> 5], j & 31u);
+    if (tj == BF_MIGRATE_GONE) continue;
+    ++kept;
+    for (uint32_t h = 0; h < 2; ++h) rank[h] += tj < to[h] ? 1u : 0u;   // a gone slot's rank is never used
+  }
+  __syncwarp();
+  for (uint32_t h = 0; h < 2; ++h) {
+    const uint32_t k = lane + 32u * h;
+    if (to[h] != BF_MIGRATE_GONE) t[rank[h]] = (v[h] & ~(0xFFFFull << 32)) | (unsigned long long)to[h] << 32;
+    if (k >= kept && k < P.timer_k) t[k] = kTimerEmpty;
+  }
+}
+
 __global__ void __launch_bounds__(256) migrate_runs(const MigrateParams P) {
   extern __shared__ uint32_t smem[];
   uint32_t& block_count = smem[0];
@@ -177,6 +208,7 @@ __global__ void __launch_bounds__(256) migrate_runs(const MigrateParams P) {
         child[md.new_first / 8u + i] = v;
       }
     }
+    if (P.timers) migrate_timers(P, run, lane);
     if (lane == 0) {
       *reinterpret_cast<uint32_t*>(rec) = P.new_slot;
       *reinterpret_cast<uint64_t*>(rec + 8) = reg_new;
@@ -221,6 +253,8 @@ __global__ void __launch_bounds__(256) redrive_runs(const RedriveParams P) {
   const bool hit = *reinterpret_cast<const uint32_t*>(rec) == q.slot;   // no request of this launch writes the slot word
   if (lane == 0) P.status[i] = hit ? 1u : 0u;
   if (!hit) return;
+  if (P.timers)   // the whole step-timer annotation goes (storyrun_controller.go:477-478, :524-525)
+    for (uint32_t k = lane; k < P.timer_k; k += 32u) P.timers[(size_t)q.run * P.timer_k + k] = kTimerEmpty;
   const uint8_t* topo = reinterpret_cast<const uint8_t*>(P.slots[q.slot].addr);
   const TopoHeader* th = reinterpret_cast<const TopoHeader*>(topo);
   const uint32_t S = th->S, TW = th->W, W = P.words, key = P.key[i];
@@ -354,6 +388,13 @@ __global__ void __launch_bounds__(256) retire_runs(const RetireParams P) {
   }
   for (uint32_t k = lane; k < sv; k += 32u) s[k] = make_uint4(0u, 0u, 0u, 0u);
   if (lane == 0) P.mark[from] = 0u;
+  if (P.timers) {   // each lane stores over only the slots it read itself
+    unsigned long long* ts = P.timers + (size_t)from * P.timer_k;
+    for (uint32_t k = lane; k < P.timer_k; k += 32u) {
+      if (to != kRetireNoMove) P.timers[(size_t)to * P.timer_k + k] = ts[k];
+      ts[k] = kTimerEmpty;
+    }
+  }
 }
 
 cudaError_t launch_retire(const RetireParams& P, cudaStream_t stream) {
@@ -402,6 +443,20 @@ DI uint32_t result_word_extent(const bf_layout& R, uint32_t o, uint32_t v) {
   return 0u;
 }
 
+// The timer slots of one run (lane t reads slots t, t + 32): an armed step s needs s + 1 steps, a code that writes needs the
+// decision planes.  -> the armed slots this lane saw
+DI uint32_t timer_extent(const unsigned long long* t, uint32_t K, uint32_t lane, uint32_t& steps, uint32_t& fields) {
+  uint32_t armed = 0u;
+  for (uint32_t k = lane; k < K; k += 32u) {
+    const unsigned long long v = t[k];
+    if (!timer_armed(v)) continue;
+    ++armed;
+    steps = max(steps, timer_step(v) + 1u);
+    if (timer_code(v) != BF_DEC_PENDING) fields |= BF_F_DECISION;
+  }
+  return armed;
+}
+
 // One warp per record, grid-stride: lane t reads the 16-byte vectors t, t + 32, ... of the state record (and of the result record
 // of a run below n_runs that a later tick may compare with), so a warp streams each record once with coalesced loads; lane 0 adds the S and the child area of the
 // run's topology when its slot is alive.  Warp reductions, then each warp folds its record's extents into its running maxima (its
@@ -424,6 +479,7 @@ __global__ void __launch_bounds__(256) extent_runs(const ExtentParams P) {
       state_word_extent(P.L, o + 8u, q.z, steps, child, fields);
       state_word_extent(P.L, o + 12u, q.w, steps, child, fields);
     }
+    if (P.timers) timer_extent(P.timers + (size_t)r * P.timer_k, P.timer_k, lane, steps, fields);
     if (r < P.n_runs) {
       const uint32_t m = P.mark[r];
       const bool baseline = r < P.prev_runs || (r < P.eval_runs && !((m & 1u) && (m >> 1) > P.full_epoch));
@@ -485,6 +541,7 @@ __global__ void __launch_bounds__(256) transfer_fit(const TransferParams P) {
     state_word_extent(P.F, o + 8u, q.z, steps, child, fields);
     state_word_extent(P.F, o + 12u, q.w, steps, child, fields);
   }
+  uint32_t armed = P.src_timers ? timer_extent(P.src_timers + (size_t)r * P.src_k, P.src_k, lane, steps, fields) : 0u;
   const uint32_t m = P.src_mark[r];
   const bool baseline = r < P.prev_runs || (r < P.eval_runs && !((m & 1u) && (m >> 1) > P.full_epoch));
   const uint8_t* res = P.src_result + (size_t)r * P.F.result_stride;
@@ -504,12 +561,14 @@ __global__ void __launch_bounds__(256) transfer_fit(const TransferParams P) {
   steps = __reduce_max_sync(FULL, steps);
   child = __reduce_max_sync(FULL, child);
   fields = __reduce_or_sync(FULL, fields);
+  armed = __reduce_add_sync(FULL, armed);
   if (lane == 0) {
     const bf_layout& T = P.T;
     const uint32_t placed = (T.off_cond != BF_OFF_NONE ? BF_F_COND : 0u) | (T.off_decision != BF_OFF_NONE ? BF_F_DECISION : 0u) |
                             (T.off_child != BF_OFF_NONE ? BF_F_CHILD : 0u);
-    P.extent[i] = make_uint4(steps, child, fields, 0u);
-    if (steps > T.steps_max || (T.off_child != BF_OFF_NONE && child > T.child_nibbles) || (fields & ~placed)) atomicMin(P.unfit, i);
+    P.extent[i] = make_uint4(steps, child, fields, armed);
+    if (steps > T.steps_max || (T.off_child != BF_OFF_NONE && child > T.child_nibbles) || (fields & ~placed) || armed > P.dst_k)
+      atomicMin(P.unfit, i);
   }
 }
 
@@ -527,6 +586,9 @@ __global__ void __launch_bounds__(256) transfer_runs(const TransferParams P) {
   d = reinterpret_cast<uint32_t*>(P.dst_result + (size_t)to * P.T.result_stride);
   for (uint32_t o = lane * 4u; o < P.T.result_stride; o += 128u) d[o >> 2] = reshape_result_word(s, o, P.F, P.T);
   if (lane == 0) P.dst_mark[to] = P.mark_value;
+  // the run's armed slots (at most dst_k, transfer_fit) lead the source's slots: copied in order, empty slots behind them
+  for (uint32_t k = lane; P.dst_timers && k < P.dst_k; k += 32u)
+    P.dst_timers[(size_t)to * P.dst_k + k] = P.src_timers && k < P.src_k ? P.src_timers[(size_t)r * P.src_k + k] : kTimerEmpty;
 }
 
 cudaError_t launch_transfer_fit(const TransferParams& P, cudaStream_t stream) {
@@ -538,6 +600,200 @@ cudaError_t launch_transfer_fit(const TransferParams& P, cudaStream_t stream) {
 cudaError_t launch_transfer(const TransferParams& P, cudaStream_t stream) {
   if (P.n == 0) return cudaSuccess;
   transfer_runs<<<(P.n - 1u) / 8u + 1u, 256, 0, stream>>>(P);
+  return cudaGetLastError();
+}
+
+// ---- step timers (bf_resident_timers*, bf_resident_fire) ----------------------------------------------------------------------
+// Relay (bf_resident_timers, reshape): one thread per slot of the new area.
+__global__ void __launch_bounds__(256) relay_timers(const TimerRelayParams P) {
+  const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= (size_t)P.n * P.dst_k) return;
+  const uint32_t r = (uint32_t)(i / P.dst_k), k = (uint32_t)(i % P.dst_k);
+  P.dst[i] = P.src && r < P.n_src && k < P.src_k ? P.src[(size_t)r * P.src_k + k] : kTimerEmpty;
+}
+
+cudaError_t launch_relay_timers(const TimerRelayParams& P, cudaStream_t stream) {
+  const size_t n = (size_t)P.n * P.dst_k;
+  if (n == 0) return cudaSuccess;
+  relay_timers<<<(unsigned)((n + 255) / 256), 256, 0, stream>>>(P);
+  return cudaGetLastError();
+}
+
+// the first index of req[lo, hi) whose step is >= s (requests of one group ascend by step)
+DI uint32_t req_lower_bound(const bf_timer* req, uint32_t lo, uint32_t hi, uint32_t s) {
+  while (lo < hi) {
+    const uint32_t mid = (lo + hi) >> 1;
+    if (req[mid].step < s) lo = mid + 1; else hi = mid;
+  }
+  return lo;
+}
+
+// Arm, both launches: one warp per request group (one run).  The warp stages the run's slots in shared memory and marks the armed
+// slots a request names (replaced or cancelled).  The check launch counts the run's armed slots after the merge and lowers
+// P.overflow to its group when they pass timer_k; the merge launch, which runs only when no group overflows, stores every kept
+// slot and every arming request at its rank by step: a kept slot at its index among the kept slots plus the arming requests of
+// lower steps, a request at its index among the arming requests plus the kept slots of lower steps.  Empty slots follow.
+template <bool kMerge>
+__global__ void __launch_bounds__(256) arm_timers(const TimerArmParams P) {
+  __shared__ unsigned long long stage[8][BF_TIMER_MAX_SLOTS];
+  const uint32_t warp = threadIdx.x >> 5, lane = threadIdx.x & 31u, g = blockIdx.x * 8u + warp;
+  if (g >= P.n_groups) return;
+  const uint32_t lo = P.first[g], hi = P.first[g + 1], K = P.timer_k, run = P.req[lo].run;
+  unsigned long long* t = P.timers + (size_t)run * K;
+  unsigned long long* st = stage[warp];
+  uint32_t matched[2], armed[2];
+  for (uint32_t h = 0; h < 2; ++h) {
+    const uint32_t k = lane + 32u * h;
+    const unsigned long long v = k < K ? t[k] : kTimerEmpty;
+    st[k] = v;
+    const bool a = timer_armed(v);
+    const uint32_t j = a ? req_lower_bound(P.req, lo, hi, timer_step(v)) : hi;
+    armed[h] = __ballot_sync(FULL, a);
+    matched[h] = __ballot_sync(FULL, a && j < hi && P.req[j].step == timer_step(v));
+  }
+  const uint32_t arms = P.arm_before[hi] - P.arm_before[lo];
+  const uint32_t E = __popc(armed[0]) + __popc(armed[1]), M = __popc(matched[0]) + __popc(matched[1]), total = E - M + arms;
+  if (!kMerge) {
+    if (lane == 0 && total > K) atomicMin(P.overflow, g);
+    return;
+  }
+  __syncwarp();
+  auto matched_below = [&](uint32_t k) {   // matched slots among [0, k)
+    return k <= 32u ? __popc(matched[0] & (k == 32u ? FULL : (1u << k) - 1u))
+                    : __popc(matched[0]) + __popc(matched[1] & (k == 64u ? FULL : (1u << (k - 32u)) - 1u));
+  };
+  for (uint32_t h = 0; h < 2; ++h) {   // kept slots
+    const uint32_t k = lane + 32u * h;
+    if (k >= E || ((matched[h] >> lane) & 1u)) continue;
+    const unsigned long long v = st[k];
+    const uint32_t j = req_lower_bound(P.req, lo, hi, timer_step(v));
+    t[k - matched_below(k) + P.arm_before[j] - P.arm_before[lo]] = v;
+  }
+  for (uint32_t j = lo + lane; j < hi; j += 32u) {   // arming requests
+    const bf_timer q = P.req[j];
+    if (q.deadline == BF_TIMER_NONE) continue;
+    uint32_t a = 0, b = E;   // kept or matched slots of lower steps: the first staged slot at or above q.step
+    while (a < b) {
+      const uint32_t mid = (a + b) >> 1;
+      if (timer_step(st[mid]) < q.step) a = mid + 1; else b = mid;
+    }
+    t[P.arm_before[j] - P.arm_before[lo] + a - matched_below(a)] =
+        (unsigned long long)q.deadline | (unsigned long long)q.step << 32 | (unsigned long long)q.code << 48;
+  }
+  for (uint32_t k = total + lane; k < K; k += 32u) t[k] = kTimerEmpty;
+}
+
+cudaError_t launch_arm_timers(const TimerArmParams& P, bool merge, cudaStream_t stream) {
+  if (P.n_groups == 0) return cudaSuccess;
+  const uint32_t grid = (P.n_groups - 1u) / 8u + 1u;
+  if (merge) arm_timers<true><<<grid, 256, 0, stream>>>(P);
+  else arm_timers<false><<<grid, 256, 0, stream>>>(P);
+  return cudaGetLastError();
+}
+
+// the code of step s in the nbits planes at `off`
+DI uint32_t get_planes(const uint8_t* rec, uint32_t off, uint32_t words, uint32_t nbits, uint32_t s) {
+  const uint32_t* w = reinterpret_cast<const uint32_t*>(rec + off) + (s >> 5);
+  uint32_t code = 0;
+  for (uint32_t b = 0; b < nbits; ++b) code |= ((w[b * words] >> (s & 31u)) & 1u) << b;
+  return code;
+}
+
+// One run's armed slots against `now`: fired (due, step not terminal) -> 1, pruned (step terminal) -> 2, kept -> 0
+DI uint32_t fire_kind(const FireParams& P, const uint8_t* rec, unsigned long long v) {
+  if ((BF_LUT_TERMINAL >> get_planes(rec, P.off_phase, P.words, 4, timer_step(v))) & 1u) return 2u;
+  return timer_deadline(v) <= P.now ? 1u : 0u;
+}
+DI uint32_t fired_of_run(const FireParams& P, uint32_t r) {
+  if (r >= P.n_runs) return 0u;
+  const uint8_t* rec = P.state + (size_t)r * P.state_stride;
+  const unsigned long long* t = P.timers + (size_t)r * P.timer_k;
+  uint32_t n = 0;
+  for (uint32_t k = 0; k < P.timer_k; ++k) {
+    const unsigned long long v = t[k];
+    if (!timer_armed(v)) break;   // armed slots lead
+    n += fire_kind(P, rec, v) == 1u ? 1u : 0u;
+  }
+  return n;
+}
+
+// Fire, first launch: one thread per run (a warp per chunk of 32 runs) counts its fired timers; each CTA stores its total.  CTA 0
+// initialises the four output words, which the second launch accumulates into.
+__global__ void __launch_bounds__(256) fire_count(const FireParams P) {
+  __shared__ uint32_t warp_sum[8];
+  const uint32_t r = blockIdx.x * 256u + threadIdx.x, lane = threadIdx.x & 31u;
+  const uint32_t n = __reduce_add_sync(FULL, fired_of_run(P, r));
+  if (lane == 0) warp_sum[threadIdx.x >> 5] = n;
+  if (blockIdx.x == 0 && threadIdx.x < 4) P.out[threadIdx.x] = threadIdx.x == 3 ? BF_TIMER_NONE : 0u;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    uint32_t sum = 0;
+    for (uint32_t w = 0; w < 8; ++w) sum += warp_sum[w];
+    P.block_sums[blockIdx.x] = sum;
+  }
+}
+
+// Fire, second launch: each CTA sums the totals of the CTAs before it, scans its runs' counts (the same counts: nothing changed
+// in between) and each thread walks its run's slots once: a pruned slot goes, a fired one is listed at its place in run order
+// (written when its code writes and the decision code is still PENDING: the planes of the delta scatter, and the touch mark), a
+// kept one moves down over the gaps; empty slots close the run.  Warp sums and a warp minimum go to the four output words.
+__global__ void __launch_bounds__(256) fire_apply(const FireParams P) {
+  __shared__ uint32_t base_part[8], warp_incl[8];
+  const uint32_t r = blockIdx.x * 256u + threadIdx.x, lane = threadIdx.x & 31u, warp = threadIdx.x >> 5;
+  uint32_t before = 0;   // fired timers of the CTAs before this one: each warp sums a strided share
+  for (uint32_t b = threadIdx.x; b < blockIdx.x; b += 256u) before += P.block_sums[b];
+  before = __reduce_add_sync(FULL, before);
+  const uint32_t mine = fired_of_run(P, r);
+  uint32_t incl = mine;   // inclusive warp scan
+  for (uint32_t d = 1; d < 32; d <<= 1) {
+    const uint32_t x = __shfl_up_sync(FULL, incl, d);
+    if (lane >= d) incl += x;
+  }
+  if (lane == 31) warp_incl[warp] = incl;
+  if (lane == 0) base_part[warp] = before;
+  __syncthreads();
+  uint32_t pos = incl - mine;
+  for (uint32_t w = 0; w < 8; ++w) pos += base_part[w] + (w < warp ? warp_incl[w] : 0u);
+  uint32_t written = 0, pruned = 0, next = BF_TIMER_NONE, touched = 0;
+  if (r < P.n_runs) {
+    uint8_t* rec = P.state + (size_t)r * P.state_stride;
+    unsigned long long* t = P.timers + (size_t)r * P.timer_k;
+    uint32_t keep = 0, k = 0;
+    for (; k < P.timer_k; ++k) {
+      const unsigned long long v = t[k];
+      if (!timer_armed(v)) break;
+      const uint32_t kind = fire_kind(P, rec, v);
+      if (kind == 2u) { ++pruned; continue; }
+      if (kind == 0u) { t[keep++] = v; next = min(next, timer_deadline(v)); continue; }
+      const uint32_t s = timer_step(v), code = timer_code(v);
+      bool w = false;
+      if (code != BF_DEC_PENDING && P.off_decision != BF_OFF_NONE && get_planes(rec, P.off_decision, P.words, 2, s) == BF_DEC_PENDING) {
+        set_planes(rec, P.off_decision, P.words, 2, s, code);
+        w = true;
+      }
+      written += w ? 1u : 0u;
+      touched |= w ? 1u : 0u;
+      if (pos < P.fired_cap) P.fired[pos] = bf_fired{r, (uint16_t)s, (uint8_t)code, (uint8_t)(w ? 1u : 0u)};
+      ++pos;
+    }
+    for (uint32_t e = keep; e < k; ++e) t[e] = kTimerEmpty;
+    if (touched) atomicMax(P.mark + r, P.mark_value);   // max: an upload's "must list" bit stays
+  }
+  const uint32_t f = __reduce_add_sync(FULL, mine), wr = __reduce_add_sync(FULL, written), pr = __reduce_add_sync(FULL, pruned);
+  next = __reduce_min_sync(FULL, next);
+  if (lane == 0) {
+    if (f) atomicAdd(P.out, f);
+    if (wr) atomicAdd(P.out + 1, wr);
+    if (pr) atomicAdd(P.out + 2, pr);
+    if (next != BF_TIMER_NONE) atomicMin(P.out + 3, next);
+  }
+}
+
+cudaError_t launch_fire(const FireParams& P, cudaStream_t stream) {
+  if (P.n_runs == 0) return cudaSuccess;
+  const uint32_t grid = (P.n_runs - 1u) / 256u + 1u;
+  fire_count<<<grid, 256, 0, stream>>>(P);
+  fire_apply<<<grid, 256, 0, stream>>>(P);
   return cudaGetLastError();
 }
 

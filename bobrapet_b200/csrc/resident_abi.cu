@@ -356,11 +356,13 @@ int bf_resident_migrate(bf_ctx* c, uint32_t h, bf_migration* m) {
   m->migrated = 0;
   BF_CUDA(c, cudaSetDevice(c->device));
   cudaStream_t s = c->stream;
-  const size_t o_inv = 16, o_desc = round_up_sz(o_inv + inv.size() * 2, 16), bytes = o_desc + descs.size() * sizeof(bf::MigrateDesc);
+  const size_t o_inv = 16, o_desc = round_up_sz(o_inv + inv.size() * 2, 16), o_fwd = o_desc + descs.size() * sizeof(bf::MigrateDesc),
+               bytes = o_fwd + (r->timer_k ? (size_t)mo.S * 2 : 0);
   if (int rc = c->d_mig.ensure(c, bytes)) return rc;
   std::vector<uint8_t> blob(bytes, 0);   // the counter starts at zero
   memcpy(blob.data() + o_inv, inv.data(), inv.size() * 2);
   if (!descs.empty()) memcpy(blob.data() + o_desc, descs.data(), descs.size() * sizeof(bf::MigrateDesc));
+  if (r->timer_k) memcpy(blob.data() + o_fwd, m->step_map, (size_t)mo.S * 2);   // the timers are re-keyed forwards
   r->end_snapshot(c);   // as after an upload
   bf::MigrateParams P{};
   P.state = r->d_state; P.mark = r->d_mark; P.mark_value = r->mark_must_list();
@@ -370,6 +372,8 @@ int bf_resident_migrate(bf_ctx* c, uint32_t h, bf_migration* m) {
   P.n_runs = m->n_runs; P.old_slot = m->old_slot; P.new_slot = m->new_slot;
   P.words = L.words; P.state_stride = L.state_stride; P.off_phase = L.off_phase; P.off_cond = L.off_cond;
   P.off_decision = L.off_decision; P.off_child = L.off_child; P.child_nibbles = L.child_nibbles;
+  P.timers = r->d_timers; P.timer_k = r->timer_k; P.n_old_steps = mo.S;
+  P.fwd = reinterpret_cast<const uint16_t*>(c->d_mig + o_fwd);
   cudaError_t e = cudaMemcpyAsync(c->d_mig, blob.data(), bytes, cudaMemcpyHostToDevice, s);
   if (e == cudaSuccess) e = bf::launch_migrate(P, s);
   if (e == cudaSuccess) e = cudaMemcpyAsync(&c->pinned->word, c->d_mig, 4, cudaMemcpyDeviceToHost, s);
@@ -430,6 +434,7 @@ int bf_resident_redrive(bf_ctx* c, uint32_t h, const bf_redrive* req, uint32_t n
   P.masks = d_mask; P.status = d; P.slots = c->slots_dev; P.n = n;
   P.words = L.words; P.state_stride = L.state_stride; P.off_phase = L.off_phase; P.off_cond = L.off_cond;
   P.off_decision = L.off_decision; P.off_child = L.off_child;
+  P.timers = r->d_timers; P.timer_k = r->timer_k;
   std::vector<uint8_t> status(n);
   cudaStream_t s = c->stream;
   cudaError_t e = cudaMemcpyAsync(d + o_req, blob.data(), blob.size(), cudaMemcpyHostToDevice, s);
@@ -473,6 +478,10 @@ int bf_resident_reshape(bf_ctx* c, uint32_t h, const bf_layout* layout, uint32_t
   BF_CUDA(c, cudaSetDevice(c->device));
   Resident nb;
   if (cudaError_t e = nb.alloc(T, capacity)) return fail(c, BF_ENOMEM, std::string("resident reshape: ") + cudaGetErrorString(e));
+  const bool timers_grow = r->timer_k && capacity > r->cap;   // the area follows the capacity: empty slots for the new runs
+  if (timers_grow)
+    if (cudaError_t e = nb.d_timers.alloc((size_t)capacity * r->timer_k))
+      return fail(c, BF_ENOMEM, std::string("resident reshape (timers): ") + cudaGetErrorString(e));
   const size_t old_mark = r->d_mark.cap * sizeof(uint32_t), new_mark = nb.d_mark.cap * sizeof(uint32_t);
   bf::ReshapeParams P{};
   P.old_state = r->d_state; P.old_result = r->d_result; P.state = nb.d_state; P.result = nb.d_result;
@@ -481,10 +490,15 @@ int bf_resident_reshape(bf_ctx* c, uint32_t h, const bf_layout* layout, uint32_t
   cudaError_t e = bf::launch_reshape(P, s);
   if (e == cudaSuccess) e = cudaMemcpyAsync(nb.d_mark, r->d_mark, old_mark, cudaMemcpyDeviceToDevice, s);   // with the list-build padding
   if (e == cudaSuccess && new_mark > old_mark) e = cudaMemsetAsync(reinterpret_cast<uint8_t*>(nb.d_mark.p) + old_mark, 0, new_mark - old_mark, s);
+  if (e == cudaSuccess && timers_grow) {
+    e = bf::launch_relay_timers({r->d_timers, nb.d_timers, capacity, r->cap, r->timer_k, r->timer_k}, s);
+    c->stats.kernel_launches += 1;
+  }
   const cudaError_t es = cudaStreamSynchronize(s);
   if (e == cudaSuccess) e = es;
   if (e != cudaSuccess) return cuda_fail(c, e, "bf_resident_reshape");   // the old buffers were only read: the batch is as it was
   r->end_snapshot(c);   // as after an upload
+  if (timers_grow) r->d_timers = std::move(nb.d_timers);
   r->adopt(std::move(nb), T, capacity);
   if (results_may_change) r->need_full = true;
   return BF_OK;
@@ -499,6 +513,7 @@ static int extent_async(bf_ctx* c, Resident* r, uint32_t n_runs, const bf_layout
   bf::ExtentParams P{};
   P.state = r->d_state; P.result = r->d_result; P.mark = r->d_mark; P.slots = c->slots_dev; P.n_slots = (uint32_t)c->slots_host.size();
   P.n_records = r->cap; P.n_runs = n_runs; P.L = r->L; P.R = R; P.out = c->d_extent;
+  P.timers = r->d_timers; P.timer_k = r->timer_k;
   // only result records a later tick compares with count: the changed-only baseline and the touched one (ctx.h)
   P.prev_runs = r->prev_valid ? r->prev_runs : 0u; P.eval_runs = r->touched_baseline_runs(); P.full_epoch = r->full_epoch;
   BF_CUDA(c, cudaMemsetAsync(c->d_extent, 0, 3 * sizeof(unsigned long long), s));
@@ -659,10 +674,14 @@ int bf_resident_retire(bf_ctx* c, uint32_t h, bf_retire* rt) {
   Resident nb;
   if (resize)
     if (cudaError_t e = nb.alloc(L, cap)) return fail(c, BF_ENOMEM, std::string("resident retire: ") + cudaGetErrorString(e));
+  if (resize && r->timer_k)
+    if (cudaError_t e = nb.d_timers.alloc((size_t)cap * r->timer_k))
+      return fail(c, BF_ENOMEM, std::string("resident retire (timers): ") + cudaGetErrorString(e));
   r->end_snapshot(c);   // as after an upload
   bf::RetireParams P{};
   P.state = r->d_state; P.result = r->d_result; P.mark = r->d_mark; P.mark_value = r->mark_must_list();
   P.to = c->d_retire; P.m = m; P.n = n; P.state_stride = L.state_stride; P.result_stride = L.result_stride;
+  P.timers = r->d_timers; P.timer_k = r->timer_k;
   cudaStream_t s = c->stream;
   cudaError_t e = n ? cudaMemcpyAsync(c->d_retire, to.data(), (size_t)n * 4, cudaMemcpyHostToDevice, s) : cudaSuccess;
   if (e == cudaSuccess) e = bf::launch_retire(P, s);
@@ -670,9 +689,12 @@ int bf_resident_retire(bf_ctx* c, uint32_t h, bf_retire* rt) {
     if (e == cudaSuccess) e = cudaMemcpyAsync(nb.d_state, r->d_state, (size_t)cap * L.state_stride, cudaMemcpyDeviceToDevice, s);
     if (e == cudaSuccess) e = cudaMemcpyAsync(nb.d_result, r->d_result, (size_t)cap * L.result_stride, cudaMemcpyDeviceToDevice, s);
     if (e == cudaSuccess) e = cudaMemcpyAsync(nb.d_mark, r->d_mark, nb.d_mark.cap * sizeof(uint32_t), cudaMemcpyDeviceToDevice, s);
+    if (e == cudaSuccess && r->timer_k)
+      e = cudaMemcpyAsync(nb.d_timers, r->d_timers, (size_t)cap * r->timer_k * 8, cudaMemcpyDeviceToDevice, s);
   }
   if (int rc = r->sync_in_place(c, e, "bf_resident_retire")) return rc;
   c->stats.kernel_launches += n ? 1 : 0;
+  if (resize && r->timer_k) r->d_timers = std::move(nb.d_timers);
   if (resize) r->adopt(std::move(nb), L, cap);
   r->compact_to(m, N, to);
   write_moves(to, m, rt->moves_from, rt->moves_to);
@@ -731,6 +753,7 @@ int bf_resident_transfer(bf_ctx* c, uint32_t hs, uint32_t hd, bf_transfer* t) {
   if (T.off_skip_dep == BF_OFF_NONE) P.R.off_skip_dep = BF_OFF_NONE;
   if (T.off_phase_out == BF_OFF_NONE) P.R.off_phase_out = BF_OFF_NONE;
   P.extent = reinterpret_cast<uint4*>(c->d_transfer + o_ext); P.unfit = reinterpret_cast<uint32_t*>(c->d_transfer.p);
+  P.src_timers = src->d_timers; P.src_k = src->timer_k; P.dst_timers = dst->d_timers; P.dst_k = dst->timer_k;
   cudaStream_t s = c->stream;
   BF_CUDA(c, cudaMemcpyAsync(c->d_transfer, blob.data(), blob.size(), cudaMemcpyHostToDevice, s));
   BF_CUDA(c, bf::launch_transfer_fit(P, s));
@@ -747,7 +770,8 @@ int bf_resident_transfer(bf_ctx* c, uint32_t hs, uint32_t hd, bf_transfer* t) {
     t->why.widest_run = x[0] ? t->runs[unfit] : BF_EXTENT_NO_RUN;
     return fail(c, BF_EINVAL, "runs[" + std::to_string(unfit) + "] (run " + std::to_string(t->runs[unfit]) +
                                   ") does not fit the destination layout: it needs steps_max " + std::to_string(x[0]) +
-                                  ", child_nibbles " + std::to_string(x[1]) + ", fields " + std::to_string(x[2]));
+                                  ", child_nibbles " + std::to_string(x[1]) + ", fields " + std::to_string(x[2]) + ", " +
+                                  std::to_string(x[3]) + " timer slot(s) of the destination's " + std::to_string(dst->timer_k));
   }
   // every arrival's record is a changed-only baseline of the source: the destination's may reach over them
   bool src_baseline = src->prev_valid;
@@ -758,6 +782,7 @@ int bf_resident_transfer(bf_ctx* c, uint32_t hs, uint32_t hd, bf_transfer* t) {
   Q.state = src->d_state; Q.result = src->d_result; Q.mark = src->d_mark; Q.mark_value = src->mark_must_list();
   Q.to = reinterpret_cast<const uint32_t*>(c->d_transfer + o_to); Q.m = m; Q.n = n;
   Q.state_stride = F.state_stride; Q.result_stride = F.result_stride;
+  Q.timers = src->d_timers; Q.timer_k = src->timer_k;
   cudaError_t e = bf::launch_transfer(P, s);
   if (e == cudaSuccess) e = bf::launch_retire(Q, s);   // behind the transfer on the stream: the sources are read first
   if (int rc = src->sync_in_place(c, e, "bf_resident_transfer")) { dst->records_unknown(); return rc; }
@@ -766,5 +791,149 @@ int bf_resident_transfer(bf_ctx* c, uint32_t hs, uint32_t hd, bf_transfer* t) {
   dst->received(D, n, src_baseline);
   write_moves(to, m, t->moves_from, t->moves_to);
   t->src_n_runs = m; t->dst_n_runs = D + n; t->n_moves = n_moves;
+  return BF_OK;
+}
+
+// ---- step timers (resident.cu) ------------------------------------------------------------------------------------------------
+// The area of K slots per run: created with every slot empty, or grown to a larger K with each run's slots kept in place (one
+// relay launch into new slots, one synchronisation; the old area is freed once the new one is filled).
+int bf_resident_timers(bf_ctx* c, uint32_t h, uint32_t K) {
+  auto [g, r] = lock_resident(c, h);
+  if (!r) return BF_EINVAL;
+  if (K < 1 || K > BF_TIMER_MAX_SLOTS) return fail(c, BF_EINVAL, "slots_per_run must be within [1, 64]");
+  if (K < r->timer_k) return fail(c, BF_EINVAL, "slots_per_run cannot shrink (" + std::to_string(r->timer_k) + " now)");
+  if (K == r->timer_k) return BF_OK;
+  BF_CUDA(c, cudaSetDevice(c->device));
+  DevBuf<unsigned long long> area;
+  if (cudaError_t e = area.alloc((size_t)r->cap * K)) return fail(c, BF_ENOMEM, std::string("timer area: ") + cudaGetErrorString(e));
+  cudaError_t e = bf::launch_relay_timers({r->d_timers, area, r->cap, r->cap, r->timer_k, K}, c->stream);
+  const cudaError_t es = cudaStreamSynchronize(c->stream);
+  if (e == cudaSuccess) e = es;
+  if (e != cudaSuccess) return cuda_fail(c, e, "bf_resident_timers");   // the old area was only read
+  c->stats.kernel_launches += 1;
+  r->d_timers = std::move(area);
+  r->timer_k = K;
+  return BF_OK;
+}
+
+// Arms and cancels: every argument is checked on the host (the requests sorted by (run, step), which also finds duplicates), then
+// one H2D copy, the check launch, one D2H copy of the overflow word and one synchronisation before anything is written; then the
+// merge launch and one synchronisation.
+int bf_resident_timers_arm(bf_ctx* c, uint32_t h, const bf_timer* req, uint32_t n) {
+  auto [g, r] = lock_resident(c, h);
+  if (!r) return BF_EINVAL;
+  if (!r->timer_k) return fail(c, BF_EINVAL, "the batch has no timer area (bf_resident_timers)");
+  if (n && !req) return fail(c, BF_EINVAL, "null requests");
+  const bf_layout& L = r->L;
+  for (uint32_t i = 0; i < n; ++i) {
+    const bf_timer& q = req[i];
+    auto at = [i] { return "request " + std::to_string(i) + ": "; };
+    if (q.run >= r->cap) return fail(c, BF_EINVAL, at() + "run outside the resident batch");
+    if (q.step >= L.steps_max) return fail(c, BF_EINVAL, at() + "step outside the batch layout (steps_max)");
+    if (q.code > BF_DEC_TIMED_OUT) return fail(c, BF_EINVAL, at() + "code is not a BF_DEC_* code");
+    if (q.reserved || q.reserved2) return fail(c, BF_EINVAL, at() + "reserved fields must be 0");
+    if (q.code != BF_DEC_PENDING && L.off_decision == BF_OFF_NONE)
+      return fail(c, BF_EINVAL, at() + "a code that writes needs decision planes (BF_F_DECISION)");
+  }
+  if (n == 0) return BF_OK;
+  std::vector<uint32_t> order(n);
+  for (uint32_t i = 0; i < n; ++i) order[i] = i;
+  auto key = [&](uint32_t i) { return (uint64_t)req[i].run << 16 | req[i].step; };
+  std::stable_sort(order.begin(), order.end(), [&](uint32_t a, uint32_t b) { return key(a) < key(b); });
+  std::vector<bf_timer> sorted(n);
+  std::vector<uint32_t> first, arm_before(n + 1, 0);
+  for (uint32_t j = 0; j < n; ++j) {
+    sorted[j] = req[order[j]];
+    if (j && key(order[j]) == key(order[j - 1]))
+      return fail(c, BF_EINVAL, "requests " + std::to_string(order[j - 1]) + " and " + std::to_string(order[j]) + " name the same (run, step)");
+    if (j == 0 || sorted[j].run != sorted[j - 1].run) first.push_back(j);
+    arm_before[j + 1] = arm_before[j] + (sorted[j].deadline != BF_TIMER_NONE ? 1u : 0u);
+  }
+  const uint32_t G = (uint32_t)first.size();
+  first.push_back(n);
+  BF_CUDA(c, cudaSetDevice(c->device));
+  const size_t o_first = 16, o_arm = o_first + (size_t)(G + 1) * 4, o_req = round_up_sz(o_arm + (size_t)(n + 1) * 4, 16),
+               bytes = o_req + (size_t)n * sizeof(bf_timer);
+  if (int rc = c->d_timer.ensure(c, bytes)) return rc;
+  std::vector<uint8_t> blob(bytes, 0);
+  const uint32_t none = 0xFFFFFFFFu;
+  memcpy(blob.data(), &none, 4);
+  memcpy(blob.data() + o_first, first.data(), (size_t)(G + 1) * 4);
+  memcpy(blob.data() + o_arm, arm_before.data(), (size_t)(n + 1) * 4);
+  memcpy(blob.data() + o_req, sorted.data(), (size_t)n * sizeof(bf_timer));
+  bf::TimerArmParams P{};
+  P.timers = r->d_timers; P.timer_k = r->timer_k; P.n_groups = G;
+  P.req = reinterpret_cast<const bf_timer*>(c->d_timer + o_req);
+  P.first = reinterpret_cast<const uint32_t*>(c->d_timer + o_first);
+  P.arm_before = reinterpret_cast<const uint32_t*>(c->d_timer + o_arm);
+  P.overflow = reinterpret_cast<uint32_t*>(c->d_timer.p);
+  cudaStream_t s = c->stream;
+  BF_CUDA(c, cudaMemcpyAsync(c->d_timer, blob.data(), bytes, cudaMemcpyHostToDevice, s));
+  BF_CUDA(c, bf::launch_arm_timers(P, false, s));
+  BF_CUDA(c, cudaMemcpyAsync(&c->pinned->word, c->d_timer, 4, cudaMemcpyDeviceToHost, s));
+  BF_CUDA(c, cudaStreamSynchronize(s));
+  c->stats.kernel_launches += 1;
+  if (c->pinned->word != none)
+    return fail(c, BF_ENOMEM, "run " + std::to_string(sorted[first[c->pinned->word]].run) + " would hold more than " +
+                                  std::to_string(r->timer_k) + " armed timers");
+  cudaError_t e = bf::launch_arm_timers(P, true, s);
+  const cudaError_t es = cudaStreamSynchronize(s);
+  if (e == cudaSuccess) e = es;
+  if (e != cudaSuccess) return cuda_fail(c, e, "bf_resident_timers_arm");
+  c->stats.kernel_launches += 1;
+  return BF_OK;
+}
+
+// Due timers against `now` (resident.cu): the count and apply launches, the D2H copy of the four output words, one
+// synchronisation.  A pinned list is posted to by the kernel itself; any other gets the entries that fired copied after it.
+int bf_resident_fire(bf_ctx* c, uint32_t h, uint32_t now, bf_fire_out* out) {
+  auto [g, r] = lock_resident(c, h);
+  if (!out || out->struct_size != sizeof(bf_fire_out)) return fail(c, BF_EINVAL, "null bf_fire_out or bad struct_size");
+  if (!r) return BF_EINVAL;
+  if (!r->timer_k) return fail(c, BF_EINVAL, "the batch has no timer area (bf_resident_timers)");
+  const uint32_t N = out->n_runs;
+  if (N > r->cap) return fail(c, BF_EINVAL, "n_runs exceeds the resident batch");
+  if (out->fired_cap && !out->fired) return fail(c, BF_EINVAL, "null fired with a non-zero fired_cap");
+  out->n_fired = out->n_written = out->n_pruned = 0;
+  out->next_deadline = BF_TIMER_NONE;
+  if (N == 0) return BF_OK;
+  BF_CUDA(c, cudaSetDevice(c->device));
+  const uint32_t grid = (N - 1) / 256 + 1;
+  // the list is at most N * K long: a larger fired_cap stages no more than that
+  const uint32_t cap = (uint32_t)std::min<uint64_t>(out->fired_cap, (uint64_t)N * r->timer_k);
+  bf_fired* posted = static_cast<bf_fired*>(bf::pinned_dev(out->fired));
+  const size_t o_sums = 16, o_list = round_up_sz(o_sums + (size_t)grid * 4, 16), bytes = o_list + (posted ? 0 : (size_t)cap * 8);
+  if (int rc = c->d_timer.ensure(c, bytes)) return rc;
+  r->end_snapshot(c);   // as a delta
+  bf::FireParams P{};
+  P.state = r->d_state; P.timers = r->d_timers; P.mark = r->d_mark; P.mark_value = r->mark_touched();
+  P.n_runs = N; P.timer_k = r->timer_k; P.now = now;
+  P.words = r->L.words; P.state_stride = r->L.state_stride; P.off_phase = r->L.off_phase; P.off_decision = r->L.off_decision;
+  P.out = reinterpret_cast<uint32_t*>(c->d_timer.p);
+  P.block_sums = reinterpret_cast<uint32_t*>(c->d_timer + o_sums);
+  P.fired = posted ? posted : reinterpret_cast<bf_fired*>(c->d_timer + o_list);
+  P.fired_cap = cap;
+  cudaStream_t s = c->stream;
+  uint32_t* words = c->pinned->fire;
+  cudaError_t e = bf::launch_fire(P, s);
+  if (e == cudaSuccess) e = cudaMemcpyAsync(words, P.out, 16, cudaMemcpyDeviceToHost, s);
+  if (int rc = r->sync_in_place(c, e, "bf_resident_fire")) return rc;
+  c->stats.kernel_launches += 2;
+  if (const uint32_t listed = std::min(words[0], cap); listed && !posted)
+    BF_CUDA(c, cudaMemcpy(out->fired, P.fired, (size_t)listed * 8, cudaMemcpyDeviceToHost));
+  out->n_fired = words[0]; out->n_written = words[1]; out->n_pruned = words[2]; out->next_deadline = words[3];
+  r->pending += out->n_written;   // the touched-list bound counts the written codes as it counts deltas
+  return BF_OK;
+}
+
+int bf_resident_timers_download(bf_ctx* c, uint32_t h, uint32_t first, uint32_t n, void* slots) {
+  auto [g, r] = lock_resident(c, h);
+  if (!r) return BF_EINVAL;
+  if (!r->timer_k) return fail(c, BF_EINVAL, "the batch has no timer area (bf_resident_timers)");
+  if ((uint64_t)first + n > r->cap || (n && !slots)) return fail(c, BF_EINVAL, "run range outside the resident batch");
+  if (n == 0) return BF_OK;
+  BF_CUDA(c, cudaSetDevice(c->device));
+  BF_CUDA(c, cudaMemcpyAsync(slots, r->d_timers + (size_t)first * r->timer_k, (size_t)n * r->timer_k * 8, cudaMemcpyDeviceToHost, c->stream));
+  BF_CUDA(c, cudaStreamSynchronize(c->stream));
   return BF_OK;
 }

@@ -296,6 +296,43 @@ class Frontier:
         return {"src_n_runs": int(t.src_n_runs), "dst_n_runs": int(t.dst_n_runs), "moves_from": mf[:t.n_moves].copy(),
                 "moves_to": mt[:t.n_moves].copy()}
 
+    # -- step timers of a resident batch (bf_resident_timers*, bf_resident_fire)
+    TIMER_DTYPE = np.dtype([("run", "<u4"), ("step", "<u2"), ("code", "u1"), ("reserved", "u1"), ("deadline", "<u4"),
+                            ("reserved2", "<u4")])                                             # bf_timer, 16 B
+    SLOT_DTYPE = np.dtype([("deadline", "<u4"), ("step", "<u2"), ("code", "u1"), ("reserved", "u1")])   # bf_timer_slot, 8 B
+    FIRED_DTYPE = np.dtype([("run", "<u4"), ("step", "<u2"), ("code", "u1"), ("written", "u1")])         # bf_fired, 8 B
+
+    def resident_timers(self, handle: int, slots_per_run: int):
+        """bf_resident_timers: create the batch's timer area with K = slots_per_run slots per run, or grow K keeping every slot"""
+        self._check(self._lib.bf_resident_timers(self._ctx, handle, int(slots_per_run)), "bf_resident_timers")
+
+    def resident_timers_arm(self, handle: int, requests: np.ndarray):
+        """bf_resident_timers_arm: arm (or replace) the timer of each (run, step); deadline A.TIMER_NONE cancels it.
+        requests: TIMER_DTYPE, at most one per (run, step)"""
+        rq = np.ascontiguousarray(requests, dtype=self.TIMER_DTYPE)
+        self._check(self._lib.bf_resident_timers_arm(self._ctx, handle, rq.ctypes.data if rq.shape[0] else None, rq.shape[0]),
+                    "bf_resident_timers_arm")
+
+    def resident_fire(self, handle: int, n_runs: int, now: int, fired_cap: Optional[int] = None,
+                      fired: Optional[np.ndarray] = None) -> dict:
+        """bf_resident_fire: fire the due timers of runs [0, n_runs) at `now` -> dict(n_fired, n_written, n_pruned,
+        next_deadline, fired); fired (FIRED_DTYPE) holds the first min(n_fired, fired_cap) entries, ascending by run and step"""
+        if fired is None:
+            fired = np.zeros(max(fired_cap if fired_cap is not None else 4096, 1), dtype=self.FIRED_DTYPE)
+        cap = fired.shape[0] if fired_cap is None else fired_cap
+        assert fired.dtype == self.FIRED_DTYPE and fired.flags["C_CONTIGUOUS"] and fired.shape[0] >= cap
+        fo = A.FireOut(struct_size=C.sizeof(A.FireOut), n_runs=int(n_runs), fired=fired.ctypes.data, fired_cap=cap)
+        self._check(self._lib.bf_resident_fire(self._ctx, handle, int(now), C.byref(fo)), "bf_resident_fire")
+        return {"n_fired": int(fo.n_fired), "n_written": int(fo.n_written), "n_pruned": int(fo.n_pruned),
+                "next_deadline": int(fo.next_deadline), "fired": fired[:min(int(fo.n_fired), cap)].copy()}
+
+    def resident_timers_download(self, handle: int, first_run: int, n_runs: int, slots_per_run: int) -> np.ndarray:
+        """bf_resident_timers_download -> the raw slots, SLOT_DTYPE array of shape (n_runs, slots_per_run)"""
+        out = np.zeros((n_runs, slots_per_run), dtype=self.SLOT_DTYPE)
+        self._check(self._lib.bf_resident_timers_download(self._ctx, handle, first_run, n_runs, out.ctypes.data),
+                    "bf_resident_timers_download")
+        return out
+
     # -- resident batches: device-side state, delta uploads (row f2)
     DELTA_DTYPE = np.dtype([("run", "<u4"), ("index", "<u2"), ("field", "u1"), ("code", "u1")])
 

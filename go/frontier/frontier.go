@@ -468,6 +468,63 @@ func (r *Resident) TransferTo(dst *Resident, srcN, dstN uint32, runs []uint32) (
 	return t, r.c.err(rc)
 }
 
+// Timer is one arm request of ArmTimers (bf_timer): firing at Deadline writes Code (a DecSucceed for a sleep, a timed-out code
+// for a gate or wait) as the step's decision code; Code 0 (pending) is wake-only; Deadline TimerNone cancels.
+type Timer struct {
+	Run      uint32
+	Step     uint16
+	Code     uint8
+	_        uint8
+	Deadline uint32
+	_        uint32
+}
+
+// Fired is one due timer of Fire (bf_fired): Written is 1 when its code was written and the run touched.
+type Fired struct {
+	Run     uint32
+	Step    uint16
+	Code    uint8
+	Written uint8
+}
+
+// TimerNone is an empty slot's deadline, a cancel's deadline, and NextDeadline when nothing is armed.
+const TimerNone = 0xFFFFFFFF
+
+// FireResult is what Fire reports.  NextDeadline is the batcher's next wake-up: sleep until min(NextDeadline, the next event).
+type FireResult struct {
+	NFired, NWritten, NPruned, NextDeadline uint32
+	Fired                                   []Fired
+}
+
+// EnableTimers gives the batch slotsPerRun timer slots per run (1..64), or grows them keeping every armed timer
+// (bf_resident_timers).  Retire, TransferTo, Migrate and Redrive re-key the timers with the runs from then on.
+func (r *Resident) EnableTimers(slotsPerRun uint32) error {
+	return r.c.err(C.bf_resident_timers(r.c.p, r.handle, C.uint32_t(slotsPerRun)))
+}
+
+// ArmTimers arms, replaces or cancels the timers of (run, step) pairs (bf_resident_timers_arm): the sleepUntil, gateTimeoutAt,
+// waitTimeoutAt and pollInterval entries of a run's step-timers annotation.  A refusal changes nothing.
+func (r *Resident) ArmTimers(timers []Timer) error {
+	var tp *C.bf_timer
+	if len(timers) > 0 {
+		tp = (*C.bf_timer)(unsafe.Pointer(&timers[0]))
+	}
+	return r.c.err(C.bf_resident_timers_arm(r.c.p, r.handle, tp, C.uint32_t(len(timers))))
+}
+
+// Fire fires the timers of runs [0, n) due at now (bf_resident_fire), before TickTouched: the written codes touch their runs
+// as deltas do.  fired receives the first len(fired) due timers, ascending by run and step.
+func (r *Resident) Fire(n, now uint32, fired []Fired) (FireResult, error) {
+	var fp *C.bf_fired
+	if len(fired) > 0 {
+		fp = (*C.bf_fired)(unsafe.Pointer(&fired[0]))
+	}
+	var counts [5]C.uint32_t
+	rc := C.bfgo_resident_fire(r.c.p, r.handle, C.uint32_t(n), C.uint32_t(now), fp, C.uint32_t(len(fired)), &counts[0])
+	return FireResult{NFired: uint32(counts[0]), NWritten: uint32(counts[1]), NPruned: uint32(counts[2]),
+		NextDeadline: uint32(counts[3]), Fired: fired[:counts[4]]}, r.c.err(rc)
+}
+
 // Group is one operator process driving several GPUs (bf_group_*): contiguous blocks of runs per device, one NCCL
 // all-gather of the per-shard counts per pass, limiter totals all-reduced across the shards.
 type Group struct{ p *C.bf_group }

@@ -185,6 +185,21 @@ static inline int bfgo_resident_transfer(bf_ctx* c, uint32_t src, uint32_t dst, 
   return rc;
 }
 
+/* Step timers.  bf_resident_timers and bf_resident_timers_arm are called directly (flat arguments already); bf_resident_fire with
+ * the bf_fire_out built here on the C stack.  counts[5] = n_fired, n_written, n_pruned, next_deadline, entries written into
+ * fired (min(n_fired, fired_cap)). */
+static inline int bfgo_resident_fire(bf_ctx* c, uint32_t handle, uint32_t n_runs, uint32_t now, bf_fired* fired, uint32_t fired_cap,
+                                     uint32_t* counts) {
+  bf_fire_out o;
+  memset(&o, 0, sizeof o);
+  o.struct_size = (uint32_t)sizeof o;
+  o.n_runs = n_runs; o.fired = fired; o.fired_cap = fired_cap;
+  const int rc = bf_resident_fire(c, handle, now, &o);
+  counts[0] = o.n_fired; counts[1] = o.n_written; counts[2] = o.n_pruned; counts[3] = o.next_deadline;
+  counts[4] = o.n_fired < fired_cap ? o.n_fired : fired_cap;
+  return rc;
+}
+
 static inline void bfgo_tables(bf_sched_tables* t, uint32_t n_stories, uint32_t n_queues, int32_t global_limit, uint32_t global_base,
                                const int32_t* story_limit, const uint32_t* story_base, const int32_t* queue_limit,
                                const int32_t* queue_aging_s, const uint32_t* queue_base, const int32_t* queue_max_priority_base) {

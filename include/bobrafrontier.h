@@ -786,6 +786,92 @@ typedef struct bf_transfer {
 
 int bf_resident_transfer(bf_ctx* ctx, uint32_t src_handle, uint32_t dst_handle, bf_transfer* t);
 
+/* ------------------------------------------------------------------ step timers (time-driven transitions of a resident batch)
+ * The reference compares `now` with each run's step timers on every reconcile: sleepUntil fires a sleep step (checkSyncSleepSteps,
+ * dag.go:1217-1288), gateTimeoutAt and waitTimeoutAt time out a gate or a wait (dag.go:1455-1547, :1291-1452), the timers live per
+ * step in the runs.bubustack.io/step-timers annotation (stepTimerStore, dag.go:64,110-171) and the nearest one sets the requeue
+ * (setPollInterval :201-208, RequeueAfter :366-370).  A resident batch keeps these timers itself, in a side area of K slots per
+ * run, so that retire, transfer, migrate and redrive re-key them with the runs and a batcher keeps no timer table of its own.
+ * The area is separate from the state records: bf_layout and the record bytes do not change, and a batch that never calls
+ * bf_resident_timers launches nothing more than before for any call.
+ * Time is a u32 in units the host chooses, one clock for deadlines and `now` (suggested: seconds since the batcher's epoch; the
+ * annotation's metav1.Time values have second resolution).  A timer is DUE iff deadline <= now (`remaining <= 0`, :1266;
+ * `!now.Before(timeoutAt)`, :1434, :1529).
+ * Slot layout, canonical so that downloads compare byte for byte: a run's armed slots first, ascending by step; an empty slot is
+ * deadline = BF_TIMER_NONE with every other byte 0.
+ *
+ * bf_resident_timers(handle, K): creates the area (every slot empty) or grows K, keeping every armed slot.  1 <= K <= 64; a smaller
+ *   K than the current one is BF_EINVAL.  bf_resident_destroy frees the area.
+ * bf_resident_timers_arm(handle, req, n) (host buffer, synchronous): arms the timer of (run, step), replacing an armed one;
+ *   deadline = BF_TIMER_NONE cancels it.  `code` is what firing writes as the step's decision code: BF_DEC_SUCCEED (a sleep),
+ *   BF_DEC_TIMED_OUT (a gate or wait timeout), BF_DEC_FAIL, or BF_DEC_PENDING = wake-only (reported when due, writes nothing: a
+ *   wait step's pollInterval, :1440, where the host re-evaluates `until`).  Checked before anything changes, else BF_EINVAL and
+ *   nothing changed: the handle; the area exists; run < capacity, step < steps_max; code <= 3, reserved fields 0; a non-PENDING
+ *   code needs decision planes (BF_F_DECISION); at most one request per (run, step).  A run whose K slots would overflow is
+ *   BF_ENOMEM and nothing changed (bf_last_error names the run).  Arming touches no run.
+ * bf_resident_fire(handle, now, out) over runs [0, out->n_runs), for each armed slot:
+ *   - the step's phase code is terminal (BF_LUT_TERMINAL): the slot is disarmed ("pruned") and written nowhere, due or not
+ *     (pruneTerminal, dag.go:173-190);
+ *   - else, when due: disarmed and listed in `fired`.  When code != BF_DEC_PENDING and the step's decision code is still
+ *     BF_DEC_PENDING, the code is written exactly as a BF_DELTA_DECISION delta writes it and the run is touched as by a delta
+ *     (written = 1); an approve / reject already delivered takes precedence over a timeout (:1501-1533).  A due timer whose
+ *     decision code is already set, or a wake-only one, is listed with written = 0 and touches nothing.
+ *   Slots of runs at or above n_runs are untouched.  Deltas given later apply after the fire.  Like a delta, the fire ends the
+ *   evaluated snapshot (bf_schedule must follow a new pass).  next_deadline is the batcher's next wake-up: the batch form of
+ *   RequeueAfter.  Two launches, one D2H copy of the counts and one synchronisation; a fired list in pinned memory is written by
+ *   the kernel in place, any other gets the entries that fired copied after the synchronisation.
+ * bf_resident_timers_download(handle, first_run, n_runs, slots): the raw slots (n_runs * K of them), for tests and resyncs.
+ *
+ * What the other calls do to the area (each launches nothing more when the batch has none):
+ *   upload: nothing.  retire: retired runs' slots are emptied, moved runs' slots move with them byte for byte, slots of
+ *   [m, old n_runs) are emptied; a new capacity re-allocates the area.  transfer: the moved runs' armed slots arrive in the
+ *   destination's canonical layout and the source follows retire; a moved run with more armed slots than the destination's K (0
+ *   without an area) is unfit (BF_EINVAL, both batches byte-identical).  migrate: each slot of a migrated run is re-indexed
+ *   through step_map and the run's slots re-sorted; a slot of a BF_MIGRATE_GONE step, or of a step at or above n_old_steps, is
+ *   cancelled.  redrive: every slot of a run with status_out = 1 is emptied, for both kinds of request (the reference deletes
+ *   the whole annotation, storyrun_controller.go:456-525).  reshape: a larger capacity extends the area with empty slots.
+ *   extent / narrow / transfer fit: an armed slot at step s counts s + 1 towards steps_max (over every record below the
+ *   capacity, as state records count) and a non-PENDING one sets BF_F_DECISION in `fields`, so a narrow never drops the decision
+ *   planes a pending timeout needs nor the width of an armed step.                                                         */
+#define BF_TIMER_NONE 0xFFFFFFFFu
+#define BF_TIMER_MAX_SLOTS 64u
+typedef struct bf_timer_slot {  /* 8 B                                                                                    */
+  uint32_t deadline;            /* BF_TIMER_NONE: empty                                                                  */
+  uint16_t step;
+  uint8_t code;                 /* BF_DEC_*                                                                              */
+  uint8_t reserved;
+} bf_timer_slot;
+typedef struct bf_timer {       /* 16 B arm request                                                                      */
+  uint32_t run;
+  uint16_t step;
+  uint8_t code;                 /* BF_DEC_*: what firing writes; BF_DEC_PENDING = wake-only                             */
+  uint8_t reserved;             /* 0                                                                                     */
+  uint32_t deadline;            /* BF_TIMER_NONE cancels                                                                 */
+  uint32_t reserved2;           /* 0                                                                                     */
+} bf_timer;
+typedef struct bf_fired {       /* 8 B                                                                                   */
+  uint32_t run;
+  uint16_t step;
+  uint8_t code;                 /* the slot's code                                                                       */
+  uint8_t written;              /* 1: the code was written into the decision planes and the run touched                 */
+} bf_fired;
+typedef struct bf_fire_out {
+  uint32_t struct_size;         /* sizeof(bf_fire_out)                                                                   */
+  uint32_t n_runs;              /* in: runs [0, n_runs) are fired, n_runs <= capacity                                    */
+  uint32_t n_fired;             /* out: due timers listed (the true count, also past fired_cap)                          */
+  uint32_t n_written;           /* out: of those, the ones that wrote their code                                         */
+  uint32_t n_pruned;            /* out: slots disarmed because their step is terminal                                    */
+  uint32_t next_deadline;       /* out: earliest deadline still armed in [0, n_runs), or BF_TIMER_NONE                   */
+  bf_fired* fired;              /* [fired_cap] out: ascending by run, then by step                                       */
+  uint32_t fired_cap;
+  uint32_t reserved;            /* 0                                                                                     */
+} bf_fire_out;
+
+int bf_resident_timers(bf_ctx* ctx, uint32_t handle, uint32_t slots_per_run);
+int bf_resident_timers_arm(bf_ctx* ctx, uint32_t handle, const bf_timer* requests, uint32_t n);
+int bf_resident_fire(bf_ctx* ctx, uint32_t handle, uint32_t now, bf_fire_out* out);
+int bf_resident_timers_download(bf_ctx* ctx, uint32_t handle, uint32_t first_run, uint32_t n_runs, void* slots);
+
 /* ------------------------------------------------------------------ device groups (SURVEY.md row e)
  * The reference is ONE operator process (cmd/main.go:220, StoryRunReconciler storyrun_controller.go:216), so the
  * multi-GPU path must be reachable from one process through this ABI: a group owns one ctx per device and an NCCL
