@@ -175,6 +175,15 @@ class SchedOut(C.Structure):
                 ("queue_running", C.c_void_p), ("queue_max_priority", C.c_void_p), ("global_running", C.c_void_p)]
 
 
+SEVT_LAUNCH, SEVT_QUEUED_STORY, SEVT_QUEUED_SCHED = 0x1, 0x2, 0x4   # BF_SEVT_*: event kinds of bf_resident_schedule
+
+
+class ResidentSchedPart(C.Structure):
+    _fields_ = [("struct_size", C.c_uint32), ("handle", C.c_uint32), ("n_runs", C.c_uint32), ("runs_cap", C.c_uint32),
+                ("runs", C.c_void_p), ("heads", C.c_void_p), ("events", C.c_void_p), ("events_cap", C.c_uint64),
+                ("n_listed", C.c_uint32), ("full", C.c_uint32), ("n_events", C.c_uint64)]
+
+
 def sched_stride(words: int) -> int:
     return (16 + 12 * words + 15) & ~15
 
@@ -219,6 +228,11 @@ SYMBOLS = [
     ("bf_resident_timers_arm", C.c_int, [C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32]),
     ("bf_resident_fire", C.c_int, [C.c_void_p, C.c_uint32, C.c_uint32, C.POINTER(FireOut)]),
     ("bf_resident_timers_download", C.c_int, [C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32, C.c_void_p]),
+    ("bf_resident_sched", C.c_int, [C.c_void_p, C.c_uint32]),
+    ("bf_resident_sched_put", C.c_int, [C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32]),
+    ("bf_resident_sched_download", C.c_int, [C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32, C.c_void_p]),
+    ("bf_resident_schedule", C.c_int, [C.c_void_p, C.POINTER(SchedTables), C.c_uint32, C.POINTER(ResidentSchedPart), C.c_uint32,
+                                       C.POINTER(SchedOut)]),
     ("bf_group_create", C.c_int, [C.POINTER(C.c_void_p), C.POINTER(C.c_int32), C.c_uint32, C.POINTER(Config)]),
     ("bf_group_destroy", None, [C.c_void_p]),
     ("bf_group_size", C.c_uint32, [C.c_void_p]),

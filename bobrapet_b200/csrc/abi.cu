@@ -649,6 +649,7 @@ static int fill_sched_params(bf_ctx* c, const bf_batch* b, const bf_sched_tables
   P.child_nibbles = L.child_nibbles;
   P.result_stride = L.result_stride; P.off_ready = L.off_ready; P.stride = BF_SCHED_STRIDE(L.words);
   P.slots = c->slots_dev;
+  P.now = BF_SCHED_NONE;   // runs[r].queued_elapsed_s is the elapsed time itself
   return BF_OK;
 }
 
@@ -727,12 +728,12 @@ int schedule_host(bf_ctx* c, const bf_batch* b, const bf_sched_run* runs, const 
   P.queue_base = (with_bases && t->queue_running_base) ? reinterpret_cast<const uint32_t*>(d + o_qb) : nullptr;
   P.queue_maxprio_base = t->queue_max_priority_base ? reinterpret_cast<const int32_t*>(d + o_pb) : nullptr;
   if (!with_bases) P.global_base = 0;
-  cudaError_t e = bf::launch_schedule(P, (uint32_t)c->sm_count, s, 1);
+  cudaError_t e = bf::launch_schedule(P, (uint32_t)c->sm_count, s, bf::kSchedTotals);
   if (e == cudaSuccess && between) {
     const SchedTotals tot{P.story_running, P.queue_running, P.queue_maxprio, P.global_running, (uint32_t)ns, (uint32_t)nq};
     if (int rc = between(user, tot, s)) { cudaStreamSynchronize(s); return rc; }
   }
-  if (e == cudaSuccess) e = bf::launch_schedule(P, (uint32_t)c->sm_count, s, 2);
+  if (e == cudaSuccess) e = bf::launch_schedule(P, (uint32_t)c->sm_count, s, bf::kSchedApply);
   c->stats.kernel_launches += 3;
   auto down = [&](void* dst, size_t o, size_t bytes) -> cudaError_t {
     return (dst && bytes) ? cudaMemcpyAsync(dst, d + o, bytes, cudaMemcpyDeviceToHost, s) : cudaSuccess;

@@ -42,7 +42,9 @@ cudaError_t launch_transfer(const TransferParams& P, cudaStream_t stream);
 cudaError_t launch_relay_timers(const TimerRelayParams& P, cudaStream_t stream);
 cudaError_t launch_arm_timers(const TimerArmParams& P, bool merge, cudaStream_t stream);
 cudaError_t launch_fire(const FireParams& P, cudaStream_t stream);
-cudaError_t launch_schedule(const SchedParams& P, uint32_t sm_count, cudaStream_t stream, uint32_t phases = 3);
+cudaError_t launch_schedule(const SchedParams& P, uint32_t sm_count, cudaStream_t stream, uint32_t phases = kSchedTotals | kSchedApply);
+cudaError_t launch_resident_schedule(const ResSchedParams& R, cudaStream_t stream);
+cudaError_t launch_sched_put(const SchedPutParams& P, cudaStream_t stream);
 cudaError_t launch_closure(const Slot* slots, const uint32_t* slot_ids, const uint32_t* starts, uint32_t n, uint32_t n_slots,
                            uint32_t words_out, uint32_t* masks, cudaStream_t stream);
 cudaError_t launch_validate(const Slot* slots, const uint32_t* slot_ids, uint32_t n, uint32_t n_slots, uint32_t* status,
@@ -199,6 +201,9 @@ struct bf_ctx {
   DevBuf<unsigned long long> d_extent;
   // transfers (bf_resident_transfer): [0, 16) the unfit word | source runs | retire moves | per-run extents (uint4)
   DevBuf<uint8_t> d_transfer;
+  // resident schedules (bf_resident_schedule): tables | totals | per part: run events, CTA sums, the two totals, staged lists;
+  // puts (bf_resident_sched_put): the requests
+  DevBuf<uint8_t> d_rsched;
   // step timers: arms ([0, 16) the overflow word | group starts | arming prefix | sorted requests) and fires ([0, 16) the four
   // output words | per-CTA fired counts | the fired list)
   DevBuf<uint8_t> d_timer;
@@ -276,6 +281,13 @@ inline int cuda_fail(bf_ctx* c, cudaError_t e, const char* what) {
 //   d_timers, timer_k  the step-timer area (bf_resident_timers): cap * timer_k slots, or none (timer_k = 0).  Arm and fire
 //                      change it; retire, transfer, migrate and redrive re-key it in the launches that move the records;
 //                      reshape and a retire to a new capacity re-allocate it; narrow keeps it (the capacity stays).
+//   d_sched_in,        the limiter inputs (bf_resident_sched): cap records, or none.  Put changes them; retire and transfer move
+//   d_sched_rec,       them with their runs; reshape and a retire to a new capacity re-allocate them.  d_sched_rec: the records
+//   sched_base_runs    of the last bf_resident_schedule, cap * BF_SCHED_STRIDE(L.words) bytes; a run at or above sched_base_runs,
+//                      or whose stored reason is kSchedNoBase (uploads, migrations, moves, arrivals), has no baseline.  A change of
+//                      words zeroes sched_base_runs.
+//   ticked             runs covered by a tick since the last call that changed d_state (state_changed), or -1: none since.  A
+//                      resident schedule over n runs needs ticked >= n.
 // A call that changes d_state ends the evaluated snapshot (end_snapshot): bf_schedule must follow a new pass.
 struct Resident {
   bool alive = false, prev_valid = false, need_full = true;
@@ -285,12 +297,26 @@ struct Resident {
   DevBuf<uint32_t> d_mark;
   DevBuf<unsigned long long> d_timers;
   uint32_t timer_k = 0;
+  DevBuf<bf_sched_run> d_sched_in;
+  DevBuf<uint8_t> d_sched_rec;
+  uint32_t sched_base_runs = 0;
+  int64_t ticked = -1;
   uint64_t slot_changes_seen = 0, pending = 0;
   std::map<uint32_t, uint32_t> uploaded;
 
   uint32_t mark_touched() const { return epoch << 1; }
   uint32_t mark_must_list() const { return epoch << 1 | 1u; }
   void end_snapshot(bf_ctx* c) const { if (c->snap.holds(d_state)) c->snap.valid = false; }
+  // a call changes d_state: bf_schedule and bf_resident_schedule must both follow a new tick
+  void state_changed(bf_ctx* c) { end_snapshot(c); ticked = -1; }
+  void tick_done(uint32_t n_runs) { ticked = std::max<int64_t>(ticked, n_runs); }
+  uint32_t sched_stride() const { return BF_SCHED_STRIDE(L.words); }
+  // schedule records for `capacity` runs of `words` words, every run without a baseline (all bytes 0xFF: reason kSchedNoBase)
+  static cudaError_t alloc_sched_rec(DevBuf<uint8_t>& rec, uint32_t capacity, uint32_t words, cudaStream_t s) {
+    const size_t bytes = (size_t)capacity * BF_SCHED_STRIDE(words);
+    cudaError_t e = rec.alloc(bytes);
+    return e == cudaSuccess ? cudaMemsetAsync(rec, 0xFF, bytes, s) : e;
+  }
   // the runs [first, end) were uploaded: the part at or above full_runs, merged with the ranges it touches
   void note_uploaded(uint32_t first, uint32_t end) {
     uint32_t lo = std::max(first, full_runs), hi = end;
@@ -357,6 +383,7 @@ struct Resident {
   // uploaded at its new index, and its result record moved with it (a changed-only tick compares it with its own record).
   void compact_to(uint32_t m, uint32_t N, const std::vector<uint32_t>& moves) {
     full_runs = std::min(full_runs, m);
+    sched_base_runs = std::min(sched_base_runs, m);
     uploaded.erase(uploaded.lower_bound(m), uploaded.end());
     for (auto& u : uploaded) u.second = std::min(u.second, m);
     for (uint32_t to : moves)

@@ -240,6 +240,8 @@ struct MigrateParams {
   unsigned long long* timers;    // [capacity][timer_k] the batch's timer slots (bf_timer_slot), or nullptr: no area
   const uint16_t* fwd;           // [n_old_steps] the step map (new index of old step i, or BF_MIGRATE_GONE), for the timers
   uint32_t timer_k, n_old_steps;
+  uint8_t* sched_rec;            // [capacity][sched_stride] the last schedule records (kSchedNoBase), or nullptr: no area
+  uint32_t sched_stride;
 };
 
 // bf_resident_redrive (resident.cu): the reset sets of the requests are cleared in the records of their runs
@@ -266,6 +268,8 @@ struct ReshapeParams {
   uint8_t* result;               // [n_new][to.result_stride]
   uint32_t n_old, n_new;         // runs r >= n_old get zero records
   bf_layout from, to;
+  const bf_sched_run* old_sched_in;   // the limiter inputs, or nullptr: no area (runs r >= n_old get kSchedDefault)
+  bf_sched_run* sched_in;             // [n_new]
 };
 
 // bf_resident_retire (resident.cu): the runs [m, m + n) vacate their indices; the live ones among them move below m
@@ -280,6 +284,9 @@ struct RetireParams {
   uint32_t state_stride, result_stride;   // multiples of 16
   unsigned long long* timers;    // [capacity][timer_k] timer slots, or nullptr: a mover's slots move with it, vacated ones empty
   uint32_t timer_k;
+  bf_sched_run* sched_in;        // [capacity] limiter inputs, or nullptr: a mover's move with it, vacated ones get kSchedDefault
+  uint8_t* sched_rec;            // [capacity][sched_stride] last schedule records: a mover's target loses its baseline
+  uint32_t sched_stride;
 };
 
 // bf_resident_extent / _narrow (resident.cu): the smallest layout a batch's records and the topologies of its runs allow.  Each
@@ -325,6 +332,10 @@ struct TransferParams {
   const unsigned long long* src_timers;   // [src capacity][src_k] or nullptr
   unsigned long long* dst_timers;         // [dst capacity][dst_k] or nullptr: an arrival's armed slots, the rest empty
   uint32_t src_k, dst_k;                  // a run with more armed slots than dst_k is unfit
+  const bf_sched_run* src_sched_in;       // limiter inputs, or nullptr (an arrival gets kSchedDefault)
+  bf_sched_run* dst_sched_in;             // or nullptr: the destination has no area (then neither has the source)
+  uint8_t* dst_sched_rec;                 // [dst capacity][dst_sched_stride]: an arrival has no baseline
+  uint32_t dst_sched_stride;
 };
 
 // step timers (resident.cu): slot = deadline | step << 32 | code << 48 (bf_timer_slot read as one little-endian u64); an empty
@@ -390,6 +401,40 @@ struct SchedParams {
   int32_t global_limit;
   uint32_t n_stories, n_queues, n_slots, n_runs;
   uint32_t words, state_stride, off_phase, off_child, child_nibbles, result_stride, off_ready, stride;
+  uint32_t now;                // BF_SCHED_NONE: runs[r].queued_elapsed_s holds the elapsed time; else its queue origin
+};
+
+// the phases of launch_schedule (limiters.cu): the totals' start, the counting into them, the truncation against them
+enum : uint32_t { kSchedInit = 1, kSchedCount = 2, kSchedApply = 4, kSchedTotals = kSchedInit | kSchedCount };
+
+// The limiter inputs of a run never put (bf_resident_sched): no keys, priority 0, nothing queued, phase 0
+constexpr bf_sched_run kSchedDefault = {BF_SCHED_NONE, BF_SCHED_NONE, 0, BF_SCHED_NONE, 0, {0u, 0u, 0u}};
+// The reason word of a stored schedule record whose run has no baseline: no limiter writes it, so every new record differs
+constexpr uint32_t kSchedNoBase = 0xFFFFFFFFu;
+
+// bf_resident_schedule, per part (limiters.cu): S holds the part's batch (state, current result, inputs area as runs, the now of
+// the call) and the shared tables and totals; S.records is the batch's schedule-record area, compared and overwritten in place.
+// Runs are taken in CTAs of 256 (8 warps of 32 consecutive runs), the same partition in both launches.
+struct ResSchedParams {
+  SchedParams S;
+  uint32_t base_runs;              // the previous schedule's n_runs: runs at or above it have no baseline
+  uint32_t* run_events;            // [n_runs] events of a listed run, kSchedUnlisted for the others (sched_limit_runs)
+  uint32_t* cta_listed;            // [CTAs] listed runs per CTA, then (sched_scan_ctas) those of the CTAs before it
+  unsigned long long* cta_events;  // [CTAs] their events, likewise
+  unsigned long long* totals;      // [2] out: n_listed, n_events (written by the last CTA of sched_list_runs)
+  uint32_t* runs;                  // [runs_cap]
+  bf_sched_header* heads;          // [runs_cap]
+  uint16_t* events;                // [events_cap]
+  uint32_t runs_cap;
+  unsigned long long events_cap;
+};
+constexpr uint32_t kSchedUnlisted = 0xFFFFFFFFu;
+
+// bf_resident_sched_put: req[i] is written into area[req[i].run]
+struct SchedPutParams {
+  bf_sched_run* area;
+  const bf_sched_put* req;
+  uint32_t n;
 };
 
 }  // namespace bf

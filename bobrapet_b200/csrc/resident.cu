@@ -210,6 +210,7 @@ __global__ void __launch_bounds__(256) migrate_runs(const MigrateParams P) {
     }
     if (P.timers) migrate_timers(P, run, lane);
     if (lane == 0) {
+      if (P.sched_rec) *reinterpret_cast<uint32_t*>(P.sched_rec + (size_t)run * P.sched_stride + 12) = kSchedNoBase;
       *reinterpret_cast<uint32_t*>(rec) = P.new_slot;
       *reinterpret_cast<uint64_t*>(rec + 8) = reg_new;
       P.mark[run] = P.mark_value;
@@ -361,6 +362,7 @@ __global__ void __launch_bounds__(256) reshape_runs(const ReshapeParams P) {
   s = reinterpret_cast<const uint32_t*>(P.old_result + (size_t)r * P.from.result_stride);
   d = reinterpret_cast<uint32_t*>(P.result + (size_t)r * P.to.result_stride);
   for (uint32_t o = lane * 4u; o < P.to.result_stride; o += 128u) d[o >> 2] = keep ? reshape_result_word(s, o, P.from, P.to) : 0u;
+  if (P.sched_in && lane == 0) P.sched_in[r] = keep ? P.old_sched_in[r] : kSchedDefault;
 }
 
 cudaError_t launch_reshape(const ReshapeParams& P, cudaStream_t stream) {
@@ -388,6 +390,13 @@ __global__ void __launch_bounds__(256) retire_runs(const RetireParams P) {
   }
   for (uint32_t k = lane; k < sv; k += 32u) s[k] = make_uint4(0u, 0u, 0u, 0u);
   if (lane == 0) P.mark[from] = 0u;
+  if (P.sched_in && lane == 0) {   // a mover's inputs move with it and its target has no baseline; the vacated index gets the defaults
+    if (to != kRetireNoMove) {
+      P.sched_in[to] = P.sched_in[from];
+      *reinterpret_cast<uint32_t*>(P.sched_rec + (size_t)to * P.sched_stride + 12) = kSchedNoBase;
+    }
+    P.sched_in[from] = kSchedDefault;
+  }
   if (P.timers) {   // each lane stores over only the slots it read itself
     unsigned long long* ts = P.timers + (size_t)from * P.timer_k;
     for (uint32_t k = lane; k < P.timer_k; k += 32u) {
@@ -586,6 +595,10 @@ __global__ void __launch_bounds__(256) transfer_runs(const TransferParams P) {
   d = reinterpret_cast<uint32_t*>(P.dst_result + (size_t)to * P.T.result_stride);
   for (uint32_t o = lane * 4u; o < P.T.result_stride; o += 128u) d[o >> 2] = reshape_result_word(s, o, P.F, P.T);
   if (lane == 0) P.dst_mark[to] = P.mark_value;
+  if (P.dst_sched_in && lane == 0) {   // the run's limiter inputs arrive with it, without a baseline
+    P.dst_sched_in[to] = P.src_sched_in ? P.src_sched_in[r] : kSchedDefault;
+    *reinterpret_cast<uint32_t*>(P.dst_sched_rec + (size_t)to * P.dst_sched_stride + 12) = kSchedNoBase;
+  }
   // the run's armed slots (at most dst_k, transfer_fit) lead the source's slots: copied in order, empty slots behind them
   for (uint32_t k = lane; P.dst_timers && k < P.dst_k; k += 32u)
     P.dst_timers[(size_t)to * P.dst_k + k] = P.src_timers && k < P.src_k ? P.src_timers[(size_t)r * P.src_k + k] : kTimerEmpty;

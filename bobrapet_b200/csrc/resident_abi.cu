@@ -58,9 +58,11 @@ int bf_resident_upload(bf_ctx* c, uint32_t h, uint32_t first, uint32_t n, const 
   if ((uint64_t)first + n > r->cap || (n && !records)) return fail(c, BF_EINVAL, "run range outside the resident batch");
   if (n == 0) return BF_OK;
   BF_CUDA(c, cudaSetDevice(c->device));
-  r->end_snapshot(c);
+  r->state_changed(c);
   r->prev_valid = false;   // full records arrived: the next changed-only tick lists every run
   BF_CUDA(c, cudaMemcpyAsync(r->d_state + (size_t)first * r->L.state_stride, records, (size_t)n * r->L.state_stride, cudaMemcpyHostToDevice, c->stream));
+  if (r->d_sched_in)   // the uploaded runs have no schedule baseline: kSchedNoBase in the reason word of each stored record
+    BF_CUDA(c, cudaMemset2DAsync(r->d_sched_rec + (size_t)first * r->sched_stride() + 12, r->sched_stride(), 0xFF, 4, n, c->stream));
   BF_CUDA(c, bf::launch_mark_runs(r->d_mark, first, n, r->mark_must_list(), c->stream));
   c->stats.kernel_launches += 1;
   r->pending += n;
@@ -123,7 +125,7 @@ int bf_resident_apply(bf_ctx* c, uint32_t h, const bf_delta* deltas, uint32_t n)
   if (n && !deltas) return fail(c, BF_EINVAL, "null deltas");
   if (n == 0) return BF_OK;
   BF_CUDA(c, cudaSetDevice(c->device));
-  r->end_snapshot(c);
+  r->state_changed(c);
   r->pending += n;
   const int rc = resident_apply_async(c, r, deltas, n);
   cudaError_t e = rc == BF_OK ? cudaMemcpyAsync(&c->pinned->word, c->d_rejected, 4, cudaMemcpyDeviceToHost, c->stream) : cudaSuccess;
@@ -139,6 +141,7 @@ int bf_resident_apply(bf_ctx* c, uint32_t h, const bf_delta* deltas, uint32_t n)
 static int resident_tick_locked(bf_ctx* c, Resident* r, const bf_delta* deltas, uint32_t n_deltas, uint32_t n_runs, uint32_t flags,
                                 uint32_t max_iterations, void* result, bf_counts* counts, bf_compact_out* co = nullptr) {
   c->snap.valid = false;
+  if (n_deltas) r->ticked = -1;
   if (co && co->struct_size != sizeof(bf_compact_out)) return fail(c, BF_EINVAL, "bad bf_compact_out.struct_size");
   if (co && co->events_cap && !co->events) return fail(c, BF_EINVAL, "null events with a non-zero events_cap");
   if (n_runs > r->cap || (n_runs && !result && !co)) return fail(c, BF_EINVAL, "n_runs exceeds the resident batch / null result");
@@ -188,6 +191,7 @@ static int resident_tick_locked(bf_ctx* c, Resident* r, const bf_delta* deltas, 
   r->records_unknown();
   if (rc != BF_OK) return rc;
   if (int rc2 = r->full_tick_done(c, n_runs, flags, max_iterations, s)) return rc2;
+  r->tick_done(n_runs);
   if (tail_delivers) c->rejected_clean = true;
   const uint64_t rejected = tail_delivers ? c->pinned->tail.rejected : c->pinned->word;
   if (int rc2 = bf::publish_pass(c, n_runs, L, r->d_state, r->d_result, counts, co, first_slice, c->last_events)) return rc2;
@@ -237,6 +241,7 @@ static int touched_tick_locked(bf_ctx* c, Resident* r, const bf_delta* deltas, u
   }
 
   c->snap.valid = false;
+  if (n_deltas) r->ticked = -1;
   cudaStream_t s = c->stream;
   const bf_layout& L = r->L;
   const uint32_t bound = (uint32_t)std::min<uint64_t>(n_runs, r->pending + n_deltas);   // >= the touched runs below n_runs
@@ -303,6 +308,7 @@ static int touched_tick_locked(bf_ctx* c, Resident* r, const bf_delta* deltas, u
     r->pending = tail.carried;   // every touched run below n_runs was evaluated: the ones above it are all that is left
     c->rejected_clean = true;    // delivered and cleared by the emit kernel
   }
+  r->tick_done(n_runs);
   if (int rc2 = bf::publish_pass(c, n_runs, L, r->d_state, r->d_result, counts, &co, first_slice, c->last_touched_events)) return rc2;
   out->full = 0; out->n_listed = co.n_listed; out->n_evaluated = (uint32_t)tail.evaluated; out->n_events = co.n_events;
   return rejected_deltas(c, rejected, true);
@@ -363,7 +369,7 @@ int bf_resident_migrate(bf_ctx* c, uint32_t h, bf_migration* m) {
   memcpy(blob.data() + o_inv, inv.data(), inv.size() * 2);
   if (!descs.empty()) memcpy(blob.data() + o_desc, descs.data(), descs.size() * sizeof(bf::MigrateDesc));
   if (r->timer_k) memcpy(blob.data() + o_fwd, m->step_map, (size_t)mo.S * 2);   // the timers are re-keyed forwards
-  r->end_snapshot(c);   // as after an upload
+  r->state_changed(c);   // as after an upload
   bf::MigrateParams P{};
   P.state = r->d_state; P.mark = r->d_mark; P.mark_value = r->mark_must_list();
   P.migrated = reinterpret_cast<uint32_t*>(c->d_mig.p);
@@ -374,6 +380,7 @@ int bf_resident_migrate(bf_ctx* c, uint32_t h, bf_migration* m) {
   P.off_decision = L.off_decision; P.off_child = L.off_child; P.child_nibbles = L.child_nibbles;
   P.timers = r->d_timers; P.timer_k = r->timer_k; P.n_old_steps = mo.S;
   P.fwd = reinterpret_cast<const uint16_t*>(c->d_mig + o_fwd);
+  P.sched_rec = r->d_sched_rec; P.sched_stride = r->sched_stride();
   cudaError_t e = cudaMemcpyAsync(c->d_mig, blob.data(), bytes, cudaMemcpyHostToDevice, s);
   if (e == cudaSuccess) e = bf::launch_migrate(P, s);
   if (e == cudaSuccess) e = cudaMemcpyAsync(&c->pinned->word, c->d_mig, 4, cudaMemcpyDeviceToHost, s);
@@ -424,7 +431,7 @@ int bf_resident_redrive(bf_ctx* c, uint32_t h, const bf_redrive* req, uint32_t n
     memcpy(blob.data() + (o_ks - o_req), key_slot.data(), K * 4);
     memcpy(blob.data() + (o_ks - o_req) + K * 4, key_step.data(), K * 4);
   }
-  r->end_snapshot(c);   // as after an upload
+  r->state_changed(c);   // as after an upload
   uint8_t* d = c->d_redrive;
   uint32_t* d_ks = reinterpret_cast<uint32_t*>(d + o_ks);
   uint32_t* d_mask = reinterpret_cast<uint32_t*>(d + o_mask);
@@ -482,12 +489,23 @@ int bf_resident_reshape(bf_ctx* c, uint32_t h, const bf_layout* layout, uint32_t
   if (timers_grow)
     if (cudaError_t e = nb.d_timers.alloc((size_t)capacity * r->timer_k))
       return fail(c, BF_ENOMEM, std::string("resident reshape (timers): ") + cudaGetErrorString(e));
+  // the limiter inputs follow the capacity (defaults for the new runs); the schedule records follow the capacity and the words,
+  // and keep their baselines when the words stay
+  const bool sched = r->d_sched_in, sched_grow = sched && capacity > r->cap, sched_relay = sched && (sched_grow || T.words != F.words);
+  cudaStream_t s = c->stream;
+  if (sched_grow)
+    if (cudaError_t e = nb.d_sched_in.alloc(capacity)) return fail(c, BF_ENOMEM, std::string("resident reshape (limiter inputs): ") + cudaGetErrorString(e));
+  if (sched_relay)
+    if (cudaError_t e = Resident::alloc_sched_rec(nb.d_sched_rec, capacity, T.words, s))
+      return fail(c, BF_ENOMEM, std::string("resident reshape (schedule records): ") + cudaGetErrorString(e));
   const size_t old_mark = r->d_mark.cap * sizeof(uint32_t), new_mark = nb.d_mark.cap * sizeof(uint32_t);
   bf::ReshapeParams P{};
   P.old_state = r->d_state; P.old_result = r->d_result; P.state = nb.d_state; P.result = nb.d_result;
   P.n_old = r->cap; P.n_new = capacity; P.from = F; P.to = T;
-  cudaStream_t s = c->stream;
+  if (sched_grow) { P.old_sched_in = r->d_sched_in; P.sched_in = nb.d_sched_in; }
   cudaError_t e = bf::launch_reshape(P, s);
+  if (e == cudaSuccess && sched_relay && T.words == F.words)
+    e = cudaMemcpyAsync(nb.d_sched_rec, r->d_sched_rec, (size_t)r->cap * r->sched_stride(), cudaMemcpyDeviceToDevice, s);
   if (e == cudaSuccess) e = cudaMemcpyAsync(nb.d_mark, r->d_mark, old_mark, cudaMemcpyDeviceToDevice, s);   // with the list-build padding
   if (e == cudaSuccess && new_mark > old_mark) e = cudaMemsetAsync(reinterpret_cast<uint8_t*>(nb.d_mark.p) + old_mark, 0, new_mark - old_mark, s);
   if (e == cudaSuccess && timers_grow) {
@@ -497,8 +515,11 @@ int bf_resident_reshape(bf_ctx* c, uint32_t h, const bf_layout* layout, uint32_t
   const cudaError_t es = cudaStreamSynchronize(s);
   if (e == cudaSuccess) e = es;
   if (e != cudaSuccess) return cuda_fail(c, e, "bf_resident_reshape");   // the old buffers were only read: the batch is as it was
-  r->end_snapshot(c);   // as after an upload
+  r->state_changed(c);   // as after an upload
   if (timers_grow) r->d_timers = std::move(nb.d_timers);
+  if (sched_grow) r->d_sched_in = std::move(nb.d_sched_in);
+  if (sched_relay) r->d_sched_rec = std::move(nb.d_sched_rec);
+  if (T.words != F.words) r->sched_base_runs = 0;
   r->adopt(std::move(nb), T, capacity);
   if (results_may_change) r->need_full = true;
   return BF_OK;
@@ -615,7 +636,8 @@ int bf_resident_narrow(bf_ctx* c, uint32_t h, const bf_layout* layout, bf_extent
   if (T.off_child != BF_OFF_NONE && T.child_nibbles < e->child_nibbles)
     return fail(c, BF_EINVAL, "the batch needs child_nibbles " + std::to_string(e->child_nibbles));
   if (e->fields & ~placed) return fail(c, BF_EINVAL, "the new layout drops an input field holding a non-default code");
-  r->end_snapshot(c);   // as after an upload
+  r->state_changed(c);   // as after an upload
+  if (T.words != F.words) r->sched_base_runs = 0;   // the schedule records keep their area, which the smaller stride fits
   r->adopt(std::move(nb), T, r->cap);
   r->narrowed(N, results_may_change);
   return BF_OK;
@@ -677,11 +699,18 @@ int bf_resident_retire(bf_ctx* c, uint32_t h, bf_retire* rt) {
   if (resize && r->timer_k)
     if (cudaError_t e = nb.d_timers.alloc((size_t)cap * r->timer_k))
       return fail(c, BF_ENOMEM, std::string("resident retire (timers): ") + cudaGetErrorString(e));
-  r->end_snapshot(c);   // as after an upload
+  const bool sched = r->d_sched_in;
+  if (resize && sched) {
+    cudaError_t e = nb.d_sched_in.alloc(cap);
+    if (e == cudaSuccess) e = nb.d_sched_rec.alloc((size_t)cap * r->sched_stride());
+    if (e != cudaSuccess) return fail(c, BF_ENOMEM, std::string("resident retire (limiter inputs): ") + cudaGetErrorString(e));
+  }
+  r->state_changed(c);   // as after an upload
   bf::RetireParams P{};
   P.state = r->d_state; P.result = r->d_result; P.mark = r->d_mark; P.mark_value = r->mark_must_list();
   P.to = c->d_retire; P.m = m; P.n = n; P.state_stride = L.state_stride; P.result_stride = L.result_stride;
   P.timers = r->d_timers; P.timer_k = r->timer_k;
+  P.sched_in = r->d_sched_in; P.sched_rec = r->d_sched_rec; P.sched_stride = r->sched_stride();
   cudaStream_t s = c->stream;
   cudaError_t e = n ? cudaMemcpyAsync(c->d_retire, to.data(), (size_t)n * 4, cudaMemcpyHostToDevice, s) : cudaSuccess;
   if (e == cudaSuccess) e = bf::launch_retire(P, s);
@@ -691,10 +720,14 @@ int bf_resident_retire(bf_ctx* c, uint32_t h, bf_retire* rt) {
     if (e == cudaSuccess) e = cudaMemcpyAsync(nb.d_mark, r->d_mark, nb.d_mark.cap * sizeof(uint32_t), cudaMemcpyDeviceToDevice, s);
     if (e == cudaSuccess && r->timer_k)
       e = cudaMemcpyAsync(nb.d_timers, r->d_timers, (size_t)cap * r->timer_k * 8, cudaMemcpyDeviceToDevice, s);
+    if (e == cudaSuccess && sched) e = cudaMemcpyAsync(nb.d_sched_in, r->d_sched_in, (size_t)cap * sizeof(bf_sched_run), cudaMemcpyDeviceToDevice, s);
+    if (e == cudaSuccess && sched)
+      e = cudaMemcpyAsync(nb.d_sched_rec, r->d_sched_rec, (size_t)cap * r->sched_stride(), cudaMemcpyDeviceToDevice, s);
   }
   if (int rc = r->sync_in_place(c, e, "bf_resident_retire")) return rc;
   c->stats.kernel_launches += n ? 1 : 0;
   if (resize && r->timer_k) r->d_timers = std::move(nb.d_timers);
+  if (resize && sched) { r->d_sched_in = std::move(nb.d_sched_in); r->d_sched_rec = std::move(nb.d_sched_rec); }
   if (resize) r->adopt(std::move(nb), L, cap);
   r->compact_to(m, N, to);
   write_moves(to, m, rt->moves_from, rt->moves_to);
@@ -727,6 +760,8 @@ int bf_resident_transfer(bf_ctx* c, uint32_t hs, uint32_t hd, bf_transfer* t) {
     gone[q] = 1;
   }
   if (n == 0) { t->n_moves = 0; return BF_OK; }
+  if (src->d_sched_in && !dst->d_sched_in)
+    return fail(c, BF_EINVAL, "the source batch has limiter inputs and the destination has no area for them (bf_resident_sched)");
   const uint32_t m = N - n;
   std::vector<uint32_t> to;
   const uint32_t n_moves = retire_moves(gone, m, n, to);
@@ -754,6 +789,8 @@ int bf_resident_transfer(bf_ctx* c, uint32_t hs, uint32_t hd, bf_transfer* t) {
   if (T.off_phase_out == BF_OFF_NONE) P.R.off_phase_out = BF_OFF_NONE;
   P.extent = reinterpret_cast<uint4*>(c->d_transfer + o_ext); P.unfit = reinterpret_cast<uint32_t*>(c->d_transfer.p);
   P.src_timers = src->d_timers; P.src_k = src->timer_k; P.dst_timers = dst->d_timers; P.dst_k = dst->timer_k;
+  P.src_sched_in = src->d_sched_in; P.dst_sched_in = dst->d_sched_in; P.dst_sched_rec = dst->d_sched_rec;
+  P.dst_sched_stride = dst->sched_stride();
   cudaStream_t s = c->stream;
   BF_CUDA(c, cudaMemcpyAsync(c->d_transfer, blob.data(), blob.size(), cudaMemcpyHostToDevice, s));
   BF_CUDA(c, bf::launch_transfer_fit(P, s));
@@ -776,13 +813,14 @@ int bf_resident_transfer(bf_ctx* c, uint32_t hs, uint32_t hd, bf_transfer* t) {
   // every arrival's record is a changed-only baseline of the source: the destination's may reach over them
   bool src_baseline = src->prev_valid;
   for (uint32_t i = 0; i < n && src_baseline; ++i) src_baseline = t->runs[i] < src->prev_runs;
-  src->end_snapshot(c);   // as after an upload, both batches
-  dst->end_snapshot(c);
+  src->state_changed(c);   // as after an upload, both batches
+  dst->state_changed(c);
   bf::RetireParams Q{};
   Q.state = src->d_state; Q.result = src->d_result; Q.mark = src->d_mark; Q.mark_value = src->mark_must_list();
   Q.to = reinterpret_cast<const uint32_t*>(c->d_transfer + o_to); Q.m = m; Q.n = n;
   Q.state_stride = F.state_stride; Q.result_stride = F.result_stride;
   Q.timers = src->d_timers; Q.timer_k = src->timer_k;
+  Q.sched_in = src->d_sched_in; Q.sched_rec = src->d_sched_rec; Q.sched_stride = src->sched_stride();
   cudaError_t e = bf::launch_transfer(P, s);
   if (e == cudaSuccess) e = bf::launch_retire(Q, s);   // behind the transfer on the stream: the sources are read first
   if (int rc = src->sync_in_place(c, e, "bf_resident_transfer")) { dst->records_unknown(); return rc; }
@@ -923,6 +961,7 @@ int bf_resident_fire(bf_ctx* c, uint32_t h, uint32_t now, bf_fire_out* out) {
     BF_CUDA(c, cudaMemcpy(out->fired, P.fired, (size_t)listed * 8, cudaMemcpyDeviceToHost));
   out->n_fired = words[0]; out->n_written = words[1]; out->n_pruned = words[2]; out->next_deadline = words[3];
   r->pending += out->n_written;   // the touched-list bound counts the written codes as it counts deltas
+  if (out->n_written) r->ticked = -1;
   return BF_OK;
 }
 
@@ -935,5 +974,222 @@ int bf_resident_timers_download(bf_ctx* c, uint32_t h, uint32_t first, uint32_t 
   BF_CUDA(c, cudaSetDevice(c->device));
   BF_CUDA(c, cudaMemcpyAsync(slots, r->d_timers + (size_t)first * r->timer_k, (size_t)n * r->timer_k * 8, cudaMemcpyDeviceToHost, c->stream));
   BF_CUDA(c, cudaStreamSynchronize(c->stream));
+  return BF_OK;
+}
+
+// ---- resident limiters (limiters.cu) ------------------------------------------------------------------------------------------
+// The inputs area: one upload of the defaults and the schedule records' fill, one synchronisation.
+int bf_resident_sched(bf_ctx* c, uint32_t h) {
+  auto [g, r] = lock_resident(c, h);
+  if (!r) return BF_EINVAL;
+  if (r->d_sched_in) return BF_OK;
+  BF_CUDA(c, cudaSetDevice(c->device));
+  DevBuf<bf_sched_run> in;
+  DevBuf<uint8_t> rec;
+  const std::vector<bf_sched_run> defaults(r->cap, bf::kSchedDefault);
+  cudaError_t e = in.alloc(r->cap);
+  if (e == cudaSuccess) e = Resident::alloc_sched_rec(rec, r->cap, r->L.words, c->stream);
+  if (e != cudaSuccess) return fail(c, BF_ENOMEM, std::string("limiter inputs: ") + cudaGetErrorString(e));
+  e = cudaMemcpyAsync(in, defaults.data(), (size_t)r->cap * sizeof(bf_sched_run), cudaMemcpyHostToDevice, c->stream);
+  const cudaError_t es = cudaStreamSynchronize(c->stream);
+  if (e == cudaSuccess) e = es;
+  if (e != cudaSuccess) return cuda_fail(c, e, "bf_resident_sched");
+  r->d_sched_in = std::move(in);
+  r->d_sched_rec = std::move(rec);
+  r->sched_base_runs = 0;
+  return BF_OK;
+}
+
+// Puts: every request checked on the host first, then one H2D copy, one launch, one synchronisation.  No state record changes.
+int bf_resident_sched_put(bf_ctx* c, uint32_t h, const bf_sched_put* req, uint32_t n) {
+  auto [g, r] = lock_resident(c, h);
+  if (!r) return BF_EINVAL;
+  if (!r->d_sched_in) return fail(c, BF_EINVAL, "the batch has no limiter inputs (bf_resident_sched)");
+  if (n && !req) return fail(c, BF_EINVAL, "null requests");
+  std::vector<uint32_t> seen;   // request index + 1 per run named so far
+  for (uint32_t i = 0; i < n; ++i) {
+    const bf_sched_put& q = req[i];
+    auto at = [i] { return "request " + std::to_string(i) + ": "; };
+    if (q.run >= r->cap) return fail(c, BF_EINVAL, at() + "run outside the resident batch");
+    if (q.reserved[0] || q.reserved[1]) return fail(c, BF_EINVAL, at() + "reserved fields must be 0");
+    if (seen.empty()) seen.assign(r->cap, 0u);
+    if (seen[q.run]) return fail(c, BF_EINVAL, "requests " + std::to_string(seen[q.run] - 1) + " and " + std::to_string(i) + " name the same run");
+    seen[q.run] = i + 1;
+  }
+  if (n == 0) return BF_OK;
+  BF_CUDA(c, cudaSetDevice(c->device));
+  if (int rc = c->d_rsched.ensure(c, (size_t)n * sizeof(bf_sched_put))) return rc;
+  bf::SchedPutParams P{r->d_sched_in, reinterpret_cast<const bf_sched_put*>(c->d_rsched.p), n};
+  cudaStream_t s = c->stream;
+  cudaError_t e = cudaMemcpyAsync(c->d_rsched, req, (size_t)n * sizeof(bf_sched_put), cudaMemcpyHostToDevice, s);
+  if (e == cudaSuccess) e = bf::launch_sched_put(P, s);
+  const cudaError_t es = cudaStreamSynchronize(s);
+  if (e == cudaSuccess) e = es;
+  if (e != cudaSuccess) return cuda_fail(c, e, "bf_resident_sched_put");
+  c->stats.kernel_launches += 1;
+  return BF_OK;
+}
+
+int bf_resident_sched_download(bf_ctx* c, uint32_t h, uint32_t first, uint32_t n, bf_sched_put* out) {
+  auto [g, r] = lock_resident(c, h);
+  if (!r) return BF_EINVAL;
+  if (!r->d_sched_in) return fail(c, BF_EINVAL, "the batch has no limiter inputs (bf_resident_sched)");
+  if ((uint64_t)first + n > r->cap || (n && !out)) return fail(c, BF_EINVAL, "run range outside the resident batch");
+  if (n == 0) return BF_OK;
+  BF_CUDA(c, cudaSetDevice(c->device));
+  std::vector<bf_sched_run> in(n);
+  BF_CUDA(c, cudaMemcpyAsync(in.data(), r->d_sched_in + first, (size_t)n * sizeof(bf_sched_run), cudaMemcpyDeviceToHost, c->stream));
+  BF_CUDA(c, cudaStreamSynchronize(c->stream));
+  for (uint32_t i = 0; i < n; ++i)
+    out[i] = bf_sched_put{first + i, in[i].story_key, in[i].queue_key, in[i].priority, in[i].queued_elapsed_s, in[i].run_phase, {0u, 0u}};
+  return BF_OK;
+}
+
+// One schedule over several resident batches: every check first; then the tables' upload, the totals' start, a count launch per
+// part into the shared totals, the limit-and-compare, CTA-scan and list launches per part, the D2H copies of the totals and of each part's
+// two counts, one synchronisation, and the lists of parts whose buffers are not pinned.
+int bf_resident_schedule(bf_ctx* c, const bf_sched_tables* t, uint32_t now, bf_resident_sched_part* parts, uint32_t n_parts,
+                         bf_sched_out* totals) {
+  if (!c) return BF_EINVAL;
+  std::lock_guard<std::mutex> g(c->mu);
+  if (!t || t->struct_size != sizeof(bf_sched_tables)) return fail(c, BF_EINVAL, "bad bf_sched_tables.struct_size");
+  if ((t->n_stories && !t->story_limit) || (t->n_queues && (!t->queue_limit || !t->queue_aging_s)))
+    return fail(c, BF_EINVAL, "null limit table");
+  if (!totals || totals->struct_size != sizeof(bf_sched_out)) return fail(c, BF_EINVAL, "bad bf_sched_out.struct_size");
+  if (now == BF_SCHED_NONE) return fail(c, BF_EINVAL, "now must be below BF_SCHED_NONE");
+  if (n_parts && !parts) return fail(c, BF_EINVAL, "null parts");
+  std::vector<Resident*> rs(n_parts);
+  for (uint32_t i = 0; i < n_parts; ++i) {
+    const bf_resident_sched_part& p = parts[i];
+    auto at = [&] { return "part " + std::to_string(i) + " (batch " + std::to_string(p.handle) + "): "; };
+    if (p.struct_size != sizeof(bf_resident_sched_part)) return fail(c, BF_EINVAL, "part " + std::to_string(i) + ": bad struct_size");
+    Resident* r = p.handle < c->resident.size() && c->resident[p.handle].alive ? &c->resident[p.handle] : nullptr;
+    if (!r) return fail(c, BF_EINVAL, at() + "unknown resident batch");
+    for (uint32_t k = 0; k < i; ++k)
+      if (parts[k].handle == p.handle) return fail(c, BF_EINVAL, at() + "the batch is also part " + std::to_string(k));
+    if (!r->d_sched_in) return fail(c, BF_EINVAL, at() + "the batch has no limiter inputs (bf_resident_sched)");
+    if (p.n_runs > r->cap) return fail(c, BF_EINVAL, at() + "n_runs exceeds the resident batch");
+    if (p.runs_cap && (!p.runs || !p.heads)) return fail(c, BF_EINVAL, at() + "null runs / heads with a non-zero runs_cap");
+    if (p.events_cap && !p.events) return fail(c, BF_EINVAL, at() + "null events with a non-zero events_cap");
+    if (r->ticked < (int64_t)p.n_runs)
+      return fail(c, BF_EINVAL, at() + "its state records changed since its last tick over " + std::to_string(p.n_runs) +
+                                    " runs: a tick must come between them and the schedule");
+    rs[i] = r;
+  }
+  BF_CUDA(c, cudaSetDevice(c->device));
+  cudaStream_t s = c->stream;
+  if (int rc = bf::sync_slots(c, s)) return rc;   // topology puts and drops since the ticks count as they stand now
+  // one device allocation: tables | totals | per part: run events | CTA listed | CTA events | two totals | staged lists
+  const size_t ns = t->n_stories, nq = t->n_queues;
+  size_t off = 0;
+  auto take = [&](size_t bytes) { const size_t o = off; off = round_up_sz(off + bytes, 16); return o; };
+  const size_t o_sl = take(ns * 4), o_ql = take(nq * 4), o_qa = take(nq * 4), o_sb = take(ns * 4), o_qb = take(nq * 4),
+               o_pb = take(nq * 4), o_sr = take(ns * 4), o_qr = take(nq * 4), o_mp = take(nq * 4), o_gl = take(4);
+  struct Plan { size_t ev, cl, ce, tot, runs, heads, events; uint32_t rcap; uint64_t ecap; uint32_t* p_runs; bf_sched_header* p_heads; uint16_t* p_events; };
+  std::vector<Plan> plan(n_parts);
+  for (uint32_t i = 0; i < n_parts; ++i) {
+    const bf_resident_sched_part& p = parts[i];
+    Plan& q = plan[i];
+    const size_t grid = ((size_t)p.n_runs + 255) / 256;
+    q.rcap = std::min(p.runs_cap, p.n_runs);
+    q.ecap = std::min<uint64_t>(p.events_cap, (uint64_t)p.n_runs * rs[i]->L.words * 32);
+    q.p_runs = q.rcap ? static_cast<uint32_t*>(bf::pinned_dev(p.runs)) : nullptr;
+    q.p_heads = q.rcap ? static_cast<bf_sched_header*>(bf::pinned_dev(p.heads)) : nullptr;
+    q.p_events = q.ecap ? static_cast<uint16_t*>(bf::pinned_dev(p.events)) : nullptr;
+    const bool stage_runs = q.rcap && !(q.p_runs && q.p_heads);
+    q.ev = take((size_t)p.n_runs * 4); q.cl = take(grid * 4); q.ce = take(grid * 8); q.tot = take(16);
+    q.runs = take(stage_runs ? (size_t)q.rcap * 4 : 0); q.heads = take(stage_runs ? (size_t)q.rcap * sizeof(bf_sched_header) : 0);
+    q.events = take(q.ecap && !q.p_events ? (size_t)q.ecap * 2 : 0);
+    if (!stage_runs && q.rcap) q.runs = q.heads = SIZE_MAX;   // posted in place
+  }
+  if (int rc = c->d_rsched.ensure(c, off ? off : 16)) return rc;
+  uint8_t* d = c->d_rsched;
+  auto up = [&](size_t o, const void* src, size_t bytes) -> cudaError_t {
+    return (src && bytes) ? cudaMemcpyAsync(d + o, src, bytes, cudaMemcpyHostToDevice, s) : cudaSuccess;
+  };
+  BF_CUDA(c, up(o_sl, t->story_limit, ns * 4));
+  BF_CUDA(c, up(o_ql, t->queue_limit, nq * 4));
+  BF_CUDA(c, up(o_qa, t->queue_aging_s, nq * 4));
+  BF_CUDA(c, up(o_sb, t->story_running_base, ns * 4));
+  BF_CUDA(c, up(o_qb, t->queue_running_base, nq * 4));
+  BF_CUDA(c, up(o_pb, t->queue_max_priority_base, nq * 4));
+  bf::SchedParams S{};
+  S.n_stories = t->n_stories; S.n_queues = t->n_queues; S.global_limit = t->global_limit; S.global_base = t->global_running_base;
+  S.n_slots = (uint32_t)c->slots_host.size(); S.slots = c->slots_dev; S.now = now;
+  S.story_running = reinterpret_cast<uint32_t*>(d + o_sr); S.queue_running = reinterpret_cast<uint32_t*>(d + o_qr);
+  S.queue_maxprio = reinterpret_cast<int32_t*>(d + o_mp); S.global_running = reinterpret_cast<uint32_t*>(d + o_gl);
+  S.story_limit = reinterpret_cast<const int32_t*>(d + o_sl); S.queue_limit = reinterpret_cast<const int32_t*>(d + o_ql);
+  S.queue_aging = reinterpret_cast<const int32_t*>(d + o_qa);
+  S.story_base = t->story_running_base ? reinterpret_cast<const uint32_t*>(d + o_sb) : nullptr;
+  S.queue_base = t->queue_running_base ? reinterpret_cast<const uint32_t*>(d + o_qb) : nullptr;
+  S.queue_maxprio_base = t->queue_max_priority_base ? reinterpret_cast<const int32_t*>(d + o_pb) : nullptr;
+  auto part_params = [&](uint32_t i) {
+    const Resident* r = rs[i];
+    const bf_layout& L = r->L;
+    bf::SchedParams P = S;
+    P.state = r->d_state; P.result = r->d_result; P.runs = r->d_sched_in; P.records = r->d_sched_rec; P.n_runs = parts[i].n_runs;
+    P.words = L.words; P.state_stride = L.state_stride; P.off_phase = L.off_phase; P.off_child = L.off_child;
+    P.child_nibbles = L.child_nibbles; P.result_stride = L.result_stride; P.off_ready = L.off_ready; P.stride = r->sched_stride();
+    return P;
+  };
+  std::vector<unsigned long long> part_tot((size_t)n_parts * 2, 0ull);
+  uint64_t launches = 1;
+  auto body = [&]() -> cudaError_t {
+    cudaError_t e = bf::launch_schedule(S, (uint32_t)c->sm_count, s, bf::kSchedInit);
+    for (uint32_t i = 0; i < n_parts && e == cudaSuccess; ++i)
+      if (parts[i].n_runs) { e = bf::launch_schedule(part_params(i), (uint32_t)c->sm_count, s, bf::kSchedCount); ++launches; }
+    for (uint32_t i = 0; i < n_parts && e == cudaSuccess; ++i) {
+      const Plan& q = plan[i];
+      bf::ResSchedParams R{};
+      R.S = part_params(i);
+      R.base_runs = rs[i]->sched_base_runs;
+      R.run_events = reinterpret_cast<uint32_t*>(d + q.ev);
+      R.cta_listed = reinterpret_cast<uint32_t*>(d + q.cl);
+      R.cta_events = reinterpret_cast<unsigned long long*>(d + q.ce);
+      R.totals = reinterpret_cast<unsigned long long*>(d + q.tot);
+      R.runs_cap = q.rcap; R.events_cap = q.ecap;
+      if (q.rcap) {
+        R.runs = q.runs == SIZE_MAX ? q.p_runs : reinterpret_cast<uint32_t*>(d + q.runs);
+        R.heads = q.heads == SIZE_MAX ? q.p_heads : reinterpret_cast<bf_sched_header*>(d + q.heads);
+      }
+      if (q.ecap) R.events = q.p_events ? q.p_events : reinterpret_cast<uint16_t*>(d + q.events);
+      if (parts[i].n_runs) {
+        e = bf::launch_resident_schedule(R, s);
+        launches += 3;
+        if (e == cudaSuccess) e = cudaMemcpyAsync(&part_tot[2 * i], R.totals, 16, cudaMemcpyDeviceToHost, s);
+      }
+    }
+    auto down = [&](void* dst, size_t o, size_t bytes) -> cudaError_t {
+      return (dst && bytes) ? cudaMemcpyAsync(dst, d + o, bytes, cudaMemcpyDeviceToHost, s) : cudaSuccess;
+    };
+    if (e == cudaSuccess) e = down(totals->story_running, o_sr, ns * 4);
+    if (e == cudaSuccess) e = down(totals->queue_running, o_qr, nq * 4);
+    if (e == cudaSuccess) e = down(totals->queue_max_priority, o_mp, nq * 4);
+    if (e == cudaSuccess) e = down(totals->global_running, o_gl, 4);
+    return e;
+  };
+  cudaError_t e = body();
+  const cudaError_t es = cudaStreamSynchronize(s);   // never return with copies into the caller's buffers in flight
+  if (e == cudaSuccess) e = es;
+  c->stats.kernel_launches += launches;
+  if (e != cudaSuccess) {   // the schedule records may be half written: no baseline survives
+    for (Resident* r : rs) r->sched_base_runs = 0;
+    return cuda_fail(c, e, "bf_resident_schedule");
+  }
+  for (uint32_t i = 0; i < n_parts; ++i) {
+    bf_resident_sched_part& p = parts[i];
+    const Plan& q = plan[i];
+    p.n_listed = (uint32_t)part_tot[2 * i];
+    p.n_events = part_tot[2 * i + 1];
+    p.full = p.n_listed == p.n_runs ? 1u : 0u;
+    rs[i]->sched_base_runs = p.n_runs;
+    const uint32_t nl = std::min(p.n_listed, q.rcap);
+    if (nl && q.runs != SIZE_MAX) {
+      BF_CUDA(c, cudaMemcpy(p.runs, d + q.runs, (size_t)nl * 4, cudaMemcpyDeviceToHost));
+      BF_CUDA(c, cudaMemcpy(p.heads, d + q.heads, (size_t)nl * sizeof(bf_sched_header), cudaMemcpyDeviceToHost));
+    }
+    const uint64_t ne = std::min<uint64_t>(p.n_events, q.ecap);
+    if (ne && !q.p_events) BF_CUDA(c, cudaMemcpy(p.events, d + q.events, (size_t)ne * 2, cudaMemcpyDeviceToHost));
+  }
   return BF_OK;
 }

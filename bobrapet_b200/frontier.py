@@ -333,6 +333,74 @@ class Frontier:
                     "bf_resident_timers_download")
         return out
 
+    # -- limiter inputs and schedules of resident batches (bf_resident_sched*, bf_resident_schedule)
+    SCHED_PUT_DTYPE = np.dtype([("run", "<u4"), ("story_key", "<u4"), ("queue_key", "<u4"), ("priority", "<i4"),
+                                ("queued_since", "<u4"), ("run_phase", "<u4"), ("reserved", "<u4", (2,))])   # bf_sched_put, 32 B
+    SCHED_HEAD_DTYPE = np.dtype([("n_launch", "<u4"), ("n_queued_story", "<u4"), ("n_queued_sched", "<u4"),
+                                 ("reason", "<u4")])                                                         # bf_sched_header
+
+    def resident_sched(self, handle: int):
+        """bf_resident_sched: create the batch's limiter-inputs area, every run at the defaults"""
+        self._check(self._lib.bf_resident_sched(self._ctx, handle), "bf_resident_sched")
+
+    def resident_sched_put(self, handle: int, requests: np.ndarray):
+        """bf_resident_sched_put: write the limiter inputs of each requests[i].run (SCHED_PUT_DTYPE, at most one per run)"""
+        rq = np.ascontiguousarray(requests, dtype=self.SCHED_PUT_DTYPE)
+        self._check(self._lib.bf_resident_sched_put(self._ctx, handle, rq.ctypes.data if rq.shape[0] else None, rq.shape[0]),
+                    "bf_resident_sched_put")
+
+    def resident_sched_download(self, handle: int, first_run: int, n_runs: int) -> np.ndarray:
+        """bf_resident_sched_download -> the stored inputs of runs [first_run, first_run + n_runs), SCHED_PUT_DTYPE"""
+        out = np.zeros(n_runs, dtype=self.SCHED_PUT_DTYPE)
+        self._check(self._lib.bf_resident_sched_download(self._ctx, handle, first_run, n_runs, out.ctypes.data),
+                    "bf_resident_sched_download")
+        return out
+
+    def resident_schedule(self, parts, tables: dict, now: int) -> dict:
+        """bf_resident_schedule over several resident batches against one set of totals.  parts: list of dicts with handle,
+        n_runs and optionally runs_cap / events_cap (default: n_runs and n_runs * 1024) and pinned buffers runs / heads / events.
+        tables: Frontier.schedule's keyword arguments.  -> dict(parts=[dict(runs, heads, events, n_listed, full, n_events)],
+        story_running, queue_running, queue_max_priority, global_running)"""
+        sl = np.ascontiguousarray(tables["story_limit"], dtype=np.int32)
+        ql = np.ascontiguousarray(tables["queue_limit"], dtype=np.int32)
+        qa = np.ascontiguousarray(tables["queue_aging_s"], dtype=np.int32)
+        arr = lambda k, dt: None if tables.get(k) is None else np.ascontiguousarray(tables[k], dtype=dt)  # noqa: E731
+        sb, qb, pb = arr("story_running_base", np.uint32), arr("queue_running_base", np.uint32), arr("queue_max_priority_base", np.int32)
+        t = A.SchedTables(struct_size=C.sizeof(A.SchedTables), n_stories=sl.size, n_queues=ql.size,
+                          global_limit=int(tables.get("global_limit", 0)), global_running_base=int(tables.get("global_running_base", 0)),
+                          story_limit=sl.ctypes.data, story_running_base=(sb.ctypes.data if sb is not None else None),
+                          queue_limit=ql.ctypes.data, queue_aging_s=qa.ctypes.data,
+                          queue_running_base=(qb.ctypes.data if qb is not None else None),
+                          queue_max_priority_base=(pb.ctypes.data if pb is not None else None))
+        ps = (A.ResidentSchedPart * max(len(parts), 1))()
+        bufs = []
+        for i, p in enumerate(parts):
+            n = int(p["n_runs"])
+            rcap = int(p.get("runs_cap", n))
+            ecap = int(p.get("events_cap", n * 1024))
+            runs = p.get("runs", np.zeros(max(rcap, 1), np.uint32))
+            heads = p.get("heads", np.zeros(max(rcap, 1), self.SCHED_HEAD_DTYPE))
+            events = p.get("events", np.zeros(max(ecap, 1), np.uint16))
+            bufs.append((runs, heads, events, rcap, ecap))
+            ps[i] = A.ResidentSchedPart(struct_size=C.sizeof(A.ResidentSchedPart), handle=int(p["handle"]), n_runs=n, runs_cap=rcap,
+                                        runs=runs.ctypes.data, heads=heads.ctypes.data, events=events.ctypes.data, events_cap=ecap)
+        sr = np.zeros(max(sl.size, 1), dtype=np.uint32)
+        qr = np.zeros(max(ql.size, 1), dtype=np.uint32)
+        mp = np.zeros(max(ql.size, 1), dtype=np.int32)
+        gr = np.zeros(1, dtype=np.uint32)
+        out = A.SchedOut(struct_size=C.sizeof(A.SchedOut), records=None, story_running=sr.ctypes.data, queue_running=qr.ctypes.data,
+                         queue_max_priority=mp.ctypes.data, global_running=gr.ctypes.data)
+        self._check(self._lib.bf_resident_schedule(self._ctx, C.byref(t), int(now), ps, len(parts), C.byref(out)),
+                    "bf_resident_schedule")
+        res = []
+        for i, (runs, heads, events, rcap, ecap) in enumerate(bufs):
+            q = ps[i]
+            nl = min(int(q.n_listed), rcap)
+            res.append({"runs": runs[:nl].copy(), "heads": heads[:nl].copy(), "events": events[:min(int(q.n_events), ecap)].copy(),
+                        "n_listed": int(q.n_listed), "full": int(q.full), "n_events": int(q.n_events)})
+        return {"parts": res, "story_running": sr[:sl.size], "queue_running": qr[:ql.size], "queue_max_priority": mp[:ql.size],
+                "global_running": int(gr[0])}
+
     # -- resident batches: device-side state, delta uploads (row f2)
     DELTA_DTYPE = np.dtype([("run", "<u4"), ("index", "<u2"), ("field", "u1"), ("code", "u1")])
 

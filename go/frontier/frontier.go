@@ -525,6 +525,138 @@ func (r *Resident) Fire(n, now uint32, fired []Fired) (FireResult, error) {
 		NextDeadline: uint32(counts[3]), Fired: fired[:counts[4]]}, r.c.err(rc)
 }
 
+// SchedPut is one limiter-input request of PutSched (bf_sched_put, 32 bytes, no pointers).  QueuedSince is the StartedAt of the
+// run's earliest queued step on the clock of ScheduleResident's now (SchedNone: nothing queued); the device ages from it.
+type SchedPut struct {
+	Run, StoryKey, QueueKey uint32
+	Priority                int32
+	QueuedSince, RunPhase   uint32
+	_                       [2]uint32
+}
+
+// SchedNone is a key, a queue origin or an elapsed time that is absent (BF_SCHED_NONE).
+const SchedNone = 0xFFFFFFFF
+
+// SchedHeader mirrors bf_sched_header: the steps to launch, queued by the Story's limit and queued by the scheduling limits,
+// and why the latter were queued (BF_QUEUED_*).
+type SchedHeader struct {
+	NLaunch, NQueuedStory, NQueuedSched, Reason uint32
+}
+
+// Event kinds of ScheduleResident (BF_SEVT_*).
+const (
+	SevtLaunch      = 0x1
+	SevtQueuedStory = 0x2
+	SevtQueuedSched = 0x4
+)
+
+// EnableSched gives the batch its limiter-inputs area, every run at the defaults (no keys, priority 0, nothing queued)
+// (bf_resident_sched).  Retire and TransferTo move the inputs with the runs from then on.
+func (r *Resident) EnableSched() error { return r.c.err(C.bf_resident_sched(r.c.p, r.handle)) }
+
+// PutSched writes the limiter inputs of chosen runs (bf_resident_sched_put): when the batcher first packs a run, and again when
+// its keys, priority, StoryRun phase or queue origin change.  At most one request per run; a refusal changes nothing.
+func (r *Resident) PutSched(reqs []SchedPut) error {
+	var rp *C.bf_sched_put
+	if len(reqs) > 0 {
+		rp = (*C.bf_sched_put)(unsafe.Pointer(&reqs[0]))
+	}
+	return r.c.err(C.bf_resident_sched_put(r.c.p, r.handle, rp, C.uint32_t(len(reqs))))
+}
+
+// SchedBuffers are the list buffers of one ScheduleResident part, in pinned C memory so that the kernels write them in place.
+type SchedBuffers struct {
+	Runs   []uint32
+	Heads  []SchedHeader
+	Events []uint16
+	mem    [3]unsafe.Pointer
+}
+
+// NewSchedBuffers allocates the lists of one part: runsCap runs and heads, eventsCap events.
+func (c *Ctx) NewSchedBuffers(runsCap, eventsCap uint32) (*SchedBuffers, error) {
+	b := &SchedBuffers{}
+	sizes := [3]C.size_t{C.size_t(runsCap) * 4, C.size_t(runsCap) * 16, C.size_t(eventsCap) * 2}
+	for i, n := range sizes {
+		if n == 0 {
+			n = 16
+		}
+		if err := c.err(C.bf_alloc_pinned(c.p, n, &b.mem[i])); err != nil {
+			c.FreeSchedBuffers(b)
+			return nil, err
+		}
+	}
+	b.Runs = unsafe.Slice((*uint32)(b.mem[0]), runsCap)
+	b.Heads = unsafe.Slice((*SchedHeader)(b.mem[1]), runsCap)
+	b.Events = unsafe.Slice((*uint16)(b.mem[2]), eventsCap)
+	return b, nil
+}
+
+// FreeSchedBuffers returns the buffers' pinned memory.
+func (c *Ctx) FreeSchedBuffers(b *SchedBuffers) {
+	for i, p := range b.mem {
+		if p != nil {
+			C.bf_free_pinned(c.p, p)
+			b.mem[i] = nil
+		}
+	}
+}
+
+// SchedPart is one batch of ScheduleResident: its runs [0, N) are counted and limited, and the listed ones land in Buf.
+type SchedPart struct {
+	R   *Resident
+	N   uint32
+	Buf *SchedBuffers
+}
+
+// SchedListed is what ScheduleResident reports per part: Buf holds the first min(NListed, len(Buf.Runs)) listed runs and the
+// first min(NEvents, len(Buf.Events)) events; Full when every run of [0, N) was listed.
+type SchedListed struct {
+	NListed uint32
+	Full    bool
+	NEvents uint64
+}
+
+// ScheduleResident limits the runs of every part against one set of totals (bf_resident_schedule): the tables' bases plus
+// the Running StepRuns and queue priority maxima of all parts, so the limits and the priority ordering hold across width
+// classes.  Call it once per tick after TickTouched of every batch; only the runs whose schedule changed are listed.
+func (c *Ctx) ScheduleResident(now uint32, t *SchedTables, parts ...SchedPart) ([]SchedListed, *SchedResult, error) {
+	res := &SchedResult{
+		StoryRunning: make([]uint32, len(t.StoryLimit)),
+		QueueRunning: make([]uint32, len(t.QueueLimit)),
+		QueueMaxPrio: make([]int32, len(t.QueueLimit)),
+	}
+	ps := make([]C.bf_resident_sched_part, len(parts))   // Go memory holding only C pointers
+	for i, p := range parts {
+		capRuns := len(p.Buf.Runs)
+		if len(p.Buf.Heads) < capRuns {
+			capRuns = len(p.Buf.Heads)
+		}
+		var rp *C.uint32_t
+		var hp *C.bf_sched_header
+		var ep *C.uint16_t
+		if capRuns > 0 {
+			rp, hp = (*C.uint32_t)(unsafe.Pointer(&p.Buf.Runs[0])), (*C.bf_sched_header)(unsafe.Pointer(&p.Buf.Heads[0]))
+		}
+		if len(p.Buf.Events) > 0 {
+			ep = (*C.uint16_t)(unsafe.Pointer(&p.Buf.Events[0]))
+		}
+		C.bfgo_sched_part(&ps[i], p.R.handle, C.uint32_t(p.N), rp, hp, C.uint32_t(capRuns), ep, C.uint64_t(len(p.Buf.Events)))
+	}
+	var pp *C.bf_resident_sched_part
+	if len(ps) > 0 {
+		pp = &ps[0]
+	}
+	rc := C.bfgo_resident_schedule(c.p, C.uint32_t(now), C.uint32_t(len(t.StoryLimit)), C.uint32_t(len(t.QueueLimit)),
+		C.int32_t(t.GlobalLimit), C.uint32_t(t.GlobalBase), i32p(t.StoryLimit), u32p(t.StoryRunningBase), i32p(t.QueueLimit),
+		i32p(t.QueueAgingS), u32p(t.QueueRunningBase), i32p(t.QueueMaxPriorityBase), pp, C.uint32_t(len(ps)),
+		u32p(res.StoryRunning), u32p(res.QueueRunning), i32p(res.QueueMaxPrio), (*C.uint32_t)(unsafe.Pointer(&res.GlobalRunning)))
+	out := make([]SchedListed, len(parts))
+	for i := range ps {
+		out[i] = SchedListed{NListed: uint32(ps[i].n_listed), Full: ps[i].full != 0, NEvents: uint64(ps[i].n_events)}
+	}
+	return out, res, c.err(rc)
+}
+
 // Group is one operator process driving several GPUs (bf_group_*): contiguous blocks of runs per device, one NCCL
 // all-gather of the per-shard counts per pass, limiter totals all-reduced across the shards.
 type Group struct{ p *C.bf_group }

@@ -73,6 +73,40 @@ func RowsTouched(runs, head []uint32, events []uint16, set func(run uint32, row 
 	return true
 }
 
+// SchedRow is one run's schedule from ScheduleResident: its header and the steps of its three masks, ascending.
+type SchedRow struct {
+	Header                         SchedHeader
+	Launch, QueuedStory, QueuedSched []uint16
+}
+
+// RowsScheduled decodes the listed runs of a ScheduleResident part: runs[:k], heads[:k] and events with k = min(NListed, buffer
+// length), set called once per listed run.  False when the events do not cover the heads (NEvents past the buffer): resync.
+// The launch steps go to StepExecutor.Execute, the queued ones to markQueuedSteps.
+func RowsScheduled(runs []uint32, heads []SchedHeader, events []uint16, set func(run uint32, row SchedRow)) bool {
+	pos := 0
+	for i, h := range heads {
+		n := int(h.NLaunch + h.NQueuedStory + h.NQueuedSched)
+		if i >= len(runs) || pos+n > len(events) {
+			return false
+		}
+		row := SchedRow{Header: h}
+		for _, e := range events[pos : pos+n] {
+			step := e & 0x3FF
+			switch e >> 10 {
+			case SevtLaunch:
+				row.Launch = append(row.Launch, step)
+			case SevtQueuedStory:
+				row.QueuedStory = append(row.QueuedStory, step)
+			default:
+				row.QueuedSched = append(row.QueuedSched, step)
+			}
+		}
+		set(runs[i], row)
+		pos += n
+	}
+	return true
+}
+
 // Steps turns the row back into the three results of findReadySteps (dag.go:2631-2641) over `steps` =
 // allStorySteps(story) — index i of the packed topology is &steps[i].
 func (r Row) Steps(steps []bubuv1alpha1.Step) (ready, skipped []*bubuv1alpha1.Step, reasons map[string]string) {

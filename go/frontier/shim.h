@@ -233,6 +233,31 @@ static inline int bfgo_schedule(bf_ctx* c, const bf_layout* L, uint32_t n_runs, 
   return bf_schedule(c, &b, runs, &t, &o);
 }
 
+/* Resident limiters.  bf_resident_sched, _sched_put and _sched_download are called directly (flat arguments already); a part of
+ * bf_resident_schedule is filled here (its list buffers are C memory, pinned for the kernels to write them in place), and the call
+ * takes the tables flat as bfgo_schedule does. */
+static inline void bfgo_sched_part(bf_resident_sched_part* p, uint32_t handle, uint32_t n_runs, uint32_t* runs, bf_sched_header* heads,
+                                   uint32_t runs_cap, uint16_t* events, uint64_t events_cap) {
+  memset(p, 0, sizeof *p);
+  p->struct_size = (uint32_t)sizeof *p;
+  p->handle = handle; p->n_runs = n_runs;
+  p->runs = runs; p->heads = heads; p->runs_cap = runs_cap; p->events = events; p->events_cap = events_cap;
+}
+
+static inline int bfgo_resident_schedule(bf_ctx* c, uint32_t now, uint32_t n_stories, uint32_t n_queues, int32_t global_limit,
+                                         uint32_t global_base, const int32_t* story_limit, const uint32_t* story_base,
+                                         const int32_t* queue_limit, const int32_t* queue_aging_s, const uint32_t* queue_base,
+                                         const int32_t* queue_max_priority_base, bf_resident_sched_part* parts, uint32_t n_parts,
+                                         uint32_t* story_running, uint32_t* queue_running, int32_t* queue_max_priority,
+                                         uint32_t* global_running) {
+  bf_sched_tables t;
+  bf_sched_out o;
+  bfgo_tables(&t, n_stories, n_queues, global_limit, global_base, story_limit, story_base, queue_limit, queue_aging_s, queue_base,
+              queue_max_priority_base);
+  bfgo_sched_out(&o, NULL, story_running, queue_running, queue_max_priority, global_running);
+  return bf_resident_schedule(c, &t, now, parts, n_parts, &o);
+}
+
 static inline int bfgo_group_eval(bf_group* g, const bf_layout* L, uint32_t n_runs, uint32_t flags, uint32_t max_iterations,
                                   const void* state, void* result, bf_counts* shard_counts, bf_counts* global_counts) {
   bf_batch b;

@@ -872,6 +872,89 @@ int bf_resident_timers_arm(bf_ctx* ctx, uint32_t handle, const bf_timer* request
 int bf_resident_fire(bf_ctx* ctx, uint32_t handle, uint32_t now, bf_fire_out* out);
 int bf_resident_timers_download(bf_ctx* ctx, uint32_t handle, uint32_t first_run, uint32_t n_runs, void* slots);
 
+/* ------------------------------------------------------------------ resident limiters (the schedule of resident batches)
+ * bf_schedule uploads one bf_sched_run per run and downloads one schedule record per run on every call, and limits one batch
+ * against bases the host supplies.  A resident batch may instead keep its limiter inputs on the device, and one call limits
+ * several resident batches of the ctx (width classes) against ONE set of totals and lists only the runs whose schedule changed.
+ * The inputs are kept in a side area of one bf_sched_run-sized record per run, like the timer slots: bf_layout and the state
+ * records do not change, and a batch that never calls bf_resident_sched launches nothing more than before for any call.
+ *
+ * bf_resident_sched(handle): creates the area, every run at the defaults: both keys BF_SCHED_NONE, priority 0, queued_since
+ *   BF_SCHED_NONE, run_phase 0 (counted in no story or queue total; only the global limit applies).  Again on a batch that has
+ *   one: BF_OK, nothing changes.  bf_resident_destroy frees it.
+ * bf_resident_sched_put(handle, req, n) (host buffer, synchronous): writes the inputs of each req[i].run.  Checked before
+ *   anything changes, else BF_EINVAL and nothing changed: the area exists; run < capacity; reserved fields 0; at most one
+ *   request per run.  A put touches no run and changes no state record, so it neither needs nor ends a tick.
+ * bf_resident_sched_download(handle, first_run, n_runs, out): the stored inputs (out[i].run = first_run + i), for tests and resyncs.
+ *
+ * Time: queued_since is the origin of the run's queueing on the same u32 clock as `now` (the step timers' clock, suggested: seconds
+ *   since the batcher's epoch).  The device derives queued_elapsed_s of bf_sched_run as: BF_SCHED_NONE when queued_since is
+ *   BF_SCHED_NONE, else now - queued_since when now > queued_since, else 0 (Go's `elapsed <= 0` keeps the base priority).  The
+ *   difference is taken in whole clock units: a host that wants Go's truncation of sub-second differences picks a clock of that
+ *   resolution.  The clamp at INT32_MAX and the wrapping int32 sum of the limiter block apply as for bf_schedule.  So aging
+ *   advances with `now` alone, and a host puts a run only when its keys, priority, StoryRun phase or queue origin change.
+ *
+ * bf_resident_schedule(tables, now, parts, n_parts, totals): one schedule over the resident batches parts[i].handle.
+ *   Totals: the table bases, plus the Running StepRuns and the queue priority maxima of every run [0, n_runs) of every part, under
+ *   the count rules of the limiter block.  Each run is then limited against these shared totals: its record is bit for bit what
+ *   bf_schedule gives that run for a batch whose bf_sched_run records are the stored inputs (elapsed derived as above) and whose
+ *   bases are the tables' plus the other parts' contributions (Running counts added, queue priority maxima by maximum).
+ *   totals->story_running, queue_running, queue_max_priority, global_running (host arrays, each may be NULL) receive the totals;
+ *   totals->records is not used.
+ *   Listing: each batch keeps the records of its last schedule on the device.  A run is listed when its new record differs from
+ *   the one the batch's previous schedule gave that index, or when there is no such record: the batch's first schedule, runs at or
+ *   above the previous schedule's n_runs, runs uploaded, migrated, moved by retire or transfer, or received by transfer since, and
+ *   every run after a reshape or narrow changed `words`.  full = 1 when every run of [0, n_runs) was listed.  A listed run's head
+ *   is its record's bf_sched_header, and its events are the steps of its launch, queued_story and queued_sched masks, one
+ *   (step | kind << 10) per step, kind BF_SEVT_*, run-major and step-ascending.  runs / heads / events receive the first
+ *   runs_cap / runs_cap / events_cap entries; n_listed and n_events are the true counts.  Pinned buffers are written by the
+ *   kernels in place; any other gets the entries copied after the synchronisation.
+ *   Checked before anything is written, else BF_EINVAL and nothing changed (inputs, state records, schedule records): the struct
+ *   sizes and tables (as bf_schedule); now != BF_SCHED_NONE; each handle live, listed once, with an inputs area; n_runs <=
+ *   capacity; null runs / heads / events with a non-zero cap; and a tick of any kind over at least n_runs ran on the batch since
+ *   the last call that changed its state records (apply, upload, migrate, redrive, retire, transfer, reshape, narrow, a tick's
+ *   deltas, a fire that wrote a code); bf_last_error names the batch.  The call changes no state record and leaves bf_schedule's
+ *   snapshot as it was.  The slot table is read as it stands at the call.  Launches: one for the totals' start, then four per
+ *   part (count, limit and compare, scan of the per-CTA counts, list), one synchronisation.
+ *
+ * What the other calls do to the area (each launches nothing more when the batch has none): upload, migrate, redrive: nothing
+ *   (the inputs are per run, not per step).  retire: moved runs carry their inputs; retired and vacated indices return to the
+ *   defaults; a new capacity re-allocates the area.  transfer: the inputs arrive with their runs (the defaults from a source
+ *   without an area); a destination without an area refuses a source that has one (BF_EINVAL, both batches byte-identical).
+ *   reshape: a larger capacity extends the area with defaults.  narrow: keeps the area.                                     */
+typedef struct bf_sched_put {   /* 32 B                                                                                    */
+  uint32_t run;
+  uint32_t story_key, queue_key;  /* as bf_sched_run; BF_SCHED_NONE (or any key past the tables) = none                    */
+  int32_t priority;
+  uint32_t queued_since;          /* clock of `now`; BF_SCHED_NONE = no queued step with a StartedAt                          */
+  uint32_t run_phase;             /* BF_PHASE_* of StoryRun.Status.Phase                                                      */
+  uint32_t reserved[2];           /* 0                                                                                        */
+} bf_sched_put;
+
+#define BF_SEVT_LAUNCH 0x1u         /* in launch: hand to StepExecutor.Execute                                               */
+#define BF_SEVT_QUEUED_STORY 0x2u   /* in queued_story                                                                       */
+#define BF_SEVT_QUEUED_SCHED 0x4u   /* in queued_sched                                                                       */
+
+typedef struct bf_resident_sched_part {
+  uint32_t struct_size;         /* sizeof(bf_resident_sched_part)                                                          */
+  uint32_t handle;
+  uint32_t n_runs;              /* runs [0, n_runs) of the batch are counted and limited                                   */
+  uint32_t runs_cap;
+  uint32_t* runs;               /* [runs_cap] out: ascending indices of the listed runs                                    */
+  bf_sched_header* heads;       /* [runs_cap] out: the schedule header of runs[i]                                          */
+  uint16_t* events;             /* [events_cap] out: step | kind << 10, run-major, step-ascending                          */
+  uint64_t events_cap;
+  uint32_t n_listed;            /* out: listed runs (the true count, also past runs_cap)                                   */
+  uint32_t full;                /* out: 1 when every run of [0, n_runs) was listed                                          */
+  uint64_t n_events;            /* out: events of the listed runs (the true count, also past events_cap)                   */
+} bf_resident_sched_part;
+
+int bf_resident_sched(bf_ctx* ctx, uint32_t handle);
+int bf_resident_sched_put(bf_ctx* ctx, uint32_t handle, const bf_sched_put* requests, uint32_t n);
+int bf_resident_sched_download(bf_ctx* ctx, uint32_t handle, uint32_t first_run, uint32_t n_runs, bf_sched_put* out);
+int bf_resident_schedule(bf_ctx* ctx, const bf_sched_tables* tables, uint32_t now, bf_resident_sched_part* parts, uint32_t n_parts,
+                         bf_sched_out* totals);
+
 /* ------------------------------------------------------------------ device groups (SURVEY.md row e)
  * The reference is ONE operator process (cmd/main.go:220, StoryRunReconciler storyrun_controller.go:216), so the
  * multi-GPU path must be reachable from one process through this ABI: a group owns one ctx per device and an NCCL
