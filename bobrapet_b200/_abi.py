@@ -184,6 +184,10 @@ class ResidentSchedPart(C.Structure):
                 ("n_listed", C.c_uint32), ("full", C.c_uint32), ("n_events", C.c_uint64)]
 
 
+STOP_NONE, STOP_TIMEOUT, STOP_CANCEL, STOP_HOST = 0, 1, 2, 3   # BF_STOP_*: why a run of a resident batch is stopped
+FIRED_DRAIN, FIRED_STORY = 0xFFFE, 0xFFFF                       # bf_fired.step of a drain deadline / a story timeout
+
+
 def sched_stride(words: int) -> int:
     return (16 + 12 * words + 15) & ~15
 
@@ -233,6 +237,9 @@ SYMBOLS = [
     ("bf_resident_sched_download", C.c_int, [C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32, C.c_void_p]),
     ("bf_resident_schedule", C.c_int, [C.c_void_p, C.POINTER(SchedTables), C.c_uint32, C.POINTER(ResidentSchedPart), C.c_uint32,
                                        C.POINTER(SchedOut)]),
+    ("bf_resident_runctl", C.c_int, [C.c_void_p, C.c_uint32]),
+    ("bf_resident_runctl_put", C.c_int, [C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32]),
+    ("bf_resident_runctl_download", C.c_int, [C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32, C.c_void_p]),
     ("bf_group_create", C.c_int, [C.POINTER(C.c_void_p), C.POINTER(C.c_int32), C.c_uint32, C.POINTER(Config)]),
     ("bf_group_destroy", None, [C.c_void_p]),
     ("bf_group_size", C.c_uint32, [C.c_void_p]),

@@ -45,6 +45,8 @@ cudaError_t launch_fire(const FireParams& P, cudaStream_t stream);
 cudaError_t launch_schedule(const SchedParams& P, uint32_t sm_count, cudaStream_t stream, uint32_t phases = kSchedTotals | kSchedApply);
 cudaError_t launch_resident_schedule(const ResSchedParams& R, cudaStream_t stream);
 cudaError_t launch_sched_put(const SchedPutParams& P, cudaStream_t stream);
+cudaError_t launch_runctl_put(const RunCtlPutParams& P, cudaStream_t stream);
+cudaError_t launch_runctl_restop(const RunCtlRestopParams& P, cudaStream_t stream);
 cudaError_t launch_closure(const Slot* slots, const uint32_t* slot_ids, const uint32_t* starts, uint32_t n, uint32_t n_slots,
                            uint32_t words_out, uint32_t* masks, cudaStream_t stream);
 cudaError_t launch_validate(const Slot* slots, const uint32_t* slot_ids, uint32_t n, uint32_t n_slots, uint32_t* status,
@@ -204,6 +206,8 @@ struct bf_ctx {
   // resident schedules (bf_resident_schedule): tables | totals | per part: run events, CTA sums, the two totals, staged lists;
   // puts (bf_resident_sched_put): the requests
   DevBuf<uint8_t> d_rsched;
+  // run-control puts (bf_resident_runctl_put): the requests
+  DevBuf<bf_run_ctl_put> d_runctl_put;
   // step timers: arms ([0, 16) the overflow word | group starts | arming prefix | sorted requests) and fires ([0, 16) the four
   // output words | per-CTA fired counts | the fired list)
   DevBuf<uint8_t> d_timer;
@@ -286,6 +290,9 @@ inline int cuda_fail(bf_ctx* c, cudaError_t e, const char* what) {
 //   sched_base_runs    of the last bf_resident_schedule, cap * BF_SCHED_STRIDE(L.words) bytes; a run at or above sched_base_runs,
 //                      or whose stored reason is kSchedNoBase (uploads, migrations, moves, arrivals), has no baseline.  A change of
 //                      words zeroes sched_base_runs.
+//   d_runctl           the run-control records (bf_resident_runctl): cap records, or none.  Put and fire change them (a stop also
+//                      rewrites the run's flags byte); deltas, uploads and redrives honour them; retire and transfer move them with
+//                      their runs; reshape and a retire to a new capacity re-allocate them; narrow and migrate leave them.
 //   ticked             runs covered by a tick since the last call that changed d_state (state_changed), or -1: none since.  A
 //                      resident schedule over n runs needs ticked >= n.
 // A call that changes d_state ends the evaluated snapshot (end_snapshot): bf_schedule must follow a new pass.
@@ -300,6 +307,7 @@ struct Resident {
   DevBuf<bf_sched_run> d_sched_in;
   DevBuf<uint8_t> d_sched_rec;
   uint32_t sched_base_runs = 0;
+  DevBuf<bf_run_ctl> d_runctl;
   int64_t ticked = -1;
   uint64_t slot_changes_seen = 0, pending = 0;
   std::map<uint32_t, uint32_t> uploaded;

@@ -218,6 +218,7 @@ struct DeltaParams {
   uint32_t* rejected;  // count of deltas outside the record (bad run / index / absent field)
   uint32_t* mark;      // [n_runs] touch marks (Resident in ctx.h, touched ticks): every delta of a run in range raises its mark to mark_value
   uint32_t mark_value;
+  bf_run_ctl* runctl;  // [n_runs] run-control records, or nullptr: no area (a RUN_FLAGS delta of a stopped run goes to saved_flags)
 };
 
 // bf_resident_migrate (resident.cu): the records of the runs on old_slot are re-indexed in place to new_slot's step indices
@@ -258,6 +259,7 @@ struct RedriveParams {
   uint32_t words, state_stride, off_phase, off_cond, off_decision, off_child;
   unsigned long long* timers;    // [capacity][timer_k] timer slots, or nullptr: an applied request empties its run's
   uint32_t timer_k;
+  bf_run_ctl* runctl;            // [capacity] run-control records, or nullptr: an applied request lifts its run's stop
 };
 
 // bf_resident_reshape (resident.cu): both record arrays re-laid from layout `from` into new buffers at layout `to`
@@ -270,6 +272,8 @@ struct ReshapeParams {
   bf_layout from, to;
   const bf_sched_run* old_sched_in;   // the limiter inputs, or nullptr: no area (runs r >= n_old get kSchedDefault)
   bf_sched_run* sched_in;             // [n_new]
+  const bf_run_ctl* old_runctl;       // run-control records, or nullptr: no area (runs r >= n_old get kRunCtlDefault)
+  bf_run_ctl* runctl;                 // [n_new]
 };
 
 // bf_resident_retire (resident.cu): the runs [m, m + n) vacate their indices; the live ones among them move below m
@@ -287,6 +291,7 @@ struct RetireParams {
   bf_sched_run* sched_in;        // [capacity] limiter inputs, or nullptr: a mover's move with it, vacated ones get kSchedDefault
   uint8_t* sched_rec;            // [capacity][sched_stride] last schedule records: a mover's target loses its baseline
   uint32_t sched_stride;
+  bf_run_ctl* runctl;            // [capacity] run-control records, or nullptr: a mover's move with it, vacated ones get kRunCtlDefault
 };
 
 // bf_resident_extent / _narrow (resident.cu): the smallest layout a batch's records and the topologies of its runs allow.  Each
@@ -336,6 +341,8 @@ struct TransferParams {
   bf_sched_run* dst_sched_in;             // or nullptr: the destination has no area (then neither has the source)
   uint8_t* dst_sched_rec;                 // [dst capacity][dst_sched_stride]: an arrival has no baseline
   uint32_t dst_sched_stride;
+  const bf_run_ctl* src_runctl;           // run-control records, or nullptr (an arrival gets kRunCtlDefault)
+  bf_run_ctl* dst_runctl;                 // or nullptr: a run whose record is not the default is unfit (extent.w bit 31)
 };
 
 // step timers (resident.cu): slot = deadline | step << 32 | code << 48 (bf_timer_slot read as one little-endian u64); an empty
@@ -378,6 +385,8 @@ struct FireParams {
   uint32_t* out;                   // [4] n_fired, n_written, n_pruned, next_deadline (fire_count initialises them)
   bf_fired* fired;                 // [fired_cap]
   uint32_t fired_cap;
+  bf_run_ctl* runctl;              // [n_runs] run-control records, or nullptr: no story or drain deadlines (timers must be set)
+  bf_sched_run* sched_in;          // limiter inputs, or nullptr: a story timeout sets its run's run_phase to BF_PHASE_TIMEOUT
 };
 
 // limiters.cu (rows a9 / f4)
@@ -429,6 +438,38 @@ struct ResSchedParams {
   unsigned long long events_cap;
 };
 constexpr uint32_t kSchedUnlisted = 0xFFFFFFFFu;
+
+// run control (resident.cu): the record of a run never put, and the run_flags byte of a stopped run
+constexpr bf_run_ctl kRunCtlDefault = {0xFFFFFFFFu, 0xFFFFFFFFu, 0u, 0u, {0u, 0u, 0u, 0u, 0u, 0u}};
+constexpr uint32_t kStoppedFlags = BF_RF_HOST_GROUP | (uint32_t)BF_GROUP_DONE << BF_RF_HOST_GROUP_SHIFT;
+
+// What a stop needs besides the record and its run-control record: the batch's timer slots (emptied), its limiter inputs (a
+// timeout's run_phase), its touch marks (touched as by a delta).  Each may be nullptr but mark.
+struct StopParams {
+  unsigned long long* timers;
+  uint32_t timer_k;
+  bf_sched_run* sched_in;
+  uint32_t* mark;
+  uint32_t mark_value;
+};
+
+// bf_resident_runctl_put: req[i] is written into area[req[i].run], and a request with a stop stops its run (record r of state)
+struct RunCtlPutParams {
+  bf_run_ctl* area;
+  const bf_run_ctl_put* req;
+  uint32_t n;
+  uint8_t* state;
+  uint32_t state_stride;
+  StopParams stop;
+};
+
+// bf_resident_upload of a batch with run control: every stopped run of [first, first + n) saves its uploaded flags byte and is
+// stopped again
+struct RunCtlRestopParams {
+  bf_run_ctl* area;
+  uint8_t* state;
+  uint32_t state_stride, first, n;
+};
 
 // bf_resident_sched_put: req[i] is written into area[req[i].run]
 struct SchedPutParams {

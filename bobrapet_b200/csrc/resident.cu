@@ -24,6 +24,61 @@ DI void set_byte(uint8_t* rec, uint32_t byte_off, uint32_t mask, uint32_t value)
   atomicOr(w, value << sh);
 }
 
+// ---- run control (bf_resident_runctl*): stops and run-level deadlines --------------------------------------------------------
+DI bool runctl_default(const bf_run_ctl& c) {
+  const uint4 v = *reinterpret_cast<const uint4*>(&c);
+  return v.x == BF_TIMER_NONE && v.y == BF_TIMER_NONE && v.z == 0u && v.w == 0u;
+}
+DI bool deadline_due(uint32_t d, uint32_t now) { return d != BF_TIMER_NONE && d <= now; }
+
+// Stops run `run` (record rec, run-control record ctl) for `reason`, unless it is stopped already: saves its flags byte, writes
+// the stopped byte, empties its step-timer slots, marks the run touched and, for a timeout, sets its limiter inputs' run_phase.
+// The caller is the only thread writing this run's records in its launch.  -> 1 when the run was stopped now
+DI uint32_t stop_run(uint8_t* rec, bf_run_ctl* ctl, uint32_t run, uint32_t reason, const StopParams& S) {
+  if (ctl->stop) return 0u;
+  ctl->saved_flags = rec[4];
+  ctl->stop = (uint8_t)reason;
+  set_byte(rec, 4u, 0xFFu, kStoppedFlags);
+  for (uint32_t k = 0; S.timers && k < S.timer_k; ++k) S.timers[(size_t)run * S.timer_k + k] = kTimerEmpty;
+  if (reason == BF_STOP_TIMEOUT && S.sched_in) S.sched_in[run].run_phase = BF_PHASE_TIMEOUT;
+  atomicMax(S.mark + run, S.mark_value);   // max: an upload's "must list" bit stays
+  return 1u;
+}
+
+// Put: one thread per request (one request per run).  Deadlines are stored, then the stop applies.
+__global__ void __launch_bounds__(256) runctl_put(const RunCtlPutParams P) {
+  const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= P.n) return;
+  const bf_run_ctl_put q = P.req[i];
+  bf_run_ctl* ctl = P.area + q.run;
+  ctl->story_deadline = q.story_deadline;
+  ctl->drain_deadline = q.drain_deadline;
+  if (q.stop) stop_run(P.state + (size_t)q.run * P.state_stride, ctl, q.run, q.stop, P.stop);
+}
+
+cudaError_t launch_runctl_put(const RunCtlPutParams& P, cudaStream_t stream) {
+  if (P.n == 0) return cudaSuccess;
+  runctl_put<<<(P.n + 255) / 256, 256, 0, stream>>>(P);
+  return cudaGetLastError();
+}
+
+// After an upload: one thread per uploaded run; a stopped one keeps the uploaded byte as its saved flags and is stopped again.
+__global__ void __launch_bounds__(256) runctl_restop(const RunCtlRestopParams P) {
+  const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= P.n) return;
+  bf_run_ctl* ctl = P.area + P.first + i;
+  if (!ctl->stop) return;
+  uint8_t* rec = P.state + (size_t)(P.first + i) * P.state_stride;
+  ctl->saved_flags = rec[4];
+  set_byte(rec, 4u, 0xFFu, kStoppedFlags);
+}
+
+cudaError_t launch_runctl_restop(const RunCtlRestopParams& P, cudaStream_t stream) {
+  if (P.n == 0) return cudaSuccess;
+  runctl_restop<<<(P.n + 255) / 256, 256, 0, stream>>>(P);
+  return cudaGetLastError();
+}
+
 __global__ void __launch_bounds__(256) apply_deltas(const DeltaParams P) {
   const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= P.n) return;
@@ -49,8 +104,9 @@ __global__ void __launch_bounds__(256) apply_deltas(const DeltaParams P) {
       ok = P.off_child != BF_OFF_NONE && d.index < P.child_nibbles && d.code < 15u;
       if (ok) set_byte(rec, P.off_child + (d.index >> 1), 0xFu << ((d.index & 1u) * 4u), (uint32_t)d.code << ((d.index & 1u) * 4u));
       break;
-    case BF_DELTA_RUN_FLAGS:
-      set_byte(rec, 4u, 0xFFu, d.code);
+    case BF_DELTA_RUN_FLAGS:   // a stopped run keeps its stop: the byte is what a redrive restores
+      if (P.runctl && P.runctl[d.run].stop) set_byte(reinterpret_cast<uint8_t*>(P.runctl + d.run), 9u, 0xFFu, d.code);
+      else set_byte(rec, 4u, 0xFFu, d.code);
       break;
     case BF_DELTA_REGISTERED: {
       ok = d.index < BF_MAX_PARALLEL;
@@ -299,6 +355,13 @@ __global__ void __launch_bounds__(256) redrive_runs(const RedriveParams P) {
   if (lane == 0) {
     const unsigned long long gone = (unsigned long long)reg[1] << 32 | reg[0];
     if (gone) atomicAnd(reinterpret_cast<unsigned long long*>(rec + 8), ~gone);
+    if (P.runctl) {   // the stop goes (one exchange: of two requests of a run, one restores), the drain deadline too
+      bf_run_ctl* ctl = P.runctl + q.run;
+      const uint32_t was = atomicExch(reinterpret_cast<uint32_t*>(ctl) + 2, 0u);   // stop | saved_flags << 8
+      if (was & 0xFFu) set_byte(rec, 4u, 0xFFu, (was >> 8) & 0xFFu);
+      ctl->drain_deadline = BF_TIMER_NONE;
+      if (key == BF_REDRIVE_ALL) ctl->story_deadline = BF_TIMER_NONE;   // StartedAt = nil (storyrun_controller.go:414-438)
+    }
     atomicAnd(reinterpret_cast<uint32_t*>(rec + 4), ~(uint32_t)BF_RF_TOPOLOGY_TERMINATED);   // run_flags is the low byte
     atomicMax(P.mark + q.run, P.mark_value);   // max: an upload's "must list" bit stays
   }
@@ -363,6 +426,7 @@ __global__ void __launch_bounds__(256) reshape_runs(const ReshapeParams P) {
   d = reinterpret_cast<uint32_t*>(P.result + (size_t)r * P.to.result_stride);
   for (uint32_t o = lane * 4u; o < P.to.result_stride; o += 128u) d[o >> 2] = keep ? reshape_result_word(s, o, P.from, P.to) : 0u;
   if (P.sched_in && lane == 0) P.sched_in[r] = keep ? P.old_sched_in[r] : kSchedDefault;
+  if (P.runctl && lane == 0) P.runctl[r] = keep ? P.old_runctl[r] : kRunCtlDefault;
 }
 
 cudaError_t launch_reshape(const ReshapeParams& P, cudaStream_t stream) {
@@ -396,6 +460,10 @@ __global__ void __launch_bounds__(256) retire_runs(const RetireParams P) {
       *reinterpret_cast<uint32_t*>(P.sched_rec + (size_t)to * P.sched_stride + 12) = kSchedNoBase;
     }
     P.sched_in[from] = kSchedDefault;
+  }
+  if (P.runctl && lane == 0) {
+    if (to != kRetireNoMove) P.runctl[to] = P.runctl[from];
+    P.runctl[from] = kRunCtlDefault;
   }
   if (P.timers) {   // each lane stores over only the slots it read itself
     unsigned long long* ts = P.timers + (size_t)from * P.timer_k;
@@ -575,8 +643,10 @@ __global__ void __launch_bounds__(256) transfer_fit(const TransferParams P) {
     const bf_layout& T = P.T;
     const uint32_t placed = (T.off_cond != BF_OFF_NONE ? BF_F_COND : 0u) | (T.off_decision != BF_OFF_NONE ? BF_F_DECISION : 0u) |
                             (T.off_child != BF_OFF_NONE ? BF_F_CHILD : 0u);
-    P.extent[i] = make_uint4(steps, child, fields, armed);
-    if (steps > T.steps_max || (T.off_child != BF_OFF_NONE && child > T.child_nibbles) || (fields & ~placed) || armed > P.dst_k)
+    const bool ctl_lost = P.src_runctl && !P.dst_runctl && !runctl_default(P.src_runctl[r]);   // no area to arrive in
+    P.extent[i] = make_uint4(steps, child, fields, armed | (ctl_lost ? 0x80000000u : 0u));
+    if (steps > T.steps_max || (T.off_child != BF_OFF_NONE && child > T.child_nibbles) || (fields & ~placed) || armed > P.dst_k ||
+        ctl_lost)
       atomicMin(P.unfit, i);
   }
 }
@@ -602,6 +672,7 @@ __global__ void __launch_bounds__(256) transfer_runs(const TransferParams P) {
   // the run's armed slots (at most dst_k, transfer_fit) lead the source's slots: copied in order, empty slots behind them
   for (uint32_t k = lane; P.dst_timers && k < P.dst_k; k += 32u)
     P.dst_timers[(size_t)to * P.dst_k + k] = P.src_timers && k < P.src_k ? P.src_timers[(size_t)r * P.src_k + k] : kTimerEmpty;
+  if (P.dst_runctl && lane == 0) P.dst_runctl[to] = P.src_runctl ? P.src_runctl[r] : kRunCtlDefault;
 }
 
 cudaError_t launch_transfer_fit(const TransferParams& P, cudaStream_t stream) {
@@ -717,11 +788,18 @@ DI uint32_t fire_kind(const FireParams& P, const uint8_t* rec, unsigned long lon
   if ((BF_LUT_TERMINAL >> get_planes(rec, P.off_phase, P.words, 4, timer_step(v))) & 1u) return 2u;
   return timer_deadline(v) <= P.now ? 1u : 0u;
 }
+// a run whose story timeout fires now: not stopped and its story deadline due
+DI bool story_fires(const FireParams& P, const bf_run_ctl& c) { return !c.stop && deadline_due(c.story_deadline, P.now); }
 DI uint32_t fired_of_run(const FireParams& P, uint32_t r) {
   if (r >= P.n_runs) return 0u;
+  uint32_t n = 0;
+  if (P.runctl) {   // run level: the drain deadline, and a story timeout, which stands for every step slot
+    const bf_run_ctl c = P.runctl[r];
+    n = deadline_due(c.drain_deadline, P.now) ? 1u : 0u;
+    if (story_fires(P, c)) return n + 1u;
+  }
   const uint8_t* rec = P.state + (size_t)r * P.state_stride;
   const unsigned long long* t = P.timers + (size_t)r * P.timer_k;
-  uint32_t n = 0;
   for (uint32_t k = 0; k < P.timer_k; ++k) {
     const unsigned long long v = t[k];
     if (!timer_armed(v)) break;   // armed slots lead
@@ -768,7 +846,22 @@ __global__ void __launch_bounds__(256) fire_apply(const FireParams P) {
   uint32_t pos = incl - mine;
   for (uint32_t w = 0; w < 8; ++w) pos += base_part[w] + (w < warp ? warp_incl[w] : 0u);
   uint32_t written = 0, pruned = 0, next = BF_TIMER_NONE, touched = 0;
-  if (r < P.n_runs) {
+  if (r < P.n_runs && P.runctl && story_fires(P, P.runctl[r])) {   // the story timeout: no step slot fires, each is pruned
+    uint8_t* rec = P.state + (size_t)r * P.state_stride;
+    bf_run_ctl* ctl = P.runctl + r;
+    for (uint32_t k = 0; k < P.timer_k && timer_armed(P.timers[(size_t)r * P.timer_k + k]); ++k) ++pruned;
+    const uint32_t drain = ctl->drain_deadline;
+    stop_run(rec, ctl, r, BF_STOP_TIMEOUT, StopParams{P.timers, P.timer_k, P.sched_in, P.mark, P.mark_value});
+    written = 1u;
+    if (deadline_due(drain, P.now)) {   // BF_FIRED_DRAIN < BF_FIRED_STORY: listed first
+      ctl->drain_deadline = BF_TIMER_NONE;
+      if (pos < P.fired_cap) P.fired[pos] = bf_fired{r, (uint16_t)BF_FIRED_DRAIN, (uint8_t)BF_DEC_PENDING, 0u};
+      ++pos;
+    } else if (drain != BF_TIMER_NONE) {
+      next = drain;
+    }
+    if (pos < P.fired_cap) P.fired[pos] = bf_fired{r, (uint16_t)BF_FIRED_STORY, (uint8_t)BF_DEC_TIMED_OUT, 1u};
+  } else if (r < P.n_runs) {
     uint8_t* rec = P.state + (size_t)r * P.state_stride;
     unsigned long long* t = P.timers + (size_t)r * P.timer_k;
     uint32_t keep = 0, k = 0;
@@ -791,6 +884,17 @@ __global__ void __launch_bounds__(256) fire_apply(const FireParams P) {
     }
     for (uint32_t e = keep; e < k; ++e) t[e] = kTimerEmpty;
     if (touched) atomicMax(P.mark + r, P.mark_value);   // max: an upload's "must list" bit stays
+    if (P.runctl) {   // after the steps (BF_FIRED_DRAIN sorts above every step); a stopped run's story deadline is dormant
+      bf_run_ctl* ctl = P.runctl + r;
+      const uint32_t drain = ctl->drain_deadline;
+      if (deadline_due(drain, P.now)) {
+        ctl->drain_deadline = BF_TIMER_NONE;
+        if (pos < P.fired_cap) P.fired[pos] = bf_fired{r, (uint16_t)BF_FIRED_DRAIN, (uint8_t)BF_DEC_PENDING, 0u};
+      } else {
+        next = min(next, drain);
+      }
+      if (!ctl->stop) next = min(next, ctl->story_deadline);
+    }
   }
   const uint32_t f = __reduce_add_sync(FULL, mine), wr = __reduce_add_sync(FULL, written), pr = __reduce_add_sync(FULL, pruned);
   next = __reduce_min_sync(FULL, next);

@@ -65,6 +65,10 @@ int bf_resident_upload(bf_ctx* c, uint32_t h, uint32_t first, uint32_t n, const 
     BF_CUDA(c, cudaMemset2DAsync(r->d_sched_rec + (size_t)first * r->sched_stride() + 12, r->sched_stride(), 0xFF, 4, n, c->stream));
   BF_CUDA(c, bf::launch_mark_runs(r->d_mark, first, n, r->mark_must_list(), c->stream));
   c->stats.kernel_launches += 1;
+  if (r->d_runctl) {   // stops persist: a stopped run's uploaded flags byte is its saved one
+    BF_CUDA(c, bf::launch_runctl_restop({r->d_runctl, r->d_state, r->L.state_stride, first, n}, c->stream));
+    c->stats.kernel_launches += 1;
+  }
   r->pending += n;
   r->note_uploaded(first, first + n);
   BF_CUDA(c, cudaStreamSynchronize(c->stream));
@@ -107,6 +111,7 @@ static int resident_apply_async(bf_ctx* c, Resident* r, const bf_delta* deltas, 
   P.off_decision = r->L.off_decision; P.off_child = r->L.off_child; P.child_nibbles = r->L.child_nibbles;
   P.rejected = c->d_rejected;
   P.mark = r->d_mark; P.mark_value = r->mark_touched();
+  P.runctl = r->d_runctl;
   BF_CUDA(c, bf::launch_apply_deltas(P, s));
   c->stats.kernel_launches += 1;
   return BF_OK;
@@ -441,7 +446,7 @@ int bf_resident_redrive(bf_ctx* c, uint32_t h, const bf_redrive* req, uint32_t n
   P.masks = d_mask; P.status = d; P.slots = c->slots_dev; P.n = n;
   P.words = L.words; P.state_stride = L.state_stride; P.off_phase = L.off_phase; P.off_cond = L.off_cond;
   P.off_decision = L.off_decision; P.off_child = L.off_child;
-  P.timers = r->d_timers; P.timer_k = r->timer_k;
+  P.timers = r->d_timers; P.timer_k = r->timer_k; P.runctl = r->d_runctl;
   std::vector<uint8_t> status(n);
   cudaStream_t s = c->stream;
   cudaError_t e = cudaMemcpyAsync(d + o_req, blob.data(), blob.size(), cudaMemcpyHostToDevice, s);
@@ -495,6 +500,9 @@ int bf_resident_reshape(bf_ctx* c, uint32_t h, const bf_layout* layout, uint32_t
   cudaStream_t s = c->stream;
   if (sched_grow)
     if (cudaError_t e = nb.d_sched_in.alloc(capacity)) return fail(c, BF_ENOMEM, std::string("resident reshape (limiter inputs): ") + cudaGetErrorString(e));
+  const bool runctl_grow = r->d_runctl && capacity > r->cap;   // defaults for the new runs, in the reshape launch
+  if (runctl_grow)
+    if (cudaError_t e = nb.d_runctl.alloc(capacity)) return fail(c, BF_ENOMEM, std::string("resident reshape (run control): ") + cudaGetErrorString(e));
   if (sched_relay)
     if (cudaError_t e = Resident::alloc_sched_rec(nb.d_sched_rec, capacity, T.words, s))
       return fail(c, BF_ENOMEM, std::string("resident reshape (schedule records): ") + cudaGetErrorString(e));
@@ -503,6 +511,7 @@ int bf_resident_reshape(bf_ctx* c, uint32_t h, const bf_layout* layout, uint32_t
   P.old_state = r->d_state; P.old_result = r->d_result; P.state = nb.d_state; P.result = nb.d_result;
   P.n_old = r->cap; P.n_new = capacity; P.from = F; P.to = T;
   if (sched_grow) { P.old_sched_in = r->d_sched_in; P.sched_in = nb.d_sched_in; }
+  if (runctl_grow) { P.old_runctl = r->d_runctl; P.runctl = nb.d_runctl; }
   cudaError_t e = bf::launch_reshape(P, s);
   if (e == cudaSuccess && sched_relay && T.words == F.words)
     e = cudaMemcpyAsync(nb.d_sched_rec, r->d_sched_rec, (size_t)r->cap * r->sched_stride(), cudaMemcpyDeviceToDevice, s);
@@ -518,6 +527,7 @@ int bf_resident_reshape(bf_ctx* c, uint32_t h, const bf_layout* layout, uint32_t
   r->state_changed(c);   // as after an upload
   if (timers_grow) r->d_timers = std::move(nb.d_timers);
   if (sched_grow) r->d_sched_in = std::move(nb.d_sched_in);
+  if (runctl_grow) r->d_runctl = std::move(nb.d_runctl);
   if (sched_relay) r->d_sched_rec = std::move(nb.d_sched_rec);
   if (T.words != F.words) r->sched_base_runs = 0;
   r->adopt(std::move(nb), T, capacity);
@@ -705,12 +715,15 @@ int bf_resident_retire(bf_ctx* c, uint32_t h, bf_retire* rt) {
     if (e == cudaSuccess) e = nb.d_sched_rec.alloc((size_t)cap * r->sched_stride());
     if (e != cudaSuccess) return fail(c, BF_ENOMEM, std::string("resident retire (limiter inputs): ") + cudaGetErrorString(e));
   }
+  if (resize && r->d_runctl)
+    if (cudaError_t e = nb.d_runctl.alloc(cap)) return fail(c, BF_ENOMEM, std::string("resident retire (run control): ") + cudaGetErrorString(e));
   r->state_changed(c);   // as after an upload
   bf::RetireParams P{};
   P.state = r->d_state; P.result = r->d_result; P.mark = r->d_mark; P.mark_value = r->mark_must_list();
   P.to = c->d_retire; P.m = m; P.n = n; P.state_stride = L.state_stride; P.result_stride = L.result_stride;
   P.timers = r->d_timers; P.timer_k = r->timer_k;
   P.sched_in = r->d_sched_in; P.sched_rec = r->d_sched_rec; P.sched_stride = r->sched_stride();
+  P.runctl = r->d_runctl;
   cudaStream_t s = c->stream;
   cudaError_t e = n ? cudaMemcpyAsync(c->d_retire, to.data(), (size_t)n * 4, cudaMemcpyHostToDevice, s) : cudaSuccess;
   if (e == cudaSuccess) e = bf::launch_retire(P, s);
@@ -723,11 +736,14 @@ int bf_resident_retire(bf_ctx* c, uint32_t h, bf_retire* rt) {
     if (e == cudaSuccess && sched) e = cudaMemcpyAsync(nb.d_sched_in, r->d_sched_in, (size_t)cap * sizeof(bf_sched_run), cudaMemcpyDeviceToDevice, s);
     if (e == cudaSuccess && sched)
       e = cudaMemcpyAsync(nb.d_sched_rec, r->d_sched_rec, (size_t)cap * r->sched_stride(), cudaMemcpyDeviceToDevice, s);
+    if (e == cudaSuccess && r->d_runctl)
+      e = cudaMemcpyAsync(nb.d_runctl, r->d_runctl, (size_t)cap * sizeof(bf_run_ctl), cudaMemcpyDeviceToDevice, s);
   }
   if (int rc = r->sync_in_place(c, e, "bf_resident_retire")) return rc;
   c->stats.kernel_launches += n ? 1 : 0;
   if (resize && r->timer_k) r->d_timers = std::move(nb.d_timers);
   if (resize && sched) { r->d_sched_in = std::move(nb.d_sched_in); r->d_sched_rec = std::move(nb.d_sched_rec); }
+  if (resize && r->d_runctl) r->d_runctl = std::move(nb.d_runctl);
   if (resize) r->adopt(std::move(nb), L, cap);
   r->compact_to(m, N, to);
   write_moves(to, m, rt->moves_from, rt->moves_to);
@@ -791,6 +807,7 @@ int bf_resident_transfer(bf_ctx* c, uint32_t hs, uint32_t hd, bf_transfer* t) {
   P.src_timers = src->d_timers; P.src_k = src->timer_k; P.dst_timers = dst->d_timers; P.dst_k = dst->timer_k;
   P.src_sched_in = src->d_sched_in; P.dst_sched_in = dst->d_sched_in; P.dst_sched_rec = dst->d_sched_rec;
   P.dst_sched_stride = dst->sched_stride();
+  P.src_runctl = src->d_runctl; P.dst_runctl = dst->d_runctl;
   cudaStream_t s = c->stream;
   BF_CUDA(c, cudaMemcpyAsync(c->d_transfer, blob.data(), blob.size(), cudaMemcpyHostToDevice, s));
   BF_CUDA(c, bf::launch_transfer_fit(P, s));
@@ -808,7 +825,8 @@ int bf_resident_transfer(bf_ctx* c, uint32_t hs, uint32_t hd, bf_transfer* t) {
     return fail(c, BF_EINVAL, "runs[" + std::to_string(unfit) + "] (run " + std::to_string(t->runs[unfit]) +
                                   ") does not fit the destination layout: it needs steps_max " + std::to_string(x[0]) +
                                   ", child_nibbles " + std::to_string(x[1]) + ", fields " + std::to_string(x[2]) + ", " +
-                                  std::to_string(x[3]) + " timer slot(s) of the destination's " + std::to_string(dst->timer_k));
+                                  std::to_string(x[3] & 0x7FFFFFFFu) + " timer slot(s) of the destination's " + std::to_string(dst->timer_k) +
+                                  ((x[3] >> 31) ? ", and a run-control area (bf_resident_runctl) for its stop or deadlines" : ""));
   }
   // every arrival's record is a changed-only baseline of the source: the destination's may reach over them
   bool src_baseline = src->prev_valid;
@@ -821,6 +839,7 @@ int bf_resident_transfer(bf_ctx* c, uint32_t hs, uint32_t hd, bf_transfer* t) {
   Q.state_stride = F.state_stride; Q.result_stride = F.result_stride;
   Q.timers = src->d_timers; Q.timer_k = src->timer_k;
   Q.sched_in = src->d_sched_in; Q.sched_rec = src->d_sched_rec; Q.sched_stride = src->sched_stride();
+  Q.runctl = src->d_runctl;
   cudaError_t e = bf::launch_transfer(P, s);
   if (e == cudaSuccess) e = bf::launch_retire(Q, s);   // behind the transfer on the stream: the sources are read first
   if (int rc = src->sync_in_place(c, e, "bf_resident_transfer")) { dst->records_unknown(); return rc; }
@@ -928,7 +947,7 @@ int bf_resident_fire(bf_ctx* c, uint32_t h, uint32_t now, bf_fire_out* out) {
   auto [g, r] = lock_resident(c, h);
   if (!out || out->struct_size != sizeof(bf_fire_out)) return fail(c, BF_EINVAL, "null bf_fire_out or bad struct_size");
   if (!r) return BF_EINVAL;
-  if (!r->timer_k) return fail(c, BF_EINVAL, "the batch has no timer area (bf_resident_timers)");
+  if (!r->timer_k && !r->d_runctl) return fail(c, BF_EINVAL, "the batch has neither a timer area (bf_resident_timers) nor run control (bf_resident_runctl)");
   const uint32_t N = out->n_runs;
   if (N > r->cap) return fail(c, BF_EINVAL, "n_runs exceeds the resident batch");
   if (out->fired_cap && !out->fired) return fail(c, BF_EINVAL, "null fired with a non-zero fired_cap");
@@ -937,8 +956,8 @@ int bf_resident_fire(bf_ctx* c, uint32_t h, uint32_t now, bf_fire_out* out) {
   if (N == 0) return BF_OK;
   BF_CUDA(c, cudaSetDevice(c->device));
   const uint32_t grid = (N - 1) / 256 + 1;
-  // the list is at most N * K long: a larger fired_cap stages no more than that
-  const uint32_t cap = (uint32_t)std::min<uint64_t>(out->fired_cap, (uint64_t)N * r->timer_k);
+  // the list is at most N * (K + 2) long (with run control: a drain and a story entry per run): a larger fired_cap stages no more
+  const uint32_t cap = (uint32_t)std::min<uint64_t>(out->fired_cap, (uint64_t)N * (r->timer_k + (r->d_runctl ? 2u : 0u)));
   bf_fired* posted = static_cast<bf_fired*>(bf::pinned_dev(out->fired));
   const size_t o_sums = 16, o_list = round_up_sz(o_sums + (size_t)grid * 4, 16), bytes = o_list + (posted ? 0 : (size_t)cap * 8);
   if (int rc = c->d_timer.ensure(c, bytes)) return rc;
@@ -951,6 +970,7 @@ int bf_resident_fire(bf_ctx* c, uint32_t h, uint32_t now, bf_fire_out* out) {
   P.block_sums = reinterpret_cast<uint32_t*>(c->d_timer + o_sums);
   P.fired = posted ? posted : reinterpret_cast<bf_fired*>(c->d_timer + o_list);
   P.fired_cap = cap;
+  P.runctl = r->d_runctl; P.sched_in = r->d_sched_in;
   cudaStream_t s = c->stream;
   uint32_t* words = c->pinned->fire;
   cudaError_t e = bf::launch_fire(P, s);
@@ -960,7 +980,7 @@ int bf_resident_fire(bf_ctx* c, uint32_t h, uint32_t now, bf_fire_out* out) {
   if (const uint32_t listed = std::min(words[0], cap); listed && !posted)
     BF_CUDA(c, cudaMemcpy(out->fired, P.fired, (size_t)listed * 8, cudaMemcpyDeviceToHost));
   out->n_fired = words[0]; out->n_written = words[1]; out->n_pruned = words[2]; out->next_deadline = words[3];
-  r->pending += out->n_written;   // the touched-list bound counts the written codes as it counts deltas
+  r->pending += out->n_written;   // the touched-list bound counts the written codes and the timeouts as it counts deltas
   if (out->n_written) r->ticked = -1;
   return BF_OK;
 }
@@ -1191,5 +1211,70 @@ int bf_resident_schedule(bf_ctx* c, const bf_sched_tables* t, uint32_t now, bf_r
     const uint64_t ne = std::min<uint64_t>(p.n_events, q.ecap);
     if (ne && !q.p_events) BF_CUDA(c, cudaMemcpy(p.events, d + q.events, (size_t)ne * 2, cudaMemcpyDeviceToHost));
   }
+  return BF_OK;
+}
+
+// ---- StoryRun stops and deadlines (resident.cu) -------------------------------------------------------------------------------
+// The area: every record at the default (deadlines BF_TIMER_NONE, the rest 0) by two memsets, one synchronisation.
+int bf_resident_runctl(bf_ctx* c, uint32_t h) {
+  auto [g, r] = lock_resident(c, h);
+  if (!r) return BF_EINVAL;
+  if (r->d_runctl) return BF_OK;
+  BF_CUDA(c, cudaSetDevice(c->device));
+  DevBuf<bf_run_ctl> area;
+  if (cudaError_t e = area.alloc(r->cap)) return fail(c, BF_ENOMEM, std::string("run control: ") + cudaGetErrorString(e));
+  cudaError_t e = cudaMemsetAsync(area, 0, (size_t)r->cap * sizeof(bf_run_ctl), c->stream);
+  if (e == cudaSuccess) e = cudaMemset2DAsync(area, sizeof(bf_run_ctl), 0xFF, 8, r->cap, c->stream);   // both deadlines
+  const cudaError_t es = cudaStreamSynchronize(c->stream);
+  if (e == cudaSuccess) e = es;
+  if (e != cudaSuccess) return cuda_fail(c, e, "bf_resident_runctl");
+  r->d_runctl = std::move(area);
+  return BF_OK;
+}
+
+// Puts: every request checked on the host first, then one H2D copy, one launch, one synchronisation.  A put with a stop changes
+// state records: it ends the snapshot and the schedule's tick, and its runs count towards the touched-list bound.
+int bf_resident_runctl_put(bf_ctx* c, uint32_t h, const bf_run_ctl_put* req, uint32_t n) {
+  auto [g, r] = lock_resident(c, h);
+  if (!r) return BF_EINVAL;
+  if (!r->d_runctl) return fail(c, BF_EINVAL, "the batch has no run-control area (bf_resident_runctl)");
+  if (n && !req) return fail(c, BF_EINVAL, "null requests");
+  std::vector<uint32_t> seen;   // request index + 1 per run named so far
+  uint32_t stops = 0;
+  for (uint32_t i = 0; i < n; ++i) {
+    const bf_run_ctl_put& q = req[i];
+    auto at = [i] { return "request " + std::to_string(i) + ": "; };
+    if (q.run >= r->cap) return fail(c, BF_EINVAL, at() + "run outside the resident batch");
+    if (q.stop > BF_STOP_HOST) return fail(c, BF_EINVAL, at() + "stop is not a BF_STOP_* code");
+    if (q.reserved[0] || q.reserved[1] || q.reserved[2]) return fail(c, BF_EINVAL, at() + "reserved fields must be 0");
+    if (seen.empty()) seen.assign(r->cap, 0u);
+    if (seen[q.run]) return fail(c, BF_EINVAL, "requests " + std::to_string(seen[q.run] - 1) + " and " + std::to_string(i) + " name the same run");
+    seen[q.run] = i + 1;
+    stops += q.stop ? 1u : 0u;
+  }
+  if (n == 0) return BF_OK;
+  BF_CUDA(c, cudaSetDevice(c->device));
+  if (int rc = c->d_runctl_put.ensure(c, n)) return rc;
+  if (stops) r->state_changed(c);   // as a delta
+  bf::RunCtlPutParams P{};
+  P.area = r->d_runctl; P.req = c->d_runctl_put; P.n = n; P.state = r->d_state; P.state_stride = r->L.state_stride;
+  P.stop = bf::StopParams{r->d_timers, r->timer_k, r->d_sched_in, r->d_mark, r->mark_touched()};
+  cudaError_t e = cudaMemcpyAsync(c->d_runctl_put, req, (size_t)n * sizeof(bf_run_ctl_put), cudaMemcpyHostToDevice, c->stream);
+  if (e == cudaSuccess) e = bf::launch_runctl_put(P, c->stream);
+  if (int rc = r->sync_in_place(c, e, "bf_resident_runctl_put")) return rc;
+  c->stats.kernel_launches += 1;
+  r->pending += stops;   // the touched-list bound counts the stopped runs as it counts deltas
+  return BF_OK;
+}
+
+int bf_resident_runctl_download(bf_ctx* c, uint32_t h, uint32_t first, uint32_t n, bf_run_ctl* out) {
+  auto [g, r] = lock_resident(c, h);
+  if (!r) return BF_EINVAL;
+  if (!r->d_runctl) return fail(c, BF_EINVAL, "the batch has no run-control area (bf_resident_runctl)");
+  if ((uint64_t)first + n > r->cap || (n && !out)) return fail(c, BF_EINVAL, "run range outside the resident batch");
+  if (n == 0) return BF_OK;
+  BF_CUDA(c, cudaSetDevice(c->device));
+  BF_CUDA(c, cudaMemcpyAsync(out, r->d_runctl + first, (size_t)n * sizeof(bf_run_ctl), cudaMemcpyDeviceToHost, c->stream));
+  BF_CUDA(c, cudaStreamSynchronize(c->stream));
   return BF_OK;
 }

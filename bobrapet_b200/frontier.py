@@ -333,6 +333,30 @@ class Frontier:
                     "bf_resident_timers_download")
         return out
 
+    # -- StoryRun stops and deadlines of a resident batch (bf_resident_runctl*; bf_resident_fire reports the deadlines)
+    RUNCTL_DTYPE = np.dtype([("story_deadline", "<u4"), ("drain_deadline", "<u4"), ("stop", "u1"), ("saved_flags", "u1"),
+                             ("reserved", "u1", (6,))])                                        # bf_run_ctl, 16 B
+    RUNCTL_PUT_DTYPE = np.dtype([("run", "<u4"), ("story_deadline", "<u4"), ("drain_deadline", "<u4"), ("stop", "u1"),
+                                 ("reserved", "u1", (3,))])                                    # bf_run_ctl_put, 16 B
+
+    def resident_runctl(self, handle: int):
+        """bf_resident_runctl: create the batch's run-control area, every run at the default (no deadline, not stopped)"""
+        self._check(self._lib.bf_resident_runctl(self._ctx, handle), "bf_resident_runctl")
+
+    def resident_runctl_put(self, handle: int, requests: np.ndarray):
+        """bf_resident_runctl_put: write both deadlines of each requests[i].run and stop it when stop != A.STOP_NONE
+        (RUNCTL_PUT_DTYPE, at most one per run)"""
+        rq = np.ascontiguousarray(requests, dtype=self.RUNCTL_PUT_DTYPE)
+        self._check(self._lib.bf_resident_runctl_put(self._ctx, handle, rq.ctypes.data if rq.shape[0] else None, rq.shape[0]),
+                    "bf_resident_runctl_put")
+
+    def resident_runctl_download(self, handle: int, first_run: int, n_runs: int) -> np.ndarray:
+        """bf_resident_runctl_download -> the records of runs [first_run, first_run + n_runs), RUNCTL_DTYPE"""
+        out = np.zeros(n_runs, dtype=self.RUNCTL_DTYPE)
+        self._check(self._lib.bf_resident_runctl_download(self._ctx, handle, first_run, n_runs, out.ctypes.data),
+                    "bf_resident_runctl_download")
+        return out
+
     # -- limiter inputs and schedules of resident batches (bf_resident_sched*, bf_resident_schedule)
     SCHED_PUT_DTYPE = np.dtype([("run", "<u4"), ("story_key", "<u4"), ("queue_key", "<u4"), ("priority", "<i4"),
                                 ("queued_since", "<u4"), ("run_phase", "<u4"), ("reserved", "<u4", (2,))])   # bf_sched_put, 32 B

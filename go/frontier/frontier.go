@@ -525,6 +525,54 @@ func (r *Resident) Fire(n, now uint32, fired []Fired) (FireResult, error) {
 		NextDeadline: uint32(counts[3]), Fired: fired[:counts[4]]}, r.c.err(rc)
 }
 
+// Run-level entries of a Fire: Step holds one of these instead of a step index.
+const (
+	FiredDrain = 0xFFFE // the graceful-cancel drain deadline is due: force-delete the run's StepRuns (wake-only)
+	FiredStory = 0xFFFF // the story timeout fired: the run is stopped; patch the StoryRun to Timeout and retire it when done
+)
+
+// IsStoryTimeout reports a story timeout (enforceStoryTimeout): the device stopped the run.
+func (f Fired) IsStoryTimeout() bool { return f.Step == FiredStory }
+
+// IsDrain reports a due graceful-cancel drain deadline (handleGracefulCancel's force-delete time); it wrote nothing.
+func (f Fired) IsDrain() bool { return f.Step == FiredDrain }
+
+// Why a run is stopped (BF_STOP_*).
+const (
+	StopNone    = 0
+	StopTimeout = 1 // policy.timeouts.story elapsed
+	StopCancel  = 2 // spec.cancelRequested
+	StopHost    = 3 // any other reason the host stops DAG evaluation
+)
+
+// RunCtl is one run-control request of PutRunCtl (bf_run_ctl_put, 16 bytes, no pointers): both deadlines on Fire's clock
+// (TimerNone: none) and a stop (StopNone: deadlines only).
+type RunCtl struct {
+	Run, StoryDeadline, DrainDeadline uint32
+	Stop                              uint8
+	reserved                          [3]uint8
+}
+
+// EnableRunCtl gives the batch its run-control area (bf_resident_runctl): stops and story / drain deadlines kept on the device.
+func (r *Resident) EnableRunCtl() error { return r.c.err(C.bf_resident_runctl(r.c.p, r.handle)) }
+
+// PutRunCtl writes the deadlines of chosen runs and stops those with a Stop (bf_resident_runctl_put): StartedAt +
+// timeouts.story when a run is first packed or its StartedAt is set; StopCancel with observedAt + gracefulShutdownTimeout on
+// cancelRequested.  A stopped run lists no ready step and no launch until a redrive.  At most one request per run; a refusal
+// changes nothing.  One request goes through the flat shim wrapper, several through one call.
+func (r *Resident) PutRunCtl(reqs []RunCtl) error {
+	if len(reqs) == 1 {
+		q := reqs[0]
+		return r.c.err(C.bfgo_resident_runctl_put1(r.c.p, r.handle, C.uint32_t(q.Run), C.uint32_t(q.StoryDeadline),
+			C.uint32_t(q.DrainDeadline), C.uint8_t(q.Stop)))
+	}
+	var rp *C.bf_run_ctl_put
+	if len(reqs) > 0 {
+		rp = (*C.bf_run_ctl_put)(unsafe.Pointer(&reqs[0]))
+	}
+	return r.c.err(C.bf_resident_runctl_put(r.c.p, r.handle, rp, C.uint32_t(len(reqs))))
+}
+
 // SchedPut is one limiter-input request of PutSched (bf_sched_put, 32 bytes, no pointers).  QueuedSince is the StartedAt of the
 // run's earliest queued step on the clock of ScheduleResident's now (SchedNone: nothing queued); the device ages from it.
 type SchedPut struct {

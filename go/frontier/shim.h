@@ -200,6 +200,16 @@ static inline int bfgo_resident_fire(bf_ctx* c, uint32_t handle, uint32_t n_runs
   return rc;
 }
 
+/* StoryRun stops and deadlines.  bf_resident_runctl is called directly; a put of one run's deadlines and stop is built here on
+ * the C stack (bf_resident_runctl_put takes any number: a batcher with many sends them through bf_resident_runctl_put itself). */
+static inline int bfgo_resident_runctl_put1(bf_ctx* c, uint32_t handle, uint32_t run, uint32_t story_deadline, uint32_t drain_deadline,
+                                            uint8_t stop) {
+  bf_run_ctl_put q;
+  memset(&q, 0, sizeof q);
+  q.run = run; q.story_deadline = story_deadline; q.drain_deadline = drain_deadline; q.stop = stop;
+  return bf_resident_runctl_put(c, handle, &q, 1);
+}
+
 static inline void bfgo_tables(bf_sched_tables* t, uint32_t n_stories, uint32_t n_queues, int32_t global_limit, uint32_t global_base,
                                const int32_t* story_limit, const uint32_t* story_base, const int32_t* queue_limit,
                                const int32_t* queue_aging_s, const uint32_t* queue_base, const int32_t* queue_max_priority_base) {

@@ -869,6 +869,7 @@ typedef struct bf_fire_out {
 
 int bf_resident_timers(bf_ctx* ctx, uint32_t handle, uint32_t slots_per_run);
 int bf_resident_timers_arm(bf_ctx* ctx, uint32_t handle, const bf_timer* requests, uint32_t n);
+/* bf_resident_fire needs a timer area or a run-control area (bf_resident_runctl, which adds the run-level entries).          */
 int bf_resident_fire(bf_ctx* ctx, uint32_t handle, uint32_t now, bf_fire_out* out);
 int bf_resident_timers_download(bf_ctx* ctx, uint32_t handle, uint32_t first_run, uint32_t n_runs, void* slots);
 
@@ -954,6 +955,79 @@ int bf_resident_sched_put(bf_ctx* ctx, uint32_t handle, const bf_sched_put* requ
 int bf_resident_sched_download(bf_ctx* ctx, uint32_t handle, uint32_t first_run, uint32_t n_runs, bf_sched_put* out);
 int bf_resident_schedule(bf_ctx* ctx, const bf_sched_tables* tables, uint32_t now, bf_resident_sched_part* parts, uint32_t n_parts,
                          bf_sched_out* totals);
+
+/* ------------------------------------------------------------------ StoryRun stops and deadlines (run control of a resident batch)
+ * Above the steps, the reference stops DAG-evaluating a StoryRun for three reasons: its story timeout (enforceStoryTimeout,
+ * dag.go:544-578, checked at the start of every iteration :393-398, before the gate / sleep / wait syncs :409-420: once
+ * now - Status.StartedAt >= policy.timeouts.story the run becomes Timeout), a graceful cancel (spec.cancelRequested returns from
+ * Reconcile before the DAG, storyrun_controller.go:279-280; handleGracefulCancel :1517-1578 force-deletes the StepRuns once
+ * !now.Before(observedAt + gracefulShutdownTimeout)) and a terminal phase (:281-287).  A resident batch keeps the stop and both
+ * deadlines itself, in a side area of one 16-byte record per run, so that its runs stop producing ready steps and launches on the
+ * device and bf_resident_fire reports the run-level deadlines with the step timers.  bf_layout, the record bytes and the pass
+ * do not change, and a batch that never calls bf_resident_runctl launches nothing more than before for any call.
+ * Time is the step timers' clock (a u32 the host chooses; `now` of bf_resident_fire).  A deadline is DUE iff it is not
+ * BF_TIMER_NONE and deadline <= now.
+ *
+ * Stop.  Stopping a run saves its run_flags byte in saved_flags and writes BF_RF_HOST_GROUP | BF_GROUP_DONE << BF_RF_HOST_GROUP_SHIFT
+ *   into the record: both frontier kernels evaluate such a run as "finalize on host" (BF_GROUP_DONE) with no candidates, so it
+ *   lists no ready step, no event and no launch.  The pass may still apply its stage G/H phase rewrites to the result record of a
+ *   host-group run (phase_out, BF_SUM_PHASE_CHANGED); the host ignores those for a stopped run.  A stop also empties the run's
+ *   step-timer slots (the reference never applies them again), touches the run as a delta does (the next touched tick evaluates
+ *   it and lists it when its result changed), ends the evaluated snapshot and the schedule's tick (bf_resident_schedule must follow
+ *   a new tick).  A BF_STOP_TIMEOUT stop also writes run_phase = BF_PHASE_TIMEOUT into the run's limiter inputs when the batch has
+ *   that area: the run makes no demand in priority ordering (storyRunHasDemand, dag.go:1981-1999), while its Running steps still
+ *   count in the totals (its StepRuns still exist).  A stopped run keeps its stop until a redrive: a put cannot clear it, and
+ *   stopping it again changes nothing (the first reason and the saved byte stay).
+ *
+ * bf_resident_runctl(handle): creates the area, every record at the default {BF_TIMER_NONE, BF_TIMER_NONE, BF_STOP_NONE, 0}.
+ *   Again on a batch that has one: BF_OK, nothing changes.  bf_resident_destroy frees it.
+ * bf_resident_runctl_put(handle, req, n) (host buffer, synchronous): writes both deadlines of each req[i].run; stop != BF_STOP_NONE
+ *   stops the run now.  Checked before anything changes, else BF_EINVAL and nothing changed: the area exists; run < capacity;
+ *   stop <= BF_STOP_HOST; reserved fields 0; at most one request per run.  A put that only changes deadlines touches no run.
+ * bf_resident_runctl_download(handle, first_run, n_runs, out): the raw records, for tests and resyncs.
+ * bf_resident_fire (step timers section) also runs on a batch with this area and no timer area.  For each run below n_runs:
+ *   1. not stopped and story_deadline due: the run is stopped with BF_STOP_TIMEOUT and listed as (run, BF_FIRED_STORY,
+ *      BF_DEC_TIMED_OUT, written = 1); its armed step slots are disarmed and counted in n_pruned, none listed or written (the
+ *      story timeout precedes the step syncs, dag.go:393-409);
+ *   2. otherwise its step slots fire as described there;
+ *   3. drain_deadline due: disarmed and listed as (run, BF_FIRED_DRAIN, BF_DEC_PENDING, written = 0), wake-only (the host's
+ *      force-delete).
+ *   The list stays ascending by run, then step; n_written counts the timeouts.  next_deadline is the minimum over the armed step
+ *   slots, the drain deadlines and the story deadlines of runs not stopped (a stopped run's story deadline is kept, dormant).
+ *
+ * What the other calls do to the area (each launches nothing more when the batch has none):
+ *   delta scatter: a BF_DELTA_RUN_FLAGS delta of a stopped run is written into saved_flags; the record keeps the stop.
+ *   upload: deadlines and stops persist; a stopped run's uploaded flags byte becomes saved_flags and the record is stopped again
+ *     (one more launch over the uploaded range), so a resync from a host mirror that knows nothing of stops keeps them.
+ *   redrive (both kinds, runs with status_out = 1): a stopped run's record gets saved_flags without BF_RF_TOPOLOGY_TERMINATED and
+ *     the stop is cleared; the drain deadline is disarmed; BF_REDRIVE_ALL also disarms the story deadline (resetStoryRunForRedrive
+ *     sets StartedAt = nil, storyrun_controller.go:414-438), a step redrive keeps it (resetStoryRunForStepRedrive keeps StartedAt:
+ *     a timed-out run redriven from a step times out again at the next fire, as in the reference).
+ *   retire: records move with their runs, retired and vacated indices get the default; a new capacity re-allocates the area.
+ *   transfer: records arrive with their runs (the default from a source without an area); a destination without an area refuses a
+ *     moved run whose record is not the default (BF_EINVAL, both batches byte-identical).
+ *   reshape: a larger capacity extends the area with defaults.  narrow: keeps the area; extent and the fit do not change (a stop
+ *     needs no width and no planes).  migrate: nothing.                                                                     */
+enum { BF_STOP_NONE = 0, BF_STOP_TIMEOUT = 1, BF_STOP_CANCEL = 2, BF_STOP_HOST = 3 };
+typedef struct bf_run_ctl {     /* 16 B; the default is {BF_TIMER_NONE, BF_TIMER_NONE, 0, 0, {0}}                           */
+  uint32_t story_deadline;      /* StartedAt + policy.timeouts.story on the timers' clock, BF_TIMER_NONE: none               */
+  uint32_t drain_deadline;      /* graceful-cancel force-delete time, wake-only, BF_TIMER_NONE: none                         */
+  uint8_t stop;                 /* BF_STOP_*                                                                                 */
+  uint8_t saved_flags;          /* the run's own run_flags byte while stopped, else 0                                        */
+  uint8_t reserved[6];
+} bf_run_ctl;
+typedef struct bf_run_ctl_put { /* 16 B                                                                                      */
+  uint32_t run;
+  uint32_t story_deadline, drain_deadline;   /* BF_TIMER_NONE: none                                                          */
+  uint8_t stop;                 /* BF_STOP_NONE: deadlines only; else stop the run now                                       */
+  uint8_t reserved[3];          /* 0                                                                                         */
+} bf_run_ctl_put;
+#define BF_FIRED_DRAIN 0xFFFEu  /* bf_fired.step of a drain deadline                                                         */
+#define BF_FIRED_STORY 0xFFFFu  /* bf_fired.step of a story timeout                                                          */
+
+int bf_resident_runctl(bf_ctx* ctx, uint32_t handle);
+int bf_resident_runctl_put(bf_ctx* ctx, uint32_t handle, const bf_run_ctl_put* requests, uint32_t n);
+int bf_resident_runctl_download(bf_ctx* ctx, uint32_t handle, uint32_t first_run, uint32_t n_runs, bf_run_ctl* out);
 
 /* ------------------------------------------------------------------ device groups (SURVEY.md row e)
  * The reference is ONE operator process (cmd/main.go:220, StoryRunReconciler storyrun_controller.go:216), so the
