@@ -188,6 +188,15 @@ STOP_NONE, STOP_TIMEOUT, STOP_CANCEL, STOP_HOST = 0, 1, 2, 3   # BF_STOP_*: why 
 FIRED_DRAIN, FIRED_STORY = 0xFFFE, 0xFFFF                       # bf_fired.step of a drain deadline / a story timeout
 
 
+COMMIT_HOLD, COMMIT_ERROR, COMMIT_PHASE = 1, 2, 3   # BF_COMMIT_*: bf_commit_entry.kind
+COMMIT_NONE = 0xFFFFFFFF                           # BF_COMMIT_NONE: bad_run / bad_step of a refusal of the whole call
+
+
+class CommitOut(C.Structure):
+    _fields_ = [(n, C.c_uint32) for n in ("struct_size", "n_runs_written", "n_skipped", "n_launched", "n_queued", "n_failed",
+                                          "bad_run", "bad_step")]
+
+
 def sched_stride(words: int) -> int:
     return (16 + 12 * words + 15) & ~15
 
@@ -240,6 +249,7 @@ SYMBOLS = [
     ("bf_resident_runctl", C.c_int, [C.c_void_p, C.c_uint32]),
     ("bf_resident_runctl_put", C.c_int, [C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32]),
     ("bf_resident_runctl_download", C.c_int, [C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32, C.c_void_p]),
+    ("bf_resident_commit", C.c_int, [C.c_void_p, C.c_uint32, C.c_uint32, C.c_void_p, C.c_uint32, C.POINTER(CommitOut)]),
     ("bf_group_create", C.c_int, [C.POINTER(C.c_void_p), C.POINTER(C.c_int32), C.c_uint32, C.POINTER(Config)]),
     ("bf_group_destroy", None, [C.c_void_p]),
     ("bf_group_size", C.c_uint32, [C.c_void_p]),

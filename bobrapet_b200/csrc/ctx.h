@@ -47,6 +47,7 @@ cudaError_t launch_resident_schedule(const ResSchedParams& R, cudaStream_t strea
 cudaError_t launch_sched_put(const SchedPutParams& P, cudaStream_t stream);
 cudaError_t launch_runctl_put(const RunCtlPutParams& P, cudaStream_t stream);
 cudaError_t launch_runctl_restop(const RunCtlRestopParams& P, cudaStream_t stream);
+cudaError_t launch_commit(const CommitParams& P, bool apply, cudaStream_t stream);
 cudaError_t launch_closure(const Slot* slots, const uint32_t* slot_ids, const uint32_t* starts, uint32_t n, uint32_t n_slots,
                            uint32_t words_out, uint32_t* masks, cudaStream_t stream);
 cudaError_t launch_validate(const Slot* slots, const uint32_t* slot_ids, uint32_t n, uint32_t n_slots, uint32_t* status,
@@ -173,6 +174,7 @@ struct bf_ctx {
     uint32_t word;         // a 4-byte device counter: rejected deltas where no compaction delivers them, migrated runs
     bf::ResultTail tail;   // written by a compaction's last kernel; a pass without one copies its counts into tail.counts
     uint32_t fire[4];      // bf_resident_fire: n_fired, n_written, n_pruned, next_deadline
+    uint32_t commit[8];    // bf_resident_commit: the offender key (two words), then the five counts
     bf_counts counts() const { return {tail.counts[0], tail.counts[1], tail.counts[2], tail.counts[3]}; }
   }* pinned = nullptr;
   DevBuf<bf_expansion> d_exp;
@@ -211,6 +213,8 @@ struct bf_ctx {
   // step timers: arms ([0, 16) the overflow word | group starts | arming prefix | sorted requests) and fires ([0, 16) the four
   // output words | per-CTA fired counts | the fired list)
   DevBuf<uint8_t> d_timer;
+  // tick commits (bf_resident_commit): [0, 8) the offender key | [8, 28) the five counts | the sorted entries
+  DevBuf<uint8_t> d_commit;
 
   // limiters (bf_schedule): the records the last pass evaluated (bf_eval's staging or a resident batch), read in place.  Cleared
   // (valid = false) when a pass starts or a call changes those records (end_snapshot); assigned whole once a pass went through.
@@ -295,6 +299,9 @@ inline int cuda_fail(bf_ctx* c, cudaError_t e, const char* what) {
 //                      their runs; reshape and a retire to a new capacity re-allocate them; narrow and migrate leave them.
 //   ticked             runs covered by a tick since the last call that changed d_state (state_changed), or -1: none since.  A
 //                      resident schedule over n runs needs ticked >= n.
+//   single_ticked      runs covered by single-pass ticks since the last tick with BF_EVAL_FIXPOINT, or -1.  scheduled: runs covered
+//                      by a bf_resident_schedule since the last tick, or -1.  A commit over n runs needs ticked, single_ticked and,
+//                      with a limiter area, scheduled >= n; a commit that writes changes d_state.
 // A call that changes d_state ends the evaluated snapshot (end_snapshot): bf_schedule must follow a new pass.
 struct Resident {
   bool alive = false, prev_valid = false, need_full = true;
@@ -308,7 +315,7 @@ struct Resident {
   DevBuf<uint8_t> d_sched_rec;
   uint32_t sched_base_runs = 0;
   DevBuf<bf_run_ctl> d_runctl;
-  int64_t ticked = -1;
+  int64_t ticked = -1, single_ticked = -1, scheduled = -1;
   uint64_t slot_changes_seen = 0, pending = 0;
   std::map<uint32_t, uint32_t> uploaded;
 
@@ -317,7 +324,11 @@ struct Resident {
   void end_snapshot(bf_ctx* c) const { if (c->snap.holds(d_state)) c->snap.valid = false; }
   // a call changes d_state: bf_schedule and bf_resident_schedule must both follow a new tick
   void state_changed(bf_ctx* c) { end_snapshot(c); ticked = -1; }
-  void tick_done(uint32_t n_runs) { ticked = std::max<int64_t>(ticked, n_runs); }
+  void tick_done(uint32_t n_runs, uint32_t flags) {
+    ticked = std::max<int64_t>(ticked, n_runs);
+    single_ticked = (flags & BF_EVAL_FIXPOINT) ? -1 : std::max<int64_t>(single_ticked, n_runs);
+    scheduled = -1;
+  }
   uint32_t sched_stride() const { return BF_SCHED_STRIDE(L.words); }
   // schedule records for `capacity` runs of `words` words, every run without a baseline (all bytes 0xFF: reason kSchedNoBase)
   static cudaError_t alloc_sched_rec(DevBuf<uint8_t>& rec, uint32_t capacity, uint32_t words, cudaStream_t s) {

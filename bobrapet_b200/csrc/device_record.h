@@ -471,6 +471,25 @@ struct RunCtlRestopParams {
   uint32_t state_stride, first, n;
 };
 
+// bf_resident_commit (resident.cu): commit_check over runs [0, n_runs) lowers *offender, then commit_apply writes the records.
+// Entries are sorted by (run, step).  The offender key is run << 32 | step << 8 | reason (kCommitNotLaunched, ...).
+enum : uint32_t { kCommitNotLaunched = 1, kCommitNotStop = 2, kCommitNoPhase = 3 };
+struct CommitParams {
+  uint8_t* state;
+  const uint8_t* result;         // the current result records
+  const uint8_t* sched_rec;      // [n_runs][sched_stride] the last schedule records, or nullptr: launched = ready, nothing queued
+  const Slot* slots;
+  uint32_t n_slots;
+  const bf_commit_entry* entries;   // [n_entries], ascending by (run, step)
+  uint32_t n_entries;
+  uint32_t n_runs;
+  uint32_t words, state_stride, off_phase, result_stride, off_ready, off_skip, off_fail, sched_stride;
+  uint32_t* mark;                // a written run's is raised to mark_value, as by a delta
+  uint32_t mark_value;
+  unsigned long long* offender;  // [1] commit_check: lowest key (atomicMin; ~0 from the caller)
+  uint32_t* counts;              // [5] commit_apply: runs written, skipped, launched, queued, failed (zeroed by the caller)
+};
+
 // bf_resident_sched_put: req[i] is written into area[req[i].run]
 struct SchedPutParams {
   bf_sched_run* area;

@@ -366,12 +366,7 @@ __global__ void __launch_bounds__(RB == 2 ? 768 : 512, RB == 1 ? 2 : 1) frontier
       if (rc.group == BF_GROUP_DONE) break;
       // ------------- launch effects (dag.go:1735-1775, step_executor.go:132-185) -------------
       const uint32_t o0 = p0, o1 = p1, o2 = p2, o3 = p3;
-      pset<BF_PHASE_SKIPPED>(it_skip, p0, p1, p2, p3);
-      const uint32_t none_or_q = ~(p0 | p1 | p2 | p3) | (~p0 & p1 & p2 & p3);  // code 0 or 14
-      pset<BF_PHASE_SUCCEEDED>(it_ready & T_COND, p0, p1, p2, p3);
-      pset<BF_PHASE_PAUSED>(it_ready & SYNC_T, p0, p1, p2, p3);
-      pset<BF_PHASE_RUNNING>(it_ready & T_PAR, p0, p1, p2, p3);
-      pset<BF_PHASE_RUNNING>(it_ready & ~T_COND & ~SYNC_T & ~T_PAR & ~T_STOP & none_or_q, p0, p1, p2, p3);
+      launch_effects(it_skip, it_ready, T_COND, SYNC_T, T_PAR, T_STOP, p0, p1, p2, p3);
       const uint32_t fl = redux_or(((it_ready | it_skip) != 0 ? 1u : 0u) | ((it_ready & T_STOP) != 0 ? 2u : 0u) |
                                    (((p0 ^ o0) | (p1 ^ o1) | (p2 ^ o2) | (p3 ^ o3)) != 0 ? 4u : 0u));
       marked = marked || (fl & 4u);

@@ -64,6 +64,19 @@ DI void pset(uint32_t m, uint32_t& p0, uint32_t& p1, uint32_t& p2, uint32_t& p3)
   p2 = (CODE & 4) ? (p2 | m) : (p2 & ~m);
   p3 = (CODE & 8) ? (p3 | m) : (p3 & ~m);
 }
+// Launch effects of Execute (dag.go:1735-1775, step_executor.go:132-185) on one word of codes: the skipped steps become Skipped,
+// launched condition steps Succeeded, sleep / wait / gate steps Paused, parallel steps Running, and the other launched steps but
+// stop steps Running when their code is 0 or 14.  The fixpoint applies them in registers between iterations; bf_resident_commit
+// writes them into the records.
+DI void launch_effects(uint32_t skip, uint32_t launched, uint32_t T_COND, uint32_t SYNC_T, uint32_t T_PAR, uint32_t T_STOP,
+                       uint32_t& p0, uint32_t& p1, uint32_t& p2, uint32_t& p3) {
+  pset<BF_PHASE_SKIPPED>(skip, p0, p1, p2, p3);
+  const uint32_t none_or_q = ~(p0 | p1 | p2 | p3) | (~p0 & p1 & p2 & p3);  // code 0 or 14
+  pset<BF_PHASE_SUCCEEDED>(launched & T_COND, p0, p1, p2, p3);
+  pset<BF_PHASE_PAUSED>(launched & SYNC_T, p0, p1, p2, p3);
+  pset<BF_PHASE_RUNNING>(launched & T_PAR, p0, p1, p2, p3);
+  pset<BF_PHASE_RUNNING>(launched & ~T_COND & ~SYNC_T & ~T_PAR & ~T_STOP & none_or_q, p0, p1, p2, p3);
+}
 DI uint32_t squeeze4(uint32_t x) {  // bits 0,4,..,28 -> low byte
   x = (x | (x >> 3)) & 0x03030303u;
   x = (x | (x >> 6)) & 0x000F000Fu;

@@ -914,4 +914,168 @@ cudaError_t launch_fire(const FireParams& P, cudaStream_t stream) {
   return cudaGetLastError();
 }
 
+// ---- tick commits (bf_resident_commit) --------------------------------------------------------------------------------------
+// One warp per run; lane w holds word w of the run's masks and codes (words <= 32).  Both launches read a run the same way: its
+// topology's step types, the masks of its current result record (and of its schedule record), and its entries [lo, hi), found by
+// a binary search every lane runs alike.  A run with no mask bit and no entry leaves at once.
+struct CommitRun {
+  const uint8_t* topo;          // nullptr: dead slot, or a topology wider than the layout (no masks)
+  uint32_t TW, VALID;
+  uint32_t launched, queued, skip, fail;
+  uint32_t T_COND, SYNC_T, T_PAR, T_STOP;
+  uint32_t lo, hi;
+};
+
+DI bool commit_run(const CommitParams& P, uint32_t r, uint32_t lane, CommitRun& c) {
+  const uint32_t slot = *reinterpret_cast<const uint32_t*>(P.state + (size_t)r * P.state_stride);
+  const Slot sl = slot < P.n_slots ? P.slots[slot] : Slot{};
+  const TopoHeader* th = reinterpret_cast<const TopoHeader*>(sl.addr);
+  c.topo = sl.addr && th->W <= P.words ? reinterpret_cast<const uint8_t*>(sl.addr) : nullptr;
+  c.TW = c.topo ? th->W : 0u;
+  c.VALID = c.launched = c.queued = c.skip = c.fail = 0u;
+  uint32_t t0 = 0u, t1 = 0u, t2 = 0u;
+  if (lane < c.TW) {
+    c.VALID = bmsk_clamp(0u, th->S - lane * 32u);
+    const uint32_t* pl = reinterpret_cast<const uint32_t*>(c.topo + th->off_planes) + lane;
+    t0 = pl[PL_T0 * c.TW]; t1 = pl[PL_T1 * c.TW]; t2 = pl[PL_T2 * c.TW];
+    const uint8_t* res = P.result + (size_t)r * P.result_stride;
+    const uint32_t ready = reinterpret_cast<const uint32_t*>(res + P.off_ready)[lane];
+    c.skip = reinterpret_cast<const uint32_t*>(res + P.off_skip)[lane];
+    if (P.off_fail != BF_OFF_NONE) c.fail = reinterpret_cast<const uint32_t*>(res + P.off_fail)[lane];
+    c.launched = ready;
+    if (P.sched_rec) {
+      const uint32_t* sr = reinterpret_cast<const uint32_t*>(P.sched_rec + (size_t)r * P.sched_stride + 16) + lane;
+      c.launched = sr[0];
+      c.queued = sr[P.words] | sr[2u * P.words];
+    }
+  }
+  c.T_COND = t0 & ~t1 & ~t2;
+  c.SYNC_T = t0 & (t1 | t2);
+  c.T_PAR = ~t0 & t1 & ~t2 & c.VALID;
+  c.T_STOP = ~t0 & ~t1 & t2 & c.VALID;
+  uint32_t a = 0u, b = P.n_entries;
+  while (a < b) { const uint32_t m = (a + b) >> 1; if (P.entries[m].run < r) a = m + 1u; else b = m; }
+  c.lo = a; b = P.n_entries;
+  while (a < b) { const uint32_t m = (a + b) >> 1; if (P.entries[m].run <= r) a = m + 1u; else b = m; }
+  c.hi = a;
+  return __any_sync(FULL, (c.launched | c.queued | c.skip | c.fail) != 0u) || c.lo != c.hi;
+}
+
+// The entries of a run: lane w collects the HOLD and PHASE bits of its word; err: the run has an ERROR entry.  With check, the
+// lowest offending entry's key (entries ascend by step) is returned, else ~0.
+DI unsigned long long commit_entries(const CommitParams& P, uint32_t r, uint32_t lane, const CommitRun& c, bool check,
+                                     uint32_t& hold, uint32_t& phased, bool& err) {
+  hold = phased = 0u; err = false;
+  unsigned long long bad = ~0ull;
+  for (uint32_t i = c.lo; i < c.hi; ++i) {   // warp-uniform trip count
+    const bf_commit_entry e = P.entries[i];
+    const uint32_t w = e.step >> 5, bit = 1u << (e.step & 31u);   // step < steps_max: w < words <= 32
+    if (lane == w) {
+      if (e.kind == BF_COMMIT_HOLD) hold |= bit;
+      if (e.kind == BF_COMMIT_PHASE) phased |= bit;
+    }
+    err = err || e.kind == BF_COMMIT_ERROR;
+    if (!check) continue;
+    const uint32_t lw = __shfl_sync(FULL, c.launched, w), sw = __shfl_sync(FULL, c.T_STOP, w);
+    const uint32_t why = !(lw & bit) ? kCommitNotLaunched : (e.kind == BF_COMMIT_PHASE && !(sw & bit)) ? kCommitNotStop : 0u;
+    if (why && bad == ~0ull) bad = (unsigned long long)r << 32 | (unsigned long long)e.step << 8 | why;
+  }
+  return bad;
+}
+
+// Check: every entry names a launched step (a PHASE entry a stop step), and every launched stop step of a run without an ERROR
+// entry has a HOLD or PHASE entry.  Lane 0 lowers P.offender to the run's first offence.  Nothing is written.
+__global__ void __launch_bounds__(256) commit_check(const CommitParams P) {
+  const uint32_t r = blockIdx.x * 8u + (threadIdx.x >> 5), lane = threadIdx.x & 31u;
+  if (r >= P.n_runs) return;
+  CommitRun c;
+  if (!commit_run(P, r, lane, c)) return;
+  uint32_t hold, phased;
+  bool err;
+  unsigned long long bad = commit_entries(P, r, lane, c, true, hold, phased, err);
+  const uint32_t miss = err ? 0u : c.launched & c.T_STOP & ~hold & ~phased;
+  const uint32_t lanes = __ballot_sync(FULL, miss != 0u);
+  if (lanes) {
+    const uint32_t w = __ffs(lanes) - 1u;
+    const uint32_t step = w * 32u + __ffs(__shfl_sync(FULL, miss, w)) - 1u;
+    bad = min(bad, (unsigned long long)r << 32 | (unsigned long long)step << 8 | kCommitNoPhase);
+  }
+  if (lane == 0 && bad != ~0ull) atomicMin(P.offender, bad);
+}
+
+// Apply (after a check that found no offender): the writes of the contract on the codes as the pass reads them (code 15 as 0),
+// stored only where a code changed; lanes p and p + 32 set the registered bits of launched parallel descs.
+__global__ void __launch_bounds__(256) commit_apply(const CommitParams P) {
+  const uint32_t r = blockIdx.x * 8u + (threadIdx.x >> 5), lane = threadIdx.x & 31u;
+  if (r >= P.n_runs) return;
+  CommitRun c;
+  if (!commit_run(P, r, lane, c)) return;
+  uint32_t hold, phased;
+  bool err;
+  commit_entries(P, r, lane, c, false, hold, phased, err);
+  if (err) return;   // Execute failed: nothing of this reconcile is persisted
+  uint8_t* rec = P.state + (size_t)r * P.state_stride;
+  uint32_t* ph = reinterpret_cast<uint32_t*>(rec + P.off_phase) + lane;
+  uint32_t p[4] = {0u, 0u, 0u, 0u};
+  if (lane < c.TW)
+    for (uint32_t b = 0; b < 4; ++b) p[b] = ph[b * P.words];
+  const uint32_t keep = c.VALID & ~(p[0] & p[1] & p[2] & p[3]);
+  const uint32_t m0 = p[0] & keep, m1 = p[1] & keep, m2 = p[2] & keep, m3 = p[3] & keep;
+  uint32_t n0 = m0, n1 = m1, n2 = m2, n3 = m3;
+  const uint32_t SK = c.skip, FA = c.fail & ~SK, LA = c.launched & ~SK & ~FA & ~hold, QU = c.queued & ~SK & ~FA & ~c.launched;
+  pset<BF_PHASE_FAILED>(FA, n0, n1, n2, n3);
+  launch_effects(SK, LA, c.T_COND, c.SYNC_T, c.T_PAR, c.T_STOP, n0, n1, n2, n3);
+  pset<BF_PHASE_PENDING_QUEUED>(QU, n0, n1, n2, n3);
+  for (uint32_t i = c.lo; i < c.hi; ++i) {   // the stop steps' phases (a PHASE entry names a launched stop step)
+    const bf_commit_entry e = P.entries[i];
+    const uint32_t bit = 1u << (e.step & 31u);
+    if (e.kind != BF_COMMIT_PHASE || lane != (e.step >> 5u) || !(LA & bit)) continue;
+    n0 = (e.code & 1u) ? n0 | bit : n0 & ~bit;
+    n1 = (e.code & 2u) ? n1 | bit : n1 & ~bit;
+    n2 = (e.code & 4u) ? n2 | bit : n2 & ~bit;
+    n3 = (e.code & 8u) ? n3 | bit : n3 & ~bit;
+  }
+  const uint32_t dirty = (n0 ^ m0) | (n1 ^ m1) | (n2 ^ m2) | (n3 ^ m3);
+  if (dirty) {
+    ph[0] = (p[0] & ~dirty) | (n0 & dirty);
+    ph[P.words] = (p[1] & ~dirty) | (n1 & dirty);
+    ph[2u * P.words] = (p[2] & ~dirty) | (n2 & dirty);
+    ph[3u * P.words] = (p[3] & ~dirty) | (n3 & dirty);
+  }
+  // launched parallel steps register their children (step_executor.go:808-809)
+  const TopoHeader* th = reinterpret_cast<const TopoHeader*>(c.topo);
+  const ParDesc* pd = reinterpret_cast<const ParDesc*>(c.topo + th->off_par);
+  const unsigned long long reg = *reinterpret_cast<const unsigned long long*>(rec + 8);
+  const uint32_t n_par = th->P;
+  uint32_t set[2], reg_only = 0u;
+  for (uint32_t h = 0; h < 2; ++h) {   // BF_MAX_PARALLEL = 64 descs: lane p and lane p + 32
+    const uint32_t q = lane + 32u * h;
+    const uint32_t stp = q < n_par ? pd[q].step : 0u;
+    const uint32_t lw = __shfl_sync(FULL, LA, (stp >> 5) & 31u), dw = __shfl_sync(FULL, dirty, (stp >> 5) & 31u);
+    const bool in = q < n_par && ((lw >> (stp & 31u)) & 1u);
+    set[h] = __ballot_sync(FULL, in);
+    if (in && !((reg >> q) & 1ull) && !((dw >> (stp & 31u)) & 1u)) ++reg_only;   // counted once per step
+  }
+  const unsigned long long newly = ((unsigned long long)set[1] << 32 | set[0]) & ~reg;
+  const uint32_t written = __any_sync(FULL, dirty != 0u) || newly != 0ull;
+  const uint32_t n_skip = redux_add(__popc(dirty & SK)), n_launch = redux_add(__popc(dirty & LA) + reg_only);
+  const uint32_t n_queue = redux_add(__popc(dirty & QU)), n_fail = redux_add(__popc(dirty & FA));
+  if (lane == 0 && written) {
+    if (newly) *reinterpret_cast<unsigned long long*>(rec + 8) = reg | newly;
+    atomicMax(P.mark + r, P.mark_value);   // max: an upload's "must list" bit stays
+    atomicAdd(P.counts, 1u);
+    if (n_skip) atomicAdd(P.counts + 1, n_skip);
+    if (n_launch) atomicAdd(P.counts + 2, n_launch);
+    if (n_queue) atomicAdd(P.counts + 3, n_queue);
+    if (n_fail) atomicAdd(P.counts + 4, n_fail);
+  }
+}
+
+cudaError_t launch_commit(const CommitParams& P, bool apply, cudaStream_t stream) {
+  if (P.n_runs == 0) return cudaSuccess;
+  if (apply) commit_apply<<<(P.n_runs - 1u) / 8u + 1u, 256, 0, stream>>>(P);
+  else commit_check<<<(P.n_runs - 1u) / 8u + 1u, 256, 0, stream>>>(P);
+  return cudaGetLastError();
+}
+
 }  // namespace bf

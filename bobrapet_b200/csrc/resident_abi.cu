@@ -196,7 +196,7 @@ static int resident_tick_locked(bf_ctx* c, Resident* r, const bf_delta* deltas, 
   r->records_unknown();
   if (rc != BF_OK) return rc;
   if (int rc2 = r->full_tick_done(c, n_runs, flags, max_iterations, s)) return rc2;
-  r->tick_done(n_runs);
+  r->tick_done(n_runs, flags);
   if (tail_delivers) c->rejected_clean = true;
   const uint64_t rejected = tail_delivers ? c->pinned->tail.rejected : c->pinned->word;
   if (int rc2 = bf::publish_pass(c, n_runs, L, r->d_state, r->d_result, counts, co, first_slice, c->last_events)) return rc2;
@@ -313,7 +313,7 @@ static int touched_tick_locked(bf_ctx* c, Resident* r, const bf_delta* deltas, u
     r->pending = tail.carried;   // every touched run below n_runs was evaluated: the ones above it are all that is left
     c->rejected_clean = true;    // delivered and cleared by the emit kernel
   }
-  r->tick_done(n_runs);
+  r->tick_done(n_runs, flags);
   if (int rc2 = bf::publish_pass(c, n_runs, L, r->d_state, r->d_result, counts, &co, first_slice, c->last_touched_events)) return rc2;
   out->full = 0; out->n_listed = co.n_listed; out->n_evaluated = (uint32_t)tail.evaluated; out->n_events = co.n_events;
   return rejected_deltas(c, rejected, true);
@@ -1188,6 +1188,7 @@ int bf_resident_schedule(bf_ctx* c, const bf_sched_tables* t, uint32_t now, bf_r
     if (e == cudaSuccess) e = down(totals->global_running, o_gl, 4);
     return e;
   };
+  for (Resident* r : rs) r->scheduled = -1;   // a commit reads the records this call writes
   cudaError_t e = body();
   const cudaError_t es = cudaStreamSynchronize(s);   // never return with copies into the caller's buffers in flight
   if (e == cudaSuccess) e = es;
@@ -1203,6 +1204,7 @@ int bf_resident_schedule(bf_ctx* c, const bf_sched_tables* t, uint32_t now, bf_r
     p.n_events = part_tot[2 * i + 1];
     p.full = p.n_listed == p.n_runs ? 1u : 0u;
     rs[i]->sched_base_runs = p.n_runs;
+    rs[i]->scheduled = std::max<int64_t>(rs[i]->scheduled, p.n_runs);
     const uint32_t nl = std::min(p.n_listed, q.rcap);
     if (nl && q.runs != SIZE_MAX) {
       BF_CUDA(c, cudaMemcpy(p.runs, d + q.runs, (size_t)nl * 4, cudaMemcpyDeviceToHost));
@@ -1276,5 +1278,101 @@ int bf_resident_runctl_download(bf_ctx* c, uint32_t h, uint32_t first, uint32_t 
   BF_CUDA(c, cudaSetDevice(c->device));
   BF_CUDA(c, cudaMemcpyAsync(out, r->d_runctl + first, (size_t)n * sizeof(bf_run_ctl), cudaMemcpyDeviceToHost, c->stream));
   BF_CUDA(c, cudaStreamSynchronize(c->stream));
+  return BF_OK;
+}
+
+// ---- tick commits (resident.cu) -----------------------------------------------------------------------------------------------
+// The host checks the call and the entries, sorts them by (run, step) and uploads them; the check launch lowers the first
+// offender, which one D2H copy and one synchronisation bring back before anything is written; then the apply launch and the
+// counts.  A commit that wrote a run changes the state records: it ends the snapshot and the tick a schedule or a commit needs.
+int bf_resident_commit(bf_ctx* c, uint32_t h, uint32_t n_runs, const bf_commit_entry* entries, uint32_t n, bf_commit_out* out) {
+  auto [g, r] = lock_resident(c, h);
+  if (!out || out->struct_size != sizeof(bf_commit_out)) return fail(c, BF_EINVAL, "null bf_commit_out or bad struct_size");
+  *out = bf_commit_out{};
+  out->struct_size = sizeof(bf_commit_out);
+  out->bad_run = out->bad_step = BF_COMMIT_NONE;
+  if (!r) return BF_EINVAL;
+  auto refuse = [&](uint32_t run, uint32_t step, const std::string& msg) {
+    out->bad_run = run; out->bad_step = step;
+    return fail(c, BF_EINVAL, msg);
+  };
+  const bf_layout& L = r->L;
+  if (n_runs > r->cap) return refuse(BF_COMMIT_NONE, BF_COMMIT_NONE, "n_runs exceeds the resident batch");
+  if (n && !entries) return refuse(BF_COMMIT_NONE, BF_COMMIT_NONE, "null entries");
+  if (L.off_cond != BF_OFF_NONE && L.off_fail == BF_OFF_NONE)
+    return refuse(BF_COMMIT_NONE, BF_COMMIT_NONE, "the layout has cond planes but no BF_F_OUT_FAIL: the cond-FAIL steps are unknown");
+  const std::string over = " over " + std::to_string(n_runs) + " runs";
+  if (r->ticked < (int64_t)n_runs)
+    return refuse(BF_COMMIT_NONE, BF_COMMIT_NONE, "the state records changed since the last tick" + over + ": a tick must come between them and the commit");
+  if (c->slot_changes != r->slot_changes_seen)   // every tick that went through left them equal (a change makes the next tick full)
+    return refuse(BF_COMMIT_NONE, BF_COMMIT_NONE, "a topology slot was dropped or reused since the last tick: the masks may not fit the slot's steps");
+  if (r->single_ticked < (int64_t)n_runs)
+    return refuse(BF_COMMIT_NONE, BF_COMMIT_NONE, "no single-pass tick" + over + " since the last BF_EVAL_FIXPOINT tick: commits follow single-pass ticks");
+  if (r->d_sched_in && r->scheduled < (int64_t)n_runs)
+    return refuse(BF_COMMIT_NONE, BF_COMMIT_NONE, "the batch has limiter inputs and no bf_resident_schedule" + over + " ran since its last tick");
+  std::vector<std::pair<uint64_t, uint32_t>> order(n);   // (run << 16 | step, index)
+  for (uint32_t i = 0; i < n; ++i) {
+    const bf_commit_entry& e = entries[i];
+    auto at = [i] { return "entry " + std::to_string(i) + ": "; };
+    if (e.run >= n_runs) return refuse(e.run, e.step, at() + "run outside [0, n_runs)");
+    if (e.step >= L.steps_max) return refuse(e.run, e.step, at() + "step outside the layout");
+    if (e.kind < BF_COMMIT_HOLD || e.kind > BF_COMMIT_PHASE) return refuse(e.run, e.step, at() + "kind is not a BF_COMMIT_* code");
+    if (e.kind == BF_COMMIT_PHASE ? (e.code < BF_PHASE_PENDING || e.code > BF_PHASE_SKIPPED) : e.code != 0)
+      return refuse(e.run, e.step, at() + "bad code (a BF_COMMIT_PHASE entry takes BF_PHASE_PENDING .. BF_PHASE_SKIPPED, the others 0)");
+    order[i] = {(uint64_t)e.run << 16 | e.step, i};
+  }
+  std::sort(order.begin(), order.end());
+  for (uint32_t i = 1; i < n; ++i)
+    if (order[i].first == order[i - 1].first) {
+      const bf_commit_entry& e = entries[order[i].second];
+      return refuse(e.run, e.step, "entries " + std::to_string(order[i - 1].second) + " and " + std::to_string(order[i].second) +
+                                       " name the same (run, step)");
+    }
+  if (n_runs == 0) return BF_OK;
+  BF_CUDA(c, cudaSetDevice(c->device));
+  cudaStream_t s = c->stream;
+  if (int rc = bf::sync_slots(c, s)) return rc;   // the slot table as it stands now
+  const size_t o_entries = 32, bytes = o_entries + (size_t)n * sizeof(bf_commit_entry);
+  if (int rc = c->d_commit.ensure(c, bytes)) return rc;
+  std::vector<uint8_t> blob(bytes, 0);
+  memset(blob.data(), 0xFF, 8);   // no offender yet; the counts start at zero
+  for (uint32_t i = 0; i < n; ++i) memcpy(blob.data() + o_entries + (size_t)i * sizeof(bf_commit_entry), &entries[order[i].second], sizeof(bf_commit_entry));
+  bf::CommitParams P{};
+  P.state = r->d_state; P.result = r->d_result; P.sched_rec = r->d_sched_in ? r->d_sched_rec.p : nullptr;
+  P.slots = c->slots_dev; P.n_slots = (uint32_t)c->slots_host.size();
+  P.entries = reinterpret_cast<const bf_commit_entry*>(c->d_commit + o_entries); P.n_entries = n; P.n_runs = n_runs;
+  P.words = L.words; P.state_stride = L.state_stride; P.off_phase = L.off_phase; P.result_stride = L.result_stride;
+  P.off_ready = L.off_ready; P.off_skip = L.off_skip; P.off_fail = L.off_fail; P.sched_stride = r->sched_stride();
+  P.mark = r->d_mark; P.mark_value = r->mark_touched();
+  P.offender = reinterpret_cast<unsigned long long*>(c->d_commit.p);
+  P.counts = reinterpret_cast<uint32_t*>(c->d_commit + 8);
+  uint32_t* host = c->pinned->commit;
+  cudaError_t e = cudaMemcpyAsync(c->d_commit, blob.data(), bytes, cudaMemcpyHostToDevice, s);
+  if (e == cudaSuccess) e = bf::launch_commit(P, false, s);
+  if (e == cudaSuccess) e = cudaMemcpyAsync(host, c->d_commit, 8, cudaMemcpyDeviceToHost, s);
+  const cudaError_t es = cudaStreamSynchronize(s);
+  if (e == cudaSuccess) e = es;
+  if (e != cudaSuccess) return cuda_fail(c, e, "bf_resident_commit (check)");
+  c->stats.kernel_launches += 1;
+  uint64_t key;
+  memcpy(&key, host, 8);
+  if (key != ~0ull) {
+    const uint32_t run = (uint32_t)(key >> 32), step = (uint32_t)(key >> 8) & 0xFFFFFFu, why = (uint32_t)key & 0xFFu;
+    const std::string at = "run " + std::to_string(run) + " step " + std::to_string(step) + ": ";
+    return refuse(run, step, at + (why == bf::kCommitNotLaunched ? "an entry names a step the tick did not launch"
+                                   : why == bf::kCommitNotStop   ? "a BF_COMMIT_PHASE entry names a step that is not a stop step"
+                                                                 : "a launched stop step has no BF_COMMIT_PHASE entry"));
+  }
+  e = bf::launch_commit(P, true, s);
+  if (e == cudaSuccess) e = cudaMemcpyAsync(host, c->d_commit + 8, 20, cudaMemcpyDeviceToHost, s);
+  if (int rc = r->sync_in_place(c, e, "bf_resident_commit")) { r->state_changed(c); return rc; }
+  c->stats.kernel_launches += 1;
+  uint32_t k[5];
+  memcpy(k, host, sizeof k);
+  out->n_runs_written = k[0]; out->n_skipped = k[1]; out->n_launched = k[2]; out->n_queued = k[3]; out->n_failed = k[4];
+  if (k[0]) {   // as a delta: the written runs are touched, and the tick a schedule or a commit needs is over
+    r->state_changed(c);
+    r->pending += k[0];
+  }
   return BF_OK;
 }

@@ -357,6 +357,27 @@ class Frontier:
                     "bf_resident_runctl_download")
         return out
 
+    # -- tick commits of a resident batch (bf_resident_commit)
+    COMMIT_DTYPE = np.dtype([("run", "<u4"), ("step", "<u2"), ("kind", "u1"), ("code", "u1")])   # bf_commit_entry, 8 B
+
+    def resident_commit(self, handle: int, n_runs: int, entries=None) -> dict:
+        """bf_resident_commit: write the skips, launches and queue marks of the last tick (and schedule) of runs [0, n_runs)
+        into the state records.  entries: COMMIT_DTYPE (or (run, step, kind, code) tuples), at most one per (run, step).
+        -> dict(n_runs_written, n_skipped, n_launched, n_queued, n_failed).  A refusal raises FrontierError with .bad_run and
+        .bad_step (A.COMMIT_NONE for a refusal of the whole call)"""
+        ents = np.zeros(0, dtype=self.COMMIT_DTYPE) if entries is None else entries
+        if not isinstance(ents, np.ndarray):
+            ents = np.array([tuple(e) for e in ents], dtype=self.COMMIT_DTYPE)
+        ents = np.ascontiguousarray(ents, dtype=self.COMMIT_DTYPE)
+        out = A.CommitOut(struct_size=C.sizeof(A.CommitOut))
+        rc = self._lib.bf_resident_commit(self._ctx, handle, int(n_runs), ents.ctypes.data if ents.shape[0] else None,
+                                          ents.shape[0], C.byref(out))
+        if rc != A.BF_OK:
+            err = A.FrontierError(rc, "bf_resident_commit: %s" % self._lib.bf_last_error(self._ctx).decode())
+            err.bad_run, err.bad_step = int(out.bad_run), int(out.bad_step)
+            raise err
+        return {k: int(getattr(out, k)) for k in ("n_runs_written", "n_skipped", "n_launched", "n_queued", "n_failed")}
+
     # -- limiter inputs and schedules of resident batches (bf_resident_sched*, bf_resident_schedule)
     SCHED_PUT_DTYPE = np.dtype([("run", "<u4"), ("story_key", "<u4"), ("queue_key", "<u4"), ("priority", "<i4"),
                                 ("queued_since", "<u4"), ("run_phase", "<u4"), ("reserved", "<u4", (2,))])   # bf_sched_put, 32 B

@@ -573,6 +573,43 @@ func (r *Resident) PutRunCtl(reqs []RunCtl) error {
 	return r.c.err(C.bf_resident_runctl_put(r.c.p, r.handle, rp, C.uint32_t(len(reqs))))
 }
 
+// Kinds of a CommitEntry (BF_COMMIT_*): what the host's StepExecutor.Execute did with a launched step other than launch it.
+const (
+	CommitHold  = 1          // Execute was blocked on template evaluation: the step gets no launch write
+	CommitError = 2          // Execute failed: the whole run gets no write (nothing of the reconcile is persisted)
+	CommitPhase = 3          // Code is the with.phase of a launched stop step (executeStopStep)
+	CommitNone  = 0xFFFFFFFF // BadRun / BadStep of a refusal of the whole call
+)
+
+// CommitEntry is one exception of Commit (bf_commit_entry, 8 bytes, no pointers), at most one per (run, step).
+type CommitEntry struct {
+	Run        uint32
+	Step       uint16
+	Kind, Code uint8
+}
+
+// CommitResult is what Commit wrote (steps whose code changed) and, on a refusal, the first offending (run, step).
+type CommitResult struct {
+	RunsWritten, Skipped, Launched, Queued, Failed uint32
+	BadRun, BadStep                                uint32
+}
+
+// Commit writes the decisions of the last tick and schedule of runs [0, n) into the batch's records (bf_resident_commit):
+// skipped steps Skipped, cond-FAIL steps Failed, launched steps what Execute writes for their type, queued steps Pending
+// queued.  Call it after Execute has run the launches of ScheduleResident (or of TickTouched without limiter inputs); entries
+// report the held steps, the runs whose Execute failed and the phase of every launched stop step.  The batcher then sends no
+// echo deltas for these writes.  A refusal changes nothing and names the offender in BadRun / BadStep.
+func (r *Resident) Commit(n uint32, entries []CommitEntry) (CommitResult, error) {
+	var ep *C.bf_commit_entry
+	if len(entries) > 0 {
+		ep = (*C.bf_commit_entry)(unsafe.Pointer(&entries[0]))
+	}
+	var k [7]C.uint32_t
+	rc := C.bfgo_resident_commit(r.c.p, r.handle, C.uint32_t(n), ep, C.uint32_t(len(entries)), &k[0])
+	res := CommitResult{uint32(k[0]), uint32(k[1]), uint32(k[2]), uint32(k[3]), uint32(k[4]), uint32(k[5]), uint32(k[6])}
+	return res, r.c.err(rc)
+}
+
 // SchedPut is one limiter-input request of PutSched (bf_sched_put, 32 bytes, no pointers).  QueuedSince is the StartedAt of the
 // run's earliest queued step on the clock of ScheduleResident's now (SchedNone: nothing queued); the device ages from it.
 type SchedPut struct {

@@ -210,6 +210,19 @@ static inline int bfgo_resident_runctl_put1(bf_ctx* c, uint32_t handle, uint32_t
   return bf_resident_runctl_put(c, handle, &q, 1);
 }
 
+/* Tick commits.  The entries are passed as they are (bf_commit_entry holds no pointers); the out block comes back flat:
+ * counts[0..6] = runs written, skipped, launched, queued, failed, bad_run, bad_step. */
+static inline int bfgo_resident_commit(bf_ctx* c, uint32_t handle, uint32_t n_runs, const bf_commit_entry* entries, uint32_t n,
+                                       uint32_t* counts) {
+  bf_commit_out o;
+  memset(&o, 0, sizeof o);
+  o.struct_size = (uint32_t)sizeof o;
+  const int rc = bf_resident_commit(c, handle, n_runs, entries, n, &o);
+  counts[0] = o.n_runs_written; counts[1] = o.n_skipped; counts[2] = o.n_launched; counts[3] = o.n_queued; counts[4] = o.n_failed;
+  counts[5] = o.bad_run; counts[6] = o.bad_step;
+  return rc;
+}
+
 static inline void bfgo_tables(bf_sched_tables* t, uint32_t n_stories, uint32_t n_queues, int32_t global_limit, uint32_t global_base,
                                const int32_t* story_limit, const uint32_t* story_base, const int32_t* queue_limit,
                                const int32_t* queue_aging_s, const uint32_t* queue_base, const int32_t* queue_max_priority_base) {

@@ -1029,6 +1029,75 @@ int bf_resident_runctl(bf_ctx* ctx, uint32_t handle);
 int bf_resident_runctl_put(bf_ctx* ctx, uint32_t handle, const bf_run_ctl_put* requests, uint32_t n);
 int bf_resident_runctl_download(bf_ctx* ctx, uint32_t handle, uint32_t first_run, uint32_t n_runs, bf_run_ctl* out);
 
+/* ------------------------------------------------------------------ tick commits (the decisions of a tick written back)
+ * After a tick the reference writes, in the same reconcile, what the decisions of that iteration did to StepStates: skipped steps
+ * become Skipped (dag.go:1734-1746), queued steps Pending with a "Queued due to ..." message (markQueuedSteps, :1999-2018; code 14
+ * here), and each launched step what StepExecutor.Execute writes for its type (step_executor.go:132-185).  bf_resident_commit makes
+ * these writes in the stored state records of runs [0, n_runs), so that a batcher sends no echo deltas for its own decisions: a step
+ * downstream of a skip becomes ready at the next tick, and a launched step is no longer listed as ready.
+ *
+ * The writes, from the current result record of each run (the one the last tick left) and, when the batch has a limiter area
+ * (bf_resident_sched), its last schedule record:
+ *   skip mask                                      -> BF_PHASE_SKIPPED
+ *   fail mask (cond FAIL, dag.go:2744-2748)        -> BF_PHASE_FAILED
+ *   launched condition step                        -> BF_PHASE_SUCCEEDED                          (step_executor.go:168-170)
+ *   launched sleep / gate / wait step              -> BF_PHASE_PAUSED                             (:171-179)
+ *   launched parallel step                         -> BF_PHASE_RUNNING and its children_registered bit set (:808-809)
+ *   launched stop step                             -> the code of its BF_COMMIT_PHASE entry        (:1096-1106)
+ *   launched engram / executeStory step            -> BF_PHASE_RUNNING when its code is 0 or 14, else unchanged (dag.go:1770-1774)
+ *   queued step (queued_story | queued_sched)      -> BF_PHASE_PENDING_QUEUED                      (dag.go:1999-2018)
+ * The launched steps are the schedule record's launch mask when the batch has a limiter area, else the ready mask (nothing is then
+ * queued).  The masks are taken disjoint in this order: fail without skip, launched and queued without either.  A run whose topology
+ * slot is dead, or does not fit the layout, has no masks.  A phase code 15 reads as 0, as the pass reads it; a step the commit does
+ * not write keeps its bytes.
+ *
+ * Entries report what the host's Execute did, at most one per (run, step), each naming a launched step:
+ *   BF_COMMIT_HOLD   Execute was blocked on template evaluation (dag.go:1750-1761): that step gets no launch write.
+ *   BF_COMMIT_ERROR  Execute failed: the reference returns the error and persists nothing of that reconcile (dag.go:1763-1768,
+ *                    :342-345), so the whole run gets no write.
+ *   BF_COMMIT_PHASE  the with.phase of a launched stop step (code: BF_PHASE_PENDING .. BF_PHASE_SKIPPED).  Every launched stop step
+ *                    of a run without a BF_COMMIT_ERROR entry needs one, or a BF_COMMIT_HOLD entry.
+ * Checked before anything changes, else BF_EINVAL, nothing changed, and bad_run / bad_step name the first offender (BF_COMMIT_NONE
+ * for a refusal of the whole call).  In this order: struct_size and the handle; n_runs <= capacity; entries not NULL when n > 0;
+ * the layout has cond planes but no BF_F_OUT_FAIL (the device cannot know the cond-FAIL steps); the batch's state records changed
+ * since its last tick over n_runs (the rule of bf_resident_schedule); a topology slot of the ctx was dropped, or a dropped one
+ * reused, since the batch's last tick (the masks were evaluated against the step types the slot had then); a tick with BF_EVAL_FIXPOINT ran since the last single-pass
+ * tick over n_runs (the fixpoint applies these effects in memory, under unlimited limiters); the batch has a limiter area and no
+ * bf_resident_schedule over at least n_runs of it ran since its last tick.  Then each entry in array order: run < n_runs,
+ * step < steps_max, kind and code (0 for HOLD and ERROR); then the lowest (run, step) named twice; then, on the device, the lowest
+ * (run, step) that is an entry naming a step not launched, a BF_COMMIT_PHASE entry of a step that is not a stop step, or a
+ * launched stop step without an entry.
+ *
+ * Idempotent: a run whose writes are in place is not changed.  A run whose record changed is touched as by a delta (the next
+ * bf_resident_tick_touched evaluates it), and a commit that changed anything ends the evaluated snapshot and the tick a schedule
+ * or a commit needs.  The step timers are not armed (the batcher arms the deadlines of launched sleeps, gates and waits), and a
+ * stopped run (bf_resident_runctl) has no candidates, so it gets nothing.  The counts are steps whose code the commit changed (a
+ * launched parallel step also when only its registered bit was set).  Stage G / H / I rewrites (gate syncs, joins, fail-fast and
+ * compensation skips) are not persisted: each pass recomputes them from the state.  One H2D copy of the sorted entries, the check
+ * launch, one D2H copy and one synchronisation before anything is written; then the apply launch, one D2H copy and one
+ * synchronisation.                                                                                                          */
+enum { BF_COMMIT_HOLD = 1, BF_COMMIT_ERROR = 2, BF_COMMIT_PHASE = 3 };
+#define BF_COMMIT_NONE 0xFFFFFFFFu
+typedef struct bf_commit_entry { /* 8 B, one per (run, step) the host's Execute did not launch normally                        */
+  uint32_t run;
+  uint16_t step;
+  uint8_t kind;                  /* BF_COMMIT_*                                                                               */
+  uint8_t code;                  /* BF_COMMIT_PHASE: the phase code executeStopStep writes; else 0                            */
+} bf_commit_entry;
+typedef struct bf_commit_out {
+  uint32_t struct_size;          /* sizeof(bf_commit_out)                                                                     */
+  uint32_t n_runs_written;       /* out: runs whose state record changed (touched)                                            */
+  uint32_t n_skipped;            /* out: steps written as BF_PHASE_SKIPPED                                                    */
+  uint32_t n_launched;           /* out: launched steps written                                                               */
+  uint32_t n_queued;             /* out: steps written as BF_PHASE_PENDING_QUEUED                                             */
+  uint32_t n_failed;             /* out: steps written as BF_PHASE_FAILED by a cond FAIL                                      */
+  uint32_t bad_run;              /* out on a refusal: the offending run, or BF_COMMIT_NONE                                    */
+  uint32_t bad_step;             /* out on a refusal: the offending step, or BF_COMMIT_NONE                                   */
+} bf_commit_out;
+
+int bf_resident_commit(bf_ctx* ctx, uint32_t handle, uint32_t n_runs, const bf_commit_entry* entries, uint32_t n_entries,
+                       bf_commit_out* out);
+
 /* ------------------------------------------------------------------ device groups (SURVEY.md row e)
  * The reference is ONE operator process (cmd/main.go:220, StoryRunReconciler storyrun_controller.go:216), so the
  * multi-GPU path must be reachable from one process through this ABI: a group owns one ctx per device and an NCCL
