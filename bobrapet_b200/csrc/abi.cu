@@ -96,7 +96,10 @@ void plan_pack(const bf_ctx* c, const bf_batch& b, const bf::Knobs& k, uint32_t 
   // with 1/k of the shared memory
   const uint32_t ctas_per_sm = k.pack_ctas >= 1 && k.pack_ctas <= 4 ? (uint32_t)k.pack_ctas : 1u;
   const uint32_t group_bytes = R * stage_bytes;
-  // per-warp scratch (frontier_pack.cu): status bytes R x st_stride | fix-up words | walk table R x 16, in units of 256 bytes
+  // per-warp scratch (frontier_pack.cu): status pairs 512 B | fix-up words | walk table R x 16, in units of 256 bytes.  The
+  // reservation is still that of the status-byte layout before it (R x st_stride bytes of status, st_stride = 256 at wq = 8,
+  // 32 wq + 16 otherwise), 512 - 1024 bytes per warp more than the kernel reads: a smaller one moves slot groups and shared
+  // memory of every launch shape, a change to be measured for itself (warps per CTA measured flat from 20 to 28, DESIGN §5).
   const uint32_t st_stride = wq == 8 ? 256u : 32u * wq + 16u;
   const uint32_t work = round_up(R * st_stride + 128u + 16u * R, 256);
   auto groups_for = [&](uint32_t warps) -> uint32_t {   // slot groups that fit beside `warps` scratch areas

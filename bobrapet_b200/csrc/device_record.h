@@ -13,13 +13,13 @@
 //   fixed-width rows (ell = K in {2, 4}; taken when no step has more than K needs and S*K entries are not
 //   larger than the CSR block they replace; S > 256): row_ptr is implicit (row i starts at entry i*K)
 //   +32 = off_col col_idx   u16[32*W][K]      the needs of step i, unused entries (and the rows past S) = PAD
-//                                             PAD = 32*W: the status byte just past the last step word, always 0
-//                                             ("satisfied, not failed"), so a padded entry never changes a verdict
+//                                             PAD = 32*W: the status just past the last step word, always
+//                                             "satisfied, not failed", so a padded entry never changes a verdict
 //
 //   fixed-width rows with BYTE entries (ell = 0x100 | K; taken for every topology of at most 256 steps that qualifies
 //   for fixed-width rows): a step index fits a byte, so the adjacency is HALF the size again
 //   +32 = off_col col_idx   u8[32*W][K]       the needs of step i; a row shorter than K repeats its first entry (the OR
-//                                             over a row's status bytes is idempotent); there is no PAD index (32*W = 256
+//                                             over a row's statuses is idempotent); there is no PAD index (32*W = 256
 //                                             does not fit a byte at S = 256), so a row WITHOUT needs holds its own index
 //                                             and its step is flagged in a ninth static plane, NODEP: flagged steps never
 //                                             enter the walk, their dependencies are trivially met

@@ -348,7 +348,7 @@ __global__ void __launch_bounds__(RB == 2 ? 768 : 512, RB == 1 ? 2 : 1) frontier
         if (CD) {
           // item j: word j of the run; the scratch holds fail words for the run's words only (the lanes of `act`)
           auto fixup = [&](uint32_t j, uint32_t candw, uint32_t fclass, uint32_t& mb, uint32_t& fb) {
-            fixup_item(lane, candw, j, ell, rp_a, col_a, st_a, mfail_a, fclass, mb, fb);
+            fixup_item(lane, candw, j, ell, rp_a, col_a, [&](uint32_t d) { return lds_u8(st_a + d); }, mfail_a, fclass, mb, fb);
           };
           if (stage_cond(lane, c0, c1, dc, mfail_a, act, S, fixup, met_w, fd_w, ready_w, skipc_w, fail_w, p0, p1, p2, p3)) marked = true;
         }

@@ -50,25 +50,68 @@ __device__ unsigned long long g_trace[8][160][4];
 __device__ unsigned int g_launch;
 DI unsigned long long gtime() { unsigned long long t; asm volatile("mov.u64 %0, %globaltimer;" : "=l"(t)); return t; }
 #endif
+#ifdef PACK_STAGES  // stage probe (tools/stage_probe.py, lib_ab builds only): SM cycles per region of a group trip, summed over all warps:
+// 0 ticket + barrier wait, 1 planes + stages G / B / I / D-prep, 2 stage C, 3 walk (with the second link's load issue),
+// 4 load_cut + cond fix-up + stage E, 5 issue; 6 counts trips.  Lane i accumulates region i (one register).
+__device__ unsigned long long g_stages[8];
+#define PROBE(i) do { const uint32_t t_ = (uint32_t)clock(); pr_acc += lane == (i) ? t_ - pr_t : 0u; pr_t = t_; } while (0)
+#else
+#define PROBE(i) do { } while (0)
+#endif
+
+// ---- status of the steps of a group: bit words, not bytes.
+// Stage C stores each lane's U (not satisfied) and FD (failed dependency) words once per trip, interleaved by half words into
+// a pair of 32-bit status words, one per 16 steps: the word of steps 0 - 15 holds U in its low half and FD in its high half,
+// the word of steps 16 - 31 FD in its low half and U in its high half.  Rotated right by d & 31 (shf.r.wrap takes the low 5
+// bits of d by itself), the status word of step d has d's U bit at bit 0 and its FD bit at bit 16 in either half, so one 32-bit
+// load serves both tests.  Word pair w of run g lies at st0 + g * 16 Wq + 8 w: a run's pairs start on a 16 Wq-byte boundary
+// and pairs Wq .. 2 Wq - 1 stay zero, so dependency d's status word is at base | ((d >> 2) & ~3) (a shift and one LOP3).
+// The PAD entry of u16 fixed-width rows (d = 32 W, device_record.h) reads pair W: a lane of the run with w >= W (U = FD = 0),
+// or for W = Wq the zero pair behind the run's words — "satisfied".  All lanes of one item read the status of the same run,
+// at most 2 Wq distinct words in 8 Wq contiguous bytes: broadcast loads without bank conflicts.
+constexpr uint32_t ST_BYTES = 512;   // status of the R runs of a group: R * 16 * Wq = 512 bytes at every Wq
+constexpr uint32_t ST_U = 1u, ST_FD = 1u << 16;   // the bits of a rotated status word (dep_status)
+
+// dependency d of the run whose status starts at st, rotated: bit 0 not satisfied, bit 16 failed dependency, the other bits
+// without meaning.  Only the low 5 bits of d and the bits `off_mask` keeps of d >> 2 are read.
+DI uint32_t dep_status(uint32_t st, uint32_t d, uint32_t off_mask) {
+  const uint32_t v = lds_u32(st | ((d >> 2) & off_mask));
+  return __funnelshift_r(v, v, d);
+}
+
+// phase 3 of an item (phases 1 and 2: row_locate / row_fetch, kernel_common.cuh): OR of the rotated status words of the row's
+// dependencies (CSR: masked by the row length)
+template <int FMT>
+DI uint32_t row_status_bits(uint32_t p, uint32_t n, const uint32_t (&x)[4], uint32_t st) {
+  constexpr int E = (FMT == FMT_ELL2 || FMT == FMT_ELL2B) ? 2 : 4;
+  uint32_t s[E], r = 0;
+#pragma unroll
+  for (int e = 0; e < E; ++e) s[e] = dep_status(st, x[e], ~3u);
+#pragma unroll
+  for (int e = 0; e < E; ++e) r |= (fmt_traits<FMT>::fixed || (uint32_t)e < n) ? s[e] : 0u;
+  if (FMT == FMT_CSRL)
+    for (uint32_t q = 4; q < n; ++q) r |= dep_status(st, lds_u16(p + q * 2u), ~3u);
+  return r;
+}
 
 // ---- stage D over the (run, word) items of a group.
-// Where the rows and status bytes of run g live: CSR formats read the per-run table {col_a, rp_a, st_a, max_deg | ell << 16}
+// Where the rows and status pairs of run g live: CSR formats read the per-run table {col_a, rp_a, st_a, max_deg | ell << 16}
 // written in stage C; fixed-width rows always start 32 bytes into the run's topology buffer, so their addresses are
 // computed (two multiply-adds, no dependent shared-memory load in front of the row fetch).
 struct WalkCtx {
   uint32_t tab_a;      // per-run table (16 B entries)
   uint32_t col0;       // fixed-width formats: col_idx of run 0 of the group (topology buffer 0 + 32)
   uint32_t topo_buf;   // bytes between the topology buffers of consecutive runs
-  uint32_t st0;        // status bytes of run 0
-  uint32_t st_stride;  // bytes between the status areas of consecutive runs
+  uint32_t st0;        // status pairs of run 0
+  uint32_t st_run;     // bytes between the status of consecutive runs (16 * Wq)
 };
 
 // K items at once (independent load chains); FMT as in kernel_common.cuh — the caller guarantees that every live run
 // of the group has this row format (else it takes walk_items_any).
-// AL (byte-entry rows of four, 8 words per run): the status bytes of a run start on a 256-byte boundary, so the address of a
-// dependency's status byte is ONE byte permute — byte k of the row word over the low byte of the base — instead of an
-// extract and an add.  Fixed-width rows exist for every step of a word, so all 32 lanes fetch and the candidate word (the
-// same in every lane after the shuffle) masks the ballot instead of every lane's predicate.
+// AL (byte-entry rows of four, 8 words per run): the row word shifted right by 8 e is entry e as far as dep_status reads it
+// (its low 5 bits, and bits 4 .. 7 through the offset mask 0x3C), so no entry is extracted.
+// Fixed-width rows exist for every step of a word, so all 32 lanes fetch and the candidate word (the same in every lane
+// after the shuffle) masks the ballot instead of every lane's predicate.
 template <int K, int FMT, bool NEED_FD, bool AL = false>
 DI void walk_items_k(uint32_t lane, uint32_t CAND, uint32_t& todo, uint32_t lg, const WalkCtx& C, uint32_t& met_w, uint32_t& fd_w) {
   const uint32_t wmask = (1u << lg) - 1u;
@@ -84,21 +127,21 @@ DI void walk_items_k(uint32_t lane, uint32_t CAND, uint32_t& todo, uint32_t lg, 
     for (int k = 0; k < K; ++k) {
       cw[k] = __shfl_sync(FULL, CAND, L[k]);
       const uint32_t g = L[k] >> 3, i = (L[k] & 7u) * 32u + lane;
-      st[k] = C.st0 + g * 256u;
+      st[k] = C.st0 + g * 128u;
       p[k] = C.col0 + g * C.topo_buf + i * 4u;
     }
 #pragma unroll
     for (int k = 0; k < K; ++k) n[k] = lds_u32(p[k]);   // the row: four byte entries
 #pragma unroll
     for (int k = 0; k < K; ++k)
-      wv[k] = lds_u8(__byte_perm(n[k], st[k], 0x7650)) | lds_u8(__byte_perm(n[k], st[k], 0x7651)) |
-              lds_u8(__byte_perm(n[k], st[k], 0x7652)) | lds_u8(__byte_perm(n[k], st[k], 0x7653));
+      wv[k] = dep_status(st[k], n[k], 0x3Cu) | dep_status(st[k], n[k] >> 8, 0x3Cu) | dep_status(st[k], n[k] >> 16, 0x3Cu) |
+              dep_status(st[k], n[k] >> 24, 0x3Cu);
 #pragma unroll
     for (int k = 0; k < K; ++k) {
-      const uint32_t m = __ballot_sync(FULL, (wv[k] & 1u) == 0) & cw[k];
+      const uint32_t m = __ballot_sync(FULL, (wv[k] & ST_U) == 0) & cw[k];
       if (lane == L[k]) met_w = m;
       if (NEED_FD) {
-        const uint32_t f = __ballot_sync(FULL, (wv[k] & 2u) != 0) & cw[k];
+        const uint32_t f = __ballot_sync(FULL, (wv[k] & ST_FD) != 0) & cw[k];
         if (lane == L[k]) fd_w = f;
       }
     }
@@ -110,7 +153,7 @@ DI void walk_items_k(uint32_t lane, uint32_t CAND, uint32_t& todo, uint32_t lg, 
     const uint32_t g = L[k] >> lg, i = (L[k] & wmask) * 32u + lane;
     c[k] = (cw[k] >> lane) & 1u;
     if (fmt_traits<FMT>::fixed) {
-      st[k] = C.st0 + g * C.st_stride;
+      st[k] = C.st0 + g * C.st_run;
       p[k] = C.col0 + g * C.topo_buf + i * fmt_traits<FMT>::row_bytes;   // rows exist for every step of the word (device_record.h)
       n[k] = (uint32_t)(FMT & 0xFF);
     } else {
@@ -122,21 +165,21 @@ DI void walk_items_k(uint32_t lane, uint32_t CAND, uint32_t& todo, uint32_t lg, 
 #pragma unroll
   for (int k = 0; k < K; ++k) row_fetch<FMT>(p[k], n[k], x[k]);
 #pragma unroll
-  for (int k = 0; k < K; ++k) wv[k] = row_status<FMT>(p[k], n[k], x[k], st[k]);
+  for (int k = 0; k < K; ++k) wv[k] = row_status_bits<FMT>(p[k], n[k], x[k], st[k]);
 #pragma unroll
   for (int k = 0; k < K; ++k) {
     if (fmt_traits<FMT>::fixed) {   // every lane holds a real row: mask the ballot with the (lane-uniform) candidate word
-      const uint32_t m = __ballot_sync(FULL, (wv[k] & 0x01010101u) == 0) & cw[k];
+      const uint32_t m = __ballot_sync(FULL, (wv[k] & ST_U) == 0) & cw[k];
       if (lane == L[k]) met_w = m;
       if (NEED_FD) {
-        const uint32_t f = __ballot_sync(FULL, (wv[k] & 0x02020202u) != 0) & cw[k];
+        const uint32_t f = __ballot_sync(FULL, (wv[k] & ST_FD) != 0) & cw[k];
         if (lane == L[k]) fd_w = f;
       }
     } else {
-      const uint32_t m = __ballot_sync(FULL, c[k] && (wv[k] & 0x01010101u) == 0);
+      const uint32_t m = __ballot_sync(FULL, c[k] && (wv[k] & ST_U) == 0);
       if (lane == L[k]) met_w = m;
       if (NEED_FD) {
-        const uint32_t f = __ballot_sync(FULL, c[k] && (wv[k] & 0x02020202u) != 0);
+        const uint32_t f = __ballot_sync(FULL, c[k] && (wv[k] & ST_FD) != 0);
         if (lane == L[k]) fd_w = f;
       }
     }
@@ -212,19 +255,17 @@ __global__ void __launch_bounds__(32 * PACK_MAX_WARPS, PACK_MIN_BLOCKS) frontier
   const uint32_t bars_bytes = (NG * 12u + 127u) & ~127u;
   const uint32_t group_bytes = R * (P.state_stride + P.topo_buf_bytes);
   const uint32_t groups_a = pin(smem_base + 128u + bars_bytes);
-  // scratch (per warp, 256-byte aligned, work_bytes a multiple of 256): [status bytes: R x st_stride][fix-up fail words 128 B]
-  // [walk table: R x 16 B].  st_stride = 32*Wq + 16 (the PAD byte of a full-width run with u16 rows lives in the + 16) except at
-  // Wq = 8, where it is 256 so that every run's status bytes start on a 256-byte boundary (walk_items_k, AL; no topology of
-  // 8 words has u16 fixed-width rows: plan_record, topology.cu)
-  const uint32_t st_stride = Wq == 8u ? 256u : 32u * Wq + 16u;
+  // scratch (per warp, 256-byte aligned, work_bytes a multiple of 256, at least ST_BYTES + 128 + 16 R): [status pairs: R x 16 Wq]
+  // [fix-up fail words 128 B][walk table: R x 16 B]
+  const uint32_t st_run = 16u * Wq;
   const uint32_t scratch_a = ((groups_a + NG * group_bytes + 255u) & ~255u) + warp * P.work_bytes;
   const uint32_t st0_a = scratch_a;
-  const uint32_t mfail_a = st0_a + R * st_stride;
+  const uint32_t mfail_a = st0_a + ST_BYTES;
   const uint32_t tab_a = mfail_a + 128u;
   // !CD passes (no fix-up): the fix-up words of the NW warps hold the needed word of slot group sg (issue(); NG <= 32 NW)
   // at word sg % 32 of warp sg / 32, an address recomputed from the parameters at each use (a register more spills)
   auto need_a = [&](uint32_t sg) {
-    return ((groups_a + NG * (R * (P.state_stride + P.topo_buf_bytes)) + 255u) & ~255u) + (sg >> 5) * P.work_bytes + R * st_stride + (sg & 31u) * 4u;
+    return ((groups_a + NG * (R * (P.state_stride + P.topo_buf_bytes)) + 255u) & ~255u) + (sg >> 5) * P.work_bytes + ST_BYTES + (sg & 31u) * 4u;
   };
 
   if (threadIdx.x < 5) blk_counts[threadIdx.x] = 0ull;   // four counters + the group ticket
@@ -233,7 +274,7 @@ __global__ void __launch_bounds__(32 * PACK_MAX_WARPS, PACK_MIN_BLOCKS) frontier
     sts_u32(armed_a + 4u * threadIdx.x, 0u);
     fence_barrier_init();
   }
-  for (uint32_t x = lane * 4u; x < P.work_bytes; x += 128u) sts_u32(scratch_a + x, 0u);  // PAD bytes start as 0 and stay 0
+  for (uint32_t x = lane * 4u; x < P.work_bytes; x += 128u) sts_u32(scratch_a + x, 0u);  // the PAD pairs start as 0 and stay 0
   __syncthreads();
 
   // ---- the CTA's groups: global group id = blockIdx.x + t * gridDim.x, runs R * gid .. R * gid + R - 1
@@ -405,6 +446,9 @@ __global__ void __launch_bounds__(32 * PACK_MAX_WARPS, PACK_MIN_BLOCKS) frontier
 
   // the next group to consume: a CTA-wide ticket counter behind the four block counters (smem_p + 32)
   const uint32_t ng_magic = NG > 1u ? (uint32_t)(0x100000000ull / NG) + 1u : 0u;   // t / NG = umulhi(t, ng_magic), exact for t < 2^32 / NG (NG = 1: T <= 1, t = 0)
+#ifdef PACK_STAGES
+  uint32_t pr_acc = 0, pr_t = (uint32_t)clock();
+#endif
   for (;;) {
     uint32_t t = 0;
     if (lane == 0) t = atomicAdd(reinterpret_cast<uint32_t*>(smem_p + 32), 1u);
@@ -422,6 +466,7 @@ __global__ void __launch_bounds__(32 * PACK_MAX_WARPS, PACK_MIN_BLOCKS) frontier
     // before), so first wait until the arming warp has published use u; from then on the barrier is in phase u.
     while ((int32_t)(lds_poll_u32(armed_a + 4u * cur_sg) - (cur_use + 1u)) < 0) __nanosleep(32);
     mbar_wait(bars + 8u * cur_sg, cur_use & 1u);
+    PROBE(0);
 #ifdef PACK_TRACE
     if (t == 0) tr_first = gtime();
 #endif
@@ -476,7 +521,7 @@ __global__ void __launch_bounds__(32 * PACK_MAX_WARPS, PACK_MIN_BLOCKS) frontier
     const uint32_t GM = VALID & ~G1 & ~G2;
     const bool realtime = rflags & BF_RF_REALTIME;
 
-    // ---------------- stages G, B, I and D-prep (stages.cuh); U & VALID: the PAD byte of a narrower run reads "satisfied"
+    // ---------------- stages G, B, I and D-prep (stages.cuh); U & VALID: the PAD entry of a narrower run reads "satisfied"
     if (has_dec) stage_g(SYNC_T, TS, d0, d1, p0, p1, p2, p3);
     const RunClass rc = stage_bi<CD>(gmask, rflags, n_main, n_comp, n_final, AF, GM, G1, G2, p0, p1, p2, p3);
     uint32_t summary = rc.sum | rc.group;
@@ -485,40 +530,30 @@ __global__ void __launch_bounds__(32 * PACK_MAX_WARPS, PACK_MIN_BLOCKS) frontier
     // the floor cut: the walk takes the words the producer staged (bit `lane` of the slot group's needed word); a word it
     // left out has met = FREE, fd = 0
     const uint32_t CAND = FF ? ((lds_u32(need_a(cur_sg)) >> lane) & 1u ? dc.CAND : 0u) : dc.CAND;
-    // ------------- stage C: one status byte per step (bit0 unmet, bit1 failed-dep), all R runs -------------
+    // ------------- stage C: each lane's status word pair (U and FD interleaved by half words), all R runs -------------
     const bool any_fd = __any_sync(FULL, dc.skip_on_failed);           // some run of the group has a failed-dependency class
     const int my_fmt = fmt_of(ell, max_deg);
     const int fmt0 = __shfl_sync(FULL, live ? my_fmt : -1, __ffs(__ballot_sync(FULL, live) | 0x80000000u) - 1);  // format of the first live run
     const bool mixed = __any_sync(FULL, live && my_fmt != fmt0);
+    PROBE(1);
     __syncwarp();
-#pragma unroll
-    for (uint32_t it = 0; it < 4; ++it) {
-      const uint32_t item = it * 32 + lane;  // 8 steps: byte (item & 3) of the word held by lane item >> 2
-      const uint32_t sh = (item & 3u) * 8u;
-      const uint32_t ub = __shfl_sync(FULL, U, item >> 2) >> sh;
-      uint32_t vx = bits4_to_bytes(ub & 0xFu), vy = bits4_to_bytes((ub >> 4) & 0xFu);
-      if (any_fd) {  // warp-uniform
-        const uint32_t fb = __shfl_sync(FULL, FD, item >> 2) >> sh;
-        vx |= bits4_to_bytes(fb & 0xFu) << 1;
-        vy |= bits4_to_bytes((fb >> 4) & 0xFu) << 1;
-      }
-      sts_v2(st0_a + item * 8u + (item >> (2u + lg)) * (st_stride - 32u * Wq), vx, vy);   // run (item >> (2 + lg)) starts at st0 + run * st_stride
-    }
+    const uint32_t my_st = st0_a + g * st_run;
+    sts_v2(my_st + w * 8u, __byte_perm(U, FD, 0x5410), __byte_perm(U, FD, 0x3276));   // {U lo, FD lo}, {FD hi, U hi}
     // per-run walk entry: CSR / row bases, status base, longest row and row format
     const uint32_t col_a = tr_a + (h1.x & 0xFFFFu);
-    const uint32_t my_st = st0_a + g * st_stride;
     if (w == 0) sts_v4(tab_a + g * 16u, col_a, tr_a + (uint32_t)sizeof(TopoHeader), my_st, max_deg | (ell << 16));
     __syncwarp();
+    PROBE(2);
     // second link of the group I shall issue (its slot id, requested when I drew my ticket, has arrived by now — asking for
     // it right behind the barrier wait stalled every trip for a DRAM round trip); consumed by issue() at the end of the trip
     load_ent();
     // ------------- stage D: walk the needs rows (dag.go:2711-2733) -------------
     uint32_t met_w, fd_w;
-    const WalkCtx wctx{tab_a, grp_a + R * P.state_stride + (uint32_t)sizeof(TopoHeader), P.topo_buf_bytes, st0_a, st_stride};
+    const WalkCtx wctx{tab_a, grp_a + R * P.state_stride + (uint32_t)sizeof(TopoHeader), P.topo_buf_bytes, st0_a, st_run};
     if (mixed) {
       if (any_fd) walk_items_any<true>(lane, CAND, lg, wctx, met_w, fd_w);
       else walk_items_any<false>(lane, CAND, lg, wctx, met_w, fd_w);
-    } else if (fmt0 == FMT_ELL4B && Wq == 8u) {   // 129 .. 256 steps: status bytes on 256-byte boundaries
+    } else if (fmt0 == FMT_ELL4B && Wq == 8u) {   // 129 .. 256 steps: entries used in place in the row word
       if (any_fd) walk_items<FMT_ELL4B, true, true>(lane, CAND, lg, wctx, met_w, fd_w);
       else walk_items<FMT_ELL4B, false, true>(lane, CAND, lg, wctx, met_w, fd_w);
     } else if (fmt0 == FMT_ELL4B) {
@@ -541,13 +576,15 @@ __global__ void __launch_bounds__(32 * PACK_MAX_WARPS, PACK_MIN_BLOCKS) frontier
       else walk_items<FMT_CSRL, false>(lane, CAND, lg, wctx, met_w, fd_w);
     }
     met_w |= dc.FREE;
+    PROBE(3);
     load_cut(t + NG, 0u);   // the phase words and masks for the cut of the group I shall issue (issue() reduces them)
     uint32_t ready_w = met_w, skipc_w = 0, fail_w = 0;
     if (CD) {
-      // item L: word L & (Wq - 1) of run L >> lg, its rows and status bytes from the run's walk-table entry
+      // item L: word L & (Wq - 1) of run L >> lg, its rows and status pairs from the run's walk-table entry
       auto fixup = [&](uint32_t L, uint32_t candw, uint32_t fclass, uint32_t& mb, uint32_t& fb) {
         const uint4 te = lds_v4(tab_a + (L >> lg) * 16u);
-        fixup_item(lane, candw, L & ((1u << lg) - 1u), te.w >> 16, te.y, te.x, te.z, mfail_a + ((L >> lg) << lg) * 4u, fclass, mb, fb);
+        auto status = [&](uint32_t d) { const uint32_t s = dep_status(te.z, d, ~3u); return (s & ST_U) | ((s >> 15) & 2u); };
+        fixup_item(lane, candw, L & ((1u << lg) - 1u), te.w >> 16, te.y, te.x, status, mfail_a + ((L >> lg) << lg) * 4u, fclass, mb, fb);
       };
       stage_cond(lane, c0, c1, dc, mfail_a, true, 32u * Wmax, fixup, met_w, fd_w, ready_w, skipc_w, fail_w, p0, p1, p2, p3);
     }
@@ -587,7 +624,12 @@ __global__ void __launch_bounds__(32 * PACK_MAX_WARPS, PACK_MIN_BLOCKS) frontier
     lane_evals += (w == 0 && live) ? S : 0u;
 
     __syncwarp();  // every lane is done with this slot group's buffers
+    PROBE(4);
     issue(t + NG, cur_sg, cur_use + 1u, 0u);  // re-arm it with group t + NG (consumed by whichever warp draws that ticket)
+    PROBE(5);
+#ifdef PACK_STAGES
+    pr_acc += lane == 6u ? 1u : 0u;   // trips
+#endif
 #ifdef PACK_TRACE
     if (t == 0 && lane == 0 && blockIdx.x < 160) g_trace[tr_launch][blockIdx.x][1] = tr_first;
     tr_last = gtime();
@@ -595,6 +637,9 @@ __global__ void __launch_bounds__(32 * PACK_MAX_WARPS, PACK_MIN_BLOCKS) frontier
   }
 #ifdef PACK_TRACE
   if (lane == 0 && blockIdx.x < 160) atomicMax(&g_trace[tr_launch][blockIdx.x][2], tr_last);
+#endif
+#ifdef PACK_STAGES
+  if (lane < 7u) atomicAdd(&g_stages[lane], (unsigned long long)pr_acc);
 #endif
 
   // ---- BF_EVAL_PIPELINED: this grid may have started before the preceding kernel of the stream ended (it reads and writes
@@ -649,6 +694,13 @@ extern "C" int bf_debug_pack_trace(unsigned long long* out, unsigned int* launch
   cudaDeviceSynchronize();
   if (cudaMemcpyFromSymbol(out, g_trace, sizeof(g_trace)) != cudaSuccess) return -1;
   return cudaMemcpyFromSymbol(launch, g_launch, sizeof(unsigned int)) == cudaSuccess ? 0 : -1;
+}
+#endif
+#ifdef PACK_STAGES
+extern "C" int bf_debug_pack_stages(unsigned long long* out) {   // the totals since the last call, then zeroed
+  static const unsigned long long zero[8] = {};
+  if (cudaDeviceSynchronize() != cudaSuccess || cudaMemcpyFromSymbol(out, g_stages, sizeof(g_stages)) != cudaSuccess) return -1;
+  return cudaMemcpyToSymbol(g_stages, zero, sizeof(g_stages)) == cudaSuccess ? 0 : -1;
 }
 #endif
 

@@ -127,16 +127,17 @@ DI void sts_v4(uint32_t a, uint32_t x, uint32_t y, uint32_t z, uint32_t w) {
   asm volatile("st.shared.v4.u32 [%0], {%1, %2, %3, %4};" ::"r"(a), "r"(x), "r"(y), "r"(z), "r"(w) : "memory");
 }
 DI void red_or_shared(uint32_t a, uint32_t v) { asm volatile("red.shared.or.b32 [%0], %1;" ::"r"(a), "r"(v) : "memory"); }
-DI void sts_v2(uint32_t a, uint32_t x, uint32_t y) { asm volatile("st.shared.v2.u32 [%0], {%1, %2};" ::"r"(a), "r"(x), "r"(y) : "memory"); }
-// generic pointer of a shared-window address (rare paths only: parallel join, in-loop failure fix-up)
+DI void sts_v2(uint32_t a, uint32_t x, uint32_t y) { asm volatile("st.shared.v2.u32 [%0], {%1, %2};" ::"r"(a), "r"(x), "r"(y) : "memory"); }// generic pointer of a shared-window address (rare paths only: parallel join, in-loop failure fix-up)
 DI const uint8_t* gptr(uint32_t a) { return static_cast<const uint8_t*>(__cvta_shared_to_generic(a)); }
 // keep a loop-invariant value in a register instead of letting the compiler rematerialise it from constants
 DI uint32_t pin(uint32_t v) { asm volatile("" : "+r"(v)); return v; }
 
 // ------------------------------------------------------------------ stage D: the dependency walk
 // findReadySteps' inner loop (dag.go:2711-2733): one step per lane over the `needs` row of every candidate step,
-// visiting only the 32-step words that hold a candidate.  Status byte of a dependency: bit0 = not satisfied,
-// bit1 = failed dependency; the byte at index PAD = 32*W (just past the last step word) is always 0.
+// visiting only the 32-step words that hold a candidate.  The row formats and their fetch (row_locate, row_fetch) are
+// shared; how a dependency's status is kept is each kernel's own: the one-run-per-warp kernel (frontier_kernel.cu, the
+// walks below) keeps one status byte per step, bit0 = not satisfied, bit1 = failed dependency, with the byte at index
+// PAD = 32*W (just past the last step word) always 0; the packed-lanes kernel keeps bit words (frontier_pack.cu).
 //
 // Row formats (device_record.h), a compile-time parameter of the hot walks:
 //   FMT_CSR4   CSR, no row longer than 4: the first four entries are fetched branch-free and clamp-free (col_idx carries
@@ -191,9 +192,10 @@ DI void row_fetch(uint32_t p, uint32_t n, uint32_t (&x)[4]) {
   x[0] = lds_u16(p); x[1] = lds_u16(p + 2u);
   if (FMT != FMT_ELL2) { x[2] = lds_u16(p + 4u); x[3] = lds_u16(p + 6u); }
 }
-// phase 3: OR of the status bytes of the row's dependencies (CSR: one byte lane per entry, masked by the row length)
+// phase 3, one-run-per-warp kernel: OR of the status bytes of the row's dependencies (CSR: one byte lane per entry, masked by
+// the row length)
 template <int FMT>
-DI uint32_t row_status(uint32_t p, uint32_t n, const uint32_t (&x)[4], uint32_t st_addr) {
+DI uint32_t row_status_bytes(uint32_t p, uint32_t n, const uint32_t (&x)[4], uint32_t st_addr) {
   if (FMT == FMT_ELL2 || FMT == FMT_ELL2B) return lds_u8(st_addr + x[0]) | lds_u8(st_addr + x[1]);
   const uint32_t s0 = lds_u8(st_addr + x[0]), s1 = lds_u8(st_addr + x[1]), s2 = lds_u8(st_addr + x[2]), s3 = lds_u8(st_addr + x[3]);
   if (FMT == FMT_ELL4 || FMT == FMT_ELL4B || FMT == FMT_ELL4P) return s0 | s1 | s2 | s3;
@@ -224,7 +226,7 @@ DI void walk_group(uint32_t lane, uint32_t CAND, uint32_t& todo, uint32_t rp_add
 #pragma unroll
   for (int k = 0; k < K; ++k) row_fetch<FMT>(p[k], n[k], x[k]);
 #pragma unroll
-  for (int k = 0; k < K; ++k) w[k] = row_status<FMT>(p[k], n[k], x[k], st_addr);
+  for (int k = 0; k < K; ++k) w[k] = row_status_bytes<FMT>(p[k], n[k], x[k], st_addr);
 #pragma unroll
   for (int k = 0; k < K; ++k) {
     if (fmt_traits<FMT>::fixed) {   // every lane holds a real row: the (lane-uniform) candidate word masks the ballot
@@ -284,8 +286,10 @@ DI void walk_words_fmt(int fmt, uint32_t lane, uint32_t CAND, uint32_t rp_addr, 
 
 // ---- the fix-up walk (rare): a step set Failed earlier in this same loop (dag.go:2744/2810 mutate stepStates while
 // `completed` stays as built at :497) is visible to LATER steps of the list only.  Plain loop over every entry of the
-// row, any format.  The item (word j of the run whose CAND word is held by lane `owner`) is given by the caller.
-DI void fixup_item(uint32_t lane, uint32_t candw, uint32_t j, uint32_t ell, uint32_t rp_addr, uint32_t col_addr, uint32_t st_addr,
+// row, any format.  The item (word j of the run whose CAND word is held by lane `owner`) is given by the caller, and so is
+// `status(d)`: dependency d's status in the kernel's own representation, as bit0 = not satisfied, bit1 = failed dependency.
+template <class Status>
+DI void fixup_item(uint32_t lane, uint32_t candw, uint32_t j, uint32_t ell, uint32_t rp_addr, uint32_t col_addr, Status status,
                    uint32_t mfail_addr, uint32_t failed_class, uint32_t& metb, uint32_t& fdb) {
   const bool cand = (candw >> lane) & 1u;
   const uint32_t i = j * 32u + lane;
@@ -300,7 +304,7 @@ DI void fixup_item(uint32_t lane, uint32_t candw, uint32_t j, uint32_t ell, uint
     for (uint32_t e = 0; e < n; ++e) {
       const uint32_t d = (ell & ELL_PACK10) ? (e < 3u ? (lo10 >> (10u * e)) & 0x3FFu : (lo10 >> 30) | (hi10 << 2))
                                             : (eb == 1u ? lds_u8(p + e) : lds_u16(p + e * 2u));
-      uint32_t sb = lds_u8(st_addr + d);
+      uint32_t sb = status(d);
       if (d < i && ((lds_u32(mfail_addr + (d >> 5) * 4u) >> (d & 31u)) & 1u)) sb = failed_class;  // PAD >= i: never
       acc |= sb;
     }

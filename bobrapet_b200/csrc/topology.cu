@@ -108,8 +108,9 @@ int plan_record(const bf_topology& t, RecPlan& p, std::string& why, bool host_ka
     if (ell_rows <= 256 && forced != 2 && K * ell_rows + 4 * p.W <= csr_bytes) p.ell = K | bf::ELL_BYTE;
     // 10-bit entries: topologies of more than 512 steps (never staged by the packed-lanes kernel) with rows of up to 4 needs
     else if (K == 4 && p.W > 16 && forced != 2 && 5 * ell_rows + 4 * p.W <= csr_bytes) p.ell = 4 | bf::ELL_PACK10;
-    // (no u16 rows at 8 words: their PAD index 256 has no status byte — the packed kernel keeps a run's status bytes on a
-    //  256-byte stride there; such a topology has byte entries unless BF_TOPO_FORMAT forbids them, then CSR)
+    // (no u16 rows at 8 words: such a topology has byte entries unless BF_TOPO_FORMAT forbids them, then CSR.  The packed
+    //  kernel's status words read PAD = 256 as satisfied too, the zero pair behind a run's words; the rule keeps these
+    //  topologies' record format.)
     else if (2 * K * ell_rows <= csr_bytes && ell_rows != 256) p.ell = K;
   }
   if (p.ell) {
