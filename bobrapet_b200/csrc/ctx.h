@@ -262,6 +262,89 @@ inline int cuda_fail(bf_ctx* c, cudaError_t e, const char* what) {
     if (e__ != cudaSuccess) return bf::cuda_fail(c, e__, #call); \
   } while (0)
 
+// The per-run side areas of a resident batch, each with one entry per run of the capacity, or absent:
+//   d_timers, timer_k  step-timer slots (bf_resident_timers): timer_k slots per run, or none (timer_k = 0).  Arm and fire change
+//                      them.
+//   d_sched_in         limiter inputs (bf_resident_sched), or none.  Put changes them.
+//   d_sched_rec,       with the inputs: the records of the last bf_resident_schedule, BF_SCHED_STRIDE(words) bytes per run.  A run
+//   sched_base_runs    at or above sched_base_runs, or whose stored reason is kSchedNoBase, has no baseline.
+//   d_runctl           run-control records (bf_resident_runctl), or none.  Put and fire change them (a stop also rewrites the run's
+//                      flags byte, empties its timers and, for a timeout, sets its inputs' run_phase); deltas, uploads and redrives
+//                      honour them.
+// The calls that move or reset runs carry every area in the launches that handle the records, through view() (resident.cu):
+// retire and transfer move a run's entries with it and reset the ones it leaves, migrate re-keys its timers, redrive empties its
+// timers and lifts its stop, and a run that is moved, migrated or uploaded has no schedule baseline.  Reshape and a retire to a
+// new capacity allocate the areas anew (alloc_resized), fill them and adopt them; narrow keeps them (the capacity stays, and a
+// smaller stride fits the schedule records).  A change of words drops every schedule baseline (Resident::adopt).
+struct RunAreas {
+  DevBuf<unsigned long long> d_timers;
+  uint32_t timer_k = 0;
+  DevBuf<bf_sched_run> d_sched_in;
+  DevBuf<uint8_t> d_sched_rec;
+  uint32_t sched_base_runs = 0;
+  DevBuf<bf_run_ctl> d_runctl;
+
+  bf::RunAreasView view(uint32_t words) const {
+    return {d_timers, timer_k, d_sched_in, d_sched_rec, BF_SCHED_STRIDE(words), d_runctl};
+  }
+  // schedule records for `capacity` runs of `words` words, every run without a baseline (all bytes 0xFF: reason kSchedNoBase)
+  static cudaError_t alloc_sched_rec(DevBuf<uint8_t>& rec, uint32_t capacity, uint32_t words, cudaStream_t s) {
+    const size_t bytes = (size_t)capacity * BF_SCHED_STRIDE(words);
+    cudaError_t e = rec.alloc(bytes);
+    return e == cudaSuccess ? cudaMemsetAsync(rec, 0xFF, bytes, s) : e;
+  }
+  // Allocates into the empty set n, for `capacity` runs of `words` words, each area this set holds whose size changes from `cap`
+  // runs of `old_words`.  Schedule records that no copy from here fills (relay, copy_prefix) start without a baseline.  -> "" or
+  // the error of the failed allocation, naming its area; this set is unchanged either way.
+  std::string alloc_resized(RunAreas& n, uint32_t cap, uint32_t capacity, uint32_t old_words, uint32_t words, cudaStream_t s) const {
+    const bool resize = capacity != cap, relaid = resize || words != old_words;
+    cudaError_t e = cudaSuccess;
+    const char* area = "timers";
+    if (resize && timer_k) { e = n.d_timers.alloc((size_t)capacity * timer_k); n.timer_k = timer_k; }
+    if (e == cudaSuccess && resize && d_sched_in) { area = "limiter inputs"; e = n.d_sched_in.alloc(capacity); }
+    if (e == cudaSuccess && resize && d_runctl) { area = "run control"; e = n.d_runctl.alloc(capacity); }
+    if (e == cudaSuccess && relaid && d_sched_in) {
+      area = "schedule records";
+      e = capacity < cap && words == old_words ? n.d_sched_rec.alloc((size_t)capacity * BF_SCHED_STRIDE(words))
+                                               : alloc_sched_rec(n.d_sched_rec, capacity, words, s);
+    }
+    return e == cudaSuccess ? std::string() : std::string("(") + area + "): " + cudaGetErrorString(e);
+  }
+  // Reshape: the timers of n (alloc_resized from `cap` runs of `old_words`) take each run's slots from here, empty past cap (one
+  // relay launch, counted in launches), and with the words unchanged n's schedule records take the first cap runs' records.
+  // reshape_runs fills n's limiter inputs and run control.
+  cudaError_t relay(RunAreas& n, uint32_t cap, uint32_t capacity, uint32_t old_words, uint32_t words, cudaStream_t s,
+                    uint64_t& launches) const {
+    cudaError_t e = cudaSuccess;
+    if (n.d_sched_rec && words == old_words)
+      e = cudaMemcpyAsync(n.d_sched_rec, d_sched_rec, (size_t)cap * BF_SCHED_STRIDE(words), cudaMemcpyDeviceToDevice, s);
+    if (e == cudaSuccess && n.d_timers) {
+      e = bf::launch_relay_timers({d_timers, n.d_timers, capacity, cap, timer_k, timer_k}, s);
+      launches += 1;
+    }
+    return e;
+  }
+  // Retire to a smaller capacity: the first `capacity` runs of every area into n (alloc_resized), device to device.
+  cudaError_t copy_prefix(RunAreas& n, uint32_t capacity, uint32_t words, cudaStream_t s) const {
+    const auto copy = [&](void* to, const void* from, size_t per_run) {
+      return cudaMemcpyAsync(to, from, capacity * per_run, cudaMemcpyDeviceToDevice, s);
+    };
+    cudaError_t e = cudaSuccess;
+    if (timer_k) e = copy(n.d_timers, d_timers, (size_t)timer_k * 8);
+    if (e == cudaSuccess && d_sched_in) e = copy(n.d_sched_in, d_sched_in, sizeof(bf_sched_run));
+    if (e == cudaSuccess && d_sched_in) e = copy(n.d_sched_rec, d_sched_rec, BF_SCHED_STRIDE(words));
+    if (e == cudaSuccess && d_runctl) e = copy(n.d_runctl, d_runctl, sizeof(bf_run_ctl));
+    return e;
+  }
+  // takes every area n holds in place of this set's
+  void adopt(RunAreas&& n) {
+    if (n.d_timers) d_timers = std::move(n.d_timers);
+    if (n.d_sched_in) d_sched_in = std::move(n.d_sched_in);
+    if (n.d_sched_rec) d_sched_rec = std::move(n.d_sched_rec);
+    if (n.d_runctl) d_runctl = std::move(n.d_runctl);
+  }
+};
+
 // A device-resident batch (row f2), with the bookkeeping of touched ticks that tests/resident_model.py restates under the
 // same names.  Each field and the calls that change it:
 //   L, cap, d_state,   create, and reshape / retire / narrow (adopt).  d_state also: upload, deltas, migrate, redrive, retire.
@@ -286,17 +369,7 @@ inline int cuda_fail(bf_ctx* c, cudaError_t e, const char* what) {
 //   (transfer)         the source compacts as by retire (compact_to); the destination takes the arrivals as uploads (received).
 //   uploaded           merged [first, end) ranges, keyed by first, of the runs at or above full_runs uploaded since the last full
 //                      tick (note_uploaded); compact_to clips them; full_tick_done clears them.
-//   d_timers, timer_k  the step-timer area (bf_resident_timers): cap * timer_k slots, or none (timer_k = 0).  Arm and fire
-//                      change it; retire, transfer, migrate and redrive re-key it in the launches that move the records;
-//                      reshape and a retire to a new capacity re-allocate it; narrow keeps it (the capacity stays).
-//   d_sched_in,        the limiter inputs (bf_resident_sched): cap records, or none.  Put changes them; retire and transfer move
-//   d_sched_rec,       them with their runs; reshape and a retire to a new capacity re-allocate them.  d_sched_rec: the records
-//   sched_base_runs    of the last bf_resident_schedule, cap * BF_SCHED_STRIDE(L.words) bytes; a run at or above sched_base_runs,
-//                      or whose stored reason is kSchedNoBase (uploads, migrations, moves, arrivals), has no baseline.  A change of
-//                      words zeroes sched_base_runs.
-//   d_runctl           the run-control records (bf_resident_runctl): cap records, or none.  Put and fire change them (a stop also
-//                      rewrites the run's flags byte); deltas, uploads and redrives honour them; retire and transfer move them with
-//                      their runs; reshape and a retire to a new capacity re-allocate them; narrow and migrate leave them.
+//   areas              the per-run side areas (RunAreas): step timers, limiter inputs and schedule records, run control.
 //   ticked             runs covered by a tick since the last call that changed d_state (state_changed), or -1: none since.  A
 //                      resident schedule over n runs needs ticked >= n.
 //   single_ticked      runs covered by single-pass ticks since the last tick with BF_EVAL_FIXPOINT, or -1.  scheduled: runs covered
@@ -309,12 +382,7 @@ struct Resident {
   uint32_t cap = 0, prev_runs = 0, epoch = 1, full_epoch = 0, full_runs = 0, last_fixpoint = 0, last_max_iter = 0;
   DevBuf<uint8_t> d_state, d_result, d_result_prev;
   DevBuf<uint32_t> d_mark;
-  DevBuf<unsigned long long> d_timers;
-  uint32_t timer_k = 0;
-  DevBuf<bf_sched_run> d_sched_in;
-  DevBuf<uint8_t> d_sched_rec;
-  uint32_t sched_base_runs = 0;
-  DevBuf<bf_run_ctl> d_runctl;
+  RunAreas areas;
   int64_t ticked = -1, single_ticked = -1, scheduled = -1;
   uint64_t slot_changes_seen = 0, pending = 0;
   std::map<uint32_t, uint32_t> uploaded;
@@ -329,13 +397,7 @@ struct Resident {
     single_ticked = (flags & BF_EVAL_FIXPOINT) ? -1 : std::max<int64_t>(single_ticked, n_runs);
     scheduled = -1;
   }
-  uint32_t sched_stride() const { return BF_SCHED_STRIDE(L.words); }
-  // schedule records for `capacity` runs of `words` words, every run without a baseline (all bytes 0xFF: reason kSchedNoBase)
-  static cudaError_t alloc_sched_rec(DevBuf<uint8_t>& rec, uint32_t capacity, uint32_t words, cudaStream_t s) {
-    const size_t bytes = (size_t)capacity * BF_SCHED_STRIDE(words);
-    cudaError_t e = rec.alloc(bytes);
-    return e == cudaSuccess ? cudaMemsetAsync(rec, 0xFF, bytes, s) : e;
-  }
+  bf::RunAreasView areas_view() const { return areas.view(L.words); }
   // the runs [first, end) were uploaded: the part at or above full_runs, merged with the ranges it touches
   void note_uploaded(uint32_t first, uint32_t end) {
     uint32_t lo = std::max(first, full_runs), hi = end;
@@ -386,23 +448,26 @@ struct Resident {
     const cudaError_t e = d_result_prev ? cudaSuccess : d_result_prev.alloc((size_t)cap * L.result_stride);
     return e == cudaSuccess ? BF_OK : bf::fail(c, BF_ENOMEM, std::string("resident batch (second result buffer): ") + cudaGetErrorString(e));
   }
-  // the state, result and touch-mark buffers of a new batch (create), or of new ones a batch adopts (reshape, retire): a call
-  // that fails first frees them with its locals
+  // the state, result and touch-mark buffers of a new batch (create), or of new ones a batch adopts (reshape, retire, narrow): a
+  // call that fails first frees them with its locals
   cudaError_t alloc(const bf_layout& layout, uint32_t capacity) {
     cudaError_t e = d_state.alloc((size_t)capacity * layout.state_stride);
     if (e == cudaSuccess) e = d_result.alloc((size_t)capacity * layout.result_stride);
     return e == cudaSuccess ? d_mark.alloc(((size_t)capacity + 3) / 4 * 4) : e;   // padded: the list build reads four marks at a time
   }
-  // new buffers at a new layout and capacity; the second result buffer is allocated at the new size when next used
+  // new buffers at a new layout and capacity, with the side areas b holds (the others stay); the second result buffer is
+  // allocated at the new size when next used
   void adopt(Resident&& b, const bf_layout& layout, uint32_t capacity) {
     d_state = std::move(b.d_state); d_result = std::move(b.d_result); d_result_prev.reset(); d_mark = std::move(b.d_mark);
+    areas.adopt(std::move(b.areas));
+    if (layout.words != L.words) areas.sched_base_runs = 0;
     L = layout; cap = capacity;
   }
   // retire left the runs [0, m) of [0, N); moves[i] is the new index of run m + i, or kRetireNoMove.  A moved run counts as
   // uploaded at its new index, and its result record moved with it (a changed-only tick compares it with its own record).
   void compact_to(uint32_t m, uint32_t N, const std::vector<uint32_t>& moves) {
     full_runs = std::min(full_runs, m);
-    sched_base_runs = std::min(sched_base_runs, m);
+    areas.sched_base_runs = std::min(areas.sched_base_runs, m);
     uploaded.erase(uploaded.lower_bound(m), uploaded.end());
     for (auto& u : uploaded) u.second = std::min(u.second, m);
     for (uint32_t to : moves)

@@ -210,6 +210,17 @@ struct TouchedParams {
 };
 
 // resident.cu (row f2)
+// A resident batch's per-run side areas (RunAreas in ctx.h), as the launches that move, re-key or reset runs see them.  An
+// absent area is nullptr (and timer_k 0); sched_rec is present exactly when sched_in is.
+struct RunAreasView {
+  unsigned long long* timers;    // [capacity][timer_k] step-timer slots (bf_timer_slot)
+  uint32_t timer_k;
+  bf_sched_run* sched_in;        // [capacity] limiter inputs
+  uint8_t* sched_rec;            // [capacity][sched_stride] the last schedule records (reason kSchedNoBase: no baseline)
+  uint32_t sched_stride;
+  bf_run_ctl* runctl;            // [capacity] run-control records
+};
+
 struct DeltaParams {
   uint8_t* state;
   const bf_delta* deltas;
@@ -238,11 +249,9 @@ struct MigrateParams {
   uint32_t n_runs, old_slot, new_slot;
   uint32_t words, state_stride, off_phase, off_cond, off_decision, off_child;
   uint32_t child_nibbles;        // of the layout; the child area is ceil(child_nibbles / 8) u32 words
-  unsigned long long* timers;    // [capacity][timer_k] the batch's timer slots (bf_timer_slot), or nullptr: no area
+  RunAreasView areas;            // a migrated run's timer slots are re-keyed through fwd, and its schedule record has no baseline
   const uint16_t* fwd;           // [n_old_steps] the step map (new index of old step i, or BF_MIGRATE_GONE), for the timers
-  uint32_t timer_k, n_old_steps;
-  uint8_t* sched_rec;            // [capacity][sched_stride] the last schedule records (kSchedNoBase), or nullptr: no area
-  uint32_t sched_stride;
+  uint32_t n_old_steps;
 };
 
 // bf_resident_redrive (resident.cu): the reset sets of the requests are cleared in the records of their runs
@@ -257,9 +266,7 @@ struct RedriveParams {
   const Slot* slots;
   uint32_t n;
   uint32_t words, state_stride, off_phase, off_cond, off_decision, off_child;
-  unsigned long long* timers;    // [capacity][timer_k] timer slots, or nullptr: an applied request empties its run's
-  uint32_t timer_k;
-  bf_run_ctl* runctl;            // [capacity] run-control records, or nullptr: an applied request lifts its run's stop
+  RunAreasView areas;            // an applied request empties its run's timer slots and lifts its stop
 };
 
 // bf_resident_reshape (resident.cu): both record arrays re-laid from layout `from` into new buffers at layout `to`
@@ -270,10 +277,8 @@ struct ReshapeParams {
   uint8_t* result;               // [n_new][to.result_stride]
   uint32_t n_old, n_new;         // runs r >= n_old get zero records
   bf_layout from, to;
-  const bf_sched_run* old_sched_in;   // the limiter inputs, or nullptr: no area (runs r >= n_old get kSchedDefault)
-  bf_sched_run* sched_in;             // [n_new]
-  const bf_run_ctl* old_runctl;       // run-control records, or nullptr: no area (runs r >= n_old get kRunCtlDefault)
-  bf_run_ctl* runctl;                 // [n_new]
+  RunAreasView old_areas;        // areas holds the limiter inputs and run control of a new capacity, or none: runs r < n_old keep
+  RunAreasView areas;            // theirs, the others get the defaults (its timers and schedule records are filled by the host)
 };
 
 // bf_resident_retire (resident.cu): the runs [m, m + n) vacate their indices; the live ones among them move below m
@@ -286,63 +291,50 @@ struct RetireParams {
   const uint32_t* to;            // [n] the new index of run m + i, or kRetireNoMove for a retired run
   uint32_t m, n;
   uint32_t state_stride, result_stride;   // multiples of 16
-  unsigned long long* timers;    // [capacity][timer_k] timer slots, or nullptr: a mover's slots move with it, vacated ones empty
-  uint32_t timer_k;
-  bf_sched_run* sched_in;        // [capacity] limiter inputs, or nullptr: a mover's move with it, vacated ones get kSchedDefault
-  uint8_t* sched_rec;            // [capacity][sched_stride] last schedule records: a mover's target loses its baseline
-  uint32_t sched_stride;
-  bf_run_ctl* runctl;            // [capacity] run-control records, or nullptr: a mover's move with it, vacated ones get kRunCtlDefault
+  RunAreasView areas;            // a mover's entries move with it (its target has no schedule baseline), vacated ones are reset
 };
 
 // bf_resident_extent / _narrow (resident.cu): the smallest layout a batch's records and the topologies of its runs allow.  Each
 // extent is reduced into out[] as extent << 32 | ~index, so that one 64-bit atomicMax keeps the largest extent and the lowest
 // index that needs it.
-struct ExtentParams {
-  const uint8_t* state;          // [n_records][L.state_stride]
-  const uint8_t* result;         // [n_runs][L.result_stride]: the current result records
+// The batch whose runs' extents are taken (extent_runs, transfer_fit): a run's state record and timer slots always count (an armed
+// step s needs s + 1 steps, a non-PENDING code BF_F_DECISION); its result record counts when a later tick may compare with it.
+struct ExtentBatch {
+  const uint8_t* state;          // [capacity][L.state_stride]
+  const uint8_t* result;         // [capacity][L.result_stride]: the current result records
   const uint32_t* mark;          // touch marks (Resident in ctx.h)
+  RunAreasView areas;
   const Slot* slots;
   uint32_t n_slots;
-  uint32_t n_records;            // state records scanned (the capacity)
-  uint32_t n_runs;               // runs whose slot counts, and whose result record counts when a later tick may compare with it:
-  uint32_t prev_runs;            //   run r < prev_runs (the changed-only baseline), or
+  uint32_t prev_runs;            // a result record counts for run r < prev_runs (the changed-only baseline), or for
   uint32_t eval_runs;            //   run r < eval_runs (the touched baseline) not marked "must list" after full_epoch
   uint32_t full_epoch;
   bf_layout L;                   // the batch's layout
   bf_layout R;                   // L with the result fields that do not count set to BF_OFF_NONE
-  unsigned long long* out;       // [3], zeroed by the caller: steps, child nibbles (both extent << 32 | ~index), BF_F_* input fields
-  const unsigned long long* timers;   // [n_records][timer_k] timer slots, or nullptr: an armed step s counts s + 1, a non-PENDING
-  uint32_t timer_k;                   //   code BF_F_DECISION
 };
 
-// bf_resident_transfer (resident.cu): runs[i] of the source batch (layout F) is checked against the destination layout T
+struct ExtentParams {
+  ExtentBatch B;
+  uint32_t n_records;            // state records scanned (the capacity)
+  uint32_t n_runs;               // runs whose slot and result record count
+  unsigned long long* out;       // [3], zeroed by the caller: steps, child nibbles (both extent << 32 | ~index), BF_F_* input fields
+};
+
+// bf_resident_transfer (resident.cu): runs[i] of the source batch (layout src.L) is checked against the destination layout T
 // (transfer_fit), then re-laid into destination record dst_first + i (transfer_runs).  The source's compaction is retire_runs.
 struct TransferParams {
-  const uint8_t* src_state;
-  const uint8_t* src_result;     // the source's current result records
-  const uint32_t* src_mark;
+  ExtentBatch src;               // src.R: the result fields T keeps
   uint8_t* dst_state;
   uint8_t* dst_result;
   uint32_t* dst_mark;            // an arrival's becomes mark_value (touched and must be listed)
   uint32_t mark_value;
+  RunAreasView dst_areas;        // an arrival's entries, or the defaults where the source has no area.  A run with more armed slots
+                                 // than dst_areas.timer_k, or with run control other than the default and no area here, is unfit
   const uint32_t* runs;          // [n] source indices
   uint32_t n, dst_first;
-  const Slot* slots;
-  uint32_t n_slots;
-  uint32_t prev_runs, eval_runs, full_epoch;   // the source's baselines: which result records count (ExtentParams)
-  bf_layout F, T;
-  bf_layout R;                   // F with the result fields T lacks set to BF_OFF_NONE
-  uint4* extent;                 // [n] out: steps, child nibbles, BF_F_* input fields of each run
+  bf_layout T;
+  uint4* extent;                 // [n] out: steps, child nibbles, BF_F_* input fields, armed slots | 1 << 31 for lost run control
   uint32_t* unfit;               // [1] the lowest i that T cannot hold (atomicMin; 0xFFFFFFFF from the caller)
-  const unsigned long long* src_timers;   // [src capacity][src_k] or nullptr
-  unsigned long long* dst_timers;         // [dst capacity][dst_k] or nullptr: an arrival's armed slots, the rest empty
-  uint32_t src_k, dst_k;                  // a run with more armed slots than dst_k is unfit
-  const bf_sched_run* src_sched_in;       // limiter inputs, or nullptr (an arrival gets kSchedDefault)
-  bf_sched_run* dst_sched_in;             // or nullptr: the destination has no area (then neither has the source)
-  uint8_t* dst_sched_rec;                 // [dst capacity][dst_sched_stride]: an arrival has no baseline
-  uint32_t dst_sched_stride;
-  const bf_run_ctl* src_runctl;           // run-control records, or nullptr (an arrival gets kRunCtlDefault)
-  bf_run_ctl* dst_runctl;                 // or nullptr: a run whose record is not the default is unfit (extent.w bit 31)
 };
 
 // step timers (resident.cu): slot = deadline | step << 32 | code << 48 (bf_timer_slot read as one little-endian u64); an empty
@@ -376,17 +368,16 @@ struct TimerArmParams {
 // bf_resident_fire: one thread per run, a warp per chunk of 32 runs
 struct FireParams {
   uint8_t* state;
-  unsigned long long* timers;
+  RunAreasView areas;              // timer slots; run control, or none: no story or drain deadlines (then timers are set); limiter
+                                   // inputs, or none: a story timeout sets its run's run_phase to BF_PHASE_TIMEOUT
   uint32_t* mark;                  // a run whose code was written is raised to mark_value, as by a delta
   uint32_t mark_value;
-  uint32_t n_runs, timer_k, now;
+  uint32_t n_runs, now;
   uint32_t words, state_stride, off_phase, off_decision;
   uint32_t* block_sums;            // [blocks] fired timers per block (fire_count), read by fire_apply for its offsets
   uint32_t* out;                   // [4] n_fired, n_written, n_pruned, next_deadline (fire_count initialises them)
   bf_fired* fired;                 // [fired_cap]
   uint32_t fired_cap;
-  bf_run_ctl* runctl;              // [n_runs] run-control records, or nullptr: no story or drain deadlines (timers must be set)
-  bf_sched_run* sched_in;          // limiter inputs, or nullptr: a story timeout sets its run's run_phase to BF_PHASE_TIMEOUT
 };
 
 // limiters.cu (rows a9 / f4)
@@ -444,11 +435,9 @@ constexpr bf_run_ctl kRunCtlDefault = {0xFFFFFFFFu, 0xFFFFFFFFu, 0u, 0u, {0u, 0u
 constexpr uint32_t kStoppedFlags = BF_RF_HOST_GROUP | (uint32_t)BF_GROUP_DONE << BF_RF_HOST_GROUP_SHIFT;
 
 // What a stop needs besides the record and its run-control record: the batch's timer slots (emptied), its limiter inputs (a
-// timeout's run_phase), its touch marks (touched as by a delta).  Each may be nullptr but mark.
+// timeout's run_phase), its touch marks (touched as by a delta).
 struct StopParams {
-  unsigned long long* timers;
-  uint32_t timer_k;
-  bf_sched_run* sched_in;
+  RunAreasView areas;
   uint32_t* mark;
   uint32_t mark_value;
 };

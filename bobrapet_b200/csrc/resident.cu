@@ -31,6 +31,40 @@ DI bool runctl_default(const bf_run_ctl& c) {
 }
 DI bool deadline_due(uint32_t d, uint32_t now) { return d != BF_TIMER_NONE && d <= now; }
 
+// ---- a run's side areas (RunAreasView) in the launches that move or reset runs: one warp per run ------------------------------
+// The lanes share the timer slots (lane t takes slots t, t + 32); lane 0 writes the one-record areas.
+DI void drop_baseline(const RunAreasView& A, uint32_t r) {   // run r's schedule record has no baseline
+  if (A.sched_rec) *reinterpret_cast<uint32_t*>(A.sched_rec + (size_t)r * A.sched_stride + 12) = kSchedNoBase;
+}
+DI void empty_timers(const RunAreasView& A, uint32_t r, uint32_t lane) {
+  for (uint32_t k = lane; A.timers && k < A.timer_k; k += 32u) A.timers[(size_t)r * A.timer_k + k] = kTimerEmpty;
+}
+// Run r is vacated: its timer slots empty, its limiter inputs and run control at the defaults.
+DI void vacate_areas(const RunAreasView& A, uint32_t r, uint32_t lane) {
+  empty_timers(A, r, lane);
+  if (lane == 0 && A.sched_in) A.sched_in[r] = kSchedDefault;
+  if (lane == 0 && A.runctl) A.runctl[r] = kRunCtlDefault;
+}
+// Run r of S arrives at index `to` of D (S may be D: a move within a batch).  Its armed slots lead its slots and number at most
+// D.timer_k (transfer_fit): they are copied in order, empty slots behind them.  Its limiter inputs and run control are copied,
+// or set to the defaults where S has no area, and its schedule record at `to` has no baseline.  Each lane reads the same slots
+// of r that vacate_areas has it empty, so a move may vacate r behind it.
+DI void arrive_areas(const RunAreasView& S, uint32_t r, const RunAreasView& D, uint32_t to, uint32_t lane) {
+  for (uint32_t k = lane; D.timers && k < D.timer_k; k += 32u)
+    D.timers[(size_t)to * D.timer_k + k] = S.timers && k < S.timer_k ? S.timers[(size_t)r * S.timer_k + k] : kTimerEmpty;
+  if (lane != 0) return;
+  if (D.sched_in) {
+    D.sched_in[to] = S.sched_in ? S.sched_in[r] : kSchedDefault;
+    drop_baseline(D, to);
+  }
+  if (D.runctl) D.runctl[to] = S.runctl ? S.runctl[r] : kRunCtlDefault;
+}
+// Reshape (lane 0): run r of the new limiter inputs and run control keeps its old entries (keep), else takes the defaults.
+DI void keep_areas(const RunAreasView& from, const RunAreasView& to, uint32_t r, bool keep) {
+  if (to.sched_in) to.sched_in[r] = keep ? from.sched_in[r] : kSchedDefault;
+  if (to.runctl) to.runctl[r] = keep ? from.runctl[r] : kRunCtlDefault;
+}
+
 // Stops run `run` (record rec, run-control record ctl) for `reason`, unless it is stopped already: saves its flags byte, writes
 // the stopped byte, empties its step-timer slots, marks the run touched and, for a timeout, sets its limiter inputs' run_phase.
 // The caller is the only thread writing this run's records in its launch.  -> 1 when the run was stopped now
@@ -39,8 +73,9 @@ DI uint32_t stop_run(uint8_t* rec, bf_run_ctl* ctl, uint32_t run, uint32_t reaso
   ctl->saved_flags = rec[4];
   ctl->stop = (uint8_t)reason;
   set_byte(rec, 4u, 0xFFu, kStoppedFlags);
-  for (uint32_t k = 0; S.timers && k < S.timer_k; ++k) S.timers[(size_t)run * S.timer_k + k] = kTimerEmpty;
-  if (reason == BF_STOP_TIMEOUT && S.sched_in) S.sched_in[run].run_phase = BF_PHASE_TIMEOUT;
+  const RunAreasView& A = S.areas;
+  for (uint32_t k = 0; A.timers && k < A.timer_k; ++k) A.timers[(size_t)run * A.timer_k + k] = kTimerEmpty;
+  if (reason == BF_STOP_TIMEOUT && A.sched_in) A.sched_in[run].run_phase = BF_PHASE_TIMEOUT;
   atomicMax(S.mark + run, S.mark_value);   // max: an upload's "must list" bit stays
   return 1u;
 }
@@ -182,12 +217,13 @@ __host__ __device__ inline uint32_t migrate_stage_words(const MigrateParams& P) 
 // gone step, or one past the map, cancels the slot), ranks the survivors by their new step (the map is injective: no ties) and,
 // after every lane has read, stores them in that order with empty slots behind.
 DI void migrate_timers(const MigrateParams& P, uint32_t run, uint32_t lane) {
-  unsigned long long* t = P.timers + (size_t)run * P.timer_k;
+  const uint32_t K = P.areas.timer_k;
+  unsigned long long* t = P.areas.timers + (size_t)run * K;
   unsigned long long v[2];
   uint32_t to[2];
   for (uint32_t h = 0; h < 2; ++h) {
     const uint32_t k = lane + 32u * h;
-    v[h] = k < P.timer_k ? t[k] : kTimerEmpty;
+    v[h] = k < K ? t[k] : kTimerEmpty;
     to[h] = BF_MIGRATE_GONE;
     if (timer_armed(v[h])) {
       const uint32_t s = timer_step(v[h]);
@@ -205,7 +241,7 @@ DI void migrate_timers(const MigrateParams& P, uint32_t run, uint32_t lane) {
   for (uint32_t h = 0; h < 2; ++h) {
     const uint32_t k = lane + 32u * h;
     if (to[h] != BF_MIGRATE_GONE) t[rank[h]] = (v[h] & ~(0xFFFFull << 32)) | (unsigned long long)to[h] << 32;
-    if (k >= kept && k < P.timer_k) t[k] = kTimerEmpty;
+    if (k >= kept && k < K) t[k] = kTimerEmpty;
   }
 }
 
@@ -264,9 +300,9 @@ __global__ void __launch_bounds__(256) migrate_runs(const MigrateParams P) {
         child[md.new_first / 8u + i] = v;
       }
     }
-    if (P.timers) migrate_timers(P, run, lane);
+    if (P.areas.timers) migrate_timers(P, run, lane);
     if (lane == 0) {
-      if (P.sched_rec) *reinterpret_cast<uint32_t*>(P.sched_rec + (size_t)run * P.sched_stride + 12) = kSchedNoBase;
+      drop_baseline(P.areas, run);
       *reinterpret_cast<uint32_t*>(rec) = P.new_slot;
       *reinterpret_cast<uint64_t*>(rec + 8) = reg_new;
       P.mark[run] = P.mark_value;
@@ -310,8 +346,7 @@ __global__ void __launch_bounds__(256) redrive_runs(const RedriveParams P) {
   const bool hit = *reinterpret_cast<const uint32_t*>(rec) == q.slot;   // no request of this launch writes the slot word
   if (lane == 0) P.status[i] = hit ? 1u : 0u;
   if (!hit) return;
-  if (P.timers)   // the whole step-timer annotation goes (storyrun_controller.go:477-478, :524-525)
-    for (uint32_t k = lane; k < P.timer_k; k += 32u) P.timers[(size_t)q.run * P.timer_k + k] = kTimerEmpty;
+  empty_timers(P.areas, q.run, lane);   // the whole step-timer annotation goes (storyrun_controller.go:477-478, :524-525)
   const uint8_t* topo = reinterpret_cast<const uint8_t*>(P.slots[q.slot].addr);
   const TopoHeader* th = reinterpret_cast<const TopoHeader*>(topo);
   const uint32_t S = th->S, TW = th->W, W = P.words, key = P.key[i];
@@ -355,8 +390,8 @@ __global__ void __launch_bounds__(256) redrive_runs(const RedriveParams P) {
   if (lane == 0) {
     const unsigned long long gone = (unsigned long long)reg[1] << 32 | reg[0];
     if (gone) atomicAnd(reinterpret_cast<unsigned long long*>(rec + 8), ~gone);
-    if (P.runctl) {   // the stop goes (one exchange: of two requests of a run, one restores), the drain deadline too
-      bf_run_ctl* ctl = P.runctl + q.run;
+    if (P.areas.runctl) {   // the stop goes (one exchange: of two requests of a run, one restores), the drain deadline too
+      bf_run_ctl* ctl = P.areas.runctl + q.run;
       const uint32_t was = atomicExch(reinterpret_cast<uint32_t*>(ctl) + 2, 0u);   // stop | saved_flags << 8
       if (was & 0xFFu) set_byte(rec, 4u, 0xFFu, (was >> 8) & 0xFFu);
       ctl->drain_deadline = BF_TIMER_NONE;
@@ -425,8 +460,7 @@ __global__ void __launch_bounds__(256) reshape_runs(const ReshapeParams P) {
   s = reinterpret_cast<const uint32_t*>(P.old_result + (size_t)r * P.from.result_stride);
   d = reinterpret_cast<uint32_t*>(P.result + (size_t)r * P.to.result_stride);
   for (uint32_t o = lane * 4u; o < P.to.result_stride; o += 128u) d[o >> 2] = keep ? reshape_result_word(s, o, P.from, P.to) : 0u;
-  if (P.sched_in && lane == 0) P.sched_in[r] = keep ? P.old_sched_in[r] : kSchedDefault;
-  if (P.runctl && lane == 0) P.runctl[r] = keep ? P.old_runctl[r] : kRunCtlDefault;
+  if (lane == 0) keep_areas(P.old_areas, P.areas, r, keep);
 }
 
 cudaError_t launch_reshape(const ReshapeParams& P, cudaStream_t stream) {
@@ -436,9 +470,10 @@ cudaError_t launch_reshape(const ReshapeParams& P, cudaStream_t stream) {
 }
 
 // Retire (bf_resident_retire).  One warp per vacated index m + i: when the run there lives on, the warp copies its state record
-// and current result record to its target (16-byte accesses, lane t takes vectors t, t + 32, ...) and lane 0 marks the target;
-// then the warp zeroes the vacated state record and its mark.  Targets lie below m and vacated indices at or above it, and
-// each lane zeroes only the vectors it read itself, so no warp reads what another writes.
+// and current result record to its target (16-byte accesses, lane t takes vectors t, t + 32, ...) and its side areas, and lane 0
+// marks the target; then the warp zeroes the vacated state record and its mark and vacates its areas.  Targets lie below m and
+// vacated indices at or above it, and each lane zeroes only the vectors and slots it read itself, so no warp reads what another
+// writes.
 __global__ void __launch_bounds__(256) retire_runs(const RetireParams P) {
   const uint32_t i = blockIdx.x * 8u + (threadIdx.x >> 5), lane = threadIdx.x & 31u;
   if (i >= P.n) return;
@@ -451,27 +486,11 @@ __global__ void __launch_bounds__(256) retire_runs(const RetireParams P) {
     uint4* rd = reinterpret_cast<uint4*>(P.result + (size_t)to * P.result_stride);
     for (uint32_t k = lane; k < (P.result_stride >> 4); k += 32u) rd[k] = rs[k];
     if (lane == 0) P.mark[to] = P.mark_value;
+    arrive_areas(P.areas, from, P.areas, to, lane);
   }
   for (uint32_t k = lane; k < sv; k += 32u) s[k] = make_uint4(0u, 0u, 0u, 0u);
   if (lane == 0) P.mark[from] = 0u;
-  if (P.sched_in && lane == 0) {   // a mover's inputs move with it and its target has no baseline; the vacated index gets the defaults
-    if (to != kRetireNoMove) {
-      P.sched_in[to] = P.sched_in[from];
-      *reinterpret_cast<uint32_t*>(P.sched_rec + (size_t)to * P.sched_stride + 12) = kSchedNoBase;
-    }
-    P.sched_in[from] = kSchedDefault;
-  }
-  if (P.runctl && lane == 0) {
-    if (to != kRetireNoMove) P.runctl[to] = P.runctl[from];
-    P.runctl[from] = kRunCtlDefault;
-  }
-  if (P.timers) {   // each lane stores over only the slots it read itself
-    unsigned long long* ts = P.timers + (size_t)from * P.timer_k;
-    for (uint32_t k = lane; k < P.timer_k; k += 32u) {
-      if (to != kRetireNoMove) P.timers[(size_t)to * P.timer_k + k] = ts[k];
-      ts[k] = kTimerEmpty;
-    }
-  }
+  vacate_areas(P.areas, from, lane);
 }
 
 cudaError_t launch_retire(const RetireParams& P, cudaStream_t stream) {
@@ -534,11 +553,44 @@ DI uint32_t timer_extent(const unsigned long long* t, uint32_t K, uint32_t lane,
   return armed;
 }
 
-// One warp per record, grid-stride: lane t reads the 16-byte vectors t, t + 32, ... of the state record (and of the result record
-// of a run below n_runs that a later tick may compare with), so a warp streams each record once with coalesced loads; lane 0 adds the S and the child area of the
-// run's topology when its slot is alive.  Warp reductions, then each warp folds its record's extents into its running maxima (its
-// records ascend, so the running maximum keeps the lowest index), the CTA's warps meet in shared memory and one thread per CTA
-// adds the CTA's three words to P.out.
+// The extent of run r of B (one warp; each lane's part, which the caller reduces): lane t reads the 16-byte vectors t, t + 32, ...
+// of its state record and slots t, t + 32 of its timers; when r is a run, also of its result record when a later tick compares
+// with it (the fields B.R places), and lane 0 adds the S and the child area of its topology when its slot is alive.  -> the
+// armed slots this lane saw
+DI uint32_t run_extent(const ExtentBatch& B, uint32_t r, bool is_run, uint32_t lane, uint32_t& steps, uint32_t& child, uint32_t& fields) {
+  const uint8_t* s = B.state + (size_t)r * B.L.state_stride;
+  for (uint32_t o = lane * 16u; o < B.L.state_stride; o += 512u) {
+    const uint4 q = *reinterpret_cast<const uint4*>(s + o);
+    state_word_extent(B.L, o, q.x, steps, child, fields);
+    state_word_extent(B.L, o + 4u, q.y, steps, child, fields);
+    state_word_extent(B.L, o + 8u, q.z, steps, child, fields);
+    state_word_extent(B.L, o + 12u, q.w, steps, child, fields);
+  }
+  const RunAreasView& A = B.areas;
+  const uint32_t armed = A.timers ? timer_extent(A.timers + (size_t)r * A.timer_k, A.timer_k, lane, steps, fields) : 0u;
+  if (!is_run) return armed;
+  const uint32_t m = B.mark[r];
+  const bool baseline = r < B.prev_runs || (r < B.eval_runs && !((m & 1u) && (m >> 1) > B.full_epoch));
+  const uint8_t* res = B.result + (size_t)r * B.L.result_stride;
+  for (uint32_t o = lane * 16u; baseline && o < B.L.result_stride; o += 512u) {
+    const uint4 q = *reinterpret_cast<const uint4*>(res + o);
+    steps = max(steps, max(max(result_word_extent(B.R, o, q.x), result_word_extent(B.R, o + 4u, q.y)),
+                           max(result_word_extent(B.R, o + 8u, q.z), result_word_extent(B.R, o + 12u, q.w))));
+  }
+  if (lane == 0) {
+    const uint32_t slot = *reinterpret_cast<const uint32_t*>(s);
+    const Slot sl = slot < B.n_slots ? B.slots[slot] : Slot{};
+    if (sl.addr) {
+      steps = max(steps, sl.meta & 0xFFFFu);
+      child = max(child, (uint32_t)reinterpret_cast<const TopoHeader*>(sl.addr)->child_nibbles);
+    }
+  }
+  return armed;
+}
+
+// One warp per record, grid-stride, each record streamed once with coalesced loads (run_extent; the runs are those below n_runs).
+// Warp reductions, then each warp folds its record's extents into its running maxima (its records ascend, so the running maximum
+// keeps the lowest index), the CTA's warps meet in shared memory and one thread per CTA adds the CTA's three words to P.out.
 __global__ void __launch_bounds__(256) extent_runs(const ExtentParams P) {
   __shared__ unsigned long long cta[3];
   if (threadIdx.x < 3) cta[threadIdx.x] = 0ull;
@@ -548,33 +600,7 @@ __global__ void __launch_bounds__(256) extent_runs(const ExtentParams P) {
   uint32_t all_fields = 0u;
   for (uint32_t r = blockIdx.x * 8u + (threadIdx.x >> 5); r < P.n_records; r += warps) {
     uint32_t steps = 0u, child = 0u, fields = 0u;
-    const uint8_t* s = P.state + (size_t)r * P.L.state_stride;
-    for (uint32_t o = lane * 16u; o < P.L.state_stride; o += 512u) {
-      const uint4 q = *reinterpret_cast<const uint4*>(s + o);
-      state_word_extent(P.L, o, q.x, steps, child, fields);
-      state_word_extent(P.L, o + 4u, q.y, steps, child, fields);
-      state_word_extent(P.L, o + 8u, q.z, steps, child, fields);
-      state_word_extent(P.L, o + 12u, q.w, steps, child, fields);
-    }
-    if (P.timers) timer_extent(P.timers + (size_t)r * P.timer_k, P.timer_k, lane, steps, fields);
-    if (r < P.n_runs) {
-      const uint32_t m = P.mark[r];
-      const bool baseline = r < P.prev_runs || (r < P.eval_runs && !((m & 1u) && (m >> 1) > P.full_epoch));
-      const uint8_t* res = P.result + (size_t)r * P.L.result_stride;
-      for (uint32_t o = lane * 16u; baseline && o < P.L.result_stride; o += 512u) {
-        const uint4 q = *reinterpret_cast<const uint4*>(res + o);
-        steps = max(steps, max(max(result_word_extent(P.R, o, q.x), result_word_extent(P.R, o + 4u, q.y)),
-                               max(result_word_extent(P.R, o + 8u, q.z), result_word_extent(P.R, o + 12u, q.w))));
-      }
-      if (lane == 0) {
-        const uint32_t slot = *reinterpret_cast<const uint32_t*>(s);
-        const Slot sl = slot < P.n_slots ? P.slots[slot] : Slot{};
-        if (sl.addr) {
-          steps = max(steps, sl.meta & 0xFFFFu);
-          child = max(child, (uint32_t)reinterpret_cast<const TopoHeader*>(sl.addr)->child_nibbles);
-        }
-      }
-    }
+    run_extent(P.B, r, r < P.n_runs, lane, steps, child, fields);
     steps = __reduce_max_sync(FULL, steps);
     child = __reduce_max_sync(FULL, child);
     all_fields |= __reduce_or_sync(FULL, fields);
@@ -602,39 +628,14 @@ cudaError_t launch_extent(const ExtentParams& P, uint32_t sm_count, cudaStream_t
   return cudaGetLastError();
 }
 
-// Transfer (bf_resident_transfer), fit check.  One warp per listed run: the extent of its state record, of its result record when
-// a later tick of the source compares with it (counting the planes T keeps), and of its slot when alive, as extent_runs takes
-// them.  Lane 0 stores the run's extent and, when T cannot hold it, lowers P.unfit to its position.
+// Transfer (bf_resident_transfer), fit check.  One warp per listed run: its extent as extent_runs takes it (run_extent, counting
+// the result planes T keeps).  Lane 0 stores the run's extent and, when T cannot hold it, lowers P.unfit to its position.
 __global__ void __launch_bounds__(256) transfer_fit(const TransferParams P) {
   const uint32_t i = blockIdx.x * 8u + (threadIdx.x >> 5), lane = threadIdx.x & 31u;
   if (i >= P.n) return;
   const uint32_t r = P.runs[i];
   uint32_t steps = 0u, child = 0u, fields = 0u;
-  const uint8_t* s = P.src_state + (size_t)r * P.F.state_stride;
-  for (uint32_t o = lane * 16u; o < P.F.state_stride; o += 512u) {
-    const uint4 q = *reinterpret_cast<const uint4*>(s + o);
-    state_word_extent(P.F, o, q.x, steps, child, fields);
-    state_word_extent(P.F, o + 4u, q.y, steps, child, fields);
-    state_word_extent(P.F, o + 8u, q.z, steps, child, fields);
-    state_word_extent(P.F, o + 12u, q.w, steps, child, fields);
-  }
-  uint32_t armed = P.src_timers ? timer_extent(P.src_timers + (size_t)r * P.src_k, P.src_k, lane, steps, fields) : 0u;
-  const uint32_t m = P.src_mark[r];
-  const bool baseline = r < P.prev_runs || (r < P.eval_runs && !((m & 1u) && (m >> 1) > P.full_epoch));
-  const uint8_t* res = P.src_result + (size_t)r * P.F.result_stride;
-  for (uint32_t o = lane * 16u; baseline && o < P.F.result_stride; o += 512u) {
-    const uint4 q = *reinterpret_cast<const uint4*>(res + o);
-    steps = max(steps, max(max(result_word_extent(P.R, o, q.x), result_word_extent(P.R, o + 4u, q.y)),
-                           max(result_word_extent(P.R, o + 8u, q.z), result_word_extent(P.R, o + 12u, q.w))));
-  }
-  if (lane == 0) {
-    const uint32_t slot = *reinterpret_cast<const uint32_t*>(s);
-    const Slot sl = slot < P.n_slots ? P.slots[slot] : Slot{};
-    if (sl.addr) {
-      steps = max(steps, sl.meta & 0xFFFFu);
-      child = max(child, (uint32_t)reinterpret_cast<const TopoHeader*>(sl.addr)->child_nibbles);
-    }
-  }
+  uint32_t armed = run_extent(P.src, r, true, lane, steps, child, fields);
   steps = __reduce_max_sync(FULL, steps);
   child = __reduce_max_sync(FULL, child);
   fields = __reduce_or_sync(FULL, fields);
@@ -643,36 +644,32 @@ __global__ void __launch_bounds__(256) transfer_fit(const TransferParams P) {
     const bf_layout& T = P.T;
     const uint32_t placed = (T.off_cond != BF_OFF_NONE ? BF_F_COND : 0u) | (T.off_decision != BF_OFF_NONE ? BF_F_DECISION : 0u) |
                             (T.off_child != BF_OFF_NONE ? BF_F_CHILD : 0u);
-    const bool ctl_lost = P.src_runctl && !P.dst_runctl && !runctl_default(P.src_runctl[r]);   // no area to arrive in
+    const bf_run_ctl* ctl = P.src.areas.runctl;
+    const bool ctl_lost = ctl && !P.dst_areas.runctl && !runctl_default(ctl[r]);   // no area to arrive in
     P.extent[i] = make_uint4(steps, child, fields, armed | (ctl_lost ? 0x80000000u : 0u));
-    if (steps > T.steps_max || (T.off_child != BF_OFF_NONE && child > T.child_nibbles) || (fields & ~placed) || armed > P.dst_k ||
-        ctl_lost)
+    if (steps > T.steps_max || (T.off_child != BF_OFF_NONE && child > T.child_nibbles) || (fields & ~placed) ||
+        armed > P.dst_areas.timer_k || ctl_lost)
       atomicMin(P.unfit, i);
   }
 }
 
 // Transfer, the move.  One warp per listed run: lane t stores words t, t + 32, ... of destination record dst_first + i, each
-// re-laid from F to T by its byte offset as reshape_runs does (state, then current result), and lane 0 marks the arrival.  The
-// source records are only read; retire_runs compacts the source behind this launch on the same stream.
+// re-laid from src.L to T by its byte offset as reshape_runs does (state, then current result), lane 0 marks the arrival, and
+// the run's side areas arrive with it.  The source records are only read; retire_runs compacts the source behind this launch on
+// the same stream.
 __global__ void __launch_bounds__(256) transfer_runs(const TransferParams P) {
   const uint32_t i = blockIdx.x * 8u + (threadIdx.x >> 5), lane = threadIdx.x & 31u;
   if (i >= P.n) return;
   const uint32_t r = P.runs[i], to = P.dst_first + i;
-  const uint32_t* s = reinterpret_cast<const uint32_t*>(P.src_state + (size_t)r * P.F.state_stride);
+  const bf_layout& F = P.src.L;
+  const uint32_t* s = reinterpret_cast<const uint32_t*>(P.src.state + (size_t)r * F.state_stride);
   uint32_t* d = reinterpret_cast<uint32_t*>(P.dst_state + (size_t)to * P.T.state_stride);
-  for (uint32_t o = lane * 4u; o < P.T.state_stride; o += 128u) d[o >> 2] = reshape_state_word(s, o, P.F, P.T);
-  s = reinterpret_cast<const uint32_t*>(P.src_result + (size_t)r * P.F.result_stride);
+  for (uint32_t o = lane * 4u; o < P.T.state_stride; o += 128u) d[o >> 2] = reshape_state_word(s, o, F, P.T);
+  s = reinterpret_cast<const uint32_t*>(P.src.result + (size_t)r * F.result_stride);
   d = reinterpret_cast<uint32_t*>(P.dst_result + (size_t)to * P.T.result_stride);
-  for (uint32_t o = lane * 4u; o < P.T.result_stride; o += 128u) d[o >> 2] = reshape_result_word(s, o, P.F, P.T);
+  for (uint32_t o = lane * 4u; o < P.T.result_stride; o += 128u) d[o >> 2] = reshape_result_word(s, o, F, P.T);
   if (lane == 0) P.dst_mark[to] = P.mark_value;
-  if (P.dst_sched_in && lane == 0) {   // the run's limiter inputs arrive with it, without a baseline
-    P.dst_sched_in[to] = P.src_sched_in ? P.src_sched_in[r] : kSchedDefault;
-    *reinterpret_cast<uint32_t*>(P.dst_sched_rec + (size_t)to * P.dst_sched_stride + 12) = kSchedNoBase;
-  }
-  // the run's armed slots (at most dst_k, transfer_fit) lead the source's slots: copied in order, empty slots behind them
-  for (uint32_t k = lane; P.dst_timers && k < P.dst_k; k += 32u)
-    P.dst_timers[(size_t)to * P.dst_k + k] = P.src_timers && k < P.src_k ? P.src_timers[(size_t)r * P.src_k + k] : kTimerEmpty;
-  if (P.dst_runctl && lane == 0) P.dst_runctl[to] = P.src_runctl ? P.src_runctl[r] : kRunCtlDefault;
+  arrive_areas(P.src.areas, r, P.dst_areas, to, lane);
 }
 
 cudaError_t launch_transfer_fit(const TransferParams& P, cudaStream_t stream) {
@@ -793,14 +790,14 @@ DI bool story_fires(const FireParams& P, const bf_run_ctl& c) { return !c.stop &
 DI uint32_t fired_of_run(const FireParams& P, uint32_t r) {
   if (r >= P.n_runs) return 0u;
   uint32_t n = 0;
-  if (P.runctl) {   // run level: the drain deadline, and a story timeout, which stands for every step slot
-    const bf_run_ctl c = P.runctl[r];
+  if (P.areas.runctl) {   // run level: the drain deadline, and a story timeout, which stands for every step slot
+    const bf_run_ctl c = P.areas.runctl[r];
     n = deadline_due(c.drain_deadline, P.now) ? 1u : 0u;
     if (story_fires(P, c)) return n + 1u;
   }
   const uint8_t* rec = P.state + (size_t)r * P.state_stride;
-  const unsigned long long* t = P.timers + (size_t)r * P.timer_k;
-  for (uint32_t k = 0; k < P.timer_k; ++k) {
+  const unsigned long long* t = P.areas.timers + (size_t)r * P.areas.timer_k;
+  for (uint32_t k = 0; k < P.areas.timer_k; ++k) {
     const unsigned long long v = t[k];
     if (!timer_armed(v)) break;   // armed slots lead
     n += fire_kind(P, rec, v) == 1u ? 1u : 0u;
@@ -846,12 +843,12 @@ __global__ void __launch_bounds__(256) fire_apply(const FireParams P) {
   uint32_t pos = incl - mine;
   for (uint32_t w = 0; w < 8; ++w) pos += base_part[w] + (w < warp ? warp_incl[w] : 0u);
   uint32_t written = 0, pruned = 0, next = BF_TIMER_NONE, touched = 0;
-  if (r < P.n_runs && P.runctl && story_fires(P, P.runctl[r])) {   // the story timeout: no step slot fires, each is pruned
+  if (r < P.n_runs && P.areas.runctl && story_fires(P, P.areas.runctl[r])) {   // the story timeout: no step slot fires, each is pruned
     uint8_t* rec = P.state + (size_t)r * P.state_stride;
-    bf_run_ctl* ctl = P.runctl + r;
-    for (uint32_t k = 0; k < P.timer_k && timer_armed(P.timers[(size_t)r * P.timer_k + k]); ++k) ++pruned;
+    bf_run_ctl* ctl = P.areas.runctl + r;
+    for (uint32_t k = 0; k < P.areas.timer_k && timer_armed(P.areas.timers[(size_t)r * P.areas.timer_k + k]); ++k) ++pruned;
     const uint32_t drain = ctl->drain_deadline;
-    stop_run(rec, ctl, r, BF_STOP_TIMEOUT, StopParams{P.timers, P.timer_k, P.sched_in, P.mark, P.mark_value});
+    stop_run(rec, ctl, r, BF_STOP_TIMEOUT, StopParams{P.areas, P.mark, P.mark_value});
     written = 1u;
     if (deadline_due(drain, P.now)) {   // BF_FIRED_DRAIN < BF_FIRED_STORY: listed first
       ctl->drain_deadline = BF_TIMER_NONE;
@@ -863,9 +860,9 @@ __global__ void __launch_bounds__(256) fire_apply(const FireParams P) {
     if (pos < P.fired_cap) P.fired[pos] = bf_fired{r, (uint16_t)BF_FIRED_STORY, (uint8_t)BF_DEC_TIMED_OUT, 1u};
   } else if (r < P.n_runs) {
     uint8_t* rec = P.state + (size_t)r * P.state_stride;
-    unsigned long long* t = P.timers + (size_t)r * P.timer_k;
+    unsigned long long* t = P.areas.timers + (size_t)r * P.areas.timer_k;
     uint32_t keep = 0, k = 0;
-    for (; k < P.timer_k; ++k) {
+    for (; k < P.areas.timer_k; ++k) {
       const unsigned long long v = t[k];
       if (!timer_armed(v)) break;
       const uint32_t kind = fire_kind(P, rec, v);
@@ -884,8 +881,8 @@ __global__ void __launch_bounds__(256) fire_apply(const FireParams P) {
     }
     for (uint32_t e = keep; e < k; ++e) t[e] = kTimerEmpty;
     if (touched) atomicMax(P.mark + r, P.mark_value);   // max: an upload's "must list" bit stays
-    if (P.runctl) {   // after the steps (BF_FIRED_DRAIN sorts above every step); a stopped run's story deadline is dormant
-      bf_run_ctl* ctl = P.runctl + r;
+    if (P.areas.runctl) {   // after the steps (BF_FIRED_DRAIN sorts above every step); a stopped run's story deadline is dormant
+      bf_run_ctl* ctl = P.areas.runctl + r;
       const uint32_t drain = ctl->drain_deadline;
       if (deadline_due(drain, P.now)) {
         ctl->drain_deadline = BF_TIMER_NONE;

@@ -4,6 +4,7 @@
 #include <stdlib.h>
 #include <string.h>
 
+#include <array>
 #include <unordered_map>
 
 #include "ctx.h"
@@ -12,12 +13,15 @@ using bf::cuda_fail; using bf::fail; using bf::round_up_sz;
 
 // the bf_resident_* definitions take their C linkage from include/bobrafrontier.h
 // ---- resident batches (row f2: incremental state upload) --------------------------------------------------
+// the live batch of handle h, or nullptr (the caller holds the ctx lock)
+static Resident* live_batch(bf_ctx* c, uint32_t h) { return h < c->resident.size() && c->resident[h].alive ? &c->resident[h] : nullptr; }
+
 // The ctx lock, which the caller holds for the call, and the live batch of handle h.  The batch is nullptr for a null ctx (no
 // lock then) and for an unknown handle (its error set; an argument check that fails after this one sets its own instead).
 static std::pair<std::unique_lock<std::mutex>, Resident*> lock_resident(bf_ctx* c, uint32_t h) {
   if (!c) return {};
   std::unique_lock<std::mutex> g(c->mu);
-  Resident* r = h < c->resident.size() && c->resident[h].alive ? &c->resident[h] : nullptr;
+  Resident* r = live_batch(c, h);
   if (!r) fail(c, BF_EINVAL, "unknown resident batch");
   return {std::move(g), r};
 }
@@ -61,12 +65,13 @@ int bf_resident_upload(bf_ctx* c, uint32_t h, uint32_t first, uint32_t n, const 
   r->state_changed(c);
   r->prev_valid = false;   // full records arrived: the next changed-only tick lists every run
   BF_CUDA(c, cudaMemcpyAsync(r->d_state + (size_t)first * r->L.state_stride, records, (size_t)n * r->L.state_stride, cudaMemcpyHostToDevice, c->stream));
-  if (r->d_sched_in)   // the uploaded runs have no schedule baseline: kSchedNoBase in the reason word of each stored record
-    BF_CUDA(c, cudaMemset2DAsync(r->d_sched_rec + (size_t)first * r->sched_stride() + 12, r->sched_stride(), 0xFF, 4, n, c->stream));
+  const bf::RunAreasView A = r->areas_view();
+  if (A.sched_rec)   // the uploaded runs have no schedule baseline: kSchedNoBase in the reason word of each stored record
+    BF_CUDA(c, cudaMemset2DAsync(A.sched_rec + (size_t)first * A.sched_stride + 12, A.sched_stride, 0xFF, 4, n, c->stream));
   BF_CUDA(c, bf::launch_mark_runs(r->d_mark, first, n, r->mark_must_list(), c->stream));
   c->stats.kernel_launches += 1;
-  if (r->d_runctl) {   // stops persist: a stopped run's uploaded flags byte is its saved one
-    BF_CUDA(c, bf::launch_runctl_restop({r->d_runctl, r->d_state, r->L.state_stride, first, n}, c->stream));
+  if (A.runctl) {   // stops persist: a stopped run's uploaded flags byte is its saved one
+    BF_CUDA(c, bf::launch_runctl_restop({A.runctl, r->d_state, r->L.state_stride, first, n}, c->stream));
     c->stats.kernel_launches += 1;
   }
   r->pending += n;
@@ -111,7 +116,7 @@ static int resident_apply_async(bf_ctx* c, Resident* r, const bf_delta* deltas, 
   P.off_decision = r->L.off_decision; P.off_child = r->L.off_child; P.child_nibbles = r->L.child_nibbles;
   P.rejected = c->d_rejected;
   P.mark = r->d_mark; P.mark_value = r->mark_touched();
-  P.runctl = r->d_runctl;
+  P.runctl = r->areas.d_runctl;
   BF_CUDA(c, bf::launch_apply_deltas(P, s));
   c->stats.kernel_launches += 1;
   return BF_OK;
@@ -368,12 +373,12 @@ int bf_resident_migrate(bf_ctx* c, uint32_t h, bf_migration* m) {
   BF_CUDA(c, cudaSetDevice(c->device));
   cudaStream_t s = c->stream;
   const size_t o_inv = 16, o_desc = round_up_sz(o_inv + inv.size() * 2, 16), o_fwd = o_desc + descs.size() * sizeof(bf::MigrateDesc),
-               bytes = o_fwd + (r->timer_k ? (size_t)mo.S * 2 : 0);
+               bytes = o_fwd + (r->areas.timer_k ? (size_t)mo.S * 2 : 0);
   if (int rc = c->d_mig.ensure(c, bytes)) return rc;
   std::vector<uint8_t> blob(bytes, 0);   // the counter starts at zero
   memcpy(blob.data() + o_inv, inv.data(), inv.size() * 2);
   if (!descs.empty()) memcpy(blob.data() + o_desc, descs.data(), descs.size() * sizeof(bf::MigrateDesc));
-  if (r->timer_k) memcpy(blob.data() + o_fwd, m->step_map, (size_t)mo.S * 2);   // the timers are re-keyed forwards
+  if (r->areas.timer_k) memcpy(blob.data() + o_fwd, m->step_map, (size_t)mo.S * 2);   // the timers are re-keyed forwards
   r->state_changed(c);   // as after an upload
   bf::MigrateParams P{};
   P.state = r->d_state; P.mark = r->d_mark; P.mark_value = r->mark_must_list();
@@ -383,9 +388,8 @@ int bf_resident_migrate(bf_ctx* c, uint32_t h, bf_migration* m) {
   P.n_runs = m->n_runs; P.old_slot = m->old_slot; P.new_slot = m->new_slot;
   P.words = L.words; P.state_stride = L.state_stride; P.off_phase = L.off_phase; P.off_cond = L.off_cond;
   P.off_decision = L.off_decision; P.off_child = L.off_child; P.child_nibbles = L.child_nibbles;
-  P.timers = r->d_timers; P.timer_k = r->timer_k; P.n_old_steps = mo.S;
+  P.areas = r->areas_view(); P.n_old_steps = mo.S;
   P.fwd = reinterpret_cast<const uint16_t*>(c->d_mig + o_fwd);
-  P.sched_rec = r->d_sched_rec; P.sched_stride = r->sched_stride();
   cudaError_t e = cudaMemcpyAsync(c->d_mig, blob.data(), bytes, cudaMemcpyHostToDevice, s);
   if (e == cudaSuccess) e = bf::launch_migrate(P, s);
   if (e == cudaSuccess) e = cudaMemcpyAsync(&c->pinned->word, c->d_mig, 4, cudaMemcpyDeviceToHost, s);
@@ -446,7 +450,7 @@ int bf_resident_redrive(bf_ctx* c, uint32_t h, const bf_redrive* req, uint32_t n
   P.masks = d_mask; P.status = d; P.slots = c->slots_dev; P.n = n;
   P.words = L.words; P.state_stride = L.state_stride; P.off_phase = L.off_phase; P.off_cond = L.off_cond;
   P.off_decision = L.off_decision; P.off_child = L.off_child;
-  P.timers = r->d_timers; P.timer_k = r->timer_k; P.runctl = r->d_runctl;
+  P.areas = r->areas_view();
   std::vector<uint8_t> status(n);
   cudaStream_t s = c->stream;
   cudaError_t e = cudaMemcpyAsync(d + o_req, blob.data(), blob.size(), cudaMemcpyHostToDevice, s);
@@ -464,6 +468,11 @@ int bf_resident_redrive(bf_ctx* c, uint32_t h, const bf_redrive* req, uint32_t n
   return BF_OK;
 }
 
+// the offsets of the fields a layout may leave out, in one order: cond, decision, child, then the optional output fields
+static std::array<uint32_t, 7> optional_fields(const bf_layout& L) {
+  return {L.off_cond, L.off_decision, L.off_child, L.off_fail, L.off_needs_cond, L.off_skip_dep, L.off_phase_out};
+}
+
 // A live batch grows its capacity and / or layout (resident.cu).  All checks come first, and the new buffers are allocated and
 // filled before the old ones are freed, so a rejected or failed call changes nothing.  One launch (both record arrays), one
 // device copy of the touch marks, one synchronisation.
@@ -478,75 +487,62 @@ int bf_resident_reshape(bf_ctx* c, uint32_t h, const bf_layout* layout, uint32_t
   if (F.fields & ~T.fields) return fail(c, BF_EINVAL, "reshape cannot drop a field");
   if (F.off_child != BF_OFF_NONE && T.child_nibbles < F.child_nibbles) return fail(c, BF_EINVAL, "reshape cannot shrink the child area");
   // the kernel follows the offsets: every field the batch places must have a place in the new layout
-  const uint32_t from[] = {F.off_cond, F.off_decision, F.off_child, F.off_fail, F.off_needs_cond, F.off_skip_dep, F.off_phase_out};
-  const uint32_t to[] = {T.off_cond, T.off_decision, T.off_child, T.off_fail, T.off_needs_cond, T.off_skip_dep, T.off_phase_out};
+  const auto from = optional_fields(F), to = optional_fields(T);
   // zero decision planes are PENDING, which a pass applies to RUNNING gate / sleep / wait steps (an absent plane leaves them
   // alone), and added output masks may gain bits: either may change a result the touch marks know nothing of
   bool results_may_change = false;
-  for (int i = 0; i < 7; ++i) {
+  for (size_t i = 0; i < from.size(); ++i) {
     if (from[i] != BF_OFF_NONE && to[i] == BF_OFF_NONE) return fail(c, BF_EINVAL, "the new layout drops a field the batch has");
     if (i != 0 && i != 2 && from[i] == BF_OFF_NONE && to[i] != BF_OFF_NONE) results_may_change = true;
   }
   BF_CUDA(c, cudaSetDevice(c->device));
+  cudaStream_t s = c->stream;
   Resident nb;
   if (cudaError_t e = nb.alloc(T, capacity)) return fail(c, BF_ENOMEM, std::string("resident reshape: ") + cudaGetErrorString(e));
-  const bool timers_grow = r->timer_k && capacity > r->cap;   // the area follows the capacity: empty slots for the new runs
-  if (timers_grow)
-    if (cudaError_t e = nb.d_timers.alloc((size_t)capacity * r->timer_k))
-      return fail(c, BF_ENOMEM, std::string("resident reshape (timers): ") + cudaGetErrorString(e));
-  // the limiter inputs follow the capacity (defaults for the new runs); the schedule records follow the capacity and the words,
+  // the side areas follow the capacity (the new runs' entries empty or the defaults); the schedule records follow the words too,
   // and keep their baselines when the words stay
-  const bool sched = r->d_sched_in, sched_grow = sched && capacity > r->cap, sched_relay = sched && (sched_grow || T.words != F.words);
-  cudaStream_t s = c->stream;
-  if (sched_grow)
-    if (cudaError_t e = nb.d_sched_in.alloc(capacity)) return fail(c, BF_ENOMEM, std::string("resident reshape (limiter inputs): ") + cudaGetErrorString(e));
-  const bool runctl_grow = r->d_runctl && capacity > r->cap;   // defaults for the new runs, in the reshape launch
-  if (runctl_grow)
-    if (cudaError_t e = nb.d_runctl.alloc(capacity)) return fail(c, BF_ENOMEM, std::string("resident reshape (run control): ") + cudaGetErrorString(e));
-  if (sched_relay)
-    if (cudaError_t e = Resident::alloc_sched_rec(nb.d_sched_rec, capacity, T.words, s))
-      return fail(c, BF_ENOMEM, std::string("resident reshape (schedule records): ") + cudaGetErrorString(e));
+  if (std::string e = r->areas.alloc_resized(nb.areas, r->cap, capacity, F.words, T.words, s); !e.empty())
+    return fail(c, BF_ENOMEM, "resident reshape " + e);
   const size_t old_mark = r->d_mark.cap * sizeof(uint32_t), new_mark = nb.d_mark.cap * sizeof(uint32_t);
   bf::ReshapeParams P{};
   P.old_state = r->d_state; P.old_result = r->d_result; P.state = nb.d_state; P.result = nb.d_result;
   P.n_old = r->cap; P.n_new = capacity; P.from = F; P.to = T;
-  if (sched_grow) { P.old_sched_in = r->d_sched_in; P.sched_in = nb.d_sched_in; }
-  if (runctl_grow) { P.old_runctl = r->d_runctl; P.runctl = nb.d_runctl; }
+  P.old_areas = r->areas_view(); P.areas = nb.areas.view(T.words);
   cudaError_t e = bf::launch_reshape(P, s);
-  if (e == cudaSuccess && sched_relay && T.words == F.words)
-    e = cudaMemcpyAsync(nb.d_sched_rec, r->d_sched_rec, (size_t)r->cap * r->sched_stride(), cudaMemcpyDeviceToDevice, s);
+  if (e == cudaSuccess) e = r->areas.relay(nb.areas, r->cap, capacity, F.words, T.words, s, c->stats.kernel_launches);
   if (e == cudaSuccess) e = cudaMemcpyAsync(nb.d_mark, r->d_mark, old_mark, cudaMemcpyDeviceToDevice, s);   // with the list-build padding
   if (e == cudaSuccess && new_mark > old_mark) e = cudaMemsetAsync(reinterpret_cast<uint8_t*>(nb.d_mark.p) + old_mark, 0, new_mark - old_mark, s);
-  if (e == cudaSuccess && timers_grow) {
-    e = bf::launch_relay_timers({r->d_timers, nb.d_timers, capacity, r->cap, r->timer_k, r->timer_k}, s);
-    c->stats.kernel_launches += 1;
-  }
   const cudaError_t es = cudaStreamSynchronize(s);
   if (e == cudaSuccess) e = es;
   if (e != cudaSuccess) return cuda_fail(c, e, "bf_resident_reshape");   // the old buffers were only read: the batch is as it was
   r->state_changed(c);   // as after an upload
-  if (timers_grow) r->d_timers = std::move(nb.d_timers);
-  if (sched_grow) r->d_sched_in = std::move(nb.d_sched_in);
-  if (runctl_grow) r->d_runctl = std::move(nb.d_runctl);
-  if (sched_relay) r->d_sched_rec = std::move(nb.d_sched_rec);
-  if (T.words != F.words) r->sched_base_runs = 0;
   r->adopt(std::move(nb), T, capacity);
   if (results_may_change) r->need_full = true;
   return BF_OK;
 }
 
-// The extent kernel over the batch, counting the result fields R places, on the ctx stream; the caller downloads the three words
-// of c->d_extent (download_extent) behind whatever else it launches.  Nothing of the batch changes.
-static int extent_async(bf_ctx* c, Resident* r, uint32_t n_runs, const bf_layout& R) {
+// Batch r as the extent kernels read it (after sync_slots), counting the result planes of its layout that layout T keeps.  Only
+// result records a later tick compares with count: the changed-only baseline and the touched one (ctx.h).
+static bf::ExtentBatch extent_batch(bf_ctx* c, const Resident* r, const bf_layout& T) {
+  bf::ExtentBatch B{};
+  B.state = r->d_state; B.result = r->d_result; B.mark = r->d_mark; B.areas = r->areas_view();
+  B.slots = c->slots_dev; B.n_slots = (uint32_t)c->slots_host.size();
+  B.prev_runs = r->prev_valid ? r->prev_runs : 0u; B.eval_runs = r->touched_baseline_runs(); B.full_epoch = r->full_epoch;
+  B.L = B.R = r->L;
+  if (T.off_fail == BF_OFF_NONE) B.R.off_fail = BF_OFF_NONE;
+  if (T.off_needs_cond == BF_OFF_NONE) B.R.off_needs_cond = BF_OFF_NONE;
+  if (T.off_skip_dep == BF_OFF_NONE) B.R.off_skip_dep = BF_OFF_NONE;
+  if (T.off_phase_out == BF_OFF_NONE) B.R.off_phase_out = BF_OFF_NONE;
+  return B;
+}
+
+// The extent kernel over the batch, counting the result fields layout T keeps, on the ctx stream; the caller downloads the three
+// words of c->d_extent (download_extent) behind whatever else it launches.  Nothing of the batch changes.
+static int extent_async(bf_ctx* c, Resident* r, uint32_t n_runs, const bf_layout& T) {
   cudaStream_t s = c->stream;
   if (int rc = c->d_extent.ensure(c, 3)) return rc;
   if (int rc = bf::sync_slots(c, s)) return rc;
-  bf::ExtentParams P{};
-  P.state = r->d_state; P.result = r->d_result; P.mark = r->d_mark; P.slots = c->slots_dev; P.n_slots = (uint32_t)c->slots_host.size();
-  P.n_records = r->cap; P.n_runs = n_runs; P.L = r->L; P.R = R; P.out = c->d_extent;
-  P.timers = r->d_timers; P.timer_k = r->timer_k;
-  // only result records a later tick compares with count: the changed-only baseline and the touched one (ctx.h)
-  P.prev_runs = r->prev_valid ? r->prev_runs : 0u; P.eval_runs = r->touched_baseline_runs(); P.full_epoch = r->full_epoch;
+  const bf::ExtentParams P{extent_batch(c, r, T), r->cap, n_runs, c->d_extent};
   BF_CUDA(c, cudaMemsetAsync(c->d_extent, 0, 3 * sizeof(unsigned long long), s));
   BF_CUDA(c, bf::launch_extent(P, c->sm_count, s));
   c->stats.kernel_launches += 1;
@@ -606,23 +602,17 @@ int bf_resident_narrow(bf_ctx* c, uint32_t h, const bf_layout* layout, bf_extent
   // the kernel follows the offsets: every field the new layout places must be placed by the batch's.  Dropping decision planes
   // (zero ones are PENDING, which a pass applies; absent ones skip it), the child area (a registered parallel step without
   // branches joins with an area and not without one) or an output mask (the event kinds change) may change any run's result
-  const uint32_t from[] = {F.off_cond, F.off_decision, F.off_child, F.off_fail, F.off_needs_cond, F.off_skip_dep, F.off_phase_out};
-  const uint32_t to[] = {T.off_cond, T.off_decision, T.off_child, T.off_fail, T.off_needs_cond, T.off_skip_dep, T.off_phase_out};
+  const auto from = optional_fields(F), to = optional_fields(T);
   bool results_may_change = false;
-  for (int i = 0; i < 7; ++i) {
+  for (size_t i = 0; i < from.size(); ++i) {
     if (from[i] == BF_OFF_NONE && to[i] != BF_OFF_NONE) return reject("the new layout places a field the batch lacks");
     if (i != 0 && from[i] != BF_OFF_NONE && to[i] == BF_OFF_NONE) results_may_change = true;
   }
-  bf_layout R = F;   // the result planes that count: those the new layout keeps
-  if (T.off_fail == BF_OFF_NONE) R.off_fail = BF_OFF_NONE;
-  if (T.off_needs_cond == BF_OFF_NONE) R.off_needs_cond = BF_OFF_NONE;
-  if (T.off_skip_dep == BF_OFF_NONE) R.off_skip_dep = BF_OFF_NONE;
-  if (T.off_phase_out == BF_OFF_NONE) R.off_phase_out = BF_OFF_NONE;
   const bool same = memcmp(&F, &T, sizeof T) == 0;
   Resident nb;
   if (!same)
     if (cudaError_t e2 = nb.alloc(T, r->cap)) return fail(c, BF_ENOMEM, std::string("resident narrow: ") + cudaGetErrorString(e2));
-  if (int rc = extent_async(c, r, N, R)) { cudaStreamSynchronize(c->stream); return rc; }
+  if (int rc = extent_async(c, r, N, T)) { cudaStreamSynchronize(c->stream); return rc; }
   cudaStream_t s = c->stream;
   cudaError_t err = cudaSuccess;
   if (!same) {
@@ -647,7 +637,6 @@ int bf_resident_narrow(bf_ctx* c, uint32_t h, const bf_layout* layout, bf_extent
     return fail(c, BF_EINVAL, "the batch needs child_nibbles " + std::to_string(e->child_nibbles));
   if (e->fields & ~placed) return fail(c, BF_EINVAL, "the new layout drops an input field holding a non-default code");
   r->state_changed(c);   // as after an upload
-  if (T.words != F.words) r->sched_base_runs = 0;   // the schedule records keep their area, which the smaller stride fits
   r->adopt(std::move(nb), T, r->cap);
   r->narrowed(N, results_may_change);
   return BF_OK;
@@ -703,47 +692,28 @@ int bf_resident_retire(bf_ctx* c, uint32_t h, bf_retire* rt) {
   BF_CUDA(c, cudaSetDevice(c->device));
   if (int rc = c->d_retire.ensure(c, n ? n : 1)) return rc;
   const bf_layout& L = r->L;
+  cudaStream_t s = c->stream;
   Resident nb;
-  if (resize)
+  if (resize) {
     if (cudaError_t e = nb.alloc(L, cap)) return fail(c, BF_ENOMEM, std::string("resident retire: ") + cudaGetErrorString(e));
-  if (resize && r->timer_k)
-    if (cudaError_t e = nb.d_timers.alloc((size_t)cap * r->timer_k))
-      return fail(c, BF_ENOMEM, std::string("resident retire (timers): ") + cudaGetErrorString(e));
-  const bool sched = r->d_sched_in;
-  if (resize && sched) {
-    cudaError_t e = nb.d_sched_in.alloc(cap);
-    if (e == cudaSuccess) e = nb.d_sched_rec.alloc((size_t)cap * r->sched_stride());
-    if (e != cudaSuccess) return fail(c, BF_ENOMEM, std::string("resident retire (limiter inputs): ") + cudaGetErrorString(e));
+    if (std::string e = r->areas.alloc_resized(nb.areas, r->cap, cap, L.words, L.words, s); !e.empty())
+      return fail(c, BF_ENOMEM, "resident retire " + e);
   }
-  if (resize && r->d_runctl)
-    if (cudaError_t e = nb.d_runctl.alloc(cap)) return fail(c, BF_ENOMEM, std::string("resident retire (run control): ") + cudaGetErrorString(e));
   r->state_changed(c);   // as after an upload
   bf::RetireParams P{};
   P.state = r->d_state; P.result = r->d_result; P.mark = r->d_mark; P.mark_value = r->mark_must_list();
   P.to = c->d_retire; P.m = m; P.n = n; P.state_stride = L.state_stride; P.result_stride = L.result_stride;
-  P.timers = r->d_timers; P.timer_k = r->timer_k;
-  P.sched_in = r->d_sched_in; P.sched_rec = r->d_sched_rec; P.sched_stride = r->sched_stride();
-  P.runctl = r->d_runctl;
-  cudaStream_t s = c->stream;
+  P.areas = r->areas_view();
   cudaError_t e = n ? cudaMemcpyAsync(c->d_retire, to.data(), (size_t)n * 4, cudaMemcpyHostToDevice, s) : cudaSuccess;
   if (e == cudaSuccess) e = bf::launch_retire(P, s);
   if (resize) {   // in place first, then the prefix into the new buffers (the mark padding past cap is never read)
     if (e == cudaSuccess) e = cudaMemcpyAsync(nb.d_state, r->d_state, (size_t)cap * L.state_stride, cudaMemcpyDeviceToDevice, s);
     if (e == cudaSuccess) e = cudaMemcpyAsync(nb.d_result, r->d_result, (size_t)cap * L.result_stride, cudaMemcpyDeviceToDevice, s);
     if (e == cudaSuccess) e = cudaMemcpyAsync(nb.d_mark, r->d_mark, nb.d_mark.cap * sizeof(uint32_t), cudaMemcpyDeviceToDevice, s);
-    if (e == cudaSuccess && r->timer_k)
-      e = cudaMemcpyAsync(nb.d_timers, r->d_timers, (size_t)cap * r->timer_k * 8, cudaMemcpyDeviceToDevice, s);
-    if (e == cudaSuccess && sched) e = cudaMemcpyAsync(nb.d_sched_in, r->d_sched_in, (size_t)cap * sizeof(bf_sched_run), cudaMemcpyDeviceToDevice, s);
-    if (e == cudaSuccess && sched)
-      e = cudaMemcpyAsync(nb.d_sched_rec, r->d_sched_rec, (size_t)cap * r->sched_stride(), cudaMemcpyDeviceToDevice, s);
-    if (e == cudaSuccess && r->d_runctl)
-      e = cudaMemcpyAsync(nb.d_runctl, r->d_runctl, (size_t)cap * sizeof(bf_run_ctl), cudaMemcpyDeviceToDevice, s);
+    if (e == cudaSuccess) e = r->areas.copy_prefix(nb.areas, cap, L.words, s);
   }
   if (int rc = r->sync_in_place(c, e, "bf_resident_retire")) return rc;
   c->stats.kernel_launches += n ? 1 : 0;
-  if (resize && r->timer_k) r->d_timers = std::move(nb.d_timers);
-  if (resize && sched) { r->d_sched_in = std::move(nb.d_sched_in); r->d_sched_rec = std::move(nb.d_sched_rec); }
-  if (resize && r->d_runctl) r->d_runctl = std::move(nb.d_runctl);
   if (resize) r->adopt(std::move(nb), L, cap);
   r->compact_to(m, N, to);
   write_moves(to, m, rt->moves_from, rt->moves_to);
@@ -761,7 +731,7 @@ int bf_resident_transfer(bf_ctx* c, uint32_t hs, uint32_t hd, bf_transfer* t) {
   t->unfit = BF_EXTENT_NO_RUN;
   t->why = bf_extent{};
   if (!src) return BF_EINVAL;
-  Resident* dst = hd < c->resident.size() && c->resident[hd].alive ? &c->resident[hd] : nullptr;
+  Resident* dst = live_batch(c, hd);
   if (!dst) return fail(c, BF_EINVAL, "unknown resident batch");
   if (hs == hd) return fail(c, BF_EINVAL, "a transfer from a batch to itself");
   const uint32_t N = t->src_n_runs, D = t->dst_n_runs, n = t->n;
@@ -776,7 +746,7 @@ int bf_resident_transfer(bf_ctx* c, uint32_t hs, uint32_t hd, bf_transfer* t) {
     gone[q] = 1;
   }
   if (n == 0) { t->n_moves = 0; return BF_OK; }
-  if (src->d_sched_in && !dst->d_sched_in)
+  if (src->areas.d_sched_in && !dst->areas.d_sched_in)
     return fail(c, BF_EINVAL, "the source batch has limiter inputs and the destination has no area for them (bf_resident_sched)");
   const uint32_t m = N - n;
   std::vector<uint32_t> to;
@@ -790,24 +760,13 @@ int bf_resident_transfer(bf_ctx* c, uint32_t hs, uint32_t hd, bf_transfer* t) {
   memcpy(blob.data(), &none, 4);
   memcpy(blob.data() + o_runs, t->runs, (size_t)n * 4);
   memcpy(blob.data() + o_to, to.data(), (size_t)n * 4);
-  const bf_layout F = src->L, T = dst->L;
+  const bf_layout F = src->L;
   bf::TransferParams P{};
-  P.src_state = src->d_state; P.src_result = src->d_result; P.src_mark = src->d_mark;
+  P.src = extent_batch(c, src, dst->L);   // the source's result records as a later tick of it compares them (bf_resident_extent)
   P.dst_state = dst->d_state; P.dst_result = dst->d_result; P.dst_mark = dst->d_mark; P.mark_value = dst->mark_must_list();
-  P.runs = reinterpret_cast<const uint32_t*>(c->d_transfer + o_runs); P.n = n; P.dst_first = D;
-  P.slots = c->slots_dev; P.n_slots = (uint32_t)c->slots_host.size();
-  // only result records a later tick of the source compares with count (bf_resident_extent's rule)
-  P.prev_runs = src->prev_valid ? src->prev_runs : 0u; P.eval_runs = src->touched_baseline_runs(); P.full_epoch = src->full_epoch;
-  P.F = F; P.T = T; P.R = F;
-  if (T.off_fail == BF_OFF_NONE) P.R.off_fail = BF_OFF_NONE;
-  if (T.off_needs_cond == BF_OFF_NONE) P.R.off_needs_cond = BF_OFF_NONE;
-  if (T.off_skip_dep == BF_OFF_NONE) P.R.off_skip_dep = BF_OFF_NONE;
-  if (T.off_phase_out == BF_OFF_NONE) P.R.off_phase_out = BF_OFF_NONE;
+  P.dst_areas = dst->areas_view();
+  P.runs = reinterpret_cast<const uint32_t*>(c->d_transfer + o_runs); P.n = n; P.dst_first = D; P.T = dst->L;
   P.extent = reinterpret_cast<uint4*>(c->d_transfer + o_ext); P.unfit = reinterpret_cast<uint32_t*>(c->d_transfer.p);
-  P.src_timers = src->d_timers; P.src_k = src->timer_k; P.dst_timers = dst->d_timers; P.dst_k = dst->timer_k;
-  P.src_sched_in = src->d_sched_in; P.dst_sched_in = dst->d_sched_in; P.dst_sched_rec = dst->d_sched_rec;
-  P.dst_sched_stride = dst->sched_stride();
-  P.src_runctl = src->d_runctl; P.dst_runctl = dst->d_runctl;
   cudaStream_t s = c->stream;
   BF_CUDA(c, cudaMemcpyAsync(c->d_transfer, blob.data(), blob.size(), cudaMemcpyHostToDevice, s));
   BF_CUDA(c, bf::launch_transfer_fit(P, s));
@@ -825,7 +784,7 @@ int bf_resident_transfer(bf_ctx* c, uint32_t hs, uint32_t hd, bf_transfer* t) {
     return fail(c, BF_EINVAL, "runs[" + std::to_string(unfit) + "] (run " + std::to_string(t->runs[unfit]) +
                                   ") does not fit the destination layout: it needs steps_max " + std::to_string(x[0]) +
                                   ", child_nibbles " + std::to_string(x[1]) + ", fields " + std::to_string(x[2]) + ", " +
-                                  std::to_string(x[3] & 0x7FFFFFFFu) + " timer slot(s) of the destination's " + std::to_string(dst->timer_k) +
+                                  std::to_string(x[3] & 0x7FFFFFFFu) + " timer slot(s) of the destination's " + std::to_string(P.dst_areas.timer_k) +
                                   ((x[3] >> 31) ? ", and a run-control area (bf_resident_runctl) for its stop or deadlines" : ""));
   }
   // every arrival's record is a changed-only baseline of the source: the destination's may reach over them
@@ -836,10 +795,7 @@ int bf_resident_transfer(bf_ctx* c, uint32_t hs, uint32_t hd, bf_transfer* t) {
   bf::RetireParams Q{};
   Q.state = src->d_state; Q.result = src->d_result; Q.mark = src->d_mark; Q.mark_value = src->mark_must_list();
   Q.to = reinterpret_cast<const uint32_t*>(c->d_transfer + o_to); Q.m = m; Q.n = n;
-  Q.state_stride = F.state_stride; Q.result_stride = F.result_stride;
-  Q.timers = src->d_timers; Q.timer_k = src->timer_k;
-  Q.sched_in = src->d_sched_in; Q.sched_rec = src->d_sched_rec; Q.sched_stride = src->sched_stride();
-  Q.runctl = src->d_runctl;
+  Q.state_stride = F.state_stride; Q.result_stride = F.result_stride; Q.areas = P.src.areas;
   cudaError_t e = bf::launch_transfer(P, s);
   if (e == cudaSuccess) e = bf::launch_retire(Q, s);   // behind the transfer on the stream: the sources are read first
   if (int rc = src->sync_in_place(c, e, "bf_resident_transfer")) { dst->records_unknown(); return rc; }
@@ -858,18 +814,18 @@ int bf_resident_timers(bf_ctx* c, uint32_t h, uint32_t K) {
   auto [g, r] = lock_resident(c, h);
   if (!r) return BF_EINVAL;
   if (K < 1 || K > BF_TIMER_MAX_SLOTS) return fail(c, BF_EINVAL, "slots_per_run must be within [1, 64]");
-  if (K < r->timer_k) return fail(c, BF_EINVAL, "slots_per_run cannot shrink (" + std::to_string(r->timer_k) + " now)");
-  if (K == r->timer_k) return BF_OK;
+  if (K < r->areas.timer_k) return fail(c, BF_EINVAL, "slots_per_run cannot shrink (" + std::to_string(r->areas.timer_k) + " now)");
+  if (K == r->areas.timer_k) return BF_OK;
   BF_CUDA(c, cudaSetDevice(c->device));
   DevBuf<unsigned long long> area;
   if (cudaError_t e = area.alloc((size_t)r->cap * K)) return fail(c, BF_ENOMEM, std::string("timer area: ") + cudaGetErrorString(e));
-  cudaError_t e = bf::launch_relay_timers({r->d_timers, area, r->cap, r->cap, r->timer_k, K}, c->stream);
+  cudaError_t e = bf::launch_relay_timers({r->areas.d_timers, area, r->cap, r->cap, r->areas.timer_k, K}, c->stream);
   const cudaError_t es = cudaStreamSynchronize(c->stream);
   if (e == cudaSuccess) e = es;
   if (e != cudaSuccess) return cuda_fail(c, e, "bf_resident_timers");   // the old area was only read
   c->stats.kernel_launches += 1;
-  r->d_timers = std::move(area);
-  r->timer_k = K;
+  r->areas.d_timers = std::move(area);
+  r->areas.timer_k = K;
   return BF_OK;
 }
 
@@ -879,7 +835,7 @@ int bf_resident_timers(bf_ctx* c, uint32_t h, uint32_t K) {
 int bf_resident_timers_arm(bf_ctx* c, uint32_t h, const bf_timer* req, uint32_t n) {
   auto [g, r] = lock_resident(c, h);
   if (!r) return BF_EINVAL;
-  if (!r->timer_k) return fail(c, BF_EINVAL, "the batch has no timer area (bf_resident_timers)");
+  if (!r->areas.timer_k) return fail(c, BF_EINVAL, "the batch has no timer area (bf_resident_timers)");
   if (n && !req) return fail(c, BF_EINVAL, "null requests");
   const bf_layout& L = r->L;
   for (uint32_t i = 0; i < n; ++i) {
@@ -919,7 +875,7 @@ int bf_resident_timers_arm(bf_ctx* c, uint32_t h, const bf_timer* req, uint32_t 
   memcpy(blob.data() + o_arm, arm_before.data(), (size_t)(n + 1) * 4);
   memcpy(blob.data() + o_req, sorted.data(), (size_t)n * sizeof(bf_timer));
   bf::TimerArmParams P{};
-  P.timers = r->d_timers; P.timer_k = r->timer_k; P.n_groups = G;
+  P.timers = r->areas.d_timers; P.timer_k = r->areas.timer_k; P.n_groups = G;
   P.req = reinterpret_cast<const bf_timer*>(c->d_timer + o_req);
   P.first = reinterpret_cast<const uint32_t*>(c->d_timer + o_first);
   P.arm_before = reinterpret_cast<const uint32_t*>(c->d_timer + o_arm);
@@ -932,7 +888,7 @@ int bf_resident_timers_arm(bf_ctx* c, uint32_t h, const bf_timer* req, uint32_t 
   c->stats.kernel_launches += 1;
   if (c->pinned->word != none)
     return fail(c, BF_ENOMEM, "run " + std::to_string(sorted[first[c->pinned->word]].run) + " would hold more than " +
-                                  std::to_string(r->timer_k) + " armed timers");
+                                  std::to_string(r->areas.timer_k) + " armed timers");
   cudaError_t e = bf::launch_arm_timers(P, true, s);
   const cudaError_t es = cudaStreamSynchronize(s);
   if (e == cudaSuccess) e = es;
@@ -947,7 +903,8 @@ int bf_resident_fire(bf_ctx* c, uint32_t h, uint32_t now, bf_fire_out* out) {
   auto [g, r] = lock_resident(c, h);
   if (!out || out->struct_size != sizeof(bf_fire_out)) return fail(c, BF_EINVAL, "null bf_fire_out or bad struct_size");
   if (!r) return BF_EINVAL;
-  if (!r->timer_k && !r->d_runctl) return fail(c, BF_EINVAL, "the batch has neither a timer area (bf_resident_timers) nor run control (bf_resident_runctl)");
+  const bf::RunAreasView A = r->areas_view();
+  if (!A.timers && !A.runctl) return fail(c, BF_EINVAL, "the batch has neither a timer area (bf_resident_timers) nor run control (bf_resident_runctl)");
   const uint32_t N = out->n_runs;
   if (N > r->cap) return fail(c, BF_EINVAL, "n_runs exceeds the resident batch");
   if (out->fired_cap && !out->fired) return fail(c, BF_EINVAL, "null fired with a non-zero fired_cap");
@@ -957,20 +914,19 @@ int bf_resident_fire(bf_ctx* c, uint32_t h, uint32_t now, bf_fire_out* out) {
   BF_CUDA(c, cudaSetDevice(c->device));
   const uint32_t grid = (N - 1) / 256 + 1;
   // the list is at most N * (K + 2) long (with run control: a drain and a story entry per run): a larger fired_cap stages no more
-  const uint32_t cap = (uint32_t)std::min<uint64_t>(out->fired_cap, (uint64_t)N * (r->timer_k + (r->d_runctl ? 2u : 0u)));
+  const uint32_t cap = (uint32_t)std::min<uint64_t>(out->fired_cap, (uint64_t)N * (A.timer_k + (A.runctl ? 2u : 0u)));
   bf_fired* posted = static_cast<bf_fired*>(bf::pinned_dev(out->fired));
   const size_t o_sums = 16, o_list = round_up_sz(o_sums + (size_t)grid * 4, 16), bytes = o_list + (posted ? 0 : (size_t)cap * 8);
   if (int rc = c->d_timer.ensure(c, bytes)) return rc;
   r->end_snapshot(c);   // as a delta
   bf::FireParams P{};
-  P.state = r->d_state; P.timers = r->d_timers; P.mark = r->d_mark; P.mark_value = r->mark_touched();
-  P.n_runs = N; P.timer_k = r->timer_k; P.now = now;
+  P.state = r->d_state; P.areas = A; P.mark = r->d_mark; P.mark_value = r->mark_touched();
+  P.n_runs = N; P.now = now;
   P.words = r->L.words; P.state_stride = r->L.state_stride; P.off_phase = r->L.off_phase; P.off_decision = r->L.off_decision;
   P.out = reinterpret_cast<uint32_t*>(c->d_timer.p);
   P.block_sums = reinterpret_cast<uint32_t*>(c->d_timer + o_sums);
   P.fired = posted ? posted : reinterpret_cast<bf_fired*>(c->d_timer + o_list);
   P.fired_cap = cap;
-  P.runctl = r->d_runctl; P.sched_in = r->d_sched_in;
   cudaStream_t s = c->stream;
   uint32_t* words = c->pinned->fire;
   cudaError_t e = bf::launch_fire(P, s);
@@ -988,11 +944,12 @@ int bf_resident_fire(bf_ctx* c, uint32_t h, uint32_t now, bf_fire_out* out) {
 int bf_resident_timers_download(bf_ctx* c, uint32_t h, uint32_t first, uint32_t n, void* slots) {
   auto [g, r] = lock_resident(c, h);
   if (!r) return BF_EINVAL;
-  if (!r->timer_k) return fail(c, BF_EINVAL, "the batch has no timer area (bf_resident_timers)");
+  if (!r->areas.timer_k) return fail(c, BF_EINVAL, "the batch has no timer area (bf_resident_timers)");
   if ((uint64_t)first + n > r->cap || (n && !slots)) return fail(c, BF_EINVAL, "run range outside the resident batch");
   if (n == 0) return BF_OK;
   BF_CUDA(c, cudaSetDevice(c->device));
-  BF_CUDA(c, cudaMemcpyAsync(slots, r->d_timers + (size_t)first * r->timer_k, (size_t)n * r->timer_k * 8, cudaMemcpyDeviceToHost, c->stream));
+  const RunAreas& a = r->areas;
+  BF_CUDA(c, cudaMemcpyAsync(slots, a.d_timers + (size_t)first * a.timer_k, (size_t)n * a.timer_k * 8, cudaMemcpyDeviceToHost, c->stream));
   BF_CUDA(c, cudaStreamSynchronize(c->stream));
   return BF_OK;
 }
@@ -1002,21 +959,21 @@ int bf_resident_timers_download(bf_ctx* c, uint32_t h, uint32_t first, uint32_t 
 int bf_resident_sched(bf_ctx* c, uint32_t h) {
   auto [g, r] = lock_resident(c, h);
   if (!r) return BF_EINVAL;
-  if (r->d_sched_in) return BF_OK;
+  if (r->areas.d_sched_in) return BF_OK;
   BF_CUDA(c, cudaSetDevice(c->device));
   DevBuf<bf_sched_run> in;
   DevBuf<uint8_t> rec;
   const std::vector<bf_sched_run> defaults(r->cap, bf::kSchedDefault);
   cudaError_t e = in.alloc(r->cap);
-  if (e == cudaSuccess) e = Resident::alloc_sched_rec(rec, r->cap, r->L.words, c->stream);
+  if (e == cudaSuccess) e = RunAreas::alloc_sched_rec(rec, r->cap, r->L.words, c->stream);
   if (e != cudaSuccess) return fail(c, BF_ENOMEM, std::string("limiter inputs: ") + cudaGetErrorString(e));
   e = cudaMemcpyAsync(in, defaults.data(), (size_t)r->cap * sizeof(bf_sched_run), cudaMemcpyHostToDevice, c->stream);
   const cudaError_t es = cudaStreamSynchronize(c->stream);
   if (e == cudaSuccess) e = es;
   if (e != cudaSuccess) return cuda_fail(c, e, "bf_resident_sched");
-  r->d_sched_in = std::move(in);
-  r->d_sched_rec = std::move(rec);
-  r->sched_base_runs = 0;
+  r->areas.d_sched_in = std::move(in);
+  r->areas.d_sched_rec = std::move(rec);
+  r->areas.sched_base_runs = 0;
   return BF_OK;
 }
 
@@ -1024,7 +981,7 @@ int bf_resident_sched(bf_ctx* c, uint32_t h) {
 int bf_resident_sched_put(bf_ctx* c, uint32_t h, const bf_sched_put* req, uint32_t n) {
   auto [g, r] = lock_resident(c, h);
   if (!r) return BF_EINVAL;
-  if (!r->d_sched_in) return fail(c, BF_EINVAL, "the batch has no limiter inputs (bf_resident_sched)");
+  if (!r->areas.d_sched_in) return fail(c, BF_EINVAL, "the batch has no limiter inputs (bf_resident_sched)");
   if (n && !req) return fail(c, BF_EINVAL, "null requests");
   std::vector<uint32_t> seen;   // request index + 1 per run named so far
   for (uint32_t i = 0; i < n; ++i) {
@@ -1039,7 +996,7 @@ int bf_resident_sched_put(bf_ctx* c, uint32_t h, const bf_sched_put* req, uint32
   if (n == 0) return BF_OK;
   BF_CUDA(c, cudaSetDevice(c->device));
   if (int rc = c->d_rsched.ensure(c, (size_t)n * sizeof(bf_sched_put))) return rc;
-  bf::SchedPutParams P{r->d_sched_in, reinterpret_cast<const bf_sched_put*>(c->d_rsched.p), n};
+  bf::SchedPutParams P{r->areas.d_sched_in, reinterpret_cast<const bf_sched_put*>(c->d_rsched.p), n};
   cudaStream_t s = c->stream;
   cudaError_t e = cudaMemcpyAsync(c->d_rsched, req, (size_t)n * sizeof(bf_sched_put), cudaMemcpyHostToDevice, s);
   if (e == cudaSuccess) e = bf::launch_sched_put(P, s);
@@ -1053,12 +1010,12 @@ int bf_resident_sched_put(bf_ctx* c, uint32_t h, const bf_sched_put* req, uint32
 int bf_resident_sched_download(bf_ctx* c, uint32_t h, uint32_t first, uint32_t n, bf_sched_put* out) {
   auto [g, r] = lock_resident(c, h);
   if (!r) return BF_EINVAL;
-  if (!r->d_sched_in) return fail(c, BF_EINVAL, "the batch has no limiter inputs (bf_resident_sched)");
+  if (!r->areas.d_sched_in) return fail(c, BF_EINVAL, "the batch has no limiter inputs (bf_resident_sched)");
   if ((uint64_t)first + n > r->cap || (n && !out)) return fail(c, BF_EINVAL, "run range outside the resident batch");
   if (n == 0) return BF_OK;
   BF_CUDA(c, cudaSetDevice(c->device));
   std::vector<bf_sched_run> in(n);
-  BF_CUDA(c, cudaMemcpyAsync(in.data(), r->d_sched_in + first, (size_t)n * sizeof(bf_sched_run), cudaMemcpyDeviceToHost, c->stream));
+  BF_CUDA(c, cudaMemcpyAsync(in.data(), r->areas.d_sched_in + first, (size_t)n * sizeof(bf_sched_run), cudaMemcpyDeviceToHost, c->stream));
   BF_CUDA(c, cudaStreamSynchronize(c->stream));
   for (uint32_t i = 0; i < n; ++i)
     out[i] = bf_sched_put{first + i, in[i].story_key, in[i].queue_key, in[i].priority, in[i].queued_elapsed_s, in[i].run_phase, {0u, 0u}};
@@ -1083,11 +1040,11 @@ int bf_resident_schedule(bf_ctx* c, const bf_sched_tables* t, uint32_t now, bf_r
     const bf_resident_sched_part& p = parts[i];
     auto at = [&] { return "part " + std::to_string(i) + " (batch " + std::to_string(p.handle) + "): "; };
     if (p.struct_size != sizeof(bf_resident_sched_part)) return fail(c, BF_EINVAL, "part " + std::to_string(i) + ": bad struct_size");
-    Resident* r = p.handle < c->resident.size() && c->resident[p.handle].alive ? &c->resident[p.handle] : nullptr;
+    Resident* r = live_batch(c, p.handle);
     if (!r) return fail(c, BF_EINVAL, at() + "unknown resident batch");
     for (uint32_t k = 0; k < i; ++k)
       if (parts[k].handle == p.handle) return fail(c, BF_EINVAL, at() + "the batch is also part " + std::to_string(k));
-    if (!r->d_sched_in) return fail(c, BF_EINVAL, at() + "the batch has no limiter inputs (bf_resident_sched)");
+    if (!r->areas.d_sched_in) return fail(c, BF_EINVAL, at() + "the batch has no limiter inputs (bf_resident_sched)");
     if (p.n_runs > r->cap) return fail(c, BF_EINVAL, at() + "n_runs exceeds the resident batch");
     if (p.runs_cap && (!p.runs || !p.heads)) return fail(c, BF_EINVAL, at() + "null runs / heads with a non-zero runs_cap");
     if (p.events_cap && !p.events) return fail(c, BF_EINVAL, at() + "null events with a non-zero events_cap");
@@ -1147,9 +1104,10 @@ int bf_resident_schedule(bf_ctx* c, const bf_sched_tables* t, uint32_t now, bf_r
     const Resident* r = rs[i];
     const bf_layout& L = r->L;
     bf::SchedParams P = S;
-    P.state = r->d_state; P.result = r->d_result; P.runs = r->d_sched_in; P.records = r->d_sched_rec; P.n_runs = parts[i].n_runs;
+    const bf::RunAreasView A = r->areas_view();
+    P.state = r->d_state; P.result = r->d_result; P.runs = A.sched_in; P.records = A.sched_rec; P.n_runs = parts[i].n_runs;
     P.words = L.words; P.state_stride = L.state_stride; P.off_phase = L.off_phase; P.off_child = L.off_child;
-    P.child_nibbles = L.child_nibbles; P.result_stride = L.result_stride; P.off_ready = L.off_ready; P.stride = r->sched_stride();
+    P.child_nibbles = L.child_nibbles; P.result_stride = L.result_stride; P.off_ready = L.off_ready; P.stride = A.sched_stride;
     return P;
   };
   std::vector<unsigned long long> part_tot((size_t)n_parts * 2, 0ull);
@@ -1162,7 +1120,7 @@ int bf_resident_schedule(bf_ctx* c, const bf_sched_tables* t, uint32_t now, bf_r
       const Plan& q = plan[i];
       bf::ResSchedParams R{};
       R.S = part_params(i);
-      R.base_runs = rs[i]->sched_base_runs;
+      R.base_runs = rs[i]->areas.sched_base_runs;
       R.run_events = reinterpret_cast<uint32_t*>(d + q.ev);
       R.cta_listed = reinterpret_cast<uint32_t*>(d + q.cl);
       R.cta_events = reinterpret_cast<unsigned long long*>(d + q.ce);
@@ -1194,7 +1152,7 @@ int bf_resident_schedule(bf_ctx* c, const bf_sched_tables* t, uint32_t now, bf_r
   if (e == cudaSuccess) e = es;
   c->stats.kernel_launches += launches;
   if (e != cudaSuccess) {   // the schedule records may be half written: no baseline survives
-    for (Resident* r : rs) r->sched_base_runs = 0;
+    for (Resident* r : rs) r->areas.sched_base_runs = 0;
     return cuda_fail(c, e, "bf_resident_schedule");
   }
   for (uint32_t i = 0; i < n_parts; ++i) {
@@ -1203,7 +1161,7 @@ int bf_resident_schedule(bf_ctx* c, const bf_sched_tables* t, uint32_t now, bf_r
     p.n_listed = (uint32_t)part_tot[2 * i];
     p.n_events = part_tot[2 * i + 1];
     p.full = p.n_listed == p.n_runs ? 1u : 0u;
-    rs[i]->sched_base_runs = p.n_runs;
+    rs[i]->areas.sched_base_runs = p.n_runs;
     rs[i]->scheduled = std::max<int64_t>(rs[i]->scheduled, p.n_runs);
     const uint32_t nl = std::min(p.n_listed, q.rcap);
     if (nl && q.runs != SIZE_MAX) {
@@ -1221,7 +1179,7 @@ int bf_resident_schedule(bf_ctx* c, const bf_sched_tables* t, uint32_t now, bf_r
 int bf_resident_runctl(bf_ctx* c, uint32_t h) {
   auto [g, r] = lock_resident(c, h);
   if (!r) return BF_EINVAL;
-  if (r->d_runctl) return BF_OK;
+  if (r->areas.d_runctl) return BF_OK;
   BF_CUDA(c, cudaSetDevice(c->device));
   DevBuf<bf_run_ctl> area;
   if (cudaError_t e = area.alloc(r->cap)) return fail(c, BF_ENOMEM, std::string("run control: ") + cudaGetErrorString(e));
@@ -1230,7 +1188,7 @@ int bf_resident_runctl(bf_ctx* c, uint32_t h) {
   const cudaError_t es = cudaStreamSynchronize(c->stream);
   if (e == cudaSuccess) e = es;
   if (e != cudaSuccess) return cuda_fail(c, e, "bf_resident_runctl");
-  r->d_runctl = std::move(area);
+  r->areas.d_runctl = std::move(area);
   return BF_OK;
 }
 
@@ -1239,7 +1197,7 @@ int bf_resident_runctl(bf_ctx* c, uint32_t h) {
 int bf_resident_runctl_put(bf_ctx* c, uint32_t h, const bf_run_ctl_put* req, uint32_t n) {
   auto [g, r] = lock_resident(c, h);
   if (!r) return BF_EINVAL;
-  if (!r->d_runctl) return fail(c, BF_EINVAL, "the batch has no run-control area (bf_resident_runctl)");
+  if (!r->areas.d_runctl) return fail(c, BF_EINVAL, "the batch has no run-control area (bf_resident_runctl)");
   if (n && !req) return fail(c, BF_EINVAL, "null requests");
   std::vector<uint32_t> seen;   // request index + 1 per run named so far
   uint32_t stops = 0;
@@ -1259,8 +1217,8 @@ int bf_resident_runctl_put(bf_ctx* c, uint32_t h, const bf_run_ctl_put* req, uin
   if (int rc = c->d_runctl_put.ensure(c, n)) return rc;
   if (stops) r->state_changed(c);   // as a delta
   bf::RunCtlPutParams P{};
-  P.area = r->d_runctl; P.req = c->d_runctl_put; P.n = n; P.state = r->d_state; P.state_stride = r->L.state_stride;
-  P.stop = bf::StopParams{r->d_timers, r->timer_k, r->d_sched_in, r->d_mark, r->mark_touched()};
+  P.area = r->areas.d_runctl; P.req = c->d_runctl_put; P.n = n; P.state = r->d_state; P.state_stride = r->L.state_stride;
+  P.stop = bf::StopParams{r->areas_view(), r->d_mark, r->mark_touched()};
   cudaError_t e = cudaMemcpyAsync(c->d_runctl_put, req, (size_t)n * sizeof(bf_run_ctl_put), cudaMemcpyHostToDevice, c->stream);
   if (e == cudaSuccess) e = bf::launch_runctl_put(P, c->stream);
   if (int rc = r->sync_in_place(c, e, "bf_resident_runctl_put")) return rc;
@@ -1272,11 +1230,11 @@ int bf_resident_runctl_put(bf_ctx* c, uint32_t h, const bf_run_ctl_put* req, uin
 int bf_resident_runctl_download(bf_ctx* c, uint32_t h, uint32_t first, uint32_t n, bf_run_ctl* out) {
   auto [g, r] = lock_resident(c, h);
   if (!r) return BF_EINVAL;
-  if (!r->d_runctl) return fail(c, BF_EINVAL, "the batch has no run-control area (bf_resident_runctl)");
+  if (!r->areas.d_runctl) return fail(c, BF_EINVAL, "the batch has no run-control area (bf_resident_runctl)");
   if ((uint64_t)first + n > r->cap || (n && !out)) return fail(c, BF_EINVAL, "run range outside the resident batch");
   if (n == 0) return BF_OK;
   BF_CUDA(c, cudaSetDevice(c->device));
-  BF_CUDA(c, cudaMemcpyAsync(out, r->d_runctl + first, (size_t)n * sizeof(bf_run_ctl), cudaMemcpyDeviceToHost, c->stream));
+  BF_CUDA(c, cudaMemcpyAsync(out, r->areas.d_runctl + first, (size_t)n * sizeof(bf_run_ctl), cudaMemcpyDeviceToHost, c->stream));
   BF_CUDA(c, cudaStreamSynchronize(c->stream));
   return BF_OK;
 }
@@ -1308,7 +1266,8 @@ int bf_resident_commit(bf_ctx* c, uint32_t h, uint32_t n_runs, const bf_commit_e
     return refuse(BF_COMMIT_NONE, BF_COMMIT_NONE, "a topology slot was dropped or reused since the last tick: the masks may not fit the slot's steps");
   if (r->single_ticked < (int64_t)n_runs)
     return refuse(BF_COMMIT_NONE, BF_COMMIT_NONE, "no single-pass tick" + over + " since the last BF_EVAL_FIXPOINT tick: commits follow single-pass ticks");
-  if (r->d_sched_in && r->scheduled < (int64_t)n_runs)
+  const bf::RunAreasView A = r->areas_view();
+  if (A.sched_in && r->scheduled < (int64_t)n_runs)
     return refuse(BF_COMMIT_NONE, BF_COMMIT_NONE, "the batch has limiter inputs and no bf_resident_schedule" + over + " ran since its last tick");
   std::vector<std::pair<uint64_t, uint32_t>> order(n);   // (run << 16 | step, index)
   for (uint32_t i = 0; i < n; ++i) {
@@ -1338,11 +1297,11 @@ int bf_resident_commit(bf_ctx* c, uint32_t h, uint32_t n_runs, const bf_commit_e
   memset(blob.data(), 0xFF, 8);   // no offender yet; the counts start at zero
   for (uint32_t i = 0; i < n; ++i) memcpy(blob.data() + o_entries + (size_t)i * sizeof(bf_commit_entry), &entries[order[i].second], sizeof(bf_commit_entry));
   bf::CommitParams P{};
-  P.state = r->d_state; P.result = r->d_result; P.sched_rec = r->d_sched_in ? r->d_sched_rec.p : nullptr;
+  P.state = r->d_state; P.result = r->d_result; P.sched_rec = A.sched_rec;
   P.slots = c->slots_dev; P.n_slots = (uint32_t)c->slots_host.size();
   P.entries = reinterpret_cast<const bf_commit_entry*>(c->d_commit + o_entries); P.n_entries = n; P.n_runs = n_runs;
   P.words = L.words; P.state_stride = L.state_stride; P.off_phase = L.off_phase; P.result_stride = L.result_stride;
-  P.off_ready = L.off_ready; P.off_skip = L.off_skip; P.off_fail = L.off_fail; P.sched_stride = r->sched_stride();
+  P.off_ready = L.off_ready; P.off_skip = L.off_skip; P.off_fail = L.off_fail; P.sched_stride = A.sched_stride;
   P.mark = r->d_mark; P.mark_value = r->mark_touched();
   P.offender = reinterpret_cast<unsigned long long*>(c->d_commit.p);
   P.counts = reinterpret_cast<uint32_t*>(c->d_commit + 8);
