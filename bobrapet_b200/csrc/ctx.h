@@ -195,26 +195,12 @@ struct bf_ctx {
   DevBuf<uint32_t> d_tlist, d_tpos_head, d_truns, d_thead;
   DevBuf<unsigned long long> d_tsums;
   uint64_t last_touched_events = 0;   // events of the previous touched tick (sizes the first D2H)
-  // migrations (bf_resident_migrate): [0, 16) the migrated-run counter | inverse step map | desc table
-  DevBuf<uint8_t> d_mig;
-  // redrives (bf_resident_redrive): statuses | requests | key per request | key slots | key steps | closure masks
-  DevBuf<uint8_t> d_redrive;
-  // retirements (bf_resident_retire): the new index of each vacated run
-  DevBuf<uint32_t> d_retire;
-  // extents (bf_resident_extent / _narrow): the three words extent_runs reduces into
-  DevBuf<unsigned long long> d_extent;
-  // transfers (bf_resident_transfer): [0, 16) the unfit word | source runs | retire moves | per-run extents (uint4)
-  DevBuf<uint8_t> d_transfer;
-  // resident schedules (bf_resident_schedule): tables | totals | per part: run events, CTA sums, the two totals, staged lists;
-  // puts (bf_resident_sched_put): the requests
-  DevBuf<uint8_t> d_rsched;
-  // run-control puts (bf_resident_runctl_put): the requests
-  DevBuf<bf_run_ctl_put> d_runctl_put;
-  // step timers: arms ([0, 16) the overflow word | group starts | arming prefix | sorted requests) and fires ([0, 16) the four
-  // output words | per-CTA fired counts | the fired list)
-  DevBuf<uint8_t> d_timer;
-  // tick commits (bf_resident_commit): [0, 8) the offender key | [8, 28) the five counts | the sorted entries
-  DevBuf<uint8_t> d_commit;
+  // The device inputs and outputs of one resident call that is not a tick (migrate, redrive, retire, extent, narrow, transfer,
+  // timers_arm, fire, sched_put, schedule, runctl_put, commit), laid out by the call (CallStage, resident_abi.cu).  They are
+  // valid from the call's staging until it returns: a call reads only bytes it uploaded, set or had a kernel write during the
+  // same call, so every counter or sentinel word it reads is written by that call.  ensure only grows it, so the largest call
+  // sizes it and a steady-state call allocates nothing.
+  DevBuf<uint8_t> d_call;
 
   // limiters (bf_schedule): the records the last pass evaluated (bf_eval's staging or a resident batch), read in place.  Cleared
   // (valid = false) when a pass starts or a call changes those records (end_snapshot); assigned whole once a pass went through.
@@ -254,6 +240,13 @@ inline int fail(bf_ctx* c, int code, const std::string& msg) {
 }
 inline int cuda_fail(bf_ctx* c, cudaError_t e, const char* what) {
   return fail(c, BF_ECUDA, std::string(what) + ": " + cudaGetErrorString(e));
+}
+// The synchronisation that ends a call, so that it never returns with work or copies into the caller's buffers in flight.  The
+// first error, of the call's own work (e) or of the synchronisation, fails the call as `what`.
+inline int end_call(bf_ctx* c, cudaError_t e, const char* what) {
+  const cudaError_t es = cudaStreamSynchronize(c->stream);
+  if (e == cudaSuccess) e = es;
+  return e == cudaSuccess ? BF_OK : cuda_fail(c, e, what);
 }
 }  // namespace bf
 #define BF_CUDA(c, call)                                       \
@@ -435,14 +428,12 @@ struct Resident {
     return BF_OK;
   }
   void records_unknown() { need_full = true; prev_valid = false; }
-  // the synchronise that ends a call rewriting records in place (migrate, redrive, retire): after a failure some records may
-  // have changed, so the next touched tick evaluates and lists every run
+  // the end of a call rewriting records in place (bf::end_call): after a failure some records may have changed, so the next
+  // touched tick evaluates and lists every run
   int sync_in_place(bf_ctx* c, cudaError_t e, const char* what) {
-    const cudaError_t es = cudaStreamSynchronize(c->stream);
-    if (e == cudaSuccess) e = es;
-    if (e == cudaSuccess) return BF_OK;
-    records_unknown();
-    return bf::cuda_fail(c, e, what);
+    const int rc = bf::end_call(c, e, what);
+    if (rc != BF_OK) records_unknown();
+    return rc;
   }
   int result_prev(bf_ctx* c) {
     const cudaError_t e = d_result_prev ? cudaSuccess : d_result_prev.alloc((size_t)cap * L.result_stride);

@@ -5,6 +5,8 @@
 #include <string.h>
 
 #include <array>
+#include <functional>
+#include <type_traits>
 #include <unordered_map>
 
 #include "ctx.h"
@@ -24,6 +26,71 @@ static std::pair<std::unique_lock<std::mutex>, Resident*> lock_resident(bf_ctx* 
   Resident* r = live_batch(c, h);
   if (!r) fail(c, BF_EINVAL, "unknown resident batch");
   return {std::move(g), r};
+}
+
+// The sections of one call's device inputs and outputs in c->d_call (ctx.h), each 16-byte aligned (the uint4 extents, the
+// 8-byte words) in the order taken.  up() takes a section the call uploads, copied into the host image at once; out() takes one
+// that only the device writes.  A call takes its uploaded sections first, so that one H2D copy carries them.  send() ensures
+// d_call, points each taken pointer at its section and issues that copy (none when nothing is uploaded).
+struct CallStage {
+  std::vector<uint8_t> image;   // the uploaded sections, as the copy carries them
+  size_t size = 0;
+  std::vector<std::function<void(uint8_t*)>> points;   // each points a taken pointer into d_call
+
+  template <typename T>
+  size_t take(T*& p, size_t bytes) {
+    const size_t o = size;
+    size = round_up_sz(o + bytes, 16);
+    points.push_back([&p, o](uint8_t* d) { p = reinterpret_cast<T*>(d + o); });
+    return o;
+  }
+  template <typename T>
+  void up(T*& p, const std::remove_const_t<T>* src, size_t n) {
+    const size_t o = take(p, n * sizeof(T));
+    image.resize(o + n * sizeof(T));
+    if (n) memcpy(image.data() + o, src, n * sizeof(T));
+  }
+  template <typename T>
+  void out(T*& p, size_t n) { take(p, n * sizeof(T)); }
+  int send(bf_ctx* c, const char* what) {
+    if (int rc = c->d_call.ensure(c, std::max<size_t>(size, 16))) return rc;
+    for (const auto& point : points) point(c->d_call);
+    if (image.empty()) return BF_OK;
+    const cudaError_t e = cudaMemcpyAsync(c->d_call, image.data(), image.size(), cudaMemcpyHostToDevice, c->stream);
+    return e == cudaSuccess ? BF_OK : cuda_fail(c, e, what);
+  }
+};
+
+// Request i names `run` (below cap); each run may be named once.  seen holds request index + 1 per run named so far.
+static int name_run_once(bf_ctx* c, std::vector<uint32_t>& seen, uint32_t cap, uint32_t run, uint32_t i) {
+  if (seen.empty()) seen.assign(cap, 0u);
+  if (seen[run]) return fail(c, BF_EINVAL, "requests " + std::to_string(seen[run] - 1) + " and " + std::to_string(i) + " name the same run");
+  seen[run] = i + 1;
+  return BF_OK;
+}
+
+// The order of n requests by (run, step), ties by index.  -> false when two name the same (run, step): the first such pair of
+// that order, as (earlier, later) in it, is in clash.
+template <typename Q>
+static bool order_by_run_step(const Q* q, uint32_t n, std::vector<uint32_t>& order, std::pair<uint32_t, uint32_t>& clash) {
+  order.resize(n);
+  for (uint32_t i = 0; i < n; ++i) order[i] = i;
+  auto key = [&](uint32_t i) { return (uint64_t)q[i].run << 16 | q[i].step; };
+  std::stable_sort(order.begin(), order.end(), [&](uint32_t a, uint32_t b) { return key(a) < key(b); });
+  for (uint32_t j = 1; j < n; ++j)
+    if (key(order[j]) == key(order[j - 1])) { clash = {order[j - 1], order[j]}; return false; }
+  return true;
+}
+
+// The runs [first, first + n) of a per-run device array (the state records or a side area), per_run bytes each, into the
+// caller's buffer: the range check, one D2H copy, one synchronisation
+static int download_runs(bf_ctx* c, const Resident* r, uint32_t first, uint32_t n, void* out, const void* area, size_t per_run) {
+  if ((uint64_t)first + n > r->cap || (n && !out)) return fail(c, BF_EINVAL, "run range outside the resident batch");
+  if (n == 0) return BF_OK;
+  BF_CUDA(c, cudaSetDevice(c->device));
+  BF_CUDA(c, cudaMemcpyAsync(out, static_cast<const uint8_t*>(area) + first * per_run, n * per_run, cudaMemcpyDeviceToHost, c->stream));
+  BF_CUDA(c, cudaStreamSynchronize(c->stream));
+  return BF_OK;
 }
 
 int bf_resident_create(bf_ctx* c, const bf_layout* L, uint32_t capacity, uint32_t* handle_out) {
@@ -83,12 +150,7 @@ int bf_resident_upload(bf_ctx* c, uint32_t h, uint32_t first, uint32_t n, const 
 int bf_resident_download(bf_ctx* c, uint32_t h, uint32_t first, uint32_t n, void* records) {
   auto [g, r] = lock_resident(c, h);
   if (!r) return BF_EINVAL;
-  if ((uint64_t)first + n > r->cap || (n && !records)) return fail(c, BF_EINVAL, "run range outside the resident batch");
-  if (n == 0) return BF_OK;
-  BF_CUDA(c, cudaSetDevice(c->device));
-  BF_CUDA(c, cudaMemcpyAsync(records, r->d_state + (size_t)first * r->L.state_stride, (size_t)n * r->L.state_stride, cudaMemcpyDeviceToHost, c->stream));
-  BF_CUDA(c, cudaStreamSynchronize(c->stream));
-  return BF_OK;
+  return download_runs(c, r, first, n, records, r->d_state, r->L.state_stride);
 }
 
 // H2D of the deltas + the scatter kernel on the ctx stream, no synchronisation; the rejected counter is read by the caller
@@ -372,27 +434,23 @@ int bf_resident_migrate(bf_ctx* c, uint32_t h, bf_migration* m) {
   m->migrated = 0;
   BF_CUDA(c, cudaSetDevice(c->device));
   cudaStream_t s = c->stream;
-  const size_t o_inv = 16, o_desc = round_up_sz(o_inv + inv.size() * 2, 16), o_fwd = o_desc + descs.size() * sizeof(bf::MigrateDesc),
-               bytes = o_fwd + (r->areas.timer_k ? (size_t)mo.S * 2 : 0);
-  if (int rc = c->d_mig.ensure(c, bytes)) return rc;
-  std::vector<uint8_t> blob(bytes, 0);   // the counter starts at zero
-  memcpy(blob.data() + o_inv, inv.data(), inv.size() * 2);
-  if (!descs.empty()) memcpy(blob.data() + o_desc, descs.data(), descs.size() * sizeof(bf::MigrateDesc));
-  if (r->areas.timer_k) memcpy(blob.data() + o_fwd, m->step_map, (size_t)mo.S * 2);   // the timers are re-keyed forwards
-  r->state_changed(c);   // as after an upload
   bf::MigrateParams P{};
+  const uint32_t zero = 0;
+  CallStage st;
+  st.up(P.migrated, &zero, 1);
+  st.up(P.inv, inv.data(), inv.size());
+  st.up(P.desc, descs.data(), descs.size());
+  st.up(P.fwd, m->step_map, r->areas.timer_k ? mo.S : 0);   // the timers are re-keyed forwards
+  if (int rc = st.send(c, "bf_resident_migrate")) return rc;
+  r->state_changed(c);   // as after an upload
   P.state = r->d_state; P.mark = r->d_mark; P.mark_value = r->mark_must_list();
-  P.migrated = reinterpret_cast<uint32_t*>(c->d_mig.p);
-  P.inv = reinterpret_cast<const uint16_t*>(c->d_mig + o_inv);
-  P.desc = reinterpret_cast<const bf::MigrateDesc*>(c->d_mig + o_desc); P.n_desc = (uint32_t)descs.size();
+  P.n_desc = (uint32_t)descs.size();
   P.n_runs = m->n_runs; P.old_slot = m->old_slot; P.new_slot = m->new_slot;
   P.words = L.words; P.state_stride = L.state_stride; P.off_phase = L.off_phase; P.off_cond = L.off_cond;
   P.off_decision = L.off_decision; P.off_child = L.off_child; P.child_nibbles = L.child_nibbles;
   P.areas = r->areas_view(); P.n_old_steps = mo.S;
-  P.fwd = reinterpret_cast<const uint16_t*>(c->d_mig + o_fwd);
-  cudaError_t e = cudaMemcpyAsync(c->d_mig, blob.data(), bytes, cudaMemcpyHostToDevice, s);
-  if (e == cudaSuccess) e = bf::launch_migrate(P, s);
-  if (e == cudaSuccess) e = cudaMemcpyAsync(&c->pinned->word, c->d_mig, 4, cudaMemcpyDeviceToHost, s);
+  cudaError_t e = bf::launch_migrate(P, s);
+  if (e == cudaSuccess) e = cudaMemcpyAsync(&c->pinned->word, P.migrated, 4, cudaMemcpyDeviceToHost, s);
   if (int rc = r->sync_in_place(c, e, "bf_resident_migrate")) return rc;
   c->stats.kernel_launches += m->n_runs ? 1 : 0;
   m->migrated = c->pinned->word;
@@ -430,34 +488,28 @@ int bf_resident_redrive(bf_ctx* c, uint32_t h, const bf_redrive* req, uint32_t n
   BF_CUDA(c, cudaSetDevice(c->device));
   if (int rc = bf::sync_slots(c, c->stream)) return rc;
   const size_t K = key_slot.size();
-  const size_t o_req = round_up_sz(n, 16), o_key = o_req + (size_t)n * sizeof(bf_redrive), o_ks = o_key + (size_t)n * 4,
-               o_mask = round_up_sz(o_ks + K * 8, 16), bytes = o_mask + K * L.words * 4;
-  if (int rc = c->d_redrive.ensure(c, bytes)) return rc;
-  std::vector<uint8_t> blob(o_mask - o_req);   // requests | keys | key slots | key steps (the statuses are written by the kernel)
-  memcpy(blob.data(), req, (size_t)n * sizeof(bf_redrive));
-  memcpy(blob.data() + (o_key - o_req), key.data(), (size_t)n * 4);
-  if (K) {
-    memcpy(blob.data() + (o_ks - o_req), key_slot.data(), K * 4);
-    memcpy(blob.data() + (o_ks - o_req) + K * 4, key_step.data(), K * 4);
-  }
-  r->state_changed(c);   // as after an upload
-  uint8_t* d = c->d_redrive;
-  uint32_t* d_ks = reinterpret_cast<uint32_t*>(d + o_ks);
-  uint32_t* d_mask = reinterpret_cast<uint32_t*>(d + o_mask);
   bf::RedriveParams P{};
+  const uint32_t *d_key_slot, *d_key_step;
+  uint32_t* d_mask;
+  CallStage st;   // the statuses and the closure masks are written by the kernels
+  st.up(P.req, req, n);
+  st.up(P.key, key.data(), n);
+  st.up(d_key_slot, key_slot.data(), K);
+  st.up(d_key_step, key_step.data(), K);
+  st.out(P.status, n);
+  st.out(d_mask, K * L.words);
+  if (int rc = st.send(c, "bf_resident_redrive")) return rc;
+  r->state_changed(c);   // as after an upload
   P.state = r->d_state; P.mark = r->d_mark; P.mark_value = r->mark_touched();   // as by a delta
-  P.req = reinterpret_cast<const bf_redrive*>(d + o_req); P.key = reinterpret_cast<const uint32_t*>(d + o_key);
-  P.masks = d_mask; P.status = d; P.slots = c->slots_dev; P.n = n;
+  P.masks = d_mask; P.slots = c->slots_dev; P.n = n;
   P.words = L.words; P.state_stride = L.state_stride; P.off_phase = L.off_phase; P.off_cond = L.off_cond;
   P.off_decision = L.off_decision; P.off_child = L.off_child;
   P.areas = r->areas_view();
   std::vector<uint8_t> status(n);
   cudaStream_t s = c->stream;
-  cudaError_t e = cudaMemcpyAsync(d + o_req, blob.data(), blob.size(), cudaMemcpyHostToDevice, s);
-  if (e == cudaSuccess)
-    e = bf::launch_closure(c->slots_dev, d_ks, d_ks + K, (uint32_t)K, (uint32_t)c->slots_host.size(), L.words, d_mask, s);
+  cudaError_t e = bf::launch_closure(c->slots_dev, d_key_slot, d_key_step, (uint32_t)K, (uint32_t)c->slots_host.size(), L.words, d_mask, s);
   if (e == cudaSuccess) e = bf::launch_redrive(P, s);
-  if (e == cudaSuccess) e = cudaMemcpyAsync(status.data(), d, n, cudaMemcpyDeviceToHost, s);
+  if (e == cudaSuccess) e = cudaMemcpyAsync(status.data(), P.status, n, cudaMemcpyDeviceToHost, s);
   if (int rc = r->sync_in_place(c, e, "bf_resident_redrive")) return rc;
   c->stats.kernel_launches += K ? 2 : 1;
   uint32_t applied = 0;
@@ -512,9 +564,7 @@ int bf_resident_reshape(bf_ctx* c, uint32_t h, const bf_layout* layout, uint32_t
   if (e == cudaSuccess) e = r->areas.relay(nb.areas, r->cap, capacity, F.words, T.words, s, c->stats.kernel_launches);
   if (e == cudaSuccess) e = cudaMemcpyAsync(nb.d_mark, r->d_mark, old_mark, cudaMemcpyDeviceToDevice, s);   // with the list-build padding
   if (e == cudaSuccess && new_mark > old_mark) e = cudaMemsetAsync(reinterpret_cast<uint8_t*>(nb.d_mark.p) + old_mark, 0, new_mark - old_mark, s);
-  const cudaError_t es = cudaStreamSynchronize(s);
-  if (e == cudaSuccess) e = es;
-  if (e != cudaSuccess) return cuda_fail(c, e, "bf_resident_reshape");   // the old buffers were only read: the batch is as it was
+  if (int rc = bf::end_call(c, e, "bf_resident_reshape")) return rc;   // the old buffers were only read: the batch is as it was
   r->state_changed(c);   // as after an upload
   r->adopt(std::move(nb), T, capacity);
   if (results_may_change) r->need_full = true;
@@ -536,21 +586,21 @@ static bf::ExtentBatch extent_batch(bf_ctx* c, const Resident* r, const bf_layou
   return B;
 }
 
-// The extent kernel over the batch, counting the result fields layout T keeps, on the ctx stream; the caller downloads the three
-// words of c->d_extent (download_extent) behind whatever else it launches.  Nothing of the batch changes.
+// The extent kernel over the batch, counting the result fields layout T keeps, on the ctx stream, into three words at the start
+// of c->d_call; the caller downloads them (download_extent) behind whatever else it launches.  Nothing of the batch changes.
 static int extent_async(bf_ctx* c, Resident* r, uint32_t n_runs, const bf_layout& T) {
   cudaStream_t s = c->stream;
-  if (int rc = c->d_extent.ensure(c, 3)) return rc;
+  if (int rc = c->d_call.ensure(c, 3 * sizeof(unsigned long long))) return rc;
   if (int rc = bf::sync_slots(c, s)) return rc;
-  const bf::ExtentParams P{extent_batch(c, r, T), r->cap, n_runs, c->d_extent};
-  BF_CUDA(c, cudaMemsetAsync(c->d_extent, 0, 3 * sizeof(unsigned long long), s));
+  const bf::ExtentParams P{extent_batch(c, r, T), r->cap, n_runs, reinterpret_cast<unsigned long long*>(c->d_call.p)};
+  BF_CUDA(c, cudaMemsetAsync(c->d_call, 0, 3 * sizeof(unsigned long long), s));
   BF_CUDA(c, bf::launch_extent(P, c->sm_count, s));
   c->stats.kernel_launches += 1;
   return BF_OK;
 }
 
 static cudaError_t download_extent(bf_ctx* c, unsigned long long* out) {
-  return cudaMemcpyAsync(out, c->d_extent, 3 * sizeof(unsigned long long), cudaMemcpyDeviceToHost, c->stream);
+  return cudaMemcpyAsync(out, c->d_call, 3 * sizeof(unsigned long long), cudaMemcpyDeviceToHost, c->stream);
 }
 
 static void fill_extent(const unsigned long long* out, bf_extent* e) {
@@ -624,9 +674,7 @@ int bf_resident_narrow(bf_ctx* c, uint32_t h, const bf_layout* layout, bf_extent
     c->stats.kernel_launches += 1;
   }
   if (err == cudaSuccess) err = download_extent(c, out);
-  const cudaError_t es = cudaStreamSynchronize(s);
-  if (err == cudaSuccess) err = es;
-  if (err != cudaSuccess) return cuda_fail(c, err, "bf_resident_narrow");   // the old buffers were only read: the batch is as it was
+  if (int rc = bf::end_call(c, err, "bf_resident_narrow")) return rc;   // the old buffers were only read: the batch is as it was
   fill_extent(out, e);
   if (same) return BF_OK;
   const uint32_t placed = (T.off_cond != BF_OFF_NONE ? BF_F_COND : 0u) | (T.off_decision != BF_OFF_NONE ? BF_F_DECISION : 0u) |
@@ -690,7 +738,6 @@ int bf_resident_retire(bf_ctx* c, uint32_t h, bf_retire* rt) {
   std::vector<uint32_t> to;
   const uint32_t n_moves = retire_moves(gone, m, n, to);
   BF_CUDA(c, cudaSetDevice(c->device));
-  if (int rc = c->d_retire.ensure(c, n ? n : 1)) return rc;
   const bf_layout& L = r->L;
   cudaStream_t s = c->stream;
   Resident nb;
@@ -699,13 +746,15 @@ int bf_resident_retire(bf_ctx* c, uint32_t h, bf_retire* rt) {
     if (std::string e = r->areas.alloc_resized(nb.areas, r->cap, cap, L.words, L.words, s); !e.empty())
       return fail(c, BF_ENOMEM, "resident retire " + e);
   }
-  r->state_changed(c);   // as after an upload
   bf::RetireParams P{};
+  CallStage st;
+  st.up(P.to, to.data(), n);
+  if (int rc = st.send(c, "bf_resident_retire")) return rc;
+  r->state_changed(c);   // as after an upload
   P.state = r->d_state; P.result = r->d_result; P.mark = r->d_mark; P.mark_value = r->mark_must_list();
-  P.to = c->d_retire; P.m = m; P.n = n; P.state_stride = L.state_stride; P.result_stride = L.result_stride;
+  P.m = m; P.n = n; P.state_stride = L.state_stride; P.result_stride = L.result_stride;
   P.areas = r->areas_view();
-  cudaError_t e = n ? cudaMemcpyAsync(c->d_retire, to.data(), (size_t)n * 4, cudaMemcpyHostToDevice, s) : cudaSuccess;
-  if (e == cudaSuccess) e = bf::launch_retire(P, s);
+  cudaError_t e = bf::launch_retire(P, s);
   if (resize) {   // in place first, then the prefix into the new buffers (the mark padding past cap is never read)
     if (e == cudaSuccess) e = cudaMemcpyAsync(nb.d_state, r->d_state, (size_t)cap * L.state_stride, cudaMemcpyDeviceToDevice, s);
     if (e == cudaSuccess) e = cudaMemcpyAsync(nb.d_result, r->d_result, (size_t)cap * L.result_stride, cudaMemcpyDeviceToDevice, s);
@@ -752,31 +801,30 @@ int bf_resident_transfer(bf_ctx* c, uint32_t hs, uint32_t hd, bf_transfer* t) {
   std::vector<uint32_t> to;
   const uint32_t n_moves = retire_moves(gone, m, n, to);
   BF_CUDA(c, cudaSetDevice(c->device));
-  const size_t o_runs = 16, o_to = o_runs + (size_t)n * 4, o_ext = round_up_sz(o_to + (size_t)n * 4, 16), bytes = o_ext + (size_t)n * 16;
-  if (int rc = c->d_transfer.ensure(c, bytes)) return rc;
   if (int rc = bf::sync_slots(c, c->stream)) return rc;
-  std::vector<uint8_t> blob(o_ext, 0);   // unfit word | runs | moves
-  const uint32_t none = BF_EXTENT_NO_RUN;
-  memcpy(blob.data(), &none, 4);
-  memcpy(blob.data() + o_runs, t->runs, (size_t)n * 4);
-  memcpy(blob.data() + o_to, to.data(), (size_t)n * 4);
-  const bf_layout F = src->L;
   bf::TransferParams P{};
+  bf::RetireParams Q{};   // the source's compaction behind the transfer
+  const uint32_t none = BF_EXTENT_NO_RUN;
+  CallStage st;
+  st.up(P.unfit, &none, 1);
+  st.up(P.runs, t->runs, n);
+  st.up(Q.to, to.data(), n);
+  st.out(P.extent, n);
+  if (int rc = st.send(c, "bf_resident_transfer")) return rc;
+  const bf_layout F = src->L;
   P.src = extent_batch(c, src, dst->L);   // the source's result records as a later tick of it compares them (bf_resident_extent)
   P.dst_state = dst->d_state; P.dst_result = dst->d_result; P.dst_mark = dst->d_mark; P.mark_value = dst->mark_must_list();
   P.dst_areas = dst->areas_view();
-  P.runs = reinterpret_cast<const uint32_t*>(c->d_transfer + o_runs); P.n = n; P.dst_first = D; P.T = dst->L;
-  P.extent = reinterpret_cast<uint4*>(c->d_transfer + o_ext); P.unfit = reinterpret_cast<uint32_t*>(c->d_transfer.p);
+  P.n = n; P.dst_first = D; P.T = dst->L;
   cudaStream_t s = c->stream;
-  BF_CUDA(c, cudaMemcpyAsync(c->d_transfer, blob.data(), blob.size(), cudaMemcpyHostToDevice, s));
   BF_CUDA(c, bf::launch_transfer_fit(P, s));
-  BF_CUDA(c, cudaMemcpyAsync(&c->pinned->word, c->d_transfer, 4, cudaMemcpyDeviceToHost, s));
+  BF_CUDA(c, cudaMemcpyAsync(&c->pinned->word, P.unfit, 4, cudaMemcpyDeviceToHost, s));
   BF_CUDA(c, cudaStreamSynchronize(s));
   c->stats.kernel_launches += 1;
   const uint32_t unfit = c->pinned->word;
   if (unfit != BF_EXTENT_NO_RUN) {   // the refused run's extent, read on this path only
     uint32_t x[4] = {};
-    BF_CUDA(c, cudaMemcpy(x, c->d_transfer + o_ext + (size_t)unfit * 16, 16, cudaMemcpyDeviceToHost));
+    BF_CUDA(c, cudaMemcpy(x, P.extent + unfit, sizeof x, cudaMemcpyDeviceToHost));
     t->unfit = unfit;
     t->why.struct_size = sizeof(bf_extent); t->why.n_runs = N;
     t->why.steps_max = std::max(1u, x[0]); t->why.child_nibbles = x[1]; t->why.fields = x[2];
@@ -792,10 +840,8 @@ int bf_resident_transfer(bf_ctx* c, uint32_t hs, uint32_t hd, bf_transfer* t) {
   for (uint32_t i = 0; i < n && src_baseline; ++i) src_baseline = t->runs[i] < src->prev_runs;
   src->state_changed(c);   // as after an upload, both batches
   dst->state_changed(c);
-  bf::RetireParams Q{};
   Q.state = src->d_state; Q.result = src->d_result; Q.mark = src->d_mark; Q.mark_value = src->mark_must_list();
-  Q.to = reinterpret_cast<const uint32_t*>(c->d_transfer + o_to); Q.m = m; Q.n = n;
-  Q.state_stride = F.state_stride; Q.result_stride = F.result_stride; Q.areas = P.src.areas;
+  Q.m = m; Q.n = n; Q.state_stride = F.state_stride; Q.result_stride = F.result_stride; Q.areas = P.src.areas;
   cudaError_t e = bf::launch_transfer(P, s);
   if (e == cudaSuccess) e = bf::launch_retire(Q, s);   // behind the transfer on the stream: the sources are read first
   if (int rc = src->sync_in_place(c, e, "bf_resident_transfer")) { dst->records_unknown(); return rc; }
@@ -819,10 +865,8 @@ int bf_resident_timers(bf_ctx* c, uint32_t h, uint32_t K) {
   BF_CUDA(c, cudaSetDevice(c->device));
   DevBuf<unsigned long long> area;
   if (cudaError_t e = area.alloc((size_t)r->cap * K)) return fail(c, BF_ENOMEM, std::string("timer area: ") + cudaGetErrorString(e));
-  cudaError_t e = bf::launch_relay_timers({r->areas.d_timers, area, r->cap, r->cap, r->areas.timer_k, K}, c->stream);
-  const cudaError_t es = cudaStreamSynchronize(c->stream);
-  if (e == cudaSuccess) e = es;
-  if (e != cudaSuccess) return cuda_fail(c, e, "bf_resident_timers");   // the old area was only read
+  const cudaError_t e = bf::launch_relay_timers({r->areas.d_timers, area, r->cap, r->cap, r->areas.timer_k, K}, c->stream);
+  if (int rc = bf::end_call(c, e, "bf_resident_timers")) return rc;   // the old area was only read
   c->stats.kernel_launches += 1;
   r->areas.d_timers = std::move(area);
   r->areas.timer_k = K;
@@ -849,50 +893,38 @@ int bf_resident_timers_arm(bf_ctx* c, uint32_t h, const bf_timer* req, uint32_t 
       return fail(c, BF_EINVAL, at() + "a code that writes needs decision planes (BF_F_DECISION)");
   }
   if (n == 0) return BF_OK;
-  std::vector<uint32_t> order(n);
-  for (uint32_t i = 0; i < n; ++i) order[i] = i;
-  auto key = [&](uint32_t i) { return (uint64_t)req[i].run << 16 | req[i].step; };
-  std::stable_sort(order.begin(), order.end(), [&](uint32_t a, uint32_t b) { return key(a) < key(b); });
+  std::vector<uint32_t> order;
+  std::pair<uint32_t, uint32_t> clash;
+  if (!order_by_run_step(req, n, order, clash))
+    return fail(c, BF_EINVAL, "requests " + std::to_string(clash.first) + " and " + std::to_string(clash.second) + " name the same (run, step)");
   std::vector<bf_timer> sorted(n);
   std::vector<uint32_t> first, arm_before(n + 1, 0);
   for (uint32_t j = 0; j < n; ++j) {
     sorted[j] = req[order[j]];
-    if (j && key(order[j]) == key(order[j - 1]))
-      return fail(c, BF_EINVAL, "requests " + std::to_string(order[j - 1]) + " and " + std::to_string(order[j]) + " name the same (run, step)");
     if (j == 0 || sorted[j].run != sorted[j - 1].run) first.push_back(j);
     arm_before[j + 1] = arm_before[j] + (sorted[j].deadline != BF_TIMER_NONE ? 1u : 0u);
   }
   const uint32_t G = (uint32_t)first.size();
   first.push_back(n);
   BF_CUDA(c, cudaSetDevice(c->device));
-  const size_t o_first = 16, o_arm = o_first + (size_t)(G + 1) * 4, o_req = round_up_sz(o_arm + (size_t)(n + 1) * 4, 16),
-               bytes = o_req + (size_t)n * sizeof(bf_timer);
-  if (int rc = c->d_timer.ensure(c, bytes)) return rc;
-  std::vector<uint8_t> blob(bytes, 0);
-  const uint32_t none = 0xFFFFFFFFu;
-  memcpy(blob.data(), &none, 4);
-  memcpy(blob.data() + o_first, first.data(), (size_t)(G + 1) * 4);
-  memcpy(blob.data() + o_arm, arm_before.data(), (size_t)(n + 1) * 4);
-  memcpy(blob.data() + o_req, sorted.data(), (size_t)n * sizeof(bf_timer));
   bf::TimerArmParams P{};
+  const uint32_t none = 0xFFFFFFFFu;
+  CallStage st;
+  st.up(P.overflow, &none, 1);
+  st.up(P.first, first.data(), G + 1);
+  st.up(P.arm_before, arm_before.data(), n + 1);
+  st.up(P.req, sorted.data(), n);
+  if (int rc = st.send(c, "bf_resident_timers_arm")) return rc;
   P.timers = r->areas.d_timers; P.timer_k = r->areas.timer_k; P.n_groups = G;
-  P.req = reinterpret_cast<const bf_timer*>(c->d_timer + o_req);
-  P.first = reinterpret_cast<const uint32_t*>(c->d_timer + o_first);
-  P.arm_before = reinterpret_cast<const uint32_t*>(c->d_timer + o_arm);
-  P.overflow = reinterpret_cast<uint32_t*>(c->d_timer.p);
   cudaStream_t s = c->stream;
-  BF_CUDA(c, cudaMemcpyAsync(c->d_timer, blob.data(), bytes, cudaMemcpyHostToDevice, s));
   BF_CUDA(c, bf::launch_arm_timers(P, false, s));
-  BF_CUDA(c, cudaMemcpyAsync(&c->pinned->word, c->d_timer, 4, cudaMemcpyDeviceToHost, s));
+  BF_CUDA(c, cudaMemcpyAsync(&c->pinned->word, P.overflow, 4, cudaMemcpyDeviceToHost, s));
   BF_CUDA(c, cudaStreamSynchronize(s));
   c->stats.kernel_launches += 1;
   if (c->pinned->word != none)
     return fail(c, BF_ENOMEM, "run " + std::to_string(sorted[first[c->pinned->word]].run) + " would hold more than " +
                                   std::to_string(r->areas.timer_k) + " armed timers");
-  cudaError_t e = bf::launch_arm_timers(P, true, s);
-  const cudaError_t es = cudaStreamSynchronize(s);
-  if (e == cudaSuccess) e = es;
-  if (e != cudaSuccess) return cuda_fail(c, e, "bf_resident_timers_arm");
+  if (int rc = bf::end_call(c, bf::launch_arm_timers(P, true, s), "bf_resident_timers_arm")) return rc;
   c->stats.kernel_launches += 1;
   return BF_OK;
 }
@@ -915,17 +947,18 @@ int bf_resident_fire(bf_ctx* c, uint32_t h, uint32_t now, bf_fire_out* out) {
   const uint32_t grid = (N - 1) / 256 + 1;
   // the list is at most N * (K + 2) long (with run control: a drain and a story entry per run): a larger fired_cap stages no more
   const uint32_t cap = (uint32_t)std::min<uint64_t>(out->fired_cap, (uint64_t)N * (A.timer_k + (A.runctl ? 2u : 0u)));
-  bf_fired* posted = static_cast<bf_fired*>(bf::pinned_dev(out->fired));
-  const size_t o_sums = 16, o_list = round_up_sz(o_sums + (size_t)grid * 4, 16), bytes = o_list + (posted ? 0 : (size_t)cap * 8);
-  if (int rc = c->d_timer.ensure(c, bytes)) return rc;
-  r->end_snapshot(c);   // as a delta
   bf::FireParams P{};
+  P.fired = static_cast<bf_fired*>(bf::pinned_dev(out->fired));   // a pinned list is posted to in place
+  const bool staged = !P.fired;
+  CallStage st;
+  st.out(P.out, 4);
+  st.out(P.block_sums, grid);
+  if (staged) st.out(P.fired, cap);
+  if (int rc = st.send(c, "bf_resident_fire")) return rc;
+  r->end_snapshot(c);   // as a delta
   P.state = r->d_state; P.areas = A; P.mark = r->d_mark; P.mark_value = r->mark_touched();
   P.n_runs = N; P.now = now;
   P.words = r->L.words; P.state_stride = r->L.state_stride; P.off_phase = r->L.off_phase; P.off_decision = r->L.off_decision;
-  P.out = reinterpret_cast<uint32_t*>(c->d_timer.p);
-  P.block_sums = reinterpret_cast<uint32_t*>(c->d_timer + o_sums);
-  P.fired = posted ? posted : reinterpret_cast<bf_fired*>(c->d_timer + o_list);
   P.fired_cap = cap;
   cudaStream_t s = c->stream;
   uint32_t* words = c->pinned->fire;
@@ -933,7 +966,7 @@ int bf_resident_fire(bf_ctx* c, uint32_t h, uint32_t now, bf_fire_out* out) {
   if (e == cudaSuccess) e = cudaMemcpyAsync(words, P.out, 16, cudaMemcpyDeviceToHost, s);
   if (int rc = r->sync_in_place(c, e, "bf_resident_fire")) return rc;
   c->stats.kernel_launches += 2;
-  if (const uint32_t listed = std::min(words[0], cap); listed && !posted)
+  if (const uint32_t listed = std::min(words[0], cap); listed && staged)
     BF_CUDA(c, cudaMemcpy(out->fired, P.fired, (size_t)listed * 8, cudaMemcpyDeviceToHost));
   out->n_fired = words[0]; out->n_written = words[1]; out->n_pruned = words[2]; out->next_deadline = words[3];
   r->pending += out->n_written;   // the touched-list bound counts the written codes and the timeouts as it counts deltas
@@ -945,13 +978,7 @@ int bf_resident_timers_download(bf_ctx* c, uint32_t h, uint32_t first, uint32_t 
   auto [g, r] = lock_resident(c, h);
   if (!r) return BF_EINVAL;
   if (!r->areas.timer_k) return fail(c, BF_EINVAL, "the batch has no timer area (bf_resident_timers)");
-  if ((uint64_t)first + n > r->cap || (n && !slots)) return fail(c, BF_EINVAL, "run range outside the resident batch");
-  if (n == 0) return BF_OK;
-  BF_CUDA(c, cudaSetDevice(c->device));
-  const RunAreas& a = r->areas;
-  BF_CUDA(c, cudaMemcpyAsync(slots, a.d_timers + (size_t)first * a.timer_k, (size_t)n * a.timer_k * 8, cudaMemcpyDeviceToHost, c->stream));
-  BF_CUDA(c, cudaStreamSynchronize(c->stream));
-  return BF_OK;
+  return download_runs(c, r, first, n, slots, r->areas.d_timers, (size_t)r->areas.timer_k * 8);
 }
 
 // ---- resident limiters (limiters.cu) ------------------------------------------------------------------------------------------
@@ -968,9 +995,7 @@ int bf_resident_sched(bf_ctx* c, uint32_t h) {
   if (e == cudaSuccess) e = RunAreas::alloc_sched_rec(rec, r->cap, r->L.words, c->stream);
   if (e != cudaSuccess) return fail(c, BF_ENOMEM, std::string("limiter inputs: ") + cudaGetErrorString(e));
   e = cudaMemcpyAsync(in, defaults.data(), (size_t)r->cap * sizeof(bf_sched_run), cudaMemcpyHostToDevice, c->stream);
-  const cudaError_t es = cudaStreamSynchronize(c->stream);
-  if (e == cudaSuccess) e = es;
-  if (e != cudaSuccess) return cuda_fail(c, e, "bf_resident_sched");
+  if (int rc = bf::end_call(c, e, "bf_resident_sched")) return rc;
   r->areas.d_sched_in = std::move(in);
   r->areas.d_sched_rec = std::move(rec);
   r->areas.sched_base_runs = 0;
@@ -983,26 +1008,21 @@ int bf_resident_sched_put(bf_ctx* c, uint32_t h, const bf_sched_put* req, uint32
   if (!r) return BF_EINVAL;
   if (!r->areas.d_sched_in) return fail(c, BF_EINVAL, "the batch has no limiter inputs (bf_resident_sched)");
   if (n && !req) return fail(c, BF_EINVAL, "null requests");
-  std::vector<uint32_t> seen;   // request index + 1 per run named so far
+  std::vector<uint32_t> seen;
   for (uint32_t i = 0; i < n; ++i) {
     const bf_sched_put& q = req[i];
     auto at = [i] { return "request " + std::to_string(i) + ": "; };
     if (q.run >= r->cap) return fail(c, BF_EINVAL, at() + "run outside the resident batch");
     if (q.reserved[0] || q.reserved[1]) return fail(c, BF_EINVAL, at() + "reserved fields must be 0");
-    if (seen.empty()) seen.assign(r->cap, 0u);
-    if (seen[q.run]) return fail(c, BF_EINVAL, "requests " + std::to_string(seen[q.run] - 1) + " and " + std::to_string(i) + " name the same run");
-    seen[q.run] = i + 1;
+    if (int rc = name_run_once(c, seen, r->cap, q.run, i)) return rc;
   }
   if (n == 0) return BF_OK;
   BF_CUDA(c, cudaSetDevice(c->device));
-  if (int rc = c->d_rsched.ensure(c, (size_t)n * sizeof(bf_sched_put))) return rc;
-  bf::SchedPutParams P{r->areas.d_sched_in, reinterpret_cast<const bf_sched_put*>(c->d_rsched.p), n};
-  cudaStream_t s = c->stream;
-  cudaError_t e = cudaMemcpyAsync(c->d_rsched, req, (size_t)n * sizeof(bf_sched_put), cudaMemcpyHostToDevice, s);
-  if (e == cudaSuccess) e = bf::launch_sched_put(P, s);
-  const cudaError_t es = cudaStreamSynchronize(s);
-  if (e == cudaSuccess) e = es;
-  if (e != cudaSuccess) return cuda_fail(c, e, "bf_resident_sched_put");
+  bf::SchedPutParams P{r->areas.d_sched_in, nullptr, n};
+  CallStage st;
+  st.up(P.req, req, n);
+  if (int rc = st.send(c, "bf_resident_sched_put")) return rc;
+  if (int rc = bf::end_call(c, bf::launch_sched_put(P, c->stream), "bf_resident_sched_put")) return rc;
   c->stats.kernel_launches += 1;
   return BF_OK;
 }
@@ -1011,14 +1031,14 @@ int bf_resident_sched_download(bf_ctx* c, uint32_t h, uint32_t first, uint32_t n
   auto [g, r] = lock_resident(c, h);
   if (!r) return BF_EINVAL;
   if (!r->areas.d_sched_in) return fail(c, BF_EINVAL, "the batch has no limiter inputs (bf_resident_sched)");
-  if ((uint64_t)first + n > r->cap || (n && !out)) return fail(c, BF_EINVAL, "run range outside the resident batch");
-  if (n == 0) return BF_OK;
-  BF_CUDA(c, cudaSetDevice(c->device));
-  std::vector<bf_sched_run> in(n);
-  BF_CUDA(c, cudaMemcpyAsync(in.data(), r->areas.d_sched_in + first, (size_t)n * sizeof(bf_sched_run), cudaMemcpyDeviceToHost, c->stream));
-  BF_CUDA(c, cudaStreamSynchronize(c->stream));
-  for (uint32_t i = 0; i < n; ++i)
-    out[i] = bf_sched_put{first + i, in[i].story_key, in[i].queue_key, in[i].priority, in[i].queued_elapsed_s, in[i].run_phase, {0u, 0u}};
+  // the inputs land in the caller's buffer and become puts there, one record at a time
+  static_assert(sizeof(bf_sched_run) == sizeof(bf_sched_put), "a put takes the place of its run's inputs");
+  if (int rc = download_runs(c, r, first, n, out, r->areas.d_sched_in, sizeof(bf_sched_run))) return rc;
+  for (uint32_t i = 0; i < n; ++i) {
+    bf_sched_run in;
+    memcpy(&in, &out[i], sizeof in);
+    out[i] = bf_sched_put{first + i, in.story_key, in.queue_key, in.priority, in.queued_elapsed_s, in.run_phase, {0u, 0u}};
+  }
   return BF_OK;
 }
 
@@ -1056,50 +1076,39 @@ int bf_resident_schedule(bf_ctx* c, const bf_sched_tables* t, uint32_t now, bf_r
   BF_CUDA(c, cudaSetDevice(c->device));
   cudaStream_t s = c->stream;
   if (int rc = bf::sync_slots(c, s)) return rc;   // topology puts and drops since the ticks count as they stand now
-  // one device allocation: tables | totals | per part: run events | CTA listed | CTA events | two totals | staged lists
+  // tables | totals | per part: run events | CTA listed | CTA events | two totals | staged lists
   const size_t ns = t->n_stories, nq = t->n_queues;
-  size_t off = 0;
-  auto take = [&](size_t bytes) { const size_t o = off; off = round_up_sz(off + bytes, 16); return o; };
-  const size_t o_sl = take(ns * 4), o_ql = take(nq * 4), o_qa = take(nq * 4), o_sb = take(ns * 4), o_qb = take(nq * 4),
-               o_pb = take(nq * 4), o_sr = take(ns * 4), o_qr = take(nq * 4), o_mp = take(nq * 4), o_gl = take(4);
-  struct Plan { size_t ev, cl, ce, tot, runs, heads, events; uint32_t rcap; uint64_t ecap; uint32_t* p_runs; bf_sched_header* p_heads; uint16_t* p_events; };
+  bf::SchedParams S{};
+  CallStage st;
+  st.up(S.story_limit, t->story_limit, ns);
+  st.up(S.queue_limit, t->queue_limit, nq);
+  st.up(S.queue_aging, t->queue_aging_s, nq);
+  if (t->story_running_base) st.up(S.story_base, t->story_running_base, ns);
+  if (t->queue_running_base) st.up(S.queue_base, t->queue_running_base, nq);
+  if (t->queue_max_priority_base) st.up(S.queue_maxprio_base, t->queue_max_priority_base, nq);
+  st.out(S.story_running, ns); st.out(S.queue_running, nq); st.out(S.queue_maxprio, nq); st.out(S.global_running, 1);
+  // each part's lists go straight into the caller's buffers when they are pinned, else into staged ones copied after the call
+  struct Plan { bf::ResSchedParams R; bool stage_runs, stage_events; };
   std::vector<Plan> plan(n_parts);
   for (uint32_t i = 0; i < n_parts; ++i) {
     const bf_resident_sched_part& p = parts[i];
     Plan& q = plan[i];
+    bf::ResSchedParams& R = q.R;
     const size_t grid = ((size_t)p.n_runs + 255) / 256;
-    q.rcap = std::min(p.runs_cap, p.n_runs);
-    q.ecap = std::min<uint64_t>(p.events_cap, (uint64_t)p.n_runs * rs[i]->L.words * 32);
-    q.p_runs = q.rcap ? static_cast<uint32_t*>(bf::pinned_dev(p.runs)) : nullptr;
-    q.p_heads = q.rcap ? static_cast<bf_sched_header*>(bf::pinned_dev(p.heads)) : nullptr;
-    q.p_events = q.ecap ? static_cast<uint16_t*>(bf::pinned_dev(p.events)) : nullptr;
-    const bool stage_runs = q.rcap && !(q.p_runs && q.p_heads);
-    q.ev = take((size_t)p.n_runs * 4); q.cl = take(grid * 4); q.ce = take(grid * 8); q.tot = take(16);
-    q.runs = take(stage_runs ? (size_t)q.rcap * 4 : 0); q.heads = take(stage_runs ? (size_t)q.rcap * sizeof(bf_sched_header) : 0);
-    q.events = take(q.ecap && !q.p_events ? (size_t)q.ecap * 2 : 0);
-    if (!stage_runs && q.rcap) q.runs = q.heads = SIZE_MAX;   // posted in place
+    R.runs_cap = std::min(p.runs_cap, p.n_runs);
+    R.events_cap = std::min<uint64_t>(p.events_cap, (uint64_t)p.n_runs * rs[i]->L.words * 32);
+    R.runs = R.runs_cap ? static_cast<uint32_t*>(bf::pinned_dev(p.runs)) : nullptr;
+    R.heads = R.runs_cap ? static_cast<bf_sched_header*>(bf::pinned_dev(p.heads)) : nullptr;
+    R.events = R.events_cap ? static_cast<uint16_t*>(bf::pinned_dev(p.events)) : nullptr;
+    q.stage_runs = R.runs_cap && !(R.runs && R.heads);
+    q.stage_events = R.events_cap && !R.events;
+    st.out(R.run_events, p.n_runs); st.out(R.cta_listed, grid); st.out(R.cta_events, grid); st.out(R.totals, 2);
+    if (q.stage_runs) { st.out(R.runs, R.runs_cap); st.out(R.heads, R.runs_cap); }
+    if (q.stage_events) st.out(R.events, R.events_cap);
   }
-  if (int rc = c->d_rsched.ensure(c, off ? off : 16)) return rc;
-  uint8_t* d = c->d_rsched;
-  auto up = [&](size_t o, const void* src, size_t bytes) -> cudaError_t {
-    return (src && bytes) ? cudaMemcpyAsync(d + o, src, bytes, cudaMemcpyHostToDevice, s) : cudaSuccess;
-  };
-  BF_CUDA(c, up(o_sl, t->story_limit, ns * 4));
-  BF_CUDA(c, up(o_ql, t->queue_limit, nq * 4));
-  BF_CUDA(c, up(o_qa, t->queue_aging_s, nq * 4));
-  BF_CUDA(c, up(o_sb, t->story_running_base, ns * 4));
-  BF_CUDA(c, up(o_qb, t->queue_running_base, nq * 4));
-  BF_CUDA(c, up(o_pb, t->queue_max_priority_base, nq * 4));
-  bf::SchedParams S{};
+  if (int rc = st.send(c, "bf_resident_schedule")) return rc;
   S.n_stories = t->n_stories; S.n_queues = t->n_queues; S.global_limit = t->global_limit; S.global_base = t->global_running_base;
   S.n_slots = (uint32_t)c->slots_host.size(); S.slots = c->slots_dev; S.now = now;
-  S.story_running = reinterpret_cast<uint32_t*>(d + o_sr); S.queue_running = reinterpret_cast<uint32_t*>(d + o_qr);
-  S.queue_maxprio = reinterpret_cast<int32_t*>(d + o_mp); S.global_running = reinterpret_cast<uint32_t*>(d + o_gl);
-  S.story_limit = reinterpret_cast<const int32_t*>(d + o_sl); S.queue_limit = reinterpret_cast<const int32_t*>(d + o_ql);
-  S.queue_aging = reinterpret_cast<const int32_t*>(d + o_qa);
-  S.story_base = t->story_running_base ? reinterpret_cast<const uint32_t*>(d + o_sb) : nullptr;
-  S.queue_base = t->queue_running_base ? reinterpret_cast<const uint32_t*>(d + o_qb) : nullptr;
-  S.queue_maxprio_base = t->queue_max_priority_base ? reinterpret_cast<const int32_t*>(d + o_pb) : nullptr;
   auto part_params = [&](uint32_t i) {
     const Resident* r = rs[i];
     const bf_layout& L = r->L;
@@ -1117,43 +1126,30 @@ int bf_resident_schedule(bf_ctx* c, const bf_sched_tables* t, uint32_t now, bf_r
     for (uint32_t i = 0; i < n_parts && e == cudaSuccess; ++i)
       if (parts[i].n_runs) { e = bf::launch_schedule(part_params(i), (uint32_t)c->sm_count, s, bf::kSchedCount); ++launches; }
     for (uint32_t i = 0; i < n_parts && e == cudaSuccess; ++i) {
-      const Plan& q = plan[i];
-      bf::ResSchedParams R{};
+      bf::ResSchedParams R = plan[i].R;
       R.S = part_params(i);
       R.base_runs = rs[i]->areas.sched_base_runs;
-      R.run_events = reinterpret_cast<uint32_t*>(d + q.ev);
-      R.cta_listed = reinterpret_cast<uint32_t*>(d + q.cl);
-      R.cta_events = reinterpret_cast<unsigned long long*>(d + q.ce);
-      R.totals = reinterpret_cast<unsigned long long*>(d + q.tot);
-      R.runs_cap = q.rcap; R.events_cap = q.ecap;
-      if (q.rcap) {
-        R.runs = q.runs == SIZE_MAX ? q.p_runs : reinterpret_cast<uint32_t*>(d + q.runs);
-        R.heads = q.heads == SIZE_MAX ? q.p_heads : reinterpret_cast<bf_sched_header*>(d + q.heads);
-      }
-      if (q.ecap) R.events = q.p_events ? q.p_events : reinterpret_cast<uint16_t*>(d + q.events);
       if (parts[i].n_runs) {
         e = bf::launch_resident_schedule(R, s);
         launches += 3;
         if (e == cudaSuccess) e = cudaMemcpyAsync(&part_tot[2 * i], R.totals, 16, cudaMemcpyDeviceToHost, s);
       }
     }
-    auto down = [&](void* dst, size_t o, size_t bytes) -> cudaError_t {
-      return (dst && bytes) ? cudaMemcpyAsync(dst, d + o, bytes, cudaMemcpyDeviceToHost, s) : cudaSuccess;
+    auto down = [&](void* dst, const void* from, size_t bytes) -> cudaError_t {
+      return (dst && bytes) ? cudaMemcpyAsync(dst, from, bytes, cudaMemcpyDeviceToHost, s) : cudaSuccess;
     };
-    if (e == cudaSuccess) e = down(totals->story_running, o_sr, ns * 4);
-    if (e == cudaSuccess) e = down(totals->queue_running, o_qr, nq * 4);
-    if (e == cudaSuccess) e = down(totals->queue_max_priority, o_mp, nq * 4);
-    if (e == cudaSuccess) e = down(totals->global_running, o_gl, 4);
+    if (e == cudaSuccess) e = down(totals->story_running, S.story_running, ns * 4);
+    if (e == cudaSuccess) e = down(totals->queue_running, S.queue_running, nq * 4);
+    if (e == cudaSuccess) e = down(totals->queue_max_priority, S.queue_maxprio, nq * 4);
+    if (e == cudaSuccess) e = down(totals->global_running, S.global_running, 4);
     return e;
   };
   for (Resident* r : rs) r->scheduled = -1;   // a commit reads the records this call writes
-  cudaError_t e = body();
-  const cudaError_t es = cudaStreamSynchronize(s);   // never return with copies into the caller's buffers in flight
-  if (e == cudaSuccess) e = es;
+  const cudaError_t e = body();
   c->stats.kernel_launches += launches;
-  if (e != cudaSuccess) {   // the schedule records may be half written: no baseline survives
+  if (int rc = bf::end_call(c, e, "bf_resident_schedule")) {   // the schedule records may be half written: no baseline survives
     for (Resident* r : rs) r->areas.sched_base_runs = 0;
-    return cuda_fail(c, e, "bf_resident_schedule");
+    return rc;
   }
   for (uint32_t i = 0; i < n_parts; ++i) {
     bf_resident_sched_part& p = parts[i];
@@ -1163,13 +1159,13 @@ int bf_resident_schedule(bf_ctx* c, const bf_sched_tables* t, uint32_t now, bf_r
     p.full = p.n_listed == p.n_runs ? 1u : 0u;
     rs[i]->areas.sched_base_runs = p.n_runs;
     rs[i]->scheduled = std::max<int64_t>(rs[i]->scheduled, p.n_runs);
-    const uint32_t nl = std::min(p.n_listed, q.rcap);
-    if (nl && q.runs != SIZE_MAX) {
-      BF_CUDA(c, cudaMemcpy(p.runs, d + q.runs, (size_t)nl * 4, cudaMemcpyDeviceToHost));
-      BF_CUDA(c, cudaMemcpy(p.heads, d + q.heads, (size_t)nl * sizeof(bf_sched_header), cudaMemcpyDeviceToHost));
+    const uint32_t nl = std::min(p.n_listed, q.R.runs_cap);
+    if (nl && q.stage_runs) {
+      BF_CUDA(c, cudaMemcpy(p.runs, q.R.runs, (size_t)nl * 4, cudaMemcpyDeviceToHost));
+      BF_CUDA(c, cudaMemcpy(p.heads, q.R.heads, (size_t)nl * sizeof(bf_sched_header), cudaMemcpyDeviceToHost));
     }
-    const uint64_t ne = std::min<uint64_t>(p.n_events, q.ecap);
-    if (ne && !q.p_events) BF_CUDA(c, cudaMemcpy(p.events, d + q.events, (size_t)ne * 2, cudaMemcpyDeviceToHost));
+    const uint64_t ne = std::min<uint64_t>(p.n_events, q.R.events_cap);
+    if (ne && q.stage_events) BF_CUDA(c, cudaMemcpy(p.events, q.R.events, (size_t)ne * 2, cudaMemcpyDeviceToHost));
   }
   return BF_OK;
 }
@@ -1185,9 +1181,7 @@ int bf_resident_runctl(bf_ctx* c, uint32_t h) {
   if (cudaError_t e = area.alloc(r->cap)) return fail(c, BF_ENOMEM, std::string("run control: ") + cudaGetErrorString(e));
   cudaError_t e = cudaMemsetAsync(area, 0, (size_t)r->cap * sizeof(bf_run_ctl), c->stream);
   if (e == cudaSuccess) e = cudaMemset2DAsync(area, sizeof(bf_run_ctl), 0xFF, 8, r->cap, c->stream);   // both deadlines
-  const cudaError_t es = cudaStreamSynchronize(c->stream);
-  if (e == cudaSuccess) e = es;
-  if (e != cudaSuccess) return cuda_fail(c, e, "bf_resident_runctl");
+  if (int rc = bf::end_call(c, e, "bf_resident_runctl")) return rc;
   r->areas.d_runctl = std::move(area);
   return BF_OK;
 }
@@ -1199,7 +1193,7 @@ int bf_resident_runctl_put(bf_ctx* c, uint32_t h, const bf_run_ctl_put* req, uin
   if (!r) return BF_EINVAL;
   if (!r->areas.d_runctl) return fail(c, BF_EINVAL, "the batch has no run-control area (bf_resident_runctl)");
   if (n && !req) return fail(c, BF_EINVAL, "null requests");
-  std::vector<uint32_t> seen;   // request index + 1 per run named so far
+  std::vector<uint32_t> seen;
   uint32_t stops = 0;
   for (uint32_t i = 0; i < n; ++i) {
     const bf_run_ctl_put& q = req[i];
@@ -1207,21 +1201,19 @@ int bf_resident_runctl_put(bf_ctx* c, uint32_t h, const bf_run_ctl_put* req, uin
     if (q.run >= r->cap) return fail(c, BF_EINVAL, at() + "run outside the resident batch");
     if (q.stop > BF_STOP_HOST) return fail(c, BF_EINVAL, at() + "stop is not a BF_STOP_* code");
     if (q.reserved[0] || q.reserved[1] || q.reserved[2]) return fail(c, BF_EINVAL, at() + "reserved fields must be 0");
-    if (seen.empty()) seen.assign(r->cap, 0u);
-    if (seen[q.run]) return fail(c, BF_EINVAL, "requests " + std::to_string(seen[q.run] - 1) + " and " + std::to_string(i) + " name the same run");
-    seen[q.run] = i + 1;
+    if (int rc = name_run_once(c, seen, r->cap, q.run, i)) return rc;
     stops += q.stop ? 1u : 0u;
   }
   if (n == 0) return BF_OK;
   BF_CUDA(c, cudaSetDevice(c->device));
-  if (int rc = c->d_runctl_put.ensure(c, n)) return rc;
-  if (stops) r->state_changed(c);   // as a delta
   bf::RunCtlPutParams P{};
-  P.area = r->areas.d_runctl; P.req = c->d_runctl_put; P.n = n; P.state = r->d_state; P.state_stride = r->L.state_stride;
+  CallStage st;
+  st.up(P.req, req, n);
+  if (int rc = st.send(c, "bf_resident_runctl_put")) return rc;
+  if (stops) r->state_changed(c);   // as a delta
+  P.area = r->areas.d_runctl; P.n = n; P.state = r->d_state; P.state_stride = r->L.state_stride;
   P.stop = bf::StopParams{r->areas_view(), r->d_mark, r->mark_touched()};
-  cudaError_t e = cudaMemcpyAsync(c->d_runctl_put, req, (size_t)n * sizeof(bf_run_ctl_put), cudaMemcpyHostToDevice, c->stream);
-  if (e == cudaSuccess) e = bf::launch_runctl_put(P, c->stream);
-  if (int rc = r->sync_in_place(c, e, "bf_resident_runctl_put")) return rc;
+  if (int rc = r->sync_in_place(c, bf::launch_runctl_put(P, c->stream), "bf_resident_runctl_put")) return rc;
   c->stats.kernel_launches += 1;
   r->pending += stops;   // the touched-list bound counts the stopped runs as it counts deltas
   return BF_OK;
@@ -1231,12 +1223,7 @@ int bf_resident_runctl_download(bf_ctx* c, uint32_t h, uint32_t first, uint32_t 
   auto [g, r] = lock_resident(c, h);
   if (!r) return BF_EINVAL;
   if (!r->areas.d_runctl) return fail(c, BF_EINVAL, "the batch has no run-control area (bf_resident_runctl)");
-  if ((uint64_t)first + n > r->cap || (n && !out)) return fail(c, BF_EINVAL, "run range outside the resident batch");
-  if (n == 0) return BF_OK;
-  BF_CUDA(c, cudaSetDevice(c->device));
-  BF_CUDA(c, cudaMemcpyAsync(out, r->areas.d_runctl + first, (size_t)n * sizeof(bf_run_ctl), cudaMemcpyDeviceToHost, c->stream));
-  BF_CUDA(c, cudaStreamSynchronize(c->stream));
-  return BF_OK;
+  return download_runs(c, r, first, n, out, r->areas.d_runctl, sizeof(bf_run_ctl));
 }
 
 // ---- tick commits (resident.cu) -----------------------------------------------------------------------------------------------
@@ -1269,7 +1256,6 @@ int bf_resident_commit(bf_ctx* c, uint32_t h, uint32_t n_runs, const bf_commit_e
   const bf::RunAreasView A = r->areas_view();
   if (A.sched_in && r->scheduled < (int64_t)n_runs)
     return refuse(BF_COMMIT_NONE, BF_COMMIT_NONE, "the batch has limiter inputs and no bf_resident_schedule" + over + " ran since its last tick");
-  std::vector<std::pair<uint64_t, uint32_t>> order(n);   // (run << 16 | step, index)
   for (uint32_t i = 0; i < n; ++i) {
     const bf_commit_entry& e = entries[i];
     auto at = [i] { return "entry " + std::to_string(i) + ": "; };
@@ -1278,40 +1264,37 @@ int bf_resident_commit(bf_ctx* c, uint32_t h, uint32_t n_runs, const bf_commit_e
     if (e.kind < BF_COMMIT_HOLD || e.kind > BF_COMMIT_PHASE) return refuse(e.run, e.step, at() + "kind is not a BF_COMMIT_* code");
     if (e.kind == BF_COMMIT_PHASE ? (e.code < BF_PHASE_PENDING || e.code > BF_PHASE_SKIPPED) : e.code != 0)
       return refuse(e.run, e.step, at() + "bad code (a BF_COMMIT_PHASE entry takes BF_PHASE_PENDING .. BF_PHASE_SKIPPED, the others 0)");
-    order[i] = {(uint64_t)e.run << 16 | e.step, i};
   }
-  std::sort(order.begin(), order.end());
-  for (uint32_t i = 1; i < n; ++i)
-    if (order[i].first == order[i - 1].first) {
-      const bf_commit_entry& e = entries[order[i].second];
-      return refuse(e.run, e.step, "entries " + std::to_string(order[i - 1].second) + " and " + std::to_string(order[i].second) +
-                                       " name the same (run, step)");
-    }
+  std::vector<uint32_t> order;
+  std::pair<uint32_t, uint32_t> clash;
+  if (!order_by_run_step(entries, n, order, clash)) {
+    const bf_commit_entry& e = entries[clash.second];
+    return refuse(e.run, e.step, "entries " + std::to_string(clash.first) + " and " + std::to_string(clash.second) + " name the same (run, step)");
+  }
   if (n_runs == 0) return BF_OK;
   BF_CUDA(c, cudaSetDevice(c->device));
   cudaStream_t s = c->stream;
   if (int rc = bf::sync_slots(c, s)) return rc;   // the slot table as it stands now
-  const size_t o_entries = 32, bytes = o_entries + (size_t)n * sizeof(bf_commit_entry);
-  if (int rc = c->d_commit.ensure(c, bytes)) return rc;
-  std::vector<uint8_t> blob(bytes, 0);
-  memset(blob.data(), 0xFF, 8);   // no offender yet; the counts start at zero
-  for (uint32_t i = 0; i < n; ++i) memcpy(blob.data() + o_entries + (size_t)i * sizeof(bf_commit_entry), &entries[order[i].second], sizeof(bf_commit_entry));
+  std::vector<bf_commit_entry> sorted(n);
+  for (uint32_t i = 0; i < n; ++i) sorted[i] = entries[order[i]];
   bf::CommitParams P{};
+  const unsigned long long no_offender = ~0ull;
+  const uint32_t zero_counts[5] = {};
+  CallStage st;
+  st.up(P.offender, &no_offender, 1);
+  st.up(P.counts, zero_counts, 5);
+  st.up(P.entries, sorted.data(), n);
+  if (int rc = st.send(c, "bf_resident_commit (check)")) return rc;
   P.state = r->d_state; P.result = r->d_result; P.sched_rec = A.sched_rec;
   P.slots = c->slots_dev; P.n_slots = (uint32_t)c->slots_host.size();
-  P.entries = reinterpret_cast<const bf_commit_entry*>(c->d_commit + o_entries); P.n_entries = n; P.n_runs = n_runs;
+  P.n_entries = n; P.n_runs = n_runs;
   P.words = L.words; P.state_stride = L.state_stride; P.off_phase = L.off_phase; P.result_stride = L.result_stride;
   P.off_ready = L.off_ready; P.off_skip = L.off_skip; P.off_fail = L.off_fail; P.sched_stride = A.sched_stride;
   P.mark = r->d_mark; P.mark_value = r->mark_touched();
-  P.offender = reinterpret_cast<unsigned long long*>(c->d_commit.p);
-  P.counts = reinterpret_cast<uint32_t*>(c->d_commit + 8);
   uint32_t* host = c->pinned->commit;
-  cudaError_t e = cudaMemcpyAsync(c->d_commit, blob.data(), bytes, cudaMemcpyHostToDevice, s);
-  if (e == cudaSuccess) e = bf::launch_commit(P, false, s);
-  if (e == cudaSuccess) e = cudaMemcpyAsync(host, c->d_commit, 8, cudaMemcpyDeviceToHost, s);
-  const cudaError_t es = cudaStreamSynchronize(s);
-  if (e == cudaSuccess) e = es;
-  if (e != cudaSuccess) return cuda_fail(c, e, "bf_resident_commit (check)");
+  cudaError_t e = bf::launch_commit(P, false, s);
+  if (e == cudaSuccess) e = cudaMemcpyAsync(host, P.offender, 8, cudaMemcpyDeviceToHost, s);
+  if (int rc = bf::end_call(c, e, "bf_resident_commit (check)")) return rc;
   c->stats.kernel_launches += 1;
   uint64_t key;
   memcpy(&key, host, 8);
@@ -1323,7 +1306,7 @@ int bf_resident_commit(bf_ctx* c, uint32_t h, uint32_t n_runs, const bf_commit_e
                                                                  : "a launched stop step has no BF_COMMIT_PHASE entry"));
   }
   e = bf::launch_commit(P, true, s);
-  if (e == cudaSuccess) e = cudaMemcpyAsync(host, c->d_commit + 8, 20, cudaMemcpyDeviceToHost, s);
+  if (e == cudaSuccess) e = cudaMemcpyAsync(host, P.counts, 20, cudaMemcpyDeviceToHost, s);
   if (int rc = r->sync_in_place(c, e, "bf_resident_commit")) { r->state_changed(c); return rc; }
   c->stats.kernel_launches += 1;
   uint32_t k[5];
