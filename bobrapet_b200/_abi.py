@@ -197,6 +197,10 @@ class CommitOut(C.Structure):
                                           "bad_run", "bad_step")]
 
 
+class CommitArm(C.Structure):
+    _fields_ = [(n, C.c_uint32) for n in ("struct_size", "now", "n_armed", "next_deadline")]
+
+
 def sched_stride(words: int) -> int:
     return (16 + 12 * words + 15) & ~15
 
@@ -214,6 +218,7 @@ SYMBOLS = [
     ("bf_topology_check", C.c_int, [C.c_void_p, C.POINTER(C.c_uint32), C.c_uint32, C.POINTER(C.c_uint32)]),
     ("bf_topology_closure", C.c_int, [C.c_void_p, C.POINTER(C.c_uint32), C.POINTER(C.c_uint32), C.c_uint32, C.c_uint32, C.POINTER(C.c_uint32)]),
     ("bf_topology_drop", C.c_int, [C.c_void_p, C.c_uint32]),
+    ("bf_topology_timings", C.c_int, [C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32]),
     ("bf_topology_child_first", C.c_int, [C.c_void_p, C.c_uint32, C.POINTER(C.c_uint32), C.c_uint32]),
     ("bf_layout_init", C.c_int, [C.POINTER(Layout), C.c_uint32, C.c_uint32, C.c_uint32]),
     ("bf_eval", C.c_int, [C.c_void_p, C.POINTER(Batch)]),
@@ -250,6 +255,8 @@ SYMBOLS = [
     ("bf_resident_runctl_put", C.c_int, [C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32]),
     ("bf_resident_runctl_download", C.c_int, [C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32, C.c_void_p]),
     ("bf_resident_commit", C.c_int, [C.c_void_p, C.c_uint32, C.c_uint32, C.c_void_p, C.c_uint32, C.POINTER(CommitOut)]),
+    ("bf_resident_commit_timed", C.c_int, [C.c_void_p, C.c_uint32, C.c_uint32, C.c_void_p, C.c_uint32, C.POINTER(CommitOut),
+                                           C.POINTER(CommitArm)]),
     ("bf_group_create", C.c_int, [C.POINTER(C.c_void_p), C.POINTER(C.c_int32), C.c_uint32, C.POINTER(Config)]),
     ("bf_group_destroy", None, [C.c_void_p]),
     ("bf_group_size", C.c_uint32, [C.c_void_p]),

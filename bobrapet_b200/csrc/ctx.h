@@ -127,6 +127,8 @@ struct TopoMeta {
   std::vector<uint32_t> child_first;
   std::vector<uint16_t> par_step, par_branches;   // step and branch count of each parallel desc (bf_resident_migrate)
   uint32_t child_nibbles = 0;
+  std::vector<uint8_t> types;            // BF_STEP_* of each step (bf_topology_timings checks the codes against them)
+  std::vector<bf_step_timing> timings;   // bf_topology_timings, ascending by step
   bool fits(const bf_layout& L) const { return S <= L.steps_max && (L.off_child == BF_OFF_NONE || child_nibbles <= L.child_nibbles); }
 };
 
@@ -160,6 +162,13 @@ struct bf_ctx {
   uint32_t n_with_parallel = 0;  // live topologies that have parallel steps
   uint64_t slot_changes = 0;     // slot drops and reuses so far: either changes what the runs holding the slot evaluate
                                  // to, so a touched tick after one evaluates every run
+  // step timings of every slot (bf_topology_timings) as one table, slot s at [tim_first[s], tim_first[s + 1]), built and copied
+  // to the device by the first arming commit after a change (sync_timings); nothing is allocated until a slot has timings
+  bool timings_dirty = false;
+  std::vector<uint32_t> tim_first_host;
+  std::vector<bf_step_timing> tim_host;
+  DevBuf<uint32_t> tim_first_dev;
+  DevBuf<bf_step_timing> tim_dev;
 
   // host-API staging
   DevBuf<uint8_t> d_state, d_result;
@@ -499,6 +508,8 @@ namespace bf {
 // the topology arena (topology.cu)
 int grow_arena(bf_ctx* c, size_t need_total);
 int sync_slots(bf_ctx* c, cudaStream_t stream);
+// the timing table of a commit that arms (one copy when a timing changed since the last): P.tim stays nullptr when no slot has one
+int sync_timings(bf_ctx* c, cudaStream_t stream, CommitTimings& P);
 uint32_t largest_record(bf_ctx* c, uint32_t w);
 
 // host helpers of a pass, defined in abi.cu and used by resident_abi.cu too

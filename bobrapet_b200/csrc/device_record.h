@@ -461,8 +461,20 @@ struct RunCtlRestopParams {
 };
 
 // bf_resident_commit (resident.cu): commit_check over runs [0, n_runs) lowers *offender, then commit_apply writes the records.
-// Entries are sorted by (run, step).  The offender key is run << 32 | step << 8 | reason (kCommitNotLaunched, ...).
-enum : uint32_t { kCommitNotLaunched = 1, kCommitNotStop = 2, kCommitNoPhase = 3 };
+// Entries are sorted by (run, step).  The offender key is run << 32 | step << 8 | reason (kCommitNotLaunched, ...).  With a
+// timing table (bf_resident_commit_timed) both launches also take the arms: the check adds kCommitNoDecision and
+// kCommitOverflow, the apply merges the new slots into the timer area.
+enum : uint32_t { kCommitNotLaunched = 1, kCommitNotStop = 2, kCommitNoPhase = 3, kCommitNoDecision = 4, kCommitOverflow = 5 };
+// the step timings of every topology slot (bf_topology_timings), one table: slot s has tim[first[s], first[s + 1]), ascending by step
+struct CommitTimings {
+  const bf_step_timing* tim;     // or nullptr: the commit arms nothing
+  const uint32_t* first;         // [n_slots + 1]
+  uint32_t n_slots;              // slots at or above it have no timings
+  unsigned long long* timers;    // the batch's timer area, timer_k slots per run
+  uint32_t timer_k, now;
+  bool decision;                 // the layout has decision planes
+  uint32_t* out;                 // [2] commit_apply: slots armed (atomicAdd), earliest deadline armed (atomicMin; NONE from the caller)
+};
 struct CommitParams {
   uint8_t* state;
   const uint8_t* result;         // the current result records
@@ -477,6 +489,7 @@ struct CommitParams {
   uint32_t mark_value;
   unsigned long long* offender;  // [1] commit_check: lowest key (atomicMin; ~0 from the caller)
   uint32_t* counts;              // [5] commit_apply: runs written, skipped, launched, queued, failed (zeroed by the caller)
+  CommitTimings arm;             // arm.tim = nullptr: no arming
 };
 
 // bf_resident_sched_put: req[i] is written into area[req[i].run]

@@ -112,6 +112,8 @@ struct StepDef {
   std::string if_expr, with_raw;
   std::vector<std::string> needs;
   std::vector<std::pair<std::string, bool>> branches;
+  int timing_code = -1;   // bfh_story_set_step_timing: BF_DEC_* and delay, or -1: none
+  uint32_t timing_delay = 0;
 };
 
 inline void set_code(uint8_t* base, uint32_t W, int nbits, uint32_t i, int v) {
@@ -272,6 +274,19 @@ int bfh_story_set_policy(bfh_story* s, int cont, int realtime) {
   return BF_OK;
 }
 
+int bfh_story_set_step_timing(bfh_story* s, int step, int code, uint32_t delay) {
+  if (!s || step < 0 || (size_t)step >= s->defs.size()) return BF_EINVAL;
+  const int ty = s->defs[step].type;
+  const bool ok = code < 0 || (ty == BF_STEP_SLEEP ? code == BF_DEC_SUCCEED || code == BF_DEC_FAIL
+                             : ty == BF_STEP_GATE  ? code == BF_DEC_TIMED_OUT || code == BF_DEC_FAIL
+                             : ty == BF_STEP_WAIT  ? code == BF_DEC_TIMED_OUT || code == BF_DEC_PENDING || code == BF_DEC_FAIL
+                                                   : false);
+  if (!ok) { s->err = "step " + s->defs[step].name + ": its type does not take timing code " + std::to_string(code); return BF_EINVAL; }
+  s->defs[step].timing_code = code;
+  s->defs[step].timing_delay = code < 0 ? 0u : delay;
+  return BF_OK;
+}
+
 int bfh_story_finalize(bfh_story* s) {
   if (!s) return BF_EINVAL;
   if (s->finalized) return BF_OK;
@@ -385,7 +400,18 @@ int bfh_story_upload(bfh_story* s, bf_ctx* ctx, uint32_t* slot_out) {
   t.parallel = s->par.data(); t.n_parallel = (uint32_t)s->par.size();
   t.branch_allow_bits = s->allow_bits.empty() ? nullptr : s->allow_bits.data();
   t.n_branch_allow_bits = (uint32_t)s->allow_bits.size() * 8;
-  const int rc = bf_topology_put(ctx, &t, slot_out);
+  int rc = bf_topology_put(ctx, &t, slot_out);
+  std::vector<bf_step_timing> tim;
+  for (uint32_t i = 0; rc == BF_OK && i < t.n_steps; ++i) {
+    const StepDef& d = s->defs[s->order[i]];
+    if (d.timing_code >= 0) tim.push_back(bf_step_timing{(uint16_t)i, (uint8_t)d.timing_code, 0, d.timing_delay});
+  }
+  if (!tim.empty() && (rc = bf_topology_timings(ctx, *slot_out, tim.data(), (uint32_t)tim.size())) != BF_OK) {
+    const std::string why = bf_last_error(ctx);
+    bf_topology_drop(ctx, *slot_out);
+    s->err = why;
+    return rc;
+  }
   if (rc != BF_OK) s->err = bf_last_error(ctx);
   return rc;
 }

@@ -911,7 +911,7 @@ cudaError_t launch_fire(const FireParams& P, cudaStream_t stream) {
   return cudaGetLastError();
 }
 
-// ---- tick commits (bf_resident_commit) --------------------------------------------------------------------------------------
+// ---- tick commits (bf_resident_commit*) -------------------------------------------------------------------------------------
 // One warp per run; lane w holds word w of the run's masks and codes (words <= 32).  Both launches read a run the same way: its
 // topology's step types, the masks of its current result record (and of its schedule record), and its entries [lo, hi), found by
 // a binary search every lane runs alike.  A run with no mask bit and no entry leaves at once.
@@ -920,11 +920,11 @@ struct CommitRun {
   uint32_t TW, VALID;
   uint32_t launched, queued, skip, fail;
   uint32_t T_COND, SYNC_T, T_PAR, T_STOP;
-  uint32_t lo, hi;
+  uint32_t lo, hi, slot;
 };
 
 DI bool commit_run(const CommitParams& P, uint32_t r, uint32_t lane, CommitRun& c) {
-  const uint32_t slot = *reinterpret_cast<const uint32_t*>(P.state + (size_t)r * P.state_stride);
+  const uint32_t slot = c.slot = *reinterpret_cast<const uint32_t*>(P.state + (size_t)r * P.state_stride);
   const Slot sl = slot < P.n_slots ? P.slots[slot] : Slot{};
   const TopoHeader* th = reinterpret_cast<const TopoHeader*>(sl.addr);
   c.topo = sl.addr && th->W <= P.words ? reinterpret_cast<const uint8_t*>(sl.addr) : nullptr;
@@ -980,8 +980,74 @@ DI unsigned long long commit_entries(const CommitParams& P, uint32_t r, uint32_t
   return bad;
 }
 
+// The timer arms of run r (whole warp, with a timing table): each timing of the run's slot whose step is in ARM (lane w holds
+// word w: the launched sleep / gate / wait steps) and that no armed slot of the run names is a new arm; an armed slot stays.
+// Lane t holds slots t and t + 32 (armed slots lead, ascending by step).  The timings ascend by step and are walked 32 at a time,
+// so new arms come in step order: a new arm's rank is the new arms before it plus the armed slots of lower steps (counted over
+// the slots, read through shuffles, which also finds a stored slot), a kept slot's is its index plus the new arms of lower
+// steps, as arm_timers ranks them.  Check: -> the key of the run's first arming offence (a non-PENDING code without decision
+// planes at its step, more than timer_k slots at the lowest new step), else ~0; nothing is written.  Apply (after a check that
+// found none): stores the moved and the new slots and adds the arms and their earliest deadline to A.out.
+DI unsigned long long commit_arms(const CommitTimings& A, uint32_t r, uint32_t lane, uint32_t slot, uint32_t ARM, bool apply) {
+  if (slot >= A.n_slots || !__any_sync(FULL, ARM != 0u)) return ~0ull;
+  const uint32_t lo = A.first[slot], hi = A.first[slot + 1], K = A.timer_k;
+  if (lo == hi) return ~0ull;
+  unsigned long long* t = A.timers + (size_t)r * K;
+  const unsigned long long v0 = lane < K ? t[lane] : kTimerEmpty, v1 = lane + 32u < K ? t[lane + 32u] : kTimerEmpty;
+  const uint32_t s0 = timer_step(v0), s1 = timer_step(v1);
+  const uint32_t E = __popc(__ballot_sync(FULL, timer_armed(v0))) + __popc(__ballot_sync(FULL, timer_armed(v1)));
+  uint32_t n_new = 0, first_new = 0, first_dec = ~0u, nb0 = 0, nb1 = 0, next = BF_TIMER_NONE;
+  for (uint32_t j0 = lo; j0 < hi; j0 += 32u) {   // warp-uniform trip count
+    const uint32_t j = j0 + lane;
+    const bf_step_timing q = j < hi ? A.tim[j] : bf_step_timing{0, 0, 0, 0};
+    const uint32_t s = q.step;
+    uint32_t below = 0;   // armed slots of lower steps; a run holds few, so each lane compares with every one
+    bool stored = false;
+    for (uint32_t k = 0; k < E; ++k) {
+      const uint32_t sk = __shfl_sync(FULL, k < 32u ? s0 : s1, k & 31u);
+      below += sk < s ? 1u : 0u;
+      stored = stored || sk == s;
+    }
+    const uint32_t aw = __shfl_sync(FULL, ARM, (s >> 5) & 31u);   // every lane shuffles, also those past hi
+    const bool fresh = j < hi && ((aw >> (s & 31u)) & 1u) && !stored;
+    const uint32_t m = __ballot_sync(FULL, fresh);
+    if (!m) continue;
+    if (n_new == 0) first_new = __shfl_sync(FULL, s, __ffs(m) - 1);
+    if (!apply) {
+      const uint32_t nd = A.decision ? 0u : __ballot_sync(FULL, fresh && q.code != BF_DEC_PENDING);
+      if (nd && first_dec == ~0u) first_dec = __shfl_sync(FULL, s, __ffs(nd) - 1);
+    } else {
+      if (fresh) {
+        const uint32_t dl = (uint32_t)min((unsigned long long)A.now + q.delay, (unsigned long long)BF_TIMER_NONE - 1ull);
+        t[n_new + __popc(m & ((1u << lane) - 1u)) + below] = (unsigned long long)dl | (unsigned long long)s << 32 | (unsigned long long)q.code << 48;
+        next = min(next, dl);
+      }
+      for (uint32_t x = m; x; x &= x - 1u) {   // each new arm moves the kept slots of higher steps up one
+        const uint32_t sn = __shfl_sync(FULL, s, __ffs(x) - 1);
+        nb0 += timer_armed(v0) && s0 > sn ? 1u : 0u;
+        nb1 += timer_armed(v1) && s1 > sn ? 1u : 0u;
+      }
+    }
+    n_new += __popc(m);
+  }
+  if (!apply) {   // a decision offence at the lowest new step wins over the overflow there
+    if (first_dec != ~0u && (first_dec == first_new || E + n_new <= K))
+      return (unsigned long long)r << 32 | (unsigned long long)first_dec << 8 | kCommitNoDecision;
+    return E + n_new > K ? (unsigned long long)r << 32 | (unsigned long long)first_new << 8 | kCommitOverflow : ~0ull;
+  }
+  if (nb0) t[lane + nb0] = v0;   // the slots read above were loaded before any store (the ballots order them)
+  if (nb1) t[lane + 32u + nb1] = v1;
+  next = __reduce_min_sync(FULL, next);
+  if (lane == 0 && n_new) {
+    atomicAdd(A.out, n_new);
+    atomicMin(A.out + 1, next);
+  }
+  return ~0ull;
+}
+
 // Check: every entry names a launched step (a PHASE entry a stop step), and every launched stop step of a run without an ERROR
-// entry has a HOLD or PHASE entry.  Lane 0 lowers P.offender to the run's first offence.  Nothing is written.
+// entry has a HOLD or PHASE entry; with a timing table, the arming offences too.  Lane 0 lowers P.offender to the run's first
+// offence.  Nothing is written.
 __global__ void __launch_bounds__(256) commit_check(const CommitParams P) {
   const uint32_t r = blockIdx.x * 8u + (threadIdx.x >> 5), lane = threadIdx.x & 31u;
   if (r >= P.n_runs) return;
@@ -998,10 +1064,14 @@ __global__ void __launch_bounds__(256) commit_check(const CommitParams P) {
     bad = min(bad, (unsigned long long)r << 32 | (unsigned long long)step << 8 | kCommitNoPhase);
   }
   if (lane == 0 && bad != ~0ull) atomicMin(P.offender, bad);
+  if (!P.arm.tim || err) return;
+  bad = commit_arms(P.arm, r, lane, c.slot, c.launched & ~c.skip & ~c.fail & ~hold & c.SYNC_T, false);
+  if (lane == 0 && bad != ~0ull) atomicMin(P.offender, bad);
 }
 
 // Apply (after a check that found no offender): the writes of the contract on the codes as the pass reads them (code 15 as 0),
-// stored only where a code changed; lanes p and p + 32 set the registered bits of launched parallel descs.
+// stored only where a code changed; lanes p and p + 32 set the registered bits of launched parallel descs; with a timing table,
+// the arms of the launched sleep / gate / wait steps.
 __global__ void __launch_bounds__(256) commit_apply(const CommitParams P) {
   const uint32_t r = blockIdx.x * 8u + (threadIdx.x >> 5), lane = threadIdx.x & 31u;
   if (r >= P.n_runs) return;
@@ -1020,6 +1090,7 @@ __global__ void __launch_bounds__(256) commit_apply(const CommitParams P) {
   const uint32_t m0 = p[0] & keep, m1 = p[1] & keep, m2 = p[2] & keep, m3 = p[3] & keep;
   uint32_t n0 = m0, n1 = m1, n2 = m2, n3 = m3;
   const uint32_t SK = c.skip, FA = c.fail & ~SK, LA = c.launched & ~SK & ~FA & ~hold, QU = c.queued & ~SK & ~FA & ~c.launched;
+  if (P.arm.tim) commit_arms(P.arm, r, lane, c.slot, LA & c.SYNC_T, true);
   pset<BF_PHASE_FAILED>(FA, n0, n1, n2, n3);
   launch_effects(SK, LA, c.T_COND, c.SYNC_T, c.T_PAR, c.T_STOP, n0, n1, n2, n3);
   pset<BF_PHASE_PENDING_QUEUED>(QU, n0, n1, n2, n3);

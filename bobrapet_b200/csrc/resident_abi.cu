@@ -1230,17 +1230,27 @@ int bf_resident_runctl_download(bf_ctx* c, uint32_t h, uint32_t first, uint32_t 
 // The host checks the call and the entries, sorts them by (run, step) and uploads them; the check launch lowers the first
 // offender, which one D2H copy and one synchronisation bring back before anything is written; then the apply launch and the
 // counts.  A commit that wrote a run changes the state records: it ends the snapshot and the tick a schedule or a commit needs.
-int bf_resident_commit(bf_ctx* c, uint32_t h, uint32_t n_runs, const bf_commit_entry* entries, uint32_t n, bf_commit_out* out) {
+// With `arm` the same launches take the arms too (resident.cu): the timing table is copied up first when a timing changed, and
+// the counts copied back carry the arms' two words.
+int bf_resident_commit_timed(bf_ctx* c, uint32_t h, uint32_t n_runs, const bf_commit_entry* entries, uint32_t n, bf_commit_out* out,
+                             bf_commit_arm* arm) {
   auto [g, r] = lock_resident(c, h);
   if (!out || out->struct_size != sizeof(bf_commit_out)) return fail(c, BF_EINVAL, "null bf_commit_out or bad struct_size");
   *out = bf_commit_out{};
   out->struct_size = sizeof(bf_commit_out);
   out->bad_run = out->bad_step = BF_COMMIT_NONE;
-  if (!r) return BF_EINVAL;
-  auto refuse = [&](uint32_t run, uint32_t step, const std::string& msg) {
+  auto refuse = [&](uint32_t run, uint32_t step, const std::string& msg, int code = BF_EINVAL) {
     out->bad_run = run; out->bad_step = step;
-    return fail(c, BF_EINVAL, msg);
+    return fail(c, code, msg);
   };
+  if (arm) {
+    if (arm->struct_size != sizeof(bf_commit_arm)) return fail(c, BF_EINVAL, "bad bf_commit_arm struct_size");
+    arm->n_armed = 0;
+    arm->next_deadline = BF_TIMER_NONE;
+  }
+  if (!r) return BF_EINVAL;
+  if (arm && !r->areas.timer_k) return refuse(BF_COMMIT_NONE, BF_COMMIT_NONE, "the batch has no timer area (bf_resident_timers) to arm");
+  if (arm && arm->now == BF_TIMER_NONE) return refuse(BF_COMMIT_NONE, BF_COMMIT_NONE, "now must not be BF_TIMER_NONE");
   const bf_layout& L = r->L;
   if (n_runs > r->cap) return refuse(BF_COMMIT_NONE, BF_COMMIT_NONE, "n_runs exceeds the resident batch");
   if (n && !entries) return refuse(BF_COMMIT_NONE, BF_COMMIT_NONE, "null entries");
@@ -1279,12 +1289,19 @@ int bf_resident_commit(bf_ctx* c, uint32_t h, uint32_t n_runs, const bf_commit_e
   for (uint32_t i = 0; i < n; ++i) sorted[i] = entries[order[i]];
   bf::CommitParams P{};
   const unsigned long long no_offender = ~0ull;
-  const uint32_t zero_counts[5] = {};
+  const uint32_t zero_counts[7] = {0u, 0u, 0u, 0u, 0u, 0u, BF_TIMER_NONE};   // the five counts, then the arms' count and deadline
+  const uint32_t n_counts = arm ? 7u : 5u;
+  if (arm)
+    if (int rc = bf::sync_timings(c, s, P.arm)) return rc;
   CallStage st;
   st.up(P.offender, &no_offender, 1);
-  st.up(P.counts, zero_counts, 5);
+  st.up(P.counts, zero_counts, n_counts);
   st.up(P.entries, sorted.data(), n);
   if (int rc = st.send(c, "bf_resident_commit (check)")) return rc;
+  if (P.arm.tim) {
+    P.arm.timers = r->areas.d_timers; P.arm.timer_k = r->areas.timer_k; P.arm.now = arm->now;
+    P.arm.decision = L.off_decision != BF_OFF_NONE; P.arm.out = P.counts + 5;
+  }
   P.state = r->d_state; P.result = r->d_result; P.sched_rec = A.sched_rec;
   P.slots = c->slots_dev; P.n_slots = (uint32_t)c->slots_host.size();
   P.n_entries = n; P.n_runs = n_runs;
@@ -1301,20 +1318,28 @@ int bf_resident_commit(bf_ctx* c, uint32_t h, uint32_t n_runs, const bf_commit_e
   if (key != ~0ull) {
     const uint32_t run = (uint32_t)(key >> 32), step = (uint32_t)(key >> 8) & 0xFFFFFFu, why = (uint32_t)key & 0xFFu;
     const std::string at = "run " + std::to_string(run) + " step " + std::to_string(step) + ": ";
+    if (why == bf::kCommitOverflow)
+      return refuse(run, step, at + "the run would hold more than " + std::to_string(r->areas.timer_k) + " armed timers", BF_ENOMEM);
     return refuse(run, step, at + (why == bf::kCommitNotLaunched ? "an entry names a step the tick did not launch"
                                    : why == bf::kCommitNotStop   ? "a BF_COMMIT_PHASE entry names a step that is not a stop step"
-                                                                 : "a launched stop step has no BF_COMMIT_PHASE entry"));
+                                   : why == bf::kCommitNoPhase   ? "a launched stop step has no BF_COMMIT_PHASE entry"
+                                                                 : "a timing that writes needs decision planes (BF_F_DECISION)"));
   }
   e = bf::launch_commit(P, true, s);
-  if (e == cudaSuccess) e = cudaMemcpyAsync(host, P.counts, 20, cudaMemcpyDeviceToHost, s);
+  if (e == cudaSuccess) e = cudaMemcpyAsync(host, P.counts, 4 * n_counts, cudaMemcpyDeviceToHost, s);
   if (int rc = r->sync_in_place(c, e, "bf_resident_commit")) { r->state_changed(c); return rc; }
   c->stats.kernel_launches += 1;
-  uint32_t k[5];
-  memcpy(k, host, sizeof k);
+  uint32_t k[7];
+  memcpy(k, host, 4 * n_counts);
   out->n_runs_written = k[0]; out->n_skipped = k[1]; out->n_launched = k[2]; out->n_queued = k[3]; out->n_failed = k[4];
+  if (arm) { arm->n_armed = k[5]; arm->next_deadline = k[6]; }
   if (k[0]) {   // as a delta: the written runs are touched, and the tick a schedule or a commit needs is over
     r->state_changed(c);
     r->pending += k[0];
   }
   return BF_OK;
+}
+
+int bf_resident_commit(bf_ctx* c, uint32_t h, uint32_t n_runs, const bf_commit_entry* entries, uint32_t n, bf_commit_out* out) {
+  return bf_resident_commit_timed(c, h, n_runs, entries, n, out, nullptr);
 }

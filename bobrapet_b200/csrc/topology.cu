@@ -319,6 +319,9 @@ int put_many_locked(bf_ctx* c, const bf_topology* topos, uint32_t count, uint32_
     m.child_nibbles = plans[i].child_nibbles;
     m.par_step.resize(m.P); m.par_branches.resize(m.P);
     for (uint32_t q = 0; q < m.P; ++q) { m.par_step[q] = topos[i].parallel[q].step; m.par_branches[q] = topos[i].parallel[q].branches; }
+    m.types.resize(m.S);
+    for (uint32_t k = 0; k < m.S; ++k) m.types[k] = topos[i].step_flags[k] & BF_SF_TYPE_MASK;
+    m.timings.clear();
     c->slots_host[slot] = bf::Slot{(uint64_t)(uintptr_t)(c->arena + m.offset), m.bytes,
                                    m.S | (m.P << 16) | (bf::slot_row_bytes(plans[i].ell) << 24)};
     memcpy(&c->ff_host[(size_t)slot * bf::FF_STRIDE], plans[i].ff, sizeof plans[i].ff);
@@ -379,6 +382,29 @@ int sync_slots(bf_ctx* c, cudaStream_t stream) {
   return BF_OK;
 }
 
+int sync_timings(bf_ctx* c, cudaStream_t stream, CommitTimings& P) {
+  if (c->timings_dirty) {
+    c->tim_first_host.assign(c->meta.size() + 1, 0u);
+    c->tim_host.clear();
+    for (size_t s = 0; s < c->meta.size(); ++s) {
+      c->tim_host.insert(c->tim_host.end(), c->meta[s].timings.begin(), c->meta[s].timings.end());
+      c->tim_first_host[s + 1] = (uint32_t)c->tim_host.size();
+    }
+    const size_t n = c->tim_host.size();
+    if (n) {
+      if (int rc = c->tim_first_dev.ensure(c, c->tim_first_host.size())) return rc;
+      if (int rc = c->tim_dev.ensure(c, n)) return rc;
+      BF_CUDA(c, cudaMemcpyAsync(c->tim_first_dev, c->tim_first_host.data(), c->tim_first_host.size() * 4, cudaMemcpyHostToDevice, stream));
+      BF_CUDA(c, cudaMemcpyAsync(c->tim_dev, c->tim_host.data(), n * sizeof(bf_step_timing), cudaMemcpyHostToDevice, stream));
+    }
+    c->timings_dirty = false;   // the host arrays stay until the next change: the copies read them after this returns
+  }
+  if (!c->tim_host.empty()) {
+    P.tim = c->tim_dev; P.first = c->tim_first_dev; P.n_slots = (uint32_t)c->tim_first_host.size() - 1u;
+  }
+  return BF_OK;
+}
+
 // the largest live record among the topologies of at most w words (ceil(S/32)), 0 when there is none; drops and arena
 // compactions since the last call recompute the maxima first
 uint32_t largest_record(bf_ctx* c, uint32_t w) {
@@ -418,6 +444,7 @@ static int drop_locked(bf_ctx* c, uint32_t slot) {
   if (slot >= c->meta.size() || !c->meta[slot].alive) return fail(c, BF_ETOPO, "drop of an unknown slot");
   c->meta[slot].alive = false;
   c->slot_changes++;
+  if (!c->meta[slot].timings.empty()) { c->meta[slot].timings.clear(); c->timings_dirty = true; }
   if (c->meta[slot].P) c->n_with_parallel--;
   c->slots_host[slot] = bf::Slot{0, 0, 0};
   memset(&c->ff_host[(size_t)slot * bf::FF_STRIDE], 0, bf::FF_STRIDE * sizeof(uint32_t));
@@ -500,6 +527,35 @@ int bf_topology_drop(bf_ctx* c, uint32_t slot) {
   if (!c) return BF_EINVAL;
   std::lock_guard<std::mutex> g(c->mu);
   return drop_locked(c, slot);
+}
+
+int bf_topology_timings(bf_ctx* c, uint32_t slot, const bf_step_timing* t, uint32_t n) {
+  if (!c) return BF_EINVAL;
+  std::lock_guard<std::mutex> g(c->mu);
+  if (slot >= c->meta.size() || !c->meta[slot].alive) return fail(c, BF_EINVAL, "unknown topology slot");
+  if (n && !t) return fail(c, BF_EINVAL, "null timings");
+  TopoMeta& m = c->meta[slot];
+  std::vector<bf_step_timing> v(t, t + n);
+  for (uint32_t i = 0; i < n; ++i) {
+    const bf_step_timing& q = v[i];
+    auto at = [i] { return "timing " + std::to_string(i) + ": "; };
+    if (q.step >= m.S) return fail(c, BF_EINVAL, at() + "step outside the topology");
+    if (q.reserved) return fail(c, BF_EINVAL, at() + "reserved must be 0");
+    const uint32_t ty = m.types[q.step], code = q.code;
+    const bool ok = ty == BF_STEP_SLEEP ? code == BF_DEC_SUCCEED || code == BF_DEC_FAIL
+                  : ty == BF_STEP_GATE  ? code == BF_DEC_TIMED_OUT || code == BF_DEC_FAIL
+                  : ty == BF_STEP_WAIT  ? code == BF_DEC_TIMED_OUT || code == BF_DEC_PENDING || code == BF_DEC_FAIL
+                                        : false;
+    if (!ok) return fail(c, BF_EINVAL, at() + "the step's type does not take this code (sleep: SUCCEED / FAIL, gate: TIMED_OUT / FAIL, "
+                                              "wait: TIMED_OUT / PENDING / FAIL, other types: none)");
+  }
+  std::sort(v.begin(), v.end(), [](const bf_step_timing& a, const bf_step_timing& b) { return a.step < b.step; });
+  for (uint32_t i = 1; i < n; ++i)
+    if (v[i].step == v[i - 1].step) return fail(c, BF_EINVAL, "step " + std::to_string(v[i].step) + " has two timings");
+  if (v.empty() && m.timings.empty()) return BF_OK;
+  m.timings = std::move(v);
+  c->timings_dirty = true;
+  return BF_OK;
 }
 
 int bf_topology_child_first(const bf_ctx* c, uint32_t slot, uint32_t* out, uint32_t cap) {

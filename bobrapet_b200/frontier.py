@@ -123,6 +123,18 @@ class Frontier:
     def drop_topology(self, slot: int):
         self._check(self._lib.bf_topology_drop(self._ctx, int(slot)), "bf_topology_drop")
 
+    TIMING_DTYPE = np.dtype([("step", "<u2"), ("code", "u1"), ("reserved", "u1"), ("delay", "<u4")])   # bf_step_timing, 8 B
+
+    def put_timings(self, slot: int, entries=None):
+        """bf_topology_timings: replace the step timings of a live slot (TIMING_DTYPE or (step, code, delay) tuples; none clears
+        them).  A timed resident_commit arms the launched sleep, gate and wait steps that have one."""
+        ents = np.zeros(0, dtype=self.TIMING_DTYPE) if entries is None else entries
+        if not isinstance(ents, np.ndarray):
+            ents = np.array([(int(s), int(c), 0, int(d)) for s, c, d in ents], dtype=self.TIMING_DTYPE)
+        ents = np.ascontiguousarray(ents, dtype=self.TIMING_DTYPE)
+        self._check(self._lib.bf_topology_timings(self._ctx, int(slot), ents.ctypes.data if ents.shape[0] else None, ents.shape[0]),
+                    "bf_topology_timings")
+
     def child_first(self, slot: int) -> np.ndarray:
         out = np.zeros(A.MAX_PARALLEL, dtype=np.uint32)
         n = self._lib.bf_topology_child_first(self._ctx, int(slot), out.ctypes.data_as(C.POINTER(C.c_uint32)), A.MAX_PARALLEL)
@@ -360,23 +372,31 @@ class Frontier:
     # -- tick commits of a resident batch (bf_resident_commit)
     COMMIT_DTYPE = np.dtype([("run", "<u4"), ("step", "<u2"), ("kind", "u1"), ("code", "u1")])   # bf_commit_entry, 8 B
 
-    def resident_commit(self, handle: int, n_runs: int, entries=None) -> dict:
+    def resident_commit(self, handle: int, n_runs: int, entries=None, now: Optional[int] = None) -> dict:
         """bf_resident_commit: write the skips, launches and queue marks of the last tick (and schedule) of runs [0, n_runs)
         into the state records.  entries: COMMIT_DTYPE (or (run, step, kind, code) tuples), at most one per (run, step).
-        -> dict(n_runs_written, n_skipped, n_launched, n_queued, n_failed).  A refusal raises FrontierError with .bad_run and
-        .bad_step (A.COMMIT_NONE for a refusal of the whole call)"""
+        With `now` (bf_resident_commit_timed) the launched sleep, gate and wait steps with a timing (put_timings) are armed too.
+        -> dict(n_runs_written, n_skipped, n_launched, n_queued, n_failed), with `now` also n_armed and next_deadline.  A
+        refusal raises FrontierError with .bad_run and .bad_step (A.COMMIT_NONE for a refusal of the whole call)"""
         ents = np.zeros(0, dtype=self.COMMIT_DTYPE) if entries is None else entries
         if not isinstance(ents, np.ndarray):
             ents = np.array([tuple(e) for e in ents], dtype=self.COMMIT_DTYPE)
         ents = np.ascontiguousarray(ents, dtype=self.COMMIT_DTYPE)
         out = A.CommitOut(struct_size=C.sizeof(A.CommitOut))
-        rc = self._lib.bf_resident_commit(self._ctx, handle, int(n_runs), ents.ctypes.data if ents.shape[0] else None,
-                                          ents.shape[0], C.byref(out))
+        ep = ents.ctypes.data if ents.shape[0] else None
+        if now is None:
+            rc = self._lib.bf_resident_commit(self._ctx, handle, int(n_runs), ep, ents.shape[0], C.byref(out))
+        else:
+            arm = A.CommitArm(struct_size=C.sizeof(A.CommitArm), now=int(now))
+            rc = self._lib.bf_resident_commit_timed(self._ctx, handle, int(n_runs), ep, ents.shape[0], C.byref(out), C.byref(arm))
         if rc != A.BF_OK:
             err = A.FrontierError(rc, "bf_resident_commit: %s" % self._lib.bf_last_error(self._ctx).decode())
             err.bad_run, err.bad_step = int(out.bad_run), int(out.bad_step)
             raise err
-        return {k: int(getattr(out, k)) for k in ("n_runs_written", "n_skipped", "n_launched", "n_queued", "n_failed")}
+        got = {k: int(getattr(out, k)) for k in ("n_runs_written", "n_skipped", "n_launched", "n_queued", "n_failed")}
+        if now is not None:
+            got.update(n_armed=int(arm.n_armed), next_deadline=int(arm.next_deadline))
+        return got
 
     # -- limiter inputs and schedules of resident batches (bf_resident_sched*, bf_resident_schedule)
     SCHED_PUT_DTYPE = np.dtype([("run", "<u4"), ("story_key", "<u4"), ("queue_key", "<u4"), ("priority", "<i4"),

@@ -109,6 +109,25 @@ func (c *Ctx) PutTopology(t *Topology) (uint32, error) {
 
 func (c *Ctx) DropTopology(slot uint32) error { return c.err(C.bf_topology_drop(c.p, C.uint32_t(slot))) }
 
+// StepTiming is one step's timer (bf_step_timing, 8 bytes, no pointers): Code is the BF_DEC_* code the armed timer writes
+// when it fires, Delay its clock units after the now of the commit that arms it.  PackStory emits them.
+type StepTiming struct {
+	Step  uint16
+	Code  uint8
+	_     uint8
+	Delay uint32
+}
+
+// PutTimings replaces the step timings of a live slot (bf_topology_timings); none clears them.  CommitTimed arms the
+// launched sleep, gate and wait steps that have one.  A drop discards them.
+func (c *Ctx) PutTimings(slot uint32, timings []StepTiming) error {
+	var tp *C.bf_step_timing
+	if len(timings) > 0 {
+		tp = (*C.bf_step_timing)(unsafe.Pointer(&timings[0]))
+	}
+	return c.err(C.bfgo_topology_timings(c.p, C.uint32_t(slot), tp, C.uint32_t(len(timings))))
+}
+
 // Batch is a pair of pinned C buffers (bf_alloc_pinned) laid out by bf_layout_init; the packer writes state
 // records into State, the library writes result records into Result.  Both are C memory: no cgo pointer rule applies.
 type Batch struct {
@@ -608,6 +627,21 @@ func (r *Resident) Commit(n uint32, entries []CommitEntry) (CommitResult, error)
 	rc := C.bfgo_resident_commit(r.c.p, r.handle, C.uint32_t(n), ep, C.uint32_t(len(entries)), &k[0])
 	res := CommitResult{uint32(k[0]), uint32(k[1]), uint32(k[2]), uint32(k[3]), uint32(k[4]), uint32(k[5]), uint32(k[6])}
 	return res, r.c.err(rc)
+}
+
+// CommitTimed is Commit that also arms the step timers of the launched sleep, gate and wait steps with a timing (PutTimings)
+// at now + Delay (bf_resident_commit_timed); a step whose timer is already armed keeps it.  Armed is the number of slots it
+// armed and NextDeadline the earliest of them (TimerNone: none): sleep until the smaller of it and Fire's NextDeadline.  A
+// run that would hold more than the batch's slots per run is refused with ENOMEM: grow them with EnableTimers and repeat.
+func (r *Resident) CommitTimed(n, now uint32, entries []CommitEntry) (res CommitResult, armed, nextDeadline uint32, err error) {
+	var ep *C.bf_commit_entry
+	if len(entries) > 0 {
+		ep = (*C.bf_commit_entry)(unsafe.Pointer(&entries[0]))
+	}
+	var k [9]C.uint32_t
+	rc := C.bfgo_resident_commit_timed(r.c.p, r.handle, C.uint32_t(n), ep, C.uint32_t(len(entries)), C.uint32_t(now), &k[0])
+	res = CommitResult{uint32(k[0]), uint32(k[1]), uint32(k[2]), uint32(k[3]), uint32(k[4]), uint32(k[5]), uint32(k[6])}
+	return res, uint32(k[7]), uint32(k[8]), r.c.err(rc)
 }
 
 // SchedPut is one limiter-input request of PutSched (bf_sched_put, 32 bytes, no pointers).  QueuedSince is the StartedAt of the

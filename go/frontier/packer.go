@@ -9,8 +9,10 @@ package frontier
 // bobrapet_b200/csrc/host_mirror.cc (tests/test_host_mirror.py), and tests/packing.py is the test-side statement.
 
 import (
+	"encoding/json"
 	"regexp"
 	"strings"
+	"time"
 
 	runsv1alpha1 "github.com/bubustack/bobrapet/api/runs/v1alpha1"
 	bubuv1alpha1 "github.com/bubustack/bobrapet/api/v1alpha1"
@@ -102,14 +104,17 @@ type PackedStory struct {
 	Index    map[string]uint16 // step name -> index
 	Branches [][]string        // per parallel desc: branch names in with.steps order
 	Unknown  []string          // dependency names that match no step ("unknown step dependencies", dag.go:3087-3098)
+	Timings  []StepTiming      // for Ctx.PutTimings: the sleep, gate and wait steps' timers, ascending by step (stepTiming)
 }
 
 // PackStory builds the CSR of buildDependencyGraphs (dag.go:3024-3073) over allStorySteps.  The reference builds the
 // graph from the CURRENT group's step list, so alias -> name resolution sees only that group's names, while a
 // dependency may name a step of any group: both rules are kept (per-group alias maps, global index space).
 // parallelBranches(step) returns the branch names and allowFailure flags of a `parallel` step's with.steps
-// (parseParallelBranches, dag.go:1202-1214) — JSON decoding stays with the caller.
-func PackStory(story *bubuv1alpha1.Story, parallelBranches func(*bubuv1alpha1.Step) ([]string, []bool), onTimeoutSkip func(*bubuv1alpha1.Step) bool) *PackedStory {
+// (parseParallelBranches, dag.go:1202-1214) — JSON decoding stays with the caller.  unit is the step timers' clock unit
+// (Resident.Fire's now): each sleep, gate and wait step gets its timing in Timings (0: none are packed).
+func PackStory(story *bubuv1alpha1.Story, parallelBranches func(*bubuv1alpha1.Step) ([]string, []bool), onTimeoutSkip func(*bubuv1alpha1.Step) bool,
+	unit time.Duration) *PackedStory {
 	groups := [][]bubuv1alpha1.Step{story.Spec.Steps, story.Spec.Compensations, story.Spec.Finally}
 	ps := &PackedStory{Index: map[string]uint16{}}
 	for _, g := range groups {
@@ -183,6 +188,11 @@ func PackStory(story *bubuv1alpha1.Story, parallelBranches func(*bubuv1alpha1.St
 				f |= sfOnTimeoutSkip
 			}
 			t.StepFlags = append(t.StepFlags, f)
+			if unit > 0 {
+				if code, delay, ok := stepTiming(s, typeCode(s), unit); ok {
+					ps.Timings = append(ps.Timings, StepTiming{Step: ps.Index[s.Name], Code: code, Delay: delay})
+				}
+			}
 			if typeCode(s) == 2 && parallelBranches != nil {
 				names, allow := parallelBranches(s)
 				first := uint32(8 * len(t.AllowBits))
@@ -199,6 +209,98 @@ func PackStory(story *bubuv1alpha1.Story, parallelBranches func(*bubuv1alpha1.St
 		}
 	}
 	return ps
+}
+
+// decision codes a timer writes (BF_DEC_*)
+const (
+	decPending  = 0
+	decSucceed  = 1
+	decFail     = 2
+	decTimedOut = 3
+)
+
+// positive is parsePositiveDuration (steprun_controller.go:1364)
+func positive(raw string) (time.Duration, bool) {
+	d, err := time.ParseDuration(raw)
+	return d, err == nil && d > 0
+}
+
+// units rounds d up to whole clock units, so that no armed timer fires before the reference's deadline
+func units(d, unit time.Duration) uint32 {
+	n := (d + unit - 1) / unit
+	if d > 0 && n <= 0 || n > 0xFFFFFFFF {
+		return 0xFFFFFFFF
+	}
+	return uint32(n)
+}
+
+// stepTiming is what parseSleepConfig / parseGateConfig / parseWaitConfig (dag.go:1549-1653) make of a step's `with`: the
+// code its timer writes and its delay in clock units, or ok = false (no timer: a gate without a timeout takes its decision
+// as a delta).  A `with` the reference refuses fails the step at once (FAIL, 0: :1239-1249, :1331-1341, :1477-1487); a sleep
+// without a duration completes on its next sync (SUCCEED, 0: :1252-1254).  tests/step_timings.py states the same rules.
+func stepTiming(s *bubuv1alpha1.Step, ty uint8, unit time.Duration) (code uint8, delay uint32, ok bool) {
+	onTimeout := func(raw string) bool {
+		v := strings.ToLower(strings.TrimSpace(raw))
+		return v == "" || v == "fail" || v == "skip"
+	}
+	switch ty {
+	case 3: // sleep
+		if s.With == nil || len(s.With.Raw) == 0 {
+			return decSucceed, 0, true
+		}
+		var raw struct {
+			Duration string `json:"duration"`
+		}
+		if json.Unmarshal(s.With.Raw, &raw) != nil {
+			return decFail, 0, true
+		}
+		if strings.TrimSpace(raw.Duration) == "" {
+			return decSucceed, 0, true
+		}
+		d, good := positive(raw.Duration)
+		if !good {
+			return decFail, 0, true
+		}
+		return decSucceed, units(d, unit), true
+	case 7, 5: // gate, wait
+		if s.With == nil {
+			if ty == 5 {
+				return decFail, 0, true
+			}
+			return 0, 0, false
+		}
+		var raw struct {
+			Until        string `json:"until"`
+			Timeout      string `json:"timeout,omitempty"`
+			PollInterval string `json:"pollInterval,omitempty"`
+			OnTimeout    string `json:"onTimeout,omitempty"`
+		}
+		if json.Unmarshal(s.With.Raw, &raw) != nil || !onTimeout(raw.OnTimeout) || (ty == 5 && strings.TrimSpace(raw.Until) == "") {
+			return decFail, 0, true
+		}
+		var timeout, poll time.Duration
+		if raw.Timeout != "" {
+			d, good := positive(raw.Timeout)
+			if !good {
+				return decFail, 0, true
+			}
+			timeout = d
+		}
+		if raw.PollInterval != "" {
+			d, good := positive(raw.PollInterval)
+			if !good {
+				return decFail, 0, true
+			}
+			poll = d
+		}
+		switch {
+		case timeout > 0:
+			return decTimedOut, units(timeout, unit), true
+		case ty == 5 && poll > 0:
+			return decPending, units(poll, unit), true // wake-only: the host re-evaluates until
+		}
+	}
+	return 0, 0, false
 }
 
 // run flag bits (BF_RF_*)

@@ -223,6 +223,27 @@ static inline int bfgo_resident_commit(bf_ctx* c, uint32_t handle, uint32_t n_ru
   return rc;
 }
 
+/* Tick commits that arm step timers: as bfgo_resident_commit, and counts[7..8] = slots armed, earliest deadline armed. */
+static inline int bfgo_resident_commit_timed(bf_ctx* c, uint32_t handle, uint32_t n_runs, const bf_commit_entry* entries, uint32_t n,
+                                             uint32_t now, uint32_t* counts) {
+  bf_commit_out o;
+  memset(&o, 0, sizeof o);
+  o.struct_size = (uint32_t)sizeof o;
+  bf_commit_arm a;
+  memset(&a, 0, sizeof a);
+  a.struct_size = (uint32_t)sizeof a;
+  a.now = now;
+  const int rc = bf_resident_commit_timed(c, handle, n_runs, entries, n, &o, &a);
+  counts[0] = o.n_runs_written; counts[1] = o.n_skipped; counts[2] = o.n_launched; counts[3] = o.n_queued; counts[4] = o.n_failed;
+  counts[5] = o.bad_run; counts[6] = o.bad_step; counts[7] = a.n_armed; counts[8] = a.next_deadline;
+  return rc;
+}
+
+/* Step timings of a topology slot (bf_step_timing holds no pointers): passed as they are. */
+static inline int bfgo_topology_timings(bf_ctx* c, uint32_t slot, const bf_step_timing* t, uint32_t n) {
+  return bf_topology_timings(c, slot, t, n);
+}
+
 static inline void bfgo_tables(bf_sched_tables* t, uint32_t n_stories, uint32_t n_queues, int32_t global_limit, uint32_t global_base,
                                const int32_t* story_limit, const uint32_t* story_base, const int32_t* queue_limit,
                                const int32_t* queue_aging_s, const uint32_t* queue_base, const int32_t* queue_max_priority_base) {

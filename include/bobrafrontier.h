@@ -307,6 +307,28 @@ int bf_topology_closure(bf_ctx* ctx, const uint32_t* slots, const uint32_t* step
                         uint32_t* masks_out);
 
 int bf_topology_drop(bf_ctx* ctx, uint32_t slot);
+
+/* Step timings of a topology slot: how long each sleep sleeps and when each gate or wait times out, for the tick commits that
+ * arm the step timers of the steps they launch (bf_resident_commit_timed).  The reference sets a step's StartedAt when it
+ * launches it (markStepState, step_executor.go:171-179; ensureStepStateTimes, step_state.go:25-33) and the deadline is StartedAt
+ * plus the step's with.duration / with.timeout / with.pollInterval, so the timing is static per Story generation: `delay` in
+ * clock units after the `now` of the arming commit, and `code` what the armed timer writes when it fires.
+ * bf_topology_timings(slot, t, n) replaces the slot's set; n = 0 clears it.  Checked before anything changes, else BF_EINVAL and
+ * nothing changed: the slot is alive; each step is below the slot's S and named at most once (any order); reserved is 0; the
+ * step's type (its BF_SF_* flags at the put) allows the code:
+ *   sleep: BF_DEC_SUCCEED or BF_DEC_FAIL;  gate: BF_DEC_TIMED_OUT or BF_DEC_FAIL;
+ *   wait:  BF_DEC_TIMED_OUT, BF_DEC_PENDING (wake-only: its pollInterval) or BF_DEC_FAIL;  every other type: none.
+ * Timings belong to the slot: bf_topology_drop discards them and a put that reuses the slot starts with none.  They change no
+ * pass result, so the topology record, bf_topology_record_build and the touched ticks' slot bookkeeping ignore them.  The ctx
+ * keeps them on the host and copies one table of all of them to the device at the first arming commit after a change; a ctx
+ * that never calls this allocates and copies nothing for them.                                                              */
+typedef struct bf_step_timing {  /* 8 B                                                                                       */
+  uint16_t step;                 /* allStorySteps index, < S of the slot                                                     */
+  uint8_t code;                  /* BF_DEC_*: what the armed timer writes when it fires                                      */
+  uint8_t reserved;              /* 0                                                                                        */
+  uint32_t delay;                /* clock units after `now` of the arming commit                                             */
+} bf_step_timing;
+int bf_topology_timings(bf_ctx* ctx, uint32_t slot, const bf_step_timing* timings, uint32_t n);
 /* Nibble offset of parallel desc p's children inside the child area.          */
 int bf_topology_child_first(const bf_ctx* ctx, uint32_t slot, uint32_t* child_first_out, uint32_t cap);
 
@@ -1070,8 +1092,8 @@ int bf_resident_runctl_download(bf_ctx* ctx, uint32_t handle, uint32_t first_run
  *
  * Idempotent: a run whose writes are in place is not changed.  A run whose record changed is touched as by a delta (the next
  * bf_resident_tick_touched evaluates it), and a commit that changed anything ends the evaluated snapshot and the tick a schedule
- * or a commit needs.  The step timers are not armed (the batcher arms the deadlines of launched sleeps, gates and waits), and a
- * stopped run (bf_resident_runctl) has no candidates, so it gets nothing.  The counts are steps whose code the commit changed (a
+ * or a commit needs.  bf_resident_commit arms no step timer (bf_resident_commit_timed below arms those of the launched sleeps,
+ * gates and waits), and a stopped run (bf_resident_runctl) has no candidates, so it gets nothing.  The counts are steps whose code the commit changed (a
  * launched parallel step also when only its registered bit was set).  Stage G / H / I rewrites (gate syncs, joins, fail-fast and
  * compensation skips) are not persisted: each pass recomputes them from the state.  One H2D copy of the sorted entries, the check
  * launch, one D2H copy and one synchronisation before anything is written; then the apply launch, one D2H copy and one
@@ -1097,6 +1119,30 @@ typedef struct bf_commit_out {
 
 int bf_resident_commit(bf_ctx* ctx, uint32_t handle, uint32_t n_runs, const bf_commit_entry* entries, uint32_t n_entries,
                        bf_commit_out* out);
+
+/* bf_resident_commit_timed(..., out, arm) is bf_resident_commit (arm = NULL is exactly that call) that also arms the step timers of
+ * the steps it launches, as the reference arms them when it launches a step (ensureSleepUntil / ensureWaitTimeoutAt /
+ * ensureGateTimeoutAt, dag.go:128-171).  For each run the commit writes (no BF_COMMIT_ERROR entry), each launched step after the
+ * commit's masks (launched, not skipped, not cond-FAIL, no BF_COMMIT_HOLD entry) that is a sleep, gate or wait step and has a
+ * timing in the run's slot (bf_topology_timings):
+ *   - no armed slot of the run names the step: {deadline = min(now + delay, BF_TIMER_NONE - 1), step, code} is armed into the
+ *     run's slots in the canonical order (a delay of 0 is due at `now`: the next bf_resident_fire fires it);
+ *   - an armed slot names it: that slot stays as it is and is not counted (the stored deadline wins, dag.go:128-171).
+ * Checked before anything changes, in addition to bf_resident_commit's checks, with bad_run / bad_step as there: arm->struct_size,
+ * arm->now != BF_TIMER_NONE and the batch's timer area (bf_resident_timers), BF_EINVAL for the whole call; then, on the device
+ * and together with the entry offences (the lowest (run, step) of all of them), a run that would arm a non-PENDING code on a
+ * batch without decision planes (BF_EINVAL, at that step), and a run whose armed slots plus its new arms exceed K (BF_ENOMEM,
+ * at the lowest step it would newly arm; grow K with bf_resident_timers and repeat the commit).  Arming touches no run (every
+ * armed step is a written step); stopped runs, dead slots and slots wider than the layout have no masks and arm nothing.  The
+ * arms are made by the same two launches; the copies of the counts carry two more words.                                      */
+typedef struct bf_commit_arm {
+  uint32_t struct_size;          /* sizeof(bf_commit_arm)                                                                     */
+  uint32_t now;                  /* in: the clock of bf_resident_fire; != BF_TIMER_NONE                                       */
+  uint32_t n_armed;              /* out: slots this call armed                                                                */
+  uint32_t next_deadline;        /* out: earliest deadline this call armed, or BF_TIMER_NONE                                  */
+} bf_commit_arm;
+int bf_resident_commit_timed(bf_ctx* ctx, uint32_t handle, uint32_t n_runs, const bf_commit_entry* entries, uint32_t n_entries,
+                             bf_commit_out* out, bf_commit_arm* arm);
 
 /* ------------------------------------------------------------------ device groups (SURVEY.md row e)
  * The reference is ONE operator process (cmd/main.go:220, StoryRunReconciler storyrun_controller.go:216), so the

@@ -50,7 +50,12 @@ int bfh_story_finalize(bfh_story* s);
 int bfh_story_dims(const bfh_story* s, uint32_t* n_steps, uint32_t* n_edges, uint32_t* n_parallel);
 /* Copy out the packed form (row_ptr[S+1], col_idx[E], step_flags[S]); any pointer may be NULL. */
 int bfh_story_csr(const bfh_story* s, uint32_t* row_ptr, uint16_t* col_idx, uint8_t* step_flags);
-int bfh_story_upload(bfh_story* s, bf_ctx* ctx, uint32_t* slot_out); /* bf_topology_put of the packed form */
+/* The timing of a sleep, gate or wait step (insertion handle `step`) that bfh_story_upload puts after the topology
+ * (bf_topology_timings: code BF_DEC_*, delay in clock units after the arming commit's `now`); code -1 removes it.  Parsing
+ * `with` (duration, timeout, pollInterval) stays with the caller, as on_timeout_skip does.  BF_EINVAL when the step's type
+ * does not take the code (the rules of bf_topology_timings). */
+int bfh_story_set_step_timing(bfh_story* s, int step, int code, uint32_t delay);
+int bfh_story_upload(bfh_story* s, bf_ctx* ctx, uint32_t* slot_out); /* bf_topology_put of the packed form, then its timings */
 int bfh_story_step_index(const bfh_story* s, const char* name);      /* index in allStorySteps order, or -1 */
 const char* bfh_story_step_name(const bfh_story* s, uint32_t index);
 uint32_t bfh_story_run_flags(const bfh_story* s);                     /* BF_RF_FAIL_FAST / BF_RF_REALTIME from the policy */
