@@ -44,6 +44,8 @@
 #pragma once
 #include <stdint.h>
 
+#include "retire_moves.h"   // kRetireNoMove
+
 namespace bf {
 
 struct TopoHeader {
@@ -282,7 +284,6 @@ struct ReshapeParams {
 };
 
 // bf_resident_retire (resident.cu): the runs [m, m + n) vacate their indices; the live ones among them move below m
-constexpr uint32_t kRetireNoMove = 0xFFFFFFFFu;
 struct RetireParams {
   uint8_t* state;
   uint8_t* result;               // the current result records

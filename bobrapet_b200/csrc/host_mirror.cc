@@ -12,6 +12,7 @@
 #include <vector>
 
 #include "../../include/bobrafrontier_host.h"
+#include "retire_moves.h"
 
 namespace {
 
@@ -821,29 +822,35 @@ static void relay_planes(uint8_t* dst, const uint8_t* src, uint32_t to_off, uint
 
 static uint32_t child_area_bytes(const bf_layout& L) { return L.off_child == BF_OFF_NONE ? 0u : ((L.child_nibbles + 1) / 2 + 3) / 4 * 4; }
 
-// The mirror's state and result records re-laid from F to T into nr (zeroed), as bf_resident_reshape / _narrow re-lay the
-// device's: the headers kept, each plane and mask its low words, the child area its low bytes.
-static void relay_records(const bfh_batch* b, HostRecords& nr, const bf_layout& F, const bf_layout& T) {
+// Run r's state and result records in `from` (layout F) re-laid to run q of `to` (layout T), as bf_resident_reshape, _narrow and
+// _transfer re-lay the device's: the whole destination records written, the headers kept, each plane and mask its low words,
+// the child area its low bytes, everything else zero.
+static void relay_record(const HostRecords& from, uint32_t r, const bf_layout& F, HostRecords& to, uint32_t q, const bf_layout& T) {
   const uint32_t Wn = T.words, Wo = F.words;
-  for (uint32_t r = 0; r < b->cap; ++r) {
-    const uint8_t* s = b->rec.state + (size_t)r * F.state_stride;
-    uint8_t* d = nr.state + (size_t)r * T.state_stride;
-    memcpy(d, s, sizeof(bf_run_header));
-    relay_planes(d, s, T.off_phase, F.off_phase, 4, Wn, Wo);
-    relay_planes(d, s, T.off_cond, F.off_cond, 2, Wn, Wo);
-    relay_planes(d, s, T.off_decision, F.off_decision, 2, Wn, Wo);
-    if (F.off_child != BF_OFF_NONE && T.off_child != BF_OFF_NONE)
-      memcpy(d + T.off_child, s + F.off_child, std::min(child_area_bytes(F), child_area_bytes(T)));
-    s = b->rec.result + (size_t)r * F.result_stride;
-    d = nr.result + (size_t)r * T.result_stride;
-    memcpy(d, s, sizeof(bf_result_header));
-    relay_planes(d, s, T.off_ready, F.off_ready, 1, Wn, Wo);
-    relay_planes(d, s, T.off_skip, F.off_skip, 1, Wn, Wo);
-    relay_planes(d, s, T.off_fail, F.off_fail, 1, Wn, Wo);
-    relay_planes(d, s, T.off_needs_cond, F.off_needs_cond, 1, Wn, Wo);
-    relay_planes(d, s, T.off_skip_dep, F.off_skip_dep, 1, Wn, Wo);
-    relay_planes(d, s, T.off_phase_out, F.off_phase_out, 4, Wn, Wo);
-  }
+  const uint8_t* s = from.state + (size_t)r * F.state_stride;
+  uint8_t* d = to.state + (size_t)q * T.state_stride;
+  memset(d, 0, T.state_stride);
+  memcpy(d, s, sizeof(bf_run_header));
+  relay_planes(d, s, T.off_phase, F.off_phase, 4, Wn, Wo);
+  relay_planes(d, s, T.off_cond, F.off_cond, 2, Wn, Wo);
+  relay_planes(d, s, T.off_decision, F.off_decision, 2, Wn, Wo);
+  if (F.off_child != BF_OFF_NONE && T.off_child != BF_OFF_NONE)
+    memcpy(d + T.off_child, s + F.off_child, std::min(child_area_bytes(F), child_area_bytes(T)));
+  s = from.result + (size_t)r * F.result_stride;
+  d = to.result + (size_t)q * T.result_stride;
+  memset(d, 0, T.result_stride);
+  memcpy(d, s, sizeof(bf_result_header));
+  relay_planes(d, s, T.off_ready, F.off_ready, 1, Wn, Wo);
+  relay_planes(d, s, T.off_skip, F.off_skip, 1, Wn, Wo);
+  relay_planes(d, s, T.off_fail, F.off_fail, 1, Wn, Wo);
+  relay_planes(d, s, T.off_needs_cond, F.off_needs_cond, 1, Wn, Wo);
+  relay_planes(d, s, T.off_skip_dep, F.off_skip_dep, 1, Wn, Wo);
+  relay_planes(d, s, T.off_phase_out, F.off_phase_out, 4, Wn, Wo);
+}
+
+// every record of the mirror re-laid from F to T into nr, at the same index
+static void relay_records(const bfh_batch* b, HostRecords& nr, const bf_layout& F, const bf_layout& T) {
+  for (uint32_t r = 0; r < b->cap; ++r) relay_record(b->rec, r, F, nr, r, T);
 }
 
 int bfh_batch_reshape(bfh_batch* b, uint32_t steps_max, uint32_t child_nibbles, uint32_t fields, uint32_t capacity) {
@@ -874,6 +881,58 @@ int bfh_batch_reshape(bfh_batch* b, uint32_t steps_max, uint32_t child_nibbles, 
 // steps needed by plane word w holding v: one past its highest set bit
 static uint32_t word_extent(uint32_t w, uint32_t v) { return v ? 32u * w + 32u - (uint32_t)__builtin_clz(v) : 0u; }
 
+// the input fields (BF_F_COND, _DECISION, _CHILD) layout T has a place for
+static uint32_t placed(const bf_layout& T) {
+  return (T.off_cond != BF_OFF_NONE ? BF_F_COND : 0u) | (T.off_decision != BF_OFF_NONE ? BF_F_DECISION : 0u) |
+         (T.off_child != BF_OFF_NONE ? BF_F_CHILD : 0u);
+}
+
+struct RunExtent {
+  uint32_t steps = 0, child = 0, fields = 0;   // steps_max and child_nibbles it needs, the input fields holding a non-default code
+};
+
+// The extent of bf_resident_extent over run r of a mirror alone, against a target layout T: the code planes and child nibbles of
+// its record (any r < cap), its Story (r < n), and the result planes T keeps when the last eval evaluated it (r < evaluated).
+static RunExtent run_extent(const bfh_batch* b, uint32_t r, const bf_layout& T) {
+  const bf_layout& F = b->L;
+  const uint32_t W = F.words;
+  RunExtent e;
+  auto planes = [&](const uint8_t* rec, uint32_t off, uint32_t n, uint32_t field) {
+    if (off == BF_OFF_NONE) return;
+    const uint32_t* p = reinterpret_cast<const uint32_t*>(rec + off);
+    for (uint32_t k = 0; k < n * W; ++k)
+      if (p[k]) { e.steps = std::max(e.steps, word_extent(k % W, p[k])); e.fields |= field; }
+  };
+  const uint8_t* rec = b->rec.state + (size_t)r * F.state_stride;
+  planes(rec, F.off_phase, 4, 0);
+  planes(rec, F.off_cond, 2, BF_F_COND);
+  planes(rec, F.off_decision, 2, BF_F_DECISION);
+  for (uint32_t i = 0; F.off_child != BF_OFF_NONE && i < F.child_nibbles; ++i)
+    if ((rec[F.off_child + i / 2] >> ((i & 1u) * 4u)) & 0xFu) { e.child = std::max(e.child, i + 1); e.fields |= BF_F_CHILD; }
+  if (r >= b->n) return e;
+  e.steps = std::max(e.steps, (uint32_t)b->story_of_run[r]->flags.size());
+  e.child = std::max(e.child, b->story_of_run[r]->child_nibbles);
+  if (r >= b->evaluated) return e;   // a run added since the last eval has no results yet
+  const uint8_t* res = b->rec.result + (size_t)r * F.result_stride;
+  auto kept = [](uint32_t to, uint32_t from) { return to != BF_OFF_NONE ? from : BF_OFF_NONE; };
+  planes(res, F.off_ready, 1, 0);
+  planes(res, F.off_skip, 1, 0);
+  planes(res, kept(T.off_fail, F.off_fail), 1, 0);
+  planes(res, kept(T.off_needs_cond, F.off_needs_cond), 1, 0);
+  planes(res, kept(T.off_skip_dep, F.off_skip_dep), 1, 0);
+  planes(res, kept(T.off_phase_out, F.off_phase_out), 4, 0);
+  return e;
+}
+
+// whether a pending delta still has its place in layout T
+static bool delta_fits(const bf_delta& d, const bf_layout& T) {
+  return d.field == BF_DELTA_PHASE      ? d.index < T.steps_max
+         : d.field == BF_DELTA_COND     ? T.off_cond != BF_OFF_NONE && d.index < T.steps_max
+         : d.field == BF_DELTA_DECISION ? T.off_decision != BF_OFF_NONE && d.index < T.steps_max
+         : d.field == BF_DELTA_CHILD    ? T.off_child != BF_OFF_NONE && d.index < T.child_nibbles
+                                        : true;
+}
+
 int bfh_batch_narrow(bfh_batch* b, uint32_t steps_max, uint32_t child_nibbles, uint32_t fields) {
   if (!b) return BF_EINVAL;
   bf_layout T;
@@ -885,51 +944,16 @@ int bfh_batch_narrow(bfh_batch* b, uint32_t steps_max, uint32_t child_nibbles, u
     return BF_EINVAL;
   }
   if (memcmp(&F, &T, sizeof T) == 0) return BF_OK;
-  // the extent of bf_resident_narrow over the mirror's own records, the stories of its runs and the result records of the runs
-  // the last eval evaluated
-  uint32_t steps = 0, child = 0, in_fields = 0;
-  const uint32_t W = F.words;
+  RunExtent x;   // the extent of bf_resident_narrow: every record of the mirror, the runs' Stories, the evaluated results
   for (uint32_t r = 0; r < b->cap; ++r) {
-    const uint8_t* rec = b->rec.state + (size_t)r * F.state_stride;
-    auto planes = [&](uint32_t off, uint32_t n, uint32_t field) {
-      if (off == BF_OFF_NONE) return;
-      const uint32_t* p = reinterpret_cast<const uint32_t*>(rec + off);
-      for (uint32_t k = 0; k < n * W; ++k)
-        if (p[k]) { steps = std::max(steps, word_extent(k % W, p[k])); in_fields |= field; }
-    };
-    planes(F.off_phase, 4, 0);
-    planes(F.off_cond, 2, BF_F_COND);
-    planes(F.off_decision, 2, BF_F_DECISION);
-    for (uint32_t i = 0; F.off_child != BF_OFF_NONE && i < F.child_nibbles; ++i)
-      if ((rec[F.off_child + i / 2] >> ((i & 1u) * 4u)) & 0xFu) { child = std::max(child, i + 1); in_fields |= BF_F_CHILD; }
-    if (r >= b->n) continue;
-    steps = std::max(steps, (uint32_t)b->story_of_run[r]->flags.size());
-    child = std::max(child, b->story_of_run[r]->child_nibbles);
-    if (r >= b->evaluated) continue;   // a run added since the last eval has no results yet
-    const uint8_t* res = b->rec.result + (size_t)r * F.result_stride;
-    const std::pair<uint32_t, uint32_t> masks[] = {{F.off_ready, 1}, {F.off_skip, 1}, {T.off_fail != BF_OFF_NONE ? F.off_fail : BF_OFF_NONE, 1},
-                                                   {T.off_needs_cond != BF_OFF_NONE ? F.off_needs_cond : BF_OFF_NONE, 1},
-                                                   {T.off_skip_dep != BF_OFF_NONE ? F.off_skip_dep : BF_OFF_NONE, 1},
-                                                   {T.off_phase_out != BF_OFF_NONE ? F.off_phase_out : BF_OFF_NONE, 4}};
-    for (const auto& m : masks) {
-      if (m.first == BF_OFF_NONE) continue;
-      const uint32_t* p = reinterpret_cast<const uint32_t*>(res + m.first);
-      for (uint32_t k = 0; k < m.second * W; ++k) steps = std::max(steps, word_extent(k % W, p[k]));
-    }
+    const RunExtent e = run_extent(b, r, T);
+    x.steps = std::max(x.steps, e.steps); x.child = std::max(x.child, e.child); x.fields |= e.fields;
   }
-  const uint32_t placed = (T.off_cond != BF_OFF_NONE ? BF_F_COND : 0u) | (T.off_decision != BF_OFF_NONE ? BF_F_DECISION : 0u) |
-                          (T.off_child != BF_OFF_NONE ? BF_F_CHILD : 0u);
-  if (steps > T.steps_max) { b->err = "the batch needs steps_max " + std::to_string(steps); return BF_EINVAL; }
-  if (T.off_child != BF_OFF_NONE && child > T.child_nibbles) { b->err = "the batch needs child_nibbles " + std::to_string(child); return BF_EINVAL; }
-  if (in_fields & ~placed) { b->err = "the new layout drops an input field holding a non-default code"; return BF_EINVAL; }
-  for (const bf_delta& d : b->deltas) {   // a pending delta must still have its place: none is dropped
-    const bool fits = d.field == BF_DELTA_PHASE ? d.index < T.steps_max
-                      : d.field == BF_DELTA_COND ? T.off_cond != BF_OFF_NONE && d.index < T.steps_max
-                      : d.field == BF_DELTA_DECISION ? T.off_decision != BF_OFF_NONE && d.index < T.steps_max
-                      : d.field == BF_DELTA_CHILD ? T.off_child != BF_OFF_NONE && d.index < T.child_nibbles
-                      : true;
-    if (!fits) { b->err = "a pending delta of run " + std::to_string(d.run) + " lies outside the new layout"; return BF_EINVAL; }
-  }
+  if (x.steps > T.steps_max) { b->err = "the batch needs steps_max " + std::to_string(x.steps); return BF_EINVAL; }
+  if (T.off_child != BF_OFF_NONE && x.child > T.child_nibbles) { b->err = "the batch needs child_nibbles " + std::to_string(x.child); return BF_EINVAL; }
+  if (x.fields & ~placed(T)) { b->err = "the new layout drops an input field holding a non-default code"; return BF_EINVAL; }
+  for (const bf_delta& d : b->deltas)   // a pending delta must still have its place: none is dropped
+    if (!delta_fits(d, T)) { b->err = "a pending delta of run " + std::to_string(d.run) + " lies outside the new layout"; return BF_EINVAL; }
   HostRecords nr;
   if (!nr.alloc(b->ctx, (size_t)b->cap * T.state_stride, (size_t)b->cap * T.result_stride)) {
     b->err = "out of host memory";
@@ -950,6 +974,39 @@ int bfh_batch_narrow(bfh_batch* b, uint32_t steps_max, uint32_t child_nibbles, u
   return BF_OK;
 }
 
+// The mirror compacted once the n runs marked in `gone` have left it (retired or transferred) and the device has agreed, as
+// bf_resident_retire compacts the device's records: the live runs of [m, N) move into the freed indices by the move rule of
+// retire_moves.h and [m, N) is zeroed; the pending deltas of leaving runs go, those of moved runs apply at the new index (no two
+// keys meet: a target has left); the moves go out to moves_from / moves_to.  -> the number of moves
+static int compact_runs(bfh_batch* b, const std::vector<uint8_t>& gone, uint32_t n, uint32_t* moves_from, uint32_t* moves_to) {
+  const uint32_t N = b->n, m = N - n;
+  std::vector<uint32_t> to;
+  const uint32_t n_moves = bf::retire_moves(gone, m, n, to);
+  const size_t ss = b->L.state_stride, rs = b->L.result_stride;
+  for (uint32_t i = 0; i < n; ++i) {
+    if (to[i] == bf::kRetireNoMove) continue;
+    memcpy(b->rec.state + to[i] * ss, b->rec.state + (m + i) * ss, ss);
+    memcpy(b->rec.result + to[i] * rs, b->rec.result + (m + i) * rs, rs);
+    b->story_of_run[to[i]] = b->story_of_run[m + i];
+  }
+  memset(b->rec.state + (size_t)m * ss, 0, (size_t)n * ss);
+  memset(b->rec.result + (size_t)m * rs, 0, (size_t)n * rs);
+  b->story_of_run.resize(m);
+  rewrite_deltas(b, [&](bf_delta& d) {
+    if (d.run < N && gone[d.run]) return false;
+    if (d.run >= m) d.run = to[d.run - m];
+    return true;
+  });
+  b->n = m;
+  if (b->uploaded > m) b->uploaded = m;
+  // a run moved from at or above `evaluated` takes its unevaluated record below it
+  for (uint32_t i = 0; i < n; ++i)
+    if (to[i] != bf::kRetireNoMove && m + i >= b->evaluated) b->evaluated = std::min(b->evaluated, to[i]);
+  if (b->evaluated > m) b->evaluated = m;
+  bf::write_moves(to, m, moves_from, moves_to);
+  return (int)n_moves;
+}
+
 int bfh_batch_retire(bfh_batch* b, const uint32_t* runs, uint32_t n, uint32_t capacity, uint32_t* moves_from, uint32_t* moves_to) {
   if (!b) return BF_EINVAL;
   const uint32_t N = b->n;
@@ -962,13 +1019,6 @@ int bfh_batch_retire(bfh_batch* b, const uint32_t* runs, uint32_t n, uint32_t ca
   const uint32_t m = N - n, cap = capacity ? capacity : b->cap;
   if (cap < m || cap > b->cap) { b->err = "capacity must be 0 or within [size - n, the current capacity]"; return BF_EINVAL; }
   if (n == 0 && cap == b->cap) return 0;
-  // the move rule of bf_resident_retire: the k-th retired index below m receives the k-th live index of [m, N)
-  std::vector<uint32_t> from, to, new_index(n, UINT32_MAX);   // new_index[i]: where run m + i goes
-  for (uint32_t i = 0, hole = 0; i < n; ++i) {
-    if (gone[m + i]) continue;
-    while (!gone[hole]) ++hole;
-    from.push_back(m + i); to.push_back(hole); new_index[i] = hole++;
-  }
   const bf_layout& L = b->L;
   HostRecords nr;
   if (cap != b->cap && !nr.alloc(b->ctx, (size_t)cap * L.state_stride, (size_t)cap * L.result_stride)) {
@@ -984,36 +1034,14 @@ int bfh_batch_retire(bfh_batch* b, const uint32_t* runs, uint32_t n, uint32_t ca
     }
     if (rc != BF_OK) { b->err = bf_last_error(b->ctx); return rc; }
   }
-  const size_t ss = L.state_stride, rs = L.result_stride;
-  for (size_t k = 0; k < from.size(); ++k) {
-    memcpy(b->rec.state + to[k] * ss, b->rec.state + from[k] * ss, ss);
-    memcpy(b->rec.result + to[k] * rs, b->rec.result + from[k] * rs, rs);
-    b->story_of_run[to[k]] = b->story_of_run[from[k]];
-  }
-  memset(b->rec.state + (size_t)m * ss, 0, (size_t)n * ss);
-  memset(b->rec.result + (size_t)m * rs, 0, (size_t)n * rs);
-  b->story_of_run.resize(m);
+  const int n_moves = compact_runs(b, gone, n, moves_from, moves_to);
   if (nr.state) {
-    memcpy(nr.state, b->rec.state, (size_t)m * ss);
-    memcpy(nr.result, b->rec.result, (size_t)m * rs);
+    memcpy(nr.state, b->rec.state, (size_t)m * L.state_stride);
+    memcpy(nr.result, b->rec.result, (size_t)m * L.result_stride);
     b->rec.swap(nr);
     b->cap = cap;
   }
-  // pending deltas: those of retired runs go, those of moved runs apply at the new index (no two keys meet: a target was retired)
-  rewrite_deltas(b, [&](bf_delta& d) {
-    if (gone[d.run]) return false;
-    if (d.run >= m) d.run = new_index[d.run - m];
-    return true;
-  });
-  b->n = m;
-  if (b->uploaded > m) b->uploaded = m;
-  // a run moved from at or above `evaluated` takes its unevaluated record below it
-  for (size_t k = 0; k < from.size(); ++k)
-    if (from[k] >= b->evaluated) b->evaluated = std::min(b->evaluated, to[k]);
-  if (b->evaluated > m) b->evaluated = m;
-  if (moves_from && !from.empty()) memcpy(moves_from, from.data(), from.size() * 4);
-  if (moves_to && !to.empty()) memcpy(moves_to, to.data(), to.size() * 4);
-  return (int)from.size();
+  return n_moves;
 }
 
 int bfh_batch_transfer(bfh_batch* src, bfh_batch* dst, const uint32_t* runs, uint32_t n, uint32_t* moves_from, uint32_t* moves_to) {
@@ -1030,58 +1058,16 @@ int bfh_batch_transfer(bfh_batch* src, bfh_batch* dst, const uint32_t* runs, uin
     gone[runs[i]] = 1;
   }
   if (n == 0) return 0;
-  // each run must fit the destination layout by bf_resident_narrow's test applied to it alone: its record, its Story and the
-  // result record of a run the last eval covered (the planes T keeps)
+  // each run must fit the destination layout by bf_resident_narrow's test applied to it alone
   const bf_layout F = src->L, T = dst->L;
-  const uint32_t W = F.words;
-  const uint32_t placed = (T.off_cond != BF_OFF_NONE ? BF_F_COND : 0u) | (T.off_decision != BF_OFF_NONE ? BF_F_DECISION : 0u) |
-                          (T.off_child != BF_OFF_NONE ? BF_F_CHILD : 0u);
   for (uint32_t i = 0; i < n; ++i) {
-    const uint32_t r = runs[i];
-    uint32_t steps = (uint32_t)src->story_of_run[r]->flags.size(), child = src->story_of_run[r]->child_nibbles, in_fields = 0;
-    const uint8_t* rec = src->rec.state + (size_t)r * F.state_stride;
-    auto planes = [&](uint32_t off, uint32_t np, uint32_t field) {
-      if (off == BF_OFF_NONE) return;
-      const uint32_t* p = reinterpret_cast<const uint32_t*>(rec + off);
-      for (uint32_t k = 0; k < np * W; ++k)
-        if (p[k]) { steps = std::max(steps, word_extent(k % W, p[k])); in_fields |= field; }
-    };
-    planes(F.off_phase, 4, 0);
-    planes(F.off_cond, 2, BF_F_COND);
-    planes(F.off_decision, 2, BF_F_DECISION);
-    for (uint32_t k = 0; F.off_child != BF_OFF_NONE && k < F.child_nibbles; ++k)
-      if ((rec[F.off_child + k / 2] >> ((k & 1u) * 4u)) & 0xFu) { child = std::max(child, k + 1); in_fields |= BF_F_CHILD; }
-    if (r < src->evaluated) {
-      const uint8_t* res = src->rec.result + (size_t)r * F.result_stride;
-      const std::pair<uint32_t, uint32_t> masks[] = {{F.off_ready, 1}, {F.off_skip, 1}, {T.off_fail != BF_OFF_NONE ? F.off_fail : BF_OFF_NONE, 1},
-                                                     {T.off_needs_cond != BF_OFF_NONE ? F.off_needs_cond : BF_OFF_NONE, 1},
-                                                     {T.off_skip_dep != BF_OFF_NONE ? F.off_skip_dep : BF_OFF_NONE, 1},
-                                                     {T.off_phase_out != BF_OFF_NONE ? F.off_phase_out : BF_OFF_NONE, 4}};
-      for (const auto& mk : masks) {
-        if (mk.first == BF_OFF_NONE) continue;
-        const uint32_t* p = reinterpret_cast<const uint32_t*>(res + mk.first);
-        for (uint32_t k = 0; k < mk.second * W; ++k) steps = std::max(steps, word_extent(k % W, p[k]));
-      }
-    }
-    if (steps > T.steps_max || (T.off_child != BF_OFF_NONE && child > T.child_nibbles) || (in_fields & ~placed))
-      return refuse("runs[" + std::to_string(i) + "] (run " + std::to_string(r) + ") does not fit the destination layout");
+    const RunExtent e = run_extent(src, runs[i], T);
+    if (e.steps > T.steps_max || (T.off_child != BF_OFF_NONE && e.child > T.child_nibbles) || (e.fields & ~placed(T)))
+      return refuse("runs[" + std::to_string(i) + "] (run " + std::to_string(runs[i]) + ") does not fit the destination layout");
   }
-  for (const bf_delta& d : src->deltas) {   // a pending delta of a moved run must still have its place: none is dropped
-    if (d.run >= N || !gone[d.run]) continue;
-    const bool fits = d.field == BF_DELTA_PHASE ? d.index < T.steps_max
-                      : d.field == BF_DELTA_COND ? T.off_cond != BF_OFF_NONE && d.index < T.steps_max
-                      : d.field == BF_DELTA_DECISION ? T.off_decision != BF_OFF_NONE && d.index < T.steps_max
-                      : d.field == BF_DELTA_CHILD ? T.off_child != BF_OFF_NONE && d.index < T.child_nibbles
-                      : true;
-    if (!fits) return refuse("a pending delta of run " + std::to_string(d.run) + " lies outside the destination layout");
-  }
-  const uint32_t m = N - n;
-  std::vector<uint32_t> from, to, new_index(n, UINT32_MAX);   // the move rule of bfh_batch_retire
-  for (uint32_t i = 0, hole = 0; i < n; ++i) {
-    if (gone[m + i]) continue;
-    while (!gone[hole]) ++hole;
-    from.push_back(m + i); to.push_back(hole); new_index[i] = hole++;
-  }
+  for (const bf_delta& d : src->deltas)   // a pending delta of a moved run must still have its place: none is dropped
+    if (d.run < N && gone[d.run] && !delta_fits(d, T))
+      return refuse("a pending delta of run " + std::to_string(d.run) + " lies outside the destination layout");
   if (src->resident) {   // every run of both batches on the device first, then the device: it fails without changes, and so do the mirrors
     int rc = flush_uploads(src);
     if (rc == BF_OK) rc = flush_uploads(dst);
@@ -1093,27 +1079,8 @@ int bfh_batch_transfer(bfh_batch* src, bfh_batch* dst, const uint32_t* runs, uin
     if (rc != BF_OK) { src->err = dst->err = bf_last_error(src->ctx); return rc; }
   }
   // arrivals: re-laid at the destination layout, in the order of runs[]
-  const size_t ss = F.state_stride, rs = F.result_stride;
   for (uint32_t i = 0; i < n; ++i) {
-    const uint8_t* s = src->rec.state + (size_t)runs[i] * ss;
-    uint8_t* d = dst->rec.state + (size_t)(D + i) * T.state_stride;
-    memset(d, 0, T.state_stride);
-    memcpy(d, s, sizeof(bf_run_header));
-    relay_planes(d, s, T.off_phase, F.off_phase, 4, T.words, W);
-    relay_planes(d, s, T.off_cond, F.off_cond, 2, T.words, W);
-    relay_planes(d, s, T.off_decision, F.off_decision, 2, T.words, W);
-    if (F.off_child != BF_OFF_NONE && T.off_child != BF_OFF_NONE)
-      memcpy(d + T.off_child, s + F.off_child, std::min(child_area_bytes(F), child_area_bytes(T)));
-    s = src->rec.result + (size_t)runs[i] * rs;
-    d = dst->rec.result + (size_t)(D + i) * T.result_stride;
-    memset(d, 0, T.result_stride);
-    memcpy(d, s, sizeof(bf_result_header));
-    relay_planes(d, s, T.off_ready, F.off_ready, 1, T.words, W);
-    relay_planes(d, s, T.off_skip, F.off_skip, 1, T.words, W);
-    relay_planes(d, s, T.off_fail, F.off_fail, 1, T.words, W);
-    relay_planes(d, s, T.off_needs_cond, F.off_needs_cond, 1, T.words, W);
-    relay_planes(d, s, T.off_skip_dep, F.off_skip_dep, 1, T.words, W);
-    relay_planes(d, s, T.off_phase_out, F.off_phase_out, 4, T.words, W);
+    relay_record(src->rec, runs[i], F, dst->rec, D + i, T);
     dst->story_of_run.push_back(src->story_of_run[runs[i]]);
   }
   // pending deltas of moved runs go to the destination's log under their new index (no key meets one there: every index from
@@ -1131,28 +1098,7 @@ int bfh_batch_transfer(bfh_batch* src, bfh_batch* dst, const uint32_t* runs, uin
   dst->n = D + n;
   if (dst->resident) dst->uploaded = dst->n;
   if (all_evaluated) dst->evaluated = dst->n;
-  // the source compacts as bfh_batch_retire does
-  for (size_t k = 0; k < from.size(); ++k) {
-    memcpy(src->rec.state + to[k] * ss, src->rec.state + from[k] * ss, ss);
-    memcpy(src->rec.result + to[k] * rs, src->rec.result + from[k] * rs, rs);
-    src->story_of_run[to[k]] = src->story_of_run[from[k]];
-  }
-  memset(src->rec.state + (size_t)m * ss, 0, (size_t)n * ss);
-  memset(src->rec.result + (size_t)m * rs, 0, (size_t)n * rs);
-  src->story_of_run.resize(m);
-  rewrite_deltas(src, [&](bf_delta& d) {
-    if (d.run < N && gone[d.run]) return false;
-    if (d.run >= m) d.run = new_index[d.run - m];
-    return true;
-  });
-  src->n = m;
-  if (src->uploaded > m) src->uploaded = m;
-  for (size_t k = 0; k < from.size(); ++k)
-    if (from[k] >= src->evaluated) src->evaluated = std::min(src->evaluated, to[k]);
-  if (src->evaluated > m) src->evaluated = m;
-  if (moves_from && !from.empty()) memcpy(moves_from, from.data(), from.size() * 4);
-  if (moves_to && !to.empty()) memcpy(moves_to, to.data(), to.size() * 4);
-  return (int)from.size();
+  return compact_runs(src, gone, n, moves_from, moves_to);   // after the arrivals, which read the source's records
 }
 
 int bfh_batch_set_resident(bfh_batch* b, int on) {

@@ -11,7 +11,7 @@
 
 #include "ctx.h"
 
-using bf::cuda_fail; using bf::fail; using bf::round_up_sz;
+using bf::cuda_fail; using bf::fail; using bf::retire_moves; using bf::round_up_sz; using bf::write_moves;
 
 // the bf_resident_* definitions take their C linkage from include/bobrafrontier.h
 // ---- resident batches (row f2: incremental state upload) --------------------------------------------------
@@ -688,30 +688,6 @@ int bf_resident_narrow(bf_ctx* c, uint32_t h, const bf_layout* layout, bf_extent
   r->adopt(std::move(nb), T, r->cap);
   r->narrowed(N, results_may_change);
   return BF_OK;
-}
-
-// The move rule of a retirement, shared with transfers: the k-th retired index below m (ascending) receives the k-th live index
-// of [m, m + n); there are as many of each.  to[i] is the new index of run m + i, or kRetireNoMove.  -> the number of moves
-static uint32_t retire_moves(const std::vector<uint8_t>& gone, uint32_t m, uint32_t n, std::vector<uint32_t>& to) {
-  to.assign(n, bf::kRetireNoMove);
-  uint32_t n_moves = 0;
-  for (uint32_t i = 0, hole = 0; i < n; ++i) {
-    if (gone[m + i]) continue;
-    while (!gone[hole]) ++hole;
-    to[i] = hole++;
-    ++n_moves;
-  }
-  return n_moves;
-}
-
-// the moves of `to` into the caller's arrays (either may be NULL), ascending by target
-static void write_moves(const std::vector<uint32_t>& to, uint32_t m, uint32_t* moves_from, uint32_t* moves_to) {
-  for (uint32_t i = 0, k = 0; i < to.size() && (moves_from || moves_to); ++i) {
-    if (to[i] == bf::kRetireNoMove) continue;
-    if (moves_from) moves_from[k] = m + i;
-    if (moves_to) moves_to[k] = to[i];
-    ++k;
-  }
 }
 
 // Runs leave a live batch (resident.cu): the last live runs move into the indices the retired ones free, so the batch's runs
