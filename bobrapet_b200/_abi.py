@@ -201,6 +201,18 @@ class CommitArm(C.Structure):
     _fields_ = [(n, C.c_uint32) for n in ("struct_size", "now", "n_armed", "next_deadline")]
 
 
+OUTCOME_NONE, OUTCOME_SUCCEEDED, OUTCOME_DEPENDENCY_FAILED, OUTCOME_COMPENSATED = 0, 1, 2, 3   # BF_OUTCOME_*: bf_status_rec.outcome
+OUTCOME_COMPENSATION_FAILED, OUTCOME_CLEANUP_FAILED, OUTCOME_TIMED_OUT = 4, 5, 6
+OUTCOME_CANCELED, OUTCOME_STOPPED, OUTCOME_DEAD = 7, 8, 9
+STATUS_EVT_FAILED, STATUS_EVT_ALLOWED = 0x1, 0x2   # BF_STATUS_EVT_*: kind of a status event (bits 14-15)
+STATUS_NO_STEP = 0xFFFF                            # BF_STATUS_NO_STEP: first_failed of a run without a listed failed set
+
+
+class StatusOut(C.Structure):
+    _fields_ = [("struct_size", C.c_uint32), ("reserved", C.c_uint32), ("records", C.c_void_p), ("events", C.c_void_p),
+                ("events_cap", C.c_uint64), ("n_events", C.c_uint64)]
+
+
 def sched_stride(words: int) -> int:
     return (16 + 12 * words + 15) & ~15
 
@@ -257,6 +269,7 @@ SYMBOLS = [
     ("bf_resident_commit", C.c_int, [C.c_void_p, C.c_uint32, C.c_uint32, C.c_void_p, C.c_uint32, C.POINTER(CommitOut)]),
     ("bf_resident_commit_timed", C.c_int, [C.c_void_p, C.c_uint32, C.c_uint32, C.c_void_p, C.c_uint32, C.POINTER(CommitOut),
                                            C.POINTER(CommitArm)]),
+    ("bf_resident_status", C.c_int, [C.c_void_p, C.c_uint32, C.c_uint32, C.c_void_p, C.c_uint32, C.POINTER(StatusOut)]),
     ("bf_group_create", C.c_int, [C.POINTER(C.c_void_p), C.POINTER(C.c_int32), C.c_uint32, C.POINTER(Config)]),
     ("bf_group_destroy", None, [C.c_void_p]),
     ("bf_group_size", C.c_uint32, [C.c_void_p]),

@@ -48,6 +48,7 @@ cudaError_t launch_sched_put(const SchedPutParams& P, cudaStream_t stream);
 cudaError_t launch_runctl_put(const RunCtlPutParams& P, cudaStream_t stream);
 cudaError_t launch_runctl_restop(const RunCtlRestopParams& P, cudaStream_t stream);
 cudaError_t launch_commit(const CommitParams& P, bool apply, cudaStream_t stream);
+cudaError_t launch_status(const StatusParams& P, uint32_t smem_bytes, cudaStream_t stream);
 cudaError_t launch_closure(const Slot* slots, const uint32_t* slot_ids, const uint32_t* starts, uint32_t n, uint32_t n_slots,
                            uint32_t words_out, uint32_t* masks, cudaStream_t stream);
 cudaError_t launch_validate(const Slot* slots, const uint32_t* slot_ids, uint32_t n, uint32_t n_slots, uint32_t* status,
@@ -184,6 +185,7 @@ struct bf_ctx {
     bf::ResultTail tail;   // written by a compaction's last kernel; a pass without one copies its counts into tail.counts
     uint32_t fire[4];      // bf_resident_fire: n_fired, n_written, n_pruned, next_deadline
     uint32_t commit[8];    // bf_resident_commit: the offender key (two words), then the five counts
+    unsigned long long status_events;   // bf_resident_status: the events of the call
     bf_counts counts() const { return {tail.counts[0], tail.counts[1], tail.counts[2], tail.counts[3]}; }
   }* pinned = nullptr;
   DevBuf<bf_expansion> d_exp;

@@ -493,6 +493,28 @@ struct CommitParams {
   CommitTimings arm;             // arm.tim = nullptr: no arming
 };
 
+// bf_resident_status (resident.cu): one warp per listed run.  status_count stores each listed run's event count and each CTA's
+// total, status_scan turns the CTA totals into the events of the CTAs before each and posts the sum, status_list writes the
+// records and the events.  With a child area each warp has a shared stage for stage H: the state record, the topology record
+// (topo_bytes: the largest record the layout fits) and 256 scratch bytes.
+static_assert(sizeof(bf_status_rec) == 32, "bf_status_rec must be 32 bytes");
+constexpr uint32_t kStatusStaticSmem = 32;   // status_runs' static shared memory (one word per warp), beside the warps' stages
+struct StatusParams {
+  const uint8_t* state;
+  const Slot* slots;
+  uint32_t n_slots;
+  const bf_run_ctl* runctl;         // or nullptr: no run is stopped
+  const uint32_t* runs;             // [n] ascending, or nullptr: listed run i is run i
+  uint32_t n, warps_per_block;
+  uint32_t words, state_stride, off_phase, off_decision, off_child, topo_bytes;
+  uint32_t* run_events;             // [n] events of each listed run (status_count)
+  unsigned long long* cta_events;   // [CTAs] events of each CTA, then (status_scan) of the CTAs before it
+  unsigned long long* total;        // [1] events of the call (status_scan)
+  bf_status_rec* records;           // [n]
+  uint16_t* events;                 // [events_cap]
+  unsigned long long events_cap;
+};
+
 // bf_resident_sched_put: req[i] is written into area[req[i].run]
 struct SchedPutParams {
   bf_sched_run* area;

@@ -203,107 +203,8 @@ __global__ void __launch_bounds__(RB == 2 ? 768 : 512, RB == 1 ? 2 : 1) frontier
 
     for (uint32_t it = 0; it < cap; ++it) {
       ++iters;
-      // ---------------- stage H: parallel join (dag.go:1131-1198) ----------------
-      // A registered parallel step that is neither absent nor terminal joins when every child is terminal: Failed if a
-      // terminal child neither succeeded / was skipped nor is an allowFailure branch, else Succeeded.  Child phases are
-      // nibbles, eight per word: one lane classifies eight children with the bit-plane tables (SWAR), a sub-warp of SW
-      // lanes covers one descriptor, 32 / SW descriptors per round, and the verdicts reach the lanes that own the parents'
-      // words through two scratch words per step word (the status-byte area is not in use yet at this point).
-      if (CH && has_child && nP != 0) {
-        const uint32_t ACTIVE = T_PAR & (p0 | p1 | p2 | p3) & ~plut<BF_LUT_TERMINAL>(p0, p1, p2, p3);
-        if (__any_sync(FULL, ACTIVE != 0)) {
-          const uint32_t pd_a = tr_a + h1.z, child_a = sr_a + P.off_child;
-          // which descriptors join at all: registered, with children, parent neither absent nor terminal (lane q <-> desc q,
-          // second round for descs 32..63), and the widest of them — usually none or a few of the run's descriptors
-          uint32_t take_lo = 0, take_hi = 0, mb = 0;
-          for (uint32_t q0 = 0; q0 < nP; q0 += 32) {
-            const uint32_t q = q0 + lane;
-            const uint32_t sb = q < nP ? lds_u32(pd_a + q * 16u) : 0u;   // step | branches << 16
-            const uint32_t actw = __shfl_sync(FULL, ACTIVE, ((sb & 0xFFFFu) >> 5) & 31u);
-            const uint32_t reg = lds_u32(sr_a + 8u + (q0 >> 3));          // children_registered, 32 descs per word
-            const bool tk = q < nP && (sb >> 16) != 0u && ((reg >> lane) & 1u) != 0u && ((actw >> (sb & 31u)) & 1u) != 0u;
-            const uint32_t m = __ballot_sync(FULL, tk);
-            if (q0 == 0) take_lo = m; else take_hi = m;
-            if (tk) mb = max(mb, sb >> 16);
-          }
-          mb = __reduce_max_sync(FULL, mb);
-          const uint32_t mw = (mb + 7u) >> 3;   // child words of the widest joining descriptor
-          if ((take_lo | take_hi) == 0u) {
-            // nothing to join in this pass
-          } else if (mw <= 32u) {
-            const uint32_t lgs = mw > 1u ? 32u - (uint32_t)__clz(mw - 1u) : 0u;   // sub-warp of SW = 2^lgs >= mw lanes per descriptor
-            const uint32_t SW = 1u << lgs, DPI = 32u >> lgs, sub = lane >> lgs, wi = lane & (SW - 1u);
-            const uint32_t gm = (SW == 32u ? FULL : ((1u << SW) - 1u)) << (sub << lgs);
-            const uint32_t dmask = DPI == 32u ? FULL : ((1u << DPI) - 1u);
-            const uint32_t tS = st_a, tF = st_a + 4u * Wt;
-            __syncwarp();
-            if (act) { sts_u32(tS + lane * 4u, 0u); sts_u32(tF + lane * 4u, 0u); }
-            __syncwarp();
-            for (uint32_t q0 = 0; q0 < nP; q0 += DPI) {
-              const uint32_t tw = q0 < 32u ? take_lo >> q0 : take_hi >> (q0 - 32u);   // DPI divides 32: a round never straddles the words
-              if ((tw & dmask) == 0u) continue;                                       // warp-uniform
-              const uint32_t q = q0 + sub;
-              const bool take = (tw >> sub) & 1u;
-              uint4 d = make_uint4(0u, 0u, 0u, 0u);
-              if (take) d = lds_v4(pd_a + q * 16u);          // step | branches << 16, child_first, allow_off, -
-              const uint32_t step = d.x & 0xFFFFu, br = d.x >> 16, wj = step >> 5, wb = step & 31u;
-              bool nd = false, fl = false;
-              if (take && wi * 8u < br) {
-                const uint32_t cw = lds_u32(child_a + (d.y >> 1) + wi * 4u);   // child_first is a multiple of 8 nibbles
-                const uint32_t vm = 0x11111111u & bmsk_clamp(0u, min(8u, br - wi * 8u) * 4u);
-                uint32_t x0 = cw & 0x11111111u, x1 = (cw >> 1) & 0x11111111u, x2 = (cw >> 2) & 0x11111111u, x3 = (cw >> 3) & 0x11111111u;
-                const uint32_t keep = ~(x0 & x1 & x2 & x3);                     // the reserved code 15 reads as 0
-                x0 &= keep; x1 &= keep; x2 &= keep; x3 &= keep;
-                const uint32_t done = plut<BF_LUT_TERMINAL>(x0, x1, x2, x3);
-                const uint32_t ab = (lds_u32(tr_a + d.z + (wi >> 2) * 4u) >> ((wi & 3u) * 8u)) & 0xFFu;   // allowFailure bits of my 8 branches
-                const uint32_t okc = plut<BF_LUT_COMPLETED0>(x0, x1, x2, x3) | spread4(ab);
-                nd = (vm & ~done) != 0u;
-                fl = (vm & done & ~okc) != 0u;
-              }
-              const uint32_t ndm = __ballot_sync(FULL, nd), flm = __ballot_sync(FULL, fl);
-              if (take && wi == 0u && (ndm & gm) == 0u) red_or_shared(((flm & gm) ? tF : tS) + wj * 4u, 1u << wb);
-            }
-            __syncwarp();
-            uint32_t sS = 0, sF = 0;
-            if (act) { sS = lds_u32(tS + lane * 4u); sF = lds_u32(tF + lane * 4u); }
-            if (__any_sync(FULL, (sS | sF) != 0u)) marked = true;
-            pset<BF_PHASE_SUCCEEDED>(sS, p0, p1, p2, p3);
-            pset<BF_PHASE_FAILED>(sF, p0, p1, p2, p3);
-            __syncwarp();
-          } else {   // more than 256 branches on one step: one descriptor at a time, one child per lane
-            const uint8_t* sr = gptr(sr_a);
-            const uint8_t* tr = gptr(tr_a);
-            const uint64_t registered = *reinterpret_cast<const uint64_t*>(sr + 8);
-            const ParDesc* pd = reinterpret_cast<const ParDesc*>(tr + h1.z);
-            const uint8_t* child = sr + P.off_child;
-            for (uint32_t q = 0; q < nP; ++q) {
-              if (!((registered >> q) & 1ull)) continue;
-              const ParDesc d = pd[q];
-              if (d.branches == 0) continue;  // no children to wait for (dag.go:1140-1143)
-              const uint32_t wj = d.step >> 5, wb = d.step & 31u;
-              if (!((__shfl_sync(FULL, ACTIVE, wj) >> wb) & 1u)) continue;
-              const uint32_t* allow = reinterpret_cast<const uint32_t*>(tr + d.allow_off);
-              bool all_done = true, any_failed = false;
-              for (uint32_t b = lane; b < d.branches; b += 32) {
-                const uint32_t cph = get_nibble(child, d.child_first + b);
-                const bool done = cph != 0 && ((BF_LUT_TERMINAL >> cph) & 1u);
-                const bool okc = cph == BF_PHASE_SUCCEEDED || cph == BF_PHASE_SKIPPED || ((allow[b >> 5] >> (b & 31u)) & 1u);
-                all_done = all_done && done;
-                any_failed = any_failed || (done && !okc);
-              }
-              all_done = __all_sync(FULL, all_done);
-              any_failed = __any_sync(FULL, any_failed);
-              if (all_done) {
-                marked = true;
-                if (lane == wj) {  // the lane that owns word wj rewrites its planes
-                  const uint32_t m = 1u << wb;
-                  if (any_failed) pset<BF_PHASE_FAILED>(m, p0, p1, p2, p3); else pset<BF_PHASE_SUCCEEDED>(m, p0, p1, p2, p3);
-                }
-              }
-            }
-          }
-        }
-      }
+      // ---------------- stage H: parallel join (stages.cuh) ----------------
+      if (CH && has_child && nP != 0) marked = stage_h(P, lane, act, Wt, nP, T_PAR, sr_a, tr_a, h1.z, st_a, marked, p0, p1, p2, p3);
 
       // ---------------- stages G, B, I and D-prep (stages.cuh) ----------------
       if (has_dec) gdirty |= stage_g(SYNC_T, TS, d0, d1, p0, p1, p2, p3);

@@ -4,7 +4,7 @@
 // atomicOr / atomicAnd on the record's u32 words, so deltas of different steps that share a word compose; byte
 // fields use a word-wide atomic on the containing u32.  At most one delta per (run, field, index) per launch
 // (contract in include/bobrafrontier.h), so no ordering between threads is needed.
-#include "kernel_common.cuh"
+#include "stages.cuh"
 
 namespace bf {
 
@@ -1143,6 +1143,201 @@ cudaError_t launch_commit(const CommitParams& P, bool apply, cudaStream_t stream
   if (P.n_runs == 0) return cudaSuccess;
   if (apply) commit_apply<<<(P.n_runs - 1u) / 8u + 1u, 256, 0, stream>>>(P);
   else commit_check<<<(P.n_runs - 1u) / 8u + 1u, 256, 0, stream>>>(P);
+  return cudaGetLastError();
+}
+
+// ---- run status (bf_resident_status) ------------------------------------------------------------------------------------------
+// One warp per listed run; lane w holds word w of its codes (words <= 32).  The codes of the state record (15 read as 0) take the
+// stages of a single pass: H (only when a registered parallel step is live, after the warp has copied both records into its
+// shared stage), G and I.  The counts, the failed set and the allowed failures are bit-plane tables over the result.
+struct RunStatus {
+  bf_status_rec rec;   // every field but first_event (warp-uniform)
+  uint32_t EV, FL;     // this lane's word of the listed steps, and of those the ones in the failed set
+  uint32_t p0, p1, p2, p3;
+};
+
+DI void run_status(const StatusParams& P, uint32_t i, uint32_t lane, uint32_t stage_a, RunStatus& s) {
+  const uint32_t r = P.runs ? P.runs[i] : i;
+  const uint8_t* rec = P.state + (size_t)r * P.state_stride;
+  const uint32_t slot = *reinterpret_cast<const uint32_t*>(rec);
+  const uint8_t* topo = slot < P.n_slots ? reinterpret_cast<const uint8_t*>(P.slots[slot].addr) : nullptr;
+  s.rec = bf_status_rec{};
+  s.rec.run = r;
+  s.rec.first_failed = BF_STATUS_NO_STEP;
+  s.EV = s.FL = s.p0 = s.p1 = s.p2 = s.p3 = 0u;
+  const TopoHeader th = topo ? *reinterpret_cast<const TopoHeader*>(topo) : TopoHeader{};
+  const uint32_t Wt = th.W, S = th.S;
+  if (Wt - 1u >= P.words) {   // dead slot, or wider than the layout
+    s.rec.outcome = BF_OUTCOME_DEAD;
+    return;
+  }
+  const bool act = lane < Wt;
+  const uint32_t rflags = rec[4];
+  uint32_t t0 = 0, t1 = 0, t2 = 0, AF = 0, TS = 0, G1 = 0, G2 = 0, VALID = 0, d0 = 0, d1 = 0;
+  uint32_t p0 = 0, p1 = 0, p2 = 0, p3 = 0;
+  if (act) {
+    const uint32_t* pl = reinterpret_cast<const uint32_t*>(topo + th.off_planes) + lane;
+    t0 = pl[PL_T0 * Wt]; t1 = pl[PL_T1 * Wt]; t2 = pl[PL_T2 * Wt];
+    AF = pl[PL_AF * Wt]; TS = pl[PL_TS * Wt]; G1 = pl[PL_G1 * Wt]; G2 = pl[PL_G2 * Wt];
+    VALID = bmsk_clamp(0u, S - lane * 32u);
+    const uint32_t* ph = reinterpret_cast<const uint32_t*>(rec + P.off_phase) + lane;
+    p0 = ph[0]; p1 = ph[P.words]; p2 = ph[2u * P.words]; p3 = ph[3u * P.words];
+    const uint32_t keep = VALID & ~(p0 & p1 & p2 & p3);
+    p0 &= keep; p1 &= keep; p2 &= keep; p3 &= keep;
+    if (P.off_decision != BF_OFF_NONE) {
+      const uint32_t* dw = reinterpret_cast<const uint32_t*>(rec + P.off_decision) + lane;
+      d0 = dw[0]; d1 = dw[P.words];
+    }
+  }
+  const uint32_t GM = VALID & ~G1 & ~G2;
+  const uint32_t SYNC_T = t0 & (t1 | t2);
+  const uint32_t T_PAR = ~t0 & t1 & ~t2 & VALID;
+  if (P.off_child != BF_OFF_NONE && th.P != 0 &&
+      __any_sync(FULL, (T_PAR & (p0 | p1 | p2 | p3) & ~plut<BF_LUT_TERMINAL>(p0, p1, p2, p3)) != 0u)) {
+    const uint32_t sr_a = stage_a, tr_a = stage_a + P.state_stride;
+    for (uint32_t x = lane; x < P.state_stride / 16u; x += 32u) {
+      const uint4 v = reinterpret_cast<const uint4*>(rec)[x];
+      sts_v4(sr_a + 16u * x, v.x, v.y, v.z, v.w);
+    }
+    for (uint32_t x = lane; x < th.rec_bytes / 16u; x += 32u) {
+      const uint4 v = reinterpret_cast<const uint4*>(topo)[x];
+      sts_v4(tr_a + 16u * x, v.x, v.y, v.z, v.w);
+    }
+    __syncwarp();
+    stage_h(P, lane, act, Wt, th.P, T_PAR, sr_a, tr_a, th.off_par, tr_a + P.topo_bytes, false, p0, p1, p2, p3);   // the codes, not whether they changed
+    __syncwarp();
+  }
+  if (P.off_decision != BF_OFF_NONE) stage_g(SYNC_T, TS, d0, d1, p0, p1, p2, p3);
+  const RunClass rc = stage_bi<true>(FULL, rflags, th.n_main, th.n_comp, th.n_final, AF, GM, G1, G2, p0, p1, p2, p3);
+
+  const uint32_t TERM = plut<BF_LUT_TERMINAL>(p0, p1, p2, p3) & ~plut<BF_LUT_COMPLETED0>(p0, p1, p2, p3);
+  const uint32_t FAILED = TERM & ~AF, ALLOWED = TERM & AF;
+  const uint32_t ac = redux_add((uint32_t)__popc(plut<0x0104u>(p0, p1, p2, p3)) | (uint32_t)__popc(plut<0x0008u>(p0, p1, p2, p3)) << 16);
+  const uint32_t fk = redux_add((uint32_t)__popc(plut<0x0010u>(p0, p1, p2, p3)) | (uint32_t)__popc(plut<0x2000u>(p0, p1, p2, p3)) << 16);
+  const uint32_t fb = redux_or(((FAILED & G2) ? 1u : 0u) | ((FAILED & G1) ? 2u : 0u) | ((FAILED & GM) ? 4u : 0u));
+  const uint32_t stop = P.runctl ? P.runctl[r].stop : BF_STOP_NONE;
+  uint32_t outcome, FL = 0u;
+  if (stop != BF_STOP_NONE) outcome = stop == BF_STOP_TIMEOUT ? BF_OUTCOME_TIMED_OUT : stop == BF_STOP_CANCEL ? BF_OUTCOME_CANCELED : BF_OUTCOME_STOPPED;
+  else if (rc.group != BF_GROUP_DONE) outcome = BF_OUTCOME_NONE;
+  else if (fb & 1u) { outcome = BF_OUTCOME_CLEANUP_FAILED; FL = FAILED & G2; }
+  else if (fb & 2u) { outcome = BF_OUTCOME_COMPENSATION_FAILED; FL = FAILED & G1; }
+  else if (fb & 4u) { outcome = th.n_comp ? BF_OUTCOME_COMPENSATED : BF_OUTCOME_DEPENDENCY_FAILED; FL = FAILED & GM; }
+  else outcome = BF_OUTCOME_SUCCEEDED;
+  const uint32_t phase = outcome == BF_OUTCOME_SUCCEEDED ? BF_PHASE_SUCCEEDED
+                         : outcome == BF_OUTCOME_COMPENSATED ? BF_PHASE_COMPENSATED
+                         : outcome == BF_OUTCOME_TIMED_OUT ? BF_PHASE_TIMEOUT
+                         : outcome == BF_OUTCOME_CANCELED ? BF_PHASE_FINISHED
+                         : outcome >= BF_OUTCOME_DEPENDENCY_FAILED && outcome <= BF_OUTCOME_CLEANUP_FAILED ? BF_PHASE_FAILED : 0u;
+  s.EV = FL | ALLOWED;
+  s.FL = FL;
+  s.p0 = p0; s.p1 = p1; s.p2 = p2; s.p3 = p3;
+  s.rec.n_events = (uint16_t)redux_add((uint32_t)__popc(s.EV));
+  s.rec.first_failed = (uint16_t)__reduce_min_sync(FULL, FL ? lane * 32u + (uint32_t)__ffs(FL) - 1u : BF_STATUS_NO_STEP);
+  s.rec.summary = (uint16_t)(rc.sum | rc.group);
+  s.rec.group = (uint8_t)rc.group;
+  s.rec.outcome = (uint8_t)outcome;
+  s.rec.story_phase = (uint8_t)phase;
+  s.rec.active = (uint16_t)(ac & 0xFFFFu); s.rec.completed = (uint16_t)(ac >> 16);
+  s.rec.failed = (uint16_t)(fk & 0xFFFFu); s.rec.skipped = (uint16_t)(fk >> 16);
+}
+
+// Count (kList = false): each listed run's events, and each CTA's total.  List (kList = true, after status_scan): the same runs
+// again, each record with the offset of its first event (the CTAs before, then the warps before in its CTA) and its events, lane by
+// lane in step order.
+template <bool kList>
+__global__ void __launch_bounds__(256, 1) status_runs(const StatusParams P) {
+  extern __shared__ __align__(16) uint8_t status_stage[];
+  __shared__ uint32_t warp_events[kStatusStaticSmem / 4];
+  const uint32_t warp = threadIdx.x >> 5, lane = threadIdx.x & 31u;
+  const uint32_t i = blockIdx.x * P.warps_per_block + warp;
+  const uint32_t stage_a = smem_u32(status_stage) + warp * (P.off_child != BF_OFF_NONE ? P.state_stride + P.topo_bytes + 256u : 0u);
+  RunStatus s;
+  if (!kList) {
+    uint32_t ne = 0;
+    if (i < P.n) {
+      run_status(P, i, lane, stage_a, s);
+      ne = s.rec.n_events;
+      if (lane == 0) P.run_events[i] = ne;
+    }
+    if (lane == 0) warp_events[warp] = ne;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+      unsigned long long sum = 0;
+      for (uint32_t w = 0; w < P.warps_per_block; ++w) sum += warp_events[w];
+      P.cta_events[blockIdx.x] = sum;
+    }
+    return;
+  }
+  if (i >= P.n) return;
+  run_status(P, i, lane, stage_a, s);
+  const uint32_t first = blockIdx.x * P.warps_per_block;
+  const unsigned long long base = P.cta_events[blockIdx.x] + redux_add(first + lane < i ? P.run_events[first + lane] : 0u);
+  s.rec.first_event = (uint32_t)base;
+  if (lane == 0) {
+    const uint4* v = reinterpret_cast<const uint4*>(&s.rec);
+    uint4* o = reinterpret_cast<uint4*>(P.records + i);
+    o[0] = v[0]; o[1] = v[1];
+  }
+  const uint32_t mine = (uint32_t)__popc(s.EV);
+  uint32_t incl = mine;
+  for (uint32_t d = 1; d < 32; d <<= 1) {
+    const uint32_t x = __shfl_up_sync(FULL, incl, d);
+    if (lane >= d) incl += x;
+  }
+  unsigned long long pos = base + incl - mine;
+  if (pos >= P.events_cap) return;
+  for (uint32_t x = s.EV; x; x &= x - 1u, ++pos) {
+    const uint32_t b = (uint32_t)__ffs(x) - 1u;
+    const uint32_t ph = ((s.p0 >> b) & 1u) | ((s.p1 >> b) & 1u) << 1 | ((s.p2 >> b) & 1u) << 2 | ((s.p3 >> b) & 1u) << 3;
+    const uint32_t kind = ((s.FL >> b) & 1u) ? BF_STATUS_EVT_FAILED : BF_STATUS_EVT_ALLOWED;
+    if (pos < P.events_cap) P.events[pos] = (uint16_t)((lane * 32u + b) | ph << 10 | kind << 14);
+  }
+}
+
+// One CTA: the CTA totals become the events of the CTAs before each (exclusive scan in place); the sum goes to P.total.
+__global__ void __launch_bounds__(1024) status_scan(const StatusParams P, uint32_t n_ctas) {
+  __shared__ unsigned long long s_e[32];
+  const uint32_t lane = threadIdx.x & 31u, warp = threadIdx.x >> 5;
+  unsigned long long carry = 0;
+  for (uint32_t base = 0; base < n_ctas; base += 1024u) {
+    const uint32_t i = base + threadIdx.x;
+    const unsigned long long e = i < n_ctas ? P.cta_events[i] : 0ull;
+    unsigned long long ie = e;
+#pragma unroll
+    for (int d = 1; d < 32; d <<= 1) {
+      const unsigned long long b = __shfl_up_sync(FULL, ie, d);
+      if ((int)lane >= d) ie += b;
+    }
+    if (lane == 31) s_e[warp] = ie;
+    __syncthreads();
+    if (warp == 0) {   // the warp totals' inclusive scan
+      unsigned long long we = s_e[lane];
+#pragma unroll
+      for (int d = 1; d < 32; d <<= 1) {
+        const unsigned long long b = __shfl_up_sync(FULL, we, d);
+        if ((int)lane >= d) we += b;
+      }
+      s_e[lane] = we;
+    }
+    __syncthreads();
+    if (i < n_ctas) P.cta_events[i] = carry + (warp ? s_e[warp - 1] : 0ull) + ie - e;
+    carry += s_e[31];
+    __syncthreads();   // s_e is rewritten by the next chunk
+  }
+  if (threadIdx.x == 0) *P.total = carry;
+}
+
+cudaError_t launch_status(const StatusParams& P, uint32_t smem_bytes, cudaStream_t stream) {
+  if (P.n == 0) return cudaSuccess;
+  if (smem_bytes > 48u * 1024u) {
+    cudaError_t e = cudaFuncSetAttribute(status_runs<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes);
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(status_runs<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes);
+    if (e != cudaSuccess) return e;
+  }
+  const uint32_t grid = (P.n - 1u) / P.warps_per_block + 1u, threads = 32u * P.warps_per_block;
+  status_runs<false><<<grid, threads, smem_bytes, stream>>>(P);
+  status_scan<<<1, 1024, 0, stream>>>(P, grid);
+  status_runs<true><<<grid, threads, smem_bytes, stream>>>(P);
   return cudaGetLastError();
 }
 

@@ -1319,3 +1319,66 @@ int bf_resident_commit_timed(bf_ctx* c, uint32_t h, uint32_t n_runs, const bf_co
 int bf_resident_commit(bf_ctx* c, uint32_t h, uint32_t n_runs, const bf_commit_entry* entries, uint32_t n, bf_commit_out* out) {
   return bf_resident_commit_timed(c, h, n_runs, entries, n, out, nullptr);
 }
+
+// ---- run status (resident.cu) ---------------------------------------------------------------------------------------------------
+// Read-only: the count, scan and list launches over the listed runs, the D2H copy of the event total, one synchronisation.  Pinned
+// lists and outputs are used in place; staged records are copied with the total, staged events after the synchronisation, once
+// their number is known (a second, blocking copy).
+int bf_resident_status(bf_ctx* c, uint32_t h, uint32_t n_runs, const uint32_t* runs, uint32_t n, bf_status_out* out) {
+  auto [g, r] = lock_resident(c, h);
+  if (!out || out->struct_size != sizeof(bf_status_out)) return fail(c, BF_EINVAL, "null bf_status_out or bad struct_size");
+  if (!r) return BF_EINVAL;
+  const bf_layout& L = r->L;
+  if (n_runs > r->cap) return fail(c, BF_EINVAL, "n_runs exceeds the resident batch");
+  if (!runs && n != n_runs) return fail(c, BF_EINVAL, "runs == NULL lists every run of [0, n_runs): n must equal n_runs");
+  for (uint32_t i = 0; runs && i < n; ++i) {
+    if (runs[i] >= n_runs) return fail(c, BF_EINVAL, "runs[" + std::to_string(i) + "] is not below n_runs");
+    if (i && runs[i] <= runs[i - 1]) return fail(c, BF_EINVAL, "runs[" + std::to_string(i) + "] does not ascend");
+  }
+  if (n && !out->records) return fail(c, BF_EINVAL, "null records");
+  if (out->events_cap && !out->events) return fail(c, BF_EINVAL, "null events with a non-zero events_cap");
+  uint32_t wpb = 8, topo = 0, per_warp = 0;
+  if (L.off_child != BF_OFF_NONE) {   // a shared stage per warp for the parallel join
+    topo = bf::largest_record(c, L.words);
+    per_warp = L.state_stride + topo + 256u;
+    wpb = std::min<uint32_t>(8u, (227u * 1024u - bf::kStatusStaticSmem) / per_warp);
+    if (!wpb) return fail(c, BF_ENOMEM, "a topology record and a state record do not fit one warp's shared memory");
+  }
+  out->n_events = 0;
+  if (n == 0) return BF_OK;
+  BF_CUDA(c, cudaSetDevice(c->device));
+  cudaStream_t s = c->stream;
+  if (int rc = bf::sync_slots(c, s)) return rc;
+  const uint32_t grid = (n - 1u) / wpb + 1u;
+  // the list is at most n * steps_max long: a larger events_cap stages no more
+  const uint64_t cap = std::min<uint64_t>(out->events_cap, (uint64_t)n * L.steps_max);
+  bf::StatusParams P{};
+  P.runs = runs ? static_cast<const uint32_t*>(bf::pinned_dev(runs)) : nullptr;
+  P.records = static_cast<bf_status_rec*>(bf::pinned_dev(out->records));
+  P.events = cap ? static_cast<uint16_t*>(bf::pinned_dev(out->events)) : nullptr;
+  const bool staged_records = !P.records, staged_events = cap && !P.events;
+  CallStage st;
+  if (runs && !P.runs) st.up(P.runs, runs, n);
+  st.out(P.run_events, n);
+  st.out(P.cta_events, grid);
+  st.out(P.total, 1);
+  if (staged_records) st.out(P.records, n);
+  if (staged_events) st.out(P.events, cap);
+  if (int rc = st.send(c, "bf_resident_status")) return rc;
+  P.state = r->d_state; P.slots = c->slots_dev; P.n_slots = (uint32_t)c->slots_host.size();
+  P.runctl = r->areas_view().runctl;
+  P.n = n; P.warps_per_block = wpb;
+  P.words = L.words; P.state_stride = L.state_stride; P.off_phase = L.off_phase; P.off_decision = L.off_decision;
+  P.off_child = L.off_child; P.topo_bytes = topo;
+  P.events_cap = cap;
+  cudaError_t e = bf::launch_status(P, wpb * per_warp, s);
+  if (e == cudaSuccess) e = cudaMemcpyAsync(&c->pinned->status_events, P.total, 8, cudaMemcpyDeviceToHost, s);
+  if (e == cudaSuccess && staged_records) e = cudaMemcpyAsync(out->records, P.records, (size_t)n * sizeof(bf_status_rec), cudaMemcpyDeviceToHost, s);
+  if (int rc = bf::end_call(c, e, "bf_resident_status")) return rc;
+  c->stats.kernel_launches += 3;
+  const uint64_t total = c->pinned->status_events;
+  if (const uint64_t listed = std::min<uint64_t>(total, cap); listed && staged_events)
+    BF_CUDA(c, cudaMemcpy(out->events, P.events, (size_t)listed * 2, cudaMemcpyDeviceToHost));
+  out->n_events = total;
+  return BF_OK;
+}

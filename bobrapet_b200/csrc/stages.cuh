@@ -1,5 +1,6 @@
 // stages.cuh — the bit-plane stages of a frontier pass around the dependency walk, one definition for both kernels:
-// frontier_kernel.cu (one run per warp) and frontier_pack.cu (a group of R = 32 / Wq runs per warp).
+// frontier_kernel.cu (one run per warp) and frontier_pack.cu (a group of R = 32 / Wq runs per warp).  Stage H, the parallel
+// join, is also taken by the run-status kernel (resident.cu), which reports the phases a single pass would leave.
 //
 // A lane holds word w (32 steps) of one run: w = lane in the general kernel, lane = g * Wq + w in the packed-lanes kernel.
 // Per-run reductions run over `gmask`, the lanes of the caller's run (FULL in the general kernel).  No collective sits under
@@ -28,6 +29,116 @@ namespace bf {
 //     SAT ⊆ COMPLETED0 ∪ TERM ∪ RT_SAT and FD ⊆ TERM; mark_cs needs a compensation step, mark_ff fires only under
 //     condition (2), and only the topology-terminated branch sets other Failed codes.  The producer stages and the walk
 //     reads no rows of a word whose dependency floor lies above the highest such step (the floor cut, frontier_pack.cu).
+
+// ------------------------------------------------------------------ stage H: parallel join (dag.go:1131-1198)
+// A registered parallel step that is neither absent nor terminal joins when every child is terminal: Failed if a terminal child
+// neither succeeded / was skipped nor is an allowFailure branch, else Succeeded.  Child phases are nibbles, eight per word: one
+// lane classifies eight children with the bit-plane tables (SWAR), a sub-warp of SW lanes covers one descriptor, 32 / SW
+// descriptors per round, and the verdicts reach the lanes that own the parents' words through two scratch words per step word.
+// One run per warp, its records in shared memory: the state record at sr_a (children_registered at +8, the child area at
+// P.off_child), the topology record at tr_a (descs at off_par, allowFailure words at each desc's allow_off); scr_a holds 8 * Wt
+// scratch bytes; P holds the launch parameters (KParams, StatusParams), whose off_child is read where it is used.  Lane w holds
+// word w (act: w < Wt) and T_PAR its parallel steps.  Returns `marked`, set to true where a join rewrites a code.  `marked` goes in
+// and out by value and off_child is read from P at its uses, as in the inline code this replaced: with a reference or an
+// argument instead, ptxas allocates one frontier_kernel build differently (<CD, CH, XO> with RB = 2 spilled 8 bytes fewer).
+template <class Params>
+DI bool stage_h(const Params& P, uint32_t lane, bool act, uint32_t Wt, uint32_t nP, uint32_t T_PAR, uint32_t sr_a, uint32_t tr_a,
+                uint32_t off_par, uint32_t scr_a, bool marked, uint32_t& p0, uint32_t& p1, uint32_t& p2, uint32_t& p3) {
+  const uint32_t ACTIVE = T_PAR & (p0 | p1 | p2 | p3) & ~plut<BF_LUT_TERMINAL>(p0, p1, p2, p3);
+  if (__any_sync(FULL, ACTIVE != 0)) {
+    const uint32_t pd_a = tr_a + off_par, child_a = sr_a + P.off_child;
+    // which descriptors join at all: registered, with children, parent neither absent nor terminal (lane q <-> desc q,
+    // second round for descs 32..63), and the widest of them — usually none or a few of the run's descriptors
+    uint32_t take_lo = 0, take_hi = 0, mb = 0;
+    for (uint32_t q0 = 0; q0 < nP; q0 += 32) {
+      const uint32_t q = q0 + lane;
+      const uint32_t sb = q < nP ? lds_u32(pd_a + q * 16u) : 0u;   // step | branches << 16
+      const uint32_t actw = __shfl_sync(FULL, ACTIVE, ((sb & 0xFFFFu) >> 5) & 31u);
+      const uint32_t reg = lds_u32(sr_a + 8u + (q0 >> 3));          // children_registered, 32 descs per word
+      const bool tk = q < nP && (sb >> 16) != 0u && ((reg >> lane) & 1u) != 0u && ((actw >> (sb & 31u)) & 1u) != 0u;
+      const uint32_t m = __ballot_sync(FULL, tk);
+      if (q0 == 0) take_lo = m; else take_hi = m;
+      if (tk) mb = max(mb, sb >> 16);
+    }
+    mb = __reduce_max_sync(FULL, mb);
+    const uint32_t mw = (mb + 7u) >> 3;   // child words of the widest joining descriptor
+    if ((take_lo | take_hi) == 0u) {
+      // nothing to join in this pass
+    } else if (mw <= 32u) {
+      const uint32_t lgs = mw > 1u ? 32u - (uint32_t)__clz(mw - 1u) : 0u;   // sub-warp of SW = 2^lgs >= mw lanes per descriptor
+      const uint32_t SW = 1u << lgs, DPI = 32u >> lgs, sub = lane >> lgs, wi = lane & (SW - 1u);
+      const uint32_t gm = (SW == 32u ? FULL : ((1u << SW) - 1u)) << (sub << lgs);
+      const uint32_t dmask = DPI == 32u ? FULL : ((1u << DPI) - 1u);
+      const uint32_t tS = scr_a, tF = scr_a + 4u * Wt;
+      __syncwarp();
+      if (act) { sts_u32(tS + lane * 4u, 0u); sts_u32(tF + lane * 4u, 0u); }
+      __syncwarp();
+      for (uint32_t q0 = 0; q0 < nP; q0 += DPI) {
+        const uint32_t tw = q0 < 32u ? take_lo >> q0 : take_hi >> (q0 - 32u);   // DPI divides 32: a round never straddles the words
+        if ((tw & dmask) == 0u) continue;                                       // warp-uniform
+        const uint32_t q = q0 + sub;
+        const bool take = (tw >> sub) & 1u;
+        uint4 d = make_uint4(0u, 0u, 0u, 0u);
+        if (take) d = lds_v4(pd_a + q * 16u);          // step | branches << 16, child_first, allow_off, -
+        const uint32_t step = d.x & 0xFFFFu, br = d.x >> 16, wj = step >> 5, wb = step & 31u;
+        bool nd = false, fl = false;
+        if (take && wi * 8u < br) {
+          const uint32_t cw = lds_u32(child_a + (d.y >> 1) + wi * 4u);   // child_first is a multiple of 8 nibbles
+          const uint32_t vm = 0x11111111u & bmsk_clamp(0u, min(8u, br - wi * 8u) * 4u);
+          uint32_t x0 = cw & 0x11111111u, x1 = (cw >> 1) & 0x11111111u, x2 = (cw >> 2) & 0x11111111u, x3 = (cw >> 3) & 0x11111111u;
+          const uint32_t keep = ~(x0 & x1 & x2 & x3);                     // the reserved code 15 reads as 0
+          x0 &= keep; x1 &= keep; x2 &= keep; x3 &= keep;
+          const uint32_t done = plut<BF_LUT_TERMINAL>(x0, x1, x2, x3);
+          const uint32_t ab = (lds_u32(tr_a + d.z + (wi >> 2) * 4u) >> ((wi & 3u) * 8u)) & 0xFFu;   // allowFailure bits of my 8 branches
+          const uint32_t okc = plut<BF_LUT_COMPLETED0>(x0, x1, x2, x3) | spread4(ab);
+          nd = (vm & ~done) != 0u;
+          fl = (vm & done & ~okc) != 0u;
+        }
+        const uint32_t ndm = __ballot_sync(FULL, nd), flm = __ballot_sync(FULL, fl);
+        if (take && wi == 0u && (ndm & gm) == 0u) red_or_shared(((flm & gm) ? tF : tS) + wj * 4u, 1u << wb);
+      }
+      __syncwarp();
+      uint32_t sS = 0, sF = 0;
+      if (act) { sS = lds_u32(tS + lane * 4u); sF = lds_u32(tF + lane * 4u); }
+      if (__any_sync(FULL, (sS | sF) != 0u)) marked = true;
+      pset<BF_PHASE_SUCCEEDED>(sS, p0, p1, p2, p3);
+      pset<BF_PHASE_FAILED>(sF, p0, p1, p2, p3);
+      __syncwarp();
+    } else {   // more than 256 branches on one step: one descriptor at a time, one child per lane
+      const uint8_t* sr = gptr(sr_a);
+      const uint8_t* tr = gptr(tr_a);
+      const uint64_t registered = *reinterpret_cast<const uint64_t*>(sr + 8);
+      const ParDesc* pd = reinterpret_cast<const ParDesc*>(tr + off_par);
+      const uint8_t* child = sr + P.off_child;
+      for (uint32_t q = 0; q < nP; ++q) {
+        if (!((registered >> q) & 1ull)) continue;
+        const ParDesc d = pd[q];
+        if (d.branches == 0) continue;  // no children to wait for (dag.go:1140-1143)
+        const uint32_t wj = d.step >> 5, wb = d.step & 31u;
+        if (!((__shfl_sync(FULL, ACTIVE, wj) >> wb) & 1u)) continue;
+        const uint32_t* allow = reinterpret_cast<const uint32_t*>(tr + d.allow_off);
+        bool all_done = true, any_failed = false;
+        for (uint32_t b = lane; b < d.branches; b += 32) {
+          const uint32_t cph = get_nibble(child, d.child_first + b);
+          const bool done = cph != 0 && ((BF_LUT_TERMINAL >> cph) & 1u);
+          const bool okc = cph == BF_PHASE_SUCCEEDED || cph == BF_PHASE_SKIPPED || ((allow[b >> 5] >> (b & 31u)) & 1u);
+          all_done = all_done && done;
+          any_failed = any_failed || (done && !okc);
+        }
+        all_done = __all_sync(FULL, all_done);
+        any_failed = __any_sync(FULL, any_failed);
+        if (all_done) {
+          marked = true;
+          if (lane == wj) {  // the lane that owns word wj rewrites its planes
+            const uint32_t m = 1u << wb;
+            if (any_failed) pset<BF_PHASE_FAILED>(m, p0, p1, p2, p3); else pset<BF_PHASE_SUCCEEDED>(m, p0, p1, p2, p3);
+          }
+        }
+      }
+    }
+  }
+  return marked;
+}
 
 // ------------------------------------------------------------------ stage G: gate / sleep / wait sync
 // dag.go:1469-1533, 1235-1277, 1327-1437.  A RUNNING sync step (SYNC_T: sleep, wait, gate) takes the code its decision

@@ -65,6 +65,7 @@ class Frontier:
     def __init__(self, device: int = 0, arena_bytes: int = 0, _borrowed_ctx=None, reserve_sms: int = 0):
         self._lib = A.load()
         self._owned = _borrowed_ctx is None
+        self._steps_max: Dict[int, int] = {}   # steps_max of each resident batch's layout
         if _borrowed_ctx is not None:       # a shard's ctx owned by a FrontierGroup
             self._ctx = C.c_void_p(_borrowed_ctx)
             return
@@ -256,6 +257,7 @@ class Frontier:
         """bf_resident_reshape: grow the batch to layout L (from make_layout) and `capacity` runs in place, keeping every run's
         state, the current result records and the touch marks"""
         self._check(self._lib.bf_resident_reshape(self._ctx, handle, C.byref(L), capacity), "bf_resident_reshape")
+        self._steps_max[handle] = int(L.steps_max)
 
     def resident_retire(self, handle: int, n_runs: int, runs, capacity: int = 0):
         """bf_resident_retire: take `runs` (distinct indices below n_runs) out of the batch; the last live runs move into the
@@ -286,6 +288,7 @@ class Frontier:
             err = A.FrontierError(rc, "bf_resident_narrow: %s" % self._lib.bf_last_error(self._ctx).decode())
             err.extent = e.as_dict()
             raise err
+        self._steps_max[handle] = int(L.steps_max)
         return e.as_dict()
 
     def resident_transfer(self, src: int, dst: int, src_n: int, dst_n: int, runs) -> dict:
@@ -398,6 +401,29 @@ class Frontier:
             got.update(n_armed=int(arm.n_armed), next_deadline=int(arm.next_deadline))
         return got
 
+    # -- run status of resident batches (bf_resident_status)
+    STATUS_DTYPE = np.dtype([("run", "<u4"), ("first_event", "<u4"), ("n_events", "<u2"), ("first_failed", "<u2"),
+                             ("summary", "<u2"), ("group", "u1"), ("outcome", "u1"), ("story_phase", "u1"),
+                             ("reserved", "u1", (7,)), ("active", "<u2"), ("completed", "<u2"), ("failed", "<u2"),
+                             ("skipped", "<u2")])   # bf_status_rec, 32 B
+
+    def resident_status(self, handle: int, n_runs: int, runs=None, events_cap: Optional[int] = None):
+        """bf_resident_status: the status of the listed runs (runs: strictly ascending, below n_runs; None: every run of
+        [0, n_runs)) after the stage G / H / I rewrites of a single pass, without changing anything.  events_cap: events to
+        fetch (default: every one the runs can have, steps_max of the batch's layout per run).  -> (records STATUS_DTYPE[len(runs)], events u16[min(n_events, events_cap)],
+        n_events)"""
+        rl = None if runs is None else np.ascontiguousarray(runs, dtype=np.uint32)
+        n = int(n_runs) if rl is None else rl.shape[0]
+        recs = np.zeros(n, dtype=self.STATUS_DTYPE)
+        if events_cap is None:
+            events_cap = n * self._steps_max[handle]
+        events = np.zeros(max(int(events_cap), 1), dtype=np.uint16)
+        out = A.StatusOut(struct_size=C.sizeof(A.StatusOut), records=recs.ctypes.data if n else None,
+                          events=events.ctypes.data if events_cap else None, events_cap=int(events_cap))
+        self._check(self._lib.bf_resident_status(self._ctx, handle, int(n_runs), None if rl is None else rl.ctypes.data, n,
+                                                 C.byref(out)), "bf_resident_status")
+        return recs, events[:min(int(out.n_events), int(events_cap))].copy(), int(out.n_events)
+
     # -- limiter inputs and schedules of resident batches (bf_resident_sched*, bf_resident_schedule)
     SCHED_PUT_DTYPE = np.dtype([("run", "<u4"), ("story_key", "<u4"), ("queue_key", "<u4"), ("priority", "<i4"),
                                 ("queued_since", "<u4"), ("run_phase", "<u4"), ("reserved", "<u4", (2,))])   # bf_sched_put, 32 B
@@ -472,6 +498,7 @@ class Frontier:
     def resident_create(self, L: A.Layout, capacity: int) -> int:
         h = C.c_uint32()
         self._check(self._lib.bf_resident_create(self._ctx, C.byref(L), capacity, C.byref(h)), "bf_resident_create")
+        self._steps_max[h.value] = int(L.steps_max)   # sizes resident_status's default event buffer
         return h.value
 
     def resident_destroy(self, handle: int):

@@ -644,6 +644,66 @@ func (r *Resident) CommitTimed(n, now uint32, entries []CommitEntry) (res Commit
 	return res, uint32(k[7]), uint32(k[8]), r.c.err(rc)
 }
 
+// Outcomes of a StatusRecord (BF_OUTCOME_*) and the kinds of its events (BF_STATUS_EVT_*).
+const (
+	OutcomeNone               = 0 // the run's group is not done
+	OutcomeSucceeded          = 1 // no group failed: evaluate the Story's output template (finalizeSuccessfulRun) before Succeeded
+	OutcomeDependencyFailed   = 2 // Failed, reason DependencyFailed
+	OutcomeCompensated        = 3 // Compensated, reason Compensated
+	OutcomeCompensationFailed = 4 // Failed, reason CompensationFailed
+	OutcomeCleanupFailed      = 5 // Failed, reason CleanupFailed
+	OutcomeTimedOut           = 6 // stopped at its story deadline: Timeout
+	OutcomeCanceled           = 7 // stopped by a cancel: Finished once the drain ends
+	OutcomeStopped            = 8 // stopped by the host
+	OutcomeDead               = 9 // the run's topology slot is dead or wider than the layout
+	StatusEvtFailed           = 1 // a step of the deciding failed set (status.error's failedSteps)
+	StatusEvtAllowed          = 2 // an allowed failure (status.allowedFailures)
+	StatusNoStep              = 0xFFFF
+)
+
+// StatusRecord is one run's report of Status (bf_status_rec, 32 bytes, no pointers).  Its events are
+// events[FirstEvent : FirstEvent+NEvents]; Active / Completed / Failed / Skipped are the step counters of the status.
+type StatusRecord struct {
+	Run, FirstEvent                    uint32
+	NEvents, FirstFailed, Summary      uint16
+	Group, Outcome, StoryPhase         uint8
+	_                                  [7]uint8
+	Active, Completed, Failed, Skipped uint16
+}
+
+// StatusEvent splits an event of Status: step | phase << 10 | kind << 14.
+func StatusEvent(e uint16) (step uint16, phase, kind uint8) {
+	return e & 0x3FF, uint8(e>>10) & 0xF, uint8(e >> 14)
+}
+
+// Status reports the listed runs' status after the gate, sleep, wait and join syncs and the fail-fast and compensation marking
+// a single tick would apply now (bf_resident_status), changing nothing on the device.  runs must ascend strictly below n; nil
+// lists every run of [0, n).  statuses receives one record per listed run; events the first len(events) of nEvents events.
+func (r *Resident) Status(n uint32, runs []uint32, statuses []StatusRecord, events []uint16) (nEvents uint64, err error) {
+	count := int(n)
+	var rp *C.uint32_t
+	if runs != nil {
+		count = len(runs)
+		if count > 0 {
+			rp = (*C.uint32_t)(unsafe.Pointer(&runs[0]))
+		}
+	}
+	if len(statuses) < count {
+		return 0, fmt.Errorf("frontier: statuses holds %d records for %d runs", len(statuses), count)
+	}
+	var sp *C.bf_status_rec
+	if count > 0 {
+		sp = (*C.bf_status_rec)(unsafe.Pointer(&statuses[0]))
+	}
+	var ep *C.uint16_t
+	if len(events) > 0 {
+		ep = (*C.uint16_t)(unsafe.Pointer(&events[0]))
+	}
+	var ne C.uint64_t
+	rc := C.bfgo_resident_status(r.c.p, r.handle, C.uint32_t(n), rp, C.uint32_t(count), sp, ep, C.uint64_t(len(events)), &ne)
+	return uint64(ne), r.c.err(rc)
+}
+
 // SchedPut is one limiter-input request of PutSched (bf_sched_put, 32 bytes, no pointers).  QueuedSince is the StartedAt of the
 // run's earliest queued step on the clock of ScheduleResident's now (SchedNone: nothing queued); the device ages from it.
 type SchedPut struct {

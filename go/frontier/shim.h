@@ -239,6 +239,19 @@ static inline int bfgo_resident_commit_timed(bf_ctx* c, uint32_t handle, uint32_
   return rc;
 }
 
+/* Run status.  The records (bf_status_rec holds no pointers) and events land in the caller's buffers; *n_events = the events of
+ * the listed runs, of which the first events_cap were written.  runs == NULL with n == n_runs lists every run of [0, n_runs). */
+static inline int bfgo_resident_status(bf_ctx* c, uint32_t handle, uint32_t n_runs, const uint32_t* runs, uint32_t n,
+                                       bf_status_rec* records, uint16_t* events, uint64_t events_cap, uint64_t* n_events) {
+  bf_status_out o;
+  memset(&o, 0, sizeof o);
+  o.struct_size = (uint32_t)sizeof o;
+  o.records = records; o.events = events; o.events_cap = events_cap;
+  const int rc = bf_resident_status(c, handle, n_runs, runs, n, &o);
+  *n_events = o.n_events;
+  return rc;
+}
+
 /* Step timings of a topology slot (bf_step_timing holds no pointers): passed as they are. */
 static inline int bfgo_topology_timings(bf_ctx* c, uint32_t slot, const bf_step_timing* t, uint32_t n) {
   return bf_topology_timings(c, slot, t, n);

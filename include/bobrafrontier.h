@@ -1144,6 +1144,82 @@ typedef struct bf_commit_arm {
 int bf_resident_commit_timed(bf_ctx* ctx, uint32_t handle, uint32_t n_runs, const bf_commit_entry* entries, uint32_t n_entries,
                              bf_commit_out* out, bf_commit_arm* arm);
 
+/* ------------------------------------------------------------------ run status (what a batcher persists of a run's status)
+ * When group selection finds nothing left to run (BF_GROUP_DONE, dag.go:482-495) the reference finalizes the StoryRun
+ * (finalizeStoryRun, dag.go:693-754): the failed set of the finally, compensation or main group, in that order, decides its phase
+ * and condition reason, the message names the set's first failed step, and status.error lists every step of the set with its
+ * phase (BuildStoryRunError, pkg/runs/status/storyrun.go:165).  On every persist it also writes status.allowedFailures
+ * (syncAllowedFailures, dag.go:478, :3393-3430) and the step counters (updateStepProgress / summarizeStepProgress, :904-942).  All
+ * of these read the phases after the pass's rewrites, which only the device holds.  bf_resident_status reports them for the
+ * listed runs of a resident batch.
+ *
+ * The phases are those of the run's state record after stages G (gate / sleep / wait decisions), H (parallel join) and I
+ * (fail-fast and compensation-skip marking, topology-terminated fails): the stages, with the parameters, a single-pass tick
+ * applies to the record now.  Stage D's cond-FAIL writes are not among them (they reach the record through a commit).
+ *
+ * runs[n]: strictly ascending, each below n_runs; runs == NULL with n == n_runs lists every run of [0, n_runs).  One record per
+ * listed run, in list order:
+ *   group      the BF_GROUP_* of that pass (the host's group for host-group runs, BF_GROUP_DONE for a stopped run)
+ *   summary    its BF_SUM_* group, done and failed bits (no BF_SUM_PHASE_CHANGED, no iteration count; 0 besides the group for a
+ *              host-group run)
+ *   outcome    BF_OUTCOME_NONE when the group is not BF_GROUP_DONE; else from the failed sets (failed: terminal and not completed
+ *              under allowFailure, as buildStateMaps): finally's -> CLEANUP_FAILED, else compensation's -> COMPENSATION_FAILED, else
+ *              main's -> COMPENSATED when the topology has compensation steps, else DEPENDENCY_FAILED; none -> SUCCEEDED.  A run
+ *              stopped in the batch's run control (bf_resident_runctl) takes TIMED_OUT, CANCELED or STOPPED from its stop reason
+ *              and lists no failed set.  A dead topology slot, or one wider than the layout: DEAD, group and summary 0, counts 0,
+ *              no events.
+ *   story_phase  the BF_PHASE_* the reference writes for the outcome: SUCCEEDED -> Succeeded (provisional: the host still
+ *              evaluates the Story's output template, finalizeSuccessfulRun, dag.go:2871, which can block or fail), the three
+ *              failures -> Failed, COMPENSATED -> Compensated, TIMED_OUT -> Timeout (dag.go:566-571), CANCELED -> Finished
+ *              (storyrun_controller.go:1557; the host sets it once its drain ends), otherwise 0
+ *   first_failed  the lowest step of the listed failed set, or BF_STATUS_NO_STEP
+ *   active / completed / failed / skipped   steps whose code is Running or Paused / Succeeded / Failed / Skipped (code 14 and
+ *              code 0 count in none, as summarizeStepProgress)
+ *   n_events, first_event   the run's events are events[first_event .. first_event + n_events) of the call's list
+ * events: one u16 per listed step, step | phase << 10 | kind << 14, run-major and step-ascending:
+ *   BF_STATUS_EVT_FAILED    a step of the listed failed set (the failedSteps of status.error)
+ *   BF_STATUS_EVT_ALLOWED   a terminal step with allowFailure that is neither Succeeded nor Skipped (collectAllowedFailures),
+ *                           in every run that is not dead, finished or not
+ * n_events is the true count; only the first events_cap events are written (as bf_compact_out).
+ * Read-only: no record, result, side area, touch mark or tick state changes, so the call may sit anywhere in the per-tick loop.
+ * Refused before any launch with BF_EINVAL and nothing written: struct_size, the handle, n_runs > capacity, runs not strictly
+ * ascending or not below n_runs, runs == NULL with n != n_runs, records == NULL with n > 0, events == NULL with events_cap > 0.
+ * Pinned buffers (runs, records, events) are used in place; others go through the call's staging.  One synchronisation, and with
+ * events not in pinned memory a second one: their copy follows the synchronisation that brings back their number.            */
+enum {
+  BF_OUTCOME_NONE = 0, BF_OUTCOME_SUCCEEDED = 1, BF_OUTCOME_DEPENDENCY_FAILED = 2, BF_OUTCOME_COMPENSATED = 3,
+  BF_OUTCOME_COMPENSATION_FAILED = 4, BF_OUTCOME_CLEANUP_FAILED = 5, BF_OUTCOME_TIMED_OUT = 6, BF_OUTCOME_CANCELED = 7,
+  BF_OUTCOME_STOPPED = 8, BF_OUTCOME_DEAD = 9
+};
+#define BF_STATUS_EVT_FAILED 0x1u
+#define BF_STATUS_EVT_ALLOWED 0x2u
+#define BF_STATUS_EVENT_STEP(e) ((uint32_t)(e) & 0x3FFu)
+#define BF_STATUS_EVENT_PHASE(e) (((uint32_t)(e) >> 10) & 0xFu)
+#define BF_STATUS_EVENT_KIND(e) ((uint32_t)(e) >> 14)
+#define BF_STATUS_NO_STEP 0xFFFFu
+typedef struct bf_status_rec {   /* 32 B                                                                                         */
+  uint32_t run;
+  uint32_t first_event;
+  uint16_t n_events;
+  uint16_t first_failed;         /* BF_STATUS_NO_STEP: none                                                                    */
+  uint16_t summary;
+  uint8_t group;
+  uint8_t outcome;               /* BF_OUTCOME_*                                                                               */
+  uint8_t story_phase;           /* BF_PHASE_*                                                                                 */
+  uint8_t reserved[7];
+  uint16_t active, completed, failed, skipped;
+} bf_status_rec;
+typedef struct bf_status_out {
+  uint32_t struct_size;          /* sizeof(bf_status_out)                                                                      */
+  uint32_t reserved;
+  bf_status_rec* records;        /* [n] out                                                                                    */
+  uint16_t* events;              /* [events_cap] out                                                                           */
+  uint64_t events_cap;
+  uint64_t n_events;             /* out: events of the listed runs; when > events_cap only the first events_cap were written  */
+} bf_status_out;
+
+int bf_resident_status(bf_ctx* ctx, uint32_t handle, uint32_t n_runs, const uint32_t* runs, uint32_t n, bf_status_out* out);
+
 /* ------------------------------------------------------------------ device groups (SURVEY.md row e)
  * The reference is ONE operator process (cmd/main.go:220, StoryRunReconciler storyrun_controller.go:216), so the
  * multi-GPU path must be reachable from one process through this ABI: a group owns one ctx per device and an NCCL
