@@ -213,6 +213,23 @@ class StatusOut(C.Structure):
                 ("events_cap", C.c_uint64), ("n_events", C.c_uint64)]
 
 
+RESYNC_CHECK = 0x1          # BF_RESYNC_CHECK: compare and list only
+RESYNC_ALL_FIELDS = 0x3F    # BF_RESYNC_FIELD(BF_DELTA_PHASE) | ... | BF_RESYNC_FIELD(BF_DELTA_REGISTERED)
+RESYNC_NONE = 0xFFFFFFFF    # BF_RESYNC_NONE: bf_resync.bad_run of a refusal that names no run
+
+
+def resync_field(f: int) -> int:
+    """BF_RESYNC_FIELD(f) for a BF_DELTA_* field"""
+    return 1 << f
+
+
+class Resync(C.Structure):
+    _fields_ = [("struct_size", C.c_uint32), ("n_runs", C.c_uint32), ("runs", C.c_void_p), ("n", C.c_uint32),
+                ("fields", C.c_uint32), ("records", C.c_void_p), ("flags", C.c_uint32), ("drifted_cap", C.c_uint32),
+                ("drifted", C.c_void_p), ("n_drifted", C.c_uint32), ("n_written", C.c_uint32), ("items", C.c_void_p),
+                ("items_cap", C.c_uint64), ("n_items", C.c_uint64), ("bad_run", C.c_uint32), ("reserved", C.c_uint32)]
+
+
 def sched_stride(words: int) -> int:
     return (16 + 12 * words + 15) & ~15
 
@@ -270,6 +287,7 @@ SYMBOLS = [
     ("bf_resident_commit_timed", C.c_int, [C.c_void_p, C.c_uint32, C.c_uint32, C.c_void_p, C.c_uint32, C.POINTER(CommitOut),
                                            C.POINTER(CommitArm)]),
     ("bf_resident_status", C.c_int, [C.c_void_p, C.c_uint32, C.c_uint32, C.c_void_p, C.c_uint32, C.POINTER(StatusOut)]),
+    ("bf_resident_resync", C.c_int, [C.c_void_p, C.c_uint32, C.POINTER(Resync)]),
     ("bf_group_create", C.c_int, [C.POINTER(C.c_void_p), C.POINTER(C.c_int32), C.c_uint32, C.POINTER(Config)]),
     ("bf_group_destroy", None, [C.c_void_p]),
     ("bf_group_size", C.c_uint32, [C.c_void_p]),

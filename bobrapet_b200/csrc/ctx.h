@@ -49,6 +49,7 @@ cudaError_t launch_runctl_put(const RunCtlPutParams& P, cudaStream_t stream);
 cudaError_t launch_runctl_restop(const RunCtlRestopParams& P, cudaStream_t stream);
 cudaError_t launch_commit(const CommitParams& P, bool apply, cudaStream_t stream);
 cudaError_t launch_status(const StatusParams& P, uint32_t smem_bytes, cudaStream_t stream);
+cudaError_t launch_resync(const ResyncParams& P, uint32_t smem_bytes, cudaStream_t stream);
 cudaError_t launch_closure(const Slot* slots, const uint32_t* slot_ids, const uint32_t* starts, uint32_t n, uint32_t n_slots,
                            uint32_t words_out, uint32_t* masks, cudaStream_t stream);
 cudaError_t launch_validate(const Slot* slots, const uint32_t* slot_ids, uint32_t n, uint32_t n_slots, uint32_t* status,
@@ -186,6 +187,7 @@ struct bf_ctx {
     uint32_t fire[4];      // bf_resident_fire: n_fired, n_written, n_pruned, next_deadline
     uint32_t commit[8];    // bf_resident_commit: the offender key (two words), then the five counts
     unsigned long long status_events;   // bf_resident_status: the events of the call
+    unsigned long long resync[2];       // bf_resident_resync: the items and the drifted runs of the call
     bf_counts counts() const { return {tail.counts[0], tail.counts[1], tail.counts[2], tail.counts[3]}; }
   }* pinned = nullptr;
   DevBuf<bf_expansion> d_exp;
@@ -207,7 +209,7 @@ struct bf_ctx {
   DevBuf<unsigned long long> d_tsums;
   uint64_t last_touched_events = 0;   // events of the previous touched tick (sizes the first D2H)
   // The device inputs and outputs of one resident call that is not a tick (migrate, redrive, retire, extent, narrow, transfer,
-  // timers_arm, fire, sched_put, schedule, runctl_put, commit), laid out by the call (CallStage, resident_abi.cu).  They are
+  // timers_arm, fire, sched_put, schedule, runctl_put, commit, status, resync), laid out by the call (CallStage, resident_abi.cu).  They are
   // valid from the call's staging until it returns: a call reads only bytes it uploaded, set or had a kernel write during the
   // same call, so every counter or sentinel word it reads is written by that call.  ensure only grows it, so the largest call
   // sizes it and a steady-state call allocates nothing.

@@ -494,7 +494,7 @@ struct CommitParams {
 };
 
 // bf_resident_status (resident.cu): one warp per listed run.  status_count stores each listed run's event count and each CTA's
-// total, status_scan turns the CTA totals into the events of the CTAs before each and posts the sum, status_list writes the
+// total, cta_scan turns the CTA totals into the events of the CTAs before each and posts the sum, status_list writes the
 // records and the events.  With a child area each warp has a shared stage for stage H: the state record, the topology record
 // (topo_bytes: the largest record the layout fits) and 256 scratch bytes.
 static_assert(sizeof(bf_status_rec) == 32, "bf_status_rec must be 32 bytes");
@@ -508,11 +508,39 @@ struct StatusParams {
   uint32_t n, warps_per_block;
   uint32_t words, state_stride, off_phase, off_decision, off_child, topo_bytes;
   uint32_t* run_events;             // [n] events of each listed run (status_count)
-  unsigned long long* cta_events;   // [CTAs] events of each CTA, then (status_scan) of the CTAs before it
-  unsigned long long* total;        // [1] events of the call (status_scan)
+  unsigned long long* cta_events;   // [CTAs] events of each CTA, then (cta_scan) of the CTAs before it
+  unsigned long long* total;        // [1] events of the call (cta_scan)
   bf_status_rec* records;           // [n]
   uint16_t* events;                 // [events_cap]
   unsigned long long events_cap;
+};
+
+// bf_resident_resync (resident.cu): one warp per listed run, the shared stage of StatusParams.  resync_runs<false> stores each
+// listed run's item count and each CTA's items and drifted runs (cta: [2][CTAs]), cta_scan turns them into the items and drifted
+// runs of the CTAs before each and posts the sums (total[2]), resync_runs<true> visits the runs with items: their items, their
+// drifted entries and, unless check, their repair.
+static_assert(sizeof(bf_drift) == 16, "bf_drift must be 16 bytes");
+struct ResyncParams {
+  uint8_t* state;
+  const Slot* slots;
+  uint32_t n_slots;
+  bf_run_ctl* runctl;               // or nullptr: no run is stopped
+  RunAreasView areas;               // a slot-drifted run's schedule baseline is dropped
+  uint32_t* mark;
+  uint32_t mark_touched, mark_must_list;
+  const uint32_t* runs;             // [n] ascending, or nullptr: listed run i is run i
+  const uint8_t* records;           // [n] the caller's records, list order
+  uint32_t n, warps_per_block;
+  uint32_t words, state_stride, off_phase, off_cond, off_decision, off_child, child_nibbles, topo_bytes;
+  uint32_t fields;                  // BF_RESYNC_FIELD bits of the fields the layout places
+  bool check;
+  uint32_t* run_items;              // [n] items of each listed run
+  unsigned long long* cta;          // [2][CTAs] items and drifted runs of each CTA, then (cta_scan) of the CTAs before it
+  unsigned long long* total;        // [2] items and drifted runs of the call
+  uint32_t* drifted;                // [drifted_cap]
+  uint32_t drifted_cap;
+  bf_drift* items;                  // [items_cap]
+  unsigned long long items_cap;
 };
 
 // bf_resident_sched_put: req[i] is written into area[req[i].run]

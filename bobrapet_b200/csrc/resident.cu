@@ -1146,10 +1146,76 @@ cudaError_t launch_commit(const CommitParams& P, bool apply, cudaStream_t stream
   return cudaGetLastError();
 }
 
+// ---- a single pass's stages over one state record (bf_resident_status, bf_resident_resync) ------------------------------------
+// One warp per run; lane w holds word w of its codes (words <= 32).  The topology planes of lane word w that stages G, H and I read.
+struct PassTopo {
+  uint32_t VALID, AF, TS, G1, G2, SYNC_T, T_PAR;
+};
+DI PassTopo pass_topo(const uint8_t* topo, const TopoHeader& th, uint32_t lane, bool act) {
+  uint32_t t0 = 0, t1 = 0, t2 = 0;
+  PassTopo T{};
+  if (act) {
+    const uint32_t Wt = th.W;
+    const uint32_t* pl = reinterpret_cast<const uint32_t*>(topo + th.off_planes) + lane;
+    t0 = pl[PL_T0 * Wt]; t1 = pl[PL_T1 * Wt]; t2 = pl[PL_T2 * Wt];
+    T.AF = pl[PL_AF * Wt]; T.TS = pl[PL_TS * Wt]; T.G1 = pl[PL_G1 * Wt]; T.G2 = pl[PL_G2 * Wt];
+    T.VALID = bmsk_clamp(0u, th.S - lane * 32u);
+  }
+  T.SYNC_T = t0 & (t1 | t2);
+  T.T_PAR = ~t0 & t1 & ~t2 & T.VALID;
+  return T;
+}
+// Word `lane` of the 4 phase planes (p) or the 2 planes (p0, p1) of a code at `off` of a record, masked to `valid`; a phase code
+// 15 reads as 0.
+DI void load_phases(const uint8_t* rec, uint32_t off, uint32_t words, uint32_t lane, uint32_t valid, uint32_t& p0, uint32_t& p1,
+                    uint32_t& p2, uint32_t& p3) {
+  const uint32_t* ph = reinterpret_cast<const uint32_t*>(rec + off) + lane;
+  p0 = ph[0]; p1 = ph[words]; p2 = ph[2u * words]; p3 = ph[3u * words];
+  const uint32_t keep = valid & ~(p0 & p1 & p2 & p3);
+  p0 &= keep; p1 &= keep; p2 &= keep; p3 &= keep;
+}
+DI void load_codes2(const uint8_t* rec, uint32_t off, uint32_t words, uint32_t lane, uint32_t valid, uint32_t& c0, uint32_t& c1) {
+  const uint32_t* cw = reinterpret_cast<const uint32_t*>(rec + off) + lane;
+  c0 = cw[0] & valid; c1 = cw[words] & valid;
+}
+
+// Stages H, G and I of a single pass over the codes p (decisions d0, d1) of a run with flags byte rflags, as bf_resident_status
+// applies them.  Stage H runs only when a registered parallel step is live: the warp first copies the state record `rec` and the
+// topology record into its shared stage at stage_a (P.topo_bytes for the topology record, 256 scratch bytes behind it); with
+// `over`, the children_registered bits (sel & 1) and the child area (sel & 2) are taken from that record instead.
+template <class Params>
+DI RunClass single_pass(const Params& P, uint32_t lane, bool act, const TopoHeader& th, const uint8_t* topo, const PassTopo& T,
+                        uint32_t rflags, const uint8_t* rec, const uint8_t* over, uint32_t sel, uint32_t stage_a, uint32_t d0,
+                        uint32_t d1, uint32_t& p0, uint32_t& p1, uint32_t& p2, uint32_t& p3) {
+  if (P.off_child != BF_OFF_NONE && th.P != 0 &&
+      __any_sync(FULL, (T.T_PAR & (p0 | p1 | p2 | p3) & ~plut<BF_LUT_TERMINAL>(p0, p1, p2, p3)) != 0u)) {
+    const uint32_t sr_a = stage_a, tr_a = stage_a + P.state_stride;
+    __syncwarp();   // a stage H before this one may still read the stage
+    for (uint32_t x = lane; x < P.state_stride / 16u; x += 32u) {
+      const uint4 v = reinterpret_cast<const uint4*>(rec)[x];
+      sts_v4(sr_a + 16u * x, v.x, v.y, v.z, v.w);
+    }
+    for (uint32_t x = lane; x < th.rec_bytes / 16u; x += 32u) {
+      const uint4 v = reinterpret_cast<const uint4*>(topo)[x];
+      sts_v4(tr_a + 16u * x, v.x, v.y, v.z, v.w);
+    }
+    if (over) {
+      __syncwarp();
+      if ((sel & 1u) && lane < 2u) sts_u32(sr_a + 8u + 4u * lane, reinterpret_cast<const uint32_t*>(over + 8)[lane]);
+      for (uint32_t x = lane; (sel & 2u) && x < (P.state_stride - P.off_child) / 4u; x += 32u)
+        sts_u32(sr_a + P.off_child + 4u * x, reinterpret_cast<const uint32_t*>(over + P.off_child)[x]);
+    }
+    __syncwarp();
+    stage_h(P, lane, act, th.W, th.P, T.T_PAR, sr_a, tr_a, th.off_par, tr_a + P.topo_bytes, false, p0, p1, p2, p3);   // the codes, not whether they changed
+    __syncwarp();
+  }
+  if (P.off_decision != BF_OFF_NONE) stage_g(T.SYNC_T, T.TS, d0, d1, p0, p1, p2, p3);
+  return stage_bi<true>(FULL, rflags, th.n_main, th.n_comp, th.n_final, T.AF, T.VALID & ~T.G1 & ~T.G2, T.G1, T.G2, p0, p1, p2, p3);
+}
+
 // ---- run status (bf_resident_status) ------------------------------------------------------------------------------------------
-// One warp per listed run; lane w holds word w of its codes (words <= 32).  The codes of the state record (15 read as 0) take the
-// stages of a single pass: H (only when a registered parallel step is live, after the warp has copied both records into its
-// shared stage), G and I.  The counts, the failed set and the allowed failures are bit-plane tables over the result.
+// The codes of the state record take the stages of a single pass (single_pass).  The counts, the failed set and the allowed
+// failures are bit-plane tables over the result.
 struct RunStatus {
   bf_status_rec rec;   // every field but first_event (warp-uniform)
   uint32_t EV, FL;     // this lane's word of the listed steps, and of those the ones in the failed set
@@ -1166,49 +1232,20 @@ DI void run_status(const StatusParams& P, uint32_t i, uint32_t lane, uint32_t st
   s.rec.first_failed = BF_STATUS_NO_STEP;
   s.EV = s.FL = s.p0 = s.p1 = s.p2 = s.p3 = 0u;
   const TopoHeader th = topo ? *reinterpret_cast<const TopoHeader*>(topo) : TopoHeader{};
-  const uint32_t Wt = th.W, S = th.S;
-  if (Wt - 1u >= P.words) {   // dead slot, or wider than the layout
+  if (th.W - 1u >= P.words) {   // dead slot, or wider than the layout
     s.rec.outcome = BF_OUTCOME_DEAD;
     return;
   }
-  const bool act = lane < Wt;
+  const bool act = lane < th.W;
   const uint32_t rflags = rec[4];
-  uint32_t t0 = 0, t1 = 0, t2 = 0, AF = 0, TS = 0, G1 = 0, G2 = 0, VALID = 0, d0 = 0, d1 = 0;
-  uint32_t p0 = 0, p1 = 0, p2 = 0, p3 = 0;
+  const PassTopo T = pass_topo(topo, th, lane, act);
+  uint32_t p0 = 0, p1 = 0, p2 = 0, p3 = 0, d0 = 0, d1 = 0;
   if (act) {
-    const uint32_t* pl = reinterpret_cast<const uint32_t*>(topo + th.off_planes) + lane;
-    t0 = pl[PL_T0 * Wt]; t1 = pl[PL_T1 * Wt]; t2 = pl[PL_T2 * Wt];
-    AF = pl[PL_AF * Wt]; TS = pl[PL_TS * Wt]; G1 = pl[PL_G1 * Wt]; G2 = pl[PL_G2 * Wt];
-    VALID = bmsk_clamp(0u, S - lane * 32u);
-    const uint32_t* ph = reinterpret_cast<const uint32_t*>(rec + P.off_phase) + lane;
-    p0 = ph[0]; p1 = ph[P.words]; p2 = ph[2u * P.words]; p3 = ph[3u * P.words];
-    const uint32_t keep = VALID & ~(p0 & p1 & p2 & p3);
-    p0 &= keep; p1 &= keep; p2 &= keep; p3 &= keep;
-    if (P.off_decision != BF_OFF_NONE) {
-      const uint32_t* dw = reinterpret_cast<const uint32_t*>(rec + P.off_decision) + lane;
-      d0 = dw[0]; d1 = dw[P.words];
-    }
+    load_phases(rec, P.off_phase, P.words, lane, T.VALID, p0, p1, p2, p3);
+    if (P.off_decision != BF_OFF_NONE) load_codes2(rec, P.off_decision, P.words, lane, ~0u, d0, d1);
   }
-  const uint32_t GM = VALID & ~G1 & ~G2;
-  const uint32_t SYNC_T = t0 & (t1 | t2);
-  const uint32_t T_PAR = ~t0 & t1 & ~t2 & VALID;
-  if (P.off_child != BF_OFF_NONE && th.P != 0 &&
-      __any_sync(FULL, (T_PAR & (p0 | p1 | p2 | p3) & ~plut<BF_LUT_TERMINAL>(p0, p1, p2, p3)) != 0u)) {
-    const uint32_t sr_a = stage_a, tr_a = stage_a + P.state_stride;
-    for (uint32_t x = lane; x < P.state_stride / 16u; x += 32u) {
-      const uint4 v = reinterpret_cast<const uint4*>(rec)[x];
-      sts_v4(sr_a + 16u * x, v.x, v.y, v.z, v.w);
-    }
-    for (uint32_t x = lane; x < th.rec_bytes / 16u; x += 32u) {
-      const uint4 v = reinterpret_cast<const uint4*>(topo)[x];
-      sts_v4(tr_a + 16u * x, v.x, v.y, v.z, v.w);
-    }
-    __syncwarp();
-    stage_h(P, lane, act, Wt, th.P, T_PAR, sr_a, tr_a, th.off_par, tr_a + P.topo_bytes, false, p0, p1, p2, p3);   // the codes, not whether they changed
-    __syncwarp();
-  }
-  if (P.off_decision != BF_OFF_NONE) stage_g(SYNC_T, TS, d0, d1, p0, p1, p2, p3);
-  const RunClass rc = stage_bi<true>(FULL, rflags, th.n_main, th.n_comp, th.n_final, AF, GM, G1, G2, p0, p1, p2, p3);
+  const uint32_t AF = T.AF, G1 = T.G1, G2 = T.G2, GM = T.VALID & ~G1 & ~G2;
+  const RunClass rc = single_pass(P, lane, act, th, topo, T, rflags, rec, nullptr, 0u, stage_a, d0, d1, p0, p1, p2, p3);
 
   const uint32_t TERM = plut<BF_LUT_TERMINAL>(p0, p1, p2, p3) & ~plut<BF_LUT_COMPLETED0>(p0, p1, p2, p3);
   const uint32_t FAILED = TERM & ~AF, ALLOWED = TERM & AF;
@@ -1241,7 +1278,7 @@ DI void run_status(const StatusParams& P, uint32_t i, uint32_t lane, uint32_t st
   s.rec.failed = (uint16_t)(fk & 0xFFFFu); s.rec.skipped = (uint16_t)(fk >> 16);
 }
 
-// Count (kList = false): each listed run's events, and each CTA's total.  List (kList = true, after status_scan): the same runs
+// Count (kList = false): each listed run's events, and each CTA's total.  List (kList = true, after cta_scan): the same runs
 // again, each record with the offset of its first event (the CTAs before, then the warps before in its CTA) and its events, lane by
 // lane in step order.
 template <bool kList>
@@ -1294,37 +1331,43 @@ __global__ void __launch_bounds__(256, 1) status_runs(const StatusParams P) {
   }
 }
 
-// One CTA: the CTA totals become the events of the CTAs before each (exclusive scan in place); the sum goes to P.total.
-__global__ void __launch_bounds__(1024) status_scan(const StatusParams P, uint32_t n_ctas) {
+// One CTA: for each of K arrays of n_ctas per-CTA totals (array k at cta + k * n_ctas), the totals become the sums of the CTAs
+// before each (exclusive scan in place); array k's sum goes to total[k].  bf_resident_status scans its events (K = 1),
+// bf_resident_resync its items and drifted runs (K = 2).
+template <uint32_t K>
+__global__ void __launch_bounds__(1024) cta_scan(unsigned long long* cta, unsigned long long* total, uint32_t n_ctas) {
   __shared__ unsigned long long s_e[32];
   const uint32_t lane = threadIdx.x & 31u, warp = threadIdx.x >> 5;
-  unsigned long long carry = 0;
-  for (uint32_t base = 0; base < n_ctas; base += 1024u) {
-    const uint32_t i = base + threadIdx.x;
-    const unsigned long long e = i < n_ctas ? P.cta_events[i] : 0ull;
-    unsigned long long ie = e;
-#pragma unroll
-    for (int d = 1; d < 32; d <<= 1) {
-      const unsigned long long b = __shfl_up_sync(FULL, ie, d);
-      if ((int)lane >= d) ie += b;
-    }
-    if (lane == 31) s_e[warp] = ie;
-    __syncthreads();
-    if (warp == 0) {   // the warp totals' inclusive scan
-      unsigned long long we = s_e[lane];
+  for (uint32_t k = 0; k < K; ++k) {
+    unsigned long long* a = cta + (size_t)k * n_ctas;
+    unsigned long long carry = 0;
+    for (uint32_t base = 0; base < n_ctas; base += 1024u) {
+      const uint32_t i = base + threadIdx.x;
+      const unsigned long long e = i < n_ctas ? a[i] : 0ull;
+      unsigned long long ie = e;
 #pragma unroll
       for (int d = 1; d < 32; d <<= 1) {
-        const unsigned long long b = __shfl_up_sync(FULL, we, d);
-        if ((int)lane >= d) we += b;
+        const unsigned long long b = __shfl_up_sync(FULL, ie, d);
+        if ((int)lane >= d) ie += b;
       }
-      s_e[lane] = we;
+      if (lane == 31) s_e[warp] = ie;
+      __syncthreads();
+      if (warp == 0) {   // the warp totals' inclusive scan
+        unsigned long long we = s_e[lane];
+#pragma unroll
+        for (int d = 1; d < 32; d <<= 1) {
+          const unsigned long long b = __shfl_up_sync(FULL, we, d);
+          if ((int)lane >= d) we += b;
+        }
+        s_e[lane] = we;
+      }
+      __syncthreads();
+      if (i < n_ctas) a[i] = carry + (warp ? s_e[warp - 1] : 0ull) + ie - e;
+      carry += s_e[31];
+      __syncthreads();   // s_e is rewritten by the next chunk
     }
-    __syncthreads();
-    if (i < n_ctas) P.cta_events[i] = carry + (warp ? s_e[warp - 1] : 0ull) + ie - e;
-    carry += s_e[31];
-    __syncthreads();   // s_e is rewritten by the next chunk
+    if (threadIdx.x == 0) total[k] = carry;
   }
-  if (threadIdx.x == 0) *P.total = carry;
 }
 
 cudaError_t launch_status(const StatusParams& P, uint32_t smem_bytes, cudaStream_t stream) {
@@ -1336,8 +1379,282 @@ cudaError_t launch_status(const StatusParams& P, uint32_t smem_bytes, cudaStream
   }
   const uint32_t grid = (P.n - 1u) / P.warps_per_block + 1u, threads = 32u * P.warps_per_block;
   status_runs<false><<<grid, threads, smem_bytes, stream>>>(P);
-  status_scan<<<1, 1024, 0, stream>>>(P, grid);
+  cta_scan<1><<<1, 1024, 0, stream>>>(P.cta_events, P.total, grid);
   status_runs<true><<<grid, threads, smem_bytes, stream>>>(P);
+  return cudaGetLastError();
+}
+
+// ---- resyncs (bf_resident_resync) -------------------------------------------------------------------------------------------
+// One warp per listed run; lane w holds word w of its codes.  The device's record and the caller's record as the repair would leave
+// it (the device's codes in the fields not selected) both take single_pass on a live slot; each field is compared by XOR of its
+// plane words under the mask of the steps compared (the phases' 15 -> 0 is applied as they are loaded).
+constexpr uint32_t kSelPhase = 1u << BF_DELTA_PHASE, kSelCond = 1u << BF_DELTA_COND, kSelDecision = 1u << BF_DELTA_DECISION,
+                   kSelChild = 1u << BF_DELTA_CHILD, kSelFlags = 1u << BF_DELTA_RUN_FLAGS, kSelRegistered = 1u << BF_DELTA_REGISTERED;
+
+struct RunDrift {
+  uint32_t r, slot_dev, slot_rec;
+  const uint8_t *dev, *rec, *topo;
+  TopoHeader th;
+  bool live, stopped;
+  uint32_t PH, CO, DE;                        // this lane's word of the differing steps of each selected field
+  uint32_t a0, a1, a2, a3, b0, b1, b2, b3;    // device / record phases (after the stages on a live slot)
+  uint32_t c0, c1, k0, k1, d0, d1, e0, e1;    // device / record cond and decision codes
+  unsigned long long descs, reg;              // descs whose nibbles and bits are compared; the differing registered bits
+  uint32_t flags_dev, flags_rec;
+  uint32_t n;                                 // items of the run (warp-uniform)
+};
+
+// The nibbles (bit k: nibble 8x + k) of child word x that are compared and differ: every nibble of the layout on a dead slot, else
+// those of the descs in `descs`.  vd, vr: the device's and the caller's word, each nibble 15 read as 0.
+DI uint32_t child_diff(const ResyncParams& P, const RunDrift& d, uint32_t x, uint32_t& vd, uint32_t& vr) {
+  auto canon = [](uint32_t w) {
+    const uint32_t f = w & (w >> 1) & (w >> 2) & (w >> 3) & 0x11111111u;
+    return w & ~(f * 0xFu);
+  };
+  vd = canon(reinterpret_cast<const uint32_t*>(d.dev + P.off_child)[x]);
+  vr = canon(reinterpret_cast<const uint32_t*>(d.rec + P.off_child)[x]);
+  const uint32_t lo = 8u * x, hi = min(lo + 8u, P.child_nibbles);
+  uint32_t cm = 0;
+  if (!d.live) {
+    cm = hi > lo ? (1u << (hi - lo)) - 1u : 0u;
+  } else {
+    const ParDesc* pd = reinterpret_cast<const ParDesc*>(d.topo + d.th.off_par);
+    for (unsigned long long q = d.descs; q; q &= q - 1ull) {
+      const ParDesc dq = pd[__ffsll((long long)q) - 1];
+      const uint32_t a = max(dq.child_first, lo), b = min(dq.child_first + dq.branches, hi);
+      if (a < b) cm |= ((1u << (b - a)) - 1u) << (a - lo);
+    }
+  }
+  const uint32_t x4 = vd ^ vr;
+  return squeeze4((x4 | (x4 >> 1) | (x4 >> 2) | (x4 >> 3)) & 0x11111111u) & cm;
+}
+
+DI void run_drift(const ResyncParams& P, uint32_t i, uint32_t lane, uint32_t stage_a, RunDrift& d) {
+  d.r = P.runs ? P.runs[i] : i;
+  d.dev = P.state + (size_t)d.r * P.state_stride;
+  d.rec = P.records + (size_t)i * P.state_stride;
+  d.slot_dev = *reinterpret_cast<const uint32_t*>(d.dev);
+  d.slot_rec = *reinterpret_cast<const uint32_t*>(d.rec);
+  d.PH = d.CO = d.DE = 0u;
+  d.a0 = d.a1 = d.a2 = d.a3 = d.b0 = d.b1 = d.b2 = d.b3 = 0u;
+  d.c0 = d.c1 = d.k0 = d.k1 = d.d0 = d.d1 = d.e0 = d.e1 = 0u;
+  d.descs = d.reg = 0ull;
+  d.stopped = P.runctl && P.runctl[d.r].stop;
+  if (d.slot_dev != d.slot_rec) {   // codes of two topologies are not comparable
+    d.n = 1u;
+    return;
+  }
+  const uint32_t sel = P.fields;
+  d.topo = d.slot_dev < P.n_slots ? reinterpret_cast<const uint8_t*>(P.slots[d.slot_dev].addr) : nullptr;
+  d.th = d.topo ? *reinterpret_cast<const TopoHeader*>(d.topo) : TopoHeader{};
+  d.live = d.th.W - 1u < P.words;
+  d.flags_dev = d.stopped ? P.runctl[d.r].saved_flags : d.dev[4];
+  d.flags_rec = d.rec[4];
+  const bool act = lane < (d.live ? (uint32_t)d.th.W : P.words);
+  const PassTopo T = d.live ? pass_topo(d.topo, d.th, lane, act) : PassTopo{};
+  const uint32_t VAL = d.live ? T.VALID : (act ? ~0u : 0u);
+  const uint8_t* rp = (sel & kSelPhase) ? d.rec : d.dev;   // where the caller's side takes each code from
+  const uint8_t* rd = (sel & kSelDecision) ? d.rec : d.dev;
+  if (act) {
+    load_phases(d.dev, P.off_phase, P.words, lane, VAL, d.a0, d.a1, d.a2, d.a3);
+    load_phases(rp, P.off_phase, P.words, lane, VAL, d.b0, d.b1, d.b2, d.b3);
+    if (P.off_cond != BF_OFF_NONE) {
+      load_codes2(d.dev, P.off_cond, P.words, lane, VAL, d.c0, d.c1);
+      load_codes2(d.rec, P.off_cond, P.words, lane, VAL, d.k0, d.k1);
+    }
+    if (P.off_decision != BF_OFF_NONE) {
+      load_codes2(d.dev, P.off_decision, P.words, lane, VAL, d.d0, d.d1);
+      load_codes2(rd, P.off_decision, P.words, lane, VAL, d.e0, d.e1);
+    }
+  }
+  uint32_t NT = VAL;   // the steps whose input codes are compared
+  if (d.live) {
+    const uint32_t rflags_rec = d.stopped ? d.dev[4] : (sel & kSelFlags) ? d.flags_rec : d.dev[4];
+    single_pass(P, lane, act, d.th, d.topo, T, d.dev[4], d.dev, nullptr, 0u, stage_a, d.d0, d.d1, d.a0, d.a1, d.a2, d.a3);
+    single_pass(P, lane, act, d.th, d.topo, T, rflags_rec, d.dev, d.rec,
+                ((sel & kSelRegistered) ? 1u : 0u) | ((sel & kSelChild) ? 2u : 0u), stage_a, d.e0, d.e1, d.b0, d.b1, d.b2, d.b3);
+    NT &= ~(plut<BF_LUT_TERMINAL>(d.a0, d.a1, d.a2, d.a3) & plut<BF_LUT_TERMINAL>(d.b0, d.b1, d.b2, d.b3));
+    const ParDesc* pd = reinterpret_cast<const ParDesc*>(d.topo + d.th.off_par);
+    for (uint32_t q0 = 0; q0 < d.th.P; q0 += 32u) {   // desc q <-> lane q - q0
+      const uint32_t q = q0 + lane;
+      const uint32_t step = q < d.th.P ? pd[q].step : 0u;
+      const uint32_t ntw = __shfl_sync(FULL, NT, (step >> 5) & 31u);
+      const uint32_t m = __ballot_sync(FULL, q < d.th.P && ((ntw >> (step & 31u)) & 1u));
+      d.descs |= (unsigned long long)m << q0;
+    }
+  } else {
+    d.descs = ~0ull;
+  }
+  if (sel & kSelPhase) d.PH = VAL & ((d.a0 ^ d.b0) | (d.a1 ^ d.b1) | (d.a2 ^ d.b2) | (d.a3 ^ d.b3));
+  if (sel & kSelCond) d.CO = NT & ((d.c0 ^ d.k0) | (d.c1 ^ d.k1));
+  if (sel & kSelDecision) d.DE = NT & ((d.d0 ^ d.e0) | (d.d1 ^ d.e1));
+  if (sel & kSelRegistered)
+    d.reg = (*reinterpret_cast<const unsigned long long*>(d.dev + 8) ^ *reinterpret_cast<const unsigned long long*>(d.rec + 8)) & d.descs;
+  uint32_t n_child = 0;
+  if (sel & kSelChild) {
+    const uint32_t cw = (P.child_nibbles + 7u) / 8u;
+    for (uint32_t x = lane; x < cw; x += 32u) {
+      uint32_t vd, vr;
+      n_child += (uint32_t)__popc(child_diff(P, d, x, vd, vr));
+    }
+  }
+  d.n = redux_add((uint32_t)(__popc(d.PH) + __popc(d.CO) + __popc(d.DE)) + n_child) + (uint32_t)__popcll((long long)d.reg) +
+        ((sel & kSelFlags) && d.flags_dev != d.flags_rec ? 1u : 0u);
+}
+
+// Writes one item per set bit of this lane's `bits` (index lane * 32 + bit; values bit b of the planes a and b), lane by lane, from
+// item position pos -> the position after the warp's items.
+DI unsigned long long emit_words(const ResyncParams& P, uint32_t lane, uint32_t run, uint32_t field, uint32_t bits,
+                                 unsigned long long pos, uint32_t a0, uint32_t a1, uint32_t a2, uint32_t a3, uint32_t b0, uint32_t b1,
+                                 uint32_t b2, uint32_t b3) {
+  const uint32_t mine = (uint32_t)__popc(bits);
+  uint32_t incl = mine;
+  for (uint32_t s = 1; s < 32; s <<= 1) {
+    const uint32_t x = __shfl_up_sync(FULL, incl, s);
+    if (lane >= s) incl += x;
+  }
+  unsigned long long at = pos + incl - mine;
+  for (uint32_t x = bits; x && at < P.items_cap; x &= x - 1u, ++at) {
+    const uint32_t b = (uint32_t)__ffs(x) - 1u;
+    const uint32_t dv = ((a0 >> b) & 1u) | ((a1 >> b) & 1u) << 1 | ((a2 >> b) & 1u) << 2 | ((a3 >> b) & 1u) << 3;
+    const uint32_t rv = ((b0 >> b) & 1u) | ((b1 >> b) & 1u) << 1 | ((b2 >> b) & 1u) << 2 | ((b3 >> b) & 1u) << 3;
+    reinterpret_cast<uint4*>(P.items)[at] = make_uint4(run, (lane * 32u + b) | field << 16, dv, rv);
+  }
+  return pos + __shfl_sync(FULL, incl, 31);
+}
+
+// Count (kList = false): each listed run's items, and each CTA's items and drifted runs.  List (kList = true, after cta_scan): the
+// runs with items again, their items from the offset of the CTAs before and the warps before in the CTA, their drifted entries and,
+// unless the call only checks, their repair.
+template <bool kList>
+__global__ void __launch_bounds__(256, 1) resync_runs(const ResyncParams P) {
+  extern __shared__ __align__(16) uint8_t resync_stage[];
+  __shared__ uint32_t warp_items[kStatusStaticSmem / 4];
+  const uint32_t warp = threadIdx.x >> 5, lane = threadIdx.x & 31u;
+  const uint32_t i = blockIdx.x * P.warps_per_block + warp;
+  const uint32_t stage_a = smem_u32(resync_stage) + warp * (P.off_child != BF_OFF_NONE ? P.state_stride + P.topo_bytes + 256u : 0u);
+  RunDrift d;
+  if (!kList) {
+    uint32_t ni = 0;
+    if (i < P.n) {
+      run_drift(P, i, lane, stage_a, d);
+      ni = d.n;
+      if (lane == 0) P.run_items[i] = ni;
+    }
+    if (lane == 0) warp_items[warp] = ni;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+      unsigned long long sum = 0, drifted = 0;
+      for (uint32_t w = 0; w < P.warps_per_block; ++w) { sum += warp_items[w]; drifted += warp_items[w] ? 1u : 0u; }
+      const uint32_t n_ctas = (P.n - 1u) / P.warps_per_block + 1u;
+      P.cta[blockIdx.x] = sum;
+      P.cta[n_ctas + blockIdx.x] = drifted;
+    }
+    return;
+  }
+  if (i >= P.n || P.run_items[i] == 0u) return;
+  run_drift(P, i, lane, stage_a, d);
+  const uint32_t first = blockIdx.x * P.warps_per_block, n_ctas = (P.n - 1u) / P.warps_per_block + 1u;
+  const uint32_t before = first + lane < i ? P.run_items[first + lane] : 0u;
+  unsigned long long pos = P.cta[blockIdx.x] + redux_add(before);
+  const unsigned long long at = P.cta[n_ctas + blockIdx.x] + redux_add(before ? 1u : 0u);
+  if (lane == 0 && at < P.drifted_cap) P.drifted[at] = d.r;
+  const uint32_t sel = P.fields;
+  const bool slot = d.slot_dev != d.slot_rec;
+  if (slot) {
+    if (lane == 0 && pos < P.items_cap)
+      reinterpret_cast<uint4*>(P.items)[pos] = make_uint4(d.r, (uint32_t)BF_DELTA_TOPO_SLOT << 16, d.slot_dev, d.slot_rec);
+  } else {
+    pos = emit_words(P, lane, d.r, BF_DELTA_PHASE, d.PH, pos, d.a0, d.a1, d.a2, d.a3, d.b0, d.b1, d.b2, d.b3);
+    pos = emit_words(P, lane, d.r, BF_DELTA_COND, d.CO, pos, d.c0, d.c1, 0u, 0u, d.k0, d.k1, 0u, 0u);
+    pos = emit_words(P, lane, d.r, BF_DELTA_DECISION, d.DE, pos, d.d0, d.d1, 0u, 0u, d.e0, d.e1, 0u, 0u);
+    if (sel & kSelChild) {
+      const uint32_t cw = (P.child_nibbles + 7u) / 8u;
+      for (uint32_t x0 = 0; x0 < cw; x0 += 32u) {   // warp-uniform: the shuffles below take every lane
+        const uint32_t x = x0 + lane;
+        uint32_t vd = 0, vr = 0;
+        const uint32_t m = x < cw ? child_diff(P, d, x, vd, vr) : 0u;
+        const uint32_t mine = (uint32_t)__popc(m);
+        uint32_t incl = mine;
+        for (uint32_t s = 1; s < 32; s <<= 1) {
+          const uint32_t y = __shfl_up_sync(FULL, incl, s);
+          if (lane >= s) incl += y;
+        }
+        unsigned long long a = pos + incl - mine;
+        for (uint32_t y = m; y && a < P.items_cap; y &= y - 1u, ++a) {
+          const uint32_t k = (uint32_t)__ffs(y) - 1u;
+          reinterpret_cast<uint4*>(P.items)[a] =
+              make_uint4(d.r, (8u * x + k) | (uint32_t)BF_DELTA_CHILD << 16, (vd >> (4u * k)) & 0xFu, (vr >> (4u * k)) & 0xFu);
+        }
+        pos += __shfl_sync(FULL, incl, 31);
+      }
+    }
+    if (lane == 0) {
+      if ((sel & kSelFlags) && d.flags_dev != d.flags_rec) {
+        if (pos < P.items_cap)
+          reinterpret_cast<uint4*>(P.items)[pos] = make_uint4(d.r, (uint32_t)BF_DELTA_RUN_FLAGS << 16, d.flags_dev, d.flags_rec);
+        ++pos;
+      }
+      const unsigned long long rd = *reinterpret_cast<const unsigned long long*>(d.dev + 8);
+      const unsigned long long rr = *reinterpret_cast<const unsigned long long*>(d.rec + 8);
+      for (unsigned long long y = d.reg; y && pos < P.items_cap; y &= y - 1ull, ++pos) {
+        const uint32_t q = (uint32_t)__ffsll((long long)y) - 1u;
+        reinterpret_cast<uint4*>(P.items)[pos] =
+            make_uint4(d.r, q | (uint32_t)BF_DELTA_REGISTERED << 16, (uint32_t)(rd >> q) & 1u, (uint32_t)(rr >> q) & 1u);
+      }
+    }
+  }
+  if (P.check) return;
+  __syncwarp();   // every read of the device's record above is done
+  uint8_t* dev = P.state + (size_t)d.r * P.state_stride;
+  if (slot) {   // the caller's whole record; a stopped run keeps its stop, the caller's flags byte becomes its saved byte
+    for (uint32_t x = lane; x < P.state_stride / 16u; x += 32u) {
+      uint4 v = reinterpret_cast<const uint4*>(d.rec)[x];
+      if (x == 0 && d.stopped) {
+        P.runctl[d.r].saved_flags = (uint8_t)v.y;
+        v.y = (v.y & ~0xFFu) | kStoppedFlags;
+      }
+      reinterpret_cast<uint4*>(dev)[x] = v;
+    }
+    if (lane == 0) {
+      atomicMax(P.mark + d.r, P.mark_must_list);
+      drop_baseline(P.areas, d.r);
+    }
+    return;
+  }
+  uint32_t* dw = reinterpret_cast<uint32_t*>(dev);
+  const uint32_t* rw = reinterpret_cast<const uint32_t*>(d.rec);
+  if (lane < P.words) {
+    if (sel & kSelPhase)
+      for (uint32_t b = 0; b < 4u; ++b) dw[P.off_phase / 4u + b * P.words + lane] = rw[P.off_phase / 4u + b * P.words + lane];
+    if (sel & kSelCond)
+      for (uint32_t b = 0; b < 2u; ++b) dw[P.off_cond / 4u + b * P.words + lane] = rw[P.off_cond / 4u + b * P.words + lane];
+    if (sel & kSelDecision)
+      for (uint32_t b = 0; b < 2u; ++b) dw[P.off_decision / 4u + b * P.words + lane] = rw[P.off_decision / 4u + b * P.words + lane];
+  }
+  if (sel & kSelChild)
+    for (uint32_t x = lane; x < (P.child_nibbles + 7u) / 8u; x += 32u) dw[P.off_child / 4u + x] = rw[P.off_child / 4u + x];
+  if (lane == 0) {
+    if (sel & kSelRegistered) { dw[2] = rw[2]; dw[3] = rw[3]; }
+    if (sel & kSelFlags) {
+      if (d.stopped) P.runctl[d.r].saved_flags = d.rec[4];
+      else dev[4] = d.rec[4];
+    }
+    atomicMax(P.mark + d.r, P.mark_touched);   // max: an upload's "must list" bit stays
+  }
+}
+
+cudaError_t launch_resync(const ResyncParams& P, uint32_t smem_bytes, cudaStream_t stream) {
+  if (P.n == 0) return cudaSuccess;
+  if (smem_bytes > 48u * 1024u) {
+    cudaError_t e = cudaFuncSetAttribute(resync_runs<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes);
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(resync_runs<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes);
+    if (e != cudaSuccess) return e;
+  }
+  const uint32_t grid = (P.n - 1u) / P.warps_per_block + 1u, threads = 32u * P.warps_per_block;
+  resync_runs<false><<<grid, threads, smem_bytes, stream>>>(P);
+  cta_scan<2><<<1, 1024, 0, stream>>>(P.cta, P.total, grid);
+  resync_runs<true><<<grid, threads, smem_bytes, stream>>>(P);
   return cudaGetLastError();
 }
 

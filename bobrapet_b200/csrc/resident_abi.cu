@@ -1382,3 +1382,106 @@ int bf_resident_status(bf_ctx* c, uint32_t h, uint32_t n_runs, const uint32_t* r
   out->n_events = total;
   return BF_OK;
 }
+
+// ---- resyncs (resident.cu) ------------------------------------------------------------------------------------------------------
+// Every check first, so a refused call changes nothing.  The caller's records go to the call's scratch in one H2D copy straight from
+// the caller's buffer (not through CallStage's host image: they are the bulk of the call); then the count, scan and list launches,
+// the D2H copy of the totals and one synchronisation.  Pinned drifted / items buffers are written in place, others copied after it.
+int bf_resident_resync(bf_ctx* c, uint32_t h, bf_resync* q) {
+  auto [g, r] = lock_resident(c, h);
+  if (!q || q->struct_size != sizeof(bf_resync)) return fail(c, BF_EINVAL, "null bf_resync or bad struct_size");
+  q->bad_run = BF_RESYNC_NONE;
+  if (!r) return BF_EINVAL;
+  const bf_layout& L = r->L;
+  const uint32_t n = q->n, *runs = q->runs;
+  if (q->n_runs > r->cap) return fail(c, BF_EINVAL, "n_runs exceeds the resident batch");
+  if (!runs && n != q->n_runs) return fail(c, BF_EINVAL, "runs == NULL lists every run of [0, n_runs): n must equal n_runs");
+  for (uint32_t i = 0; runs && i < n; ++i) {
+    if (runs[i] >= q->n_runs) return fail(c, BF_EINVAL, "runs[" + std::to_string(i) + "] is not below n_runs");
+    if (i && runs[i] <= runs[i - 1]) return fail(c, BF_EINVAL, "runs[" + std::to_string(i) + "] does not ascend");
+  }
+  if (n && !q->records) return fail(c, BF_EINVAL, "null records");
+  if ((q->drifted_cap && !q->drifted) || (q->items_cap && !q->items)) return fail(c, BF_EINVAL, "null drifted / items with a non-zero cap");
+  if (q->flags & ~BF_RESYNC_CHECK) return fail(c, BF_EINVAL, "unknown flags");
+  if (q->fields & ~(uint32_t)BF_RESYNC_ALL_FIELDS) return fail(c, BF_EINVAL, "unknown fields");
+  const uint8_t* recs = static_cast<const uint8_t*>(q->records);
+  for (uint32_t i = 0; i < n; ++i) {   // a run may hold only a slot a put has returned (alive or dropped since)
+    uint32_t slot;
+    memcpy(&slot, recs + (size_t)i * L.state_stride, 4);
+    if (slot >= c->slots_host.size()) {
+      q->bad_run = runs ? runs[i] : i;
+      return fail(c, BF_EINVAL, "record of run " + std::to_string(q->bad_run) + " names a slot no put has returned");
+    }
+  }
+  uint32_t fields = q->fields;   // a field the layout does not place is neither compared nor written
+  if (L.off_cond == BF_OFF_NONE) fields &= ~BF_RESYNC_FIELD(BF_DELTA_COND);
+  if (L.off_decision == BF_OFF_NONE) fields &= ~BF_RESYNC_FIELD(BF_DELTA_DECISION);
+  if (L.off_child == BF_OFF_NONE) fields &= ~BF_RESYNC_FIELD(BF_DELTA_CHILD);
+  uint32_t wpb = 8, topo = 0, per_warp = 0;
+  if (L.off_child != BF_OFF_NONE) {   // a shared stage per warp for the parallel joins, as bf_resident_status
+    topo = bf::largest_record(c, L.words);
+    per_warp = L.state_stride + topo + 256u;
+    wpb = std::min<uint32_t>(8u, (227u * 1024u - bf::kStatusStaticSmem) / per_warp);
+    if (!wpb) return fail(c, BF_ENOMEM, "a topology record and a state record do not fit one warp's shared memory");
+  }
+  q->n_drifted = q->n_written = 0;
+  q->n_items = 0;
+  if (n == 0) return BF_OK;
+  BF_CUDA(c, cudaSetDevice(c->device));
+  cudaStream_t s = c->stream;
+  if (int rc = bf::sync_slots(c, s)) return rc;
+  const bool check = q->flags & BF_RESYNC_CHECK;
+  const uint32_t grid = (n - 1u) / wpb + 1u;
+  // a run has at most one item per code, nibble and registered bit of the layout, and its flags byte: a larger cap stages no more
+  const uint64_t per_run = 3ull * L.words * 32u + L.child_nibbles + 65u;
+  const uint64_t items_cap = std::min<uint64_t>(q->items_cap, (uint64_t)n * per_run);
+  const uint32_t drifted_cap = std::min(q->drifted_cap, n);
+  bf::ResyncParams P{};
+  P.runs = runs ? static_cast<const uint32_t*>(bf::pinned_dev(runs)) : nullptr;
+  P.drifted = drifted_cap ? static_cast<uint32_t*>(bf::pinned_dev(q->drifted)) : nullptr;
+  P.items = items_cap && reinterpret_cast<uintptr_t>(q->items) % 16 == 0 ? static_cast<bf_drift*>(bf::pinned_dev(q->items)) : nullptr;
+  const bool staged_drifted = drifted_cap && !P.drifted, staged_items = items_cap && !P.items;
+  uint8_t* d_records;
+  CallStage st;
+  if (runs && !P.runs) st.up(P.runs, runs, n);
+  st.out(d_records, (size_t)n * L.state_stride);
+  st.out(P.run_items, n);
+  st.out(P.cta, 2 * (size_t)grid);
+  st.out(P.total, 2);
+  if (staged_drifted) st.out(P.drifted, drifted_cap);
+  if (staged_items) st.out(P.items, items_cap);
+  if (int rc = st.send(c, "bf_resident_resync")) return rc;
+  BF_CUDA(c, cudaMemcpyAsync(d_records, recs, (size_t)n * L.state_stride, cudaMemcpyHostToDevice, s));
+  P.records = d_records;
+  P.state = r->d_state; P.slots = c->slots_dev; P.n_slots = (uint32_t)c->slots_host.size();
+  P.runctl = r->areas.d_runctl; P.areas = r->areas_view();
+  P.mark = r->d_mark; P.mark_touched = r->mark_touched(); P.mark_must_list = r->mark_must_list();
+  P.n = n; P.warps_per_block = wpb;
+  P.words = L.words; P.state_stride = L.state_stride; P.off_phase = L.off_phase; P.off_cond = L.off_cond;
+  P.off_decision = L.off_decision; P.off_child = L.off_child; P.child_nibbles = L.child_nibbles; P.topo_bytes = topo;
+  P.fields = fields; P.check = check;
+  P.drifted_cap = drifted_cap; P.items_cap = items_cap;
+  cudaError_t e = bf::launch_resync(P, wpb * per_warp, s);
+  if (e == cudaSuccess) e = cudaMemcpyAsync(c->pinned->resync, P.total, 16, cudaMemcpyDeviceToHost, s);
+  if (check) {
+    if (int rc = bf::end_call(c, e, "bf_resident_resync")) return rc;
+  } else if (int rc = r->sync_in_place(c, e, "bf_resident_resync")) {
+    r->state_changed(c);
+    return rc;
+  }
+  c->stats.kernel_launches += 3;
+  const uint64_t items = c->pinned->resync[0];
+  const uint32_t drifted = (uint32_t)c->pinned->resync[1];
+  if (!check && drifted) {   // as a commit that wrote: the evaluated snapshot and the tick end (before any copy can fail)
+    r->state_changed(c);
+    r->pending += drifted;
+  }
+  if (const uint32_t k = std::min(drifted, drifted_cap); k && staged_drifted)
+    BF_CUDA(c, cudaMemcpy(q->drifted, P.drifted, (size_t)k * 4, cudaMemcpyDeviceToHost));
+  if (const uint64_t k = std::min<uint64_t>(items, items_cap); k && staged_items)
+    BF_CUDA(c, cudaMemcpy(q->items, P.items, (size_t)k * sizeof(bf_drift), cudaMemcpyDeviceToHost));
+  q->n_items = items;
+  q->n_drifted = drifted;
+  q->n_written = check ? 0 : drifted;
+  return BF_OK;
+}

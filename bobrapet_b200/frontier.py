@@ -66,6 +66,7 @@ class Frontier:
         self._lib = A.load()
         self._owned = _borrowed_ctx is None
         self._steps_max: Dict[int, int] = {}   # steps_max of each resident batch's layout
+        self._child_nibbles: Dict[int, int] = {}   # and its child_nibbles
         if _borrowed_ctx is not None:       # a shard's ctx owned by a FrontierGroup
             self._ctx = C.c_void_p(_borrowed_ctx)
             return
@@ -258,6 +259,7 @@ class Frontier:
         state, the current result records and the touch marks"""
         self._check(self._lib.bf_resident_reshape(self._ctx, handle, C.byref(L), capacity), "bf_resident_reshape")
         self._steps_max[handle] = int(L.steps_max)
+        self._child_nibbles[handle] = int(L.child_nibbles)
 
     def resident_retire(self, handle: int, n_runs: int, runs, capacity: int = 0):
         """bf_resident_retire: take `runs` (distinct indices below n_runs) out of the batch; the last live runs move into the
@@ -289,6 +291,7 @@ class Frontier:
             err.extent = e.as_dict()
             raise err
         self._steps_max[handle] = int(L.steps_max)
+        self._child_nibbles[handle] = int(L.child_nibbles)
         return e.as_dict()
 
     def resident_transfer(self, src: int, dst: int, src_n: int, dst_n: int, runs) -> dict:
@@ -424,6 +427,39 @@ class Frontier:
                                                  C.byref(out)), "bf_resident_status")
         return recs, events[:min(int(out.n_events), int(events_cap))].copy(), int(out.n_events)
 
+    # -- resyncs of resident batches (bf_resident_resync)
+    DRIFT_DTYPE = np.dtype([("run", "<u4"), ("index", "<u2"), ("field", "u1"), ("reserved", "u1"), ("device", "<u4"),
+                            ("record", "<u4")])   # bf_drift, 16 B
+
+    def resident_resync(self, handle: int, n_runs: int, records, runs=None, fields: int = A.RESYNC_ALL_FIELDS,
+                        check: bool = False, drifted_cap: Optional[int] = None, items_cap: Optional[int] = None) -> dict:
+        """bf_resident_resync: compare the device's records of the listed runs (runs: strictly ascending, below n_runs; None:
+        every run of [0, n_runs)) with `records` (one packed state record per listed run, list order) after a single pass's
+        stages, list every difference and, unless check, repair the runs that drifted.  drifted_cap defaults to every listed
+        run, items_cap to 65 536 items (1 MiB; n_items is the true count, so a check with a larger cap lists the rest).  -> {drifted u32[min(n_drifted, cap)], items DRIFT_DTYPE[min(n_items, cap)], n_drifted,
+        n_written, n_items}.  A refusal raises FrontierError with .bad_run set."""
+        rl = None if runs is None else np.ascontiguousarray(runs, dtype=np.uint32)
+        n = int(n_runs) if rl is None else rl.shape[0]
+        recs = np.ascontiguousarray(records, dtype=np.uint8)
+        if drifted_cap is None:
+            drifted_cap = n
+        if items_cap is None:   # a buffer not in pinned memory is staged in the ctx's device scratch, which keeps its largest size
+            items_cap = min(n * (3 * 32 * ((self._steps_max[handle] + 31) // 32) + self._child_nibbles[handle] + 65), 1 << 16)
+        drifted = np.zeros(max(int(drifted_cap), 1), dtype=np.uint32)
+        items = np.zeros(max(int(items_cap), 1), dtype=self.DRIFT_DTYPE)
+        q = A.Resync(struct_size=C.sizeof(A.Resync), n_runs=int(n_runs), runs=None if rl is None else rl.ctypes.data, n=n,
+                     fields=int(fields), records=recs.ctypes.data if recs.size else None, flags=A.RESYNC_CHECK if check else 0,
+                     drifted_cap=int(drifted_cap), drifted=drifted.ctypes.data if drifted_cap else None,
+                     items=items.ctypes.data if items_cap else None, items_cap=int(items_cap))
+        rc = self._lib.bf_resident_resync(self._ctx, handle, C.byref(q))
+        if rc != 0:
+            err = A.FrontierError(rc, "bf_resident_resync: %s" % self._lib.bf_last_error(self._ctx).decode())
+            err.bad_run = int(q.bad_run)
+            raise err
+        return {"drifted": drifted[:min(int(q.n_drifted), int(drifted_cap))].copy(),
+                "items": items[:min(int(q.n_items), int(items_cap))].copy(), "n_drifted": int(q.n_drifted),
+                "n_written": int(q.n_written), "n_items": int(q.n_items)}
+
     # -- limiter inputs and schedules of resident batches (bf_resident_sched*, bf_resident_schedule)
     SCHED_PUT_DTYPE = np.dtype([("run", "<u4"), ("story_key", "<u4"), ("queue_key", "<u4"), ("priority", "<i4"),
                                 ("queued_since", "<u4"), ("run_phase", "<u4"), ("reserved", "<u4", (2,))])   # bf_sched_put, 32 B
@@ -499,6 +535,7 @@ class Frontier:
         h = C.c_uint32()
         self._check(self._lib.bf_resident_create(self._ctx, C.byref(L), capacity, C.byref(h)), "bf_resident_create")
         self._steps_max[h.value] = int(L.steps_max)   # sizes resident_status's default event buffer
+        self._child_nibbles[h.value] = int(L.child_nibbles)   # and, with it, resident_resync's default item buffer
         return h.value
 
     def resident_destroy(self, handle: int):

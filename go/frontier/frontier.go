@@ -704,6 +704,67 @@ func (r *Resident) Status(n uint32, runs []uint32, statuses []StatusRecord, even
 	return uint64(ne), r.c.err(rc)
 }
 
+// Drift is one difference Resync found (bf_drift, 16 bytes, no pointers): Field is a Delta* field, Index the step, child nibble or
+// parallel desc it names, Device and Record the compared values, the device's and the caller's.
+type Drift struct {
+	Run            uint32
+	Index          uint16
+	Field          uint8
+	Reserved       uint8
+	Device, Record uint32
+}
+
+// Resync flags and fields (BF_RESYNC_*): ResyncCheck compares and lists only; ResyncField(f) selects a Delta* field.
+const (
+	ResyncCheck     = 0x1
+	ResyncAllFields = 0x3F
+)
+
+// ResyncField is BF_RESYNC_FIELD(f) for a Delta* field.
+func ResyncField(f uint8) uint32 { return 1 << f }
+
+// Resync compares the device's records of the listed runs (runs: strictly ascending, below n; nil: every run of [0, n)) with
+// records packed from the cluster (one state record per listed run, in list order), lists every difference into drifted and
+// items, and without ResyncCheck repairs the runs that drifted (bf_resident_resync).  The counts are the true ones; only the first
+// len(drifted) / len(items) entries are written.  On a refusal that names a run (a record holding a slot no put has returned),
+// badRun is that run, else SchedNone.
+func (r *Resident) Resync(n uint32, runs []uint32, records []byte, fields uint32, check bool, drifted []uint32,
+	items []Drift) (nDrifted, nWritten uint32, nItems uint64, badRun uint32, err error) {
+	count := int(n)
+	var rp *C.uint32_t
+	if runs != nil {
+		count = len(runs)
+		if count > 0 {
+			rp = (*C.uint32_t)(unsafe.Pointer(&runs[0]))
+		}
+	}
+	if need := count * int(r.layout.state_stride); len(records) < need {
+		return 0, 0, 0, SchedNone, fmt.Errorf("frontier: records holds %d bytes for %d runs of %d", len(records), count,
+			int(r.layout.state_stride))
+	}
+	var recp unsafe.Pointer
+	if len(records) > 0 {
+		recp = unsafe.Pointer(&records[0])
+	}
+	var dp *C.uint32_t
+	if len(drifted) > 0 {
+		dp = (*C.uint32_t)(unsafe.Pointer(&drifted[0]))
+	}
+	var ip *C.bf_drift
+	if len(items) > 0 {
+		ip = (*C.bf_drift)(unsafe.Pointer(&items[0]))
+	}
+	var flags C.uint32_t
+	if check {
+		flags = ResyncCheck
+	}
+	var nd, nw, bad C.uint32_t
+	var ni C.uint64_t
+	rc := C.bfgo_resident_resync(r.c.p, r.handle, C.uint32_t(n), rp, C.uint32_t(count), recp, C.uint32_t(fields), flags, dp,
+		C.uint32_t(len(drifted)), ip, C.uint64_t(len(items)), &nd, &nw, &ni, &bad)
+	return uint32(nd), uint32(nw), uint64(ni), uint32(bad), r.c.err(rc)
+}
+
 // SchedPut is one limiter-input request of PutSched (bf_sched_put, 32 bytes, no pointers).  QueuedSince is the StartedAt of the
 // run's earliest queued step on the clock of ScheduleResident's now (SchedNone: nothing queued); the device ages from it.
 type SchedPut struct {

@@ -1220,6 +1220,82 @@ typedef struct bf_status_out {
 
 int bf_resident_status(bf_ctx* ctx, uint32_t handle, uint32_t n_runs, const uint32_t* runs, uint32_t n, bf_status_out* out);
 
+/* ------------------------------------------------------------------ resyncs (does the device still agree with the cluster?)
+ * The reference rebuilds its state from the StepRuns and the fresh status on every reconcile (syncStateFromStepRuns, dag.go:965-1009)
+ * and merges its writes back into the cluster object (persistMergedStates, :774-793), so drift never outlives one reconcile.  A
+ * resident batch keeps state across ticks, so a lost watch event or a failed status PATCH persists until something overwrites it.
+ * bf_resident_resync compares the device's state records of the listed runs with records the caller packed from the cluster (same
+ * format and layout as bf_resident_upload), lists every difference and, without BF_RESYNC_CHECK, repairs only the runs that drifted.
+ *
+ * What is compared (record = the caller's record as the repair would leave it on the device: the device's record with the caller's
+ * codes in the selected fields; for a stopped run the flags byte the stages read is the stopped byte on both sides):
+ *   - slot: topo_slot, always.  A run whose slot differs has exactly one item, BF_DELTA_TOPO_SLOT (index 0), and nothing else.
+ *   - a live slot that fits the layout: both sides take the stages of a single pass that bf_resident_status applies (H, G, I; no
+ *     stage D cond-FAIL writes; a stopped run evaluated with its stopped flags byte).  Then for each field selected in `fields`:
+ *       PHASE      the resulting codes of steps < S (code 15 read as 0 before the stages);
+ *       COND, DECISION   the input codes of steps whose resulting phase is not terminal on at least one side (a step terminal on
+ *                  both no longer reads them);
+ *       CHILD      the nibbles (15 read as 0) of the slot's parallel descs whose step is not terminal on at least one side;
+ *       REGISTERED the children_registered bits of those same descs;
+ *       RUN_FLAGS  the byte; for a stopped run the device's saved byte (bf_run_ctl.saved_flags), not the stopped byte.
+ *   - a dead slot, or one wider than the layout: no stages.  Every code of the layout as stored (words * 32 steps, phases and
+ *     nibbles with 15 read as 0), every child nibble of the layout, all 64 registered bits and the flags byte.
+ *   - never compared: the reserved header bytes, codes at or past S of a live slot, nibbles and registered bits outside its descs,
+ *     padding.  A field the layout does not place (cond, decision, child area) is neither compared nor written.
+ * Items (bf_drift) are ordered by (run, field, index); device and record are the compared values (a PHASE item carries the phases
+ * after the stages).  Why the stages come first: their rewrites are never stored (a fired sleep is Paused with decision SUCCEED on
+ * the device and Succeeded in the cluster; a joined parallel step Running here and Succeeded / Failed there; a fail-fast skip 0
+ * here and Skipped there), so equal states differ as bytes and agree only after them.
+ *
+ * Repair (without BF_RESYNC_CHECK), of the drifted runs only:
+ *   - slot drift: the whole record becomes the caller's bytes; the run is touched as by a migrate (listed by the next touched tick
+ *     even if its result is unchanged) and its schedule baseline is dropped (listed by the next bf_resident_schedule);
+ *   - otherwise: each selected field's storage (all of its planes' words, the whole child area, all 64 registered bits, the flags
+ *     byte) becomes the caller's and the rest stays the device's; the run is touched as by a delta (the next touched tick evaluates
+ *     it and lists it when its result changed) and keeps its schedule baseline;
+ *   - a stopped run stays stopped: the caller's flags byte becomes its saved byte and the record keeps the stopped byte;
+ *   - timers, limiter inputs, result records and the changed-only baseline are not touched.  pending grows by n_written.
+ * A resync that wrote something ends the evaluated snapshot and the tick (bf_resident_schedule and bf_resident_commit must follow a
+ * new tick), as a commit that wrote.  One that wrote nothing, and every BF_RESYNC_CHECK call, changes nothing at all.
+ * Refused before anything is written, BF_EINVAL and nothing changed: struct_size or the handle; n_runs > capacity; runs not strictly
+ * ascending or not below n_runs; runs == NULL with n != n_runs; records == NULL with n > 0; drifted / items NULL with a non-zero
+ * cap; unknown flags or fields bits; a record naming a slot no put has returned (bad_run names its run, else BF_RESYNC_NONE).
+ * One H2D copy of the records (and one of a run list not in pinned memory), three launches (count, scan, list and repair), one D2H
+ * copy of the totals, one synchronisation.  Pinned drifted / items buffers are written in place; others are staged in the ctx's
+ * device scratch (16 B per item of items_cap, clamped to what the listed runs can have; the scratch keeps its largest size for
+ * the ctx's lifetime, so size items_cap to the drift expected: n_items is the true count) and copied after the synchronisation. */
+#define BF_RESYNC_CHECK 0x1u                 /* flags: compare and list only; nothing changes                                   */
+#define BF_RESYNC_FIELD(f) (1u << (f))       /* fields: BF_DELTA_PHASE .. BF_DELTA_REGISTERED; the slot is always compared       */
+#define BF_RESYNC_ALL_FIELDS 0x3Fu
+#define BF_RESYNC_NONE 0xFFFFFFFFu
+typedef struct bf_drift {        /* 16 B                                                                                       */
+  uint32_t run;
+  uint16_t index;                /* step (PHASE / COND / DECISION), child nibble (CHILD), desc (REGISTERED), else 0             */
+  uint8_t field;                 /* BF_DELTA_*                                                                                 */
+  uint8_t reserved;
+  uint32_t device, record;       /* the compared values: the device's and the caller's                                        */
+} bf_drift;
+typedef struct bf_resync {
+  uint32_t struct_size;          /* sizeof(bf_resync)                                                                          */
+  uint32_t n_runs;               /* in: the batch's runs are [0, n_runs)                                                       */
+  const uint32_t* runs;          /* in: [n] strictly ascending, below n_runs; NULL with n == n_runs: every run of [0, n_runs)  */
+  uint32_t n;
+  uint32_t fields;               /* in: BF_RESYNC_FIELD(BF_DELTA_*) bits                                                       */
+  const void* records;           /* in: n state records in list order, the batch's layout                                      */
+  uint32_t flags;                /* in: BF_RESYNC_CHECK                                                                        */
+  uint32_t drifted_cap;
+  uint32_t* drifted;             /* [drifted_cap] out: ascending runs with at least one item                                   */
+  uint32_t n_drifted;            /* out: the true count                                                                        */
+  uint32_t n_written;            /* out: runs repaired (0 with BF_RESYNC_CHECK)                                                */
+  bf_drift* items;               /* [items_cap] out                                                                            */
+  uint64_t items_cap;
+  uint64_t n_items;              /* out: the true count; only the first items_cap were written                                */
+  uint32_t bad_run;              /* out on a refusal: the run whose record names an unknown slot, else BF_RESYNC_NONE          */
+  uint32_t reserved;
+} bf_resync;
+
+int bf_resident_resync(bf_ctx* ctx, uint32_t handle, bf_resync* r);
+
 /* ------------------------------------------------------------------ device groups (SURVEY.md row e)
  * The reference is ONE operator process (cmd/main.go:220, StoryRunReconciler storyrun_controller.go:216), so the
  * multi-GPU path must be reachable from one process through this ABI: a group owns one ctx per device and an NCCL
