@@ -201,6 +201,14 @@ class CommitArm(C.Structure):
     _fields_ = [(n, C.c_uint32) for n in ("struct_size", "now", "n_armed", "next_deadline")]
 
 
+COMMIT_WRITE_TIMER = 0x10   # BF_COMMIT_WRITE_TIMER: bf_commit_write.field of a timer-arm item (else DELTA_PHASE / DELTA_REGISTERED)
+
+
+class CommitJournal(C.Structure):
+    _fields_ = [("struct_size", C.c_uint32), ("reserved", C.c_uint32), ("items", C.c_void_p), ("items_cap", C.c_uint64),
+                ("n_items", C.c_uint64), ("runs", C.c_void_p), ("runs_cap", C.c_uint32), ("n_runs_listed", C.c_uint32)]
+
+
 OUTCOME_NONE, OUTCOME_SUCCEEDED, OUTCOME_DEPENDENCY_FAILED, OUTCOME_COMPENSATED = 0, 1, 2, 3   # BF_OUTCOME_*: bf_status_rec.outcome
 OUTCOME_COMPENSATION_FAILED, OUTCOME_CLEANUP_FAILED, OUTCOME_TIMED_OUT = 4, 5, 6
 OUTCOME_CANCELED, OUTCOME_STOPPED, OUTCOME_DEAD = 7, 8, 9
@@ -286,6 +294,8 @@ SYMBOLS = [
     ("bf_resident_commit", C.c_int, [C.c_void_p, C.c_uint32, C.c_uint32, C.c_void_p, C.c_uint32, C.POINTER(CommitOut)]),
     ("bf_resident_commit_timed", C.c_int, [C.c_void_p, C.c_uint32, C.c_uint32, C.c_void_p, C.c_uint32, C.POINTER(CommitOut),
                                            C.POINTER(CommitArm)]),
+    ("bf_resident_commit_journal", C.c_int, [C.c_void_p, C.c_uint32, C.c_uint32, C.c_void_p, C.c_uint32, C.POINTER(CommitOut),
+                                             C.POINTER(CommitArm), C.POINTER(CommitJournal)]),
     ("bf_resident_status", C.c_int, [C.c_void_p, C.c_uint32, C.c_uint32, C.c_void_p, C.c_uint32, C.POINTER(StatusOut)]),
     ("bf_resident_resync", C.c_int, [C.c_void_p, C.c_uint32, C.POINTER(Resync)]),
     ("bf_group_create", C.c_int, [C.POINTER(C.c_void_p), C.POINTER(C.c_int32), C.c_uint32, C.POINTER(Config)]),

@@ -188,6 +188,7 @@ struct bf_ctx {
     uint32_t commit[8];    // bf_resident_commit: the offender key (two words), then the five counts
     unsigned long long status_events;   // bf_resident_status: the events of the call
     unsigned long long resync[2];       // bf_resident_resync: the items and the drifted runs of the call
+    unsigned long long commit_journal[2];   // bf_resident_commit_journal: the items and the written runs of the call
     bf_counts counts() const { return {tail.counts[0], tail.counts[1], tail.counts[2], tail.counts[3]}; }
   }* pinned = nullptr;
   DevBuf<bf_expansion> d_exp;

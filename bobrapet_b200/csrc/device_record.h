@@ -491,7 +491,19 @@ struct CommitParams {
   unsigned long long* offender;  // [1] commit_check: lowest key (atomicMin; ~0 from the caller)
   uint32_t* counts;              // [5] commit_apply: runs written, skipped, launched, queued, failed (zeroed by the caller)
   CommitTimings arm;             // arm.tim = nullptr: no arming
+  // bf_resident_commit_journal (the <true> builds of both launches): commit_check stores each run's journal word and each CTA's
+  // items and written runs (cta: [2][CTAs]), cta_scan turns them into those of the CTAs before each and posts the sums
+  // (total[2]), commit_apply writes each run's items and its entry in runs at those offsets
+  uint32_t* run_items;           // [n_runs] items << 8 | new arms << 1 | written
+  unsigned long long* cta;       // [2][CTAs] items and written runs of each CTA, then (cta_scan) of the CTAs before it
+  unsigned long long* total;     // [2] items and written runs of the call
+  bf_commit_write* items;        // [items_cap]
+  unsigned long long items_cap;
+  uint32_t* runs;                // [runs_cap]
+  uint32_t runs_cap;
 };
+static_assert(sizeof(bf_commit_write) == 16, "bf_commit_write must be 16 bytes");
+constexpr uint32_t kJournalArmsShift = 1, kJournalItemsShift = 8;   // new arms <= BF_TIMER_MAX_SLOTS < 128
 
 // bf_resident_status (resident.cu): one warp per listed run.  status_count stores each listed run's event count and each CTA's
 // total, cta_scan turns the CTA totals into the events of the CTAs before each and posts the sum, status_list writes the

@@ -911,6 +911,45 @@ cudaError_t launch_fire(const FireParams& P, cudaStream_t stream) {
   return cudaGetLastError();
 }
 
+// One CTA: for each of K arrays of n_ctas per-CTA totals (array k at cta + k * n_ctas), the totals become the sums of the CTAs
+// before each (exclusive scan in place); array k's sum goes to total[k].  bf_resident_status scans its events (K = 1),
+// bf_resident_resync its items and drifted runs, bf_resident_commit_journal its items and written runs (K = 2).
+template <uint32_t K>
+__global__ void __launch_bounds__(1024) cta_scan(unsigned long long* cta, unsigned long long* total, uint32_t n_ctas) {
+  __shared__ unsigned long long s_e[32];
+  const uint32_t lane = threadIdx.x & 31u, warp = threadIdx.x >> 5;
+  for (uint32_t k = 0; k < K; ++k) {
+    unsigned long long* a = cta + (size_t)k * n_ctas;
+    unsigned long long carry = 0;
+    for (uint32_t base = 0; base < n_ctas; base += 1024u) {
+      const uint32_t i = base + threadIdx.x;
+      const unsigned long long e = i < n_ctas ? a[i] : 0ull;
+      unsigned long long ie = e;
+#pragma unroll
+      for (int d = 1; d < 32; d <<= 1) {
+        const unsigned long long b = __shfl_up_sync(FULL, ie, d);
+        if ((int)lane >= d) ie += b;
+      }
+      if (lane == 31) s_e[warp] = ie;
+      __syncthreads();
+      if (warp == 0) {   // the warp totals' inclusive scan
+        unsigned long long we = s_e[lane];
+#pragma unroll
+        for (int d = 1; d < 32; d <<= 1) {
+          const unsigned long long b = __shfl_up_sync(FULL, we, d);
+          if ((int)lane >= d) we += b;
+        }
+        s_e[lane] = we;
+      }
+      __syncthreads();
+      if (i < n_ctas) a[i] = carry + (warp ? s_e[warp - 1] : 0ull) + ie - e;
+      carry += s_e[31];
+      __syncthreads();   // s_e is rewritten by the next chunk
+    }
+    if (threadIdx.x == 0) total[k] = carry;
+  }
+}
+
 // ---- tick commits (bf_resident_commit*) -------------------------------------------------------------------------------------
 // One warp per run; lane w holds word w of the run's masks and codes (words <= 32).  Both launches read a run the same way: its
 // topology's step types, the masks of its current result record (and of its schedule record), and its entries [lo, hi), found by
@@ -980,15 +1019,24 @@ DI unsigned long long commit_entries(const CommitParams& P, uint32_t r, uint32_t
   return bad;
 }
 
+// Where commit_apply<true> lists a run's new arms: its TIMER items start at items[at] (nullptr: no journal, nothing listed)
+struct ArmItems {
+  bf_commit_write* items;
+  unsigned long long at, cap;
+};
+
 // The timer arms of run r (whole warp, with a timing table): each timing of the run's slot whose step is in ARM (lane w holds
 // word w: the launched sleep / gate / wait steps) and that no armed slot of the run names is a new arm; an armed slot stays.
 // Lane t holds slots t and t + 32 (armed slots lead, ascending by step).  The timings ascend by step and are walked 32 at a time,
 // so new arms come in step order: a new arm's rank is the new arms before it plus the armed slots of lower steps (counted over
 // the slots, read through shuffles, which also finds a stored slot), a kept slot's is its index plus the new arms of lower
 // steps, as arm_timers ranks them.  Check: -> the key of the run's first arming offence (a non-PENDING code without decision
-// planes at its step, more than timer_k slots at the lowest new step), else ~0; nothing is written.  Apply (after a check that
-// found none): stores the moved and the new slots and adds the arms and their earliest deadline to A.out.
-DI unsigned long long commit_arms(const CommitTimings& A, uint32_t r, uint32_t lane, uint32_t slot, uint32_t ARM, bool apply) {
+// planes at its step, more than timer_k slots at the lowest new step), else ~0; nothing is written; n_armed: the new arms.
+// Apply (after a check that found none): stores the moved and the new slots, lists the new arms in step order at J, and adds
+// the arms and their earliest deadline to A.out.
+DI unsigned long long commit_arms(const CommitTimings& A, uint32_t r, uint32_t lane, uint32_t slot, uint32_t ARM, bool apply,
+                                  uint32_t& n_armed, const ArmItems& J) {
+  n_armed = 0;
   if (slot >= A.n_slots || !__any_sync(FULL, ARM != 0u)) return ~0ull;
   const uint32_t lo = A.first[slot], hi = A.first[slot + 1], K = A.timer_k;
   if (lo == hi) return ~0ull;
@@ -1019,8 +1067,11 @@ DI unsigned long long commit_arms(const CommitTimings& A, uint32_t r, uint32_t l
     } else {
       if (fresh) {
         const uint32_t dl = (uint32_t)min((unsigned long long)A.now + q.delay, (unsigned long long)BF_TIMER_NONE - 1ull);
-        t[n_new + __popc(m & ((1u << lane) - 1u)) + below] = (unsigned long long)dl | (unsigned long long)s << 32 | (unsigned long long)q.code << 48;
+        const uint32_t rank = n_new + __popc(m & ((1u << lane) - 1u));
+        t[rank + below] = (unsigned long long)dl | (unsigned long long)s << 32 | (unsigned long long)q.code << 48;
         next = min(next, dl);
+        if (J.items && J.at + rank < J.cap)
+          reinterpret_cast<uint4*>(J.items)[J.at + rank] = make_uint4(r, s | BF_COMMIT_WRITE_TIMER << 16 | (uint32_t)q.code << 24, BF_TIMER_NONE, dl);
       }
       for (uint32_t x = m; x; x &= x - 1u) {   // each new arm moves the kept slots of higher steps up one
         const uint32_t sn = __shfl_sync(FULL, s, __ffs(x) - 1);
@@ -1030,6 +1081,7 @@ DI unsigned long long commit_arms(const CommitTimings& A, uint32_t r, uint32_t l
     }
     n_new += __popc(m);
   }
+  n_armed = n_new;
   if (!apply) {   // a decision offence at the lowest new step wins over the overflow there
     if (first_dec != ~0u && (first_dec == first_new || E + n_new <= K))
       return (unsigned long long)r << 32 | (unsigned long long)first_dec << 8 | kCommitNoDecision;
@@ -1045,14 +1097,69 @@ DI unsigned long long commit_arms(const CommitTimings& A, uint32_t r, uint32_t l
   return ~0ull;
 }
 
-// Check: every entry names a launched step (a PHASE entry a stop step), and every launched stop step of a run without an ERROR
-// entry has a HOLD or PHASE entry; with a timing table, the arming offences too.  Lane 0 lowers P.offender to the run's first
-// offence.  Nothing is written.
-__global__ void __launch_bounds__(256) commit_check(const CommitParams P) {
-  const uint32_t r = blockIdx.x * 8u + (threadIdx.x >> 5), lane = threadIdx.x & 31u;
-  if (r >= P.n_runs) return;
+// The writes of run r (no ERROR entry, a slot that fits: c.topo set) on the codes as the pass reads them (code 15 as 0): lane w's
+// stored planes p, new codes n and the steps whose code changes (dirty), and the disjoint masks; commit_registered adds the
+// registered bits newly set (lanes p and p + 32 look at the launched parallel descs; reg_only counts the steps whose bit alone
+// changes).  commit_apply stores them; commit_check<true> counts them, so that both launches agree on every item.  between(LA)
+// runs once the masks are known (commit_apply arms there).
+struct CommitWrites {
+  uint32_t p[4], n0, n1, n2, n3, dirty;
+  uint32_t SK, FA, LA, QU;
+  unsigned long long reg, newly;
+  uint32_t reg_only;
+};
+template <typename Between>
+DI void commit_writes(const CommitParams& P, uint32_t lane, const CommitRun& c, const uint8_t* rec, uint32_t hold, CommitWrites& w,
+                      Between between) {
+  const uint32_t* ph = reinterpret_cast<const uint32_t*>(rec + P.off_phase) + lane;
+  for (uint32_t b = 0; b < 4; ++b) w.p[b] = 0u;
+  if (lane < c.TW)
+    for (uint32_t b = 0; b < 4; ++b) w.p[b] = ph[b * P.words];
+  const uint32_t keep = c.VALID & ~(w.p[0] & w.p[1] & w.p[2] & w.p[3]);
+  const uint32_t m0 = w.p[0] & keep, m1 = w.p[1] & keep, m2 = w.p[2] & keep, m3 = w.p[3] & keep;
+  uint32_t n0 = m0, n1 = m1, n2 = m2, n3 = m3;
+  w.SK = c.skip; w.FA = c.fail & ~w.SK; w.LA = c.launched & ~w.SK & ~w.FA & ~hold; w.QU = c.queued & ~w.SK & ~w.FA & ~c.launched;
+  between(w.LA);
+  pset<BF_PHASE_FAILED>(w.FA, n0, n1, n2, n3);
+  launch_effects(w.SK, w.LA, c.T_COND, c.SYNC_T, c.T_PAR, c.T_STOP, n0, n1, n2, n3);
+  pset<BF_PHASE_PENDING_QUEUED>(w.QU, n0, n1, n2, n3);
+  for (uint32_t i = c.lo; i < c.hi; ++i) {   // the stop steps' phases (a PHASE entry names a launched stop step)
+    const bf_commit_entry e = P.entries[i];
+    const uint32_t bit = 1u << (e.step & 31u);
+    if (e.kind != BF_COMMIT_PHASE || lane != (e.step >> 5u) || !(w.LA & bit)) continue;
+    n0 = (e.code & 1u) ? n0 | bit : n0 & ~bit;
+    n1 = (e.code & 2u) ? n1 | bit : n1 & ~bit;
+    n2 = (e.code & 4u) ? n2 | bit : n2 & ~bit;
+    n3 = (e.code & 8u) ? n3 | bit : n3 & ~bit;
+  }
+  w.n0 = n0; w.n1 = n1; w.n2 = n2; w.n3 = n3;
+  w.dirty = (n0 ^ m0) | (n1 ^ m1) | (n2 ^ m2) | (n3 ^ m3);
+}
+// launched parallel steps register their children (step_executor.go:808-809)
+DI void commit_registered(uint32_t lane, const CommitRun& c, const uint8_t* rec, CommitWrites& w) {
+  const TopoHeader* th = reinterpret_cast<const TopoHeader*>(c.topo);
+  const ParDesc* pd = reinterpret_cast<const ParDesc*>(c.topo + th->off_par);
+  w.reg = *reinterpret_cast<const unsigned long long*>(rec + 8);
+  const uint32_t n_par = th->P;
+  uint32_t set[2];
+  w.reg_only = 0u;
+  for (uint32_t h = 0; h < 2; ++h) {   // BF_MAX_PARALLEL = 64 descs: lane p and lane p + 32
+    const uint32_t q = lane + 32u * h;
+    const uint32_t stp = q < n_par ? pd[q].step : 0u;
+    const uint32_t lw = __shfl_sync(FULL, w.LA, (stp >> 5) & 31u), dw = __shfl_sync(FULL, w.dirty, (stp >> 5) & 31u);
+    const bool in = q < n_par && ((lw >> (stp & 31u)) & 1u);
+    set[h] = __ballot_sync(FULL, in);
+    if (in && !((w.reg >> q) & 1ull) && !((dw >> (stp & 31u)) & 1u)) ++w.reg_only;   // counted once per step
+  }
+  w.newly = ((unsigned long long)set[1] << 32 | set[0]) & ~w.reg;
+}
+
+// The per-run part of commit_check: lane 0 lowers P.offender to the run's first offence.  -> with kJournal, the run's journal
+// word (its items, new arms and whether its record changes; 0 for a run that writes nothing), else 0.
+template <bool kJournal>
+DI uint32_t check_run(const CommitParams& P, uint32_t r, uint32_t lane) {
   CommitRun c;
-  if (!commit_run(P, r, lane, c)) return;
+  if (!commit_run(P, r, lane, c)) return 0u;
   uint32_t hold, phased;
   bool err;
   unsigned long long bad = commit_entries(P, r, lane, c, true, hold, phased, err);
@@ -1064,14 +1171,53 @@ __global__ void __launch_bounds__(256) commit_check(const CommitParams P) {
     bad = min(bad, (unsigned long long)r << 32 | (unsigned long long)step << 8 | kCommitNoPhase);
   }
   if (lane == 0 && bad != ~0ull) atomicMin(P.offender, bad);
-  if (!P.arm.tim || err) return;
-  bad = commit_arms(P.arm, r, lane, c.slot, c.launched & ~c.skip & ~c.fail & ~hold & c.SYNC_T, false);
-  if (lane == 0 && bad != ~0ull) atomicMin(P.offender, bad);
+  if (err) return 0u;
+  uint32_t armed = 0;
+  if (P.arm.tim) {
+    bad = commit_arms(P.arm, r, lane, c.slot, c.launched & ~c.skip & ~c.fail & ~hold & c.SYNC_T, false, armed, ArmItems{});
+    if (lane == 0 && bad != ~0ull) atomicMin(P.offender, bad);
+  }
+  if (!kJournal || !c.topo) return 0u;   // a dead or too-wide slot has no masks: it writes nothing (an entry on it is refused)
+  const uint8_t* rec = P.state + (size_t)r * P.state_stride;
+  CommitWrites w;
+  commit_writes(P, lane, c, rec, hold, w, [](uint32_t) {});
+  commit_registered(lane, c, rec, w);
+  const uint32_t items = redux_add(__popc(w.dirty)) + __popcll(w.newly) + armed;
+  const bool written = __any_sync(FULL, w.dirty != 0u) || w.newly != 0ull;
+  return items << kJournalItemsShift | armed << kJournalArmsShift | (written ? 1u : 0u);
 }
 
-// Apply (after a check that found no offender): the writes of the contract on the codes as the pass reads them (code 15 as 0),
-// stored only where a code changed; lanes p and p + 32 set the registered bits of launched parallel descs; with a timing table,
-// the arms of the launched sleep / gate / wait steps.
+// Check: every entry names a launched step (a PHASE entry a stop step), and every launched stop step of a run without an ERROR
+// entry has a HOLD or PHASE entry; with a timing table, the arming offences too.  Lane 0 lowers P.offender to the run's first
+// offence.  Nothing is written but, with kJournal, each run's journal word and each CTA's items and written runs.
+template <bool kJournal>
+__global__ void __launch_bounds__(256) commit_check(const CommitParams P) {
+  const uint32_t r = blockIdx.x * 8u + (threadIdx.x >> 5), lane = threadIdx.x & 31u;
+  if (!kJournal) {
+    if (r < P.n_runs) check_run<false>(P, r, lane);
+    return;
+  }
+  __shared__ uint32_t warp_word[8];
+  const uint32_t jw = r < P.n_runs ? check_run<true>(P, r, lane) : 0u;
+  if (lane == 0) {
+    warp_word[threadIdx.x >> 5] = jw;
+    if (r < P.n_runs) P.run_items[r] = jw;
+  }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    unsigned long long items = 0, written = 0;
+    for (uint32_t w = 0; w < 8; ++w) { items += warp_word[w] >> kJournalItemsShift; written += warp_word[w] & 1u; }
+    const uint32_t n_ctas = (P.n_runs - 1u) / 8u + 1u;
+    P.cta[blockIdx.x] = items;
+    P.cta[n_ctas + blockIdx.x] = written;
+  }
+}
+
+// Apply (after a check that found no offender): the writes of commit_writes, stored only where a code changed; the registered
+// bits of launched parallel descs; with a timing table, the arms of the launched sleep / gate / wait steps.  With kJournal each
+// run with a journal word lists its items (PHASE by step, REGISTERED by desc, TIMER by step) from the offset of the CTAs before
+// and the warps before in its CTA, and its entry in runs when its record changed.
+template <bool kJournal>
 __global__ void __launch_bounds__(256) commit_apply(const CommitParams P) {
   const uint32_t r = blockIdx.x * 8u + (threadIdx.x >> 5), lane = threadIdx.x & 31u;
   if (r >= P.n_runs) return;
@@ -1082,54 +1228,59 @@ __global__ void __launch_bounds__(256) commit_apply(const CommitParams P) {
   commit_entries(P, r, lane, c, false, hold, phased, err);
   if (err) return;   // Execute failed: nothing of this reconcile is persisted
   uint8_t* rec = P.state + (size_t)r * P.state_stride;
+  uint32_t jw = 0, armed;
+  unsigned long long pos = 0;
+  if (kJournal && (jw = P.run_items[r]) != 0u) {
+    const uint32_t first = blockIdx.x * 8u, n_ctas = (P.n_runs - 1u) / 8u + 1u;
+    const uint32_t before = first + lane < r ? P.run_items[first + lane] : 0u;
+    pos = P.cta[blockIdx.x] + redux_add(before >> kJournalItemsShift);
+    const unsigned long long at = P.cta[n_ctas + blockIdx.x] + redux_add(before & 1u);
+    if (lane == 0 && (jw & 1u) && at < P.runs_cap) P.runs[at] = r;
+  }
+  CommitWrites w;
+  commit_writes(P, lane, c, rec, hold, w, [&](uint32_t LA) {
+    if (!P.arm.tim) return;
+    const uint32_t n_arms = (jw >> kJournalArmsShift) & ((1u << (kJournalItemsShift - kJournalArmsShift)) - 1u);
+    const ArmItems J{kJournal && jw ? P.items : nullptr, pos + (jw >> kJournalItemsShift) - n_arms, P.items_cap};
+    commit_arms(P.arm, r, lane, c.slot, LA & c.SYNC_T, true, armed, J);
+  });
+  const uint32_t dirty = w.dirty;
   uint32_t* ph = reinterpret_cast<uint32_t*>(rec + P.off_phase) + lane;
-  uint32_t p[4] = {0u, 0u, 0u, 0u};
-  if (lane < c.TW)
-    for (uint32_t b = 0; b < 4; ++b) p[b] = ph[b * P.words];
-  const uint32_t keep = c.VALID & ~(p[0] & p[1] & p[2] & p[3]);
-  const uint32_t m0 = p[0] & keep, m1 = p[1] & keep, m2 = p[2] & keep, m3 = p[3] & keep;
-  uint32_t n0 = m0, n1 = m1, n2 = m2, n3 = m3;
-  const uint32_t SK = c.skip, FA = c.fail & ~SK, LA = c.launched & ~SK & ~FA & ~hold, QU = c.queued & ~SK & ~FA & ~c.launched;
-  if (P.arm.tim) commit_arms(P.arm, r, lane, c.slot, LA & c.SYNC_T, true);
-  pset<BF_PHASE_FAILED>(FA, n0, n1, n2, n3);
-  launch_effects(SK, LA, c.T_COND, c.SYNC_T, c.T_PAR, c.T_STOP, n0, n1, n2, n3);
-  pset<BF_PHASE_PENDING_QUEUED>(QU, n0, n1, n2, n3);
-  for (uint32_t i = c.lo; i < c.hi; ++i) {   // the stop steps' phases (a PHASE entry names a launched stop step)
-    const bf_commit_entry e = P.entries[i];
-    const uint32_t bit = 1u << (e.step & 31u);
-    if (e.kind != BF_COMMIT_PHASE || lane != (e.step >> 5u) || !(LA & bit)) continue;
-    n0 = (e.code & 1u) ? n0 | bit : n0 & ~bit;
-    n1 = (e.code & 2u) ? n1 | bit : n1 & ~bit;
-    n2 = (e.code & 4u) ? n2 | bit : n2 & ~bit;
-    n3 = (e.code & 8u) ? n3 | bit : n3 & ~bit;
-  }
-  const uint32_t dirty = (n0 ^ m0) | (n1 ^ m1) | (n2 ^ m2) | (n3 ^ m3);
   if (dirty) {
-    ph[0] = (p[0] & ~dirty) | (n0 & dirty);
-    ph[P.words] = (p[1] & ~dirty) | (n1 & dirty);
-    ph[2u * P.words] = (p[2] & ~dirty) | (n2 & dirty);
-    ph[3u * P.words] = (p[3] & ~dirty) | (n3 & dirty);
+    ph[0] = (w.p[0] & ~dirty) | (w.n0 & dirty);
+    ph[P.words] = (w.p[1] & ~dirty) | (w.n1 & dirty);
+    ph[2u * P.words] = (w.p[2] & ~dirty) | (w.n2 & dirty);
+    ph[3u * P.words] = (w.p[3] & ~dirty) | (w.n3 & dirty);
   }
-  // launched parallel steps register their children (step_executor.go:808-809)
-  const TopoHeader* th = reinterpret_cast<const TopoHeader*>(c.topo);
-  const ParDesc* pd = reinterpret_cast<const ParDesc*>(c.topo + th->off_par);
-  const unsigned long long reg = *reinterpret_cast<const unsigned long long*>(rec + 8);
-  const uint32_t n_par = th->P;
-  uint32_t set[2], reg_only = 0u;
-  for (uint32_t h = 0; h < 2; ++h) {   // BF_MAX_PARALLEL = 64 descs: lane p and lane p + 32
-    const uint32_t q = lane + 32u * h;
-    const uint32_t stp = q < n_par ? pd[q].step : 0u;
-    const uint32_t lw = __shfl_sync(FULL, LA, (stp >> 5) & 31u), dw = __shfl_sync(FULL, dirty, (stp >> 5) & 31u);
-    const bool in = q < n_par && ((lw >> (stp & 31u)) & 1u);
-    set[h] = __ballot_sync(FULL, in);
-    if (in && !((reg >> q) & 1ull) && !((dw >> (stp & 31u)) & 1u)) ++reg_only;   // counted once per step
+  commit_registered(lane, c, rec, w);
+  if (kJournal && jw) {   // PHASE items lane by lane in step order, then REGISTERED items by desc
+    const uint32_t mine = (uint32_t)__popc(dirty);
+    uint32_t incl = mine;
+    for (uint32_t d = 1; d < 32; d <<= 1) {
+      const uint32_t x = __shfl_up_sync(FULL, incl, d);
+      if (lane >= d) incl += x;
+    }
+    unsigned long long at = pos + incl - mine;
+    for (uint32_t x = dirty; x && at < P.items_cap; x &= x - 1u, ++at) {
+      const uint32_t b = (uint32_t)__ffs(x) - 1u;
+      const uint32_t was = ((w.p[0] >> b) & 1u) | ((w.p[1] >> b) & 1u) << 1 | ((w.p[2] >> b) & 1u) << 2 | ((w.p[3] >> b) & 1u) << 3;
+      const uint32_t now = ((w.n0 >> b) & 1u) | ((w.n1 >> b) & 1u) << 1 | ((w.n2 >> b) & 1u) << 2 | ((w.n3 >> b) & 1u) << 3;
+      reinterpret_cast<uint4*>(P.items)[at] = make_uint4(r, (lane * 32u + b) | (uint32_t)BF_DELTA_PHASE << 16, was, now);
+    }
+    const unsigned long long reg_at = pos + __shfl_sync(FULL, incl, 31);
+    for (uint32_t h = 0; h < 2; ++h) {
+      const uint32_t q = lane + 32u * h;
+      if (!((w.newly >> q) & 1ull)) continue;
+      const unsigned long long a = reg_at + __popcll(w.newly & ((1ull << q) - 1ull));
+      if (a < P.items_cap) reinterpret_cast<uint4*>(P.items)[a] = make_uint4(r, q | (uint32_t)BF_DELTA_REGISTERED << 16, 0u, 1u);
+    }
   }
-  const unsigned long long newly = ((unsigned long long)set[1] << 32 | set[0]) & ~reg;
+  const unsigned long long newly = w.newly;
   const uint32_t written = __any_sync(FULL, dirty != 0u) || newly != 0ull;
-  const uint32_t n_skip = redux_add(__popc(dirty & SK)), n_launch = redux_add(__popc(dirty & LA) + reg_only);
-  const uint32_t n_queue = redux_add(__popc(dirty & QU)), n_fail = redux_add(__popc(dirty & FA));
+  const uint32_t n_skip = redux_add(__popc(dirty & w.SK)), n_launch = redux_add(__popc(dirty & w.LA) + w.reg_only);
+  const uint32_t n_queue = redux_add(__popc(dirty & w.QU)), n_fail = redux_add(__popc(dirty & w.FA));
   if (lane == 0 && written) {
-    if (newly) *reinterpret_cast<unsigned long long*>(rec + 8) = reg | newly;
+    if (newly) *reinterpret_cast<unsigned long long*>(rec + 8) = w.reg | newly;
     atomicMax(P.mark + r, P.mark_value);   // max: an upload's "must list" bit stays
     atomicAdd(P.counts, 1u);
     if (n_skip) atomicAdd(P.counts + 1, n_skip);
@@ -1139,10 +1290,19 @@ __global__ void __launch_bounds__(256) commit_apply(const CommitParams P) {
   }
 }
 
+// Without a journal: the check, or the apply.  With one (P.run_items set): the check and the scan, or the apply.
 cudaError_t launch_commit(const CommitParams& P, bool apply, cudaStream_t stream) {
   if (P.n_runs == 0) return cudaSuccess;
-  if (apply) commit_apply<<<(P.n_runs - 1u) / 8u + 1u, 256, 0, stream>>>(P);
-  else commit_check<<<(P.n_runs - 1u) / 8u + 1u, 256, 0, stream>>>(P);
+  const uint32_t grid = (P.n_runs - 1u) / 8u + 1u;
+  if (!P.run_items) {
+    if (apply) commit_apply<false><<<grid, 256, 0, stream>>>(P);
+    else commit_check<false><<<grid, 256, 0, stream>>>(P);
+  } else if (apply) {
+    commit_apply<true><<<grid, 256, 0, stream>>>(P);
+  } else {
+    commit_check<true><<<grid, 256, 0, stream>>>(P);
+    cta_scan<2><<<1, 1024, 0, stream>>>(P.cta, P.total, grid);
+  }
   return cudaGetLastError();
 }
 
@@ -1328,45 +1488,6 @@ __global__ void __launch_bounds__(256, 1) status_runs(const StatusParams P) {
     const uint32_t ph = ((s.p0 >> b) & 1u) | ((s.p1 >> b) & 1u) << 1 | ((s.p2 >> b) & 1u) << 2 | ((s.p3 >> b) & 1u) << 3;
     const uint32_t kind = ((s.FL >> b) & 1u) ? BF_STATUS_EVT_FAILED : BF_STATUS_EVT_ALLOWED;
     if (pos < P.events_cap) P.events[pos] = (uint16_t)((lane * 32u + b) | ph << 10 | kind << 14);
-  }
-}
-
-// One CTA: for each of K arrays of n_ctas per-CTA totals (array k at cta + k * n_ctas), the totals become the sums of the CTAs
-// before each (exclusive scan in place); array k's sum goes to total[k].  bf_resident_status scans its events (K = 1),
-// bf_resident_resync its items and drifted runs (K = 2).
-template <uint32_t K>
-__global__ void __launch_bounds__(1024) cta_scan(unsigned long long* cta, unsigned long long* total, uint32_t n_ctas) {
-  __shared__ unsigned long long s_e[32];
-  const uint32_t lane = threadIdx.x & 31u, warp = threadIdx.x >> 5;
-  for (uint32_t k = 0; k < K; ++k) {
-    unsigned long long* a = cta + (size_t)k * n_ctas;
-    unsigned long long carry = 0;
-    for (uint32_t base = 0; base < n_ctas; base += 1024u) {
-      const uint32_t i = base + threadIdx.x;
-      const unsigned long long e = i < n_ctas ? a[i] : 0ull;
-      unsigned long long ie = e;
-#pragma unroll
-      for (int d = 1; d < 32; d <<= 1) {
-        const unsigned long long b = __shfl_up_sync(FULL, ie, d);
-        if ((int)lane >= d) ie += b;
-      }
-      if (lane == 31) s_e[warp] = ie;
-      __syncthreads();
-      if (warp == 0) {   // the warp totals' inclusive scan
-        unsigned long long we = s_e[lane];
-#pragma unroll
-        for (int d = 1; d < 32; d <<= 1) {
-          const unsigned long long b = __shfl_up_sync(FULL, we, d);
-          if ((int)lane >= d) we += b;
-        }
-        s_e[lane] = we;
-      }
-      __syncthreads();
-      if (i < n_ctas) a[i] = carry + (warp ? s_e[warp - 1] : 0ull) + ie - e;
-      carry += s_e[31];
-      __syncthreads();   // s_e is rewritten by the next chunk
-    }
-    if (threadIdx.x == 0) total[k] = carry;
   }
 }
 

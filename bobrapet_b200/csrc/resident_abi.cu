@@ -59,6 +59,20 @@ struct CallStage {
     const cudaError_t e = cudaMemcpyAsync(c->d_call, image.data(), image.size(), cudaMemcpyHostToDevice, c->stream);
     return e == cudaSuccess ? BF_OK : cuda_fail(c, e, what);
   }
+  // After send(), for out() sections sized from what the call's first launches found: d_call grows to hold them, keeping the
+  // first `kept` bytes (the sections taken before), and every taken pointer is pointed at its section again.  A growth frees
+  // the old scratch, which waits for the device; a scratch already large enough costs nothing.
+  int grow(bf_ctx* c, size_t kept, const char* what) {
+    if (size > c->d_call.cap) {
+      decltype(c->d_call) grown;
+      if (int rc = grown.ensure(c, size)) return rc;
+      const cudaError_t e = cudaMemcpyAsync(grown, c->d_call, kept, cudaMemcpyDeviceToDevice, c->stream);
+      if (e != cudaSuccess) return cuda_fail(c, e, what);
+      c->d_call = std::move(grown);
+    }
+    for (const auto& point : points) point(c->d_call);
+    return BF_OK;
+  }
 };
 
 // Request i names `run` (below cap); each run may be named once.  seen holds request index + 1 per run named so far.
@@ -1207,10 +1221,19 @@ int bf_resident_runctl_download(bf_ctx* c, uint32_t h, uint32_t first, uint32_t 
 // offender, which one D2H copy and one synchronisation bring back before anything is written; then the apply launch and the
 // counts.  A commit that wrote a run changes the state records: it ends the snapshot and the tick a schedule or a commit needs.
 // With `arm` the same launches take the arms too (resident.cu): the timing table is copied up first when a timing changed, and
-// the counts copied back carry the arms' two words.
-int bf_resident_commit_timed(bf_ctx* c, uint32_t h, uint32_t n_runs, const bf_commit_entry* entries, uint32_t n, bf_commit_out* out,
-                             bf_commit_arm* arm) {
+// the counts copied back carry the arms' two words.  With `journal` the check launch also counts each run's items and a scan
+// launch follows it; the totals come back with the offender, so staged items and runs are copied before the second
+// synchronisation.  bf_resident_commit, _timed and _journal are this one call.
+static int resident_commit(bf_ctx* c, uint32_t h, uint32_t n_runs, const bf_commit_entry* entries, uint32_t n, bf_commit_out* out,
+                           bf_commit_arm* arm, bf_commit_journal* journal, bool journaled) {
   auto [g, r] = lock_resident(c, h);
+  if (journaled) {
+    if (!journal || journal->struct_size != sizeof(bf_commit_journal)) return fail(c, BF_EINVAL, "null bf_commit_journal or bad struct_size");
+    if ((journal->items_cap && !journal->items) || (journal->runs_cap && !journal->runs))
+      return fail(c, BF_EINVAL, "null items / runs with a non-zero cap");
+    journal->n_items = 0;
+    journal->n_runs_listed = 0;
+  }
   if (!out || out->struct_size != sizeof(bf_commit_out)) return fail(c, BF_EINVAL, "null bf_commit_out or bad struct_size");
   *out = bf_commit_out{};
   out->struct_size = sizeof(bf_commit_out);
@@ -1273,7 +1296,21 @@ int bf_resident_commit_timed(bf_ctx* c, uint32_t h, uint32_t n_runs, const bf_co
   st.up(P.offender, &no_offender, 1);
   st.up(P.counts, zero_counts, n_counts);
   st.up(P.entries, sorted.data(), n);
+  const uint32_t grid = (n_runs - 1u) / 8u + 1u;
+  bool staged_items = false, staged_runs = false;
+  if (journaled) {   // pinned items / runs are written in place; the others are staged once their numbers are known
+    P.items_cap = journal->items_cap;
+    P.runs_cap = std::min(journal->runs_cap, n_runs);
+    P.items = P.items_cap && reinterpret_cast<uintptr_t>(journal->items) % 16 == 0 ? static_cast<bf_commit_write*>(bf::pinned_dev(journal->items)) : nullptr;
+    P.runs = P.runs_cap ? static_cast<uint32_t*>(bf::pinned_dev(journal->runs)) : nullptr;
+    staged_items = P.items_cap && !P.items;
+    staged_runs = P.runs_cap && !P.runs;
+    st.out(P.run_items, n_runs);
+    st.out(P.cta, 2 * (size_t)grid);
+    st.out(P.total, 2);
+  }
   if (int rc = st.send(c, "bf_resident_commit (check)")) return rc;
+  const size_t sent = st.size;
   if (P.arm.tim) {
     P.arm.timers = r->areas.d_timers; P.arm.timer_k = r->areas.timer_k; P.arm.now = arm->now;
     P.arm.decision = L.off_decision != BF_OFF_NONE; P.arm.out = P.counts + 5;
@@ -1287,8 +1324,9 @@ int bf_resident_commit_timed(bf_ctx* c, uint32_t h, uint32_t n_runs, const bf_co
   uint32_t* host = c->pinned->commit;
   cudaError_t e = bf::launch_commit(P, false, s);
   if (e == cudaSuccess) e = cudaMemcpyAsync(host, P.offender, 8, cudaMemcpyDeviceToHost, s);
+  if (e == cudaSuccess && journaled) e = cudaMemcpyAsync(c->pinned->commit_journal, P.total, 16, cudaMemcpyDeviceToHost, s);
   if (int rc = bf::end_call(c, e, "bf_resident_commit (check)")) return rc;
-  c->stats.kernel_launches += 1;
+  c->stats.kernel_launches += journaled ? 2 : 1;
   uint64_t key;
   memcpy(&key, host, 8);
   if (key != ~0ull) {
@@ -1301,14 +1339,29 @@ int bf_resident_commit_timed(bf_ctx* c, uint32_t h, uint32_t n_runs, const bf_co
                                    : why == bf::kCommitNoPhase   ? "a launched stop step has no BF_COMMIT_PHASE entry"
                                                                  : "a timing that writes needs decision planes (BF_F_DECISION)"));
   }
+  const uint64_t n_items = journaled ? c->pinned->commit_journal[0] : 0;
+  const uint32_t n_listed = journaled ? (uint32_t)c->pinned->commit_journal[1] : 0;
+  if (staged_items || staged_runs) {   // the staging holds what the apply lists and the copies bring back, no more
+    if (staged_items) P.items_cap = std::min<uint64_t>(n_items, P.items_cap);
+    if (staged_runs) P.runs_cap = std::min(n_listed, P.runs_cap);
+    if (staged_items && P.items_cap) st.out(P.items, P.items_cap);
+    if (staged_runs && P.runs_cap) st.out(P.runs, P.runs_cap);
+    if (int rc = st.grow(c, sent, "bf_resident_commit")) return rc;
+    if (P.arm.tim) P.arm.out = P.counts + 5;   // the arms' words behind the counts, where grow() may have moved them
+  }
   e = bf::launch_commit(P, true, s);
   if (e == cudaSuccess) e = cudaMemcpyAsync(host, P.counts, 4 * n_counts, cudaMemcpyDeviceToHost, s);
+  if (const uint64_t k = std::min<uint64_t>(n_items, P.items_cap); e == cudaSuccess && k && staged_items)
+    e = cudaMemcpyAsync(journal->items, P.items, (size_t)k * sizeof(bf_commit_write), cudaMemcpyDeviceToHost, s);
+  if (const uint32_t k = std::min(n_listed, P.runs_cap); e == cudaSuccess && k && staged_runs)
+    e = cudaMemcpyAsync(journal->runs, P.runs, (size_t)k * 4, cudaMemcpyDeviceToHost, s);
   if (int rc = r->sync_in_place(c, e, "bf_resident_commit")) { r->state_changed(c); return rc; }
   c->stats.kernel_launches += 1;
   uint32_t k[7];
   memcpy(k, host, 4 * n_counts);
   out->n_runs_written = k[0]; out->n_skipped = k[1]; out->n_launched = k[2]; out->n_queued = k[3]; out->n_failed = k[4];
   if (arm) { arm->n_armed = k[5]; arm->next_deadline = k[6]; }
+  if (journaled) { journal->n_items = n_items; journal->n_runs_listed = n_listed; }
   if (k[0]) {   // as a delta: the written runs are touched, and the tick a schedule or a commit needs is over
     r->state_changed(c);
     r->pending += k[0];
@@ -1316,8 +1369,18 @@ int bf_resident_commit_timed(bf_ctx* c, uint32_t h, uint32_t n_runs, const bf_co
   return BF_OK;
 }
 
+int bf_resident_commit_journal(bf_ctx* c, uint32_t h, uint32_t n_runs, const bf_commit_entry* entries, uint32_t n, bf_commit_out* out,
+                               bf_commit_arm* arm, bf_commit_journal* journal) {
+  return resident_commit(c, h, n_runs, entries, n, out, arm, journal, true);
+}
+
+int bf_resident_commit_timed(bf_ctx* c, uint32_t h, uint32_t n_runs, const bf_commit_entry* entries, uint32_t n, bf_commit_out* out,
+                             bf_commit_arm* arm) {
+  return resident_commit(c, h, n_runs, entries, n, out, arm, nullptr, false);
+}
+
 int bf_resident_commit(bf_ctx* c, uint32_t h, uint32_t n_runs, const bf_commit_entry* entries, uint32_t n, bf_commit_out* out) {
-  return bf_resident_commit_timed(c, h, n_runs, entries, n, out, nullptr);
+  return resident_commit(c, h, n_runs, entries, n, out, nullptr, nullptr, false);
 }
 
 // ---- run status (resident.cu) ---------------------------------------------------------------------------------------------------

@@ -378,30 +378,47 @@ class Frontier:
     # -- tick commits of a resident batch (bf_resident_commit)
     COMMIT_DTYPE = np.dtype([("run", "<u4"), ("step", "<u2"), ("kind", "u1"), ("code", "u1")])   # bf_commit_entry, 8 B
 
-    def resident_commit(self, handle: int, n_runs: int, entries=None, now: Optional[int] = None) -> dict:
+    COMMIT_WRITE_DTYPE = np.dtype([("run", "<u4"), ("index", "<u2"), ("field", "u1"), ("code", "u1"), ("before", "<u4"),
+                                   ("after", "<u4")])   # bf_commit_write, 16 B
+
+    def resident_commit(self, handle: int, n_runs: int, entries=None, now: Optional[int] = None,
+                        journal_cap: Optional[int] = None) -> dict:
         """bf_resident_commit: write the skips, launches and queue marks of the last tick (and schedule) of runs [0, n_runs)
         into the state records.  entries: COMMIT_DTYPE (or (run, step, kind, code) tuples), at most one per (run, step).
         With `now` (bf_resident_commit_timed) the launched sleep, gate and wait steps with a timing (put_timings) are armed too.
-        -> dict(n_runs_written, n_skipped, n_launched, n_queued, n_failed), with `now` also n_armed and next_deadline.  A
-        refusal raises FrontierError with .bad_run and .bad_step (A.COMMIT_NONE for a refusal of the whole call)"""
+        With journal_cap (bf_resident_commit_journal) the call also lists what it wrote, up to journal_cap items.
+        -> dict(n_runs_written, n_skipped, n_launched, n_queued, n_failed), with `now` also n_armed and next_deadline, with
+        journal_cap also items (COMMIT_WRITE_DTYPE[min(n_items, journal_cap)]), n_items, runs (u32, the runs whose record
+        changed) and n_runs_listed.  A refusal raises FrontierError with .bad_run and .bad_step (A.COMMIT_NONE for a refusal
+        of the whole call)"""
         ents = np.zeros(0, dtype=self.COMMIT_DTYPE) if entries is None else entries
         if not isinstance(ents, np.ndarray):
             ents = np.array([tuple(e) for e in ents], dtype=self.COMMIT_DTYPE)
         ents = np.ascontiguousarray(ents, dtype=self.COMMIT_DTYPE)
         out = A.CommitOut(struct_size=C.sizeof(A.CommitOut))
         ep = ents.ctypes.data if ents.shape[0] else None
-        if now is None:
+        arm = None if now is None else A.CommitArm(struct_size=C.sizeof(A.CommitArm), now=int(now))
+        if journal_cap is not None:
+            items = np.zeros(max(int(journal_cap), 1), dtype=self.COMMIT_WRITE_DTYPE)
+            runs = np.zeros(max(int(n_runs), 1), dtype=np.uint32)
+            j = A.CommitJournal(struct_size=C.sizeof(A.CommitJournal), items=items.ctypes.data if journal_cap else None,
+                                items_cap=int(journal_cap), runs=runs.ctypes.data if n_runs else None, runs_cap=int(n_runs))
+            rc = self._lib.bf_resident_commit_journal(self._ctx, handle, int(n_runs), ep, ents.shape[0], C.byref(out),
+                                                      None if arm is None else C.byref(arm), C.byref(j))
+        elif arm is None:
             rc = self._lib.bf_resident_commit(self._ctx, handle, int(n_runs), ep, ents.shape[0], C.byref(out))
         else:
-            arm = A.CommitArm(struct_size=C.sizeof(A.CommitArm), now=int(now))
             rc = self._lib.bf_resident_commit_timed(self._ctx, handle, int(n_runs), ep, ents.shape[0], C.byref(out), C.byref(arm))
         if rc != A.BF_OK:
             err = A.FrontierError(rc, "bf_resident_commit: %s" % self._lib.bf_last_error(self._ctx).decode())
             err.bad_run, err.bad_step = int(out.bad_run), int(out.bad_step)
             raise err
         got = {k: int(getattr(out, k)) for k in ("n_runs_written", "n_skipped", "n_launched", "n_queued", "n_failed")}
-        if now is not None:
+        if arm is not None:
             got.update(n_armed=int(arm.n_armed), next_deadline=int(arm.next_deadline))
+        if journal_cap is not None:
+            got.update(items=items[:min(int(j.n_items), int(journal_cap))].copy(), n_items=int(j.n_items),
+                       runs=runs[:int(j.n_runs_listed)].copy(), n_runs_listed=int(j.n_runs_listed))
         return got
 
     # -- run status of resident batches (bf_resident_status)

@@ -644,6 +644,105 @@ func (r *Resident) CommitTimed(n, now uint32, entries []CommitEntry) (res Commit
 	return res, uint32(k[7]), uint32(k[8]), r.c.err(rc)
 }
 
+// Fields of a CommitWrite: a step's phase code (BF_DELTA_PHASE), a parallel desc's children_registered bit
+// (BF_DELTA_REGISTERED) or a newly armed step timer (BF_COMMIT_WRITE_TIMER).
+const (
+	CommitWritePhase      = 0
+	CommitWriteRegistered = 5
+	CommitWriteTimer      = 0x10
+)
+
+// CommitWrite is one item of a commit's journal (bf_commit_write, 16 bytes, no pointers): a step whose stored phase code changed
+// (Before: the stored nibble, 15 as stored; After: the code written), a desc whose registered bit was set (0 -> 1), or a timer
+// slot armed for step Index (Code: the armed decision code; Before: TimerNone; After: the deadline).
+type CommitWrite struct {
+	Run         uint32
+	Index       uint16
+	Field, Code uint8
+	Before      uint32
+	After       uint32
+}
+
+// Journal is what CommitJournal wrote.  Items and Runs are the prefixes of the caller's buffers that were filled; NItems and
+// NRuns are the true counts (larger than the buffers when they were too small: the commit itself was applied in full).
+type Journal struct {
+	Items               []CommitWrite
+	NItems              uint64
+	Runs                []uint32 // ascending runs whose record changed: the runs the commit wrote
+	NRuns               uint32
+	Armed, NextDeadline uint32
+}
+
+// CommitJournal is Commit (now == TimerNone) or CommitTimed (any other now) that also lists every write it made, in
+// bf_resident_commit_journal's order (run, then phase, registered and timer items, then index), into items and runs.  The
+// batcher persists these writes to StoryRun.status instead of re-deriving them (GroupWrites builds the per-run PATCH), and
+// takes the runs whose status to read (Status) from Journal.Runs.  A refusal changes nothing and lists nothing.
+func (r *Resident) CommitJournal(n, now uint32, entries []CommitEntry, items []CommitWrite, runs []uint32) (CommitResult, Journal, error) {
+	var ep *C.bf_commit_entry
+	if len(entries) > 0 {
+		ep = (*C.bf_commit_entry)(unsafe.Pointer(&entries[0]))
+	}
+	var ip *C.bf_commit_write
+	if len(items) > 0 {
+		ip = (*C.bf_commit_write)(unsafe.Pointer(&items[0]))
+	}
+	var rp *C.uint32_t
+	if len(runs) > 0 {
+		rp = (*C.uint32_t)(unsafe.Pointer(&runs[0]))
+	}
+	var k [10]C.uint32_t
+	var nItems C.uint64_t
+	rc := C.bfgo_resident_commit_journal(r.c.p, r.handle, C.uint32_t(n), ep, C.uint32_t(len(entries)), C.uint32_t(now), ip,
+		C.uint64_t(len(items)), rp, C.uint32_t(len(runs)), &k[0], &nItems)
+	res := CommitResult{uint32(k[0]), uint32(k[1]), uint32(k[2]), uint32(k[3]), uint32(k[4]), uint32(k[5]), uint32(k[6])}
+	j := Journal{NItems: uint64(nItems), NRuns: uint32(k[9]), Armed: uint32(k[7]), NextDeadline: uint32(k[8])}
+	j.Items = items[:minU64(j.NItems, uint64(len(items)))]
+	j.Runs = runs[:minU64(uint64(j.NRuns), uint64(len(runs)))]
+	return res, j, r.c.err(rc)
+}
+
+func minU64(a, b uint64) uint64 {
+	if a < b {
+		return a
+	}
+	return b
+}
+
+// RunWrites are one run's items of a journal, split by field, each ascending by index: what one StoryRun status PATCH carries.
+// A Phases item whose Before is 0 or 15 (no phase yet) and whose After is not is a step that starts now, and one whose After is
+// terminal a step that finishes now: the StartedAt / FinishedAt that ensureStepStateTimes (step_state.go:25) sets.
+type RunWrites struct {
+	Run        uint32
+	Phases     []CommitWrite
+	Registered []uint16 // parallel descs whose children_registered bit was set
+	Timers     []CommitWrite
+}
+
+// GroupWrites splits a journal's items (ordered by run) into one RunWrites per run, in run order.  The slices share items.
+func GroupWrites(items []CommitWrite) []RunWrites {
+	var out []RunWrites
+	for i := 0; i < len(items); {
+		j := i
+		for j < len(items) && items[j].Run == items[i].Run {
+			j++
+		}
+		w := RunWrites{Run: items[i].Run}
+		for _, it := range items[i:j] {
+			switch it.Field {
+			case CommitWritePhase:
+				w.Phases = append(w.Phases, it)
+			case CommitWriteRegistered:
+				w.Registered = append(w.Registered, it.Index)
+			case CommitWriteTimer:
+				w.Timers = append(w.Timers, it)
+			}
+		}
+		out = append(out, w)
+		i = j
+	}
+	return out
+}
+
 // Outcomes of a StatusRecord (BF_OUTCOME_*) and the kinds of its events (BF_STATUS_EVT_*).
 const (
 	OutcomeNone               = 0 // the run's group is not done

@@ -1144,6 +1144,45 @@ typedef struct bf_commit_arm {
 int bf_resident_commit_timed(bf_ctx* ctx, uint32_t handle, uint32_t n_runs, const bf_commit_entry* entries, uint32_t n_entries,
                              bf_commit_out* out, bf_commit_arm* arm);
 
+/* bf_resident_commit_journal(..., out, arm, journal) is bf_resident_commit_timed (arm = NULL: bf_resident_commit) that also lists
+ * what it wrote, so that a batcher persists the same writes to StepStates (and a host mirror applies them) without a second copy of
+ * the commit's rules.  Checks, refusals, writes, touches, arms and counts are exactly those of the call it extends.  Items
+ * (bf_commit_write), one per changed byte or slot:
+ *   BF_DELTA_PHASE         a step whose stored code changed: before = the stored nibble (15 as stored), after = the code written
+ *   BF_DELTA_REGISTERED    a parallel desc whose children_registered bit the commit set: before = 0, after = 1
+ *   BF_COMMIT_WRITE_TIMER  a timer slot `arm` newly armed: code = the armed code, before = BF_TIMER_NONE, after = the deadline (a
+ *                          kept stored slot is not listed, so these items number arm->n_armed)
+ * ordered by (run, field in that order, index); nothing else is listed: a second commit of the same tick, BF_COMMIT_ERROR runs,
+ * HOLD steps, stopped runs and dead or too-wide slots list nothing.  runs: the ascending runs whose state record changed (the
+ * touched runs; n_runs_listed == out->n_runs_written).  n_items and n_runs_listed are the true counts; only the first items_cap /
+ * runs_cap are written.  A refusal writes nothing and leaves both counts 0.  A NULL journal or a wrong struct_size, and items /
+ * runs NULL with a non-zero cap, are BF_EINVAL before anything else is checked or written.
+ * Cost: the check launch also counts each run's items, one scan launch (as bf_resident_status) turns the counts into offsets, and
+ * the apply launch writes the items there: one launch more than bf_resident_commit_timed and no further synchronisation.  Pinned
+ * buffers (items 16-byte aligned) are written in place; others are staged in the ctx's device scratch, sized after the check
+ * launch to what will be copied (16 B per item of min(n_items, items_cap), 4 B per run of min(n_runs_listed, runs_cap)), and
+ * copied before the final synchronisation.  A scratch that has to grow for them waits for the device once.                  */
+#define BF_COMMIT_WRITE_TIMER 0x10u   /* field of a timer-arm item; PHASE and REGISTERED items use BF_DELTA_PHASE / _REGISTERED       */
+typedef struct bf_commit_write { /* 16 B                                                                                        */
+  uint32_t run;
+  uint16_t index;                /* step (PHASE, TIMER) or parallel desc (REGISTERED)                                           */
+  uint8_t field;                 /* BF_DELTA_PHASE, BF_DELTA_REGISTERED, BF_COMMIT_WRITE_TIMER                                  */
+  uint8_t code;                  /* TIMER: the armed code; else 0                                                               */
+  uint32_t before, after;        /* PHASE: stored nibble / code written; REGISTERED: 0 / 1; TIMER: BF_TIMER_NONE / deadline     */
+} bf_commit_write;
+typedef struct bf_commit_journal {
+  uint32_t struct_size;          /* sizeof(bf_commit_journal)                                                                   */
+  uint32_t reserved;
+  bf_commit_write* items;        /* [items_cap] out                                                                             */
+  uint64_t items_cap;
+  uint64_t n_items;              /* out: the true count; only the first items_cap are written                                   */
+  uint32_t* runs;                /* [runs_cap] out: ascending runs whose record changed                                         */
+  uint32_t runs_cap;
+  uint32_t n_runs_listed;        /* out: the true count, == bf_commit_out.n_runs_written                                        */
+} bf_commit_journal;
+int bf_resident_commit_journal(bf_ctx* ctx, uint32_t handle, uint32_t n_runs, const bf_commit_entry* entries, uint32_t n_entries,
+                               bf_commit_out* out, bf_commit_arm* arm, bf_commit_journal* journal);
+
 /* ------------------------------------------------------------------ run status (what a batcher persists of a run's status)
  * When group selection finds nothing left to run (BF_GROUP_DONE, dag.go:482-495) the reference finalizes the StoryRun
  * (finalizeStoryRun, dag.go:693-754): the failed set of the finally, compensation or main group, in that order, decides its phase

@@ -163,6 +163,15 @@ int bfh_batch_transfer(bfh_batch* src, bfh_batch* dst, const uint32_t* runs, uin
 /* One frontier pass over the batch through bf_eval (or, in resident mode, bf_resident_*) (eval_flags: BF_EVAL_*). */
 int bfh_batch_eval(bfh_batch* b, uint32_t eval_flags, bf_counts* counts);
 
+/* A tick commit in resident mode (see bf_resident_commit), after bfh_batch_eval: bf_resident_commit_journal over the runs of that
+ * eval on the device, whose PHASE and REGISTERED items the mirror applies to its own records.  It logs no delta.  An item whose
+ * (run, field, index) a delta logged since the eval covers is not applied: the next eval applies that delta after the commit on
+ * the device as well, so it wins on both sides.  The journal is sized from the mirror's last results (ready, skip and fail steps
+ * and ready parallel steps), so it is never cut short.  Timers are not armed (the mirror holds no timer area).  After the call
+ * and the next eval the mirror's records equal the device's for every uploaded run.  Not resident: BF_EINVAL.  A refusal
+ * (bad_run / bad_step in out, which may be NULL) changes neither the device nor the mirror.                                 */
+int bfh_batch_commit(bfh_batch* b, const bf_commit_entry* entries, uint32_t n, bf_commit_out* out);
+
 /* Results of the last pass.  Step lists come back in list order (ascending index), the order the
  * concurrency limiters' readySteps[:slots] relies on (dag.go:1796-1798). */
 uint32_t bfh_run_summary(const bfh_batch* b, uint32_t run);
