@@ -1413,8 +1413,9 @@ int bf_resident_status(bf_ctx* c, uint32_t h, uint32_t n_runs, const uint32_t* r
   cudaStream_t s = c->stream;
   if (int rc = bf::sync_slots(c, s)) return rc;
   const uint32_t grid = (n - 1u) / wpb + 1u;
-  // the list is at most n * steps_max long: a larger events_cap stages no more
-  const uint64_t cap = std::min<uint64_t>(out->events_cap, (uint64_t)n * L.steps_max);
+  // the list is at most n * 32 * words long (a run on a topology past steps_max but within the words is live): a larger
+  // events_cap stages no more
+  const uint64_t cap = std::min<uint64_t>(out->events_cap, (uint64_t)n * 32u * L.words);
   bf::StatusParams P{};
   P.runs = runs ? static_cast<const uint32_t*>(bf::pinned_dev(runs)) : nullptr;
   P.records = static_cast<bf_status_rec*>(bf::pinned_dev(out->records));

@@ -430,13 +430,13 @@ class Frontier:
     def resident_status(self, handle: int, n_runs: int, runs=None, events_cap: Optional[int] = None):
         """bf_resident_status: the status of the listed runs (runs: strictly ascending, below n_runs; None: every run of
         [0, n_runs)) after the stage G / H / I rewrites of a single pass, without changing anything.  events_cap: events to
-        fetch (default: every one the runs can have, steps_max of the batch's layout per run).  -> (records STATUS_DTYPE[len(runs)], events u16[min(n_events, events_cap)],
+        fetch (default: every one the runs can have, 32 * words of the batch's layout per run).  -> (records STATUS_DTYPE[len(runs)], events u16[min(n_events, events_cap)],
         n_events)"""
         rl = None if runs is None else np.ascontiguousarray(runs, dtype=np.uint32)
         n = int(n_runs) if rl is None else rl.shape[0]
         recs = np.zeros(n, dtype=self.STATUS_DTYPE)
         if events_cap is None:
-            events_cap = n * self._steps_max[handle]
+            events_cap = n * 32 * ((self._steps_max[handle] + 31) // 32)
         events = np.zeros(max(int(events_cap), 1), dtype=np.uint16)
         out = A.StatusOut(struct_size=C.sizeof(A.StatusOut), records=recs.ctypes.data if n else None,
                           events=events.ctypes.data if events_cap else None, events_cap=int(events_cap))
@@ -551,7 +551,7 @@ class Frontier:
     def resident_create(self, L: A.Layout, capacity: int) -> int:
         h = C.c_uint32()
         self._check(self._lib.bf_resident_create(self._ctx, C.byref(L), capacity, C.byref(h)), "bf_resident_create")
-        self._steps_max[h.value] = int(L.steps_max)   # sizes resident_status's default event buffer
+        self._steps_max[h.value] = int(L.steps_max)   # its words size resident_status's default event buffer
         self._child_nibbles[h.value] = int(L.child_nibbles)   # and, with it, resident_resync's default item buffer
         return h.value
 

@@ -1205,8 +1205,9 @@ int bf_resident_commit_journal(bf_ctx* ctx, uint32_t handle, uint32_t n_runs, co
  *              under allowFailure, as buildStateMaps): finally's -> CLEANUP_FAILED, else compensation's -> COMPENSATION_FAILED, else
  *              main's -> COMPENSATED when the topology has compensation steps, else DEPENDENCY_FAILED; none -> SUCCEEDED.  A run
  *              stopped in the batch's run control (bf_resident_runctl) takes TIMED_OUT, CANCELED or STOPPED from its stop reason
- *              and lists no failed set.  A dead topology slot, or one wider than the layout: DEAD, group and summary 0, counts 0,
- *              no events.
+ *              and lists no failed set.  A dead topology slot, or one wider than the layout (of more words than L.words): DEAD,
+ *              group and summary 0, counts 0, no events.  A topology of more than L.steps_max steps but no more words is live and
+ *              lists events up to 32 * L.words, as many as its steps.
  *   story_phase  the BF_PHASE_* the reference writes for the outcome: SUCCEEDED -> Succeeded (provisional: the host still
  *              evaluates the Story's output template, finalizeSuccessfulRun, dag.go:2871, which can block or fail), the three
  *              failures -> Failed, COMPENSATED -> Compensated, TIMED_OUT -> Timeout (dag.go:566-571), CANCELED -> Finished
@@ -1219,7 +1220,8 @@ int bf_resident_commit_journal(bf_ctx* ctx, uint32_t handle, uint32_t n_runs, co
  *   BF_STATUS_EVT_FAILED    a step of the listed failed set (the failedSteps of status.error)
  *   BF_STATUS_EVT_ALLOWED   a terminal step with allowFailure that is neither Succeeded nor Skipped (collectAllowedFailures),
  *                           in every run that is not dead, finished or not
- * n_events is the true count; only the first events_cap events are written (as bf_compact_out).
+ * n_events is the true count; only the first events_cap events are written (as bf_compact_out); a run has at most
+ * 32 * L.words events.
  * Read-only: no record, result, side area, touch mark or tick state changes, so the call may sit anywhere in the per-tick loop.
  * Refused before any launch with BF_EINVAL and nothing written: struct_size, the handle, n_runs > capacity, runs not strictly
  * ascending or not below n_runs, runs == NULL with n != n_runs, records == NULL with n > 0, events == NULL with events_cap > 0.

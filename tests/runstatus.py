@@ -39,7 +39,8 @@ def status(L, ts, slots, state, n_runs, runs=None, runctl=None, events_cap=None)
     """-> (records STATUS_DTYPE[len(runs)], events u16[min(n_events, events_cap)], n_events) for the listed runs (None: every
     run of [0, n_runs)), as bf_resident_status reports them"""
     runs = np.arange(n_runs, dtype=np.uint32) if runs is None else np.asarray(runs, dtype=np.uint32)
-    L2 = make_layout(L.steps_max, L.child_nibbles, (L.fields & IN_FIELDS) | A.F_OUT_PHASE | A.F_OUT_FAIL)
+    # the width of the layout, not its steps_max: a slot whose S passes steps_max but not 32 * words is live on the device
+    L2 = make_layout(32 * L.words, L.child_nibbles, (L.fields & IN_FIELDS) | A.F_OUT_PHASE | A.F_OUT_FAIL)
     assert L2.state_stride == L.state_stride
     info = {}   # slot -> (S, allowFailure, group per step, n_comp)
     s0 = 0
@@ -49,7 +50,7 @@ def status(L, ts, slots, state, n_runs, runs=None, runctl=None, events_cap=None)
         g = (fl >> A.SF_GROUP_SHIFT) & 3
         info[int(slots[i])] = (S, (fl & A.SF_ALLOW_FAILURE) != 0, g, int((g == 1).sum()))
         s0 += S
-    # dead: a slot no topology holds, or one wider than the layout (the oracle refuses both; the device reports them DEAD)
+    # dead: a slot no topology holds, or one of more words than the layout (the oracle refuses both; the device reports them DEAD)
     slot_of = [int(state[r][:4].view("<u4")[0]) for r in runs]
     alive = [k for k, sl in enumerate(slot_of) if sl in info and (info[sl][0] + 31) // 32 <= L.words]
     res = np.zeros((runs.size, L2.result_stride), np.uint8)
