@@ -202,6 +202,7 @@ class CommitArm(C.Structure):
 
 
 COMMIT_WRITE_TIMER = 0x10   # BF_COMMIT_WRITE_TIMER: bf_commit_write.field of a timer-arm item (else DELTA_PHASE / DELTA_REGISTERED)
+COMMIT_WRITE_REWRITE = 0x1   # BF_COMMIT_WRITE_REWRITE: bf_commit_write.code of a PHASE item whose code comes from stages G / H / I
 
 
 class CommitJournal(C.Structure):
@@ -296,6 +297,8 @@ SYMBOLS = [
                                            C.POINTER(CommitArm)]),
     ("bf_resident_commit_journal", C.c_int, [C.c_void_p, C.c_uint32, C.c_uint32, C.c_void_p, C.c_uint32, C.POINTER(CommitOut),
                                              C.POINTER(CommitArm), C.POINTER(CommitJournal)]),
+    ("bf_resident_commit_rewrites", C.c_int, [C.c_void_p, C.c_uint32, C.c_uint32, C.c_void_p, C.c_uint32, C.POINTER(CommitOut),
+                                              C.POINTER(CommitArm), C.POINTER(CommitJournal), C.POINTER(C.c_uint32)]),
     ("bf_resident_status", C.c_int, [C.c_void_p, C.c_uint32, C.c_uint32, C.c_void_p, C.c_uint32, C.POINTER(StatusOut)]),
     ("bf_resident_resync", C.c_int, [C.c_void_p, C.c_uint32, C.POINTER(Resync)]),
     ("bf_group_create", C.c_int, [C.POINTER(C.c_void_p), C.POINTER(C.c_int32), C.c_uint32, C.POINTER(Config)]),

@@ -49,6 +49,7 @@ cudaError_t launch_runctl_put(const RunCtlPutParams& P, cudaStream_t stream);
 cudaError_t launch_runctl_restop(const RunCtlRestopParams& P, cudaStream_t stream);
 cudaError_t launch_commit(const CommitParams& P, bool apply, cudaStream_t stream);
 cudaError_t launch_status(const StatusParams& P, uint32_t smem_bytes, cudaStream_t stream);
+cudaError_t launch_rewrites(const RewriteParams& P, uint32_t smem_bytes, cudaStream_t stream);
 cudaError_t launch_resync(const ResyncParams& P, uint32_t smem_bytes, cudaStream_t stream);
 cudaError_t launch_closure(const Slot* slots, const uint32_t* slot_ids, const uint32_t* starts, uint32_t n, uint32_t n_slots,
                            uint32_t words_out, uint32_t* masks, cudaStream_t stream);

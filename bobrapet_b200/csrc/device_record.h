@@ -501,9 +501,31 @@ struct CommitParams {
   unsigned long long items_cap;
   uint32_t* runs;                // [runs_cap]
   uint32_t runs_cap;
+  // bf_resident_commit_rewrites (the rewriting builds of both launches): the writes of a run flagged in rw_runs start from its
+  // codes after the stages G / H / I of a single pass, which rewrite_runs left in rw_planes; commit_apply adds the steps written
+  // from them (no mask bit) to *rewritten
+  const uint32_t* rw_runs;       // [n_runs] 1: the stages rewrote a code of the run, 0: its stored codes are the base
+  const uint32_t* rw_planes;     // [n_runs][4][words] the phase planes after the stages (flagged runs only)
+  uint32_t* rewritten;           // [1] steps written from the stages (zeroed by the caller)
 };
 static_assert(sizeof(bf_commit_write) == 16, "bf_commit_write must be 16 bytes");
 constexpr uint32_t kJournalArmsShift = 1, kJournalItemsShift = 8;   // new arms <= BF_TIMER_MAX_SLOTS < 128
+
+// bf_resident_commit_rewrites (resident.cu): rewrite_runs, one warp per run of [0, n_runs) and the shared stage of StatusParams,
+// takes a run through the stages of a single pass when its current result record carries BF_SUM_PHASE_CHANGED, it is not stopped
+// and its slot is live and fits the layout; a run whose codes the stages changed is flagged in rw_runs and its planes stored in
+// rw_planes, every other run is flagged 0.
+struct RewriteParams {
+  const uint8_t* state;
+  const uint8_t* result;            // the current result records (their summary word)
+  const Slot* slots;
+  uint32_t n_slots;
+  const bf_run_ctl* runctl;         // or nullptr: no run is stopped
+  uint32_t n_runs, warps_per_block;
+  uint32_t words, state_stride, off_phase, off_decision, off_child, topo_bytes, result_stride;
+  uint32_t* rw_runs;                // [n_runs]
+  uint32_t* rw_planes;              // [n_runs][4][words]
+};
 
 // bf_resident_status (resident.cu): one warp per listed run.  status_count stores each listed run's event count and each CTA's
 // total, cta_scan turns the CTA totals into the events of the CTAs before each and posts the sum, status_list writes the

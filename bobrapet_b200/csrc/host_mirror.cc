@@ -564,17 +564,22 @@ int bfh_run_set_child_phase(bfh_batch* b, uint32_t run, uint32_t q, uint32_t bra
 // The device writes the commit (bf_resident_commit_journal) and the mirror applies the PHASE and REGISTERED items of its journal,
 // so that the commit's rules live only in the kernel.  An item whose (run, field, index) a pending delta covers is skipped: the
 // next eval applies that delta after the commit, on the device too.  The journal is sized from the last results: a run lists at
-// most its ready, skip and fail steps and its ready parallel steps' descs.
-int bfh_batch_commit(bfh_batch* b, const bf_commit_entry* entries, uint32_t n, bf_commit_out* out) {
+// most its ready, skip and fail steps and its ready parallel steps' descs.  With rewrites (bfh_batch_commit_rewrites) a run whose
+// result carries BF_SUM_PHASE_CHANGED may list a PHASE item for any step of its Story instead.
+static int mirror_commit(bfh_batch* b, const bf_commit_entry* entries, uint32_t n, bf_commit_out* out, uint32_t* n_rewritten,
+                         bool rewrites, const char* what) {
   if (!b) return BF_EINVAL;
-  if (!b->resident) { b->err = "bfh_batch_commit needs resident mode"; return BF_EINVAL; }
+  if (!b->resident) { b->err = std::string(what) + " needs resident mode"; return BF_EINVAL; }
   const bf_layout& L = b->L;
   const uint32_t runs = b->evaluated;
   uint64_t cap = 0;
   for (uint32_t r = 0; r < runs; ++r) {
     const uint8_t* res = b->rec.result + (size_t)r * L.result_stride;
     auto word = [&](uint32_t off, uint32_t w) { return off == BF_OFF_NONE ? 0u : reinterpret_cast<const uint32_t*>(res + off)[w]; };
-    for (uint32_t w = 0; w < L.words; ++w) cap += (uint64_t)__builtin_popcount(word(L.off_ready, w) | word(L.off_skip, w) | word(L.off_fail, w));
+    const bool rewriting = rewrites && (reinterpret_cast<const bf_result_header*>(res)->summary & BF_SUM_PHASE_CHANGED);
+    if (rewriting) cap += 32ull * L.words;
+    else
+      for (uint32_t w = 0; w < L.words; ++w) cap += (uint64_t)__builtin_popcount(word(L.off_ready, w) | word(L.off_skip, w) | word(L.off_fail, w));
     for (const bf_parallel_desc& d : b->story_of_run[r]->par) cap += (word(L.off_ready, d.step >> 5) >> (d.step & 31u)) & 1u;
   }
   std::vector<bf_commit_write> items(cap);
@@ -583,12 +588,15 @@ int bfh_batch_commit(bfh_batch* b, const bf_commit_entry* entries, uint32_t n, b
   bf_commit_journal j{};
   j.struct_size = sizeof j;
   j.items = items.data(); j.items_cap = cap;
-  const int rc = bf_resident_commit_journal(b->ctx, b->handle, runs, entries, n, &o, nullptr, &j);
+  uint32_t nrw = 0;
+  const int rc = rewrites ? bf_resident_commit_rewrites(b->ctx, b->handle, runs, entries, n, &o, nullptr, &j, &nrw)
+                          : bf_resident_commit_journal(b->ctx, b->handle, runs, entries, n, &o, nullptr, &j);
   if (out) *out = o;
+  if (n_rewritten) *n_rewritten = nrw;
   if (rc != BF_OK) { b->err = bf_last_error(b->ctx); return rc; }
   // cap bounds the journal: the commit reads the result records this mirror holds (the last eval's), the mirror's batch has no
   // limiter area (launched = ready, nothing queued) and the call arms nothing, so every PHASE item is a ready, skip or fail step
-  // and every REGISTERED item the desc of a ready parallel step
+  // (any step of a rewriting run) and every REGISTERED item the desc of a ready parallel step
   assert(j.n_items <= cap);
   for (uint64_t i = 0; i < std::min<uint64_t>(j.n_items, cap); ++i) {
     const bf_commit_write& w = items[i];
@@ -598,6 +606,14 @@ int bfh_batch_commit(bfh_batch* b, const bf_commit_entry* entries, uint32_t n, b
     else if (w.field == BF_DELTA_REGISTERED) reinterpret_cast<bf_run_header*>(rec)->children_registered |= 1ull << w.index;
   }
   return BF_OK;
+}
+
+int bfh_batch_commit(bfh_batch* b, const bf_commit_entry* entries, uint32_t n, bf_commit_out* out) {
+  return mirror_commit(b, entries, n, out, nullptr, false, "bfh_batch_commit");
+}
+
+int bfh_batch_commit_rewrites(bfh_batch* b, const bf_commit_entry* entries, uint32_t n, bf_commit_out* out, uint32_t* n_rewritten) {
+  return mirror_commit(b, entries, n, out, n_rewritten, true, "bfh_batch_commit_rewrites");
 }
 
 int bfh_batch_eval(bfh_batch* b, uint32_t eval_flags, bf_counts* counts) {

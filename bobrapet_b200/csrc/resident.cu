@@ -953,7 +953,7 @@ __global__ void __launch_bounds__(1024) cta_scan(unsigned long long* cta, unsign
 // ---- tick commits (bf_resident_commit*) -------------------------------------------------------------------------------------
 // One warp per run; lane w holds word w of the run's masks and codes (words <= 32).  Both launches read a run the same way: its
 // topology's step types, the masks of its current result record (and of its schedule record), and its entries [lo, hi), found by
-// a binary search every lane runs alike.  A run with no mask bit and no entry leaves at once.
+// a binary search every lane runs alike.  A run with no mask bit, no entry and (kRewrite) no rewrite leaves at once.
 struct CommitRun {
   const uint8_t* topo;          // nullptr: dead slot, or a topology wider than the layout (no masks)
   uint32_t TW, VALID;
@@ -962,6 +962,7 @@ struct CommitRun {
   uint32_t lo, hi, slot;
 };
 
+template <bool kRewrite>
 DI bool commit_run(const CommitParams& P, uint32_t r, uint32_t lane, CommitRun& c) {
   const uint32_t slot = c.slot = *reinterpret_cast<const uint32_t*>(P.state + (size_t)r * P.state_stride);
   const Slot sl = slot < P.n_slots ? P.slots[slot] : Slot{};
@@ -994,7 +995,7 @@ DI bool commit_run(const CommitParams& P, uint32_t r, uint32_t lane, CommitRun& 
   c.lo = a; b = P.n_entries;
   while (a < b) { const uint32_t m = (a + b) >> 1; if (P.entries[m].run <= r) a = m + 1u; else b = m; }
   c.hi = a;
-  return __any_sync(FULL, (c.launched | c.queued | c.skip | c.fail) != 0u) || c.lo != c.hi;
+  return __any_sync(FULL, (c.launched | c.queued | c.skip | c.fail) != 0u) || c.lo != c.hi || (kRewrite && P.rw_runs[r]);
 }
 
 // The entries of a run: lane w collects the HOLD and PHASE bits of its word; err: the run has an ERROR entry.  With check, the
@@ -1101,16 +1102,18 @@ DI unsigned long long commit_arms(const CommitTimings& A, uint32_t r, uint32_t l
 // stored planes p, new codes n and the steps whose code changes (dirty), and the disjoint masks; commit_registered adds the
 // registered bits newly set (lanes p and p + 32 look at the launched parallel descs; reg_only counts the steps whose bit alone
 // changes).  commit_apply stores them; commit_check<true> counts them, so that both launches agree on every item.  between(LA)
-// runs once the masks are known (commit_apply arms there).
+// runs once the masks are known (commit_apply arms there).  With kRewrite the masks write over the base codes rewrite_runs left
+// for run r when it flagged it (the codes after a single pass's stages), else over the stored codes; dirty stays the steps whose
+// stored code changes.
 struct CommitWrites {
   uint32_t p[4], n0, n1, n2, n3, dirty;
   uint32_t SK, FA, LA, QU;
   unsigned long long reg, newly;
   uint32_t reg_only;
 };
-template <typename Between>
-DI void commit_writes(const CommitParams& P, uint32_t lane, const CommitRun& c, const uint8_t* rec, uint32_t hold, CommitWrites& w,
-                      Between between) {
+template <bool kRewrite, typename Between>
+DI void commit_writes(const CommitParams& P, uint32_t r, uint32_t lane, const CommitRun& c, const uint8_t* rec, uint32_t hold,
+                      CommitWrites& w, Between between) {
   const uint32_t* ph = reinterpret_cast<const uint32_t*>(rec + P.off_phase) + lane;
   for (uint32_t b = 0; b < 4; ++b) w.p[b] = 0u;
   if (lane < c.TW)
@@ -1118,6 +1121,10 @@ DI void commit_writes(const CommitParams& P, uint32_t lane, const CommitRun& c, 
   const uint32_t keep = c.VALID & ~(w.p[0] & w.p[1] & w.p[2] & w.p[3]);
   const uint32_t m0 = w.p[0] & keep, m1 = w.p[1] & keep, m2 = w.p[2] & keep, m3 = w.p[3] & keep;
   uint32_t n0 = m0, n1 = m1, n2 = m2, n3 = m3;
+  if (kRewrite && P.rw_runs[r] && lane < c.TW) {   // warp-uniform flag
+    const uint32_t* b = P.rw_planes + (size_t)r * 4u * P.words + lane;
+    n0 = b[0]; n1 = b[P.words]; n2 = b[2u * P.words]; n3 = b[3u * P.words];
+  }
   w.SK = c.skip; w.FA = c.fail & ~w.SK; w.LA = c.launched & ~w.SK & ~w.FA & ~hold; w.QU = c.queued & ~w.SK & ~w.FA & ~c.launched;
   between(w.LA);
   pset<BF_PHASE_FAILED>(w.FA, n0, n1, n2, n3);
@@ -1156,10 +1163,10 @@ DI void commit_registered(uint32_t lane, const CommitRun& c, const uint8_t* rec,
 
 // The per-run part of commit_check: lane 0 lowers P.offender to the run's first offence.  -> with kJournal, the run's journal
 // word (its items, new arms and whether its record changes; 0 for a run that writes nothing), else 0.
-template <bool kJournal>
+template <bool kJournal, bool kRewrite>
 DI uint32_t check_run(const CommitParams& P, uint32_t r, uint32_t lane) {
   CommitRun c;
-  if (!commit_run(P, r, lane, c)) return 0u;
+  if (!commit_run<kRewrite>(P, r, lane, c)) return 0u;
   uint32_t hold, phased;
   bool err;
   unsigned long long bad = commit_entries(P, r, lane, c, true, hold, phased, err);
@@ -1180,7 +1187,7 @@ DI uint32_t check_run(const CommitParams& P, uint32_t r, uint32_t lane) {
   if (!kJournal || !c.topo) return 0u;   // a dead or too-wide slot has no masks: it writes nothing (an entry on it is refused)
   const uint8_t* rec = P.state + (size_t)r * P.state_stride;
   CommitWrites w;
-  commit_writes(P, lane, c, rec, hold, w, [](uint32_t) {});
+  commit_writes<kRewrite>(P, r, lane, c, rec, hold, w, [](uint32_t) {});
   commit_registered(lane, c, rec, w);
   const uint32_t items = redux_add(__popc(w.dirty)) + __popcll(w.newly) + armed;
   const bool written = __any_sync(FULL, w.dirty != 0u) || w.newly != 0ull;
@@ -1189,16 +1196,17 @@ DI uint32_t check_run(const CommitParams& P, uint32_t r, uint32_t lane) {
 
 // Check: every entry names a launched step (a PHASE entry a stop step), and every launched stop step of a run without an ERROR
 // entry has a HOLD or PHASE entry; with a timing table, the arming offences too.  Lane 0 lowers P.offender to the run's first
-// offence.  Nothing is written but, with kJournal, each run's journal word and each CTA's items and written runs.
-template <bool kJournal>
-__global__ void __launch_bounds__(256) commit_check(const CommitParams P) {
+// offence.  Nothing is written but, with kJournal, each run's journal word and each CTA's items and written runs.  The kernels
+// commit_check (kRewrite = false) and commit_check_rewrites (both true) are this body.
+template <bool kJournal, bool kRewrite>
+DI void commit_check_body(const CommitParams& P) {
   const uint32_t r = blockIdx.x * 8u + (threadIdx.x >> 5), lane = threadIdx.x & 31u;
   if (!kJournal) {
-    if (r < P.n_runs) check_run<false>(P, r, lane);
+    if (r < P.n_runs) check_run<false, kRewrite>(P, r, lane);
     return;
   }
   __shared__ uint32_t warp_word[8];
-  const uint32_t jw = r < P.n_runs ? check_run<true>(P, r, lane) : 0u;
+  const uint32_t jw = r < P.n_runs ? check_run<true, kRewrite>(P, r, lane) : 0u;
   if (lane == 0) {
     warp_word[threadIdx.x >> 5] = jw;
     if (r < P.n_runs) P.run_items[r] = jw;
@@ -1212,17 +1220,22 @@ __global__ void __launch_bounds__(256) commit_check(const CommitParams P) {
     P.cta[n_ctas + blockIdx.x] = written;
   }
 }
+template <bool kJournal>
+__global__ void __launch_bounds__(256) commit_check(const CommitParams P) { commit_check_body<kJournal, false>(P); }
+__global__ void __launch_bounds__(256) commit_check_rewrites(const CommitParams P) { commit_check_body<true, true>(P); }
 
 // Apply (after a check that found no offender): the writes of commit_writes, stored only where a code changed; the registered
 // bits of launched parallel descs; with a timing table, the arms of the launched sleep / gate / wait steps.  With kJournal each
 // run with a journal word lists its items (PHASE by step, REGISTERED by desc, TIMER by step) from the offset of the CTAs before
-// and the warps before in its CTA, and its entry in runs when its record changed.
-template <bool kJournal>
-__global__ void __launch_bounds__(256) commit_apply(const CommitParams P) {
+// and the warps before in its CTA, and its entry in runs when its record changed.  With kRewrite a PHASE item of a step without
+// a mask bit (its code comes from the stages) carries BF_COMMIT_WRITE_REWRITE, and those steps are added to *P.rewritten.  The
+// kernels commit_apply (kRewrite = false) and commit_apply_rewrites (both true) are this body.
+template <bool kJournal, bool kRewrite>
+DI void commit_apply_body(const CommitParams& P) {
   const uint32_t r = blockIdx.x * 8u + (threadIdx.x >> 5), lane = threadIdx.x & 31u;
   if (r >= P.n_runs) return;
   CommitRun c;
-  if (!commit_run(P, r, lane, c)) return;
+  if (!commit_run<kRewrite>(P, r, lane, c)) return;
   uint32_t hold, phased;
   bool err;
   commit_entries(P, r, lane, c, false, hold, phased, err);
@@ -1238,7 +1251,7 @@ __global__ void __launch_bounds__(256) commit_apply(const CommitParams P) {
     if (lane == 0 && (jw & 1u) && at < P.runs_cap) P.runs[at] = r;
   }
   CommitWrites w;
-  commit_writes(P, lane, c, rec, hold, w, [&](uint32_t LA) {
+  commit_writes<kRewrite>(P, r, lane, c, rec, hold, w, [&](uint32_t LA) {
     if (!P.arm.tim) return;
     const uint32_t n_arms = (jw >> kJournalArmsShift) & ((1u << (kJournalItemsShift - kJournalArmsShift)) - 1u);
     const ArmItems J{kJournal && jw ? P.items : nullptr, pos + (jw >> kJournalItemsShift) - n_arms, P.items_cap};
@@ -1261,11 +1274,13 @@ __global__ void __launch_bounds__(256) commit_apply(const CommitParams P) {
       if (lane >= d) incl += x;
     }
     unsigned long long at = pos + incl - mine;
+    const uint32_t staged = kRewrite ? ~(w.SK | w.FA | w.LA | w.QU) : 0u;
     for (uint32_t x = dirty; x && at < P.items_cap; x &= x - 1u, ++at) {
       const uint32_t b = (uint32_t)__ffs(x) - 1u;
       const uint32_t was = ((w.p[0] >> b) & 1u) | ((w.p[1] >> b) & 1u) << 1 | ((w.p[2] >> b) & 1u) << 2 | ((w.p[3] >> b) & 1u) << 3;
       const uint32_t now = ((w.n0 >> b) & 1u) | ((w.n1 >> b) & 1u) << 1 | ((w.n2 >> b) & 1u) << 2 | ((w.n3 >> b) & 1u) << 3;
-      reinterpret_cast<uint4*>(P.items)[at] = make_uint4(r, (lane * 32u + b) | (uint32_t)BF_DELTA_PHASE << 16, was, now);
+      const uint32_t code = ((staged >> b) & 1u) ? BF_COMMIT_WRITE_REWRITE << 24 : 0u;
+      reinterpret_cast<uint4*>(P.items)[at] = make_uint4(r, (lane * 32u + b) | (uint32_t)BF_DELTA_PHASE << 16 | code, was, now);
     }
     const unsigned long long reg_at = pos + __shfl_sync(FULL, incl, 31);
     for (uint32_t h = 0; h < 2; ++h) {
@@ -1288,9 +1303,17 @@ __global__ void __launch_bounds__(256) commit_apply(const CommitParams P) {
     if (n_queue) atomicAdd(P.counts + 3, n_queue);
     if (n_fail) atomicAdd(P.counts + 4, n_fail);
   }
+  if (kRewrite) {
+    const uint32_t n_rw = redux_add(__popc(dirty & ~(w.SK | w.FA | w.LA | w.QU)));
+    if (lane == 0 && n_rw) atomicAdd(P.rewritten, n_rw);
+  }
 }
+template <bool kJournal>
+__global__ void __launch_bounds__(256) commit_apply(const CommitParams P) { commit_apply_body<kJournal, false>(P); }
+__global__ void __launch_bounds__(256) commit_apply_rewrites(const CommitParams P) { commit_apply_body<true, true>(P); }
 
-// Without a journal: the check, or the apply.  With one (P.run_items set): the check and the scan, or the apply.
+// Without a journal: the check, or the apply.  With one (P.run_items set): the check and the scan, or the apply; with P.rw_runs
+// set (after rewrite_runs) their rewriting builds.
 cudaError_t launch_commit(const CommitParams& P, bool apply, cudaStream_t stream) {
   if (P.n_runs == 0) return cudaSuccess;
   const uint32_t grid = (P.n_runs - 1u) / 8u + 1u;
@@ -1298,9 +1321,11 @@ cudaError_t launch_commit(const CommitParams& P, bool apply, cudaStream_t stream
     if (apply) commit_apply<false><<<grid, 256, 0, stream>>>(P);
     else commit_check<false><<<grid, 256, 0, stream>>>(P);
   } else if (apply) {
-    commit_apply<true><<<grid, 256, 0, stream>>>(P);
+    if (P.rw_runs) commit_apply_rewrites<<<grid, 256, 0, stream>>>(P);
+    else commit_apply<true><<<grid, 256, 0, stream>>>(P);
   } else {
-    commit_check<true><<<grid, 256, 0, stream>>>(P);
+    if (P.rw_runs) commit_check_rewrites<<<grid, 256, 0, stream>>>(P);
+    else commit_check<true><<<grid, 256, 0, stream>>>(P);
     cta_scan<2><<<1, 1024, 0, stream>>>(P.cta, P.total, grid);
   }
   return cudaGetLastError();
@@ -1502,6 +1527,54 @@ cudaError_t launch_status(const StatusParams& P, uint32_t smem_bytes, cudaStream
   status_runs<false><<<grid, threads, smem_bytes, stream>>>(P);
   cta_scan<1><<<1, 1024, 0, stream>>>(P.cta_events, P.total, grid);
   status_runs<true><<<grid, threads, smem_bytes, stream>>>(P);
+  return cudaGetLastError();
+}
+
+// ---- rewrites of a single pass (bf_resident_commit_rewrites) ------------------------------------------------------------------
+// One warp per run of [0, n_runs), the shared stage of status_runs.  Only a run whose pass rewrote a phase (BF_SUM_PHASE_CHANGED in
+// its current result record, which the pass that left it derived from the same codes) can have a rewrite; a stopped run, a dead
+// slot and a slot wider than the layout have none.  Such a run takes single_pass (stages H, G and I, no stage-D cond FAIL), and is
+// flagged with its planes stored when a code (15 read as 0) changed.
+__global__ void __launch_bounds__(256, 1) rewrite_runs(const RewriteParams P) {
+  extern __shared__ __align__(16) uint8_t rewrite_stage[];
+  const uint32_t warp = threadIdx.x >> 5, lane = threadIdx.x & 31u;
+  const uint32_t r = blockIdx.x * P.warps_per_block + warp;
+  if (r >= P.n_runs) return;
+  const uint32_t stage_a = smem_u32(rewrite_stage) + warp * (P.off_child != BF_OFF_NONE ? P.state_stride + P.topo_bytes + 256u : 0u);
+  const uint8_t* rec = P.state + (size_t)r * P.state_stride;
+  const uint32_t summary = *reinterpret_cast<const uint32_t*>(P.result + (size_t)r * P.result_stride);
+  const uint32_t slot = *reinterpret_cast<const uint32_t*>(rec);
+  const uint8_t* topo = slot < P.n_slots ? reinterpret_cast<const uint8_t*>(P.slots[slot].addr) : nullptr;
+  const TopoHeader th = topo ? *reinterpret_cast<const TopoHeader*>(topo) : TopoHeader{};
+  const bool stopped = P.runctl && P.runctl[r].stop != BF_STOP_NONE;
+  uint32_t changed = 0u;
+  if ((summary & BF_SUM_PHASE_CHANGED) && th.W - 1u < P.words && !stopped) {   // warp-uniform
+    const bool act = lane < th.W;
+    const PassTopo T = pass_topo(topo, th, lane, act);
+    uint32_t p0 = 0, p1 = 0, p2 = 0, p3 = 0, d0 = 0, d1 = 0;
+    if (act) {
+      load_phases(rec, P.off_phase, P.words, lane, T.VALID, p0, p1, p2, p3);
+      if (P.off_decision != BF_OFF_NONE) load_codes2(rec, P.off_decision, P.words, lane, ~0u, d0, d1);
+    }
+    const uint32_t m0 = p0, m1 = p1, m2 = p2, m3 = p3;
+    single_pass(P, lane, act, th, topo, T, rec[4], rec, nullptr, 0u, stage_a, d0, d1, p0, p1, p2, p3);
+    changed = __any_sync(FULL, ((p0 ^ m0) | (p1 ^ m1) | (p2 ^ m2) | (p3 ^ m3)) != 0u) ? 1u : 0u;
+    if (changed && lane < P.words) {
+      uint32_t* b = P.rw_planes + (size_t)r * 4u * P.words + lane;
+      b[0] = p0; b[P.words] = p1; b[2u * P.words] = p2; b[3u * P.words] = p3;
+    }
+  }
+  if (lane == 0) P.rw_runs[r] = changed;
+}
+
+cudaError_t launch_rewrites(const RewriteParams& P, uint32_t smem_bytes, cudaStream_t stream) {
+  if (P.n_runs == 0) return cudaSuccess;
+  if (smem_bytes > 48u * 1024u) {
+    const cudaError_t e = cudaFuncSetAttribute(rewrite_runs, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes);
+    if (e != cudaSuccess) return e;
+  }
+  const uint32_t grid = (P.n_runs - 1u) / P.warps_per_block + 1u;
+  rewrite_runs<<<grid, 32u * P.warps_per_block, smem_bytes, stream>>>(P);
   return cudaGetLastError();
 }
 

@@ -1223,10 +1223,17 @@ int bf_resident_runctl_download(bf_ctx* c, uint32_t h, uint32_t first, uint32_t 
 // With `arm` the same launches take the arms too (resident.cu): the timing table is copied up first when a timing changed, and
 // the counts copied back carry the arms' two words.  With `journal` the check launch also counts each run's items and a scan
 // launch follows it; the totals come back with the offender, so staged items and runs are copied before the second
-// synchronisation.  bf_resident_commit, _timed and _journal are this one call.
+// synchronisation.  With `rewritten` (bf_resident_commit_rewrites, journaled) rewrite_runs runs before the check launch: the
+// staged planes are taken with the call's other sections, so the apply after a growth still finds them.  bf_resident_commit,
+// _timed, _journal and _rewrites are this one call.
 static int resident_commit(bf_ctx* c, uint32_t h, uint32_t n_runs, const bf_commit_entry* entries, uint32_t n, bf_commit_out* out,
-                           bf_commit_arm* arm, bf_commit_journal* journal, bool journaled) {
+                           bf_commit_arm* arm, bf_commit_journal* journal, bool journaled, uint32_t* rewritten = nullptr,
+                           bool rewrites = false) {
   auto [g, r] = lock_resident(c, h);
+  if (rewrites) {
+    if (!rewritten) return fail(c, BF_EINVAL, "null n_rewritten");
+    *rewritten = 0;
+  }
   if (journaled) {
     if (!journal || journal->struct_size != sizeof(bf_commit_journal)) return fail(c, BF_EINVAL, "null bf_commit_journal or bad struct_size");
     if ((journal->items_cap && !journal->items) || (journal->runs_cap && !journal->runs))
@@ -1288,8 +1295,9 @@ static int resident_commit(bf_ctx* c, uint32_t h, uint32_t n_runs, const bf_comm
   for (uint32_t i = 0; i < n; ++i) sorted[i] = entries[order[i]];
   bf::CommitParams P{};
   const unsigned long long no_offender = ~0ull;
-  const uint32_t zero_counts[7] = {0u, 0u, 0u, 0u, 0u, 0u, BF_TIMER_NONE};   // the five counts, then the arms' count and deadline
-  const uint32_t n_counts = arm ? 7u : 5u;
+  // the five counts, then the arms' count and deadline, then the steps written from the stages
+  const uint32_t zero_counts[8] = {0u, 0u, 0u, 0u, 0u, 0u, BF_TIMER_NONE, 0u};
+  const uint32_t n_counts = rewrites ? 8u : arm ? 7u : 5u;
   if (arm)
     if (int rc = bf::sync_timings(c, s, P.arm)) return rc;
   CallStage st;
@@ -1309,6 +1317,18 @@ static int resident_commit(bf_ctx* c, uint32_t h, uint32_t n_runs, const bf_comm
     st.out(P.cta, 2 * (size_t)grid);
     st.out(P.total, 2);
   }
+  bf::RewriteParams W{};
+  uint32_t rw_wpb = 8, rw_topo = 0, rw_per_warp = 0;
+  if (rewrites) {   // the shared stage of bf_resident_status per warp for the joins
+    if (L.off_child != BF_OFF_NONE) {
+      rw_topo = bf::largest_record(c, L.words);
+      rw_per_warp = L.state_stride + rw_topo + 256u;
+      rw_wpb = std::min<uint32_t>(8u, (227u * 1024u - bf::kStatusStaticSmem) / rw_per_warp);
+      if (!rw_wpb) return fail(c, BF_ENOMEM, "a topology record and a state record do not fit one warp's shared memory");
+    }
+    st.out(W.rw_runs, n_runs);
+    st.out(W.rw_planes, (size_t)n_runs * 4u * L.words);
+  }
   if (int rc = st.send(c, "bf_resident_commit (check)")) return rc;
   const size_t sent = st.size;
   if (P.arm.tim) {
@@ -1321,12 +1341,21 @@ static int resident_commit(bf_ctx* c, uint32_t h, uint32_t n_runs, const bf_comm
   P.words = L.words; P.state_stride = L.state_stride; P.off_phase = L.off_phase; P.result_stride = L.result_stride;
   P.off_ready = L.off_ready; P.off_skip = L.off_skip; P.off_fail = L.off_fail; P.sched_stride = A.sched_stride;
   P.mark = r->d_mark; P.mark_value = r->mark_touched();
+  cudaError_t e = cudaSuccess;
+  if (rewrites) {
+    W.state = r->d_state; W.result = r->d_result; W.slots = c->slots_dev; W.n_slots = P.n_slots; W.runctl = A.runctl;
+    W.n_runs = n_runs; W.warps_per_block = rw_wpb;
+    W.words = L.words; W.state_stride = L.state_stride; W.off_phase = L.off_phase; W.off_decision = L.off_decision;
+    W.off_child = L.off_child; W.topo_bytes = rw_topo; W.result_stride = L.result_stride;
+    e = bf::launch_rewrites(W, rw_wpb * rw_per_warp, s);
+    P.rw_runs = W.rw_runs; P.rw_planes = W.rw_planes; P.rewritten = P.counts + 7;
+  }
   uint32_t* host = c->pinned->commit;
-  cudaError_t e = bf::launch_commit(P, false, s);
+  if (e == cudaSuccess) e = bf::launch_commit(P, false, s);
   if (e == cudaSuccess) e = cudaMemcpyAsync(host, P.offender, 8, cudaMemcpyDeviceToHost, s);
   if (e == cudaSuccess && journaled) e = cudaMemcpyAsync(c->pinned->commit_journal, P.total, 16, cudaMemcpyDeviceToHost, s);
   if (int rc = bf::end_call(c, e, "bf_resident_commit (check)")) return rc;
-  c->stats.kernel_launches += journaled ? 2 : 1;
+  c->stats.kernel_launches += (journaled ? 2 : 1) + (rewrites ? 1 : 0);
   uint64_t key;
   memcpy(&key, host, 8);
   if (key != ~0ull) {
@@ -1348,6 +1377,7 @@ static int resident_commit(bf_ctx* c, uint32_t h, uint32_t n_runs, const bf_comm
     if (staged_runs && P.runs_cap) st.out(P.runs, P.runs_cap);
     if (int rc = st.grow(c, sent, "bf_resident_commit")) return rc;
     if (P.arm.tim) P.arm.out = P.counts + 5;   // the arms' words behind the counts, where grow() may have moved them
+    if (rewrites) { P.rw_runs = W.rw_runs; P.rw_planes = W.rw_planes; P.rewritten = P.counts + 7; }
   }
   e = bf::launch_commit(P, true, s);
   if (e == cudaSuccess) e = cudaMemcpyAsync(host, P.counts, 4 * n_counts, cudaMemcpyDeviceToHost, s);
@@ -1357,16 +1387,22 @@ static int resident_commit(bf_ctx* c, uint32_t h, uint32_t n_runs, const bf_comm
     e = cudaMemcpyAsync(journal->runs, P.runs, (size_t)k * 4, cudaMemcpyDeviceToHost, s);
   if (int rc = r->sync_in_place(c, e, "bf_resident_commit")) { r->state_changed(c); return rc; }
   c->stats.kernel_launches += 1;
-  uint32_t k[7];
+  uint32_t k[8];
   memcpy(k, host, 4 * n_counts);
   out->n_runs_written = k[0]; out->n_skipped = k[1]; out->n_launched = k[2]; out->n_queued = k[3]; out->n_failed = k[4];
   if (arm) { arm->n_armed = k[5]; arm->next_deadline = k[6]; }
   if (journaled) { journal->n_items = n_items; journal->n_runs_listed = n_listed; }
+  if (rewrites) *rewritten = k[7];
   if (k[0]) {   // as a delta: the written runs are touched, and the tick a schedule or a commit needs is over
     r->state_changed(c);
     r->pending += k[0];
   }
   return BF_OK;
+}
+
+int bf_resident_commit_rewrites(bf_ctx* c, uint32_t h, uint32_t n_runs, const bf_commit_entry* entries, uint32_t n,
+                                bf_commit_out* out, bf_commit_arm* arm, bf_commit_journal* journal, uint32_t* n_rewritten) {
+  return resident_commit(c, h, n_runs, entries, n, out, arm, journal, true, n_rewritten, true);
 }
 
 int bf_resident_commit_journal(bf_ctx* c, uint32_t h, uint32_t n_runs, const bf_commit_entry* entries, uint32_t n, bf_commit_out* out,

@@ -382,11 +382,14 @@ class Frontier:
                                    ("after", "<u4")])   # bf_commit_write, 16 B
 
     def resident_commit(self, handle: int, n_runs: int, entries=None, now: Optional[int] = None,
-                        journal_cap: Optional[int] = None) -> dict:
+                        journal_cap: Optional[int] = None, rewrites: bool = False) -> dict:
         """bf_resident_commit: write the skips, launches and queue marks of the last tick (and schedule) of runs [0, n_runs)
         into the state records.  entries: COMMIT_DTYPE (or (run, step, kind, code) tuples), at most one per (run, step).
         With `now` (bf_resident_commit_timed) the launched sleep, gate and wait steps with a timing (put_timings) are armed too.
         With journal_cap (bf_resident_commit_journal) the call also lists what it wrote, up to journal_cap items.
+        With rewrites (bf_resident_commit_rewrites; needs journal_cap) the writes start from the codes after a single pass's
+        stages G, H and I, so that the sleeps, gates, waits, joins and fail-fast skips that pass rewrote are stored and listed
+        (PHASE items with code A.COMMIT_WRITE_REWRITE), and the result also holds n_rewritten.
         -> dict(n_runs_written, n_skipped, n_launched, n_queued, n_failed), with `now` also n_armed and next_deadline, with
         journal_cap also items (COMMIT_WRITE_DTYPE[min(n_items, journal_cap)]), n_items, runs (u32, the runs whose record
         changed) and n_runs_listed.  A refusal raises FrontierError with .bad_run and .bad_step (A.COMMIT_NONE for a refusal
@@ -395,7 +398,10 @@ class Frontier:
         if not isinstance(ents, np.ndarray):
             ents = np.array([tuple(e) for e in ents], dtype=self.COMMIT_DTYPE)
         ents = np.ascontiguousarray(ents, dtype=self.COMMIT_DTYPE)
+        if rewrites and journal_cap is None:
+            raise ValueError("resident_commit(rewrites=True) needs journal_cap: the rewrites are persisted from the journal")
         out = A.CommitOut(struct_size=C.sizeof(A.CommitOut))
+        n_rw = C.c_uint32(0)
         ep = ents.ctypes.data if ents.shape[0] else None
         arm = None if now is None else A.CommitArm(struct_size=C.sizeof(A.CommitArm), now=int(now))
         if journal_cap is not None:
@@ -403,8 +409,12 @@ class Frontier:
             runs = np.zeros(max(int(n_runs), 1), dtype=np.uint32)
             j = A.CommitJournal(struct_size=C.sizeof(A.CommitJournal), items=items.ctypes.data if journal_cap else None,
                                 items_cap=int(journal_cap), runs=runs.ctypes.data if n_runs else None, runs_cap=int(n_runs))
-            rc = self._lib.bf_resident_commit_journal(self._ctx, handle, int(n_runs), ep, ents.shape[0], C.byref(out),
-                                                      None if arm is None else C.byref(arm), C.byref(j))
+            if rewrites:
+                rc = self._lib.bf_resident_commit_rewrites(self._ctx, handle, int(n_runs), ep, ents.shape[0], C.byref(out),
+                                                           None if arm is None else C.byref(arm), C.byref(j), C.byref(n_rw))
+            else:
+                rc = self._lib.bf_resident_commit_journal(self._ctx, handle, int(n_runs), ep, ents.shape[0], C.byref(out),
+                                                          None if arm is None else C.byref(arm), C.byref(j))
         elif arm is None:
             rc = self._lib.bf_resident_commit(self._ctx, handle, int(n_runs), ep, ents.shape[0], C.byref(out))
         else:
@@ -419,6 +429,8 @@ class Frontier:
         if journal_cap is not None:
             got.update(items=items[:min(int(j.n_items), int(journal_cap))].copy(), n_items=int(j.n_items),
                        runs=runs[:int(j.n_runs_listed)].copy(), n_runs_listed=int(j.n_runs_listed))
+        if rewrites:
+            got["n_rewritten"] = int(n_rw.value)
         return got
 
     # -- run status of resident batches (bf_resident_status)

@@ -50,6 +50,7 @@ _SYMS = [
     ("bfh_batch_transfer", C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p]),
     ("bfh_batch_eval", C.c_int, [C.c_void_p, C.c_uint32, C.POINTER(A.Counts)]),
     ("bfh_batch_commit", C.c_int, [C.c_void_p, C.c_void_p, C.c_uint32, C.POINTER(A.CommitOut)]),
+    ("bfh_batch_commit_rewrites", C.c_int, [C.c_void_p, C.c_void_p, C.c_uint32, C.POINTER(A.CommitOut), C.POINTER(C.c_uint32)]),
     ("bfh_batch_set_resident", C.c_int, [C.c_void_p, C.c_int]),
     ("bfh_batch_traffic", C.c_int, [C.c_void_p, C.POINTER(C.c_uint64), C.POINTER(C.c_uint64), C.POINTER(C.c_uint32)]),
     ("bfh_run_summary", C.c_uint32, [C.c_void_p, C.c_uint32]),
@@ -304,23 +305,32 @@ class HostBatch:
         self._chk(self._l.bfh_batch_eval(self._p, flags, C.byref(c)), "bfh_batch_eval")
         return {"ready": c.ready, "skip": c.skip, "expansion": c.expansion, "evals": c.evals}
 
-    def commit(self, entries=None) -> dict:
+    def commit(self, entries=None, rewrites: bool = False) -> dict:
         """bfh_batch_commit: the tick commit of the last eval's runs on the device (resident mode), its writes applied to the
         mirror's records except where a delta logged since the eval covers them.  entries: Frontier.COMMIT_DTYPE rows (or
-        tuples).  -> dict(n_runs_written, n_skipped, n_launched, n_queued, n_failed); a refusal raises FrontierError with
-        .bad_run and .bad_step"""
+        tuples).  With rewrites (bfh_batch_commit_rewrites) the commit also stores the phases a single pass's stages G, H and I
+        rewrote, and the result holds n_rewritten.  -> dict(n_runs_written, n_skipped, n_launched, n_queued, n_failed); a refusal
+        raises FrontierError with .bad_run and .bad_step"""
         from .frontier import Frontier
         ents = np.zeros(0, Frontier.COMMIT_DTYPE) if entries is None else entries
         if not isinstance(ents, np.ndarray):
             ents = np.array([tuple(e) for e in ents], dtype=Frontier.COMMIT_DTYPE)
         ents = np.ascontiguousarray(ents, dtype=Frontier.COMMIT_DTYPE)
         out = A.CommitOut(struct_size=C.sizeof(A.CommitOut))
-        rc = self._l.bfh_batch_commit(self._p, ents.ctypes.data if ents.shape[0] else None, ents.shape[0], C.byref(out))
+        ep = ents.ctypes.data if ents.shape[0] else None
+        nrw = C.c_uint32(0)
+        if rewrites:
+            rc = self._l.bfh_batch_commit_rewrites(self._p, ep, ents.shape[0], C.byref(out), C.byref(nrw))
+        else:
+            rc = self._l.bfh_batch_commit(self._p, ep, ents.shape[0], C.byref(out))
         if rc < 0:
             err = A.FrontierError(rc, "bfh_batch_commit: %s" % self._l.bfh_batch_error(self._p).decode())
             err.bad_run, err.bad_step = int(out.bad_run), int(out.bad_step)
             raise err
-        return {k: int(getattr(out, k)) for k in ("n_runs_written", "n_skipped", "n_launched", "n_queued", "n_failed")}
+        got = {k: int(getattr(out, k)) for k in ("n_runs_written", "n_skipped", "n_launched", "n_queued", "n_failed")}
+        if rewrites:
+            got["n_rewritten"] = int(nrw.value)
+        return got
 
     def _list(self, fn, run, cap=1024):
         out = np.zeros(cap, np.uint32)

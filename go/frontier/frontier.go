@@ -652,6 +652,10 @@ const (
 	CommitWriteTimer      = 0x10
 )
 
+// CommitWriteRewrite is the Code of a phase item of CommitRewrites whose code comes from the stages G / H / I of a single pass
+// (BF_COMMIT_WRITE_REWRITE), not from the tick's masks.
+const CommitWriteRewrite = 0x1
+
 // CommitWrite is one item of a commit's journal (bf_commit_write, 16 bytes, no pointers): a step whose stored phase code changed
 // (Before: the stored nibble, 15 as stored; After: the code written), a desc whose registered bit was set (0 -> 1), or a timer
 // slot armed for step Index (Code: the armed decision code; Before: TimerNone; After: the deadline).
@@ -699,6 +703,35 @@ func (r *Resident) CommitJournal(n, now uint32, entries []CommitEntry, items []C
 	j.Items = items[:minU64(j.NItems, uint64(len(items)))]
 	j.Runs = runs[:minU64(uint64(j.NRuns), uint64(len(runs)))]
 	return res, j, r.c.err(rc)
+}
+
+// CommitRewrites is CommitJournal through bf_resident_commit_rewrites: the commit also stores the phases a single pass's stages
+// G, H and I rewrote (fired sleeps, decided or timed-out gates and waits, joined parallel steps, fail-fast and compensation
+// skips, a terminated topology's Failed codes), and lists each as a phase item with Code CommitWriteRewrite.  The batcher persists
+// them in the same status PATCH (GroupWrites: a rewrite whose After is terminal finishes its step).  -> also the number of steps
+// written from the stages.
+func (r *Resident) CommitRewrites(n, now uint32, entries []CommitEntry, items []CommitWrite, runs []uint32) (CommitResult, Journal, uint32, error) {
+	var ep *C.bf_commit_entry
+	if len(entries) > 0 {
+		ep = (*C.bf_commit_entry)(unsafe.Pointer(&entries[0]))
+	}
+	var ip *C.bf_commit_write
+	if len(items) > 0 {
+		ip = (*C.bf_commit_write)(unsafe.Pointer(&items[0]))
+	}
+	var rp *C.uint32_t
+	if len(runs) > 0 {
+		rp = (*C.uint32_t)(unsafe.Pointer(&runs[0]))
+	}
+	var k [11]C.uint32_t
+	var nItems C.uint64_t
+	rc := C.bfgo_resident_commit_rewrites(r.c.p, r.handle, C.uint32_t(n), ep, C.uint32_t(len(entries)), C.uint32_t(now), ip,
+		C.uint64_t(len(items)), rp, C.uint32_t(len(runs)), &k[0], &nItems)
+	res := CommitResult{uint32(k[0]), uint32(k[1]), uint32(k[2]), uint32(k[3]), uint32(k[4]), uint32(k[5]), uint32(k[6])}
+	j := Journal{NItems: uint64(nItems), NRuns: uint32(k[9]), Armed: uint32(k[7]), NextDeadline: uint32(k[8])}
+	j.Items = items[:minU64(j.NItems, uint64(len(items)))]
+	j.Runs = runs[:minU64(uint64(j.NRuns), uint64(len(runs)))]
+	return res, j, uint32(k[10]), r.c.err(rc)
 }
 
 func minU64(a, b uint64) uint64 {

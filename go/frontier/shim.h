@@ -265,6 +265,32 @@ static inline int bfgo_resident_commit_journal(bf_ctx* c, uint32_t handle, uint3
   return rc;
 }
 
+/* bfgo_resident_commit_journal through bf_resident_commit_rewrites: counts[10] = the steps written from the stages G / H / I. */
+static inline int bfgo_resident_commit_rewrites(bf_ctx* c, uint32_t handle, uint32_t n_runs, const bf_commit_entry* entries, uint32_t n,
+                                                uint32_t now, bf_commit_write* items, uint64_t items_cap, uint32_t* runs,
+                                                uint32_t runs_cap, uint32_t* counts, uint64_t* n_items) {
+  bf_commit_out o;
+  memset(&o, 0, sizeof o);
+  o.struct_size = (uint32_t)sizeof o;
+  bf_commit_arm a;
+  memset(&a, 0, sizeof a);
+  a.struct_size = (uint32_t)sizeof a;
+  a.now = now;
+  bf_commit_journal j;
+  memset(&j, 0, sizeof j);
+  j.struct_size = (uint32_t)sizeof j;
+  j.items = items; j.items_cap = items_cap; j.runs = runs; j.runs_cap = runs_cap;
+  uint32_t nrw = 0;
+  const int rc = bf_resident_commit_rewrites(c, handle, n_runs, entries, n, &o, now == BF_TIMER_NONE ? NULL : &a, &j, &nrw);
+  counts[0] = o.n_runs_written; counts[1] = o.n_skipped; counts[2] = o.n_launched; counts[3] = o.n_queued; counts[4] = o.n_failed;
+  counts[5] = o.bad_run; counts[6] = o.bad_step;
+  counts[7] = now == BF_TIMER_NONE ? 0u : a.n_armed; counts[8] = now == BF_TIMER_NONE ? BF_TIMER_NONE : a.next_deadline;
+  counts[9] = j.n_runs_listed;
+  counts[10] = nrw;
+  *n_items = j.n_items;
+  return rc;
+}
+
 /* Run status.  The records (bf_status_rec holds no pointers) and events land in the caller's buffers; *n_events = the events of
  * the listed runs, of which the first events_cap were written.  runs == NULL with n == n_runs lists every run of [0, n_runs). */
 static inline int bfgo_resident_status(bf_ctx* c, uint32_t handle, uint32_t n_runs, const uint32_t* runs, uint32_t n,

@@ -1095,7 +1095,8 @@ int bf_resident_runctl_download(bf_ctx* ctx, uint32_t handle, uint32_t first_run
  * or a commit needs.  bf_resident_commit arms no step timer (bf_resident_commit_timed below arms those of the launched sleeps,
  * gates and waits), and a stopped run (bf_resident_runctl) has no candidates, so it gets nothing.  The counts are steps whose code the commit changed (a
  * launched parallel step also when only its registered bit was set).  Stage G / H / I rewrites (gate syncs, joins, fail-fast and
- * compensation skips) are not persisted: each pass recomputes them from the state.  One H2D copy of the sorted entries, the check
+ * compensation skips) are not persisted by this call, _timed or _journal: each pass recomputes them from the state
+ * (bf_resident_commit_rewrites below stores them).  One H2D copy of the sorted entries, the check
  * launch, one D2H copy and one synchronisation before anything is written; then the apply launch, one D2H copy and one
  * synchronisation.                                                                                                          */
 enum { BF_COMMIT_HOLD = 1, BF_COMMIT_ERROR = 2, BF_COMMIT_PHASE = 3 };
@@ -1167,7 +1168,7 @@ typedef struct bf_commit_write { /* 16 B                                        
   uint32_t run;
   uint16_t index;                /* step (PHASE, TIMER) or parallel desc (REGISTERED)                                           */
   uint8_t field;                 /* BF_DELTA_PHASE, BF_DELTA_REGISTERED, BF_COMMIT_WRITE_TIMER                                  */
-  uint8_t code;                  /* TIMER: the armed code; else 0                                                               */
+  uint8_t code;                  /* TIMER: the armed code; PHASE: 0 or BF_COMMIT_WRITE_REWRITE (_rewrites); else 0              */
   uint32_t before, after;        /* PHASE: stored nibble / code written; REGISTERED: 0 / 1; TIMER: BF_TIMER_NONE / deadline     */
 } bf_commit_write;
 typedef struct bf_commit_journal {
@@ -1182,6 +1183,37 @@ typedef struct bf_commit_journal {
 } bf_commit_journal;
 int bf_resident_commit_journal(bf_ctx* ctx, uint32_t handle, uint32_t n_runs, const bf_commit_entry* entries, uint32_t n_entries,
                                bf_commit_out* out, bf_commit_arm* arm, bf_commit_journal* journal);
+
+/* bf_resident_commit_rewrites(..., out, arm, journal, n_rewritten) is bf_resident_commit_journal (arm = NULL allowed) that also
+ * stores the phases a single pass's stages G, H and I rewrite, as the reference persists the StepStates its checkSync* and
+ * markFailFastSkipped / markCompensationsSkipped wrote (persistMergedStates, dag.go:774-793): a fired sleep, an approved, rejected
+ * or timed-out gate or wait (stage G), a joined parallel step (stage H), fail-fast and compensation skips and the Failed codes of a
+ * terminated realtime topology (stage I).  The journal is required (a rewrite the batcher never hears of is not persisted in the
+ * cluster); NULL, or a wrong struct_size, is BF_EINVAL as for bf_resident_commit_journal, and so is a NULL n_rewritten.
+ *
+ * The writes of a run start from its codes after the stages bf_resident_status applies (no stage-D cond-FAIL write: the fail mask
+ * still writes those) instead of its stored codes, and are stored where they differ from the stored codes (15 read as 0, as
+ * always).  A run with a BF_COMMIT_ERROR entry, a stopped run, and a run on a dead or too-wide slot get no rewrite (nor, as before,
+ * any other write); a HOLD step takes no launch write, and the rest of its run takes its rewrites.  Checks, refusals, entries,
+ * arms and touches are those of bf_resident_commit_journal.  A run whose only writes are rewrites is a written run: touched,
+ * listed in journal->runs and counted in out->n_runs_written, and a commit that wrote ends the tick as any other.
+ *
+ * Items as bf_resident_commit_journal, in the same order; a PHASE item of a step that has no mask bit (not skipped, cond-FAIL,
+ * launched or queued: its new code comes from the stages) carries code = BF_COMMIT_WRITE_REWRITE, every other item code 0 (or
+ * the armed code of a TIMER item).  The counts of out keep counting the mask writes; *n_rewritten is the number of steps written
+ * from the stages (the items marked BF_COMMIT_WRITE_REWRITE).  A commit that wrote ends the tick, so a second call needs a new
+ * tick; that tick evaluates the written records, and a run whose stages rewrite again over them (a fail-fast skip after stored
+ * Failed codes, say) is flagged by its new result record and takes those rewrites at the next call.
+ *
+ * Precondition that makes it cheap and exact: only a run whose current result record carries BF_SUM_PHASE_CHANGED can have a
+ * rewrite, because the tick that left that record took the same stages over the same stored codes and flags any phase they
+ * change (a commit or any other write in between is refused, or ends the tick, as for every commit).  So one more launch, one warp
+ * per run, evaluates the stages of those runs alone and stages their planes in the ctx's device scratch (16 B per run and word,
+ * plus 4 B per run); the check and apply launches read them there.  One launch more than bf_resident_commit_journal and no further
+ * synchronisation.                                                                                                            */
+#define BF_COMMIT_WRITE_REWRITE 0x1u  /* bf_commit_write.code of a PHASE item whose code comes from the stages G / H / I          */
+int bf_resident_commit_rewrites(bf_ctx* ctx, uint32_t handle, uint32_t n_runs, const bf_commit_entry* entries, uint32_t n_entries,
+                                bf_commit_out* out, bf_commit_arm* arm, bf_commit_journal* journal, uint32_t* n_rewritten);
 
 /* ------------------------------------------------------------------ run status (what a batcher persists of a run's status)
  * When group selection finds nothing left to run (BF_GROUP_DONE, dag.go:482-495) the reference finalizes the StoryRun

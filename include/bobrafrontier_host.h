@@ -172,6 +172,12 @@ int bfh_batch_eval(bfh_batch* b, uint32_t eval_flags, bf_counts* counts);
  * (bad_run / bad_step in out, which may be NULL) changes neither the device nor the mirror.                                 */
 int bfh_batch_commit(bfh_batch* b, const bf_commit_entry* entries, uint32_t n, bf_commit_out* out);
 
+/* bfh_batch_commit through bf_resident_commit_rewrites: the device also stores the phases a single pass's stages G, H and I
+ * rewrite, and the mirror applies those PHASE items as the others (pending deltas win the same way).  The journal is sized as
+ * bfh_batch_commit's, with every step of the Story for a run whose last result carries BF_SUM_PHASE_CHANGED.  *n_rewritten
+ * (may be NULL) is the call's count of steps written from the stages.                                                       */
+int bfh_batch_commit_rewrites(bfh_batch* b, const bf_commit_entry* entries, uint32_t n, bf_commit_out* out, uint32_t* n_rewritten);
+
 /* Results of the last pass.  Step lists come back in list order (ascending index), the order the
  * concurrency limiters' readySteps[:slots] relies on (dag.go:1796-1798). */
 uint32_t bfh_run_summary(const bfh_batch* b, uint32_t run);
