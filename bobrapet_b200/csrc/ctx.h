@@ -187,9 +187,9 @@ struct bf_ctx {
     bf::ResultTail tail;   // written by a compaction's last kernel; a pass without one copies its counts into tail.counts
     uint32_t fire[4];      // bf_resident_fire: n_fired, n_written, n_pruned, next_deadline
     uint32_t commit[8];    // bf_resident_commit: the offender key (two words), then the five counts
-    unsigned long long status_events;   // bf_resident_status: the events of the call
-    unsigned long long resync[2];       // bf_resident_resync: the items and the drifted runs of the call
-    unsigned long long commit_journal[2];   // bf_resident_commit_journal: the items and the written runs of the call
+    // the totals of a call's lists: bf_resident_status its events; bf_resident_resync its items and drifted runs;
+    // bf_resident_commit_journal its items and written runs (every call holds the ctx lock, so they share the words)
+    unsigned long long list_totals[2];
     bf_counts counts() const { return {tail.counts[0], tail.counts[1], tail.counts[2], tail.counts[3]}; }
   }* pinned = nullptr;
   DevBuf<bf_expansion> d_exp;

@@ -420,9 +420,8 @@ struct ResSchedParams {
   SchedParams S;
   uint32_t base_runs;              // the previous schedule's n_runs: runs at or above it have no baseline
   uint32_t* run_events;            // [n_runs] events of a listed run, kSchedUnlisted for the others (sched_limit_runs)
-  uint32_t* cta_listed;            // [CTAs] listed runs per CTA, then (sched_scan_ctas) those of the CTAs before it
-  unsigned long long* cta_events;  // [CTAs] their events, likewise
-  unsigned long long* totals;      // [2] out: n_listed, n_events (written by the last CTA of sched_list_runs)
+  unsigned long long* cta;         // [2][CTAs] listed runs and events of each CTA, then (cta_scan) of the CTAs before it
+  unsigned long long* totals;      // [2] out: n_listed, n_events (cta_scan)
   uint32_t* runs;                  // [runs_cap]
   bf_sched_header* heads;          // [runs_cap]
   uint16_t* events;                // [events_cap]
@@ -527,12 +526,17 @@ struct RewriteParams {
   uint32_t* rw_planes;              // [n_runs][4][words]
 };
 
-// bf_resident_status (resident.cu): one warp per listed run.  status_count stores each listed run's event count and each CTA's
-// total, cta_scan turns the CTA totals into the events of the CTAs before each and posts the sum, status_list writes the
-// records and the events.  With a child area each warp has a shared stage for stage H: the state record, the topology record
-// (topo_bytes: the largest record the layout fits) and 256 scratch bytes.
+// bf_resident_status (resident.cu): one warp per listed run.  status_runs<false> stores each listed run's event count and each
+// CTA's total, cta_scan turns the CTA totals into the events of the CTAs before each and posts the sum, status_runs<true> writes
+// the records and the events.
 static_assert(sizeof(bf_status_rec) == 32, "bf_status_rec must be 32 bytes");
-constexpr uint32_t kStatusStaticSmem = 32;   // status_runs' static shared memory (one word per warp), beside the warps' stages
+// The single-pass launches (status_runs, resync_runs, rewrite_runs): their static shared memory (one word per warp,
+// store_cta_totals), beside the warps' shared stages.  With a child area each warp has a stage for stage H: the state record,
+// the topology record (topo_bytes: the largest record the layout fits) and 256 scratch bytes; without one, none.
+constexpr uint32_t kStatusStaticSmem = 32;
+__host__ __device__ inline uint32_t pass_stage_bytes(uint32_t off_child, uint32_t state_stride, uint32_t topo_bytes) {
+  return off_child != BF_OFF_NONE ? state_stride + topo_bytes + 256u : 0u;
+}
 struct StatusParams {
   const uint8_t* state;
   const Slot* slots;
@@ -541,8 +545,8 @@ struct StatusParams {
   const uint32_t* runs;             // [n] ascending, or nullptr: listed run i is run i
   uint32_t n, warps_per_block;
   uint32_t words, state_stride, off_phase, off_decision, off_child, topo_bytes;
-  uint32_t* run_events;             // [n] events of each listed run (status_count)
-  unsigned long long* cta_events;   // [CTAs] events of each CTA, then (cta_scan) of the CTAs before it
+  uint32_t* run_events;             // [n] events of each listed run (status_runs<false>)
+  unsigned long long* cta;          // [CTAs] events of each CTA, then (cta_scan) of the CTAs before it
   unsigned long long* total;        // [1] events of the call (cta_scan)
   bf_status_rec* records;           // [n]
   uint16_t* events;                 // [events_cap]

@@ -104,6 +104,53 @@ DI uint32_t get_nibble(const uint8_t* base, uint32_t i) {
 DI uint32_t redux_or(uint32_t v) { return __reduce_or_sync(FULL, v); }
 DI uint32_t redux_add(uint32_t v) { return __reduce_add_sync(FULL, v); }
 
+// ---- per-run lists (bf_resident_schedule, _status, _resync, _commit_journal): count, scan, list ------------------------------
+// A count launch gives each warp one word for its run (or runs) and stores each CTA's K totals; cta_scan (resident.cu) turns each
+// of the K arrays of CTA totals into the totals of the CTAs before each and posts the sums; the list launch rebuilds each run's
+// offsets from them and writes its items.  part(word, k) is a word's share of total k, the same in both launches.
+cudaError_t launch_cta_scan(unsigned long long* cta, unsigned long long* total, uint32_t n_ctas, uint32_t K, cudaStream_t stream);
+
+// Count (every thread of the CTA): lane 0 of each warp passes its word (0 for a warp without a run); thread 0 stores total k of
+// the CTA's words at cta[k * gridDim.x + blockIdx.x].  Its 32 bytes of static shared memory are kStatusStaticSmem.
+template <uint32_t K, class Part>
+DI void store_cta_totals(uint32_t word, unsigned long long* cta, Part part) {
+  __shared__ uint32_t warp_word[8];
+  if ((threadIdx.x & 31u) == 0) warp_word[threadIdx.x >> 5] = word;
+  __syncthreads();
+  if (threadIdx.x != 0) return;
+  for (uint32_t k = 0; k < K; ++k) {
+    unsigned long long sum = 0;
+    for (uint32_t w = 0; w < (blockDim.x >> 5); ++w) sum += part(warp_word[w], k);
+    cta[k * gridDim.x + blockIdx.x] = sum;
+  }
+}
+
+// List (whole warp): the offsets of the run whose word is run_words[i], the CTA's runs starting at run_words[first]: the totals of
+// the CTAs before (after cta_scan) and of the warps before it in its CTA.
+template <uint32_t K, class Part>
+DI void run_offsets(const unsigned long long* cta, const uint32_t* run_words, uint32_t first, uint32_t i, Part part,
+                    unsigned long long (&base)[K]) {
+  const uint32_t lane = threadIdx.x & 31u;
+  const uint32_t before = first + lane < i ? run_words[first + lane] : 0u;
+  for (uint32_t k = 0; k < K; ++k) base[k] = cta[k * gridDim.x + blockIdx.x] + redux_add(part(before, k));
+}
+
+// Emit (whole warp): one item per set bit of this lane's `bits`, lane by lane and bit by bit (step order when lane w holds word
+// w of the steps), from position pos; store(b, at) writes bit b's item at `at`, for every at below cap.  -> the position after
+// the warp's items
+template <class Store>
+DI unsigned long long emit_bits(uint32_t bits, unsigned long long pos, unsigned long long cap, Store store) {
+  const uint32_t lane = threadIdx.x & 31u, mine = (uint32_t)__popc(bits);
+  uint32_t incl = mine;
+  for (uint32_t d = 1; d < 32; d <<= 1) {
+    const uint32_t x = __shfl_up_sync(FULL, incl, d);
+    if (lane >= d) incl += x;
+  }
+  unsigned long long at = pos + incl - mine;
+  for (uint32_t x = bits; x && at < cap; x &= x - 1u, ++at) store((uint32_t)__ffs(x) - 1u, at);
+  return pos + __shfl_sync(FULL, incl, 31);
+}
+
 DI uint32_t bmsk_clamp(uint32_t pos, uint32_t width) {
   uint32_t r;
   asm("bmsk.clamp.b32 %0, %1, %2;" : "=r"(r) : "r"(pos), "r"(width));

@@ -216,15 +216,16 @@ cudaError_t launch_schedule(const SchedParams& P, uint32_t sm_count, cudaStream_
 // Limit and compare: warp w of CTA b takes runs 256 b + 32 w + j, j = 0..31, one after the other.  Each run's new record goes
 // over its stored one in the batch's schedule-record area; the run is listed when there was no baseline (at or above base_runs,
 // or kSchedNoBase in the stored reason) or some header or mask word differs.  Every lane reads the words it then writes, so the
-// comparison needs no staging.  run_events[r] and the CTA's listed runs and events feed sched_list_runs.
+// comparison needs no staging.  run_events[r] and the CTA's listed runs and events feed cta_scan and sched_list_runs.
+// A warp's word for the CTA's totals is its events << 8 | its listed runs (at most 32 runs of 3 * 1024 events).
+struct SchedPart {
+  DI uint32_t operator()(uint32_t w, uint32_t k) const { return k ? w >> 8 : w & 0xFFu; }
+};
 __global__ void __launch_bounds__(256) sched_limit_runs(const ResSchedParams R) {
-  __shared__ uint32_t w_listed[8];
-  __shared__ unsigned long long w_events[8];
   const SchedParams& P = R.S;
   const uint32_t lane = threadIdx.x & 31u, warp = threadIdx.x >> 5;
   const uint32_t global_running = *P.global_running;
-  uint32_t listed = 0;
-  unsigned long long events = 0;
+  uint32_t listed = 0, events = 0;
   for (uint32_t j = 0; j < 32u; ++j) {
     const uint32_t r = blockIdx.x * 256u + warp * 32u + j;
     if (r >= P.n_runs) break;
@@ -252,72 +253,17 @@ __global__ void __launch_bounds__(256) sched_limit_runs(const ResSchedParams R) 
       if (list) { ++listed; events += ev; }
     }
   }
-  if (lane == 0) { w_listed[warp] = listed; w_events[warp] = events; }
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    uint32_t l = 0;
-    unsigned long long e = 0;
-    for (uint32_t w = 0; w < 8u; ++w) { l += w_listed[w]; e += w_events[w]; }
-    R.cta_listed[blockIdx.x] = l;
-    R.cta_events[blockIdx.x] = e;
-  }
+  store_cta_totals<2>(events << 8 | listed, R.cta, SchedPart{});
 }
 
-// The CTA totals of sched_limit_runs become exclusive prefixes in place: one CTA of 1024 threads walks them in chunks, a warp
-// scan and a scan of the warp totals per chunk, carrying the running sum, so the list launch reads its offsets in O(1).
-__global__ void __launch_bounds__(1024) sched_scan_ctas(const ResSchedParams R, uint32_t n_ctas) {
-  __shared__ uint32_t s_l[32];
-  __shared__ unsigned long long s_e[32];
-  const uint32_t lane = threadIdx.x & 31u, warp = threadIdx.x >> 5;
-  uint32_t carry_l = 0;
-  unsigned long long carry_e = 0;
-  for (uint32_t base = 0; base < n_ctas; base += 1024u) {
-    const uint32_t i = base + threadIdx.x;
-    const uint32_t l = i < n_ctas ? R.cta_listed[i] : 0u;
-    const unsigned long long e = i < n_ctas ? R.cta_events[i] : 0ull;
-    uint32_t il = l;
-    unsigned long long ie = e;
-#pragma unroll
-    for (int d = 1; d < 32; d <<= 1) {
-      const uint32_t a = __shfl_up_sync(FULL, il, d);
-      const unsigned long long b = __shfl_up_sync(FULL, ie, d);
-      if ((int)lane >= d) { il += a; ie += b; }
-    }
-    if (lane == 31) { s_l[warp] = il; s_e[warp] = ie; }
-    __syncthreads();
-    if (warp == 0) {   // the warp totals' inclusive scan
-      uint32_t wl = s_l[lane];
-      unsigned long long we = s_e[lane];
-#pragma unroll
-      for (int d = 1; d < 32; d <<= 1) {
-        const uint32_t a = __shfl_up_sync(FULL, wl, d);
-        const unsigned long long b = __shfl_up_sync(FULL, we, d);
-        if ((int)lane >= d) { wl += a; we += b; }
-      }
-      s_l[lane] = wl; s_e[lane] = we;
-    }
-    __syncthreads();
-    const uint32_t before_l = carry_l + (warp ? s_l[warp - 1] : 0u) + il - l;
-    const unsigned long long before_e = carry_e + (warp ? s_e[warp - 1] : 0ull) + ie - e;
-    if (i < n_ctas) { R.cta_listed[i] = before_l; R.cta_events[i] = before_e; }
-    carry_l += s_l[31];
-    carry_e += s_e[31];
-    __syncthreads();   // s_l / s_e are rewritten by the next chunk
-  }
-}
-
-// List: the same partition.  Each CTA reads the listed runs and events of the CTAs before it (sched_scan_ctas), scans its own
-// 256 runs, and each warp writes its listed runs in order: lane 0 the index and the header, the lanes of the
-// mask words their steps' events (ascending: word by lane, bit by bit).  The last CTA posts the two totals.
+// List: the same partition.  Each CTA reads the listed runs and events of the CTAs before it (cta_scan), scans its own 256 runs,
+// and each warp writes its listed runs in order: lane 0 the index and the header, the lanes of the mask words their steps'
+// events (ascending: word by lane, bit by bit).
 __global__ void __launch_bounds__(256) sched_list_runs(const ResSchedParams R) {
   __shared__ uint32_t s_l[8];
   __shared__ unsigned long long s_e[8];
-  __shared__ uint32_t s_base_l;
-  __shared__ unsigned long long s_base_e;
   const SchedParams& P = R.S;
   const uint32_t lane = threadIdx.x & 31u, warp = threadIdx.x >> 5;
-  if (threadIdx.x == 0) { s_base_l = R.cta_listed[blockIdx.x]; s_base_e = R.cta_events[blockIdx.x]; }
-  __syncthreads();
   // this thread's run, and the inclusive scans of listed runs and events over the warp
   const uint32_t r = blockIdx.x * 256u + threadIdx.x;
   const uint32_t v = r < P.n_runs ? R.run_events[r] : kSchedUnlisted;
@@ -333,20 +279,14 @@ __global__ void __launch_bounds__(256) sched_list_runs(const ResSchedParams R) {
   }
   if (lane == 31) { s_l[warp] = il; s_e[warp] = ie; }
   __syncthreads();
-  uint32_t wl = s_base_l;
-  unsigned long long we = s_base_e;
+  unsigned long long wl = R.cta[blockIdx.x], we = R.cta[gridDim.x + blockIdx.x];
   for (uint32_t w = 0; w < warp; ++w) { wl += s_l[w]; we += s_e[w]; }
-  const uint32_t pos_mine = wl + il - mine_l;
-  const unsigned long long off_mine = we + ie - mine_e;
-  if (blockIdx.x == gridDim.x - 1 && threadIdx.x == 255) {
-    R.totals[0] = wl + il;
-    R.totals[1] = we + ie;
-  }
+  const unsigned long long pos_mine = wl + il - mine_l, off_mine = we + ie - mine_e;
   for (uint32_t j = 0; j < 32u; ++j) {
     const bool listed = __shfl_sync(FULL, mine_l, j) != 0u;
     if (!listed) continue;
     const uint32_t rj = blockIdx.x * 256u + warp * 32u + j;
-    const uint32_t pos = __shfl_sync(FULL, pos_mine, j);
+    const unsigned long long pos = __shfl_sync(FULL, pos_mine, j);
     const unsigned long long off = __shfl_sync(FULL, off_mine, j);
     const uint8_t* rec = P.records + (size_t)rj * P.stride;
     if (lane == 0 && pos < R.runs_cap) {
@@ -356,21 +296,10 @@ __global__ void __launch_bounds__(256) sched_list_runs(const ResSchedParams R) {
     const uint32_t* m = reinterpret_cast<const uint32_t*>(rec + 16);
     const uint32_t launch = lane < P.words ? m[lane] : 0u, qs = lane < P.words ? m[P.words + lane] : 0u,
                    qd = lane < P.words ? m[2 * P.words + lane] : 0u;
-    uint32_t bits = launch | qs | qd;
-    const uint32_t c = (uint32_t)__popc(bits);
-    uint32_t incl = c;
-#pragma unroll
-    for (int d = 1; d < 32; d <<= 1) {
-      const uint32_t a = __shfl_up_sync(FULL, incl, d);
-      if ((int)lane >= d) incl += a;
-    }
-    unsigned long long e = off + (incl - c);
-    for (; bits && e < R.events_cap; ++e) {
-      const uint32_t b = __ffs(bits) - 1u;
-      bits &= bits - 1u;
+    emit_bits(launch | qs | qd, off, R.events_cap, [&](uint32_t b, unsigned long long e) {
       const uint32_t kind = (launch >> b) & 1u ? BF_SEVT_LAUNCH : ((qs >> b) & 1u ? BF_SEVT_QUEUED_STORY : BF_SEVT_QUEUED_SCHED);
       R.events[e] = (uint16_t)((lane * 32u + b) | kind << 10);
-    }
+    });
   }
 }
 
@@ -378,7 +307,7 @@ cudaError_t launch_resident_schedule(const ResSchedParams& R, cudaStream_t strea
   if (R.S.n_runs == 0) return cudaSuccess;
   const uint32_t grid = (R.S.n_runs - 1u) / 256u + 1u;
   sched_limit_runs<<<grid, 256, 0, stream>>>(R);
-  sched_scan_ctas<<<1, 1024, 0, stream>>>(R, grid);
+  if (const cudaError_t e = launch_cta_scan(R.cta, R.totals, grid, 2, stream)) return e;
   sched_list_runs<<<grid, 256, 0, stream>>>(R);
   return cudaGetLastError();
 }

@@ -912,42 +912,76 @@ cudaError_t launch_fire(const FireParams& P, cudaStream_t stream) {
 }
 
 // One CTA: for each of K arrays of n_ctas per-CTA totals (array k at cta + k * n_ctas), the totals become the sums of the CTAs
-// before each (exclusive scan in place); array k's sum goes to total[k].  bf_resident_status scans its events (K = 1),
-// bf_resident_resync its items and drifted runs, bf_resident_commit_journal its items and written runs (K = 2).
+// before each (exclusive scan in place); array k's sum goes to total[k].  The K arrays are walked together in chunks of 1024, a
+// warp scan and a scan of the warp totals per chunk, carrying the running sums.  bf_resident_status scans its events (K = 1),
+// bf_resident_schedule its listed runs and events, bf_resident_resync its items and drifted runs, bf_resident_commit_journal its
+// items and written runs (K = 2).
 template <uint32_t K>
 __global__ void __launch_bounds__(1024) cta_scan(unsigned long long* cta, unsigned long long* total, uint32_t n_ctas) {
-  __shared__ unsigned long long s_e[32];
+  __shared__ unsigned long long s_e[K][32];
   const uint32_t lane = threadIdx.x & 31u, warp = threadIdx.x >> 5;
-  for (uint32_t k = 0; k < K; ++k) {
-    unsigned long long* a = cta + (size_t)k * n_ctas;
-    unsigned long long carry = 0;
-    for (uint32_t base = 0; base < n_ctas; base += 1024u) {
-      const uint32_t i = base + threadIdx.x;
-      const unsigned long long e = i < n_ctas ? a[i] : 0ull;
-      unsigned long long ie = e;
+  unsigned long long carry[K] = {};
+  for (uint32_t base = 0; base < n_ctas; base += 1024u) {
+    const uint32_t i = base + threadIdx.x;
+    unsigned long long e[K], ie[K];
+    for (uint32_t k = 0; k < K; ++k) ie[k] = e[k] = i < n_ctas ? cta[(size_t)k * n_ctas + i] : 0ull;
 #pragma unroll
-      for (int d = 1; d < 32; d <<= 1) {
-        const unsigned long long b = __shfl_up_sync(FULL, ie, d);
-        if ((int)lane >= d) ie += b;
+    for (int d = 1; d < 32; d <<= 1)
+      for (uint32_t k = 0; k < K; ++k) {
+        const unsigned long long b = __shfl_up_sync(FULL, ie[k], d);
+        if ((int)lane >= d) ie[k] += b;
       }
-      if (lane == 31) s_e[warp] = ie;
-      __syncthreads();
-      if (warp == 0) {   // the warp totals' inclusive scan
-        unsigned long long we = s_e[lane];
+    if (lane == 31)
+      for (uint32_t k = 0; k < K; ++k) s_e[k][warp] = ie[k];
+    __syncthreads();
+    if (warp == 0) {   // the warp totals' inclusive scans
+      for (uint32_t k = 0; k < K; ++k) {
+        unsigned long long we = s_e[k][lane];
 #pragma unroll
         for (int d = 1; d < 32; d <<= 1) {
           const unsigned long long b = __shfl_up_sync(FULL, we, d);
           if ((int)lane >= d) we += b;
         }
-        s_e[lane] = we;
+        s_e[k][lane] = we;
       }
-      __syncthreads();
-      if (i < n_ctas) a[i] = carry + (warp ? s_e[warp - 1] : 0ull) + ie - e;
-      carry += s_e[31];
-      __syncthreads();   // s_e is rewritten by the next chunk
     }
-    if (threadIdx.x == 0) total[k] = carry;
+    __syncthreads();
+    for (uint32_t k = 0; k < K; ++k) {
+      if (i < n_ctas) cta[(size_t)k * n_ctas + i] = carry[k] + (warp ? s_e[k][warp - 1] : 0ull) + ie[k] - e[k];
+      carry[k] += s_e[k][31];
+    }
+    __syncthreads();   // s_e is rewritten by the next chunk
   }
+  if (threadIdx.x == 0)
+    for (uint32_t k = 0; k < K; ++k) total[k] = carry[k];
+}
+
+cudaError_t launch_cta_scan(unsigned long long* cta, unsigned long long* total, uint32_t n_ctas, uint32_t K, cudaStream_t stream) {
+  if (K == 1) cta_scan<1><<<1, 1024, 0, stream>>>(cta, total, n_ctas);
+  else cta_scan<2><<<1, 1024, 0, stream>>>(cta, total, n_ctas);
+  return cudaGetLastError();
+}
+
+// Past 48 KiB of dynamic shared memory a kernel opts in before its launch.
+template <class Params>
+static cudaError_t allow_smem(void (*kernel)(Params), uint32_t smem_bytes) {
+  return smem_bytes > 48u * 1024u ? cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes)
+                                  : cudaSuccess;
+}
+
+// The count launch, cta_scan over its K arrays of CTA totals and the list launch of P.n runs, P.warps_per_block warps and
+// smem_bytes of shared stages per CTA (bf_resident_status, bf_resident_resync).
+template <uint32_t K, class Params>
+static cudaError_t launch_listing(void (*count)(Params), void (*list)(Params), const Params& P, uint32_t smem_bytes, cudaStream_t stream) {
+  if (P.n == 0) return cudaSuccess;
+  cudaError_t e = allow_smem(count, smem_bytes);
+  if (e == cudaSuccess) e = allow_smem(list, smem_bytes);
+  if (e != cudaSuccess) return e;
+  const uint32_t grid = (P.n - 1u) / P.warps_per_block + 1u, threads = 32u * P.warps_per_block;
+  count<<<grid, threads, smem_bytes, stream>>>(P);
+  cta_scan<K><<<1, 1024, 0, stream>>>(P.cta, P.total, grid);
+  list<<<grid, threads, smem_bytes, stream>>>(P);
+  return cudaGetLastError();
 }
 
 // ---- tick commits (bf_resident_commit*) -------------------------------------------------------------------------------------
@@ -1161,6 +1195,11 @@ DI void commit_registered(uint32_t lane, const CommitRun& c, const uint8_t* rec,
   w.newly = ((unsigned long long)set[1] << 32 | set[0]) & ~w.reg;
 }
 
+// a run's journal word's share of the items (k = 0) and of the written runs (k = 1)
+struct JournalPart {
+  DI uint32_t operator()(uint32_t w, uint32_t k) const { return k ? w & 1u : w >> kJournalItemsShift; }
+};
+
 // The per-run part of commit_check: lane 0 lowers P.offender to the run's first offence.  -> with kJournal, the run's journal
 // word (its items, new arms and whether its record changes; 0 for a run that writes nothing), else 0.
 template <bool kJournal, bool kRewrite>
@@ -1205,20 +1244,9 @@ DI void commit_check_body(const CommitParams& P) {
     if (r < P.n_runs) check_run<false, kRewrite>(P, r, lane);
     return;
   }
-  __shared__ uint32_t warp_word[8];
   const uint32_t jw = r < P.n_runs ? check_run<true, kRewrite>(P, r, lane) : 0u;
-  if (lane == 0) {
-    warp_word[threadIdx.x >> 5] = jw;
-    if (r < P.n_runs) P.run_items[r] = jw;
-  }
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    unsigned long long items = 0, written = 0;
-    for (uint32_t w = 0; w < 8; ++w) { items += warp_word[w] >> kJournalItemsShift; written += warp_word[w] & 1u; }
-    const uint32_t n_ctas = (P.n_runs - 1u) / 8u + 1u;
-    P.cta[blockIdx.x] = items;
-    P.cta[n_ctas + blockIdx.x] = written;
-  }
+  if (lane == 0 && r < P.n_runs) P.run_items[r] = jw;
+  store_cta_totals<2>(jw, P.cta, JournalPart{});
 }
 template <bool kJournal>
 __global__ void __launch_bounds__(256) commit_check(const CommitParams P) { commit_check_body<kJournal, false>(P); }
@@ -1244,11 +1272,10 @@ DI void commit_apply_body(const CommitParams& P) {
   uint32_t jw = 0, armed;
   unsigned long long pos = 0;
   if (kJournal && (jw = P.run_items[r]) != 0u) {
-    const uint32_t first = blockIdx.x * 8u, n_ctas = (P.n_runs - 1u) / 8u + 1u;
-    const uint32_t before = first + lane < r ? P.run_items[first + lane] : 0u;
-    pos = P.cta[blockIdx.x] + redux_add(before >> kJournalItemsShift);
-    const unsigned long long at = P.cta[n_ctas + blockIdx.x] + redux_add(before & 1u);
-    if (lane == 0 && (jw & 1u) && at < P.runs_cap) P.runs[at] = r;
+    unsigned long long base[2];
+    run_offsets<2>(P.cta, P.run_items, blockIdx.x * 8u, r, JournalPart{}, base);
+    pos = base[0];
+    if (lane == 0 && (jw & 1u) && base[1] < P.runs_cap) P.runs[base[1]] = r;
   }
   CommitWrites w;
   commit_writes<kRewrite>(P, r, lane, c, rec, hold, w, [&](uint32_t LA) {
@@ -1267,22 +1294,13 @@ DI void commit_apply_body(const CommitParams& P) {
   }
   commit_registered(lane, c, rec, w);
   if (kJournal && jw) {   // PHASE items lane by lane in step order, then REGISTERED items by desc
-    const uint32_t mine = (uint32_t)__popc(dirty);
-    uint32_t incl = mine;
-    for (uint32_t d = 1; d < 32; d <<= 1) {
-      const uint32_t x = __shfl_up_sync(FULL, incl, d);
-      if (lane >= d) incl += x;
-    }
-    unsigned long long at = pos + incl - mine;
     const uint32_t staged = kRewrite ? ~(w.SK | w.FA | w.LA | w.QU) : 0u;
-    for (uint32_t x = dirty; x && at < P.items_cap; x &= x - 1u, ++at) {
-      const uint32_t b = (uint32_t)__ffs(x) - 1u;
+    const unsigned long long reg_at = emit_bits(dirty, pos, P.items_cap, [&](uint32_t b, unsigned long long at) {
       const uint32_t was = ((w.p[0] >> b) & 1u) | ((w.p[1] >> b) & 1u) << 1 | ((w.p[2] >> b) & 1u) << 2 | ((w.p[3] >> b) & 1u) << 3;
       const uint32_t now = ((w.n0 >> b) & 1u) | ((w.n1 >> b) & 1u) << 1 | ((w.n2 >> b) & 1u) << 2 | ((w.n3 >> b) & 1u) << 3;
       const uint32_t code = ((staged >> b) & 1u) ? BF_COMMIT_WRITE_REWRITE << 24 : 0u;
       reinterpret_cast<uint4*>(P.items)[at] = make_uint4(r, (lane * 32u + b) | (uint32_t)BF_DELTA_PHASE << 16 | code, was, now);
-    }
-    const unsigned long long reg_at = pos + __shfl_sync(FULL, incl, 31);
+    });
     for (uint32_t h = 0; h < 2; ++h) {
       const uint32_t q = lane + 32u * h;
       if (!((w.newly >> q) & 1ull)) continue;
@@ -1326,7 +1344,7 @@ cudaError_t launch_commit(const CommitParams& P, bool apply, cudaStream_t stream
   } else {
     if (P.rw_runs) commit_check_rewrites<<<grid, 256, 0, stream>>>(P);
     else commit_check<true><<<grid, 256, 0, stream>>>(P);
-    cta_scan<2><<<1, 1024, 0, stream>>>(P.cta, P.total, grid);
+    return launch_cta_scan(P.cta, P.total, grid, 2, stream);
   }
   return cudaGetLastError();
 }
@@ -1466,13 +1484,17 @@ DI void run_status(const StatusParams& P, uint32_t i, uint32_t lane, uint32_t st
 // Count (kList = false): each listed run's events, and each CTA's total.  List (kList = true, after cta_scan): the same runs
 // again, each record with the offset of its first event (the CTAs before, then the warps before in its CTA) and its events, lane by
 // lane in step order.
+// a word's share of each total when the word is the total (one array of CTA totals)
+struct WordPart {
+  DI uint32_t operator()(uint32_t w, uint32_t) const { return w; }
+};
+
 template <bool kList>
 __global__ void __launch_bounds__(256, 1) status_runs(const StatusParams P) {
   extern __shared__ __align__(16) uint8_t status_stage[];
-  __shared__ uint32_t warp_events[kStatusStaticSmem / 4];
   const uint32_t warp = threadIdx.x >> 5, lane = threadIdx.x & 31u;
   const uint32_t i = blockIdx.x * P.warps_per_block + warp;
-  const uint32_t stage_a = smem_u32(status_stage) + warp * (P.off_child != BF_OFF_NONE ? P.state_stride + P.topo_bytes + 256u : 0u);
+  const uint32_t stage_a = smem_u32(status_stage) + warp * pass_stage_bytes(P.off_child, P.state_stride, P.topo_bytes);
   RunStatus s;
   if (!kList) {
     uint32_t ne = 0;
@@ -1481,53 +1503,28 @@ __global__ void __launch_bounds__(256, 1) status_runs(const StatusParams P) {
       ne = s.rec.n_events;
       if (lane == 0) P.run_events[i] = ne;
     }
-    if (lane == 0) warp_events[warp] = ne;
-    __syncthreads();
-    if (threadIdx.x == 0) {
-      unsigned long long sum = 0;
-      for (uint32_t w = 0; w < P.warps_per_block; ++w) sum += warp_events[w];
-      P.cta_events[blockIdx.x] = sum;
-    }
+    store_cta_totals<1>(ne, P.cta, WordPart{});
     return;
   }
   if (i >= P.n) return;
   run_status(P, i, lane, stage_a, s);
-  const uint32_t first = blockIdx.x * P.warps_per_block;
-  const unsigned long long base = P.cta_events[blockIdx.x] + redux_add(first + lane < i ? P.run_events[first + lane] : 0u);
-  s.rec.first_event = (uint32_t)base;
+  unsigned long long base[1];
+  run_offsets<1>(P.cta, P.run_events, blockIdx.x * P.warps_per_block, i, WordPart{}, base);
+  s.rec.first_event = (uint32_t)base[0];
   if (lane == 0) {
     const uint4* v = reinterpret_cast<const uint4*>(&s.rec);
     uint4* o = reinterpret_cast<uint4*>(P.records + i);
     o[0] = v[0]; o[1] = v[1];
   }
-  const uint32_t mine = (uint32_t)__popc(s.EV);
-  uint32_t incl = mine;
-  for (uint32_t d = 1; d < 32; d <<= 1) {
-    const uint32_t x = __shfl_up_sync(FULL, incl, d);
-    if (lane >= d) incl += x;
-  }
-  unsigned long long pos = base + incl - mine;
-  if (pos >= P.events_cap) return;
-  for (uint32_t x = s.EV; x; x &= x - 1u, ++pos) {
-    const uint32_t b = (uint32_t)__ffs(x) - 1u;
+  emit_bits(s.EV, base[0], P.events_cap, [&](uint32_t b, unsigned long long at) {
     const uint32_t ph = ((s.p0 >> b) & 1u) | ((s.p1 >> b) & 1u) << 1 | ((s.p2 >> b) & 1u) << 2 | ((s.p3 >> b) & 1u) << 3;
     const uint32_t kind = ((s.FL >> b) & 1u) ? BF_STATUS_EVT_FAILED : BF_STATUS_EVT_ALLOWED;
-    if (pos < P.events_cap) P.events[pos] = (uint16_t)((lane * 32u + b) | ph << 10 | kind << 14);
-  }
+    P.events[at] = (uint16_t)((lane * 32u + b) | ph << 10 | kind << 14);
+  });
 }
 
 cudaError_t launch_status(const StatusParams& P, uint32_t smem_bytes, cudaStream_t stream) {
-  if (P.n == 0) return cudaSuccess;
-  if (smem_bytes > 48u * 1024u) {
-    cudaError_t e = cudaFuncSetAttribute(status_runs<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes);
-    if (e == cudaSuccess) e = cudaFuncSetAttribute(status_runs<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes);
-    if (e != cudaSuccess) return e;
-  }
-  const uint32_t grid = (P.n - 1u) / P.warps_per_block + 1u, threads = 32u * P.warps_per_block;
-  status_runs<false><<<grid, threads, smem_bytes, stream>>>(P);
-  cta_scan<1><<<1, 1024, 0, stream>>>(P.cta_events, P.total, grid);
-  status_runs<true><<<grid, threads, smem_bytes, stream>>>(P);
-  return cudaGetLastError();
+  return launch_listing<1>(status_runs<false>, status_runs<true>, P, smem_bytes, stream);
 }
 
 // ---- rewrites of a single pass (bf_resident_commit_rewrites) ------------------------------------------------------------------
@@ -1540,7 +1537,7 @@ __global__ void __launch_bounds__(256, 1) rewrite_runs(const RewriteParams P) {
   const uint32_t warp = threadIdx.x >> 5, lane = threadIdx.x & 31u;
   const uint32_t r = blockIdx.x * P.warps_per_block + warp;
   if (r >= P.n_runs) return;
-  const uint32_t stage_a = smem_u32(rewrite_stage) + warp * (P.off_child != BF_OFF_NONE ? P.state_stride + P.topo_bytes + 256u : 0u);
+  const uint32_t stage_a = smem_u32(rewrite_stage) + warp * pass_stage_bytes(P.off_child, P.state_stride, P.topo_bytes);
   const uint8_t* rec = P.state + (size_t)r * P.state_stride;
   const uint32_t summary = *reinterpret_cast<const uint32_t*>(P.result + (size_t)r * P.result_stride);
   const uint32_t slot = *reinterpret_cast<const uint32_t*>(rec);
@@ -1569,10 +1566,7 @@ __global__ void __launch_bounds__(256, 1) rewrite_runs(const RewriteParams P) {
 
 cudaError_t launch_rewrites(const RewriteParams& P, uint32_t smem_bytes, cudaStream_t stream) {
   if (P.n_runs == 0) return cudaSuccess;
-  if (smem_bytes > 48u * 1024u) {
-    const cudaError_t e = cudaFuncSetAttribute(rewrite_runs, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes);
-    if (e != cudaSuccess) return e;
-  }
+  if (const cudaError_t e = allow_smem(rewrite_runs, smem_bytes)) return e;
   const uint32_t grid = (P.n_runs - 1u) / P.warps_per_block + 1u;
   rewrite_runs<<<grid, 32u * P.warps_per_block, smem_bytes, stream>>>(P);
   return cudaGetLastError();
@@ -1696,26 +1690,22 @@ DI void run_drift(const ResyncParams& P, uint32_t i, uint32_t lane, uint32_t sta
         ((sel & kSelFlags) && d.flags_dev != d.flags_rec ? 1u : 0u);
 }
 
-// Writes one item per set bit of this lane's `bits` (index lane * 32 + bit; values bit b of the planes a and b), lane by lane, from
-// item position pos -> the position after the warp's items.
+// One item per set bit of this lane's `bits` (index lane * 32 + bit; values bit b of the planes a and b), from item position pos
+// -> the position after the warp's items.
 DI unsigned long long emit_words(const ResyncParams& P, uint32_t lane, uint32_t run, uint32_t field, uint32_t bits,
                                  unsigned long long pos, uint32_t a0, uint32_t a1, uint32_t a2, uint32_t a3, uint32_t b0, uint32_t b1,
                                  uint32_t b2, uint32_t b3) {
-  const uint32_t mine = (uint32_t)__popc(bits);
-  uint32_t incl = mine;
-  for (uint32_t s = 1; s < 32; s <<= 1) {
-    const uint32_t x = __shfl_up_sync(FULL, incl, s);
-    if (lane >= s) incl += x;
-  }
-  unsigned long long at = pos + incl - mine;
-  for (uint32_t x = bits; x && at < P.items_cap; x &= x - 1u, ++at) {
-    const uint32_t b = (uint32_t)__ffs(x) - 1u;
+  return emit_bits(bits, pos, P.items_cap, [&](uint32_t b, unsigned long long at) {
     const uint32_t dv = ((a0 >> b) & 1u) | ((a1 >> b) & 1u) << 1 | ((a2 >> b) & 1u) << 2 | ((a3 >> b) & 1u) << 3;
     const uint32_t rv = ((b0 >> b) & 1u) | ((b1 >> b) & 1u) << 1 | ((b2 >> b) & 1u) << 2 | ((b3 >> b) & 1u) << 3;
     reinterpret_cast<uint4*>(P.items)[at] = make_uint4(run, (lane * 32u + b) | field << 16, dv, rv);
-  }
-  return pos + __shfl_sync(FULL, incl, 31);
+  });
 }
+
+// a listed run's item count's share of the items (k = 0) and of the drifted runs (k = 1)
+struct DriftPart {
+  DI uint32_t operator()(uint32_t w, uint32_t k) const { return k ? (w ? 1u : 0u) : w; }
+};
 
 // Count (kList = false): each listed run's items, and each CTA's items and drifted runs.  List (kList = true, after cta_scan): the
 // runs with items again, their items from the offset of the CTAs before and the warps before in the CTA, their drifted entries and,
@@ -1723,10 +1713,9 @@ DI unsigned long long emit_words(const ResyncParams& P, uint32_t lane, uint32_t 
 template <bool kList>
 __global__ void __launch_bounds__(256, 1) resync_runs(const ResyncParams P) {
   extern __shared__ __align__(16) uint8_t resync_stage[];
-  __shared__ uint32_t warp_items[kStatusStaticSmem / 4];
   const uint32_t warp = threadIdx.x >> 5, lane = threadIdx.x & 31u;
   const uint32_t i = blockIdx.x * P.warps_per_block + warp;
-  const uint32_t stage_a = smem_u32(resync_stage) + warp * (P.off_child != BF_OFF_NONE ? P.state_stride + P.topo_bytes + 256u : 0u);
+  const uint32_t stage_a = smem_u32(resync_stage) + warp * pass_stage_bytes(P.off_child, P.state_stride, P.topo_bytes);
   RunDrift d;
   if (!kList) {
     uint32_t ni = 0;
@@ -1735,24 +1724,15 @@ __global__ void __launch_bounds__(256, 1) resync_runs(const ResyncParams P) {
       ni = d.n;
       if (lane == 0) P.run_items[i] = ni;
     }
-    if (lane == 0) warp_items[warp] = ni;
-    __syncthreads();
-    if (threadIdx.x == 0) {
-      unsigned long long sum = 0, drifted = 0;
-      for (uint32_t w = 0; w < P.warps_per_block; ++w) { sum += warp_items[w]; drifted += warp_items[w] ? 1u : 0u; }
-      const uint32_t n_ctas = (P.n - 1u) / P.warps_per_block + 1u;
-      P.cta[blockIdx.x] = sum;
-      P.cta[n_ctas + blockIdx.x] = drifted;
-    }
+    store_cta_totals<2>(ni, P.cta, DriftPart{});
     return;
   }
   if (i >= P.n || P.run_items[i] == 0u) return;
   run_drift(P, i, lane, stage_a, d);
-  const uint32_t first = blockIdx.x * P.warps_per_block, n_ctas = (P.n - 1u) / P.warps_per_block + 1u;
-  const uint32_t before = first + lane < i ? P.run_items[first + lane] : 0u;
-  unsigned long long pos = P.cta[blockIdx.x] + redux_add(before);
-  const unsigned long long at = P.cta[n_ctas + blockIdx.x] + redux_add(before ? 1u : 0u);
-  if (lane == 0 && at < P.drifted_cap) P.drifted[at] = d.r;
+  unsigned long long base[2];
+  run_offsets<2>(P.cta, P.run_items, blockIdx.x * P.warps_per_block, i, DriftPart{}, base);
+  unsigned long long pos = base[0];
+  if (lane == 0 && base[1] < P.drifted_cap) P.drifted[base[1]] = d.r;
   const uint32_t sel = P.fields;
   const bool slot = d.slot_dev != d.slot_rec;
   if (slot) {
@@ -1768,19 +1748,10 @@ __global__ void __launch_bounds__(256, 1) resync_runs(const ResyncParams P) {
         const uint32_t x = x0 + lane;
         uint32_t vd = 0, vr = 0;
         const uint32_t m = x < cw ? child_diff(P, d, x, vd, vr) : 0u;
-        const uint32_t mine = (uint32_t)__popc(m);
-        uint32_t incl = mine;
-        for (uint32_t s = 1; s < 32; s <<= 1) {
-          const uint32_t y = __shfl_up_sync(FULL, incl, s);
-          if (lane >= s) incl += y;
-        }
-        unsigned long long a = pos + incl - mine;
-        for (uint32_t y = m; y && a < P.items_cap; y &= y - 1u, ++a) {
-          const uint32_t k = (uint32_t)__ffs(y) - 1u;
+        pos = emit_bits(m, pos, P.items_cap, [&](uint32_t k, unsigned long long a) {
           reinterpret_cast<uint4*>(P.items)[a] =
               make_uint4(d.r, (8u * x + k) | (uint32_t)BF_DELTA_CHILD << 16, (vd >> (4u * k)) & 0xFu, (vr >> (4u * k)) & 0xFu);
-        }
-        pos += __shfl_sync(FULL, incl, 31);
+        });
       }
     }
     if (lane == 0) {
@@ -1839,17 +1810,7 @@ __global__ void __launch_bounds__(256, 1) resync_runs(const ResyncParams P) {
 }
 
 cudaError_t launch_resync(const ResyncParams& P, uint32_t smem_bytes, cudaStream_t stream) {
-  if (P.n == 0) return cudaSuccess;
-  if (smem_bytes > 48u * 1024u) {
-    cudaError_t e = cudaFuncSetAttribute(resync_runs<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes);
-    if (e == cudaSuccess) e = cudaFuncSetAttribute(resync_runs<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes);
-    if (e != cudaSuccess) return e;
-  }
-  const uint32_t grid = (P.n - 1u) / P.warps_per_block + 1u, threads = 32u * P.warps_per_block;
-  resync_runs<false><<<grid, threads, smem_bytes, stream>>>(P);
-  cta_scan<2><<<1, 1024, 0, stream>>>(P.cta, P.total, grid);
-  resync_runs<true><<<grid, threads, smem_bytes, stream>>>(P);
-  return cudaGetLastError();
+  return launch_listing<2>(resync_runs<false>, resync_runs<true>, P, smem_bytes, stream);
 }
 
 }  // namespace bf

@@ -75,6 +75,69 @@ struct CallStage {
   }
 };
 
+// One output list of a call (bf_resident_schedule, _status, _resync, _commit_journal): the kernels write it in place when the
+// caller's buffer is pinned, and, for items the kernels store as uint4 (vec16), 16-byte aligned; else into the call's scratch
+// (stage(), or stage_at() once the number of items is known), from where copy() or copy_async() bring min(total, cap) items back.
+template <typename T>
+struct OutList {
+  T* host;
+  uint64_t cap;          // clamped by the caller
+  T* dev = nullptr;      // where the kernels write
+  bool staged = false;
+  OutList(void* buf, uint64_t cap, bool vec16 = false) : host(static_cast<T*>(buf)), cap(cap) {
+    if (cap && (!vec16 || reinterpret_cast<uintptr_t>(buf) % 16 == 0)) dev = static_cast<T*>(bf::pinned_dev(buf));
+    staged = cap && !dev;
+  }
+  // a and b are written in place only together: when one is staged, both are
+  template <typename U>
+  void pair(OutList<U>& b) {
+    if (staged == b.staged) return;
+    dev = nullptr; b.dev = nullptr;
+    staged = cap != 0; b.staged = b.cap != 0;
+  }
+  void stage(CallStage& st) { if (staged) st.out(dev, cap); }
+  void stage_at(CallStage& st, uint64_t total) {   // the staging holds what the list gets and the copy brings back, no more
+    if (!staged) return;
+    cap = std::min(total, cap);
+    if (cap) st.out(dev, cap);
+  }
+  size_t bytes(uint64_t total) const { return staged ? (size_t)std::min(total, cap) * sizeof(T) : 0; }
+  cudaError_t copy_async(uint64_t total, cudaStream_t s) const {
+    const size_t b = bytes(total);
+    return b ? cudaMemcpyAsync(host, dev, b, cudaMemcpyDeviceToHost, s) : cudaSuccess;
+  }
+  cudaError_t copy(uint64_t total) const {
+    const size_t b = bytes(total);
+    return b ? cudaMemcpy(host, dev, b, cudaMemcpyDeviceToHost) : cudaSuccess;
+  }
+};
+
+// The shared stage of the single-pass launches (status, resync, the rewriting commit): per warp pass_stage_bytes, up to 8 warps
+// per CTA within the 227 KiB a CTA can opt in to beside the launches' static words.
+struct PassStage {
+  uint32_t wpb = 8, topo = 0, per_warp = 0;
+  uint32_t smem() const { return wpb * per_warp; }
+};
+static int plan_pass_stage(bf_ctx* c, const bf_layout& L, PassStage& ps) {
+  if (L.off_child == BF_OFF_NONE) return BF_OK;   // no stage H, no stage
+  ps.topo = bf::largest_record(c, L.words);
+  ps.per_warp = bf::pass_stage_bytes(L.off_child, L.state_stride, ps.topo);
+  ps.wpb = std::min<uint32_t>(8u, (227u * 1024u - bf::kStatusStaticSmem) / ps.per_warp);
+  return ps.wpb ? BF_OK : fail(c, BF_ENOMEM, "a topology record and a state record do not fit one warp's shared memory");
+}
+
+// The listed runs of a status or resync call: n_runs within the batch, and runs ascending below n_runs, or runs == NULL for
+// every run of [0, n_runs)
+static int check_run_list(bf_ctx* c, const Resident* r, uint32_t n_runs, const uint32_t* runs, uint32_t n) {
+  if (n_runs > r->cap) return fail(c, BF_EINVAL, "n_runs exceeds the resident batch");
+  if (!runs && n != n_runs) return fail(c, BF_EINVAL, "runs == NULL lists every run of [0, n_runs): n must equal n_runs");
+  for (uint32_t i = 0; runs && i < n; ++i) {
+    if (runs[i] >= n_runs) return fail(c, BF_EINVAL, "runs[" + std::to_string(i) + "] is not below n_runs");
+    if (i && runs[i] <= runs[i - 1]) return fail(c, BF_EINVAL, "runs[" + std::to_string(i) + "] does not ascend");
+  }
+  return BF_OK;
+}
+
 // Request i names `run` (below cap); each run may be named once.  seen holds request index + 1 per run named so far.
 static int name_run_once(bf_ctx* c, std::vector<uint32_t>& seen, uint32_t cap, uint32_t run, uint32_t i) {
   if (seen.empty()) seen.assign(cap, 0u);
@@ -1066,7 +1129,7 @@ int bf_resident_schedule(bf_ctx* c, const bf_sched_tables* t, uint32_t now, bf_r
   BF_CUDA(c, cudaSetDevice(c->device));
   cudaStream_t s = c->stream;
   if (int rc = bf::sync_slots(c, s)) return rc;   // topology puts and drops since the ticks count as they stand now
-  // tables | totals | per part: run events | CTA listed | CTA events | two totals | staged lists
+  // tables | totals | per part: run events | CTA listed runs and events | two totals | staged lists
   const size_t ns = t->n_stories, nq = t->n_queues;
   bf::SchedParams S{};
   CallStage st;
@@ -1078,23 +1141,24 @@ int bf_resident_schedule(bf_ctx* c, const bf_sched_tables* t, uint32_t now, bf_r
   if (t->queue_max_priority_base) st.up(S.queue_maxprio_base, t->queue_max_priority_base, nq);
   st.out(S.story_running, ns); st.out(S.queue_running, nq); st.out(S.queue_maxprio, nq); st.out(S.global_running, 1);
   // each part's lists go straight into the caller's buffers when they are pinned, else into staged ones copied after the call
-  struct Plan { bf::ResSchedParams R; bool stage_runs, stage_events; };
-  std::vector<Plan> plan(n_parts);
+  struct Plan {
+    bf::ResSchedParams R;
+    OutList<uint32_t> runs;
+    OutList<bf_sched_header> heads;
+    OutList<uint16_t> events;
+  };
+  std::vector<Plan> plan;
+  plan.reserve(n_parts);   // the staged lists' pointers are taken in place
   for (uint32_t i = 0; i < n_parts; ++i) {
     const bf_resident_sched_part& p = parts[i];
-    Plan& q = plan[i];
-    bf::ResSchedParams& R = q.R;
+    const uint32_t runs_cap = std::min(p.runs_cap, p.n_runs);
+    plan.push_back(Plan{{}, {p.runs, runs_cap}, {p.heads, runs_cap},
+                        {p.events, std::min<uint64_t>(p.events_cap, (uint64_t)p.n_runs * rs[i]->L.words * 32)}});
+    Plan& q = plan.back();
+    q.runs.pair(q.heads);
     const size_t grid = ((size_t)p.n_runs + 255) / 256;
-    R.runs_cap = std::min(p.runs_cap, p.n_runs);
-    R.events_cap = std::min<uint64_t>(p.events_cap, (uint64_t)p.n_runs * rs[i]->L.words * 32);
-    R.runs = R.runs_cap ? static_cast<uint32_t*>(bf::pinned_dev(p.runs)) : nullptr;
-    R.heads = R.runs_cap ? static_cast<bf_sched_header*>(bf::pinned_dev(p.heads)) : nullptr;
-    R.events = R.events_cap ? static_cast<uint16_t*>(bf::pinned_dev(p.events)) : nullptr;
-    q.stage_runs = R.runs_cap && !(R.runs && R.heads);
-    q.stage_events = R.events_cap && !R.events;
-    st.out(R.run_events, p.n_runs); st.out(R.cta_listed, grid); st.out(R.cta_events, grid); st.out(R.totals, 2);
-    if (q.stage_runs) { st.out(R.runs, R.runs_cap); st.out(R.heads, R.runs_cap); }
-    if (q.stage_events) st.out(R.events, R.events_cap);
+    st.out(q.R.run_events, p.n_runs); st.out(q.R.cta, 2 * grid); st.out(q.R.totals, 2);
+    q.runs.stage(st); q.heads.stage(st); q.events.stage(st);
   }
   if (int rc = st.send(c, "bf_resident_schedule")) return rc;
   S.n_stories = t->n_stories; S.n_queues = t->n_queues; S.global_limit = t->global_limit; S.global_base = t->global_running_base;
@@ -1116,8 +1180,11 @@ int bf_resident_schedule(bf_ctx* c, const bf_sched_tables* t, uint32_t now, bf_r
     for (uint32_t i = 0; i < n_parts && e == cudaSuccess; ++i)
       if (parts[i].n_runs) { e = bf::launch_schedule(part_params(i), (uint32_t)c->sm_count, s, bf::kSchedCount); ++launches; }
     for (uint32_t i = 0; i < n_parts && e == cudaSuccess; ++i) {
-      bf::ResSchedParams R = plan[i].R;
+      const Plan& q = plan[i];
+      bf::ResSchedParams R = q.R;
       R.S = part_params(i);
+      R.runs = q.runs.dev; R.heads = q.heads.dev; R.events = q.events.dev;
+      R.runs_cap = (uint32_t)q.runs.cap; R.events_cap = q.events.cap;
       R.base_runs = rs[i]->areas.sched_base_runs;
       if (parts[i].n_runs) {
         e = bf::launch_resident_schedule(R, s);
@@ -1149,13 +1216,9 @@ int bf_resident_schedule(bf_ctx* c, const bf_sched_tables* t, uint32_t now, bf_r
     p.full = p.n_listed == p.n_runs ? 1u : 0u;
     rs[i]->areas.sched_base_runs = p.n_runs;
     rs[i]->scheduled = std::max<int64_t>(rs[i]->scheduled, p.n_runs);
-    const uint32_t nl = std::min(p.n_listed, q.R.runs_cap);
-    if (nl && q.stage_runs) {
-      BF_CUDA(c, cudaMemcpy(p.runs, q.R.runs, (size_t)nl * 4, cudaMemcpyDeviceToHost));
-      BF_CUDA(c, cudaMemcpy(p.heads, q.R.heads, (size_t)nl * sizeof(bf_sched_header), cudaMemcpyDeviceToHost));
-    }
-    const uint64_t ne = std::min<uint64_t>(p.n_events, q.R.events_cap);
-    if (ne && q.stage_events) BF_CUDA(c, cudaMemcpy(p.events, q.R.events, (size_t)ne * 2, cudaMemcpyDeviceToHost));
+    BF_CUDA(c, q.runs.copy(p.n_listed));
+    BF_CUDA(c, q.heads.copy(p.n_listed));
+    BF_CUDA(c, q.events.copy(p.n_events));
   }
   return BF_OK;
 }
@@ -1305,27 +1368,18 @@ static int resident_commit(bf_ctx* c, uint32_t h, uint32_t n_runs, const bf_comm
   st.up(P.counts, zero_counts, n_counts);
   st.up(P.entries, sorted.data(), n);
   const uint32_t grid = (n_runs - 1u) / 8u + 1u;
-  bool staged_items = false, staged_runs = false;
-  if (journaled) {   // pinned items / runs are written in place; the others are staged once their numbers are known
-    P.items_cap = journal->items_cap;
-    P.runs_cap = std::min(journal->runs_cap, n_runs);
-    P.items = P.items_cap && reinterpret_cast<uintptr_t>(journal->items) % 16 == 0 ? static_cast<bf_commit_write*>(bf::pinned_dev(journal->items)) : nullptr;
-    P.runs = P.runs_cap ? static_cast<uint32_t*>(bf::pinned_dev(journal->runs)) : nullptr;
-    staged_items = P.items_cap && !P.items;
-    staged_runs = P.runs_cap && !P.runs;
+  // pinned items / runs are written in place; the others are staged once their numbers are known
+  OutList<bf_commit_write> items(journaled ? journal->items : nullptr, journaled ? journal->items_cap : 0, true);
+  OutList<uint32_t> listed(journaled ? journal->runs : nullptr, journaled ? std::min(journal->runs_cap, n_runs) : 0);
+  if (journaled) {
     st.out(P.run_items, n_runs);
     st.out(P.cta, 2 * (size_t)grid);
     st.out(P.total, 2);
   }
   bf::RewriteParams W{};
-  uint32_t rw_wpb = 8, rw_topo = 0, rw_per_warp = 0;
+  PassStage ps;
   if (rewrites) {   // the shared stage of bf_resident_status per warp for the joins
-    if (L.off_child != BF_OFF_NONE) {
-      rw_topo = bf::largest_record(c, L.words);
-      rw_per_warp = L.state_stride + rw_topo + 256u;
-      rw_wpb = std::min<uint32_t>(8u, (227u * 1024u - bf::kStatusStaticSmem) / rw_per_warp);
-      if (!rw_wpb) return fail(c, BF_ENOMEM, "a topology record and a state record do not fit one warp's shared memory");
-    }
+    if (int rc = plan_pass_stage(c, L, ps)) return rc;
     st.out(W.rw_runs, n_runs);
     st.out(W.rw_planes, (size_t)n_runs * 4u * L.words);
   }
@@ -1344,16 +1398,17 @@ static int resident_commit(bf_ctx* c, uint32_t h, uint32_t n_runs, const bf_comm
   cudaError_t e = cudaSuccess;
   if (rewrites) {
     W.state = r->d_state; W.result = r->d_result; W.slots = c->slots_dev; W.n_slots = P.n_slots; W.runctl = A.runctl;
-    W.n_runs = n_runs; W.warps_per_block = rw_wpb;
+    W.n_runs = n_runs; W.warps_per_block = ps.wpb;
     W.words = L.words; W.state_stride = L.state_stride; W.off_phase = L.off_phase; W.off_decision = L.off_decision;
-    W.off_child = L.off_child; W.topo_bytes = rw_topo; W.result_stride = L.result_stride;
-    e = bf::launch_rewrites(W, rw_wpb * rw_per_warp, s);
+    W.off_child = L.off_child; W.topo_bytes = ps.topo; W.result_stride = L.result_stride;
+    e = bf::launch_rewrites(W, ps.smem(), s);
     P.rw_runs = W.rw_runs; P.rw_planes = W.rw_planes; P.rewritten = P.counts + 7;
   }
   uint32_t* host = c->pinned->commit;
+  unsigned long long* totals = c->pinned->list_totals;
   if (e == cudaSuccess) e = bf::launch_commit(P, false, s);
   if (e == cudaSuccess) e = cudaMemcpyAsync(host, P.offender, 8, cudaMemcpyDeviceToHost, s);
-  if (e == cudaSuccess && journaled) e = cudaMemcpyAsync(c->pinned->commit_journal, P.total, 16, cudaMemcpyDeviceToHost, s);
+  if (e == cudaSuccess && journaled) e = cudaMemcpyAsync(totals, P.total, 16, cudaMemcpyDeviceToHost, s);
   if (int rc = bf::end_call(c, e, "bf_resident_commit (check)")) return rc;
   c->stats.kernel_launches += (journaled ? 2 : 1) + (rewrites ? 1 : 0);
   uint64_t key;
@@ -1368,23 +1423,21 @@ static int resident_commit(bf_ctx* c, uint32_t h, uint32_t n_runs, const bf_comm
                                    : why == bf::kCommitNoPhase   ? "a launched stop step has no BF_COMMIT_PHASE entry"
                                                                  : "a timing that writes needs decision planes (BF_F_DECISION)"));
   }
-  const uint64_t n_items = journaled ? c->pinned->commit_journal[0] : 0;
-  const uint32_t n_listed = journaled ? (uint32_t)c->pinned->commit_journal[1] : 0;
-  if (staged_items || staged_runs) {   // the staging holds what the apply lists and the copies bring back, no more
-    if (staged_items) P.items_cap = std::min<uint64_t>(n_items, P.items_cap);
-    if (staged_runs) P.runs_cap = std::min(n_listed, P.runs_cap);
-    if (staged_items && P.items_cap) st.out(P.items, P.items_cap);
-    if (staged_runs && P.runs_cap) st.out(P.runs, P.runs_cap);
+  const uint64_t n_items = journaled ? totals[0] : 0;
+  const uint32_t n_listed = journaled ? (uint32_t)totals[1] : 0;
+  if (items.staged || listed.staged) {
+    items.stage_at(st, n_items);
+    listed.stage_at(st, n_listed);
     if (int rc = st.grow(c, sent, "bf_resident_commit")) return rc;
     if (P.arm.tim) P.arm.out = P.counts + 5;   // the arms' words behind the counts, where grow() may have moved them
     if (rewrites) { P.rw_runs = W.rw_runs; P.rw_planes = W.rw_planes; P.rewritten = P.counts + 7; }
   }
+  P.items = items.dev; P.items_cap = items.cap;
+  P.runs = listed.dev; P.runs_cap = (uint32_t)listed.cap;
   e = bf::launch_commit(P, true, s);
   if (e == cudaSuccess) e = cudaMemcpyAsync(host, P.counts, 4 * n_counts, cudaMemcpyDeviceToHost, s);
-  if (const uint64_t k = std::min<uint64_t>(n_items, P.items_cap); e == cudaSuccess && k && staged_items)
-    e = cudaMemcpyAsync(journal->items, P.items, (size_t)k * sizeof(bf_commit_write), cudaMemcpyDeviceToHost, s);
-  if (const uint32_t k = std::min(n_listed, P.runs_cap); e == cudaSuccess && k && staged_runs)
-    e = cudaMemcpyAsync(journal->runs, P.runs, (size_t)k * 4, cudaMemcpyDeviceToHost, s);
+  if (e == cudaSuccess) e = items.copy_async(n_items, s);
+  if (e == cudaSuccess) e = listed.copy_async(n_listed, s);
   if (int rc = r->sync_in_place(c, e, "bf_resident_commit")) { r->state_changed(c); return rc; }
   c->stats.kernel_launches += 1;
   uint32_t k[8];
@@ -1428,58 +1481,45 @@ int bf_resident_status(bf_ctx* c, uint32_t h, uint32_t n_runs, const uint32_t* r
   if (!out || out->struct_size != sizeof(bf_status_out)) return fail(c, BF_EINVAL, "null bf_status_out or bad struct_size");
   if (!r) return BF_EINVAL;
   const bf_layout& L = r->L;
-  if (n_runs > r->cap) return fail(c, BF_EINVAL, "n_runs exceeds the resident batch");
-  if (!runs && n != n_runs) return fail(c, BF_EINVAL, "runs == NULL lists every run of [0, n_runs): n must equal n_runs");
-  for (uint32_t i = 0; runs && i < n; ++i) {
-    if (runs[i] >= n_runs) return fail(c, BF_EINVAL, "runs[" + std::to_string(i) + "] is not below n_runs");
-    if (i && runs[i] <= runs[i - 1]) return fail(c, BF_EINVAL, "runs[" + std::to_string(i) + "] does not ascend");
-  }
+  if (int rc = check_run_list(c, r, n_runs, runs, n)) return rc;
   if (n && !out->records) return fail(c, BF_EINVAL, "null records");
   if (out->events_cap && !out->events) return fail(c, BF_EINVAL, "null events with a non-zero events_cap");
-  uint32_t wpb = 8, topo = 0, per_warp = 0;
-  if (L.off_child != BF_OFF_NONE) {   // a shared stage per warp for the parallel join
-    topo = bf::largest_record(c, L.words);
-    per_warp = L.state_stride + topo + 256u;
-    wpb = std::min<uint32_t>(8u, (227u * 1024u - bf::kStatusStaticSmem) / per_warp);
-    if (!wpb) return fail(c, BF_ENOMEM, "a topology record and a state record do not fit one warp's shared memory");
-  }
+  PassStage ps;
+  if (int rc = plan_pass_stage(c, L, ps)) return rc;
   out->n_events = 0;
   if (n == 0) return BF_OK;
   BF_CUDA(c, cudaSetDevice(c->device));
   cudaStream_t s = c->stream;
   if (int rc = bf::sync_slots(c, s)) return rc;
-  const uint32_t grid = (n - 1u) / wpb + 1u;
+  const uint32_t grid = (n - 1u) / ps.wpb + 1u;
   // the list is at most n * 32 * words long (a run on a topology past steps_max but within the words is live): a larger
   // events_cap stages no more
-  const uint64_t cap = std::min<uint64_t>(out->events_cap, (uint64_t)n * 32u * L.words);
+  OutList<bf_status_rec> records(out->records, n);
+  OutList<uint16_t> events(out->events, std::min<uint64_t>(out->events_cap, (uint64_t)n * 32u * L.words));
   bf::StatusParams P{};
   P.runs = runs ? static_cast<const uint32_t*>(bf::pinned_dev(runs)) : nullptr;
-  P.records = static_cast<bf_status_rec*>(bf::pinned_dev(out->records));
-  P.events = cap ? static_cast<uint16_t*>(bf::pinned_dev(out->events)) : nullptr;
-  const bool staged_records = !P.records, staged_events = cap && !P.events;
   CallStage st;
   if (runs && !P.runs) st.up(P.runs, runs, n);
   st.out(P.run_events, n);
-  st.out(P.cta_events, grid);
+  st.out(P.cta, grid);
   st.out(P.total, 1);
-  if (staged_records) st.out(P.records, n);
-  if (staged_events) st.out(P.events, cap);
+  records.stage(st);
+  events.stage(st);
   if (int rc = st.send(c, "bf_resident_status")) return rc;
+  P.records = records.dev; P.events = events.dev; P.events_cap = events.cap;
   P.state = r->d_state; P.slots = c->slots_dev; P.n_slots = (uint32_t)c->slots_host.size();
   P.runctl = r->areas_view().runctl;
-  P.n = n; P.warps_per_block = wpb;
+  P.n = n; P.warps_per_block = ps.wpb;
   P.words = L.words; P.state_stride = L.state_stride; P.off_phase = L.off_phase; P.off_decision = L.off_decision;
-  P.off_child = L.off_child; P.topo_bytes = topo;
-  P.events_cap = cap;
-  cudaError_t e = bf::launch_status(P, wpb * per_warp, s);
-  if (e == cudaSuccess) e = cudaMemcpyAsync(&c->pinned->status_events, P.total, 8, cudaMemcpyDeviceToHost, s);
-  if (e == cudaSuccess && staged_records) e = cudaMemcpyAsync(out->records, P.records, (size_t)n * sizeof(bf_status_rec), cudaMemcpyDeviceToHost, s);
+  P.off_child = L.off_child; P.topo_bytes = ps.topo;
+  unsigned long long* totals = c->pinned->list_totals;
+  cudaError_t e = bf::launch_status(P, ps.smem(), s);
+  if (e == cudaSuccess) e = cudaMemcpyAsync(totals, P.total, 8, cudaMemcpyDeviceToHost, s);
+  if (e == cudaSuccess) e = records.copy_async(n, s);
   if (int rc = bf::end_call(c, e, "bf_resident_status")) return rc;
   c->stats.kernel_launches += 3;
-  const uint64_t total = c->pinned->status_events;
-  if (const uint64_t listed = std::min<uint64_t>(total, cap); listed && staged_events)
-    BF_CUDA(c, cudaMemcpy(out->events, P.events, (size_t)listed * 2, cudaMemcpyDeviceToHost));
-  out->n_events = total;
+  BF_CUDA(c, events.copy(totals[0]));
+  out->n_events = totals[0];
   return BF_OK;
 }
 
@@ -1494,12 +1534,7 @@ int bf_resident_resync(bf_ctx* c, uint32_t h, bf_resync* q) {
   if (!r) return BF_EINVAL;
   const bf_layout& L = r->L;
   const uint32_t n = q->n, *runs = q->runs;
-  if (q->n_runs > r->cap) return fail(c, BF_EINVAL, "n_runs exceeds the resident batch");
-  if (!runs && n != q->n_runs) return fail(c, BF_EINVAL, "runs == NULL lists every run of [0, n_runs): n must equal n_runs");
-  for (uint32_t i = 0; runs && i < n; ++i) {
-    if (runs[i] >= q->n_runs) return fail(c, BF_EINVAL, "runs[" + std::to_string(i) + "] is not below n_runs");
-    if (i && runs[i] <= runs[i - 1]) return fail(c, BF_EINVAL, "runs[" + std::to_string(i) + "] does not ascend");
-  }
+  if (int rc = check_run_list(c, r, q->n_runs, runs, n)) return rc;
   if (n && !q->records) return fail(c, BF_EINVAL, "null records");
   if ((q->drifted_cap && !q->drifted) || (q->items_cap && !q->items)) return fail(c, BF_EINVAL, "null drifted / items with a non-zero cap");
   if (q->flags & ~BF_RESYNC_CHECK) return fail(c, BF_EINVAL, "unknown flags");
@@ -1517,13 +1552,8 @@ int bf_resident_resync(bf_ctx* c, uint32_t h, bf_resync* q) {
   if (L.off_cond == BF_OFF_NONE) fields &= ~BF_RESYNC_FIELD(BF_DELTA_COND);
   if (L.off_decision == BF_OFF_NONE) fields &= ~BF_RESYNC_FIELD(BF_DELTA_DECISION);
   if (L.off_child == BF_OFF_NONE) fields &= ~BF_RESYNC_FIELD(BF_DELTA_CHILD);
-  uint32_t wpb = 8, topo = 0, per_warp = 0;
-  if (L.off_child != BF_OFF_NONE) {   // a shared stage per warp for the parallel joins, as bf_resident_status
-    topo = bf::largest_record(c, L.words);
-    per_warp = L.state_stride + topo + 256u;
-    wpb = std::min<uint32_t>(8u, (227u * 1024u - bf::kStatusStaticSmem) / per_warp);
-    if (!wpb) return fail(c, BF_ENOMEM, "a topology record and a state record do not fit one warp's shared memory");
-  }
+  PassStage ps;
+  if (int rc = plan_pass_stage(c, L, ps)) return rc;
   q->n_drifted = q->n_written = 0;
   q->n_items = 0;
   if (n == 0) return BF_OK;
@@ -1531,16 +1561,13 @@ int bf_resident_resync(bf_ctx* c, uint32_t h, bf_resync* q) {
   cudaStream_t s = c->stream;
   if (int rc = bf::sync_slots(c, s)) return rc;
   const bool check = q->flags & BF_RESYNC_CHECK;
-  const uint32_t grid = (n - 1u) / wpb + 1u;
+  const uint32_t grid = (n - 1u) / ps.wpb + 1u;
   // a run has at most one item per code, nibble and registered bit of the layout, and its flags byte: a larger cap stages no more
   const uint64_t per_run = 3ull * L.words * 32u + L.child_nibbles + 65u;
-  const uint64_t items_cap = std::min<uint64_t>(q->items_cap, (uint64_t)n * per_run);
-  const uint32_t drifted_cap = std::min(q->drifted_cap, n);
+  OutList<uint32_t> drifted_list(q->drifted, std::min(q->drifted_cap, n));
+  OutList<bf_drift> items_list(q->items, std::min<uint64_t>(q->items_cap, (uint64_t)n * per_run), true);
   bf::ResyncParams P{};
   P.runs = runs ? static_cast<const uint32_t*>(bf::pinned_dev(runs)) : nullptr;
-  P.drifted = drifted_cap ? static_cast<uint32_t*>(bf::pinned_dev(q->drifted)) : nullptr;
-  P.items = items_cap && reinterpret_cast<uintptr_t>(q->items) % 16 == 0 ? static_cast<bf_drift*>(bf::pinned_dev(q->items)) : nullptr;
-  const bool staged_drifted = drifted_cap && !P.drifted, staged_items = items_cap && !P.items;
   uint8_t* d_records;
   CallStage st;
   if (runs && !P.runs) st.up(P.runs, runs, n);
@@ -1548,21 +1575,23 @@ int bf_resident_resync(bf_ctx* c, uint32_t h, bf_resync* q) {
   st.out(P.run_items, n);
   st.out(P.cta, 2 * (size_t)grid);
   st.out(P.total, 2);
-  if (staged_drifted) st.out(P.drifted, drifted_cap);
-  if (staged_items) st.out(P.items, items_cap);
+  drifted_list.stage(st);
+  items_list.stage(st);
   if (int rc = st.send(c, "bf_resident_resync")) return rc;
   BF_CUDA(c, cudaMemcpyAsync(d_records, recs, (size_t)n * L.state_stride, cudaMemcpyHostToDevice, s));
   P.records = d_records;
   P.state = r->d_state; P.slots = c->slots_dev; P.n_slots = (uint32_t)c->slots_host.size();
   P.runctl = r->areas.d_runctl; P.areas = r->areas_view();
   P.mark = r->d_mark; P.mark_touched = r->mark_touched(); P.mark_must_list = r->mark_must_list();
-  P.n = n; P.warps_per_block = wpb;
+  P.n = n; P.warps_per_block = ps.wpb;
   P.words = L.words; P.state_stride = L.state_stride; P.off_phase = L.off_phase; P.off_cond = L.off_cond;
-  P.off_decision = L.off_decision; P.off_child = L.off_child; P.child_nibbles = L.child_nibbles; P.topo_bytes = topo;
+  P.off_decision = L.off_decision; P.off_child = L.off_child; P.child_nibbles = L.child_nibbles; P.topo_bytes = ps.topo;
   P.fields = fields; P.check = check;
-  P.drifted_cap = drifted_cap; P.items_cap = items_cap;
-  cudaError_t e = bf::launch_resync(P, wpb * per_warp, s);
-  if (e == cudaSuccess) e = cudaMemcpyAsync(c->pinned->resync, P.total, 16, cudaMemcpyDeviceToHost, s);
+  P.drifted = drifted_list.dev; P.drifted_cap = (uint32_t)drifted_list.cap;
+  P.items = items_list.dev; P.items_cap = items_list.cap;
+  unsigned long long* totals = c->pinned->list_totals;
+  cudaError_t e = bf::launch_resync(P, ps.smem(), s);
+  if (e == cudaSuccess) e = cudaMemcpyAsync(totals, P.total, 16, cudaMemcpyDeviceToHost, s);
   if (check) {
     if (int rc = bf::end_call(c, e, "bf_resident_resync")) return rc;
   } else if (int rc = r->sync_in_place(c, e, "bf_resident_resync")) {
@@ -1570,16 +1599,14 @@ int bf_resident_resync(bf_ctx* c, uint32_t h, bf_resync* q) {
     return rc;
   }
   c->stats.kernel_launches += 3;
-  const uint64_t items = c->pinned->resync[0];
-  const uint32_t drifted = (uint32_t)c->pinned->resync[1];
+  const uint64_t items = totals[0];
+  const uint32_t drifted = (uint32_t)totals[1];
   if (!check && drifted) {   // as a commit that wrote: the evaluated snapshot and the tick end (before any copy can fail)
     r->state_changed(c);
     r->pending += drifted;
   }
-  if (const uint32_t k = std::min(drifted, drifted_cap); k && staged_drifted)
-    BF_CUDA(c, cudaMemcpy(q->drifted, P.drifted, (size_t)k * 4, cudaMemcpyDeviceToHost));
-  if (const uint64_t k = std::min<uint64_t>(items, items_cap); k && staged_items)
-    BF_CUDA(c, cudaMemcpy(q->items, P.items, (size_t)k * sizeof(bf_drift), cudaMemcpyDeviceToHost));
+  BF_CUDA(c, drifted_list.copy(drifted));
+  BF_CUDA(c, items_list.copy(items));
   q->n_items = items;
   q->n_drifted = drifted;
   q->n_written = check ? 0 : drifted;

@@ -1,5 +1,6 @@
-"""The device lists of bf_resident_status, bf_resident_resync and bf_resident_commit_journal at every launch shape their offsets are
-built from, against the host models tests/runstatus.py, tests/resync.py and tests/commit_journal.py.
+"""The device lists of bf_resident_status, bf_resident_resync, bf_resident_commit_journal and bf_resident_schedule at every launch
+shape their offsets are built from, against the host models tests/runstatus.py, tests/resync.py, tests/commit_journal.py and
+tests/sched_resident.py.
 
 Each call counts per run, scans the per-CTA totals (cta_scan, in 1024-CTA chunks with a carry) and lists each run's entries from
 the CTAs before it, the warps before it in its CTA and the lanes before it in its warp.  The cases here put 8 down to 1 warps in a
@@ -21,8 +22,10 @@ from oracle.packed import child_first_of
 from tests import commit_journal as J
 from tests import resync as RS
 from tests import runstatus as ST
+from tests import schedref as SR
 from tests.test_gpu_commit_timers import put_all, random_timings
 from tests.test_gpu_resync import _subset
+from tests.test_gpu_sched_resident import Resident, _inputs, _schedule
 
 pytestmark = pytest.mark.gpu
 
@@ -576,3 +579,49 @@ def test_status_lists_every_event_past_steps_max(fr):
     check_status(fr, h, L, ts, slots, st, n, 8)
     items = check_resync(fr, h, L, RS.Topos(ts, slots), st, drifted_records(rng, L, st, [int(s) for s in slots]), n, 8)
     assert items.size
+
+
+# (CTAs of 256 runs): bf_resident_schedule's listed runs and events are scanned across 1024-CTA chunks
+SCHED_GRIDS = [1023, 1024, 1025, 2049]
+
+
+@pytest.mark.parametrize("ctas", SCHED_GRIDS)
+def test_schedule_grids_across_scan_chunks(fr, ctas):
+    """bf_resident_schedule over grids of 1023 to 2049 CTAs: a first schedule lists every run; then, before each further
+    schedule, the first 1 to 13 runs of every CTA (uneven counts) lose their baseline by an upload of their own record, and only
+    they are listed: runs, heads, events and totals against the host model, with the caps at the totals and cut at the first
+    listed run of CTA 1024 (of the last CTA on a grid of one chunk)"""
+    rng = np.random.default_rng(ctas * 17)
+    n = 256 * (ctas - 1) + 1 + ctas % 255
+    ts = topologies(rng, small_specs(rng, 12, 6, 32))
+    slots = fr.put_topologies(ts)
+    L = make_layout(32, 0, A.F_COND | A.F_DECISION | A.F_ALL_OUT)
+    st = records(rng, L, ts, slots, rng.integers(0, ts.count, size=n))
+    now = 20_000
+    tables = SR.random_tables(rng, 40, 5, n, maxprio_base=True)
+    b = Resident(fr, L, st, n, SR.from_topology_set(ts, slots))
+    try:
+        b.put(_inputs(rng, n, 40, 5, now))
+        fr.resident_tick(b.h, L, n, NONE_D)
+        cur = [b.current()]
+        got, _, _ = _schedule(fr, [b], tables, now, caps=[dict(runs_cap=n, events_cap=32 * n)], cur=cur)
+        assert got["parts"][0]["full"] == 1
+        first = np.arange(ctas) * 256
+        lose = np.minimum(1 + np.arange(ctas) * 7 % 13, n - first)
+        cut_cta = min(1024, ctas - 1)
+        for cut in (False, True):
+            for r0, k in zip(first, lose):
+                fr.resident_upload(b.h, int(r0), st[r0:r0 + k])
+                b.model.upload(int(r0), int(k))
+            fr.resident_tick(b.h, L, n, NONE_D)
+            caps = dict(runs_cap=n, events_cap=32 * n)
+            if cut:   # the same runs as the schedule before are listed, so its list gives the offsets of CTA cut_cta
+                j = int(lose[:cut_cta].sum())
+                caps = dict(runs_cap=j, events_cap=int(want["heads"][:j, :3].sum()))
+            got, w, _ = _schedule(fr, [b], tables, now, caps=[caps], cur=cur)
+            want = w["parts"][0]
+            assert np.array_equal(np.bincount(want["listed"] // 256, minlength=ctas), lose), "the listed runs per CTA"
+            assert got["parts"][0]["runs"].size == min(caps["runs_cap"], want["listed"].size)
+            assert got["parts"][0]["events"].size == min(caps["events_cap"], want["n_events"])
+    finally:
+        b.close()
