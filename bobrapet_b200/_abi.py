@@ -239,6 +239,21 @@ class Resync(C.Structure):
                 ("items_cap", C.c_uint64), ("n_items", C.c_uint64), ("bad_run", C.c_uint32), ("reserved", C.c_uint32)]
 
 
+RESYNC_AREA_TIMERS, RESYNC_AREA_SCHED, RESYNC_AREA_RUNCTL = 0x1, 0x2, 0x4   # BF_RESYNC_AREA_*: areas of bf_resident_resync_areas
+RESYNC_ALL_AREAS = 0x7
+DRIFT_TIMER, DRIFT_TIMER_CODE = 8, 9                   # BF_DRIFT_*: bf_drift.field of bf_resident_resync_areas
+DRIFT_SCHED_STORY_KEY, DRIFT_SCHED_QUEUE_KEY, DRIFT_SCHED_PRIORITY, DRIFT_SCHED_QUEUED_SINCE, DRIFT_SCHED_RUN_PHASE = 10, 11, 12, 13, 14
+DRIFT_STORY_DEADLINE, DRIFT_DRAIN_DEADLINE, DRIFT_STOP = 15, 16, 17
+
+
+class ResyncAreas(C.Structure):
+    _fields_ = [("struct_size", C.c_uint32), ("n_runs", C.c_uint32), ("runs", C.c_void_p), ("n", C.c_uint32),
+                ("areas", C.c_uint32), ("flags", C.c_uint32), ("fired_now", C.c_uint32), ("timers", C.c_void_p),
+                ("sched", C.c_void_p), ("runctl", C.c_void_p), ("drifted_cap", C.c_uint32), ("n_drifted", C.c_uint32),
+                ("drifted", C.c_void_p), ("n_written", C.c_uint32), ("bad_run", C.c_uint32), ("items", C.c_void_p),
+                ("items_cap", C.c_uint64), ("n_items", C.c_uint64)]
+
+
 def sched_stride(words: int) -> int:
     return (16 + 12 * words + 15) & ~15
 
@@ -301,6 +316,7 @@ SYMBOLS = [
                                               C.POINTER(CommitArm), C.POINTER(CommitJournal), C.POINTER(C.c_uint32)]),
     ("bf_resident_status", C.c_int, [C.c_void_p, C.c_uint32, C.c_uint32, C.c_void_p, C.c_uint32, C.POINTER(StatusOut)]),
     ("bf_resident_resync", C.c_int, [C.c_void_p, C.c_uint32, C.POINTER(Resync)]),
+    ("bf_resident_resync_areas", C.c_int, [C.c_void_p, C.c_uint32, C.POINTER(ResyncAreas)]),
     ("bf_group_create", C.c_int, [C.POINTER(C.c_void_p), C.POINTER(C.c_int32), C.c_uint32, C.POINTER(Config)]),
     ("bf_group_destroy", None, [C.c_void_p]),
     ("bf_group_size", C.c_uint32, [C.c_void_p]),

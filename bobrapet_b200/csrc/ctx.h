@@ -51,6 +51,7 @@ cudaError_t launch_commit(const CommitParams& P, bool apply, cudaStream_t stream
 cudaError_t launch_status(const StatusParams& P, uint32_t smem_bytes, cudaStream_t stream);
 cudaError_t launch_rewrites(const RewriteParams& P, uint32_t smem_bytes, cudaStream_t stream);
 cudaError_t launch_resync(const ResyncParams& P, uint32_t smem_bytes, cudaStream_t stream);
+cudaError_t launch_resync_areas(const ResyncAreasParams& P, cudaStream_t stream);
 cudaError_t launch_closure(const Slot* slots, const uint32_t* slot_ids, const uint32_t* starts, uint32_t n, uint32_t n_slots,
                            uint32_t words_out, uint32_t* masks, cudaStream_t stream);
 cudaError_t launch_validate(const Slot* slots, const uint32_t* slot_ids, uint32_t n, uint32_t n_slots, uint32_t* status,
@@ -188,8 +189,9 @@ struct bf_ctx {
     uint32_t fire[4];      // bf_resident_fire: n_fired, n_written, n_pruned, next_deadline
     uint32_t commit[8];    // bf_resident_commit: the offender key (two words), then the five counts
     // the totals of a call's lists: bf_resident_status its events; bf_resident_resync its items and drifted runs;
-    // bf_resident_commit_journal its items and written runs (every call holds the ctx lock, so they share the words)
-    unsigned long long list_totals[2];
+    // bf_resident_commit_journal its items and written runs; bf_resident_resync_areas its items, drifted, written and stopped runs
+    // (every call holds the ctx lock, so they share the words)
+    unsigned long long list_totals[4];
     bf_counts counts() const { return {tail.counts[0], tail.counts[1], tail.counts[2], tail.counts[3]}; }
   }* pinned = nullptr;
   DevBuf<bf_expansion> d_exp;

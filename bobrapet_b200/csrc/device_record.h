@@ -581,6 +581,34 @@ struct ResyncParams {
   unsigned long long items_cap;
 };
 
+// bf_resident_resync_areas (resident.cu): one warp per listed run, no shared stage.  resync_area_runs<false> stores each listed
+// run's item count and each CTA's items and drifted runs, cta_scan turns them into those of the CTAs before each and posts the sums
+// (total[0..1]), resync_area_runs<true> visits the runs with items: their items, their drifted entries and, unless check, their
+// repair, adding the runs written and the runs stopped to total[2] and total[3] (zeroed by the count launch).
+static_assert(sizeof(bf_timer_slot) == 8 && sizeof(bf_sched_put) == 32 && sizeof(bf_run_ctl) == 16, "resync area rows");
+struct ResyncAreasParams {
+  uint8_t* state;
+  RunAreasView areas;               // the device's areas; those the call selects are present
+  uint32_t* mark;                   // a run the repair stops is raised to mark_touched, as by a delta
+  uint32_t mark_touched;
+  const uint32_t* runs;             // [n] ascending, or nullptr: listed run i is run i
+  const unsigned long long* timers; // [n][areas.timer_k] the caller's slots, list order (TIMERS selected)
+  const bf_sched_put* sched;        // [n] (SCHED selected)
+  const bf_run_ctl* runctl;         // [n] (RUNCTL selected)
+  uint32_t n, warps_per_block;
+  uint32_t words, state_stride, off_phase, off_decision;
+  uint32_t sel;                     // BF_RESYNC_AREA_* bits
+  uint32_t fired_now;
+  bool check;
+  uint32_t* run_items;              // [n] items of each listed run
+  unsigned long long* cta;          // [2][CTAs] items and drifted runs of each CTA, then (cta_scan) of the CTAs before it
+  unsigned long long* total;        // [4] items, drifted runs, written runs, stopped runs
+  uint32_t* drifted;                // [drifted_cap]
+  uint32_t drifted_cap;
+  bf_drift* items;                  // [items_cap]
+  unsigned long long items_cap;
+};
+
 // bf_resident_sched_put: req[i] is written into area[req[i].run]
 struct SchedPutParams {
   bf_sched_run* area;

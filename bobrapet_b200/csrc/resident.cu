@@ -1813,4 +1813,189 @@ cudaError_t launch_resync(const ResyncParams& P, uint32_t smem_bytes, cudaStream
   return launch_listing<2>(resync_runs<false>, resync_runs<true>, P, smem_bytes, stream);
 }
 
+// ---- side-area resyncs (bf_resident_resync_areas) ---------------------------------------------------------------------------
+// One warp per listed run; lane t holds slots t and t + 32 of both sides (armed slots lead, ascending by step), as commit_arms holds
+// them.  One warp-uniform walk over the longer armed list matches each slot with the other side's slot of its step by shuffles.  The
+// item flags of each slot kind are then ballots, and an item's rank among its field's items is the ballot below it plus, for a TIMER
+// item, the other side's TIMER items of lower steps (a walk over those items alone: a run without timer drift walks nothing).  A
+// slot step's stored phase and decision are read straight from the device's state record.  Lanes 0-4 take the limiter inputs,
+// lanes 0-2 the story deadline, drain deadline and stop.
+struct AreaDrift {
+  uint32_t r;
+  bf_run_ctl dc, rc;                   // the device's and the caller's run control (the device's where RUNCTL is not selected)
+  bool stopped;                        // stopped on the device or by the caller's run control: no timers compared or written
+  unsigned long long dv[2], cv[2];     // this lane's device / caller slots t, t + 32
+  unsigned long long dev_of_c[2];      // the device's slot at the step of cv[j], or kTimerEmpty
+  unsigned long long TD, TC, CC, KEEP; // ballots over slot indices: device-only TIMER items, caller-side TIMER items, TIMER_CODE
+                                       // items, caller slots the repair keeps (not taken as fired)
+  uint32_t SM, RM;                     // differing limiter inputs (bit f), differing story deadline / drain deadline / stop (bits 0-2)
+  uint32_t nT, nC, n;                  // TIMER items, TIMER_CODE items, all items (warp-uniform)
+};
+
+DI unsigned long long ballot64(bool lo, bool hi) {
+  return (unsigned long long)__ballot_sync(FULL, lo) | (unsigned long long)__ballot_sync(FULL, hi) << 32;
+}
+DI unsigned long long below64(unsigned long long m, uint32_t k) { return m & ((1ull << k) - 1ull); }
+
+DI void area_drift(const ResyncAreasParams& P, uint32_t i, uint32_t lane, AreaDrift& d) {
+  d.r = P.runs ? P.runs[i] : i;
+  d.dc = P.areas.runctl ? P.areas.runctl[d.r] : kRunCtlDefault;
+  d.rc = (P.sel & BF_RESYNC_AREA_RUNCTL) ? P.runctl[i] : d.dc;
+  d.stopped = d.dc.stop || d.rc.stop;
+  const uint8_t* rec = P.state + (size_t)d.r * P.state_stride;
+  const uint32_t K = P.areas.timer_k;
+  const bool timers = (P.sel & BF_RESYNC_AREA_TIMERS) && !d.stopped;
+  bool tc[2] = {false, false}, cc[2] = {false, false}, keep[2] = {false, false}, td[2] = {false, false};
+  for (uint32_t j = 0; j < 2; ++j) {
+    const uint32_t k = lane + 32u * j;
+    d.dv[j] = timers && k < K ? P.areas.timers[(size_t)d.r * K + k] : kTimerEmpty;
+    d.cv[j] = timers && k < K ? P.timers[(size_t)i * K + k] : kTimerEmpty;
+    d.dev_of_c[j] = kTimerEmpty;
+  }
+  if (timers) {
+    const uint32_t Ed = (uint32_t)__popcll((long long)ballot64(timer_armed(d.dv[0]), timer_armed(d.dv[1])));
+    const uint32_t Ec = (uint32_t)__popcll((long long)ballot64(timer_armed(d.cv[0]), timer_armed(d.cv[1])));
+    bool rec_at[2] = {false, false};   // the caller has a slot at the step of dv[j]
+    for (uint32_t k = 0; k < max(Ed, Ec); ++k) {   // warp-uniform trip count
+      const unsigned long long a = __shfl_sync(FULL, k < 32u ? d.dv[0] : d.dv[1], k & 31u);
+      const unsigned long long b = __shfl_sync(FULL, k < 32u ? d.cv[0] : d.cv[1], k & 31u);
+      for (uint32_t j = 0; j < 2; ++j) {
+        if (timer_armed(a) && timer_armed(d.cv[j]) && timer_step(a) == timer_step(d.cv[j])) d.dev_of_c[j] = a;
+        if (timer_armed(b) && timer_armed(d.dv[j]) && timer_step(b) == timer_step(d.dv[j])) rec_at[j] = true;
+      }
+    }
+    for (uint32_t j = 0; j < 2; ++j) {
+      const unsigned long long c = d.cv[j], v = d.dv[j], m = d.dev_of_c[j];
+      if (timer_armed(c)) {
+        const uint32_t s = timer_step(c);
+        const bool live = !((BF_LUT_TERMINAL >> get_planes(rec, P.off_phase, P.words, 4, s)) & 1u);
+        const bool matched = timer_armed(m);
+        const uint32_t dec = P.off_decision != BF_OFF_NONE ? get_planes(rec, P.off_decision, P.words, 2, s) : (uint32_t)BF_DEC_PENDING;
+        const bool fired = !matched && P.fired_now != BF_TIMER_NONE && timer_deadline(c) <= P.fired_now &&
+                           (timer_code(c) == BF_DEC_PENDING || dec != BF_DEC_PENDING);
+        tc[j] = live && (matched ? timer_deadline(m) != timer_deadline(c) : !fired);
+        cc[j] = live && matched && timer_code(m) != timer_code(c);
+        keep[j] = !fired;
+      }
+      if (timer_armed(v) && !rec_at[j])
+        td[j] = !((BF_LUT_TERMINAL >> get_planes(rec, P.off_phase, P.words, 4, timer_step(v))) & 1u);
+    }
+  }
+  d.TD = ballot64(td[0], td[1]);
+  d.TC = ballot64(tc[0], tc[1]);
+  d.CC = ballot64(cc[0], cc[1]);
+  d.KEEP = ballot64(keep[0], keep[1]);
+  bool sm = false, rm = false;
+  if ((P.sel & BF_RESYNC_AREA_SCHED) && lane < 5u)
+    sm = reinterpret_cast<const uint32_t*>(P.areas.sched_in + d.r)[lane] != reinterpret_cast<const uint32_t*>(P.sched + i)[1u + lane];
+  if ((P.sel & BF_RESYNC_AREA_RUNCTL) && lane < 3u) {
+    const uint32_t dd = d.dc.drain_deadline, rd = d.rc.drain_deadline;
+    rm = lane == 0u ? d.dc.story_deadline != d.rc.story_deadline
+       : lane == 1u ? dd != rd && !(dd == BF_TIMER_NONE && deadline_due(rd, P.fired_now) && P.fired_now != BF_TIMER_NONE)
+                    : d.dc.stop != d.rc.stop;
+  }
+  d.SM = __ballot_sync(FULL, sm);
+  d.RM = __ballot_sync(FULL, rm);
+  d.nT = (uint32_t)(__popcll((long long)d.TD) + __popcll((long long)d.TC));
+  d.nC = (uint32_t)__popcll((long long)d.CC);
+  d.n = d.nT + d.nC + (uint32_t)(__popc(d.SM) + __popc(d.RM));
+}
+
+DI void put_drift(const ResyncAreasParams& P, unsigned long long at, uint32_t run, uint32_t index, uint32_t field, uint32_t dv, uint32_t rv) {
+  if (at < P.items_cap) reinterpret_cast<uint4*>(P.items)[at] = make_uint4(run, index | field << 16, dv, rv);
+}
+
+// Count (kList = false): each listed run's items, and each CTA's items and drifted runs.  List (kList = true, after cta_scan): the
+// runs with items again, their items from the offsets of the CTAs and warps before them, their drifted entries and, unless the
+// call only checks, their repair.
+template <bool kList>
+__global__ void __launch_bounds__(256) resync_area_runs(const ResyncAreasParams P) {
+  const uint32_t warp = threadIdx.x >> 5, lane = threadIdx.x & 31u;
+  const uint32_t i = blockIdx.x * P.warps_per_block + warp;
+  AreaDrift d;
+  if (!kList) {
+    if (blockIdx.x == 0 && threadIdx.x < 2) P.total[2 + threadIdx.x] = 0ull;   // the list launch adds into them
+    uint32_t ni = 0;
+    if (i < P.n) {
+      area_drift(P, i, lane, d);
+      ni = d.n;
+      if (lane == 0) P.run_items[i] = ni;
+    }
+    store_cta_totals<2>(ni, P.cta, DriftPart{});
+    return;
+  }
+  if (i >= P.n || P.run_items[i] == 0u) return;
+  area_drift(P, i, lane, d);
+  unsigned long long base[2];
+  run_offsets<2>(P.cta, P.run_items, blockIdx.x * P.warps_per_block, i, DriftPart{}, base);
+  if (lane == 0 && base[1] < P.drifted_cap) P.drifted[base[1]] = d.r;
+  const unsigned long long pos = base[0];
+  // TIMER items of lower steps on the other side: a walk over the set bits of the other side's (warp-uniform) item ballot
+  uint32_t cross_c[2] = {0u, 0u}, cross_d[2] = {0u, 0u};
+  for (unsigned long long m = d.TD; m; m &= m - 1ull) {
+    const uint32_t k = (uint32_t)__ffsll((long long)m) - 1u;
+    const uint32_t s = timer_step(__shfl_sync(FULL, k < 32u ? d.dv[0] : d.dv[1], k & 31u));
+    for (uint32_t j = 0; j < 2; ++j) cross_c[j] += s < timer_step(d.cv[j]) ? 1u : 0u;
+  }
+  for (unsigned long long m = d.TC; m; m &= m - 1ull) {
+    const uint32_t k = (uint32_t)__ffsll((long long)m) - 1u;
+    const uint32_t s = timer_step(__shfl_sync(FULL, k < 32u ? d.cv[0] : d.cv[1], k & 31u));
+    for (uint32_t j = 0; j < 2; ++j) cross_d[j] += s < timer_step(d.dv[j]) ? 1u : 0u;
+  }
+  for (uint32_t j = 0; j < 2; ++j) {
+    const uint32_t k = lane + 32u * j;
+    const unsigned long long c = d.cv[j], v = d.dv[j], m = d.dev_of_c[j];
+    if ((d.TC >> k) & 1ull)
+      put_drift(P, pos + __popcll((long long)below64(d.TC, k)) + cross_c[j], d.r, timer_step(c), BF_DRIFT_TIMER,
+                timer_armed(m) ? timer_deadline(m) : BF_TIMER_NONE, timer_deadline(c));
+    if ((d.TD >> k) & 1ull)
+      put_drift(P, pos + __popcll((long long)below64(d.TD, k)) + cross_d[j], d.r, timer_step(v), BF_DRIFT_TIMER, timer_deadline(v),
+                BF_TIMER_NONE);
+    if ((d.CC >> k) & 1ull)
+      put_drift(P, pos + d.nT + __popcll((long long)below64(d.CC, k)), d.r, timer_step(c), BF_DRIFT_TIMER_CODE, timer_code(m),
+                timer_code(c));
+  }
+  const unsigned long long at_sched = pos + d.nT + d.nC, at_ctl = at_sched + __popc(d.SM);
+  const uint32_t below = (1u << lane) - 1u;
+  if ((d.SM >> lane) & 1u)
+    put_drift(P, at_sched + __popc(d.SM & below), d.r, 0u, BF_DRIFT_SCHED_STORY_KEY + lane,
+              reinterpret_cast<const uint32_t*>(P.areas.sched_in + d.r)[lane], reinterpret_cast<const uint32_t*>(P.sched + i)[1u + lane]);
+  if ((d.RM >> lane) & 1u) {
+    const uint32_t dv = lane == 0u ? d.dc.story_deadline : lane == 1u ? d.dc.drain_deadline : d.dc.stop;
+    const uint32_t rv = lane == 0u ? d.rc.story_deadline : lane == 1u ? d.rc.drain_deadline : d.rc.stop;
+    put_drift(P, at_ctl + __popc(d.RM & below), d.r, 0u, BF_DRIFT_STORY_DEADLINE + lane, dv, rv);
+  }
+  if (P.check) return;
+  __syncwarp();   // every read of the device's areas above is done
+  bool wrote = false;
+  if ((P.sel & BF_RESYNC_AREA_TIMERS) && !d.stopped && d.nT + d.nC) {   // the caller's slots minus those taken as fired
+    const uint32_t K = P.areas.timer_k, n_keep = (uint32_t)__popcll((long long)d.KEEP);
+    unsigned long long* t = P.areas.timers + (size_t)d.r * K;
+    for (uint32_t j = 0; j < 2; ++j) {
+      const uint32_t k = lane + 32u * j;
+      if (k < K && timer_armed(d.cv[j]) && ((d.KEEP >> k) & 1ull)) t[__popcll((long long)below64(d.KEEP, k))] = d.cv[j];
+      if (k < K && k >= n_keep) t[k] = kTimerEmpty;
+    }
+    wrote = true;
+  }
+  if (lane != 0) return;
+  if ((P.sel & BF_RESYNC_AREA_SCHED) && d.SM) {
+    const bf_sched_put q = P.sched[i];
+    P.areas.sched_in[d.r] = bf_sched_run{q.story_key, q.queue_key, q.priority, q.queued_since, q.run_phase, {0u, 0u, 0u}};
+    wrote = true;
+  }
+  bf_run_ctl* ctl = P.areas.runctl ? P.areas.runctl + d.r : nullptr;
+  if (d.RM & 1u) ctl->story_deadline = d.rc.story_deadline;
+  if (d.RM & 2u) ctl->drain_deadline = d.rc.drain_deadline;
+  wrote = wrote || (d.RM & 3u);
+  const bool stop = (P.sel & BF_RESYNC_AREA_RUNCTL) && d.rc.stop && !d.dc.stop;
+  if (stop) stop_run(P.state + (size_t)d.r * P.state_stride, ctl, d.r, d.rc.stop, StopParams{P.areas, P.mark, P.mark_touched});
+  if (wrote || stop) atomicAdd(P.total + 2, 1ull);
+  if (stop) atomicAdd(P.total + 3, 1ull);
+}
+
+cudaError_t launch_resync_areas(const ResyncAreasParams& P, cudaStream_t stream) {
+  return launch_listing<2>(resync_area_runs<false>, resync_area_runs<true>, P, 0u, stream);
+}
+
 }  // namespace bf

@@ -1612,3 +1612,119 @@ int bf_resident_resync(bf_ctx* c, uint32_t h, bf_resync* q) {
   q->n_written = check ? 0 : drifted;
   return BF_OK;
 }
+
+// ---- side-area resyncs (resident.cu) ---------------------------------------------------------------------------------------------
+// Every check first, on the host, so a refused call changes nothing.  Each selected area's rows go to the call's scratch in one H2D
+// copy straight from the caller's array; then the count, scan and list launches, the D2H copy of the totals and one synchronisation.
+// Pinned drifted / items buffers are written in place, others copied after it.
+int bf_resident_resync_areas(bf_ctx* c, uint32_t h, bf_resync_areas* q) {
+  auto [g, r] = lock_resident(c, h);
+  if (!q || q->struct_size != sizeof(bf_resync_areas)) return fail(c, BF_EINVAL, "null bf_resync_areas or bad struct_size");
+  q->bad_run = BF_RESYNC_NONE;
+  if (!r) return BF_EINVAL;
+  const bf_layout& L = r->L;
+  const uint32_t n = q->n, *runs = q->runs, sel = q->areas;
+  if (int rc = check_run_list(c, r, q->n_runs, runs, n)) return rc;
+  if (q->flags & ~BF_RESYNC_CHECK) return fail(c, BF_EINVAL, "unknown flags");
+  if (sel & ~BF_RESYNC_ALL_AREAS) return fail(c, BF_EINVAL, "unknown areas");
+  const bool t_sel = sel & BF_RESYNC_AREA_TIMERS, s_sel = sel & BF_RESYNC_AREA_SCHED, c_sel = sel & BF_RESYNC_AREA_RUNCTL;
+  if ((t_sel && !r->areas.timer_k) || (s_sel && !r->areas.d_sched_in) || (c_sel && !r->areas.d_runctl))
+    return fail(c, BF_EINVAL, "a selected area the batch has no area for");
+  if (n && ((t_sel && !q->timers) || (s_sel && !q->sched) || (c_sel && !q->runctl)))
+    return fail(c, BF_EINVAL, "null array of a selected area");
+  if ((q->drifted_cap && !q->drifted) || (q->items_cap && !q->items)) return fail(c, BF_EINVAL, "null drifted / items with a non-zero cap");
+  const uint32_t K = r->areas.timer_k;
+  auto refuse = [&](uint32_t i, const std::string& why) {
+    q->bad_run = runs ? runs[i] : i;
+    return fail(c, BF_EINVAL, "run " + std::to_string(q->bad_run) + ": " + why);
+  };
+  for (uint32_t i = 0; i < n; ++i) {
+    const uint32_t run = runs ? runs[i] : i;
+    if (t_sel) {   // canonical: armed slots first, strictly ascending by step; empty slots all NONE and zero
+      const bf_timer_slot* row = q->timers + (size_t)i * K;
+      bool empty_seen = false;
+      for (uint32_t k = 0; k < K; ++k) {
+        const bf_timer_slot& t = row[k];
+        if (t.deadline == BF_TIMER_NONE) {
+          if (t.step || t.code || t.reserved) return refuse(i, "an empty timer slot with non-zero bytes");
+          empty_seen = true;
+          continue;
+        }
+        if (empty_seen) return refuse(i, "an armed timer slot after an empty one");
+        if (k && t.step <= row[k - 1].step) return refuse(i, "timer slots not strictly ascending by step");
+        if (t.step >= L.steps_max || t.code > 3 || t.reserved) return refuse(i, "a timer slot's step, code or reserved byte");
+        if (t.code != BF_DEC_PENDING && L.off_decision == BF_OFF_NONE) return refuse(i, "a non-PENDING timer code without decision planes");
+      }
+    }
+    if (s_sel) {
+      const bf_sched_put& s = q->sched[i];
+      if (s.run != run || s.reserved[0] || s.reserved[1]) return refuse(i, "a limiter-input row's run or reserved words");
+    }
+    if (c_sel) {
+      const bf_run_ctl& k = q->runctl[i];
+      bool zero = k.saved_flags == 0;
+      for (uint8_t b : k.reserved) zero = zero && b == 0;
+      if (k.stop > BF_STOP_HOST || !zero) return refuse(i, "a run-control row's stop, saved_flags or reserved bytes");
+    }
+  }
+  q->n_drifted = q->n_written = 0;
+  q->n_items = 0;
+  if (n == 0) return BF_OK;
+  BF_CUDA(c, cudaSetDevice(c->device));
+  cudaStream_t s = c->stream;
+  const bool check = q->flags & BF_RESYNC_CHECK;
+  bf::ResyncAreasParams P{};
+  P.warps_per_block = 8;
+  const uint32_t grid = (n - 1u) / P.warps_per_block + 1u;
+  // a run has at most two items per slot pair, five inputs and three run-control fields: a larger cap stages no more
+  const uint64_t per_run = 2ull * K + 8u;
+  OutList<uint32_t> drifted_list(q->drifted, std::min(q->drifted_cap, n));
+  OutList<bf_drift> items_list(q->items, std::min<uint64_t>(q->items_cap, (uint64_t)n * per_run), true);
+  P.runs = runs ? static_cast<const uint32_t*>(bf::pinned_dev(runs)) : nullptr;
+  CallStage st;
+  if (runs && !P.runs) st.up(P.runs, runs, n);
+  if (t_sel) st.out(P.timers, (size_t)n * K);
+  if (s_sel) st.out(P.sched, n);
+  if (c_sel) st.out(P.runctl, n);
+  st.out(P.run_items, n);
+  st.out(P.cta, 2 * (size_t)grid);
+  st.out(P.total, 4);
+  drifted_list.stage(st);
+  items_list.stage(st);
+  if (int rc = st.send(c, "bf_resident_resync_areas")) return rc;
+  auto up = [&](const void* dst, const void* src, size_t bytes) {
+    return bytes ? cudaMemcpyAsync(const_cast<void*>(dst), src, bytes, cudaMemcpyHostToDevice, s) : cudaSuccess;
+  };
+  if (t_sel) BF_CUDA(c, up(P.timers, q->timers, (size_t)n * K * sizeof(bf_timer_slot)));
+  if (s_sel) BF_CUDA(c, up(P.sched, q->sched, (size_t)n * sizeof(bf_sched_put)));
+  if (c_sel) BF_CUDA(c, up(P.runctl, q->runctl, (size_t)n * sizeof(bf_run_ctl)));
+  P.state = r->d_state; P.areas = r->areas_view();
+  P.mark = r->d_mark; P.mark_touched = r->mark_touched();
+  P.n = n;
+  P.words = L.words; P.state_stride = L.state_stride; P.off_phase = L.off_phase; P.off_decision = L.off_decision;
+  P.sel = sel; P.fired_now = q->fired_now; P.check = check;
+  P.drifted = drifted_list.dev; P.drifted_cap = (uint32_t)drifted_list.cap;
+  P.items = items_list.dev; P.items_cap = items_list.cap;
+  unsigned long long* totals = c->pinned->list_totals;
+  cudaError_t e = bf::launch_resync_areas(P, s);
+  if (e == cudaSuccess) e = cudaMemcpyAsync(totals, P.total, 32, cudaMemcpyDeviceToHost, s);
+  if (check) {
+    if (int rc = bf::end_call(c, e, "bf_resident_resync_areas")) return rc;
+  } else if (int rc = r->sync_in_place(c, e, "bf_resident_resync_areas")) {
+    r->state_changed(c);
+    return rc;
+  }
+  c->stats.kernel_launches += 3;
+  const uint64_t items = totals[0];
+  const uint32_t drifted = (uint32_t)totals[1], written = check ? 0u : (uint32_t)totals[2], stopped = check ? 0u : (uint32_t)totals[3];
+  if (stopped) {   // as bf_resident_runctl_put with a stop: the evaluated snapshot and the tick end (before any copy can fail)
+    r->state_changed(c);
+    r->pending += stopped;
+  }
+  BF_CUDA(c, drifted_list.copy(drifted));
+  BF_CUDA(c, items_list.copy(items));
+  q->n_items = items;
+  q->n_drifted = drifted;
+  q->n_written = written;
+  return BF_OK;
+}

@@ -67,6 +67,7 @@ class Frontier:
         self._owned = _borrowed_ctx is None
         self._steps_max: Dict[int, int] = {}   # steps_max of each resident batch's layout
         self._child_nibbles: Dict[int, int] = {}   # and its child_nibbles
+        self._timer_k: Dict[int, int] = {}   # slots per run of each resident batch's timer area (resident_timers)
         if _borrowed_ctx is not None:       # a shard's ctx owned by a FrontierGroup
             self._ctx = C.c_void_p(_borrowed_ctx)
             return
@@ -323,6 +324,7 @@ class Frontier:
     def resident_timers(self, handle: int, slots_per_run: int):
         """bf_resident_timers: create the batch's timer area with K = slots_per_run slots per run, or grow K keeping every slot"""
         self._check(self._lib.bf_resident_timers(self._ctx, handle, int(slots_per_run)), "bf_resident_timers")
+        self._timer_k[handle] = int(slots_per_run)   # the row width resident_resync_areas checks its timers against
 
     def resident_timers_arm(self, handle: int, requests: np.ndarray):
         """bf_resident_timers_arm: arm (or replace) the timer of each (run, step); deadline A.TIMER_NONE cancels it.
@@ -489,6 +491,53 @@ class Frontier:
                 "items": items[:min(int(q.n_items), int(items_cap))].copy(), "n_drifted": int(q.n_drifted),
                 "n_written": int(q.n_written), "n_items": int(q.n_items)}
 
+    def resident_resync_areas(self, handle: int, n_runs: int, runs=None, timers=None, sched=None, runctl=None,
+                              fired_now: int = A.TIMER_NONE, check: bool = False, drifted_cap: Optional[int] = None,
+                              items_cap: Optional[int] = None) -> dict:
+        """bf_resident_resync_areas: compare the device's step timers, limiter inputs and run control of the listed runs (runs:
+        strictly ascending, below n_runs; None: every run of [0, n_runs)) with the caller's, list every difference and, unless
+        check, repair the runs that drifted.  Each area given is selected: timers SLOT_DTYPE of shape (n, K) with K the batch's
+        slots per run (resident_timers; any other shape is a ValueError, as the library reads n * K slots), sched
+        SCHED_PUT_DTYPE[n] (.run = the listed run), runctl RUNCTL_DTYPE[n] (saved_flags 0).  fired_now: `now` of the last
+        resident_fire on the batch (A.TIMER_NONE: none).  drifted_cap defaults to every listed run, items_cap to 65 536 items.
+        -> {drifted u32[min(n_drifted, cap)], items DRIFT_DTYPE[min(n_items, cap)], n_drifted, n_written, n_items}.  A refusal
+        raises FrontierError with .bad_run set."""
+        rl = None if runs is None else np.ascontiguousarray(runs, dtype=np.uint32)
+        n = int(n_runs) if rl is None else rl.shape[0]
+        areas = 0
+        arrays = []
+        for bit, arr, dt in ((A.RESYNC_AREA_TIMERS, timers, self.SLOT_DTYPE), (A.RESYNC_AREA_SCHED, sched, self.SCHED_PUT_DTYPE),
+                             (A.RESYNC_AREA_RUNCTL, runctl, self.RUNCTL_DTYPE)):
+            if arr is not None:
+                areas |= bit
+                arr = np.ascontiguousarray(arr, dtype=dt)
+                if arr.shape[0] != n:
+                    raise ValueError("one row per listed run: %d rows for %d runs" % (arr.shape[0], n))
+                K = self._timer_k.get(handle)
+                if bit == A.RESYNC_AREA_TIMERS and K is not None and arr.shape != (n, K):
+                    raise ValueError("timers must have shape (%d, %d), the batch's slots per run: got %s" % (n, K, arr.shape))
+            arrays.append(arr)
+        ptr = lambda a: a.ctypes.data if a is not None and a.size else None  # noqa: E731
+        if drifted_cap is None:
+            drifted_cap = n
+        if items_cap is None:   # a buffer not in pinned memory is staged in the ctx's device scratch, which keeps its largest size
+            items_cap = 1 << 16
+        drifted = np.zeros(max(int(drifted_cap), 1), dtype=np.uint32)
+        items = np.zeros(max(int(items_cap), 1), dtype=self.DRIFT_DTYPE)
+        q = A.ResyncAreas(struct_size=C.sizeof(A.ResyncAreas), n_runs=int(n_runs), runs=None if rl is None else rl.ctypes.data,
+                          n=n, areas=areas, flags=A.RESYNC_CHECK if check else 0, fired_now=int(fired_now),
+                          timers=ptr(arrays[0]), sched=ptr(arrays[1]), runctl=ptr(arrays[2]), drifted_cap=int(drifted_cap),
+                          drifted=drifted.ctypes.data if drifted_cap else None, items=items.ctypes.data if items_cap else None,
+                          items_cap=int(items_cap))
+        rc = self._lib.bf_resident_resync_areas(self._ctx, handle, C.byref(q))
+        if rc != 0:
+            err = A.FrontierError(rc, "bf_resident_resync_areas: %s" % self._lib.bf_last_error(self._ctx).decode())
+            err.bad_run = int(q.bad_run)
+            raise err
+        return {"drifted": drifted[:min(int(q.n_drifted), int(drifted_cap))].copy(),
+                "items": items[:min(int(q.n_items), int(items_cap))].copy(), "n_drifted": int(q.n_drifted),
+                "n_written": int(q.n_written), "n_items": int(q.n_items)}
+
     # -- limiter inputs and schedules of resident batches (bf_resident_sched*, bf_resident_schedule)
     SCHED_PUT_DTYPE = np.dtype([("run", "<u4"), ("story_key", "<u4"), ("queue_key", "<u4"), ("priority", "<i4"),
                                 ("queued_since", "<u4"), ("run_phase", "<u4"), ("reserved", "<u4", (2,))])   # bf_sched_put, 32 B
@@ -565,6 +614,7 @@ class Frontier:
         self._check(self._lib.bf_resident_create(self._ctx, C.byref(L), capacity, C.byref(h)), "bf_resident_create")
         self._steps_max[h.value] = int(L.steps_max)   # its words size resident_status's default event buffer
         self._child_nibbles[h.value] = int(L.child_nibbles)   # and, with it, resident_resync's default item buffer
+        self._timer_k.pop(h.value, None)
         return h.value
 
     def resident_destroy(self, handle: int):

@@ -279,6 +279,7 @@ type Resident struct {
 	c      *Ctx
 	handle C.uint32_t
 	layout C.bf_layout
+	timerK uint32 // slots per run of the timer area (EnableTimers), 0 without one
 }
 
 func (c *Ctx) NewResident(layout C.bf_layout, capacity uint32) (*Resident, error) {
@@ -518,7 +519,11 @@ type FireResult struct {
 // EnableTimers gives the batch slotsPerRun timer slots per run (1..64), or grows them keeping every armed timer
 // (bf_resident_timers).  Retire, TransferTo, Migrate and Redrive re-key the timers with the runs from then on.
 func (r *Resident) EnableTimers(slotsPerRun uint32) error {
-	return r.c.err(C.bf_resident_timers(r.c.p, r.handle, C.uint32_t(slotsPerRun)))
+	err := r.c.err(C.bf_resident_timers(r.c.p, r.handle, C.uint32_t(slotsPerRun)))
+	if err == nil {
+		r.timerK = slotsPerRun
+	}
+	return err
 }
 
 // ArmTimers arms, replaces or cancels the timers of (run, step) pairs (bf_resident_timers_arm): the sleepUntil, gateTimeoutAt,
@@ -894,6 +899,108 @@ func (r *Resident) Resync(n uint32, runs []uint32, records []byte, fields uint32
 	var ni C.uint64_t
 	rc := C.bfgo_resident_resync(r.c.p, r.handle, C.uint32_t(n), rp, C.uint32_t(count), recp, C.uint32_t(fields), flags, dp,
 		C.uint32_t(len(drifted)), ip, C.uint64_t(len(items)), &nd, &nw, &ni, &bad)
+	return uint32(nd), uint32(nw), uint64(ni), uint32(bad), r.c.err(rc)
+}
+
+// TimerSlot is one step-timer slot of a run as the batch keeps it (bf_timer_slot, 8 bytes, no pointers): Deadline TimerNone is an
+// empty slot, whose other bytes are 0.  A run's armed slots come first, ascending by step.
+type TimerSlot struct {
+	Deadline uint32
+	Step     uint16
+	Code     uint8
+	_        uint8
+}
+
+// RunCtlRecord is a run's run control as the batch keeps it (bf_run_ctl, 16 bytes, no pointers); ResyncAreas takes SavedFlags 0.
+type RunCtlRecord struct {
+	StoryDeadline, DrainDeadline uint32
+	Stop, SavedFlags             uint8
+	_                            [6]uint8
+}
+
+// Areas of ResyncAreas (BF_RESYNC_AREA_*) and the Drift fields it lists (BF_DRIFT_*, clear of the Delta* fields).
+const (
+	ResyncAreaTimers = 0x1
+	ResyncAreaSched  = 0x2
+	ResyncAreaRunCtl = 0x4
+
+	DriftTimer            = 8  // Index = step; the deadlines, TimerNone for a side without a slot at the step
+	DriftTimerCode        = 9  // Index = step; the codes of the two slots at the step
+	DriftSchedStoryKey    = 10 // the five limiter inputs, in SchedPut order
+	DriftSchedQueueKey    = 11
+	DriftSchedPriority    = 12
+	DriftSchedQueuedSince = 13
+	DriftSchedRunPhase    = 14
+	DriftStoryDeadline    = 15
+	DriftDrainDeadline    = 16
+	DriftStop             = 17 // the Stop* reasons
+)
+
+// ResyncAreas compares the device's step timers, limiter inputs and run control of the listed runs (runs: strictly ascending,
+// below n; nil: every run of [0, n)) with the areas packed from the cluster, one row per listed run in list order (timers: the
+// slots-per-run slots of each run, canonical, from the step-timers annotation; sched: SchedPut with Run the listed run; runctl:
+// the deadlines and the stop), lists every difference into drifted and items, and without ResyncCheck repairs the runs that
+// drifted (bf_resident_resync_areas).  A nil slice leaves its area out.  firedNow is the now of the last Fire (TimerNone: none): a
+// slot the annotation still holds after a fire disarmed it is taken as fired.  Resync the records first.  The counts are the true
+// ones; only the first len(drifted) / len(items) entries are written.  On a refusal that names a run, badRun is that run, else
+// SchedNone.
+func (r *Resident) ResyncAreas(n uint32, runs []uint32, timers []TimerSlot, sched []SchedPut, runctl []RunCtlRecord,
+	firedNow uint32, check bool, drifted []uint32, items []Drift) (nDrifted, nWritten uint32, nItems uint64, badRun uint32, err error) {
+	count := int(n)
+	var rp *C.uint32_t
+	if runs != nil {
+		count = len(runs)
+		if count > 0 {
+			rp = (*C.uint32_t)(unsafe.Pointer(&runs[0]))
+		}
+	}
+	var areas C.uint32_t
+	var tp *C.bf_timer_slot
+	var sp *C.bf_sched_put
+	var cp *C.bf_run_ctl
+	if timers != nil {
+		areas |= ResyncAreaTimers
+		if len(timers) != count*int(r.timerK) {
+			return 0, 0, 0, SchedNone, fmt.Errorf("frontier: timers holds %d slots for %d runs of %d", len(timers), count, r.timerK)
+		}
+		if len(timers) > 0 {
+			tp = (*C.bf_timer_slot)(unsafe.Pointer(&timers[0]))
+		}
+	}
+	if sched != nil {
+		areas |= ResyncAreaSched
+		if len(sched) != count {
+			return 0, 0, 0, SchedNone, fmt.Errorf("frontier: sched holds %d rows for %d runs", len(sched), count)
+		}
+		if count > 0 {
+			sp = (*C.bf_sched_put)(unsafe.Pointer(&sched[0]))
+		}
+	}
+	if runctl != nil {
+		areas |= ResyncAreaRunCtl
+		if len(runctl) != count {
+			return 0, 0, 0, SchedNone, fmt.Errorf("frontier: runctl holds %d rows for %d runs", len(runctl), count)
+		}
+		if count > 0 {
+			cp = (*C.bf_run_ctl)(unsafe.Pointer(&runctl[0]))
+		}
+	}
+	var dp *C.uint32_t
+	if len(drifted) > 0 {
+		dp = (*C.uint32_t)(unsafe.Pointer(&drifted[0]))
+	}
+	var ip *C.bf_drift
+	if len(items) > 0 {
+		ip = (*C.bf_drift)(unsafe.Pointer(&items[0]))
+	}
+	var flags C.uint32_t
+	if check {
+		flags = ResyncCheck
+	}
+	var nd, nw, bad C.uint32_t
+	var ni C.uint64_t
+	rc := C.bfgo_resident_resync_areas(r.c.p, r.handle, C.uint32_t(n), rp, C.uint32_t(count), areas, tp, sp, cp,
+		C.uint32_t(firedNow), flags, dp, C.uint32_t(len(drifted)), ip, C.uint64_t(len(items)), &nd, &nw, &ni, &bad)
 	return uint32(nd), uint32(nw), uint64(ni), uint32(bad), r.c.err(rc)
 }
 

@@ -320,6 +320,25 @@ static inline int bfgo_resident_resync(bf_ctx* c, uint32_t handle, uint32_t n_ru
   return rc;
 }
 
+/* Side-area resync.  The caller's rows of each area in `areas` (bf_timer_slot, bf_sched_put, bf_run_ctl: no pointers), the run
+ * list and the outputs are the caller's buffers; the counts and, on a refusal that names a run, *bad_run come back through the
+ * pointers. */
+static inline int bfgo_resident_resync_areas(bf_ctx* c, uint32_t handle, uint32_t n_runs, const uint32_t* runs, uint32_t n,
+                                             uint32_t areas, const bf_timer_slot* timers, const bf_sched_put* sched,
+                                             const bf_run_ctl* runctl, uint32_t fired_now, uint32_t flags, uint32_t* drifted,
+                                             uint32_t drifted_cap, bf_drift* items, uint64_t items_cap, uint32_t* n_drifted,
+                                             uint32_t* n_written, uint64_t* n_items, uint32_t* bad_run) {
+  bf_resync_areas q;
+  memset(&q, 0, sizeof q);
+  q.struct_size = (uint32_t)sizeof q;
+  q.n_runs = n_runs; q.runs = runs; q.n = n; q.areas = areas; q.flags = flags; q.fired_now = fired_now;
+  q.timers = timers; q.sched = sched; q.runctl = runctl;
+  q.drifted = drifted; q.drifted_cap = drifted_cap; q.items = items; q.items_cap = items_cap;
+  const int rc = bf_resident_resync_areas(c, handle, &q);
+  *n_drifted = q.n_drifted; *n_written = q.n_written; *n_items = q.n_items; *bad_run = q.bad_run;
+  return rc;
+}
+
 /* Step timings of a topology slot (bf_step_timing holds no pointers): passed as they are. */
 static inline int bfgo_topology_timings(bf_ctx* c, uint32_t slot, const bf_step_timing* t, uint32_t n) {
   return bf_topology_timings(c, slot, t, n);

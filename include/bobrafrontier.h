@@ -1369,6 +1369,91 @@ typedef struct bf_resync {
 
 int bf_resident_resync(bf_ctx* ctx, uint32_t handle, bf_resync* r);
 
+/* bf_resident_resync_areas: the same for the per-run side areas a batcher persists outside the state records: the step timers (the
+ * runs.bubustack.io/step-timers annotation, stepTimerStore dag.go:64,110-190), the limiter inputs (labels, priority, queue origin
+ * and StoryRun phase) and the run control (StartedAt + policy.timeouts.story, spec.cancelRequested).  The caller packs each selected
+ * area (`areas`) for the listed runs, in list order, as the upload calls take them; the device compares them with its own, lists
+ * every difference and, without BF_RESYNC_CHECK, repairs only the runs that drifted.  Resync the records first: the timer rules read
+ * the device's phases and decisions.
+ *
+ * What is compared: what the device's next bf_resident_fire and bf_resident_schedule would do, not raw bytes.
+ *   - TIMERS (run not stopped on the device, and not stopped by the caller's run control when RUNCTL is selected: a stopped run's slots
+ *     are empty by the stop rule, so such a run compares and writes no timers).  The slots of a step are compared only when the
+ *     device's STORED phase code at that step is not terminal (BF_LUT_TERMINAL): a slot at a terminal step is dormant and the next
+ *     fire prunes it (pruneTerminal, dag.go:173-190).  A step with a slot on both sides lists BF_DRIFT_TIMER when the deadlines
+ *     differ and BF_DRIFT_TIMER_CODE when the codes differ.  A step with a slot on one side lists BF_DRIFT_TIMER with BF_TIMER_NONE
+ *     on the other side, except a caller slot TAKEN AS FIRED: the device has no slot at its step, fired_now != BF_TIMER_NONE, its
+ *     deadline <= fired_now, and its code is BF_DEC_PENDING (wake-only) or the device's decision code at the step is not
+ *     BF_DEC_PENDING.  The fire disarms a due slot while the annotation keeps it until the step is terminal, so such a slot is
+ *     equal.  A due caller slot whose step still has decision PENDING on the device is drift: the stuck step the repair re-arms.
+ *   - SCHED: the five stored inputs (story_key, queue_key, priority, queued_since, run_phase), one item each (index 0).
+ *   - RUNCTL: story_deadline as stored (a stopped run keeps it, dormant); drain_deadline by the taken-as-fired rule (a caller drain
+ *     deadline the device no longer has, due at fired_now, is equal: the fire disarms it); the stop by reason (BF_DRIFT_STOP).
+ * Items (bf_drift) are ordered by (run, field, index); device and record are the compared values (deadlines, codes, inputs, stop
+ * reasons).  The field codes below are disjoint from BF_DELTA_*, so one loop consumes the items of both resync calls.
+ *
+ * Repair (without BF_RESYNC_CHECK), of the drifted runs and, in a run, of the areas it lists items for:
+ *   - timers: the run's K slots become the caller's slots minus those taken as fired, in the canonical layout.  Touches no run;
+ *   - limiter inputs: the run's inputs become the caller's.  Touches no run and needs no new tick: the next schedule lists the run
+ *     when its schedule changes;
+ *   - deadlines: each drifted deadline takes the caller's value;
+ *   - a caller stop on a run the device has not stopped stops the run exactly as bf_resident_runctl_put does (saved flags byte,
+ *     stopped byte, timers emptied, run_phase = BF_PHASE_TIMEOUT for BF_STOP_TIMEOUT with a limiter area, the run touched, the
+ *     evaluated snapshot and the schedule's tick ended).  This runs after the inputs are written.  A device stop the caller lacks,
+ *     or a stop of another reason, is listed and kept: only a redrive lifts a stop, and stopping again changes nothing.
+ *   n_written counts the runs whose areas or record the repair changed (a run whose only items are a kept stop is not one).  A call
+ *   that wrote no stop changes no state record and ends nothing; every BF_RESYNC_CHECK call changes nothing at all.
+ * Refused before anything is written, BF_EINVAL and nothing changed, bad_run naming the first offending run where there is one (else
+ * BF_RESYNC_NONE): struct_size or the handle; n_runs > capacity, runs not strictly ascending or not below n_runs, runs == NULL with
+ * n != n_runs; unknown flags or areas bits; a selected area the batch has no area for (bf_resident_timers / _sched / _runctl: a caller
+ * packing an area for a batch without one has a bug); a NULL array of a selected area with n > 0; drifted / items NULL with a
+ * non-zero cap; a timer row that is not canonical (armed slots first, strictly ascending by step, step < steps_max, code <= 3, a
+ * non-PENDING code only with decision planes, reserved 0; an empty slot is deadline BF_TIMER_NONE with every other byte 0); a sched
+ * row whose run is not the listed run, or with non-zero reserved words; a runctl row with stop > BF_STOP_HOST or non-zero
+ * saved_flags / reserved bytes.
+ * Cost: one H2D copy per selected area straight from the caller's array (and one of a run list not in pinned memory), three launches
+ * (count, scan, list and repair: one warp per listed run, lane t on slots t and t + 32, no shared stage), one D2H copy of the totals,
+ * one synchronisation.  Pinned drifted / items buffers are written in place, others staged and copied after it.  A batch that never
+ * calls this launches nothing more than before.                                                                                  */
+#define BF_RESYNC_AREA_TIMERS 0x1u
+#define BF_RESYNC_AREA_SCHED 0x2u
+#define BF_RESYNC_AREA_RUNCTL 0x4u
+#define BF_RESYNC_ALL_AREAS 0x7u
+enum {                            /* bf_drift.field of bf_resident_resync_areas (BF_DELTA_* end at 6)                           */
+  BF_DRIFT_TIMER = 8,             /* index = step; the deadlines, BF_TIMER_NONE for a side without a slot at the step            */
+  BF_DRIFT_TIMER_CODE = 9,        /* index = step; the codes of the two slots at the step                                        */
+  BF_DRIFT_SCHED_STORY_KEY = 10,  /* index 0; the five stored limiter inputs, in bf_sched_put order                              */
+  BF_DRIFT_SCHED_QUEUE_KEY = 11,
+  BF_DRIFT_SCHED_PRIORITY = 12,
+  BF_DRIFT_SCHED_QUEUED_SINCE = 13,
+  BF_DRIFT_SCHED_RUN_PHASE = 14,
+  BF_DRIFT_STORY_DEADLINE = 15,   /* index 0; the deadlines                                                                      */
+  BF_DRIFT_DRAIN_DEADLINE = 16,
+  BF_DRIFT_STOP = 17              /* index 0; the BF_STOP_* reasons                                                              */
+};
+typedef struct bf_resync_areas {
+  uint32_t struct_size;           /* sizeof(bf_resync_areas)                                                                     */
+  uint32_t n_runs;                /* in: the batch's runs are [0, n_runs)                                                        */
+  const uint32_t* runs;           /* in: [n] strictly ascending, below n_runs; NULL with n == n_runs: every run of [0, n_runs)   */
+  uint32_t n;
+  uint32_t areas;                 /* in: BF_RESYNC_AREA_* bits                                                                   */
+  uint32_t flags;                 /* in: BF_RESYNC_CHECK                                                                         */
+  uint32_t fired_now;             /* in: `now` of the last bf_resident_fire on this batch, BF_TIMER_NONE: none                   */
+  const bf_timer_slot* timers;    /* in: [n * K] each run's K slots (K: the batch's current K), canonical, list order            */
+  const bf_sched_put* sched;      /* in: [n] .run = the listed run, reserved 0                                                   */
+  const bf_run_ctl* runctl;       /* in: [n] saved_flags and reserved 0                                                          */
+  uint32_t drifted_cap;
+  uint32_t n_drifted;             /* out: the true count                                                                         */
+  uint32_t* drifted;              /* [drifted_cap] out: ascending runs with at least one item                                    */
+  uint32_t n_written;             /* out: runs the repair changed (0 with BF_RESYNC_CHECK)                                       */
+  uint32_t bad_run;               /* out on a refusal: the offending run, else BF_RESYNC_NONE                                    */
+  bf_drift* items;                /* [items_cap] out                                                                             */
+  uint64_t items_cap;
+  uint64_t n_items;               /* out: the true count; only the first items_cap were written                                 */
+} bf_resync_areas;
+
+int bf_resident_resync_areas(bf_ctx* ctx, uint32_t handle, bf_resync_areas* r);
+
 /* ------------------------------------------------------------------ device groups (SURVEY.md row e)
  * The reference is ONE operator process (cmd/main.go:220, StoryRunReconciler storyrun_controller.go:216), so the
  * multi-GPU path must be reachable from one process through this ABI: a group owns one ctx per device and an NCCL
