@@ -116,6 +116,11 @@ class TouchedOut(C.Structure):
                 ("events", C.c_void_p), ("events_cap", C.c_uint64), ("n_events", C.c_uint64)]
 
 
+class TickPart(C.Structure):
+    _fields_ = [("struct_size", C.c_uint32), ("handle", C.c_uint32), ("deltas", C.c_void_p), ("n_deltas", C.c_uint32),
+                ("n_runs", C.c_uint32), ("out", C.c_void_p), ("counts", C.c_void_p)]
+
+
 MIGRATE_GONE = 0xFFFF   # BF_MIGRATE_GONE: the old step has no step of the new generation
 
 
@@ -288,6 +293,7 @@ SYMBOLS = [
     ("bf_eval_compact", C.c_int, [C.c_void_p, C.POINTER(Batch), C.POINTER(CompactOut)]),
     ("bf_resident_tick_compact", C.c_int, [C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.POINTER(CompactOut), C.POINTER(Counts)]),
     ("bf_resident_tick_touched", C.c_int, [C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.POINTER(TouchedOut), C.POINTER(Counts)]),
+    ("bf_resident_tick_touched_many", C.c_int, [C.c_void_p, C.c_uint32, C.c_uint32, C.POINTER(TickPart), C.c_uint32, C.POINTER(C.c_uint32)]),
     ("bf_resident_migrate", C.c_int, [C.c_void_p, C.c_uint32, C.POINTER(Migration)]),
     ("bf_resident_redrive", C.c_int, [C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_void_p, C.POINTER(C.c_uint32)]),
     ("bf_resident_reshape", C.c_int, [C.c_void_p, C.c_uint32, C.POINTER(Layout), C.c_uint32]),

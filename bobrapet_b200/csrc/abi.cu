@@ -526,6 +526,7 @@ void bf_destroy(bf_ctx* c) {
     if (c->ev_k[k]) cudaEventDestroy(c->ev_k[k]);
   }
   cudaFreeHost(c->pinned);
+  if (c->part_tails) cudaFreeHost(c->part_tails);
   delete c;   // the device buffers of the ctx and of its resident batches free themselves
 }
 

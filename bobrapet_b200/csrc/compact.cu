@@ -67,13 +67,13 @@ __global__ void __launch_bounds__(CB) compact_heads(const CompactParams P) {
   }
 }
 
-// sum of v[0 .. blockIdx.x): what the blocks before mine produced (every thread of the block gets it)
-__device__ __forceinline__ unsigned long long blocks_before(const unsigned long long* v) {
+// sum of v[0 .. b): what the blocks before mine (block b of its launch or of its part) produced (every thread of the block gets it)
+__device__ __forceinline__ unsigned long long blocks_before(const unsigned long long* v, uint32_t b = blockIdx.x) {
   __shared__ unsigned long long sh64[CB / 32];
   __shared__ unsigned long long base_s;
   const uint32_t lane = threadIdx.x & 31u, warp = threadIdx.x >> 5;
   unsigned long long part = 0;
-  for (uint32_t b = threadIdx.x; b < blockIdx.x; b += CB) part += v[b];
+  for (uint32_t k = threadIdx.x; k < b; k += CB) part += v[k];
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) part += __shfl_down_sync(0xffffffffu, part, o);
   if (lane == 0) sh64[warp] = part;
@@ -197,25 +197,26 @@ __device__ __forceinline__ uint32_t touched_bits(const TouchedParams& P, uint32_
 }
 
 // touched runs per block of CB * SCAN_RUNS runs: below n_scan (the list) and at or above it (carried to a later tick)
-__global__ void __launch_bounds__(CB) touched_count(const TouchedParams P) {
-  const uint32_t bits = touched_bits(P, (blockIdx.x * CB + threadIdx.x) * SCAN_RUNS);
+// (each body runs as block b of nblocks of its tick: the whole launch for one tick, the tick's blocks of a launch over several)
+__device__ __forceinline__ void touched_count_body(const TouchedParams& P, uint32_t b) {
+  const uint32_t bits = touched_bits(P, (b * CB + threadIdx.x) * SCAN_RUNS);
   uint32_t tot;   // a block counts at most 2048 runs of each kind: one packed scan
   block_scan(__popc(bits & 0xFu) | (__popc(bits >> SCAN_RUNS) << 16), &tot);
-  if (threadIdx.x == 0) { P.scan_sums[blockIdx.x] = tot & 0xFFFFu; P.carry_sums[blockIdx.x] = tot >> 16; }
+  if (threadIdx.x == 0) { P.scan_sums[b] = tot & 0xFFFFu; P.carry_sums[b] = tot >> 16; }
 }
 
 // the ascending list: every block writes its touched runs after those of the blocks before it; the last block stores the count
-__global__ void __launch_bounds__(CB) touched_list(const TouchedParams P) {
-  const unsigned long long base = blocks_before(P.scan_sums);
-  const uint32_t r0 = (blockIdx.x * CB + threadIdx.x) * SCAN_RUNS;
+__device__ __forceinline__ void touched_list_body(const TouchedParams& P, uint32_t b, uint32_t nblocks) {
+  const unsigned long long base = blocks_before(P.scan_sums, b);
+  const uint32_t r0 = (b * CB + threadIdx.x) * SCAN_RUNS;
   uint32_t bits = touched_bits(P, r0) & 0xFu;
   uint32_t btot;
   unsigned long long at = base + block_scan(__popc(bits), &btot);
   for (; bits; bits &= bits - 1, ++at)
     if (at < P.bound) P.list[at] = r0 + __ffs(bits) - 1;   // (the host's bound holds: every touched run has a delta or upload behind it)
-  if (blockIdx.x == gridDim.x - 1) {
+  if (b == nblocks - 1) {
     // the touched runs this tick leaves for a later one: the host's next bound starts from them (posted to the pinned tail)
-    const unsigned long long carried = blocks_before(P.carry_sums) + P.carry_sums[blockIdx.x];
+    const unsigned long long carried = blocks_before(P.carry_sums, b) + P.carry_sums[b];
     if (threadIdx.x == 0) {
       *P.list_count = (uint32_t)min(base + btot, (unsigned long long)P.bound);
       P.C.host_tail->carried = carried;
@@ -225,9 +226,9 @@ __global__ void __launch_bounds__(CB) touched_list(const TouchedParams P) {
 
 // per list position: compare the run's new record with its current one (the bytes compact_heads compares), list it when they
 // differ or it must be listed, bring the current record up to date and clear the run's mark; head word and events as compact_heads
-__global__ void __launch_bounds__(CB) touched_heads(const TouchedParams P) {
+__device__ __forceinline__ void touched_heads_body(const TouchedParams& P, uint32_t b) {
   const CompactParams& C = P.C;
-  const uint32_t i = blockIdx.x * CB + threadIdx.x;
+  const uint32_t i = b * CB + threadIdx.x;
   const uint32_t n = min(*P.list_count, P.bound);
   uint32_t c = 0, listed = 0;
   if (i < n) {
@@ -258,15 +259,15 @@ __global__ void __launch_bounds__(CB) touched_heads(const TouchedParams P) {
   // events of a block <= 512 * 1024 < 2^20, listed runs <= 512: one packed scan
   uint32_t tot;
   block_scan(c | (listed << 20), &tot);
-  if (threadIdx.x == 0) { P.sums[blockIdx.x] = tot & 0xFFFFFu; P.sums_listed[blockIdx.x] = tot >> 20; }
+  if (threadIdx.x == 0) { P.sums[b] = tot & 0xFFFFFu; P.sums_listed[b] = tot >> 20; }
 }
 
 // the listed runs in list order: runs[] and head[] (first runs_cap), events as compact_emit (same staging and capacity rules)
-__global__ void __launch_bounds__(CB) touched_emit(const TouchedParams P) {
+__device__ __forceinline__ void touched_emit_body(const TouchedParams& P, uint32_t b, uint32_t nblocks) {
   __shared__ uint16_t stage[STAGE_EVENTS];
   const CompactParams& C = P.C;
-  const unsigned long long base = blocks_before(P.sums), base_l = blocks_before(P.sums_listed);
-  const uint32_t i = blockIdx.x * CB + threadIdx.x;
+  const unsigned long long base = blocks_before(P.sums, b), base_l = blocks_before(P.sums_listed, b);
+  const uint32_t i = b * CB + threadIdx.x;
   const uint32_t n = min(*P.list_count, P.bound);
   const uint32_t hw = i < n ? P.pos_head[i] : 0u;
   const uint32_t listed = (hw & BF_HEAD_LISTED) ? 1u : 0u, c = hw >> BF_HEAD_COUNT_SHIFT;
@@ -278,7 +279,7 @@ __global__ void __launch_bounds__(CB) touched_emit(const TouchedParams P) {
     const unsigned long long k = base_l + (before_p >> 20);
     if (k < P.runs_cap) { P.out_runs[k] = r; P.out_head[k] = hw; }
   }
-  if (blockIdx.x == gridDim.x - 1 && threadIdx.x == 0) {
+  if (b == nblocks - 1 && threadIdx.x == 0) {
     ResultTail& t = *C.host_tail;   // pinned host memory: visible to the host once the stream has been synchronised
     t.events = base + btot;
     for (int k = 0; k < 4; ++k) t.counts[k] = C.counts ? C.counts[k] : 0ull;
@@ -292,6 +293,53 @@ __global__ void __launch_bounds__(CB) touched_emit(const TouchedParams P) {
   if (!staged) return;
   __syncthreads();
   write_slice(C, base, btot, stage);
+}
+
+__global__ void __launch_bounds__(CB) touched_count(const TouchedParams P) { touched_count_body(P, blockIdx.x); }
+__global__ void __launch_bounds__(CB) touched_list(const TouchedParams P) { touched_list_body(P, blockIdx.x, gridDim.x); }
+__global__ void __launch_bounds__(CB) touched_heads(const TouchedParams P) { touched_heads_body(P, blockIdx.x); }
+__global__ void __launch_bounds__(CB) touched_emit(const TouchedParams P) { touched_emit_body(P, blockIdx.x, gridDim.x); }
+
+// ---- several touched ticks in one launch per stage (bf_resident_tick_touched_many): the blocks of tick k are
+// [first[k], first[k + 1]) of the launch; each runs the single tick's body as block blockIdx.x - first[k] of its tick
+struct PartBlock { uint32_t k, b, n; };
+__device__ __forceinline__ PartBlock part_block(const uint32_t* first, uint32_t n_parts) {
+  uint32_t lo = 0, hi = n_parts;   // the last k with first[k] <= blockIdx.x
+  while (hi - lo > 1) {
+    const uint32_t mid = (lo + hi) / 2;
+    if (first[mid] <= blockIdx.x) lo = mid; else hi = mid;
+  }
+  return {lo, blockIdx.x - first[lo], first[lo + 1] - first[lo]};
+}
+__global__ void __launch_bounds__(CB) touched_count_many(const TouchedParams* __restrict__ T, const uint32_t* __restrict__ first, uint32_t n) {
+  const PartBlock p = part_block(first, n);
+  touched_count_body(T[p.k], p.b);
+}
+__global__ void __launch_bounds__(CB) touched_list_many(const TouchedParams* __restrict__ T, const uint32_t* __restrict__ first, uint32_t n) {
+  const PartBlock p = part_block(first, n);
+  touched_list_body(T[p.k], p.b, p.n);
+}
+__global__ void __launch_bounds__(CB) touched_heads_many(const TouchedParams* __restrict__ T, const uint32_t* __restrict__ first, uint32_t n) {
+  const PartBlock p = part_block(first, n);
+  touched_heads_body(T[p.k], p.b);
+}
+__global__ void __launch_bounds__(CB) touched_emit_many(const TouchedParams* __restrict__ T, const uint32_t* __restrict__ first, uint32_t n) {
+  const PartBlock p = part_block(first, n);
+  touched_emit_body(T[p.k], p.b, p.n);
+}
+
+// T, list_first and compact_first are device arrays of n ticks; list_first / compact_first hold the block starts of each tick
+// (ceil(n_marks / 2048) list blocks, ceil(bound / 512) compaction blocks, every tick at least one) and the total at [n]
+cudaError_t launch_touched_list_many(const TouchedParams* T, const uint32_t* list_first, uint32_t n, uint32_t blocks, cudaStream_t stream) {
+  touched_count_many<<<blocks, CB, 0, stream>>>(T, list_first, n);
+  touched_list_many<<<blocks, CB, 0, stream>>>(T, list_first, n);
+  return cudaGetLastError();
+}
+cudaError_t launch_touched_compact_many(const TouchedParams* T, const uint32_t* compact_first, uint32_t n, uint32_t blocks,
+                                        cudaStream_t stream) {
+  touched_heads_many<<<blocks, CB, 0, stream>>>(T, compact_first, n);
+  touched_emit_many<<<blocks, CB, 0, stream>>>(T, compact_first, n);
+  return cudaGetLastError();
 }
 
 cudaError_t launch_touched_list(const TouchedParams& P, cudaStream_t stream) {

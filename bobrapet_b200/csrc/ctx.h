@@ -30,6 +30,10 @@ cudaError_t launch_apply_deltas(const DeltaParams& P, cudaStream_t stream);
 cudaError_t launch_compact(const CompactParams& P, cudaStream_t stream);
 cudaError_t launch_touched_list(const TouchedParams& P, cudaStream_t stream);
 cudaError_t launch_touched_compact(const TouchedParams& P, cudaStream_t stream);
+cudaError_t launch_apply_deltas_many(const DeltaParams* parts, const uint32_t* first, uint32_t n_parts, uint32_t n, cudaStream_t stream);
+cudaError_t launch_touched_list_many(const TouchedParams* T, const uint32_t* list_first, uint32_t n, uint32_t blocks, cudaStream_t stream);
+cudaError_t launch_touched_compact_many(const TouchedParams* T, const uint32_t* compact_first, uint32_t n, uint32_t blocks,
+                                        cudaStream_t stream);
 cudaError_t launch_mark_runs(uint32_t* mark, uint32_t first, uint32_t n, uint32_t value, cudaStream_t stream);
 cudaError_t launch_move_records(const uint8_t* src, uint8_t* dst, const void* moves, uint32_t n, cudaStream_t stream);
 cudaError_t launch_migrate(const MigrateParams& P, cudaStream_t stream);
@@ -124,6 +128,15 @@ struct DevBuf {
 
 struct Resident;
 
+// The device scratch of one touched tick: [0] = list length, [1..] = the list | head word per list position | listed runs and
+// their heads (when the caller's buffers are not pinned) | per-block sums | the event list (bf_resident_tick_touched_many's
+// pageable event buffers; the single call stages them in bf_ctx::d_events)
+struct TouchScratch {
+  DevBuf<uint32_t> list, pos_head, runs, head;
+  DevBuf<unsigned long long> sums;
+  DevBuf<uint16_t> events;
+};
+
 struct TopoMeta {
   bool alive = false;
   uint32_t S = 0, E = 0, P = 0, bytes = 0;
@@ -207,11 +220,13 @@ struct bf_ctx {
   DevBuf<uint32_t> d_exp_counts;
   DevBuf<unsigned long long> d_offsets, d_block_sums;
   DevBuf<uint32_t> d_defer;  // [0] = count, [1..] = run ids
-  // touched ticks: [0] = list length, [1..] = the list | head word per list position | listed runs and their heads (when the
-  // caller's buffers are not pinned) | per-block sums
-  DevBuf<uint32_t> d_tlist, d_tpos_head, d_truns, d_thead;
-  DevBuf<unsigned long long> d_tsums;
+  // touched ticks: [0] for bf_resident_tick_touched, one per part for bf_resident_tick_touched_many (whose parts are all in
+  // flight before its one synchronisation)
+  std::vector<TouchScratch> touch = std::vector<TouchScratch>(1);
   uint64_t last_touched_events = 0;   // events of the previous touched tick (sizes the first D2H)
+  // bf_resident_tick_touched_many: the small results of each part, pinned (the single call uses pinned->tail)
+  bf::ResultTail* part_tails = nullptr;
+  uint32_t part_tails_cap = 0;
   // The device inputs and outputs of one resident call that is not a tick (migrate, redrive, retire, extent, narrow, transfer,
   // timers_arm, fire, sched_put, schedule, runctl_put, commit, status, resync), laid out by the call (CallStage, resident_abi.cu).  They are
   // valid from the call's staging until it returns: a call reads only bytes it uploaded, set or had a kernel write during the

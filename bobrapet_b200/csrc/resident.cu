@@ -114,10 +114,7 @@ cudaError_t launch_runctl_restop(const RunCtlRestopParams& P, cudaStream_t strea
   return cudaGetLastError();
 }
 
-__global__ void __launch_bounds__(256) apply_deltas(const DeltaParams P) {
-  const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= P.n) return;
-  const bf_delta d = P.deltas[i];
+__device__ __forceinline__ void apply_delta(const DeltaParams& P, const bf_delta d) {
   bool ok = d.run < P.n_runs;
   if (ok) atomicMax(P.mark + d.run, P.mark_value);   // touch mark (Resident in ctx.h, touched ticks); max: an upload's "must list" bit stays
   uint8_t* rec = P.state + (size_t)d.run * P.state_stride;
@@ -161,6 +158,27 @@ __global__ void __launch_bounds__(256) apply_deltas(const DeltaParams P) {
   if (!ok) atomicAdd(P.rejected, 1u);
 }
 
+__global__ void __launch_bounds__(256) apply_deltas(const DeltaParams P) {
+  const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= P.n) return;
+  apply_delta(P, P.deltas[i]);
+}
+
+// The deltas of several batches in one launch (bf_resident_tick_touched_many): delta i of the launch is delta i - first[k] of
+// batch k for the last k with first[k] <= i; first[n_parts] is the total
+__global__ void __launch_bounds__(256) apply_deltas_many(const DeltaParams* __restrict__ parts, const uint32_t* __restrict__ first,
+                                                         uint32_t n_parts) {
+  const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= first[n_parts]) return;
+  uint32_t lo = 0, hi = n_parts;
+  while (hi - lo > 1) {
+    const uint32_t mid = (lo + hi) / 2;
+    if (first[mid] <= i) lo = mid; else hi = mid;
+  }
+  const DeltaParams& P = parts[lo];
+  apply_delta(P, P.deltas[i - first[lo]]);
+}
+
 // Touch marks of runs [first, first + n) after an upload: epoch << 1 | 1 ("must list", Resident in ctx.h)
 __global__ void __launch_bounds__(256) mark_runs(uint32_t* mark, uint32_t first, uint32_t n, uint32_t value) {
   const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -188,6 +206,12 @@ __global__ void __launch_bounds__(256) move_records(const uint8_t* __restrict__ 
 cudaError_t launch_move_records(const uint8_t* src, uint8_t* dst, const void* moves, uint32_t n, cudaStream_t stream) {
   if (n == 0) return cudaSuccess;
   move_records<<<(n + 7) / 8, 256, 0, stream>>>(src, dst, static_cast<const ulonglong4*>(moves), n);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_apply_deltas_many(const DeltaParams* parts, const uint32_t* first, uint32_t n_parts, uint32_t n, cudaStream_t stream) {
+  if (n == 0) return cudaSuccess;
+  apply_deltas_many<<<(n + 255) / 256, 256, 0, stream>>>(parts, first, n_parts);
   return cudaGetLastError();
 }
 

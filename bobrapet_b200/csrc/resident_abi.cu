@@ -230,6 +230,24 @@ int bf_resident_download(bf_ctx* c, uint32_t h, uint32_t first, uint32_t n, void
   return download_runs(c, r, first, n, records, r->d_state, r->L.state_stride);
 }
 
+// The scatter of n deltas (device-visible) into batch r, counting rejected ones in *rejected
+static bf::DeltaParams delta_params(const Resident* r, const bf_delta* d_src, uint32_t n, uint32_t* rejected) {
+  bf::DeltaParams P{};
+  P.state = r->d_state; P.deltas = d_src; P.n = n; P.n_runs = r->cap;
+  P.words = r->L.words; P.state_stride = r->L.state_stride; P.off_phase = r->L.off_phase; P.off_cond = r->L.off_cond;
+  P.off_decision = r->L.off_decision; P.off_child = r->L.off_child; P.child_nibbles = r->L.child_nibbles;
+  P.rejected = rejected;
+  P.mark = r->d_mark; P.mark_value = r->mark_touched();
+  P.runctl = r->areas.d_runctl;
+  return P;
+}
+
+// The device address the scatter reads n deltas from in place: pinned host memory (one launch instead of a copy and a launch;
+// BF_NO_ZC_DELTAS restores the upload), else nullptr
+static const bf_delta* deltas_in_place(const bf_delta* deltas) {
+  return getenv("BF_NO_ZC_DELTAS") ? nullptr : static_cast<const bf_delta*>(bf::pinned_dev(deltas));
+}
+
 // H2D of the deltas + the scatter kernel on the ctx stream, no synchronisation; the rejected counter is read by the caller
 static int resident_apply_async(bf_ctx* c, Resident* r, const bf_delta* deltas, uint32_t n) {
   if (int rc = c->d_deltas.ensure(c, n ? n : 1)) return rc;
@@ -240,23 +258,11 @@ static int resident_apply_async(bf_ctx* c, Resident* r, const bf_delta* deltas, 
   c->rejected_clean = false;   // the scatter kernel may count; whoever reads the counter decides whether it is clean again
   // deltas in pinned host memory are read by the scatter kernel itself over PCIe (one launch instead of a copy and a launch:
   // BF_NO_ZC_DELTAS restores the upload), any other buffer is uploaded first
-  const bf_delta* d_src = c->d_deltas;
-  bool direct = false;
-  if (!getenv("BF_NO_ZC_DELTAS")) {
-    if (void* d = bf::pinned_dev(deltas)) {
-      d_src = static_cast<const bf_delta*>(d);
-      direct = true;
-    }
-  }
+  const bf_delta* d_src = deltas_in_place(deltas);
+  const bool direct = d_src != nullptr;
+  if (!direct) d_src = c->d_deltas;
   if (!direct) BF_CUDA(c, cudaMemcpyAsync(c->d_deltas, deltas, (size_t)n * sizeof(bf_delta), cudaMemcpyHostToDevice, s));
-  bf::DeltaParams P{};
-  P.state = r->d_state; P.deltas = d_src; P.n = n; P.n_runs = r->cap;
-  P.words = r->L.words; P.state_stride = r->L.state_stride; P.off_phase = r->L.off_phase; P.off_cond = r->L.off_cond;
-  P.off_decision = r->L.off_decision; P.off_child = r->L.off_child; P.child_nibbles = r->L.child_nibbles;
-  P.rejected = c->d_rejected;
-  P.mark = r->d_mark; P.mark_value = r->mark_touched();
-  P.runctl = r->areas.d_runctl;
-  BF_CUDA(c, bf::launch_apply_deltas(P, s));
+  BF_CUDA(c, bf::launch_apply_deltas(delta_params(r, d_src, n, c->d_rejected), s));
   c->stats.kernel_launches += 1;
   return BF_OK;
 }
@@ -366,16 +372,99 @@ int bf_resident_tick_compact(bf_ctx* c, uint32_t h, const bf_delta* deltas, uint
   return resident_tick_locked(c, r, deltas, n_deltas, n_runs, flags, max_iterations, nullptr, counts, out);
 }
 
-// A touched tick: scatter -> list build -> pass over the list (into the second result buffer) -> list-mode compaction, which
-// brings the current result records up to date.  Falls back to a full compact tick where the baseline rules require one.
-static int touched_tick_locked(bf_ctx* c, Resident* r, const bf_delta* deltas, uint32_t n_deltas, uint32_t n_runs, uint32_t flags,
-                               uint32_t max_iterations, bf_touched_out* out, bf_counts* counts) {
-  if (out->struct_size != sizeof(bf_touched_out)) return fail(c, BF_EINVAL, "bad bf_touched_out.struct_size");
+// The argument checks of a touched tick, made before anything changes: bf_resident_tick_touched's, and each part's of
+// bf_resident_tick_touched_many (whose flags are the call's, checked once)
+static int check_touched_flags(bf_ctx* c, uint32_t flags) {
   if (flags & ~(uint32_t)(BF_EVAL_FIXPOINT | BF_EVAL_NO_COUNTS)) return fail(c, BF_EINVAL, "touched ticks take BF_EVAL_FIXPOINT and BF_EVAL_NO_COUNTS only");
+  return BF_OK;
+}
+static int check_touched(bf_ctx* c, const Resident* r, const bf_delta* deltas, uint32_t n_deltas, uint32_t n_runs,
+                         const bf_touched_out* out) {
+  if (out->struct_size != sizeof(bf_touched_out)) return fail(c, BF_EINVAL, "bad bf_touched_out.struct_size");
   if (out->runs_cap && (!out->runs || !out->head)) return fail(c, BF_EINVAL, "null runs / head with a non-zero runs_cap");
   if (out->events_cap && !out->events) return fail(c, BF_EINVAL, "null events with a non-zero events_cap");
   if (n_runs > r->cap) return fail(c, BF_EINVAL, "n_runs exceeds the resident batch");
   if (n_deltas && !deltas) return fail(c, BF_EINVAL, "null deltas");
+  return BF_OK;
+}
+
+// A touched tick that is not full: what its launches and its end need
+struct TouchedTick {
+  Resident* r;
+  uint32_t n_runs, n_deltas;
+  bf_touched_out* out;
+  TouchScratch* ts;
+  uint32_t bound = 0, runs_n = 0;
+  bool posted_lists = false, posted_events = false;   // written in place by the kernels (the caller's buffers are pinned)
+  bf::TouchedParams T{};   // the list build and the compaction, with bound > 0
+};
+
+// The host side of a touched tick that is not full, before its launches: the batch's bookkeeping, the bound on its list, its
+// scratch, and the parameters of its list build and compaction (host tail, counts and rejected counter as for a single tick;
+// bf_resident_tick_touched_many points them elsewhere).  Lists go to the caller's pinned buffers in place, else to t.ts (runs,
+// head) and `events`, for the caller to download.  With t.bound == 0 nothing below n_runs can be touched: no launch beyond the
+// scatter.
+static int touched_prepare(bf_ctx* c, TouchedTick& t, uint32_t flags, DevBuf<uint16_t>& events) {
+  Resident* r = t.r;
+  TouchScratch& ts = *t.ts;
+  c->snap.valid = false;
+  if (t.n_deltas) r->ticked = -1;
+  const uint32_t bound = t.bound = (uint32_t)std::min<uint64_t>(t.n_runs, r->pending + t.n_deltas);   // >= the touched runs below n_runs
+  r->pending += t.n_deltas;
+  const uint64_t cap = t.out->events ? t.out->events_cap : 0;
+  const uint32_t runs_n = t.runs_n = std::min(bound, t.out->runs_cap);
+  if (int rc = r->result_prev(c)) return rc;
+  const uint32_t nb = (bound + 511) / 512, nbl = (r->cap + 2047) / 2048;
+  if (int rc = ts.list.ensure(c, (size_t)bound + 1)) return rc;
+  if (int rc = ts.pos_head.ensure(c, bound ? bound : 1)) return rc;
+  if (int rc = ts.sums.ensure(c, 2 * (size_t)nb + 2 * (size_t)nbl + 1)) return rc;
+  if (int rc = events.ensure(c, cap ? (size_t)cap : 1)) return rc;
+  uint32_t* p_runs = static_cast<uint32_t*>(bf::pinned_dev(t.out->runs));
+  uint32_t* p_head = static_cast<uint32_t*>(bf::pinned_dev(t.out->head));
+  uint16_t* p_events = cap ? static_cast<uint16_t*>(bf::pinned_dev(t.out->events)) : nullptr;
+  t.posted_lists = p_runs && p_head; t.posted_events = p_events != nullptr;
+  if (!t.posted_lists) {
+    if (int rc = ts.runs.ensure(c, runs_n ? runs_n : 1)) return rc;
+    if (int rc = ts.head.ensure(c, runs_n ? runs_n : 1)) return rc;
+  }
+  bf::TouchedParams& T = t.T;
+  T.C = bf::compact_params(c, r->L, bound, !(flags & BF_EVAL_NO_COUNTS), true);
+  T.C.result = r->d_result_prev; T.C.prev_result = r->d_result;
+  T.C.events = p_events ? p_events : events.p; T.C.cap = cap;
+  T.mark = r->d_mark; T.full_epoch = r->full_epoch; T.n_scan = t.n_runs; T.n_marks = r->cap; T.bound = bound;
+  T.list = ts.list + 1; T.list_count = ts.list; T.pos_head = ts.pos_head;
+  T.sums = ts.sums; T.sums_listed = ts.sums + nb; T.scan_sums = ts.sums + 2 * (size_t)nb;
+  T.carry_sums = T.scan_sums + nbl;
+  T.out_runs = t.posted_lists ? p_runs : ts.runs.p; T.out_head = t.posted_lists ? p_head : ts.head.p; T.runs_cap = runs_n;
+  return BF_OK;
+}
+
+// The pass of a touched tick over its list (into the batch's second result buffer), adding its counts into `counts`
+static int touched_pass(bf_ctx* c, const TouchedTick& t, uint32_t flags, uint32_t max_iterations, unsigned long long* counts) {
+  bf_batch db{};
+  db.struct_size = sizeof(bf_batch);
+  db.flags = flags | BF_EVAL_COUNTS_SET; db.max_iterations = max_iterations; db.layout = t.r->L; db.n_runs = t.bound;
+  return bf::run_pass(c, db, t.r->d_state, t.r->d_result_prev, nullptr, counts, c->stream, t.ts->list + 1, t.ts->list);
+}
+
+// The end of a touched tick that is not full, once the stream is synchronised, from the tail its last kernel posted (zero where
+// no kernel ran): the batch's pending runs and tick, the evaluated snapshot, the counts and the out fields.  Both touched calls
+// end their list-mode ticks here.
+static void touched_end(bf_ctx* c, const TouchedTick& t, uint32_t flags, const bf::ResultTail& tail, bf_counts* counts) {
+  Resident* r = t.r;
+  if (t.bound) r->pending = tail.carried;   // every touched run below n_runs was evaluated: the ones above it are all that is left
+  r->tick_done(t.n_runs, flags);
+  c->snap = {true, t.n_runs, r->L, r->d_state, r->d_result};
+  if (counts) *counts = {tail.counts[0], tail.counts[1], tail.counts[2], tail.counts[3]};
+  t.out->full = 0; t.out->n_listed = (uint32_t)tail.listed; t.out->n_evaluated = (uint32_t)tail.evaluated; t.out->n_events = tail.events;
+}
+
+// A touched tick: scatter -> list build -> pass over the list -> list-mode compaction, which brings the current result records up
+// to date; or a full compact tick where the baseline rules require one.
+static int touched_tick_locked(bf_ctx* c, Resident* r, const bf_delta* deltas, uint32_t n_deltas, uint32_t n_runs, uint32_t flags,
+                               uint32_t max_iterations, bf_touched_out* out, bf_counts* counts) {
+  if (int rc = check_touched_flags(c, flags)) return rc;
+  if (int rc = check_touched(c, r, deltas, n_deltas, n_runs, out)) return rc;
   BF_CUDA(c, cudaSetDevice(c->device));
   bf_compact_out co{};   // the event list, as a compact tick returns it
   co.struct_size = sizeof co; co.events = out->events; co.events_cap = out->events_cap;
@@ -389,57 +478,26 @@ static int touched_tick_locked(bf_ctx* c, Resident* r, const bf_delta* deltas, u
     return rc;
   }
 
-  c->snap.valid = false;
-  if (n_deltas) r->ticked = -1;
   cudaStream_t s = c->stream;
-  const bf_layout& L = r->L;
-  const uint32_t bound = (uint32_t)std::min<uint64_t>(n_runs, r->pending + n_deltas);   // >= the touched runs below n_runs
-  r->pending += n_deltas;
-  const uint64_t cap = out->events ? out->events_cap : 0;
-  const uint32_t runs_n = std::min(bound, out->runs_cap);
-  if (int rc = r->result_prev(c)) return rc;
-  const uint32_t nb = (bound + 511) / 512, nbl = (r->cap + 2047) / 2048;
-  if (int rc = c->d_tlist.ensure(c, (size_t)bound + 1)) return rc;
-  if (int rc = c->d_tpos_head.ensure(c, bound ? bound : 1)) return rc;
-  if (int rc = c->d_tsums.ensure(c, 2 * (size_t)nb + 2 * (size_t)nbl + 1)) return rc;
-  if (int rc = c->d_events.ensure(c, cap ? (size_t)cap : 1)) return rc;
-  // the caller's pinned buffers get the lists posted by the emit kernel, any other buffer gets them by a download
-  uint32_t* p_runs = static_cast<uint32_t*>(bf::pinned_dev(out->runs));
-  uint32_t* p_head = static_cast<uint32_t*>(bf::pinned_dev(out->head));
-  uint16_t* p_events = cap ? static_cast<uint16_t*>(bf::pinned_dev(out->events)) : nullptr;
-  if (!p_runs || !p_head) {
-    if (int rc = c->d_truns.ensure(c, runs_n ? runs_n : 1)) return rc;
-    if (int rc = c->d_thead.ensure(c, runs_n ? runs_n : 1)) return rc;
-  }
+  TouchedTick t{r, n_runs, n_deltas, out, &c->touch[0]};
   uint64_t first_slice = 0;
   auto body = [&]() -> int {
+    if (int rc = touched_prepare(c, t, flags, c->d_events)) return rc;
     if (int rc = resident_apply_async(c, r, deltas, n_deltas)) return rc;
-    if (bound == 0) {   // nothing below n_runs can be touched: no launch beyond the scatter
+    if (t.bound == 0) {   // no launch beyond the scatter
       if (n_deltas) BF_CUDA(c, cudaMemcpyAsync(&c->pinned->word, c->d_rejected, 4, cudaMemcpyDeviceToHost, s));
       return BF_OK;
     }
-    bf::TouchedParams T{};
-    T.C = bf::compact_params(c, L, bound, !(flags & BF_EVAL_NO_COUNTS), true);
-    T.C.result = r->d_result_prev; T.C.prev_result = r->d_result;
-    T.C.events = p_events ? p_events : c->d_events; T.C.cap = cap;
-    T.mark = r->d_mark; T.full_epoch = r->full_epoch; T.n_scan = n_runs; T.n_marks = r->cap; T.bound = bound;
-    T.list = c->d_tlist + 1; T.list_count = c->d_tlist; T.pos_head = c->d_tpos_head;
-    T.sums = c->d_tsums; T.sums_listed = c->d_tsums + nb; T.scan_sums = c->d_tsums + 2 * (size_t)nb;
-    T.carry_sums = T.scan_sums + nbl;
-    T.out_runs = p_runs && p_head ? p_runs : c->d_truns; T.out_head = p_runs && p_head ? p_head : c->d_thead; T.runs_cap = runs_n;
     c->rejected_clean = false;   // the emit kernel delivers and clears the counter; a failed call leaves it to be zeroed
-    BF_CUDA(c, bf::launch_touched_list(T, s));
-    bf_batch db{};
-    db.struct_size = sizeof(bf_batch);
-    db.flags = flags | BF_EVAL_COUNTS_SET; db.max_iterations = max_iterations; db.layout = L; db.n_runs = bound;
-    if (int rc = bf::run_pass(c, db, r->d_state, r->d_result_prev, nullptr, c->d_counts, s, c->d_tlist + 1, c->d_tlist)) return rc;
-    BF_CUDA(c, bf::launch_touched_compact(T, s));
+    BF_CUDA(c, bf::launch_touched_list(t.T, s));
+    if (int rc = touched_pass(c, t, flags, max_iterations, c->d_counts)) return rc;
+    BF_CUDA(c, bf::launch_touched_compact(t.T, s));
     c->stats.kernel_launches += 4;
-    if (runs_n && !(p_runs && p_head)) {
-      BF_CUDA(c, cudaMemcpyAsync(out->runs, c->d_truns, (size_t)runs_n * 4, cudaMemcpyDeviceToHost, s));
-      BF_CUDA(c, cudaMemcpyAsync(out->head, c->d_thead, (size_t)runs_n * 4, cudaMemcpyDeviceToHost, s));
+    if (t.runs_n && !t.posted_lists) {
+      BF_CUDA(c, cudaMemcpyAsync(out->runs, t.ts->runs, (size_t)t.runs_n * 4, cudaMemcpyDeviceToHost, s));
+      BF_CUDA(c, cudaMemcpyAsync(out->head, t.ts->head, (size_t)t.runs_n * 4, cudaMemcpyDeviceToHost, s));
     }
-    return bf::events_first(c, out->events, c->last_touched_events, 1024, cap, p_events != nullptr, s, first_slice);
+    return bf::events_first(c, out->events, c->last_touched_events, 1024, co.events ? co.events_cap : 0, t.posted_events, s, first_slice);
   };
   const int rc = body();
   const cudaError_t es = cudaStreamSynchronize(s);
@@ -450,16 +508,14 @@ static int touched_tick_locked(bf_ctx* c, Resident* r, const bf_delta* deltas, u
   }
   bf::ResultTail& tail = c->pinned->tail;
   uint64_t rejected = tail.rejected;
-  if (bound == 0) {   // no kernel ran: the counter is zeroed before its next use
+  if (t.bound == 0) {   // no kernel ran: the counter is zeroed before its next use
     rejected = n_deltas ? c->pinned->word : 0u;
-    tail = bf::ResultTail{};   // no kernel wrote the tail: compact_finish and the counts read nothing evaluated or listed
+    tail = bf::ResultTail{};   // no kernel wrote the tail: nothing evaluated or listed
   } else {
-    r->pending = tail.carried;   // every touched run below n_runs was evaluated: the ones above it are all that is left
     c->rejected_clean = true;    // delivered and cleared by the emit kernel
   }
-  r->tick_done(n_runs, flags);
-  if (int rc2 = bf::publish_pass(c, n_runs, L, r->d_state, r->d_result, counts, &co, first_slice, c->last_touched_events)) return rc2;
-  out->full = 0; out->n_listed = co.n_listed; out->n_evaluated = (uint32_t)tail.evaluated; out->n_events = co.n_events;
+  touched_end(c, t, flags, tail, counts);
+  if (int rc2 = bf::compact_finish(c, &co, first_slice, c->last_touched_events)) return rc2;   // the events the first slice missed
   return rejected_deltas(c, rejected, true);
 }
 
@@ -469,6 +525,188 @@ int bf_resident_tick_touched(bf_ctx* c, uint32_t h, const bf_delta* deltas, uint
   if (!out) return fail(c, BF_EINVAL, "null bf_touched_out");
   if (!r) return BF_EINVAL;
   return touched_tick_locked(c, r, deltas, n_deltas, n_runs, flags, max_iterations, out, counts);
+}
+
+// Several touched ticks, one per part, with one synchronisation.  Every part is checked first.  A part whose tick is full runs as
+// its single call does (own synchronisation).  The other parts tick together: one upload of their part tables, deltas and zeroed
+// counters; one scatter launch over every part's deltas; one list-build launch pair over every part's touch marks; one pass per
+// part (each batch has its own kernel build and launch plan), back to back; one compaction launch pair over every part's list;
+// one D2H of the parts' rejected-delta counters; one synchronisation.  Each part has its own list scratch, counts block, pinned
+// tail and counter, so no part's results are overwritten before the host reads them.  The parts then end in part order as
+// single ticks end (touched_end), pageable lists are downloaded now that their lengths are known, and the evaluated snapshot is
+// the last part's, as after the per-part calls.
+int bf_resident_tick_touched_many(bf_ctx* c, uint32_t flags, uint32_t max_iterations, bf_tick_part* parts, uint32_t n_parts,
+                                  uint32_t* bad_part) {
+  if (bad_part) *bad_part = BF_COMMIT_NONE;
+  if (!c) return BF_EINVAL;
+  std::lock_guard<std::mutex> g(c->mu);
+  if (n_parts && !parts) return fail(c, BF_EINVAL, "null parts");
+  if (int rc = check_touched_flags(c, flags)) return rc;
+  auto name = [&](uint32_t k, int rc) {   // a refusal or failure of part k
+    if (bad_part) *bad_part = k;
+    c->err = "parts[" + std::to_string(k) + "]: " + c->err;
+    return rc;
+  };
+  std::vector<Resident*> rs(n_parts);
+  std::unordered_map<uint32_t, uint32_t> named;   // handle -> the part naming it
+  for (uint32_t k = 0; k < n_parts; ++k) {
+    const bf_tick_part& p = parts[k];
+    if (p.struct_size != sizeof(bf_tick_part)) return name(k, fail(c, BF_EINVAL, "bad bf_tick_part.struct_size"));
+    if (!p.out) return name(k, fail(c, BF_EINVAL, "null bf_touched_out"));
+    if (!(rs[k] = live_batch(c, p.handle))) return name(k, fail(c, BF_EINVAL, "unknown resident batch"));
+    if (!named.emplace(p.handle, k).second)
+      return name(k, fail(c, BF_EINVAL, "parts " + std::to_string(named[p.handle]) + " and " + std::to_string(k) + " name the same resident batch"));
+    if (int rc = check_touched(c, rs[k], p.deltas, p.n_deltas, p.n_runs, p.out)) return name(k, rc);
+  }
+  if (n_parts == 0) return BF_OK;
+  BF_CUDA(c, cudaSetDevice(c->device));
+  // after a failure the records and marks of any part may be half updated: every part's next touched tick is full
+  auto failed = [&](uint32_t k, int rc) {
+    for (Resident* r : rs) r->need_full = true;
+    return name(k, rc);
+  };
+  uint32_t first_rejected = BF_COMMIT_NONE;
+  std::string rejected_msg;
+  auto note_rejected = [&](uint32_t k, uint64_t n) {
+    if (!n || first_rejected <= k) return;
+    first_rejected = k;
+    rejected_deltas(c, n, true);
+    rejected_msg = c->err;
+  };
+
+  std::vector<uint32_t> group;   // the parts that tick together, ascending
+  for (uint32_t k = 0; k < n_parts; ++k) {
+    const bf_tick_part& p = parts[k];
+    if (!rs[k]->full_due(c, p.n_runs, flags, max_iterations)) { group.push_back(k); continue; }
+    const int rc = touched_tick_locked(c, rs[k], p.deltas, p.n_deltas, p.n_runs, flags, max_iterations, p.out, p.counts);
+    if (rc == BF_EINVAL && first_rejected > k) {   // the checks passed, so rejected deltas: the others were applied and the pass ran
+      first_rejected = k;
+      rejected_msg = c->err;
+    } else if (rc != BF_OK && rc != BF_EINVAL) {
+      return failed(k, rc);
+    }
+  }
+
+  const uint32_t n = (uint32_t)group.size();
+  if (n) {
+    if (c->part_tails_cap < n) {   // pinned: a tail per part, then a rejected-delta count per part
+      bf::ResultTail* nt = nullptr;
+      const cudaError_t e = cudaHostAlloc(&nt, (size_t)n * (sizeof(bf::ResultTail) + 4), cudaHostAllocDefault);
+      if (e != cudaSuccess) { cudaGetLastError(); return failed(group[0], fail(c, BF_ENOMEM, std::string("cudaHostAlloc: ") + cudaGetErrorString(e))); }
+      if (c->part_tails) cudaFreeHost(c->part_tails);
+      c->part_tails = nt; c->part_tails_cap = n;
+    }
+    uint32_t* h_rejected = reinterpret_cast<uint32_t*>(c->part_tails + c->part_tails_cap);
+    if (c->touch.size() < n) c->touch.resize(n);
+    std::vector<TouchedTick> ticks;
+    ticks.reserve(n);
+    for (uint32_t i = 0; i < n; ++i) {
+      const bf_tick_part& p = parts[group[i]];
+      ticks.push_back(TouchedTick{rs[group[i]], p.n_runs, p.n_deltas, p.out, &c->touch[i]});
+      c->part_tails[i] = bf::ResultTail{};
+      if (int rc = touched_prepare(c, ticks[i], flags, c->touch[i].events)) return failed(group[i], rc);
+    }
+    // one upload: delta tables | delta starts | list-mode tables | list-build starts | compaction starts | counters | counts |
+    // pageable deltas.  The tables hold device addresses inside it, so it is laid out and allocated first.
+    std::vector<uint32_t> listed;   // the ticks with launches beyond the scatter
+    for (uint32_t i = 0; i < n; ++i)
+      if (ticks[i].bound) listed.push_back(i);
+    const uint32_t m = (uint32_t)listed.size();
+    size_t at = 0;
+    auto take = [&](size_t bytes) { const size_t o = at; at = round_up_sz(at + bytes, 16); return o; };
+    const size_t o_dp = take(n * sizeof(bf::DeltaParams)), o_df = take((n + 1) * 4), o_tp = take(m * sizeof(bf::TouchedParams));
+    const size_t o_lf = take((m + 1) * 4), o_cf = take((m + 1) * 4), o_rej = take(n * 4), o_cnt = take((size_t)n * 32);
+    std::vector<const bf_delta*> in_place(n);
+    uint64_t staged = 0, total = 0;
+    for (uint32_t i = 0; i < n; ++i) {
+      in_place[i] = ticks[i].n_deltas ? deltas_in_place(parts[group[i]].deltas) : nullptr;
+      if (!in_place[i]) staged += ticks[i].n_deltas;
+      total += ticks[i].n_deltas;
+    }
+    if (total >= (1ull << 32)) return failed(group[0], fail(c, BF_EINVAL, "more than 2^32 - 1 deltas in one call"));
+    const size_t o_d = take(staged * sizeof(bf_delta));
+    if (int rc = c->d_call.ensure(c, std::max<size_t>(at, 16))) return failed(group[0], rc);
+    uint8_t* d = c->d_call;
+    std::vector<uint8_t> image(at, 0);
+    auto* dp = reinterpret_cast<bf::DeltaParams*>(image.data() + o_dp);
+    auto* df = reinterpret_cast<uint32_t*>(image.data() + o_df);
+    auto* tp = reinterpret_cast<bf::TouchedParams*>(image.data() + o_tp);
+    auto* lf = reinterpret_cast<uint32_t*>(image.data() + o_lf);
+    auto* cf = reinterpret_cast<uint32_t*>(image.data() + o_cf);
+    auto* cnt = reinterpret_cast<unsigned long long*>(d + o_cnt);
+    auto* rej = reinterpret_cast<uint32_t*>(d + o_rej);
+    uint64_t off = 0, soff = 0;
+    for (uint32_t i = 0; i < n; ++i) {
+      const bf_delta* src = in_place[i];
+      if (!src) {
+        src = reinterpret_cast<const bf_delta*>(d + o_d) + soff;
+        if (ticks[i].n_deltas) memcpy(image.data() + o_d + soff * sizeof(bf_delta), parts[group[i]].deltas, (size_t)ticks[i].n_deltas * sizeof(bf_delta));
+        soff += ticks[i].n_deltas;
+      }
+      dp[i] = delta_params(ticks[i].r, src, ticks[i].n_deltas, rej + i);
+      df[i] = (uint32_t)off;
+      off += ticks[i].n_deltas;
+    }
+    df[n] = (uint32_t)off;
+    uint32_t lb = 0, cb = 0;
+    for (uint32_t j = 0; j < m; ++j) {
+      const uint32_t i = listed[j];
+      bf::TouchedParams T = ticks[i].T;
+      T.C.host_tail = &c->part_tails[i];
+      T.C.counts = (flags & BF_EVAL_NO_COUNTS) ? nullptr : cnt + 4 * (size_t)i;
+      T.C.rejected = nullptr;   // the counters come back in one copy behind the compaction
+      tp[j] = T;
+      lf[j] = lb; cf[j] = cb;
+      lb += (T.n_marks + 2047) / 2048; cb += (T.bound + 511) / 512;
+    }
+    lf[m] = lb; cf[m] = cb;
+    cudaStream_t s = c->stream;
+    auto issue = [&]() -> int {
+      BF_CUDA(c, cudaMemcpyAsync(d, image.data(), at, cudaMemcpyHostToDevice, s));
+      BF_CUDA(c, bf::launch_apply_deltas_many(reinterpret_cast<bf::DeltaParams*>(d + o_dp), reinterpret_cast<uint32_t*>(d + o_df), n,
+                                              (uint32_t)total, s));
+      if (m) {
+        const auto* dtp = reinterpret_cast<const bf::TouchedParams*>(d + o_tp);
+        BF_CUDA(c, bf::launch_touched_list_many(dtp, reinterpret_cast<uint32_t*>(d + o_lf), m, lb, s));
+        for (uint32_t j = 0; j < m; ++j)
+          if (int rc = touched_pass(c, ticks[listed[j]], flags, max_iterations, cnt + 4 * (size_t)listed[j])) return rc;
+        BF_CUDA(c, bf::launch_touched_compact_many(dtp, reinterpret_cast<uint32_t*>(d + o_cf), m, cb, s));
+      }
+      c->stats.kernel_launches += (total ? 1 : 0) + (m ? 4 : 0);
+      BF_CUDA(c, cudaMemcpyAsync(h_rejected, rej, (size_t)n * 4, cudaMemcpyDeviceToHost, s));
+      return BF_OK;
+    };
+    const int rc = issue();
+    const cudaError_t es = cudaStreamSynchronize(s);
+    if (rc != BF_OK) return failed(group[0], rc);
+    if (es != cudaSuccess) return failed(group[0], cuda_fail(c, es, "cudaStreamSynchronize"));
+    for (uint32_t i = 0; i < n; ++i) {
+      const uint32_t k = group[i];
+      const TouchedTick& t = ticks[i];
+      const bf::ResultTail& tail = c->part_tails[i];
+      touched_end(c, t, flags, tail, parts[k].counts);
+      c->last_touched_events = tail.events;
+      // pageable lists: downloaded now that their lengths are known
+      bf_touched_out* out = t.out;
+      const uint32_t nl = std::min(out->n_listed, out->runs_cap);
+      const uint64_t ne = std::min<uint64_t>(tail.events, out->events ? out->events_cap : 0);
+      cudaError_t e = cudaSuccess;
+      if (nl && !t.posted_lists) {
+        e = cudaMemcpyAsync(out->runs, t.ts->runs, (size_t)nl * 4, cudaMemcpyDeviceToHost, s);
+        if (e == cudaSuccess) e = cudaMemcpyAsync(out->head, t.ts->head, (size_t)nl * 4, cudaMemcpyDeviceToHost, s);
+      }
+      if (e == cudaSuccess && ne && !t.posted_events) e = cudaMemcpyAsync(out->events, t.ts->events, (size_t)ne * 2, cudaMemcpyDeviceToHost, s);
+      if (e != cudaSuccess) { cudaStreamSynchronize(s); return failed(k, cuda_fail(c, e, "cudaMemcpyAsync")); }
+      note_rejected(k, h_rejected[i]);
+    }
+    if (const int rc2 = bf::end_call(c, cudaSuccess, "cudaMemcpyAsync")) return failed(group[0], rc2);
+  }
+  Resident* last = rs[n_parts - 1];   // the evaluated snapshot is the last part's, as after the per-part calls
+  c->snap = {true, parts[n_parts - 1].n_runs, last->L, last->d_state, last->d_result};
+  if (first_rejected == BF_COMMIT_NONE) return BF_OK;
+  if (bad_part) *bad_part = first_rejected;
+  c->err = "parts[" + std::to_string(first_rejected) + "]: " + rejected_msg;
+  return BF_EINVAL;
 }
 
 // A Story edited while its runs are live: re-index the runs of old_slot to new_slot's step indices in place (resident.cu).  All

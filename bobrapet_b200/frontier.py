@@ -234,6 +234,50 @@ class Frontier:
                 "n_listed": int(to.n_listed), "n_evaluated": int(to.n_evaluated), "n_events": int(to.n_events),
                 "counts": {"ready": counts.ready, "skip": counts.skip, "expansion": counts.expansion, "evals": counts.evals}}
 
+    def resident_tick_touched_many(self, parts, flags: int = 0, max_iterations: int = 0):
+        """bf_resident_tick_touched_many: the touched ticks of several resident batches of this ctx in one call and one
+        synchronisation.  Each part is a dict with handle, n_runs, deltas, runs_cap and events_cap, and optionally runs / head /
+        events buffers (as resident_tick_touched takes them) and counts=False (pass no counts block).  -> one dict per part,
+        shaped as resident_tick_touched returns it (counts None without a counts block).  A refusal or failure raises
+        FrontierError with .bad_part set: the part it names, or A.COMMIT_NONE."""
+        n = len(parts)
+        cparts = (A.TickPart * max(n, 1))()
+        keep = []
+        for k, p in enumerate(parts):
+            deltas = p["deltas"]
+            assert deltas.dtype == self.DELTA_DTYPE and deltas.flags["C_CONTIGUOUS"]
+            runs_cap, events_cap = p["runs_cap"], p["events_cap"]
+            runs, head, events = p.get("runs"), p.get("head"), p.get("events")
+            if runs is None:
+                runs = np.zeros(max(runs_cap, 1), dtype=np.uint32)
+            if head is None:
+                head = np.zeros(max(runs_cap, 1), dtype=np.uint32)
+            if events is None:
+                events = np.zeros(max(events_cap, 1), dtype=np.uint16)
+            for a, dt, m in ((runs, np.uint32, runs_cap), (head, np.uint32, runs_cap), (events, np.uint16, events_cap)):
+                assert a.dtype == dt and a.flags["C_CONTIGUOUS"] and a.shape[0] >= m
+            to = A.TouchedOut(struct_size=C.sizeof(A.TouchedOut), runs=runs.ctypes.data, head=head.ctypes.data, runs_cap=runs_cap,
+                              events=events.ctypes.data, events_cap=events_cap)
+            counts = A.Counts() if p.get("counts", True) else None
+            cparts[k] = A.TickPart(struct_size=C.sizeof(A.TickPart), handle=p["handle"], deltas=deltas.ctypes.data,
+                                   n_deltas=deltas.shape[0], n_runs=p["n_runs"], out=C.addressof(to),
+                                   counts=(C.addressof(counts) if counts is not None else None))
+            keep.append((to, counts, runs, head, events, runs_cap, events_cap))
+        bad = C.c_uint32(0)
+        rc = self._lib.bf_resident_tick_touched_many(self._ctx, flags, max_iterations, cparts, n, C.byref(bad))
+        if rc != A.BF_OK:
+            err = A.FrontierError(rc, "bf_resident_tick_touched_many: %s" % self._lib.bf_last_error(self._ctx).decode())
+            err.bad_part = bad.value
+            raise err
+        res = []
+        for to, counts, runs, head, events, runs_cap, events_cap in keep:
+            nl = min(int(to.n_listed), runs_cap)
+            res.append({"full": int(to.full), "runs": runs[:nl], "head": head[:nl], "events": events[:min(int(to.n_events), events_cap)],
+                        "n_listed": int(to.n_listed), "n_evaluated": int(to.n_evaluated), "n_events": int(to.n_events),
+                        "counts": None if counts is None else
+                        {"ready": counts.ready, "skip": counts.skip, "expansion": counts.expansion, "evals": counts.evals}})
+        return res
+
     def resident_migrate(self, handle: int, old_slot: int, new_slot: int, step_map, n_runs: int) -> int:
         """bf_resident_migrate: move the runs in [0, n_runs) on old_slot to new_slot (an edited Story), re-indexing their step
         state in place.  step_map[i] = new index of old step i, or A.MIGRATE_GONE.  -> number of runs migrated."""

@@ -347,6 +347,60 @@ func (r *Resident) TickTouched(deltas []Delta, n, flags uint32, runs, head []uin
 	return Touched{Full: full != 0, NListed: uint32(nl), NEvaluated: uint32(ne), NEvents: uint64(nev)}, k, r.c.err(rc)
 }
 
+// TickPart is one batch of Ctx.TickTouched, with the arguments Resident.TickTouched takes for it.
+type TickPart struct {
+	R      *Resident
+	Deltas []Delta
+	N      uint32
+	Runs   []uint32
+	Head   []uint32
+	Events []uint16
+}
+
+// TickTouched runs the touched ticks of several batches of this ctx, e.g. one per width class, in one call and one
+// synchronisation (bf_resident_tick_touched_many).  Part i gets what parts[i].R.TickTouched would give, called in order; its
+// lists land in parts[i].Runs / Head / Events as there.  badPart names the first refused part, or the first part with a
+// rejected delta (the call still ticked every part then), or is CommitNone.  Pass the same batches to ScheduleResident next.
+func (c *Ctx) TickTouched(flags uint32, parts ...TickPart) (ts []Touched, ks []Counts, badPart uint32, err error) {
+	n := len(parts)
+	handles, nRuns := make([]uint32, n), make([]uint32, n)
+	deltaFirst, runsFirst, eventsFirst := make([]uint32, n+1), make([]uint32, n+1), make([]uint64, n+1)
+	var deltas []Delta
+	for i, p := range parts {
+		handles[i], nRuns[i] = p.R.handle, p.N
+		deltas = append(deltas, p.Deltas...)
+		capRuns := len(p.Runs)
+		if len(p.Head) < capRuns {
+			capRuns = len(p.Head)
+		}
+		deltaFirst[i+1] = deltaFirst[i] + uint32(len(p.Deltas))
+		runsFirst[i+1] = runsFirst[i] + uint32(capRuns)
+		eventsFirst[i+1] = eventsFirst[i] + uint64(len(p.Events))
+	}
+	// one flat buffer per list (Go memory without Go pointers), copied back into each part's slices
+	runs, head, events := make([]uint32, runsFirst[n]+1), make([]uint32, runsFirst[n]+1), make([]uint16, eventsFirst[n]+1)
+	var dp *C.bf_delta
+	if len(deltas) > 0 {
+		dp = (*C.bf_delta)(unsafe.Pointer(&deltas[0]))
+	}
+	full, nl, ne := make([]uint32, n+1), make([]uint32, n+1), make([]uint32, n+1)
+	nev := make([]uint64, n+1)
+	ks = make([]Counts, n+1)
+	var bad C.uint32_t
+	rc := C.bfgo_resident_tick_touched_many(c.p, C.uint32_t(flags), 0, C.uint32_t(n), u32p(handles), u32p(nRuns), dp, u32p(deltaFirst),
+		u32p(runs), u32p(head), u32p(runsFirst), (*C.uint16_t)(unsafe.Pointer(&events[0])),
+		(*C.uint64_t)(unsafe.Pointer(&eventsFirst[0])), u32p(full), u32p(nl), u32p(ne), (*C.uint64_t)(unsafe.Pointer(&nev[0])),
+		(*C.bf_counts)(unsafe.Pointer(&ks[0])), &bad)
+	ts = make([]Touched, n)
+	for i, p := range parts {
+		ts[i] = Touched{Full: full[i] != 0, NListed: nl[i], NEvaluated: ne[i], NEvents: nev[i]}
+		copy(p.Runs, runs[runsFirst[i]:runsFirst[i+1]])
+		copy(p.Head, head[runsFirst[i]:runsFirst[i+1]])
+		copy(p.Events, events[eventsFirst[i]:eventsFirst[i+1]])
+	}
+	return ts, ks[:n], uint32(bad), c.err(rc)
+}
+
 // MigrateGone marks an old step that has no step of the new Story generation (BF_MIGRATE_GONE).
 const MigrateGone = 0xFFFF
 

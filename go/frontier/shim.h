@@ -14,6 +14,7 @@
 #ifndef BOBRAFRONTIER_GO_SHIM_H_
 #define BOBRAFRONTIER_GO_SHIM_H_
 
+#include <stdlib.h>
 #include <string.h>
 
 #include "bobrafrontier.h"
@@ -94,6 +95,53 @@ static inline int bfgo_resident_tick_touched(bf_ctx* c, uint32_t handle, const b
   *n_listed = to.n_listed;
   *n_evaluated = to.n_evaluated;
   *n_events = to.n_events;
+  return rc;
+}
+
+/* bf_resident_tick_touched_many over flat arrays: part k is batch handles[k] over n_runs[k] runs, its deltas are
+ * deltas[delta_first[k] .. delta_first[k + 1]), its runs / head lists runs[runs_first[k] ..] and head[runs_first[k] ..] up to
+ * runs_first[k + 1], its events events[events_first[k] .. events_first[k + 1]); its outputs land at index k of full, n_listed,
+ * n_evaluated, n_events and counts.  The part and out structs are built here, in C memory.                                 */
+static inline int bfgo_resident_tick_touched_many(bf_ctx* c, uint32_t flags, uint32_t max_iterations, uint32_t n_parts,
+                                                  const uint32_t* handles, const uint32_t* n_runs, const bf_delta* deltas,
+                                                  const uint32_t* delta_first, uint32_t* runs, uint32_t* head,
+                                                  const uint32_t* runs_first, uint16_t* events, const uint64_t* events_first,
+                                                  uint32_t* full, uint32_t* n_listed, uint32_t* n_evaluated, uint64_t* n_events,
+                                                  bf_counts* counts, uint32_t* bad_part) {
+  bf_tick_part* parts = (bf_tick_part*)calloc(n_parts ? n_parts : 1, sizeof(bf_tick_part));
+  bf_touched_out* outs = (bf_touched_out*)calloc(n_parts ? n_parts : 1, sizeof(bf_touched_out));
+  if (!parts || !outs) {
+    free(parts);
+    free(outs);
+    *bad_part = 0xFFFFFFFFu;
+    return BF_ENOMEM;
+  }
+  for (uint32_t k = 0; k < n_parts; ++k) {
+    bf_touched_out* o = &outs[k];
+    o->struct_size = (uint32_t)sizeof *o;
+    o->runs_cap = runs_first[k + 1] - runs_first[k];
+    o->runs = o->runs_cap ? runs + runs_first[k] : NULL;
+    o->head = o->runs_cap ? head + runs_first[k] : NULL;
+    o->events_cap = events_first[k + 1] - events_first[k];
+    o->events = o->events_cap ? events + events_first[k] : NULL;
+    bf_tick_part* p = &parts[k];
+    p->struct_size = (uint32_t)sizeof *p;
+    p->handle = handles[k];
+    p->n_deltas = delta_first[k + 1] - delta_first[k];
+    p->deltas = p->n_deltas ? deltas + delta_first[k] : NULL;
+    p->n_runs = n_runs[k];
+    p->out = o;
+    p->counts = &counts[k];
+  }
+  const int rc = bf_resident_tick_touched_many(c, flags, max_iterations, parts, n_parts, bad_part);
+  for (uint32_t k = 0; k < n_parts; ++k) {
+    full[k] = outs[k].full;
+    n_listed[k] = outs[k].n_listed;
+    n_evaluated[k] = outs[k].n_evaluated;
+    n_events[k] = outs[k].n_events;
+  }
+  free(parts);
+  free(outs);
   return rc;
 }
 

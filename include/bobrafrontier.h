@@ -576,6 +576,40 @@ typedef struct bf_touched_out {
 int bf_resident_tick_touched(bf_ctx* ctx, uint32_t handle, const bf_delta* deltas, uint32_t n_deltas, uint32_t n_runs,
                              uint32_t flags, uint32_t max_iterations, bf_touched_out* out, bf_counts* counts);
 
+/* Touched ticks of several resident batches of one ctx in one call, e.g. one batch per width class (INTEGRATION.md step 5).
+ * Each part is one bf_resident_tick_touched: its handle, deltas, n_runs, out and counts mean what that call's arguments mean;
+ * flags and max_iterations are shared.
+ *   - Equivalence: every batch and touch mark, every counts block, the out fields and the listed entries of runs / head /
+ *     events (the first min(n_listed, runs_cap) and min(n_events, events_cap)) end as after calling bf_resident_tick_touched
+ *     once per part in array order, including the full rules, the truncation at the caps with true counts and the tick that
+ *     bf_resident_schedule and the commits read.  Entries past those are not defined by either call.
+ *   - Refusals come first: flags (as bf_resident_tick_touched takes them) and parts, then every part (struct_size, a live
+ *     handle, n_runs within the batch, the out, runs, head and events pointers, null deltas), and no two parts may name one
+ *     batch.  On a refusal the call returns BF_EINVAL, *bad_part names the first bad part (BF_COMMIT_NONE for bad flags, null
+ *     parts or a null ctx) and nothing changed.
+ *   - Deltas are handled as by the single call: a rejected delta still touches its run and the others are applied; every part
+ *     still ticks, and the call returns BF_EINVAL with *bad_part = the first part that had a rejected delta.
+ *   - Any other failure (BF_ECUDA, BF_ENOMEM) returns with *bad_part = the part it was met in.  Parts may then have ticked, in
+ *     part or not at all: the next touched tick of every part is full, and the caller resends every part's deltas (a delta
+ *     writes a code, so one applied twice changes nothing).
+ *   - The parts whose ticks are not full run together: one scatter launch over all their deltas, one list build over all their
+ *     touch marks, one pass per part back to back, one compaction over all their lists, one synchronisation.  Pinned buffers
+ *     are written in place; pageable ones are copied back once their lengths are known.  A part whose tick is full (see above)
+ *     runs as its single call does, with a synchronisation of its own.
+ * n_parts == 0 is a no-op; *bad_part = BF_COMMIT_NONE on success (bad_part may be NULL).                                      */
+typedef struct bf_tick_part {
+  uint32_t struct_size;          /* sizeof(bf_tick_part)                                                                 */
+  uint32_t handle;               /* resident batch of this ctx                                                           */
+  const bf_delta* deltas;        /* as bf_resident_tick_touched                                                          */
+  uint32_t n_deltas;
+  uint32_t n_runs;
+  bf_touched_out* out;           /* as bf_resident_tick_touched (full, runs, head, events)                               */
+  bf_counts* counts;             /* may be NULL                                                                          */
+} bf_tick_part;
+
+int bf_resident_tick_touched_many(bf_ctx* ctx, uint32_t flags, uint32_t max_iterations, bf_tick_part* parts, uint32_t n_parts,
+                                  uint32_t* bad_part);
+
 /* ------------------------------------------------------------------ migrations (a Story edited while its runs are live)
  * The reference does not pin a StoryRun to the Story generation it started with: every reconcile loads the current Story
  * (getStoryForRun, storyrun_controller.go:1297-1313) and walks allStorySteps of that spec, with StepStates, Gates and
