@@ -215,6 +215,13 @@ class CommitJournal(C.Structure):
                 ("n_items", C.c_uint64), ("runs", C.c_void_p), ("runs_cap", C.c_uint32), ("n_runs_listed", C.c_uint32)]
 
 
+COMMIT_SCOPE_REWRITES = 0x1   # BF_COMMIT_SCOPE_REWRITES: bf_commit_scope.flags of a touched commit matching bf_resident_commit_rewrites
+
+
+class CommitScope(C.Structure):
+    _fields_ = [(n, C.c_uint32) for n in ("struct_size", "flags", "full", "n_considered")]
+
+
 OUTCOME_NONE, OUTCOME_SUCCEEDED, OUTCOME_DEPENDENCY_FAILED, OUTCOME_COMPENSATED = 0, 1, 2, 3   # BF_OUTCOME_*: bf_status_rec.outcome
 OUTCOME_COMPENSATION_FAILED, OUTCOME_CLEANUP_FAILED, OUTCOME_TIMED_OUT = 4, 5, 6
 OUTCOME_CANCELED, OUTCOME_STOPPED, OUTCOME_DEAD = 7, 8, 9
@@ -320,6 +327,10 @@ SYMBOLS = [
                                              C.POINTER(CommitArm), C.POINTER(CommitJournal)]),
     ("bf_resident_commit_rewrites", C.c_int, [C.c_void_p, C.c_uint32, C.c_uint32, C.c_void_p, C.c_uint32, C.POINTER(CommitOut),
                                               C.POINTER(CommitArm), C.POINTER(CommitJournal), C.POINTER(C.c_uint32)]),
+    ("bf_resident_commit_marks", C.c_int, [C.c_void_p, C.c_uint32]),
+    ("bf_resident_commit_touched", C.c_int, [C.c_void_p, C.c_uint32, C.c_uint32, C.c_void_p, C.c_uint32, C.POINTER(CommitOut),
+                                             C.POINTER(CommitArm), C.POINTER(CommitJournal), C.POINTER(C.c_uint32),
+                                             C.POINTER(CommitScope)]),
     ("bf_resident_status", C.c_int, [C.c_void_p, C.c_uint32, C.c_uint32, C.c_void_p, C.c_uint32, C.POINTER(StatusOut)]),
     ("bf_resident_resync", C.c_int, [C.c_void_p, C.c_uint32, C.POINTER(Resync)]),
     ("bf_resident_resync_areas", C.c_int, [C.c_void_p, C.c_uint32, C.POINTER(ResyncAreas)]),

@@ -54,6 +54,13 @@ cudaError_t launch_runctl_restop(const RunCtlRestopParams& P, cudaStream_t strea
 cudaError_t launch_commit(const CommitParams& P, bool apply, cudaStream_t stream);
 cudaError_t launch_status(const StatusParams& P, uint32_t smem_bytes, cudaStream_t stream);
 cudaError_t launch_rewrites(const RewriteParams& P, uint32_t smem_bytes, cudaStream_t stream);
+cudaError_t launch_commit_list(const CommitListParams& L, bool apply, uint32_t max_n, uint32_t ctas, cudaStream_t stream);
+cudaError_t launch_rewrites_list(const RewriteParams& P, const uint32_t* list, const unsigned long long* n_list, uint32_t ctas,
+                                 uint32_t smem_bytes, cudaStream_t stream);
+cudaError_t launch_due_list(const DueListParams& D, cudaStream_t stream);
+cudaError_t launch_due_mark_list(uint32_t* due, const uint32_t* list, const uint32_t* count, uint32_t bound, uint32_t ctas,
+                                 cudaStream_t stream);
+cudaError_t launch_due_mark_sched(uint32_t* due, const uint32_t* run_events, uint32_t n_runs, cudaStream_t stream);
 cudaError_t launch_resync(const ResyncParams& P, uint32_t smem_bytes, cudaStream_t stream);
 cudaError_t launch_resync_areas(const ResyncAreasParams& P, cudaStream_t stream);
 cudaError_t launch_closure(const Slot* slots, const uint32_t* slot_ids, const uint32_t* starts, uint32_t n, uint32_t n_slots,
@@ -182,6 +189,7 @@ struct bf_ctx {
   // step timings of every slot (bf_topology_timings) as one table, slot s at [tim_first[s], tim_first[s + 1]), built and copied
   // to the device by the first arming commit after a change (sync_timings); nothing is allocated until a slot has timings
   bool timings_dirty = false;
+  uint64_t timing_changes = 0;   // timings calls and drops that changed a slot's timings: a touched commit after one that arms is full
   std::vector<uint32_t> tim_first_host;
   std::vector<bf_step_timing> tim_host;
   DevBuf<uint32_t> tim_first_dev;
@@ -296,6 +304,10 @@ inline int end_call(bf_ctx* c, cudaError_t e, const char* what) {
 //   d_runctl           run-control records (bf_resident_runctl), or none.  Put and fire change them (a stop also rewrites the run's
 //                      flags byte, empties its timers and, for a timeout, sets its inputs' run_phase); deltas, uploads and redrives
 //                      honour them.
+//   d_due              commit-due bits (bf_resident_commit_marks), one per run in words of 32, or none.  Touched ticks set the bits
+//                      of the runs they evaluate, bf_resident_schedule those of the runs whose record changed, a touched commit
+//                      clears those of the runs it considered that no entry named.  Bits at or past the capacity stay set.  Only
+//                      ever too many bits cost anything (work, not results), so moves need not re-key them.
 // The calls that move or reset runs carry every area in the launches that handle the records, through view() (resident.cu):
 // retire and transfer move a run's entries with it and reset the ones it leaves, migrate re-keys its timers, redrive empties its
 // timers and lifts its stop, and a run that is moved, migrated or uploaded has no schedule baseline.  Reshape and a retire to a
@@ -308,7 +320,9 @@ struct RunAreas {
   DevBuf<uint8_t> d_sched_rec;
   uint32_t sched_base_runs = 0;
   DevBuf<bf_run_ctl> d_runctl;
+  DevBuf<uint32_t> d_due;
 
+  static size_t due_words(uint32_t capacity) { return ((size_t)capacity + 31) / 32; }
   bf::RunAreasView view(uint32_t words) const {
     return {d_timers, timer_k, d_sched_in, d_sched_rec, BF_SCHED_STRIDE(words), d_runctl};
   }
@@ -328,6 +342,11 @@ struct RunAreas {
     if (resize && timer_k) { e = n.d_timers.alloc((size_t)capacity * timer_k); n.timer_k = timer_k; }
     if (e == cudaSuccess && resize && d_sched_in) { area = "limiter inputs"; e = n.d_sched_in.alloc(capacity); }
     if (e == cudaSuccess && resize && d_runctl) { area = "run control"; e = n.d_runctl.alloc(capacity); }
+    if (e == cudaSuccess && resize && d_due) {   // every bit set: copy_due keeps the old runs' below them
+      area = "commit-due bits";
+      e = n.d_due.alloc(due_words(capacity));
+      if (e == cudaSuccess) e = cudaMemsetAsync(n.d_due, 0xFF, n.d_due.cap * 4, s);
+    }
     if (e == cudaSuccess && relaid && d_sched_in) {
       area = "schedule records";
       e = capacity < cap && words == old_words ? n.d_sched_rec.alloc((size_t)capacity * BF_SCHED_STRIDE(words))
@@ -347,7 +366,7 @@ struct RunAreas {
       e = bf::launch_relay_timers({d_timers, n.d_timers, capacity, cap, timer_k, timer_k}, s);
       launches += 1;
     }
-    return e;
+    return e == cudaSuccess ? copy_due(n, std::min(cap, capacity), s) : e;
   }
   // Retire to a smaller capacity: the first `capacity` runs of every area into n (alloc_resized), device to device.
   cudaError_t copy_prefix(RunAreas& n, uint32_t capacity, uint32_t words, cudaStream_t s) const {
@@ -359,7 +378,13 @@ struct RunAreas {
     if (e == cudaSuccess && d_sched_in) e = copy(n.d_sched_in, d_sched_in, sizeof(bf_sched_run));
     if (e == cudaSuccess && d_sched_in) e = copy(n.d_sched_rec, d_sched_rec, BF_SCHED_STRIDE(words));
     if (e == cudaSuccess && d_runctl) e = copy(n.d_runctl, d_runctl, sizeof(bf_run_ctl));
-    return e;
+    return e == cudaSuccess ? copy_due(n, capacity, s) : e;
+  }
+  // Reshape and retire to a new capacity: n's commit-due bits (alloc_resized, all set) take this set's whole words below `runs`,
+  // the runs both capacities hold; the runs of a partial last word stay due.
+  cudaError_t copy_due(RunAreas& n, uint32_t runs, cudaStream_t s) const {
+    if (!n.d_due || runs < 32) return cudaSuccess;
+    return cudaMemcpyAsync(n.d_due, d_due, (size_t)(runs / 32) * 4, cudaMemcpyDeviceToDevice, s);
   }
   // takes every area n holds in place of this set's
   void adopt(RunAreas&& n) {
@@ -367,6 +392,7 @@ struct RunAreas {
     if (n.d_sched_in) d_sched_in = std::move(n.d_sched_in);
     if (n.d_sched_rec) d_sched_rec = std::move(n.d_sched_rec);
     if (n.d_runctl) d_runctl = std::move(n.d_runctl);
+    if (n.d_due) d_due = std::move(n.d_due);
   }
 };
 
@@ -394,7 +420,12 @@ struct RunAreas {
 //   (transfer)         the source compacts as by retire (compact_to); the destination takes the arrivals as uploads (received).
 //   uploaded           merged [first, end) ranges, keyed by first, of the runs at or above full_runs uploaded since the last full
 //                      tick (note_uploaded); compact_to clips them; full_tick_done clears them.
-//   areas              the per-run side areas (RunAreas): step timers, limiter inputs and schedule records, run control.
+//   areas              the per-run side areas (RunAreas): step timers, limiter inputs and schedule records, run control, commit-due
+//                      bits.
+//   commit_all,        with the commit-due bits: the next touched commit considers every run of [0, n_runs) (and sets the bits
+//   commit_form,       at or past n_runs).  Set by enabling the bits, a full tick (resident_tick_locked), a failed tick or commit;
+//   commit_timings     a touched commit is full also when its form (arm, journal, rewrites: commit_form) or, arming, the ctx's
+//                      timing_changes (commit_timings) differ from the last touched commit's.  A touched commit clears it.
 //   ticked             runs covered by a tick since the last call that changed d_state (state_changed), or -1: none since.  A
 //                      resident schedule over n runs needs ticked >= n.
 //   single_ticked      runs covered by single-pass ticks since the last tick with BF_EVAL_FIXPOINT, or -1.  scheduled: runs covered
@@ -409,6 +440,9 @@ struct Resident {
   DevBuf<uint32_t> d_mark;
   RunAreas areas;
   int64_t ticked = -1, single_ticked = -1, scheduled = -1;
+  bool commit_all = true;
+  uint32_t commit_form = ~0u;
+  uint64_t commit_timings = 0;
   uint64_t slot_changes_seen = 0, pending = 0;
   std::map<uint32_t, uint32_t> uploaded;
 

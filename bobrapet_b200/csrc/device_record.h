@@ -510,6 +510,31 @@ struct CommitParams {
 static_assert(sizeof(bf_commit_write) == 16, "bf_commit_write must be 16 bytes");
 constexpr uint32_t kJournalArmsShift = 1, kJournalItemsShift = 8;   // new arms <= BF_TIMER_MAX_SLOTS < 128
 
+// bf_resident_commit_touched (resident.cu): the list-mode builds of the commit launches.  Warp i of the list takes run list[i]
+// (list == nullptr: run i), i below *n_list; the launch's CTAs walk blocks of 8 list positions, so the journal's words and CTA
+// totals are those of list positions, ceil(*n_list / 8) blocks of them.  The apply clears the commit-due bit of each run it
+// takes that no entry names and sets the bit of one that an entry names.  A separate parameter block, so the full-form builds
+// keep theirs.
+struct CommitListParams {
+  CommitParams P;
+  const uint32_t* list;                 // [*n_list] ascending runs, or nullptr: [0, *n_list)
+  const unsigned long long* n_list;     // [1] the list length (the list build's scan, or uploaded)
+  uint32_t* due;                        // [ceil(capacity / 32)] the batch's commit-due bits (apply)
+};
+// The run list of a touched commit (launch_listing over groups of 32 due words, one warp per group and lane w on word w): the
+// due bits of [0, n_runs) and the runs the entries name.  due_count stores each group's runs (group_runs) and each CTA's total,
+// cta_scan<1> turns those into the runs of the CTAs before each and posts the list length (total), due_list writes the runs.
+struct DueListParams {
+  const uint32_t* due;
+  const bf_commit_entry* entries;       // [n_entries], ascending by (run, step)
+  uint32_t n_entries, n_runs;
+  uint32_t n, warps_per_block;          // groups (launch_listing's runs) and 8
+  uint32_t* group_runs;                 // [n]
+  unsigned long long* cta;              // [CTAs]
+  unsigned long long* total;            // [1] out: the list length
+  uint32_t* list;                       // [n_runs] out
+};
+
 // bf_resident_commit_rewrites (resident.cu): rewrite_runs, one warp per run of [0, n_runs) and the shared stage of StatusParams,
 // takes a run through the stages of a single pass when its current result record carries BF_SUM_PHASE_CHANGED, it is not stopped
 // and its slot is live and fits the layout; a run whose codes the stages changed is flagged in rw_runs and its planes stored in

@@ -112,8 +112,10 @@ cudaError_t launch_cta_scan(unsigned long long* cta, unsigned long long* total, 
 
 // Count (every thread of the CTA): lane 0 of each warp passes its word (0 for a warp without a run); thread 0 stores total k of
 // the CTA's words at cta[k * gridDim.x + blockIdx.x].  Its 32 bytes of static shared memory are kStatusStaticSmem.
+// The _at forms take the block and the number of blocks in place of the CTA's own: a launch whose CTAs walk several blocks of
+// runs (the touched commit's list-mode builds) stores and reads one total per block.
 template <uint32_t K, class Part>
-DI void store_cta_totals(uint32_t word, unsigned long long* cta, Part part) {
+DI void store_cta_totals_at(uint32_t word, unsigned long long* cta, Part part, uint32_t block, uint32_t n_blocks) {
   __shared__ uint32_t warp_word[8];
   if ((threadIdx.x & 31u) == 0) warp_word[threadIdx.x >> 5] = word;
   __syncthreads();
@@ -121,18 +123,27 @@ DI void store_cta_totals(uint32_t word, unsigned long long* cta, Part part) {
   for (uint32_t k = 0; k < K; ++k) {
     unsigned long long sum = 0;
     for (uint32_t w = 0; w < (blockDim.x >> 5); ++w) sum += part(warp_word[w], k);
-    cta[k * gridDim.x + blockIdx.x] = sum;
+    cta[k * n_blocks + block] = sum;
   }
+}
+template <uint32_t K, class Part>
+DI void store_cta_totals(uint32_t word, unsigned long long* cta, Part part) {
+  store_cta_totals_at<K>(word, cta, part, blockIdx.x, gridDim.x);
 }
 
 // List (whole warp): the offsets of the run whose word is run_words[i], the CTA's runs starting at run_words[first]: the totals of
 // the CTAs before (after cta_scan) and of the warps before it in its CTA.
 template <uint32_t K, class Part>
-DI void run_offsets(const unsigned long long* cta, const uint32_t* run_words, uint32_t first, uint32_t i, Part part,
-                    unsigned long long (&base)[K]) {
+DI void run_offsets_at(const unsigned long long* cta, const uint32_t* run_words, uint32_t first, uint32_t i, Part part,
+                       unsigned long long (&base)[K], uint32_t block, uint32_t n_blocks) {
   const uint32_t lane = threadIdx.x & 31u;
   const uint32_t before = first + lane < i ? run_words[first + lane] : 0u;
-  for (uint32_t k = 0; k < K; ++k) base[k] = cta[k * gridDim.x + blockIdx.x] + redux_add(part(before, k));
+  for (uint32_t k = 0; k < K; ++k) base[k] = cta[k * n_blocks + block] + redux_add(part(before, k));
+}
+template <uint32_t K, class Part>
+DI void run_offsets(const unsigned long long* cta, const uint32_t* run_words, uint32_t first, uint32_t i, Part part,
+                    unsigned long long (&base)[K]) {
+  run_offsets_at<K>(cta, run_words, first, i, part, base, blockIdx.x, gridDim.x);
 }
 
 // Emit (whole warp): one item per set bit of this lane's `bits`, lane by lane and bit by bit (step order when lane w holds word

@@ -941,7 +941,7 @@ cudaError_t launch_fire(const FireParams& P, cudaStream_t stream) {
 // bf_resident_schedule its listed runs and events, bf_resident_resync its items and drifted runs, bf_resident_commit_journal its
 // items and written runs (K = 2).
 template <uint32_t K>
-__global__ void __launch_bounds__(1024) cta_scan(unsigned long long* cta, unsigned long long* total, uint32_t n_ctas) {
+DI void cta_scan_body(unsigned long long* cta, unsigned long long* total, uint32_t n_ctas) {
   __shared__ unsigned long long s_e[K][32];
   const uint32_t lane = threadIdx.x & 31u, warp = threadIdx.x >> 5;
   unsigned long long carry[K] = {};
@@ -979,6 +979,15 @@ __global__ void __launch_bounds__(1024) cta_scan(unsigned long long* cta, unsign
   if (threadIdx.x == 0)
     for (uint32_t k = 0; k < K; ++k) total[k] = carry[k];
 }
+template <uint32_t K>
+__global__ void __launch_bounds__(1024) cta_scan(unsigned long long* cta, unsigned long long* total, uint32_t n_ctas) {
+  cta_scan_body<K>(cta, total, n_ctas);
+}
+// The journal scan of a touched commit: one total per block of 8 list positions, ceil(*n_list / 8) of them
+template <uint32_t K>
+__global__ void __launch_bounds__(1024) cta_scan_list(unsigned long long* cta, unsigned long long* total, const unsigned long long* n_list) {
+  cta_scan_body<K>(cta, total, (uint32_t)((*n_list + 7u) / 8u));
+}
 
 cudaError_t launch_cta_scan(unsigned long long* cta, unsigned long long* total, uint32_t n_ctas, uint32_t K, cudaStream_t stream) {
   if (K == 1) cta_scan<1><<<1, 1024, 0, stream>>>(cta, total, n_ctas);
@@ -987,8 +996,8 @@ cudaError_t launch_cta_scan(unsigned long long* cta, unsigned long long* total, 
 }
 
 // Past 48 KiB of dynamic shared memory a kernel opts in before its launch.
-template <class Params>
-static cudaError_t allow_smem(void (*kernel)(Params), uint32_t smem_bytes) {
+template <class... Params>
+static cudaError_t allow_smem(void (*kernel)(Params...), uint32_t smem_bytes) {
   return smem_bytes > 48u * 1024u ? cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes)
                                   : cudaSuccess;
 }
@@ -1219,6 +1228,10 @@ DI void commit_registered(uint32_t lane, const CommitRun& c, const uint8_t* rec,
   w.newly = ((unsigned long long)set[1] << 32 | set[0]) & ~w.reg;
 }
 
+// a word's share of each total when the word is the total (one array of CTA totals)
+struct WordPart {
+  DI uint32_t operator()(uint32_t w, uint32_t) const { return w; }
+};
 // a run's journal word's share of the items (k = 0) and of the written runs (k = 1)
 struct JournalPart {
   DI uint32_t operator()(uint32_t w, uint32_t k) const { return k ? w & 1u : w >> kJournalItemsShift; }
@@ -1261,16 +1274,22 @@ DI uint32_t check_run(const CommitParams& P, uint32_t r, uint32_t lane) {
 // entry has a HOLD or PHASE entry; with a timing table, the arming offences too.  Lane 0 lowers P.offender to the run's first
 // offence.  Nothing is written but, with kJournal, each run's journal word and each CTA's items and written runs.  The kernels
 // commit_check (kRewrite = false) and commit_check_rewrites (both true) are this body.
+// commit_check_at: warp position i (its journal word and block total) takes run r when `has`.
 template <bool kJournal, bool kRewrite>
-DI void commit_check_body(const CommitParams& P) {
-  const uint32_t r = blockIdx.x * 8u + (threadIdx.x >> 5), lane = threadIdx.x & 31u;
+DI void commit_check_at(const CommitParams& P, uint32_t i, uint32_t r, bool has, uint32_t block, uint32_t n_blocks) {
+  const uint32_t lane = threadIdx.x & 31u;
   if (!kJournal) {
-    if (r < P.n_runs) check_run<false, kRewrite>(P, r, lane);
+    if (has) check_run<false, kRewrite>(P, r, lane);
     return;
   }
-  const uint32_t jw = r < P.n_runs ? check_run<true, kRewrite>(P, r, lane) : 0u;
-  if (lane == 0 && r < P.n_runs) P.run_items[r] = jw;
-  store_cta_totals<2>(jw, P.cta, JournalPart{});
+  const uint32_t jw = has ? check_run<true, kRewrite>(P, r, lane) : 0u;
+  if (lane == 0 && has) P.run_items[i] = jw;
+  store_cta_totals_at<2>(jw, P.cta, JournalPart{}, block, n_blocks);
+}
+template <bool kJournal, bool kRewrite>
+DI void commit_check_body(const CommitParams& P) {
+  const uint32_t r = blockIdx.x * 8u + (threadIdx.x >> 5);
+  commit_check_at<kJournal, kRewrite>(P, r, r, r < P.n_runs, blockIdx.x, gridDim.x);
 }
 template <bool kJournal>
 __global__ void __launch_bounds__(256) commit_check(const CommitParams P) { commit_check_body<kJournal, false>(P); }
@@ -1282,10 +1301,10 @@ __global__ void __launch_bounds__(256) commit_check_rewrites(const CommitParams 
 // and the warps before in its CTA, and its entry in runs when its record changed.  With kRewrite a PHASE item of a step without
 // a mask bit (its code comes from the stages) carries BF_COMMIT_WRITE_REWRITE, and those steps are added to *P.rewritten.  The
 // kernels commit_apply (kRewrite = false) and commit_apply_rewrites (both true) are this body.
+// commit_apply_at: warp position i (its journal word, in block `block` of n_blocks) takes run r.
 template <bool kJournal, bool kRewrite>
-DI void commit_apply_body(const CommitParams& P) {
-  const uint32_t r = blockIdx.x * 8u + (threadIdx.x >> 5), lane = threadIdx.x & 31u;
-  if (r >= P.n_runs) return;
+DI void commit_apply_at(const CommitParams& P, uint32_t i, uint32_t r, uint32_t block, uint32_t n_blocks) {
+  const uint32_t lane = threadIdx.x & 31u;
   CommitRun c;
   if (!commit_run<kRewrite>(P, r, lane, c)) return;
   uint32_t hold, phased;
@@ -1295,9 +1314,9 @@ DI void commit_apply_body(const CommitParams& P) {
   uint8_t* rec = P.state + (size_t)r * P.state_stride;
   uint32_t jw = 0, armed;
   unsigned long long pos = 0;
-  if (kJournal && (jw = P.run_items[r]) != 0u) {
+  if (kJournal && (jw = P.run_items[i]) != 0u) {
     unsigned long long base[2];
-    run_offsets<2>(P.cta, P.run_items, blockIdx.x * 8u, r, JournalPart{}, base);
+    run_offsets_at<2>(P.cta, P.run_items, block * 8u, i, JournalPart{}, base, block, n_blocks);
     pos = base[0];
     if (lane == 0 && (jw & 1u) && base[1] < P.runs_cap) P.runs[base[1]] = r;
   }
@@ -1350,6 +1369,12 @@ DI void commit_apply_body(const CommitParams& P) {
     if (lane == 0 && n_rw) atomicAdd(P.rewritten, n_rw);
   }
 }
+template <bool kJournal, bool kRewrite>
+DI void commit_apply_body(const CommitParams& P) {
+  const uint32_t r = blockIdx.x * 8u + (threadIdx.x >> 5);
+  if (r >= P.n_runs) return;
+  commit_apply_at<kJournal, kRewrite>(P, r, r, blockIdx.x, gridDim.x);
+}
 template <bool kJournal>
 __global__ void __launch_bounds__(256) commit_apply(const CommitParams P) { commit_apply_body<kJournal, false>(P); }
 __global__ void __launch_bounds__(256) commit_apply_rewrites(const CommitParams P) { commit_apply_body<true, true>(P); }
@@ -1370,6 +1395,119 @@ cudaError_t launch_commit(const CommitParams& P, bool apply, cudaStream_t stream
     else commit_check<true><<<grid, 256, 0, stream>>>(P);
     return launch_cta_scan(P.cta, P.total, grid, 2, stream);
   }
+  return cudaGetLastError();
+}
+
+// ---- touched commits (bf_resident_commit_touched) ------------------------------------------------------------------------------
+// The list-mode builds of both launches (CommitListParams): each CTA walks blocks b = blockIdx.x, + gridDim.x, ... of 8 list
+// positions while 8 b < *n_list; warp w of block b takes position 8 b + w, and runs the full form's per-run body on run list[i]
+// with the journal's words and block totals indexed by position.  The list ascends, so items and runs come out ordered by run
+// as in the full form.
+DI uint32_t list_run(const CommitListParams& L, uint32_t i) { return L.list ? L.list[i] : i; }
+template <bool kJournal, bool kRewrite>
+__global__ void __launch_bounds__(256) commit_check_list(const CommitListParams L) {
+  const uint32_t n = (uint32_t)*L.n_list, n_blocks = (n + 7u) / 8u;
+  for (uint32_t b = blockIdx.x; b < n_blocks; b += gridDim.x) {   // CTA-uniform
+    const uint32_t i = b * 8u + (threadIdx.x >> 5);
+    commit_check_at<kJournal, kRewrite>(L.P, i, i < n ? list_run(L, i) : 0u, i < n, b, n_blocks);
+    if (kJournal) __syncthreads();   // the block's warp words are read before the next block stores its own
+  }
+}
+// The apply also keeps the commit-due bits of the runs it takes: a run an entry names stays due (the next commit checks it
+// again), every other one is cleared.
+template <bool kJournal, bool kRewrite>
+__global__ void __launch_bounds__(256) commit_apply_list(const CommitListParams L) {
+  const uint32_t n = (uint32_t)*L.n_list, n_blocks = (n + 7u) / 8u, lane = threadIdx.x & 31u;
+  for (uint32_t b = blockIdx.x; b < n_blocks; b += gridDim.x) {
+    const uint32_t i = b * 8u + (threadIdx.x >> 5);
+    if (i >= n) break;
+    const uint32_t r = list_run(L, i);
+    if (lane == 0) {
+      uint32_t a = 0u, e = L.P.n_entries;
+      while (a < e) { const uint32_t m = (a + e) >> 1; if (L.P.entries[m].run < r) a = m + 1u; else e = m; }
+      const uint32_t bit = 1u << (r & 31u);
+      if (a < L.P.n_entries && L.P.entries[a].run == r) atomicOr(L.due + (r >> 5), bit);
+      else atomicAnd(L.due + (r >> 5), ~bit);
+    }
+    commit_apply_at<kJournal, kRewrite>(L.P, i, r, b, n_blocks);
+  }
+}
+
+// The check (and with a journal its scan), or the apply, of a touched commit over at most max_n list positions, `ctas` CTAs
+cudaError_t launch_commit_list(const CommitListParams& L, bool apply, uint32_t max_n, uint32_t ctas, cudaStream_t stream) {
+  if (max_n == 0) return cudaSuccess;
+  const uint32_t grid = std::min((max_n - 1u) / 8u + 1u, std::max(ctas, 1u));
+  if (!L.P.run_items) {
+    if (apply) commit_apply_list<false, false><<<grid, 256, 0, stream>>>(L);
+    else commit_check_list<false, false><<<grid, 256, 0, stream>>>(L);
+  } else if (apply) {
+    if (L.P.rw_runs) commit_apply_list<true, true><<<grid, 256, 0, stream>>>(L);
+    else commit_apply_list<true, false><<<grid, 256, 0, stream>>>(L);
+  } else {
+    if (L.P.rw_runs) commit_check_list<true, true><<<grid, 256, 0, stream>>>(L);
+    else commit_check_list<true, false><<<grid, 256, 0, stream>>>(L);
+    cta_scan_list<2><<<1, 1024, 0, stream>>>(L.P.cta, L.P.total, L.n_list);
+  }
+  return cudaGetLastError();
+}
+
+// The due word w of a touched commit's list: its commit-due bits and the runs entries name, below n_runs
+DI uint32_t due_word(const DueListParams& D, uint32_t w) {
+  const uint32_t first = w * 32u;
+  if (first >= D.n_runs) return 0u;
+  uint32_t bits = D.due[w];
+  uint32_t a = 0u, e = D.n_entries;
+  while (a < e) { const uint32_t m = (a + e) >> 1; if (D.entries[m].run < first) a = m + 1u; else e = m; }
+  for (; a < D.n_entries && D.entries[a].run < first + 32u; ++a) bits |= 1u << (D.entries[a].run & 31u);
+  const uint32_t left = D.n_runs - first;
+  return left < 32u ? bits & ((1u << left) - 1u) : bits;
+}
+// Count: group g (warp) takes due words 32 g + lane; its runs, and each CTA's total.  List (after cta_scan<1>): the same groups
+// again, each writing its runs from its offset, lane by lane and bit by bit (ascending).
+template <bool kList>
+__global__ void __launch_bounds__(256) due_runs(const DueListParams D) {
+  const uint32_t g = blockIdx.x * 8u + (threadIdx.x >> 5), lane = threadIdx.x & 31u;
+  const uint32_t w = g * 32u + lane, bits = g < D.n ? due_word(D, w) : 0u;
+  if (!kList) {
+    const uint32_t k = redux_add((uint32_t)__popc(bits));
+    if (lane == 0 && g < D.n) D.group_runs[g] = k;
+    store_cta_totals<1>(k, D.cta, WordPart{});
+    return;
+  }
+  if (g >= D.n) return;
+  unsigned long long base[1];
+  run_offsets<1>(D.cta, D.group_runs, blockIdx.x * 8u, g, WordPart{}, base);
+  emit_bits(bits, base[0], D.n_runs, [&](uint32_t b, unsigned long long at) { D.list[at] = w * 32u + b; });
+}
+cudaError_t launch_due_list(const DueListParams& D, cudaStream_t stream) {
+  return launch_listing<1>(due_runs<false>, due_runs<true>, D, 0u, stream);
+}
+
+// The touched tick's evaluated runs (list[0, min(*count, bound))) become commit-due; a grid-stride loop of `ctas` CTAs
+__global__ void __launch_bounds__(256) due_mark_list(uint32_t* due, const uint32_t* list, const uint32_t* count, uint32_t bound) {
+  const uint32_t n = min(*count, bound);
+  for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+    const uint32_t r = list[i];
+    atomicOr(due + (r >> 5), 1u << (r & 31u));
+  }
+}
+cudaError_t launch_due_mark_list(uint32_t* due, const uint32_t* list, const uint32_t* count, uint32_t bound, uint32_t ctas,
+                                 cudaStream_t stream) {
+  if (bound == 0) return cudaSuccess;
+  due_mark_list<<<std::min((bound - 1u) / 256u + 1u, std::max(ctas, 1u)), 256, 0, stream>>>(due, list, count, bound);
+  return cudaGetLastError();
+}
+
+// The runs whose schedule record bf_resident_schedule changed (listed: run_events[r] != kSchedUnlisted) become commit-due; one
+// thread per run, one word per warp
+__global__ void __launch_bounds__(256) due_mark_sched(uint32_t* due, const uint32_t* run_events, uint32_t n_runs) {
+  const uint32_t r = blockIdx.x * blockDim.x + threadIdx.x;
+  const uint32_t m = __ballot_sync(FULL, r < n_runs && run_events[r] != kSchedUnlisted);
+  if ((threadIdx.x & 31u) == 0 && m) atomicOr(due + (r >> 5), m);
+}
+cudaError_t launch_due_mark_sched(uint32_t* due, const uint32_t* run_events, uint32_t n_runs, cudaStream_t stream) {
+  if (n_runs == 0) return cudaSuccess;
+  due_mark_sched<<<(n_runs - 1u) / 256u + 1u, 256, 0, stream>>>(due, run_events, n_runs);
   return cudaGetLastError();
 }
 
@@ -1508,10 +1646,6 @@ DI void run_status(const StatusParams& P, uint32_t i, uint32_t lane, uint32_t st
 // Count (kList = false): each listed run's events, and each CTA's total.  List (kList = true, after cta_scan): the same runs
 // again, each record with the offset of its first event (the CTAs before, then the warps before in its CTA) and its events, lane by
 // lane in step order.
-// a word's share of each total when the word is the total (one array of CTA totals)
-struct WordPart {
-  DI uint32_t operator()(uint32_t w, uint32_t) const { return w; }
-};
 
 template <bool kList>
 __global__ void __launch_bounds__(256, 1) status_runs(const StatusParams P) {
@@ -1556,12 +1690,8 @@ cudaError_t launch_status(const StatusParams& P, uint32_t smem_bytes, cudaStream
 // its current result record, which the pass that left it derived from the same codes) can have a rewrite; a stopped run, a dead
 // slot and a slot wider than the layout have none.  Such a run takes single_pass (stages H, G and I, no stage-D cond FAIL), and is
 // flagged with its planes stored when a code (15 read as 0) changed.
-__global__ void __launch_bounds__(256, 1) rewrite_runs(const RewriteParams P) {
-  extern __shared__ __align__(16) uint8_t rewrite_stage[];
-  const uint32_t warp = threadIdx.x >> 5, lane = threadIdx.x & 31u;
-  const uint32_t r = blockIdx.x * P.warps_per_block + warp;
-  if (r >= P.n_runs) return;
-  const uint32_t stage_a = smem_u32(rewrite_stage) + warp * pass_stage_bytes(P.off_child, P.state_stride, P.topo_bytes);
+DI void rewrite_run(const RewriteParams& P, uint32_t r, uint32_t stage_a) {
+  const uint32_t lane = threadIdx.x & 31u;
   const uint8_t* rec = P.state + (size_t)r * P.state_stride;
   const uint32_t summary = *reinterpret_cast<const uint32_t*>(P.result + (size_t)r * P.result_stride);
   const uint32_t slot = *reinterpret_cast<const uint32_t*>(rec);
@@ -1587,12 +1717,36 @@ __global__ void __launch_bounds__(256, 1) rewrite_runs(const RewriteParams P) {
   }
   if (lane == 0) P.rw_runs[r] = changed;
 }
+__global__ void __launch_bounds__(256, 1) rewrite_runs(const RewriteParams P) {
+  extern __shared__ __align__(16) uint8_t rewrite_stage[];
+  const uint32_t warp = threadIdx.x >> 5;
+  const uint32_t r = blockIdx.x * P.warps_per_block + warp;
+  if (r >= P.n_runs) return;
+  rewrite_run(P, r, smem_u32(rewrite_stage) + warp * pass_stage_bytes(P.off_child, P.state_stride, P.topo_bytes));
+}
+// The list-mode build (bf_resident_commit_touched): the warps walk the list positions below *n_list, `ctas` CTAs of them, and
+// take run list[i] (list == nullptr: run i); rw_runs and rw_planes stay indexed by run.
+__global__ void __launch_bounds__(256, 1) rewrite_runs_list(const RewriteParams P, const uint32_t* list, const unsigned long long* n_list) {
+  extern __shared__ __align__(16) uint8_t rewrite_stage[];
+  const uint32_t warp = threadIdx.x >> 5, n = (uint32_t)*n_list;
+  const uint32_t stage_a = smem_u32(rewrite_stage) + warp * pass_stage_bytes(P.off_child, P.state_stride, P.topo_bytes);
+  for (uint32_t i = blockIdx.x * P.warps_per_block + warp; i < n; i += gridDim.x * P.warps_per_block)   // warp-uniform
+    rewrite_run(P, list ? list[i] : i, stage_a);
+}
 
 cudaError_t launch_rewrites(const RewriteParams& P, uint32_t smem_bytes, cudaStream_t stream) {
   if (P.n_runs == 0) return cudaSuccess;
   if (const cudaError_t e = allow_smem(rewrite_runs, smem_bytes)) return e;
   const uint32_t grid = (P.n_runs - 1u) / P.warps_per_block + 1u;
   rewrite_runs<<<grid, 32u * P.warps_per_block, smem_bytes, stream>>>(P);
+  return cudaGetLastError();
+}
+cudaError_t launch_rewrites_list(const RewriteParams& P, const uint32_t* list, const unsigned long long* n_list, uint32_t ctas,
+                                 uint32_t smem_bytes, cudaStream_t stream) {
+  if (P.n_runs == 0) return cudaSuccess;
+  if (const cudaError_t e = allow_smem(rewrite_runs_list, smem_bytes)) return e;
+  const uint32_t grid = std::min((P.n_runs - 1u) / P.warps_per_block + 1u, std::max(ctas, 1u));
+  rewrite_runs_list<<<grid, 32u * P.warps_per_block, smem_bytes, stream>>>(P, list, n_list);
   return cudaGetLastError();
 }
 

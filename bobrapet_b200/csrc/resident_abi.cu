@@ -296,6 +296,7 @@ int bf_resident_apply(bf_ctx* c, uint32_t h, const bf_delta* deltas, uint32_t n)
 static int resident_tick_locked(bf_ctx* c, Resident* r, const bf_delta* deltas, uint32_t n_deltas, uint32_t n_runs, uint32_t flags,
                                 uint32_t max_iterations, void* result, bf_counts* counts, bf_compact_out* co = nullptr) {
   c->snap.valid = false;
+  r->commit_all = true;   // a full tick may change any run's result: the next touched commit considers every run
   if (n_deltas) r->ticked = -1;
   if (co && co->struct_size != sizeof(bf_compact_out)) return fail(c, BF_EINVAL, "bad bf_compact_out.struct_size");
   if (co && co->events_cap && !co->events) return fail(c, BF_EINVAL, "null events with a non-zero events_cap");
@@ -459,6 +460,16 @@ static void touched_end(bf_ctx* c, const TouchedTick& t, uint32_t flags, const b
   t.out->full = 0; t.out->n_listed = (uint32_t)tail.listed; t.out->n_evaluated = (uint32_t)tail.evaluated; t.out->n_events = tail.events;
 }
 
+// With commit-due bits (bf_resident_commit_marks), the runs a touched tick evaluates become due: one launch over its list, behind
+// the list build
+static int mark_commit_due(bf_ctx* c, const TouchedTick& t) {
+  uint32_t* due = t.r->areas.d_due;
+  if (!due) return BF_OK;
+  BF_CUDA(c, bf::launch_due_mark_list(due, t.T.list, t.T.list_count, t.bound, (uint32_t)c->sm_count * 4u, c->stream));
+  c->stats.kernel_launches += 1;
+  return BF_OK;
+}
+
 // A touched tick: scatter -> list build -> pass over the list -> list-mode compaction, which brings the current result records up
 // to date; or a full compact tick where the baseline rules require one.
 static int touched_tick_locked(bf_ctx* c, Resident* r, const bf_delta* deltas, uint32_t n_deltas, uint32_t n_runs, uint32_t flags,
@@ -490,6 +501,7 @@ static int touched_tick_locked(bf_ctx* c, Resident* r, const bf_delta* deltas, u
     }
     c->rejected_clean = false;   // the emit kernel delivers and clears the counter; a failed call leaves it to be zeroed
     BF_CUDA(c, bf::launch_touched_list(t.T, s));
+    if (int rc = mark_commit_due(c, t)) return rc;
     if (int rc = touched_pass(c, t, flags, max_iterations, c->d_counts)) return rc;
     BF_CUDA(c, bf::launch_touched_compact(t.T, s));
     c->stats.kernel_launches += 4;
@@ -502,7 +514,7 @@ static int touched_tick_locked(bf_ctx* c, Resident* r, const bf_delta* deltas, u
   const int rc = body();
   const cudaError_t es = cudaStreamSynchronize(s);
   if (rc != BF_OK || es != cudaSuccess) {   // marks and current records may be half updated: the next touched tick is a full one
-    r->need_full = true; c->rejected_clean = false;
+    r->need_full = true; r->commit_all = true; c->rejected_clean = false;
     if (rc != BF_OK) return rc;
     return cuda_fail(c, es, "cudaStreamSynchronize");
   }
@@ -562,7 +574,7 @@ int bf_resident_tick_touched_many(bf_ctx* c, uint32_t flags, uint32_t max_iterat
   BF_CUDA(c, cudaSetDevice(c->device));
   // after a failure the records and marks of any part may be half updated: every part's next touched tick is full
   auto failed = [&](uint32_t k, int rc) {
-    for (Resident* r : rs) r->need_full = true;
+    for (Resident* r : rs) { r->need_full = true; r->commit_all = true; }
     return name(k, rc);
   };
   uint32_t first_rejected = BF_COMMIT_NONE;
@@ -668,6 +680,8 @@ int bf_resident_tick_touched_many(bf_ctx* c, uint32_t flags, uint32_t max_iterat
       if (m) {
         const auto* dtp = reinterpret_cast<const bf::TouchedParams*>(d + o_tp);
         BF_CUDA(c, bf::launch_touched_list_many(dtp, reinterpret_cast<uint32_t*>(d + o_lf), m, lb, s));
+        for (uint32_t j = 0; j < m; ++j)
+          if (int rc = mark_commit_due(c, ticks[listed[j]])) return rc;
         for (uint32_t j = 0; j < m; ++j)
           if (int rc = touched_pass(c, ticks[listed[j]], flags, max_iterations, cnt + 4 * (size_t)listed[j])) return rc;
         BF_CUDA(c, bf::launch_touched_compact_many(dtp, reinterpret_cast<uint32_t*>(d + o_cf), m, cb, s));
@@ -1427,6 +1441,10 @@ int bf_resident_schedule(bf_ctx* c, const bf_sched_tables* t, uint32_t now, bf_r
       if (parts[i].n_runs) {
         e = bf::launch_resident_schedule(R, s);
         launches += 3;
+        if (e == cudaSuccess && rs[i]->areas.d_due) {   // the runs whose record changed become commit-due
+          e = bf::launch_due_mark_sched(rs[i]->areas.d_due, R.run_events, parts[i].n_runs, s);
+          launches += 1;
+        }
         if (e == cudaSuccess) e = cudaMemcpyAsync(&part_tot[2 * i], R.totals, 16, cudaMemcpyDeviceToHost, s);
       }
     }
@@ -1443,7 +1461,7 @@ int bf_resident_schedule(bf_ctx* c, const bf_sched_tables* t, uint32_t now, bf_r
   const cudaError_t e = body();
   c->stats.kernel_launches += launches;
   if (int rc = bf::end_call(c, e, "bf_resident_schedule")) {   // the schedule records may be half written: no baseline survives
-    for (Resident* r : rs) r->areas.sched_base_runs = 0;
+    for (Resident* r : rs) { r->areas.sched_base_runs = 0; r->commit_all = true; }
     return rc;
   }
   for (uint32_t i = 0; i < n_parts; ++i) {
@@ -1525,12 +1543,20 @@ int bf_resident_runctl_download(bf_ctx* c, uint32_t h, uint32_t first, uint32_t 
 // the counts copied back carry the arms' two words.  With `journal` the check launch also counts each run's items and a scan
 // launch follows it; the totals come back with the offender, so staged items and runs are copied before the second
 // synchronisation.  With `rewritten` (bf_resident_commit_rewrites, journaled) rewrite_runs runs before the check launch: the
-// staged planes are taken with the call's other sections, so the apply after a growth still finds them.  bf_resident_commit,
-// _timed, _journal and _rewrites are this one call.
+// staged planes are taken with the call's other sections, so the apply after a growth still finds them.  With `scope`
+// (bf_resident_commit_touched) the same checks and staging feed the list-mode builds of the launches: over the list of due runs
+// that the count, scan and list launches build in front of them, or, when the call is full, over [0, n_runs) with every due bit
+// set first.  bf_resident_commit, _timed, _journal, _rewrites and _touched are this one call.
 static int resident_commit(bf_ctx* c, uint32_t h, uint32_t n_runs, const bf_commit_entry* entries, uint32_t n, bf_commit_out* out,
                            bf_commit_arm* arm, bf_commit_journal* journal, bool journaled, uint32_t* rewritten = nullptr,
-                           bool rewrites = false) {
+                           bool rewrites = false, bf_commit_scope* scope = nullptr) {
   auto [g, r] = lock_resident(c, h);
+  if (scope) {   // bf_resident_commit_touched: the form is picked by arm, journal and the scope's flags
+    if (scope->struct_size != sizeof(bf_commit_scope)) return fail(c, BF_EINVAL, "bad bf_commit_scope.struct_size");
+    scope->full = scope->n_considered = 0;
+    if (scope->flags & ~BF_COMMIT_SCOPE_REWRITES) return fail(c, BF_EINVAL, "bf_commit_scope.flags takes BF_COMMIT_SCOPE_REWRITES only");
+    if (rewrites && !journal) return fail(c, BF_EINVAL, "BF_COMMIT_SCOPE_REWRITES needs a journal");
+  }
   if (rewrites) {
     if (!rewritten) return fail(c, BF_EINVAL, "null n_rewritten");
     *rewritten = 0;
@@ -1556,6 +1582,7 @@ static int resident_commit(bf_ctx* c, uint32_t h, uint32_t n_runs, const bf_comm
     arm->next_deadline = BF_TIMER_NONE;
   }
   if (!r) return BF_EINVAL;
+  if (scope && !r->areas.d_due) return refuse(BF_COMMIT_NONE, BF_COMMIT_NONE, "the batch has no commit-due area (bf_resident_commit_marks)");
   if (arm && !r->areas.timer_k) return refuse(BF_COMMIT_NONE, BF_COMMIT_NONE, "the batch has no timer area (bf_resident_timers) to arm");
   if (arm && arm->now == BF_TIMER_NONE) return refuse(BF_COMMIT_NONE, BF_COMMIT_NONE, "now must not be BF_TIMER_NONE");
   const bf_layout& L = r->L;
@@ -1605,6 +1632,21 @@ static int resident_commit(bf_ctx* c, uint32_t h, uint32_t n_runs, const bf_comm
   st.up(P.offender, &no_offender, 1);
   st.up(P.counts, zero_counts, n_counts);
   st.up(P.entries, sorted.data(), n);
+  // a touched commit: full, or the run list of its due bits and entries (groups of 32 due words)
+  const uint32_t form = (arm ? 1u : 0u) | (journaled ? 2u : 0u) | (rewrites ? 4u : 0u);
+  const bool full = scope && (r->commit_all || r->commit_form != form || (arm && r->commit_timings != c->timing_changes));
+  const bool by_list = scope && !full;
+  const unsigned long long all_runs = n_runs;
+  const unsigned long long* n_up = nullptr;
+  bf::DueListParams D{};
+  if (scope && full) st.up(n_up, &all_runs, 1);
+  if (by_list) {
+    D.n = (uint32_t)((RunAreas::due_words(n_runs) + 31) / 32); D.warps_per_block = 8;
+    st.out(D.group_runs, D.n);
+    st.out(D.cta, (D.n + 7) / 8);
+    st.out(D.total, 1);
+    st.out(D.list, n_runs);
+  }
   const uint32_t grid = (n_runs - 1u) / 8u + 1u;
   // pinned items / runs are written in place; the others are staged once their numbers are known
   OutList<bf_commit_write> items(journaled ? journal->items : nullptr, journaled ? journal->items_cap : 0, true);
@@ -1633,25 +1675,44 @@ static int resident_commit(bf_ctx* c, uint32_t h, uint32_t n_runs, const bf_comm
   P.words = L.words; P.state_stride = L.state_stride; P.off_phase = L.off_phase; P.result_stride = L.result_stride;
   P.off_ready = L.off_ready; P.off_skip = L.off_skip; P.off_fail = L.off_fail; P.sched_stride = A.sched_stride;
   P.mark = r->d_mark; P.mark_value = r->mark_touched();
+  // the list-mode parameters of a touched commit, as the sections stand (after a growth too)
+  const uint32_t list_ctas = (uint32_t)c->sm_count * 4u;
+  auto list_params = [&] {
+    bf::CommitListParams LP{};
+    LP.P = P; LP.list = by_list ? D.list : nullptr; LP.n_list = by_list ? D.total : n_up; LP.due = r->areas.d_due;
+    return LP;
+  };
+  const bool was_all = r->commit_all;
+  r->commit_all = true;   // until the call went through or was refused: a failed commit leaves every run due
   cudaError_t e = cudaSuccess;
+  if (by_list) {
+    D.due = r->areas.d_due; D.entries = P.entries; D.n_entries = n; D.n_runs = n_runs;
+    if (e == cudaSuccess) e = bf::launch_due_list(D, s);
+  }
   if (rewrites) {
     W.state = r->d_state; W.result = r->d_result; W.slots = c->slots_dev; W.n_slots = P.n_slots; W.runctl = A.runctl;
     W.n_runs = n_runs; W.warps_per_block = ps.wpb;
     W.words = L.words; W.state_stride = L.state_stride; W.off_phase = L.off_phase; W.off_decision = L.off_decision;
     W.off_child = L.off_child; W.topo_bytes = ps.topo; W.result_stride = L.result_stride;
-    e = bf::launch_rewrites(W, ps.smem(), s);
+    if (e == cudaSuccess)
+      e = scope ? bf::launch_rewrites_list(W, by_list ? D.list : nullptr, by_list ? D.total : n_up, (uint32_t)c->sm_count * 2u,
+                                           ps.smem(), s)
+                : bf::launch_rewrites(W, ps.smem(), s);
     P.rw_runs = W.rw_runs; P.rw_planes = W.rw_planes; P.rewritten = P.counts + 7;
   }
   uint32_t* host = c->pinned->commit;
   unsigned long long* totals = c->pinned->list_totals;
-  if (e == cudaSuccess) e = bf::launch_commit(P, false, s);
+  if (e == cudaSuccess) e = scope ? bf::launch_commit_list(list_params(), false, n_runs, list_ctas, s) : bf::launch_commit(P, false, s);
   if (e == cudaSuccess) e = cudaMemcpyAsync(host, P.offender, 8, cudaMemcpyDeviceToHost, s);
   if (e == cudaSuccess && journaled) e = cudaMemcpyAsync(totals, P.total, 16, cudaMemcpyDeviceToHost, s);
+  if (e == cudaSuccess && by_list) e = cudaMemcpyAsync(totals + 2, D.total, 8, cudaMemcpyDeviceToHost, s);
   if (int rc = bf::end_call(c, e, "bf_resident_commit (check)")) return rc;
-  c->stats.kernel_launches += (journaled ? 2 : 1) + (rewrites ? 1 : 0);
+  c->stats.kernel_launches += (journaled ? 2 : 1) + (rewrites ? 1 : 0) + (by_list ? 3 : 0);
+  if (scope) { scope->full = full ? 1u : 0u; scope->n_considered = full ? n_runs : (uint32_t)totals[2]; }
   uint64_t key;
   memcpy(&key, host, 8);
   if (key != ~0ull) {
+    r->commit_all = was_all;   // refused: nothing written, no due bit cleared
     const uint32_t run = (uint32_t)(key >> 32), step = (uint32_t)(key >> 8) & 0xFFFFFFu, why = (uint32_t)key & 0xFFu;
     const std::string at = "run " + std::to_string(run) + " step " + std::to_string(step) + ": ";
     if (why == bf::kCommitOverflow)
@@ -1672,7 +1733,9 @@ static int resident_commit(bf_ctx* c, uint32_t h, uint32_t n_runs, const bf_comm
   }
   P.items = items.dev; P.items_cap = items.cap;
   P.runs = listed.dev; P.runs_cap = (uint32_t)listed.cap;
-  e = bf::launch_commit(P, true, s);
+  e = cudaSuccess;
+  if (scope && full) e = cudaMemsetAsync(r->areas.d_due, 0xFF, r->areas.d_due.cap * 4, s);   // the runs at or past n_runs stay due
+  if (e == cudaSuccess) e = scope ? bf::launch_commit_list(list_params(), true, n_runs, list_ctas, s) : bf::launch_commit(P, true, s);
   if (e == cudaSuccess) e = cudaMemcpyAsync(host, P.counts, 4 * n_counts, cudaMemcpyDeviceToHost, s);
   if (e == cudaSuccess) e = items.copy_async(n_items, s);
   if (e == cudaSuccess) e = listed.copy_async(n_listed, s);
@@ -1688,7 +1751,33 @@ static int resident_commit(bf_ctx* c, uint32_t h, uint32_t n_runs, const bf_comm
     r->state_changed(c);
     r->pending += k[0];
   }
+  r->commit_all = scope ? false : was_all;
+  if (scope) { r->commit_form = form; r->commit_timings = c->timing_changes; }
   return BF_OK;
+}
+
+int bf_resident_commit_marks(bf_ctx* c, uint32_t h) {
+  auto [g, r] = lock_resident(c, h);
+  if (!r) return BF_EINVAL;
+  BF_CUDA(c, cudaSetDevice(c->device));
+  if (!r->areas.d_due) {
+    const cudaError_t e = r->areas.d_due.alloc(RunAreas::due_words(r->cap));
+    if (e != cudaSuccess) return fail(c, BF_ENOMEM, std::string("commit-due bits: ") + cudaGetErrorString(e));
+  }
+  r->commit_all = true;
+  cudaError_t e = cudaMemsetAsync(r->areas.d_due, 0xFF, r->areas.d_due.cap * 4, c->stream);
+  return bf::end_call(c, e, "bf_resident_commit_marks");
+}
+
+int bf_resident_commit_touched(bf_ctx* c, uint32_t h, uint32_t n_runs, const bf_commit_entry* entries, uint32_t n, bf_commit_out* out,
+                               bf_commit_arm* arm, bf_commit_journal* journal, uint32_t* n_rewritten, bf_commit_scope* scope) {
+  if (!scope) {
+    if (!c) return BF_EINVAL;
+    std::lock_guard<std::mutex> g(c->mu);
+    return fail(c, BF_EINVAL, "null bf_commit_scope");
+  }
+  const bool rewrites = (scope->flags & BF_COMMIT_SCOPE_REWRITES) != 0;
+  return resident_commit(c, h, n_runs, entries, n, out, arm, journal, journal != nullptr, n_rewritten, rewrites, scope);
 }
 
 int bf_resident_commit_rewrites(bf_ctx* c, uint32_t h, uint32_t n_runs, const bf_commit_entry* entries, uint32_t n,

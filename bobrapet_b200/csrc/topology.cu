@@ -444,7 +444,7 @@ static int drop_locked(bf_ctx* c, uint32_t slot) {
   if (slot >= c->meta.size() || !c->meta[slot].alive) return fail(c, BF_ETOPO, "drop of an unknown slot");
   c->meta[slot].alive = false;
   c->slot_changes++;
-  if (!c->meta[slot].timings.empty()) { c->meta[slot].timings.clear(); c->timings_dirty = true; }
+  if (!c->meta[slot].timings.empty()) { c->meta[slot].timings.clear(); c->timings_dirty = true; ++c->timing_changes; }
   if (c->meta[slot].P) c->n_with_parallel--;
   c->slots_host[slot] = bf::Slot{0, 0, 0};
   memset(&c->ff_host[(size_t)slot * bf::FF_STRIDE], 0, bf::FF_STRIDE * sizeof(uint32_t));
@@ -555,6 +555,7 @@ int bf_topology_timings(bf_ctx* c, uint32_t slot, const bf_step_timing* t, uint3
   if (v.empty() && m.timings.empty()) return BF_OK;
   m.timings = std::move(v);
   c->timings_dirty = true;
+  ++c->timing_changes;
   return BF_OK;
 }
 

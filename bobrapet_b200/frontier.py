@@ -427,8 +427,13 @@ class Frontier:
     COMMIT_WRITE_DTYPE = np.dtype([("run", "<u4"), ("index", "<u2"), ("field", "u1"), ("code", "u1"), ("before", "<u4"),
                                    ("after", "<u4")])   # bf_commit_write, 16 B
 
+    def resident_commit_marks(self, handle: int) -> None:
+        """bf_resident_commit_marks: enable the batch's commit-due bits (every run due), which resident_commit(touched=True)
+        needs"""
+        self._check(self._lib.bf_resident_commit_marks(self._ctx, handle), "bf_resident_commit_marks")
+
     def resident_commit(self, handle: int, n_runs: int, entries=None, now: Optional[int] = None,
-                        journal_cap: Optional[int] = None, rewrites: bool = False) -> dict:
+                        journal_cap: Optional[int] = None, rewrites: bool = False, touched: bool = False) -> dict:
         """bf_resident_commit: write the skips, launches and queue marks of the last tick (and schedule) of runs [0, n_runs)
         into the state records.  entries: COMMIT_DTYPE (or (run, step, kind, code) tuples), at most one per (run, step).
         With `now` (bf_resident_commit_timed) the launched sleep, gate and wait steps with a timing (put_timings) are armed too.
@@ -439,7 +444,8 @@ class Frontier:
         -> dict(n_runs_written, n_skipped, n_launched, n_queued, n_failed), with `now` also n_armed and next_deadline, with
         journal_cap also items (COMMIT_WRITE_DTYPE[min(n_items, journal_cap)]), n_items, runs (u32, the runs whose record
         changed) and n_runs_listed.  A refusal raises FrontierError with .bad_run and .bad_step (A.COMMIT_NONE for a refusal
-        of the whole call)"""
+        of the whole call).  With touched (bf_resident_commit_touched; needs resident_commit_marks) the same form considers only
+        the runs whose writes may not be in place, with the same results, and the dict also holds full and n_considered"""
         ents = np.zeros(0, dtype=self.COMMIT_DTYPE) if entries is None else entries
         if not isinstance(ents, np.ndarray):
             ents = np.array([tuple(e) for e in ents], dtype=self.COMMIT_DTYPE)
@@ -450,21 +456,28 @@ class Frontier:
         n_rw = C.c_uint32(0)
         ep = ents.ctypes.data if ents.shape[0] else None
         arm = None if now is None else A.CommitArm(struct_size=C.sizeof(A.CommitArm), now=int(now))
+        scope = A.CommitScope(struct_size=C.sizeof(A.CommitScope), flags=A.COMMIT_SCOPE_REWRITES if rewrites else 0)
+        j = None
         if journal_cap is not None:
             items = np.zeros(max(int(journal_cap), 1), dtype=self.COMMIT_WRITE_DTYPE)
             runs = np.zeros(max(int(n_runs), 1), dtype=np.uint32)
             j = A.CommitJournal(struct_size=C.sizeof(A.CommitJournal), items=items.ctypes.data if journal_cap else None,
                                 items_cap=int(journal_cap), runs=runs.ctypes.data if n_runs else None, runs_cap=int(n_runs))
-            if rewrites:
-                rc = self._lib.bf_resident_commit_rewrites(self._ctx, handle, int(n_runs), ep, ents.shape[0], C.byref(out),
-                                                           None if arm is None else C.byref(arm), C.byref(j), C.byref(n_rw))
-            else:
-                rc = self._lib.bf_resident_commit_journal(self._ctx, handle, int(n_runs), ep, ents.shape[0], C.byref(out),
-                                                          None if arm is None else C.byref(arm), C.byref(j))
+        a = None if arm is None else C.byref(arm)
+        if touched:
+            rc = self._lib.bf_resident_commit_touched(self._ctx, handle, int(n_runs), ep, ents.shape[0], C.byref(out), a,
+                                                      None if j is None else C.byref(j), C.byref(n_rw) if rewrites else None,
+                                                      C.byref(scope))
+        elif rewrites:
+            rc = self._lib.bf_resident_commit_rewrites(self._ctx, handle, int(n_runs), ep, ents.shape[0], C.byref(out), a,
+                                                       C.byref(j), C.byref(n_rw))
+        elif j is not None:
+            rc = self._lib.bf_resident_commit_journal(self._ctx, handle, int(n_runs), ep, ents.shape[0], C.byref(out), a,
+                                                      C.byref(j))
         elif arm is None:
             rc = self._lib.bf_resident_commit(self._ctx, handle, int(n_runs), ep, ents.shape[0], C.byref(out))
         else:
-            rc = self._lib.bf_resident_commit_timed(self._ctx, handle, int(n_runs), ep, ents.shape[0], C.byref(out), C.byref(arm))
+            rc = self._lib.bf_resident_commit_timed(self._ctx, handle, int(n_runs), ep, ents.shape[0], C.byref(out), a)
         if rc != A.BF_OK:
             err = A.FrontierError(rc, "bf_resident_commit: %s" % self._lib.bf_last_error(self._ctx).decode())
             err.bad_run, err.bad_step = int(out.bad_run), int(out.bad_step)
@@ -477,6 +490,8 @@ class Frontier:
                        runs=runs[:int(j.n_runs_listed)].copy(), n_runs_listed=int(j.n_runs_listed))
         if rewrites:
             got["n_rewritten"] = int(n_rw.value)
+        if touched:
+            got.update(full=int(scope.full), n_considered=int(scope.n_considered))
         return got
 
     # -- run status of resident batches (bf_resident_status)

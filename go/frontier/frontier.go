@@ -793,6 +793,56 @@ func (r *Resident) CommitRewrites(n, now uint32, entries []CommitEntry, items []
 	return res, j, uint32(k[10]), r.c.err(rc)
 }
 
+// EnableCommitMarks gives the batch its commit-due bits (bf_resident_commit_marks), which CommitTouched needs: one bit per run,
+// every run due.  Calling it again makes every run due again.
+func (r *Resident) EnableCommitMarks() error {
+	return r.c.err(C.bf_resident_commit_marks(r.c.p, r.handle))
+}
+
+// CommitScope says what a touched commit considered: Full when it took every run of [0, n), else the runs whose writes could
+// not be in place (those the touched ticks evaluated, the schedule changed or the entries named since their last touched
+// commit); NConsidered counts them.
+type CommitScope struct {
+	Full        bool
+	NConsidered uint32
+}
+
+// CommitTouched is the commit the arguments pick, through bf_resident_commit_touched: CommitTimed when now != TimerNone, else
+// Commit; CommitJournal into items and runs when journal is set; CommitRewrites when rewrites is set too.  Its results are
+// exactly that form's, at the cost of the runs it considers instead of all n: use it in the steady-state loop, after
+// EnableCommitMarks.  -> also the steps written from the stages (rewrites) and the scope.
+func (r *Resident) CommitTouched(n, now uint32, entries []CommitEntry, journal, rewrites bool, items []CommitWrite,
+	runs []uint32) (CommitResult, Journal, uint32, CommitScope, error) {
+	var ep *C.bf_commit_entry
+	if len(entries) > 0 {
+		ep = (*C.bf_commit_entry)(unsafe.Pointer(&entries[0]))
+	}
+	var ip *C.bf_commit_write
+	if len(items) > 0 {
+		ip = (*C.bf_commit_write)(unsafe.Pointer(&items[0]))
+	}
+	var rp *C.uint32_t
+	if len(runs) > 0 {
+		rp = (*C.uint32_t)(unsafe.Pointer(&runs[0]))
+	}
+	var flags, jn C.uint32_t
+	if rewrites {
+		flags = C.BF_COMMIT_SCOPE_REWRITES
+	}
+	if journal {
+		jn = 1
+	}
+	var k [13]C.uint32_t
+	var nItems C.uint64_t
+	rc := C.bfgo_resident_commit_touched(r.c.p, r.handle, C.uint32_t(n), ep, C.uint32_t(len(entries)), C.uint32_t(now), flags, jn,
+		ip, C.uint64_t(len(items)), rp, C.uint32_t(len(runs)), &k[0], &nItems)
+	res := CommitResult{uint32(k[0]), uint32(k[1]), uint32(k[2]), uint32(k[3]), uint32(k[4]), uint32(k[5]), uint32(k[6])}
+	j := Journal{NItems: uint64(nItems), NRuns: uint32(k[9]), Armed: uint32(k[7]), NextDeadline: uint32(k[8])}
+	j.Items = items[:minU64(j.NItems, uint64(len(items)))]
+	j.Runs = runs[:minU64(uint64(j.NRuns), uint64(len(runs)))]
+	return res, j, uint32(k[10]), CommitScope{Full: k[11] != 0, NConsidered: uint32(k[12])}, r.c.err(rc)
+}
+
 func minU64(a, b uint64) uint64 {
 	if a < b {
 		return a

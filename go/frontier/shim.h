@@ -339,6 +339,42 @@ static inline int bfgo_resident_commit_rewrites(bf_ctx* c, uint32_t handle, uint
   return rc;
 }
 
+/* Touched commits (bf_resident_commit_touched) of the form the arguments pick: arming when now != BF_TIMER_NONE, journaled when
+ * journal != 0 (items and runs as bfgo_resident_commit_journal), rewriting when flags carries BF_COMMIT_SCOPE_REWRITES (needs the
+ * journal).  counts as bfgo_resident_commit_rewrites (counts[7..10] zero / BF_TIMER_NONE where the form has no such field), and
+ * counts[11] = full, counts[12] = runs considered.  bf_resident_commit_marks enables the batch's commit-due bits first. */
+static inline int bfgo_resident_commit_touched(bf_ctx* c, uint32_t handle, uint32_t n_runs, const bf_commit_entry* entries, uint32_t n,
+                                               uint32_t now, uint32_t flags, uint32_t journal, bf_commit_write* items,
+                                               uint64_t items_cap, uint32_t* runs, uint32_t runs_cap, uint32_t* counts,
+                                               uint64_t* n_items) {
+  bf_commit_out o;
+  memset(&o, 0, sizeof o);
+  o.struct_size = (uint32_t)sizeof o;
+  bf_commit_arm a;
+  memset(&a, 0, sizeof a);
+  a.struct_size = (uint32_t)sizeof a;
+  a.now = now;
+  bf_commit_journal j;
+  memset(&j, 0, sizeof j);
+  j.struct_size = (uint32_t)sizeof j;
+  j.items = items; j.items_cap = items_cap; j.runs = runs; j.runs_cap = runs_cap;
+  bf_commit_scope sc;
+  memset(&sc, 0, sizeof sc);
+  sc.struct_size = (uint32_t)sizeof sc;
+  sc.flags = flags;
+  uint32_t nrw = 0;
+  const int rc = bf_resident_commit_touched(c, handle, n_runs, entries, n, &o, now == BF_TIMER_NONE ? NULL : &a, journal ? &j : NULL,
+                                            &nrw, &sc);
+  counts[0] = o.n_runs_written; counts[1] = o.n_skipped; counts[2] = o.n_launched; counts[3] = o.n_queued; counts[4] = o.n_failed;
+  counts[5] = o.bad_run; counts[6] = o.bad_step;
+  counts[7] = now == BF_TIMER_NONE ? 0u : a.n_armed; counts[8] = now == BF_TIMER_NONE ? BF_TIMER_NONE : a.next_deadline;
+  counts[9] = journal ? j.n_runs_listed : 0u;
+  counts[10] = (flags & BF_COMMIT_SCOPE_REWRITES) ? nrw : 0u;
+  counts[11] = sc.full; counts[12] = sc.n_considered;
+  *n_items = journal ? j.n_items : 0u;
+  return rc;
+}
+
 /* Run status.  The records (bf_status_rec holds no pointers) and events land in the caller's buffers; *n_events = the events of
  * the listed runs, of which the first events_cap were written.  runs == NULL with n == n_runs lists every run of [0, n_runs). */
 static inline int bfgo_resident_status(bf_ctx* c, uint32_t handle, uint32_t n_runs, const uint32_t* runs, uint32_t n,

@@ -1249,6 +1249,66 @@ int bf_resident_commit_journal(bf_ctx* ctx, uint32_t handle, uint32_t n_runs, co
 int bf_resident_commit_rewrites(bf_ctx* ctx, uint32_t handle, uint32_t n_runs, const bf_commit_entry* entries, uint32_t n_entries,
                                 bf_commit_out* out, bf_commit_arm* arm, bf_commit_journal* journal, uint32_t* n_rewritten);
 
+/* Touched commits.  Every commit form walks all of [0, n_runs), although after the first commit almost every run's writes are
+ * already in place.  bf_resident_commit_touched considers only the runs whose writes may not be in place, and its results are
+ * those of the matching full form.
+ *
+ * bf_resident_commit_marks(ctx, handle) enables the batch's commit-due area: one bit per run, every bit set.  Reshape and a
+ * retire to a new capacity keep the bits of the runs both capacities hold; a batch that never enables the area launches, copies
+ * and writes what it did before.  Calling it again sets every bit again.
+ *
+ * The form: arm, journal and BF_COMMIT_SCOPE_REWRITES in scope->flags pick the full form the call matches, with that form's
+ * argument rules:
+ *   arm NULL, journal NULL                      bf_resident_commit
+ *   arm set,  journal NULL                      bf_resident_commit_timed
+ *   journal set, no BF_COMMIT_SCOPE_REWRITES    bf_resident_commit_journal
+ *   journal set, BF_COMMIT_SCOPE_REWRITES       bf_resident_commit_rewrites (n_rewritten required)
+ * n_rewritten is ignored without BF_COMMIT_SCOPE_REWRITES, and BF_COMMIT_SCOPE_REWRITES without a journal is BF_EINVAL.  A batch
+ * without the area is BF_EINVAL (bad_run = bad_step = BF_COMMIT_NONE).
+ *
+ * Equivalence guarantee: for any sequence of resident calls, the return code, bad_run and bad_step, every bf_commit_out and
+ * bf_commit_arm field, n_rewritten, the journal's items and runs and their true counts, the state records, timer slots and touch
+ * marks, and the batch's bookkeeping (the tick a schedule or commit needs, the touched-list bound, what the next touched tick
+ * lists) are exactly those the matching full form would have given at the same point.
+ *
+ * Why it holds: a commit is idempotent (over records whose writes are in place it writes nothing and refuses nothing), and what
+ * it writes or checks for a run is a function of that run's state record, current result record, schedule record, timer slots
+ * and run-control record, the slot's step types and timings, the run's entries and the form.  A run is due unless the last
+ * touched commit that considered it found no entry on it and none of those inputs changed since:
+ *   - a touched tick (single or _many) sets the bit of every run it evaluates, bf_resident_schedule that of every run whose
+ *     schedule record changed;
+ *   - the call considers every run of [0, n_runs) ("full") after a full tick (bf_resident_tick, _tick_compact, _eval, a touched
+ *     tick that ran full), after enabling the area, after a tick, schedule or commit that failed (CUDA or allocation), when its
+ *     form differs from the last touched commit's, and, for a form that arms, after a bf_topology_timings or a drop changed the
+ *     ctx's timings since the last touched commit;
+ *   - a run that an entry names is considered, and stays due after the commit.
+ * Every other call that changes a run's records (deltas, uploads, moves, migrations, redrives, resyncs, fires that write, stops,
+ * commits that write) touches the run, and a commit must follow a tick over n_runs (the rule of every form), which evaluates
+ * and so marks every touched run.  A commit of another form, a refused commit and a commit that fails clear no bit.
+ *
+ * Device work: without full, one count, scan and list launch triple builds the ascending list of the due runs below n_runs and
+ * the runs the entries name; the check (with a journal, and its scan over the list's blocks of 8 positions), the rewrites and the
+ * apply launches are list-mode builds of the full form's, one warp per listed run; the apply also clears the due bits.  With
+ * full, no list is built: every bit is set once the check passed (a memset, no launch) and the list-mode builds take
+ * [0, n_runs).  Launches: the full form's, plus 3 without full (so 5, 5, 6 and 7 for the four forms; 2, 2, 3 and 4 with full),
+ * none when n_runs == 0.  The
+ * commit's two synchronisations stay.  A touched tick on a batch with the area adds one launch (one per part for _many), and
+ * bf_resident_schedule one per batch with the area.
+ *
+ * scope (required): struct_size = sizeof(bf_commit_scope), flags; out: full (1: every run of [0, n_runs) was considered) and
+ * n_considered (the runs considered; n_runs with full).  Both are 0 for n_runs == 0 and on a refusal before the device. */
+#define BF_COMMIT_SCOPE_REWRITES 0x1u
+typedef struct bf_commit_scope {
+  uint32_t struct_size;          /* sizeof(bf_commit_scope)                                                                     */
+  uint32_t flags;                /* BF_COMMIT_SCOPE_REWRITES or 0                                                               */
+  uint32_t full;                 /* out                                                                                         */
+  uint32_t n_considered;         /* out                                                                                         */
+} bf_commit_scope;
+int bf_resident_commit_marks(bf_ctx* ctx, uint32_t handle);
+int bf_resident_commit_touched(bf_ctx* ctx, uint32_t handle, uint32_t n_runs, const bf_commit_entry* entries, uint32_t n_entries,
+                               bf_commit_out* out, bf_commit_arm* arm, bf_commit_journal* journal, uint32_t* n_rewritten,
+                               bf_commit_scope* scope);
+
 /* ------------------------------------------------------------------ run status (what a batcher persists of a run's status)
  * When group selection finds nothing left to run (BF_GROUP_DONE, dag.go:482-495) the reference finalizes the StoryRun
  * (finalizeStoryRun, dag.go:693-754): the failed set of the finally, compensation or main group, in that order, decides its phase
