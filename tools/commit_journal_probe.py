@@ -114,13 +114,14 @@ def main():
             written.append(o0.n_runs_written)
     gpu = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True,
                          text=True).stdout.strip()
-    q = lambda t: (np.median(t) * 1e6, np.min(t) * 1e6, np.max(t) * 1e6, len(t))  # noqa: E731
+    q = lambda t: (np.median(t) * 1e6, np.percentile(t, 25) * 1e6, np.percentile(t, 75) * 1e6, np.min(t) * 1e6, np.max(t) * 1e6,  # noqa: E731
+                   len(t))
     lines = ["commit_journal_probe: %d runs x %d steps (a quarter gates, each with a timing), K = %d, 1 %% of codes changed per tick, "
              "%d ticks after %d warm-up, the three forms rotating" % (n, S, K, a.ticks, a.warmup),
              "gpu: %s" % gpu]
     for k, label in zip(names, ("bf_resident_commit_timed", "bf_resident_commit_journal, pinned buffers",
                                 "bf_resident_commit_journal, pageable buffers")):
-        lines.append("%-8s (%s): median %.1f us, range %.1f .. %.1f (%d ticks)" % ((k, label) + q(times[k])))
+        lines.append("%-8s (%s): median %.1f us, p25 %.1f, p75 %.1f, range %.1f .. %.1f (%d ticks)" % ((k, label) + q(times[k])))
     lines.append("items per tick: median %d; runs written per commit: median %d" % (np.median(items_per_tick), np.median(written)))
     text = "\n".join(lines)
     print(text)

@@ -102,10 +102,11 @@ def main():
             n_written.append(c["n_runs_written"])
     gpu = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True,
                          text=True).stdout.strip()
+    q = lambda t: (np.median(t) * 1e6, np.percentile(t, 25) * 1e6, np.percentile(t, 75) * 1e6, np.min(t) * 1e6)  # noqa: E731
     lines = ["commit_probe: %d runs x %d steps, 1 %% of codes changed per tick, %d ticks after %d warm-up" % (n, S, a.ticks, a.warmup),
              "gpu: %s" % gpu,
-             "commit (touched tick + schedule + commit): median %.1f us, min %.1f us" % (np.median(t_commit) * 1e6, np.min(t_commit) * 1e6),
-             "echo   (touched tick + schedule + apply):  median %.1f us, min %.1f us" % (np.median(t_echo) * 1e6, np.min(t_echo) * 1e6),
+             "commit (touched tick + schedule + commit): median %.1f us, p25 %.1f, p75 %.1f, min %.1f us" % q(t_commit),
+             "echo   (touched tick + schedule + apply):  median %.1f us, p25 %.1f, p75 %.1f, min %.1f us" % q(t_echo),
              "echo deltas per tick: median %d; runs written per commit: median %d" % (np.median(n_echo), np.median(n_written))]
     text = "\n".join(lines)
     print(text)
