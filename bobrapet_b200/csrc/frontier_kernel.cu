@@ -208,7 +208,7 @@ __global__ void __launch_bounds__(RB == 2 ? 768 : 512, RB == 1 ? 2 : 1) frontier
 
       // ---------------- stages G, B, I and D-prep (stages.cuh) ----------------
       if (has_dec) gdirty |= stage_g(SYNC_T, TS, d0, d1, p0, p1, p2, p3);
-      const RunClass rc = stage_bi<CD>(FULL, rflags, n_main, n_comp, n_final, AF, GM, G1, G2, p0, p1, p2, p3);
+      const RunClass rc = stage_bi<CD>([](uint32_t v) { return redux_or(v); }, rflags, n_main, n_comp, n_final, AF, GM, G1, G2, p0, p1, p2, p3);
       marked = marked || rc.marked;
       summary = rc.sum | rc.group;
 

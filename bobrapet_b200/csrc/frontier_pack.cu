@@ -8,7 +8,9 @@
 // Here lane l = g * Wq + w holds word w (32 steps) of run g of the group, so every bit-plane stage (gate / sleep /
 // wait rewrite dag.go:1455-1547, buildStateMaps :3358-3391, fail-fast / compensation marking and group selection
 // :422-511, cond masking :2741-2843, result words) runs on all 32 lanes and its instructions are shared by R runs;
-// per-run reductions are sub-warp redux / ballots.  Only the dependency walk (dag.go:2711-2733, one step per lane
+// per-run reductions are ballots masked to the run's lanes and segmented butterflies of full-mask shuffles (seg_or / seg_add,
+// kernel_common.cuh), so the warp stays converged: a sub-warp __reduce_*_sync took a divergent fallback, once per run, on every
+// trip.  Only the dependency walk (dag.go:2711-2733, one step per lane
 // over a `needs` row) stays per (run, word).
 //
 // Data movement: the CTA (one per SM, persistent) owns a ring of NG slot groups in shared memory, each holding the R
@@ -381,7 +383,10 @@ __global__ void __launch_bounds__(32 * PACK_MAX_WARPS, PACK_MIN_BLOCKS) frontier
     if (FF) {
       const uint32_t ff_b = __ballot_sync(FULL, (plut<LUT_FAILED>(cp0, cp1, cp2, cp3) & ffm) != 0);
       const uint32_t bp = plut<BF_LUT_TERMINAL>(cp0, cp1, cp2, cp3) | (plut<BF_LUT_RT_SAT>(cp0, cp1, cp2, cp3) & (0u - ((flr >> 29) & 1u)));   // bit 29: SID_RT
-      const uint32_t hs_p = __reduce_max_sync(gmask, bp ? w * 32u + 32u - __clz(bp) : 0u);
+      // the run's highest word with such a code (the highest lane of its segment in the ballot) and that word's highest step
+      const uint32_t tb = __ballot_sync(FULL, bp != 0) & gmask;
+      const uint32_t hl = 31u - __clz(tb), hb = __shfl_sync(FULL, bp, hl);   // tb = 0: any lane, result unused
+      const uint32_t hs_p = tb ? (hl & (Wq - 1u)) * 32u + 32u - __clz(hb) : 0u;
       need_b = __ballot_sync(FULL, cpw != 0 && (flr & 0xFFFFu) <= hs_p && (ff_b & gmask) == 0);
     }
     const uint32_t cand_words = (need_b >> (lr << lg)) & wq_mask;   // of my run (issuing lanes)
@@ -523,7 +528,7 @@ __global__ void __launch_bounds__(32 * PACK_MAX_WARPS, PACK_MIN_BLOCKS) frontier
 
     // ---------------- stages G, B, I and D-prep (stages.cuh); U & VALID: the PAD entry of a narrower run reads "satisfied"
     if (has_dec) stage_g(SYNC_T, TS, d0, d1, p0, p1, p2, p3);
-    const RunClass rc = stage_bi<CD>(gmask, rflags, n_main, n_comp, n_final, AF, GM, G1, G2, p0, p1, p2, p3);
+    const RunClass rc = stage_bi<CD>([&](uint32_t v) { return seg_or(v, lg); }, rflags, n_main, n_comp, n_final, AF, GM, G1, G2, p0, p1, p2, p3);
     uint32_t summary = rc.sum | rc.group;
     const DepClass dc = stage_dprep(rc, rflags, VALID, GM, G1, G2, NODEP, p0, p1, p2, p3);
     const uint32_t U = dc.U, FD = dc.FD;
@@ -591,7 +596,7 @@ __global__ void __launch_bounds__(32 * PACK_MAX_WARPS, PACK_MIN_BLOCKS) frontier
     const uint32_t acc_ready = ready_w, acc_skip = fd_w | skipc_w;
 
     // ---------------- stage E: result records ----------------
-    const uint32_t cnt = __reduce_add_sync(gmask, (uint32_t)__popc(acc_ready) | ((uint32_t)__popc(acc_skip) << 16));
+    const uint32_t cnt = seg_add((uint32_t)__popc(acc_ready) | ((uint32_t)__popc(acc_skip) << 16), lg);   // both <= S <= 512
     bool changed = rc.marked;   // with cond / decision codes: stage G may write the code a step already has
     if (CD) changed = (__ballot_sync(FULL, ((p0 ^ q0) | (p1 ^ q1) | (p2 ^ q2) | (p3 ^ q3)) != 0) & gmask) != 0;
     // fused compaction head (compact.cu): events of the run = steps with a bit in any result mask the layout carries
@@ -603,7 +608,7 @@ __global__ void __launch_bounds__(32 * PACK_MAX_WARPS, PACK_MIN_BLOCKS) frontier
         if (P.off_needs_cond != BF_OFF_NONE) u |= realtime ? 0u : (met_w & HASIF);
         if (P.off_skip_dep != BF_OFF_NONE) u |= fd_w;
       }
-      n_events = __reduce_add_sync(gmask, (uint32_t)__popc(u));
+      n_events = seg_add((uint32_t)__popc(u), lg);
     }
     if (deferred) {
       if (w == 0) P.defer_list[atomicAdd(P.defer_count, 1u)] = r;  // the general kernel writes this run's record

@@ -103,6 +103,23 @@ DI uint32_t get_nibble(const uint8_t* base, uint32_t i) {
 }
 DI uint32_t redux_or(uint32_t v) { return __reduce_or_sync(FULL, v); }
 DI uint32_t redux_add(uint32_t v) { return __reduce_add_sync(FULL, v); }
+// Segmented reductions: every lane gets the OR / sum / max of the aligned segment of 2^lg lanes that holds it (lg warp-uniform,
+// at most 5), by a butterfly of full-mask shuffles.  A __reduce_*_sync over a sub-warp mask is one REDUX only when the mask is
+// the same in every lane; with a different mask per segment ptxas runs it once per distinct mask in a divergent fallback
+// block (WARPSYNC.COLLECTIVE on the mask register) far from the loop.  tests/test_sass_collectives.py keeps that block out of
+// the frontier kernels.
+DI uint32_t seg_or(uint32_t v, uint32_t lg) {
+  for (uint32_t o = (1u << lg) >> 1; o; o >>= 1) v |= __shfl_xor_sync(FULL, v, o);
+  return v;
+}
+DI uint32_t seg_add(uint32_t v, uint32_t lg) {
+  for (uint32_t o = (1u << lg) >> 1; o; o >>= 1) v += __shfl_xor_sync(FULL, v, o);
+  return v;
+}
+DI uint32_t seg_max(uint32_t v, uint32_t lg) {
+  for (uint32_t o = (1u << lg) >> 1; o; o >>= 1) v = max(v, __shfl_xor_sync(FULL, v, o));
+  return v;
+}
 
 // ---- per-run lists (bf_resident_schedule, _status, _resync, _commit_journal): count, scan, list ------------------------------
 // A count launch gives each warp one word for its run (or runs) and stores each CTA's K totals; cta_scan (resident.cu) turns each

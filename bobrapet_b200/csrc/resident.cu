@@ -1575,7 +1575,7 @@ DI RunClass single_pass(const Params& P, uint32_t lane, bool act, const TopoHead
     __syncwarp();
   }
   if (P.off_decision != BF_OFF_NONE) stage_g(T.SYNC_T, T.TS, d0, d1, p0, p1, p2, p3);
-  return stage_bi<true>(FULL, rflags, th.n_main, th.n_comp, th.n_final, T.AF, T.VALID & ~T.G1 & ~T.G2, T.G1, T.G2, p0, p1, p2, p3);
+  return stage_bi<true>([](uint32_t v) { return redux_or(v); }, rflags, th.n_main, th.n_comp, th.n_final, T.AF, T.VALID & ~T.G1 & ~T.G2, T.G1, T.G2, p0, p1, p2, p3);
 }
 
 // ---- run status (bf_resident_status) ------------------------------------------------------------------------------------------

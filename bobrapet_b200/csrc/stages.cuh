@@ -3,8 +3,9 @@
 // join, is also taken by the run-status kernel (resident.cu), which reports the phases a single pass would leave.
 //
 // A lane holds word w (32 steps) of one run: w = lane in the general kernel, lane = g * Wq + w in the packed-lanes kernel.
-// Per-run reductions run over `gmask`, the lanes of the caller's run (FULL in the general kernel).  No collective sits under
-// a per-run branch: a run that does not take a step still takes part in every vote.
+// Per-run reductions run over the lanes of the caller's run: `gmask` for votes (FULL in the general kernel), the caller's
+// reduction for stage I.  No collective sits under a per-run branch: a run that does not take a step still takes part in
+// every vote.
 #pragma once
 #include "kernel_common.cuh"
 
@@ -168,14 +169,16 @@ struct RunClass {
 };
 
 // Stage B, classification (dag.go:3377-3388, 2020-2033), then stage I: fail-fast / compensation marking and group selection
-// (dag.go:422-495), all per-run reductions in one sub-warp redux.or.  Host-group runs take part in every vote, never qualify
-// for a marking, and get the host's group.
+// (dag.go:422-495), all per-run reductions in one OR of ten flag bits over the run's lanes: `run_or(v)`, called by every lane
+// of the warp, returns that OR in each lane — one REDUX in the general kernel (one run per warp), a segmented butterfly in the
+// packed-lanes kernel (seg_or, kernel_common.cuh).  Host-group runs take part in every vote, never qualify for a marking, and
+// get the host's group.
 // SUM_FIRST orders two independent results and changes nothing else.  ptxas schedules the packed-lanes kernel differently
 // with each order, and each build is fastest with its own (H100 SXM at 400 W, µs per pipelined pass in three rounds): with
 // cond / decision codes, cfg4 took 56.1 - 56.3 group first and 55.0 - 55.2 summary first; without them, cfg3 took
 // 49.6 - 49.7 group first and 50.3 - 50.9 summary first (the latter with a 4-byte spill).
-template <bool SUM_FIRST>
-DI RunClass stage_bi(uint32_t gmask, uint32_t rflags, uint32_t n_main, uint32_t n_comp, uint32_t n_final, uint32_t AF,
+template <bool SUM_FIRST, class RunOr>
+DI RunClass stage_bi(RunOr run_or, uint32_t rflags, uint32_t n_main, uint32_t n_comp, uint32_t n_final, uint32_t AF,
                      uint32_t GM, uint32_t G1, uint32_t G2, uint32_t& p0, uint32_t& p1, uint32_t& p2, uint32_t& p3) {
   bool marked = false;
   const bool fail_fast = rflags & BF_RF_FAIL_FAST;
@@ -202,7 +205,7 @@ DI RunClass stage_bi(uint32_t gmask, uint32_t rflags, uint32_t n_main, uint32_t 
                   | ((FAILED & G2) != 0 ? 128u : 0u)
                   | (mark_ff != 0 ? 256u : 0u)
                   | (mark_cs != 0 ? 512u : 0u);
-  bits = __reduce_or_sync(gmask, bits);
+  bits = run_or(bits);
   bool amf = bits & 1u;
   const bool do_ff = auto_group && fail_fast && amf;
   if (do_ff) {
@@ -218,7 +221,7 @@ DI RunClass stage_bi(uint32_t gmask, uint32_t rflags, uint32_t n_main, uint32_t 
     const uint32_t mtt = tt ? (GM & (p0 | p1 | p2 | p3) & ~TERM) : 0u;
     pset<BF_PHASE_FAILED>(mtt, p0, p1, p2, p3);
     TERM |= mtt; COMPL |= mtt & AF; FAILED |= mtt & ~AF; RUN &= ~mtt; RUNQ &= ~mtt;
-    const uint32_t b2 = __reduce_or_sync(gmask, (mtt != 0 ? 1u : 0u) | ((FAILED & GM) != 0 ? 2u : 0u));
+    const uint32_t b2 = run_or((mtt != 0 ? 1u : 0u) | ((FAILED & GM) != 0 ? 2u : 0u));
     if (tt) {
       marked = marked || (b2 & 1u);
       main_done = true;
