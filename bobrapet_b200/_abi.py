@@ -158,6 +158,17 @@ class Transfer(C.Structure):
                 ("unfit", C.c_uint32), ("why", Extent)]
 
 
+SLOT_NONE = 0xFFFFFFFF   # BF_SLOT_NONE: a slot_map entry of bf_resident_transfer_ctx that maps no slot
+UNFIT_NONE, UNFIT_LAYOUT, UNFIT_SLOT_UNMAPPED, UNFIT_SLOT_PAST_MAP, UNFIT_SLOT_DEAD = 0, 1, 2, 3, 4   # BF_UNFIT_*
+
+
+class CtxTransfer(C.Structure):
+    _fields_ = [("struct_size", C.c_uint32), ("src_n_runs", C.c_uint32), ("dst_n_runs", C.c_uint32), ("runs", C.c_void_p),
+                ("n", C.c_uint32), ("slot_map", C.c_void_p), ("n_slot_map", C.c_uint32), ("moves_from", C.c_void_p),
+                ("moves_to", C.c_void_p), ("n_moves", C.c_uint32), ("unfit", C.c_uint32), ("unfit_reason", C.c_uint32),
+                ("why", Extent)]
+
+
 TIMER_NONE = 0xFFFFFFFF   # BF_TIMER_NONE: an empty slot's deadline; as a request's deadline it cancels
 TIMER_MAX_SLOTS = 64      # BF_TIMER_MAX_SLOTS
 
@@ -187,6 +198,10 @@ class ResidentSchedPart(C.Structure):
     _fields_ = [("struct_size", C.c_uint32), ("handle", C.c_uint32), ("n_runs", C.c_uint32), ("runs_cap", C.c_uint32),
                 ("runs", C.c_void_p), ("heads", C.c_void_p), ("events", C.c_void_p), ("events_cap", C.c_uint64),
                 ("n_listed", C.c_uint32), ("full", C.c_uint32), ("n_events", C.c_uint64)]
+
+
+class CtxSchedPart(C.Structure):
+    _fields_ = [("struct_size", C.c_uint32), ("reserved", C.c_uint32), ("ctx", C.c_void_p), ("part", C.POINTER(ResidentSchedPart))]
 
 
 STOP_NONE, STOP_TIMEOUT, STOP_CANCEL, STOP_HOST = 0, 1, 2, 3   # BF_STOP_*: why a run of a resident batch is stopped
@@ -308,6 +323,7 @@ SYMBOLS = [
     ("bf_resident_extent", C.c_int, [C.c_void_p, C.c_uint32, C.POINTER(Extent)]),
     ("bf_resident_narrow", C.c_int, [C.c_void_p, C.c_uint32, C.POINTER(Layout), C.POINTER(Extent)]),
     ("bf_resident_transfer", C.c_int, [C.c_void_p, C.c_uint32, C.c_uint32, C.POINTER(Transfer)]),
+    ("bf_resident_transfer_ctx", C.c_int, [C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.POINTER(CtxTransfer)]),
     ("bf_resident_timers", C.c_int, [C.c_void_p, C.c_uint32, C.c_uint32]),
     ("bf_resident_timers_arm", C.c_int, [C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32]),
     ("bf_resident_fire", C.c_int, [C.c_void_p, C.c_uint32, C.c_uint32, C.POINTER(FireOut)]),
@@ -317,6 +333,8 @@ SYMBOLS = [
     ("bf_resident_sched_download", C.c_int, [C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32, C.c_void_p]),
     ("bf_resident_schedule", C.c_int, [C.c_void_p, C.POINTER(SchedTables), C.c_uint32, C.POINTER(ResidentSchedPart), C.c_uint32,
                                        C.POINTER(SchedOut)]),
+    ("bf_resident_schedule_ctxs", C.c_int, [C.POINTER(SchedTables), C.c_uint32, C.POINTER(CtxSchedPart), C.c_uint32,
+                                            C.POINTER(SchedOut)]),
     ("bf_resident_runctl", C.c_int, [C.c_void_p, C.c_uint32]),
     ("bf_resident_runctl_put", C.c_int, [C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32]),
     ("bf_resident_runctl_download", C.c_int, [C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32, C.c_void_p]),

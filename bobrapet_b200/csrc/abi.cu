@@ -527,6 +527,7 @@ void bf_destroy(bf_ctx* c) {
   }
   cudaFreeHost(c->pinned);
   if (c->part_tails) cudaFreeHost(c->part_tails);
+  if (c->span_totals) cudaFreeHost(c->span_totals);
   delete c;   // the device buffers of the ctx and of its resident batches free themselves
 }
 

@@ -43,6 +43,7 @@ cudaError_t launch_retire(const RetireParams& P, cudaStream_t stream);
 cudaError_t launch_extent(const ExtentParams& P, uint32_t sm_count, cudaStream_t stream);
 cudaError_t launch_transfer_fit(const TransferParams& P, cudaStream_t stream);
 cudaError_t launch_transfer(const TransferParams& P, cudaStream_t stream);
+cudaError_t launch_gather(const GatherParams& P, cudaStream_t stream);
 cudaError_t launch_relay_timers(const TimerRelayParams& P, cudaStream_t stream);
 cudaError_t launch_arm_timers(const TimerArmParams& P, bool merge, cudaStream_t stream);
 cudaError_t launch_fire(const FireParams& P, cudaStream_t stream);
@@ -235,6 +236,9 @@ struct bf_ctx {
   // bf_resident_tick_touched_many: the small results of each part, pinned (the single call uses pinned->tail)
   bf::ResultTail* part_tails = nullptr;
   uint32_t part_tails_cap = 0;
+  // bf_resident_schedule_ctxs: this ctx's own Running counts and queue priority maxima (phase 1), pinned
+  uint32_t* span_totals = nullptr;
+  size_t span_totals_cap = 0;
   // The device inputs and outputs of one resident call that is not a tick (migrate, redrive, retire, extent, narrow, transfer,
   // timers_arm, fire, sched_put, schedule, runctl_put, commit, status, resync), laid out by the call (CallStage, resident_abi.cu).  They are
   // valid from the call's staging until it returns: a call reads only bytes it uploaded, set or had a kernel write during the

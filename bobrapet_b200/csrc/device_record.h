@@ -338,6 +338,27 @@ struct TransferParams {
   uint32_t* unfit;               // [1] the lowest i that T cannot hold (atomicMin; 0xFFFFFFFF from the caller)
 };
 
+// bf_resident_transfer_ctx (resident.cu): runs[i] of the source batch is packed into staged run i, in the source layout (gather_runs).
+// The staging, copied to the destination ctx, is the source view of transfer_fit and transfer_runs there: its state records carry
+// the destination slot, ident[i] = i stands for runs, and mark[i] is 0 when the run's result record is a baseline of the source
+// (run_extent's rule) and 3 (must list after epoch 0) when not, for an ExtentBatch with prev_runs 0, eval_runs n, full_epoch 0.
+// A run whose slot the map does not carry sets reason[i] (BF_UNFIT_SLOT_*) and lowers *unfit, which transfer_fit lowers further.
+constexpr uint32_t kSlotDead = 0xFFFFFFFEu;   // slot_map entry of a slot that is not live in the source ctx
+struct GatherParams {
+  ExtentBatch src;               // the source batch, its baselines as transfer_fit would read them
+  const uint32_t* runs;          // [n] source indices
+  uint32_t n;
+  const uint32_t* slot_map;      // [n_slot_map] destination slot, BF_SLOT_NONE or kSlotDead
+  uint32_t n_slot_map;
+  uint32_t* unfit;               // [1] BF_EXTENT_NO_RUN from the caller
+  uint32_t* reason;              // [n]
+  uint32_t* ident;               // [n]
+  uint32_t* mark;                // [n]
+  uint8_t* state;                // [n][src.L.state_stride]
+  uint8_t* result;               // [n][src.L.result_stride]
+  RunAreasView areas;            // [n] entries of each area the source has (sched_rec unused)
+};
+
 // step timers (resident.cu): slot = deadline | step << 32 | code << 48 (bf_timer_slot read as one little-endian u64); an empty
 // slot is kTimerEmpty.  A run's armed slots come first, ascending by step.
 constexpr unsigned long long kTimerEmpty = 0xFFFFFFFFull;

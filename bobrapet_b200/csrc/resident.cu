@@ -708,6 +708,50 @@ cudaError_t launch_transfer(const TransferParams& P, cudaStream_t stream) {
   return cudaGetLastError();
 }
 
+// Transfer to another ctx (bf_resident_transfer_ctx), the gather on the source.  One warp per listed run: lane t copies the
+// 16-byte vectors t, t + 32, ... of its state and current result records into staged run i, the header's slot mapped to the
+// destination's, and timer slots t, t + 32; lane 0 copies its limiter inputs and run control and writes its identity index, its
+// baseline mark and its slot verdict (GatherParams).  The source is only read, so a refusal later leaves it as it was.
+__global__ void __launch_bounds__(256) gather_runs(const GatherParams P) {
+  const uint32_t i = blockIdx.x * 8u + (threadIdx.x >> 5), lane = threadIdx.x & 31u;
+  if (i >= P.n) return;
+  const ExtentBatch& B = P.src;
+  const uint32_t r = P.runs[i];
+  const uint4* s = reinterpret_cast<const uint4*>(B.state + (size_t)r * B.L.state_stride);
+  const uint32_t slot = s[0].x;
+  const uint32_t to = slot < P.n_slot_map ? P.slot_map[slot] : BF_SLOT_NONE;
+  const uint32_t why = slot >= P.n_slot_map ? (uint32_t)BF_UNFIT_SLOT_PAST_MAP
+                       : to == BF_SLOT_NONE ? (uint32_t)BF_UNFIT_SLOT_UNMAPPED
+                       : to == kSlotDead    ? (uint32_t)BF_UNFIT_SLOT_DEAD
+                                            : (uint32_t)BF_UNFIT_NONE;
+  uint4* d = reinterpret_cast<uint4*>(P.state + (size_t)i * B.L.state_stride);
+  for (uint32_t k = lane; k < (B.L.state_stride >> 4); k += 32u) {
+    uint4 v = s[k];
+    if (k == 0 && why == BF_UNFIT_NONE) v.x = to;
+    d[k] = v;
+  }
+  const uint4* rs = reinterpret_cast<const uint4*>(B.result + (size_t)r * B.L.result_stride);
+  uint4* rd = reinterpret_cast<uint4*>(P.result + (size_t)i * B.L.result_stride);
+  for (uint32_t k = lane; k < (B.L.result_stride >> 4); k += 32u) rd[k] = rs[k];
+  const RunAreasView& A = B.areas;
+  for (uint32_t k = lane; A.timers && k < A.timer_k; k += 32u) P.areas.timers[(size_t)i * A.timer_k + k] = A.timers[(size_t)r * A.timer_k + k];
+  if (lane != 0) return;
+  if (A.sched_in) P.areas.sched_in[i] = A.sched_in[r];
+  if (A.runctl) P.areas.runctl[i] = A.runctl[r];
+  const uint32_t m = B.mark[r];
+  const bool baseline = r < B.prev_runs || (r < B.eval_runs && !((m & 1u) && (m >> 1) > B.full_epoch));
+  P.mark[i] = baseline ? 0u : 3u;
+  P.ident[i] = i;
+  P.reason[i] = why;
+  if (why != BF_UNFIT_NONE) atomicMin(P.unfit, i);
+}
+
+cudaError_t launch_gather(const GatherParams& P, cudaStream_t stream) {
+  if (P.n == 0) return cudaSuccess;
+  gather_runs<<<(P.n - 1u) / 8u + 1u, 256, 0, stream>>>(P);
+  return cudaGetLastError();
+}
+
 // ---- step timers (bf_resident_timers*, bf_resident_fire) ----------------------------------------------------------------------
 // Relay (bf_resident_timers, reshape): one thread per slot of the new area.
 __global__ void __launch_bounds__(256) relay_timers(const TimerRelayParams P) {

@@ -6,6 +6,7 @@
 
 #include <array>
 #include <functional>
+#include <memory>
 #include <type_traits>
 #include <unordered_map>
 
@@ -1158,6 +1159,233 @@ int bf_resident_transfer(bf_ctx* c, uint32_t hs, uint32_t hd, bf_transfer* t) {
   return BF_OK;
 }
 
+// The locks of two distinct ctxs, taken in address order so that two calls over the same pair never wait on each other.
+static std::pair<std::unique_lock<std::mutex>, std::unique_lock<std::mutex>> lock_pair(bf_ctx* a, bf_ctx* b) {
+  if (std::less<bf_ctx*>()(b, a)) std::swap(a, b);
+  std::unique_lock<std::mutex> first(a->mu);
+  std::unique_lock<std::mutex> second(b->mu);
+  return {std::move(first), std::move(second)};
+}
+
+// The staged runs of a cross-ctx transfer, as offsets from the start of the staging (GatherParams), the same in both ctxs'
+// scratch: the unfit word, reasons, identity indices, marks, state records, result records, then each side area the source has.
+struct RunStaging {
+  size_t reason = 16, ident, mark, state, result, timers, sched_in, runctl, bytes;
+  RunStaging(uint32_t n, const bf_layout& F, const RunAreas& A) {
+    auto next = [](size_t o, size_t b) { return round_up_sz(o + b, 16); };
+    ident = next(reason, n * 4ull);
+    mark = next(ident, n * 4ull);
+    state = next(mark, n * 4ull);
+    result = next(state, (size_t)n * F.state_stride);
+    timers = next(result, (size_t)n * F.result_stride);
+    sched_in = next(timers, (size_t)n * A.timer_k * 8);
+    runctl = next(sched_in, A.d_sched_in ? n * sizeof(bf_sched_run) : 0);
+    bytes = next(runctl, A.d_runctl ? n * sizeof(bf_run_ctl) : 0);
+  }
+  // the staged runs at `base` as a source view: an ExtentBatch of layout F over the slots of the ctx holding them
+  bf::ExtentBatch view(uint8_t* base, const bf::ExtentBatch& src, const RunAreas& A, uint32_t n, const bf::Slot* slots,
+                       uint32_t n_slots) const {
+    bf::ExtentBatch B = src;
+    B.state = base + state; B.result = base + result; B.mark = reinterpret_cast<uint32_t*>(base + mark);
+    B.areas = {A.timer_k ? reinterpret_cast<unsigned long long*>(base + timers) : nullptr, A.timer_k,
+               A.d_sched_in ? reinterpret_cast<bf_sched_run*>(base + sched_in) : nullptr, nullptr, src.areas.sched_stride,
+               A.d_runctl ? reinterpret_cast<bf_run_ctl*>(base + runctl) : nullptr};
+    B.slots = slots; B.n_slots = n_slots;
+    B.prev_runs = 0; B.eval_runs = n; B.full_epoch = 0;
+    return B;
+  }
+};
+
+// The packed topology records of `slots` of ctx c (live), each at a 16-byte boundary in order, into out: one H2D copy of the
+// moves, one move_records launch into c->d_call, one D2H copy, enqueued on the ctx stream; the caller synchronises it.
+static int pack_records(bf_ctx* c, const std::vector<uint32_t>& slots, std::vector<uint8_t>& out) {
+  std::vector<unsigned long long> moves(4 * slots.size());
+  size_t off = 0;
+  for (size_t i = 0; i < slots.size(); ++i) {
+    const TopoMeta& m = c->meta[slots[i]];
+    moves[4 * i] = m.offset; moves[4 * i + 1] = off; moves[4 * i + 2] = m.bytes; moves[4 * i + 3] = 0;
+    off += round_up_sz(m.bytes, 16);
+  }
+  BF_CUDA(c, cudaSetDevice(c->device));
+  const unsigned long long* d_moves = nullptr;
+  uint8_t* packed = nullptr;
+  CallStage st;
+  st.up(d_moves, moves.data(), moves.size());
+  st.out(packed, off);
+  if (int rc = st.send(c, "bf_resident_transfer_ctx (slot map)")) return rc;
+  out.resize(off);
+  BF_CUDA(c, bf::launch_move_records(c->arena, packed, d_moves, (uint32_t)slots.size(), c->stream));
+  BF_CUDA(c, cudaMemcpyAsync(out.data(), packed, off, cudaMemcpyDeviceToHost, c->stream));
+  c->stats.kernel_launches += 1;
+  return BF_OK;
+}
+
+// Live runs move to a batch of another ctx (resident.cu): bf_resident_transfer with the source's runs gathered into a staging
+// area, copied to the destination's scratch and re-laid there from it.  Every check, the slot map's records, the gather, the
+// copy, the fit launch and its synchronisation come before anything is written, so a refused or failed call changes nothing;
+// then the transfer launch on the destination, the retire launch on the source, and one synchronisation of each.
+int bf_resident_transfer_ctx(bf_ctx* sc, uint32_t hs, bf_ctx* dc, uint32_t hd, bf_ctx_transfer* t) {
+  if (!sc || !dc) return BF_EINVAL;
+  if (sc == dc) {
+    std::lock_guard<std::mutex> g(sc->mu);
+    return fail(sc, BF_EINVAL, "a transfer within one ctx is bf_resident_transfer");
+  }
+  auto locks = lock_pair(sc, dc);
+  if (!t || t->struct_size != sizeof(bf_ctx_transfer)) return fail(sc, BF_EINVAL, "null bf_ctx_transfer or bad struct_size");
+  t->unfit = BF_EXTENT_NO_RUN;
+  t->unfit_reason = BF_UNFIT_NONE;
+  t->why = bf_extent{};
+  Resident* src = live_batch(sc, hs);
+  if (!src) return fail(sc, BF_EINVAL, "unknown resident batch (source)");
+  Resident* dst = live_batch(dc, hd);
+  if (!dst) return fail(sc, BF_EINVAL, "unknown resident batch (destination)");
+  const uint32_t N = t->src_n_runs, D = t->dst_n_runs, n = t->n, n_map = t->n_slot_map;
+  if (N > src->cap) return fail(sc, BF_EINVAL, "src_n_runs exceeds the source batch");
+  if ((uint64_t)D + n > dst->cap) return fail(sc, BF_EINVAL, "dst_n_runs + n exceeds the destination batch (reshape it first)");
+  if (n && !t->runs) return fail(sc, BF_EINVAL, "null runs");
+  if (n_map && !t->slot_map) return fail(sc, BF_EINVAL, "null slot_map with a non-zero n_slot_map");
+  std::vector<uint8_t> gone(N, 0);
+  for (uint32_t i = 0; i < n; ++i) {
+    const uint32_t q = t->runs[i];
+    if (q >= N) return fail(sc, BF_EINVAL, "runs[" + std::to_string(i) + "] is not below src_n_runs");
+    if (gone[q]) return fail(sc, BF_EINVAL, "runs[" + std::to_string(i) + "] is moved twice");
+    gone[q] = 1;
+  }
+  if (n == 0) { t->n_moves = 0; return BF_OK; }
+  if (src->areas.d_sched_in && !dst->areas.d_sched_in)
+    return fail(sc, BF_EINVAL, "the source batch has limiter inputs and the destination has no area for them (bf_resident_sched)");
+  // the map as the gather reads it: an entry of a source slot that is not live becomes kSlotDead; every other used entry must
+  // name a live destination slot holding the same packed record.  The records of the used entries are packed on each device
+  // and come back in one copy per ctx.
+  std::vector<uint32_t> dmap(t->slot_map, t->slot_map + n_map), used_s, used_d;
+  for (uint32_t s = 0; s < n_map; ++s) {
+    if (dmap[s] == BF_SLOT_NONE) continue;
+    uint32_t bs = 0, bd = 0;
+    if (bf_topology_record(sc, s, nullptr, &bs) != BF_OK) { dmap[s] = bf::kSlotDead; continue; }
+    const std::string at = "slot_map[" + std::to_string(s) + "] = " + std::to_string(dmap[s]) + ": ";
+    if (bf_topology_record(dc, dmap[s], nullptr, &bd) != BF_OK) return fail(sc, BF_EINVAL, at + "not a live slot of the destination ctx");
+    if (bs != bd) return fail(sc, BF_EINVAL, at + "its topology record differs from the source slot's");
+    used_s.push_back(s); used_d.push_back(dmap[s]);
+  }
+  if (!used_s.empty()) {
+    std::vector<uint8_t> rec_s, rec_d;
+    int rc = pack_records(sc, used_s, rec_s);
+    if (rc == BF_OK) { rc = pack_records(dc, used_d, rec_d); if (rc != BF_OK) fail(sc, rc, dc->err); }
+    const cudaError_t e1 = cudaStreamSynchronize(sc->stream), e2 = cudaStreamSynchronize(dc->stream);
+    if (rc != BF_OK) return rc;
+    if (e1 != cudaSuccess || e2 != cudaSuccess) return cuda_fail(sc, e1 != cudaSuccess ? e1 : e2, "bf_resident_transfer_ctx (slot map)");
+    size_t o = 0;
+    for (size_t i = 0; i < used_s.size(); ++i) {
+      const uint32_t b = sc->meta[used_s[i]].bytes;
+      if (memcmp(rec_s.data() + o, rec_d.data() + o, b) != 0)
+        return fail(sc, BF_EINVAL, "slot_map[" + std::to_string(used_s[i]) + "] = " + std::to_string(used_d[i]) +
+                                       ": its topology record differs from the source slot's");
+      o += round_up_sz(b, 16);
+    }
+  }
+  const uint32_t m = N - n;
+  std::vector<uint32_t> to;
+  const uint32_t n_moves = retire_moves(gone, m, n, to);
+  const bf_layout F = src->L;
+  const RunStaging stg(n, F, src->areas);
+  // the source: runs, map and moves up, the gather into the staging behind them, an event behind the gather
+  BF_CUDA(sc, cudaSetDevice(sc->device));
+  bf::GatherParams G{};
+  bf::RetireParams Q{};   // the source's compaction, once the destination took the runs
+  const uint32_t head[4] = {BF_EXTENT_NO_RUN, 0u, 0u, 0u};
+  uint8_t* s_rest = nullptr;
+  CallStage st;
+  st.up(G.runs, t->runs, n);
+  if (n_map) st.up(G.slot_map, dmap.data(), n_map);
+  st.up(Q.to, to.data(), n);
+  st.up(G.unfit, head, 4);
+  st.out(s_rest, stg.bytes - stg.reason);   // the sections follow one another: the staging starts at G.unfit
+  if (int rc = st.send(sc, "bf_resident_transfer_ctx")) return rc;
+  uint8_t* s_base = reinterpret_cast<uint8_t*>(G.unfit);
+  G.src = extent_batch(sc, src, dst->L);
+  G.n = n; G.n_slot_map = n_map;
+  const bf::ExtentBatch sv = stg.view(s_base, G.src, src->areas, n, nullptr, 0);
+  G.reason = reinterpret_cast<uint32_t*>(s_base + stg.reason); G.ident = reinterpret_cast<uint32_t*>(s_base + stg.ident);
+  G.mark = const_cast<uint32_t*>(sv.mark); G.state = const_cast<uint8_t*>(sv.state); G.result = const_cast<uint8_t*>(sv.result);
+  G.areas = sv.areas;
+  cudaEvent_t gathered = nullptr;
+  BF_CUDA(sc, cudaEventCreateWithFlags(&gathered, cudaEventDisableTiming));
+  std::unique_ptr<CUevent_st, cudaError_t (*)(cudaEvent_t)> ev_owner(gathered, cudaEventDestroy);
+  BF_CUDA(sc, bf::launch_gather(G, sc->stream));
+  BF_CUDA(sc, cudaEventRecord(gathered, sc->stream));
+  sc->stats.kernel_launches += 1;
+  // the destination: the staging copied in, the fit launch over it, its verdict down
+  BF_CUDA(sc, cudaSetDevice(dc->device));
+  if (int rc = bf::sync_slots(dc, dc->stream)) { cudaStreamSynchronize(sc->stream); return fail(sc, rc, dc->err); }
+  bf::TransferParams P{};
+  uint8_t* d_base = nullptr;
+  CallStage dt;
+  dt.out(d_base, stg.bytes);
+  dt.out(P.extent, n);
+  if (int rc = dt.send(dc, "bf_resident_transfer_ctx")) { cudaStreamSynchronize(sc->stream); return fail(sc, rc, dc->err); }
+  P.src = stg.view(d_base, G.src, src->areas, n, dc->slots_dev, (uint32_t)dc->slots_host.size());
+  P.runs = reinterpret_cast<uint32_t*>(d_base + stg.ident);
+  P.unfit = reinterpret_cast<uint32_t*>(d_base);
+  P.dst_state = dst->d_state; P.dst_result = dst->d_result; P.dst_mark = dst->d_mark; P.mark_value = dst->mark_must_list();
+  P.dst_areas = dst->areas_view();
+  P.n = n; P.dst_first = D; P.T = dst->L;
+  cudaStream_t ds = dc->stream;
+  cudaError_t e = cudaStreamWaitEvent(ds, gathered, 0);
+  if (e == cudaSuccess) e = cudaMemcpyPeerAsync(d_base, dc->device, s_base, sc->device, stg.bytes, ds);
+  if (e == cudaSuccess) e = bf::launch_transfer_fit(P, ds);
+  if (e == cudaSuccess) e = cudaMemcpyAsync(&dc->pinned->word, P.unfit, 4, cudaMemcpyDeviceToHost, ds);
+  if (e == cudaSuccess) e = cudaStreamSynchronize(ds);
+  const cudaError_t es = cudaStreamSynchronize(sc->stream);   // the gather went through before the copy; nothing else is queued
+  if (e == cudaSuccess) e = es;
+  if (e != cudaSuccess) return cuda_fail(sc, e, "bf_resident_transfer_ctx (gather, copy and fit)");
+  dc->stats.kernel_launches += 1;
+  const uint32_t unfit = dc->pinned->word;
+  if (unfit != BF_EXTENT_NO_RUN) {   // the refused run's extent and verdict, read on this path only
+    uint32_t x[4] = {}, why = 0;
+    BF_CUDA(sc, cudaMemcpy(x, P.extent + unfit, sizeof x, cudaMemcpyDeviceToHost));
+    BF_CUDA(sc, cudaMemcpy(&why, d_base + stg.reason + 4ull * unfit, 4, cudaMemcpyDeviceToHost));
+    t->unfit = unfit;
+    t->unfit_reason = why ? why : (uint32_t)BF_UNFIT_LAYOUT;
+    t->why.struct_size = sizeof(bf_extent); t->why.n_runs = N;
+    t->why.steps_max = std::max(1u, x[0]); t->why.child_nibbles = x[1]; t->why.fields = x[2];
+    t->why.widest_run = x[0] ? t->runs[unfit] : BF_EXTENT_NO_RUN;
+    if (why) {
+      static const char* const kWhy[] = {"", "", "is not mapped", "is at or past n_slot_map", "is not live in the source ctx"};
+      return fail(sc, BF_EINVAL, "runs[" + std::to_string(unfit) + "] (run " + std::to_string(t->runs[unfit]) + "): its topology slot " +
+                                     kWhy[why]);
+    }
+    return fail(sc, BF_EINVAL, "runs[" + std::to_string(unfit) + "] (run " + std::to_string(t->runs[unfit]) +
+                                   ") does not fit the destination layout: it needs steps_max " + std::to_string(x[0]) +
+                                   ", child_nibbles " + std::to_string(x[1]) + ", fields " + std::to_string(x[2]) + ", " +
+                                   std::to_string(x[3] & 0x7FFFFFFFu) + " timer slot(s) of the destination's " +
+                                   std::to_string(P.dst_areas.timer_k) +
+                                   ((x[3] >> 31) ? ", and a run-control area (bf_resident_runctl) for its stop or deadlines" : ""));
+  }
+  bool src_baseline = src->prev_valid;
+  for (uint32_t i = 0; i < n && src_baseline; ++i) src_baseline = t->runs[i] < src->prev_runs;
+  src->state_changed(sc);   // as after an upload, both batches
+  dst->state_changed(dc);
+  const cudaError_t e_dst = bf::launch_transfer(P, ds);
+  Q.state = src->d_state; Q.result = src->d_result; Q.mark = src->d_mark; Q.mark_value = src->mark_must_list();
+  Q.m = m; Q.n = n; Q.state_stride = F.state_stride; Q.result_stride = F.result_stride; Q.areas = src->areas_view();
+  // the staging holds the runs: the source compacts at once, unless the transfer could not be launched (then the runs stay)
+  e = e_dst == cudaSuccess ? cudaSetDevice(sc->device) : cudaSuccess;
+  if (e == cudaSuccess && e_dst == cudaSuccess) e = bf::launch_retire(Q, sc->stream);
+  const int r_src = src->sync_in_place(sc, e, "bf_resident_transfer_ctx (retire)");
+  const int r_dst = dst->sync_in_place(dc, e_dst, "bf_resident_transfer_ctx (transfer)");
+  sc->stats.kernel_launches += e_dst == cudaSuccess ? 1 : 0;
+  dc->stats.kernel_launches += 1;
+  if (r_src != BF_OK || r_dst != BF_OK) {   // either side may be half written: neither keeps a baseline
+    src->records_unknown(); dst->records_unknown();
+    return r_src != BF_OK ? r_src : fail(sc, r_dst, dc->err);
+  }
+  dst->received(D, n, src_baseline);
+  src->compact_to(m, N, to);
+  write_moves(to, m, t->moves_from, t->moves_to);
+  t->src_n_runs = m; t->dst_n_runs = D + n; t->n_moves = n_moves;
+  return BF_OK;
+}
+
 // ---- step timers (resident.cu) ------------------------------------------------------------------------------------------------
 // The area of K slots per run: created with every slot empty, or grown to a larger K with each run's slots kept in place (one
 // relay launch into new slots, one synchronisation; the old area is freed once the new one is filled).
@@ -1350,17 +1578,26 @@ int bf_resident_sched_download(bf_ctx* c, uint32_t h, uint32_t first, uint32_t n
 // One schedule over several resident batches: every check first; then the tables' upload, the totals' start, a count launch per
 // part into the shared totals, the limit-and-compare, CTA-scan and list launches per part, the D2H copies of the totals and of each part's
 // two counts, one synchronisation, and the lists of parts whose buffers are not pinned.
-int bf_resident_schedule(bf_ctx* c, const bf_sched_tables* t, uint32_t now, bf_resident_sched_part* parts, uint32_t n_parts,
-                         bf_sched_out* totals) {
-  if (!c) return BF_EINVAL;
-  std::lock_guard<std::mutex> g(c->mu);
+// The limiter parameters of one part: the call's S, over runs [0, n_runs) of batch r
+static bf::SchedParams sched_part_params(const bf::SchedParams& S, const Resident* r, uint32_t n_runs) {
+  const bf_layout& L = r->L;
+  bf::SchedParams P = S;
+  const bf::RunAreasView A = r->areas_view();
+  P.state = r->d_state; P.result = r->d_result; P.runs = A.sched_in; P.records = A.sched_rec; P.n_runs = n_runs;
+  P.words = L.words; P.state_stride = L.state_stride; P.off_phase = L.off_phase; P.off_child = L.off_child;
+  P.child_nibbles = L.child_nibbles; P.result_stride = L.result_stride; P.off_ready = L.off_ready; P.stride = A.sched_stride;
+  return P;
+}
+
+// The checks of one schedule over parts of ctx c (the caller holds its lock): rs receives each part's batch.
+static int check_schedule(bf_ctx* c, const bf_sched_tables* t, uint32_t now, const bf_resident_sched_part* parts, uint32_t n_parts,
+                          const bf_sched_out* totals, std::vector<Resident*>& rs) {
   if (!t || t->struct_size != sizeof(bf_sched_tables)) return fail(c, BF_EINVAL, "bad bf_sched_tables.struct_size");
   if ((t->n_stories && !t->story_limit) || (t->n_queues && (!t->queue_limit || !t->queue_aging_s)))
     return fail(c, BF_EINVAL, "null limit table");
   if (!totals || totals->struct_size != sizeof(bf_sched_out)) return fail(c, BF_EINVAL, "bad bf_sched_out.struct_size");
   if (now == BF_SCHED_NONE) return fail(c, BF_EINVAL, "now must be below BF_SCHED_NONE");
   if (n_parts && !parts) return fail(c, BF_EINVAL, "null parts");
-  std::vector<Resident*> rs(n_parts);
   for (uint32_t i = 0; i < n_parts; ++i) {
     const bf_resident_sched_part& p = parts[i];
     auto at = [&] { return "part " + std::to_string(i) + " (batch " + std::to_string(p.handle) + "): "; };
@@ -1378,6 +1615,13 @@ int bf_resident_schedule(bf_ctx* c, const bf_sched_tables* t, uint32_t now, bf_r
                                     " runs: a tick must come between them and the schedule");
     rs[i] = r;
   }
+  return BF_OK;
+}
+
+static int resident_schedule_locked(bf_ctx* c, const bf_sched_tables* t, uint32_t now, bf_resident_sched_part* parts, uint32_t n_parts,
+                                    bf_sched_out* totals) {
+  std::vector<Resident*> rs(n_parts);
+  if (int rc = check_schedule(c, t, now, parts, n_parts, totals, rs)) return rc;
   BF_CUDA(c, cudaSetDevice(c->device));
   cudaStream_t s = c->stream;
   if (int rc = bf::sync_slots(c, s)) return rc;   // topology puts and drops since the ticks count as they stand now
@@ -1415,16 +1659,7 @@ int bf_resident_schedule(bf_ctx* c, const bf_sched_tables* t, uint32_t now, bf_r
   if (int rc = st.send(c, "bf_resident_schedule")) return rc;
   S.n_stories = t->n_stories; S.n_queues = t->n_queues; S.global_limit = t->global_limit; S.global_base = t->global_running_base;
   S.n_slots = (uint32_t)c->slots_host.size(); S.slots = c->slots_dev; S.now = now;
-  auto part_params = [&](uint32_t i) {
-    const Resident* r = rs[i];
-    const bf_layout& L = r->L;
-    bf::SchedParams P = S;
-    const bf::RunAreasView A = r->areas_view();
-    P.state = r->d_state; P.result = r->d_result; P.runs = A.sched_in; P.records = A.sched_rec; P.n_runs = parts[i].n_runs;
-    P.words = L.words; P.state_stride = L.state_stride; P.off_phase = L.off_phase; P.off_child = L.off_child;
-    P.child_nibbles = L.child_nibbles; P.result_stride = L.result_stride; P.off_ready = L.off_ready; P.stride = A.sched_stride;
-    return P;
-  };
+  auto part_params = [&](uint32_t i) { return sched_part_params(S, rs[i], parts[i].n_runs); };
   std::vector<unsigned long long> part_tot((size_t)n_parts * 2, 0ull);
   uint64_t launches = 1;
   auto body = [&]() -> cudaError_t {
@@ -1475,6 +1710,139 @@ int bf_resident_schedule(bf_ctx* c, const bf_sched_tables* t, uint32_t now, bf_r
     BF_CUDA(c, q.runs.copy(p.n_listed));
     BF_CUDA(c, q.heads.copy(p.n_listed));
     BF_CUDA(c, q.events.copy(p.n_events));
+  }
+  return BF_OK;
+}
+
+int bf_resident_schedule(bf_ctx* c, const bf_sched_tables* t, uint32_t now, bf_resident_sched_part* parts, uint32_t n_parts,
+                         bf_sched_out* totals) {
+  if (!c) return BF_EINVAL;
+  std::lock_guard<std::mutex> g(c->mu);
+  return resident_schedule_locked(c, t, now, parts, n_parts, totals);
+}
+
+// Phase 1 of bf_resident_schedule_ctxs on ctx c (its lock held, its parts checked): the totals' start without bases and the
+// count launches of its parts, then the D2H copies of the four totals into c->span_totals (pinned): story_running [ns] |
+// queue_running [nq] | queue_max_priority [nq] | global_running [1].  Enqueued on the ctx stream; the caller synchronises.
+static int span_count(bf_ctx* c, const bf_sched_tables* t, uint32_t now, const std::vector<bf_resident_sched_part>& parts,
+                      const std::vector<Resident*>& rs) {
+  const size_t ns = t->n_stories, nq = t->n_queues, words = ns + 2 * nq + 1;
+  BF_CUDA(c, cudaSetDevice(c->device));
+  if (c->span_totals_cap < words) {
+    uint32_t* nt = nullptr;
+    const cudaError_t e = cudaHostAlloc(reinterpret_cast<void**>(&nt), words * 4, cudaHostAllocDefault);
+    if (e != cudaSuccess) { cudaGetLastError(); return fail(c, BF_ENOMEM, std::string("cudaHostAlloc: ") + cudaGetErrorString(e)); }
+    if (c->span_totals) cudaFreeHost(c->span_totals);
+    c->span_totals = nt; c->span_totals_cap = words;
+  }
+  cudaStream_t s = c->stream;
+  if (int rc = bf::sync_slots(c, s)) return rc;
+  bf::SchedParams S{};
+  CallStage st;
+  st.up(S.queue_aging, t->queue_aging_s, nq);
+  st.out(S.story_running, ns); st.out(S.queue_running, nq); st.out(S.queue_maxprio, nq); st.out(S.global_running, 1);
+  if (int rc = st.send(c, "bf_resident_schedule_ctxs")) return rc;
+  S.n_stories = t->n_stories; S.n_queues = t->n_queues;
+  S.n_slots = (uint32_t)c->slots_host.size(); S.slots = c->slots_dev; S.now = now;
+  cudaError_t e = bf::launch_schedule(S, (uint32_t)c->sm_count, s, bf::kSchedInit);
+  c->stats.kernel_launches += 1;
+  for (size_t i = 0; i < parts.size() && e == cudaSuccess; ++i)
+    if (parts[i].n_runs) {
+      e = bf::launch_schedule(sched_part_params(S, rs[i], parts[i].n_runs), (uint32_t)c->sm_count, s, bf::kSchedCount);
+      c->stats.kernel_launches += 1;
+    }
+  uint32_t* h = c->span_totals;
+  if (e == cudaSuccess && ns) e = cudaMemcpyAsync(h, S.story_running, ns * 4, cudaMemcpyDeviceToHost, s);
+  if (e == cudaSuccess && nq) e = cudaMemcpyAsync(h + ns, S.queue_running, nq * 4, cudaMemcpyDeviceToHost, s);
+  if (e == cudaSuccess && nq) e = cudaMemcpyAsync(h + ns + nq, S.queue_maxprio, nq * 4, cudaMemcpyDeviceToHost, s);
+  if (e == cudaSuccess) e = cudaMemcpyAsync(h + ns + 2 * nq, S.global_running, 4, cudaMemcpyDeviceToHost, s);
+  return e == cudaSuccess ? BF_OK : cuda_fail(c, e, "bf_resident_schedule_ctxs (count)");
+}
+
+// One schedule over resident batches of several ctxs: every check on every ctx first; phase 1 counts each ctx's parts alone;
+// the host gives each ctx the table bases plus the other ctxs' counts; phase 2 is bf_resident_schedule on each ctx with those.
+int bf_resident_schedule_ctxs(const bf_sched_tables* t, uint32_t now, bf_ctx_sched_part* parts, uint32_t n_parts, bf_sched_out* totals) {
+  if (!parts || n_parts == 0) return BF_EINVAL;
+  bf_ctx* c0 = parts[0].ctx;
+  for (uint32_t i = 0; i < n_parts; ++i) {
+    const bf_ctx_sched_part& p = parts[i];
+    if (p.struct_size != sizeof(bf_ctx_sched_part) || p.reserved || !p.ctx || !p.part) {
+      if (c0) { std::lock_guard<std::mutex> g(c0->mu); fail(c0, BF_EINVAL, "part " + std::to_string(i) + ": bad struct_size, reserved, ctx or part"); }
+      return BF_EINVAL;
+    }
+  }
+  // the distinct ctxs in order of first appearance, each with its parts (copies, in call order)
+  std::vector<bf_ctx*> ctxs;
+  std::vector<std::vector<uint32_t>> of;
+  for (uint32_t i = 0; i < n_parts; ++i) {
+    const size_t k = std::find(ctxs.begin(), ctxs.end(), parts[i].ctx) - ctxs.begin();
+    if (k == ctxs.size()) { ctxs.push_back(parts[i].ctx); of.emplace_back(); }
+    of[k].push_back(i);
+  }
+  std::vector<bf_ctx*> order = ctxs;
+  std::sort(order.begin(), order.end(), std::less<bf_ctx*>());
+  std::vector<std::unique_lock<std::mutex>> locks;
+  for (bf_ctx* c : order) locks.emplace_back(c->mu);
+  const size_t K = ctxs.size();
+  auto report = [&](size_t k, int code) {   // the first part's ctx carries every refusal's text too
+    if (k) ctxs[0]->err = ctxs[k]->err;
+    return code;
+  };
+  std::vector<std::vector<bf_resident_sched_part>> ps(K);
+  std::vector<std::vector<Resident*>> rs(K);
+  for (size_t k = 0; k < K; ++k) {
+    for (uint32_t i : of[k]) ps[k].push_back(*parts[i].part);
+    rs[k].resize(ps[k].size());
+    if (int rc = check_schedule(ctxs[k], t, now, ps[k].data(), (uint32_t)ps[k].size(), totals, rs[k])) return report(k, rc);
+  }
+  // phase 1: each ctx's own counts
+  int rc = BF_OK;
+  size_t started = 0, bad = 0;
+  for (; started < K && rc == BF_OK; ++started)
+    if ((rc = span_count(ctxs[started], t, now, ps[started], rs[started])) != BF_OK) bad = started;
+  for (size_t k = 0; k < started; ++k) {
+    const cudaError_t e = cudaStreamSynchronize(ctxs[k]->stream);
+    if (rc == BF_OK && e != cudaSuccess) { rc = cuda_fail(ctxs[k], e, "bf_resident_schedule_ctxs (count)"); bad = k; }
+  }
+  if (rc != BF_OK) return report(bad, rc);
+  // the bases of ctx k: the tables' plus every other ctx's counts
+  const size_t ns = t->n_stories, nq = t->n_queues;
+  std::vector<uint32_t> story_base(ns), queue_base(nq);
+  std::vector<int32_t> maxprio_base(nq);
+  auto failed = [&](int code) {   // as after a failed bf_resident_schedule, every part of every ctx
+    for (auto& v : rs)
+      for (Resident* r : v) { r->areas.sched_base_runs = 0; r->commit_all = true; r->scheduled = -1; }
+    return code;
+  };
+  for (size_t k = 0; k < K; ++k) {
+    bf_sched_tables tk = *t;
+    uint32_t global_base = t->global_running_base;
+    for (size_t s = 0; s < ns; ++s) story_base[s] = t->story_running_base ? t->story_running_base[s] : 0u;
+    for (size_t q = 0; q < nq; ++q) {
+      queue_base[q] = t->queue_running_base ? t->queue_running_base[q] : 0u;
+      maxprio_base[q] = t->queue_max_priority_base ? t->queue_max_priority_base[q] : INT32_MIN;
+    }
+    for (size_t j = 0; j < K; ++j) {
+      if (j == k) continue;
+      const uint32_t* h = ctxs[j]->span_totals;
+      for (size_t s = 0; s < ns; ++s) story_base[s] += h[s];
+      for (size_t q = 0; q < nq; ++q) {
+        queue_base[q] += h[ns + q];
+        maxprio_base[q] = std::max(maxprio_base[q], static_cast<int32_t>(h[ns + nq + q]));
+      }
+      global_base += h[ns + 2 * nq];
+    }
+    tk.story_running_base = story_base.data(); tk.queue_running_base = queue_base.data();
+    tk.queue_max_priority_base = maxprio_base.data(); tk.global_running_base = global_base;
+    // every ctx ends with the same totals: the last one hands them to the caller
+    bf_sched_out none{};
+    none.struct_size = sizeof(bf_sched_out);
+    bf_sched_out* out = k + 1 == K ? totals : &none;
+    if (int rk = resident_schedule_locked(ctxs[k], &tk, now, ps[k].data(), (uint32_t)ps[k].size(), out)) return report(k, failed(rk));
+    for (size_t i = 0; i < of[k].size(); ++i) {
+      bf_resident_sched_part& p = *parts[of[k][i]].part;
+      p.n_listed = ps[k][i].n_listed; p.full = ps[k][i].full; p.n_events = ps[k][i].n_events;
+    }
   }
   return BF_OK;
 }

@@ -359,6 +359,29 @@ class Frontier:
         return {"src_n_runs": int(t.src_n_runs), "dst_n_runs": int(t.dst_n_runs), "moves_from": mf[:t.n_moves].copy(),
                 "moves_to": mt[:t.n_moves].copy()}
 
+    def resident_transfer_ctx(self, dst_frontier: "Frontier", src: int, dst: int, src_n: int, dst_n: int, runs, slot_map) -> dict:
+        """bf_resident_transfer_ctx: resident_transfer from batch src of this ctx to batch dst of dst_frontier's ctx (another
+        device, or another ctx of the same one).  slot_map[s] is the destination slot of this ctx's slot s, or A.SLOT_NONE.
+        -> dict(src_n_runs, dst_n_runs, moves_from, moves_to).  A refusal raises FrontierError with .unfit, .unfit_reason
+        (A.UNFIT_*) and .why"""
+        rs = np.ascontiguousarray(runs, dtype=np.uint32)
+        sm = np.ascontiguousarray(slot_map, dtype=np.uint32)
+        n = rs.shape[0]
+        mf = np.zeros(max(n, 1), dtype=np.uint32)
+        mt = np.zeros(max(n, 1), dtype=np.uint32)
+        t = A.CtxTransfer(struct_size=C.sizeof(A.CtxTransfer), src_n_runs=int(src_n), dst_n_runs=int(dst_n),
+                          runs=rs.ctypes.data if n else None, n=n, slot_map=sm.ctypes.data if sm.size else None, n_slot_map=sm.size,
+                          moves_from=mf.ctypes.data, moves_to=mt.ctypes.data)
+        rc = self._lib.bf_resident_transfer_ctx(self._ctx, src, dst_frontier._ctx, dst, C.byref(t))
+        if rc != A.BF_OK:
+            err = A.FrontierError(rc, "bf_resident_transfer_ctx: %s" % self._lib.bf_last_error(self._ctx).decode())
+            err.unfit = int(t.unfit)
+            err.unfit_reason = int(t.unfit_reason)
+            err.why = t.why.as_dict()
+            raise err
+        return {"src_n_runs": int(t.src_n_runs), "dst_n_runs": int(t.dst_n_runs), "moves_from": mf[:t.n_moves].copy(),
+                "moves_to": mt[:t.n_moves].copy()}
+
     # -- step timers of a resident batch (bf_resident_timers*, bf_resident_fire)
     TIMER_DTYPE = np.dtype([("run", "<u4"), ("step", "<u2"), ("code", "u1"), ("reserved", "u1"), ("deadline", "<u4"),
                             ("reserved2", "<u4")])                                             # bf_timer, 16 B
@@ -625,45 +648,10 @@ class Frontier:
         n_runs and optionally runs_cap / events_cap (default: n_runs and n_runs * 1024) and pinned buffers runs / heads / events.
         tables: Frontier.schedule's keyword arguments.  -> dict(parts=[dict(runs, heads, events, n_listed, full, n_events)],
         story_running, queue_running, queue_max_priority, global_running)"""
-        sl = np.ascontiguousarray(tables["story_limit"], dtype=np.int32)
-        ql = np.ascontiguousarray(tables["queue_limit"], dtype=np.int32)
-        qa = np.ascontiguousarray(tables["queue_aging_s"], dtype=np.int32)
-        arr = lambda k, dt: None if tables.get(k) is None else np.ascontiguousarray(tables[k], dtype=dt)  # noqa: E731
-        sb, qb, pb = arr("story_running_base", np.uint32), arr("queue_running_base", np.uint32), arr("queue_max_priority_base", np.int32)
-        t = A.SchedTables(struct_size=C.sizeof(A.SchedTables), n_stories=sl.size, n_queues=ql.size,
-                          global_limit=int(tables.get("global_limit", 0)), global_running_base=int(tables.get("global_running_base", 0)),
-                          story_limit=sl.ctypes.data, story_running_base=(sb.ctypes.data if sb is not None else None),
-                          queue_limit=ql.ctypes.data, queue_aging_s=qa.ctypes.data,
-                          queue_running_base=(qb.ctypes.data if qb is not None else None),
-                          queue_max_priority_base=(pb.ctypes.data if pb is not None else None))
-        ps = (A.ResidentSchedPart * max(len(parts), 1))()
-        bufs = []
-        for i, p in enumerate(parts):
-            n = int(p["n_runs"])
-            rcap = int(p.get("runs_cap", n))
-            ecap = int(p.get("events_cap", n * 1024))
-            runs = p.get("runs", np.zeros(max(rcap, 1), np.uint32))
-            heads = p.get("heads", np.zeros(max(rcap, 1), self.SCHED_HEAD_DTYPE))
-            events = p.get("events", np.zeros(max(ecap, 1), np.uint16))
-            bufs.append((runs, heads, events, rcap, ecap))
-            ps[i] = A.ResidentSchedPart(struct_size=C.sizeof(A.ResidentSchedPart), handle=int(p["handle"]), n_runs=n, runs_cap=rcap,
-                                        runs=runs.ctypes.data, heads=heads.ctypes.data, events=events.ctypes.data, events_cap=ecap)
-        sr = np.zeros(max(sl.size, 1), dtype=np.uint32)
-        qr = np.zeros(max(ql.size, 1), dtype=np.uint32)
-        mp = np.zeros(max(ql.size, 1), dtype=np.int32)
-        gr = np.zeros(1, dtype=np.uint32)
-        out = A.SchedOut(struct_size=C.sizeof(A.SchedOut), records=None, story_running=sr.ctypes.data, queue_running=qr.ctypes.data,
-                         queue_max_priority=mp.ctypes.data, global_running=gr.ctypes.data)
-        self._check(self._lib.bf_resident_schedule(self._ctx, C.byref(t), int(now), ps, len(parts), C.byref(out)),
+        call = _SchedCall(tables, parts)
+        self._check(self._lib.bf_resident_schedule(self._ctx, C.byref(call.t), int(now), call.ps, len(parts), C.byref(call.out)),
                     "bf_resident_schedule")
-        res = []
-        for i, (runs, heads, events, rcap, ecap) in enumerate(bufs):
-            q = ps[i]
-            nl = min(int(q.n_listed), rcap)
-            res.append({"runs": runs[:nl].copy(), "heads": heads[:nl].copy(), "events": events[:min(int(q.n_events), ecap)].copy(),
-                        "n_listed": int(q.n_listed), "full": int(q.full), "n_events": int(q.n_events)})
-        return {"parts": res, "story_running": sr[:sl.size], "queue_running": qr[:ql.size], "queue_max_priority": mp[:ql.size],
-                "global_running": int(gr[0])}
+        return call.result()
 
     # -- resident batches: device-side state, delta uploads (row f2)
     DELTA_DTYPE = np.dtype([("run", "<u4"), ("index", "<u2"), ("field", "u1"), ("code", "u1")])
@@ -805,6 +793,74 @@ class Frontier:
         s = A.Stats()
         self._check(self._lib.bf_get_stats(self._ctx, C.byref(s)), "bf_get_stats")
         return {n: getattr(s, n) for n, _ in s._fields_}
+
+
+class _SchedCall:
+    """The arguments of one bf_resident_schedule / bf_resident_schedule_ctxs call (tables, parts with their output buffers,
+    totals), kept alive together, and the result dict they hold afterwards."""
+
+    def __init__(self, tables: dict, parts):
+        self.sl = np.ascontiguousarray(tables["story_limit"], dtype=np.int32)
+        ql = self.ql = np.ascontiguousarray(tables["queue_limit"], dtype=np.int32)
+        self.qa = np.ascontiguousarray(tables["queue_aging_s"], dtype=np.int32)
+        arr = lambda k, dt: None if tables.get(k) is None else np.ascontiguousarray(tables[k], dtype=dt)  # noqa: E731
+        self.bases = sb, qb, pb = (arr("story_running_base", np.uint32), arr("queue_running_base", np.uint32),
+                                   arr("queue_max_priority_base", np.int32))
+        self.t = A.SchedTables(struct_size=C.sizeof(A.SchedTables), n_stories=self.sl.size, n_queues=ql.size,
+                               global_limit=int(tables.get("global_limit", 0)),
+                               global_running_base=int(tables.get("global_running_base", 0)),
+                               story_limit=self.sl.ctypes.data, story_running_base=(sb.ctypes.data if sb is not None else None),
+                               queue_limit=ql.ctypes.data, queue_aging_s=self.qa.ctypes.data,
+                               queue_running_base=(qb.ctypes.data if qb is not None else None),
+                               queue_max_priority_base=(pb.ctypes.data if pb is not None else None))
+        self.ps = (A.ResidentSchedPart * max(len(parts), 1))()
+        self.bufs = []
+        for i, p in enumerate(parts):
+            n = int(p["n_runs"])
+            rcap = int(p.get("runs_cap", n))
+            ecap = int(p.get("events_cap", n * 1024))
+            runs = p.get("runs", np.zeros(max(rcap, 1), np.uint32))
+            heads = p.get("heads", np.zeros(max(rcap, 1), Frontier.SCHED_HEAD_DTYPE))
+            events = p.get("events", np.zeros(max(ecap, 1), np.uint16))
+            self.bufs.append((runs, heads, events, rcap, ecap))
+            self.ps[i] = A.ResidentSchedPart(struct_size=C.sizeof(A.ResidentSchedPart), handle=int(p["handle"]), n_runs=n,
+                                             runs_cap=rcap, runs=runs.ctypes.data, heads=heads.ctypes.data, events=events.ctypes.data,
+                                             events_cap=ecap)
+        self.sr = np.zeros(max(self.sl.size, 1), dtype=np.uint32)
+        self.qr = np.zeros(max(ql.size, 1), dtype=np.uint32)
+        self.mp = np.zeros(max(ql.size, 1), dtype=np.int32)
+        self.gr = np.zeros(1, dtype=np.uint32)
+        self.out = A.SchedOut(struct_size=C.sizeof(A.SchedOut), records=None, story_running=self.sr.ctypes.data,
+                              queue_running=self.qr.ctypes.data, queue_max_priority=self.mp.ctypes.data,
+                              global_running=self.gr.ctypes.data)
+
+    def result(self) -> dict:
+        res = []
+        for i, (runs, heads, events, rcap, ecap) in enumerate(self.bufs):
+            q = self.ps[i]
+            nl = min(int(q.n_listed), rcap)
+            res.append({"runs": runs[:nl].copy(), "heads": heads[:nl].copy(), "events": events[:min(int(q.n_events), ecap)].copy(),
+                        "n_listed": int(q.n_listed), "full": int(q.full), "n_events": int(q.n_events)})
+        ns, nq = self.sl.size, self.ql.size
+        return {"parts": res, "story_running": self.sr[:ns], "queue_running": self.qr[:nq], "queue_max_priority": self.mp[:nq],
+                "global_running": int(self.gr[0])}
+
+
+def resident_schedule_ctxs(parts, tables: dict, now: int) -> dict:
+    """bf_resident_schedule_ctxs: one schedule over resident batches of several ctxs.  parts: list of (frontier, part), each part
+    a dict as Frontier.resident_schedule takes.  -> Frontier.resident_schedule's dict, its parts in the order given"""
+    if not parts:
+        raise ValueError("resident_schedule_ctxs needs at least one part")
+    call = _SchedCall(tables, [p for _, p in parts])
+    cps = (A.CtxSchedPart * len(parts))()
+    for i, (fr, _) in enumerate(parts):
+        cps[i] = A.CtxSchedPart(struct_size=C.sizeof(A.CtxSchedPart), ctx=fr._ctx, part=C.pointer(call.ps[i]))
+    lib = parts[0][0]._lib
+    rc = lib.bf_resident_schedule_ctxs(C.byref(call.t), int(now), cps, len(parts), C.byref(call.out))
+    if rc != A.BF_OK:
+        fr = parts[0][0]
+        raise A.FrontierError(rc, "bf_resident_schedule_ctxs: %s" % fr._lib.bf_last_error(fr._ctx).decode())
+    return call.result()
 
 
 class FrontierGroup:

@@ -542,6 +542,50 @@ func (r *Resident) TransferTo(dst *Resident, srcN, dstN uint32, runs []uint32) (
 	return t, r.c.err(rc)
 }
 
+// SlotNone is a SlotMap entry of TransferToCtx that maps no slot (BF_SLOT_NONE).
+const SlotNone = 0xFFFFFFFF
+
+// Why TransferToCtx found a run unfit (BF_UNFIT_*).
+const (
+	UnfitNone         = 0 // every run fits
+	UnfitLayout       = 1 // the destination layout or its areas cannot hold the run, as for TransferTo
+	UnfitSlotUnmapped = 2 // SlotMap maps the run's slot to SlotNone
+	UnfitSlotPastMap  = 3 // the run's slot is at or past len(SlotMap)
+	UnfitSlotDead     = 4 // the run's slot is not live in the source Frontier
+)
+
+// CtxTransfer is what TransferToCtx reports: Transfer's fields, and on a refusal of a run UnfitReason (Unfit*).
+type CtxTransfer struct {
+	Transfer
+	UnfitReason uint32
+}
+
+// TransferToCtx moves runs of this batch to dst, a batch of another Frontier (another GPU, or another ctx of the same one), as
+// TransferTo does within one (bf_resident_transfer_ctx): both batches end as TransferTo leaves them, with each arrival's
+// topology slot taken through slotMap (this Frontier's slot s -> dst's slot slotMap[s], SlotNone where unmapped).  Put the same
+// Story generations into both Frontiers first; map the slots the moved runs hold, since the call compares the topology record
+// of every mapped slot with its image.  A refusal changes neither batch; Unfit and UnfitReason name the run.
+func (r *Resident) TransferToCtx(dst *Resident, srcN, dstN uint32, runs, slotMap []uint32) (CtxTransfer, error) {
+	from := make([]uint32, len(runs)+1)
+	to := make([]uint32, len(runs)+1)
+	var rp, mp *C.uint32_t
+	if len(runs) > 0 {
+		rp = (*C.uint32_t)(unsafe.Pointer(&runs[0]))
+	}
+	if len(slotMap) > 0 {
+		mp = (*C.uint32_t)(unsafe.Pointer(&slotMap[0]))
+	}
+	var counts [5]C.uint32_t
+	var why [4]C.uint32_t
+	rc := C.bfgo_resident_transfer_ctx(r.c.p, r.handle, dst.c.p, dst.handle, C.uint32_t(srcN), C.uint32_t(dstN), rp,
+		C.uint32_t(len(runs)), mp, C.uint32_t(len(slotMap)), (*C.uint32_t)(unsafe.Pointer(&from[0])),
+		(*C.uint32_t)(unsafe.Pointer(&to[0])), &counts[0], &why[0])
+	t := CtxTransfer{Transfer: Transfer{SrcN: uint32(counts[0]), DstN: uint32(counts[1]), From: from[:counts[2]], To: to[:counts[2]],
+		Unfit: uint32(counts[3]), Why: Extent{uint32(why[0]), uint32(why[1]), uint32(why[2]), uint32(why[3])}},
+		UnfitReason: uint32(counts[4])}
+	return t, r.c.err(rc)
+}
+
 // Timer is one arm request of ArmTimers (bf_timer): firing at Deadline writes Code (a DecSucceed for a sleep, a timed-out code
 // for a gate or wait) as the step's decision code; Code 0 (pending) is wake-only; Deadline TimerNone cancels.
 type Timer struct {
@@ -1238,6 +1282,49 @@ func (c *Ctx) ScheduleResident(now uint32, t *SchedTables, parts ...SchedPart) (
 		out[i] = SchedListed{NListed: uint32(ps[i].n_listed), Full: ps[i].full != 0, NEvents: uint64(ps[i].n_events)}
 	}
 	return out, res, c.err(rc)
+}
+
+// ScheduleResidentCtxs is ScheduleResident over batches of several Frontiers, e.g. one per GPU (bf_resident_schedule_ctxs):
+// each part's lists and the totals are those of one ScheduleResident over the same batches held in one Frontier, so the
+// Story, queue and global limits and the priority ordering count the Running steps of every GPU.  Call it once per tick after
+// TickTouched of every Frontier.  A refusal changes nothing, and its text names the refused part whichever Frontier holds it.
+func ScheduleResidentCtxs(now uint32, t *SchedTables, parts ...SchedPart) ([]SchedListed, *SchedResult, error) {
+	if len(parts) == 0 {
+		return nil, nil, &Error{Status: int(C.BF_EINVAL), Msg: "ScheduleResidentCtxs: no parts"}
+	}
+	res := &SchedResult{
+		StoryRunning: make([]uint32, len(t.StoryLimit)),
+		QueueRunning: make([]uint32, len(t.QueueLimit)),
+		QueueMaxPrio: make([]int32, len(t.QueueLimit)),
+	}
+	ps := make([]C.bf_resident_sched_part, len(parts)) // Go memory holding only C pointers
+	ctxs := make([]*C.bf_ctx, len(parts))
+	for i, p := range parts {
+		capRuns := len(p.Buf.Runs)
+		if len(p.Buf.Heads) < capRuns {
+			capRuns = len(p.Buf.Heads)
+		}
+		var rp *C.uint32_t
+		var hp *C.bf_sched_header
+		var ep *C.uint16_t
+		if capRuns > 0 {
+			rp, hp = (*C.uint32_t)(unsafe.Pointer(&p.Buf.Runs[0])), (*C.bf_sched_header)(unsafe.Pointer(&p.Buf.Heads[0]))
+		}
+		if len(p.Buf.Events) > 0 {
+			ep = (*C.uint16_t)(unsafe.Pointer(&p.Buf.Events[0]))
+		}
+		C.bfgo_sched_part(&ps[i], p.R.handle, C.uint32_t(p.N), rp, hp, C.uint32_t(capRuns), ep, C.uint64_t(len(p.Buf.Events)))
+		ctxs[i] = p.R.c.p
+	}
+	rc := C.bfgo_resident_schedule_ctxs(C.uint32_t(now), C.uint32_t(len(t.StoryLimit)), C.uint32_t(len(t.QueueLimit)),
+		C.int32_t(t.GlobalLimit), C.uint32_t(t.GlobalBase), i32p(t.StoryLimit), u32p(t.StoryRunningBase), i32p(t.QueueLimit),
+		i32p(t.QueueAgingS), u32p(t.QueueRunningBase), i32p(t.QueueMaxPriorityBase), &ctxs[0], &ps[0], C.uint32_t(len(ps)),
+		u32p(res.StoryRunning), u32p(res.QueueRunning), i32p(res.QueueMaxPrio), (*C.uint32_t)(unsafe.Pointer(&res.GlobalRunning)))
+	out := make([]SchedListed, len(parts))
+	for i := range ps {
+		out[i] = SchedListed{NListed: uint32(ps[i].n_listed), Full: ps[i].full != 0, NEvents: uint64(ps[i].n_events)}
+	}
+	return out, res, parts[0].R.c.err(rc)
 }
 
 // Group is one operator process driving several GPUs (bf_group_*): contiguous blocks of runs per device, one NCCL

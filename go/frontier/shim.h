@@ -236,6 +236,27 @@ static inline int bfgo_resident_transfer(bf_ctx* c, uint32_t src, uint32_t dst, 
 /* Step timers.  bf_resident_timers and bf_resident_timers_arm are called directly (flat arguments already); bf_resident_fire with
  * the bf_fire_out built here on the C stack.  counts[5] = n_fired, n_written, n_pruned, next_deadline, entries written into
  * fired (min(n_fired, fired_cap)). */
+/* bf_resident_transfer_ctx with the bf_ctx_transfer built here on the C stack.  counts[5] = src_n_runs, dst_n_runs, n_moves,
+ * unfit, unfit_reason (the n_runs given back and no moves on a refusal); why[4] as bfgo_resident_transfer. */
+static inline int bfgo_resident_transfer_ctx(bf_ctx* sc, uint32_t src, bf_ctx* dc, uint32_t dst, uint32_t src_n_runs,
+                                             uint32_t dst_n_runs, const uint32_t* runs, uint32_t n, const uint32_t* slot_map,
+                                             uint32_t n_slot_map, uint32_t* moves_from, uint32_t* moves_to, uint32_t* counts,
+                                             uint32_t* why) {
+  bf_ctx_transfer t;
+  memset(&t, 0, sizeof t);
+  t.struct_size = (uint32_t)sizeof t;
+  t.src_n_runs = src_n_runs; t.dst_n_runs = dst_n_runs; t.runs = runs; t.n = n; t.slot_map = slot_map; t.n_slot_map = n_slot_map;
+  t.moves_from = moves_from; t.moves_to = moves_to;
+  const int rc = bf_resident_transfer_ctx(sc, src, dc, dst, &t);
+  counts[0] = rc == BF_OK ? t.src_n_runs : src_n_runs;
+  counts[1] = rc == BF_OK ? t.dst_n_runs : dst_n_runs;
+  counts[2] = rc == BF_OK ? t.n_moves : 0;
+  counts[3] = t.unfit;
+  counts[4] = t.unfit_reason;
+  why[0] = t.why.steps_max; why[1] = t.why.child_nibbles; why[2] = t.why.fields; why[3] = t.why.widest_run;
+  return rc;
+}
+
 static inline int bfgo_resident_fire(bf_ctx* c, uint32_t handle, uint32_t n_runs, uint32_t now, bf_fired* fired, uint32_t fired_cap,
                                      uint32_t* counts) {
   bf_fire_out o;
@@ -484,6 +505,31 @@ static inline int bfgo_resident_schedule(bf_ctx* c, uint32_t now, uint32_t n_sto
               queue_max_priority_base);
   bfgo_sched_out(&o, NULL, story_running, queue_running, queue_max_priority, global_running);
   return bf_resident_schedule(c, &t, now, parts, n_parts, &o);
+}
+
+/* bf_resident_schedule_ctxs: part i is parts[i] (filled by bfgo_sched_part) of a batch of ctxs[i]; the bf_ctx_sched_part array
+ * that points at them is built here in C memory, so the Go side passes only C pointers. */
+static inline int bfgo_resident_schedule_ctxs(uint32_t now, uint32_t n_stories, uint32_t n_queues, int32_t global_limit,
+                                              uint32_t global_base, const int32_t* story_limit, const uint32_t* story_base,
+                                              const int32_t* queue_limit, const int32_t* queue_aging_s, const uint32_t* queue_base,
+                                              const int32_t* queue_max_priority_base, bf_ctx* const* ctxs,
+                                              bf_resident_sched_part* parts, uint32_t n_parts, uint32_t* story_running,
+                                              uint32_t* queue_running, int32_t* queue_max_priority, uint32_t* global_running) {
+  bf_sched_tables t;
+  bf_sched_out o;
+  bfgo_tables(&t, n_stories, n_queues, global_limit, global_base, story_limit, story_base, queue_limit, queue_aging_s, queue_base,
+              queue_max_priority_base);
+  bfgo_sched_out(&o, NULL, story_running, queue_running, queue_max_priority, global_running);
+  bf_ctx_sched_part* cp = (bf_ctx_sched_part*)calloc(n_parts ? n_parts : 1, sizeof *cp);
+  if (!cp) return BF_ENOMEM;
+  for (uint32_t i = 0; i < n_parts; ++i) {
+    cp[i].struct_size = (uint32_t)sizeof *cp;
+    cp[i].ctx = ctxs[i];
+    cp[i].part = &parts[i];
+  }
+  const int rc = bf_resident_schedule_ctxs(&t, now, cp, n_parts, &o);
+  free(cp);
+  return rc;
 }
 
 static inline int bfgo_group_eval(bf_group* g, const bf_layout* L, uint32_t n_runs, uint32_t flags, uint32_t max_iterations,

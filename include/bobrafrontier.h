@@ -826,7 +826,7 @@ int bf_resident_narrow(bf_ctx* ctx, uint32_t handle, const bf_layout* layout, bf
  * had the arrivals always been there, when its last tick covered dst_n_runs and the source's last tick covered every moved
  * run (else it lists every run).  Both batches end their evaluated snapshot (bf_schedule must follow a new pass).
  * Cost: one H2D copy (runs and moves), the fit launch, one D2H copy and one synchronisation before anything is written; then
- * the transfer and retire launches and one synchronisation.  Moving runs to another ctx (another GPU) is not offered.       */
+ * the transfer and retire launches and one synchronisation.  bf_resident_transfer_ctx moves runs to a batch of another ctx.  */
 typedef struct bf_transfer {
   uint32_t struct_size;        /* sizeof(bf_transfer)                                                                 */
   uint32_t src_n_runs;         /* in: source runs are [0, src_n_runs); out: src_n_runs - n                            */
@@ -841,6 +841,52 @@ typedef struct bf_transfer {
 } bf_transfer;
 
 int bf_resident_transfer(bf_ctx* ctx, uint32_t src_handle, uint32_t dst_handle, bf_transfer* t);
+
+/* ------------------------------------------------------------------ transfers between ctxs (live runs move to another GPU)
+ * bf_resident_transfer_ctx moves live runs from the batch src_handle of src_ctx to the batch dst_handle of dst_ctx, which may live
+ * on another device: to rebalance a batcher's runs over its GPUs, or to drain one.  The contract is bf_resident_transfer's, for
+ * two ctxs: afterwards both batches are byte for byte what bf_resident_transfer leaves when both live in one ctx (state and
+ * current result records re-laid to the destination layout, timer slots, limiter inputs, run control, touch and commit
+ * bookkeeping, the changed-only baseline rule, no schedule baseline for the arrivals, the moves), except one field: the topology
+ * slot in each arrival's bf_run_header is slot_map[its source slot].
+ * Slots belong to a ctx, so the caller puts the same Story generations into both ctxs and passes the map: slot_map[s] is the
+ * destination slot of source slot s, or BF_SLOT_NONE.  Every entry other than BF_SLOT_NONE whose source slot is live must name a
+ * live destination slot whose packed topology record (bf_topology_record) equals the source slot's byte for byte; the host
+ * reads both records once per call for these entries.  A moved run whose slot is at or past n_slot_map, unmapped, or dead in the
+ * source is unfit, as is every run bf_resident_transfer finds unfit; unfit_reason (BF_UNFIT_*) tells which.
+ * Refused, with BF_EINVAL and both ctxs byte-identical: everything bf_resident_transfer refuses; src_ctx == dst_ctx (that is
+ * bf_resident_transfer); a bad struct_size; slot_map NULL with n_slot_map > 0; a bad map entry as above.
+ * Cost: on the source stream one H2D copy (runs, map, moves) and the gather launch (one warp per moved run packs its state and
+ * result records and side-area entries, in the source layout, into the source ctx's scratch); one peer copy of that staging into
+ * the destination ctx's scratch (cudaMemcpyPeerAsync, ordered by an event; a device-to-device copy when both ctxs share a
+ * device); on the destination stream the fit launch, one D2H copy and one synchronisation before anything is written; then the
+ * transfer launch on the destination stream and the retire launch on the source stream, and one synchronisation of each.  The
+ * call holds both ctxs' locks, taken in address order.                                                                        */
+#define BF_SLOT_NONE 0xFFFFFFFFu
+enum {                          /* bf_ctx_transfer.unfit_reason                                                               */
+  BF_UNFIT_NONE = 0,            /* every run fits                                                                             */
+  BF_UNFIT_LAYOUT = 1,          /* the destination layout or its areas cannot hold the run (bf_resident_transfer's test)      */
+  BF_UNFIT_SLOT_UNMAPPED = 2,   /* slot_map[slot] is BF_SLOT_NONE                                                             */
+  BF_UNFIT_SLOT_PAST_MAP = 3,   /* slot >= n_slot_map                                                                         */
+  BF_UNFIT_SLOT_DEAD = 4        /* the run's slot is not live in the source ctx                                               */
+};
+typedef struct bf_ctx_transfer {
+  uint32_t struct_size;         /* sizeof(bf_ctx_transfer)                                                                    */
+  uint32_t src_n_runs;          /* in / out, as bf_transfer                                                                   */
+  uint32_t dst_n_runs;          /* in / out, as bf_transfer                                                                   */
+  const uint32_t* runs;         /* [n] as bf_transfer                                                                         */
+  uint32_t n;
+  const uint32_t* slot_map;     /* [n_slot_map] source slot -> destination slot, BF_SLOT_NONE                                 */
+  uint32_t n_slot_map;
+  uint32_t* moves_from;         /* [n] out, may be NULL, as bf_transfer                                                       */
+  uint32_t* moves_to;           /* [n] out, may be NULL                                                                       */
+  uint32_t n_moves;             /* out                                                                                        */
+  uint32_t unfit;               /* out: position in runs[] of the first unfit run, BF_EXTENT_NO_RUN when all fit              */
+  uint32_t unfit_reason;        /* out: BF_UNFIT_* of that run                                                                */
+  bf_extent why;                /* out on a fit refusal: that run's own extent                                                */
+} bf_ctx_transfer;
+
+int bf_resident_transfer_ctx(bf_ctx* src_ctx, uint32_t src_handle, bf_ctx* dst_ctx, uint32_t dst_handle, bf_ctx_transfer* t);
 
 /* ------------------------------------------------------------------ step timers (time-driven transitions of a resident batch)
  * The reference compares `now` with each run's step timers on every reconcile: sleepUntil fires a sleep step (checkSyncSleepSteps,
@@ -1011,6 +1057,28 @@ int bf_resident_sched_put(bf_ctx* ctx, uint32_t handle, const bf_sched_put* requ
 int bf_resident_sched_download(bf_ctx* ctx, uint32_t handle, uint32_t first_run, uint32_t n_runs, bf_sched_put* out);
 int bf_resident_schedule(bf_ctx* ctx, const bf_sched_tables* tables, uint32_t now, bf_resident_sched_part* parts, uint32_t n_parts,
                          bf_sched_out* totals);
+
+/* bf_resident_schedule_ctxs(tables, now, parts, n_parts, totals): one schedule over resident batches of several ctxs (one per
+ *   GPU, e.g. the shards of a group through bf_group_ctx), so that the Story, queue and global limits and priority ordering hold
+ *   over all of them.  Story and queue keys and the tables are global to the call.  Every part's records, lists, full flag and
+ *   commit-due marks, and the totals, equal those of one bf_resident_schedule over the same batches held in one ctx; with one
+ *   ctx the call is bf_resident_schedule.  Each part is checked on its own ctx as bf_resident_schedule checks it (a batch may
+ *   appear once), with n_parts >= 1, non-null ctx and part pointers and struct_size; a refusal is BF_EINVAL with nothing changed,
+ *   and bf_last_error of the first part's ctx says why (also of the refused part's own ctx).  Afterwards each batch
+ *   is scheduled for its commits as after bf_resident_schedule; a failure leaves every part as after a failed bf_resident_schedule.
+ *   Plan: the distinct ctxs are locked in address order.  Phase 1, per ctx on its stream: the totals' start without bases, a count
+ *   launch per part, one D2H copy of the four totals arrays into pinned memory, one synchronisation per ctx.  The host gives ctx k
+ *   the table bases plus every other ctx's counts (uint32 sums, as the device atomics add them; queue priority maxima by maximum,
+ *   INT32_MIN for none).  Phase 2, per ctx: bf_resident_schedule of its parts with those bases.  The exchange is
+ *   n_stories + 2 * n_queues + 1 words per ctx through the host; no collective library is involved.                            */
+typedef struct bf_ctx_sched_part {
+  uint32_t struct_size;         /* sizeof(bf_ctx_sched_part)                                                               */
+  uint32_t reserved;            /* 0                                                                                         */
+  bf_ctx* ctx;
+  bf_resident_sched_part* part; /* a part of bf_resident_schedule, of a batch of ctx                                         */
+} bf_ctx_sched_part;
+
+int bf_resident_schedule_ctxs(const bf_sched_tables* tables, uint32_t now, bf_ctx_sched_part* parts, uint32_t n_parts, bf_sched_out* totals);
 
 /* ------------------------------------------------------------------ StoryRun stops and deadlines (run control of a resident batch)
  * Above the steps, the reference stops DAG-evaluating a StoryRun for three reasons: its story timeout (enforceStoryTimeout,
