@@ -8,7 +8,8 @@ The per-area rules are not restated here; only how they compose:
   - transfer: a source with limiter inputs needs a destination with them (refused with no unfit run); then a run is unfit when
     it has more armed timer slots than the destination's K (0 without a timer area), or a run-control record that is not the
     default and no run-control area to arrive in; arrivals take the defaults of the areas the source lacks, and lose their
-    schedule baseline; the source follows retire;
+    schedule baseline; the source follows retire; into a batch of another ctx, each arrival's header slot goes through the
+    caller's slot map and nothing else differs;
   - reshape: every area grows to the new capacity with its defaults, and a change of words drops every schedule baseline;
   - narrow: the areas are kept, and a change of words drops every schedule baseline;
   - migrate: the timers are re-keyed and the migrated runs lose their schedule baseline;
@@ -21,7 +22,7 @@ from bobrapet_b200.records import pack_state
 from tests import runctl as R
 from tests import sched_resident as SRM
 from tests import timers as T
-from tests.transfer import relay_state
+from tests.transfer import map_slots, relay_state
 
 TIMERS, SCHED, RUNCTL = 1, 2, 4
 SUBSETS = tuple(range(8))
@@ -200,9 +201,11 @@ class AreaBatch:
             lost.add("runctl")
         return lost
 
-    def transfer(self, dst, dst_first, runs):
+    def transfer(self, dst, dst_first, runs, slot_map=None):
         """bf_resident_transfer of `runs` (source runs [0, self.n)) to dst at dst_first, the fit of the areas only (both
-        layouts must hold every run) -> (m, {from: to}); raises Refused, nothing changed"""
+        layouts must hold every run) -> (m, {from: to}); raises Refused, nothing changed.  slot_map: bf_resident_transfer_ctx,
+        dst in another ctx: each arrival's header slot becomes slot_map[its source slot] (every moved slot mapped), the rest as
+        within one ctx"""
         runs = [int(r) for r in runs]
         if runs and self.sched is not None and dst.sched is None:
             raise Refused("the source has limiter inputs and the destination no area for them")
@@ -214,6 +217,8 @@ class AreaBatch:
             return self.n, {}
         k, ix = len(runs), np.asarray(runs, np.int64)
         dst.state[dst_first:dst_first + k] = relay_state(self.L, dst.L, self.state[ix])
+        if slot_map is not None:
+            map_slots(dst.state[dst_first:dst_first + k], slot_map)
         if dst.timers is not None:
             dst.timers = T.transfer(self.timers, dst.timers, self.n, dst_first, runs)[1]
         if dst.runctl is not None:

@@ -46,6 +46,13 @@ def relay_result(F, T, result):
     return out
 
 
+def map_slots(state, slot_map):
+    """state records (in place) with the topology slot of each header, the first 4 bytes, replaced by slot_map[slot]"""
+    w = np.ascontiguousarray(state[:, 0:4]).view("<u4").reshape(-1)
+    state[:, 0:4] = np.asarray(slot_map, "<u4")[w.astype(np.int64)].reshape(-1, 1).view(np.uint8)
+    return state
+
+
 def placed(T):
     return (COND if T.off_cond != A.OFF_NONE else 0) | (DEC if T.off_decision != A.OFF_NONE else 0) | \
            (CHILD if T.off_child != A.OFF_NONE else 0)
@@ -69,14 +76,36 @@ def fits(e, T):
                 e["fields"] & ~placed(T))
 
 
-def transfer(src, dst, src_n, dst_n, runs):
+def slot_reason(src, r, slot_map):
+    """bf_resident_transfer_ctx's verdict on the slot of source run r: A.UNFIT_SLOT_PAST_MAP, _UNMAPPED, _DEAD (not live in the
+    source's registry) or A.UNFIT_NONE"""
+    s = int(np.ascontiguousarray(src.state[r, 0:4]).view("<u4")[0])
+    if s >= len(slot_map):
+        return A.UNFIT_SLOT_PAST_MAP
+    if int(slot_map[s]) == A.SLOT_NONE:
+        return A.UNFIT_SLOT_UNMAPPED
+    return A.UNFIT_SLOT_DEAD if s not in src.reg.live else A.UNFIT_NONE
+
+
+def bad_map_entry(src, dst, slot_map):
+    """the first entry bf_resident_transfer_ctx refuses the whole call for: a source slot that is live, mapped to a slot that is
+    not live in the destination's registry or holds another Story (another packed record) -> slot, or None"""
+    for s, t in enumerate(int(x) for x in slot_map):
+        if t != A.SLOT_NONE and s in src.reg.live and (t not in dst.reg.live or dst.reg.live[t] != src.reg.live[s]):
+            return s
+    return None
+
+
+def transfer(src, dst, src_n, dst_n, runs, slot_map=None):
     """bf_resident_transfer over two model batches -> dict(src_n_runs, dst_n_runs, moves_from, moves_to).  A refusal raises
-    RM.Refused with .unfit (and .why for a fit refusal)"""
+    RM.Refused with .unfit (and .why for a fit refusal).  slot_map: bf_resident_transfer_ctx, src and dst in two ctxs with their
+    own registries: the map's entries are checked once the runs are, a run's slot verdict (.reason, A.UNFIT_*) counts with its
+    fit in the order of runs, and each arrival's header slot is slot_map[its source slot]; the rest is the rule of one ctx"""
     runs = [int(r) for r in runs]
 
-    def refuse(why, unfit=A.EXTENT_NO_RUN, e=None):
+    def refuse(why, unfit=A.EXTENT_NO_RUN, e=None, reason=A.UNFIT_NONE):
         err = RM.Refused(A.BF_EINVAL, why)
-        err.unfit, err.why = unfit, e
+        err.unfit, err.why, err.reason = unfit, e, reason
         return err
     if src is dst:
         raise refuse("a transfer from a batch to itself")
@@ -86,15 +115,22 @@ def transfer(src, dst, src_n, dst_n, runs):
         raise refuse("dst_n_runs + n exceeds the destination batch")
     if any(r >= src_n for r in runs) or len(set(runs)) != len(runs):
         raise refuse("runs")
+    if runs and slot_map is not None and bad_map_entry(src, dst, slot_map) is not None:
+        raise refuse("slot_map[%d]" % bad_map_entry(src, dst, slot_map))
     F, T = src.L, dst.L
     for i, r in enumerate(runs):
+        why = A.UNFIT_NONE if slot_map is None else slot_reason(src, r, slot_map)
+        if why != A.UNFIT_NONE:
+            raise refuse("run %d: its slot" % r, i, None, why)
         e = run_extent(src, r, src_n, T)
         if not fits(e, T):
-            raise refuse("run %d does not fit" % r, i, e)
+            raise refuse("run %d does not fit" % r, i, e, A.UNFIT_LAYOUT)
     if not runs:
         return {"src_n_runs": src_n, "dst_n_runs": dst_n, "moves_from": np.zeros(0, np.uint32), "moves_to": np.zeros(0, np.uint32)}
     ix, n = np.asarray(runs, np.int64), len(runs)
     st, cur = relay_state(F, T, src.state[ix]), relay_result(F, T, src.cur[ix])
+    if slot_map is not None:
+        map_slots(st, slot_map)
     src_baseline = src.prev_valid and all(r < src.prev_runs for r in runs)
     m, mf, mt = src.retire(src_n, runs, 0)
     dst._end_snapshot()
@@ -135,4 +171,34 @@ class TransferRig(NarrowRig):
             for k in ("moves_from", "moves_to"):
                 self.check(np.array_equal(got[k], want[k]), "%s differ" % k)
         self.sync()
+        return want
+
+    def transfer_ctx(self, dst_rig, src, dst, src_n, dst_n, runs, slot_map):
+        """bf_resident_transfer_ctx from batch src of this rig's ctx to batch dst of dst_rig's, against the model: status,
+        unfit, unfit_reason, the extent of a fit refusal, counts and moves; then both ctxs' batches against their models"""
+        self.log.append("transfer_ctx b%d -> ctx b%d n %d / %d runs %d map %d" % (self.handles[src], dst_rig.handles[dst], src_n,
+                                                                                 dst_n, len(runs), len(slot_map)))
+        try:
+            want, refused = transfer(src, dst, src_n, dst_n, runs, slot_map), None
+        except RM.Refused as e:
+            want, refused = None, e
+        try:
+            got, status = self.fr.resident_transfer_ctx(dst_rig.fr, self.handles[src], dst_rig.handles[dst], src_n, dst_n,
+                                                        np.asarray(runs, np.uint32), slot_map), A.BF_OK
+        except A.FrontierError as d:
+            got, status = d, d.status
+        self.check(status == (refused.status if refused else A.BF_OK),
+                   "transfer_ctx status %d, the model says %s (%s)" % (status, refused or "accept", got if status else ""))
+        if refused is not None:
+            self.check(got.unfit == refused.unfit, "unfit %d, want %d (%s)" % (got.unfit, refused.unfit, got))
+            self.check(got.unfit_reason == refused.reason, "unfit_reason %d, want %d" % (got.unfit_reason, refused.reason))
+            if refused.why is not None:
+                self.check(got.why == refused.why, "why %s, want %s" % (got.why, refused.why))
+        else:
+            for k in ("src_n_runs", "dst_n_runs"):
+                self.check(got[k] == want[k], "%s %d, want %d" % (k, got[k], want[k]))
+            for k in ("moves_from", "moves_to"):
+                self.check(np.array_equal(got[k], want[k]), "%s differ" % k)
+        self.sync()
+        dst_rig.sync()
         return want
